@@ -1,11 +1,13 @@
 #!/usr/bin/env python
-"""bench.py -- headline benchmark of the B200-native KNN hot path (BASELINE.json metric).
+"""bench.py -- headline benchmark of the H100-native KNN hot path (BASELINE.json metric).
 
   python bench.py --gpus N --steps K --warmup W            # our arm (CUDA through the C ABI)
   python bench.py --impl reference --steps K --warmup W    # the reference's CPU algorithm (oracle port)
+  python bench.py --steps K --dump-outputs DIR              # also write the last timed step's results as .npy
 
 Workload (config.workload): exact brute-force cosine KNN, k=10, batch of 1024 f64 queries per step over a
-10M x 768 f32 corpus (the configuration BASELINE.json's metric is quoted on; it fits one B200).  With N
+10M x 768 f32 corpus (the configuration BASELINE.json's metric is quoted on; 54 GB with its screen copies,
+it fits one 80 GB H100).  With N
 GPUs the SAME 10M-row corpus is row-sharded N ways (strong scaling); every rank screens + exactly re-ranks
 its shard, ONE NCCL all-gather (issued by the library on its own stream) moves the per-shard top-k blocks and
 a merge kernel on every rank produces the global top-k.  Data are synthetic: a counter-based generator
@@ -20,7 +22,10 @@ Numbers on the JSON line:
   parity_checked  after the timed region the last batch is re-checked: >= 8 queries through the exact kernel
           (SDB_SCREEN_NONE_EXACT) and, at N=1, >= 2 queries through the CPU oracle over ALL rows (read back from
           the device-resident master copy); any difference in rows, order or f64 bits aborts the run.
-One JSON line is printed by rank 0 (see README / the driver contract for the keys).
+  --dump-outputs DIR  after the timed steps, the rows, distances and counts the device-resident path returned for
+          its last timed batch are written to DIR/{rows,dist,count}.npy (float64; row ids are exact below 2**53).
+          Inputs depend only on the arguments, so two builds can be compared output for output.
+One JSON line is printed by rank 0 (see README for the keys).
 """
 import argparse
 import json
@@ -40,8 +45,8 @@ WORKLOADS = {
     "northstar_10Mx768_b1024_k10_cosine_bruteforce": (10_000_000, 768, 1024, 10),
     "c2_1Mx768_b1024_k10_cosine_bruteforce": (1_000_000, 768, 1024, 10),
     "tiny_100kx128_b64_k10_cosine_bruteforce": (100_000, 128, 64, 10),
-    # BASELINE config 4 (quoted there on 8 GPUs; 107 GB of corpus + screen copies still fit one B200)
-    "c4_10Mx1536_b4096_k100_cosine_bruteforce": (10_000_000, 1536, 4096, 100),
+    # BASELINE config 4 at half the rows: 5M x 1536 is 54 GB of corpus + screen copies, which fits one 80 GB H100
+    "c4_5Mx1536_b4096_k100_cosine_bruteforce": (5_000_000, 1536, 4096, 100),
 }
 SEED_CORPUS = 0x5DB00002
 SEED_QUERY = 0x5DB0A000
@@ -54,7 +59,8 @@ def peaks():
         d = json.load(open(p))
         return {"hbm_gbs": d["hbm_gbs"], "bf16_tflops": d["bf16_tflops"],
                 "bf16_tflops_sustained": d["bf16_tflops_sustained"], "source": "measured"}
-    return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0, "source": "fallback"}
+    # NVIDIA's H100 SXM data sheet (700 W card, dense): never reached in practice, a ceiling only
+    return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0, "bf16_tflops_sustained": 989.0, "source": "H100 SXM data sheet"}
 
 
 def host_threads():
@@ -289,6 +295,8 @@ def main():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-parity", action="store_true")
     ap.add_argument("--no-extras", action="store_true", help="skip the HBM-regime table and the int8 peak")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the last timed step's results (rows, dist, count) as float64 .npy files to DIR")
     args = ap.parse_args()
     rows, dim, batch, k = WORKLOADS[args.workload]
     if args.warmup < 3:
@@ -488,6 +496,12 @@ def main():
     ms_value, wall_value = timed(lambda: run_pipelined(submit_dev, args.warmup, n_batches, True))
     launches = ctx.kernel_launches() - launches0
     stats = col.stats()
+    if args.dump_outputs and rank == 0:
+        # results of the last timed batch, still in its output slot (the later phases use other buffers)
+        o = d_out[(n_batches - 1) % DEPTH]
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        for name, t in (("rows", o[0]), ("dist", o[1]), ("count", o[2])):
+            np.save(os.path.join(args.dump_outputs, name + ".npy"), t.cpu().numpy().astype(np.float64))
     tick("timed e2e")
     # ---- timed: end to end through the host-buffer plugin call (`e2e`) ----
     ms_e2e, wall_e2e = timed(lambda: run_sync_calls(args.warmup, n_batches))
@@ -604,20 +618,12 @@ def main():
             else:
                 peak = pk["bf16_tflops_sustained"]
                 peak_src = pk["source"] + " (sustained cuBLAS bf16)"
-            roof = {"bound": "tensor", "kernel": "screen_tc_kernel<cosine,int8> (tcgen05 kind::i8)" if i8 else "screen_tc_kernel (tcgen05 kind::f16 bf16)",
+            roof = {"bound": "tensor", "kernel": "screen_tc_kernel<cosine,int8> (wgmma s8)" if i8 else "screen_tc_kernel (wgmma bf16)",
                     "achieved": ach, "peak": peak, "unit": "TOP/s" if i8 else "TFLOP/s", "frac": ach / peak,
                     "peak_source": peak_src, "traffic": None, "algorithmic_flops_per_launch": flops,
                     "launch_note": f"the screen runs as {stats['n_passes']} launch(es) of this kernel per step (a scored sample, then one streaming "
                                    "launch with in-kernel threshold refinement); 'achieved' = flops of all of them / CUDA-event time of the whole "
                                    "screen phase on the library stream (includes the selection kernels)"}
-            try:  # DRAM traffic of the dominant launch, from the committed ncu capture (not re-measured here)
-                tr = json.load(open(os.path.join(ROOT, "profiles", "ncu_traffic.json")))["screen_tc_int8" if i8 else "screen_tc_bf16"]
-                if rows == 10_000_000 and world == 1:
-                    roof["traffic"] = tr["bytes"]
-                    roof["traffic_note"] = ("dram read+write bytes of ONE launch, ncu --set full: " + tr.get("launch", "largest pass launch")
-                                            + "; " + tr["source"] + f"; algorithmic bytes of that launch {tr['algorithmic_bytes_same_launch']:.4g}")
-            except Exception:
-                pass
         else:
             passes_over_corpus = (batch + 7) // 8
             byts = passes_over_corpus * (n_shard * dim * 4.0 + n_shard * 4.0) + batch * dim * 4.0

@@ -1,5 +1,5 @@
 /*
- * sdbgpu.h -- C ABI of the B200-native KNN / HNSW / graph-expansion engine.
+ * sdbgpu.h -- C ABI of the H100-native KNN / HNSW / graph-expansion engine.
  *
  * This is the drop-in boundary for SurrealDB's vector-similarity and graph-scan hot path
  * (SURVEY.md section 8b).  The reference has NO FFI of its own (pure Rust, SURVEY F4/F5), so each
@@ -37,7 +37,7 @@ typedef enum {
   SDB_EINVAL = 1,     /* bad argument                                                               */
   SDB_EDIM = 2,       /* dimension mismatch -> Error::InvalidVectorDimension (idx/trees/vector.rs:643) */
   SDB_ENOMEM = 3,
-  SDB_ECUDA = 4,      /* CUDA runtime/driver failure, or no sm_100 device                           */
+  SDB_ECUDA = 4,      /* CUDA runtime/driver failure, or no sm_90 device                            */
   SDB_ECANCELLED = 5, /* cancel flag observed -> Error::QueryCancelled (exec/operators/knn_topk.rs:186) */
   SDB_EUNSUPPORTED = 6,
   SDB_EOVERFLOW = 7,  /* caller-provided output capacity too small / too many batches in flight      */
@@ -69,9 +69,9 @@ typedef enum { SDB_F32 = 0, SDB_F64 = 1 } sdb_dtype;
 typedef enum {
   SDB_SCREEN_AUTO = 0,
   SDB_SCREEN_SIMT_F32 = 1,   /* f32 streaming SIMT kernel                                             */
-  SDB_SCREEN_TC_BF16 = 2,    /* tcgen05 kind::f16, bf16 operands                                        */
+  SDB_SCREEN_TC_BF16 = 2,    /* wgmma bf16 operands, f32 accumulation                                    */
   SDB_SCREEN_NONE_EXACT = 3, /* no screen: exact f64 kernel for every query                              */
-  SDB_SCREEN_TC_INT8 = 4     /* tcgen05 kind::i8, int8 copy of the normalised rows (cosine); falls back to bf16 */
+  SDB_SCREEN_TC_INT8 = 4     /* wgmma s8, int8 copy         of the normalised rows (cosine); falls back to bf16 */
 } sdb_screen;
 
 /* counters of the last brute-force call on a corpus (diagnostics / bench roofline arithmetic) */

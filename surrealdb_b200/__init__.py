@@ -1,8 +1,8 @@
-"""sdbgpu -- B200-native KNN / HNSW / graph-expansion engine behind SurrealDB's operator surface.
+"""sdbgpu -- H100-native KNN / HNSW / graph-expansion engine behind SurrealDB's operator surface.
 
 Python here is only the host-side mirror of the reference's operator interface (KnnTopK, KnnScan /
 HnswIndex.knn_search, GraphEdgeScan) on top of the C ABI in include/sdbgpu.h; all compute is
-hand-written sm_100a CUDA in surrealdb_b200/csrc.
+hand-written sm_90a CUDA in surrealdb_b200/csrc.
 """
 from ._lib import SdbError, SO_PATH  # noqa: F401
 from .engine import Context, VectorColumn  # noqa: F401

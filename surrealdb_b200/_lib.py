@@ -1,6 +1,6 @@
 """ctypes loader of the C-ABI library (surrealdb_b200/csrc/libsdbgpu.so, declared in include/sdbgpu.h).
 
-There is NO CPU fallback: if the shared library is missing this module raises, and if no B200 is
+There is NO CPU fallback: if the shared library is missing this module raises, and if no H100 is
 visible every call returns SDB_ECUDA which is raised as SdbError.
 """
 import ctypes as C

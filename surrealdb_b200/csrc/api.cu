@@ -763,7 +763,7 @@ using namespace sdb;
 extern "C" {
 
 const char* sdb_last_error(void) { return g_err; }
-const char* sdb_version(void) { return "sdbgpu 0.1.0 (sm_100a)"; }
+const char* sdb_version(void) { return "sdbgpu 0.1.0 (sm_90a)"; }
 
 sdb_status sdb_ctx_create(int device, sdb_ctx** out) {
   if (!out) return SDB_EINVAL;
@@ -780,8 +780,8 @@ sdb_status sdb_ctx_create(int device, sdb_ctx** out) {
   }
   cudaDeviceProp prop;
   SDB_CUDA(cudaGetDeviceProperties(&prop, device));
-  if (prop.major != 10) {
-    set_error("device %d is sm_%d%d; this library ships sm_100a code only", device, prop.major, prop.minor);
+  if (prop.major != 9 || prop.minor != 0) {
+    set_error("device %d is sm_%d%d; this library ships sm_90a code only", device, prop.major, prop.minor);
     return SDB_ECUDA;
   }
   SDB_CUDA(cudaSetDevice(device));

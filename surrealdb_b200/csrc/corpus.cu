@@ -1,7 +1,7 @@
 // corpus.cu -- device-resident vector column: per-row exact magnitudes, screening norms, bf16 screen
 // copy, special-row list.  Data layout in HBM (DESIGN.md section 4):
 //   rows   [cap][dim]        f32|f64  master copy (exact re-rank reads it; the SIMT screen streams it)
-//   bf16   [cap][dim_pad]    bf16     screen copy, K-major rows = tcgen05 "B" operand via TMA
+//   bf16   [cap][dim_pad]    bf16     screen copy, K-major rows = wgmma "B" operand via TMA
 //   mag    [cap]             f64      sqrt(sum x^2), the reference's `magnitude()` arithmetic
 //   snorm  [cap]             f32      cosine: 1/|x|, euclid: |x|^2, NaN => row never screened in
 #include <algorithm>

@@ -31,7 +31,7 @@ void set_error(const char* fmt, ...);
     if (s__ != SDB_OK) return s__;     \
   } while (0)
 
-constexpr int TILE_ROWS = 256;    // screening tile = 256 corpus rows (one tcgen05 N=256 MMA tile)
+constexpr int TILE_ROWS = 256;    // screening tile = 256 corpus rows (one wgmma N=256 MMA tile)
 constexpr int PASS_RATIO = 8;     // default geometric threshold-refinement ratio (api.cu:pass_ratio picks per batch size)
 constexpr int SPECIAL_CAP = 1024; // rows with zero / non-finite norm handled by exact ranking
 
@@ -39,7 +39,7 @@ constexpr int SPECIAL_CAP = 1024; // rows with zero / non-finite norm handled by
 // Number::cmp on Floats (val/number.rs:620-633): -0.0 == 0.0, otherwise f64::total_cmp.
 // All bit manipulation is done on integers obtained through an opaque move: nvcc otherwise rewrites
 // `bits(d) | signbit` into fneg(fabs(d)), implements it with a DADD, and the DADD canonicalises NaNs --
-// which silently destroyed the sign/payload of NaN distances (found on B200, round 1).
+// which silently destroyed the sign/payload of NaN distances.
 __host__ __device__ inline uint64_t f64_bits(double d) {
   uint64_t b;
 #ifdef __CUDA_ARCH__
@@ -119,7 +119,7 @@ struct Comm;  // comm.cu: NCCL communicator attached to a context (nullptr = sin
 
 struct Ctx {
   int device = 0;
-  int sm_count = 148;
+  int sm_count = 132;
   cudaStream_t stream = nullptr;
   cudaStream_t stream2 = nullptr;      // odd ticket slots: batch i+1 runs here, so its screen overlaps batch i's tail
   cudaStream_t copy_stream = nullptr;  // host<->device copies of the asynchronous entry points

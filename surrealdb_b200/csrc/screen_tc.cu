@@ -1,58 +1,52 @@
-// screen_tc.cu -- K2: tcgen05 bf16 GEMM screen with a fused threshold-filter epilogue (sm_100a only).
+// screen_tc.cu -- K2: wgmma bf16 / int8 GEMM screen with a fused threshold-filter epilogue (sm_90a).
 //
-//   scores[q][x] = <q~, x~>  (bf16 operands, fp32 accumulation in TMEM), q = queries (M), x = corpus rows (N)
+//   scores[q][x] = <q~, x~>  (bf16 or int8 operands, fp32 / s32 accumulation in registers), q = queries (M),
+//   x = corpus rows (N)
 //
 // One CTA = one SM, persistent over work items (corpus tile of 256 rows) x (block of 128 queries):
-//   warp 0      TMA producer : cp.async.bulk.tensor 2-D tiles (SWIZZLE_128B) of A (128 x 64) and B (256 x 64)
-//                              into a 4-stage shared-memory ring, completion on mbarriers
-//   warp 1      MMA issuer   : one elected thread issues tcgen05.mma.cta_group::1.kind::f16 (M=128, N=256, K=16)
-//                              accumulating into one of two 256-column TMEM stages; tcgen05.commit frees the
-//                              smem stage / publishes the accumulator
-//   warps 2..9  epilogue     : tcgen05.ld the accumulator (thread = query, 256 columns = corpus rows), scale by
-//                              the row's screening norm, compare with the query's threshold tau and append the
-//                              rare survivors to the query's candidate list -- the 128 x 256 score tile is never
-//                              written to memory (at 1024 x 10M it would be 41 GB).
-//   warp 10     refiner      : (streaming mode) raises the thresholds WHILE the kernel runs.  Every survivor is also
-//                              counted (fire-and-forget RED) in its query's 256-bin score histogram in L2; the refiner
-//                              of CTA b owns the queries q = b (mod grid), reads their histograms, finds the bin in
-//                              which the count from the top reaches k -- a proof that the k-th best score seen so far
-//                              is at least that bin's lower edge -- and publishes tau = edge - margin.  The epilogue
-//                              threads re-read tau (ld.cg, L2) at every work item.  One launch therefore covers the
-//                              whole corpus: no per-pass launches, compactions or host round trips.
-// The epilogue of tile i overlaps the MMAs of tile i+1 through the two TMEM stages.
+//   warp 8          TMA producer : cp.async.bulk.tensor 2-D tiles (SWIZZLE_128B) of A (128 x 64) and B (256 x 64)
+//                                  into a 4-stage shared-memory ring, completion on mbarriers
+//   warpgroups 0, 1 consumers    : each issues wgmma.mma_async m64n256 (K = 16 bf16 / 32 int8 per instruction) for
+//                                  its 64 queries of the item, then filters its 64 x 256 accumulator straight from the
+//                                  registers: scale by the row's screening norm, compare with the query's threshold
+//                                  tau and append the rare survivors to the query's candidate lists -- the 128 x 256
+//                                  score tile is never written to memory (at 1024 x 10M it would be 41 GB).
+//   warp 9          refiner      : (streaming mode) raises the thresholds WHILE the kernel runs.  Every survivor is also
+//                                  counted (fire-and-forget RED) in its query's 256-bin score histogram in L2; the
+//                                  refiner of CTA b owns the queries q = b (mod grid), reads their histograms, finds the
+//                                  bin in which the count from the top reaches k -- a proof that the k-th best score
+//                                  seen so far is at least that bin's lower edge -- and publishes tau = edge - margin.
+//                                  The consumers re-read tau (ld.cg, L2) at every work item.  One launch therefore covers
+//                                  the whole corpus: no per-pass launches, compactions or host round trips.
+// The producer runs up to STAGES k-blocks ahead, so the loads of item i+1 overlap the epilogue of item i.
 //
 // Replaces, as the *screen*, the distance loop of KnnTopK::execute (exec/operators/knn_topk.rs:185-228);
 // exactness is restored by candidates.cu (f64 re-rank + error-bound proof) and exact.cu.
 #include <cuda.h>
+
+#include <type_traits>
 
 #include "internal.cuh"
 
 namespace sdb {
 
 namespace tc {
-constexpr uint32_t BLOCK_M = 128;   // queries per work item
+constexpr uint32_t BLOCK_M = 128;   // queries per work item (two warpgroups of 64)
 constexpr uint32_t BLOCK_N = 256;   // corpus rows per work item (= TILE_ROWS)
 constexpr uint32_t BLOCK_K = 64;    // bf16 elements per smem stage row = 128 bytes = one swizzle atom
-constexpr uint32_t UMMA_K = 16;
+constexpr uint32_t WG_M = 64;       // queries per consumer warpgroup (wgmma M)
 constexpr uint32_t STAGES = 4;
 constexpr uint32_t A_BYTES = BLOCK_M * BLOCK_K * 2;  // 16 KB
 constexpr uint32_t B_BYTES = BLOCK_N * BLOCK_K * 2;  // 32 KB
 constexpr uint32_t STAGE_BYTES = A_BYTES + B_BYTES;
-constexpr uint32_t ACC_STAGES = 2;
-constexpr uint32_t TMEM_COLS = 512;
-constexpr uint32_t EPI_WARPS = 8;             // two warps per TMEM lane quarter, each takes half the columns
-constexpr uint32_t REFINE_WARP = 2 + EPI_WARPS;  // warp 10
-constexpr uint32_t THREADS = 64 + EPI_WARPS * 32 + 32;
+constexpr uint32_t CONS_WARPS = 8;                 // two consumer warpgroups
+constexpr uint32_t PROD_WARP = CONS_WARPS;         // warp 8
+constexpr uint32_t THREADS = (CONS_WARPS + 2) * 32;
 constexpr uint32_t MAX_MBLOCKS = 16;           // queries per launch <= 2048 (the driver splits larger batches)
 constexpr uint32_t SUBCAP = 16;                // private candidate slots per (query, CTA, column half) and pass
-constexpr uint32_t SMEM_BYTES = STAGES * STAGE_BYTES + ACC_STAGES * BLOCK_N * 4 + 256 + MAX_MBLOCKS * 256 * 4 +
-                                EPI_WARPS * 32 * 4 /* survivor scratch */ + 1024;
+constexpr uint32_t SMEM_BYTES = STAGES * STAGE_BYTES + 2 * BLOCK_N * 4 + 256 + MAX_MBLOCKS * 256 * 4 + 1024;
 static_assert(BLOCK_N == TILE_ROWS, "screen tile must match the pass schedule tile");
-
-// instruction descriptor (cute::UMMA::InstrDescriptor bit layout): D=f32, A=B=bf16, both K-major
-constexpr uint32_t IDESC = (1u << 4) | (1u << 7) | (1u << 10) | ((BLOCK_N >> 3) << 17) | ((BLOCK_M >> 4) << 24);
-// kind::i8: D = s32 (c_format 2), A = B = signed 8-bit (format 1), K-major; UMMA_K = 32 (still 32 bytes per step)
-constexpr uint32_t IDESC_I8 = (2u << 4) | (1u << 7) | (1u << 10) | ((BLOCK_N >> 3) << 17) | ((BLOCK_M >> 4) << 24);
+static_assert(SMEM_BYTES <= 227 * 1024, "screen CTA must fit the shared memory of one SM");
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 
@@ -87,120 +81,101 @@ __device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* map
       ::"r"(dst), "l"(map), "r"(c0), "r"(c1), "r"(bar)
       : "memory");
 }
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void umma_i8(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc, uint32_t acc) {
+
+// ---- wgmma (one warpgroup, M=64 N=256, both operands K-major in shared memory) ---------------------------------------
+// Accumulator layout (PTX "wgmma register fragment", m64nNk16): register d[4j + 2i + c] of lane l in warp w of the
+// warpgroup holds row 16w + l/4 + 8i, column 8j + 2(l%4) + c.
+#define SDB_WG_REGS                                                                                   \
+  "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "                           \
+  "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "                  \
+  "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "                  \
+  "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, "                  \
+  "%64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, "                  \
+  "%80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, "                  \
+  "%96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, "      \
+  "%112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127}"
+#define SDB_WG8(C, i) C(d[i]), C(d[i + 1]), C(d[i + 2]), C(d[i + 3]), C(d[i + 4]), C(d[i + 5]), C(d[i + 6]), C(d[i + 7])
+#define SDB_WG128(C)                                                                                     \
+  SDB_WG8(C, 0), SDB_WG8(C, 8), SDB_WG8(C, 16), SDB_WG8(C, 24), SDB_WG8(C, 32), SDB_WG8(C, 40), SDB_WG8(C, 48), \
+      SDB_WG8(C, 56), SDB_WG8(C, 64), SDB_WG8(C, 72), SDB_WG8(C, 80), SDB_WG8(C, 88), SDB_WG8(C, 96),             \
+      SDB_WG8(C, 104), SDB_WG8(C, 112), SDB_WG8(C, 120)
+
+__device__ __forceinline__ void wgmma_bf16(float (&d)[128], uint64_t a_desc, uint64_t b_desc, uint32_t acc) {
   asm volatile(
       "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::i8 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(acc)
-      : "memory");
+      "setp.ne.b32 p, %130, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n256k16.f32.bf16.bf16 " SDB_WG_REGS ", %128, %129, p, 1, 1, 0, 0;\n\t}"
+      : SDB_WG128("+f")
+      : "l"(a_desc), "l"(b_desc), "r"(acc));
 }
-__device__ __forceinline__ void umma_bf16(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc, uint32_t acc) {
+__device__ __forceinline__ void wgmma_i8(uint32_t (&d)[128], uint64_t a_desc, uint64_t b_desc, uint32_t acc) {
   asm volatile(
       "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(acc)
-      : "memory");
+      "setp.ne.b32 p, %130, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n256k32.s32.s8.s8 " SDB_WG_REGS ", %128, %129, p;\n\t}"
+      : SDB_WG128("+r")
+      : "l"(a_desc), "l"(b_desc), "r"(acc));
 }
-// shared-memory matrix descriptor: K-major, SWIZZLE_128B, 8-row groups 1024 B apart (cute::UMMA::SmemDescriptor)
+// keeps the compiler from moving accumulator reads / writes across the asynchronous wgmma window
+__device__ __forceinline__ void acc_fence(float (&d)[128]) {
+#pragma unroll
+  for (int i = 0; i < 128; i++) asm volatile("" : "+f"(d[i])::"memory");
+}
+__device__ __forceinline__ void acc_fence(uint32_t (&d)[128]) {
+#pragma unroll
+  for (int i = 0; i < 128; i++) asm volatile("" : "+r"(d[i])::"memory");
+}
+#undef SDB_WG128
+#undef SDB_WG8
+#undef SDB_WG_REGS
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() {
+  asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
+}
+// shared-memory matrix descriptor (Hopper GMMA): K-major, SWIZZLE_128B, 8-row groups 1024 B apart
 __device__ __forceinline__ uint64_t make_desc(uint32_t saddr) {
   uint64_t d = 0;
   d |= (uint64_t)((saddr >> 4) & 0x3FFF);  // start address
   d |= (uint64_t)1 << 16;                  // leading byte offset (unused for swizzled K-major; canonical 1)
   d |= (uint64_t)(1024 >> 4) << 32;        // stride byte offset: next 8-row core-matrix group
-  d |= (uint64_t)1 << 46;                  // descriptor version (Blackwell)
-  d |= (uint64_t)2 << 61;                  // SWIZZLE_128B
+  d |= (uint64_t)1 << 62;                  // SWIZZLE_128B
   return d;
 }
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&v)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-        "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]),
-        "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]),
-        "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-      : "r"(taddr)
-      : "memory");
-}
 
-// ---- survivors: warp-cooperative, control-flow uniform --------------------------------------------------------------
-// A chunk is 32 columns (corpus rows) of ONE query per lane.  When some lane's chunk maximum reaches its threshold the
-// whole warp handles that lane's chunk together: the lane publishes its 32 values to a 128-byte scratch line, every
-// lane picks up one column, compares it with the owner's threshold, and the survivors (ballot) are written side by
-// side into the owner query's private sub-list (position = popcount prefix), each also counted in the query's
-// histogram (streaming mode; a fire-and-forget RED).  No per-lane divergent scan, no calls: an event costs ~40 warp
-// instructions whatever the number of survivors -- the per-lane version cost ~130 per survivor, and since the
-// accumulator stage is released only when the slowest of the 8 epilogue warps is done, that doubled the time of a
-// short (1.25M-row) launch.
-// vals: this lane's 32 values (int accumulators or scaled float scores as bits); all 32 lanes must call.
-template <bool INT8, int MODE>
-__device__ __forceinline__ void warp_survivors(uint32_t hits, const uint32_t (&vals)[32], uint32_t* scratch /* [32] per warp */,
-                                               uint32_t lane, float my_tau, int tau_i, float2 my_hp, uint32_t q_base,
-                                               uint32_t row_first, const float* __restrict__ snorm, Cand* __restrict__ cand,
-                                               uint32_t* __restrict__ cand_cnt, uint32_t cap, Cand* __restrict__ sub,
-                                               uint32_t n_slots, uint32_t slot, uint32_t* s_cnt_warp /* [32] */,
-                                               uint32_t* hist) {
-  while (hits) {
-    const uint32_t L = __ffs(hits) - 1;
-    hits &= hits - 1;
-    if (lane == L) {
-#pragma unroll
-      for (int i = 0; i < 32; i += 4)
-        *reinterpret_cast<uint4*>(scratch + i) = make_uint4(vals[i], vals[i + 1], vals[i + 2], vals[i + 3]);
-    }
-    __syncwarp();
-    const uint32_t xb = scratch[lane];  // column `lane` of the owner's chunk
-    const float tau_f = __shfl_sync(0xffffffffu, my_tau, L);
-    const int tau_n = __shfl_sync(0xffffffffu, tau_i, L);
-    const float hp_lo = __shfl_sync(0xffffffffu, my_hp.x, L);  // the owner query's histogram geometry (streaming mode)
-    const float hp_inv = __shfl_sync(0xffffffffu, my_hp.y, L);
-    const uint32_t qL = q_base + L;
-    const uint32_t r = row_first + lane;
-    bool surv = INT8 ? ((int)xb >= tau_n) : (__uint_as_float(xb) >= tau_f);  // NaN scores never pass
-    if (INT8 && surv && (int)xb == 0) {
-      // invalid rows (skipped / special / padding) are all-zero in the int8 copy and score exactly 0: only a zero
-      // score needs the look-up of the row's screening norm
-      const float sn = __ldg(snorm + r);
-      surv = sn == sn;
-    }
-    const uint32_t smask = __ballot_sync(0xffffffffu, surv);
-    if (smask) {  // uniform
-      const uint32_t base = s_cnt_warp[L];  // broadcast read: appends of this (query, CTA, column half) so far
-      if (surv) {
-        const uint32_t pos = base + __popc(smask & ((1u << lane) - 1u));
-        const float score = INT8 ? __int2float_rn((int)xb) : __uint_as_float(xb);
-        const uint2 cd = make_uint2(__float_as_uint(score), r);
-        if (pos < SUBCAP) {
-          *reinterpret_cast<uint2*>(sub + ((size_t)qL * n_slots + slot) * SUBCAP + pos) = cd;
-        } else {  // private slots full: spill to the query's shared list
-          const uint32_t p2 = atomicAdd(cand_cnt + qL, 1u);
-          if (p2 < cap) *reinterpret_cast<uint2*>(cand + (size_t)qL * cap + p2) = cd;
-        }
-        if (MODE == 2) {
-          HistParam hp;
-          hp.lo = hp_lo;
-          hp.inv_w0 = hp_inv;
-          hp.w0 = 0.f;
-          hp.margin = 0.f;
-          atomicAdd(hist + (size_t)qL * HIST_BINS + hist_bin(hp, score), 1u);
-        }
-      }
-      __syncwarp();
-      if (lane == 0) s_cnt_warp[L] = base + __popc(smask);
-    }
-    __syncwarp();  // scratch and counter are reused by the next event
+// one survivor (query q = mb * BLOCK_M + row, corpus column col of the tile): appended to the (query, CTA, column
+// half) private sub-list, spilling to the query's shared list when that is full; streaming mode also counts it in the
+// query's histogram (a fire-and-forget RED)
+template <int MODE>
+__device__ __forceinline__ void append_survivor(float score, uint32_t q, uint32_t row, uint32_t col, uint32_t row0,
+                                                float2 hpv, uint32_t* s_cnt_mb, Cand* __restrict__ cand,
+                                                uint32_t* __restrict__ cand_cnt, uint32_t cap, Cand* __restrict__ sub,
+                                                uint32_t* hist) {
+  const uint32_t half = col >> 7;
+  const uint32_t pos = atomicAdd(s_cnt_mb + half * BLOCK_M + row, 1u);
+  const uint2 cd = make_uint2(__float_as_uint(score), row0 + col);
+  const uint32_t n_slots = gridDim.x * 2;
+  if (pos < SUBCAP) {
+    *reinterpret_cast<uint2*>(sub + ((size_t)q * n_slots + blockIdx.x * 2 + half) * SUBCAP + pos) = cd;
+  } else {  // private slots full: spill to the query's shared list
+    const uint32_t p2 = atomicAdd(cand_cnt + q, 1u);
+    if (p2 < cap) *reinterpret_cast<uint2*>(cand + (size_t)q * cap + p2) = cd;
+  }
+  if (MODE == 2) {
+    HistParam hp;
+    hp.lo = hpv.x;
+    hp.inv_w0 = hpv.y;
+    hp.w0 = 0.f;
+    hp.margin = 0.f;
+    atomicAdd(hist + (size_t)q * HIST_BINS + hist_bin(hp, score), 1u);
   }
 }
 
 // MODE 0: pass 0 -- every score of the pass's tiles goes to a fixed slot of the query's main list (tau = -inf)
 // MODE 1: threshold pass -- survivors of a fixed tau (legacy multi-pass schedule)
 // MODE 2: streaming pass -- tau is re-read at every work item and raised by the refiner warps while the kernel runs
-// MODE 3: probe -- nothing is appended; every epilogue thread writes the maximum of each 32-column chunk it sees
+// MODE 3: probe -- nothing is appended; the maximum of every 32-column chunk of every query is written
 //         (probe[q][tile * 8 + chunk]).  The chunk maxima belong to DISJOINT row sets, so the k-th largest of them is a
 //         lower bound of the k-th best score of the corpus: the seed of the streaming pass's thresholds, at the cost
 //         of one round of MMAs and no candidate traffic.
@@ -217,47 +192,30 @@ screen_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constan
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* smem_a = smem;                                  // [STAGES][128][64] bf16
   uint8_t* smem_b = smem + STAGES * A_BYTES;               // [STAGES][256][64] bf16
-  float* s_snorm = reinterpret_cast<float*>(smem + STAGES * STAGE_BYTES);  // [ACC_STAGES][256]
-  uint64_t* bars = reinterpret_cast<uint64_t*>(s_snorm + ACC_STAGES * BLOCK_N);
+  float* s_snorm = reinterpret_cast<float*>(smem + STAGES * STAGE_BYTES);  // [2][256]
+  uint64_t* bars = reinterpret_cast<uint64_t*>(s_snorm + 2 * BLOCK_N);
   uint64_t* full_bar = bars;                      // [STAGES]
   uint64_t* empty_bar = bars + STAGES;            // [STAGES]
-  uint64_t* tfull_bar = bars + 2 * STAGES;        // [ACC_STAGES]
-  uint64_t* tempty_bar = bars + 2 * STAGES + ACC_STAGES;  // [ACC_STAGES]
-  uint32_t* s_tmem = reinterpret_cast<uint32_t*>(bars + 2 * STAGES + 2 * ACC_STAGES);
-  uint32_t* s_done = s_tmem + 1;  // epilogue warps that have finished (the refiner's exit condition)
-  uint32_t* s_cnt = s_tmem + 4;   // [n_mblocks][256] private append counters of the epilogue threads
-  uint32_t* s_scratch = s_cnt + MAX_MBLOCKS * 256;  // [EPI_WARPS][32] one chunk of one lane, for the survivor hand-over
+  uint32_t* s_done = reinterpret_cast<uint32_t*>(bars + 2 * STAGES);  // consumer warps that have finished
+  uint32_t* s_cnt = reinterpret_cast<uint32_t*>(reinterpret_cast<uint8_t*>(bars) + 256);  // [n_mblocks][2][128]
 
   const uint32_t warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const uint32_t n_items = pass.count * n_mblocks;
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     asm volatile("prefetch.tensormap [%0];" ::"l"(&map_a) : "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(&map_b) : "memory");
     for (uint32_t s = 0; s < STAGES; s++) {
       mbar_init(smem_u32(&full_bar[s]), 1);
-      mbar_init(smem_u32(&empty_bar[s]), 1);
-    }
-    for (uint32_t a = 0; a < ACC_STAGES; a++) {
-      mbar_init(smem_u32(&tfull_bar[a]), 1);
-      mbar_init(smem_u32(&tempty_bar[a]), EPI_WARPS);  // one arrive per epilogue warp
+      mbar_init(smem_u32(&empty_bar[s]), CONS_WARPS);  // one arrive per consumer warp
     }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     *s_done = 0;
   }
   for (uint32_t i = threadIdx.x; i < n_mblocks * 256; i += blockDim.x) s_cnt[i] = 0;
-  if (warp == 1) {  // TMEM allocation (whole warp), address lands in shared memory
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(s_tmem)),
-                 "n"(TMEM_COLS)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem_base = *s_tmem;
 
-  if (warp == 0) {
+  if (warp == PROD_WARP) {
     // ===================== TMA producer =====================
     if (lane == 0) {
       uint32_t it = 0;
@@ -275,193 +233,179 @@ screen_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constan
       }
     }
     __syncwarp();
-  } else if (warp == 1) {
-    // ===================== MMA issuer =====================
-    if (lane == 0) {
-      uint32_t it = 0, j = 0;
-      for (uint32_t w = blockIdx.x; w < n_items; w += gridDim.x, j++) {
-        const uint32_t a = j % ACC_STAGES, pa = (j / ACC_STAGES) & 1;
-        mbar_wait(smem_u32(&tempty_bar[a]), pa ^ 1);  // epilogue has drained this accumulator stage
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        const uint32_t d_tmem = tmem_base + a * BLOCK_N;
-        for (uint32_t kb = 0; kb < k_blocks; kb++, it++) {
-          const uint32_t s = it % STAGES, ph = (it / STAGES) & 1;
-          mbar_wait(smem_u32(&full_bar[s]), ph);
-          asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-          const uint64_t da = make_desc(smem_u32(smem_a + s * A_BYTES));
-          const uint64_t db = make_desc(smem_u32(smem_b + s * B_BYTES));
-#pragma unroll
-          for (uint32_t k = 0; k < BLOCK_K / UMMA_K; k++) {
-            // advance 32 bytes (16 bf16) inside the 128-byte swizzle atom: +2 in the (>>4) start-address field
-            if (INT8) umma_i8(d_tmem, da + 2 * k, db + 2 * k, IDESC_I8, (kb | k) != 0);
-            else umma_bf16(d_tmem, da + 2 * k, db + 2 * k, IDESC, (kb | k) != 0);
-          }
-          umma_commit(smem_u32(&empty_bar[s]));  // smem stage reusable once these MMAs retire
-        }
-        umma_commit(smem_u32(&tfull_bar[a]));  // accumulator complete
-      }
-    }
-    __syncwarp();
-  } else if (warp < REFINE_WARP) {
-    // ===================== epilogue (8 warps; thread = query row, warp pair splits the 256 columns) ==========
-    const uint32_t wq = warp & 3;                 // TMEM lane quarter this warp may access
-    const uint32_t half = (warp - 2) >> 2;        // 0: columns 0..127, 1: columns 128..255
-    const uint32_t row_in_tile = wq * 32 + lane;
-    const uint32_t et = threadIdx.x - 64;         // 0..255
+  } else if (warp < CONS_WARPS) {
+    // ===================== consumers (2 warpgroups; warpgroup g = queries 64g..64g+63 of the item) ==========
+    const uint32_t ct = threadIdx.x;              // 0..255
+    const uint32_t g = warp >> 2;
+    const uint32_t row_base = g * WG_M + (warp & 3) * 16 + (lane >> 2);  // rows row_base and row_base + 8
+    const uint32_t col_l = 2 * (lane & 3);        // this lane's first column in every group of 8
     constexpr bool pass0 = MODE == 0;             // pass 0: tau = -inf everywhere, positions are deterministic
-    const uint32_t cbase = half * (BLOCK_N / 2);
-    uint32_t j = 0;
-    // the threshold of the first item; later items prefetch theirs while the current one is processed
-    uint32_t w = blockIdx.x;
-    float next_tau = __int_as_float(0x7f800000);
-    float2 next_hp = make_float2(0.f, 0.f);  // streaming mode: (lo, 1/w0) of the query's histogram
-    if (w < n_items) {
-      const uint32_t q0 = item_mb(w, n_mblocks) * BLOCK_M + row_in_tile;
-      if (q0 < nq) {
-        next_tau = __ldcg(tau + q0);
-        if (MODE == 2) next_hp = __ldg(reinterpret_cast<const float2*>(hparam + q0));
-      }
-    }
-    for (; w < n_items; w += gridDim.x, j++) {
+    using Acc = typename std::conditional<INT8, uint32_t, float>::type;
+    Acc acc[128];
+    uint32_t it = 0, j = 0;
+    for (uint32_t w = blockIdx.x; w < n_items; w += gridDim.x, j++) {
       const uint32_t tidx = w / n_mblocks;
       const uint32_t tile = pass_tile(pass, tidx);
       const uint32_t mb = item_mb(w, n_mblocks);
-      const uint32_t a = j % ACC_STAGES, pa = (j / ACC_STAGES) & 1;
-      const uint32_t q = mb * BLOCK_M + row_in_tile;
-      const float my_tau = next_tau;
-      const float2 my_hp = next_hp;
-      {  // prefetch the next item's threshold (a global load whose latency would otherwise sit in front of the wait)
-        const uint32_t wn = w + gridDim.x;
-        next_tau = __int_as_float(0x7f800000);
-        if (wn < n_items) {
-          const uint32_t qn = item_mb(wn, n_mblocks) * BLOCK_M + row_in_tile;
-          if (qn < nq) {
-            next_tau = __ldcg(tau + qn);  // L2: sees the refiners' updates
-            if (MODE == 2) next_hp = __ldg(reinterpret_cast<const float2*>(hparam + qn));
-          }
+      const uint32_t row0 = tile * BLOCK_N;
+      // thresholds of this thread's two queries (L2: sees the refiners' updates); the loads complete under the MMAs
+      float my_tau[2];
+      float2 my_hp[2];
+#pragma unroll
+      for (int i = 0; i < 2; i++) {
+        const uint32_t q = mb * BLOCK_M + row_base + 8 * i;
+        my_tau[i] = __int_as_float(0x7f800000);
+        my_hp[i] = make_float2(0.f, 0.f);
+        if (q < nq) {
+          my_tau[i] = __ldcg(tau + q);
+          if (MODE == 2) my_hp[i] = __ldg(reinterpret_cast<const float2*>(hparam + q));
         }
       }
-      const size_t row0 = (size_t)tile * BLOCK_N;
-      float* sn = s_snorm + a * BLOCK_N;
+      float* sn = s_snorm + (j & 1) * BLOCK_N;
       if (!INT8 || MODE == 3) {
-        // stage this tile's screening norms (safe: every epilogue thread passed the named barrier of item j-1
-        // only after finishing item j-2, the previous user of s_snorm[a])
-        sn[et] = __ldg(snorm + row0 + et);
+        // stage this tile's screening norms (safe: every consumer thread passed the named barrier of item j-1 only
+        // after finishing item j-2, the previous user of this buffer)
+        sn[ct] = __ldg(snorm + row0 + ct);
         asm volatile("bar.sync 1, 256;" ::: "memory");
       }
-      // integer threshold for the int8 screen: acc >= tau  <=>  acc >= ceil(tau)
-      int tau_i = 0x7fffffff;
-      if (INT8) {
-        const float ct = ceilf(my_tau);
-        tau_i = ct >= 2147483520.f ? 0x7fffffff : (ct <= -2147483520.f ? (int)0x80000000 : (int)ct);
+
+      // ---- MMAs: one k-block in flight behind the one being issued ----
+      const uint32_t a_off = g * (WG_M * 128);  // this warpgroup's 64 rows of the A stage
+      for (uint32_t kb = 0; kb < k_blocks; kb++, it++) {
+        const uint32_t s = it % STAGES, ph = (it / STAGES) & 1;
+        mbar_wait(smem_u32(&full_bar[s]), ph);
+        const uint64_t da = make_desc(smem_u32(smem_a + s * A_BYTES + a_off));
+        const uint64_t db = make_desc(smem_u32(smem_b + s * B_BYTES));
+        wgmma_fence();
+        acc_fence(acc);
+#pragma unroll
+        for (uint32_t kk = 0; kk < 4; kk++) {
+          // advance 32 bytes (16 bf16 / 32 int8) inside the 128-byte swizzle atom: +2 in the (>>4) address field
+          if constexpr (INT8) wgmma_i8(acc, da + 2 * kk, db + 2 * kk, (kb | kk) != 0);
+          else wgmma_bf16(acc, da + 2 * kk, db + 2 * kk, (kb | kk) != 0);
+        }
+        wgmma_commit();
+        acc_fence(acc);
+        if (kb > 0) {
+          wgmma_wait<1>();  // the previous k-block's MMAs have read their stage
+          if (lane == 0) mbar_arrive(smem_u32(&empty_bar[(it - 1) % STAGES]));
+        }
       }
-      mbar_wait(smem_u32(&tfull_bar[a]), pa);
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-      const uint32_t taddr = tmem_base + ((wq * 32) << 16) + a * BLOCK_N + cbase;
-      Cand* my_cand = cand + (size_t)q * cap;
-      const uint32_t n_slots = gridDim.x * 2;
-      const uint32_t my_cnt = smem_u32(s_cnt + mb * 256 + et);
-      Cand* my_sub = sub + ((size_t)q * n_slots + blockIdx.x * 2 + half) * SUBCAP;
-      {
-      uint32_t va[32], vb[32];
-      tmem_ld32(taddr, va);
+      wgmma_wait<0>();
+      acc_fence(acc);
+      if (lane == 0) mbar_arrive(smem_u32(&empty_bar[(it - 1) % STAGES]));
+
+      // ---- epilogue straight from the registers ----
+      if constexpr (!INT8) {
 #pragma unroll
-      for (uint32_t cc = 0; cc < BLOCK_N / 2 / 32; cc++) {
-        const uint32_t c0 = cc * 32;
-        uint32_t(&v)[32] = (cc & 1) ? vb : va;
-        asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-        if (cc + 1 < BLOCK_N / 2 / 32) tmem_ld32(taddr + c0 + 32, (cc & 1) ? va : vb);  // next chunk in flight
-        if (INT8) {
-          int gm[4];  // maxima of the four groups of 8 columns: the slow path only scans groups that hold a survivor
+        for (int jj = 0; jj < 32; jj++) {
+          const float2 n2 = *reinterpret_cast<const float2*>(sn + 8 * jj + col_l);
 #pragma unroll
-          for (int g = 0; g < 4; g++) {
-            gm[g] = (int)v[8 * g];
-#pragma unroll
-            for (int i = 1; i < 8; i++) gm[g] = max(gm[g], (int)v[8 * g + i]);
+          for (int i = 0; i < 2; i++) {
+            float& a0 = acc[4 * jj + 2 * i];
+            float& a1 = acc[4 * jj + 2 * i + 1];
+            a0 = COSINE ? a0 * n2.x : fmaf(2.f, a0, -n2.x);
+            a1 = COSINE ? a1 * n2.y : fmaf(2.f, a1, -n2.y);
           }
-          const int m = max(max(gm[0], gm[1]), max(gm[2], gm[3]));
-          if (MODE == 3) {
-            // invalid rows (NaN screening norm) score 0 in the integer screen: they must not pose as a real score
-            int pm = (int)0x80000000;
+        }
+      }
 #pragma unroll
-            for (int i = 0; i < 32; i++) {
-              const float snv = sn[cbase + c0 + i];
-              if (snv == snv) pm = max(pm, (int)v[i]);
-            }
-            if (q < nq)
-              probe[(size_t)q * probe_stride + tidx * 8 + half * 4 + cc] =
-                  pm == (int)0x80000000 ? __int_as_float(0xff800000) : __int2float_rd(pm);
-          } else if (pass0) {
-            if (q < nq) {
+      for (int i = 0; i < 2; i++) {
+        const uint32_t row = row_base + 8 * i;
+        const uint32_t q = mb * BLOCK_M + row;
+        if (MODE == 3) {
+          // maximum of every 32-column chunk: 8 values per lane, the quad of lanes sharing the row covers the chunk
 #pragma unroll
-              for (int i = 0; i < 32; i++) {
-                Cand cd;
-                cd.score = __int2float_rn((int)v[i]);
-                cd.row = (uint32_t)(row0 + cbase + c0 + i);
-                my_cand[(size_t)tidx * BLOCK_N + cbase + c0 + i] = cd;
+          for (int h = 0; h < 8; h++) {
+            float m = __int_as_float(0xff800000);  // -inf: no valid row in the chunk
+#pragma unroll
+            for (int jj = 4 * h; jj < 4 * h + 4; jj++) {
+#pragma unroll
+              for (int c = 0; c < 2; c++) {
+                if constexpr (INT8) {
+                  // invalid rows (NaN screening norm) score 0 in the integer screen: they must not pose as a score
+                  const float snv = sn[8 * jj + col_l + c];
+                  if (snv == snv) m = fmaxf(m, __int2float_rd((int)acc[4 * jj + 2 * i + c]));
+                } else {
+                  m = fmaxf(m, acc[4 * jj + 2 * i + c]);  // fmaxf drops NaNs
+                }
               }
             }
-          } else {
-            const uint32_t hits = __ballot_sync(0xffffffffu, m >= tau_i);
-            if (hits)  // rare, uniform across the warp
-              warp_survivors<true, MODE>(hits, v, s_scratch + (warp - 2) * 32, lane, my_tau, tau_i, my_hp,
-                                         mb * BLOCK_M + wq * 32, (uint32_t)(row0 + cbase + c0), snorm, cand, cand_cnt, cap,
-                                         sub, gridDim.x * 2, blockIdx.x * 2 + half, s_cnt + mb * 256 + (et - lane), hist);
+            m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 1));
+            m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 2));
+            if ((lane & 3) == 0 && q < nq) probe[(size_t)q * probe_stride + tidx * 8 + h] = m;
+          }
+        } else if (pass0) {
+          if (q < nq) {  // every (finite or NaN) score goes to its fixed slot; compaction drops the NaNs
+            Cand* my_cand = cand + (size_t)q * cap + (size_t)tidx * BLOCK_N;
+#pragma unroll
+            for (int jj = 0; jj < 32; jj++) {
+              const uint32_t col = 8 * jj + col_l;
+              float s0, s1;
+              if constexpr (INT8) {
+                s0 = __int2float_rn((int)acc[4 * jj + 2 * i]);
+                s1 = __int2float_rn((int)acc[4 * jj + 2 * i + 1]);
+              } else {
+                s0 = acc[4 * jj + 2 * i];
+                s1 = acc[4 * jj + 2 * i + 1];
+              }
+              *reinterpret_cast<uint2*>(my_cand + col) = make_uint2(__float_as_uint(s0), row0 + col);
+              *reinterpret_cast<uint2*>(my_cand + col + 1) = make_uint2(__float_as_uint(s1), row0 + col + 1);
+            }
           }
         } else {
-          float sc[32];
-          float gmf[4];
+          // survivors are rare: one max over the lane's 64 values decides whether the lane scans them
+          uint32_t* s_cnt_mb = s_cnt + mb * 256;
+          if constexpr (INT8) {
+            // integer threshold: acc >= tau  <=>  acc >= ceil(tau)
+            const float ct_ = ceilf(my_tau[i]);
+            const int tau_i = ct_ >= 2147483520.f ? 0x7fffffff : (ct_ <= -2147483520.f ? (int)0x80000000 : (int)ct_);
+            int m = (int)0x80000000;
 #pragma unroll
-          for (int g = 0; g < 4; g++) gmf[g] = __int_as_float(0xff800000);
+            for (int jj = 0; jj < 32; jj++) m = max(m, max((int)acc[4 * jj + 2 * i], (int)acc[4 * jj + 2 * i + 1]));
+            if (m >= tau_i) {
 #pragma unroll
-          for (int i = 0; i < 32; i += 4) {
-            const float4 n4 = *reinterpret_cast<const float4*>(sn + cbase + c0 + i);
-            sc[i + 0] = COSINE ? __uint_as_float(v[i + 0]) * n4.x : fmaf(2.f, __uint_as_float(v[i + 0]), -n4.x);
-            sc[i + 1] = COSINE ? __uint_as_float(v[i + 1]) * n4.y : fmaf(2.f, __uint_as_float(v[i + 1]), -n4.y);
-            sc[i + 2] = COSINE ? __uint_as_float(v[i + 2]) * n4.z : fmaf(2.f, __uint_as_float(v[i + 2]), -n4.z);
-            sc[i + 3] = COSINE ? __uint_as_float(v[i + 3]) * n4.w : fmaf(2.f, __uint_as_float(v[i + 3]), -n4.w);
-            gmf[i >> 3] = fmaxf(gmf[i >> 3], fmaxf(fmaxf(sc[i + 0], sc[i + 1]), fmaxf(sc[i + 2], sc[i + 3])));  // fmaxf drops NaNs
-          }
-          const float m = fmaxf(fmaxf(gmf[0], gmf[1]), fmaxf(gmf[2], gmf[3]));
-          if (MODE == 3) {
-            if (q < nq) probe[(size_t)q * probe_stride + tidx * 8 + half * 4 + cc] = m;  // -inf: no valid row in the chunk
-          } else if (pass0) {
-            if (q < nq) {  // every (finite or NaN) score goes to its fixed slot; compaction drops the NaNs
+              for (int jj = 0; jj < 32; jj++) {
 #pragma unroll
-              for (int i = 0; i < 32; i++) {
-                Cand cd;
-                cd.score = sc[i];
-                cd.row = (uint32_t)(row0 + cbase + c0 + i);
-                my_cand[(size_t)tidx * BLOCK_N + cbase + c0 + i] = cd;
+                for (int c = 0; c < 2; c++) {
+                  const int v = (int)acc[4 * jj + 2 * i + c];
+                  const uint32_t col = 8 * jj + col_l + c;
+                  // invalid rows (skipped / special / padding) are all-zero in the int8 copy and score exactly 0:
+                  // only a zero score needs the look-up of the row's screening norm
+                  if (v >= tau_i && (v != 0 || __ldg(snorm + row0 + col) == __ldg(snorm + row0 + col)))
+                    append_survivor<MODE>(__int2float_rn(v), q, row, col, row0, my_hp[i], s_cnt_mb, cand, cand_cnt,
+                                          cap, sub, hist);
+                }
               }
             }
           } else {
-            const uint32_t hits = __ballot_sync(0xffffffffu, m >= my_tau);
-            if (hits) {  // rare, uniform across the warp
-              uint32_t sb[32];
+            float m = __int_as_float(0xff800000);
 #pragma unroll
-              for (int i = 0; i < 32; i++) sb[i] = __float_as_uint(sc[i]);
-              warp_survivors<false, MODE>(hits, sb, s_scratch + (warp - 2) * 32, lane, my_tau, 0, my_hp,
-                                          mb * BLOCK_M + wq * 32, (uint32_t)(row0 + cbase + c0), snorm, cand, cand_cnt, cap,
-                                          sub, gridDim.x * 2, blockIdx.x * 2 + half, s_cnt + mb * 256 + (et - lane), hist);
+            for (int jj = 0; jj < 32; jj++) m = fmaxf(m, fmaxf(acc[4 * jj + 2 * i], acc[4 * jj + 2 * i + 1]));
+            if (m >= my_tau[i]) {
+#pragma unroll
+              for (int jj = 0; jj < 32; jj++) {
+#pragma unroll
+                for (int c = 0; c < 2; c++) {
+                  const float v = acc[4 * jj + 2 * i + c];
+                  if (v >= my_tau[i])  // NaN scores never pass
+                    append_survivor<MODE>(v, q, row, 8 * jj + col_l + c, row0, my_hp[i], s_cnt_mb, cand, cand_cnt,
+                                          cap, sub, hist);
+                }
+              }
             }
           }
         }
       }
-      }
-      asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-      __syncwarp();
-      if (lane == 0) mbar_arrive(smem_u32(&tempty_bar[a]));
     }
-    // publish the private append counters: slot (CTA, column half) of every query this thread served
+    // publish the private append counters: slot (CTA, column half) of every query
     if (MODE == 1 || MODE == 2) {
+      asm volatile("bar.sync 1, 256;" ::: "memory");
       const uint32_t n_slots = gridDim.x * 2;
+      const uint32_t half = ct / BLOCK_M, row = ct % BLOCK_M;
       for (uint32_t mb = 0; mb < n_mblocks; mb++) {
-        const uint32_t qq = mb * BLOCK_M + row_in_tile;
-        if (qq < nq) {
-          const uint32_t cnt = s_cnt[mb * 256 + et];
-          sub_cnt[(size_t)qq * n_slots + blockIdx.x * 2 + half] = cnt;
-        }
+        const uint32_t qq = mb * BLOCK_M + row;
+        if (qq < nq) sub_cnt[(size_t)qq * n_slots + blockIdx.x * 2 + half] = s_cnt[mb * 256 + half * BLOCK_M + row];
       }
     }
     __syncwarp();
@@ -476,7 +420,7 @@ screen_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constan
       float my_tau = __int_as_float(0xff800000);  // lane j: the threshold last published for owned query j
       if (lane < n_own) my_tau = __ldcg(tau + blockIdx.x + lane * stride);
       uint32_t sleep_ns = sleep_min_ns;
-      while (*done < EPI_WARPS) {
+      while (*done < CONS_WARPS) {
         bool any = false;
         for (uint32_t j = 0; j < n_own; j++) {
           const uint32_t q = blockIdx.x + j * stride;
@@ -531,9 +475,6 @@ screen_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constan
     }
   }
   __syncthreads();
-  if (warp == 1) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "n"(TMEM_COLS) : "memory");
-  }
 }
 }  // namespace tc
 
@@ -592,7 +533,7 @@ sdb_status screen_tc_pass(Corpus* c, uint32_t nq, uint32_t k, const PassDesc& p,
   if (p.count == 0) return SDB_OK;
   Ctx* ctx = c->ctx;
   if (int8 ? (!c->d_i8 || c->metric != SDB_COSINE) : !c->d_bf16) {
-    set_error("tcgen05 screen: the %s screen copy is not available for this corpus", int8 ? "int8 (cosine only)" : "bf16");
+    set_error("tensor-core screen: the %s screen copy is not available for this corpus", int8 ? "int8 (cosine only)" : "bf16");
     return SDB_EUNSUPPORTED;
   }
   const uint64_t n_pad = (c->n + TILE_ROWS - 1) / TILE_ROWS * TILE_ROWS;

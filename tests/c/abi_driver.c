@@ -1,5 +1,5 @@
 /* Plain-C driver of the drop-in boundary (SURVEY 8b "what calls it"): proves include/sdbgpu.h is C (not C++),
- * that a C caller links against libsdbgpu.so, and -- when a B200 is present -- runs one brute-force KNN, one graph
+ * that a C caller links against libsdbgpu.so, and -- when an H100 is present -- runs one brute-force KNN, one graph
  * hop and one staged HNSW load through the ABI exactly as the Rust shim of INTEGRATION.md would.
  * Exit code 0 = ok; prints "NO_GPU <message>" and exits 0 when the library refuses to start without a device
  * (that refusal is the behaviour under test on CPU-only machines). */

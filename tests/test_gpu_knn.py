@@ -191,7 +191,7 @@ def test_full_size_c2_sample_queries(ctx):
 
 
 def test_large_batches_are_chunked_correctly(ctx):
-    # batches above 2048 queries are split over several tcgen05 launches (private sub-list slots per chunk)
+    # batches above 2048 queries are split over several tensor-core screen launches (private sub-list slots per chunk)
     rng = np.random.default_rng(21)
     corpus = rng.uniform(-1, 1, (9000, 64)).astype(np.float32)
     queries = rng.uniform(-1, 1, (4500, 64))
