@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Secondary measurements for the other rows of SURVEY.md section 8 (NOT the driver's headline line):
 
-  python bench_extra.py hnsw  [--rows N --dim D --queries Q --ef 64 --k 10]
+  python bench_extra.py hnsw  [--rows N --dim D --queries Q --ef 64 --k 10 --metric M --graph-metric G]
   python bench_extra.py graph [--log2-nodes 24 --edges E --sources 1024 --hops 3]
 
 Each prints one JSON line with the metric, a roofline object computed from in-kernel counters
@@ -50,6 +50,7 @@ def bench_hnsw(a):
     dev = torch.device("cuda", 0)
     g = torch.Generator(device=dev).manual_seed(0x5DB00003)
     n, dim = a.rows, a.dim
+    gm = (a.graph_metric or a.metric).upper()  # the builders serve cosine / euclidean; the walk serves every metric
     centers = torch.nn.functional.normalize(torch.randn((4096, dim), generator=g, device=dev), dim=1)
     def sample(cnt):
         # sigma = TOTAL noise norm relative to the unit-norm centroid (per-coordinate sigma / sqrt(dim)); a per-coordinate
@@ -72,23 +73,23 @@ def bench_hnsw(a):
             tl[0] = now
     if a.builder == "incremental":
         from surrealdb_b200.hnsw_build import build_incremental
-        res = build_incremental(ctx, x, a.metric.upper(), m=a.m, m0=2 * a.m, efc=a.efc, seed=7, growth=a.growth, progress=prog,
+        res = build_incremental(ctx, x, gm, m=a.m, m0=2 * a.m, efc=a.efc, seed=7, growth=a.growth, progress=prog,
                                 settle=not a.no_settle)
         x = res["x"]  # re-ordered by level: element ids below are the NEW ids (rows of this tensor)
         layers = [(rp.cpu().numpy().astype(np.uint64), ci.cpu().numpy().astype(np.uint32)) for rp, ci in res["layers_dev"]] if not a.no_cpu else None
         entry = res["entry"]
         print(f"[build] done {time.perf_counter() - t0:.1f}s", file=sys.stderr, flush=True)
         build_s = time.perf_counter() - t0
-        idx = HnswIndex.from_device(ctx, x, res["layers_dev"], entry, a.metric.upper())
+        idx = HnswIndex.from_device(ctx, x, res["layers_dev"], entry, a.metric.upper(), minkowski_order=a.minkowski_order)
         n_layers = len(res["layers_dev"])
         deg0 = float(res["layers_dev"][0][1].numel()) / n
         xh = x.cpu().numpy() if not a.no_cpu else None
     else:
-        layers, entry, levels = build_layers(ctx, x, n, dim, a.metric.upper(), m=a.m, m0=2 * a.m, seed=7, progress=prog, prefix=a.prefix)
+        layers, entry, levels = build_layers(ctx, x, n, dim, gm, m=a.m, m0=2 * a.m, seed=7, progress=prog, prefix=a.prefix)
         print(f"[build] done {time.perf_counter() - t0:.1f}s", file=sys.stderr, flush=True)
         build_s = time.perf_counter() - t0
         xh = x.cpu().numpy()
-        idx = HnswIndex(ctx, xh, layers, entry, a.metric.upper())
+        idx = HnswIndex(ctx, xh, layers, entry, a.metric.upper(), minkowski_order=a.minkowski_order)
         n_layers = len(layers)
         deg0 = float(np.diff(layers[0][0].astype(np.int64)).mean())
     qh = queries.cpu().numpy()
@@ -116,6 +117,8 @@ def bench_hnsw(a):
     same_dev = bool(np.array_equal(d_ids.cpu().numpy()[:, :1].astype(np.uint64), ids[:, :1]))
     # recall@k against exact brute force (f64 reference arithmetic) on the same corpus
     col = VectorColumn(ctx, dim, a.metric.upper(), "F32", capacity=n)
+    if a.metric.upper() == "MINKOWSKI":
+        col.set_minkowski_order(a.minkowski_order)
     torch.cuda.synchronize()
     col.append_device(x.data_ptr(), n)
     col.finalize()
@@ -128,14 +131,17 @@ def bench_hnsw(a):
            "e2e": {"value": a.queries / (wall * 1e-3), "unit": "queries/s", "call_wall_ms": wall, "api": "sdb_hnsw_search (pageable host queries and results)",
                    "h2d_bytes": int(a.queries * dim * 4), "d2h_bytes": int(a.queries * a.k * 16 + a.queries * 20)},
            "device_results_equal_host_call": same_dev,
-           "recall_at_k": recall, "config": {"rows": n, "dim": dim, "queries": a.queries, "metric": a.metric.lower(), "data": f"4096 unit-norm centroids + gaussian noise of total norm {a.sigma}",
+           "recall_at_k": recall, "config": {"rows": n, "dim": dim, "queries": a.queries, "metric": a.metric.lower(), "graph_metric": gm.lower(),
+                                              **({"minkowski_order": a.minkowski_order} if a.metric.upper() == "MINKOWSKI" else {}), "data": f"4096 unit-norm centroids + gaussian noise of total norm {a.sigma}",
                                               "graph": ("GPU batched true insertion (hnsw_build.build_incremental): walk kernel as insertion search (efc=%d), Heuristic::select, bidirectional linking, re-selection of over-full nodes; batches grow by %.2fx" % (a.efc, a.growth)) if a.builder == "incremental" else "GPU batch-built layers (hnsw_build.py): kNN candidates" + (" from id prefixes" if a.prefix else "") + " + Heuristic::select + bidirectional re-selection", "build_s": build_s,
                                               "layers": n_layers, "visited_per_query": visited / a.queries,
                                               "expanded_per_query": expanded / a.queries},
            "roofline": {"bound": "hbm", "kernel": "hnsw_search_kernel", "achieved": byts / (ms * 1e-3) / 1e9, "peak": peak,
                         "unit": "GB/s", "frac": byts / (ms * 1e-3) / 1e9 / peak, "peak_source": src,
                         "algorithmic_bytes": byts, "traffic": None}}
-    if not a.no_cpu:
+    if a.metric in ("minkowski", "pearson", "jaccard"):  # the CPU oracle's walk does not restate these metrics
+        out["cpu_baseline"] = None
+    elif not a.no_cpu:
         from oracle import pyoracle as O
         if xh is None:
             xh = x.cpu().numpy()
@@ -376,7 +382,11 @@ if __name__ == "__main__":
     ap.add_argument("--ef", type=int, default=64)
     ap.add_argument("--k", type=int, default=10)
     ap.add_argument("--m", type=int, default=16)
-    ap.add_argument("--metric", default="euclidean", choices=["euclidean", "cosine"])
+    metrics = ["euclidean", "cosine", "manhattan", "chebyshev", "hamming", "minkowski", "pearson", "jaccard"]
+    ap.add_argument("--metric", default="euclidean", choices=metrics, help="metric of the walk (and of the recall)")
+    ap.add_argument("--graph-metric", default=None, choices=["euclidean", "cosine"],
+                    help="metric the GPU builder links the graph with (default: --metric)")
+    ap.add_argument("--minkowski-order", type=float, default=3.0)
     ap.add_argument("--sigma", type=float, default=0.15)
     ap.add_argument("--prefix", action="store_true", help="insertion-order (prefix) candidate sets in the batch builder")
     ap.add_argument("--builder", default="batch", choices=["batch", "incremental"])

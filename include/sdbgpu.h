@@ -239,7 +239,12 @@ sdb_status sdb_topk_merge_device(sdb_ctx*, uint32_t n_lists, uint32_t nq, uint32
 /* ---- HNSW search: replaces Hnsw::knn_search (idx/trees/hnsw/mod.rs:459-482) called from
  *      HnswIndex::search_graph (idx/trees/hnsw/index.rs:341-364) ------------------------------- */
 /* vectors: n_elems x dim f32 (element id = row).  Layer l adjacency is CSR over element ids;
- * row_ptr[l] has n_elems+1 entries; neighbours keep the stored order (graph.rs:104-125). */
+ * row_ptr[l] has n_elems+1 entries; neighbours keep the stored order (graph.rs:104-125).
+ * Every sdb_metric is served, with the reference's typed F32 arithmetic (idx/trees/vector.rs:218-451): all three
+ * loaders build the per-element state PEARSON (mean, sum of squared deviations: 16 bytes per element) and JACCARD
+ * (sorted distinct bit patterns: 4 * (dim + 1) bytes per element) need; SDB_ENOMEM if it does not fit.  MINKOWSKI uses
+ * order 3 until sdb_hnsw_set_minkowski_order.  PEARSON and JACCARD are similarities that the walk ranks as distances
+ * (smaller first), as the reference does. */
 sdb_status sdb_hnsw_load(sdb_ctx*, uint32_t dim, sdb_metric, uint64_t n_elems, const float* vectors,
                          uint32_t n_layers, const uint64_t* const* row_ptr, const uint32_t* const* col_idx,
                          int64_t entry_point, sdb_hnsw** out);
@@ -280,6 +285,14 @@ sdb_status sdb_hnsw_search_pending(sdb_hnsw*, const float* queries, uint32_t nq,
  * arithmetic as the walk kernel (f32 8-lane accumulation, f64 finish). */
 sdb_status sdb_vec_distance_f32(sdb_ctx*, sdb_metric, uint32_t dim, const float* query, const float* vectors, uint64_t n,
                                 double* out);
+/* The same for an index of any metric: Distance::calculate(&query, &vector) (hnsw/index.rs:407) with the index's
+ * metric and Minkowski order, i.e. what search_pendings needs.  JACCARD is asymmetric: query first, as there.
+ * query: dim floats, vectors: n x dim floats, out: n doubles (all host memory).  MINKOWSKI goes through pow(), CUDA's
+ * libm (within an ulp or two of the platform libm per call); every other metric is bit-exact. */
+sdb_status sdb_hnsw_distance(sdb_hnsw*, const float* query, const float* vectors, uint64_t n, double* out);
+/* order p of Distance::Minkowski(p) for a MINKOWSKI index (default 3; NaN -> SDB_EINVAL).  Waits for running searches
+ * on the handle; the next search uses the new order. */
+sdb_status sdb_hnsw_set_minkowski_order(sdb_hnsw*, double order);
 
 /* ---- staging: the reference's persisted HNSW state -> device (SURVEY 8a row a14).  These replace the per-key
  *      decode loops of HnswLayer::load (idx/trees/hnsw/layer.rs:526-540, UndirectedGraph::load_node

@@ -17,6 +17,8 @@
 // Algorithmic bytes per query = visited * (4*dim + 4) + expanded * 4*deg, both counters are returned.
 #include <algorithm>
 
+#include <cub/device/device_segmented_sort.cuh>
+
 #include "internal.cuh"
 #include "rowwalk.cuh"
 
@@ -32,6 +34,11 @@ struct Hnsw {
   float* d_vec = nullptr;
   float* d_sumsq = nullptr;
   double* d_norm = nullptr;  // sqrt((double)sumsq): the per-element factor of the cosine denominator (vector.rs:246)
+  double minkowski_p = 3.0;  // order of SDB_MINKOWSKI (sdb_hnsw_set_minkowski_order)
+  double* d_mean = nullptr;  // PEARSON: per-element mean (f32, widened) and sum of squared deviations (vector.rs:412-451)
+  double* d_sx2 = nullptr;
+  uint32_t* d_bits = nullptr;   // JACCARD: per-element sorted distinct bit patterns (dim-strided rows) ...
+  uint32_t* d_nbits = nullptr;  // ... and how many there are (vector.rs:329-340)
   std::vector<uint64_t*> rp;
   std::vector<uint32_t*> ci;
   const uint64_t** d_rp = nullptr;
@@ -84,17 +91,203 @@ __global__ void hnsw_sumsq_kernel(const float* __restrict__ vec, uint32_t dim, u
   }
 }
 
-// Distance::calculate for VectorType::F32 (idx/trees/vector.rs:243-289,659-672), one thread per vector: the typed
-// metric of the walk applied to vectors that are NOT part of the graph -- the new_vectors of pending updates that
-// HnswIndex::search_pendings ranks by brute force (hnsw/index.rs:398-404).  Same lane structure as the walk, so a
-// vector gets the same distance whether it is reached through the graph or through the pending log.
-template <bool COSINE>
-__global__ void typed_distance_kernel(const float* __restrict__ q, const float* __restrict__ vecs, uint32_t dim, uint64_t n,
-                                      double* __restrict__ out) {
+// ---- per-vector state of PEARSON and JACCARD (load time for the elements, per batch for queries and pending vectors)
+
+// PEARSON (vector.rs:412-451): mean = ndarray's f32 mean -- the 8-lane unrolled f32 sum (the fold of hnsw_sumsq_kernel,
+// tests/hnsw_metric_ref.py nd_sum_f32) divided by n as f32 -- widened to f64; sx2 = sequential f64 sum of (f64(x_i) - mean)^2.  Only
+// the cross term is left per pair.  One thread per vector (load time, and once per query batch).
+__global__ void pearson_stats_kernel(const float* __restrict__ vec, uint32_t dim, uint64_t n, double* __restrict__ mean,
+                                     double* __restrict__ sx2) {
   const uint64_t r = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (r >= n) return;
-  const float* a = vecs + r * dim;
-  if (COSINE) {
+  const float* a = vec + r * dim;
+  float p[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+  uint32_t i = 0;
+  for (; i + 8 <= dim; i += 8)
+#pragma unroll
+    for (int j = 0; j < 8; j++) p[j] = __fadd_rn(p[j], a[i + j]);
+  float s = 0.f;
+#pragma unroll
+  for (int j = 0; j < 4; j++) s = __fadd_rn(s, __fadd_rn(p[j], p[j + 4]));
+  for (; i < dim; i++) s = __fadd_rn(s, a[i]);
+  const double m = (double)__fdiv_rn(s, (float)dim);
+  double d2 = 0.0;
+  for (uint32_t c = 0; c < dim; c++) {
+    const double d = __dsub_rn((double)a[c], m);
+    d2 = __dadd_rn(d2, __dmul_rn(d, d));
+  }
+  mean[r] = m;
+  sx2[r] = d2;
+}
+
+// JACCARD (vector.rs:329-340) compares f32 BIT PATTERNS.  A vector's state is its sorted list of distinct patterns:
+// after a segmented sort of each row (one row = one segment), this drops the repeats in place and records the count.
+__global__ void distinct_sorted_kernel(uint32_t* __restrict__ bits, uint32_t dim, uint64_t n, uint32_t* __restrict__ nbits) {
+  const uint64_t r = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (r >= n) return;
+  uint32_t* row = bits + r * dim;
+  uint32_t u = 1, prev = row[0];
+  for (uint32_t i = 1; i < dim; i++) {
+    const uint32_t v = row[i];
+    if (v != prev) row[u++] = v;
+    prev = v;
+  }
+  nbits[r] = u;
+}
+__global__ void segment_offsets_kernel(int* __restrict__ off, uint32_t rows, uint32_t dim) {
+  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i <= rows) off[i] = (int)(i * dim);
+}
+
+// rows x dim f32 -> per row: sorted distinct bit patterns (bits, rows x dim, caller-allocated) and their count (nbits)
+sdb_status jaccard_prepare(Ctx* ctx, const float* d_vec, uint64_t rows, uint32_t dim, uint32_t* bits, uint32_t* nbits,
+                           cudaStream_t st) {
+  if (!rows) return SDB_OK;
+  const uint64_t chunk = std::max<uint64_t>(1, std::min<uint64_t>(rows, (1u << 30) / dim));  // CUB counts items in int
+  int* d_off = nullptr;
+  void* d_tmp = nullptr;
+  size_t tmp_bytes = 0;
+  const uint32_t* keys = reinterpret_cast<const uint32_t*>(d_vec);
+  if (cub::DeviceSegmentedSort::SortKeys(nullptr, tmp_bytes, keys, bits, (int)(chunk * dim), (int)chunk, d_off, d_off + 1,
+                                         st) != cudaSuccess)
+    return SDB_ECUDA;
+  if (cudaMallocAsync(&d_off, sizeof(int) * (chunk + 1), st) != cudaSuccess ||
+      cudaMallocAsync(&d_tmp, tmp_bytes ? tmp_bytes : 1, st) != cudaSuccess) {
+    if (d_off) cudaFreeAsync(d_off, st);
+    set_error("hnsw jaccard: %zu bytes of sort scratch could not be allocated", tmp_bytes + 4 * (chunk + 1));
+    return SDB_ENOMEM;
+  }
+  sdb_status rc = SDB_OK;
+  for (uint64_t r0 = 0; r0 < rows && rc == SDB_OK; r0 += chunk) {
+    const uint32_t nr = (uint32_t)std::min<uint64_t>(chunk, rows - r0);
+    segment_offsets_kernel<<<(nr + 256) / 256, 256, 0, st>>>(d_off, nr, dim);
+    count_launch(ctx);
+    size_t b = tmp_bytes;
+    if (cub::DeviceSegmentedSort::SortKeys(d_tmp, b, keys + r0 * dim, bits + r0 * dim, (int)(nr * dim), (int)nr, d_off,
+                                           d_off + 1, st) != cudaSuccess)
+      rc = SDB_ECUDA;
+    count_launch(ctx);
+  }
+  if (rc == SDB_OK) {
+    distinct_sorted_kernel<<<(unsigned)((rows + 127) / 128), 128, 0, st>>>(bits, dim, rows, nbits);
+    count_launch(ctx);
+  }
+  cudaFreeAsync(d_tmp, st);
+  cudaFreeAsync(d_off, st);
+  if (rc != SDB_OK) set_error("hnsw jaccard: segmented sort failed: %s", cudaGetErrorString(cudaGetLastError()));
+  return rc;
+}
+
+// per-query operands of the metrics that carry state (staged once per query, the same arithmetic as the elements')
+struct MetricQ {
+  double mean = 0.0, sx2 = 0.0;  // PEARSON: the query's mean and sum of squared deviations
+  double p = 3.0;                // MINKOWSKI: the order
+  uint32_t u = 0;                // JACCARD: number of distinct bit patterns of the query
+};
+
+// Per-column accumulators of the metrics that fold ONE sequential chain per row (ndarray-stats' Zip folds, the explicit
+// loops of vector.rs).  step(x, q): x = the element / pending vector, q = the query.  All of them are symmetric in their
+// two arguments (|x-q| = |q-x| exactly, products commute), so the walk's calculate(element, query) and the pending log's
+// calculate(query, vector) share them.  row_mean / row_sx2: the row's PEARSON state.
+template <int MET>
+struct RowAcc;
+template <>
+struct RowAcc<SDB_EUCLIDEAN> {  // l2_dist: f32 sum of squares, f64 sqrt
+  float s = 0.f;
+  __device__ __forceinline__ RowAcc(const MetricQ&, double, double) {}
+  __device__ __forceinline__ void step(float x, float q) {
+    const float d = __fsub_rn(x, q);
+    s = __fadd_rn(s, __fmul_rn(d, d));
+  }
+  __device__ __forceinline__ double finish() const { return __dsqrt_rn((double)s); }
+};
+template <>
+struct RowAcc<SDB_MANHATTAN> {  // l1_dist (vector.rs:377-386): f32 sum of |x-q|, then as f64
+  float s = 0.f;
+  __device__ __forceinline__ RowAcc(const MetricQ&, double, double) {}
+  __device__ __forceinline__ void step(float x, float q) { s = __fadd_rn(s, fabsf(__fsub_rn(x, q))); }
+  __device__ __forceinline__ double finish() const { return (double)s; }
+};
+template <>
+struct RowAcc<SDB_CHEBYSHEV> {  // linf_dist (vector.rs:218-233): max starts at 0, `if d > max` (a NaN never wins)
+  float m = 0.f;
+  __device__ __forceinline__ RowAcc(const MetricQ&, double, double) {}
+  __device__ __forceinline__ void step(float x, float q) {
+    const float d = fabsf(__fsub_rn(x, q));
+    if (d > m) m = d;
+  }
+  __device__ __forceinline__ double finish() const { return (double)m; }
+};
+template <>
+struct RowAcc<SDB_HAMMING> {  // vector.rs:291-314: count of x != q under f32 `!=` (NaN != NaN, 0.0 == -0.0)
+  uint32_t c = 0;
+  __device__ __forceinline__ RowAcc(const MetricQ&, double, double) {}
+  __device__ __forceinline__ void step(float x, float q) { c += x != q; }
+  __device__ __forceinline__ double finish() const { return (double)c; }
+};
+template <>
+struct RowAcc<SDB_MINKOWSKI> {  // vector.rs:388-410: f64 sum of |f64(x) - f64(q)|^p, then ^(1/p)
+  double s = 0.0, p;
+  __device__ __forceinline__ RowAcc(const MetricQ& mq, double, double) : p(mq.p) {}
+  __device__ __forceinline__ void step(float x, float q) { s = __dadd_rn(s, pow(fabs(__dsub_rn((double)x, (double)q)), p)); }
+  __device__ __forceinline__ double finish() const { return pow(s, __ddiv_rn(1.0, p)); }
+};
+template <>
+struct RowAcc<SDB_PEARSON> {  // vector.rs:412-451: sxy / sqrt(sx2 * sy2), 0.0 when that is 0 (a similarity)
+  double sxy = 0.0, mx, sx2, my, sy2;
+  __device__ __forceinline__ RowAcc(const MetricQ& mq, double row_mean, double row_sx2)
+      : mx(row_mean), sx2(row_sx2), my(mq.mean), sy2(mq.sx2) {}
+  __device__ __forceinline__ void step(float x, float q) {
+    sxy = __dadd_rn(sxy, __dmul_rn(__dsub_rn((double)x, mx), __dsub_rn((double)q, my)));
+  }
+  __device__ __forceinline__ double finish() const {
+    const double den = __dsqrt_rn(__dmul_rn(sx2, sy2));
+    return den == 0.0 ? 0.0 : __ddiv_rn(sxy, den);
+  }
+};
+
+// JACCARD from counts.  calculate(a, b): union = the distinct patterns of a; every b_i whose pattern is already in the
+// set counts -- all occurrences of a pattern a has, and the 2nd.. occurrences of one it lacks.  With u_a, u_b distinct
+// patterns and m shared: inter = dim - (u_b - m), |union| = u_a + u_b - m.  Asymmetric: the caller fixes (a, b).
+__device__ __forceinline__ double jaccard_from_counts(uint32_t dim, uint32_t ua, uint32_t ub, uint32_t m) {
+  return __ddiv_rn((double)(dim - (ub - m)), (double)(ua + ub - m));
+}
+__device__ __forceinline__ bool sorted_contains(const uint32_t* s, uint32_t n, uint32_t v) {
+  uint32_t lo = 0, hi = n;
+  while (lo < hi) {
+    const uint32_t mid = (lo + hi) >> 1;
+    if (s[mid] < v) lo = mid + 1;
+    else hi = mid;
+  }
+  return lo < n && s[lo] == v;
+}
+
+// Distance::calculate for VectorType::F32 (idx/trees/vector.rs:218-451,659-672), one thread per vector: the typed
+// metric of the walk applied to vectors that are NOT part of the graph -- the new_vectors of pending updates that
+// HnswIndex::search_pendings ranks by brute force (hnsw/index.rs:398-404) as calculate(&search.pt, &vector).  Same
+// arithmetic as the walk, so a vector gets the same distance whether it is reached through the graph or through the
+// pending log.
+struct TypedArgs {
+  const float* q;
+  const float* vecs;
+  uint32_t dim;
+  uint64_t n;
+  double* out;
+  MetricQ mq;
+  const double* v_mean;    // PEARSON: state of every vector
+  const double* v_sx2;
+  const uint32_t* q_bits;  // JACCARD: the query's sorted distinct patterns (mq.u of them) ...
+  const uint32_t* v_bits;  // ... and every vector's
+  const uint32_t* v_nbits;
+};
+template <int MET>
+__global__ void typed_distance_kernel(TypedArgs A) {
+  const uint64_t r = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (r >= A.n) return;
+  const uint32_t dim = A.dim;
+  const float* __restrict__ q = A.q;
+  const float* a = A.vecs + r * dim;
+  if (MET == SDB_COSINE) {
     float p[8] = {0, 0, 0, 0, 0, 0, 0, 0}, pa[8] = {0, 0, 0, 0, 0, 0, 0, 0}, pq[8] = {0, 0, 0, 0, 0, 0, 0, 0};
     uint32_t i = 0;
     for (; i + 8 <= dim; i += 8)
@@ -118,20 +311,26 @@ __global__ void typed_distance_kernel(const float* __restrict__ q, const float* 
     }
     const double na = __dsqrt_rn((double)sa), nb = __dsqrt_rn((double)sq);
     // calculate(a = search.pt, b = vector): dot and the product of norms are symmetric
-    out[r] = __dsub_rn(1.0, __ddiv_rn((double)dot, __dmul_rn(na, nb)));
+    A.out[r] = __dsub_rn(1.0, __ddiv_rn((double)dot, __dmul_rn(na, nb)));
+  } else if (MET == SDB_JACCARD) {
+    // calculate(a = query, b = vector)
+    const uint32_t ub = A.v_nbits[r];
+    const uint32_t* vb = A.v_bits + r * dim;
+    uint32_t m = 0;
+    for (uint32_t i = 0; i < ub; i++) m += sorted_contains(A.q_bits, A.mq.u, vb[i]);
+    A.out[r] = jaccard_from_counts(dim, A.mq.u, ub, m);
   } else {
-    float s = 0.f;
-    for (uint32_t i = 0; i < dim; i++) {
-      const float d = __fsub_rn(a[i], q[i]);
-      s = __fadd_rn(s, __fmul_rn(d, d));
-    }
-    out[r] = __dsqrt_rn((double)s);
+    RowAcc<MET == SDB_COSINE || MET == SDB_JACCARD ? SDB_EUCLIDEAN : MET> acc(
+        A.mq, MET == SDB_PEARSON ? A.v_mean[r] : 0.0, MET == SDB_PEARSON ? A.v_sx2[r] : 0.0);
+    for (uint32_t i = 0; i < dim; i++) acc.step(a[i], q[i]);
+    A.out[r] = acc.finish();
   }
 }
 
 // distance of this lane's row (or NO_ROW) to the query held in shared memory; all 32 lanes must call.
-// Scratch of the distance phase, per warp.  Euclid: a 32 x 33 float transposing tile.  Cosine: 32 compacted row ids +
-// 32 f64 results (the rows are read straight from global memory, see warp_distance<true>).
+// Scratch of the distance phase, per warp.  Every metric but cosine: a 32 x 33 float transposing tile (JACCARD uses 32
+// compacted row ids + 32 f64 results of it).  Cosine: 32 compacted row ids + 32 f64 results (the rows are read straight
+// from global memory, see warp_distance<true>).
 __host__ __device__ constexpr size_t hn_tile_bytes(bool cosine) { return cosine ? 32 * 4 + 32 * 8 : sizeof(float) * 32 * 33; }
 
 // COSINE.  ndarray's f32 dot (a6; oracle orc_nd_dot_f32) keeps 8 running sums p_j over the columns 8i+j, each one a
@@ -151,6 +350,7 @@ __device__ __forceinline__ double warp_distance(const float* __restrict__ vec, c
 // = 4 mod 32 words so the 8 lanes of a row read 8 different bank groups with one LDS.128 per 4 steps; the < 8 tail
 // columns follow at qT[8 * qs ...].
 __host__ __device__ constexpr uint32_t hn_q_stride(uint32_t dim) { return (((dim >> 3) + 27u) / 32u) * 32u + 4u; }
+// Every other metric keeps the query as dim floats (JACCARD: its <= dim sorted distinct bit patterns).
 __host__ __device__ constexpr size_t hn_q_floats(uint32_t dim, bool cosine) {
   return cosine ? (size_t)8 * hn_q_stride(dim) + 8 : (size_t)((dim + 3) & ~3u);
 }
@@ -252,14 +452,17 @@ __device__ __forceinline__ double warp_distance<true>(const float* __restrict__ 
   return my_row != NO_ROW ? res[ci] : 0.0;
 }
 
-// EUCLID.  ndarray-stats' l2_dist folds (a-b)^2 strictly sequentially over the columns: one chain per row, so a row
-// stays on ONE lane and the rows of a round are transposed through shared memory (coalesced fetches, 64 columns a step).
-template <>
-__device__ __forceinline__ double warp_distance<false>(const float* __restrict__ vec, const double* __restrict__ norm,
-                                                       uint32_t dim, uint32_t my_row, const float* s_q, double q_norm,
-                                                       float (*tile)[33]) {
+// EUCLID and the other one-chain metrics (MANHATTAN, CHEBYSHEV, HAMMING in f32; MINKOWSKI, PEARSON in f64, see RowAcc).
+// ndarray-stats' l2_dist folds (a-b)^2 strictly sequentially over the columns: one chain per row, so a row stays on ONE
+// lane and the rows of a round are transposed through shared memory (coalesced fetches, 64 columns a step).
+// row_mean / row_sx2: the PEARSON state of the elements (null for the other metrics).
+template <int MET>
+__device__ __forceinline__ double warp_distance_rows(const float* __restrict__ vec, uint32_t dim, uint32_t my_row,
+                                                     const float* s_q, float (*tile)[33], const MetricQ& mq,
+                                                     const double* __restrict__ row_mean, const double* __restrict__ row_sx2) {
   const uint32_t lane = threadIdx.x & 31u;
-  float s = 0.f;
+  RowAcc<MET> acc(mq, MET == SDB_PEARSON && my_row != NO_ROW ? __ldg(row_mean + my_row) : 0.0,
+                  MET == SDB_PEARSON && my_row != NO_ROW ? __ldg(row_sx2 + my_row) : 0.0);
   // Only a handful of the <=32 neighbours of an expanded node are new (6 on average): the valid rows are compacted and
   // handled in rounds of 16; the 32 x 33 float scratch is viewed as 16 rows x (64 columns + 2 padding words), so one
   // step moves 64 columns of every row of the round -- up to 32 independent loads per lane in flight per wait instead
@@ -295,16 +498,40 @@ __device__ __forceinline__ double warp_distance<false>(const float* __restrict__
       __syncwarp();
       if (mine) {
         const uint32_t lim = dim - c0 < 64u ? dim - c0 : 64u;
-        for (uint32_t jj = 0; jj < lim; jj++) {
-          const float d = __fsub_rn(x[jj], s_q[c0 + jj]);
-          s = __fadd_rn(s, __fmul_rn(d, d));
-        }
+        for (uint32_t jj = 0; jj < lim; jj++) acc.step(x[jj], s_q[c0 + jj]);
       }
       __syncwarp();
     }
   }
   if (my_row == NO_ROW) return 0.0;
-  return __dsqrt_rn((double)s);
+  return acc.finish();
+}
+
+// JACCARD, calculate(a = element, b = query): only m = |distinct(element) & distinct(query)| is per pair.  The query's
+// sorted distinct patterns (q_u of them) are in shared memory; the warp takes one new row at a time, every lane binary-
+// searching a 32-pattern slice of the row's distinct list.
+__device__ __forceinline__ double warp_distance_jaccard(const uint32_t* __restrict__ bits, const uint32_t* __restrict__ nbits,
+                                                        uint32_t dim, uint32_t my_row, const uint32_t* s_qb, uint32_t q_u,
+                                                        float (*tile)[33]) {
+  const uint32_t lane = threadIdx.x & 31u;
+  uint32_t* ids = reinterpret_cast<uint32_t*>(tile);
+  double* res = reinterpret_cast<double*>(ids + 32);
+  const uint32_t vmask = __ballot_sync(0xffffffffu, my_row != NO_ROW);
+  const uint32_t n_rows = __popc(vmask);
+  const uint32_t ci = __popc(vmask & ((1u << lane) - 1u));
+  if (my_row != NO_ROW) ids[ci] = my_row;
+  __syncwarp();
+  for (uint32_t r = 0; r < n_rows; r++) {
+    const uint32_t row = ids[r];
+    const uint32_t ua = __ldg(nbits + row);
+    const uint32_t* eb = bits + (size_t)row * dim;
+    uint32_t m = 0;
+    for (uint32_t i = lane; i < ua; i += 32) m += sorted_contains(s_qb, q_u, __ldg(eb + i));
+    m = __reduce_add_sync(0xffffffffu, m);
+    if (lane == 0) res[r] = jaccard_from_counts(dim, ua, q_u, m);
+  }
+  __syncwarp();
+  return my_row != NO_ROW ? res[ci] : 0.0;
 }
 
 // sorted (ascending key, FIFO inside a key) array insert by the whole warp; entries live in [head, n).  One pass from
@@ -367,10 +594,30 @@ struct HnswParams {
   uint64_t* out_counters;
   uint32_t* overflow;
   const int* cancel;  // mapped host flag (sdb_ctx_cancel): polled before every query
+  // state of the metrics that carry it (unused by cosine / euclid)
+  double mink_p;              // MINKOWSKI order
+  const double* e_mean;       // PEARSON: per element / per query mean and sum of squared deviations
+  const double* e_sx2;
+  const double* q_mean;
+  const double* q_sx2;
+  const uint32_t* e_bits;     // JACCARD: per element / per query sorted distinct bit patterns (dim-strided) and count
+  const uint32_t* e_nbits;
+  const uint32_t* q_bits;
+  const uint32_t* q_nbits;
 };
 
-template <bool COSINE, int MINB>
+template <int MET>
+__device__ __forceinline__ double walk_distance(const HnswParams& P, uint32_t my_row, const float* s_q, double q_norm,
+                                                const MetricQ& mq, float (*tile)[33]) {
+  if constexpr (MET == SDB_COSINE) return warp_distance<true>(P.vec, P.norm, P.dim, my_row, s_q, q_norm, tile);
+  else if constexpr (MET == SDB_JACCARD)
+    return warp_distance_jaccard(P.e_bits, P.e_nbits, P.dim, my_row, reinterpret_cast<const uint32_t*>(s_q), mq.u, tile);
+  else return warp_distance_rows<MET>(P.vec, P.dim, my_row, s_q, tile, mq, P.e_mean, P.e_sx2);
+}
+
+template <int MET, int MINB>
 __global__ void __launch_bounds__(HN_WARPS * 32, MINB) hnsw_search_kernel(HnswParams P) {
+  constexpr bool COSINE = MET == SDB_COSINE;
   extern __shared__ uint8_t smem_raw[];
   const uint32_t warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const uint32_t ccap = P.ccap, wcap = P.ef + 2;
@@ -395,6 +642,7 @@ __global__ void __launch_bounds__(HN_WARPS * 32, MINB) hnsw_search_kernel(HnswPa
     if (*reinterpret_cast<const volatile int*>(P.cancel)) break;  // uniform per warp: every lane reads the same word
     // stage the query (cosine: transposed, see hn_q_stride) and its 8-lane sum of squares
     double q_norm = 0.0;
+    MetricQ mq;
     if (COSINE) {
       const uint32_t qs = hn_q_stride(P.dim), d8 = P.dim & ~7u, steps = P.dim >> 3;
       const float* qg = P.queries + (size_t)q * P.dim;
@@ -423,15 +671,25 @@ __global__ void __launch_bounds__(HN_WARPS * 32, MINB) hnsw_search_kernel(HnswPa
         q_sumsq = __fadd_rn(q_sumsq, __fmul_rn(v, v));
       }
       q_norm = __dsqrt_rn((double)__shfl_sync(0xffffffffu, q_sumsq, 0));
+    } else if (MET == SDB_JACCARD) {
+      mq.u = P.q_nbits[q];
+      uint32_t* s_qb = reinterpret_cast<uint32_t*>(s_q);
+      for (uint32_t c = lane; c < mq.u; c += 32) s_qb[c] = P.q_bits[(size_t)q * P.dim + c];
+      __syncwarp();
     } else {
       for (uint32_t c = lane; c < P.dim; c += 32) s_q[c] = P.queries[(size_t)q * P.dim + c];
       __syncwarp();
+      if (MET == SDB_PEARSON) {
+        mq.mean = P.q_mean[q];
+        mq.sx2 = P.q_sx2[q];
+      }
+      if (MET == SDB_MINKOWSKI) mq.p = P.mink_p;
     }
     uint64_t n_visited = 0, n_expanded = 0;
     uint32_t n_out = 0;
     if (P.entry >= 0) {
       uint32_t ep = (uint32_t)P.entry;
-      double ep_d = warp_distance<COSINE>(P.vec, P.norm, P.dim, lane == 0 ? ep : NO_ROW, s_q, q_norm, tile);
+      double ep_d = walk_distance<MET>(P, lane == 0 ? ep : NO_ROW, s_q, q_norm, mq, tile);
       ep_d = __shfl_sync(0xffffffffu, ep_d, 0);
       n_visited++;
       for (int32_t layer = (int32_t)P.n_layers - 1; layer >= 0; layer--) {
@@ -494,7 +752,7 @@ __global__ void __launch_bounds__(HN_WARPS * 32, MINB) hnsw_search_kernel(HnswPa
             const uint32_t new_mask = __ballot_sync(0xffffffffu, is_new);
             if (!new_mask) continue;
             n_visited += __popc(new_mask);
-            const double d = warp_distance<COSINE>(P.vec, P.norm, P.dim, is_new ? nb : NO_ROW, s_q, q_norm, tile);
+            const double d = walk_distance<MET>(P, is_new ? nb : NO_ROW, s_q, q_norm, mq, tile);
             // admission in stored order                                     layer.rs:205-217
             uint32_t m = new_mask;
             while (m) {
@@ -744,7 +1002,7 @@ using namespace sdb;
 
 extern "C" void sdb_hnsw_destroy(sdb_hnsw* h);
 
-// common tail of the loaders: per-layer pointer tables + cached |x|^2
+// common tail of the loaders: per-layer pointer tables + cached |x|^2 + the per-element state of PEARSON / JACCARD
 static sdb_status hnsw_finish(sdb_hnsw* h, sdb_hnsw** out) {
   Ctx* ctx = h->ctx;
   cudaStream_t st = ctx->stream;
@@ -764,6 +1022,26 @@ static sdb_status hnsw_finish(sdb_hnsw* h, sdb_hnsw** out) {
     hnsw_sumsq_kernel<<<(unsigned)((h->n * 8 + 127) / 128), 128, 0, st>>>(h->d_vec, h->dim, h->n, h->d_sumsq, h->d_norm);
     count_launch(ctx);
   }
+  if (h->n && h->metric == SDB_PEARSON) {
+    if (cudaMalloc(&h->d_mean, sizeof(double) * h->n) != cudaSuccess || cudaMalloc(&h->d_sx2, sizeof(double) * h->n) != cudaSuccess)
+      return fail("pearson state", SDB_ENOMEM);
+    pearson_stats_kernel<<<(unsigned)((h->n + 127) / 128), 128, 0, st>>>(h->d_vec, h->dim, h->n, h->d_mean, h->d_sx2);
+    count_launch(ctx);
+  }
+  if (h->n && h->metric == SDB_JACCARD) {  // 4 * n * dim bytes: the sorted distinct patterns of every element
+    if (cudaMalloc(&h->d_bits, sizeof(uint32_t) * h->n * h->dim) != cudaSuccess ||
+        cudaMalloc(&h->d_nbits, sizeof(uint32_t) * h->n) != cudaSuccess) {
+      set_error("hnsw load: jaccard state (%llu bytes) could not be allocated",
+                (unsigned long long)(sizeof(uint32_t) * h->n * ((uint64_t)h->dim + 1)));
+      sdb_hnsw_destroy(h);
+      return SDB_ENOMEM;
+    }
+    const sdb_status rc = jaccard_prepare(ctx, h->d_vec, h->n, h->dim, h->d_bits, h->d_nbits, st);
+    if (rc != SDB_OK) {
+      sdb_hnsw_destroy(h);
+      return rc;
+    }
+  }
   if (cudaStreamSynchronize(st) != cudaSuccess || cudaGetLastError() != cudaSuccess) return fail("finish", SDB_ECUDA);
   *out = h;
   return SDB_OK;
@@ -781,6 +1059,10 @@ void sdb_hnsw_destroy(sdb_hnsw* h) {
   }
   cudaFree(h->d_sumsq);
   cudaFree(h->d_norm);
+  cudaFree(h->d_mean);
+  cudaFree(h->d_sx2);
+  cudaFree(h->d_bits);
+  cudaFree(h->d_nbits);
   cudaFree(h->d_rp);
   cudaFree(h->d_ci);
   cudaFree(h->d_visited);
@@ -793,8 +1075,8 @@ sdb_status sdb_hnsw_load(sdb_ctx* ctx, uint32_t dim, sdb_metric metric, uint64_t
   if (!ctx || !out || dim == 0 || dim > 65535 || n_elems >= 0xFFFFFFF0ull || (n_elems && !vectors) || !n_layers ||
       !row_ptr || !col_idx || entry_point >= (int64_t)n_elems)
     return SDB_EINVAL;
-  if (metric != SDB_COSINE && metric != SDB_EUCLIDEAN) {
-    set_error("hnsw: metric %d not implemented on the GPU path", (int)metric);
+  if ((unsigned)metric > SDB_PEARSON) {
+    set_error("hnsw: unknown metric %d", (int)metric);
     return SDB_EUNSUPPORTED;
   }
   *out = nullptr;
@@ -842,8 +1124,8 @@ sdb_status sdb_hnsw_load_device(sdb_ctx* ctx, uint32_t dim, sdb_metric metric, u
   if (!ctx || !out || dim == 0 || dim > 65535 || n_elems >= 0xFFFFFFF0ull || (n_elems && !d_vectors) || !n_layers ||
       !d_row_ptr || !d_col_idx || entry_point >= (int64_t)n_elems)
     return SDB_EINVAL;
-  if (metric != SDB_COSINE && metric != SDB_EUCLIDEAN) {
-    set_error("hnsw: metric %d not implemented on the GPU path", (int)metric);
+  if ((unsigned)metric > SDB_PEARSON) {
+    set_error("hnsw: unknown metric %d", (int)metric);
     return SDB_EUNSUPPORTED;
   }
   *out = nullptr;
@@ -878,8 +1160,8 @@ sdb_status sdb_hnsw_load_staged(sdb_ctx* ctx, uint32_t dim, sdb_metric metric, u
   if (!ctx || !out || dim == 0 || dim > 65535 || n_elems >= 0xFFFFFFF0ull || !n_layers || !node_blob || !node_off ||
       !node_ids || !n_nodes || entry_point >= (int64_t)n_elems || (n_vec && (!vec_blob || !vec_off)))
     return SDB_EINVAL;
-  if (metric != SDB_COSINE && metric != SDB_EUCLIDEAN) {
-    set_error("hnsw: metric %d not implemented on the GPU path", (int)metric);
+  if ((unsigned)metric > SDB_PEARSON) {
+    set_error("hnsw: unknown metric %d", (int)metric);
     return SDB_EUNSUPPORTED;
   }
   *out = nullptr;
@@ -1024,6 +1306,51 @@ sdb_status sdb_hnsw_select_neighbors_ids(sdb_ctx* ctx, const float* d_vectors, u
   return SDB_OK;
 }
 
+using WalkKernel = void (*)(HnswParams);
+static WalkKernel walk_kernel(sdb_metric metric, int occ) {
+  switch (metric) {
+    case SDB_COSINE: return occ >= 8 ? hnsw_search_kernel<SDB_COSINE, 8> : occ <= 4 ? hnsw_search_kernel<SDB_COSINE, 4> : hnsw_search_kernel<SDB_COSINE, 6>;
+    case SDB_MANHATTAN: return hnsw_search_kernel<SDB_MANHATTAN, 1>;
+    case SDB_CHEBYSHEV: return hnsw_search_kernel<SDB_CHEBYSHEV, 1>;
+    case SDB_HAMMING: return hnsw_search_kernel<SDB_HAMMING, 1>;
+    case SDB_MINKOWSKI: return hnsw_search_kernel<SDB_MINKOWSKI, 1>;
+    case SDB_PEARSON: return hnsw_search_kernel<SDB_PEARSON, 1>;
+    case SDB_JACCARD: return hnsw_search_kernel<SDB_JACCARD, 1>;
+    default: return hnsw_search_kernel<SDB_EUCLIDEAN, 1>;
+  }
+}
+
+// per-query (or per-pending-vector) state of PEARSON / JACCARD, computed with the element-side kernels
+struct BatchState {
+  double* mean = nullptr;
+  double* sx2 = nullptr;
+  uint32_t* bits = nullptr;
+  uint32_t* nbits = nullptr;
+  void release(cudaStream_t st) {
+    if (mean) cudaFreeAsync(mean, st);
+    if (sx2) cudaFreeAsync(sx2, st);
+    if (bits) cudaFreeAsync(bits, st);
+    if (nbits) cudaFreeAsync(nbits, st);
+    mean = sx2 = nullptr;
+    bits = nbits = nullptr;
+  }
+};
+static sdb_status batch_state(Ctx* ctx, sdb_metric metric, const float* d_v, uint64_t rows, uint32_t dim, BatchState& bs,
+                              cudaStream_t st) {
+  if (!rows) return SDB_OK;
+  if (metric == SDB_PEARSON) {
+    SDB_CUDA(cudaMallocAsync(&bs.mean, sizeof(double) * rows, st));
+    SDB_CUDA(cudaMallocAsync(&bs.sx2, sizeof(double) * rows, st));
+    pearson_stats_kernel<<<(unsigned)((rows + 127) / 128), 128, 0, st>>>(d_v, dim, rows, bs.mean, bs.sx2);
+    count_launch(ctx);
+  } else if (metric == SDB_JACCARD) {
+    SDB_CUDA(cudaMallocAsync(&bs.bits, sizeof(uint32_t) * rows * dim, st));
+    SDB_CUDA(cudaMallocAsync(&bs.nbits, sizeof(uint32_t) * rows, st));
+    SDB_TRY(jaccard_prepare(ctx, d_v, rows, dim, bs.bits, bs.nbits, st));
+  }
+  return SDB_OK;
+}
+
 static sdb_status hnsw_search_impl(sdb_hnsw* h, const float* queries, uint32_t nq, uint32_t k, uint32_t ef,
                                    const uint8_t* truthy, const uint8_t* noexp, uint64_t* out_elems, double* out_dist,
                                    uint32_t* out_count, uint64_t* out_counters, bool device_io = false) {
@@ -1067,8 +1394,7 @@ static sdb_status hnsw_search_impl(sdb_hnsw* h, const float* queries, uint32_t n
   }
   // cosine: 8 lanes per row keep ~16 loads in flight per lane; 80 registers (6 blocks per SM) holds that without spills
   const int occ = getenv("SDB_HNSW_OCC") ? atoi(getenv("SDB_HNSW_OCC")) : 6;  // measured r2 (1M x 768, ef 64): 6 -> 1.40M QPS, 4 -> 1.32M, 8 -> 1.02M (spills)
-  auto kern = h->metric == SDB_COSINE ? (occ >= 8 ? hnsw_search_kernel<true, 8> : occ <= 4 ? hnsw_search_kernel<true, 4> : hnsw_search_kernel<true, 6>)
-                                      : hnsw_search_kernel<false, 1>;
+  const WalkKernel kern = walk_kernel(h->metric, occ);
   SDB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   // the walk gets nothing from L1 (0.7 % hit rate): give the whole array to shared memory, or the driver's default
   // carve-out (135 KB) caps the kernel at 5 blocks per SM
@@ -1154,8 +1480,22 @@ static sdb_status hnsw_search_impl(sdb_hnsw* h, const float* queries, uint32_t n
   P.out_count = d_cnt;
   P.out_counters = d_ctr;
   P.overflow = d_ovf;
-  kern<<<grid, HN_WARPS * 32, smem, st>>>(P);
-  count_launch(ctx);
+  P.mink_p = h->minkowski_p;
+  P.e_mean = h->d_mean;
+  P.e_sx2 = h->d_sx2;
+  P.e_bits = h->d_bits;
+  P.e_nbits = h->d_nbits;
+  BatchState qs;
+  const sdb_status qrc = batch_state(ctx, h->metric, d_q, nq, h->dim, qs, st);
+  P.q_mean = qs.mean;
+  P.q_sx2 = qs.sx2;
+  P.q_bits = qs.bits;
+  P.q_nbits = qs.nbits;
+  if (qrc == SDB_OK) {
+    kern<<<grid, HN_WARPS * 32, smem, st>>>(P);
+    count_launch(ctx);
+  }
+  qs.release(st);
   h->gen += gens_per_warp * n_tables;
   uint32_t ovf = 0;
   if (!device_io) {
@@ -1178,6 +1518,7 @@ static sdb_status hnsw_search_impl(sdb_hnsw* h, const float* queries, uint32_t n
   if (d_noexp) cudaFreeAsync(d_noexp, st);
   SDB_CUDA(cudaStreamSynchronize(st));
   SDB_CUDA(cudaGetLastError());
+  if (qrc != SDB_OK) return qrc;
   if (ctx_cancelled(ctx)) {  // warps stop taking new queries once the flag is up: the outputs are incomplete
     set_error("query cancelled");
     return SDB_ECANCELLED;
@@ -1193,6 +1534,72 @@ static sdb_status hnsw_search_impl(sdb_hnsw* h, const float* queries, uint32_t n
   return SDB_OK;
 }
 
+// Distance::calculate(&query, &vector) for n host vectors on the context's stream (the caller holds the lock that
+// serialises it): typed_distance_kernel plus the PEARSON / JACCARD state of the query and of the vectors.
+static sdb_status typed_distances(Ctx* ctx, sdb_metric metric, double minkowski_p, uint32_t dim, const float* query,
+                                  const float* vectors, uint64_t n, double* out, const char* what) {
+  cudaStream_t st = ctx->stream;
+  float *d_q = nullptr, *d_v = nullptr;
+  double* d_o = nullptr;
+  BatchState qs, vs;
+  auto run = [&]() -> sdb_status {
+    SDB_CUDA(cudaMallocAsync(&d_q, sizeof(float) * dim, st));
+    SDB_CUDA(cudaMallocAsync(&d_v, sizeof(float) * n * dim, st));
+    SDB_CUDA(cudaMallocAsync(&d_o, sizeof(double) * n, st));
+    SDB_CUDA(cudaMemcpyAsync(d_q, query, sizeof(float) * dim, cudaMemcpyHostToDevice, st));
+    SDB_CUDA(cudaMemcpyAsync(d_v, vectors, sizeof(float) * n * dim, cudaMemcpyHostToDevice, st));
+    SDB_TRY(batch_state(ctx, metric, d_q, 1, dim, qs, st));
+    SDB_TRY(batch_state(ctx, metric, d_v, n, dim, vs, st));
+    TypedArgs A;
+    A.q = d_q;
+    A.vecs = d_v;
+    A.dim = dim;
+    A.n = n;
+    A.out = d_o;
+    A.mq.p = minkowski_p;
+    A.v_mean = vs.mean;
+    A.v_sx2 = vs.sx2;
+    A.q_bits = qs.bits;
+    A.v_bits = vs.bits;
+    A.v_nbits = vs.nbits;
+    if (metric == SDB_PEARSON) {  // the query's scalars travel by value
+      SDB_CUDA(cudaMemcpyAsync(&A.mq.mean, qs.mean, sizeof(double), cudaMemcpyDeviceToHost, st));
+      SDB_CUDA(cudaMemcpyAsync(&A.mq.sx2, qs.sx2, sizeof(double), cudaMemcpyDeviceToHost, st));
+      SDB_CUDA(cudaStreamSynchronize(st));
+    }
+    if (metric == SDB_JACCARD) {
+      SDB_CUDA(cudaMemcpyAsync(&A.mq.u, qs.nbits, sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
+      SDB_CUDA(cudaStreamSynchronize(st));
+    }
+    const unsigned grid = (unsigned)((n + 127) / 128);
+    switch (metric) {
+      case SDB_COSINE: typed_distance_kernel<SDB_COSINE><<<grid, 128, 0, st>>>(A); break;
+      case SDB_EUCLIDEAN: typed_distance_kernel<SDB_EUCLIDEAN><<<grid, 128, 0, st>>>(A); break;
+      case SDB_MANHATTAN: typed_distance_kernel<SDB_MANHATTAN><<<grid, 128, 0, st>>>(A); break;
+      case SDB_CHEBYSHEV: typed_distance_kernel<SDB_CHEBYSHEV><<<grid, 128, 0, st>>>(A); break;
+      case SDB_HAMMING: typed_distance_kernel<SDB_HAMMING><<<grid, 128, 0, st>>>(A); break;
+      case SDB_MINKOWSKI: typed_distance_kernel<SDB_MINKOWSKI><<<grid, 128, 0, st>>>(A); break;
+      case SDB_PEARSON: typed_distance_kernel<SDB_PEARSON><<<grid, 128, 0, st>>>(A); break;
+      case SDB_JACCARD: typed_distance_kernel<SDB_JACCARD><<<grid, 128, 0, st>>>(A); break;
+    }
+    count_launch(ctx);
+    SDB_CUDA(cudaGetLastError());
+    SDB_CUDA(cudaMemcpyAsync(out, d_o, sizeof(double) * n, cudaMemcpyDeviceToHost, st));
+    return SDB_OK;
+  };
+  const sdb_status rc = run();
+  qs.release(st);
+  vs.release(st);
+  if (d_q) cudaFreeAsync(d_q, st);
+  if (d_v) cudaFreeAsync(d_v, st);
+  if (d_o) cudaFreeAsync(d_o, st);
+  if (cudaStreamSynchronize(st) != cudaSuccess && rc == SDB_OK) {
+    set_error("%s: %s", what, cudaGetErrorString(cudaGetLastError()));
+    return SDB_ECUDA;
+  }
+  return rc;
+}
+
 sdb_status sdb_vec_distance_f32(sdb_ctx* ctx, sdb_metric metric, uint32_t dim, const float* query, const float* vectors,
                                 uint64_t n, double* out) {
   if (!ctx || !dim || (n && (!query || !vectors || !out))) return SDB_EINVAL;
@@ -1203,31 +1610,22 @@ sdb_status sdb_vec_distance_f32(sdb_ctx* ctx, sdb_metric metric, uint32_t dim, c
   if (n == 0) return SDB_OK;
   std::lock_guard<std::mutex> guard(ctx->mu);
   SDB_CUDA(cudaSetDevice(ctx->device));
-  cudaStream_t st = ctx->stream;
-  float *d_q = nullptr, *d_v = nullptr;
-  double* d_o = nullptr;
-  auto run = [&]() -> sdb_status {
-    SDB_CUDA(cudaMallocAsync(&d_q, sizeof(float) * dim, st));
-    SDB_CUDA(cudaMallocAsync(&d_v, sizeof(float) * n * dim, st));
-    SDB_CUDA(cudaMallocAsync(&d_o, sizeof(double) * n, st));
-    SDB_CUDA(cudaMemcpyAsync(d_q, query, sizeof(float) * dim, cudaMemcpyHostToDevice, st));
-    SDB_CUDA(cudaMemcpyAsync(d_v, vectors, sizeof(float) * n * dim, cudaMemcpyHostToDevice, st));
-    if (metric == SDB_COSINE) typed_distance_kernel<true><<<(unsigned)((n + 127) / 128), 128, 0, st>>>(d_q, d_v, dim, n, d_o);
-    else typed_distance_kernel<false><<<(unsigned)((n + 127) / 128), 128, 0, st>>>(d_q, d_v, dim, n, d_o);
-    count_launch(ctx);
-    SDB_CUDA(cudaGetLastError());
-    SDB_CUDA(cudaMemcpyAsync(out, d_o, sizeof(double) * n, cudaMemcpyDeviceToHost, st));
-    return SDB_OK;
-  };
-  const sdb_status rc = run();
-  if (d_q) cudaFreeAsync(d_q, st);
-  if (d_v) cudaFreeAsync(d_v, st);
-  if (d_o) cudaFreeAsync(d_o, st);
-  if (cudaStreamSynchronize(st) != cudaSuccess && rc == SDB_OK) {
-    set_error("sdb_vec_distance_f32: %s", cudaGetErrorString(cudaGetLastError()));
-    return SDB_ECUDA;
-  }
-  return rc;
+  return typed_distances(ctx, metric, 3.0, dim, query, vectors, n, out, "sdb_vec_distance_f32");
+}
+
+sdb_status sdb_hnsw_distance(sdb_hnsw* h, const float* query, const float* vectors, uint64_t n, double* out) {
+  if (!h || (n && (!query || !vectors || !out))) return SDB_EINVAL;
+  if (n == 0) return SDB_OK;
+  std::lock_guard<std::mutex> guard(h->mu);
+  SDB_CUDA(cudaSetDevice(h->ctx->device));
+  return typed_distances(h->ctx, h->metric, h->minkowski_p, h->dim, query, vectors, n, out, "sdb_hnsw_distance");
+}
+
+sdb_status sdb_hnsw_set_minkowski_order(sdb_hnsw* h, double order) {
+  if (!h || !(order == order)) return SDB_EINVAL;
+  std::lock_guard<std::mutex> guard(h->mu);  // searches hold it for their whole run
+  h->minkowski_p = order;
+  return SDB_OK;
 }
 
 sdb_status sdb_hnsw_search(sdb_hnsw* h, const float* queries, uint32_t nq, uint32_t k, uint32_t ef, uint64_t* out_elems,
