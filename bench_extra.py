@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Secondary measurements for the other rows of SURVEY.md section 8 (NOT the driver's headline line):
 
-  python bench_extra.py hnsw  [--rows N --dim D --queries Q --ef 64 --k 10 --metric M --graph-metric G]
+  python bench_extra.py hnsw  [--rows N --dim D --queries Q --ef 64 --k 10 --metric M --graph-metric G --vector-type T]
   python bench_extra.py graph [--log2-nodes 24 --edges E --sources 1024 --hops 3]
 
 Each prints one JSON line with the metric, a roofline object computed from in-kernel counters
@@ -83,7 +83,9 @@ def bench_hnsw(a):
         idx = HnswIndex.from_device(ctx, x, res["layers_dev"], entry, a.metric.upper(), minkowski_order=a.minkowski_order)
         n_layers = len(res["layers_dev"])
         deg0 = float(res["layers_dev"][0][1].numel()) / n
-        xh = x.cpu().numpy() if not a.no_cpu else None
+        xh = x.cpu().numpy() if not a.no_cpu or a.vector_type != "F32" else None
+        if a.vector_type != "F32":
+            layers = [(rp.cpu().numpy().astype(np.uint64), ci.cpu().numpy().astype(np.uint32)) for rp, ci in res["layers_dev"]]
     else:
         layers, entry, levels = build_layers(ctx, x, n, dim, gm, m=a.m, m0=2 * a.m, seed=7, progress=prog, prefix=a.prefix)
         print(f"[build] done {time.perf_counter() - t0:.1f}s", file=sys.stderr, flush=True)
@@ -92,71 +94,93 @@ def bench_hnsw(a):
         idx = HnswIndex(ctx, xh, layers, entry, a.metric.upper(), minkowski_order=a.minkowski_order)
         n_layers = len(layers)
         deg0 = float(np.diff(layers[0][0].astype(np.int64)).mean())
-    qh = queries.cpu().numpy()
-    print(f"[load] index on device {time.perf_counter() - t0:.1f}s", file=sys.stderr, flush=True)
-    idx.search_graph(qh[:256], a.k, a.ef)  # warm-up
-    (ids, dist, cnt, ctr), ms_call, wall = dev_time_ms(ctx, lambda: idx.search_graph(qh, a.k, a.ef, counters=True))
-    visited, expanded = int(ctr[:, 0].sum()), int(ctr[:, 1].sum())
-    byts = visited * (4.0 * dim + 4.0) + expanded * deg0 * 4.0
-    # `value`: queries and results resident in HBM (sdb_hnsw_search_device); the host-buffer call above is the e2e figure
-    import ctypes as C
-    from surrealdb_b200 import _lib as L
-    d_ids = torch.empty((a.queries, a.k), dtype=torch.int64, device=dev)
-    d_dist = torch.empty((a.queries, a.k), dtype=torch.float64, device=dev)
-    d_cnt = torch.empty((a.queries,), dtype=torch.int32, device=dev)
-    torch.cuda.synchronize()
-    def dev_search():
-        L.check(L.lib().sdb_hnsw_search_device(idx.h, C.c_void_p(queries.data_ptr()), a.queries, a.k, a.ef, C.c_void_p(d_ids.data_ptr()),
-                                               C.c_void_p(d_dist.data_ptr()), C.c_void_p(d_cnt.data_ptr())))
-    dev_search()
-    best = None
-    for _ in range(3):
-        _, m1, w1 = dev_time_ms(ctx, dev_search)
-        best = m1 if best is None or m1 < best else best
-    ms = best
-    same_dev = bool(np.array_equal(d_ids.cpu().numpy()[:, :1].astype(np.uint64), ids[:, :1]))
-    # recall@k against exact brute force (f64 reference arithmetic) on the same corpus
-    col = VectorColumn(ctx, dim, a.metric.upper(), "F32", capacity=n)
-    if a.metric.upper() == "MINKOWSKI":
-        col.set_minkowski_order(a.minkowski_order)
-    torch.cuda.synchronize()
-    col.append_device(x.data_ptr(), n)
-    col.finalize()
-    nr = min(a.queries, 2000)
-    rows, _, _ = col.knn(qh[:nr].astype(np.float64), a.k)
-    recall = float(np.mean([len(set(rows[i].tolist()) & set(ids[i, : cnt[i]].tolist())) / a.k for i in range(nr)]))
-    peak, src = peaks()
-    out = {"bench": "hnsw_search", "metric": f"HNSW KNN queries/sec (M={a.m}, M0={2*a.m}, ef={a.ef}, k={a.k})",
-           "value": a.queries / (ms * 1e-3), "unit": "queries/s", "device_ms": ms,
-           "e2e": {"value": a.queries / (wall * 1e-3), "unit": "queries/s", "call_wall_ms": wall, "api": "sdb_hnsw_search (pageable host queries and results)",
-                   "h2d_bytes": int(a.queries * dim * 4), "d2h_bytes": int(a.queries * a.k * 16 + a.queries * 20)},
-           "device_results_equal_host_call": same_dev,
-           "recall_at_k": recall, "config": {"rows": n, "dim": dim, "queries": a.queries, "metric": a.metric.lower(), "graph_metric": gm.lower(),
-                                              **({"minkowski_order": a.minkowski_order} if a.metric.upper() == "MINKOWSKI" else {}), "data": f"4096 unit-norm centroids + gaussian noise of total norm {a.sigma}",
-                                              "graph": ("GPU batched true insertion (hnsw_build.build_incremental): walk kernel as insertion search (efc=%d), Heuristic::select, bidirectional linking, re-selection of over-full nodes; batches grow by %.2fx" % (a.efc, a.growth)) if a.builder == "incremental" else "GPU batch-built layers (hnsw_build.py): kNN candidates" + (" from id prefixes" if a.prefix else "") + " + Heuristic::select + bidirectional re-selection", "build_s": build_s,
-                                              "layers": n_layers, "visited_per_query": visited / a.queries,
-                                              "expanded_per_query": expanded / a.queries},
-           "roofline": {"bound": "hbm", "kernel": "hnsw_search_kernel", "achieved": byts / (ms * 1e-3) / 1e9, "peak": peak,
-                        "unit": "GB/s", "frac": byts / (ms * 1e-3) / 1e9 / peak, "peak_source": src,
-                        "algorithmic_bytes": byts, "traffic": None}}
-    if a.metric in ("minkowski", "pearson", "jaccard"):  # the CPU oracle's walk does not restate these metrics
-        out["cpu_baseline"] = None
-    elif not a.no_cpu:
-        from oracle import pyoracle as O
-        if xh is None:
-            xh = x.cpu().numpy()
-        graph = {"vectors": xh, "layers": layers, "entry_point": entry, "metric": a.metric.lower()}
-        threads = os.cpu_count() or 1
-        nqc = min(a.queries, 8 * threads)
-        t0 = time.perf_counter()
-        with ThreadPoolExecutor(threads) as ex:
-            res = list(ex.map(lambda i: O.hnsw_search_csr(graph, qh[i], a.k, a.ef), range(nqc)))
-        dt = time.perf_counter() - t0
-        same = all(list(res[i][0]) == list(ids[i, : cnt[i]]) for i in range(nqc))
-        out["cpu_baseline"] = {"value": nqc / dt, "unit": "queries/s", "cores": threads, "kind": "port",
-                               "sample": f"{nqc} of the same queries, same graph, {threads} threads, {dt:.2f}s; "
-                                         f"results identical to the GPU walk: {same}"}
-    print(json.dumps(out), flush=True)
+    qh0, q_dev0, idx0 = queries.cpu().numpy(), queries, idx
+    for vt in a.vector_type.split(","):  # one JSON line per vector type, all on the same graph
+        # another vector type: the graph above is the F32 build of the same seeded data; the index holds the data in the type
+        # (integers: scaled by INT_SCALE and truncated toward zero) and is walked in that type's arithmetic
+        esz = {"F64": 8, "F32": 4, "I64": 8, "I32": 4, "I16": 2}[vt]
+        INT_SCALE = 8192.0
+        qh, queries, idx = qh0, q_dev0, idx0
+        if vt != "F32":
+            from surrealdb_b200.hnsw import VT_DTYPE, to_vector_type
+            scale = INT_SCALE if vt[0] == "I" else 1.0
+
+            def convert(h):  # in slabs: 1M x 768 f64 temporaries would need ~20 GB of host memory
+                out = np.empty(h.shape, VT_DTYPE[vt])
+                for r0 in range(0, h.shape[0], 1 << 16):
+                    out[r0:r0 + (1 << 16)] = to_vector_type(h[r0:r0 + (1 << 16)].astype(np.float64) * scale, vt)
+                return out
+            xt, qh = convert(xh), convert(qh)
+            idx = HnswIndex(ctx, xt, layers, entry, a.metric.upper(), minkowski_order=a.minkowski_order, vector_type=vt)
+            queries = torch.from_numpy(qh).to(dev)
+        print(f"[load] index on device {time.perf_counter() - t0:.1f}s", file=sys.stderr, flush=True)
+        idx.search_graph(qh[:256], a.k, a.ef)  # warm-up
+        (ids, dist, cnt, ctr), ms_call, wall = dev_time_ms(ctx, lambda: idx.search_graph(qh, a.k, a.ef, counters=True))
+        visited, expanded = int(ctr[:, 0].sum()), int(ctr[:, 1].sum())
+        byts = visited * (esz * dim + 4.0) + expanded * deg0 * 4.0
+        # `value`: queries and results resident in HBM (sdb_hnsw_search_device); the host-buffer call above is the e2e figure
+        import ctypes as C
+        from surrealdb_b200 import _lib as L
+        d_ids = torch.empty((a.queries, a.k), dtype=torch.int64, device=dev)
+        d_dist = torch.empty((a.queries, a.k), dtype=torch.float64, device=dev)
+        d_cnt = torch.empty((a.queries,), dtype=torch.int32, device=dev)
+        torch.cuda.synchronize()
+        def dev_search():
+            L.check(L.lib().sdb_hnsw_search_device(idx.h, C.c_void_p(queries.data_ptr()), a.queries, a.k, a.ef, C.c_void_p(d_ids.data_ptr()),
+                                                   C.c_void_p(d_dist.data_ptr()), C.c_void_p(d_cnt.data_ptr())))
+        dev_search()
+        best = None
+        for _ in range(3):
+            _, m1, w1 = dev_time_ms(ctx, dev_search)
+            best = m1 if best is None or m1 < best else best
+        ms = best
+        same_dev = bool(np.array_equal(d_ids.cpu().numpy()[:, :1].astype(np.uint64), ids[:, :1]))
+        # recall@k against exact brute force (f64 reference arithmetic) on the same corpus (F32 indexes: the brute-force
+        # corpora hold F32 / F64 rows only)
+        recall = None
+        if vt == "F32":
+            col = VectorColumn(ctx, dim, a.metric.upper(), "F32", capacity=n)
+            if a.metric.upper() == "MINKOWSKI":
+                col.set_minkowski_order(a.minkowski_order)
+            torch.cuda.synchronize()
+            col.append_device(x.data_ptr(), n)
+            col.finalize()
+            nr = min(a.queries, 2000)
+            rows, _, _ = col.knn(qh[:nr].astype(np.float64), a.k)
+            recall = float(np.mean([len(set(rows[i].tolist()) & set(ids[i, : cnt[i]].tolist())) / a.k for i in range(nr)]))
+        peak, src = peaks()
+        out = {"bench": "hnsw_search", "metric": f"HNSW KNN queries/sec (M={a.m}, M0={2*a.m}, ef={a.ef}, k={a.k})",
+               "value": a.queries / (ms * 1e-3), "unit": "queries/s", "device_ms": ms,
+               "e2e": {"value": a.queries / (wall * 1e-3), "unit": "queries/s", "call_wall_ms": wall, "api": "sdb_hnsw_search (pageable host queries and results)",
+                       "h2d_bytes": int(a.queries * dim * esz), "d2h_bytes": int(a.queries * a.k * 16 + a.queries * 20)},
+               "device_results_equal_host_call": same_dev,
+               "recall_at_k": recall, "config": {"rows": n, "dim": dim, "queries": a.queries, "metric": a.metric.lower(), "graph_metric": gm.lower(),
+                                                  "vector_type": vt, **({"int_scale": INT_SCALE, "data_to_int": f"x * {INT_SCALE:g}, truncated toward zero"} if vt[0] == "I" else {}),
+                                                  **({"minkowski_order": a.minkowski_order} if a.metric.upper() == "MINKOWSKI" else {}), "data": f"4096 unit-norm centroids + gaussian noise of total norm {a.sigma}",
+                                                  "graph": ("GPU batched true insertion (hnsw_build.build_incremental): walk kernel as insertion search (efc=%d), Heuristic::select, bidirectional linking, re-selection of over-full nodes; batches grow by %.2fx" % (a.efc, a.growth)) if a.builder == "incremental" else "GPU batch-built layers (hnsw_build.py): kNN candidates" + (" from id prefixes" if a.prefix else "") + " + Heuristic::select + bidirectional re-selection", "build_s": build_s,
+                                                  "layers": n_layers, "visited_per_query": visited / a.queries,
+                                                  "expanded_per_query": expanded / a.queries},
+               "roofline": {"bound": "hbm", "kernel": "hnsw_search_kernel", "achieved": byts / (ms * 1e-3) / 1e9, "peak": peak,
+                            "unit": "GB/s", "frac": byts / (ms * 1e-3) / 1e9 / peak, "peak_source": src,
+                            "algorithmic_bytes": byts, "traffic": None}}
+        if a.metric in ("minkowski", "pearson", "jaccard") or vt != "F32":  # the CPU oracle's walk does not restate these
+            out["cpu_baseline"] = None
+        elif not a.no_cpu:
+            from oracle import pyoracle as O
+            if xh is None:
+                xh = x.cpu().numpy()
+            graph = {"vectors": xh, "layers": layers, "entry_point": entry, "metric": a.metric.lower()}
+            threads = os.cpu_count() or 1
+            nqc = min(a.queries, 8 * threads)
+            t0 = time.perf_counter()
+            with ThreadPoolExecutor(threads) as ex:
+                res = list(ex.map(lambda i: O.hnsw_search_csr(graph, qh[i], a.k, a.ef), range(nqc)))
+            dt = time.perf_counter() - t0
+            same = all(list(res[i][0]) == list(ids[i, : cnt[i]]) for i in range(nqc))
+            out["cpu_baseline"] = {"value": nqc / dt, "unit": "queries/s", "cores": threads, "kind": "port",
+                                   "sample": f"{nqc} of the same queries, same graph, {threads} threads, {dt:.2f}s; "
+                                             f"results identical to the GPU walk: {same}"}
+        print(json.dumps(out), flush=True)
 
 
 def bench_graph(a):
@@ -387,6 +411,9 @@ if __name__ == "__main__":
     ap.add_argument("--graph-metric", default=None, choices=["euclidean", "cosine"],
                     help="metric the GPU builder links the graph with (default: --metric)")
     ap.add_argument("--minkowski-order", type=float, default=3.0)
+    ap.add_argument("--vector-type", default="F32",
+                    help="element type(s) of the index, F64 F32 I64 I32 I16, comma-separated (the graph is built once, in "
+                         "F32, from the same data; one result line per type)")
     ap.add_argument("--sigma", type=float, default=0.15)
     ap.add_argument("--prefix", action="store_true", help="insertion-order (prefix) candidate sets in the batch builder")
     ap.add_argument("--builder", default="batch", choices=["batch", "incremental"])

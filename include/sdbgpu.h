@@ -62,6 +62,11 @@ typedef enum {
  * values are f32-representable (the BASELINE configs) and enables the low-precision screen. */
 typedef enum { SDB_F32 = 0, SDB_F64 = 1 } sdb_dtype;
 
+/* element type of an HNSW index: catalog::VectorType (catalog/schema/index.rs:321-335), numbered as the SerializedVector
+ * variants (idx/trees/vector.rs:34-40).  An index of type T holds, and its searches take, vectors of T: double, float,
+ * int64_t, int32_t, int16_t. */
+typedef enum { SDB_VT_F64 = 0, SDB_VT_F32 = 1, SDB_VT_I64 = 2, SDB_VT_I32 = 3, SDB_VT_I16 = 4 } sdb_vector_type;
+
 /* which screening kernel sdb_knn_bruteforce uses (results are identical for all; this only moves the performance
  * point).  AUTO: cosine corpora whose normalised rows quantise well (largest relative int8 error <= 0.02 once the few
  * outlier rows are set aside) start on the int8 tensor-core screen, everything else on the bf16 one; queries whose
@@ -240,23 +245,32 @@ sdb_status sdb_topk_merge_device(sdb_ctx*, uint32_t n_lists, uint32_t nq, uint32
  *      HnswIndex::search_graph (idx/trees/hnsw/index.rs:341-364) ------------------------------- */
 /* vectors: n_elems x dim f32 (element id = row).  Layer l adjacency is CSR over element ids;
  * row_ptr[l] has n_elems+1 entries; neighbours keep the stored order (graph.rs:104-125).
- * Every sdb_metric is served, with the reference's typed F32 arithmetic (idx/trees/vector.rs:218-451): all three
- * loaders build the per-element state PEARSON (mean, sum of squared deviations: 16 bytes per element) and JACCARD
- * (sorted distinct bit patterns: 4 * (dim + 1) bytes per element) need; SDB_ENOMEM if it does not fit.  MINKOWSKI uses
- * order 3 until sdb_hnsw_set_minkowski_order.  PEARSON and JACCARD are similarities that the walk ranks as distances
- * (smaller first), as the reference does. */
+ * Every sdb_metric is served, with the reference's typed arithmetic of the index's vector type
+ * (idx/trees/vector.rs:206-451): all loaders build the per-element state COSINE (types other than F32: the norm, 8
+ * bytes per element), PEARSON (mean, sum of squared deviations: 16 bytes per element) and JACCARD (sorted distinct keys:
+ * (key bytes * dim + 4) bytes per element, keys of 8 bytes for F64 / I64 and 4 bytes otherwise) need; SDB_ENOMEM if it
+ * does not fit.  MINKOWSKI uses order 3 until sdb_hnsw_set_minkowski_order.  PEARSON and JACCARD are similarities that
+ * the walk ranks as distances (smaller first), as the reference does -- except F64 JACCARD, which the reference computes
+ * as 1 - similarity (vector.rs:316-327).  sdb_hnsw_load is sdb_hnsw_load_typed with SDB_VT_F32. */
 sdb_status sdb_hnsw_load(sdb_ctx*, uint32_t dim, sdb_metric, uint64_t n_elems, const float* vectors,
                          uint32_t n_layers, const uint64_t* const* row_ptr, const uint32_t* const* col_idx,
                          int64_t entry_point, sdb_hnsw** out);
+/* Any vector type: vectors holds n_elems x dim elements of it.  The integer types compute with wrapping `+ - * abs`,
+ * as the reference's release build does (I16 COSINE's dot product wraps in i16).  SDB_EINVAL for an unknown type;
+ * SDB_EUNSUPPORTED for I16 PEARSON with dim > 32767 (the reference panics: the mean's divisor does not fit i16). */
+sdb_status sdb_hnsw_load_typed(sdb_ctx*, uint32_t dim, sdb_metric, sdb_vector_type, uint64_t n_elems, const void* vectors,
+                               uint32_t n_layers, const uint64_t* const* row_ptr, const uint32_t* const* col_idx,
+                               int64_t entry_point, sdb_hnsw** out);
 /* Device-resident variants for index construction (SURVEY 8f-2): vectors and per-layer CSR arrays are DEVICE pointers
  * that the handle BORROWS (nothing is copied; the caller keeps them alive and unchanged while the handle exists), and
  * the search takes device queries / writes device results.  The incremental builder re-wraps the growing graph with
  * sdb_hnsw_load_device after every insertion batch and uses the walk kernel itself as the insertion search
  * (Hnsw::insert -> HnswLayer::search_multi with efc, hnsw/mod.rs:297-377, hnsw/layer.rs:342-387). */
+/* F32 only: its caller is the F32 GPU builder. */
 sdb_status sdb_hnsw_load_device(sdb_ctx*, uint32_t dim, sdb_metric, uint64_t n_elems, const float* d_vectors,
                                 uint32_t n_layers, const uint64_t* const* d_row_ptr, const uint32_t* const* d_col_idx,
                                 int64_t entry_point, sdb_hnsw** out);
-sdb_status sdb_hnsw_search_device(sdb_hnsw*, const float* d_queries, uint32_t nq, uint32_t k, uint32_t ef,
+sdb_status sdb_hnsw_search_device(sdb_hnsw*, const void* d_queries, uint32_t nq, uint32_t k, uint32_t ef,
                                   uint64_t* d_out_elems, double* d_out_dist, uint32_t* d_out_count);
 void sdb_hnsw_destroy(sdb_hnsw*);
 /* Filtered search: replaces Hnsw::knn_search_with_filter (hnsw/mod.rs:488-515; HnswLayer::search_single_with_filter /
@@ -265,7 +279,7 @@ void sdb_hnsw_destroy(sdb_hnsw*);
  * (hnsw/filter.rs:52-136) holds for element e (host, n_elems bytes).  The descent through the upper layers is
  * unfiltered, as in the reference.  SDB_EOVERFLOW = the filter is too selective for the on-chip candidate window
  * (the caller keeps the CPU path for that query). */
-sdb_status sdb_hnsw_search_filtered(sdb_hnsw*, const float* queries, uint32_t nq, uint32_t k, uint32_t ef,
+sdb_status sdb_hnsw_search_filtered(sdb_hnsw*, const void* queries, uint32_t nq, uint32_t k, uint32_t ef,
                                     const uint8_t* truthy, uint64_t* out_elems, double* out_dist, uint32_t* out_count,
                                     uint64_t* out_counters);
 
@@ -275,7 +289,7 @@ sdb_status sdb_hnsw_search_filtered(sdb_hnsw*, const float* queries, uint32_t nq
  * evaluated by the caller per element (host, n_elems bytes).  Such an element still enters the result window but is
  * never expanded (layer.rs:209), in every layer.  The filtered search needs no extra entry point: add_if_truthy
  * ignores those elements (layer.rs:287-296), i.e. the caller clears their bits in the `truthy` mask. */
-sdb_status sdb_hnsw_search_pending(sdb_hnsw*, const float* queries, uint32_t nq, uint32_t k, uint32_t ef,
+sdb_status sdb_hnsw_search_pending(sdb_hnsw*, const void* queries, uint32_t nq, uint32_t k, uint32_t ef,
                                    const uint8_t* all_docs_pending, uint64_t* out_elems, double* out_dist,
                                    uint32_t* out_count, uint64_t* out_counters);
 
@@ -285,11 +299,12 @@ sdb_status sdb_hnsw_search_pending(sdb_hnsw*, const float* queries, uint32_t nq,
  * arithmetic as the walk kernel (f32 8-lane accumulation, f64 finish). */
 sdb_status sdb_vec_distance_f32(sdb_ctx*, sdb_metric, uint32_t dim, const float* query, const float* vectors, uint64_t n,
                                 double* out);
-/* The same for an index of any metric: Distance::calculate(&query, &vector) (hnsw/index.rs:407) with the index's
- * metric and Minkowski order, i.e. what search_pendings needs.  JACCARD is asymmetric: query first, as there.
- * query: dim floats, vectors: n x dim floats, out: n doubles (all host memory).  MINKOWSKI goes through pow(), CUDA's
- * libm (within an ulp or two of the platform libm per call); every other metric is bit-exact. */
-sdb_status sdb_hnsw_distance(sdb_hnsw*, const float* query, const float* vectors, uint64_t n, double* out);
+/* The same for an index of any metric and vector type: Distance::calculate(&query, &vector) (hnsw/index.rs:407) with
+ * the index's metric, vector type and Minkowski order, i.e. what search_pendings needs.  JACCARD is asymmetric: query
+ * first, as there.  query: dim elements, vectors: n x dim elements, both of the index's vector type; out: n doubles
+ * (all host memory).  MINKOWSKI goes through pow(), CUDA's libm (within an ulp or two of the platform libm per call);
+ * every other metric is bit-exact. */
+sdb_status sdb_hnsw_distance(sdb_hnsw*, const void* query, const void* vectors, uint64_t n, double* out);
 /* order p of Distance::Minkowski(p) for a MINKOWSKI index (default 3; NaN -> SDB_EINVAL).  Waits for running searches
  * on the handle; the next search uses the new order. */
 sdb_status sdb_hnsw_set_minkowski_order(sdb_hnsw*, double order);
@@ -314,15 +329,25 @@ sdb_status sdb_stage_decode_nodes(sdb_ctx*, const uint8_t* blob, const uint64_t*
                                   uint64_t n, uint64_t n_elems, uint64_t** out_row_ptr, uint32_t** out_col_idx,
                                   uint64_t* n_bad);
 /* Both of the above fused with sdb_hnsw_load: raw He values + per-layer Hn values in, device-resident index out
- * (no host-side CSR is ever materialised).  entry_point / n_layers come from the Hs state (hnsw/mod.rs:61-72). */
+ * (no host-side CSR is ever materialised).  entry_point / n_layers come from the Hs state (hnsw/mod.rs:61-72).
+ * An F32 index: a He value of another variant is refused with SDB_EUNSUPPORTED (use sdb_hnsw_load_staged_typed). */
 sdb_status sdb_hnsw_load_staged(sdb_ctx*, uint32_t dim, sdb_metric, uint64_t n_elems, const uint8_t* vec_blob,
                                 const uint64_t* vec_off, const uint64_t* vec_ids, uint64_t n_vec, uint32_t n_layers,
                                 const uint8_t* const* node_blob, const uint64_t* const* node_off,
                                 const uint64_t* const* node_ids, const uint64_t* n_nodes, int64_t entry_point,
                                 sdb_hnsw** out, uint64_t* n_bad);
-/* queries nq x dim f32; out nq x k (element id, f64 distance) ascending; out_counters (nullable)
- * nq x 2 = {distance evaluations, expanded nodes} per query. */
-sdb_status sdb_hnsw_search(sdb_hnsw*, const float* queries, uint32_t nq, uint32_t k, uint32_t ef,
+/* The same for an index of any vector type.  He values are decoded natively (an I64 above 2^53 keeps its value); a
+ * value whose variant is not the index's type is counted in *n_bad and skipped, like any malformed value.  Refusals
+ * as sdb_hnsw_load_typed. */
+sdb_status sdb_hnsw_load_staged_typed(sdb_ctx*, uint32_t dim, sdb_metric, sdb_vector_type, uint64_t n_elems,
+                                      const uint8_t* vec_blob, const uint64_t* vec_off, const uint64_t* vec_ids,
+                                      uint64_t n_vec, uint32_t n_layers, const uint8_t* const* node_blob,
+                                      const uint64_t* const* node_off, const uint64_t* const* node_ids,
+                                      const uint64_t* n_nodes, int64_t entry_point, sdb_hnsw** out, uint64_t* n_bad);
+/* queries nq x dim elements of the index's vector type (float for sdb_hnsw_load / _device / _staged); out nq x k
+ * (element id, f64 distance) ascending; out_counters (nullable) nq x 2 = {distance evaluations, expanded nodes} per
+ * query.  The same holds for the queries of _search_device, _search_filtered and _search_pending. */
+sdb_status sdb_hnsw_search(sdb_hnsw*, const void* queries, uint32_t nq, uint32_t k, uint32_t ef,
                            uint64_t* out_elems, double* out_dist, uint32_t* out_count, uint64_t* out_counters);
 
 /* Index-construction helper (SURVEY 8f-2, "next" row): Heuristic::select, standard variant

@@ -17,6 +17,8 @@ COMM_ID_BYTES = 128
 METRIC = {"CHEBYSHEV": 0, "COSINE": 1, "EUCLIDEAN": 2, "HAMMING": 3, "JACCARD": 4, "MANHATTAN": 5,
           "MINKOWSKI": 6, "PEARSON": 7}
 DTYPE = {"F32": 0, "F64": 1}
+# sdb_vector_type: catalog::VectorType of an HNSW index, numbered as the SerializedVector variants
+VTYPE = {"F64": 0, "F32": 1, "I64": 2, "I32": 3, "I16": 4}
 VECTOR_FN = {"SIMILARITY_COSINE": 16, "DOT": 17, "MAGNITUDE": 18}
 SCREEN = {"AUTO": 0, "SIMT_F32": 1, "TC_BF16": 2, "NONE_EXACT": 3, "TC_INT8": 4}
 
@@ -29,7 +31,7 @@ ABI_SYMBOLS = [
     "sdb_knn_last_stats", "sdb_knn_submit", "sdb_knn_submit_device", "sdb_knn_wait", "sdb_comm_unique_id",
     "sdb_comm_init_rank", "sdb_comm_size", "sdb_comm_rank", "sdb_ctx_create_multi", "sdb_corpus_set_row_base",
     "sdb_knn_sharded_submit", "sdb_knn_sharded_submit_device", "sdb_knn_sharded_wait", "sdb_knn_sharded_multi",
-    "sdb_corpus_project", "sdb_topk_merge_device", "sdb_hnsw_load", "sdb_hnsw_load_device", "sdb_hnsw_search_device", "sdb_hnsw_select_neighbors_ids", "sdb_hnsw_destroy", "sdb_stage_decode_vectors", "sdb_stage_decode_nodes", "sdb_hnsw_load_staged", "sdb_hnsw_search", "sdb_hnsw_search_filtered", "sdb_hnsw_search_pending", "sdb_vec_distance_f32", "sdb_hnsw_distance", "sdb_hnsw_set_minkowski_order", "sdb_hnsw_select_neighbors",
+    "sdb_corpus_project", "sdb_topk_merge_device", "sdb_hnsw_load", "sdb_hnsw_load_typed", "sdb_hnsw_load_device", "sdb_hnsw_search_device", "sdb_hnsw_select_neighbors_ids", "sdb_hnsw_destroy", "sdb_stage_decode_vectors", "sdb_stage_decode_nodes", "sdb_hnsw_load_staged", "sdb_hnsw_load_staged_typed", "sdb_hnsw_search", "sdb_hnsw_search_filtered", "sdb_hnsw_search_pending", "sdb_vec_distance_f32", "sdb_hnsw_distance", "sdb_hnsw_set_minkowski_order", "sdb_hnsw_select_neighbors",
     "sdb_graph_load_csr", "sdb_graph_load_csr_shard", "sdb_graph_destroy", "sdb_graph_expand", "sdb_graph_expand_device", "sdb_device_free", "sdb_graph_collect", "sdb_free",
 ]
 
@@ -109,6 +111,7 @@ def lib():
     L.sdb_knn_last_stats.argtypes = [vp, C.POINTER(KnnStats)]
     L.sdb_topk_merge_device.argtypes = [vp, u32, u32, u32, vp, vp, vp, u64, u64, u64, vp, vp, vp]
     L.sdb_hnsw_load.argtypes = [vp, u32, i32, u64, vp, u32, vp, vp, C.c_int64, C.POINTER(vp)]
+    L.sdb_hnsw_load_typed.argtypes = [vp, u32, i32, i32, u64, vp, u32, vp, vp, C.c_int64, C.POINTER(vp)]
     L.sdb_hnsw_load_device.argtypes = [vp, u32, i32, u64, vp, u32, vp, vp, C.c_int64, C.POINTER(vp)]
     L.sdb_hnsw_search_device.argtypes = [vp, vp, u32, u32, u32, vp, vp, vp]
     L.sdb_hnsw_select_neighbors_ids.argtypes = [vp, vp, u32, i32, vp, u64, vp, vp, u32, u32, i32, vp, vp]
@@ -117,6 +120,8 @@ def lib():
     L.sdb_stage_decode_nodes.argtypes = [vp, vp, vp, vp, u64, u64, C.POINTER(vp), C.POINTER(vp), C.POINTER(u64)]
     L.sdb_hnsw_load_staged.argtypes = [vp, u32, i32, u64, vp, vp, vp, u64, u32, vp, vp, vp, vp, C.c_int64, C.POINTER(vp),
                                        C.POINTER(u64)]
+    L.sdb_hnsw_load_staged_typed.argtypes = [vp, u32, i32, i32, u64, vp, vp, vp, u64, u32, vp, vp, vp, vp, C.c_int64,
+                                             C.POINTER(vp), C.POINTER(u64)]
     L.sdb_hnsw_search.argtypes = [vp, vp, u32, u32, u32, vp, vp, vp, vp]
     L.sdb_hnsw_search_filtered.argtypes = [vp, vp, u32, u32, u32, vp, vp, vp, vp, vp]
     L.sdb_hnsw_search_pending.argtypes = [vp, vp, u32, u32, u32, vp, vp, vp, vp, vp]

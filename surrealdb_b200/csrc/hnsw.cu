@@ -16,6 +16,7 @@
 //
 // Algorithmic bytes per query = visited * (4*dim + 4) + expanded * 4*deg, both counters are returned.
 #include <algorithm>
+#include <type_traits>
 
 #include <cub/device/device_segmented_sort.cuh>
 
@@ -28,17 +29,19 @@ struct Hnsw {
   Ctx* ctx = nullptr;
   uint32_t dim = 0;
   sdb_metric metric = SDB_EUCLIDEAN;
+  sdb_vector_type vt = SDB_VT_F32;  // element type of the vectors (and of the queries a search takes)
   uint64_t n = 0;
   uint32_t n_layers = 0;
   int64_t entry = -1;
-  float* d_vec = nullptr;
-  float* d_sumsq = nullptr;
-  double* d_norm = nullptr;  // sqrt((double)sumsq): the per-element factor of the cosine denominator (vector.rs:246)
+  void* d_vec = nullptr;     // n x dim elements of type vt
+  float* d_sumsq = nullptr;  // F32 only
+  double* d_norm = nullptr;  // the per-element factor of the cosine denominator: sqrt((double)sumsq) (F32, vector.rs:246),
+                             // sqrt of the 8-lane f64 sum of f64(x)^2 (the other types, vector.rs:238,257)
   double minkowski_p = 3.0;  // order of SDB_MINKOWSKI (sdb_hnsw_set_minkowski_order)
-  double* d_mean = nullptr;  // PEARSON: per-element mean (f32, widened) and sum of squared deviations (vector.rs:412-451)
+  double* d_mean = nullptr;  // PEARSON: per-element mean (in the type's arithmetic, widened) and sum of squared deviations (vector.rs:412-451)
   double* d_sx2 = nullptr;
-  uint32_t* d_bits = nullptr;   // JACCARD: per-element sorted distinct bit patterns (dim-strided rows) ...
-  uint32_t* d_nbits = nullptr;  // ... and how many there are (vector.rs:329-340)
+  void* d_bits = nullptr;       // JACCARD: per-element sorted distinct keys (JKey, dim-strided rows) ...
+  uint32_t* d_nbits = nullptr;  // ... and how many there are (vector.rs:316-356)
   std::vector<uint64_t*> rp;
   std::vector<uint32_t*> ci;
   const uint64_t** d_rp = nullptr;
@@ -56,6 +59,51 @@ constexpr uint64_t KEY_MAX = 0xFFEFFFFFFFFFFFFFull;  // dist_key(f64::MAX)
 __device__ __forceinline__ double key_to_double(uint64_t key) {
   const uint64_t b = (key >> 63) ? (key & 0x7fffffffffffffffull) : ~key;
   return __longlong_as_double((long long)b);
+}
+
+// ---- element types (sdb_vector_type -> T): F64 double, F32 float, I64 long long, I32 int, I16 short
+template <typename T> constexpr bool is_f32_v = std::is_same<T, float>::value;
+template <typename T> constexpr bool is_f64_v = std::is_same<T, double>::value;
+template <typename T> constexpr bool is_i16_v = std::is_same<T, short>::value;
+template <typename T> constexpr bool is_wint_v = std::is_same<T, long long>::value || std::is_same<T, int>::value;  // I64, I32
+// JACCARD key of an element: its bit pattern (F32, F64, vector.rs:316-340) or its value (integers, :342-356); u64 for the
+// 8-byte types, u32 for the others
+template <typename T> using JKey = typename std::conditional<sizeof(T) == 8, unsigned long long, uint32_t>::type;
+// Wrapping integer arithmetic in T (the reference is a release build without overflow checks, so `+ - * abs` wrap):
+// computed in an unsigned type of at least 32 bits, truncated to T.
+template <typename T> using Wide = typename std::conditional<sizeof(T) == 8, unsigned long long, uint32_t>::type;
+template <typename T> __device__ __forceinline__ Wide<T> wide(T v) { return (Wide<T>)(typename std::make_unsigned<T>::type)v; }
+template <typename T> __device__ __forceinline__ T wrap(Wide<T> v) { return (T)(typename std::make_unsigned<T>::type)v; }
+template <typename T> __device__ __forceinline__ T wsub(T a, T b) { return wrap<T>(wide(a) - wide(b)); }
+template <typename T> __device__ __forceinline__ T wabs(T a) { return a < 0 ? wrap<T>(Wide<T>(0) - wide(a)) : a; }  // abs(MIN) = MIN
+
+// ndarray's 8-lane f64 fold (unrolled_fold, like nd_sum_f32 in f64; tests/hnsw_types_ref.py nd_sum_f64) of f64(x)^2
+// (SQ) or of f64(x): the cosine norms of every type but F32 (vector.rs:238,257) and the F64 mean.  One thread per vector.
+template <bool SQ, typename T>
+__device__ __forceinline__ double nd_sum_f64(const T* a, uint32_t dim) {
+  double p[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+  uint32_t i = 0;
+  for (; i + 8 <= dim; i += 8)
+#pragma unroll
+    for (int j = 0; j < 8; j++) {
+      const double v = (double)a[i + j];
+      p[j] = __dadd_rn(p[j], SQ ? __dmul_rn(v, v) : v);
+    }
+  double s = 0.0;
+#pragma unroll
+  for (int j = 0; j < 4; j++) s = __dadd_rn(s, __dadd_rn(p[j], p[j + 4]));
+  for (; i < dim; i++) {
+    const double v = (double)a[i];
+    s = __dadd_rn(s, SQ ? __dmul_rn(v, v) : v);
+  }
+  return s;
+}
+
+// cosine norms of the types other than F32 (load time, and once per query batch)
+template <typename T>
+__global__ void hnsw_norm_kernel(const T* __restrict__ vec, uint32_t dim, uint64_t n, double* __restrict__ norm) {
+  const uint64_t r = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (r < n) norm[r] = __dsqrt_rn(nd_sum_f64<true>(vec + r * dim, dim));
 }
 
 // ndarray-style 8-lane f32 sum of squares of every row (load time).  8 threads per row, thread j owns the partial sum
@@ -93,24 +141,35 @@ __global__ void hnsw_sumsq_kernel(const float* __restrict__ vec, uint32_t dim, u
 
 // ---- per-vector state of PEARSON and JACCARD (load time for the elements, per batch for queries and pending vectors)
 
-// PEARSON (vector.rs:412-451): mean = ndarray's f32 mean -- the 8-lane unrolled f32 sum (the fold of hnsw_sumsq_kernel,
-// tests/hnsw_metric_ref.py nd_sum_f32) divided by n as f32 -- widened to f64; sx2 = sequential f64 sum of (f64(x_i) - mean)^2.  Only
-// the cross term is left per pair.  One thread per vector (load time, and once per query batch).
-__global__ void pearson_stats_kernel(const float* __restrict__ vec, uint32_t dim, uint64_t n, double* __restrict__ mean,
+// PEARSON (vector.rs:412-451): mean = ndarray's mean in T, widened to f64 -- F32: the 8-lane unrolled f32 sum (the fold
+// of hnsw_sumsq_kernel, tests/hnsw_metric_ref.py nd_sum_f32) divided by n as f32; F64: the same in f64; integers: the
+// wrapping sum divided by n in T (truncating toward zero).  sx2 = sequential f64 sum of (f64(x_i) - mean)^2.  Only the
+// cross term is left per pair.  One thread per vector (load time, and once per query batch).
+template <typename T>
+__global__ void pearson_stats_kernel(const T* __restrict__ vec, uint32_t dim, uint64_t n, double* __restrict__ mean,
                                      double* __restrict__ sx2) {
   const uint64_t r = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (r >= n) return;
-  const float* a = vec + r * dim;
-  float p[8] = {0, 0, 0, 0, 0, 0, 0, 0};
-  uint32_t i = 0;
-  for (; i + 8 <= dim; i += 8)
+  const T* a = vec + r * dim;
+  double m;
+  if constexpr (is_f32_v<T>) {
+    float p[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+    uint32_t i = 0;
+    for (; i + 8 <= dim; i += 8)
 #pragma unroll
-    for (int j = 0; j < 8; j++) p[j] = __fadd_rn(p[j], a[i + j]);
-  float s = 0.f;
+      for (int j = 0; j < 8; j++) p[j] = __fadd_rn(p[j], a[i + j]);
+    float s = 0.f;
 #pragma unroll
-  for (int j = 0; j < 4; j++) s = __fadd_rn(s, __fadd_rn(p[j], p[j + 4]));
-  for (; i < dim; i++) s = __fadd_rn(s, a[i]);
-  const double m = (double)__fdiv_rn(s, (float)dim);
+    for (int j = 0; j < 4; j++) s = __fadd_rn(s, __fadd_rn(p[j], p[j + 4]));
+    for (; i < dim; i++) s = __fadd_rn(s, a[i]);
+    m = (double)__fdiv_rn(s, (float)dim);
+  } else if constexpr (is_f64_v<T>) {
+    m = __ddiv_rn(nd_sum_f64<false>(a, dim), (double)dim);
+  } else {  // the wrapping sum is the same in any order
+    Wide<T> w = 0;
+    for (uint32_t c = 0; c < dim; c++) w += wide(a[c]);
+    m = (double)(T)(wrap<T>(w) / (T)dim);
+  }
   double d2 = 0.0;
   for (uint32_t c = 0; c < dim; c++) {
     const double d = __dsub_rn((double)a[c], m);
@@ -120,15 +179,18 @@ __global__ void pearson_stats_kernel(const float* __restrict__ vec, uint32_t dim
   sx2[r] = d2;
 }
 
-// JACCARD (vector.rs:329-340) compares f32 BIT PATTERNS.  A vector's state is its sorted list of distinct patterns:
-// after a segmented sort of each row (one row = one segment), this drops the repeats in place and records the count.
-__global__ void distinct_sorted_kernel(uint32_t* __restrict__ bits, uint32_t dim, uint64_t n, uint32_t* __restrict__ nbits) {
+// JACCARD compares f32 / f64 BIT PATTERNS (vector.rs:316-340) and integer values (:342-356), as JKey<T>.  A vector's
+// state is its sorted list of distinct keys: after a segmented sort of each row (one row = one segment), this drops the
+// repeats in place and records the count.
+template <typename K>
+__global__ void distinct_sorted_kernel(K* __restrict__ bits, uint32_t dim, uint64_t n, uint32_t* __restrict__ nbits) {
   const uint64_t r = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (r >= n) return;
-  uint32_t* row = bits + r * dim;
-  uint32_t u = 1, prev = row[0];
+  K* row = bits + r * dim;
+  uint32_t u = 1;
+  K prev = row[0];
   for (uint32_t i = 1; i < dim; i++) {
-    const uint32_t v = row[i];
+    const K v = row[i];
     if (v != prev) row[u++] = v;
     prev = v;
   }
@@ -138,16 +200,21 @@ __global__ void segment_offsets_kernel(int* __restrict__ off, uint32_t rows, uin
   const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i <= rows) off[i] = (int)(i * dim);
 }
+// I16: the values widened to u32 keys (any injective map keeps the distinct count and the intersection)
+__global__ void widen_keys_kernel(const short* __restrict__ v, uint64_t count, uint32_t* __restrict__ keys) {
+  const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < count) keys[i] = (uint32_t)(int)v[i];
+}
 
-// rows x dim f32 -> per row: sorted distinct bit patterns (bits, rows x dim, caller-allocated) and their count (nbits)
-sdb_status jaccard_prepare(Ctx* ctx, const float* d_vec, uint64_t rows, uint32_t dim, uint32_t* bits, uint32_t* nbits,
+// rows x dim keys -> per row: sorted distinct keys (bits, rows x dim, caller-allocated) and their count (nbits)
+template <typename K>
+sdb_status jaccard_prepare(Ctx* ctx, const K* keys, uint64_t rows, uint32_t dim, K* bits, uint32_t* nbits,
                            cudaStream_t st) {
   if (!rows) return SDB_OK;
   const uint64_t chunk = std::max<uint64_t>(1, std::min<uint64_t>(rows, (1u << 30) / dim));  // CUB counts items in int
   int* d_off = nullptr;
   void* d_tmp = nullptr;
   size_t tmp_bytes = 0;
-  const uint32_t* keys = reinterpret_cast<const uint32_t*>(d_vec);
   if (cub::DeviceSegmentedSort::SortKeys(nullptr, tmp_bytes, keys, bits, (int)(chunk * dim), (int)chunk, d_off, d_off + 1,
                                          st) != cudaSuccess)
     return SDB_ECUDA;
@@ -178,6 +245,27 @@ sdb_status jaccard_prepare(Ctx* ctx, const float* d_vec, uint64_t rows, uint32_t
   return rc;
 }
 
+// rows x dim elements of type vt -> their JACCARD state (bits: rows x dim JKey, caller-allocated)
+sdb_status jaccard_prepare_typed(Ctx* ctx, sdb_vector_type vt, const void* d_vec, uint64_t rows, uint32_t dim, void* bits,
+                                 uint32_t* nbits, cudaStream_t st) {
+  if (vt == SDB_VT_F64 || vt == SDB_VT_I64)
+    return jaccard_prepare(ctx, static_cast<const unsigned long long*>(d_vec), rows, dim,
+                           static_cast<unsigned long long*>(bits), nbits, st);
+  if (vt != SDB_VT_I16)
+    return jaccard_prepare(ctx, static_cast<const uint32_t*>(d_vec), rows, dim, static_cast<uint32_t*>(bits), nbits, st);
+  if (!rows) return SDB_OK;
+  uint32_t* keys = nullptr;
+  if (cudaMallocAsync(&keys, sizeof(uint32_t) * rows * dim, st) != cudaSuccess) {
+    set_error("hnsw jaccard: %llu bytes of key scratch could not be allocated", (unsigned long long)(4 * rows * dim));
+    return SDB_ENOMEM;
+  }
+  widen_keys_kernel<<<(unsigned)((rows * dim + 255) / 256), 256, 0, st>>>(static_cast<const short*>(d_vec), rows * dim, keys);
+  count_launch(ctx);
+  const sdb_status rc = jaccard_prepare(ctx, static_cast<const uint32_t*>(keys), rows, dim, static_cast<uint32_t*>(bits), nbits, st);
+  cudaFreeAsync(keys, st);
+  return rc;
+}
+
 // per-query operands of the metrics that carry state (staged once per query, the same arithmetic as the elements')
 struct MetricQ {
   double mean = 0.0, sx2 = 0.0;  // PEARSON: the query's mean and sum of squared deviations
@@ -189,12 +277,12 @@ struct MetricQ {
 // loops of vector.rs).  step(x, q): x = the element / pending vector, q = the query.  All of them are symmetric in their
 // two arguments (|x-q| = |q-x| exactly, products commute), so the walk's calculate(element, query) and the pending log's
 // calculate(query, vector) share them.  row_mean / row_sx2: the row's PEARSON state.
-template <int MET>
+template <int MET, typename T = float>
 struct RowAcc;
 template <>
 struct RowAcc<SDB_EUCLIDEAN> {  // l2_dist: f32 sum of squares, f64 sqrt
   float s = 0.f;
-  __device__ __forceinline__ RowAcc(const MetricQ&, double, double) {}
+  __device__ __forceinline__ RowAcc(const MetricQ&, double, double, uint32_t = 0) {}
   __device__ __forceinline__ void step(float x, float q) {
     const float d = __fsub_rn(x, q);
     s = __fadd_rn(s, __fmul_rn(d, d));
@@ -204,14 +292,14 @@ struct RowAcc<SDB_EUCLIDEAN> {  // l2_dist: f32 sum of squares, f64 sqrt
 template <>
 struct RowAcc<SDB_MANHATTAN> {  // l1_dist (vector.rs:377-386): f32 sum of |x-q|, then as f64
   float s = 0.f;
-  __device__ __forceinline__ RowAcc(const MetricQ&, double, double) {}
+  __device__ __forceinline__ RowAcc(const MetricQ&, double, double, uint32_t = 0) {}
   __device__ __forceinline__ void step(float x, float q) { s = __fadd_rn(s, fabsf(__fsub_rn(x, q))); }
   __device__ __forceinline__ double finish() const { return (double)s; }
 };
 template <>
 struct RowAcc<SDB_CHEBYSHEV> {  // linf_dist (vector.rs:218-233): max starts at 0, `if d > max` (a NaN never wins)
   float m = 0.f;
-  __device__ __forceinline__ RowAcc(const MetricQ&, double, double) {}
+  __device__ __forceinline__ RowAcc(const MetricQ&, double, double, uint32_t = 0) {}
   __device__ __forceinline__ void step(float x, float q) {
     const float d = fabsf(__fsub_rn(x, q));
     if (d > m) m = d;
@@ -221,21 +309,21 @@ struct RowAcc<SDB_CHEBYSHEV> {  // linf_dist (vector.rs:218-233): max starts at 
 template <>
 struct RowAcc<SDB_HAMMING> {  // vector.rs:291-314: count of x != q under f32 `!=` (NaN != NaN, 0.0 == -0.0)
   uint32_t c = 0;
-  __device__ __forceinline__ RowAcc(const MetricQ&, double, double) {}
+  __device__ __forceinline__ RowAcc(const MetricQ&, double, double, uint32_t = 0) {}
   __device__ __forceinline__ void step(float x, float q) { c += x != q; }
   __device__ __forceinline__ double finish() const { return (double)c; }
 };
 template <>
 struct RowAcc<SDB_MINKOWSKI> {  // vector.rs:388-410: f64 sum of |f64(x) - f64(q)|^p, then ^(1/p)
   double s = 0.0, p;
-  __device__ __forceinline__ RowAcc(const MetricQ& mq, double, double) : p(mq.p) {}
+  __device__ __forceinline__ RowAcc(const MetricQ& mq, double, double, uint32_t = 0) : p(mq.p) {}
   __device__ __forceinline__ void step(float x, float q) { s = __dadd_rn(s, pow(fabs(__dsub_rn((double)x, (double)q)), p)); }
   __device__ __forceinline__ double finish() const { return pow(s, __ddiv_rn(1.0, p)); }
 };
 template <>
 struct RowAcc<SDB_PEARSON> {  // vector.rs:412-451: sxy / sqrt(sx2 * sy2), 0.0 when that is 0 (a similarity)
   double sxy = 0.0, mx, sx2, my, sy2;
-  __device__ __forceinline__ RowAcc(const MetricQ& mq, double row_mean, double row_sx2)
+  __device__ __forceinline__ RowAcc(const MetricQ& mq, double row_mean, double row_sx2, uint32_t = 0)
       : mx(row_mean), sx2(row_sx2), my(mq.mean), sy2(mq.sx2) {}
   __device__ __forceinline__ void step(float x, float q) {
     sxy = __dadd_rn(sxy, __dmul_rn(__dsub_rn((double)x, mx), __dsub_rn((double)q, my)));
@@ -246,13 +334,144 @@ struct RowAcc<SDB_PEARSON> {  // vector.rs:412-451: sxy / sqrt(sx2 * sy2), 0.0 w
   }
 };
 
+// ---- the same accumulators for the other element types T (F64 double, I64 long long, I32 int, I16 short), in each
+// type's own arithmetic (vector.rs:206-451).  The integer l1_dist / l2_dist / linf_dist are ndarray-stats' DeviationExt
+// (not vendored, like the F32 case): they accumulate in T, with wrapping `+ - * abs`, and cast to f64 at the end.
+// to_float() is `as f64` (round to nearest for I64).  A sum that is exact (integers below 2^53) or wraps is the same in
+// any order; the others are the reference's sequential folds.
+template <typename T>
+struct RowAcc<SDB_EUCLIDEAN, T> {  // F64, I64, I32: l2_dist in T; I16: euclidean(), the f64 sum of exact squares
+  typename std::conditional<is_wint_v<T>, Wide<T>, double>::type s = 0;
+  __device__ __forceinline__ RowAcc(const MetricQ&, double, double, uint32_t) {}
+  __device__ __forceinline__ void step(T x, T q) {
+    if constexpr (is_wint_v<T>) {
+      const Wide<T> d = wide(x) - wide(q);
+      s += d * d;
+    } else {
+      const double d = __dsub_rn((double)x, (double)q);
+      s = __dadd_rn(s, __dmul_rn(d, d));
+    }
+  }
+  __device__ __forceinline__ double finish() const {
+    if constexpr (is_wint_v<T>) return __dsqrt_rn((double)wrap<T>(s));
+    else return __dsqrt_rn(s);
+  }
+};
+template <typename T>
+struct RowAcc<SDB_MANHATTAN, T> {  // F64, I64, I32: l1_dist in T (wrapping abs of a wrapping difference); I16: the
+  typename std::conditional<is_wint_v<T>, Wide<T>, double>::type s = 0;  // f64 sum of |f64(x - q)|, x - q wrapping in i16
+  __device__ __forceinline__ RowAcc(const MetricQ&, double, double, uint32_t) {}
+  __device__ __forceinline__ void step(T x, T q) {
+    if constexpr (is_wint_v<T>) s += wide(wabs(wsub(x, q)));
+    else if constexpr (is_i16_v<T>) s = __dadd_rn(s, fabs((double)wsub(x, q)));
+    else s = __dadd_rn(s, fabs(__dsub_rn(x, q)));
+  }
+  __device__ __forceinline__ double finish() const {
+    if constexpr (is_wint_v<T>) return (double)wrap<T>(s);
+    else return s;
+  }
+};
+template <typename T>
+struct RowAcc<SDB_CHEBYSHEV, T> {  // F64, I64, I32: linf_dist in T (`if d > max` from 0; abs(MIN) stays negative and
+  typename std::conditional<is_i16_v<T>, double, T>::type m = 0;  // never wins); I16: fold(0.0, f64::max) of |f64(x) - f64(q)|
+  __device__ __forceinline__ RowAcc(const MetricQ&, double, double, uint32_t) {}
+  __device__ __forceinline__ void step(T x, T q) {
+    if constexpr (is_i16_v<T>) {
+      m = fmax(m, fabs(__dsub_rn((double)x, (double)q)));
+    } else if constexpr (is_f64_v<T>) {
+      const double d = fabs(__dsub_rn(x, q));
+      if (d > m) m = d;
+    } else {
+      const T d = wabs(wsub(x, q));
+      if (d > m) m = d;
+    }
+  }
+  __device__ __forceinline__ double finish() const { return (double)m; }
+};
+template <typename T>
+struct RowAcc<SDB_HAMMING, T> {  // count of x != q (F64: IEEE `!=`)
+  uint32_t c = 0;
+  __device__ __forceinline__ RowAcc(const MetricQ&, double, double, uint32_t) {}
+  __device__ __forceinline__ void step(T x, T q) { c += x != q; }
+  __device__ __forceinline__ double finish() const { return (double)c; }
+};
+template <typename T>
+struct RowAcc<SDB_MINKOWSKI, T> {  // the same f64 arithmetic for every type
+  double s = 0.0, p;
+  __device__ __forceinline__ RowAcc(const MetricQ& mq, double, double, uint32_t) : p(mq.p) {}
+  __device__ __forceinline__ void step(T x, T q) { s = __dadd_rn(s, pow(fabs(__dsub_rn((double)x, (double)q)), p)); }
+  __device__ __forceinline__ double finish() const { return pow(s, __ddiv_rn(1.0, p)); }
+};
+template <typename T>
+struct RowAcc<SDB_PEARSON, T> {  // the means come from pearson_stats_kernel<T>; the loop is f64 for every type
+  double sxy = 0.0, mx, sx2, my, sy2;
+  __device__ __forceinline__ RowAcc(const MetricQ& mq, double row_mean, double row_sx2, uint32_t)
+      : mx(row_mean), sx2(row_sx2), my(mq.mean), sy2(mq.sx2) {}
+  __device__ __forceinline__ void step(T x, T q) {
+    sxy = __dadd_rn(sxy, __dmul_rn(__dsub_rn((double)x, mx), __dsub_rn((double)q, my)));
+  }
+  __device__ __forceinline__ double finish() const {
+    const double den = __dsqrt_rn(__dmul_rn(sx2, sy2));
+    return den == 0.0 ? 0.0 : __ddiv_rn(sxy, den);
+  }
+};
+// COSINE, 1 - dot / (na * nb) with the norms of hnsw_norm_kernel.  F64: dot is ndarray's 8-lane f64 dot (the chain of
+// column c is c mod 8; the 8 chains rotate through p[] so that every index is static), folded as in nd_sum_f64, then
+// the < 8 tail columns.  Integers: a.dot(b) is a wrapping sum of wrapping products in T -- I16 wraps in i16 -- so any
+// order gives it.  row_norm / q_norm: the two norms (the product commutes, so either argument order).
+template <typename T>
+struct RowAcc<SDB_COSINE, T> {
+  double p[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+  double s = 0.0, na, nb;
+  Wide<T> w = 0;
+  uint32_t i = 0, d8;
+  __device__ __forceinline__ RowAcc(const MetricQ&, double row_norm, double q_norm, uint32_t dim)
+      : na(row_norm), nb(q_norm), d8(dim & ~7u) {}
+  __device__ __forceinline__ double fold() const {
+    double f = 0.0;
+#pragma unroll
+    for (int j = 0; j < 4; j++) f = __dadd_rn(f, __dadd_rn(p[j], p[j + 4]));
+    return f;
+  }
+  __device__ __forceinline__ void step(T x, T q) {
+    if constexpr (is_f64_v<T>) {
+      const double pr = __dmul_rn(x, q);
+      if (i < d8) {
+        const double t = __dadd_rn(p[0], pr);
+#pragma unroll
+        for (int j = 0; j < 7; j++) p[j] = p[j + 1];
+        p[7] = t;
+      } else {
+        if (i == d8) s = fold();
+        s = __dadd_rn(s, pr);
+      }
+      i++;
+    } else {
+      w += wide(x) * wide(q);
+    }
+  }
+  __device__ __forceinline__ double finish() const {
+    double dot;
+    if constexpr (is_f64_v<T>) dot = i == d8 ? fold() : s;
+    else dot = (double)wrap<T>(w);
+    return __dsub_rn(1.0, __ddiv_rn(dot, __dmul_rn(na, nb)));
+  }
+};
+
 // JACCARD from counts.  calculate(a, b): union = the distinct patterns of a; every b_i whose pattern is already in the
 // set counts -- all occurrences of a pattern a has, and the 2nd.. occurrences of one it lacks.  With u_a, u_b distinct
 // patterns and m shared: inter = dim - (u_b - m), |union| = u_a + u_b - m.  Asymmetric: the caller fixes (a, b).
 __device__ __forceinline__ double jaccard_from_counts(uint32_t dim, uint32_t ua, uint32_t ub, uint32_t m) {
   return __ddiv_rn((double)(dim - (ub - m)), (double)(ua + ub - m));
 }
-__device__ __forceinline__ bool sorted_contains(const uint32_t* s, uint32_t n, uint32_t v) {
+// jaccard_f64 (vector.rs:316-327) alone returns 1 - inter / union, a distance; every other type the similarity
+template <typename T>
+__device__ __forceinline__ double jaccard_typed(uint32_t dim, uint32_t ua, uint32_t ub, uint32_t m) {
+  if constexpr (is_f64_v<T>) return __dsub_rn(1.0, jaccard_from_counts(dim, ua, ub, m));
+  else return jaccard_from_counts(dim, ua, ub, m);
+}
+template <typename K>
+__device__ __forceinline__ bool sorted_contains(const K* s, uint32_t n, K v) {
   uint32_t lo = 0, hi = n;
   while (lo < hi) {
     const uint32_t mid = (lo + hi) >> 1;
@@ -267,27 +486,30 @@ __device__ __forceinline__ bool sorted_contains(const uint32_t* s, uint32_t n, u
 // HnswIndex::search_pendings ranks by brute force (hnsw/index.rs:398-404) as calculate(&search.pt, &vector).  Same
 // arithmetic as the walk, so a vector gets the same distance whether it is reached through the graph or through the
 // pending log.
+// The other element types use the same kernel with T and their RowAcc / JACCARD keys.
 struct TypedArgs {
-  const float* q;
-  const float* vecs;
+  const float* q;          // dim elements of T (typed as F32's)
+  const float* vecs;       // n x dim elements of T
   uint32_t dim;
   uint64_t n;
   double* out;
   MetricQ mq;
   const double* v_mean;    // PEARSON: state of every vector
   const double* v_sx2;
-  const uint32_t* q_bits;  // JACCARD: the query's sorted distinct patterns (mq.u of them) ...
+  const uint32_t* q_bits;  // JACCARD: the query's sorted distinct keys (mq.u of them, JKey<T>) ...
   const uint32_t* v_bits;  // ... and every vector's
   const uint32_t* v_nbits;
+  const double* v_norm;    // COSINE, types other than F32: the norms of every vector ...
+  const double* q_norm;    // ... and of the query
 };
-template <int MET>
+template <int MET, typename T>
 __global__ void typed_distance_kernel(TypedArgs A) {
   const uint64_t r = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (r >= A.n) return;
   const uint32_t dim = A.dim;
-  const float* __restrict__ q = A.q;
-  const float* a = A.vecs + r * dim;
-  if (MET == SDB_COSINE) {
+  const T* __restrict__ q = reinterpret_cast<const T*>(A.q);
+  const T* a = reinterpret_cast<const T*>(A.vecs) + r * dim;
+  if constexpr (MET == SDB_COSINE && is_f32_v<T>) {
     float p[8] = {0, 0, 0, 0, 0, 0, 0, 0}, pa[8] = {0, 0, 0, 0, 0, 0, 0, 0}, pq[8] = {0, 0, 0, 0, 0, 0, 0, 0};
     uint32_t i = 0;
     for (; i + 8 <= dim; i += 8)
@@ -312,16 +534,17 @@ __global__ void typed_distance_kernel(TypedArgs A) {
     const double na = __dsqrt_rn((double)sa), nb = __dsqrt_rn((double)sq);
     // calculate(a = search.pt, b = vector): dot and the product of norms are symmetric
     A.out[r] = __dsub_rn(1.0, __ddiv_rn((double)dot, __dmul_rn(na, nb)));
-  } else if (MET == SDB_JACCARD) {
+  } else if constexpr (MET == SDB_JACCARD) {
     // calculate(a = query, b = vector)
+    using K = JKey<T>;
     const uint32_t ub = A.v_nbits[r];
-    const uint32_t* vb = A.v_bits + r * dim;
+    const K* vb = reinterpret_cast<const K*>(A.v_bits) + r * dim;
     uint32_t m = 0;
-    for (uint32_t i = 0; i < ub; i++) m += sorted_contains(A.q_bits, A.mq.u, vb[i]);
-    A.out[r] = jaccard_from_counts(dim, A.mq.u, ub, m);
+    for (uint32_t i = 0; i < ub; i++) m += sorted_contains(reinterpret_cast<const K*>(A.q_bits), A.mq.u, vb[i]);
+    A.out[r] = jaccard_typed<T>(dim, A.mq.u, ub, m);
   } else {
-    RowAcc<MET == SDB_COSINE || MET == SDB_JACCARD ? SDB_EUCLIDEAN : MET> acc(
-        A.mq, MET == SDB_PEARSON ? A.v_mean[r] : 0.0, MET == SDB_PEARSON ? A.v_sx2[r] : 0.0);
+    RowAcc<MET, T> acc(A.mq, MET == SDB_PEARSON ? A.v_mean[r] : MET == SDB_COSINE ? A.v_norm[r] : 0.0,
+                       MET == SDB_PEARSON ? A.v_sx2[r] : MET == SDB_COSINE ? *A.q_norm : 0.0, dim);
     for (uint32_t i = 0; i < dim; i++) acc.step(a[i], q[i]);
     A.out[r] = acc.finish();
   }
@@ -353,6 +576,14 @@ __host__ __device__ constexpr uint32_t hn_q_stride(uint32_t dim) { return (((dim
 // Every other metric keeps the query as dim floats (JACCARD: its <= dim sorted distinct bit patterns).
 __host__ __device__ constexpr size_t hn_q_floats(uint32_t dim, bool cosine) {
   return cosine ? (size_t)8 * hn_q_stride(dim) + 8 : (size_t)((dim + 3) & ~3u);
+}
+// Bytes of the staged query, a multiple of 16.  The other element types keep dim elements of T (JACCARD: dim keys),
+// cosine included: it walks the one-chain tile path there.
+__host__ __device__ constexpr size_t hn_q_bytes_typed(uint32_t dim, size_t elem) { return ((size_t)dim * elem + 15) & ~size_t(15); }
+template <int MET, typename T>
+__host__ __device__ constexpr size_t hn_q_bytes(uint32_t dim) {
+  return is_f32_v<T> ? sizeof(float) * hn_q_floats(dim, MET == SDB_COSINE)
+                     : hn_q_bytes_typed(dim, MET == SDB_JACCARD ? sizeof(JKey<T>) : sizeof(T));
 }
 
 template <>
@@ -452,21 +683,25 @@ __device__ __forceinline__ double warp_distance<true>(const float* __restrict__ 
   return my_row != NO_ROW ? res[ci] : 0.0;
 }
 
-// EUCLID and the other one-chain metrics (MANHATTAN, CHEBYSHEV, HAMMING in f32; MINKOWSKI, PEARSON in f64, see RowAcc).
+// EUCLID and the other one-chain metrics (MANHATTAN, CHEBYSHEV, HAMMING in f32; MINKOWSKI, PEARSON in f64, see RowAcc),
+// and every metric but JACCARD for the other element types (COSINE there: RowAcc<SDB_COSINE, T>).
 // ndarray-stats' l2_dist folds (a-b)^2 strictly sequentially over the columns: one chain per row, so a row stays on ONE
-// lane and the rows of a round are transposed through shared memory (coalesced fetches, 64 columns a step).
-// row_mean / row_sx2: the PEARSON state of the elements (null for the other metrics).
-template <int MET>
-__device__ __forceinline__ double warp_distance_rows(const float* __restrict__ vec, uint32_t dim, uint32_t my_row,
-                                                     const float* s_q, float (*tile)[33], const MetricQ& mq,
-                                                     const double* __restrict__ row_mean, const double* __restrict__ row_sx2) {
+// lane and the rows of a round are transposed through shared memory (coalesced fetches, 256 bytes of a row a step).
+// row_mean / row_sx2: the PEARSON state of the elements (null for the other metrics); COSINE: row_mean = the element
+// norms, q_norm the query's.
+template <int MET, typename T = float>
+__device__ __forceinline__ double warp_distance_rows(const T* __restrict__ vec, uint32_t dim, uint32_t my_row,
+                                                     const T* s_q, float (*tile)[33], const MetricQ& mq,
+                                                     const double* __restrict__ row_mean, const double* __restrict__ row_sx2,
+                                                     double q_norm = 0.0) {
+  constexpr uint32_t CW = 256u / sizeof(T);  // columns per step (f32: 64)
   const uint32_t lane = threadIdx.x & 31u;
-  RowAcc<MET> acc(mq, MET == SDB_PEARSON && my_row != NO_ROW ? __ldg(row_mean + my_row) : 0.0,
-                  MET == SDB_PEARSON && my_row != NO_ROW ? __ldg(row_sx2 + my_row) : 0.0);
+  RowAcc<MET, T> acc(mq, (MET == SDB_PEARSON || MET == SDB_COSINE) && my_row != NO_ROW ? __ldg(row_mean + my_row) : 0.0,
+                     MET == SDB_PEARSON && my_row != NO_ROW ? __ldg(row_sx2 + my_row) : MET == SDB_COSINE ? q_norm : 0.0, dim);
   // Only a handful of the <=32 neighbours of an expanded node are new (6 on average): the valid rows are compacted and
-  // handled in rounds of 16; the 32 x 33 float scratch is viewed as 16 rows x (64 columns + 2 padding words), so one
-  // step moves 64 columns of every row of the round -- up to 32 independent loads per lane in flight per wait instead
-  // of 4.  The padding words park the compacted row ids.
+  // handled in rounds of 16; the 32 x 33 float scratch is viewed as 16 rows x (256 bytes + 2 padding words), so one
+  // step moves 64 f32 columns of every row of the round -- up to 32 independent loads per lane in flight per wait
+  // instead of 4.  The padding words park the compacted row ids.
   float(*t)[66] = reinterpret_cast<float(*)[66]>(tile);
   const uint32_t vmask = __ballot_sync(0xffffffffu, my_row != NO_ROW);
   const uint32_t n_rows = __popc(vmask);
@@ -474,7 +709,7 @@ __device__ __forceinline__ double warp_distance_rows(const float* __restrict__ v
   if (my_row != NO_ROW) t[ci & 15u][64 + (ci >> 4)] = __uint_as_float(my_row);
   __syncwarp();
   {
-    const uint32_t row_bytes = dim * 4u;
+    const uint32_t row_bytes = dim * (uint32_t)sizeof(T);
     for (uint32_t r = 0; r < n_rows; r++) {
       const char* base = reinterpret_cast<const char*>(vec + (size_t)__float_as_uint(t[r & 15u][64 + (r >> 4)]) * dim);
       for (uint32_t off = lane * 128u; off < row_bytes; off += 32u * 128u)
@@ -484,20 +719,32 @@ __device__ __forceinline__ double warp_distance_rows(const float* __restrict__ v
   for (uint32_t g0 = 0; g0 < n_rows; g0 += 16) {
     const uint32_t nr = n_rows - g0 < 16u ? n_rows - g0 : 16u;
     const bool mine = my_row != NO_ROW && (ci >> 4) == (g0 >> 4);
-    const float* x = t[ci & 15u];
-    for (uint32_t c0 = 0; c0 < dim; c0 += 64) {
-      const bool in0 = c0 + lane < dim, in1 = c0 + 32 + lane < dim;
+    const T* x = reinterpret_cast<const T*>(t[ci & 15u]);
+    for (uint32_t c0 = 0; c0 < dim; c0 += CW) {
+      if constexpr (is_f32_v<T>) {
+        const bool in0 = c0 + lane < dim, in1 = c0 + 32 + lane < dim;
 #pragma unroll 4
-      for (uint32_t r = 0; r < nr; r++) {
-        const float* src = vec + (size_t)__float_as_uint(t[r][64 + (g0 >> 4)]) * dim + c0 + lane;  // broadcast id read
-        const float v0 = in0 ? __ldg(src) : 0.f;
-        const float v1 = in1 ? __ldg(src + 32) : 0.f;
-        t[r][lane] = v0;
-        t[r][lane + 32] = v1;
+        for (uint32_t r = 0; r < nr; r++) {
+          const float* src = vec + (size_t)__float_as_uint(t[r][64 + (g0 >> 4)]) * dim + c0 + lane;  // broadcast id read
+          const float v0 = in0 ? __ldg(src) : 0.f;
+          const float v1 = in1 ? __ldg(src + 32) : 0.f;
+          t[r][lane] = v0;
+          t[r][lane + 32] = v1;
+        }
+      } else {
+#pragma unroll 4
+        for (uint32_t r = 0; r < nr; r++) {
+          const T* src = vec + (size_t)__float_as_uint(t[r][64 + (g0 >> 4)]) * dim + c0 + lane;
+          T v[CW / 32];
+#pragma unroll
+          for (uint32_t u = 0; u < CW / 32; u++) v[u] = c0 + 32u * u + lane < dim ? __ldg(src + 32u * u) : T(0);
+#pragma unroll
+          for (uint32_t u = 0; u < CW / 32; u++) reinterpret_cast<T*>(t[r])[lane + 32u * u] = v[u];
+        }
       }
       __syncwarp();
       if (mine) {
-        const uint32_t lim = dim - c0 < 64u ? dim - c0 : 64u;
+        const uint32_t lim = dim - c0 < CW ? dim - c0 : CW;
         for (uint32_t jj = 0; jj < lim; jj++) acc.step(x[jj], s_q[c0 + jj]);
       }
       __syncwarp();
@@ -508,10 +755,11 @@ __device__ __forceinline__ double warp_distance_rows(const float* __restrict__ v
 }
 
 // JACCARD, calculate(a = element, b = query): only m = |distinct(element) & distinct(query)| is per pair.  The query's
-// sorted distinct patterns (q_u of them) are in shared memory; the warp takes one new row at a time, every lane binary-
-// searching a 32-pattern slice of the row's distinct list.
-__device__ __forceinline__ double warp_distance_jaccard(const uint32_t* __restrict__ bits, const uint32_t* __restrict__ nbits,
-                                                        uint32_t dim, uint32_t my_row, const uint32_t* s_qb, uint32_t q_u,
+// sorted distinct keys (q_u of them) are in shared memory; the warp takes one new row at a time, every lane binary-
+// searching a 32-key slice of the row's distinct list.
+template <typename T = float>
+__device__ __forceinline__ double warp_distance_jaccard(const JKey<T>* __restrict__ bits, const uint32_t* __restrict__ nbits,
+                                                        uint32_t dim, uint32_t my_row, const JKey<T>* s_qb, uint32_t q_u,
                                                         float (*tile)[33]) {
   const uint32_t lane = threadIdx.x & 31u;
   uint32_t* ids = reinterpret_cast<uint32_t*>(tile);
@@ -524,11 +772,11 @@ __device__ __forceinline__ double warp_distance_jaccard(const uint32_t* __restri
   for (uint32_t r = 0; r < n_rows; r++) {
     const uint32_t row = ids[r];
     const uint32_t ua = __ldg(nbits + row);
-    const uint32_t* eb = bits + (size_t)row * dim;
+    const JKey<T>* eb = bits + (size_t)row * dim;
     uint32_t m = 0;
     for (uint32_t i = lane; i < ua; i += 32) m += sorted_contains(s_qb, q_u, __ldg(eb + i));
     m = __reduce_add_sync(0xffffffffu, m);
-    if (lane == 0) res[r] = jaccard_from_counts(dim, ua, q_u, m);
+    if (lane == 0) res[r] = jaccard_typed<T>(dim, ua, q_u, m);
   }
   __syncwarp();
   return my_row != NO_ROW ? res[ci] : 0.0;
@@ -573,13 +821,13 @@ __device__ __forceinline__ uint32_t sorted_insert(uint64_t* keys, uint32_t* ids,
 }
 
 struct HnswParams {
-  const float* vec;
+  const void* vec;        // n x dim elements of the index's type
   const double* norm;     // sqrt((double)sumsq) per element (cosine)
   const uint64_t* const* rp;
   const uint32_t* const* ci;
   uint32_t dim, n_layers;
   int64_t entry;
-  const float* queries;
+  const void* queries;    // nq x dim elements of the index's type
   uint32_t nq, k, ef;
   uint32_t ccap;          // capacity of the candidate window (entries)
   const uint8_t* truthy;  // non-null: knn_search_with_filter -- one byte per element (layer 0 only)
@@ -600,33 +848,40 @@ struct HnswParams {
   const double* e_sx2;
   const double* q_mean;
   const double* q_sx2;
-  const uint32_t* e_bits;     // JACCARD: per element / per query sorted distinct bit patterns (dim-strided) and count
+  const void* e_bits;         // JACCARD: per element / per query sorted distinct keys (JKey, dim-strided) and count
   const uint32_t* e_nbits;
-  const uint32_t* q_bits;
+  const void* q_bits;
   const uint32_t* q_nbits;
+  const double* q_norm;       // COSINE of the types other than F32: per query norm (the elements' are `norm`)
 };
 
-template <int MET>
+template <int MET, typename T>
 __device__ __forceinline__ double walk_distance(const HnswParams& P, uint32_t my_row, const float* s_q, double q_norm,
                                                 const MetricQ& mq, float (*tile)[33]) {
-  if constexpr (MET == SDB_COSINE) return warp_distance<true>(P.vec, P.norm, P.dim, my_row, s_q, q_norm, tile);
+  if constexpr (MET == SDB_COSINE && is_f32_v<T>)
+    return warp_distance<true>(static_cast<const float*>(P.vec), P.norm, P.dim, my_row, s_q, q_norm, tile);
   else if constexpr (MET == SDB_JACCARD)
-    return warp_distance_jaccard(P.e_bits, P.e_nbits, P.dim, my_row, reinterpret_cast<const uint32_t*>(s_q), mq.u, tile);
-  else return warp_distance_rows<MET>(P.vec, P.dim, my_row, s_q, tile, mq, P.e_mean, P.e_sx2);
+    return warp_distance_jaccard<T>(static_cast<const JKey<T>*>(P.e_bits), P.e_nbits, P.dim, my_row,
+                                    reinterpret_cast<const JKey<T>*>(s_q), mq.u, tile);
+  else
+    return warp_distance_rows<MET, T>(static_cast<const T*>(P.vec), P.dim, my_row, reinterpret_cast<const T*>(s_q), tile,
+                                      mq, MET == SDB_COSINE ? P.norm : P.e_mean, P.e_sx2, q_norm);
 }
 
-template <int MET, int MINB>
+// T: the element type of the index (float = F32; double, long long, int, short = F64, I64, I32, I16)
+template <int MET, int MINB, typename T>
 __global__ void __launch_bounds__(HN_WARPS * 32, MINB) hnsw_search_kernel(HnswParams P) {
-  constexpr bool COSINE = MET == SDB_COSINE;
+  constexpr bool COSINE = MET == SDB_COSINE && is_f32_v<T>;  // the 8-lane transposed path of F32 cosine
   extern __shared__ uint8_t smem_raw[];
   const uint32_t warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const uint32_t ccap = P.ccap, wcap = P.ef + 2;
   // per-warp shared layout
-  const size_t per_warp = sizeof(float) * hn_q_floats(P.dim, COSINE) + hn_tile_bytes(COSINE) + (sizeof(uint64_t) + sizeof(uint32_t)) * (ccap + wcap) + 64;
+  const size_t per_warp = hn_q_bytes<MET, T>(P.dim) + hn_tile_bytes(COSINE) + (sizeof(uint64_t) + sizeof(uint32_t)) * (ccap + wcap) + 64;
   uint8_t* base = smem_raw + (size_t)warp * ((per_warp + 15) & ~size_t(15));
   // query first (16-byte aligned: LDS.128), then the distance scratch, the 8-byte keys, the 4-byte ids
   float* s_q = reinterpret_cast<float*>(base);
-  float(*tile)[33] = reinterpret_cast<float(*)[33]>(s_q + ((hn_q_floats(P.dim, COSINE) + 3) & ~size_t(3)));
+  float(*tile)[33] = reinterpret_cast<float(*)[33]>(is_f32_v<T> ? s_q + ((hn_q_floats(P.dim, COSINE) + 3) & ~size_t(3))
+                                                                : reinterpret_cast<float*>(base + hn_q_bytes<MET, T>(P.dim)));
   uint64_t* c_key = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(tile) + hn_tile_bytes(COSINE));
   uint64_t* w_key = c_key + ccap;
   uint32_t* c_id = reinterpret_cast<uint32_t*>(w_key + wcap);
@@ -645,7 +900,7 @@ __global__ void __launch_bounds__(HN_WARPS * 32, MINB) hnsw_search_kernel(HnswPa
     MetricQ mq;
     if (COSINE) {
       const uint32_t qs = hn_q_stride(P.dim), d8 = P.dim & ~7u, steps = P.dim >> 3;
-      const float* qg = P.queries + (size_t)q * P.dim;
+      const float* qg = static_cast<const float*>(P.queries) + (size_t)q * P.dim;
       for (uint32_t c = lane; c < P.dim; c += 32) {
         const float v = qg[c];
         if (c < d8) s_q[(c & 7u) * qs + (c >> 3)] = v;
@@ -673,23 +928,25 @@ __global__ void __launch_bounds__(HN_WARPS * 32, MINB) hnsw_search_kernel(HnswPa
       q_norm = __dsqrt_rn((double)__shfl_sync(0xffffffffu, q_sumsq, 0));
     } else if (MET == SDB_JACCARD) {
       mq.u = P.q_nbits[q];
-      uint32_t* s_qb = reinterpret_cast<uint32_t*>(s_q);
-      for (uint32_t c = lane; c < mq.u; c += 32) s_qb[c] = P.q_bits[(size_t)q * P.dim + c];
+      JKey<T>* s_qb = reinterpret_cast<JKey<T>*>(s_q);
+      for (uint32_t c = lane; c < mq.u; c += 32) s_qb[c] = static_cast<const JKey<T>*>(P.q_bits)[(size_t)q * P.dim + c];
       __syncwarp();
     } else {
-      for (uint32_t c = lane; c < P.dim; c += 32) s_q[c] = P.queries[(size_t)q * P.dim + c];
+      T* s_qt = reinterpret_cast<T*>(s_q);
+      for (uint32_t c = lane; c < P.dim; c += 32) s_qt[c] = static_cast<const T*>(P.queries)[(size_t)q * P.dim + c];
       __syncwarp();
       if (MET == SDB_PEARSON) {
         mq.mean = P.q_mean[q];
         mq.sx2 = P.q_sx2[q];
       }
       if (MET == SDB_MINKOWSKI) mq.p = P.mink_p;
+      if (MET == SDB_COSINE) q_norm = P.q_norm[q];
     }
     uint64_t n_visited = 0, n_expanded = 0;
     uint32_t n_out = 0;
     if (P.entry >= 0) {
       uint32_t ep = (uint32_t)P.entry;
-      double ep_d = walk_distance<MET>(P, lane == 0 ? ep : NO_ROW, s_q, q_norm, mq, tile);
+      double ep_d = walk_distance<MET, T>(P, lane == 0 ? ep : NO_ROW, s_q, q_norm, mq, tile);
       ep_d = __shfl_sync(0xffffffffu, ep_d, 0);
       n_visited++;
       for (int32_t layer = (int32_t)P.n_layers - 1; layer >= 0; layer--) {
@@ -752,7 +1009,7 @@ __global__ void __launch_bounds__(HN_WARPS * 32, MINB) hnsw_search_kernel(HnswPa
             const uint32_t new_mask = __ballot_sync(0xffffffffu, is_new);
             if (!new_mask) continue;
             n_visited += __popc(new_mask);
-            const double d = walk_distance<MET>(P, is_new ? nb : NO_ROW, s_q, q_norm, mq, tile);
+            const double d = walk_distance<MET, T>(P, is_new ? nb : NO_ROW, s_q, q_norm, mq, tile);
             // admission in stored order                                     layer.rs:205-217
             uint32_t m = new_mask;
             while (m) {
@@ -1002,6 +1259,36 @@ using namespace sdb;
 
 extern "C" void sdb_hnsw_destroy(sdb_hnsw* h);
 
+static size_t vt_size(sdb_vector_type vt) { return vt == SDB_VT_F64 || vt == SDB_VT_I64 ? 8 : vt == SDB_VT_I16 ? 2 : 4; }
+static size_t jkey_size(sdb_vector_type vt) { return vt == SDB_VT_F64 || vt == SDB_VT_I64 ? 8 : 4; }
+// calls f(T()) with the C++ element type of vt
+template <typename F>
+static auto with_vt(sdb_vector_type vt, F&& f) {
+  switch (vt) {
+    case SDB_VT_F64: return f(double());
+    case SDB_VT_I64: return f((long long)0);
+    case SDB_VT_I32: return f(int());
+    case SDB_VT_I16: return f(short());
+    default: return f(float());
+  }
+}
+// the refusals every loader shares: unknown metric or type, and I16 PEARSON beyond the reference's i16 divisor
+static sdb_status check_index_kind(const char* what, uint32_t dim, sdb_metric metric, int vt) {
+  if ((unsigned)metric > SDB_PEARSON) {
+    set_error("hnsw: unknown metric %d", (int)metric);
+    return SDB_EUNSUPPORTED;
+  }
+  if ((unsigned)vt > SDB_VT_I16) {
+    set_error("%s: unknown vector type %d", what, vt);
+    return SDB_EINVAL;
+  }
+  if (vt == SDB_VT_I16 && metric == SDB_PEARSON && dim > 32767) {  // A::from_usize(n) fails: the reference panics
+    set_error("%s: an I16 PEARSON index of dimension %u cannot be searched (the mean's divisor does not fit i16)", what, dim);
+    return SDB_EUNSUPPORTED;
+  }
+  return SDB_OK;
+}
+
 // common tail of the loaders: per-layer pointer tables + cached |x|^2 + the per-element state of PEARSON / JACCARD
 static sdb_status hnsw_finish(sdb_hnsw* h, sdb_hnsw** out) {
   Ctx* ctx = h->ctx;
@@ -1017,26 +1304,39 @@ static sdb_status hnsw_finish(sdb_hnsw* h, sdb_hnsw** out) {
   if (cudaMemcpyAsync(h->d_rp, h->rp.data(), sizeof(void*) * n_layers, cudaMemcpyHostToDevice, st) != cudaSuccess ||
       cudaMemcpyAsync(h->d_ci, h->ci.data(), sizeof(void*) * n_layers, cudaMemcpyHostToDevice, st) != cudaSuccess)
     return fail("layer table copy", SDB_ECUDA);
-  if (h->n) {
+  const unsigned grid = (unsigned)((h->n + 127) / 128);
+  if (h->n && h->vt == SDB_VT_F32) {
     if (cudaMalloc(&h->d_norm, sizeof(double) * h->n) != cudaSuccess) return fail("norms", SDB_ENOMEM);
-    hnsw_sumsq_kernel<<<(unsigned)((h->n * 8 + 127) / 128), 128, 0, st>>>(h->d_vec, h->dim, h->n, h->d_sumsq, h->d_norm);
+    hnsw_sumsq_kernel<<<(unsigned)((h->n * 8 + 127) / 128), 128, 0, st>>>(static_cast<const float*>(h->d_vec), h->dim,
+                                                                           h->n, h->d_sumsq, h->d_norm);
+    count_launch(ctx);
+  } else if (h->n && h->metric == SDB_COSINE) {
+    if (cudaMalloc(&h->d_norm, sizeof(double) * h->n) != cudaSuccess) return fail("norms", SDB_ENOMEM);
+    with_vt(h->vt, [&](auto tag) {
+      using T = decltype(tag);
+      hnsw_norm_kernel<T><<<grid, 128, 0, st>>>(static_cast<const T*>(h->d_vec), h->dim, h->n, h->d_norm);
+    });
     count_launch(ctx);
   }
   if (h->n && h->metric == SDB_PEARSON) {
     if (cudaMalloc(&h->d_mean, sizeof(double) * h->n) != cudaSuccess || cudaMalloc(&h->d_sx2, sizeof(double) * h->n) != cudaSuccess)
       return fail("pearson state", SDB_ENOMEM);
-    pearson_stats_kernel<<<(unsigned)((h->n + 127) / 128), 128, 0, st>>>(h->d_vec, h->dim, h->n, h->d_mean, h->d_sx2);
+    with_vt(h->vt, [&](auto tag) {
+      using T = decltype(tag);
+      pearson_stats_kernel<T><<<grid, 128, 0, st>>>(static_cast<const T*>(h->d_vec), h->dim, h->n, h->d_mean, h->d_sx2);
+    });
     count_launch(ctx);
   }
-  if (h->n && h->metric == SDB_JACCARD) {  // 4 * n * dim bytes: the sorted distinct patterns of every element
-    if (cudaMalloc(&h->d_bits, sizeof(uint32_t) * h->n * h->dim) != cudaSuccess ||
+  if (h->n && h->metric == SDB_JACCARD) {  // key bytes * n * dim: the sorted distinct keys of every element
+    const size_t kb = jkey_size(h->vt);
+    if (cudaMalloc(&h->d_bits, kb * h->n * h->dim) != cudaSuccess ||
         cudaMalloc(&h->d_nbits, sizeof(uint32_t) * h->n) != cudaSuccess) {
       set_error("hnsw load: jaccard state (%llu bytes) could not be allocated",
-                (unsigned long long)(sizeof(uint32_t) * h->n * ((uint64_t)h->dim + 1)));
+                (unsigned long long)(kb * h->n * h->dim + sizeof(uint32_t) * h->n));
       sdb_hnsw_destroy(h);
       return SDB_ENOMEM;
     }
-    const sdb_status rc = jaccard_prepare(ctx, h->d_vec, h->n, h->dim, h->d_bits, h->d_nbits, st);
+    const sdb_status rc = jaccard_prepare_typed(ctx, h->vt, h->d_vec, h->n, h->dim, h->d_bits, h->d_nbits, st);
     if (rc != SDB_OK) {
       sdb_hnsw_destroy(h);
       return rc;
@@ -1072,13 +1372,16 @@ void sdb_hnsw_destroy(sdb_hnsw* h) {
 sdb_status sdb_hnsw_load(sdb_ctx* ctx, uint32_t dim, sdb_metric metric, uint64_t n_elems, const float* vectors,
                          uint32_t n_layers, const uint64_t* const* row_ptr, const uint32_t* const* col_idx,
                          int64_t entry_point, sdb_hnsw** out) {
+  return sdb_hnsw_load_typed(ctx, dim, metric, SDB_VT_F32, n_elems, vectors, n_layers, row_ptr, col_idx, entry_point, out);
+}
+
+sdb_status sdb_hnsw_load_typed(sdb_ctx* ctx, uint32_t dim, sdb_metric metric, sdb_vector_type vt, uint64_t n_elems,
+                               const void* vectors, uint32_t n_layers, const uint64_t* const* row_ptr,
+                               const uint32_t* const* col_idx, int64_t entry_point, sdb_hnsw** out) {
   if (!ctx || !out || dim == 0 || dim > 65535 || n_elems >= 0xFFFFFFF0ull || (n_elems && !vectors) || !n_layers ||
       !row_ptr || !col_idx || entry_point >= (int64_t)n_elems)
     return SDB_EINVAL;
-  if ((unsigned)metric > SDB_PEARSON) {
-    set_error("hnsw: unknown metric %d", (int)metric);
-    return SDB_EUNSUPPORTED;
-  }
+  SDB_TRY(check_index_kind("sdb_hnsw_load_typed", dim, metric, (int)vt));
   *out = nullptr;
   std::lock_guard<std::mutex> guard(ctx->mu);
   SDB_CUDA(cudaSetDevice(ctx->device));
@@ -1086,6 +1389,7 @@ sdb_status sdb_hnsw_load(sdb_ctx* ctx, uint32_t dim, sdb_metric metric, uint64_t
   h->ctx = ctx;
   h->dim = dim;
   h->metric = metric;
+  h->vt = vt;
   h->n = n_elems;
   h->n_layers = n_layers;
   h->entry = entry_point;
@@ -1096,9 +1400,10 @@ sdb_status sdb_hnsw_load(sdb_ctx* ctx, uint32_t dim, sdb_metric metric, uint64_t
     return SDB_ENOMEM;
   };
   const uint64_t nn = n_elems ? n_elems : 1;
-  if (cudaMalloc(&h->d_vec, sizeof(float) * nn * dim) != cudaSuccess) return fail("vectors");
-  if (cudaMalloc(&h->d_sumsq, sizeof(float) * nn) != cudaSuccess) return fail("sumsq");
-  if (n_elems) SDB_CUDA(cudaMemcpyAsync(h->d_vec, vectors, sizeof(float) * n_elems * dim, cudaMemcpyHostToDevice, st));
+  const size_t esz = vt_size(vt);
+  if (cudaMalloc(&h->d_vec, esz * nn * dim) != cudaSuccess) return fail("vectors");
+  if (vt == SDB_VT_F32 && cudaMalloc(&h->d_sumsq, sizeof(float) * nn) != cudaSuccess) return fail("sumsq");
+  if (n_elems) SDB_CUDA(cudaMemcpyAsync(h->d_vec, vectors, esz * n_elems * dim, cudaMemcpyHostToDevice, st));
   for (uint32_t l = 0; l < n_layers; l++) {
     const uint64_t e = n_elems ? row_ptr[l][n_elems] : 0;
     uint64_t* drp = nullptr;
@@ -1139,7 +1444,7 @@ sdb_status sdb_hnsw_load_device(sdb_ctx* ctx, uint32_t dim, sdb_metric metric, u
   h->n_layers = n_layers;
   h->entry = entry_point;
   h->borrowed = true;  // nothing is copied: the caller keeps vectors and adjacency alive while the handle exists
-  h->d_vec = const_cast<float*>(d_vectors);
+  h->d_vec = const_cast<float*>(d_vectors);  // F32 only: its one caller is the F32 GPU builder
   for (uint32_t l = 0; l < n_layers; l++) {
     h->rp.push_back(const_cast<uint64_t*>(d_row_ptr[l]));
     h->ci.push_back(const_cast<uint32_t*>(d_col_idx[l]));
@@ -1152,38 +1457,21 @@ sdb_status sdb_hnsw_load_device(sdb_ctx* ctx, uint32_t dim, sdb_metric metric, u
   return hnsw_finish(h, out);
 }
 
-sdb_status sdb_hnsw_load_staged(sdb_ctx* ctx, uint32_t dim, sdb_metric metric, uint64_t n_elems,
-                                const uint8_t* vec_blob, const uint64_t* vec_off, const uint64_t* vec_ids, uint64_t n_vec,
-                                uint32_t n_layers, const uint8_t* const* node_blob, const uint64_t* const* node_off,
-                                const uint64_t* const* node_ids, const uint64_t* n_nodes, int64_t entry_point,
-                                sdb_hnsw** out, uint64_t* n_bad) {
-  if (!ctx || !out || dim == 0 || dim > 65535 || n_elems >= 0xFFFFFFF0ull || !n_layers || !node_blob || !node_off ||
-      !node_ids || !n_nodes || entry_point >= (int64_t)n_elems || (n_vec && (!vec_blob || !vec_off)))
-    return SDB_EINVAL;
-  if ((unsigned)metric > SDB_PEARSON) {
-    set_error("hnsw: unknown metric %d", (int)metric);
-    return SDB_EUNSUPPORTED;
-  }
-  *out = nullptr;
-  // The walk kernels implement the reference's typed metrics for VectorType::F32 only (idx/trees/vector.rs:243-289
-  // computes F64 / I64 / I32 / I16 vectors in their own arithmetic).  A value of another SerializedVector variant
-  // would load -- the decoder converts it -- but be searched with the wrong arithmetic, so the load refuses it instead
-  // of reporting success (ADVICE r1).  Header = revision varint (1) + variant varint: one byte each.
-  for (uint64_t v = 0; v < n_vec; v++) {
-    const uint64_t a = vec_off[v], b = vec_off[v + 1];
-    if (b >= a + 2 && vec_blob[a] == 1 && vec_blob[a + 1] != 1 && vec_blob[a + 1] <= 4) {
-      static const char* names[] = {"F64", "F32", "I64", "I32", "I16"};
-      set_error("sdb_hnsw_load_staged: He value %llu holds a %s vector; the GPU walk implements the F32 typed metrics only "
-                "(the index keeps the reference's CPU path)", (unsigned long long)v, names[vec_blob[a + 1]]);
-      return SDB_EUNSUPPORTED;
-    }
-  }
+// native < 0: He values converted to f32 (sdb_hnsw_load_staged, which has refused the other variants); otherwise the
+// variant number of the index's type: values are decoded as they are stored and any other variant counts as bad.
+static sdb_status hnsw_load_staged_impl(sdb_ctx* ctx, uint32_t dim, sdb_metric metric, sdb_vector_type vt, int native,
+                                        uint64_t n_elems, const uint8_t* vec_blob, const uint64_t* vec_off,
+                                        const uint64_t* vec_ids, uint64_t n_vec, uint32_t n_layers,
+                                        const uint8_t* const* node_blob, const uint64_t* const* node_off,
+                                        const uint64_t* const* node_ids, const uint64_t* n_nodes, int64_t entry_point,
+                                        sdb_hnsw** out, uint64_t* n_bad) {
   std::lock_guard<std::mutex> guard(ctx->mu);
   SDB_CUDA(cudaSetDevice(ctx->device));
   sdb_hnsw* h = new sdb_hnsw();
   h->ctx = ctx;
   h->dim = dim;
   h->metric = metric;
+  h->vt = vt;
   h->n = n_elems;
   h->n_layers = n_layers;
   h->entry = entry_point;
@@ -1196,15 +1484,17 @@ sdb_status sdb_hnsw_load_staged(sdb_ctx* ctx, uint32_t dim, sdb_metric metric, u
     set_error("hnsw load: present-mask allocation failed: %s", cudaGetErrorString(cudaGetLastError()));
     rc = SDB_ENOMEM;
   }
-  if (cudaMalloc(&h->d_vec, sizeof(float) * nn * dim) != cudaSuccess ||
-      cudaMalloc(&h->d_sumsq, sizeof(float) * nn) != cudaSuccess) {
+  const size_t esz = vt_size(vt);
+  if (cudaMalloc(&h->d_vec, esz * nn * dim) != cudaSuccess ||
+      (vt == SDB_VT_F32 && cudaMalloc(&h->d_sumsq, sizeof(float) * nn) != cudaSuccess)) {
     set_error("hnsw load: vector allocation failed: %s", cudaGetErrorString(cudaGetLastError()));
     rc = SDB_ENOMEM;
   }
   // elements without an He value keep all-zero vectors; they are unreachable unless an Hn value names them
-  if (rc == SDB_OK && cudaMemsetAsync(h->d_vec, 0, sizeof(float) * nn * dim, st) != cudaSuccess) rc = SDB_ECUDA;
+  if (rc == SDB_OK && cudaMemsetAsync(h->d_vec, 0, esz * nn * dim, st) != cudaSuccess) rc = SDB_ECUDA;
   if (rc == SDB_OK)
-    rc = stage_decode_vectors(ctx, vec_blob, vec_off, vec_ids, n_vec, dim, SDB_F32, n_elems, h->d_vec, d_present, &bad, st);
+    rc = stage_decode_vectors(ctx, vec_blob, vec_off, vec_ids, n_vec, dim, SDB_F32, n_elems, h->d_vec, d_present, &bad, st,
+                              native);
   bad_total += bad;
   uint64_t n_dropped = 0;
   for (uint32_t l = 0; l < n_layers && rc == SDB_OK; l++) {
@@ -1269,6 +1559,50 @@ sdb_status sdb_hnsw_load_staged(sdb_ctx* ctx, uint32_t dim, sdb_metric metric, u
   return hnsw_finish(h, out);
 }
 
+sdb_status sdb_hnsw_load_staged(sdb_ctx* ctx, uint32_t dim, sdb_metric metric, uint64_t n_elems,
+                                const uint8_t* vec_blob, const uint64_t* vec_off, const uint64_t* vec_ids, uint64_t n_vec,
+                                uint32_t n_layers, const uint8_t* const* node_blob, const uint64_t* const* node_off,
+                                const uint64_t* const* node_ids, const uint64_t* n_nodes, int64_t entry_point,
+                                sdb_hnsw** out, uint64_t* n_bad) {
+  if (!ctx || !out || dim == 0 || dim > 65535 || n_elems >= 0xFFFFFFF0ull || !n_layers || !node_blob || !node_off ||
+      !node_ids || !n_nodes || entry_point >= (int64_t)n_elems || (n_vec && (!vec_blob || !vec_off)))
+    return SDB_EINVAL;
+  if ((unsigned)metric > SDB_PEARSON) {
+    set_error("hnsw: unknown metric %d", (int)metric);
+    return SDB_EUNSUPPORTED;
+  }
+  *out = nullptr;
+  // This loader builds an F32 index.  A value of another SerializedVector variant would load -- the decoder converts
+  // it -- but be searched in F32 arithmetic where the reference computes in the value's own type
+  // (idx/trees/vector.rs:206-451), so the load refuses it instead of reporting success.  Header = revision varint (1) +
+  // variant varint: one byte each.
+  for (uint64_t v = 0; v < n_vec; v++) {
+    const uint64_t a = vec_off[v], b = vec_off[v + 1];
+    if (b >= a + 2 && vec_blob[a] == 1 && vec_blob[a + 1] != 1 && vec_blob[a + 1] <= 4) {
+      static const char* names[] = {"F64", "F32", "I64", "I32", "I16"};
+      set_error("sdb_hnsw_load_staged: He value %llu holds a %s vector; this loader builds F32 indexes "
+                "(sdb_hnsw_load_staged_typed loads an index of that type)", (unsigned long long)v, names[vec_blob[a + 1]]);
+      return SDB_EUNSUPPORTED;
+    }
+  }
+  return hnsw_load_staged_impl(ctx, dim, metric, SDB_VT_F32, -1, n_elems, vec_blob, vec_off, vec_ids, n_vec, n_layers,
+                               node_blob, node_off, node_ids, n_nodes, entry_point, out, n_bad);
+}
+
+sdb_status sdb_hnsw_load_staged_typed(sdb_ctx* ctx, uint32_t dim, sdb_metric metric, sdb_vector_type vt, uint64_t n_elems,
+                                      const uint8_t* vec_blob, const uint64_t* vec_off, const uint64_t* vec_ids,
+                                      uint64_t n_vec, uint32_t n_layers, const uint8_t* const* node_blob,
+                                      const uint64_t* const* node_off, const uint64_t* const* node_ids,
+                                      const uint64_t* n_nodes, int64_t entry_point, sdb_hnsw** out, uint64_t* n_bad) {
+  if (!ctx || !out || dim == 0 || dim > 65535 || n_elems >= 0xFFFFFFF0ull || !n_layers || !node_blob || !node_off ||
+      !node_ids || !n_nodes || entry_point >= (int64_t)n_elems || (n_vec && (!vec_blob || !vec_off)))
+    return SDB_EINVAL;
+  SDB_TRY(check_index_kind("sdb_hnsw_load_staged_typed", dim, metric, (int)vt));
+  *out = nullptr;
+  return hnsw_load_staged_impl(ctx, dim, metric, vt, (int)vt, n_elems, vec_blob, vec_off, vec_ids, n_vec, n_layers,
+                               node_blob, node_off, node_ids, n_nodes, entry_point, out, n_bad);
+}
+
 sdb_status sdb_hnsw_select_neighbors(sdb_ctx* ctx, const float* d_vectors, uint32_t dim, sdb_metric metric, uint64_t row0,
                                      uint64_t n, const uint64_t* d_cand, const uint32_t* d_cand_cnt, uint32_t kc,
                                      uint32_t m_max, int presorted, uint32_t* d_out, uint32_t* d_out_cnt) {
@@ -1307,51 +1641,77 @@ sdb_status sdb_hnsw_select_neighbors_ids(sdb_ctx* ctx, const float* d_vectors, u
 }
 
 using WalkKernel = void (*)(HnswParams);
-static WalkKernel walk_kernel(sdb_metric metric, int occ) {
-  switch (metric) {
-    case SDB_COSINE: return occ >= 8 ? hnsw_search_kernel<SDB_COSINE, 8> : occ <= 4 ? hnsw_search_kernel<SDB_COSINE, 4> : hnsw_search_kernel<SDB_COSINE, 6>;
-    case SDB_MANHATTAN: return hnsw_search_kernel<SDB_MANHATTAN, 1>;
-    case SDB_CHEBYSHEV: return hnsw_search_kernel<SDB_CHEBYSHEV, 1>;
-    case SDB_HAMMING: return hnsw_search_kernel<SDB_HAMMING, 1>;
-    case SDB_MINKOWSKI: return hnsw_search_kernel<SDB_MINKOWSKI, 1>;
-    case SDB_PEARSON: return hnsw_search_kernel<SDB_PEARSON, 1>;
-    case SDB_JACCARD: return hnsw_search_kernel<SDB_JACCARD, 1>;
-    default: return hnsw_search_kernel<SDB_EUCLIDEAN, 1>;
-  }
+static WalkKernel walk_kernel(sdb_metric metric, sdb_vector_type vt, int occ) {
+  if (vt == SDB_VT_F32 && metric == SDB_COSINE)
+    return occ >= 8 ? hnsw_search_kernel<SDB_COSINE, 8, float> : occ <= 4 ? hnsw_search_kernel<SDB_COSINE, 4, float> : hnsw_search_kernel<SDB_COSINE, 6, float>;
+  return with_vt(vt, [&](auto tag) -> WalkKernel {
+    using T = decltype(tag);
+    switch (metric) {
+      case SDB_COSINE: return hnsw_search_kernel<SDB_COSINE, is_f32_v<T> ? 6 : 1, T>;  // (F32: returned above)
+      case SDB_MANHATTAN: return hnsw_search_kernel<SDB_MANHATTAN, 1, T>;
+      case SDB_CHEBYSHEV: return hnsw_search_kernel<SDB_CHEBYSHEV, 1, T>;
+      case SDB_HAMMING: return hnsw_search_kernel<SDB_HAMMING, 1, T>;
+      case SDB_MINKOWSKI: return hnsw_search_kernel<SDB_MINKOWSKI, 1, T>;
+      case SDB_PEARSON: return hnsw_search_kernel<SDB_PEARSON, 1, T>;
+      case SDB_JACCARD: return hnsw_search_kernel<SDB_JACCARD, 1, T>;
+      default: return hnsw_search_kernel<SDB_EUCLIDEAN, 1, T>;
+    }
+  });
 }
+// bytes of a staged query and of the distance scratch (the kernel's per-warp layout)
+static size_t walk_q_bytes(const sdb_hnsw* h) {
+  if (h->vt == SDB_VT_F32) return sizeof(float) * hn_q_floats(h->dim, h->metric == SDB_COSINE);
+  return hn_q_bytes_typed(h->dim, h->metric == SDB_JACCARD ? jkey_size(h->vt) : vt_size(h->vt));
+}
+static size_t walk_tile_bytes(const sdb_hnsw* h) { return hn_tile_bytes(h->metric == SDB_COSINE && h->vt == SDB_VT_F32); }
 
-// per-query (or per-pending-vector) state of PEARSON / JACCARD, computed with the element-side kernels
+// per-query (or per-pending-vector) state of PEARSON / JACCARD (and COSINE of the types other than F32), computed with
+// the element-side kernels
 struct BatchState {
   double* mean = nullptr;
   double* sx2 = nullptr;
-  uint32_t* bits = nullptr;
+  void* bits = nullptr;
   uint32_t* nbits = nullptr;
+  double* norm = nullptr;
   void release(cudaStream_t st) {
     if (mean) cudaFreeAsync(mean, st);
     if (sx2) cudaFreeAsync(sx2, st);
     if (bits) cudaFreeAsync(bits, st);
     if (nbits) cudaFreeAsync(nbits, st);
-    mean = sx2 = nullptr;
-    bits = nbits = nullptr;
+    if (norm) cudaFreeAsync(norm, st);
+    mean = sx2 = norm = nullptr;
+    bits = nullptr;
+    nbits = nullptr;
   }
 };
-static sdb_status batch_state(Ctx* ctx, sdb_metric metric, const float* d_v, uint64_t rows, uint32_t dim, BatchState& bs,
-                              cudaStream_t st) {
+static sdb_status batch_state(Ctx* ctx, sdb_metric metric, sdb_vector_type vt, const void* d_v, uint64_t rows,
+                              uint32_t dim, BatchState& bs, cudaStream_t st) {
   if (!rows) return SDB_OK;
+  const unsigned grid = (unsigned)((rows + 127) / 128);
   if (metric == SDB_PEARSON) {
     SDB_CUDA(cudaMallocAsync(&bs.mean, sizeof(double) * rows, st));
     SDB_CUDA(cudaMallocAsync(&bs.sx2, sizeof(double) * rows, st));
-    pearson_stats_kernel<<<(unsigned)((rows + 127) / 128), 128, 0, st>>>(d_v, dim, rows, bs.mean, bs.sx2);
+    with_vt(vt, [&](auto tag) {
+      using T = decltype(tag);
+      pearson_stats_kernel<T><<<grid, 128, 0, st>>>(static_cast<const T*>(d_v), dim, rows, bs.mean, bs.sx2);
+    });
     count_launch(ctx);
   } else if (metric == SDB_JACCARD) {
-    SDB_CUDA(cudaMallocAsync(&bs.bits, sizeof(uint32_t) * rows * dim, st));
+    SDB_CUDA(cudaMallocAsync(&bs.bits, jkey_size(vt) * rows * dim, st));
     SDB_CUDA(cudaMallocAsync(&bs.nbits, sizeof(uint32_t) * rows, st));
-    SDB_TRY(jaccard_prepare(ctx, d_v, rows, dim, bs.bits, bs.nbits, st));
+    SDB_TRY(jaccard_prepare_typed(ctx, vt, d_v, rows, dim, bs.bits, bs.nbits, st));
+  } else if (metric == SDB_COSINE && vt != SDB_VT_F32) {
+    SDB_CUDA(cudaMallocAsync(&bs.norm, sizeof(double) * rows, st));
+    with_vt(vt, [&](auto tag) {
+      using T = decltype(tag);
+      hnsw_norm_kernel<T><<<grid, 128, 0, st>>>(static_cast<const T*>(d_v), dim, rows, bs.norm);
+    });
+    count_launch(ctx);
   }
   return SDB_OK;
 }
 
-static sdb_status hnsw_search_impl(sdb_hnsw* h, const float* queries, uint32_t nq, uint32_t k, uint32_t ef,
+static sdb_status hnsw_search_impl(sdb_hnsw* h, const void* queries, uint32_t nq, uint32_t k, uint32_t ef,
                                    const uint8_t* truthy, const uint8_t* noexp, uint64_t* out_elems, double* out_dist,
                                    uint32_t* out_count, uint64_t* out_counters, bool device_io = false) {
   if (!h || (nq && (!queries || !out_count)) || (nq && k && (!out_elems || !out_dist))) return SDB_EINVAL;
@@ -1381,11 +1741,11 @@ static sdb_status hnsw_search_impl(sdb_hnsw* h, const float* queries, uint32_t n
   if (truthy) {
     ccap = 16 * ef + 34;
     if (ccap < 1024) ccap = 1024;
-    const size_t fixed = sizeof(float) * hn_q_floats(h->dim, h->metric == SDB_COSINE) + hn_tile_bytes(h->metric == SDB_COSINE) + 12 * (size_t)wcap + 64 + 16;
+    const size_t fixed = walk_q_bytes(h) + walk_tile_bytes(h) + 12 * (size_t)wcap + 64 + 16;
     const size_t room = (220 * 1024) / HN_WARPS;
     if (fixed + 12 * (size_t)ccap > room) ccap = room > fixed + 12 * (2 * (size_t)ef + 34) ? (uint32_t)((room - fixed) / 12) : 2 * ef + 34;
   }
-  size_t per_warp = sizeof(float) * hn_q_floats(h->dim, h->metric == SDB_COSINE) + hn_tile_bytes(h->metric == SDB_COSINE) + 12 * (size_t)(ccap + wcap) + 64;
+  size_t per_warp = walk_q_bytes(h) + walk_tile_bytes(h) + 12 * (size_t)(ccap + wcap) + 64;
   per_warp = (per_warp + 15) & ~size_t(15);
   const size_t smem = per_warp * HN_WARPS;
   if (smem > 220 * 1024) {
@@ -1394,7 +1754,7 @@ static sdb_status hnsw_search_impl(sdb_hnsw* h, const float* queries, uint32_t n
   }
   // cosine: 8 lanes per row keep ~16 loads in flight per lane; 80 registers (6 blocks per SM) holds that without spills
   const int occ = getenv("SDB_HNSW_OCC") ? atoi(getenv("SDB_HNSW_OCC")) : 6;  // measured r2 (1M x 768, ef 64): 6 -> 1.40M QPS, 4 -> 1.32M, 8 -> 1.02M (spills)
-  const WalkKernel kern = walk_kernel(h->metric, occ);
+  const WalkKernel kern = walk_kernel(h->metric, h->vt, occ);
   SDB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   // the walk gets nothing from L1 (0.7 % hit rate): give the whole array to shared memory, or the driver's default
   // carve-out (135 KB) caps the kernel at 5 blocks per SM
@@ -1424,23 +1784,24 @@ static sdb_status hnsw_search_impl(sdb_hnsw* h, const float* queries, uint32_t n
     SDB_CUDA(cudaMemsetAsync(h->d_visited, 0, sizeof(uint64_t) * ((size_t)h->n_tables << tl), st));
     h->gen = 1;
   }
-  float* d_q = nullptr;
+  const size_t esz = vt_size(h->vt);
+  void* d_q = nullptr;
   uint64_t* d_elems = nullptr;
   double* d_dist = nullptr;
   uint32_t* d_cnt = nullptr;
   uint64_t* d_ctr = nullptr;
   uint32_t* d_ovf = nullptr;
   if (device_io) {  // queries and outputs already live on the device (index construction): no staging
-    d_q = const_cast<float*>(queries);
+    d_q = const_cast<void*>(queries);
     d_elems = out_elems;
     d_dist = out_dist;
     d_cnt = out_count;
   } else {
-    SDB_CUDA(cudaMallocAsync(&d_q, sizeof(float) * (size_t)nq * h->dim, st));
+    SDB_CUDA(cudaMallocAsync(&d_q, esz * (size_t)nq * h->dim, st));
     SDB_CUDA(cudaMallocAsync(&d_elems, sizeof(uint64_t) * (size_t)nq * k, st));
     SDB_CUDA(cudaMallocAsync(&d_dist, sizeof(double) * (size_t)nq * k, st));
     SDB_CUDA(cudaMallocAsync(&d_cnt, sizeof(uint32_t) * nq, st));
-    SDB_CUDA(cudaMemcpyAsync(d_q, queries, sizeof(float) * (size_t)nq * h->dim, cudaMemcpyHostToDevice, st));
+    SDB_CUDA(cudaMemcpyAsync(d_q, queries, esz * (size_t)nq * h->dim, cudaMemcpyHostToDevice, st));
   }
   SDB_CUDA(cudaMallocAsync(&d_ctr, sizeof(uint64_t) * 2 * nq, st));
   SDB_CUDA(cudaMallocAsync(&d_ovf, 4, st));
@@ -1486,11 +1847,12 @@ static sdb_status hnsw_search_impl(sdb_hnsw* h, const float* queries, uint32_t n
   P.e_bits = h->d_bits;
   P.e_nbits = h->d_nbits;
   BatchState qs;
-  const sdb_status qrc = batch_state(ctx, h->metric, d_q, nq, h->dim, qs, st);
+  const sdb_status qrc = batch_state(ctx, h->metric, h->vt, d_q, nq, h->dim, qs, st);
   P.q_mean = qs.mean;
   P.q_sx2 = qs.sx2;
   P.q_bits = qs.bits;
   P.q_nbits = qs.nbits;
+  P.q_norm = qs.norm;
   if (qrc == SDB_OK) {
     kern<<<grid, HN_WARPS * 32, smem, st>>>(P);
     count_launch(ctx);
@@ -1536,32 +1898,35 @@ static sdb_status hnsw_search_impl(sdb_hnsw* h, const float* queries, uint32_t n
 
 // Distance::calculate(&query, &vector) for n host vectors on the context's stream (the caller holds the lock that
 // serialises it): typed_distance_kernel plus the PEARSON / JACCARD state of the query and of the vectors.
-static sdb_status typed_distances(Ctx* ctx, sdb_metric metric, double minkowski_p, uint32_t dim, const float* query,
-                                  const float* vectors, uint64_t n, double* out, const char* what) {
+static sdb_status typed_distances(Ctx* ctx, sdb_metric metric, sdb_vector_type vt, double minkowski_p, uint32_t dim,
+                                  const void* query, const void* vectors, uint64_t n, double* out, const char* what) {
   cudaStream_t st = ctx->stream;
-  float *d_q = nullptr, *d_v = nullptr;
+  const size_t esz = vt_size(vt);
+  void *d_q = nullptr, *d_v = nullptr;
   double* d_o = nullptr;
   BatchState qs, vs;
   auto run = [&]() -> sdb_status {
-    SDB_CUDA(cudaMallocAsync(&d_q, sizeof(float) * dim, st));
-    SDB_CUDA(cudaMallocAsync(&d_v, sizeof(float) * n * dim, st));
+    SDB_CUDA(cudaMallocAsync(&d_q, esz * dim, st));
+    SDB_CUDA(cudaMallocAsync(&d_v, esz * n * dim, st));
     SDB_CUDA(cudaMallocAsync(&d_o, sizeof(double) * n, st));
-    SDB_CUDA(cudaMemcpyAsync(d_q, query, sizeof(float) * dim, cudaMemcpyHostToDevice, st));
-    SDB_CUDA(cudaMemcpyAsync(d_v, vectors, sizeof(float) * n * dim, cudaMemcpyHostToDevice, st));
-    SDB_TRY(batch_state(ctx, metric, d_q, 1, dim, qs, st));
-    SDB_TRY(batch_state(ctx, metric, d_v, n, dim, vs, st));
+    SDB_CUDA(cudaMemcpyAsync(d_q, query, esz * dim, cudaMemcpyHostToDevice, st));
+    SDB_CUDA(cudaMemcpyAsync(d_v, vectors, esz * n * dim, cudaMemcpyHostToDevice, st));
+    SDB_TRY(batch_state(ctx, metric, vt, d_q, 1, dim, qs, st));
+    SDB_TRY(batch_state(ctx, metric, vt, d_v, n, dim, vs, st));
     TypedArgs A;
-    A.q = d_q;
-    A.vecs = d_v;
+    A.q = static_cast<const float*>(d_q);
+    A.vecs = static_cast<const float*>(d_v);
     A.dim = dim;
     A.n = n;
     A.out = d_o;
     A.mq.p = minkowski_p;
     A.v_mean = vs.mean;
     A.v_sx2 = vs.sx2;
-    A.q_bits = qs.bits;
-    A.v_bits = vs.bits;
+    A.q_bits = static_cast<const uint32_t*>(qs.bits);
+    A.v_bits = static_cast<const uint32_t*>(vs.bits);
     A.v_nbits = vs.nbits;
+    A.v_norm = vs.norm;
+    A.q_norm = qs.norm;
     if (metric == SDB_PEARSON) {  // the query's scalars travel by value
       SDB_CUDA(cudaMemcpyAsync(&A.mq.mean, qs.mean, sizeof(double), cudaMemcpyDeviceToHost, st));
       SDB_CUDA(cudaMemcpyAsync(&A.mq.sx2, qs.sx2, sizeof(double), cudaMemcpyDeviceToHost, st));
@@ -1572,16 +1937,19 @@ static sdb_status typed_distances(Ctx* ctx, sdb_metric metric, double minkowski_
       SDB_CUDA(cudaStreamSynchronize(st));
     }
     const unsigned grid = (unsigned)((n + 127) / 128);
-    switch (metric) {
-      case SDB_COSINE: typed_distance_kernel<SDB_COSINE><<<grid, 128, 0, st>>>(A); break;
-      case SDB_EUCLIDEAN: typed_distance_kernel<SDB_EUCLIDEAN><<<grid, 128, 0, st>>>(A); break;
-      case SDB_MANHATTAN: typed_distance_kernel<SDB_MANHATTAN><<<grid, 128, 0, st>>>(A); break;
-      case SDB_CHEBYSHEV: typed_distance_kernel<SDB_CHEBYSHEV><<<grid, 128, 0, st>>>(A); break;
-      case SDB_HAMMING: typed_distance_kernel<SDB_HAMMING><<<grid, 128, 0, st>>>(A); break;
-      case SDB_MINKOWSKI: typed_distance_kernel<SDB_MINKOWSKI><<<grid, 128, 0, st>>>(A); break;
-      case SDB_PEARSON: typed_distance_kernel<SDB_PEARSON><<<grid, 128, 0, st>>>(A); break;
-      case SDB_JACCARD: typed_distance_kernel<SDB_JACCARD><<<grid, 128, 0, st>>>(A); break;
-    }
+    with_vt(vt, [&](auto tag) {
+      using T = decltype(tag);
+      switch (metric) {
+        case SDB_COSINE: typed_distance_kernel<SDB_COSINE, T><<<grid, 128, 0, st>>>(A); break;
+        case SDB_EUCLIDEAN: typed_distance_kernel<SDB_EUCLIDEAN, T><<<grid, 128, 0, st>>>(A); break;
+        case SDB_MANHATTAN: typed_distance_kernel<SDB_MANHATTAN, T><<<grid, 128, 0, st>>>(A); break;
+        case SDB_CHEBYSHEV: typed_distance_kernel<SDB_CHEBYSHEV, T><<<grid, 128, 0, st>>>(A); break;
+        case SDB_HAMMING: typed_distance_kernel<SDB_HAMMING, T><<<grid, 128, 0, st>>>(A); break;
+        case SDB_MINKOWSKI: typed_distance_kernel<SDB_MINKOWSKI, T><<<grid, 128, 0, st>>>(A); break;
+        case SDB_PEARSON: typed_distance_kernel<SDB_PEARSON, T><<<grid, 128, 0, st>>>(A); break;
+        case SDB_JACCARD: typed_distance_kernel<SDB_JACCARD, T><<<grid, 128, 0, st>>>(A); break;
+      }
+    });
     count_launch(ctx);
     SDB_CUDA(cudaGetLastError());
     SDB_CUDA(cudaMemcpyAsync(out, d_o, sizeof(double) * n, cudaMemcpyDeviceToHost, st));
@@ -1610,15 +1978,15 @@ sdb_status sdb_vec_distance_f32(sdb_ctx* ctx, sdb_metric metric, uint32_t dim, c
   if (n == 0) return SDB_OK;
   std::lock_guard<std::mutex> guard(ctx->mu);
   SDB_CUDA(cudaSetDevice(ctx->device));
-  return typed_distances(ctx, metric, 3.0, dim, query, vectors, n, out, "sdb_vec_distance_f32");
+  return typed_distances(ctx, metric, SDB_VT_F32, 3.0, dim, query, vectors, n, out, "sdb_vec_distance_f32");
 }
 
-sdb_status sdb_hnsw_distance(sdb_hnsw* h, const float* query, const float* vectors, uint64_t n, double* out) {
+sdb_status sdb_hnsw_distance(sdb_hnsw* h, const void* query, const void* vectors, uint64_t n, double* out) {
   if (!h || (n && (!query || !vectors || !out))) return SDB_EINVAL;
   if (n == 0) return SDB_OK;
   std::lock_guard<std::mutex> guard(h->mu);
   SDB_CUDA(cudaSetDevice(h->ctx->device));
-  return typed_distances(h->ctx, h->metric, h->minkowski_p, h->dim, query, vectors, n, out, "sdb_hnsw_distance");
+  return typed_distances(h->ctx, h->metric, h->vt, h->minkowski_p, h->dim, query, vectors, n, out, "sdb_hnsw_distance");
 }
 
 sdb_status sdb_hnsw_set_minkowski_order(sdb_hnsw* h, double order) {
@@ -1628,17 +1996,17 @@ sdb_status sdb_hnsw_set_minkowski_order(sdb_hnsw* h, double order) {
   return SDB_OK;
 }
 
-sdb_status sdb_hnsw_search(sdb_hnsw* h, const float* queries, uint32_t nq, uint32_t k, uint32_t ef, uint64_t* out_elems,
+sdb_status sdb_hnsw_search(sdb_hnsw* h, const void* queries, uint32_t nq, uint32_t k, uint32_t ef, uint64_t* out_elems,
                            double* out_dist, uint32_t* out_count, uint64_t* out_counters) {
   return hnsw_search_impl(h, queries, nq, k, ef, nullptr, nullptr, out_elems, out_dist, out_count, out_counters);
 }
 
-sdb_status sdb_hnsw_search_device(sdb_hnsw* h, const float* d_queries, uint32_t nq, uint32_t k, uint32_t ef,
+sdb_status sdb_hnsw_search_device(sdb_hnsw* h, const void* d_queries, uint32_t nq, uint32_t k, uint32_t ef,
                                   uint64_t* d_out_elems, double* d_out_dist, uint32_t* d_out_count) {
   return hnsw_search_impl(h, d_queries, nq, k, ef, nullptr, nullptr, d_out_elems, d_out_dist, d_out_count, nullptr, true);
 }
 
-sdb_status sdb_hnsw_search_pending(sdb_hnsw* h, const float* queries, uint32_t nq, uint32_t k, uint32_t ef,
+sdb_status sdb_hnsw_search_pending(sdb_hnsw* h, const void* queries, uint32_t nq, uint32_t k, uint32_t ef,
                                    const uint8_t* all_docs_pending, uint64_t* out_elems, double* out_dist,
                                    uint32_t* out_count, uint64_t* out_counters) {
   if (!all_docs_pending) {
@@ -1648,7 +2016,7 @@ sdb_status sdb_hnsw_search_pending(sdb_hnsw* h, const float* queries, uint32_t n
   return hnsw_search_impl(h, queries, nq, k, ef, nullptr, all_docs_pending, out_elems, out_dist, out_count, out_counters);
 }
 
-sdb_status sdb_hnsw_search_filtered(sdb_hnsw* h, const float* queries, uint32_t nq, uint32_t k, uint32_t ef,
+sdb_status sdb_hnsw_search_filtered(sdb_hnsw* h, const void* queries, uint32_t nq, uint32_t k, uint32_t ef,
                                     const uint8_t* truthy, uint64_t* out_elems, double* out_dist, uint32_t* out_count,
                                     uint64_t* out_counters) {
   if (!truthy) {

@@ -350,7 +350,7 @@ sdb_status exclusive_scan(Ctx* ctx, const uint64_t* d_in, uint64_t* d_out, uint6
 // stage.cu: He / Hn value decoders (host blobs in, device arrays out)
 sdb_status stage_decode_vectors(Ctx* ctx, const uint8_t* blob, const uint64_t* off, const uint64_t* ids, uint64_t n,
                                 uint32_t dim, sdb_dtype out_dtype, uint64_t n_rows, void* d_out, uint8_t* d_present,
-                                uint64_t* n_bad, cudaStream_t st);
+                                uint64_t* n_bad, cudaStream_t st, int native = -1);  // native: see stage_vectors_kernel
 sdb_status stage_decode_nodes(Ctx* ctx, const uint8_t* blob, const uint64_t* off, const uint64_t* node_ids, uint64_t n,
                               uint64_t n_elems, uint64_t** d_row_ptr_out, uint32_t** d_col_idx_out, uint64_t* n_edges,
                               uint64_t* n_bad, cudaStream_t st);

@@ -50,7 +50,9 @@ __device__ __forceinline__ bool read_varint(const uint8_t*& p, const uint8_t* en
 }
 
 // ---- He: one warp per value ----------------------------------------------------------------------
-template <typename OUT>
+// VARIANT < 0: every variant is converted to OUT (f32 / f64; a value OUT cannot represent counts as bad).  VARIANT >= 0:
+// OUT is that variant's own element type and only values of that variant are accepted (native typed indexes).
+template <typename OUT, int VARIANT = -1>
 __global__ void __launch_bounds__(256) stage_vectors_kernel(const uint8_t* __restrict__ blob, uint64_t blob_base,
                                                             const uint64_t* __restrict__ off,
                                                             const uint64_t* __restrict__ ids, uint64_t id0, uint64_t n,
@@ -66,7 +68,7 @@ __global__ void __launch_bounds__(256) stage_vectors_kernel(const uint8_t* __res
     const uint64_t row = ids ? ids[v] : id0 + v;
     uint64_t rev = 0, variant = 0, len = 0;
     bool ok = read_varint(p, end, rev) && rev == 1 && read_varint(p, end, variant) && variant <= 4 &&
-              read_varint(p, end, len) && len == dim && row < n_rows;
+              (VARIANT < 0 || variant == (uint64_t)VARIANT) && read_varint(p, end, len) && len == dim && row < n_rows;
     const uint32_t esz = (variant == 0 || variant == 2) ? 8u : variant == 4 ? 2u : 4u;
     ok = ok && (uint64_t)(end - p) == (uint64_t)dim * esz;
     if (!ok) {  // uniform across the warp (every lane parsed the same header)
@@ -175,7 +177,7 @@ static sdb_status blob_to_device(const uint8_t* blob, uint64_t bytes, uint8_t** 
 
 sdb_status stage_decode_vectors(Ctx* ctx, const uint8_t* blob, const uint64_t* off, const uint64_t* ids, uint64_t n,
                                 uint32_t dim, sdb_dtype out_dtype, uint64_t n_rows, void* d_out, uint8_t* d_present,
-                                uint64_t* n_bad, cudaStream_t st) {
+                                uint64_t* n_bad, cudaStream_t st, int native) {
   unsigned long long* d_bad = nullptr;
   SDB_CUDA(cudaMalloc(&d_bad, 8));
   SDB_CUDA(cudaMemsetAsync(d_bad, 0, 8, st));
@@ -219,12 +221,21 @@ sdb_status stage_decode_vectors(Ctx* ctx, const uint8_t* blob, const uint64_t* o
     if (ids) chk(cudaMemcpyAsync(d_ids, ids + v0, 8 * nv, cudaMemcpyHostToDevice, st));
     if (rc != SDB_OK) break;
     const unsigned grid = (unsigned)std::min<uint64_t>((nv + 7) / 8, (uint64_t)ctx->sm_count * 16);
-    if (out_dtype == SDB_F32)
-      stage_vectors_kernel<float><<<grid, 256, 0, st>>>(d_blob, off[v0], d_off, ids ? d_ids : nullptr, v0, nv, dim, n_rows,
-                                                        (float*)d_out, d_present, d_bad);
-    else
-      stage_vectors_kernel<double><<<grid, 256, 0, st>>>(d_blob, off[v0], d_off, ids ? d_ids : nullptr, v0, nv, dim,
-                                                         n_rows, (double*)d_out, d_present, d_bad);
+    const uint64_t* d_ids_or_null = ids ? d_ids : nullptr;
+    switch (native) {  // sdb_vector_type numbers = SerializedVector variants
+      case 0: stage_vectors_kernel<double, 0><<<grid, 256, 0, st>>>(d_blob, off[v0], d_off, d_ids_or_null, v0, nv, dim, n_rows, (double*)d_out, d_present, d_bad); break;
+      case 1: stage_vectors_kernel<float, 1><<<grid, 256, 0, st>>>(d_blob, off[v0], d_off, d_ids_or_null, v0, nv, dim, n_rows, (float*)d_out, d_present, d_bad); break;
+      case 2: stage_vectors_kernel<long long, 2><<<grid, 256, 0, st>>>(d_blob, off[v0], d_off, d_ids_or_null, v0, nv, dim, n_rows, (long long*)d_out, d_present, d_bad); break;
+      case 3: stage_vectors_kernel<int, 3><<<grid, 256, 0, st>>>(d_blob, off[v0], d_off, d_ids_or_null, v0, nv, dim, n_rows, (int*)d_out, d_present, d_bad); break;
+      case 4: stage_vectors_kernel<short, 4><<<grid, 256, 0, st>>>(d_blob, off[v0], d_off, d_ids_or_null, v0, nv, dim, n_rows, (short*)d_out, d_present, d_bad); break;
+      default:
+        if (out_dtype == SDB_F32)
+          stage_vectors_kernel<float><<<grid, 256, 0, st>>>(d_blob, off[v0], d_off, ids ? d_ids : nullptr, v0, nv, dim, n_rows,
+                                                            (float*)d_out, d_present, d_bad);
+        else
+          stage_vectors_kernel<double><<<grid, 256, 0, st>>>(d_blob, off[v0], d_off, ids ? d_ids : nullptr, v0, nv, dim,
+                                                             n_rows, (double*)d_out, d_present, d_bad);
+    }
     count_launch(ctx);
     chk(cudaGetLastError());
     chk(cudaStreamSynchronize(st));  // the host source of the next chunk's copy may be pageable: keep it simple

@@ -16,6 +16,50 @@ import numpy as np
 
 from . import _lib as L
 
+# numpy element type of each sdb_vector_type (VectorType of the index definition)
+VT_DTYPE = {"F64": np.float64, "F32": np.float32, "I64": np.int64, "I32": np.int32, "I16": np.int16}
+
+
+def _int_of(x, vector_type, info):
+    """one Number -> the integer type (val/number.rs:136-166, num-traits' ToPrimitive): an integer must fit, a float is
+    truncated toward zero and must then fit (NaN and infinities never do)"""
+    if isinstance(x, (int, np.integer)) and not isinstance(x, bool):
+        v = int(x)
+    else:
+        f = float(x)
+        if f != f or f in (float("inf"), float("-inf")):
+            raise L.SdbError(L.SDB_EINVAL, f"{f} cannot be converted to {vector_type}")
+        v = int(f)  # truncation toward zero
+    if not info.min <= v <= info.max:
+        raise L.SdbError(L.SDB_EINVAL, f"{x} is out of the range of {vector_type}")
+    return v
+
+
+def to_vector_type(values, vector_type):
+    """Vector::try_from_vector (hnsw/index.rs:286, vector.rs:592-621): the numbers of a query, element or pending vector
+    as the index's vector type.  F32 / F64: a float conversion (np.float32 / np.float64).  Integer types: an integer
+    keeps its value and must fit; a float is truncated toward zero; anything out of range, or NaN, raises
+    SdbError(SDB_EINVAL)."""
+    vt = vector_type.upper()
+    dt = np.dtype(VT_DTYPE[vt])
+    if dt.kind == "f":
+        return np.ascontiguousarray(values, dt)
+    info = np.iinfo(dt)
+    a = np.asarray(values)
+    if a.dtype.kind in "iu":  # exact, range-checked without a float round trip (an I64 above 2^53 survives)
+        if a.size and (int(a.min()) < info.min or int(a.max()) > info.max):
+            raise L.SdbError(L.SDB_EINVAL, f"a value is out of the range of {vt}")
+        return np.ascontiguousarray(a.astype(dt))
+    if a.dtype.kind == "O":
+        flat = [_int_of(x, vt, info) for x in a.ravel().tolist()]
+        return np.array(flat, dt).reshape(a.shape)
+    f = a.astype(np.float64)
+    t = np.trunc(f)
+    lim = float(2 ** (8 * dt.itemsize - 1))
+    if not np.all(np.isfinite(t) & (t >= -lim) & (t < lim)):
+        raise L.SdbError(L.SDB_EINVAL, f"a value is NaN or out of the range of {vt}")
+    return np.ascontiguousarray(t.astype(dt))
+
 
 class KnnResultBuilder:
     """idx/trees/knn.rs:363-437: a BTreeSet<(FloatKey(dist), VectorId)> capped at knn entries."""
@@ -39,12 +83,17 @@ class KnnResultBuilder:
 
 
 class HnswIndex:
-    def __init__(self, ctx, vectors, layers, entry_point, metric="EUCLIDEAN", elem_docs=None, minkowski_order=3.0):
-        """vectors (n, dim) f32; layers = [(row_ptr u64[n+1], col_idx u32[e]), ...] layer 0 first;
-        elem_docs: optional list of doc-id lists per element (identical vectors share one element:
+    def __init__(self, ctx, vectors, layers, entry_point, metric="EUCLIDEAN", elem_docs=None, minkowski_order=3.0,
+                 vector_type="F32"):
+        """vectors (n, dim), converted to the vector type; layers = [(row_ptr u64[n+1], col_idx u32[e]), ...] layer 0
+        first; elem_docs: optional list of doc-id lists per element (identical vectors share one element:
         hnsw/docs.rs:161-176); default = one doc per element with the same id.  metric: any Distance
-        (DIST ... of the index definition); minkowski_order: p of Distance::Minkowski(p), used by MINKOWSKI only."""
-        vec = np.ascontiguousarray(vectors, np.float32)
+        (DIST ... of the index definition); minkowski_order: p of Distance::Minkowski(p), used by MINKOWSKI only;
+        vector_type: TYPE ... of the index definition (F64, F32, I64, I32, I16), the arithmetic of every distance."""
+        self.vector_type = vector_type.upper()
+        if self.vector_type not in L.VTYPE:
+            raise L.SdbError(L.SDB_EINVAL, f"unknown vector type {vector_type!r}")
+        vec = to_vector_type(vectors, self.vector_type)
         self.n, self.dim = vec.shape
         self.ctx, self.metric = ctx, metric.upper()
         self.elem_docs = elem_docs
@@ -56,8 +105,8 @@ class HnswIndex:
         RP = (C.c_void_p * nl)(*[a.ctypes.data for a in rps])
         CI = (C.c_void_p * nl)(*[a.ctypes.data for a in cis])
         self.h = C.c_void_p()
-        L.check(L.lib().sdb_hnsw_load(ctx.h, self.dim, L.METRIC[self.metric], self.n, C.c_void_p(vec.ctypes.data), nl,
-                                      RP, CI, int(entry_point), C.byref(self.h)))
+        L.check(L.lib().sdb_hnsw_load_typed(ctx.h, self.dim, L.METRIC[self.metric], L.VTYPE[self.vector_type], self.n,
+                                            C.c_void_p(vec.ctypes.data), nl, RP, CI, int(entry_point), C.byref(self.h)))
         self._set_order(minkowski_order)
 
     def _set_order(self, minkowski_order):
@@ -70,7 +119,7 @@ class HnswIndex:
         float32 (n, dim) tensor, layers_dev = [(row_ptr int64 (n+1), col_idx int32)] layer 0 first.  The tensors must
         stay alive (they are kept on the object)."""
         self = cls.__new__(cls)
-        self.ctx, self.metric, self.elem_docs = ctx, metric.upper(), elem_docs
+        self.ctx, self.metric, self.elem_docs, self.vector_type = ctx, metric.upper(), elem_docs, "F32"
         self.n, self.dim = int(x_dev.shape[0]), int(x_dev.shape[1])
         self.pendings, self.versions = [], None
         self._keep = (x_dev, layers_dev)
@@ -85,10 +134,11 @@ class HnswIndex:
 
     @classmethod
     def from_kv(cls, ctx, dim, state_value, he_items, hn_items_per_layer, metric="EUCLIDEAN", elem_docs=None,
-                minkowski_order=3.0):
+                minkowski_order=3.0, vector_type="F32"):
         """Loads the index straight from raw KV values (staging.py): `state_value` = the Hs value, `he_items` =
         [(element id, He value)], `hn_items_per_layer[l]` = [(node id, Hn value)] of layer l (0 first), each in key
-        order.  Decoding happens on the GPU (sdb_hnsw_load_staged).  Mirrors Hnsw::check_state + HnswLayer::load
+        order.  Decoding happens on the GPU (sdb_hnsw_load_staged, sdb_hnsw_load_staged_typed for the other vector
+        types: there an He value of another type counts in n_bad).  Mirrors Hnsw::check_state + HnswLayer::load
         (hnsw/mod.rs:187-224, hnsw/layer.rs:505-560) for indexes without legacy Hl chunks."""
         from . import staging as S
         st = S.parse_hnsw_state(state_value)
@@ -99,6 +149,9 @@ class HnswIndex:
             raise L.SdbError(L.SDB_EINVAL, f"state names {nl} layers, {len(hn_items_per_layer)} given")
         self = cls.__new__(cls)
         self.ctx, self.metric, self.dim, self.elem_docs = ctx, metric.upper(), int(dim), elem_docs
+        self.vector_type = vector_type.upper()
+        if self.vector_type not in L.VTYPE:
+            raise L.SdbError(L.SDB_EINVAL, f"unknown vector type {vector_type!r}")
         self.pendings = []
         self.versions = [st["layer0"]["version"]] + [l["version"] for l in st["layers"]]
         self.n = int(st["next_element_id"])
@@ -111,9 +164,15 @@ class HnswIndex:
         self.h = C.c_void_p()
         bad = C.c_uint64(0)
         ep = -1 if st["enter_point"] is None else int(st["enter_point"])
-        L.check(L.lib().sdb_hnsw_load_staged(ctx.h, self.dim, L.METRIC[self.metric], self.n, C.c_void_p(vb.ctypes.data),
-                                             C.c_void_p(vo.ctypes.data), C.c_void_p(vi.ctypes.data), len(he_items), nl,
-                                             NB, NO, NI, NN, ep, C.byref(self.h), C.byref(bad)))
+        if self.vector_type == "F32":
+            L.check(L.lib().sdb_hnsw_load_staged(ctx.h, self.dim, L.METRIC[self.metric], self.n, C.c_void_p(vb.ctypes.data),
+                                                 C.c_void_p(vo.ctypes.data), C.c_void_p(vi.ctypes.data), len(he_items), nl,
+                                                 NB, NO, NI, NN, ep, C.byref(self.h), C.byref(bad)))
+        else:
+            L.check(L.lib().sdb_hnsw_load_staged_typed(ctx.h, self.dim, L.METRIC[self.metric], L.VTYPE[self.vector_type],
+                                                       self.n, C.c_void_p(vb.ctypes.data), C.c_void_p(vo.ctypes.data),
+                                                       C.c_void_p(vi.ctypes.data), len(he_items), nl, NB, NO, NI, NN, ep,
+                                                       C.byref(self.h), C.byref(bad)))
         self.n_bad = bad.value
         self._set_order(minkowski_order)
         return self
@@ -131,8 +190,8 @@ class HnswIndex:
     def add_pending(self, vector_id, old_vectors, new_vectors):
         """one VectorPendingUpdate of the Hp range, in key order (hnsw/index.rs:424-452).  vector_id: an int (VectorId::
         DocId) or any other hashable (VectorId::RecordKey); new_vectors empty = deletion."""
-        self.pendings.append((vector_id, [np.asarray(v, np.float32) for v in old_vectors],
-                              [np.asarray(v, np.float32) for v in new_vectors]))
+        self.pendings.append((vector_id, [to_vector_type(v, self.vector_type) for v in old_vectors],
+                              [to_vector_type(v, self.vector_type) for v in new_vectors]))
 
     def clear_pendings(self):
         """index_pendings applied the log (hnsw/index.rs:138-211): the caller reloads the graph and drops the log"""
@@ -144,10 +203,10 @@ class HnswIndex:
         return (0, int(vid)) if isinstance(vid, (int, np.integer)) else (1, vid)
 
     def _typed_distances(self, query, vectors):
-        """Distance::calculate(&search.pt, &vector) for F32 vectors with the index's metric and Minkowski order, on the
+        """Distance::calculate(&search.pt, &vector) with the index's metric, vector type and Minkowski order, on the
         GPU (sdb_hnsw_distance)"""
-        q = np.ascontiguousarray(query, np.float32)
-        v = np.ascontiguousarray(vectors, np.float32).reshape(-1, self.dim)
+        q = to_vector_type(query, self.vector_type)
+        v = to_vector_type(vectors, self.vector_type).reshape(-1, self.dim)
         out = np.zeros(v.shape[0], np.float64)
         L.check(L.lib().sdb_hnsw_distance(self.h, C.c_void_p(q.ctypes.data), C.c_void_p(v.ctypes.data), v.shape[0],
                                           C.c_void_p(out.ctypes.data)))
@@ -156,8 +215,9 @@ class HnswIndex:
     def search_graph(self, queries, k, ef, counters=False, truthy=None, all_docs_pending=None):
         """truthy: optional predicate mask, one byte per element (Hnsw::knn_search_with_filter, hnsw/mod.rs:488-515).
         all_docs_pending: optional mask, one byte per element: every document of the element has a pending update
-        (the pending_docs argument of Hnsw::knn_search evaluated per element, hnsw/layer.rs:209,320-339)."""
-        q = np.ascontiguousarray(queries, np.float32)
+        (the pending_docs argument of Hnsw::knn_search evaluated per element, hnsw/layer.rs:209,320-339).
+        queries are converted to the index's vector type (to_vector_type)."""
+        q = to_vector_type(queries, self.vector_type)
         if q.ndim == 1:
             q = q[None, :]
         if q.shape[1] != self.dim:  # Error::InvalidVectorDimension  idx/trees/vector.rs:643-652
@@ -241,7 +301,7 @@ class HnswIndex:
             for e in range(self.n):
                 dl = docs_of(e)
                 all_pending[e] = all(int(d) in pending_docs for d in dl)  # an element without docs counts as pending
-        ids, dist, cnt = self.search_graph(np.asarray(query, np.float32)[None, :], k, ef, truthy=truthy,
+        ids, dist, cnt = self.search_graph(to_vector_type(query, self.vector_type)[None, :], k, ef, truthy=truthy,
                                            all_docs_pending=all_pending)
         for j in range(int(cnt[0])):
             d, e = float(dist[0, j]), int(ids[0, j])
