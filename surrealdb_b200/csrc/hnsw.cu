@@ -25,6 +25,16 @@
 
 namespace sdb {
 
+// Per-vector state of the metrics that carry it (vec_state_make); null where the metric needs none.
+struct VecState {
+  double* norm = nullptr;      // COSINE: the vector's factor of the denominator: sqrt((double)sumsq) (F32, vector.rs:246),
+                               // sqrt of the 8-lane f64 sum of f64(x)^2 (the other types, vector.rs:238,257)
+  double* mean = nullptr;      // PEARSON: mean (in the type's arithmetic, widened) and sum of squared deviations
+  double* sx2 = nullptr;       // (vector.rs:412-451)
+  void* bits = nullptr;        // JACCARD: sorted distinct keys (JKey, dim-strided rows) ...
+  uint32_t* nbits = nullptr;   // ... and how many there are (vector.rs:316-356)
+};
+
 struct Hnsw {
   Ctx* ctx = nullptr;
   uint32_t dim = 0;
@@ -34,14 +44,8 @@ struct Hnsw {
   uint32_t n_layers = 0;
   int64_t entry = -1;
   void* d_vec = nullptr;     // n x dim elements of type vt
-  float* d_sumsq = nullptr;  // F32 only
-  double* d_norm = nullptr;  // the per-element factor of the cosine denominator: sqrt((double)sumsq) (F32, vector.rs:246),
-                             // sqrt of the 8-lane f64 sum of f64(x)^2 (the other types, vector.rs:238,257)
   double minkowski_p = 3.0;  // order of SDB_MINKOWSKI (sdb_hnsw_set_minkowski_order)
-  double* d_mean = nullptr;  // PEARSON: per-element mean (in the type's arithmetic, widened) and sum of squared deviations (vector.rs:412-451)
-  double* d_sx2 = nullptr;
-  void* d_bits = nullptr;       // JACCARD: per-element sorted distinct keys (JKey, dim-strided rows) ...
-  uint32_t* d_nbits = nullptr;  // ... and how many there are (vector.rs:316-356)
+  VecState elems;            // the elements' metric state
   std::vector<uint64_t*> rp;
   std::vector<uint32_t*> ci;
   const uint64_t** d_rp = nullptr;
@@ -54,7 +58,6 @@ struct Hnsw {
 };
 
 constexpr int HN_WARPS = 4;
-constexpr uint64_t KEY_MAX = 0xFFEFFFFFFFFFFFFFull;  // dist_key(f64::MAX)
 
 __device__ __forceinline__ double key_to_double(uint64_t key) {
   const uint64_t b = (key >> 63) ? (key & 0x7fffffffffffffffull) : ~key;
@@ -76,25 +79,58 @@ template <typename T> __device__ __forceinline__ Wide<T> wide(T v) { return (Wid
 template <typename T> __device__ __forceinline__ T wrap(Wide<T> v) { return (T)(typename std::make_unsigned<T>::type)v; }
 template <typename T> __device__ __forceinline__ T wsub(T a, T b) { return wrap<T>(wide(a) - wide(b)); }
 template <typename T> __device__ __forceinline__ T wabs(T a) { return a < 0 ? wrap<T>(Wide<T>(0) - wide(a)) : a; }  // abs(MIN) = MIN
+// The float type the reference's float arithmetic runs in for T: f32 for F32, f64 for every other type
+template <typename T> using Real = typename std::conditional<is_f32_v<T>, float, double>::type;
+// IEEE round-to-nearest + - * in f32 or f64 (never contracted into an FMA, as in the reference)
+__device__ __forceinline__ float rn_add(float a, float b) { return __fadd_rn(a, b); }
+__device__ __forceinline__ double rn_add(double a, double b) { return __dadd_rn(a, b); }
+__device__ __forceinline__ float rn_sub(float a, float b) { return __fsub_rn(a, b); }
+__device__ __forceinline__ double rn_sub(double a, double b) { return __dsub_rn(a, b); }
+__device__ __forceinline__ float rn_mul(float a, float b) { return __fmul_rn(a, b); }
+__device__ __forceinline__ double rn_mul(double a, double b) { return __dmul_rn(a, b); }
 
-// ndarray's 8-lane f64 fold (unrolled_fold, like nd_sum_f32 in f64; tests/hnsw_types_ref.py nd_sum_f64) of f64(x)^2
-// (SQ) or of f64(x): the cosine norms of every type but F32 (vector.rs:238,257) and the F64 mean.  One thread per vector.
-template <bool SQ, typename T>
-__device__ __forceinline__ double nd_sum_f64(const T* a, uint32_t dim) {
-  double p[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+// ndarray's fold of 8 partial sums p_j (p_j = the sequential chain over the columns 8i+j of unrolled_fold / unrolled_dot):
+// ((((0+(p0+p4))+(p1+p5))+(p2+p6))+(p3+p7)).  S = float (F32) or double.
+template <typename S>
+__device__ __forceinline__ S fold8(const S p[8]) {
+  S s = 0;
+#pragma unroll
+  for (int j = 0; j < 4; j++) s = rn_add(s, rn_add(p[j], p[j + 4]));
+  return s;
+}
+// The same fold when the 8 chains of a row live on 8 consecutive lanes (lane 8g+j holds p_j): the result is on lane 8g.
+// All 32 lanes must call; only the lanes with `take` add up (the others return 0).
+__device__ __forceinline__ float quad_fold8(float p, bool take) {
+  const float sj = __fadd_rn(p, __shfl_down_sync(0xffffffffu, p, 4));
+  const float s1 = __shfl_down_sync(0xffffffffu, sj, 1);
+  const float s2 = __shfl_down_sync(0xffffffffu, sj, 2);
+  const float s3 = __shfl_down_sync(0xffffffffu, sj, 3);
+  float s = 0.f;
+  if (take) {
+    s = __fadd_rn(0.f, sj);
+    s = __fadd_rn(s, s1);
+    s = __fadd_rn(s, s2);
+    s = __fadd_rn(s, s3);
+  }
+  return s;
+}
+// ndarray's 8-lane sum of a row in S (unrolled_fold: fold8 of the 8 chains, then the < 8 tail columns in order) of S(x)^2
+// (SQ) or of S(x).  S = float: F32's sums (tests/hnsw_metric_ref.py nd_sum_f32); S = double: the f64 sums of the other
+// types (tests/hnsw_types_ref.py nd_sum_f64), the cosine norms (vector.rs:238,257) and the F64 mean.  One thread per row.
+template <typename S, bool SQ, typename T>
+__device__ __forceinline__ S nd_sum(const T* a, uint32_t dim) {
+  S p[8] = {0, 0, 0, 0, 0, 0, 0, 0};
   uint32_t i = 0;
   for (; i + 8 <= dim; i += 8)
 #pragma unroll
     for (int j = 0; j < 8; j++) {
-      const double v = (double)a[i + j];
-      p[j] = __dadd_rn(p[j], SQ ? __dmul_rn(v, v) : v);
+      const S v = (S)a[i + j];
+      p[j] = rn_add(p[j], SQ ? rn_mul(v, v) : v);
     }
-  double s = 0.0;
-#pragma unroll
-  for (int j = 0; j < 4; j++) s = __dadd_rn(s, __dadd_rn(p[j], p[j + 4]));
+  S s = fold8(p);
   for (; i < dim; i++) {
-    const double v = (double)a[i];
-    s = __dadd_rn(s, SQ ? __dmul_rn(v, v) : v);
+    const S v = (S)a[i];
+    s = rn_add(s, SQ ? rn_mul(v, v) : v);
   }
   return s;
 }
@@ -103,14 +139,13 @@ __device__ __forceinline__ double nd_sum_f64(const T* a, uint32_t dim) {
 template <typename T>
 __global__ void hnsw_norm_kernel(const T* __restrict__ vec, uint32_t dim, uint64_t n, double* __restrict__ norm) {
   const uint64_t r = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (r < n) norm[r] = __dsqrt_rn(nd_sum_f64<true>(vec + r * dim, dim));
+  if (r < n) norm[r] = __dsqrt_rn(nd_sum<double, true>(vec + r * dim, dim));
 }
 
-// ndarray-style 8-lane f32 sum of squares of every row (load time).  8 threads per row, thread j owns the partial sum
-// over the columns 8i+j (a sequential chain, as in ndarray's unrolled fold); the 8 threads of a row read one 32-byte
-// sector per step.  Also writes sqrt((double)sumsq), the element's factor of the cosine denominator.
-__global__ void hnsw_sumsq_kernel(const float* __restrict__ vec, uint32_t dim, uint64_t n, float* __restrict__ out,
-                                  double* __restrict__ norm) {
+// cosine norms of F32 elements (load time): sqrt((double)sumsq), sumsq = ndarray's 8-lane f32 sum of squares
+// (vector.rs:246).  8 threads per row, thread j owns the chain over the columns 8i+j; the 8 threads of a row read one
+// 32-byte sector per step.
+__global__ void hnsw_norm_f32_kernel(const float* __restrict__ vec, uint32_t dim, uint64_t n, double* __restrict__ norm) {
   const uint64_t t = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
   const uint64_t r = t >> 3;
   const uint32_t j = (uint32_t)t & 7u;
@@ -123,28 +158,20 @@ __global__ void hnsw_sumsq_kernel(const float* __restrict__ vec, uint32_t dim, u
       const float v = __ldg(a + 8u * i);
       p = __fadd_rn(p, __fmul_rn(v, v));
     }
-  const float sj = __fadd_rn(p, __shfl_down_sync(0xffffffffu, p, 4));
-  const float s1 = __shfl_down_sync(0xffffffffu, sj, 1);
-  const float s2 = __shfl_down_sync(0xffffffffu, sj, 2);
-  const float s3 = __shfl_down_sync(0xffffffffu, sj, 3);
+  float sum = quad_fold8(p, valid && j == 0);
   if (valid && j == 0) {
-    float sum = __fadd_rn(0.f, sj);
-    sum = __fadd_rn(sum, s1);
-    sum = __fadd_rn(sum, s2);
-    sum = __fadd_rn(sum, s3);
     const float* row = vec + r * dim;
     for (uint32_t c = dim & ~7u; c < dim; c++) sum = __fadd_rn(sum, __fmul_rn(__ldg(row + c), __ldg(row + c)));
-    out[r] = sum;
-    if (norm) norm[r] = __dsqrt_rn((double)sum);
+    norm[r] = __dsqrt_rn((double)sum);
   }
 }
 
 // ---- per-vector state of PEARSON and JACCARD (load time for the elements, per batch for queries and pending vectors)
 
-// PEARSON (vector.rs:412-451): mean = ndarray's mean in T, widened to f64 -- F32: the 8-lane unrolled f32 sum (the fold
-// of hnsw_sumsq_kernel, tests/hnsw_metric_ref.py nd_sum_f32) divided by n as f32; F64: the same in f64; integers: the
-// wrapping sum divided by n in T (truncating toward zero).  sx2 = sequential f64 sum of (f64(x_i) - mean)^2.  Only the
-// cross term is left per pair.  One thread per vector (load time, and once per query batch).
+// PEARSON (vector.rs:412-451): mean = ndarray's mean in T, widened to f64 -- F32: nd_sum in f32 divided by n as f32;
+// F64: the same in f64; integers: the wrapping sum divided by n in T (truncating toward zero).  sx2 = sequential f64
+// sum of (f64(x_i) - mean)^2.  Only the cross term is left per pair.  One thread per vector (load time, and once per
+// query batch).
 template <typename T>
 __global__ void pearson_stats_kernel(const T* __restrict__ vec, uint32_t dim, uint64_t n, double* __restrict__ mean,
                                      double* __restrict__ sx2) {
@@ -153,18 +180,9 @@ __global__ void pearson_stats_kernel(const T* __restrict__ vec, uint32_t dim, ui
   const T* a = vec + r * dim;
   double m;
   if constexpr (is_f32_v<T>) {
-    float p[8] = {0, 0, 0, 0, 0, 0, 0, 0};
-    uint32_t i = 0;
-    for (; i + 8 <= dim; i += 8)
-#pragma unroll
-      for (int j = 0; j < 8; j++) p[j] = __fadd_rn(p[j], a[i + j]);
-    float s = 0.f;
-#pragma unroll
-    for (int j = 0; j < 4; j++) s = __fadd_rn(s, __fadd_rn(p[j], p[j + 4]));
-    for (; i < dim; i++) s = __fadd_rn(s, a[i]);
-    m = (double)__fdiv_rn(s, (float)dim);
+    m = (double)__fdiv_rn(nd_sum<float, false>(a, dim), (float)dim);
   } else if constexpr (is_f64_v<T>) {
-    m = __ddiv_rn(nd_sum_f64<false>(a, dim), (double)dim);
+    m = __ddiv_rn(nd_sum<double, false>(a, dim), (double)dim);
   } else {  // the wrapping sum is the same in any order
     Wide<T> w = 0;
     for (uint32_t c = 0; c < dim; c++) w += wide(a[c]);
@@ -277,109 +295,58 @@ struct MetricQ {
 // loops of vector.rs).  step(x, q): x = the element / pending vector, q = the query.  All of them are symmetric in their
 // two arguments (|x-q| = |q-x| exactly, products commute), so the walk's calculate(element, query) and the pending log's
 // calculate(query, vector) share them.  row_mean / row_sx2: the row's PEARSON state.
-template <int MET, typename T = float>
+// Each metric is in the element type's own arithmetic (vector.rs:206-451).  The integer l1_dist / l2_dist / linf_dist
+// are ndarray-stats' DeviationExt (not vendored): they accumulate in T, with wrapping `+ - * abs`, and cast to f64 at
+// the end.  to_float() is `as f64` (round to nearest for I64).  A sum that is exact (integers below 2^53) or wraps is
+// the same in any order; the others are the reference's sequential folds.
+template <int MET, typename T>
 struct RowAcc;
-template <>
-struct RowAcc<SDB_EUCLIDEAN> {  // l2_dist: f32 sum of squares, f64 sqrt
-  float s = 0.f;
-  __device__ __forceinline__ RowAcc(const MetricQ&, double, double, uint32_t = 0) {}
-  __device__ __forceinline__ void step(float x, float q) {
-    const float d = __fsub_rn(x, q);
-    s = __fadd_rn(s, __fmul_rn(d, d));
-  }
-  __device__ __forceinline__ double finish() const { return __dsqrt_rn((double)s); }
-};
-template <>
-struct RowAcc<SDB_MANHATTAN> {  // l1_dist (vector.rs:377-386): f32 sum of |x-q|, then as f64
-  float s = 0.f;
-  __device__ __forceinline__ RowAcc(const MetricQ&, double, double, uint32_t = 0) {}
-  __device__ __forceinline__ void step(float x, float q) { s = __fadd_rn(s, fabsf(__fsub_rn(x, q))); }
-  __device__ __forceinline__ double finish() const { return (double)s; }
-};
-template <>
-struct RowAcc<SDB_CHEBYSHEV> {  // linf_dist (vector.rs:218-233): max starts at 0, `if d > max` (a NaN never wins)
-  float m = 0.f;
-  __device__ __forceinline__ RowAcc(const MetricQ&, double, double, uint32_t = 0) {}
-  __device__ __forceinline__ void step(float x, float q) {
-    const float d = fabsf(__fsub_rn(x, q));
-    if (d > m) m = d;
-  }
-  __device__ __forceinline__ double finish() const { return (double)m; }
-};
-template <>
-struct RowAcc<SDB_HAMMING> {  // vector.rs:291-314: count of x != q under f32 `!=` (NaN != NaN, 0.0 == -0.0)
-  uint32_t c = 0;
-  __device__ __forceinline__ RowAcc(const MetricQ&, double, double, uint32_t = 0) {}
-  __device__ __forceinline__ void step(float x, float q) { c += x != q; }
-  __device__ __forceinline__ double finish() const { return (double)c; }
-};
-template <>
-struct RowAcc<SDB_MINKOWSKI> {  // vector.rs:388-410: f64 sum of |f64(x) - f64(q)|^p, then ^(1/p)
-  double s = 0.0, p;
-  __device__ __forceinline__ RowAcc(const MetricQ& mq, double, double, uint32_t = 0) : p(mq.p) {}
-  __device__ __forceinline__ void step(float x, float q) { s = __dadd_rn(s, pow(fabs(__dsub_rn((double)x, (double)q)), p)); }
-  __device__ __forceinline__ double finish() const { return pow(s, __ddiv_rn(1.0, p)); }
-};
-template <>
-struct RowAcc<SDB_PEARSON> {  // vector.rs:412-451: sxy / sqrt(sx2 * sy2), 0.0 when that is 0 (a similarity)
-  double sxy = 0.0, mx, sx2, my, sy2;
-  __device__ __forceinline__ RowAcc(const MetricQ& mq, double row_mean, double row_sx2, uint32_t = 0)
-      : mx(row_mean), sx2(row_sx2), my(mq.mean), sy2(mq.sx2) {}
-  __device__ __forceinline__ void step(float x, float q) {
-    sxy = __dadd_rn(sxy, __dmul_rn(__dsub_rn((double)x, mx), __dsub_rn((double)q, my)));
-  }
-  __device__ __forceinline__ double finish() const {
-    const double den = __dsqrt_rn(__dmul_rn(sx2, sy2));
-    return den == 0.0 ? 0.0 : __ddiv_rn(sxy, den);
-  }
-};
-
-// ---- the same accumulators for the other element types T (F64 double, I64 long long, I32 int, I16 short), in each
-// type's own arithmetic (vector.rs:206-451).  The integer l1_dist / l2_dist / linf_dist are ndarray-stats' DeviationExt
-// (not vendored, like the F32 case): they accumulate in T, with wrapping `+ - * abs`, and cast to f64 at the end.
-// to_float() is `as f64` (round to nearest for I64).  A sum that is exact (integers below 2^53) or wraps is the same in
-// any order; the others are the reference's sequential folds.
+// l2_dist: the sum of squares in T (F32: f32, then an f64 sqrt); I16: euclidean(), the f64 sum of exact squares
 template <typename T>
-struct RowAcc<SDB_EUCLIDEAN, T> {  // F64, I64, I32: l2_dist in T; I16: euclidean(), the f64 sum of exact squares
-  typename std::conditional<is_wint_v<T>, Wide<T>, double>::type s = 0;
+struct RowAcc<SDB_EUCLIDEAN, T> {
+  typename std::conditional<is_wint_v<T>, Wide<T>, Real<T>>::type s = 0;
   __device__ __forceinline__ RowAcc(const MetricQ&, double, double, uint32_t) {}
   __device__ __forceinline__ void step(T x, T q) {
     if constexpr (is_wint_v<T>) {
       const Wide<T> d = wide(x) - wide(q);
       s += d * d;
     } else {
-      const double d = __dsub_rn((double)x, (double)q);
-      s = __dadd_rn(s, __dmul_rn(d, d));
+      const Real<T> d = rn_sub((Real<T>)x, (Real<T>)q);
+      s = rn_add(s, rn_mul(d, d));
     }
   }
   __device__ __forceinline__ double finish() const {
     if constexpr (is_wint_v<T>) return __dsqrt_rn((double)wrap<T>(s));
-    else return __dsqrt_rn(s);
+    else return __dsqrt_rn((double)s);
   }
 };
+// l1_dist (vector.rs:377-386): the sum of |x-q| in T, then as f64 (integers: the wrapping abs of a wrapping difference);
+// I16: the f64 sum of |f64(x - q)|, x - q wrapping in i16
 template <typename T>
-struct RowAcc<SDB_MANHATTAN, T> {  // F64, I64, I32: l1_dist in T (wrapping abs of a wrapping difference); I16: the
-  typename std::conditional<is_wint_v<T>, Wide<T>, double>::type s = 0;  // f64 sum of |f64(x - q)|, x - q wrapping in i16
+struct RowAcc<SDB_MANHATTAN, T> {
+  typename std::conditional<is_wint_v<T>, Wide<T>, Real<T>>::type s = 0;
   __device__ __forceinline__ RowAcc(const MetricQ&, double, double, uint32_t) {}
   __device__ __forceinline__ void step(T x, T q) {
     if constexpr (is_wint_v<T>) s += wide(wabs(wsub(x, q)));
     else if constexpr (is_i16_v<T>) s = __dadd_rn(s, fabs((double)wsub(x, q)));
-    else s = __dadd_rn(s, fabs(__dsub_rn(x, q)));
+    else s = rn_add(s, fabs(rn_sub(x, q)));
   }
   __device__ __forceinline__ double finish() const {
     if constexpr (is_wint_v<T>) return (double)wrap<T>(s);
-    else return s;
+    else return (double)s;
   }
 };
+// linf_dist (vector.rs:218-233): in T, max starts at 0, `if d > max` (a NaN never wins; abs(MIN) stays negative and
+// never wins); I16: fold(0.0, f64::max) of |f64(x) - f64(q)|
 template <typename T>
-struct RowAcc<SDB_CHEBYSHEV, T> {  // F64, I64, I32: linf_dist in T (`if d > max` from 0; abs(MIN) stays negative and
-  typename std::conditional<is_i16_v<T>, double, T>::type m = 0;  // never wins); I16: fold(0.0, f64::max) of |f64(x) - f64(q)|
+struct RowAcc<SDB_CHEBYSHEV, T> {
+  typename std::conditional<is_i16_v<T>, double, T>::type m = 0;
   __device__ __forceinline__ RowAcc(const MetricQ&, double, double, uint32_t) {}
   __device__ __forceinline__ void step(T x, T q) {
     if constexpr (is_i16_v<T>) {
       m = fmax(m, fabs(__dsub_rn((double)x, (double)q)));
-    } else if constexpr (is_f64_v<T>) {
-      const double d = fabs(__dsub_rn(x, q));
+    } else if constexpr (std::is_floating_point<T>::value) {
+      const T d = fabs(rn_sub(x, q));
       if (d > m) m = d;
     } else {
       const T d = wabs(wsub(x, q));
@@ -389,21 +356,23 @@ struct RowAcc<SDB_CHEBYSHEV, T> {  // F64, I64, I32: linf_dist in T (`if d > max
   __device__ __forceinline__ double finish() const { return (double)m; }
 };
 template <typename T>
-struct RowAcc<SDB_HAMMING, T> {  // count of x != q (F64: IEEE `!=`)
+struct RowAcc<SDB_HAMMING, T> {  // vector.rs:291-314: count of x != q (F32, F64: IEEE `!=`, NaN != NaN, 0.0 == -0.0)
   uint32_t c = 0;
   __device__ __forceinline__ RowAcc(const MetricQ&, double, double, uint32_t) {}
   __device__ __forceinline__ void step(T x, T q) { c += x != q; }
   __device__ __forceinline__ double finish() const { return (double)c; }
 };
 template <typename T>
-struct RowAcc<SDB_MINKOWSKI, T> {  // the same f64 arithmetic for every type
+struct RowAcc<SDB_MINKOWSKI, T> {  // vector.rs:388-410: f64 sum of |f64(x) - f64(q)|^p, then ^(1/p), for every type
   double s = 0.0, p;
   __device__ __forceinline__ RowAcc(const MetricQ& mq, double, double, uint32_t) : p(mq.p) {}
   __device__ __forceinline__ void step(T x, T q) { s = __dadd_rn(s, pow(fabs(__dsub_rn((double)x, (double)q)), p)); }
   __device__ __forceinline__ double finish() const { return pow(s, __ddiv_rn(1.0, p)); }
 };
+// vector.rs:412-451: sxy / sqrt(sx2 * sy2), 0.0 when that is 0 (a similarity).  The means come from
+// pearson_stats_kernel<T>; the loop is f64 for every type.
 template <typename T>
-struct RowAcc<SDB_PEARSON, T> {  // the means come from pearson_stats_kernel<T>; the loop is f64 for every type
+struct RowAcc<SDB_PEARSON, T> {
   double sxy = 0.0, mx, sx2, my, sy2;
   __device__ __forceinline__ RowAcc(const MetricQ& mq, double row_mean, double row_sx2, uint32_t)
       : mx(row_mean), sx2(row_sx2), my(mq.mean), sy2(mq.sx2) {}
@@ -415,10 +384,11 @@ struct RowAcc<SDB_PEARSON, T> {  // the means come from pearson_stats_kernel<T>;
     return den == 0.0 ? 0.0 : __ddiv_rn(sxy, den);
   }
 };
-// COSINE, 1 - dot / (na * nb) with the norms of hnsw_norm_kernel.  F64: dot is ndarray's 8-lane f64 dot (the chain of
-// column c is c mod 8; the 8 chains rotate through p[] so that every index is static), folded as in nd_sum_f64, then
-// the < 8 tail columns.  Integers: a.dot(b) is a wrapping sum of wrapping products in T -- I16 wraps in i16 -- so any
-// order gives it.  row_norm / q_norm: the two norms (the product commutes, so either argument order).
+// COSINE of the types other than F32 (F32 has its own 8-lane paths), 1 - dot / (na * nb) with the norms of
+// hnsw_norm_kernel.  F64: dot is ndarray's 8-lane f64 dot (the chain of column c is c mod 8; the 8 chains rotate through
+// p[] so that every index is static), folded by fold8, then the < 8 tail columns.  Integers: a.dot(b) is a wrapping sum
+// of wrapping products in T -- I16 wraps in i16 -- so any order gives it.  row_norm / q_norm: the two norms (the product
+// commutes, so either argument order).
 template <typename T>
 struct RowAcc<SDB_COSINE, T> {
   double p[8] = {0, 0, 0, 0, 0, 0, 0, 0};
@@ -427,12 +397,6 @@ struct RowAcc<SDB_COSINE, T> {
   uint32_t i = 0, d8;
   __device__ __forceinline__ RowAcc(const MetricQ&, double row_norm, double q_norm, uint32_t dim)
       : na(row_norm), nb(q_norm), d8(dim & ~7u) {}
-  __device__ __forceinline__ double fold() const {
-    double f = 0.0;
-#pragma unroll
-    for (int j = 0; j < 4; j++) f = __dadd_rn(f, __dadd_rn(p[j], p[j + 4]));
-    return f;
-  }
   __device__ __forceinline__ void step(T x, T q) {
     if constexpr (is_f64_v<T>) {
       const double pr = __dmul_rn(x, q);
@@ -442,7 +406,7 @@ struct RowAcc<SDB_COSINE, T> {
         for (int j = 0; j < 7; j++) p[j] = p[j + 1];
         p[7] = t;
       } else {
-        if (i == d8) s = fold();
+        if (i == d8) s = fold8(p);
         s = __dadd_rn(s, pr);
       }
       i++;
@@ -452,7 +416,7 @@ struct RowAcc<SDB_COSINE, T> {
   }
   __device__ __forceinline__ double finish() const {
     double dot;
-    if constexpr (is_f64_v<T>) dot = i == d8 ? fold() : s;
+    if constexpr (is_f64_v<T>) dot = i == d8 ? fold8(p) : s;
     else dot = (double)wrap<T>(w);
     return __dsub_rn(1.0, __ddiv_rn(dot, __dmul_rn(na, nb)));
   }
@@ -488,7 +452,7 @@ __device__ __forceinline__ bool sorted_contains(const K* s, uint32_t n, K v) {
 // pending log.
 // The other element types use the same kernel with T and their RowAcc / JACCARD keys.
 struct TypedArgs {
-  const float* q;          // dim elements of T (typed as F32's)
+  const float* q;          // dim elements of T (typed as F32's: as const void*, the F32 kernels compile to other loads)
   const float* vecs;       // n x dim elements of T
   uint32_t dim;
   uint64_t n;
@@ -496,8 +460,8 @@ struct TypedArgs {
   MetricQ mq;
   const double* v_mean;    // PEARSON: state of every vector
   const double* v_sx2;
-  const uint32_t* q_bits;  // JACCARD: the query's sorted distinct keys (mq.u of them, JKey<T>) ...
-  const uint32_t* v_bits;  // ... and every vector's
+  const void* q_bits;      // JACCARD: the query's sorted distinct keys (mq.u of them, JKey<T>) ...
+  const void* v_bits;      // ... and every vector's
   const uint32_t* v_nbits;
   const double* v_norm;    // COSINE, types other than F32: the norms of every vector ...
   const double* q_norm;    // ... and of the query
@@ -519,6 +483,7 @@ __global__ void typed_distance_kernel(TypedArgs A) {
         pa[j] = __fadd_rn(pa[j], __fmul_rn(a[i + j], a[i + j]));
         pq[j] = __fadd_rn(pq[j], __fmul_rn(q[i + j], q[i + j]));
       }
+    // fold8 of p, pa and pq, interleaved (three separate fold8 calls schedule differently)
     float dot = 0.f, sa = 0.f, sq = 0.f;
 #pragma unroll
     for (int j = 0; j < 4; j++) {
@@ -538,9 +503,9 @@ __global__ void typed_distance_kernel(TypedArgs A) {
     // calculate(a = query, b = vector)
     using K = JKey<T>;
     const uint32_t ub = A.v_nbits[r];
-    const K* vb = reinterpret_cast<const K*>(A.v_bits) + r * dim;
+    const K* vb = static_cast<const K*>(A.v_bits) + r * dim;
     uint32_t m = 0;
-    for (uint32_t i = 0; i < ub; i++) m += sorted_contains(reinterpret_cast<const K*>(A.q_bits), A.mq.u, vb[i]);
+    for (uint32_t i = 0; i < ub; i++) m += sorted_contains(static_cast<const K*>(A.q_bits), A.mq.u, vb[i]);
     A.out[r] = jaccard_typed<T>(dim, A.mq.u, ub, m);
   } else {
     RowAcc<MET, T> acc(A.mq, MET == SDB_PEARSON ? A.v_mean[r] : MET == SDB_COSINE ? A.v_norm[r] : 0.0,
@@ -550,46 +515,38 @@ __global__ void typed_distance_kernel(TypedArgs A) {
   }
 }
 
-// distance of this lane's row (or NO_ROW) to the query held in shared memory; all 32 lanes must call.
-// Scratch of the distance phase, per warp.  Every metric but cosine: a 32 x 33 float transposing tile (JACCARD uses 32
-// compacted row ids + 32 f64 results of it).  Cosine: 32 compacted row ids + 32 f64 results (the rows are read straight
-// from global memory, see warp_distance<true>).
-__host__ __device__ constexpr size_t hn_tile_bytes(bool cosine) { return cosine ? 32 * 4 + 32 * 8 : sizeof(float) * 32 * 33; }
-
-// COSINE.  ndarray's f32 dot (a6; oracle orc_nd_dot_f32) keeps 8 running sums p_j over the columns 8i+j, each one a
-// strictly sequential chain over i, and folds them as ((((0+(p0+p4))+(p1+p5))+(p2+p6))+(p3+p7)) followed by the <8
-// tail columns.  The 8 chains of a row are independent, so a row is given to 8 LANES (lane j = chain j) and a warp
-// works on 4 rows at a time -- two such quads interleaved when more than 4 rows are new, so every lane carries two
-// independent chains.  Lane (g, j) reads x[row_g][8i+j] directly from global memory: the 8 lanes of a row cover one 32-byte
-// sector and the 4 rows of a quad 4 sectors, i.e. a request moves as many bytes as a fully coalesced one; no shared-memory
-// transposition, 8 x fewer dependent steps per row than one lane per row (the walk was bound by issue latency: ncu r1,
-// 30 % issue-active at 13 cycles per instruction, ~6.7k instructions per expanded node).
-template <bool COSINE>
-__device__ __forceinline__ double warp_distance(const float* __restrict__ vec, const double* __restrict__ norm,
-                                                uint32_t dim, uint32_t my_row, const float* s_q, double q_norm,
-                                                float (*tile)[33]);
-
-// Cosine keeps the query TRANSPOSED in shared memory: qT[j * qs + i] = q[8i + j] (chain j contiguous), qs = hn_q_stride
-// = 4 mod 32 words so the 8 lanes of a row read 8 different bank groups with one LDS.128 per 4 steps; the < 8 tail
-// columns follow at qT[8 * qs ...].
+// ---- the walk's per-warp shared memory: the staged query, the distance scratch, then the 8-byte keys and 4-byte ids of
+// the candidate (ccap entries) and result (wcap entries) queues.  f32_cosine: the index is F32 COSINE (the 8-lane path).
+// F32 cosine keeps the query TRANSPOSED: qT[j * qs + i] = q[8i + j] (chain j contiguous), qs = hn_q_stride = 4 mod 32
+// words so the 8 lanes of a row read 8 different bank groups with one LDS.128 per 4 steps; the < 8 tail columns follow
+// at qT[8 * qs ...].
 __host__ __device__ constexpr uint32_t hn_q_stride(uint32_t dim) { return (((dim >> 3) + 27u) / 32u) * 32u + 4u; }
-// Every other metric keeps the query as dim floats (JACCARD: its <= dim sorted distinct bit patterns).
+// F32's other metrics keep the query as dim floats (JACCARD: its <= dim sorted distinct bit patterns).
 __host__ __device__ constexpr size_t hn_q_floats(uint32_t dim, bool cosine) {
   return cosine ? (size_t)8 * hn_q_stride(dim) + 8 : (size_t)((dim + 3) & ~3u);
 }
-// Bytes of the staged query, a multiple of 16.  The other element types keep dim elements of T (JACCARD: dim keys),
-// cosine included: it walks the one-chain tile path there.
-__host__ __device__ constexpr size_t hn_q_bytes_typed(uint32_t dim, size_t elem) { return ((size_t)dim * elem + 15) & ~size_t(15); }
-template <int MET, typename T>
-__host__ __device__ constexpr size_t hn_q_bytes(uint32_t dim) {
-  return is_f32_v<T> ? sizeof(float) * hn_q_floats(dim, MET == SDB_COSINE)
-                     : hn_q_bytes_typed(dim, MET == SDB_JACCARD ? sizeof(JKey<T>) : sizeof(T));
+// Bytes of the staged query, a multiple of 16.  f32: the index is F32, counted in floats; every other type keeps dim
+// elements of elem bytes (its own type, or its JACCARD keys), cosine included: it walks the one-chain tile path there.
+__host__ __device__ constexpr size_t hn_q_bytes(uint32_t dim, bool f32, bool cosine, size_t elem) {
+  return f32 ? sizeof(float) * hn_q_floats(dim, cosine) : ((size_t)dim * elem + 15) & ~size_t(15);
 }
+// Scratch of the distance phase.  F32 cosine: 32 compacted row ids + 32 f64 results (the rows are read straight from
+// global memory, see warp_distance_cosine_f32).  Every other cell: a 32 x 33 float transposing tile (JACCARD uses 32
+// compacted row ids + 32 f64 results of it).
+__host__ __device__ constexpr size_t hn_tile_bytes(bool f32_cosine) { return f32_cosine ? 32 * 4 + 32 * 8 : sizeof(float) * 32 * 33; }
 
-template <>
-__device__ __forceinline__ double warp_distance<true>(const float* __restrict__ vec, const double* __restrict__ norm,
-                                                      uint32_t dim, uint32_t my_row, const float* s_q, double q_norm,
-                                                      float (*tile)[33]) {
+// distance of this lane's row (or NO_ROW) to the query held in shared memory; all 32 lanes must call.
+// F32 COSINE.  ndarray's f32 dot (a6; oracle orc_nd_dot_f32) keeps 8 running sums p_j over the columns 8i+j, each one a
+// strictly sequential chain over i, and folds them with fold8 followed by the <8 tail columns.  The 8 chains of a row
+// are independent, so a row is given to 8 LANES (lane j = chain j) and a warp works on 4 rows at a time -- two such
+// quads interleaved when more than 4 rows are new, so every lane carries two independent chains.  Lane (g, j) reads
+// x[row_g][8i+j] directly from global memory: the 8 lanes of a row cover one 32-byte sector and the 4 rows of a quad 4
+// sectors, i.e. a request moves as many bytes as a fully coalesced one; no shared-memory transposition, 8 x fewer
+// dependent steps per row than one lane per row (the walk was bound by issue latency: ncu r1, 30 % issue-active at 13
+// cycles per instruction, ~6.7k instructions per expanded node).
+__device__ __forceinline__ double warp_distance_cosine_f32(const float* __restrict__ vec, const double* __restrict__ norm,
+                                                           uint32_t dim, uint32_t my_row, const float* s_q, double q_norm,
+                                                           float (*tile)[33]) {
   const uint32_t lane = threadIdx.x & 31u;
   const uint32_t d8 = dim & ~7u, steps = dim >> 3, qs = hn_q_stride(dim);
   uint32_t* ids = reinterpret_cast<uint32_t*>(tile);
@@ -658,21 +615,12 @@ __device__ __forceinline__ double warp_distance<true>(const float* __restrict__ 
       }
       for (; i < steps; i++) pa = __fadd_rn(pa, __fmul_rn(va ? __ldg(xa + 8u * i) : 0.f, qj[i]));
     }
-    // fold: s_j = p_j + p_(j+4) on lanes j < 4, then the sequential sum on the quad's lane 0
 #pragma unroll
     for (int h = 0; h < 2; h++) {
-      const float p = h ? pb : pa;
-      const float sj = __fadd_rn(p, __shfl_down_sync(0xffffffffu, p, 4));
-      const float s1 = __shfl_down_sync(0xffffffffu, sj, 1);
-      const float s2 = __shfl_down_sync(0xffffffffu, sj, 2);
-      const float s3 = __shfl_down_sync(0xffffffffu, sj, 3);
       const bool v = h ? vb : va;
+      float dot = quad_fold8(h ? pb : pa, v && j == 0);
       if (v && j == 0) {
         const uint32_t row = h ? rb : ra;
-        float dot = __fadd_rn(0.f, sj);
-        dot = __fadd_rn(dot, s1);
-        dot = __fadd_rn(dot, s2);
-        dot = __fadd_rn(dot, s3);
         for (uint32_t c = d8; c < dim; c++)
           dot = __fadd_rn(dot, __fmul_rn(__ldg(vec + (size_t)row * dim + c), s_q[8u * qs + (c - d8)]));
         res[h ? ib : ia] = __dsub_rn(1.0, __ddiv_rn((double)dot, __dmul_rn(h ? nb : na, q_norm)));
@@ -689,7 +637,7 @@ __device__ __forceinline__ double warp_distance<true>(const float* __restrict__ 
 // lane and the rows of a round are transposed through shared memory (coalesced fetches, 256 bytes of a row a step).
 // row_mean / row_sx2: the PEARSON state of the elements (null for the other metrics); COSINE: row_mean = the element
 // norms, q_norm the query's.
-template <int MET, typename T = float>
+template <int MET, typename T>
 __device__ __forceinline__ double warp_distance_rows(const T* __restrict__ vec, uint32_t dim, uint32_t my_row,
                                                      const T* s_q, float (*tile)[33], const MetricQ& mq,
                                                      const double* __restrict__ row_mean, const double* __restrict__ row_sx2,
@@ -757,7 +705,7 @@ __device__ __forceinline__ double warp_distance_rows(const T* __restrict__ vec, 
 // JACCARD, calculate(a = element, b = query): only m = |distinct(element) & distinct(query)| is per pair.  The query's
 // sorted distinct keys (q_u of them) are in shared memory; the warp takes one new row at a time, every lane binary-
 // searching a 32-key slice of the row's distinct list.
-template <typename T = float>
+template <typename T>
 __device__ __forceinline__ double warp_distance_jaccard(const JKey<T>* __restrict__ bits, const uint32_t* __restrict__ nbits,
                                                         uint32_t dim, uint32_t my_row, const JKey<T>* s_qb, uint32_t q_u,
                                                         float (*tile)[33]) {
@@ -859,7 +807,7 @@ template <int MET, typename T>
 __device__ __forceinline__ double walk_distance(const HnswParams& P, uint32_t my_row, const float* s_q, double q_norm,
                                                 const MetricQ& mq, float (*tile)[33]) {
   if constexpr (MET == SDB_COSINE && is_f32_v<T>)
-    return warp_distance<true>(static_cast<const float*>(P.vec), P.norm, P.dim, my_row, s_q, q_norm, tile);
+    return warp_distance_cosine_f32(static_cast<const float*>(P.vec), P.norm, P.dim, my_row, s_q, q_norm, tile);
   else if constexpr (MET == SDB_JACCARD)
     return warp_distance_jaccard<T>(static_cast<const JKey<T>*>(P.e_bits), P.e_nbits, P.dim, my_row,
                                     reinterpret_cast<const JKey<T>*>(s_q), mq.u, tile);
@@ -872,16 +820,17 @@ __device__ __forceinline__ double walk_distance(const HnswParams& P, uint32_t my
 template <int MET, int MINB, typename T>
 __global__ void __launch_bounds__(HN_WARPS * 32, MINB) hnsw_search_kernel(HnswParams P) {
   constexpr bool COSINE = MET == SDB_COSINE && is_f32_v<T>;  // the 8-lane transposed path of F32 cosine
+  constexpr size_t ELEM = MET == SDB_JACCARD ? sizeof(JKey<T>) : sizeof(T);  // bytes of a staged query element
   extern __shared__ uint8_t smem_raw[];
   const uint32_t warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const uint32_t ccap = P.ccap, wcap = P.ef + 2;
   // per-warp shared layout
-  const size_t per_warp = hn_q_bytes<MET, T>(P.dim) + hn_tile_bytes(COSINE) + (sizeof(uint64_t) + sizeof(uint32_t)) * (ccap + wcap) + 64;
+  const size_t per_warp = hn_q_bytes(P.dim, is_f32_v<T>, MET == SDB_COSINE, ELEM) + hn_tile_bytes(COSINE) + (sizeof(uint64_t) + sizeof(uint32_t)) * (ccap + wcap) + 64;
   uint8_t* base = smem_raw + (size_t)warp * ((per_warp + 15) & ~size_t(15));
   // query first (16-byte aligned: LDS.128), then the distance scratch, the 8-byte keys, the 4-byte ids
   float* s_q = reinterpret_cast<float*>(base);
   float(*tile)[33] = reinterpret_cast<float(*)[33]>(is_f32_v<T> ? s_q + ((hn_q_floats(P.dim, COSINE) + 3) & ~size_t(3))
-                                                                : reinterpret_cast<float*>(base + hn_q_bytes<MET, T>(P.dim)));
+                                                                : reinterpret_cast<float*>(base + hn_q_bytes(P.dim, false, false, ELEM)));
   uint64_t* c_key = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(tile) + hn_tile_bytes(COSINE));
   uint64_t* w_key = c_key + ccap;
   uint32_t* c_id = reinterpret_cast<uint32_t*>(w_key + wcap);
@@ -913,14 +862,7 @@ __global__ void __launch_bounds__(HN_WARPS * 32, MINB) hnsw_search_kernel(HnswPa
           const float v = s_q[lane * qs + i];
           p = __fadd_rn(p, __fmul_rn(v, v));
         }
-      const float sj = __fadd_rn(p, __shfl_down_sync(0xffffffffu, p, 4));
-      const float s1 = __shfl_down_sync(0xffffffffu, sj, 1);
-      const float s2 = __shfl_down_sync(0xffffffffu, sj, 2);
-      const float s3 = __shfl_down_sync(0xffffffffu, sj, 3);
-      float q_sumsq = __fadd_rn(0.f, sj);
-      q_sumsq = __fadd_rn(q_sumsq, s1);
-      q_sumsq = __fadd_rn(q_sumsq, s2);
-      q_sumsq = __fadd_rn(q_sumsq, s3);
+      float q_sumsq = quad_fold8(p, true);
       for (uint32_t c = d8; c < P.dim; c++) {
         const float v = s_q[8u * qs + (c - d8)];
         q_sumsq = __fadd_rn(q_sumsq, __fmul_rn(v, v));
@@ -1272,8 +1214,26 @@ static auto with_vt(sdb_vector_type vt, F&& f) {
     default: return f(float());
   }
 }
-// the refusals every loader shares: unknown metric or type, and I16 PEARSON beyond the reference's i16 divisor
-static sdb_status check_index_kind(const char* what, uint32_t dim, sdb_metric metric, int vt) {
+// calls f(std::integral_constant<int, MET>()) with the metric as a compile-time constant
+template <typename F>
+static auto with_metric(sdb_metric metric, F&& f) {
+  switch (metric) {
+    case SDB_CHEBYSHEV: return f(std::integral_constant<int, SDB_CHEBYSHEV>());
+    case SDB_COSINE: return f(std::integral_constant<int, SDB_COSINE>());
+    case SDB_HAMMING: return f(std::integral_constant<int, SDB_HAMMING>());
+    case SDB_JACCARD: return f(std::integral_constant<int, SDB_JACCARD>());
+    case SDB_MANHATTAN: return f(std::integral_constant<int, SDB_MANHATTAN>());
+    case SDB_MINKOWSKI: return f(std::integral_constant<int, SDB_MINKOWSKI>());
+    case SDB_PEARSON: return f(std::integral_constant<int, SDB_PEARSON>());
+    default: return f(std::integral_constant<int, SDB_EUCLIDEAN>());
+  }
+}
+// The checks every loader shares, after its own pointer checks: the shape of the index, then the refusals of an
+// unknown metric or type and of I16 PEARSON beyond the reference's i16 divisor.
+static sdb_status check_load(const char* what, sdb_ctx* ctx, sdb_hnsw** out, uint32_t dim, sdb_metric metric, int vt,
+                             uint64_t n_elems, uint32_t n_layers, int64_t entry_point) {
+  if (!ctx || !out || dim == 0 || dim > 65535 || n_elems >= 0xFFFFFFF0ull || !n_layers || entry_point >= (int64_t)n_elems)
+    return SDB_EINVAL;
   if ((unsigned)metric > SDB_PEARSON) {
     set_error("hnsw: unknown metric %d", (int)metric);
     return SDB_EUNSUPPORTED;
@@ -1286,10 +1246,82 @@ static sdb_status check_index_kind(const char* what, uint32_t dim, sdb_metric me
     set_error("%s: an I16 PEARSON index of dimension %u cannot be searched (the mean's divisor does not fit i16)", what, dim);
     return SDB_EUNSUPPORTED;
   }
+  *out = nullptr;
   return SDB_OK;
 }
 
-// common tail of the loaders: per-layer pointer tables + cached |x|^2 + the per-element state of PEARSON / JACCARD
+// a handle with the index's shape; the loader adds the vectors and the adjacency, hnsw_finish the rest
+static sdb_hnsw* new_hnsw(Ctx* ctx, uint32_t dim, sdb_metric metric, sdb_vector_type vt, uint64_t n, uint32_t n_layers,
+                          int64_t entry) {
+  sdb_hnsw* h = new sdb_hnsw();
+  h->ctx = ctx;
+  h->dim = dim;
+  h->metric = metric;
+  h->vt = vt;
+  h->n = n;
+  h->n_layers = n_layers;
+  h->entry = entry;
+  return h;
+}
+
+// Whose per-vector state it is, which fixes how it is allocated.  ELEMENTS: an index's elements, cudaMalloc'd and freed
+// with the index.  BATCH: the queries or pending vectors of one call, from the stream's pool and freed on the stream
+// once the call's kernels are queued.
+enum class VecSet { ELEMENTS, BATCH };
+
+// The state `metric` needs for rows x dim vectors d_v of type vt, allocated into s and computed on st: COSINE the norms
+// (none for an F32 BATCH: the walk computes the query's own, typed_distance_kernel both), PEARSON the mean and sx2,
+// JACCARD the sorted distinct keys.  What was allocated stays in s for vec_state_free, also on failure.
+static sdb_status vec_state_make(Ctx* ctx, VecSet set, sdb_metric metric, sdb_vector_type vt, const void* d_v,
+                                 uint64_t rows, uint32_t dim, VecState& s, cudaStream_t st) {
+  if (!rows) return SDB_OK;
+  auto alloc = [&](auto** p, size_t bytes) {
+    if ((set == VecSet::BATCH ? cudaMallocAsync(p, bytes, st) : cudaMalloc(p, bytes)) == cudaSuccess) return true;
+    *p = nullptr;
+    return false;
+  };
+  auto oom = [&](const char* what, size_t bytes) {
+    set_error("hnsw: %s (%zu bytes) could not be allocated: %s", what, bytes, cudaGetErrorString(cudaGetLastError()));
+    return set == VecSet::BATCH ? SDB_ECUDA : SDB_ENOMEM;
+  };
+  const unsigned grid = (unsigned)((rows + 127) / 128);
+  if (metric == SDB_COSINE && !(vt == SDB_VT_F32 && set == VecSet::BATCH)) {
+    if (!alloc(&s.norm, sizeof(double) * rows)) return oom("cosine norms", sizeof(double) * rows);
+    with_vt(vt, [&](auto tag) {
+      using T = decltype(tag);
+      if constexpr (is_f32_v<T>)
+        hnsw_norm_f32_kernel<<<(unsigned)((rows * 8 + 127) / 128), 128, 0, st>>>(static_cast<const float*>(d_v), dim,
+                                                                                  rows, s.norm);
+      else
+        hnsw_norm_kernel<T><<<grid, 128, 0, st>>>(static_cast<const T*>(d_v), dim, rows, s.norm);
+    });
+    count_launch(ctx);
+  } else if (metric == SDB_PEARSON) {
+    if (!alloc(&s.mean, sizeof(double) * rows) || !alloc(&s.sx2, sizeof(double) * rows))
+      return oom("pearson state", 2 * sizeof(double) * rows);
+    with_vt(vt, [&](auto tag) {
+      using T = decltype(tag);
+      pearson_stats_kernel<T><<<grid, 128, 0, st>>>(static_cast<const T*>(d_v), dim, rows, s.mean, s.sx2);
+    });
+    count_launch(ctx);
+  } else if (metric == SDB_JACCARD) {  // key bytes * rows * dim: the sorted distinct keys of every vector
+    const size_t kb = jkey_size(vt) * rows * dim;
+    if (!alloc(&s.bits, kb) || !alloc(&s.nbits, sizeof(uint32_t) * rows))
+      return oom("jaccard state", kb + sizeof(uint32_t) * rows);
+    return jaccard_prepare_typed(ctx, vt, d_v, rows, dim, s.bits, s.nbits, st);
+  }
+  return SDB_OK;
+}
+static void vec_state_free(VecState& s, VecSet set, cudaStream_t st) {
+  for (void* p : {(void*)s.norm, (void*)s.mean, (void*)s.sx2, s.bits, (void*)s.nbits}) {
+    if (!p) continue;
+    if (set == VecSet::BATCH) cudaFreeAsync(p, st);
+    else cudaFree(p);
+  }
+  s = VecState();
+}
+
+// common tail of the loaders: per-layer pointer tables + the elements' metric state
 static sdb_status hnsw_finish(sdb_hnsw* h, sdb_hnsw** out) {
   Ctx* ctx = h->ctx;
   cudaStream_t st = ctx->stream;
@@ -1304,43 +1336,10 @@ static sdb_status hnsw_finish(sdb_hnsw* h, sdb_hnsw** out) {
   if (cudaMemcpyAsync(h->d_rp, h->rp.data(), sizeof(void*) * n_layers, cudaMemcpyHostToDevice, st) != cudaSuccess ||
       cudaMemcpyAsync(h->d_ci, h->ci.data(), sizeof(void*) * n_layers, cudaMemcpyHostToDevice, st) != cudaSuccess)
     return fail("layer table copy", SDB_ECUDA);
-  const unsigned grid = (unsigned)((h->n + 127) / 128);
-  if (h->n && h->vt == SDB_VT_F32) {
-    if (cudaMalloc(&h->d_norm, sizeof(double) * h->n) != cudaSuccess) return fail("norms", SDB_ENOMEM);
-    hnsw_sumsq_kernel<<<(unsigned)((h->n * 8 + 127) / 128), 128, 0, st>>>(static_cast<const float*>(h->d_vec), h->dim,
-                                                                           h->n, h->d_sumsq, h->d_norm);
-    count_launch(ctx);
-  } else if (h->n && h->metric == SDB_COSINE) {
-    if (cudaMalloc(&h->d_norm, sizeof(double) * h->n) != cudaSuccess) return fail("norms", SDB_ENOMEM);
-    with_vt(h->vt, [&](auto tag) {
-      using T = decltype(tag);
-      hnsw_norm_kernel<T><<<grid, 128, 0, st>>>(static_cast<const T*>(h->d_vec), h->dim, h->n, h->d_norm);
-    });
-    count_launch(ctx);
-  }
-  if (h->n && h->metric == SDB_PEARSON) {
-    if (cudaMalloc(&h->d_mean, sizeof(double) * h->n) != cudaSuccess || cudaMalloc(&h->d_sx2, sizeof(double) * h->n) != cudaSuccess)
-      return fail("pearson state", SDB_ENOMEM);
-    with_vt(h->vt, [&](auto tag) {
-      using T = decltype(tag);
-      pearson_stats_kernel<T><<<grid, 128, 0, st>>>(static_cast<const T*>(h->d_vec), h->dim, h->n, h->d_mean, h->d_sx2);
-    });
-    count_launch(ctx);
-  }
-  if (h->n && h->metric == SDB_JACCARD) {  // key bytes * n * dim: the sorted distinct keys of every element
-    const size_t kb = jkey_size(h->vt);
-    if (cudaMalloc(&h->d_bits, kb * h->n * h->dim) != cudaSuccess ||
-        cudaMalloc(&h->d_nbits, sizeof(uint32_t) * h->n) != cudaSuccess) {
-      set_error("hnsw load: jaccard state (%llu bytes) could not be allocated",
-                (unsigned long long)(kb * h->n * h->dim + sizeof(uint32_t) * h->n));
-      sdb_hnsw_destroy(h);
-      return SDB_ENOMEM;
-    }
-    const sdb_status rc = jaccard_prepare_typed(ctx, h->vt, h->d_vec, h->n, h->dim, h->d_bits, h->d_nbits, st);
-    if (rc != SDB_OK) {
-      sdb_hnsw_destroy(h);
-      return rc;
-    }
+  const sdb_status rc = vec_state_make(ctx, VecSet::ELEMENTS, h->metric, h->vt, h->d_vec, h->n, h->dim, h->elems, st);
+  if (rc != SDB_OK) {
+    sdb_hnsw_destroy(h);
+    return rc;
   }
   if (cudaStreamSynchronize(st) != cudaSuccess || cudaGetLastError() != cudaSuccess) return fail("finish", SDB_ECUDA);
   *out = h;
@@ -1357,12 +1356,7 @@ void sdb_hnsw_destroy(sdb_hnsw* h) {
     for (auto p : h->rp) cudaFree(p);
     for (auto p : h->ci) cudaFree(p);
   }
-  cudaFree(h->d_sumsq);
-  cudaFree(h->d_norm);
-  cudaFree(h->d_mean);
-  cudaFree(h->d_sx2);
-  cudaFree(h->d_bits);
-  cudaFree(h->d_nbits);
+  vec_state_free(h->elems, VecSet::ELEMENTS, nullptr);
   cudaFree(h->d_rp);
   cudaFree(h->d_ci);
   cudaFree(h->d_visited);
@@ -1378,21 +1372,11 @@ sdb_status sdb_hnsw_load(sdb_ctx* ctx, uint32_t dim, sdb_metric metric, uint64_t
 sdb_status sdb_hnsw_load_typed(sdb_ctx* ctx, uint32_t dim, sdb_metric metric, sdb_vector_type vt, uint64_t n_elems,
                                const void* vectors, uint32_t n_layers, const uint64_t* const* row_ptr,
                                const uint32_t* const* col_idx, int64_t entry_point, sdb_hnsw** out) {
-  if (!ctx || !out || dim == 0 || dim > 65535 || n_elems >= 0xFFFFFFF0ull || (n_elems && !vectors) || !n_layers ||
-      !row_ptr || !col_idx || entry_point >= (int64_t)n_elems)
-    return SDB_EINVAL;
-  SDB_TRY(check_index_kind("sdb_hnsw_load_typed", dim, metric, (int)vt));
-  *out = nullptr;
+  if ((n_elems && !vectors) || !row_ptr || !col_idx) return SDB_EINVAL;
+  SDB_TRY(check_load("sdb_hnsw_load_typed", ctx, out, dim, metric, (int)vt, n_elems, n_layers, entry_point));
   std::lock_guard<std::mutex> guard(ctx->mu);
   SDB_CUDA(cudaSetDevice(ctx->device));
-  sdb_hnsw* h = new sdb_hnsw();
-  h->ctx = ctx;
-  h->dim = dim;
-  h->metric = metric;
-  h->vt = vt;
-  h->n = n_elems;
-  h->n_layers = n_layers;
-  h->entry = entry_point;
+  sdb_hnsw* h = new_hnsw(ctx, dim, metric, vt, n_elems, n_layers, entry_point);
   cudaStream_t st = ctx->stream;
   auto fail = [&](const char* what) {
     set_error("hnsw load: %s failed: %s", what, cudaGetErrorString(cudaGetLastError()));
@@ -1402,7 +1386,6 @@ sdb_status sdb_hnsw_load_typed(sdb_ctx* ctx, uint32_t dim, sdb_metric metric, sd
   const uint64_t nn = n_elems ? n_elems : 1;
   const size_t esz = vt_size(vt);
   if (cudaMalloc(&h->d_vec, esz * nn * dim) != cudaSuccess) return fail("vectors");
-  if (vt == SDB_VT_F32 && cudaMalloc(&h->d_sumsq, sizeof(float) * nn) != cudaSuccess) return fail("sumsq");
   if (n_elems) SDB_CUDA(cudaMemcpyAsync(h->d_vec, vectors, esz * n_elems * dim, cudaMemcpyHostToDevice, st));
   for (uint32_t l = 0; l < n_layers; l++) {
     const uint64_t e = n_elems ? row_ptr[l][n_elems] : 0;
@@ -1426,55 +1409,48 @@ sdb_status sdb_hnsw_load_typed(sdb_ctx* ctx, uint32_t dim, sdb_metric metric, sd
 sdb_status sdb_hnsw_load_device(sdb_ctx* ctx, uint32_t dim, sdb_metric metric, uint64_t n_elems, const float* d_vectors,
                                 uint32_t n_layers, const uint64_t* const* d_row_ptr, const uint32_t* const* d_col_idx,
                                 int64_t entry_point, sdb_hnsw** out) {
-  if (!ctx || !out || dim == 0 || dim > 65535 || n_elems >= 0xFFFFFFF0ull || (n_elems && !d_vectors) || !n_layers ||
-      !d_row_ptr || !d_col_idx || entry_point >= (int64_t)n_elems)
-    return SDB_EINVAL;
-  if ((unsigned)metric > SDB_PEARSON) {
-    set_error("hnsw: unknown metric %d", (int)metric);
-    return SDB_EUNSUPPORTED;
-  }
-  *out = nullptr;
+  if ((n_elems && !d_vectors) || !d_row_ptr || !d_col_idx) return SDB_EINVAL;
+  // F32 only: its one caller is the F32 GPU builder
+  SDB_TRY(check_load("sdb_hnsw_load_device", ctx, out, dim, metric, SDB_VT_F32, n_elems, n_layers, entry_point));
   std::lock_guard<std::mutex> guard(ctx->mu);
   SDB_CUDA(cudaSetDevice(ctx->device));
-  sdb_hnsw* h = new sdb_hnsw();
-  h->ctx = ctx;
-  h->dim = dim;
-  h->metric = metric;
-  h->n = n_elems;
-  h->n_layers = n_layers;
-  h->entry = entry_point;
+  sdb_hnsw* h = new_hnsw(ctx, dim, metric, SDB_VT_F32, n_elems, n_layers, entry_point);
   h->borrowed = true;  // nothing is copied: the caller keeps vectors and adjacency alive while the handle exists
-  h->d_vec = const_cast<float*>(d_vectors);  // F32 only: its one caller is the F32 GPU builder
+  h->d_vec = const_cast<float*>(d_vectors);
   for (uint32_t l = 0; l < n_layers; l++) {
     h->rp.push_back(const_cast<uint64_t*>(d_row_ptr[l]));
     h->ci.push_back(const_cast<uint32_t*>(d_col_idx[l]));
   }
-  if (cudaMalloc(&h->d_sumsq, sizeof(float) * (n_elems ? n_elems : 1)) != cudaSuccess) {
-    set_error("hnsw load: sumsq allocation failed: %s", cudaGetErrorString(cudaGetLastError()));
-    sdb_hnsw_destroy(h);
-    return SDB_ENOMEM;
-  }
   return hnsw_finish(h, out);
 }
 
-// native < 0: He values converted to f32 (sdb_hnsw_load_staged, which has refused the other variants); otherwise the
-// variant number of the index's type: values are decoded as they are stored and any other variant counts as bad.
+// native < 0: sdb_hnsw_load_staged, an F32 index: He values of another variant are refused, F32 ones converted; otherwise
+// sdb_hnsw_load_staged_typed, native = the variant number of the index's type: values are decoded as they are stored and
+// any other variant counts as bad.
 static sdb_status hnsw_load_staged_impl(sdb_ctx* ctx, uint32_t dim, sdb_metric metric, sdb_vector_type vt, int native,
                                         uint64_t n_elems, const uint8_t* vec_blob, const uint64_t* vec_off,
                                         const uint64_t* vec_ids, uint64_t n_vec, uint32_t n_layers,
                                         const uint8_t* const* node_blob, const uint64_t* const* node_off,
                                         const uint64_t* const* node_ids, const uint64_t* n_nodes, int64_t entry_point,
                                         sdb_hnsw** out, uint64_t* n_bad) {
+  if (!node_blob || !node_off || !node_ids || !n_nodes || (n_vec && (!vec_blob || !vec_off))) return SDB_EINVAL;
+  SDB_TRY(check_load(native < 0 ? "sdb_hnsw_load_staged" : "sdb_hnsw_load_staged_typed", ctx, out, dim, metric, (int)vt,
+                     n_elems, n_layers, entry_point));
+  // An F32 index refuses a value of another SerializedVector variant.  It would load -- the decoder converts it -- but
+  // be searched in F32 arithmetic where the reference computes in the value's own type (idx/trees/vector.rs:206-451).
+  // Header = revision varint (1) + variant varint: one byte each.
+  for (uint64_t v = 0; native < 0 && v < n_vec; v++) {
+    const uint64_t a = vec_off[v], b = vec_off[v + 1];
+    if (b >= a + 2 && vec_blob[a] == 1 && vec_blob[a + 1] != 1 && vec_blob[a + 1] <= 4) {
+      static const char* names[] = {"F64", "F32", "I64", "I32", "I16"};
+      set_error("sdb_hnsw_load_staged: He value %llu holds a %s vector; this loader builds F32 indexes "
+                "(sdb_hnsw_load_staged_typed loads an index of that type)", (unsigned long long)v, names[vec_blob[a + 1]]);
+      return SDB_EUNSUPPORTED;
+    }
+  }
   std::lock_guard<std::mutex> guard(ctx->mu);
   SDB_CUDA(cudaSetDevice(ctx->device));
-  sdb_hnsw* h = new sdb_hnsw();
-  h->ctx = ctx;
-  h->dim = dim;
-  h->metric = metric;
-  h->vt = vt;
-  h->n = n_elems;
-  h->n_layers = n_layers;
-  h->entry = entry_point;
+  sdb_hnsw* h = new_hnsw(ctx, dim, metric, vt, n_elems, n_layers, entry_point);
   cudaStream_t st = ctx->stream;
   const uint64_t nn = n_elems ? n_elems : 1;
   uint64_t bad_total = 0, bad = 0;
@@ -1485,8 +1461,7 @@ static sdb_status hnsw_load_staged_impl(sdb_ctx* ctx, uint32_t dim, sdb_metric m
     rc = SDB_ENOMEM;
   }
   const size_t esz = vt_size(vt);
-  if (cudaMalloc(&h->d_vec, esz * nn * dim) != cudaSuccess ||
-      (vt == SDB_VT_F32 && cudaMalloc(&h->d_sumsq, sizeof(float) * nn) != cudaSuccess)) {
+  if (cudaMalloc(&h->d_vec, esz * nn * dim) != cudaSuccess) {
     set_error("hnsw load: vector allocation failed: %s", cudaGetErrorString(cudaGetLastError()));
     rc = SDB_ENOMEM;
   }
@@ -1564,27 +1539,6 @@ sdb_status sdb_hnsw_load_staged(sdb_ctx* ctx, uint32_t dim, sdb_metric metric, u
                                 uint32_t n_layers, const uint8_t* const* node_blob, const uint64_t* const* node_off,
                                 const uint64_t* const* node_ids, const uint64_t* n_nodes, int64_t entry_point,
                                 sdb_hnsw** out, uint64_t* n_bad) {
-  if (!ctx || !out || dim == 0 || dim > 65535 || n_elems >= 0xFFFFFFF0ull || !n_layers || !node_blob || !node_off ||
-      !node_ids || !n_nodes || entry_point >= (int64_t)n_elems || (n_vec && (!vec_blob || !vec_off)))
-    return SDB_EINVAL;
-  if ((unsigned)metric > SDB_PEARSON) {
-    set_error("hnsw: unknown metric %d", (int)metric);
-    return SDB_EUNSUPPORTED;
-  }
-  *out = nullptr;
-  // This loader builds an F32 index.  A value of another SerializedVector variant would load -- the decoder converts
-  // it -- but be searched in F32 arithmetic where the reference computes in the value's own type
-  // (idx/trees/vector.rs:206-451), so the load refuses it instead of reporting success.  Header = revision varint (1) +
-  // variant varint: one byte each.
-  for (uint64_t v = 0; v < n_vec; v++) {
-    const uint64_t a = vec_off[v], b = vec_off[v + 1];
-    if (b >= a + 2 && vec_blob[a] == 1 && vec_blob[a + 1] != 1 && vec_blob[a + 1] <= 4) {
-      static const char* names[] = {"F64", "F32", "I64", "I32", "I16"};
-      set_error("sdb_hnsw_load_staged: He value %llu holds a %s vector; this loader builds F32 indexes "
-                "(sdb_hnsw_load_staged_typed loads an index of that type)", (unsigned long long)v, names[vec_blob[a + 1]]);
-      return SDB_EUNSUPPORTED;
-    }
-  }
   return hnsw_load_staged_impl(ctx, dim, metric, SDB_VT_F32, -1, n_elems, vec_blob, vec_off, vec_ids, n_vec, n_layers,
                                node_blob, node_off, node_ids, n_nodes, entry_point, out, n_bad);
 }
@@ -1594,18 +1548,15 @@ sdb_status sdb_hnsw_load_staged_typed(sdb_ctx* ctx, uint32_t dim, sdb_metric met
                                       uint64_t n_vec, uint32_t n_layers, const uint8_t* const* node_blob,
                                       const uint64_t* const* node_off, const uint64_t* const* node_ids,
                                       const uint64_t* n_nodes, int64_t entry_point, sdb_hnsw** out, uint64_t* n_bad) {
-  if (!ctx || !out || dim == 0 || dim > 65535 || n_elems >= 0xFFFFFFF0ull || !n_layers || !node_blob || !node_off ||
-      !node_ids || !n_nodes || entry_point >= (int64_t)n_elems || (n_vec && (!vec_blob || !vec_off)))
-    return SDB_EINVAL;
-  SDB_TRY(check_index_kind("sdb_hnsw_load_staged_typed", dim, metric, (int)vt));
-  *out = nullptr;
   return hnsw_load_staged_impl(ctx, dim, metric, vt, (int)vt, n_elems, vec_blob, vec_off, vec_ids, n_vec, n_layers,
                                node_blob, node_off, node_ids, n_nodes, entry_point, out, n_bad);
 }
 
-sdb_status sdb_hnsw_select_neighbors(sdb_ctx* ctx, const float* d_vectors, uint32_t dim, sdb_metric metric, uint64_t row0,
-                                     uint64_t n, const uint64_t* d_cand, const uint32_t* d_cand_cnt, uint32_t kc,
-                                     uint32_t m_max, int presorted, uint32_t* d_out, uint32_t* d_out_cnt) {
+// Heuristic::select for n elements: row0 + i, or d_elem_ids[i] when that is given
+static sdb_status select_neighbors(sdb_ctx* ctx, const float* d_vectors, uint32_t dim, sdb_metric metric, uint64_t row0,
+                                   const uint32_t* d_elem_ids, uint64_t n, const uint64_t* d_cand,
+                                   const uint32_t* d_cand_cnt, uint32_t kc, uint32_t m_max, int presorted,
+                                   uint32_t* d_out, uint32_t* d_out_cnt) {
   if (!ctx || !d_vectors || !d_cand || !d_cand_cnt || !d_out || !d_out_cnt || !dim || !kc || !m_max) return SDB_EINVAL;
   if (metric != SDB_COSINE && metric != SDB_EUCLIDEAN) return SDB_EUNSUPPORTED;
   if (n == 0) return SDB_OK;
@@ -1614,101 +1565,40 @@ sdb_status sdb_hnsw_select_neighbors(sdb_ctx* ctx, const float* d_vectors, uint3
   const size_t smem = sizeof(float) * (2 * (size_t)dim + 2 * kc) * 4;
   auto kern = metric == SDB_COSINE ? hnsw_select_kernel<true> : hnsw_select_kernel<false>;
   SDB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  kern<<<(unsigned)((n + 3) / 4), 128, smem, ctx->stream>>>(d_vectors, dim, row0, n, nullptr, d_cand, d_cand_cnt, kc, m_max, presorted, d_out, d_out_cnt);
+  kern<<<(unsigned)((n + 3) / 4), 128, smem, ctx->stream>>>(d_vectors, dim, row0, n, d_elem_ids, d_cand, d_cand_cnt, kc, m_max, presorted, d_out, d_out_cnt);
   count_launch(ctx);
   SDB_CUDA(cudaGetLastError());
   SDB_CUDA(cudaStreamSynchronize(ctx->stream));
   return SDB_OK;
+}
+
+sdb_status sdb_hnsw_select_neighbors(sdb_ctx* ctx, const float* d_vectors, uint32_t dim, sdb_metric metric, uint64_t row0,
+                                     uint64_t n, const uint64_t* d_cand, const uint32_t* d_cand_cnt, uint32_t kc,
+                                     uint32_t m_max, int presorted, uint32_t* d_out, uint32_t* d_out_cnt) {
+  return select_neighbors(ctx, d_vectors, dim, metric, row0, nullptr, n, d_cand, d_cand_cnt, kc, m_max, presorted, d_out,
+                          d_out_cnt);
 }
 
 sdb_status sdb_hnsw_select_neighbors_ids(sdb_ctx* ctx, const float* d_vectors, uint32_t dim, sdb_metric metric,
                                          const uint32_t* d_elem_ids, uint64_t n, const uint64_t* d_cand,
                                          const uint32_t* d_cand_cnt, uint32_t kc, uint32_t m_max, int presorted,
                                          uint32_t* d_out, uint32_t* d_out_cnt) {
-  if (!ctx || !d_vectors || !d_elem_ids || !d_cand || !d_cand_cnt || !d_out || !d_out_cnt || !dim || !kc || !m_max) return SDB_EINVAL;
-  if (metric != SDB_COSINE && metric != SDB_EUCLIDEAN) return SDB_EUNSUPPORTED;
-  if (n == 0) return SDB_OK;
-  std::lock_guard<std::mutex> guard(ctx->mu);
-  SDB_CUDA(cudaSetDevice(ctx->device));
-  const size_t smem = sizeof(float) * (2 * (size_t)dim + 2 * kc) * 4;
-  auto kern = metric == SDB_COSINE ? hnsw_select_kernel<true> : hnsw_select_kernel<false>;
-  SDB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  kern<<<(unsigned)((n + 3) / 4), 128, smem, ctx->stream>>>(d_vectors, dim, 0, n, d_elem_ids, d_cand, d_cand_cnt, kc, m_max, presorted, d_out, d_out_cnt);
-  count_launch(ctx);
-  SDB_CUDA(cudaGetLastError());
-  SDB_CUDA(cudaStreamSynchronize(ctx->stream));
-  return SDB_OK;
+  if (!d_elem_ids) return SDB_EINVAL;
+  return select_neighbors(ctx, d_vectors, dim, metric, 0, d_elem_ids, n, d_cand, d_cand_cnt, kc, m_max, presorted, d_out,
+                          d_out_cnt);
 }
 
 using WalkKernel = void (*)(HnswParams);
 static WalkKernel walk_kernel(sdb_metric metric, sdb_vector_type vt, int occ) {
   if (vt == SDB_VT_F32 && metric == SDB_COSINE)
     return occ >= 8 ? hnsw_search_kernel<SDB_COSINE, 8, float> : occ <= 4 ? hnsw_search_kernel<SDB_COSINE, 4, float> : hnsw_search_kernel<SDB_COSINE, 6, float>;
-  return with_vt(vt, [&](auto tag) -> WalkKernel {
+  return with_vt(vt, [&](auto tag) {
     using T = decltype(tag);
-    switch (metric) {
-      case SDB_COSINE: return hnsw_search_kernel<SDB_COSINE, is_f32_v<T> ? 6 : 1, T>;  // (F32: returned above)
-      case SDB_MANHATTAN: return hnsw_search_kernel<SDB_MANHATTAN, 1, T>;
-      case SDB_CHEBYSHEV: return hnsw_search_kernel<SDB_CHEBYSHEV, 1, T>;
-      case SDB_HAMMING: return hnsw_search_kernel<SDB_HAMMING, 1, T>;
-      case SDB_MINKOWSKI: return hnsw_search_kernel<SDB_MINKOWSKI, 1, T>;
-      case SDB_PEARSON: return hnsw_search_kernel<SDB_PEARSON, 1, T>;
-      case SDB_JACCARD: return hnsw_search_kernel<SDB_JACCARD, 1, T>;
-      default: return hnsw_search_kernel<SDB_EUCLIDEAN, 1, T>;
-    }
+    return with_metric(metric, [&](auto met) -> WalkKernel {
+      constexpr int MET = decltype(met)::value;
+      return hnsw_search_kernel<MET, MET == SDB_COSINE && is_f32_v<T> ? 6 : 1, T>;  // (F32 cosine: returned above)
+    });
   });
-}
-// bytes of a staged query and of the distance scratch (the kernel's per-warp layout)
-static size_t walk_q_bytes(const sdb_hnsw* h) {
-  if (h->vt == SDB_VT_F32) return sizeof(float) * hn_q_floats(h->dim, h->metric == SDB_COSINE);
-  return hn_q_bytes_typed(h->dim, h->metric == SDB_JACCARD ? jkey_size(h->vt) : vt_size(h->vt));
-}
-static size_t walk_tile_bytes(const sdb_hnsw* h) { return hn_tile_bytes(h->metric == SDB_COSINE && h->vt == SDB_VT_F32); }
-
-// per-query (or per-pending-vector) state of PEARSON / JACCARD (and COSINE of the types other than F32), computed with
-// the element-side kernels
-struct BatchState {
-  double* mean = nullptr;
-  double* sx2 = nullptr;
-  void* bits = nullptr;
-  uint32_t* nbits = nullptr;
-  double* norm = nullptr;
-  void release(cudaStream_t st) {
-    if (mean) cudaFreeAsync(mean, st);
-    if (sx2) cudaFreeAsync(sx2, st);
-    if (bits) cudaFreeAsync(bits, st);
-    if (nbits) cudaFreeAsync(nbits, st);
-    if (norm) cudaFreeAsync(norm, st);
-    mean = sx2 = norm = nullptr;
-    bits = nullptr;
-    nbits = nullptr;
-  }
-};
-static sdb_status batch_state(Ctx* ctx, sdb_metric metric, sdb_vector_type vt, const void* d_v, uint64_t rows,
-                              uint32_t dim, BatchState& bs, cudaStream_t st) {
-  if (!rows) return SDB_OK;
-  const unsigned grid = (unsigned)((rows + 127) / 128);
-  if (metric == SDB_PEARSON) {
-    SDB_CUDA(cudaMallocAsync(&bs.mean, sizeof(double) * rows, st));
-    SDB_CUDA(cudaMallocAsync(&bs.sx2, sizeof(double) * rows, st));
-    with_vt(vt, [&](auto tag) {
-      using T = decltype(tag);
-      pearson_stats_kernel<T><<<grid, 128, 0, st>>>(static_cast<const T*>(d_v), dim, rows, bs.mean, bs.sx2);
-    });
-    count_launch(ctx);
-  } else if (metric == SDB_JACCARD) {
-    SDB_CUDA(cudaMallocAsync(&bs.bits, jkey_size(vt) * rows * dim, st));
-    SDB_CUDA(cudaMallocAsync(&bs.nbits, sizeof(uint32_t) * rows, st));
-    SDB_TRY(jaccard_prepare_typed(ctx, vt, d_v, rows, dim, bs.bits, bs.nbits, st));
-  } else if (metric == SDB_COSINE && vt != SDB_VT_F32) {
-    SDB_CUDA(cudaMallocAsync(&bs.norm, sizeof(double) * rows, st));
-    with_vt(vt, [&](auto tag) {
-      using T = decltype(tag);
-      hnsw_norm_kernel<T><<<grid, 128, 0, st>>>(static_cast<const T*>(d_v), dim, rows, bs.norm);
-    });
-    count_launch(ctx);
-  }
-  return SDB_OK;
 }
 
 static sdb_status hnsw_search_impl(sdb_hnsw* h, const void* queries, uint32_t nq, uint32_t k, uint32_t ef,
@@ -1738,14 +1628,18 @@ static sdb_status hnsw_search_impl(sdb_hnsw* h, const void* queries, uint32_t nq
   // candidate but only truthy ones enter w, so the window is sized for a selectivity down to ~1/16 (more = EOVERFLOW)
   uint32_t ccap = 2 * ef + 34;
   const uint32_t wcap = ef + 2;
+  // bytes of a staged query and of the distance scratch (the kernel's per-warp layout)
+  const size_t q_tile = hn_q_bytes(h->dim, h->vt == SDB_VT_F32, h->metric == SDB_COSINE,
+                                   h->metric == SDB_JACCARD ? jkey_size(h->vt) : vt_size(h->vt)) +
+                        hn_tile_bytes(h->vt == SDB_VT_F32 && h->metric == SDB_COSINE);
   if (truthy) {
     ccap = 16 * ef + 34;
     if (ccap < 1024) ccap = 1024;
-    const size_t fixed = walk_q_bytes(h) + walk_tile_bytes(h) + 12 * (size_t)wcap + 64 + 16;
+    const size_t fixed = q_tile + 12 * (size_t)wcap + 64 + 16;
     const size_t room = (220 * 1024) / HN_WARPS;
     if (fixed + 12 * (size_t)ccap > room) ccap = room > fixed + 12 * (2 * (size_t)ef + 34) ? (uint32_t)((room - fixed) / 12) : 2 * ef + 34;
   }
-  size_t per_warp = walk_q_bytes(h) + walk_tile_bytes(h) + 12 * (size_t)(ccap + wcap) + 64;
+  size_t per_warp = q_tile + 12 * (size_t)(ccap + wcap) + 64;
   per_warp = (per_warp + 15) & ~size_t(15);
   const size_t smem = per_warp * HN_WARPS;
   if (smem > 220 * 1024) {
@@ -1821,7 +1715,7 @@ static sdb_status hnsw_search_impl(sdb_hnsw* h, const void* queries, uint32_t nq
   P.truthy = d_truthy;
   P.noexp = d_noexp;
   P.vec = h->d_vec;
-  P.norm = h->d_norm;
+  P.norm = h->elems.norm;
   P.rp = h->d_rp;
   P.ci = h->d_ci;
   P.dim = h->dim;
@@ -1842,12 +1736,12 @@ static sdb_status hnsw_search_impl(sdb_hnsw* h, const void* queries, uint32_t nq
   P.out_counters = d_ctr;
   P.overflow = d_ovf;
   P.mink_p = h->minkowski_p;
-  P.e_mean = h->d_mean;
-  P.e_sx2 = h->d_sx2;
-  P.e_bits = h->d_bits;
-  P.e_nbits = h->d_nbits;
-  BatchState qs;
-  const sdb_status qrc = batch_state(ctx, h->metric, h->vt, d_q, nq, h->dim, qs, st);
+  P.e_mean = h->elems.mean;
+  P.e_sx2 = h->elems.sx2;
+  P.e_bits = h->elems.bits;
+  P.e_nbits = h->elems.nbits;
+  VecState qs;
+  const sdb_status qrc = vec_state_make(ctx, VecSet::BATCH, h->metric, h->vt, d_q, nq, h->dim, qs, st);
   P.q_mean = qs.mean;
   P.q_sx2 = qs.sx2;
   P.q_bits = qs.bits;
@@ -1857,7 +1751,7 @@ static sdb_status hnsw_search_impl(sdb_hnsw* h, const void* queries, uint32_t nq
     kern<<<grid, HN_WARPS * 32, smem, st>>>(P);
     count_launch(ctx);
   }
-  qs.release(st);
+  vec_state_free(qs, VecSet::BATCH, st);
   h->gen += gens_per_warp * n_tables;
   uint32_t ovf = 0;
   if (!device_io) {
@@ -1904,15 +1798,15 @@ static sdb_status typed_distances(Ctx* ctx, sdb_metric metric, sdb_vector_type v
   const size_t esz = vt_size(vt);
   void *d_q = nullptr, *d_v = nullptr;
   double* d_o = nullptr;
-  BatchState qs, vs;
+  VecState qs, vs;
   auto run = [&]() -> sdb_status {
     SDB_CUDA(cudaMallocAsync(&d_q, esz * dim, st));
     SDB_CUDA(cudaMallocAsync(&d_v, esz * n * dim, st));
     SDB_CUDA(cudaMallocAsync(&d_o, sizeof(double) * n, st));
     SDB_CUDA(cudaMemcpyAsync(d_q, query, esz * dim, cudaMemcpyHostToDevice, st));
     SDB_CUDA(cudaMemcpyAsync(d_v, vectors, esz * n * dim, cudaMemcpyHostToDevice, st));
-    SDB_TRY(batch_state(ctx, metric, vt, d_q, 1, dim, qs, st));
-    SDB_TRY(batch_state(ctx, metric, vt, d_v, n, dim, vs, st));
+    SDB_TRY(vec_state_make(ctx, VecSet::BATCH, metric, vt, d_q, 1, dim, qs, st));
+    SDB_TRY(vec_state_make(ctx, VecSet::BATCH, metric, vt, d_v, n, dim, vs, st));
     TypedArgs A;
     A.q = static_cast<const float*>(d_q);
     A.vecs = static_cast<const float*>(d_v);
@@ -1922,8 +1816,8 @@ static sdb_status typed_distances(Ctx* ctx, sdb_metric metric, sdb_vector_type v
     A.mq.p = minkowski_p;
     A.v_mean = vs.mean;
     A.v_sx2 = vs.sx2;
-    A.q_bits = static_cast<const uint32_t*>(qs.bits);
-    A.v_bits = static_cast<const uint32_t*>(vs.bits);
+    A.q_bits = qs.bits;
+    A.v_bits = vs.bits;
     A.v_nbits = vs.nbits;
     A.v_norm = vs.norm;
     A.q_norm = qs.norm;
@@ -1939,16 +1833,7 @@ static sdb_status typed_distances(Ctx* ctx, sdb_metric metric, sdb_vector_type v
     const unsigned grid = (unsigned)((n + 127) / 128);
     with_vt(vt, [&](auto tag) {
       using T = decltype(tag);
-      switch (metric) {
-        case SDB_COSINE: typed_distance_kernel<SDB_COSINE, T><<<grid, 128, 0, st>>>(A); break;
-        case SDB_EUCLIDEAN: typed_distance_kernel<SDB_EUCLIDEAN, T><<<grid, 128, 0, st>>>(A); break;
-        case SDB_MANHATTAN: typed_distance_kernel<SDB_MANHATTAN, T><<<grid, 128, 0, st>>>(A); break;
-        case SDB_CHEBYSHEV: typed_distance_kernel<SDB_CHEBYSHEV, T><<<grid, 128, 0, st>>>(A); break;
-        case SDB_HAMMING: typed_distance_kernel<SDB_HAMMING, T><<<grid, 128, 0, st>>>(A); break;
-        case SDB_MINKOWSKI: typed_distance_kernel<SDB_MINKOWSKI, T><<<grid, 128, 0, st>>>(A); break;
-        case SDB_PEARSON: typed_distance_kernel<SDB_PEARSON, T><<<grid, 128, 0, st>>>(A); break;
-        case SDB_JACCARD: typed_distance_kernel<SDB_JACCARD, T><<<grid, 128, 0, st>>>(A); break;
-      }
+      with_metric(metric, [&](auto met) { typed_distance_kernel<decltype(met)::value, T><<<grid, 128, 0, st>>>(A); });
     });
     count_launch(ctx);
     SDB_CUDA(cudaGetLastError());
@@ -1956,8 +1841,8 @@ static sdb_status typed_distances(Ctx* ctx, sdb_metric metric, sdb_vector_type v
     return SDB_OK;
   };
   const sdb_status rc = run();
-  qs.release(st);
-  vs.release(st);
+  vec_state_free(qs, VecSet::BATCH, st);
+  vec_state_free(vs, VecSet::BATCH, st);
   if (d_q) cudaFreeAsync(d_q, st);
   if (d_v) cudaFreeAsync(d_v, st);
   if (d_o) cudaFreeAsync(d_o, st);
