@@ -144,6 +144,27 @@ __device__ __forceinline__ uint64_t make_desc(uint32_t saddr) {
   return d;
 }
 
+// value t (0..63) of row i (0, 1) of this lane's accumulator fragment, and its column in the tile
+template <typename Acc>
+__device__ __forceinline__ Acc acc_at(const Acc (&acc)[128], int i, int t) {
+  return acc[4 * (t >> 1) + 2 * i + (t & 1)];
+}
+__device__ __forceinline__ uint32_t fragment_col(int t, uint32_t col_l) { return 8 * (t >> 1) + col_l + (t & 1); }
+// the same with a run-time t, as a chain of selects: the accumulator stays in registers
+template <typename Acc>
+__device__ __forceinline__ Acc acc_at_dyn(const Acc (&acc)[128], int i, int t) {
+  Acc v = acc[2 * i];
+#pragma unroll
+  for (int u = 1; u < 64; u++) v = u == t ? acc_at(acc, i, u) : v;
+  return v;
+}
+
+// The int8 survivor scan of the epilogue is one pass of compares that sets a bit per passing value, then a rolled loop
+// over the set bits with a single copy of append_survivor.  Unrolled over all 64 values of both rows, the append is
+// inlined 128 times (~150 KB of code that every scanning warp walks through); rolled, the streaming kernel is ~8x
+// smaller and twice as fast (DESIGN.md §5).  The bf16 kernels keep the unrolled scan: at their 168 registers the
+// rolled loop spills.
+
 // one survivor (query q = mb * BLOCK_M + row, corpus column col of the tile): appended to the (query, CTA, column
 // half) private sub-list, spilling to the query's shared list when that is full; streaming mode also counts it in the
 // query's histogram (a fire-and-forget RED)
@@ -364,18 +385,20 @@ screen_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constan
 #pragma unroll
             for (int jj = 0; jj < 32; jj++) m = max(m, max((int)acc[4 * jj + 2 * i], (int)acc[4 * jj + 2 * i + 1]));
             if (m >= tau_i) {
+              uint64_t hits = 0;
 #pragma unroll
-              for (int jj = 0; jj < 32; jj++) {
-#pragma unroll
-                for (int c = 0; c < 2; c++) {
-                  const int v = (int)acc[4 * jj + 2 * i + c];
-                  const uint32_t col = 8 * jj + col_l + c;
-                  // invalid rows (skipped / special / padding) are all-zero in the int8 copy and score exactly 0:
-                  // only a zero score needs the look-up of the row's screening norm
-                  if (v >= tau_i && (v != 0 || __ldg(snorm + row0 + col) == __ldg(snorm + row0 + col)))
-                    append_survivor<MODE>(__int2float_rn(v), q, row, col, row0, my_hp[i], s_cnt_mb, cand, cand_cnt,
-                                          cap, sub, hist);
-                }
+              for (int t = 0; t < 64; t++)
+                if ((int)acc_at(acc, i, t) >= tau_i) hits |= 1ull << t;
+              while (hits) {
+                const int t = __ffsll((long long)hits) - 1;
+                hits &= hits - 1;
+                const int v = (int)acc_at_dyn(acc, i, t);
+                const uint32_t col = fragment_col(t, col_l);
+                // invalid rows (skipped / special / padding) are all-zero in the int8 copy and score exactly 0:
+                // only a zero score needs the look-up of the row's screening norm
+                if (v != 0 || __ldg(snorm + row0 + col) == __ldg(snorm + row0 + col))
+                  append_survivor<MODE>(__int2float_rn(v), q, row, col, row0, my_hp[i], s_cnt_mb, cand, cand_cnt,
+                                        cap, sub, hist);
               }
             }
           } else {
