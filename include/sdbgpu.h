@@ -118,6 +118,37 @@ void sdb_ctx_cancel_reset(sdb_ctx*);
 sdb_status sdb_debug_schedule(uint64_t n_rows, uint32_t cand_cap, uint32_t k, uint32_t nq, int streaming,
                               uint32_t* out_tiles, uint64_t cap_tiles, uint64_t* out_n, uint32_t* out_probe_tiles,
                               uint32_t cap_probe, uint32_t* out_n_probe);
+/* Test-only diagnostics of the brute-force screens (no reference seam): the state the exactness proof rests on, so that
+ * tests can compare every intermediate with a plain reference.  Every output may be NULL.
+ * sdb_debug_corpus_state, on a finalized F32 corpus (n_pad = rows rounded up to 256):
+ *   out_f[4]    i8_scale, max_rel_qerr, bf16_rel_err, max_norm
+ *   out_u[5]    n_special, n_outliers, dim_pad, dim_pad8, n_pad
+ *   out_i8      [n_pad][dim_pad8] int8 copy of the normalised rows (cosine corpora only)
+ *   out_bf16    [n_pad][dim_pad] bf16 copy (bit patterns)
+ *   out_snorm   [n_pad] screening norm (cosine 1/|x|, euclidean |x|^2; NaN: never a screen candidate)
+ *   out_special [n_special] rows ranked exactly on every query */
+sdb_status sdb_debug_corpus_state(sdb_corpus*, float* out_f, uint32_t* out_u, int8_t* out_i8, uint16_t* out_bf16,
+                                  float* out_snorm, uint32_t* out_special);
+/* sdb_debug_screen_batch: one batch of nq host queries screened with `screen` (TC_INT8, TC_BF16 or SIMT_F32) at the
+ * first rung of the ladder, through the production sequence (streaming = 0: the multi-pass schedule), with exactly
+ * cand_cap (>= 4096) candidate slots per query.  The ladder and the exact fallback do not run: flags are as the batch
+ * left them.  score_all != 0 instead runs one pass-0 launch over every tile (SIMT: tau = -inf) with max(cand_cap,
+ * n_pad) slots and selects nothing: out_a then holds every score of that kernel, and out_b / out_rr are untouched.
+ * Let cap be the slots per query.
+ *   out_qf[nq][9]  tau, margin, bscale, beps, tau2, beps2, int8 query scale, int8 query residual, qbferr
+ *                  (the int8 figures are NaN on euclidean corpora)
+ *   out_qmag[nq]   |q| in the reference's f64 arithmetic
+ *   out_qu[nq][6]  flags, qflags, entries the stage-A selections gathered before capping (the largest over the
+ *                  batch's selections; score_all: the list's count), n_a, n_b, n_e
+ *   out_q8[nq][dim_pad8], out_qbf16[nq][dim_pad]  the query's int8 and bf16 copies
+ *   out_a[nq][cap][3]   stage-A kept list: row, screen score (f32 bits), the f32 re-score of stage B (f32 bits, NaN
+ *                       when stage B did not run); entries past n_a are (0xFFFFFFFF, NaN, NaN)
+ *   out_b[nq][cap][2]   stage-B kept list: row, score; past n_b (0xFFFFFFFF, NaN)
+ *   out_rr[nq][cap + 1024]  rows of the exact re-rank (n_e: stage-B rows, then the special rows); past n_e 0xFFFFFFFF */
+sdb_status sdb_debug_screen_batch(sdb_corpus*, const double* queries, uint32_t nq, uint32_t k, sdb_screen screen,
+                                  int streaming, uint32_t cand_cap, int score_all, float* out_qf, double* out_qmag,
+                                  uint32_t* out_qu, int8_t* out_q8, uint16_t* out_qbf16, uint32_t* out_a,
+                                  uint32_t* out_b, uint32_t* out_rr);
 uint64_t sdb_ctx_kernel_launches(const sdb_ctx*);
 /* the cudaStream_t every kernel of this context is launched on (so a harness can bracket calls with
  * CUDA events on the launching stream) */

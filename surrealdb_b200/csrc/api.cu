@@ -1,6 +1,7 @@
 // api.cu -- the extern "C" boundary (include/sdbgpu.h): contexts, corpus lifecycle, brute-force KNN driver.
 #include <cmath>
 
+#include <algorithm>
 #include <chrono>
 
 #include "internal.cuh"
@@ -197,6 +198,34 @@ void trace_dump(Ctx* ctx, Ticket& t) {
   t.trace.clear();
 }
 
+// ScreenTap (test-only): what a stage-A selection is about to gather -- main list and private sub-lists, before capping
+static sdb_status tap_gathered(Corpus* c, uint32_t nq, uint32_t n_slots, cudaStream_t st) {
+  std::vector<uint32_t> cnt(nq), sub((size_t)nq * n_slots);
+  SDB_CUDA(cudaMemcpyAsync(cnt.data(), c->d_cand_cnt, sizeof(uint32_t) * nq, cudaMemcpyDeviceToHost, st));
+  if (n_slots)
+    SDB_CUDA(cudaMemcpyAsync(sub.data(), c->d_sub_cnt, sizeof(uint32_t) * sub.size(), cudaMemcpyDeviceToHost, st));
+  SDB_CUDA(cudaStreamSynchronize(st));
+  std::vector<uint32_t>& g = c->tap->gathered;
+  g.resize(nq, 0u);
+  for (uint32_t q = 0; q < nq; q++) {
+    uint64_t n = cnt[q];
+    for (uint32_t s = 0; s < n_slots; s++) n += std::min(sub[(size_t)q * n_slots + s], c->sub_cap);
+    g[q] = std::max(g[q], (uint32_t)std::min<uint64_t>(n, 0xFFFFFFFFu));
+  }
+  return SDB_OK;
+}
+// ScreenTap: the candidate lists as they stand (cnt: their counts, optional)
+static sdb_status tap_list(Corpus* c, uint32_t nq, std::vector<Cand>* list, std::vector<uint32_t>* cnt, cudaStream_t st) {
+  list->resize((size_t)nq * c->sc_cap);
+  SDB_CUDA(cudaMemcpyAsync(list->data(), c->d_cand, sizeof(Cand) * list->size(), cudaMemcpyDeviceToHost, st));
+  if (cnt) {
+    cnt->resize(nq);
+    SDB_CUDA(cudaMemcpyAsync(cnt->data(), c->d_cand_cnt, sizeof(uint32_t) * nq, cudaMemcpyDeviceToHost, st));
+  }
+  SDB_CUDA(cudaStreamSynchronize(st));
+  return SDB_OK;
+}
+
 static sdb_status enqueue_batch(Corpus* c, Ticket& t) {
   Ctx* ctx = c->ctx;
   cudaStream_t st = t.stream;
@@ -245,6 +274,7 @@ static sdb_status enqueue_batch(Corpus* c, Ticket& t) {
       SDB_TRY(screen_tc_pass(c, nq, k, p0, int8, 0, st));
       SDB_CUDA(cudaEventRecord(t.ev_main, st));
       c->last_main = t.ev_main;
+      if (c->tap) SDB_TRY(tap_gathered(c, nq, 0u, st));
       SDB_TRY(cand_select(c, nq, k, int8, 0u, false, st));
       t.n_passes++;
     } else if (pm.count) {
@@ -255,6 +285,7 @@ static sdb_status enqueue_batch(Corpus* c, Ticket& t) {
       trace_mark(ctx, t, "main_end", st);
       SDB_CUDA(cudaEventRecord(t.ev_main, st));
       c->last_main = t.ev_main;
+      if (c->tap) SDB_TRY(tap_gathered(c, nq, c->last_slots, st));
       SDB_TRY(cand_select(c, nq, k, int8, c->last_slots, false, st));
       t.n_passes += 2;
     }
@@ -269,6 +300,7 @@ static sdb_status enqueue_batch(Corpus* c, Ticket& t) {
       }
       if (!tc) SDB_TRY(screen_simt_pass(c, nq, p, st));
       else SDB_TRY(screen_tc_pass(c, nq, k, p, int8, first_pass ? 0 : 1, st));
+      if (c->tap) SDB_TRY(tap_gathered(c, nq, tc ? c->last_slots : 0u, st));
       SDB_TRY(cand_select(c, nq, k, int8, tc ? c->last_slots : 0u, false, st));
       first_pass = false;
       t.n_passes++;
@@ -276,6 +308,7 @@ static sdb_status enqueue_batch(Corpus* c, Ticket& t) {
     SDB_CUDA(cudaEventRecord(t.ev_main, st));
     c->last_main = t.ev_main;
   }
+  if (c->tap) SDB_TRY(tap_list(c, nq, &c->tap->list_a, &c->tap->cnt_a, st));
   SDB_CUDA(cudaEventRecord(t.ev_screen1, st));
   trace_mark(ctx, t, "selected", st);
   // stage B: the coarse screens' candidates are re-scored in f32 and narrowed before the (FP64-bound) exact re-rank
@@ -283,6 +316,7 @@ static sdb_status enqueue_batch(Corpus* c, Ticket& t) {
   bool refined = false;
   if (tc && c->exact && c->dtype == SDB_F32 && !no_refine) {
     SDB_TRY(cand_refine(c, nq, st));
+    if (c->tap) SDB_TRY(tap_list(c, nq, &c->tap->list_r, nullptr, st));
     SDB_TRY(cand_select(c, nq, k, false, 0u, false, st, 1));
     refined = true;
     trace_mark(ctx, t, "refined", st);
@@ -1154,6 +1188,206 @@ sdb_status sdb_debug_schedule(uint64_t n_rows, uint32_t cand_cap, uint32_t k, ui
   *out_n = n;
   *out_n_probe = np;
   return SDB_OK;
+}
+
+// Test-only diagnostics of the screens (declared in the header's diagnostics block): the corpus' screen copies and one
+// screened batch, so that tests can hold every intermediate of the proof against a plain reference.
+sdb_status sdb_debug_corpus_state(sdb_corpus* c, float* out_f, uint32_t* out_u, int8_t* out_i8, uint16_t* out_bf16,
+                                  float* out_snorm, uint32_t* out_special) {
+  if (!c) return SDB_EINVAL;
+  std::lock_guard<std::mutex> g(c->mu);
+  if (!c->finalized || c->dtype != SDB_F32 || (out_i8 && !c->d_i8) || (out_bf16 && !c->d_bf16)) {
+    set_error("sdb_debug_corpus_state: needs a finalized F32 corpus (int8 copy: cosine only)");
+    return SDB_EINVAL;
+  }
+  SDB_CUDA(cudaSetDevice(c->ctx->device));
+  SDB_CUDA(drain(c->ctx));
+  const uint64_t n_pad = (c->n + TILE_ROWS - 1) / TILE_ROWS * TILE_ROWS;
+  if (out_f) {
+    out_f[0] = c->i8_scale;
+    out_f[1] = c->max_rel_qerr;
+    out_f[2] = c->bf16_rel_err;
+    out_f[3] = c->max_norm;
+  }
+  if (out_u) {
+    out_u[0] = c->n_special;
+    out_u[1] = c->n_outliers;
+    out_u[2] = c->dim_pad;
+    out_u[3] = c->dim_pad8;
+    out_u[4] = (uint32_t)n_pad;
+  }
+  cudaStream_t st = c->ctx->copy_stream;
+  if (out_i8 && n_pad) SDB_CUDA(cudaMemcpyAsync(out_i8, c->d_i8, n_pad * c->dim_pad8, cudaMemcpyDeviceToHost, st));
+  if (out_bf16 && n_pad)
+    SDB_CUDA(cudaMemcpyAsync(out_bf16, c->d_bf16, 2 * n_pad * c->dim_pad, cudaMemcpyDeviceToHost, st));
+  if (out_snorm && n_pad) SDB_CUDA(cudaMemcpyAsync(out_snorm, c->d_snorm, 4 * n_pad, cudaMemcpyDeviceToHost, st));
+  if (out_special && c->n_special)
+    SDB_CUDA(cudaMemcpyAsync(out_special, c->d_special, 4 * c->n_special, cudaMemcpyDeviceToHost, st));
+  SDB_CUDA(cudaStreamSynchronize(st));
+  return SDB_OK;
+}
+
+sdb_status sdb_debug_screen_batch(sdb_corpus* c, const double* queries, uint32_t nq, uint32_t k, sdb_screen screen,
+                                  int streaming, uint32_t cand_cap, int score_all, float* out_qf, double* out_qmag,
+                                  uint32_t* out_qu, int8_t* out_q8, uint16_t* out_qbf16, uint32_t* out_a,
+                                  uint32_t* out_b, uint32_t* out_rr) {
+  const bool tc = screen == SDB_SCREEN_TC_INT8 || screen == SDB_SCREEN_TC_BF16;
+  if (!c || !queries || !nq || !k || k > 256 || cand_cap < 4096 || (!tc && screen != SDB_SCREEN_SIMT_F32)) {
+    set_error("sdb_debug_screen_batch: bad argument (1 <= k <= 256, cand_cap >= 4096, a TC_INT8 / TC_BF16 / SIMT_F32 screen)");
+    return SDB_EINVAL;
+  }
+  std::lock_guard<std::mutex> g(c->mu);
+  const bool int8 = screen == SDB_SCREEN_TC_INT8;
+  if (!c->finalized || c->dtype != SDB_F32 || (c->metric != SDB_COSINE && c->metric != SDB_EUCLIDEAN) ||
+      (int8 && !c->d_i8) || c->special_overflow || !c->n) {
+    set_error("sdb_debug_screen_batch: needs a finalized, non-empty F32 cosine / euclidean corpus (int8: cosine)");
+    return SDB_EINVAL;
+  }
+  Ctx* ctx = c->ctx;
+  SDB_CUDA(cudaSetDevice(ctx->device));
+  SDB_CUDA(drain(ctx));
+  Ticket* t = free_ticket(c);
+  if (!t) {
+    set_error("too many batches in flight (%d): call sdb_knn_wait first", N_TICKETS);
+    return SDB_EOVERFLOW;
+  }
+  SDB_TRY(ticket_prepare(c, *t, nq));
+  const uint64_t n_pad = (c->n + TILE_ROWS - 1) / TILE_ROWS * TILE_ROWS;
+  const uint32_t cap = score_all ? (uint32_t)std::max<uint64_t>(cand_cap, n_pad) : cand_cap;
+  // exactly `cap` slots per query: drop the batch scratch so that ensure_scratch allocates it at this size
+  activate_set(c, 0);
+  c->sc_nq = c->sc_cap = 0;
+  SDB_TRY(scratch_for(c, nq, cap));
+  cudaStream_t st = ctx->stream;
+  double* d_q = nullptr;
+  uint64_t* d_rows = nullptr;
+  double* d_dist = nullptr;
+  uint32_t* d_cnt = nullptr;
+  ScreenTap tap;
+  const sdb_screen save_screen = c->screen;
+  const bool save_stream = c->stream_refine;
+  auto run = [&]() -> sdb_status {
+    SDB_CUDA(cudaMalloc(&d_q, sizeof(double) * (size_t)nq * c->dim));
+    SDB_CUDA(cudaMalloc(&d_rows, sizeof(uint64_t) * (size_t)nq * k));
+    SDB_CUDA(cudaMalloc(&d_dist, sizeof(double) * (size_t)nq * k));
+    SDB_CUDA(cudaMalloc(&d_cnt, sizeof(uint32_t) * nq));
+    SDB_CUDA(cudaMemcpyAsync(d_q, queries, sizeof(double) * (size_t)nq * c->dim, cudaMemcpyHostToDevice, st));
+    if (score_all) {  // one pass-0 launch over every tile (SIMT: tau stays -inf), nothing selected
+      const PassDesc all{1u, 0u, (uint32_t)(n_pad / TILE_ROWS), 0u};
+      SDB_TRY(prep_queries(c, d_q, nq, st));
+      SDB_TRY(cand_begin(c, nq, (int)screen, st));
+      if (tc) SDB_TRY(screen_tc_pass(c, nq, k, all, int8, 0, st));
+      else SDB_TRY(screen_simt_pass(c, nq, all, st));
+      SDB_TRY(tap_list(c, nq, &tap.list_a, &tap.cnt_a, st));
+      tap.gathered = tap.cnt_a;
+      return SDB_OK;
+    }
+    // the production sequence of one batch at rung 0 of `screen` (no ladder, no exact fallback)
+    c->screen = screen;
+    c->stream_refine = streaming != 0;
+    t->set = 0;
+    t->stream = st;
+    t->d_queries = d_q;
+    t->nq = nq;
+    t->k = k;
+    t->row_base = 0;
+    t->d_out_rows = d_rows;
+    t->d_out_dist = d_dist;
+    t->d_out_count = d_cnt;
+    t->cancel = nullptr;
+    t->rung = 0;
+    c->tap = &tap;
+    const sdb_status rc = enqueue_batch(c, *t);
+    c->tap = nullptr;
+    SDB_TRY(rc);
+    SDB_CUDA(cudaStreamSynchronize(st));
+    if (t->screen != (int)screen) {
+      set_error("sdb_debug_screen_batch: the corpus does not offer screen %d", (int)screen);
+      return SDB_EINVAL;
+    }
+    return SDB_OK;
+  };
+  sdb_status rc = run();
+  c->tap = nullptr;
+  c->screen = save_screen;
+  c->stream_refine = save_stream;
+  if (rc == SDB_OK) {  // per-query figures and lists (columns documented in the header)
+    auto rd = [&](void* dst, const void* src, size_t bytes) {
+      if (rc == SDB_OK && cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToHost, st) != cudaSuccess) {
+        set_error("sdb_debug_screen_batch: copy-out failed");
+        rc = SDB_ECUDA;
+      }
+    };
+    const size_t cap_sz = (size_t)nq * cap;
+    std::vector<float> f[9];
+    const float* srcf[9] = {c->d_tau, c->d_margin, c->d_bscale, c->d_beps, c->d_tau2, c->d_beps2,
+                            c->d_i8 ? c->d_q8scale : nullptr, c->d_i8 ? c->d_q8err : nullptr, c->d_qbferr};
+    for (int j = 0; j < 9; j++) {
+      f[j].assign(nq, NAN);
+      if (srcf[j]) rd(f[j].data(), srcf[j], sizeof(float) * nq);
+    }
+    std::vector<uint32_t> flags(nq), qflags(nq), cnt_b(nq);
+    std::vector<Cand> list_b(score_all ? 0 : cap_sz);
+    std::vector<uint32_t> rr;
+    rd(flags.data(), c->d_flags, sizeof(uint32_t) * nq);
+    rd(qflags.data(), c->d_qflags, sizeof(uint32_t) * nq);
+    if (out_qmag) rd(out_qmag, c->d_qmag, sizeof(double) * nq);
+    if (out_q8 && c->d_i8) rd(out_q8, c->d_q8, (size_t)nq * c->dim_pad8);
+    if (out_qbf16) rd(out_qbf16, c->d_qbf16, 2 * (size_t)nq * c->dim_pad);
+    if (!score_all) {
+      rd(cnt_b.data(), c->d_cand_cnt, sizeof(uint32_t) * nq);
+      rd(list_b.data(), c->d_cand, sizeof(Cand) * cap_sz);
+      if (out_rr) {
+        rr.resize((size_t)nq * c->rr_stride);
+        rd(rr.data(), c->d_rr_row, sizeof(uint32_t) * rr.size());
+      }
+    }
+    if (rc == SDB_OK && cudaStreamSynchronize(st) != cudaSuccess) rc = SDB_ECUDA;
+    if (rc == SDB_OK) {
+      const uint32_t n_special = score_all ? 0u : c->n_special;
+      auto bits = [](float v) {
+        uint32_t u;
+        memcpy(&u, &v, 4);
+        return u;
+      };
+      for (uint32_t q = 0; q < nq; q++) {
+        if (out_qf)
+          for (int j = 0; j < 9; j++) out_qf[(size_t)q * 9 + j] = f[j][q];
+        const uint32_t n_a = std::min(tap.cnt_a[q], cap), n_b = score_all ? 0u : std::min(cnt_b[q], cap);
+        if (out_qu) {
+          uint32_t* u = out_qu + (size_t)q * 6;
+          u[0] = flags[q];
+          u[1] = qflags[q];
+          u[2] = tap.gathered.empty() ? 0u : tap.gathered[q];
+          u[3] = n_a;
+          u[4] = n_b;
+          u[5] = score_all ? 0u : n_b + n_special;
+        }
+        for (uint32_t e = 0; e < cap; e++) {
+          const size_t i = (size_t)q * cap + e;
+          if (out_a) {
+            const bool have = e < n_a;
+            out_a[3 * i] = have ? tap.list_a[i].row : 0xFFFFFFFFu;
+            out_a[3 * i + 1] = have ? bits(tap.list_a[i].score) : 0x7fc00000u;
+            out_a[3 * i + 2] = have && !tap.list_r.empty() ? bits(tap.list_r[i].score) : 0x7fc00000u;
+          }
+          if (out_b) {
+            const bool have = e < n_b;
+            out_b[2 * i] = have ? list_b[i].row : 0xFFFFFFFFu;
+            out_b[2 * i + 1] = have ? bits(list_b[i].score) : 0x7fc00000u;
+          }
+        }
+        if (out_rr && !score_all)
+          for (uint32_t e = 0; e < cap + SPECIAL_CAP; e++)
+            out_rr[(size_t)q * (cap + SPECIAL_CAP) + e] = e < n_b + n_special ? rr[(size_t)q * c->rr_stride + e] : 0xFFFFFFFFu;
+      }
+    }
+  }
+  cudaFree(d_q);
+  cudaFree(d_rows);
+  cudaFree(d_dist);
+  cudaFree(d_cnt);
+  return rc;
 }
 
 sdb_status sdb_knn_submit(sdb_corpus* c, const double* queries, uint32_t nq, uint32_t k, uint64_t* out_rows,

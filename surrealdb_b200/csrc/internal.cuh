@@ -241,8 +241,18 @@ struct Scratch {
   uint32_t sc_gen = 0;           // bumped whenever this set is reallocated
 };
 
+// Test-only snapshot of one batch's stage-A candidate lists (sdb_debug_screen_batch).  enqueue_batch fills it when
+// Corpus::tap is set, which is never the case in production.
+struct ScreenTap {
+  std::vector<uint32_t> gathered;  // per query: most entries any stage-A selection gathered, before capping
+  std::vector<Cand> list_a;        // [nq][cap]: kept list after the last stage-A selection
+  std::vector<uint32_t> cnt_a;
+  std::vector<Cand> list_r;        // [nq][cap]: the same list after cand_refine re-scored it in f32 (empty if it did not run)
+};
+
 struct Corpus : Scratch {
   Ctx* ctx = nullptr;
+  ScreenTap* tap = nullptr;  // test-only (see ScreenTap)
   uint32_t dim = 0, dim_pad = 0;  // dim_pad: bf16 screen copy row length (multiple of 64)
   sdb_dtype dtype = SDB_F32;
   sdb_metric metric = SDB_COSINE;
