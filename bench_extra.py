@@ -1,7 +1,8 @@
 #!/usr/bin/env python
 """Secondary measurements for the other rows of SURVEY.md section 8 (NOT the driver's headline line):
 
-  python bench_extra.py hnsw  [--rows N --dim D --queries Q --ef 64 --k 10 --metric M --graph-metric G --vector-type T]
+  python bench_extra.py hnsw  [--rows N --dim D --queries Q --ef 64 --k 10 --metric M --graph-metric G --vector-type T
+                               --build-in-type]
   python bench_extra.py graph [--log2-nodes 24 --edges E --sources 1024 --hops 3]
 
 Each prints one JSON line with the metric, a roofline object computed from in-kernel counters
@@ -44,13 +45,13 @@ def dev_time_ms(ctx, fn):
 
 def bench_hnsw(a):
     import torch
-    from surrealdb_b200 import Context, HnswIndex, VectorColumn
+    from surrealdb_b200 import Context, HnswIndex
     from surrealdb_b200.hnsw_build import build_layers
     ctx = Context(0)
     dev = torch.device("cuda", 0)
     g = torch.Generator(device=dev).manual_seed(0x5DB00003)
     n, dim = a.rows, a.dim
-    gm = (a.graph_metric or a.metric).upper()  # the builders serve cosine / euclidean; the walk serves every metric
+    gm = (a.graph_metric or a.metric).upper()  # metric the graph is linked with
     centers = torch.nn.functional.normalize(torch.randn((4096, dim), generator=g, device=dev), dim=1)
     def sample(cnt):
         # sigma = TOTAL noise norm relative to the unit-norm centroid (per-coordinate sigma / sqrt(dim)); a per-coordinate
@@ -63,6 +64,7 @@ def bench_hnsw(a):
         return out
     x = sample(n)
     queries = sample(a.queries)
+    x0h = x.cpu().numpy() if a.build_in_type else None  # the data in its original order (the incremental builder re-orders)
     torch.cuda.synchronize()
     t0 = time.perf_counter()
     tl = [time.perf_counter()]
@@ -71,53 +73,69 @@ def bench_hnsw(a):
             now = time.perf_counter()
             print(f"[build] layer {l} stage {a1} value {b1} +{now - tl[0]:.1f}s", file=sys.stderr, flush=True)
             tl[0] = now
-    if a.builder == "incremental":
-        from surrealdb_b200.hnsw_build import build_incremental
-        res = build_incremental(ctx, x, gm, m=a.m, m0=2 * a.m, efc=a.efc, seed=7, growth=a.growth, progress=prog,
-                                settle=not a.no_settle)
-        x = res["x"]  # re-ordered by level: element ids below are the NEW ids (rows of this tensor)
-        layers = [(rp.cpu().numpy().astype(np.uint64), ci.cpu().numpy().astype(np.uint32)) for rp, ci in res["layers_dev"]] if not a.no_cpu else None
-        entry = res["entry"]
-        print(f"[build] done {time.perf_counter() - t0:.1f}s", file=sys.stderr, flush=True)
-        build_s = time.perf_counter() - t0
-        idx = HnswIndex.from_device(ctx, x, res["layers_dev"], entry, a.metric.upper(), minkowski_order=a.minkowski_order)
-        n_layers = len(res["layers_dev"])
-        deg0 = float(res["layers_dev"][0][1].numel()) / n
-        xh = x.cpu().numpy() if not a.no_cpu or a.vector_type != "F32" else None
-        if a.vector_type != "F32":
-            layers = [(rp.cpu().numpy().astype(np.uint64), ci.cpu().numpy().astype(np.uint32)) for rp, ci in res["layers_dev"]]
-    else:
-        layers, entry, levels = build_layers(ctx, x, n, dim, gm, m=a.m, m0=2 * a.m, seed=7, progress=prog, prefix=a.prefix)
-        print(f"[build] done {time.perf_counter() - t0:.1f}s", file=sys.stderr, flush=True)
-        build_s = time.perf_counter() - t0
-        xh = x.cpu().numpy()
-        idx = HnswIndex(ctx, xh, layers, entry, a.metric.upper(), minkowski_order=a.minkowski_order)
-        n_layers = len(layers)
-        deg0 = float(np.diff(layers[0][0].astype(np.int64)).mean())
-    qh0, q_dev0, idx0 = queries.cpu().numpy(), queries, idx
-    for vt in a.vector_type.split(","):  # one JSON line per vector type, all on the same graph
-        # another vector type: the graph above is the F32 build of the same seeded data; the index holds the data in the type
-        # (integers: scaled by INT_SCALE and truncated toward zero) and is walked in that type's arithmetic
-        esz = {"F64": 8, "F32": 4, "I64": 8, "I32": 4, "I16": 2}[vt]
-        INT_SCALE = 8192.0
-        qh, queries, idx = qh0, q_dev0, idx0
-        if vt != "F32":
-            from surrealdb_b200.hnsw import VT_DTYPE, to_vector_type
-            scale = INT_SCALE if vt[0] == "I" else 1.0
+    INT_SCALE = 8192.0
+    from surrealdb_b200.hnsw import VT_DTYPE, to_vector_type
 
-            def convert(h):  # in slabs: 1M x 768 f64 temporaries would need ~20 GB of host memory
-                out = np.empty(h.shape, VT_DTYPE[vt])
-                for r0 in range(0, h.shape[0], 1 << 16):
-                    out[r0:r0 + (1 << 16)] = to_vector_type(h[r0:r0 + (1 << 16)].astype(np.float64) * scale, vt)
-                return out
-            xt, qh = convert(xh), convert(qh)
-            idx = HnswIndex(ctx, xt, layers, entry, a.metric.upper(), minkowski_order=a.minkowski_order, vector_type=vt)
+    def convert(h, vt):  # in slabs: 1M x 768 f64 temporaries would need ~20 GB of host memory
+        scale = INT_SCALE if vt[0] == "I" else 1.0
+        out = np.empty(h.shape, VT_DTYPE[vt])
+        for r0 in range(0, h.shape[0], 1 << 16):
+            out[r0:r0 + (1 << 16)] = to_vector_type(h[r0:r0 + (1 << 16)].astype(np.float64) * scale, vt)
+        return out
+
+    def build(xb, vt):
+        """builds the graph from xb (device, vector type vt) in metric gm -> (index walked in a.metric, its vectors
+        on the device, host layers or None, entry, layer count, mean layer-0 degree, build seconds)"""
+        torch.cuda.synchronize()
+        t0 = time.perf_counter()
+        if a.builder == "incremental":
+            from surrealdb_b200.hnsw_build import build_incremental
+            res = build_incremental(ctx, xb, gm, m=a.m, m0=2 * a.m, efc=a.efc, seed=7, growth=a.growth, progress=prog,
+                                    settle=not a.no_settle, vector_type=vt, minkowski_order=a.minkowski_order)
+            torch.cuda.synchronize()
+            build_s = time.perf_counter() - t0
+            xb = res["x"]  # re-ordered by level: element ids below are the NEW ids (rows of this tensor)
+            layers = [(rp.cpu().numpy().astype(np.uint64), ci.cpu().numpy().astype(np.uint32)) for rp, ci in res["layers_dev"]] if not a.no_cpu else None
+            idx = HnswIndex.from_device(ctx, xb, res["layers_dev"], res["entry"], a.metric.upper(),
+                                        minkowski_order=a.minkowski_order, vector_type=vt)
+            out = (idx, xb, layers, res["entry"], len(res["layers_dev"]), float(res["layers_dev"][0][1].numel()) / n, build_s)
+        else:
+            layers, entry, levels = build_layers(ctx, xb, n, dim, gm, m=a.m, m0=2 * a.m, seed=7, progress=prog,
+                                                 prefix=a.prefix, vector_type=vt, minkowski_order=a.minkowski_order)
+            build_s = time.perf_counter() - t0
+            idx = HnswIndex(ctx, xb.cpu().numpy(), layers, entry, a.metric.upper(), minkowski_order=a.minkowski_order,
+                            vector_type=vt)
+            out = (idx, xb, layers, entry, len(layers), float(np.diff(layers[0][0].astype(np.int64)).mean()), build_s)
+        print(f"[build] {vt} done {build_s:.1f}s", file=sys.stderr, flush=True)
+        return out
+
+    vts = a.vector_type.split(",")
+    idx = layers = entry = n_layers = deg0 = build_s = xh = None
+    if not a.build_in_type or "F32" in vts:  # the F32 graph (the one every type is walked on without --build-in-type)
+        idx, x, layers, entry, n_layers, deg0, build_s = build(x, "F32")
+        xh = x.cpu().numpy() if not a.no_cpu or a.vector_type != "F32" else None
+        if a.vector_type != "F32" and layers is None:
+            layers = [(rp.cpu().numpy().astype(np.uint64), ci.cpu().numpy().astype(np.uint32)) for rp, ci in idx._keep[1]]
+    qh0, q_dev0, idx0 = queries.cpu().numpy(), queries, idx
+    for vt in vts:  # one JSON line per vector type
+        # another vector type: the index holds the data in the type (integers: scaled by INT_SCALE and truncated toward
+        # zero) and is walked in that type's arithmetic, on the F32 graph above or (--build-in-type) on a graph built in
+        # the type
+        esz = {"F64": 8, "F32": 4, "I64": 8, "I32": 4, "I16": 2}[vt]
+        qh, queries, idx, vt_build_s, vt_layers, vt_deg0 = qh0, q_dev0, idx0, build_s, n_layers, deg0
+        if vt != "F32":
+            qh = convert(qh0, vt)
             queries = torch.from_numpy(qh).to(dev)
+            if a.build_in_type:  # the graph is built in the type's own arithmetic, from the same data in the type
+                idx, _, _, _, vt_layers, vt_deg0, vt_build_s = build(torch.from_numpy(convert(x0h, vt)).to(dev), vt)
+            else:
+                idx = HnswIndex(ctx, convert(xh, vt), layers, entry, a.metric.upper(), minkowski_order=a.minkowski_order,
+                                vector_type=vt)
         print(f"[load] index on device {time.perf_counter() - t0:.1f}s", file=sys.stderr, flush=True)
         idx.search_graph(qh[:256], a.k, a.ef)  # warm-up
         (ids, dist, cnt, ctr), ms_call, wall = dev_time_ms(ctx, lambda: idx.search_graph(qh, a.k, a.ef, counters=True))
         visited, expanded = int(ctr[:, 0].sum()), int(ctr[:, 1].sum())
-        byts = visited * (esz * dim + 4.0) + expanded * deg0 * 4.0
+        byts = visited * (esz * dim + 4.0) + expanded * vt_deg0 * 4.0
         # `value`: queries and results resident in HBM (sdb_hnsw_search_device); the host-buffer call above is the e2e figure
         import ctypes as C
         from surrealdb_b200 import _lib as L
@@ -135,30 +153,25 @@ def bench_hnsw(a):
             best = m1 if best is None or m1 < best else best
         ms = best
         same_dev = bool(np.array_equal(d_ids.cpu().numpy()[:, :1].astype(np.uint64), ids[:, :1]))
-        # recall@k against exact brute force (f64 reference arithmetic) on the same corpus (F32 indexes: the brute-force
-        # corpora hold F32 / F64 rows only)
-        recall = None
-        if vt == "F32":
-            col = VectorColumn(ctx, dim, a.metric.upper(), "F32", capacity=n)
-            if a.metric.upper() == "MINKOWSKI":
-                col.set_minkowski_order(a.minkowski_order)
-            torch.cuda.synchronize()
-            col.append_device(x.data_ptr(), n)
-            col.finalize()
-            nr = min(a.queries, 2000)
-            rows, _, _ = col.knn(qh[:nr].astype(np.float64), a.k)
-            recall = float(np.mean([len(set(rows[i].tolist()) & set(ids[i, : cnt[i]].tolist())) / a.k for i in range(nr)]))
+        # recall@k against the exact kNN in the index's own arithmetic (sdb_hnsw_knn_exact_device)
+        from surrealdb_b200.hnsw_build import knn_exact
+        nr = min(a.queries, a.recall_queries)
+        t_ids, _, t_cnt = knn_exact(idx.h, queries[:nr], a.k)
+        t_ids, t_cnt = t_ids.cpu().numpy(), t_cnt.cpu().numpy()
+        recall = float(np.mean([len(set(t_ids[i, : t_cnt[i]].tolist()) & set(ids[i, : cnt[i]].tolist())) / a.k
+                                for i in range(nr)]))
         peak, src = peaks()
         out = {"bench": "hnsw_search", "metric": f"HNSW KNN queries/sec (M={a.m}, M0={2*a.m}, ef={a.ef}, k={a.k})",
                "value": a.queries / (ms * 1e-3), "unit": "queries/s", "device_ms": ms,
                "e2e": {"value": a.queries / (wall * 1e-3), "unit": "queries/s", "call_wall_ms": wall, "api": "sdb_hnsw_search (pageable host queries and results)",
                        "h2d_bytes": int(a.queries * dim * esz), "d2h_bytes": int(a.queries * a.k * 16 + a.queries * 20)},
                "device_results_equal_host_call": same_dev,
-               "recall_at_k": recall, "config": {"rows": n, "dim": dim, "queries": a.queries, "metric": a.metric.lower(), "graph_metric": gm.lower(),
-                                                  "vector_type": vt, **({"int_scale": INT_SCALE, "data_to_int": f"x * {INT_SCALE:g}, truncated toward zero"} if vt[0] == "I" else {}),
+               "recall_at_k": recall, "recall_queries": nr, "build_s": vt_build_s, "config": {"rows": n, "dim": dim, "queries": a.queries, "metric": a.metric.lower(), "graph_metric": gm.lower(),
+                                                  "vector_type": vt, "graph_vector_type": vt if a.build_in_type else "F32", **({"int_scale": INT_SCALE, "data_to_int": f"x * {INT_SCALE:g}, truncated toward zero"} if vt[0] == "I" else {}),
                                                   **({"minkowski_order": a.minkowski_order} if a.metric.upper() == "MINKOWSKI" else {}), "data": f"4096 unit-norm centroids + gaussian noise of total norm {a.sigma}",
-                                                  "graph": ("GPU batched true insertion (hnsw_build.build_incremental): walk kernel as insertion search (efc=%d), Heuristic::select, bidirectional linking, re-selection of over-full nodes; batches grow by %.2fx" % (a.efc, a.growth)) if a.builder == "incremental" else "GPU batch-built layers (hnsw_build.py): kNN candidates" + (" from id prefixes" if a.prefix else "") + " + Heuristic::select + bidirectional re-selection", "build_s": build_s,
-                                                  "layers": n_layers, "visited_per_query": visited / a.queries,
+                                                  "graph": ("GPU batched true insertion (hnsw_build.build_incremental): walk kernel as insertion search (efc=%d), Heuristic::select, bidirectional linking, re-selection of over-full nodes; batches grow by %.2fx" % (a.efc, a.growth)) if a.builder == "incremental" else "GPU batch-built layers (hnsw_build.py): kNN candidates" + (" from id prefixes" if a.prefix else "") + " + Heuristic::select + bidirectional re-selection", "build_s": vt_build_s,
+                                                  "recall_truth": "sdb_hnsw_knn_exact_device (exact kNN in the index's arithmetic)",
+                                                  "layers": vt_layers, "visited_per_query": visited / a.queries,
                                                   "expanded_per_query": expanded / a.queries},
                "roofline": {"bound": "hbm", "kernel": "hnsw_search_kernel", "achieved": byts / (ms * 1e-3) / 1e9, "peak": peak,
                             "unit": "GB/s", "frac": byts / (ms * 1e-3) / 1e9 / peak, "peak_source": src,
@@ -408,12 +421,15 @@ if __name__ == "__main__":
     ap.add_argument("--m", type=int, default=16)
     metrics = ["euclidean", "cosine", "manhattan", "chebyshev", "hamming", "minkowski", "pearson", "jaccard"]
     ap.add_argument("--metric", default="euclidean", choices=metrics, help="metric of the walk (and of the recall)")
-    ap.add_argument("--graph-metric", default=None, choices=["euclidean", "cosine"],
+    ap.add_argument("--graph-metric", default=None, choices=metrics,
                     help="metric the GPU builder links the graph with (default: --metric)")
     ap.add_argument("--minkowski-order", type=float, default=3.0)
     ap.add_argument("--vector-type", default="F32",
                     help="element type(s) of the index, F64 F32 I64 I32 I16, comma-separated (the graph is built once, in "
-                         "F32, from the same data; one result line per type)")
+                         "F32, from the same data, unless --build-in-type; one result line per type)")
+    ap.add_argument("--build-in-type", action="store_true",
+                    help="build every --vector-type index's graph in that type's own arithmetic, from the data in the type")
+    ap.add_argument("--recall-queries", type=int, default=1000, help="queries of the recall@k against the exact kNN")
     ap.add_argument("--sigma", type=float, default=0.15)
     ap.add_argument("--prefix", action="store_true", help="insertion-order (prefix) candidate sets in the batch builder")
     ap.add_argument("--builder", default="batch", choices=["batch", "incremental"])

@@ -294,13 +294,22 @@ sdb_status sdb_hnsw_load_typed(sdb_ctx*, uint32_t dim, sdb_metric, sdb_vector_ty
                                int64_t entry_point, sdb_hnsw** out);
 /* Device-resident variants for index construction (SURVEY 8f-2): vectors and per-layer CSR arrays are DEVICE pointers
  * that the handle BORROWS (nothing is copied; the caller keeps them alive and unchanged while the handle exists), and
- * the search takes device queries / writes device results.  The incremental builder re-wraps the growing graph with
- * sdb_hnsw_load_device after every insertion batch and uses the walk kernel itself as the insertion search
- * (Hnsw::insert -> HnswLayer::search_multi with efc, hnsw/mod.rs:297-377, hnsw/layer.rs:342-387). */
-/* F32 only: its caller is the F32 GPU builder. */
+ * the search takes device queries / writes device results.  The incremental builder uses the walk kernel itself as the
+ * insertion search (Hnsw::insert -> HnswLayer::search_multi with efc, hnsw/mod.rs:297-377, hnsw/layer.rs:342-387).
+ * sdb_hnsw_load_device is sdb_hnsw_load_device_typed with SDB_VT_F32. */
 sdb_status sdb_hnsw_load_device(sdb_ctx*, uint32_t dim, sdb_metric, uint64_t n_elems, const float* d_vectors,
                                 uint32_t n_layers, const uint64_t* const* d_row_ptr, const uint32_t* const* d_col_idx,
                                 int64_t entry_point, sdb_hnsw** out);
+/* Any vector type: d_vectors holds n_elems x dim elements of it.  Refusals as sdb_hnsw_load_typed. */
+sdb_status sdb_hnsw_load_device_typed(sdb_ctx*, uint32_t dim, sdb_metric, sdb_vector_type, uint64_t n_elems,
+                                      const void* d_vectors, uint32_t n_layers, const uint64_t* const* d_row_ptr,
+                                      const uint32_t* const* d_col_idx, int64_t entry_point, sdb_hnsw** out);
+/* Swaps the adjacency of a handle from sdb_hnsw_load_device[_typed] (the new arrays are borrowed the same way; the old
+ * ones are no longer read once this returns) and keeps the elements' metric state (cosine norms, Pearson moments,
+ * Jaccard keys), which depends on the vectors only.  The builder re-points one handle at the growing graph after every
+ * insertion batch, or at layers [l .. top] to search from layer l.  SDB_EINVAL on a handle that owns its arrays. */
+sdb_status sdb_hnsw_set_layers_device(sdb_hnsw*, uint32_t n_layers, const uint64_t* const* d_row_ptr,
+                                      const uint32_t* const* d_col_idx, int64_t entry_point);
 sdb_status sdb_hnsw_search_device(sdb_hnsw*, const void* d_queries, uint32_t nq, uint32_t k, uint32_t ef,
                                   uint64_t* d_out_elems, double* d_out_dist, uint32_t* d_out_count);
 void sdb_hnsw_destroy(sdb_hnsw*);
@@ -381,8 +390,35 @@ sdb_status sdb_hnsw_load_staged_typed(sdb_ctx*, uint32_t dim, sdb_metric, sdb_ve
 sdb_status sdb_hnsw_search(sdb_hnsw*, const void* queries, uint32_t nq, uint32_t k, uint32_t ef,
                            uint64_t* out_elems, double* out_dist, uint32_t* out_count, uint64_t* out_counters);
 
+/* Exact kNN over the elements of an index, in its own arithmetic (TestCollection::knn, idx/trees/hnsw/mod.rs:1186-1197):
+ * for every query, d = Distance::calculate(element, query) -- the walk's argument order and distance code, so d equals
+ * what sdb_hnsw_search reports for the pair -- and the k smallest ordered by (total-order key of d, element id), the
+ * order of KnnResultBuilder.  d_members (device, distinct element ids, any order): the candidates, n_members of them;
+ * NULL = every element.  d_queries: nq x dim elements of the index's vector type (device); d_out_elems / d_out_dist
+ * nq x k, d_out_count nq = min(k, candidates) (device).  1 <= k <= 256, else SDB_EINVAL; a member id >= n_elems is
+ * SDB_EINVAL.  -0.0 is reported as 0.0, as by the walk.  Used for the GPU builder's candidate lists and for ground-truth
+ * recall. */
+sdb_status sdb_hnsw_knn_exact_device(sdb_hnsw*, const void* d_queries, uint32_t nq, uint32_t k, const uint32_t* d_members,
+                                     uint64_t n_members, uint64_t* d_out_elems, double* d_out_dist, uint32_t* d_out_count);
+/* Heuristic::select, standard variant (idx/trees/hnsw/heuristic.rs:61-81,201-216), for any metric and vector type, on
+ * the handle's vectors, element state and Minkowski order, with the walk's distance code: a selection made from a given
+ * candidate list equals the reference's.  Elements d_elem_ids[i] (device; NULL: row0 + i), i < n; d_cand n x kc
+ * element ids (device), d_cand_cnt valid entries per row; the element itself may appear and is skipped.  If at most
+ * m_max candidates other than the element remain, all are taken.  Otherwise candidates are visited in order and e is
+ * accepted iff e_dist > r_dist holds for no accepted r, r_dist = calculate(r, e) (elements.rs:133-140), until m_max are
+ * accepted.  presorted != 0: the list is visited as given, e_dist = calculate(e, element), the distance an insertion
+ * search or sdb_hnsw_knn_exact_device ranked it by; presorted = 0 (build_priority_list, layer.rs:389-405): e_dist =
+ * calculate(element, e) and the list is visited by e_dist, equal distances in list order.  d_out: n x m_max element
+ * ids, d_out_cnt accepted count (device).  Candidate ids must be < n_elems. */
+sdb_status sdb_hnsw_select_device(sdb_hnsw*, const uint32_t* d_elem_ids, uint64_t row0, uint64_t n, const uint64_t* d_cand,
+                                  const uint32_t* d_cand_cnt, uint32_t kc, uint32_t m_max, int presorted, uint32_t* d_out,
+                                  uint32_t* d_out_cnt);
+
 /* Index-construction helper (SURVEY 8f-2, "next" row): Heuristic::select, standard variant
- * (idx/trees/hnsw/heuristic.rs:61-81,201-216), applied in parallel to pre-ranked candidate lists.
+ * (idx/trees/hnsw/heuristic.rs:61-81,201-216), applied in parallel to pre-ranked candidate lists.  F32 COSINE and
+ * EUCLIDEAN only (SDB_EUNSUPPORTED otherwise), in its own f32 arithmetic (fused multiply-adds, squared euclidean), not
+ * the walk's: the F32 cosine / euclidean GPU builder keeps it so that its graphs do not change.  Every other metric and
+ * type: sdb_hnsw_select_device.
  * d_vectors: n x dim f32 (device) of the layer's members; d_cand: n x kc candidate member indices, nearest first
  * (e.g. the rows written by sdb_knn_bruteforce_device; the element itself is skipped), d_cand_cnt: valid entries per
  * row.  For every element: if it has <= m_max candidates all are taken, otherwise candidates are visited nearest-first

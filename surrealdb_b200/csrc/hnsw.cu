@@ -18,6 +18,7 @@
 #include <algorithm>
 #include <type_traits>
 
+#include <cub/device/device_radix_sort.cuh>
 #include <cub/device/device_segmented_sort.cuh>
 
 #include "internal.cuh"
@@ -704,8 +705,9 @@ __device__ __forceinline__ double warp_distance_rows(const T* __restrict__ vec, 
 
 // JACCARD, calculate(a = element, b = query): only m = |distinct(element) & distinct(query)| is per pair.  The query's
 // sorted distinct keys (q_u of them) are in shared memory; the warp takes one new row at a time, every lane binary-
-// searching a 32-key slice of the row's distinct list.
-template <typename T>
+// searching a 32-key slice of the row's distinct list.  QFIRST: calculate(a = query, b = element) instead, from the same
+// counts (the re-sort mode of the neighbour selection).
+template <typename T, bool QFIRST = false>
 __device__ __forceinline__ double warp_distance_jaccard(const JKey<T>* __restrict__ bits, const uint32_t* __restrict__ nbits,
                                                         uint32_t dim, uint32_t my_row, const JKey<T>* s_qb, uint32_t q_u,
                                                         float (*tile)[33]) {
@@ -724,7 +726,7 @@ __device__ __forceinline__ double warp_distance_jaccard(const JKey<T>* __restric
     uint32_t m = 0;
     for (uint32_t i = lane; i < ua; i += 32) m += sorted_contains(s_qb, q_u, __ldg(eb + i));
     m = __reduce_add_sync(0xffffffffu, m);
-    if (lane == 0) res[r] = jaccard_typed<T>(dim, ua, q_u, m);
+    if (lane == 0) res[r] = QFIRST ? jaccard_typed<T>(dim, q_u, ua, m) : jaccard_typed<T>(dim, ua, q_u, m);
   }
   __syncwarp();
   return my_row != NO_ROW ? res[ci] : 0.0;
@@ -802,6 +804,56 @@ struct HnswParams {
   const uint32_t* q_nbits;
   const double* q_norm;       // COSINE of the types other than F32: per query norm (the elements' are `norm`)
 };
+
+// Stages vector r of a set (the queries of a walk, or an element) in shared memory as the distance functions above read
+// it: F32 COSINE transposed (hn_q_stride) with its 8-lane norm computed here (the same arithmetic as the elements'
+// hnsw_norm_f32_kernel), JACCARD its sorted distinct keys, every other cell its dim elements; the set's metric state at
+// r goes to q_norm / mq.  All 32 lanes must call.  The same steps as the staging in hnsw_search_kernel, which keeps its
+// own inline copy, so that the walk's generated code stays as it was (calling this from there schedules it differently).
+template <int MET, typename T, typename I>
+__device__ __forceinline__ void stage_vector(uint32_t dim, const void* vecs, const double* norm, const double* mean,
+                                             const double* sx2, const void* bits, const uint32_t* nbits, double mink_p,
+                                             I r, float* s_q, double& q_norm, MetricQ& mq) {
+  constexpr bool COSINE = MET == SDB_COSINE && is_f32_v<T>;
+  const uint32_t lane = threadIdx.x & 31;
+  if (COSINE) {
+    const uint32_t qs = hn_q_stride(dim), d8 = dim & ~7u, steps = dim >> 3;
+    const float* qg = static_cast<const float*>(vecs) + (size_t)r * dim;
+    for (uint32_t c = lane; c < dim; c += 32) {
+      const float v = qg[c];
+      if (c < d8) s_q[(c & 7u) * qs + (c >> 3)] = v;
+      else s_q[8u * qs + (c - d8)] = v;
+    }
+    __syncwarp();
+    float p = 0.f;
+    if (lane < 8)
+      for (uint32_t i = 0; i < steps; i++) {
+        const float v = s_q[lane * qs + i];
+        p = __fadd_rn(p, __fmul_rn(v, v));
+      }
+    float q_sumsq = quad_fold8(p, true);
+    for (uint32_t c = d8; c < dim; c++) {
+      const float v = s_q[8u * qs + (c - d8)];
+      q_sumsq = __fadd_rn(q_sumsq, __fmul_rn(v, v));
+    }
+    q_norm = __dsqrt_rn((double)__shfl_sync(0xffffffffu, q_sumsq, 0));
+  } else if (MET == SDB_JACCARD) {
+    mq.u = nbits[r];
+    JKey<T>* s_qb = reinterpret_cast<JKey<T>*>(s_q);
+    for (uint32_t c = lane; c < mq.u; c += 32) s_qb[c] = static_cast<const JKey<T>*>(bits)[(size_t)r * dim + c];
+    __syncwarp();
+  } else {
+    T* s_qt = reinterpret_cast<T*>(s_q);
+    for (uint32_t c = lane; c < dim; c += 32) s_qt[c] = static_cast<const T*>(vecs)[(size_t)r * dim + c];
+    __syncwarp();
+    if (MET == SDB_PEARSON) {
+      mq.mean = mean[r];
+      mq.sx2 = sx2[r];
+    }
+    if (MET == SDB_MINKOWSKI) mq.p = mink_p;
+    if (MET == SDB_COSINE) q_norm = norm[r];
+  }
+}
 
 template <int MET, typename T>
 __device__ __forceinline__ double walk_distance(const HnswParams& P, uint32_t my_row, const float* s_q, double q_norm,
@@ -1019,7 +1071,176 @@ __global__ void __launch_bounds__(HN_WARPS * 32, MINB) hnsw_search_kernel(HnswPa
   }
 }
 
+// Bytes of one warp's staged vector and distance scratch in the kernels that share the walk's distance code.
+static size_t hn_stage_bytes(uint32_t dim, sdb_metric metric, sdb_vector_type vt) {
+  const size_t elem = metric == SDB_JACCARD ? (vt == SDB_VT_F64 || vt == SDB_VT_I64 ? 8 : 4)
+                                            : (vt == SDB_VT_F64 || vt == SDB_VT_I64 ? 8 : vt == SDB_VT_I16 ? 2 : 4);
+  return hn_q_bytes(dim, vt == SDB_VT_F32, metric == SDB_COSINE, elem) + hn_tile_bytes(vt == SDB_VT_F32 && metric == SDB_COSINE);
+}
+// the staged vector and the distance scratch of one warp (hnsw_search_kernel's layout), then `rest`
+template <int MET, typename T>
+__device__ __forceinline__ void hn_warp_layout(uint8_t* base, uint32_t dim, float*& s_q, float (*&tile)[33], uint8_t*& rest) {
+  constexpr bool COSINE = MET == SDB_COSINE && is_f32_v<T>;
+  constexpr size_t ELEM = MET == SDB_JACCARD ? sizeof(JKey<T>) : sizeof(T);
+  s_q = reinterpret_cast<float*>(base);
+  tile = reinterpret_cast<float(*)[33]>(is_f32_v<T> ? s_q + ((hn_q_floats(dim, COSINE) + 3) & ~size_t(3))
+                                                    : reinterpret_cast<float*>(base + hn_q_bytes(dim, false, false, ELEM)));
+  rest = reinterpret_cast<uint8_t*>(tile) + hn_tile_bytes(COSINE);
+}
+
+// ---- exact kNN over the elements in the walk's arithmetic (TestCollection::knn, idx/trees/hnsw/mod.rs:1186-1197) ----
+// For every query q: d = calculate(element, q) for every member element (the walk's argument order and distance code,
+// so a distance equals the one sdb_hnsw_search reports for that pair), and the k smallest in (key, element id) order,
+// the order of KnnResultBuilder.  One warp per query streams the members 32 at a time through walk_distance and keeps
+// a sorted top-k in shared memory.  members: ascending element ids (null: every element); ties then stay in id order,
+// because sorted_insert puts a new entry after its equals and a tie of the k-th entry is not admitted.
+template <int MET, typename T>
+__global__ void __launch_bounds__(HN_WARPS * 32, 1) hnsw_knn_exact_kernel(HnswParams P, const uint32_t* __restrict__ members,
+                                                                       uint64_t n_members, uint32_t per_warp) {
+  extern __shared__ uint8_t smem_raw[];
+  const uint32_t warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const uint32_t k = P.k;
+  float* s_q;
+  float(*tile)[33];
+  uint8_t* rest;
+  hn_warp_layout<MET, T>(smem_raw + (size_t)warp * per_warp, P.dim, s_q, tile, rest);
+  uint64_t* w_key = reinterpret_cast<uint64_t*>(rest);
+  uint32_t* w_id = reinterpret_cast<uint32_t*>(w_key + k + 1);
+  const uint32_t gwarp = blockIdx.x * HN_WARPS + warp, n_warps = gridDim.x * HN_WARPS;
+  for (uint32_t q = gwarp; q < P.nq; q += n_warps) {
+    double q_norm = 0.0;
+    MetricQ mq;
+    stage_vector<MET, T>(P.dim, P.queries, P.q_norm, P.q_mean, P.q_sx2, P.q_bits, P.q_nbits, P.mink_p, q, s_q, q_norm, mq);
+    uint32_t wn = 0;
+    for (uint64_t b0 = 0; b0 < n_members; b0 += 32) {
+      const uint64_t i = b0 + lane;
+      const uint32_t row = i < n_members ? (members ? __ldg(members + i) : (uint32_t)i) : NO_ROW;
+      const double d = walk_distance<MET, T>(P, row, s_q, q_norm, mq, tile);
+      const uint64_t key = dist_key(d);
+      uint32_t m = __ballot_sync(0xffffffffu, row != NO_ROW && (wn < k || key < w_key[k - 1]));
+      while (m) {  // in member order: the admission of a later lane sees the earlier ones
+        const int j = __ffs(m) - 1;
+        m &= m - 1;
+        const uint64_t kj = __shfl_sync(0xffffffffu, key, j);
+        const uint32_t idj = __shfl_sync(0xffffffffu, row, j);
+        if (wn == k) {
+          if (kj >= w_key[k - 1]) continue;
+          wn--;  // the farthest leaves
+        }
+        wn = sorted_insert(w_key, w_id, 0, wn, kj, idj);
+      }
+    }
+    for (uint32_t i = lane; i < wn; i += 32) {
+      P.out_elems[(size_t)q * k + i] = w_id[i];
+      P.out_dist[(size_t)q * k + i] = key_to_double(w_key[i]);
+    }
+    if (lane == 0) P.out_count[q] = wn;
+    __syncwarp();
+  }
+}
+
+// ---- Heuristic::select in the walk's arithmetic (standard variant, heuristic.rs:61-81,201-216), one warp per element.
+// Every distance is walk_distance with one vector staged as the walk stages a query, so each is the distance the walk
+// would compute for the pair, in the reference's argument order:
+//   e_dist, presorted: calculate(candidate, element) -- the distance the candidate list was ranked by (an insertion
+//     search or the exact kNN above, both element-first with the new element as the query);
+//   e_dist, re-sort (build_priority_list, layer.rs:389-405): calculate(element, candidate), the visiting order then by
+//     (key, list position), i.e. FIFO among equal distances;
+//   r_dist = calculate(r, e) for every accepted r (elements.rs:133-140), with e staged.
+// Only JACCARD is asymmetric; its re-sort e_dist swaps the two counts of the same intersection.  e is rejected when
+// e_dist > r_dist for some accepted r; all candidates (other than the element) are taken when there are <= m_max.
+// Shared memory per warp: the staged vector and scratch, then kc f64 e_dist, kc u32 visiting order, m_max u32 picks.
+template <int MET, typename T>
+__global__ void __launch_bounds__(HN_WARPS * 32, 1) hnsw_select_typed_kernel(HnswParams P, const uint32_t* __restrict__ elem_ids,
+                                                                          uint64_t row0, uint64_t n,
+                                                                          const uint64_t* __restrict__ cand,
+                                                                          const uint32_t* __restrict__ cand_cnt, uint32_t kc,
+                                                                          uint32_t m_max, int presorted,
+                                                                          uint32_t* __restrict__ out,
+                                                                          uint32_t* __restrict__ out_cnt, uint32_t per_warp) {
+  extern __shared__ uint8_t smem_raw[];
+  const uint32_t warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  float* s_q;
+  float(*tile)[33];
+  uint8_t* rest;
+  hn_warp_layout<MET, T>(smem_raw + (size_t)warp * per_warp, P.dim, s_q, tile, rest);
+  double* s_ed = reinterpret_cast<double*>(rest);
+  uint32_t* s_ord = reinterpret_cast<uint32_t*>(s_ed + kc);
+  uint32_t* s_acc = s_ord + kc;
+  const uint64_t n_warps = (uint64_t)gridDim.x * HN_WARPS;
+  for (uint64_t i = (uint64_t)blockIdx.x * HN_WARPS + warp; i < n; i += n_warps) {
+    const uint64_t self = elem_ids ? (uint64_t)elem_ids[i] : row0 + i;
+    const uint64_t* cl = cand + i * kc;
+    const uint32_t nc = cand_cnt[i] < kc ? cand_cnt[i] : kc;
+    uint32_t n_real = 0;  // candidates other than the element itself
+    for (uint32_t j = lane; j < nc; j += 32) n_real += cl[j] != self;
+    n_real = __reduce_add_sync(0xffffffffu, n_real);
+    const bool take_all = n_real <= m_max;
+    double q_norm = 0.0;
+    MetricQ mq;
+    if (!(presorted && take_all)) {  // e_dist of every candidate, the element staged
+      stage_vector<MET, T>(P.dim, P.vec, P.norm, P.e_mean, P.e_sx2, P.e_bits, P.e_nbits, P.mink_p, self, s_q, q_norm, mq);
+      for (uint32_t j0 = 0; j0 < nc; j0 += 32) {
+        const uint32_t j = j0 + lane;
+        const uint32_t row = j < nc && cl[j] != self ? (uint32_t)cl[j] : NO_ROW;
+        double d;
+        if constexpr (MET == SDB_JACCARD)
+          d = presorted ? walk_distance<MET, T>(P, row, s_q, q_norm, mq, tile)
+                        : warp_distance_jaccard<T, true>(static_cast<const JKey<T>*>(P.e_bits), P.e_nbits, P.dim, row,
+                                                         reinterpret_cast<const JKey<T>*>(s_q), mq.u, tile);
+        else
+          d = walk_distance<MET, T>(P, row, s_q, q_norm, mq, tile);
+        if (j < nc) s_ed[j] = d;
+      }
+      __syncwarp();
+    }
+    // visiting order: as given, or by (key of e_dist, position); the element itself goes last (it is skipped)
+    if (presorted) {
+      for (uint32_t j = lane; j < nc; j += 32) s_ord[j] = j;
+    } else {
+      for (uint32_t j = lane; j < nc; j += 32) {
+        const bool sj = cl[j] == self;
+        const uint64_t kj = dist_key(s_ed[j]);
+        uint32_t rank = 0;
+        for (uint32_t t = 0; t < nc; t++) {
+          const bool st = cl[t] == self;
+          const uint64_t kt = dist_key(s_ed[t]);
+          rank += st == sj ? (kt < kj || (kt == kj && t < j)) : (uint32_t)sj;
+        }
+        s_ord[rank] = j;
+      }
+    }
+    __syncwarp();
+    uint32_t acc = 0;
+    for (uint32_t jj = 0; jj < nc && acc < m_max; jj++) {
+      const uint32_t j = s_ord[jj];
+      const uint64_t e = cl[j];
+      if (e == self) continue;
+      bool ok = true;
+      if (!take_all) {
+        const double e_dist = s_ed[j];
+        stage_vector<MET, T>(P.dim, P.vec, P.norm, P.e_mean, P.e_sx2, P.e_bits, P.e_nbits, P.mink_p, e, s_q, q_norm, mq);
+        for (uint32_t r0 = 0; r0 < acc && ok; r0 += 32) {
+          const uint32_t row = r0 + lane < acc ? s_acc[r0 + lane] : NO_ROW;
+          const double r_dist = walk_distance<MET, T>(P, row, s_q, q_norm, mq, tile);
+          ok = !__any_sync(0xffffffffu, row != NO_ROW && e_dist > r_dist);  // is_closer: heuristic.rs:209-211
+        }
+      }
+      if (ok) {
+        if (lane == 0) s_acc[acc] = (uint32_t)e;
+        acc++;
+        __syncwarp();
+      }
+    }
+    for (uint32_t a = lane; a < acc; a += 32) out[i * m_max + a] = s_acc[a];
+    if (lane == 0) out_cnt[i] = acc;
+    __syncwarp();
+  }
+}
+
 // ---- construction helper: Heuristic::select over pre-ranked candidates, one warp per element ------------------------
+// The F32 COSINE / EUCLIDEAN GPU builder's selection (fmaf, f32, squared euclidean), kept as it is so that the graphs that
+// builder makes do not change; every other metric and type selects with hnsw_select_typed_kernel above.
 template <bool COSINE>
 __device__ __forceinline__ float warp_pair_dist(const float* a_smem, float a_n2, const float* __restrict__ b, uint32_t dim) {
   const uint32_t lane = threadIdx.x & 31u;
@@ -1321,6 +1542,26 @@ static void vec_state_free(VecState& s, VecSet set, cudaStream_t st) {
   s = VecState();
 }
 
+// the device tables of per-layer CSR pointers (h->rp, h->ci), (re)allocated for h->n_layers; the copy is queued on st
+static sdb_status upload_layer_tables(sdb_hnsw* h, cudaStream_t st) {
+  const uint32_t n_layers = h->n_layers;
+  cudaFree(h->d_rp);
+  cudaFree(h->d_ci);
+  h->d_rp = nullptr;
+  h->d_ci = nullptr;
+  if (cudaMalloc(&h->d_rp, sizeof(void*) * n_layers) != cudaSuccess ||
+      cudaMalloc(&h->d_ci, sizeof(void*) * n_layers) != cudaSuccess) {
+    set_error("hnsw: layer table allocation failed: %s", cudaGetErrorString(cudaGetLastError()));
+    return SDB_ENOMEM;
+  }
+  if (cudaMemcpyAsync(h->d_rp, h->rp.data(), sizeof(void*) * n_layers, cudaMemcpyHostToDevice, st) != cudaSuccess ||
+      cudaMemcpyAsync(h->d_ci, h->ci.data(), sizeof(void*) * n_layers, cudaMemcpyHostToDevice, st) != cudaSuccess) {
+    set_error("hnsw: layer table copy failed: %s", cudaGetErrorString(cudaGetLastError()));
+    return SDB_ECUDA;
+  }
+  return SDB_OK;
+}
+
 // common tail of the loaders: per-layer pointer tables + the elements' metric state
 static sdb_status hnsw_finish(sdb_hnsw* h, sdb_hnsw** out) {
   Ctx* ctx = h->ctx;
@@ -1330,13 +1571,12 @@ static sdb_status hnsw_finish(sdb_hnsw* h, sdb_hnsw** out) {
     sdb_hnsw_destroy(h);
     return rc;
   };
-  const uint32_t n_layers = h->n_layers;
-  if (cudaMalloc(&h->d_rp, sizeof(void*) * n_layers) != cudaSuccess) return fail("layer table", SDB_ENOMEM);
-  if (cudaMalloc(&h->d_ci, sizeof(void*) * n_layers) != cudaSuccess) return fail("layer table", SDB_ENOMEM);
-  if (cudaMemcpyAsync(h->d_rp, h->rp.data(), sizeof(void*) * n_layers, cudaMemcpyHostToDevice, st) != cudaSuccess ||
-      cudaMemcpyAsync(h->d_ci, h->ci.data(), sizeof(void*) * n_layers, cudaMemcpyHostToDevice, st) != cudaSuccess)
-    return fail("layer table copy", SDB_ECUDA);
-  const sdb_status rc = vec_state_make(ctx, VecSet::ELEMENTS, h->metric, h->vt, h->d_vec, h->n, h->dim, h->elems, st);
+  sdb_status rc = upload_layer_tables(h, st);
+  if (rc != SDB_OK) {
+    sdb_hnsw_destroy(h);
+    return rc;
+  }
+  rc = vec_state_make(ctx, VecSet::ELEMENTS, h->metric, h->vt, h->d_vec, h->n, h->dim, h->elems, st);
   if (rc != SDB_OK) {
     sdb_hnsw_destroy(h);
     return rc;
@@ -1344,6 +1584,45 @@ static sdb_status hnsw_finish(sdb_hnsw* h, sdb_hnsw** out) {
   if (cudaStreamSynchronize(st) != cudaSuccess || cudaGetLastError() != cudaSuccess) return fail("finish", SDB_ECUDA);
   *out = h;
   return SDB_OK;
+}
+
+// the element side of HnswParams: vectors, their metric state, the Minkowski order
+static HnswParams element_params(const sdb_hnsw* h) {
+  HnswParams P{};
+  P.vec = h->d_vec;
+  P.norm = h->elems.norm;
+  P.dim = h->dim;
+  P.mink_p = h->minkowski_p;
+  P.e_mean = h->elems.mean;
+  P.e_sx2 = h->elems.sx2;
+  P.e_bits = h->elems.bits;
+  P.e_nbits = h->elems.nbits;
+  return P;
+}
+
+// launches kern (4 warps per block, `per_warp` bytes of shared memory each) with enough blocks for `items` warps, at most
+// as many as are resident at once (the kernels loop)
+template <typename K, typename... A>
+static sdb_status launch_warps(Ctx* ctx, K kern, size_t per_warp, uint64_t items, const char* what, A... args) {
+  per_warp = (per_warp + 15) & ~size_t(15);
+  const size_t smem = per_warp * HN_WARPS;
+  if (smem > 220 * 1024) {
+    set_error("%s: %zu bytes of shared memory per block needed (dimension, k or candidate count too large)", what, smem);
+    return SDB_EUNSUPPORTED;
+  }
+  SDB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  int per_sm = 1;
+  SDB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, HN_WARPS * 32, smem));
+  const uint64_t grid = std::min<uint64_t>((uint64_t)ctx->sm_count * std::max(per_sm, 1), (items + HN_WARPS - 1) / HN_WARPS);
+  kern<<<(unsigned)grid, HN_WARPS * 32, smem, ctx->stream>>>(args..., (uint32_t)per_warp);
+  count_launch(ctx);
+  SDB_CUDA(cudaGetLastError());
+  return SDB_OK;
+}
+
+__global__ void members_max_kernel(const uint32_t* __restrict__ m, uint64_t n, unsigned int* __restrict__ mx) {
+  const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n) atomicMax(mx, m[i]);
 }
 
 extern "C" {
@@ -1409,19 +1688,48 @@ sdb_status sdb_hnsw_load_typed(sdb_ctx* ctx, uint32_t dim, sdb_metric metric, sd
 sdb_status sdb_hnsw_load_device(sdb_ctx* ctx, uint32_t dim, sdb_metric metric, uint64_t n_elems, const float* d_vectors,
                                 uint32_t n_layers, const uint64_t* const* d_row_ptr, const uint32_t* const* d_col_idx,
                                 int64_t entry_point, sdb_hnsw** out) {
+  return sdb_hnsw_load_device_typed(ctx, dim, metric, SDB_VT_F32, n_elems, d_vectors, n_layers, d_row_ptr, d_col_idx,
+                                    entry_point, out);
+}
+
+sdb_status sdb_hnsw_load_device_typed(sdb_ctx* ctx, uint32_t dim, sdb_metric metric, sdb_vector_type vt, uint64_t n_elems,
+                                      const void* d_vectors, uint32_t n_layers, const uint64_t* const* d_row_ptr,
+                                      const uint32_t* const* d_col_idx, int64_t entry_point, sdb_hnsw** out) {
   if ((n_elems && !d_vectors) || !d_row_ptr || !d_col_idx) return SDB_EINVAL;
-  // F32 only: its one caller is the F32 GPU builder
-  SDB_TRY(check_load("sdb_hnsw_load_device", ctx, out, dim, metric, SDB_VT_F32, n_elems, n_layers, entry_point));
+  SDB_TRY(check_load("sdb_hnsw_load_device_typed", ctx, out, dim, metric, (int)vt, n_elems, n_layers, entry_point));
   std::lock_guard<std::mutex> guard(ctx->mu);
   SDB_CUDA(cudaSetDevice(ctx->device));
-  sdb_hnsw* h = new_hnsw(ctx, dim, metric, SDB_VT_F32, n_elems, n_layers, entry_point);
+  sdb_hnsw* h = new_hnsw(ctx, dim, metric, vt, n_elems, n_layers, entry_point);
   h->borrowed = true;  // nothing is copied: the caller keeps vectors and adjacency alive while the handle exists
-  h->d_vec = const_cast<float*>(d_vectors);
+  h->d_vec = const_cast<void*>(d_vectors);
   for (uint32_t l = 0; l < n_layers; l++) {
     h->rp.push_back(const_cast<uint64_t*>(d_row_ptr[l]));
     h->ci.push_back(const_cast<uint32_t*>(d_col_idx[l]));
   }
   return hnsw_finish(h, out);
+}
+
+sdb_status sdb_hnsw_set_layers_device(sdb_hnsw* h, uint32_t n_layers, const uint64_t* const* d_row_ptr,
+                                      const uint32_t* const* d_col_idx, int64_t entry_point) {
+  if (!h || !n_layers || !d_row_ptr || !d_col_idx || entry_point >= (int64_t)h->n) return SDB_EINVAL;
+  if (!h->borrowed) {
+    set_error("sdb_hnsw_set_layers_device: the handle owns its arrays (only a handle of sdb_hnsw_load_device[_typed] can "
+              "swap its adjacency)");
+    return SDB_EINVAL;
+  }
+  std::lock_guard<std::mutex> guard(h->mu);  // searches hold it for their whole run
+  SDB_CUDA(cudaSetDevice(h->ctx->device));
+  h->rp.clear();
+  h->ci.clear();
+  for (uint32_t l = 0; l < n_layers; l++) {
+    h->rp.push_back(const_cast<uint64_t*>(d_row_ptr[l]));
+    h->ci.push_back(const_cast<uint32_t*>(d_col_idx[l]));
+  }
+  h->n_layers = n_layers;
+  h->entry = entry_point;
+  SDB_TRY(upload_layer_tables(h, h->ctx->stream));
+  SDB_CUDA(cudaStreamSynchronize(h->ctx->stream));
+  return SDB_OK;
 }
 
 // native < 0: sdb_hnsw_load_staged, an F32 index: He values of another variant are refused, F32 ones converted; otherwise
@@ -1586,6 +1894,100 @@ sdb_status sdb_hnsw_select_neighbors_ids(sdb_ctx* ctx, const float* d_vectors, u
   if (!d_elem_ids) return SDB_EINVAL;
   return select_neighbors(ctx, d_vectors, dim, metric, 0, d_elem_ids, n, d_cand, d_cand_cnt, kc, m_max, presorted, d_out,
                           d_out_cnt);
+}
+
+sdb_status sdb_hnsw_knn_exact_device(sdb_hnsw* h, const void* d_queries, uint32_t nq, uint32_t k, const uint32_t* d_members,
+                                     uint64_t n_members, uint64_t* d_out_elems, double* d_out_dist, uint32_t* d_out_count) {
+  if (!h || k == 0 || k > 256) return SDB_EINVAL;
+  if (nq && (!d_queries || !d_out_elems || !d_out_dist || !d_out_count)) return SDB_EINVAL;
+  if (!d_members) n_members = h->n;
+  if (n_members > h->n) return SDB_EINVAL;
+  if (nq == 0) return SDB_OK;
+  Ctx* ctx = h->ctx;
+  std::lock_guard<std::mutex> guard(h->mu);
+  SDB_CUDA(cudaSetDevice(ctx->device));
+  cudaStream_t st = ctx->stream;
+  uint32_t* sorted = nullptr;
+  unsigned int* d_max = nullptr;
+  void* d_tmp = nullptr;
+  VecState qs;
+  auto run = [&]() -> sdb_status {
+    if (d_members && n_members) {  // ascending ids: ties are then ranked by id; every id must name an element
+      size_t tmp_bytes = 0;
+      SDB_CUDA(cub::DeviceRadixSort::SortKeys(nullptr, tmp_bytes, d_members, sorted, n_members, 0, 32, st));
+      SDB_CUDA(cudaMallocAsync(&sorted, sizeof(uint32_t) * n_members, st));
+      SDB_CUDA(cudaMallocAsync(&d_tmp, tmp_bytes ? tmp_bytes : 1, st));
+      SDB_CUDA(cudaMallocAsync(&d_max, sizeof(unsigned int), st));
+      SDB_CUDA(cub::DeviceRadixSort::SortKeys(d_tmp, tmp_bytes, d_members, sorted, n_members, 0, 32, st));
+      count_launch(ctx);
+      SDB_CUDA(cudaMemsetAsync(d_max, 0, sizeof(unsigned int), st));
+      members_max_kernel<<<(unsigned)((n_members + 255) / 256), 256, 0, st>>>(sorted, n_members, d_max);
+      count_launch(ctx);
+      unsigned int mx = 0;
+      SDB_CUDA(cudaMemcpyAsync(&mx, d_max, sizeof(mx), cudaMemcpyDeviceToHost, st));
+      SDB_CUDA(cudaStreamSynchronize(st));
+      if (mx >= h->n) {
+        set_error("sdb_hnsw_knn_exact_device: member id %u is not an element (%llu elements)", mx, (unsigned long long)h->n);
+        return SDB_EINVAL;
+      }
+    }
+    SDB_TRY(vec_state_make(ctx, VecSet::BATCH, h->metric, h->vt, d_queries, nq, h->dim, qs, st));
+    HnswParams P = element_params(h);
+    P.queries = d_queries;
+    P.nq = nq;
+    P.k = k;
+    P.out_elems = d_out_elems;
+    P.out_dist = d_out_dist;
+    P.out_count = d_out_count;
+    P.q_mean = qs.mean;
+    P.q_sx2 = qs.sx2;
+    P.q_bits = qs.bits;
+    P.q_nbits = qs.nbits;
+    P.q_norm = qs.norm;
+    const size_t per_warp = hn_stage_bytes(h->dim, h->metric, h->vt) + 12 * ((size_t)k + 1) + 64;
+    const uint32_t* mem = d_members ? sorted : nullptr;
+    return with_vt(h->vt, [&](auto tag) {
+      using T = decltype(tag);
+      return with_metric(h->metric, [&](auto met) {
+        return launch_warps(ctx, hnsw_knn_exact_kernel<decltype(met)::value, T>, per_warp, nq, "sdb_hnsw_knn_exact_device",
+                            P, mem, n_members);
+      });
+    });
+  };
+  sdb_status rc = run();
+  vec_state_free(qs, VecSet::BATCH, st);
+  for (void* p : {(void*)sorted, (void*)d_max, d_tmp})
+    if (p) cudaFreeAsync(p, st);
+  if (cudaStreamSynchronize(st) != cudaSuccess && rc == SDB_OK) {
+    set_error("sdb_hnsw_knn_exact_device: %s", cudaGetErrorString(cudaGetLastError()));
+    rc = SDB_ECUDA;
+  }
+  return rc;
+}
+
+sdb_status sdb_hnsw_select_device(sdb_hnsw* h, const uint32_t* d_elem_ids, uint64_t row0, uint64_t n, const uint64_t* d_cand,
+                                  const uint32_t* d_cand_cnt, uint32_t kc, uint32_t m_max, int presorted, uint32_t* d_out,
+                                  uint32_t* d_out_cnt) {
+  if (!h || !kc || !m_max || (n && (!d_cand || !d_cand_cnt || !d_out || !d_out_cnt))) return SDB_EINVAL;
+  if (!d_elem_ids && row0 + n > h->n) return SDB_EINVAL;
+  if (n == 0) return SDB_OK;
+  Ctx* ctx = h->ctx;
+  std::lock_guard<std::mutex> guard(h->mu);
+  SDB_CUDA(cudaSetDevice(ctx->device));
+  const HnswParams P = element_params(h);
+  const size_t per_warp = hn_stage_bytes(h->dim, h->metric, h->vt) + 12 * (size_t)kc + 4 * (size_t)m_max + 64;
+  const sdb_status rc = with_vt(h->vt, [&](auto tag) {
+    using T = decltype(tag);
+    return with_metric(h->metric, [&](auto met) {
+      return launch_warps(ctx, hnsw_select_typed_kernel<decltype(met)::value, T>, per_warp, n, "sdb_hnsw_select_device", P,
+                          d_elem_ids, row0, n, d_cand, d_cand_cnt, kc, m_max, presorted, d_out, d_out_cnt);
+    });
+  });
+  if (cudaStreamSynchronize(ctx->stream) != cudaSuccess && rc == SDB_OK) {
+    set_error("sdb_hnsw_select_device: %s", cudaGetErrorString(cudaGetLastError()));
+    return SDB_ECUDA;
+  }
+  return rc;
 }
 
 using WalkKernel = void (*)(HnswParams);

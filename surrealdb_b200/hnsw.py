@@ -114,12 +114,18 @@ class HnswIndex:
             L.check(L.lib().sdb_hnsw_set_minkowski_order(self.h, float(minkowski_order)))
 
     @classmethod
-    def from_device(cls, ctx, x_dev, layers_dev, entry_point, metric="EUCLIDEAN", elem_docs=None, minkowski_order=3.0):
-        """wraps device-resident vectors and CSR layers WITHOUT copying them (sdb_hnsw_load_device): x_dev is a torch CUDA
-        float32 (n, dim) tensor, layers_dev = [(row_ptr int64 (n+1), col_idx int32)] layer 0 first.  The tensors must
-        stay alive (they are kept on the object)."""
+    def from_device(cls, ctx, x_dev, layers_dev, entry_point, metric="EUCLIDEAN", elem_docs=None, minkowski_order=3.0,
+                    vector_type="F32"):
+        """wraps device-resident vectors and CSR layers WITHOUT copying them (sdb_hnsw_load_device_typed): x_dev is a torch
+        CUDA (n, dim) tensor of the vector type's dtype (F64 float64, F32 float32, I64 int64, I32 int32, I16 int16),
+        layers_dev = [(row_ptr int64 (n+1), col_idx int32)] layer 0 first.  The tensors must stay alive (they are kept on
+        the object)."""
         self = cls.__new__(cls)
-        self.ctx, self.metric, self.elem_docs, self.vector_type = ctx, metric.upper(), elem_docs, "F32"
+        self.ctx, self.metric, self.elem_docs, self.vector_type = ctx, metric.upper(), elem_docs, vector_type.upper()
+        if self.vector_type not in L.VTYPE:
+            raise L.SdbError(L.SDB_EINVAL, f"unknown vector type {vector_type!r}")
+        if np.dtype(str(x_dev.dtype).replace("torch.", "")) != np.dtype(VT_DTYPE[self.vector_type]):
+            raise L.SdbError(L.SDB_EINVAL, f"{x_dev.dtype} vectors for an index of type {self.vector_type}")
         self.n, self.dim = int(x_dev.shape[0]), int(x_dev.shape[1])
         self.pendings, self.versions = [], None
         self._keep = (x_dev, layers_dev)
@@ -127,8 +133,8 @@ class HnswIndex:
         RP = (C.c_void_p * nl)(*[t[0].data_ptr() for t in layers_dev])
         CI = (C.c_void_p * nl)(*[t[1].data_ptr() for t in layers_dev])
         self.h = C.c_void_p()
-        L.check(L.lib().sdb_hnsw_load_device(ctx.h, self.dim, L.METRIC[self.metric], self.n, C.c_void_p(x_dev.data_ptr()), nl,
-                                             RP, CI, int(entry_point), C.byref(self.h)))
+        L.check(L.lib().sdb_hnsw_load_device_typed(ctx.h, self.dim, L.METRIC[self.metric], L.VTYPE[self.vector_type], self.n,
+                                                   C.c_void_p(x_dev.data_ptr()), nl, RP, CI, int(entry_point), C.byref(self.h)))
         self._set_order(minkowski_order)
         return self
 
