@@ -839,7 +839,7 @@ sdb_status sdb_ctx_create(int device, sdb_ctx** out) {
     SDB_CUDA(cudaStreamCreateWithFlags(&c->cancel_stream, cudaStreamNonBlocking));
   }
   // dynamic shared-memory limits are per device: set them for THIS device now (not behind a process-wide flag)
-  SDB_TRY(screen_tc_init_device());
+  SDB_TRY(screen_tc_init_device(c));
   SDB_TRY(candidates_init_device());
   SDB_TRY(exact_init_device());
   SDB_CUDA(cudaFuncSetAttribute(topk_merge_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));

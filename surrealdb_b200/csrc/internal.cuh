@@ -137,6 +137,7 @@ struct Ctx {
   int* d_cancel = nullptr;
   cudaStream_t cancel_stream = nullptr;
   int prio_high = 0;  // greatest launch priority of the device (cudaDeviceGetStreamPriorityRange)
+  int tc_pair_ctas = 0;  // CTAs of the int8 streaming screen launched as resident 2-CTA clusters (0: no pair launch)
   cudaEvent_t trace_epoch = nullptr;  // SDB_TRACE
   double trace_host0 = 0.0;           // host clock (s) at the epoch
 };
@@ -145,7 +146,7 @@ inline bool ctx_cancelled(const Ctx* ctx) { return ctx->h_cancel && *ctx->h_canc
 // per-device kernel attributes (dynamic shared-memory limits).  cudaFuncSetAttribute is per DEVICE, so these run in
 // sdb_ctx_create after cudaSetDevice -- never behind a process-wide flag (a second context on another GPU of the same
 // process would otherwise launch with the 48 KB default and fail).
-sdb_status screen_tc_init_device();
+sdb_status screen_tc_init_device(Ctx* ctx);
 sdb_status candidates_init_device();
 sdb_status exact_init_device();
 void comm_destroy(Ctx* ctx);  // comm.cu

@@ -18,7 +18,13 @@
 //                                  seen so far is at least that bin's lower edge -- and publishes tau = edge - margin.
 //                                  The consumers re-read tau (ld.cg, L2) at every work item.  One launch therefore covers
 //                                  the whole corpus: no per-pass launches, compactions or host round trips.
+//   warp 10         drain        : (int8 threshold passes) the consumers write their survivors into a shared-memory
+//                                  ring; this warp appends them to the candidate lists and histograms, so the
+//                                  consumers go on to the next item's MMAs instead of waiting on the appends.
 // The producer runs up to STAGES k-blocks ahead, so the loads of item i+1 overlap the epilogue of item i.
+// The int8 streaming launch with an even number of query blocks runs as 2-CTA clusters that share each corpus tile:
+// each CTA's producer multicasts one half of the B tile into both CTAs, and a stage is free once the consumer warps
+// of both CTAs have released it.
 //
 // Replaces, as the *screen*, the distance loop of KnnTopK::execute (exec/operators/knn_topk.rs:185-228);
 // exactness is restored by candidates.cu (f64 re-rank + error-bound proof) and exact.cu.
@@ -41,12 +47,24 @@ constexpr uint32_t B_BYTES = BLOCK_N * BLOCK_K * 2;  // 32 KB
 constexpr uint32_t STAGE_BYTES = A_BYTES + B_BYTES;
 constexpr uint32_t CONS_WARPS = 8;                 // two consumer warpgroups
 constexpr uint32_t PROD_WARP = CONS_WARPS;         // warp 8
-constexpr uint32_t THREADS = (CONS_WARPS + 2) * 32;
+constexpr uint32_t DRAIN_WARP = CONS_WARPS + 2;    // warp 10 (int8 threshold passes only); warp 9 is the refiner
 constexpr uint32_t MAX_MBLOCKS = 16;           // queries per launch <= 2048 (the driver splits larger batches)
 constexpr uint32_t SUBCAP = 16;                // private candidate slots per (query, CTA, column half) and pass
 constexpr uint32_t SMEM_BYTES = STAGES * STAGE_BYTES + 2 * BLOCK_N * 4 + 256 + MAX_MBLOCKS * 256 * 4 + 1024;
 static_assert(BLOCK_N == TILE_ROWS, "screen tile must match the pass schedule tile");
 static_assert(SMEM_BYTES <= 227 * 1024, "screen CTA must fit the shared memory of one SM");
+// The int8 threshold passes (MODE 1, 2) hand their survivors to a drain warp through a ring in shared memory: the
+// consumers only find the survivors, the drain warp appends them (sub-list counter, store or spill, histogram RED),
+// 32 at a time, while the consumers run the next item's MMAs.  The ring lives in the two screening-norm buffers,
+// which these kernels never stage; so the CTA's shared memory, and what it leaves to the tail kernels, is unchanged.
+constexpr uint32_t RING = 128;                     // entries: value, corpus row, (sequence << 16 | query)
+static_assert(3 * RING * 4 <= 2 * BLOCK_N * 4, "the survivor ring must fit the screening-norm buffers");
+static_assert(MAX_MBLOCKS * BLOCK_M <= 0x10000 && RING <= 32 * 1024, "ring tags: 16-bit query and sequence fields");
+template <bool INT8, int MODE>
+constexpr bool has_drain() { return INT8 && (MODE == 1 || MODE == 2); }
+// the other kernels keep 10 warps: an idle 11th warp would take the registers a tail kernel needs beside the screen
+template <bool INT8, int MODE>
+constexpr uint32_t threads() { return (CONS_WARPS + (has_drain<INT8, MODE>() ? 3 : 2)) * 32; }
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 
@@ -80,6 +98,30 @@ __device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* map
       "cp.async.bulk.tensor.2d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];"
       ::"r"(dst), "l"(map), "r"(c0), "r"(c1), "r"(bar)
       : "memory");
+}
+// the same box written to the same shared-memory offset of both CTAs of a 2-CTA cluster, completing on the mbarrier
+// at the same offset in each
+__device__ __forceinline__ void tma_load_2d_pair(uint32_t dst, const CUtensorMap* map, uint32_t c0, uint32_t c1,
+                                                 uint32_t bar) {
+  asm volatile(
+      "cp.async.bulk.tensor.2d.shared::cluster.global.tile.mbarrier::complete_tx::bytes.multicast::cluster"
+      " [%0], [%1, {%2, %3}], [%4], %5;"
+      ::"r"(dst), "l"(map), "r"(c0), "r"(c1), "r"(bar), "h"((uint16_t)0x3)
+      : "memory");
+}
+// arrive on the mbarrier at the same offset in CTA `rank` of the cluster
+__device__ __forceinline__ void mbar_arrive_cta(uint32_t bar, uint32_t rank) {
+  uint32_t remote;
+  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(remote) : "r"(bar), "r"(rank));
+  asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(remote) : "memory");
+}
+__device__ __forceinline__ uint32_t cluster_ctarank() {
+  uint32_t r;
+  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
+  return r;
+}
+__device__ __forceinline__ void cluster_sync() {
+  asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
 }
 
 // ---- wgmma (one warpgroup, M=64 N=256, both operands K-major in shared memory) ---------------------------------------
@@ -158,12 +200,15 @@ __device__ __forceinline__ Acc acc_at_dyn(const Acc (&acc)[128], int i, int t) {
   for (int u = 1; u < 64; u++) v = u == t ? acc_at(acc, i, u) : v;
   return v;
 }
+__device__ __forceinline__ uint32_t ld_volatile(const uint32_t* p) { return *reinterpret_cast<const volatile uint32_t*>(p); }
+__device__ __forceinline__ void st_volatile(uint32_t* p, uint32_t v) { *reinterpret_cast<volatile uint32_t*>(p) = v; }
 
 // The int8 survivor scan of the epilogue is one pass of compares that sets a bit per passing value, then a rolled loop
-// over the set bits with a single copy of append_survivor.  Unrolled over all 64 values of both rows, the append is
-// inlined 128 times (~150 KB of code that every scanning warp walks through); rolled, the streaming kernel is ~8x
-// smaller and twice as fast (DESIGN.md §5).  The bf16 kernels keep the unrolled scan: at their 168 registers the
-// rolled loop spills.
+// over the set bits that writes each survivor into the drain warp's ring (push_survivors); the drain warp runs the
+// single copy of append_survivor.  Unrolled over all 64 values of both rows, the append is inlined 128 times (~150 KB
+// of code that every scanning warp walks through); rolled, the streaming kernel is ~8x smaller and twice as fast
+// (DESIGN.md §5).  The bf16 kernels keep the unrolled scan with the append inlined: at their 168 registers the rolled
+// loop spills, and an 11th warp at 168 registers would leave no room for a tail kernel's block beside the screen.
 
 // one survivor (query q = mb * BLOCK_M + row, corpus column col of the tile): appended to the (query, CTA, column
 // half) private sub-list, spilling to the query's shared list when that is full; streaming mode also counts it in the
@@ -193,6 +238,42 @@ __device__ __forceinline__ void append_survivor(float score, uint32_t q, uint32_
   }
 }
 
+// Warp-collective (every lane of a consumer warp calls it): writes the values of row i that `hits` marks into the
+// drain warp's ring.  One shared atomic reserves the warp's entries; they are written in rounds of at most one entry
+// per lane, round-major, so a round's entries are consecutive.  Entry e reuses the slot of entry e - RING, so a round
+// first waits until the drain has consumed that far.  Every such wait ends.  Take the lowest entry not yet written:
+// its round has either passed its wait already, or begins with that entry.  In the second case every entry below it
+// is written, the drain consumes written entries in order without waiting on anything else, and a round of at most
+// 32 <= RING entries starting there only needs the drain to reach its first entry.  So that entry gets written, and
+// by induction so does every reserved entry.
+__device__ __forceinline__ void push_survivors(const uint32_t (&acc)[128], int i, uint64_t hits, uint32_t q,
+                                               uint32_t row0, uint32_t col_l, uint32_t lane, uint32_t* r_val,
+                                               uint32_t* r_row, uint32_t* r_tag, uint32_t* s_ring_tail,
+                                               const uint32_t* s_ring_head) {
+  const uint32_t total = __reduce_add_sync(0xffffffffu, (uint32_t)__popcll(hits));
+  if (total == 0) return;
+  uint32_t base = 0;
+  if (lane == 0) base = atomicAdd(s_ring_tail, total);
+  base = __shfl_sync(0xffffffffu, base, 0);
+  const uint32_t lt = (1u << lane) - 1;
+  for (uint32_t off = 0; off < total;) {
+    const uint32_t act = __ballot_sync(0xffffffffu, hits != 0);
+    const uint32_t e = base + off + __popc(act & lt);
+    off += __popc(act);
+    while ((int)(base + off - RING - ld_volatile(s_ring_head)) > 0) {
+    }
+    if (hits) {
+      const int t = __ffsll((long long)hits) - 1;
+      hits &= hits - 1;
+      const uint32_t slot = e % RING;
+      r_val[slot] = acc_at_dyn(acc, i, t);
+      r_row[slot] = row0 + fragment_col(t, col_l);
+      __threadfence_block();  // the entry before its tag
+      st_volatile(r_tag + slot, e << 16 | q);
+    }
+  }
+}
+
 // MODE 0: pass 0 -- every score of the pass's tiles goes to a fixed slot of the query's main list (tau = -inf)
 // MODE 1: threshold pass -- survivors of a fixed tau (legacy multi-pass schedule)
 // MODE 2: streaming pass -- tau is re-read at every work item and raised by the refiner warps while the kernel runs
@@ -201,13 +282,13 @@ __device__ __forceinline__ void append_survivor(float score, uint32_t q, uint32_
 //         lower bound of the k-th best score of the corpus: the seed of the streaming pass's thresholds, at the cost
 //         of one round of MMAs and no candidate traffic.
 template <bool COSINE, bool INT8, int MODE>
-__global__ void __launch_bounds__(THREADS, 1)
+__global__ void __launch_bounds__(threads<INT8, MODE>(), 1)
 screen_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b,
                  const float* __restrict__ snorm, uint32_t k_blocks, uint32_t n_mblocks, uint32_t nq,
                  PassDesc pass, float* tau, Cand* __restrict__ cand,
                  uint32_t* __restrict__ cand_cnt, uint32_t cap, Cand* __restrict__ sub, uint32_t* __restrict__ sub_cnt,
                  uint32_t k, const HistParam* __restrict__ hparam, uint32_t* hist, float* __restrict__ probe,
-                 uint32_t probe_stride, uint32_t sleep_min_ns, uint32_t sleep_max_ns) {
+                 uint32_t probe_stride, uint32_t sleep_min_ns, uint32_t sleep_max_ns, uint32_t pair) {
   extern __shared__ uint8_t smem_raw[];
   // SWIZZLE_128B operand tiles need 1024-byte alignment
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -218,38 +299,65 @@ screen_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constan
   uint64_t* full_bar = bars;                      // [STAGES]
   uint64_t* empty_bar = bars + STAGES;            // [STAGES]
   uint32_t* s_done = reinterpret_cast<uint32_t*>(bars + 2 * STAGES);  // consumer warps that have finished
+  uint32_t* s_ring_tail = s_done + 1;  // ring entries reserved by the consumers
+  uint32_t* s_ring_head = s_done + 2;  // ring entries the drain warp has consumed (its slots may be written again)
   uint32_t* s_cnt = reinterpret_cast<uint32_t*>(reinterpret_cast<uint8_t*>(bars) + 256);  // [n_mblocks][2][128]
+  // survivor ring (has_drain only; in the screening-norm buffers): int8 score, corpus row, (sequence << 16 | query)
+  uint32_t* r_val = reinterpret_cast<uint32_t*>(s_snorm);
+  uint32_t* r_row = r_val + RING;
+  uint32_t* r_tag = r_row + RING;
+  constexpr bool DRAIN = has_drain<INT8, MODE>();
 
   const uint32_t warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const uint32_t n_items = pass.count * n_mblocks;
+  // CTA pairs (int8 streaming launch as 2-CTA clusters, even n_mblocks): both CTAs of pair p take the same corpus
+  // tiles, CTA `rank` with query block 2 m + rank, and each loads one 128-row half of the B tile into both CTAs, so a
+  // work item pulls 192 KB instead of 288 KB from L2.  Work item w then numbers (tile, m) of the pair.
+  const bool PAIR = INT8 && MODE == 2 && pair != 0;
+  const uint32_t rank = PAIR ? cluster_ctarank() : 0;
+  const uint32_t n_mb = PAIR ? n_mblocks / 2 : n_mblocks;  // query blocks (pairs of them) per corpus tile
+  const uint32_t w_first = PAIR ? blockIdx.x / 2 : blockIdx.x, w_step = PAIR ? gridDim.x / 2 : gridDim.x;
+  const uint32_t n_items = pass.count * n_mb;
 
+  if (DRAIN) {
+    // no sequence number matches 0xFFFF before the slot is first written (sequence s lands in slot s % RING)
+    for (uint32_t i = threadIdx.x; i < RING; i += blockDim.x) r_tag[i] = 0xFFFF0000u;
+  }
   if (threadIdx.x == 0) {
+    *s_ring_tail = 0;
+    *s_ring_head = 0;
     asm volatile("prefetch.tensormap [%0];" ::"l"(&map_a) : "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(&map_b) : "memory");
     for (uint32_t s = 0; s < STAGES; s++) {
       mbar_init(smem_u32(&full_bar[s]), 1);
-      mbar_init(smem_u32(&empty_bar[s]), CONS_WARPS);  // one arrive per consumer warp
+      mbar_init(smem_u32(&empty_bar[s]), PAIR ? 2 * CONS_WARPS : CONS_WARPS);  // one arrive per consumer warp (of both CTAs)
     }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     *s_done = 0;
   }
   for (uint32_t i = threadIdx.x; i < n_mblocks * 256; i += blockDim.x) s_cnt[i] = 0;
   __syncthreads();
+  if (PAIR) cluster_sync();  // the peer's barriers are initialised before anything arrives on them or fills them
 
   if (warp == PROD_WARP) {
     // ===================== TMA producer =====================
     if (lane == 0) {
       uint32_t it = 0;
-      for (uint32_t w = blockIdx.x; w < n_items; w += gridDim.x) {
-        const uint32_t tile = pass_tile(pass, w / n_mblocks);
-        const uint32_t mb = item_mb(w, n_mblocks);
+      for (uint32_t w = w_first; w < n_items; w += w_step) {
+        const uint32_t tile = pass_tile(pass, w / n_mb);
+        const uint32_t mb = PAIR ? 2 * item_mb(w, n_mb) + rank : item_mb(w, n_mb);
         for (uint32_t kb = 0; kb < k_blocks; kb++, it++) {
           const uint32_t s = it % STAGES, ph = (it / STAGES) & 1;
+          // (pair: the stage is free in both CTAs -- the barrier counts the consumer warps of both)
           mbar_wait(smem_u32(&empty_bar[s]), ph ^ 1);
           const uint32_t fb = smem_u32(&full_bar[s]);
-          mbar_expect_tx(fb, STAGE_BYTES);
-          tma_load_2d(smem_u32(smem_a + s * A_BYTES), &map_a, kb * (INT8 ? 2 * BLOCK_K : BLOCK_K), mb * BLOCK_M, fb);
-          tma_load_2d(smem_u32(smem_b + s * B_BYTES), &map_b, kb * (INT8 ? 2 * BLOCK_K : BLOCK_K), tile * BLOCK_N, fb);
+          const uint32_t kc = kb * (INT8 ? 2 * BLOCK_K : BLOCK_K);
+          mbar_expect_tx(fb, STAGE_BYTES);  // (pair: own A, own B half, the peer's B half)
+          tma_load_2d(smem_u32(smem_a + s * A_BYTES), &map_a, kc, mb * BLOCK_M, fb);
+          if (PAIR)
+            tma_load_2d_pair(smem_u32(smem_b + s * B_BYTES + rank * (B_BYTES / 2)), &map_b, kc,
+                             tile * BLOCK_N + rank * (BLOCK_N / 2), fb);
+          else
+            tma_load_2d(smem_u32(smem_b + s * B_BYTES), &map_b, kc, tile * BLOCK_N, fb);
         }
       }
     }
@@ -264,10 +372,17 @@ screen_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constan
     using Acc = typename std::conditional<INT8, uint32_t, float>::type;
     Acc acc[128];
     uint32_t it = 0, j = 0;
-    for (uint32_t w = blockIdx.x; w < n_items; w += gridDim.x, j++) {
-      const uint32_t tidx = w / n_mblocks;
+    // a stage is released to the producer of this CTA and, in a pair, to the peer's, which fills half of it
+    auto release = [&](uint32_t s) {
+      if (lane == 0) {
+        mbar_arrive(smem_u32(&empty_bar[s]));
+        if (PAIR) mbar_arrive_cta(smem_u32(&empty_bar[s]), rank ^ 1);
+      }
+    };
+    for (uint32_t w = w_first; w < n_items; w += w_step, j++) {
+      const uint32_t tidx = w / n_mb;
       const uint32_t tile = pass_tile(pass, tidx);
-      const uint32_t mb = item_mb(w, n_mblocks);
+      const uint32_t mb = PAIR ? 2 * item_mb(w, n_mb) + rank : item_mb(w, n_mb);
       const uint32_t row0 = tile * BLOCK_N;
       // thresholds of this thread's two queries (L2: sees the refiners' updates); the loads complete under the MMAs
       float my_tau[2];
@@ -309,12 +424,12 @@ screen_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constan
         acc_fence(acc);
         if (kb > 0) {
           wgmma_wait<1>();  // the previous k-block's MMAs have read their stage
-          if (lane == 0) mbar_arrive(smem_u32(&empty_bar[(it - 1) % STAGES]));
+          release((it - 1) % STAGES);
         }
       }
       wgmma_wait<0>();
       acc_fence(acc);
-      if (lane == 0) mbar_arrive(smem_u32(&empty_bar[(it - 1) % STAGES]));
+      release((it - 1) % STAGES);
 
       // ---- epilogue straight from the registers ----
       if constexpr (!INT8) {
@@ -384,22 +499,14 @@ screen_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constan
             int m = (int)0x80000000;
 #pragma unroll
             for (int jj = 0; jj < 32; jj++) m = max(m, max((int)acc[4 * jj + 2 * i], (int)acc[4 * jj + 2 * i + 1]));
-            if (m >= tau_i) {
+            if (__any_sync(0xffffffffu, m >= tau_i)) {
               uint64_t hits = 0;
+              if (m >= tau_i) {
 #pragma unroll
-              for (int t = 0; t < 64; t++)
-                if ((int)acc_at(acc, i, t) >= tau_i) hits |= 1ull << t;
-              while (hits) {
-                const int t = __ffsll((long long)hits) - 1;
-                hits &= hits - 1;
-                const int v = (int)acc_at_dyn(acc, i, t);
-                const uint32_t col = fragment_col(t, col_l);
-                // invalid rows (skipped / special / padding) are all-zero in the int8 copy and score exactly 0:
-                // only a zero score needs the look-up of the row's screening norm
-                if (v != 0 || __ldg(snorm + row0 + col) == __ldg(snorm + row0 + col))
-                  append_survivor<MODE>(__int2float_rn(v), q, row, col, row0, my_hp[i], s_cnt_mb, cand, cand_cnt,
-                                        cap, sub, hist);
+                for (int t = 0; t < 64; t++)
+                  if ((int)acc_at(acc, i, t) >= tau_i) hits |= 1ull << t;
               }
+              push_survivors(acc, i, hits, q, row0, col_l, lane, r_val, r_row, r_tag, s_ring_tail, s_ring_head);
             }
           } else {
             float m = __int_as_float(0xff800000);
@@ -421,9 +528,16 @@ screen_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constan
         }
       }
     }
+    if (DRAIN) {
+      // this warp's ring entries are written; once all consumer warps are done the drain warp empties the ring
+      __syncwarp();
+      __threadfence_block();
+      if (lane == 0) atomicAdd(s_done, 1u);
+    }
     // publish the private append counters: slot (CTA, column half) of every query
     if (MODE == 1 || MODE == 2) {
-      asm volatile("bar.sync 1, 256;" ::: "memory");
+      if (DRAIN) asm volatile("bar.sync 2, 288;" ::: "memory");  // with the drain warp: every survivor is appended
+      else asm volatile("bar.sync 1, 256;" ::: "memory");
       const uint32_t n_slots = gridDim.x * 2;
       const uint32_t half = ct / BLOCK_M, row = ct % BLOCK_M;
       for (uint32_t mb = 0; mb < n_mblocks; mb++) {
@@ -432,7 +546,47 @@ screen_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constan
       }
     }
     __syncwarp();
-    if (lane == 0) atomicAdd(s_done, 1u);
+    if (!DRAIN && lane == 0) atomicAdd(s_done, 1u);
+  } else if (warp == DRAIN_WARP) {
+    // ===================== drain (int8 threshold passes): append the survivors of the ring, 32 at a time ==========
+    if (DRAIN) {
+      uint32_t head = 0;  // entries consumed
+      for (;;) {
+        const uint32_t e = head + lane, slot = e % RING;
+        const uint32_t tag = ld_volatile(r_tag + slot);
+        const uint32_t ready = __ballot_sync(0xffffffffu, (tag >> 16) == (e & 0xFFFFu));
+        const uint32_t n = ready == 0xffffffffu ? 32 : __ffs(~ready) - 1;  // consecutive written entries
+        if (n == 0) {
+          // finished: every consumer warp is done (its entries are reserved and written) and all are consumed
+          uint32_t fin = 0;
+          if (lane == 0 && ld_volatile(s_done) == CONS_WARPS) {
+            __threadfence_block();
+            fin = ld_volatile(s_ring_tail) == head;
+          }
+          if (__shfl_sync(0xffffffffu, fin, 0)) break;
+          __nanosleep(32);  // leave the issue slots to the consumers of this SM sub-partition
+          continue;
+        }
+        __threadfence_block();  // the entries after their tags
+        if (lane < n) {
+          const int v = (int)r_val[slot];
+          const uint32_t grow = r_row[slot], q = tag & 0xFFFFu;
+          const uint32_t col = grow % BLOCK_N, row = q % BLOCK_M;
+          // invalid rows (skipped / special / padding) are all-zero in the int8 copy and score exactly 0: only a
+          // zero score needs the look-up of the row's screening norm
+          if (v != 0 || __ldg(snorm + grow) == __ldg(snorm + grow)) {
+            const float2 hpv = MODE == 2 ? __ldg(reinterpret_cast<const float2*>(hparam + q)) : make_float2(0.f, 0.f);
+            append_survivor<MODE>(__int2float_rn(v), q, row, col, grow - col, hpv, s_cnt + q / BLOCK_M * 256, cand,
+                                  cand_cnt, cap, sub, hist);
+          }
+        }
+        __syncwarp();
+        __threadfence_block();  // the entries are read before their slots are handed back
+        head += n;
+        if (lane == 0) st_volatile(s_ring_head, head);
+      }
+      asm volatile("bar.sync 2, 288;" ::: "memory");
+    }
   } else {
     // ===================== refiner (streaming mode): raise the thresholds of the queries this CTA owns ==========
     if (MODE == 2) {
@@ -498,6 +652,7 @@ screen_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constan
     }
   }
   __syncthreads();
+  if (PAIR) cluster_sync();  // the peer's last remote arrivals on this CTA's barriers have landed
 }
 }  // namespace tc
 
@@ -542,13 +697,29 @@ static sdb_status make_map(Ctx* ctx, CUtensorMap* map, const void* base, uint64_
 
 bool screen_tc_available() { return true; }
 
-sdb_status screen_tc_init_device() {
+sdb_status screen_tc_init_device(Ctx* ctx) {
 #define SET_SMEM(COS, I8, MODE) \
   SDB_CUDA(cudaFuncSetAttribute(tc::screen_tc_kernel<COS, I8, MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tc::SMEM_BYTES))
   SET_SMEM(true, false, 0); SET_SMEM(true, false, 1); SET_SMEM(true, false, 2); SET_SMEM(true, false, 3);
   SET_SMEM(false, false, 0); SET_SMEM(false, false, 1); SET_SMEM(false, false, 2); SET_SMEM(false, false, 3);
   SET_SMEM(true, true, 0); SET_SMEM(true, true, 1); SET_SMEM(true, true, 2); SET_SMEM(true, true, 3);
 #undef SET_SMEM
+  // how many 2-CTA clusters of the int8 streaming screen are resident at once (pairs must share a GPC, so this can be
+  // fewer than half the SMs): the pair launch is persistent only if its grid is all resident
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = dim3((uint32_t)ctx->sm_count & ~1u);
+  cfg.blockDim = dim3(tc::threads<true, 2>());
+  cfg.dynamicSmemBytes = tc::SMEM_BYTES;
+  cudaLaunchAttribute attr[1];
+  attr[0].id = cudaLaunchAttributeClusterDimension;
+  attr[0].val.clusterDim.x = 2;
+  attr[0].val.clusterDim.y = 1;
+  attr[0].val.clusterDim.z = 1;
+  cfg.attrs = attr;
+  cfg.numAttrs = 1;
+  int clusters = 0;
+  SDB_CUDA(cudaOccupancyMaxActiveClusters(&clusters, tc::screen_tc_kernel<true, true, 2>, &cfg));
+  ctx->tc_pair_ctas = 2 * clusters;
   return SDB_OK;
 }
 
@@ -567,18 +738,30 @@ sdb_status screen_tc_pass(Corpus* c, uint32_t nq, uint32_t k, const PassDesc& p,
   if (const char* e = getenv("SDB_REFINE_SLEEP_MAX")) sleep_max = (uint32_t)atoi(e);
   if (sleep_min < 32) sleep_min = 32;
   if (sleep_max < sleep_min) sleep_max = sleep_min;
-  CUtensorMap map_b;
-  if (int8) SDB_TRY(make_map(ctx, &map_b, c->d_i8, n_pad, c->dim_pad8, tc::BLOCK_N, true, true));
-  else SDB_TRY(make_map(ctx, &map_b, c->d_bf16, n_pad, c->dim_pad, tc::BLOCK_N, true));
   const uint32_t k_blocks = int8 ? c->dim_pad8 / (2 * tc::BLOCK_K) : c->dim_pad / tc::BLOCK_K;
   // every launch uses the same grid so that the (CTA, half) slot numbering of the private sub-lists is stable
   const uint32_t chunk_q = tc::MAX_MBLOCKS * tc::BLOCK_M;
+  const uint32_t nq0 = nq < chunk_q ? nq : chunk_q;
+  const uint32_t mb0 = (nq0 + tc::BLOCK_M - 1) / tc::BLOCK_M;
+  const uint32_t mb_last = (nq - (nq - 1) / chunk_q * chunk_q + tc::BLOCK_M - 1) / tc::BLOCK_M;
   uint32_t grid = (uint32_t)ctx->sm_count;
   {
-    const uint32_t nq0 = nq < chunk_q ? nq : chunk_q;
-    const uint64_t items0 = (uint64_t)p.count * ((nq0 + tc::BLOCK_M - 1) / tc::BLOCK_M);
+    const uint64_t items0 = (uint64_t)p.count * mb0;
     if (grid > items0) grid = (uint32_t)items0;
   }
+  // the int8 streaming launch runs as CTA pairs sharing each corpus tile when every chunk has an even number of
+  // query blocks; its grid is the resident pairs
+  uint32_t pair = 0;
+  if (int8 && mode == 2 && mb0 % 2 == 0 && mb_last % 2 == 0) {
+    const uint32_t g2 = (grid < (uint32_t)ctx->tc_pair_ctas ? grid : (uint32_t)ctx->tc_pair_ctas) & ~1u;
+    if (g2 >= 2) {
+      grid = g2;
+      pair = 1;
+    }
+  }
+  CUtensorMap map_b;  // (pair: each CTA loads a 128-row half of the tile)
+  if (int8) SDB_TRY(make_map(ctx, &map_b, c->d_i8, n_pad, c->dim_pad8, pair ? tc::BLOCK_N / 2 : tc::BLOCK_N, true, true));
+  else SDB_TRY(make_map(ctx, &map_b, c->d_bf16, n_pad, c->dim_pad, tc::BLOCK_N, true));
   if (mode == 3 && p.count * 8 > PROBE_STRIDE) {
     set_error("screen_tc_pass: probe of %u tiles exceeds the probe buffer", p.count);
     return SDB_EINVAL;
@@ -604,21 +787,27 @@ sdb_status screen_tc_pass(Corpus* c, uint32_t nq, uint32_t k, const PassDesc& p,
     // instead of waiting behind two 13 KB selection blocks per SM
     cudaLaunchConfig_t cfg = {};
     cfg.gridDim = dim3(grid);
-    cfg.blockDim = dim3(tc::THREADS);
     cfg.dynamicSmemBytes = tc::SMEM_BYTES;
     cfg.stream = st;
-    cudaLaunchAttribute attr[1];
+    cudaLaunchAttribute attr[2];
     attr[0].id = cudaLaunchAttributePriority;
     attr[0].val.priority = ctx->prio_high;
+    attr[1].id = cudaLaunchAttributeClusterDimension;
+    attr[1].val.clusterDim.x = pair ? 2 : 1;
+    attr[1].val.clusterDim.y = 1;
+    attr[1].val.clusterDim.z = 1;
     cfg.attrs = attr;
-    cfg.numAttrs = 1;
+    cfg.numAttrs = pair ? 2 : 1;
     float* probe_ptr = c->d_probe + (size_t)q0 * PROBE_STRIDE;
     const uint32_t probe_stride = PROBE_STRIDE, cap_arg = c->sc_cap;
     const float* snorm_arg = c->d_snorm;
 #define LAUNCH_TC1(COS, I8, MODE)                                                                                    \
-  SDB_CUDA(cudaLaunchKernelEx(&cfg, tc::screen_tc_kernel<COS, I8, MODE>, map_a, map_b, snorm_arg, k_blocks, n_mblocks, \
-                              nqc, p, tau, cand, ccnt, cap_arg, sub, scnt, k, hp, hist, probe_ptr, probe_stride,       \
-                              sleep_min, sleep_max))
+  do {                                                                                                               \
+    cfg.blockDim = dim3(tc::threads<I8, MODE>());                                                                    \
+    SDB_CUDA(cudaLaunchKernelEx(&cfg, tc::screen_tc_kernel<COS, I8, MODE>, map_a, map_b, snorm_arg, k_blocks,        \
+                                n_mblocks, nqc, p, tau, cand, ccnt, cap_arg, sub, scnt, k, hp, hist, probe_ptr,      \
+                                probe_stride, sleep_min, sleep_max, pair));                                          \
+  } while (0)
 #define LAUNCH_TC(COS, I8)                   \
   do {                                       \
     if (mode == 0) LAUNCH_TC1(COS, I8, 0);   \
