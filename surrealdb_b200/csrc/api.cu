@@ -954,7 +954,7 @@ void sdb_corpus_destroy(sdb_corpus* c) {
                   c->d_hparam, c->d_hist, c->d_qbferr, c->d_stat, c->d_probe, c->d_margin2, c->d_beps2, c->d_tau2, c->d_sub, c->d_sub_cnt, c->d_rows, c->d_mag, c->d_snorm,
                   c->d_bf16, c->d_skip, c->d_removed, c->d_special, c->d_q64, c->d_q32, c->d_qbf16, c->d_qmag, c->d_qflags,
                   c->d_tau, c->d_cand, c->d_cand_cnt, c->d_flags, c->d_rr_key, c->d_rr_dist, c->d_rr_row, c->d_ex_key,
-                  c->d_sel, c->d_fb_q, c->d_fb_qmag, c->d_fb_qflags, c->d_block, c->d_gather, c->d_rp_q, c->d_rp_rows,
+                  c->d_ex_val, c->d_sel, c->d_fb_q, c->d_fb_qmag, c->d_fb_qflags, c->d_block, c->d_gather, c->d_rp_q, c->d_rp_rows,
                   c->d_rp_dist, c->d_rp_cnt};
   for (void* p : ptrs) cudaFree(p);
   for (Ticket& t : c->tickets) {

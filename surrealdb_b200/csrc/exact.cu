@@ -22,7 +22,7 @@ __global__ void __launch_bounds__(WARPS * 32) exact_keys_kernel(const T* __restr
                                                                 const double* __restrict__ qmag_p,
                                                                 const uint32_t* __restrict__ qflags_p,
                                                                 uint64_t* __restrict__ keys,
-                                                                double* __restrict__ vals /* non-null: projection */,
+                                                                double* __restrict__ vals /* non-null: every row's value */,
                                                                 double mink_p) {
   __shared__ T tile[WARPS][32][33];
   __shared__ double s_q[EX_QCHUNK];
@@ -318,9 +318,11 @@ __global__ void __launch_bounds__(256) sel_gather_kernel(const uint64_t* __restr
   }
 }
 
-// sort the k_eff gathered pairs and write the query's output row (single block)
+// sort the k_eff gathered pairs and write the query's output row (single block).  The distance is the row's computed
+// value, not the key inverted: dist_key maps -0.0 to 0.0 (they tie), and the reference returns the -0.0 it computed.
 __global__ void __launch_bounds__(1024) sel_emit_kernel(const SelState* st, const uint64_t* __restrict__ g_key,
-                                                        const uint32_t* __restrict__ g_row, uint32_t k,
+                                                        const uint32_t* __restrict__ g_row,
+                                                        const double* __restrict__ vals, uint32_t k,
                                                         uint64_t row_base, uint64_t* __restrict__ out_rows,
                                                         double* __restrict__ out_dist, uint32_t* __restrict__ out_count) {
   extern __shared__ uint64_t s_mem[];
@@ -351,10 +353,8 @@ __global__ void __launch_bounds__(1024) sel_emit_kernel(const SelState* st, cons
       __syncthreads();
     }
   for (uint32_t i = threadIdx.x; i < n; i += blockDim.x) {
-    const uint64_t key = s_key[i];
-    const uint64_t bits = (key >> 63) ? (key & 0x7fffffffffffffffull) : ~key;  // invert dist_key
     out_rows[i] = row_base + s_row[i];
-    out_dist[i] = __longlong_as_double((long long)bits);
+    out_dist[i] = vals[s_row[i]];
   }
   if (threadIdx.x == 0) *out_count = n;
 }
@@ -371,11 +371,14 @@ sdb_status exact_query(Corpus* c, const double* d_q64, const double* d_qmag, con
   Ctx* ctx = c->ctx;
   if (c->ex_cap < c->n || !c->d_ex_key) {
     cudaFree(c->d_ex_key);
+    cudaFree(c->d_ex_val);
     cudaFree(c->d_sel);
     c->d_ex_key = nullptr;
+    c->d_ex_val = nullptr;
     c->d_sel = nullptr;
     const uint64_t cap = c->cap > c->n ? c->cap : c->n;
     SDB_CUDA(cudaMalloc(&c->d_ex_key, sizeof(uint64_t) * (cap ? cap : 1)));
+    SDB_CUDA(cudaMalloc(&c->d_ex_val, sizeof(double) * (cap ? cap : 1)));
     // SelState + gather buffers (key u64[4096], row u32[4096])
     SDB_CUDA(cudaMalloc(&c->d_sel, sizeof(SelState) + 4096 * 12 + 64));
     c->ex_cap = cap;
@@ -389,16 +392,16 @@ sdb_status exact_query(Corpus* c, const double* d_q64, const double* d_qmag, con
   uint32_t* g_row = reinterpret_cast<uint32_t*>(g_key + 4096);
   const uint64_t n = c->n;
   if (n && c->metric == SDB_JACCARD) {
-    SDB_TRY(jaccard_launch(c, d_q64, c->d_ex_key, nullptr, st));
+    SDB_TRY(jaccard_launch(c, d_q64, c->d_ex_key, c->d_ex_val, st));
   } else if (n) {
     const int grid = ctx->sm_count * 8;
     if (c->dtype == SDB_F32)
       exact_keys_kernel<float, 4><<<grid, 128, 0, st>>>((const float*)c->d_rows, c->dim, n, (int)c->metric, c->d_mag,
-                                                        c->d_skip, d_q64, d_qmag, d_qflags, c->d_ex_key, nullptr, c->minkowski_p);
+                                                        c->d_skip, d_q64, d_qmag, d_qflags, c->d_ex_key, c->d_ex_val, c->minkowski_p);
     else
       exact_keys_kernel<double, 4><<<grid, 128, 0, st>>>((const double*)c->d_rows, c->dim, n, (int)c->metric,
                                                          c->d_mag, c->d_skip, d_q64, d_qmag, d_qflags, c->d_ex_key,
-                                                         nullptr, c->minkowski_p);
+                                                         c->d_ex_val, c->minkowski_p);
     count_launch(ctx);
   }
   sel_init_kernel<<<1, 256, 0, st>>>(sel, k);
@@ -412,8 +415,8 @@ sdb_status exact_query(Corpus* c, const double* d_q64, const double* d_qmag, con
   sel_gather_kernel<<<hgrid, 256, 0, st>>>(c->d_ex_key, n, sel, g_key, g_row);
   uint32_t p2 = 1;
   while (p2 < k) p2 <<= 1;
-  sel_emit_kernel<<<1, 1024, sizeof(uint64_t) * 2 * p2, st>>>(sel, g_key, g_row, k, row_base, d_out_rows, d_out_dist,
-                                                             d_out_count);
+  sel_emit_kernel<<<1, 1024, sizeof(uint64_t) * 2 * p2, st>>>(sel, g_key, g_row, c->d_ex_val, k, row_base, d_out_rows,
+                                                             d_out_dist, d_out_count);
   count_launch(ctx, 2);
   SDB_CUDA(cudaGetLastError());
   return SDB_OK;

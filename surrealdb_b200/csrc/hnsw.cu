@@ -60,6 +60,17 @@ struct Hnsw {
 
 constexpr int HN_WARPS = 4;
 
+// The queues' order (FloatKey, idx/trees/knn.rs:129-160): f64::total_cmp, so -0.0 sorts before 0.0.  Unlike the
+// brute-force path's dist_key (Number::cmp, where -0.0 equals 0.0) this key is one-to-one, and key_to_double gives back
+// the distance itself, sign of zero included.
+__device__ __forceinline__ uint64_t walk_key(double d) {
+  const uint64_t b = f64_bits(d);
+  return (b >> 63) ? ~b : (b | 0x8000000000000000ull);
+}
+// the key with -0.0 and 0.0 made equal, where the reference compares the two distances as f64
+__device__ __forceinline__ uint64_t zero_tie(uint64_t key) {
+  return key == 0x7fffffffffffffffull ? 0x8000000000000000ull : key;  // walk_key(-0.0) -> walk_key(0.0)
+}
 __device__ __forceinline__ double key_to_double(uint64_t key) {
   const uint64_t b = (key >> 63) ? (key & 0x7fffffffffffffffull) : ~key;
   return __longlong_as_double((long long)b);
@@ -961,10 +972,10 @@ __global__ void __launch_bounds__(HN_WARPS * 32, MINB) hnsw_search_kernel(HnswPa
         }
         // search_single_with_filter (layer.rs:111-149): w starts with ep only if one of its documents is truthy
         const uint8_t* truthy = layer == 0 ? P.truthy : nullptr;
-        cn = sorted_insert(c_key, c_id, head, cn, dist_key(ep_d), ep);
+        cn = sorted_insert(c_key, c_id, head, cn, walk_key(ep_d), ep);
         double fd = 1.7976931348623157e308;  // w.peek_last_dist().unwrap_or(f64::MAX)
         if (!truthy || truthy[ep]) {
-          wn = sorted_insert(w_key, w_id, 0, wn, dist_key(ep_d), ep);
+          wn = sorted_insert(w_key, w_id, 0, wn, walk_key(ep_d), ep);
           fd = ep_d;
         }
         while (head < cn) {
@@ -1012,7 +1023,7 @@ __global__ void __launch_bounds__(HN_WARPS * 32, MINB) hnsw_search_kernel(HnswPa
               const double di = __shfl_sync(0xffffffffu, d, i);
               const uint32_t idi = __shfl_sync(0xffffffffu, nb, i);
               if (di < fd || wn < ef) {
-                const uint64_t key = dist_key(di);
+                const uint64_t key = walk_key(di);
                 if (cn >= ccap) {  // slide the live window down (or, if truly full, drop the farthest tie)
                   if (head > 0) {
                     for (uint32_t lo = head; lo < cn; lo += 32) {
@@ -1039,8 +1050,9 @@ __global__ void __launch_bounds__(HN_WARPS * 32, MINB) hnsw_search_kernel(HnswPa
                   fd = key_to_double(w_key[wn - 1]);
                 }
                 if (wn == ef) {  // candidates beyond f can never be expanded any more
-                  const uint64_t fkey = w_key[wn - 1];
-                  while (cn > head && c_key[cn - 1] > fkey) cn--;
+                  // (cq_dist > fq_dist is an f64 comparison: a 0.0 candidate is not beyond a -0.0 f)
+                  const uint64_t fkey = zero_tie(w_key[wn - 1]);
+                  while (cn > head && zero_tie(c_key[cn - 1]) > fkey) cn--;
                 }
               }
             }
@@ -1116,7 +1128,7 @@ __global__ void __launch_bounds__(HN_WARPS * 32, 1) hnsw_knn_exact_kernel(HnswPa
       const uint64_t i = b0 + lane;
       const uint32_t row = i < n_members ? (members ? __ldg(members + i) : (uint32_t)i) : NO_ROW;
       const double d = walk_distance<MET, T>(P, row, s_q, q_norm, mq, tile);
-      const uint64_t key = dist_key(d);
+      const uint64_t key = walk_key(d);
       uint32_t m = __ballot_sync(0xffffffffu, row != NO_ROW && (wn < k || key < w_key[k - 1]));
       while (m) {  // in member order: the admission of a later lane sees the earlier ones
         const int j = __ffs(m) - 1;
@@ -1200,11 +1212,11 @@ __global__ void __launch_bounds__(HN_WARPS * 32, 1) hnsw_select_typed_kernel(Hns
     } else {
       for (uint32_t j = lane; j < nc; j += 32) {
         const bool sj = cl[j] == self;
-        const uint64_t kj = dist_key(s_ed[j]);
+        const uint64_t kj = walk_key(s_ed[j]);
         uint32_t rank = 0;
         for (uint32_t t = 0; t < nc; t++) {
           const bool st = cl[t] == self;
-          const uint64_t kt = dist_key(s_ed[t]);
+          const uint64_t kt = walk_key(s_ed[t]);
           rank += st == sj ? (kt < kj || (kt == kj && t < j)) : (uint32_t)sj;
         }
         s_ord[rank] = j;

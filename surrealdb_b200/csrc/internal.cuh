@@ -286,6 +286,7 @@ struct Corpus : Scratch {
   float max_norm = 0.f;
   // exact path scratch
   uint64_t* d_ex_key = nullptr;  // N keys
+  double* d_ex_val = nullptr;    // N distances (the key maps -0.0 to 0.0; the result returns the value itself)
   uint32_t* d_sel = nullptr;     // radix-select state
   uint64_t ex_cap = 0;
   double* d_fb_q = nullptr;      // fallback query scratch (one query: f64 copy, |q|, flags)

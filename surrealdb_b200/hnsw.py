@@ -61,6 +61,12 @@ def to_vector_type(values, vector_type):
     return np.ascontiguousarray(t.astype(dt))
 
 
+def _float_key(d):
+    """FloatKey's total_cmp order for a non-NaN distance: Python's float comparison ties -0.0 with 0.0, FloatKey puts
+    -0.0 first"""
+    return d, 0 if d == 0 and np.signbit(d) else 1
+
+
 class KnnResultBuilder:
     """idx/trees/knn.rs:363-437: a BTreeSet<(FloatKey(dist), VectorId)> capped at knn entries."""
 
@@ -72,9 +78,10 @@ class KnnResultBuilder:
 
     def add_vector_id_result(self, dist, vid):
         ent = (dist, self.vid_key(vid), vid)
-        if not any(e[0] == ent[0] and e[1] == ent[1] for e in self.items):  # a set: an equal pair collapses
+        # a set: an equal pair collapses
+        if not any(_float_key(e[0]) == _float_key(ent[0]) and e[1] == ent[1] for e in self.items):
             self.items.append(ent)
-            self.items.sort(key=lambda e: (e[0], e[1]))
+            self.items.sort(key=lambda e: (_float_key(e[0]), e[1]))
         if len(self.items) > self.knn:
             self.items.pop()
 

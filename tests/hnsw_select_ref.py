@@ -6,8 +6,8 @@
   select(metric, X, elem, cand, m_max, presorted, ...)    Heuristic::select, standard variant
                                                           (idx/trees/hnsw/heuristic.rs:61-81,201-216)
 
-Distances are reported as the walk reports them: through the total-order key, so -0.0 comes back as 0.0.  A NaN
-distance sorts after +inf here; on the GPU it ranks by the bit pattern the GPU produced (DESIGN.md section 8), so the
+Distances are ordered by f64::total_cmp, the order of FloatKey (idx/trees/knn.rs:129-160): -0.0 before 0.0, and each
+distance is reported as computed, -0.0 included.  A NaN distance sorts after +inf here; on the GPU it ranks by the bit pattern the GPU produced (DESIGN.md section 8), so the
 tests compare the non-NaN part of a ranking.
 """
 import numpy as np
@@ -24,11 +24,12 @@ def distances(metric, X, q, order=3.0, vector_type="F32"):
 
 
 def key(d):
-    """the walk's total-order key of an f64 distance (dist_key: -0.0 is 0.0, NaN after +inf)"""
+    """FloatKey's total-order key of an f64 distance (f64::total_cmp: -0.0 before 0.0; NaN after +inf here)"""
     d = float(d)
     if d != d:
-        return (1, 0.0)
-    return (0, d + 0.0)
+        return (1, 0)
+    b = int(np.float64(d).view(np.int64))
+    return (0, b ^ ((b >> 63) & 0x7FFFFFFFFFFFFFFF))
 
 
 def knn(metric, X, q, k, members=None, order=3.0, vector_type="F32"):
@@ -36,7 +37,7 @@ def knn(metric, X, q, k, members=None, order=3.0, vector_type="F32"):
     ids = np.arange(X.shape[0]) if members is None else np.sort(np.asarray(members, np.int64))
     d = distances(metric, np.asarray(X)[ids], q, order, vector_type)
     rank = sorted(range(ids.size), key=lambda i: (key(d[i]), int(ids[i])))[:k]
-    out = np.array([d[i] + 0.0 for i in rank], np.float64)
+    out = np.array([d[i] for i in rank], np.float64)
     return ids[rank].astype(np.int64), out
 
 

@@ -272,3 +272,43 @@ def test_refusals(ctx):
     NN = (C.c_uint64 * 1)(0)
     assert L.lib().sdb_hnsw_load_staged_typed(ctx.h, 4, L.METRIC["EUCLIDEAN"], 9, 1, None, None, None, 0, 1, NB, NO, NO,
                                               NN, -1, C.byref(h), None) == L.SDB_EINVAL
+
+
+def test_f64_pearson_negative_zero_distance(ctx):
+    # F64 PEARSON underflows to -0.0 for element 1 ([1e10, -1e10, 1e-320] against [0, 0, -1]).  The walk, the exact kNN
+    # and the document-level result order by FloatKey (total_cmp: -0.0 before 0.0) and return -0.0 with its sign; the
+    # walk still expands a 0.0 candidate when its f is -0.0 (cq_dist > fq_dist compares f64s).  Compared by bits.
+    import torch
+    import hnsw_select_ref as S
+    from surrealdb_b200.hnsw import HnswIndex
+    from surrealdb_b200.hnsw_build import knn_exact
+    rng = np.random.default_rng(0)
+    special = np.array([[1.0, -1.0, 0.0], [1e10, -1e10, 1e-320], [5.0, 5.0, 5.0], [-2.0, 2.0, 0.0]])
+    data = np.concatenate([rng.uniform(0, 1, (6, 3)) * np.array([1.0, 1.0, -1.0]), special, rng.uniform(-1, 1, (4, 3))])
+    q = np.array([[0.0, 0.0, -1.0]])
+    n = data.shape[0]
+    full = np.array([j for i in range(n) for j in range(n) if j != i], np.uint32)  # every element links every other
+    layers = [(np.arange(n + 1, dtype=np.uint64) * (n - 1), full)]
+    wi, wd = S.knn("pearson", data, q[0], n, vector_type="F64")
+    zero = [int(i) for i, d in zip(wi, wd) if d == 0.0]
+    assert len(zero) == 4 and zero[0] == 7 and np.signbit(wd[list(wi).index(7)])  # -0.0 first among the zeros
+    first = list(wi).index(7)
+    g = dict(vectors=data, layers=layers, entry_point=0)
+    for entry in (0, 7, 6):
+        g["entry_point"] = entry
+        idx = HnswIndex(ctx, data, layers, entry, "pearson", vector_type="F64")
+        for k, ef in ((first + 1, first + 1), (first + 2, first + 2), (first + 1, n), (n, n), (1, 1)):
+            ids, dist, cnt, ctr = idx.search_graph(q, k, ef, counters=True)
+            oi, od, oc = R.search_csr(g, q[0], k, ef, "pearson", vector_type="F64")
+            assert cnt[0] == oi.size and list(ids[0, : cnt[0]]) == list(oi), (entry, k, ef)
+            assert dist[0, : cnt[0]].tobytes() == od.tobytes(), (entry, k, ef)
+            assert (int(ctr[0, 0]), int(ctr[0, 1])) == oc, (entry, k, ef)
+        res = idx.knn_search(q[0], first + 2, n)
+        assert [int(v) for v, _ in res] == list(wi[: first + 2])
+        assert np.array([d for _, d in res]).tobytes() == wd[: first + 2].tobytes()
+        for k in (first + 1, first + 2, n):
+            ids, dist, cnt = knn_exact(idx.h, torch.from_numpy(q).cuda(), k)
+            ids, dist, cnt = ids.cpu().numpy(), dist.cpu().numpy(), cnt.cpu().numpy()
+            assert cnt[0] == k and list(ids[0, :k]) == list(wi[:k]), k
+            assert dist[0, :k].tobytes() == wd[:k].tobytes(), k
+        idx.close()

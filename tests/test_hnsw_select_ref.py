@@ -62,3 +62,13 @@ def test_knn_orders_by_key_then_id():
     assert np.signbit(d[1]) == False and np.isnan(d[-1])
     ids, d = S.knn("euclidean", X, np.array([0.0]), 2, members=[5, 2, 1], vector_type="F64")
     assert list(ids) == [5, 1]
+
+
+def test_knn_keeps_a_negative_zero_pearson_distance_before_zero():
+    # F64 PEARSON underflows to -0.0 for element 1: sxy is a tiny negative subnormal, the denominator about 1e10.
+    # FloatKey orders by total_cmp, so it comes before the 0.0 of elements 0 (uncorrelated) and 2 (constant)
+    X = np.array([[1.0, -1.0, 0.0], [1e10, -1e10, 1e-320], [5.0, 5.0, 5.0], [1.0, 2.0, 3.0]])
+    q = np.array([0.0, 0.0, -1.0])
+    ids, d = S.knn("pearson", X, q, 4, vector_type="F64")
+    assert list(ids) == [3, 1, 0, 2]
+    assert d[0] < 0 and d[1] == 0.0 and np.signbit(d[1]) and not np.signbit(d[2]) and not np.signbit(d[3])

@@ -11,6 +11,7 @@ import torch.distributed as dist
 import torch.multiprocessing as mp
 
 from oracle import pyoracle as O
+from select_ref import merge
 from surrealdb_b200.engine import shard_block_layout
 from surrealdb_b200.sharding import shard_range
 from surrealdb_b200.synthetic import gen_f32
@@ -19,19 +20,14 @@ ROWS, DIM, NQ, K = 3000, 24, 5, 7
 
 
 def merge_reference(blocks, nq, k):
-    """numpy statement of sdb_topk_merge_device: order by (Number::cmp key, global row), first k"""
+    """sdb_topk_merge_device over the gathered blocks (tests/select_ref.merge): order by (Number::cmp key, global
+    row), first k"""
     off_rows, off_dist, off_cnt, blk = shard_block_layout(nq, k)
-    out = []
-    for q in range(nq):
-        ent = []
-        for b in blocks:
-            rows = b[off_rows:off_dist].view(np.uint64).reshape(nq, k)
-            dst = b[off_dist:off_cnt].view(np.float64).reshape(nq, k)
-            cnt = b[off_cnt:off_cnt + 4 * nq].view(np.uint32)
-            ent += [(float(dst[q, j]), int(rows[q, j])) for j in range(int(cnt[q]))]
-        ent.sort(key=lambda e: (e[0], e[1]))
-        out.append(ent[:k])
-    return out
+    rows = np.stack([b[off_rows:off_dist].view(np.uint64).reshape(nq, k) for b in blocks])
+    dst = np.stack([b[off_dist:off_cnt].view(np.float64).reshape(nq, k) for b in blocks])
+    cnt = np.stack([b[off_cnt:off_cnt + 4 * nq].view(np.uint32) for b in blocks])
+    r, d, c = merge(rows, dst, cnt, k)
+    return [[(float(d[q, j]), int(r[q, j])) for j in range(int(c[q]))] for q in range(nq)]
 
 
 def worker(rank, world, port, q):
