@@ -149,6 +149,9 @@ sdb_status sdb_debug_screen_batch(sdb_corpus*, const double* queries, uint32_t n
                                   int streaming, uint32_t cand_cap, int score_all, float* out_qf, double* out_qmag,
                                   uint32_t* out_qu, int8_t* out_q8, uint16_t* out_qbf16, uint32_t* out_a,
                                   uint32_t* out_b, uint32_t* out_rr);
+/* Test-only: device and pinned buffers the library holds right now, process-wide (count and bytes).  Buffers handed to
+ * the caller (sdb_pinned_alloc, sdb_graph_expand_device) are not counted.  Either output may be NULL. */
+void sdb_debug_live_allocations(uint64_t* count, uint64_t* bytes);
 uint64_t sdb_ctx_kernel_launches(const sdb_ctx*);
 /* the cudaStream_t every kernel of this context is launched on (so a harness can bracket calls with
  * CUDA events on the launching stream) */

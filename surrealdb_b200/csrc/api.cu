@@ -130,8 +130,7 @@ static uint32_t n_batch_rungs(const std::vector<Rung>& r) {  // rungs a WHOLE ba
 // swap the ticket's scratch set into the corpus' active fields (see Scratch in internal.cuh)
 static void activate_set(Corpus* c, int set) {
   if (c->active_set == set) return;
-  c->sets[c->active_set] = static_cast<Scratch&>(*c);
-  static_cast<Scratch&>(*c) = c->sets[set];
+  std::swap(static_cast<Scratch&>(*c), c->parked);
   c->active_set = set;
 }
 static cudaError_t drain(Ctx* ctx) {  // both batch streams idle
@@ -152,11 +151,9 @@ static sdb_status ticket_prepare(Corpus* c, Ticket& t, uint32_t nq) {
     SDB_CUDA(cudaEventCreateWithFlags(&t.ev_main, cudaEventDisableTiming));
   }
   if (t.h_cap < nq) {
-    if (t.h_flags) cudaFreeHost(t.h_flags);
-    t.h_flags = nullptr;
     t.h_cap = 0;
     const uint32_t cap = (nq + 1023) / 1024 * 1024;
-    SDB_CUDA(cudaHostAlloc(&t.h_flags, sizeof(uint32_t) * (2 * (size_t)cap + 8), cudaHostAllocDefault));
+    SDB_CUDA(t.h_flags.reserve(2 * (size_t)cap + 8));
     t.h_qflags = t.h_flags + cap;
     t.h_stat = t.h_qflags + cap;
     t.h_cap = cap;
@@ -397,25 +394,20 @@ static sdb_status finish_local(Corpus* c, Ticket& t, uint32_t* n_fallback, bool*
       if ((t.cancel && *t.cancel) || ctx_cancelled(ctx)) break;
       const uint32_t nf = (uint32_t)fails.size();
       const size_t need_q = (size_t)nf * c->dim, need_o = (size_t)nf * k;
-      if (c->rp_cap_q < need_q || c->rp_cap_o < need_o || c->rp_cap_n < nf) {
-        cudaFree(c->d_rp_q); cudaFree(c->d_rp_rows); cudaFree(c->d_rp_dist); cudaFree(c->d_rp_cnt);
-        c->d_rp_q = nullptr; c->d_rp_rows = nullptr; c->d_rp_dist = nullptr; c->d_rp_cnt = nullptr;
-        c->rp_cap_q = c->rp_cap_o = c->rp_cap_n = 0;
-        if (cudaMalloc(&c->d_rp_q, sizeof(double) * need_q) != cudaSuccess || cudaMalloc(&c->d_rp_rows, sizeof(uint64_t) * need_o) != cudaSuccess ||
-            cudaMalloc(&c->d_rp_dist, sizeof(double) * need_o) != cudaSuccess || cudaMalloc(&c->d_rp_cnt, sizeof(uint32_t) * nf) != cudaSuccess) {
-          set_error("repair buffers: %s", cudaGetErrorString(cudaGetLastError()));
-          rc = SDB_ENOMEM;
-          break;
-        }
-        c->rp_cap_q = need_q; c->rp_cap_o = need_o; c->rp_cap_n = nf;
+      cudaError_t e = c->d_rp_q.reserve(need_q);
+      if (e == cudaSuccess) e = c->rp.reserve(need_o, nf);
+      if (e != cudaSuccess) {
+        set_error("repair buffers: %s", cudaGetErrorString(e));
+        rc = SDB_ENOMEM;
+        break;
       }
       for (uint32_t i = 0; i < nf; i++)
         cudaMemcpyAsync(c->d_rp_q + (size_t)i * c->dim, save_q + (size_t)fails[i] * c->dim, sizeof(double) * c->dim, cudaMemcpyDeviceToDevice, st);
       t.d_queries = c->d_rp_q;
       t.nq = nf;
-      t.d_out_rows = c->d_rp_rows;
-      t.d_out_dist = c->d_rp_dist;
-      t.d_out_count = c->d_rp_cnt;
+      t.d_out_rows = c->rp.rows;
+      t.d_out_dist = c->rp.dist;
+      t.d_out_count = c->rp.count;
       t.rung = rung;
       rc = enqueue_batch(c, t);
       if (rc == SDB_OK && cudaEventSynchronize(t.ev_end) != cudaSuccess) rc = SDB_ECUDA;
@@ -427,9 +419,9 @@ static sdb_status finish_local(Corpus* c, Ticket& t, uint32_t* n_fallback, bool*
           still.push_back(q);
           continue;
         }
-        cudaMemcpyAsync(save_rows + (size_t)q * k, c->d_rp_rows + (size_t)i * k, sizeof(uint64_t) * k, cudaMemcpyDeviceToDevice, st);
-        cudaMemcpyAsync(save_dist + (size_t)q * k, c->d_rp_dist + (size_t)i * k, sizeof(double) * k, cudaMemcpyDeviceToDevice, st);
-        cudaMemcpyAsync(save_cnt + q, c->d_rp_cnt + i, sizeof(uint32_t), cudaMemcpyDeviceToDevice, st);
+        cudaMemcpyAsync(save_rows + (size_t)q * k, c->rp.rows + (size_t)i * k, sizeof(uint64_t) * k, cudaMemcpyDeviceToDevice, st);
+        cudaMemcpyAsync(save_dist + (size_t)q * k, c->rp.dist + (size_t)i * k, sizeof(double) * k, cudaMemcpyDeviceToDevice, st);
+        cudaMemcpyAsync(save_cnt + q, c->rp.count + i, sizeof(uint32_t), cudaMemcpyDeviceToDevice, st);
         t.n_repaired++;
       }
       SDB_CUDA(cudaStreamSynchronize(st));
@@ -586,13 +578,7 @@ sdb_status knn_submit_for_shard(Corpus* c, const double* d_queries, const double
   if (h_queries) {  // host queries: staged through the slot's device buffer on the copy stream
     SDB_TRY(ticket_prepare(c, *t, nq));
     const size_t need_q = (size_t)nq * c->dim;
-    if (t->in_cap < need_q) {
-      cudaFree(t->d_in_q);
-      t->d_in_q = nullptr;
-      t->in_cap = 0;
-      SDB_CUDA(cudaMalloc(&t->d_in_q, sizeof(double) * need_q));
-      t->in_cap = need_q;
-    }
+    SDB_CUDA(t->d_in_q.reserve(need_q));
     cudaStream_t cs = c->ctx->copy_stream;
     SDB_CUDA(cudaMemcpyAsync(t->d_in_q, h_queries, sizeof(double) * need_q, cudaMemcpyHostToDevice, cs));
     SDB_CUDA(cudaEventRecord(t->ev_h2d, cs));
@@ -830,11 +816,9 @@ sdb_status sdb_ctx_create(int device, sdb_ctx** out) {
   SDB_CUDA(cudaStreamCreateWithFlags(&c->stream2, cudaStreamNonBlocking));
   SDB_CUDA(cudaStreamCreateWithFlags(&c->copy_stream, cudaStreamNonBlocking));
   {
-    int* hc = nullptr;
-    SDB_CUDA(cudaHostAlloc(&hc, sizeof(int), cudaHostAllocMapped));
-    *hc = 0;
-    c->h_cancel = hc;
-    SDB_CUDA(cudaMalloc(&c->d_cancel, sizeof(int)));
+    SDB_CUDA(c->h_cancel.reserve(1, nullptr, cudaHostAllocMapped));
+    *c->h_cancel = 0;
+    SDB_CUDA(c->d_cancel.reserve(1));
     SDB_CUDA(cudaMemset(c->d_cancel, 0, sizeof(int)));
     SDB_CUDA(cudaStreamCreateWithFlags(&c->cancel_stream, cudaStreamNonBlocking));
   }
@@ -860,16 +844,13 @@ void sdb_ctx_destroy(sdb_ctx* c) {
   if (c->stream) cudaStreamDestroy(c->stream);
   if (c->stream2) cudaStreamDestroy(c->stream2);
   if (c->copy_stream) cudaStreamDestroy(c->copy_stream);
-  if (c->h_stage) cudaFreeHost(c->h_stage);
-  if (c->h_cancel) cudaFreeHost((void*)c->h_cancel);
-  if (c->d_cancel) cudaFree(c->d_cancel);
   if (c->cancel_stream) cudaStreamDestroy(c->cancel_stream);
   delete c;
 }
 static void push_cancel_word(sdb_ctx* c) {  // any host thread; its own stream, so it overtakes running kernels
   if (!c->d_cancel || !c->cancel_stream) return;
   if (cudaSetDevice(c->device) != cudaSuccess) return;
-  cudaMemcpyAsync(c->d_cancel, (const void*)c->h_cancel, sizeof(int), cudaMemcpyHostToDevice, c->cancel_stream);
+  cudaMemcpyAsync(c->d_cancel, (const void*)c->h_cancel.get(), sizeof(int), cudaMemcpyHostToDevice, c->cancel_stream);
   cudaStreamSynchronize(c->cancel_stream);
 }
 void sdb_ctx_cancel(sdb_ctx* c) {
@@ -885,15 +866,15 @@ void sdb_ctx_cancel_reset(sdb_ctx* c) {
 uint64_t sdb_ctx_kernel_launches(const sdb_ctx* c) { return c ? c->launches : 0; }
 void* sdb_ctx_stream(const sdb_ctx* c) { return c ? (void*)c->stream : nullptr; }
 void* sdb_pinned_alloc(size_t bytes) {
-  void* p = nullptr;
-  if (cudaHostAlloc(&p, bytes, cudaHostAllocDefault) != cudaSuccess) {
+  PinnedBuf<uint8_t> p;
+  if (p.reserve(bytes) != cudaSuccess) {
     set_error("cudaHostAlloc(%zu) failed", bytes);
     return nullptr;
   }
-  return p;
+  return p.release();
 }
 void sdb_pinned_free(void* p) {
-  if (p) cudaFreeHost(p);
+  if (p) PinnedBuf<uint8_t>::free_released(p);
 }
 void sdb_free(void* p) { free(p); }
 
@@ -923,11 +904,11 @@ sdb_status sdb_corpus_create(sdb_ctx* ctx, uint32_t dim, sdb_dtype dt, sdb_metri
   c->cap = cap;
   const size_t esz = dt == SDB_F32 ? 4 : 8;
   const uint64_t cap_pad = (cap + TILE_ROWS - 1) / TILE_ROWS * TILE_ROWS;
-  cudaError_t e = cudaMalloc(&c->d_rows, esz * cap * dim);
-  if (e == cudaSuccess) e = cudaMalloc(&c->d_mag, sizeof(double) * cap);
-  if (e == cudaSuccess) e = cudaMalloc(&c->d_snorm, sizeof(float) * cap_pad);
-  if (e == cudaSuccess && dt == SDB_F32 && screenable) e = cudaMalloc(&c->d_bf16, sizeof(__nv_bfloat16) * cap_pad * c->dim_pad);
-  if (e == cudaSuccess && dt == SDB_F32 && m == SDB_COSINE) e = cudaMalloc(&c->d_i8, (size_t)cap_pad * c->dim_pad8);
+  cudaError_t e = c->d_rows.reserve(esz * cap * dim);
+  if (e == cudaSuccess) e = c->d_mag.reserve(cap);
+  if (e == cudaSuccess) e = c->d_snorm.reserve(cap_pad);
+  if (e == cudaSuccess && dt == SDB_F32 && screenable) e = c->d_bf16.reserve(cap_pad * c->dim_pad);
+  if (e == cudaSuccess && dt == SDB_F32 && m == SDB_COSINE) e = c->d_i8.reserve((size_t)cap_pad * c->dim_pad8);
   if (e != cudaSuccess) {
     set_error("corpus allocation failed: %s", cudaGetErrorString(e));
     sdb_corpus_destroy(c);
@@ -941,31 +922,10 @@ void sdb_corpus_destroy(sdb_corpus* c) {
   cudaSetDevice(c->ctx->device);
   drain(c->ctx);
   comm_corpus_released(c);
-  for (int si = 0; si < 2; si++) {  // the parked scratch set
-    if (si == c->active_set) continue;
-    Scratch& z = c->sets[si];
-    void* sp[] = {z.d_q64, z.d_q32, z.d_qbf16, z.d_qmag, z.d_qflags, z.d_qbferr, z.d_q8, z.d_q8scale, z.d_q8err, z.d_sub,
-                  z.d_sub_cnt, z.d_bscale, z.d_beps, z.d_margin, z.d_margin2, z.d_beps2, z.d_tau2, z.d_qlow, z.d_qcap,
-                  z.d_hparam, z.d_hist, z.d_probe, z.d_tau, z.d_cand, z.d_cand_cnt, z.d_flags, z.d_stat, z.d_rr_key,
-                  z.d_rr_dist, z.d_rr_row};
-    for (void* p : sp) cudaFree(p);
-  }
-  void* ptrs[] = {c->d_i8, c->d_q8, c->d_q8scale, c->d_q8err, c->d_bscale, c->d_beps, c->d_margin, c->d_qlow, c->d_qcap,
-                  c->d_hparam, c->d_hist, c->d_qbferr, c->d_stat, c->d_probe, c->d_margin2, c->d_beps2, c->d_tau2, c->d_sub, c->d_sub_cnt, c->d_rows, c->d_mag, c->d_snorm,
-                  c->d_bf16, c->d_skip, c->d_removed, c->d_special, c->d_q64, c->d_q32, c->d_qbf16, c->d_qmag, c->d_qflags,
-                  c->d_tau, c->d_cand, c->d_cand_cnt, c->d_flags, c->d_rr_key, c->d_rr_dist, c->d_rr_row, c->d_ex_key,
-                  c->d_ex_val, c->d_sel, c->d_fb_q, c->d_fb_qmag, c->d_fb_qflags, c->d_block, c->d_gather, c->d_rp_q, c->d_rp_rows,
-                  c->d_rp_dist, c->d_rp_cnt};
-  for (void* p : ptrs) cudaFree(p);
   for (Ticket& t : c->tickets) {
     cudaEvent_t evs[] = {t.ev_begin, t.ev_screen0, t.ev_screen1, t.ev_end, t.ev_h2d, t.ev_out, t.ev_main};
     for (cudaEvent_t e : evs)
       if (e) cudaEventDestroy(e);
-    if (t.h_flags) cudaFreeHost(t.h_flags);
-    cudaFree(t.d_in_q);
-    cudaFree(t.d_res_rows);
-    cudaFree(t.d_res_dist);
-    cudaFree(t.d_res_count);
   }
   delete c;
 }
@@ -980,7 +940,7 @@ static sdb_status append_common(sdb_corpus* c, const void* src, uint64_t n, cuda
   }
   SDB_CUDA(cudaSetDevice(c->ctx->device));
   const size_t esz = c->dtype == SDB_F32 ? 4 : 8;
-  SDB_CUDA(cudaMemcpyAsync((char*)c->d_rows + esz * c->n * c->dim, src, esz * n * c->dim, kind, c->ctx->stream));
+  SDB_CUDA(cudaMemcpyAsync((char*)c->d_rows.get() + esz * c->n * c->dim, src, esz * n * c->dim, kind, c->ctx->stream));
   SDB_CUDA(cudaStreamSynchronize(c->ctx->stream));
   c->n += n;
   c->finalized = false;
@@ -1001,7 +961,7 @@ sdb_status sdb_corpus_append_synthetic(sdb_corpus* c, uint64_t seed, uint64_t fi
   std::lock_guard<std::mutex> g(c->mu);
   if (c->n + n > c->cap) return SDB_EOVERFLOW;
   SDB_CUDA(cudaSetDevice(c->ctx->device));
-  SDB_TRY(gen_fill_f32(c->ctx, (float*)c->d_rows + c->n * c->dim, seed, first_row * c->dim, n * c->dim, c->ctx->stream));
+  SDB_TRY(gen_fill_f32(c->ctx, (float*)c->d_rows.get() + c->n * c->dim, seed, first_row * c->dim, n * c->dim, c->ctx->stream));
   SDB_CUDA(cudaStreamSynchronize(c->ctx->stream));
   c->n += n;
   c->finalized = false;
@@ -1012,10 +972,9 @@ sdb_status sdb_corpus_set_skip(sdb_corpus* c, const uint8_t* skip, uint64_t n) {
   std::lock_guard<std::mutex> g(c->mu);
   SDB_CUDA(cudaSetDevice(c->ctx->device));
   if (!skip) {
-    cudaFree(c->d_skip);
-    c->d_skip = nullptr;
+    c->d_skip.reset();
   } else {
-    if (!c->d_skip) SDB_CUDA(cudaMalloc(&c->d_skip, c->cap));
+    SDB_CUDA(c->d_skip.reserve(c->cap));
     SDB_CUDA(cudaMemsetAsync(c->d_skip, 0, c->cap, c->ctx->stream));
     SDB_CUDA(cudaMemcpyAsync(c->d_skip, skip, n, cudaMemcpyHostToDevice, c->ctx->stream));
   }
@@ -1062,7 +1021,7 @@ sdb_status sdb_corpus_read_rows(sdb_corpus* c, uint64_t first_row, uint64_t n, v
   if (n == 0) return SDB_OK;
   SDB_CUDA(cudaSetDevice(c->ctx->device));
   const size_t esz = c->dtype == SDB_F32 ? 4 : 8;
-  SDB_CUDA(cudaMemcpyAsync(out, (const char*)c->d_rows + esz * first_row * c->dim, esz * n * c->dim,
+  SDB_CUDA(cudaMemcpyAsync(out, (const char*)c->d_rows.get() + esz * first_row * c->dim, esz * n * c->dim,
                            cudaMemcpyDeviceToHost, c->ctx->copy_stream));
   SDB_CUDA(cudaStreamSynchronize(c->ctx->copy_stream));
   return SDB_OK;
@@ -1104,30 +1063,6 @@ sdb_status sdb_knn_submit_device(sdb_corpus* c, const double* d_queries, uint32_
   return SDB_OK;
 }
 
-static sdb_status ensure_slot_buffers(Corpus* c, Ticket* t, uint32_t nq, uint32_t k) {
-  const size_t need_q = (size_t)nq * c->dim, need = (size_t)nq * (k ? k : 1);
-  if (t->in_cap < need_q) {
-    cudaFree(t->d_in_q);
-    t->d_in_q = nullptr;
-    t->in_cap = 0;
-    SDB_CUDA(cudaMalloc(&t->d_in_q, sizeof(double) * need_q));
-    t->in_cap = need_q;
-  }
-  if (t->res_cap < need || t->res_cap_q < nq) {
-    cudaFree(t->d_res_rows);
-    cudaFree(t->d_res_dist);
-    cudaFree(t->d_res_count);
-    t->d_res_rows = nullptr; t->d_res_dist = nullptr; t->d_res_count = nullptr;
-    t->res_cap = t->res_cap_q = 0;
-    SDB_CUDA(cudaMalloc(&t->d_res_rows, sizeof(uint64_t) * need));
-    SDB_CUDA(cudaMalloc(&t->d_res_dist, sizeof(double) * need));
-    SDB_CUDA(cudaMalloc(&t->d_res_count, sizeof(uint32_t) * nq));
-    t->res_cap = need;
-    t->res_cap_q = nq;
-  }
-  return SDB_OK;
-}
-
 static sdb_status submit_host_locked(sdb_corpus* c, const double* queries, uint32_t nq, uint32_t k, uint64_t* out_rows,
                                      double* out_dist, uint32_t* out_count, const volatile int* cancel, Ticket** out_t) {
   Ticket* t = free_ticket(c);
@@ -1136,13 +1071,14 @@ static sdb_status submit_host_locked(sdb_corpus* c, const double* queries, uint3
     return SDB_EOVERFLOW;
   }
   SDB_TRY(ticket_prepare(c, *t, nq));
-  SDB_TRY(ensure_slot_buffers(c, t, nq, k));
+  SDB_CUDA(t->d_in_q.reserve((size_t)nq * c->dim));
+  SDB_CUDA(t->res.reserve((size_t)nq * (k ? k : 1), nq));
   // the queries travel on the copy stream, so the transfer of batch i+1 overlaps the kernels of batch i
   cudaStream_t cs = c->ctx->copy_stream;
   SDB_CUDA(cudaMemcpyAsync(t->d_in_q, queries, sizeof(double) * (size_t)nq * c->dim, cudaMemcpyHostToDevice, cs));
   SDB_CUDA(cudaEventRecord(t->ev_h2d, cs));
   t->wait_h2d = true;  // submit_locked makes the batch's stream wait for the transfer
-  SDB_TRY(submit_locked(c, t, t->d_in_q, nq, k, c->row_base, t->d_res_rows, t->d_res_dist, t->d_res_count, cancel));
+  SDB_TRY(submit_locked(c, t, t->d_in_q, nq, k, c->row_base, t->res.rows, t->res.dist, t->res.count, cancel));
   t->h_out_rows = out_rows;
   t->h_out_dist = out_dist;
   t->h_out_count = out_count;
@@ -1192,6 +1128,11 @@ sdb_status sdb_debug_schedule(uint64_t n_rows, uint32_t cand_cap, uint32_t k, ui
 
 // Test-only diagnostics of the screens (declared in the header's diagnostics block): the corpus' screen copies and one
 // screened batch, so that tests can hold every intermediate of the proof against a plain reference.
+void sdb_debug_live_allocations(uint64_t* count, uint64_t* bytes) {
+  if (count) *count = g_live_bufs.load();
+  if (bytes) *bytes = g_live_bytes.load();
+}
+
 sdb_status sdb_debug_corpus_state(sdb_corpus* c, float* out_f, uint32_t* out_u, int8_t* out_i8, uint16_t* out_bf16,
                                   float* out_snorm, uint32_t* out_special) {
   if (!c) return SDB_EINVAL;
@@ -1259,18 +1200,14 @@ sdb_status sdb_debug_screen_batch(sdb_corpus* c, const double* queries, uint32_t
   c->sc_nq = c->sc_cap = 0;
   SDB_TRY(scratch_for(c, nq, cap));
   cudaStream_t st = ctx->stream;
-  double* d_q = nullptr;
-  uint64_t* d_rows = nullptr;
-  double* d_dist = nullptr;
-  uint32_t* d_cnt = nullptr;
+  DevBuf<double> d_q;
+  ResultBufs out;
   ScreenTap tap;
   const sdb_screen save_screen = c->screen;
   const bool save_stream = c->stream_refine;
   auto run = [&]() -> sdb_status {
-    SDB_CUDA(cudaMalloc(&d_q, sizeof(double) * (size_t)nq * c->dim));
-    SDB_CUDA(cudaMalloc(&d_rows, sizeof(uint64_t) * (size_t)nq * k));
-    SDB_CUDA(cudaMalloc(&d_dist, sizeof(double) * (size_t)nq * k));
-    SDB_CUDA(cudaMalloc(&d_cnt, sizeof(uint32_t) * nq));
+    SDB_CUDA(d_q.reserve((size_t)nq * c->dim));
+    SDB_CUDA(out.reserve((size_t)nq * k, nq));
     SDB_CUDA(cudaMemcpyAsync(d_q, queries, sizeof(double) * (size_t)nq * c->dim, cudaMemcpyHostToDevice, st));
     if (score_all) {  // one pass-0 launch over every tile (SIMT: tau stays -inf), nothing selected
       const PassDesc all{1u, 0u, (uint32_t)(n_pad / TILE_ROWS), 0u};
@@ -1291,9 +1228,9 @@ sdb_status sdb_debug_screen_batch(sdb_corpus* c, const double* queries, uint32_t
     t->nq = nq;
     t->k = k;
     t->row_base = 0;
-    t->d_out_rows = d_rows;
-    t->d_out_dist = d_dist;
-    t->d_out_count = d_cnt;
+    t->d_out_rows = out.rows;
+    t->d_out_dist = out.dist;
+    t->d_out_count = out.count;
     t->cancel = nullptr;
     t->rung = 0;
     c->tap = &tap;
@@ -1321,7 +1258,7 @@ sdb_status sdb_debug_screen_batch(sdb_corpus* c, const double* queries, uint32_t
     const size_t cap_sz = (size_t)nq * cap;
     std::vector<float> f[9];
     const float* srcf[9] = {c->d_tau, c->d_margin, c->d_bscale, c->d_beps, c->d_tau2, c->d_beps2,
-                            c->d_i8 ? c->d_q8scale : nullptr, c->d_i8 ? c->d_q8err : nullptr, c->d_qbferr};
+                            c->d_i8 ? c->d_q8scale.get() : nullptr, c->d_i8 ? c->d_q8err.get() : nullptr, c->d_qbferr};
     for (int j = 0; j < 9; j++) {
       f[j].assign(nq, NAN);
       if (srcf[j]) rd(f[j].data(), srcf[j], sizeof(float) * nq);
@@ -1383,10 +1320,6 @@ sdb_status sdb_debug_screen_batch(sdb_corpus* c, const double* queries, uint32_t
       }
     }
   }
-  cudaFree(d_q);
-  cudaFree(d_rows);
-  cudaFree(d_dist);
-  cudaFree(d_cnt);
   return rc;
 }
 
@@ -1461,10 +1394,10 @@ sdb_status sdb_corpus_project(sdb_corpus* c, const double* query, int fn, double
   SDB_CUDA(cudaSetDevice(c->ctx->device));
   SDB_CUDA(drain(c->ctx));  // borrows the active scratch set for the prepared query
   cudaStream_t st = c->ctx->stream;
-  double *d_q = nullptr, *d_vals = nullptr;
-  auto run = [&]() -> sdb_status {
-    SDB_CUDA(cudaMallocAsync(&d_q, sizeof(double) * c->dim, st));
-    SDB_CUDA(cudaMallocAsync(&d_vals, sizeof(double) * c->n, st));
+  auto run = [&]() -> sdb_status {  // the temporaries are released on every path, before the synchronisation below
+    AsyncBuf<double> d_q, d_vals;
+    SDB_CUDA(d_q.reserve(c->dim, st));
+    SDB_CUDA(d_vals.reserve(c->n, st));
     if (query) SDB_CUDA(cudaMemcpyAsync(d_q, query, sizeof(double) * c->dim, cudaMemcpyHostToDevice, st));
     else SDB_CUDA(cudaMemsetAsync(d_q, 0, sizeof(double) * c->dim, st));
     SDB_TRY(scratch_for(c, 1, 4096));
@@ -1474,8 +1407,6 @@ sdb_status sdb_corpus_project(sdb_corpus* c, const double* query, int fn, double
     return SDB_OK;
   };
   const sdb_status rc = run();
-  if (d_q) cudaFreeAsync(d_q, st);  // also on the error paths
-  if (d_vals) cudaFreeAsync(d_vals, st);
   if (cudaStreamSynchronize(st) != cudaSuccess && rc == SDB_OK) {
     set_error("sdb_corpus_project: %s", cudaGetErrorString(cudaGetLastError()));
     return SDB_ECUDA;

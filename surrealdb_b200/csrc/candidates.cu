@@ -209,50 +209,53 @@ sdb_status cand_begin(Corpus* c, uint32_t nq, int screen, cudaStream_t st) {
 static sdb_status ensure_scratch(Corpus* c, uint32_t nq, uint32_t cap) {
   const uint32_t nq_pad = (nq + 127) / 128 * 128;
   if (c->sc_nq >= nq_pad && c->sc_cap >= cap) return SDB_OK;
-  void* old[] = {c->d_q64, c->d_q32, c->d_qbf16, c->d_qmag, c->d_qflags, c->d_qbferr, c->d_tau, c->d_cand, c->d_cand_cnt,
-                 c->d_flags, c->d_stat, c->d_rr_key, c->d_rr_dist, c->d_rr_row, c->d_sub, c->d_sub_cnt, c->d_q8,
-                 c->d_q8scale, c->d_q8err, c->d_bscale, c->d_beps, c->d_margin, c->d_qlow, c->d_qcap, c->d_hparam,
-                 c->d_hist, c->d_probe, c->d_margin2, c->d_beps2, c->d_tau2};
-  for (void* p : old) cudaFree(p);
   const uint32_t nqa = nq_pad > c->sc_nq ? nq_pad : c->sc_nq;
   const uint32_t capa = cap > c->sc_cap ? cap : c->sc_cap;
-  c->sc_nq = c->sc_cap = 0;
-  c->sc_gen++;  // everything below is reallocated: prepared queries, candidate lists ... are gone
-  c->rr_stride = capa + SPECIAL_CAP;
-  SDB_CUDA(cudaMalloc(&c->d_q64, sizeof(double) * (size_t)nqa * c->dim));
-  SDB_CUDA(cudaMalloc(&c->d_q32, sizeof(float) * (size_t)nqa * c->dim));
-  SDB_CUDA(cudaMalloc(&c->d_qbf16, sizeof(__nv_bfloat16) * (size_t)nqa * c->dim_pad));
-  SDB_CUDA(cudaMalloc(&c->d_qmag, sizeof(double) * nqa));
-  SDB_CUDA(cudaMalloc(&c->d_qflags, sizeof(uint32_t) * nqa));
-  SDB_CUDA(cudaMalloc(&c->d_qbferr, sizeof(float) * nqa));
-  SDB_CUDA(cudaMalloc(&c->d_tau, sizeof(float) * nqa));
-  SDB_CUDA(cudaMalloc(&c->d_cand, sizeof(Cand) * (size_t)nqa * capa));
-  SDB_CUDA(cudaMalloc(&c->d_cand_cnt, sizeof(uint32_t) * nqa));
-  SDB_CUDA(cudaMalloc(&c->d_flags, sizeof(uint32_t) * nqa));
-  SDB_CUDA(cudaMalloc(&c->d_stat, sizeof(uint32_t) * 4));
-  SDB_CUDA(cudaMalloc(&c->d_rr_key, sizeof(uint64_t) * (size_t)nqa * c->rr_stride));
-  SDB_CUDA(cudaMalloc(&c->d_rr_dist, sizeof(double) * (size_t)nqa * c->rr_stride));
-  SDB_CUDA(cudaMalloc(&c->d_rr_row, sizeof(uint32_t) * (size_t)nqa * c->rr_stride));
-  SDB_CUDA(cudaMalloc(&c->d_q8, (size_t)nqa * (c->dim_pad8 ? c->dim_pad8 : 128)));
-  SDB_CUDA(cudaMalloc(&c->d_q8scale, sizeof(float) * nqa));
-  SDB_CUDA(cudaMalloc(&c->d_q8err, sizeof(float) * nqa));
-  SDB_CUDA(cudaMalloc(&c->d_bscale, sizeof(float) * nqa));
-  SDB_CUDA(cudaMalloc(&c->d_beps, sizeof(float) * nqa));
-  SDB_CUDA(cudaMalloc(&c->d_margin, sizeof(float) * nqa));
-  SDB_CUDA(cudaMalloc(&c->d_margin2, sizeof(float) * nqa));
-  SDB_CUDA(cudaMalloc(&c->d_beps2, sizeof(float) * nqa));
-  SDB_CUDA(cudaMalloc(&c->d_tau2, sizeof(float) * nqa));
-  SDB_CUDA(cudaMalloc(&c->d_qlow, sizeof(float) * nqa));
-  SDB_CUDA(cudaMalloc(&c->d_qcap, sizeof(float) * nqa));
-  SDB_CUDA(cudaMalloc(&c->d_hparam, sizeof(HistParam) * nqa));
-  SDB_CUDA(cudaMalloc(&c->d_hist, sizeof(uint32_t) * (size_t)nqa * HIST_BINS));
-  SDB_CUDA(cudaMalloc(&c->d_probe, sizeof(float) * (size_t)nqa * PROBE_STRIDE));
-  c->sub_slots = 2 * (uint32_t)c->ctx->sm_count;
-  c->sub_cap = 16;
-  SDB_CUDA(cudaMalloc(&c->d_sub, sizeof(Cand) * (size_t)nqa * c->sub_slots * c->sub_cap));
-  SDB_CUDA(cudaMalloc(&c->d_sub_cnt, sizeof(uint32_t) * (size_t)nqa * c->sub_slots));
-  c->sc_nq = nqa;
-  c->sc_cap = capa;
+  Scratch& s = *c;
+  s = Scratch();  // everything below is reallocated: prepared queries, candidate lists ... are gone
+  auto alloc = [&]() -> sdb_status {
+    s.rr_stride = capa + SPECIAL_CAP;
+    SDB_CUDA(s.d_q64.reserve((size_t)nqa * c->dim));
+    SDB_CUDA(s.d_q32.reserve((size_t)nqa * c->dim));
+    SDB_CUDA(s.d_qbf16.reserve((size_t)nqa * c->dim_pad));
+    SDB_CUDA(s.d_qmag.reserve(nqa));
+    SDB_CUDA(s.d_qflags.reserve(nqa));
+    SDB_CUDA(s.d_qbferr.reserve(nqa));
+    SDB_CUDA(s.d_tau.reserve(nqa));
+    SDB_CUDA(s.d_cand.reserve((size_t)nqa * capa));
+    SDB_CUDA(s.d_cand_cnt.reserve(nqa));
+    SDB_CUDA(s.d_flags.reserve(nqa));
+    SDB_CUDA(s.d_stat.reserve(4));
+    SDB_CUDA(s.d_rr_key.reserve((size_t)nqa * c->rr_stride));
+    SDB_CUDA(s.d_rr_dist.reserve((size_t)nqa * c->rr_stride));
+    SDB_CUDA(s.d_rr_row.reserve((size_t)nqa * c->rr_stride));
+    SDB_CUDA(s.d_q8.reserve((size_t)nqa * (c->dim_pad8 ? c->dim_pad8 : 128)));
+    SDB_CUDA(s.d_q8scale.reserve(nqa));
+    SDB_CUDA(s.d_q8err.reserve(nqa));
+    SDB_CUDA(s.d_bscale.reserve(nqa));
+    SDB_CUDA(s.d_beps.reserve(nqa));
+    SDB_CUDA(s.d_margin.reserve(nqa));
+    SDB_CUDA(s.d_margin2.reserve(nqa));
+    SDB_CUDA(s.d_beps2.reserve(nqa));
+    SDB_CUDA(s.d_tau2.reserve(nqa));
+    SDB_CUDA(s.d_qlow.reserve(nqa));
+    SDB_CUDA(s.d_qcap.reserve(nqa));
+    SDB_CUDA(s.d_hparam.reserve(nqa));
+    SDB_CUDA(s.d_hist.reserve((size_t)nqa * HIST_BINS));
+    SDB_CUDA(s.d_probe.reserve((size_t)nqa * PROBE_STRIDE));
+    s.sub_slots = 2 * (uint32_t)c->ctx->sm_count;
+    s.sub_cap = 16;
+    SDB_CUDA(s.d_sub.reserve((size_t)nqa * c->sub_slots * c->sub_cap));
+    SDB_CUDA(s.d_sub_cnt.reserve((size_t)nqa * c->sub_slots));
+    return SDB_OK;
+  };
+  const sdb_status rc = alloc();
+  if (rc != SDB_OK) {
+    s = Scratch();  // empty: the next batch allocates it again
+    return rc;
+  }
+  s.sc_nq = nqa;
+  s.sc_cap = capa;
   return SDB_OK;
 }
 
@@ -276,11 +279,9 @@ sdb_status prep_queries(Corpus* c, const double* d_queries, uint32_t nq, cudaStr
 }
 
 sdb_status prep_fallback_query(Corpus* c, const double* d_query, cudaStream_t st) {
-  if (!c->d_fb_q) {
-    SDB_CUDA(cudaMalloc(&c->d_fb_q, sizeof(double) * c->dim));
-    SDB_CUDA(cudaMalloc(&c->d_fb_qmag, sizeof(double)));
-    SDB_CUDA(cudaMalloc(&c->d_fb_qflags, sizeof(uint32_t)));
-  }
+  SDB_CUDA(c->d_fb_q.reserve(c->dim));
+  SDB_CUDA(c->d_fb_qmag.reserve(1));
+  SDB_CUDA(c->d_fb_qflags.reserve(1));
   if (d_query != c->d_fb_q)
     SDB_CUDA(cudaMemcpyAsync(c->d_fb_q, d_query, sizeof(double) * c->dim, cudaMemcpyDeviceToDevice, st));
   // the f32 / bf16 copies are not needed by the exact kernel: q32 goes to a throw-away row of the f64 buffer's size
@@ -557,8 +558,8 @@ sdb_status cand_select(Corpus* c, uint32_t nq, uint32_t k, bool drop_invalid, ui
     return SDB_OK;
   }
   cand_select_kernel<<<nq, 256, 0, st>>>(  // 256 threads: several blocks per SM, the whole batch is one wave
-      c->d_cand, c->d_cand_cnt, c->d_tau, c->d_flags, c->sc_cap, k, c->d_margin, drop_invalid ? c->d_snorm : nullptr,
-      c->d_sub, c->d_sub_cnt, n_slots, c->sub_cap, seed_hist ? c->d_hparam : nullptr, c->d_hist, c->d_qlow, c->d_qcap,
+      c->d_cand, c->d_cand_cnt, c->d_tau, c->d_flags, c->sc_cap, k, c->d_margin, drop_invalid ? c->d_snorm.get() : nullptr,
+      c->d_sub, c->d_sub_cnt, n_slots, c->sub_cap, seed_hist ? c->d_hparam.get() : nullptr, c->d_hist, c->d_qlow, c->d_qcap,
       c->d_stat, c->d_rr_key, c->rr_stride);
   count_launch(c->ctx);
   SDB_CUDA(cudaGetLastError());
@@ -625,10 +626,10 @@ sdb_status cand_refine(Corpus* c, uint32_t nq, cudaStream_t st) {
   if (c->dtype != SDB_F32) return SDB_OK;
   const dim3 grid(nq, 8);  // 128-thread blocks (register budget beside a resident screen CTA)
   if (c->metric == SDB_COSINE)
-    cand_refine_f32_kernel<true><<<grid, 128, 0, st>>>((const float*)c->d_rows, c->dim, c->d_snorm, c->d_q32, c->d_cand,
+    cand_refine_f32_kernel<true><<<grid, 128, 0, st>>>((const float*)c->d_rows.get(), c->dim, c->d_snorm, c->d_q32, c->d_cand,
                                                        c->d_cand_cnt, c->sc_cap);
   else
-    cand_refine_f32_kernel<false><<<grid, 128, 0, st>>>((const float*)c->d_rows, c->dim, c->d_snorm, c->d_q32, c->d_cand,
+    cand_refine_f32_kernel<false><<<grid, 128, 0, st>>>((const float*)c->d_rows.get(), c->dim, c->d_snorm, c->d_q32, c->d_cand,
                                                         c->d_cand_cnt, c->sc_cap);
   count_launch(c->ctx);
   SDB_CUDA(cudaGetLastError());
@@ -863,31 +864,31 @@ sdb_status cand_rerank(Corpus* c, uint32_t nq, cudaStream_t st, bool small_sets)
   if (small_sets && c->dtype == SDB_F32 && !no_packed && (c->metric == SDB_COSINE || c->metric == SDB_EUCLIDEAN)) {
     const unsigned g = (nq + 7) / 8;
     if (c->metric == SDB_COSINE)
-      cand_rerank_packed_kernel<true><<<g, 128, 0, st>>>((const float*)c->d_rows, c->dim, c->d_mag, c->d_q64, c->d_qmag, c->d_qflags,
+      cand_rerank_packed_kernel<true><<<g, 128, 0, st>>>((const float*)c->d_rows.get(), c->dim, c->d_mag, c->d_q64, c->d_qmag, c->d_qflags,
                                                         c->d_cand, c->d_cand_cnt, c->sc_cap, c->d_special, c->n_special, nq,
                                                         c->d_rr_key, c->d_rr_dist, c->d_rr_row, c->rr_stride);
     else
-      cand_rerank_packed_kernel<false><<<g, 128, 0, st>>>((const float*)c->d_rows, c->dim, c->d_mag, c->d_q64, c->d_qmag, c->d_qflags,
+      cand_rerank_packed_kernel<false><<<g, 128, 0, st>>>((const float*)c->d_rows.get(), c->dim, c->d_mag, c->d_q64, c->d_qmag, c->d_qflags,
                                                          c->d_cand, c->d_cand_cnt, c->sc_cap, c->d_special, c->n_special, nq,
                                                          c->d_rr_key, c->d_rr_dist, c->d_rr_row, c->rr_stride);
   } else if (small_sets && c->dtype == SDB_F32)
     // (kept for A/B: one warp per query, rows transposed through 6 KB of shared memory)
-    cand_rerank_kernel<float, 1, 32, 256><<<grid, 32, 0, st>>>((const float*)c->d_rows, c->dim, (int)c->metric, c->d_mag,
+    cand_rerank_kernel<float, 1, 32, 256><<<grid, 32, 0, st>>>((const float*)c->d_rows.get(), c->dim, (int)c->metric, c->d_mag,
                                                                c->d_q64, c->d_qmag, c->d_qflags, c->d_cand, c->d_cand_cnt,
                                                                c->sc_cap, c->d_special, c->n_special, c->d_rr_key,
                                                                c->d_rr_dist, c->d_rr_row, c->rr_stride);
   else if (c->dtype == SDB_F32 && c->dim % 4 == 0 && !no_v4)
-    cand_rerank_v4_kernel<4><<<grid, 128, RRV_SMEM, st>>>((const float*)c->d_rows, c->dim, (int)c->metric, c->d_mag, c->d_q64,
+    cand_rerank_v4_kernel<4><<<grid, 128, RRV_SMEM, st>>>((const float*)c->d_rows.get(), c->dim, (int)c->metric, c->d_mag, c->d_q64,
                                                           c->d_qmag, c->d_qflags, c->d_cand, c->d_cand_cnt, c->sc_cap,
                                                           c->d_special, c->n_special, c->d_rr_key, c->d_rr_dist,
                                                           c->d_rr_row, c->rr_stride);
   else if (c->dtype == SDB_F32)
-    cand_rerank_kernel<float, 4, 32><<<grid, 128, 0, st>>>((const float*)c->d_rows, c->dim, (int)c->metric, c->d_mag,
+    cand_rerank_kernel<float, 4, 32><<<grid, 128, 0, st>>>((const float*)c->d_rows.get(), c->dim, (int)c->metric, c->d_mag,
                                                            c->d_q64, c->d_qmag, c->d_qflags, c->d_cand, c->d_cand_cnt,
                                                            c->sc_cap, c->d_special, c->n_special, c->d_rr_key,
                                                            c->d_rr_dist, c->d_rr_row, c->rr_stride);
   else
-    cand_rerank_kernel<double, 4, 32><<<grid, 128, 0, st>>>((const double*)c->d_rows, c->dim, (int)c->metric, c->d_mag,
+    cand_rerank_kernel<double, 4, 32><<<grid, 128, 0, st>>>((const double*)c->d_rows.get(), c->dim, (int)c->metric, c->d_mag,
                                                             c->d_q64, c->d_qmag, c->d_qflags, c->d_cand, c->d_cand_cnt,
                                                             c->sc_cap, c->d_special, c->n_special, c->d_rr_key,
                                                             c->d_rr_dist, c->d_rr_row, c->rr_stride);

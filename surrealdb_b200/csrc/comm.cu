@@ -127,21 +127,17 @@ static BlockLayout block_layout(uint32_t nq, uint32_t k) {
 }
 
 struct ShardSlot {  // per in-flight ticket: this rank's block, the gathered blocks, the headers on the host
-  uint8_t* d_block = nullptr;
-  uint8_t* d_gather = nullptr;   // NCCL path: own allocation
+  DevBuf<uint8_t> d_block;
+  DevBuf<uint8_t> d_gather;      // NCCL path: own allocation
   uint8_t* gather = nullptr;     // where this batch's blocks are merged from (arena slot or d_gather)
   size_t stride = 0;             // distance between two ranks' blocks inside `gather`
-  size_t block_cap = 0, gather_cap = 0;
-  uint32_t* h_hdr = nullptr;  // pinned, nranks x 4
+  PinnedBuf<uint32_t> h_hdr;     // nranks x 4 + the exchange error word
   int hdr_cap = 0;
   cudaEvent_t ev_done = nullptr;
   uint64_t *d_out_rows = nullptr, *h_out_rows = nullptr;
   double *d_out_dist = nullptr, *h_out_dist = nullptr;
   uint32_t *d_out_count = nullptr, *h_out_count = nullptr;
-  uint64_t* d_res_rows = nullptr;  // host-buffer entry points: merged result staging
-  double* d_res_dist = nullptr;
-  uint32_t* d_res_count = nullptr;
-  size_t res_cap = 0, res_cap_q = 0;
+  ResultBufs res;  // host-buffer entry points: merged result staging
 };
 
 }  // namespace sdb
@@ -166,8 +162,6 @@ sdb_status topk_merge_launch(Ctx* ctx, uint32_t n_lists, uint32_t nq, uint32_t k
 
 namespace {
 
-ShardSlot g_dummy;
-
 struct Arena;
 struct ShardState {  // hangs off the corpus through a side table (kept out of internal.cuh: only comm.cu needs it)
   ShardSlot slots[N_TICKETS];
@@ -189,42 +183,15 @@ sdb_status slot_reserve(Corpus* c, ShardSlot& s, uint32_t nq, uint32_t k, bool h
   const int nranks = c->ctx->comm ? c->ctx->comm->nranks : 1;
   const BlockLayout bl = block_layout(nq, k);
   if (!s.ev_done) SDB_CUDA(cudaEventCreateWithFlags(&s.ev_done, cudaEventDisableTiming));
-  if (s.block_cap < bl.bytes) {
-    cudaFree(s.d_block);
-    s.d_block = nullptr;
-    s.block_cap = 0;
-    SDB_CUDA(cudaMalloc(&s.d_block, bl.bytes));
-    s.block_cap = bl.bytes;
-  }
-  if (s.gather_cap < bl.bytes * nranks) {
-    cudaFree(s.d_gather);
-    s.d_gather = nullptr;
-    s.gather_cap = 0;
-    SDB_CUDA(cudaMalloc(&s.d_gather, bl.bytes * nranks));
-    s.gather_cap = bl.bytes * nranks;
-  }
+  SDB_CUDA(s.d_block.reserve(bl.bytes));
+  SDB_CUDA(s.d_gather.reserve(bl.bytes * nranks));
   if (s.hdr_cap < nranks) {
-    if (s.h_hdr) cudaFreeHost(s.h_hdr);
-    s.h_hdr = nullptr;
-    SDB_CUDA(cudaHostAlloc(&s.h_hdr, sizeof(uint32_t) * (4 * nranks + 4), cudaHostAllocDefault));
+    s.hdr_cap = 0;
+    SDB_CUDA(s.h_hdr.reserve(4 * nranks + 4));
     memset(s.h_hdr, 0, sizeof(uint32_t) * (4 * nranks + 4));  // [4 * nranks]: exchange error word (peer-to-peer path)
     s.hdr_cap = nranks;
   }
-  if (host_out) {
-    const size_t need = (size_t)nq * (k ? k : 1);
-    if (s.res_cap < need || s.res_cap_q < nq) {
-      cudaFree(s.d_res_rows);
-      cudaFree(s.d_res_dist);
-      cudaFree(s.d_res_count);
-      s.d_res_rows = nullptr; s.d_res_dist = nullptr; s.d_res_count = nullptr;
-      s.res_cap = s.res_cap_q = 0;
-      SDB_CUDA(cudaMalloc(&s.d_res_rows, sizeof(uint64_t) * need));
-      SDB_CUDA(cudaMalloc(&s.d_res_dist, sizeof(double) * need));
-      SDB_CUDA(cudaMalloc(&s.d_res_count, sizeof(uint32_t) * nq));
-      s.res_cap = need;
-      s.res_cap_q = nq;
-    }
-  }
+  if (host_out) SDB_CUDA(s.res.reserve((size_t)nq * (k ? k : 1), nq));
   return SDB_OK;
 }
 
@@ -235,7 +202,7 @@ struct PeerTable {
   uint8_t* base[MAX_P2P_RANKS];
 };
 struct Arena {
-  uint8_t* base = nullptr;  // this rank's arena (cudaMalloc: IPC-exportable)
+  DevBuf<uint8_t> base;     // this rank's arena (plain device memory: IPC-exportable)
   size_t block_cap = 0;     // bytes reserved per (slot, rank) block
   size_t flags_off = 0, acks_off = 0, ctr_off = 0, err_off = 0, bytes = 0;
   int nranks = 0;
@@ -347,8 +314,7 @@ static void arena_unmap(Arena* a, int self) {
 // (re)allocate this rank's arena for blocks of `need` bytes; the peers are mapped by the callers below
 static sdb_status arena_alloc_local(Corpus* c, Arena* a, size_t need) {
   const int R = c->ctx->comm->nranks;
-  cudaFree(a->base);
-  a->base = nullptr;
+  a->base.reset();
   a->block_cap = (need + 65535) / 65536 * 65536;
   a->nranks = R;
   const size_t gather_bytes = (size_t)N_TICKETS * R * a->block_cap;
@@ -357,7 +323,7 @@ static sdb_status arena_alloc_local(Corpus* c, Arena* a, size_t need) {
   a->ctr_off = a->acks_off + 256 * ((sizeof(uint32_t) * N_TICKETS * R + 255) / 256);
   a->err_off = a->ctr_off + 256 * ((sizeof(uint32_t) * N_TICKETS * R + 255) / 256);
   a->bytes = a->err_off + 256;
-  SDB_CUDA(cudaMalloc(&a->base, a->bytes));
+  SDB_CUDA(a->base.reserve(a->bytes));
   SDB_CUDA(cudaMemset(a->base, 0, a->bytes));
   SDB_CUDA(cudaDeviceSynchronize());
   a->seq = 0;
@@ -387,22 +353,18 @@ static sdb_status arena_ensure_ipc(Corpus* c, ShardState* ss, size_t need) {
     cudaGetLastError();
     good = 0;
   }
-  uint8_t* d_h = nullptr;
-  SDB_CUDA(cudaMalloc(&d_h, sizeof(cudaIpcMemHandle_t) * (R + 1) + 16));
+  DevBuf<uint8_t> d_h;
+  SDB_CUDA(d_h.reserve(sizeof(cudaIpcMemHandle_t) * (R + 1) + 16));
   std::vector<cudaIpcMemHandle_t> all((size_t)R);
   cudaStream_t st = ctx->stream;
-  auto bail = [&](sdb_status rc) {
-    cudaFree(d_h);
-    return rc;
-  };
-  if (cudaMemcpyAsync(d_h + sizeof(mine) * R, &mine, sizeof(mine), cudaMemcpyHostToDevice, st) != cudaSuccess) return bail(SDB_ECUDA);
+  if (cudaMemcpyAsync(d_h + sizeof(mine) * R, &mine, sizeof(mine), cudaMemcpyHostToDevice, st) != cudaSuccess) return SDB_ECUDA;
   if (g_nccl.AllGather(d_h + sizeof(mine) * R, d_h, sizeof(mine), ncclChar, cm->comm, st) != ncclSuccess) {
     set_error("exchange arena: ncclAllGather of the IPC handles failed");
-    return bail(SDB_ENCCL);
+    return SDB_ENCCL;
   }
   if (cudaMemcpyAsync(all.data(), d_h, sizeof(mine) * R, cudaMemcpyDeviceToHost, st) != cudaSuccess ||
       cudaStreamSynchronize(st) != cudaSuccess)
-    return bail(SDB_ECUDA);
+    return SDB_ECUDA;
   if (good) {
     for (int r = 0; r < R && good; r++) {
       if (r == cm->rank) {
@@ -421,15 +383,15 @@ static sdb_status arena_ensure_ipc(Corpus* c, ShardState* ss, size_t need) {
   }
   // unanimous?
   uint32_t* d_flag = reinterpret_cast<uint32_t*>(d_h + sizeof(mine) * (R + 1));
-  if (cudaMemcpyAsync(d_flag, &good, 4, cudaMemcpyHostToDevice, st) != cudaSuccess) return bail(SDB_ECUDA);
+  if (cudaMemcpyAsync(d_flag, &good, 4, cudaMemcpyHostToDevice, st) != cudaSuccess) return SDB_ECUDA;
   if (g_nccl.AllReduce(d_flag, d_flag, 1, ncclUint32, ncclMin, cm->comm, st) != ncclSuccess) {
     set_error("exchange arena: ncclAllReduce failed");
-    return bail(SDB_ENCCL);
+    return SDB_ENCCL;
   }
   uint32_t all_good = 0;
   if (cudaMemcpyAsync(&all_good, d_flag, 4, cudaMemcpyDeviceToHost, st) != cudaSuccess || cudaStreamSynchronize(st) != cudaSuccess)
-    return bail(SDB_ECUDA);
-  cudaFree(d_h);
+    return SDB_ECUDA;
+  d_h.reset();
   if (all_good) {
     a->ok = true;
     a->failed_need = 0;
@@ -506,18 +468,10 @@ void comm_corpus_released(Corpus* c) {
       }
   }
   if (!ss) return;
-  for (ShardSlot& s : ss->slots) {
-    cudaFree(s.d_block);
-    cudaFree(s.d_gather);
-    cudaFree(s.d_res_rows);
-    cudaFree(s.d_res_dist);
-    cudaFree(s.d_res_count);
-    if (s.h_hdr) cudaFreeHost(s.h_hdr);
+  for (ShardSlot& s : ss->slots)
     if (s.ev_done) cudaEventDestroy(s.ev_done);
-  }
   if (ss->arena) {
     arena_unmap(ss->arena, c->ctx->comm ? c->ctx->comm->rank : 0);
-    cudaFree(ss->arena->base);
     delete ss->arena;
   }
   delete ss;
@@ -568,9 +522,9 @@ sdb_status phase_local(Corpus* c, const double* d_queries, const double* h_queri
   const uint32_t* h_stat = knn_ticket_stat_host(c, ticket, &exact_only);
   if (exact_only) SDB_CUDA(cudaMemcpyAsync(s.d_block + bl.off_hdr, h_stat, 16, cudaMemcpyHostToDevice, st));
   else SDB_CUDA(cudaMemcpyAsync(s.d_block + bl.off_hdr, c->d_stat, 16, cudaMemcpyDeviceToDevice, st));
-  s.d_out_rows = host_out ? s.d_res_rows : d_out_rows;
-  s.d_out_dist = host_out ? s.d_res_dist : d_out_dist;
-  s.d_out_count = host_out ? s.d_res_count : d_out_count;
+  s.d_out_rows = host_out ? s.res.rows : d_out_rows;
+  s.d_out_dist = host_out ? s.res.dist : d_out_dist;
+  s.d_out_count = host_out ? s.res.count : d_out_count;
   s.h_out_rows = h_out_rows;
   s.h_out_dist = h_out_dist;
   s.h_out_count = h_out_count;
@@ -606,7 +560,7 @@ sdb_status phase_gather(const Pending& p) {
     if (S > 16) S = 16;
     if (S < 1) S = 1;
     const size_t ctr_off = a->ctr_off + sizeof(uint32_t) * ((size_t)p.slot * R);
-    exch_push_kernel<<<dim3((unsigned)R, S), 256, 0, st>>>(a->peers, a->base, reinterpret_cast<const uint4*>(s.d_block), n16,
+    exch_push_kernel<<<dim3((unsigned)R, S), 256, 0, st>>>(a->peers, a->base, reinterpret_cast<const uint4*>(s.d_block.get()), n16,
                                                             gather_off, flag_off, ack_off, ctr_off, a->err_off, need_ack, seq);
     exch_wait_kernel<<<1, 32, 0, st>>>(a->base, a->flags_off + sizeof(uint32_t) * ((size_t)p.slot * R), a->err_off, R, seq);
     SDB_CUDA(cudaGetLastError());
@@ -888,9 +842,9 @@ sdb_status sdb_knn_sharded_multi(sdb_corpus* const* shards, int n, const double*
       if (rc == SDB_OK) {
         ShardSlot& s = *ps[i].s;
         rc = slot_reserve(shards[i], s, nq, k, true);
-        s.d_out_rows = s.d_res_rows;
-        s.d_out_dist = s.d_res_dist;
-        s.d_out_count = s.d_res_count;
+        s.d_out_rows = s.res.rows;
+        s.d_out_dist = s.res.dist;
+        s.d_out_count = s.res.count;
       }
     }
     if (rc == SDB_OK) started++;

@@ -205,7 +205,7 @@ __global__ void or_mask_kernel(uint8_t* __restrict__ dst, const uint8_t* __restr
 sdb_status corpus_reapply_tombstones(Corpus* c, cudaStream_t st) {  // after the caller replaced the skip mask
   if (!c->d_removed || !c->n) return SDB_OK;
   if (!c->d_skip) {
-    SDB_CUDA(cudaMalloc(&c->d_skip, c->cap));
+    SDB_CUDA(c->d_skip.reserve(c->cap));
     SDB_CUDA(cudaMemsetAsync(c->d_skip, 0, c->cap, st));
   }
   or_mask_kernel<<<(unsigned)((c->n + 255) / 256), 256, 0, st>>>(c->d_skip, c->d_removed, c->n);
@@ -232,20 +232,20 @@ sdb_status corpus_remove_device(Corpus* c, const uint64_t* h_ids, uint64_t n) {
   Ctx* ctx = c->ctx;
   cudaStream_t st = ctx->stream;
   if (!c->d_skip) {
-    SDB_CUDA(cudaMalloc(&c->d_skip, c->cap));
+    SDB_CUDA(c->d_skip.reserve(c->cap));
     SDB_CUDA(cudaMemsetAsync(c->d_skip, 0, c->cap, st));
   }
   if (!c->d_removed) {
-    SDB_CUDA(cudaMalloc(&c->d_removed, c->cap));
+    SDB_CUDA(c->d_removed.reserve(c->cap));
     SDB_CUDA(cudaMemsetAsync(c->d_removed, 0, c->cap, st));
   }
-  uint64_t* d_ids = nullptr;
-  SDB_CUDA(cudaMallocAsync(&d_ids, sizeof(uint64_t) * n, st));
+  AsyncBuf<uint64_t> d_ids;
+  SDB_CUDA(d_ids.reserve(n, st));
   SDB_CUDA(cudaMemcpyAsync(d_ids, h_ids, sizeof(uint64_t) * n, cudaMemcpyHostToDevice, st));
-  remove_rows_kernel<<<(unsigned)((n * 32 + 255) / 256), 256, 0, st>>>(d_ids, n, c->d_skip, c->d_removed, c->finalized ? c->d_snorm : nullptr,
-                                                                       c->finalized ? c->d_i8 : nullptr, c->dim_pad8);
+  remove_rows_kernel<<<(unsigned)((n * 32 + 255) / 256), 256, 0, st>>>(d_ids, n, c->d_skip, c->d_removed, c->finalized ? c->d_snorm.get() : nullptr,
+                                                                       c->finalized ? c->d_i8.get() : nullptr, c->dim_pad8);
   count_launch(ctx);
-  SDB_CUDA(cudaFreeAsync(d_ids, st));
+  d_ids.reset();
   if (c->finalized && c->n_special) {  // a removed special row leaves the always-exact list
     std::vector<uint32_t> sp(c->n_special);
     SDB_CUDA(cudaMemcpyAsync(sp.data(), c->d_special, sizeof(uint32_t) * c->n_special, cudaMemcpyDeviceToHost, st));
@@ -269,10 +269,10 @@ sdb_status corpus_remove_device(Corpus* c, const uint64_t* h_ids, uint64_t n) {
 sdb_status corpus_finalize_device(Corpus* c) {
   Ctx* ctx = c->ctx;
   cudaStream_t st = ctx->stream;
-  uint32_t* d_tmp = nullptr;  // [0] special count, [1] max-norm bits, [2] max relative int8 error bits, [3] int8 gmax
-  SDB_CUDA(cudaMalloc(&d_tmp, 32));                                       // [4] max relative bf16 residual bits
+  DevBuf<uint32_t> d_tmp;  // [0] special count, [1] max-norm bits, [2] max relative int8 error bits, [3] int8 gmax
+  SDB_CUDA(d_tmp.reserve(8));                                            // [4] max relative bf16 residual bits
   SDB_CUDA(cudaMemsetAsync(d_tmp, 0, 32, st));
-  if (!c->d_special) SDB_CUDA(cudaMalloc(&c->d_special, sizeof(uint32_t) * SPECIAL_CAP));
+  SDB_CUDA(c->d_special.reserve(SPECIAL_CAP));
   {
     const uint64_t n_pad = (c->n + TILE_ROWS - 1) / TILE_ROWS * TILE_ROWS;
     if (n_pad > c->n) {
@@ -283,18 +283,18 @@ sdb_status corpus_finalize_device(Corpus* c) {
   if (c->n) {
     const int grid = ctx->sm_count * 8;
     if (c->dtype == SDB_F32)
-      finalize_rows_kernel<float, 8><<<grid, 256, 0, st>>>((const float*)c->d_rows, c->dim, c->n, (int)c->metric,
+      finalize_rows_kernel<float, 8><<<grid, 256, 0, st>>>((const float*)c->d_rows.get(), c->dim, c->n, (int)c->metric,
                                                         c->d_skip, c->d_mag, c->d_snorm, c->d_special, d_tmp,
                                                         d_tmp + 1);
     else
-      finalize_rows_kernel<double, 4><<<grid * 2, 128, 0, st>>>((const double*)c->d_rows, c->dim, c->n, (int)c->metric,
+      finalize_rows_kernel<double, 4><<<grid * 2, 128, 0, st>>>((const double*)c->d_rows.get(), c->dim, c->n, (int)c->metric,
                                                          c->d_skip, c->d_mag, c->d_snorm, c->d_special, d_tmp,
                                                          d_tmp + 1);
     count_launch(ctx);
     SDB_CUDA(cudaGetLastError());
     if (c->dtype == SDB_F32 && c->d_bf16) {
       const uint64_t n_pad = (c->n + TILE_ROWS - 1) / TILE_ROWS * TILE_ROWS;
-      to_bf16_kernel<<<ctx->sm_count * 16, 256, 0, st>>>((const float*)c->d_rows, c->dim, c->dim_pad, c->n, n_pad,
+      to_bf16_kernel<<<ctx->sm_count * 16, 256, 0, st>>>((const float*)c->d_rows.get(), c->dim, c->dim_pad, c->n, n_pad,
                                                          c->d_mag, c->d_snorm, c->d_bf16, d_tmp + 4);
       count_launch(ctx);
       SDB_CUDA(cudaGetLastError());
@@ -303,12 +303,12 @@ sdb_status corpus_finalize_device(Corpus* c) {
   c->n_outliers = 0;
   if (c->n && c->dtype == SDB_F32 && c->d_i8 && c->metric == SDB_COSINE) {
     const uint64_t n_pad = (c->n + TILE_ROWS - 1) / TILE_ROWS * TILE_ROWS;
-    float* d_rmax = nullptr;
-    uint32_t* d_hist = nullptr;
-    SDB_CUDA(cudaMallocAsync(&d_rmax, sizeof(float) * c->n, st));
-    SDB_CUDA(cudaMallocAsync(&d_hist, sizeof(uint32_t) * RMAX_BINS, st));
+    AsyncBuf<float> d_rmax;
+    AsyncBuf<uint32_t> d_hist;
+    SDB_CUDA(d_rmax.reserve(c->n, st));
+    SDB_CUDA(d_hist.reserve(RMAX_BINS, st));
     SDB_CUDA(cudaMemsetAsync(d_hist, 0, sizeof(uint32_t) * RMAX_BINS, st));
-    quantize_scan_kernel<<<ctx->sm_count * 8, 256, 0, st>>>((const float*)c->d_rows, c->dim, c->n, c->d_mag, c->d_snorm,
+    quantize_scan_kernel<<<ctx->sm_count * 8, 256, 0, st>>>((const float*)c->d_rows.get(), c->dim, c->n, c->d_mag, c->d_snorm,
                                                             d_tmp + 3, d_rmax, d_hist);
     count_launch(ctx);
     // ---- pick the scale: if at most 64 rows sit far above the rest (their largest normalised component is more
@@ -360,17 +360,14 @@ sdb_status corpus_finalize_device(Corpus* c) {
         }
       }
     }
-    quantize_rows_kernel<<<ctx->sm_count * 8, 256, 0, st>>>((const float*)c->d_rows, c->dim, c->dim_pad8, c->n, n_pad,
+    quantize_rows_kernel<<<ctx->sm_count * 8, 256, 0, st>>>((const float*)c->d_rows.get(), c->dim, c->dim_pad8, c->n, n_pad,
                                                             c->d_mag, c->d_snorm, d_tmp + 3, c->d_i8, d_tmp + 2);
     count_launch(ctx);
-    SDB_CUDA(cudaFreeAsync(d_rmax, st));
-    SDB_CUDA(cudaFreeAsync(d_hist, st));
     SDB_CUDA(cudaGetLastError());
   }
   uint32_t h[8] = {0, 0, 0, 0, 0, 0, 0, 0};
   SDB_CUDA(cudaMemcpyAsync(h, d_tmp, 32, cudaMemcpyDeviceToHost, st));
   SDB_CUDA(cudaStreamSynchronize(st));
-  SDB_CUDA(cudaFree(d_tmp));
   c->special_overflow = h[0] > (uint32_t)SPECIAL_CAP;
   c->n_special = h[0] > (uint32_t)SPECIAL_CAP ? (uint32_t)SPECIAL_CAP : h[0];
   float mn;

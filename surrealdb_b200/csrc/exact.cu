@@ -210,16 +210,15 @@ __global__ void __launch_bounds__(128) jaccard_keys_kernel(const T* __restrict__
 }
 static sdb_status jaccard_launch(Corpus* c, const double* d_q64, uint64_t* d_keys, double* d_vals, cudaStream_t st) {
   Ctx* ctx = c->ctx;
-  uint8_t* d_dup = nullptr;
-  SDB_CUDA(cudaMallocAsync(&d_dup, c->dim, st));
+  AsyncBuf<uint8_t> d_dup;
+  SDB_CUDA(d_dup.reserve(c->dim, st));
   jaccard_qdup_kernel<<<(c->dim + 127) / 128, 128, 0, st>>>(d_q64, c->dim, d_dup);
   const int grid = ctx->sm_count * 16;
   if (c->dtype == SDB_F32)
-    jaccard_keys_kernel<float><<<grid, 128, 0, st>>>((const float*)c->d_rows, c->dim, c->n, c->d_skip, d_q64, d_dup, d_keys, d_vals);
+    jaccard_keys_kernel<float><<<grid, 128, 0, st>>>((const float*)c->d_rows.get(), c->dim, c->n, c->d_skip, d_q64, d_dup, d_keys, d_vals);
   else
-    jaccard_keys_kernel<double><<<grid, 128, 0, st>>>((const double*)c->d_rows, c->dim, c->n, c->d_skip, d_q64, d_dup, d_keys, d_vals);
+    jaccard_keys_kernel<double><<<grid, 128, 0, st>>>((const double*)c->d_rows.get(), c->dim, c->n, c->d_skip, d_q64, d_dup, d_keys, d_vals);
   count_launch(ctx, 2);
-  SDB_CUDA(cudaFreeAsync(d_dup, st));
   SDB_CUDA(cudaGetLastError());
   return SDB_OK;
 }
@@ -369,26 +368,19 @@ sdb_status exact_query(Corpus* c, const double* d_q64, const double* d_qmag, con
                        uint64_t row_base, uint64_t* d_out_rows, double* d_out_dist, uint32_t* d_out_count,
                        cudaStream_t st) {
   Ctx* ctx = c->ctx;
-  if (c->ex_cap < c->n || !c->d_ex_key) {
-    cudaFree(c->d_ex_key);
-    cudaFree(c->d_ex_val);
-    cudaFree(c->d_sel);
-    c->d_ex_key = nullptr;
-    c->d_ex_val = nullptr;
-    c->d_sel = nullptr;
+  {
     const uint64_t cap = c->cap > c->n ? c->cap : c->n;
-    SDB_CUDA(cudaMalloc(&c->d_ex_key, sizeof(uint64_t) * (cap ? cap : 1)));
-    SDB_CUDA(cudaMalloc(&c->d_ex_val, sizeof(double) * (cap ? cap : 1)));
+    SDB_CUDA(c->d_ex_key.reserve(cap ? cap : 1));
+    SDB_CUDA(c->d_ex_val.reserve(cap ? cap : 1));
     // SelState + gather buffers (key u64[4096], row u32[4096])
-    SDB_CUDA(cudaMalloc(&c->d_sel, sizeof(SelState) + 4096 * 12 + 64));
-    c->ex_cap = cap;
+    SDB_CUDA(c->d_sel.reserve((sizeof(SelState) + 4096 * 12 + 64) / sizeof(uint32_t)));
   }
   if (k > 4096) {
     set_error("exact path supports k <= 4096 (got %u)", k);
     return SDB_EUNSUPPORTED;
   }
-  SelState* sel = reinterpret_cast<SelState*>(c->d_sel);
-  uint64_t* g_key = reinterpret_cast<uint64_t*>(reinterpret_cast<char*>(c->d_sel) + ((sizeof(SelState) + 63) / 64) * 64);
+  SelState* sel = reinterpret_cast<SelState*>(c->d_sel.get());
+  uint64_t* g_key = reinterpret_cast<uint64_t*>(reinterpret_cast<char*>(c->d_sel.get()) + ((sizeof(SelState) + 63) / 64) * 64);
   uint32_t* g_row = reinterpret_cast<uint32_t*>(g_key + 4096);
   const uint64_t n = c->n;
   if (n && c->metric == SDB_JACCARD) {
@@ -396,10 +388,10 @@ sdb_status exact_query(Corpus* c, const double* d_q64, const double* d_qmag, con
   } else if (n) {
     const int grid = ctx->sm_count * 8;
     if (c->dtype == SDB_F32)
-      exact_keys_kernel<float, 4><<<grid, 128, 0, st>>>((const float*)c->d_rows, c->dim, n, (int)c->metric, c->d_mag,
+      exact_keys_kernel<float, 4><<<grid, 128, 0, st>>>((const float*)c->d_rows.get(), c->dim, n, (int)c->metric, c->d_mag,
                                                         c->d_skip, d_q64, d_qmag, d_qflags, c->d_ex_key, c->d_ex_val, c->minkowski_p);
     else
-      exact_keys_kernel<double, 4><<<grid, 128, 0, st>>>((const double*)c->d_rows, c->dim, n, (int)c->metric,
+      exact_keys_kernel<double, 4><<<grid, 128, 0, st>>>((const double*)c->d_rows.get(), c->dim, n, (int)c->metric,
                                                          c->d_mag, c->d_skip, d_q64, d_qmag, d_qflags, c->d_ex_key,
                                                          c->d_ex_val, c->minkowski_p);
     count_launch(ctx);
@@ -431,10 +423,10 @@ sdb_status exact_project(Corpus* c, int fn, double* d_vals, cudaStream_t st) {
   if (fn == SDB_JACCARD) return jaccard_launch(c, c->d_q64, nullptr, d_vals, st);
   const int grid = ctx->sm_count * 8;
   if (c->dtype == SDB_F32)
-    exact_keys_kernel<float, 4><<<grid, 128, 0, st>>>((const float*)c->d_rows, c->dim, n, fn, c->d_mag, c->d_skip,
+    exact_keys_kernel<float, 4><<<grid, 128, 0, st>>>((const float*)c->d_rows.get(), c->dim, n, fn, c->d_mag, c->d_skip,
                                                       c->d_q64, c->d_qmag, c->d_qflags, nullptr, d_vals, c->minkowski_p);
   else
-    exact_keys_kernel<double, 4><<<grid, 128, 0, st>>>((const double*)c->d_rows, c->dim, n, fn, c->d_mag, c->d_skip,
+    exact_keys_kernel<double, 4><<<grid, 128, 0, st>>>((const double*)c->d_rows.get(), c->dim, n, fn, c->d_mag, c->d_skip,
                                                        c->d_q64, c->d_qmag, c->d_qflags, nullptr, d_vals, c->minkowski_p);
   count_launch(ctx);
   SDB_CUDA(cudaGetLastError());

@@ -17,18 +17,17 @@ namespace sdb {
 struct Graph {
   Ctx* ctx = nullptr;
   uint64_t n_rows = 0, n_edges = 0;
-  uint64_t* d_row_ptr = nullptr;
-  uint32_t* d_col_idx = nullptr;
+  DevBuf<uint64_t> d_row_ptr;
+  DevBuf<uint32_t> d_col_idx;
   bool targets_in_rows = true;  // every col_idx < n_rows (required by +collect, which indexes per-row state by target)
   // row-sharded adjacency (SURVEY 8e): this rank holds rows [row_lo, row_hi) of the n_rows-row CSR; d_row_ptr is the
   // slice rebased to 0.  An unsharded graph is the shard [0, n_rows).
   uint64_t row_lo = 0, row_hi = 0;
   bool sharded = false;
   // +collect state, kept between calls (a 50M-node graph needs 450 MB of it: allocating it per call cost 145 ms)
-  uint8_t* d_seen = nullptr;
-  uint32_t* d_first = nullptr;
-  uint32_t* d_res = nullptr;
-  uint64_t res_cap = 0;
+  DevBuf<uint8_t> d_seen;
+  DevBuf<uint32_t> d_first;
+  DevBuf<uint32_t> d_res;
   std::mutex mu;
 };
 
@@ -92,8 +91,8 @@ sdb_status exclusive_scan(Ctx* ctx, const uint64_t* d_in, uint64_t* d_out, uint6
     return SDB_OK;
   }
   const uint64_t tiles = (n + SCAN_TILE - 1) / SCAN_TILE;
-  uint64_t* d_sums = nullptr;
-  SDB_CUDA(cudaMallocAsync(&d_sums, sizeof(uint64_t) * (tiles + 1), st));
+  AsyncBuf<uint64_t> d_sums;
+  SDB_CUDA(d_sums.reserve(tiles + 1, st));
   scan_tile_kernel<<<(unsigned)tiles, SCAN_THREADS, 0, st>>>(d_in, d_out, n, d_sums);
   count_launch(ctx);
   if (tiles > 1) {
@@ -103,7 +102,6 @@ sdb_status exclusive_scan(Ctx* ctx, const uint64_t* d_in, uint64_t* d_out, uint6
   } else {
     SDB_CUDA(cudaMemcpyAsync(d_total, d_sums, 8, cudaMemcpyDeviceToDevice, st));
   }
-  SDB_CUDA(cudaFreeAsync(d_sums, st));
   SDB_CUDA(cudaGetLastError());
   return SDB_OK;
 }
@@ -196,18 +194,17 @@ __global__ void __launch_bounds__(EXP_THREADS) expand_kernel(const uint64_t* __r
   }
 }
 
-static sdb_status hop_device(Graph* g, const uint32_t* d_frontier, uint64_t n_f, uint32_t limit, uint32_t** d_out,
+// *d_out: an empty buffer, which receives the next frontier (stays empty when it has no elements)
+static sdb_status hop_device(Graph* g, const uint32_t* d_frontier, uint64_t n_f, uint32_t limit, AsyncBuf<uint32_t>* d_out,
                              uint64_t* n_out, cudaStream_t st) {
   Ctx* ctx = g->ctx;
-  *d_out = nullptr;
   *n_out = 0;
   if (n_f == 0) return SDB_OK;
-  uint64_t* d_off = nullptr;
-  uint64_t* d_total = nullptr;
-  uint32_t* d_err = nullptr;
-  SDB_CUDA(cudaMallocAsync(&d_off, sizeof(uint64_t) * (n_f + 2), st));
-  d_total = d_off + n_f;  // off[n_f] = total: exactly the sentinel the expand kernel wants
-  SDB_CUDA(cudaMallocAsync(&d_err, 4, st));
+  AsyncBuf<uint64_t> d_off;
+  AsyncBuf<uint32_t> d_err;
+  SDB_CUDA(d_off.reserve(n_f + 2, st));
+  uint64_t* d_total = d_off + n_f;  // off[n_f] = total: exactly the sentinel the expand kernel wants
+  SDB_CUDA(d_err.reserve(1, st));
   SDB_CUDA(cudaMemsetAsync(d_err, 0, 4, st));
   degree_kernel<<<(unsigned)((n_f + 255) / 256), 256, 0, st>>>(g->d_row_ptr, g->n_rows, g->row_lo, g->row_hi, d_frontier, n_f,
                                                                limit, d_off, d_err);
@@ -222,19 +219,15 @@ static sdb_status hop_device(Graph* g, const uint32_t* d_frontier, uint64_t n_f,
   SDB_CUDA(cudaMemcpyAsync(&err, d_err, 4, cudaMemcpyDeviceToHost, st));
   SDB_CUDA(cudaStreamSynchronize(st));
   if (err) {
-    cudaFreeAsync(d_off, st);
-    cudaFreeAsync(d_err, st);
     set_error("graph expand: frontier id out of range (graph has %llu rows)", (unsigned long long)g->n_rows);
     return SDB_EINVAL;
   }
   if (total > 0xFFFFFFF0ull) {
-    cudaFreeAsync(d_off, st);
-    cudaFreeAsync(d_err, st);
     set_error("graph expand: %llu results exceed the 2^32 frontier limit", (unsigned long long)total);
     return SDB_EOVERFLOW;
   }
   if (total) {
-    SDB_CUDA(cudaMallocAsync(d_out, sizeof(uint32_t) * total, st));
+    SDB_CUDA(d_out->reserve(total, st));
     if (multi) SDB_CUDA(cudaMemsetAsync(*d_out, 0, sizeof(uint32_t) * total, st));
     expand_kernel<<<(unsigned)((total + EXP_TILE - 1) / EXP_TILE), EXP_THREADS, 0, st>>>(
         g->d_row_ptr, g->d_col_idx, d_frontier, n_f, d_off, total, *d_out, g->row_lo, g->row_hi);
@@ -243,8 +236,6 @@ static sdb_status hop_device(Graph* g, const uint32_t* d_frontier, uint64_t n_f,
     // ranks IS the next frontier, in the reference's order, on every rank -- ONE exchange per hop
     if (multi) SDB_TRY(comm_allreduce_sum(ctx, *d_out, total, 4, st));
   }
-  SDB_CUDA(cudaFreeAsync(d_off, st));
-  SDB_CUDA(cudaFreeAsync(d_err, st));
   SDB_CUDA(cudaGetLastError());
   *n_out = total;
   return SDB_OK;
@@ -285,6 +276,11 @@ __global__ void collect_compact_kernel(const uint32_t* __restrict__ lvl, uint64_
 struct sdb_graph : sdb::Graph {};
 using namespace sdb;
 
+// the context's pinned staging buffer, grown to `bytes` (nullptr if that fails: the caller copies without it)
+static uint8_t* stage_buffer(Ctx* ctx, size_t bytes) {
+  return ctx->h_stage.reserve(bytes) == cudaSuccess ? ctx->h_stage.get() : nullptr;
+}
+
 extern "C" {
 
 void sdb_graph_destroy(sdb_graph* g);
@@ -314,8 +310,8 @@ static sdb_status graph_load(sdb_ctx* ctx, uint64_t n_rows, uint64_t row_lo, uin
   g->row_lo = row_lo;
   g->row_hi = row_hi;
   g->sharded = sharded;
-  cudaError_t e = cudaMalloc(&g->d_row_ptr, sizeof(uint64_t) * (n_local + 1));
-  if (e == cudaSuccess) e = cudaMalloc(&g->d_col_idx, sizeof(uint32_t) * (n_edges ? n_edges : 1));
+  cudaError_t e = g->d_row_ptr.reserve(n_local + 1);
+  if (e == cudaSuccess) e = g->d_col_idx.reserve(n_edges ? n_edges : 1);
   if (e != cudaSuccess) {
     set_error("graph allocation failed: %s", cudaGetErrorString(e));
     sdb_graph_destroy(g);
@@ -352,49 +348,32 @@ sdb_status sdb_graph_load_csr_shard(sdb_ctx* ctx, uint64_t n_rows_total, uint64_
 void sdb_graph_destroy(sdb_graph* g) {
   if (!g) return;
   cudaSetDevice(g->ctx->device);
-  cudaFree(g->d_row_ptr);
-  cudaFree(g->d_col_idx);
-  cudaFree(g->d_seen);
-  cudaFree(g->d_first);
-  cudaFree(g->d_res);
   delete g;
 }
 
-// device-resident core: frontier and result stay in HBM (the result is library-owned: sdb_device_free)
+// device-resident core: frontier and result stay in HBM (sdb_graph_expand_device hands the result to the caller)
 static sdb_status graph_expand_dev(sdb_graph* const* hops, uint32_t n_hops, const uint32_t* d_frontier, uint64_t n_frontier,
-                                   uint32_t per_source_limit, uint32_t** d_out, uint64_t* out_n, cudaStream_t st) {
-  uint32_t* d_f = nullptr;
+                                   uint32_t per_source_limit, AsyncBuf<uint32_t>* d_out, uint64_t* out_n, cudaStream_t st) {
+  AsyncBuf<uint32_t> d_f;
   uint64_t n_f = n_frontier;
   bool owned = false;  // the caller's frontier is never freed
-  const uint32_t* cur = d_frontier;
   for (uint32_t h = 0; h < n_hops && n_f; h++) {
-    uint32_t* d_next = nullptr;
+    AsyncBuf<uint32_t> d_next;
     uint64_t n_next = 0;
     if (ctx_cancelled(hops[h]->ctx)) {  // polled once per hop
-      if (owned) cudaFreeAsync(d_f, st);
       set_error("query cancelled");
       return SDB_ECANCELLED;
     }
-    sdb_status s = hop_device(hops[h], cur, n_f, per_source_limit, &d_next, &n_next, st);
-    if (owned) cudaFreeAsync(d_f, st);
-    if (s != SDB_OK) {
-      if (d_next) cudaFreeAsync(d_next, st);
-      return s;
-    }
-    d_f = d_next;
-    cur = d_next;
+    SDB_TRY(hop_device(hops[h], owned ? d_f.get() : d_frontier, n_f, per_source_limit, &d_next, &n_next, st));
+    d_f = std::move(d_next);
     owned = true;
     n_f = n_next;
   }
   if (!owned && n_f) {  // zero hops: hand back a copy
-    SDB_CUDA(cudaMallocAsync(&d_f, sizeof(uint32_t) * n_f, st));
+    SDB_CUDA(d_f.reserve(n_f, st));
     SDB_CUDA(cudaMemcpyAsync(d_f, d_frontier, sizeof(uint32_t) * n_f, cudaMemcpyDeviceToDevice, st));
   }
-  if (n_f == 0 && owned && d_f) {
-    cudaFreeAsync(d_f, st);
-    d_f = nullptr;
-  }
-  *d_out = n_f ? d_f : nullptr;
+  *d_out = std::move(d_f);
   *out_n = n_f;
   return SDB_OK;
 }
@@ -409,7 +388,9 @@ sdb_status sdb_graph_expand_device(sdb_graph* const* hops, uint32_t n_hops, cons
   Ctx* ctx = hops[0]->ctx;
   std::lock_guard<std::mutex> guard(ctx->mu);
   SDB_CUDA(cudaSetDevice(ctx->device));
-  SDB_TRY(graph_expand_dev(hops, n_hops, d_frontier, n_frontier, per_source_limit, d_out_ids, out_n, ctx->stream));
+  AsyncBuf<uint32_t> d_out;
+  SDB_TRY(graph_expand_dev(hops, n_hops, d_frontier, n_frontier, per_source_limit, &d_out, out_n, ctx->stream));
+  *d_out_ids = d_out.release();
   SDB_CUDA(cudaStreamSynchronize(ctx->stream));
   return SDB_OK;
 }
@@ -417,7 +398,7 @@ sdb_status sdb_graph_expand_device(sdb_graph* const* hops, uint32_t n_hops, cons
 void sdb_device_free(sdb_ctx* ctx, void* d_ptr) {
   if (!ctx || !d_ptr) return;
   cudaSetDevice(ctx->device);
-  cudaFreeAsync(d_ptr, ctx->stream);
+  AsyncBuf<uint32_t>::free_released(d_ptr, ctx->stream);
 }
 
 sdb_status sdb_graph_expand(sdb_graph* const* hops, uint32_t n_hops, const uint32_t* frontier, uint64_t n_frontier,
@@ -431,33 +412,24 @@ sdb_status sdb_graph_expand(sdb_graph* const* hops, uint32_t n_hops, const uint3
   std::lock_guard<std::mutex> guard(ctx->mu);
   SDB_CUDA(cudaSetDevice(ctx->device));
   cudaStream_t st = ctx->stream;
-  uint32_t* d_in = nullptr;
+  AsyncBuf<uint32_t> d_in;
   if (n_frontier) {
-    SDB_CUDA(cudaMallocAsync(&d_in, sizeof(uint32_t) * n_frontier, st));
+    SDB_CUDA(d_in.reserve(n_frontier, st));
     SDB_CUDA(cudaMemcpyAsync(d_in, frontier, sizeof(uint32_t) * n_frontier, cudaMemcpyHostToDevice, st));
   }
-  uint32_t* d_f = nullptr;
+  AsyncBuf<uint32_t> d_f;
   uint64_t n_f = 0;
-  sdb_status s = graph_expand_dev(hops, n_hops, d_in, n_frontier, per_source_limit, &d_f, &n_f, st);
-  if (d_in) cudaFreeAsync(d_in, st);
-  if (s != SDB_OK) return s;
+  SDB_TRY(graph_expand_dev(hops, n_hops, d_in, n_frontier, per_source_limit, &d_f, &n_f, st));
+  d_in.reset();
   if (n_f) {
     uint32_t* h_out = (uint32_t*)malloc(sizeof(uint32_t) * n_f);
-    if (!h_out) {
-      cudaFreeAsync(d_f, st);
-      return SDB_ENOMEM;
-    }
+    if (!h_out) return SDB_ENOMEM;
     // device -> pinned staging (full PCIe rate) -> caller-owned pageable buffer
     const size_t bytes = sizeof(uint32_t) * n_f;
-    if (ctx->h_stage_bytes < bytes) {
-      if (ctx->h_stage) cudaFreeHost(ctx->h_stage);
-      ctx->h_stage = nullptr;
-      ctx->h_stage_bytes = 0;
-      if (cudaHostAlloc(&ctx->h_stage, bytes, cudaHostAllocDefault) == cudaSuccess) ctx->h_stage_bytes = bytes;
-    }
-    void* dst = ctx->h_stage_bytes >= bytes ? ctx->h_stage : (void*)h_out;
+    void* dst = stage_buffer(ctx, bytes);
+    if (!dst) dst = h_out;
     SDB_CUDA(cudaMemcpyAsync(dst, d_f, bytes, cudaMemcpyDeviceToHost, st));
-    SDB_CUDA(cudaFreeAsync(d_f, st));
+    d_f.reset();
     SDB_CUDA(cudaStreamSynchronize(st));
     if (dst != (void*)h_out) memcpy(h_out, dst, bytes);
     *out_ids = h_out;
@@ -487,49 +459,26 @@ sdb_status sdb_graph_collect(sdb_graph* g, const uint32_t* start, uint64_t n_sta
       set_error("graph collect: start id out of range");
       return SDB_EINVAL;
     }
-  // stream-ordered temporaries are released on EVERY return path (ADVICE r1)
-  struct Temps {
+  // the stream-ordered temporaries below are released on every return path, then the stream is drained
+  struct Drain {
     cudaStream_t st;
-    std::vector<void*> ptrs;
-    ~Temps() {
-      for (void* p : ptrs)
-        if (p) cudaFreeAsync(p, st);
-      cudaStreamSynchronize(st);
-    }
-    void drop(void* p) {
-      for (auto& q : ptrs)
-        if (q == p) q = nullptr;
-      if (p) cudaFreeAsync(p, st);
-    }
-  } tmp{st, {}};
-  auto dalloc = [&](void** p, size_t bytes) -> sdb_status {
-    SDB_CUDA(cudaMallocAsync(p, bytes ? bytes : 1, st));
-    tmp.ptrs.push_back(*p);
-    return SDB_OK;
-  };
+    ~Drain() { cudaStreamSynchronize(st); }
+  } drain{st};
   const uint64_t nr = g->n_rows ? g->n_rows : 1;
-  uint8_t* d_seen = nullptr;
-  uint32_t *d_first = nullptr, *d_f = nullptr, *d_res = nullptr;
   // every node is emitted at most once (+ the start values): the result is accumulated on the device
   const uint64_t res_cap = g->n_rows + n_start;
-  if (!g->d_seen) SDB_CUDA(cudaMalloc(&g->d_seen, nr));
-  if (!g->d_first) SDB_CUDA(cudaMalloc(&g->d_first, sizeof(uint32_t) * nr));
-  if (g->res_cap < res_cap) {
-    cudaFree(g->d_res);
-    g->d_res = nullptr;
-    g->res_cap = 0;
-    SDB_CUDA(cudaMalloc(&g->d_res, sizeof(uint32_t) * (res_cap ? res_cap : 1)));
-    g->res_cap = res_cap;
-  }
-  d_seen = g->d_seen;
-  d_first = g->d_first;
-  d_res = g->d_res;
+  SDB_CUDA(g->d_seen.reserve(nr));
+  SDB_CUDA(g->d_first.reserve(nr));
+  SDB_CUDA(g->d_res.reserve(res_cap));
+  uint8_t* d_seen = g->d_seen;
+  uint32_t *d_first = g->d_first, *d_res = g->d_res;
+  AsyncBuf<uint32_t> d_f;
   uint64_t n_res = 0;
   SDB_CUDA(cudaMemsetAsync(d_seen, 0, nr, st));
   SDB_CUDA(cudaMemsetAsync(d_first, 0xFF, sizeof(uint32_t) * nr, st));
   uint64_t n_f = n_start;
   if (n_f) {
-    SDB_TRY(dalloc((void**)&d_f, sizeof(uint32_t) * n_f));
+    SDB_CUDA(d_f.reserve(n_f, st));
     SDB_CUDA(cudaMemcpyAsync(d_f, start, sizeof(uint32_t) * n_f, cudaMemcpyHostToDevice, st));
   }
   if (inclusive && n_start) {  // collect.rs:83-86: the start value is emitted and marked seen only when inclusive
@@ -546,16 +495,14 @@ sdb_status sdb_graph_collect(sdb_graph* g, const uint32_t* start, uint64_t n_sta
       set_error("query cancelled");
       return SDB_ECANCELLED;
     }
-    uint32_t* d_lvl = nullptr;
+    AsyncBuf<uint32_t> d_lvl;
     uint64_t n_lvl = 0;
     SDB_TRY(hop_device(g, d_f, n_f, 0, &d_lvl, &n_lvl, st));
-    tmp.ptrs.push_back(d_lvl);
-    tmp.drop(d_f);
-    d_f = nullptr;
+    d_f.reset();
     n_f = 0;
     if (n_lvl) {
-      uint64_t* d_pos = nullptr;
-      SDB_TRY(dalloc((void**)&d_pos, sizeof(uint64_t) * (n_lvl + 2)));
+      AsyncBuf<uint64_t> d_pos;
+      SDB_CUDA(d_pos.reserve(n_lvl + 2, st));
       const unsigned grid = (unsigned)((n_lvl + 255) / 256);
       collect_mark_kernel<<<grid, 256, 0, st>>>(d_lvl, n_lvl, d_seen, d_first);
       collect_flag_kernel<<<grid, 256, 0, st>>>(d_lvl, n_lvl, d_seen, d_first, d_pos);
@@ -565,7 +512,7 @@ sdb_status sdb_graph_collect(sdb_graph* g, const uint32_t* start, uint64_t n_sta
       SDB_CUDA(cudaMemcpyAsync(&n_next, d_pos + n_lvl, 8, cudaMemcpyDeviceToHost, st));
       SDB_CUDA(cudaStreamSynchronize(st));
       if (n_next) {
-        SDB_TRY(dalloc((void**)&d_f, sizeof(uint32_t) * n_next));
+        SDB_CUDA(d_f.reserve(n_next, st));
         collect_compact_kernel<<<grid, 256, 0, st>>>(d_lvl, n_lvl, d_pos, d_seen, d_first, d_f);
         count_launch(ctx);
         n_f = n_next;
@@ -578,9 +525,7 @@ sdb_status sdb_graph_collect(sdb_graph* g, const uint32_t* start, uint64_t n_sta
           n_res += n_next;
         }
       }
-      tmp.drop(d_pos);
     }
-    tmp.drop(d_lvl);
     depth++;
   }
   SDB_CUDA(cudaGetLastError());
@@ -590,18 +535,11 @@ sdb_status sdb_graph_collect(sdb_graph* g, const uint32_t* start, uint64_t n_sta
     // large results go through the context's pinned staging buffer (pageable D2H is several times slower)
     const size_t bytes = sizeof(uint32_t) * n_res;
     cudaError_t e = cudaSuccess;
-    if (bytes >= (1u << 20)) {
-      if (ctx->h_stage_bytes < bytes) {
-        if (ctx->h_stage) cudaFreeHost(ctx->h_stage);
-        ctx->h_stage = nullptr;
-        ctx->h_stage_bytes = 0;
-        if (cudaHostAlloc(&ctx->h_stage, bytes, cudaHostAllocDefault) == cudaSuccess) ctx->h_stage_bytes = bytes;
-      }
-    }
-    if (ctx->h_stage_bytes >= bytes && bytes >= (1u << 20)) {
-      e = cudaMemcpyAsync(ctx->h_stage, d_res, bytes, cudaMemcpyDeviceToHost, st);
+    uint8_t* stage = bytes >= (1u << 20) ? stage_buffer(ctx, bytes) : nullptr;
+    if (stage) {
+      e = cudaMemcpyAsync(stage, d_res, bytes, cudaMemcpyDeviceToHost, st);
       if (e == cudaSuccess) e = cudaStreamSynchronize(st);
-      if (e == cudaSuccess) memcpy(h_out, ctx->h_stage, bytes);
+      if (e == cudaSuccess) memcpy(h_out, stage, bytes);
     } else {
       e = cudaMemcpyAsync(h_out, d_res, bytes, cudaMemcpyDeviceToHost, st);
       if (e == cudaSuccess) e = cudaStreamSynchronize(st);

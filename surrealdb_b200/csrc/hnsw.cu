@@ -26,14 +26,17 @@
 
 namespace sdb {
 
-// Per-vector state of the metrics that carry it (vec_state_make); null where the metric needs none.
+// Per-vector state of the metrics that carry it (vec_state_make); null where the metric needs none.  K fixes how it is
+// allocated: an index's elements in device memory (Mem::Device), freed with the index; the queries or pending vectors of
+// one call from the stream's pool (Mem::Async), freed on the stream once the call's kernels are queued.
+template <Mem K>
 struct VecState {
-  double* norm = nullptr;      // COSINE: the vector's factor of the denominator: sqrt((double)sumsq) (F32, vector.rs:246),
-                               // sqrt of the 8-lane f64 sum of f64(x)^2 (the other types, vector.rs:238,257)
-  double* mean = nullptr;      // PEARSON: mean (in the type's arithmetic, widened) and sum of squared deviations
-  double* sx2 = nullptr;       // (vector.rs:412-451)
-  void* bits = nullptr;        // JACCARD: sorted distinct keys (JKey, dim-strided rows) ...
-  uint32_t* nbits = nullptr;   // ... and how many there are (vector.rs:316-356)
+  Buf<double, K> norm;      // COSINE: the vector's factor of the denominator: sqrt((double)sumsq) (F32, vector.rs:246),
+                            // sqrt of the 8-lane f64 sum of f64(x)^2 (the other types, vector.rs:238,257)
+  Buf<double, K> mean;      // PEARSON: mean (in the type's arithmetic, widened) and sum of squared deviations
+  Buf<double, K> sx2;       // (vector.rs:412-451)
+  Buf<char, K> bits;        // JACCARD: sorted distinct keys (JKey, dim-strided rows) ...
+  Buf<uint32_t, K> nbits;   // ... and how many there are (vector.rs:316-356)
 };
 
 struct Hnsw {
@@ -44,14 +47,17 @@ struct Hnsw {
   uint64_t n = 0;
   uint32_t n_layers = 0;
   int64_t entry = -1;
-  void* d_vec = nullptr;     // n x dim elements of type vt
+  void* d_vec = nullptr;     // n x dim elements of type vt (own_vec's, or the caller's for a borrowed handle)
   double minkowski_p = 3.0;  // order of SDB_MINKOWSKI (sdb_hnsw_set_minkowski_order)
-  VecState elems;            // the elements' metric state
-  std::vector<uint64_t*> rp;
+  VecState<Mem::Device> elems;  // the elements' metric state
+  std::vector<uint64_t*> rp;    // per layer CSR (own_rp / own_ci's, or the caller's for a borrowed handle)
   std::vector<uint32_t*> ci;
-  const uint64_t** d_rp = nullptr;
-  const uint32_t** d_ci = nullptr;
-  uint64_t* d_visited = nullptr;
+  DevBuf<char> own_vec;         // empty for a borrowed handle
+  std::vector<DevBuf<uint64_t>> own_rp;
+  std::vector<DevBuf<uint32_t>> own_ci;
+  DevBuf<const uint64_t*> d_rp;  // device tables of the rp / ci pointers
+  DevBuf<const uint32_t*> d_ci;
+  DevBuf<uint64_t> d_visited;
   uint32_t table_log2 = 0, n_tables = 0;
   uint32_t gen = 1;  // generations consumed so far (each warp uses gen_base + its own counter)
   bool borrowed = false;  // sdb_hnsw_load_device: vectors and CSR arrays belong to the caller
@@ -242,15 +248,13 @@ sdb_status jaccard_prepare(Ctx* ctx, const K* keys, uint64_t rows, uint32_t dim,
                            cudaStream_t st) {
   if (!rows) return SDB_OK;
   const uint64_t chunk = std::max<uint64_t>(1, std::min<uint64_t>(rows, (1u << 30) / dim));  // CUB counts items in int
-  int* d_off = nullptr;
-  void* d_tmp = nullptr;
+  AsyncBuf<int> d_off;
+  AsyncBuf<char> d_tmp;
   size_t tmp_bytes = 0;
-  if (cub::DeviceSegmentedSort::SortKeys(nullptr, tmp_bytes, keys, bits, (int)(chunk * dim), (int)chunk, d_off, d_off + 1,
-                                         st) != cudaSuccess)
+  if (cub::DeviceSegmentedSort::SortKeys(nullptr, tmp_bytes, keys, bits, (int)(chunk * dim), (int)chunk, d_off.get(),
+                                         d_off + 1, st) != cudaSuccess)
     return SDB_ECUDA;
-  if (cudaMallocAsync(&d_off, sizeof(int) * (chunk + 1), st) != cudaSuccess ||
-      cudaMallocAsync(&d_tmp, tmp_bytes ? tmp_bytes : 1, st) != cudaSuccess) {
-    if (d_off) cudaFreeAsync(d_off, st);
+  if (d_off.reserve(chunk + 1, st) != cudaSuccess || d_tmp.reserve(tmp_bytes ? tmp_bytes : 1, st) != cudaSuccess) {
     set_error("hnsw jaccard: %zu bytes of sort scratch could not be allocated", tmp_bytes + 4 * (chunk + 1));
     return SDB_ENOMEM;
   }
@@ -260,8 +264,8 @@ sdb_status jaccard_prepare(Ctx* ctx, const K* keys, uint64_t rows, uint32_t dim,
     segment_offsets_kernel<<<(nr + 256) / 256, 256, 0, st>>>(d_off, nr, dim);
     count_launch(ctx);
     size_t b = tmp_bytes;
-    if (cub::DeviceSegmentedSort::SortKeys(d_tmp, b, keys + r0 * dim, bits + r0 * dim, (int)(nr * dim), (int)nr, d_off,
-                                           d_off + 1, st) != cudaSuccess)
+    if (cub::DeviceSegmentedSort::SortKeys(d_tmp.get(), b, keys + r0 * dim, bits + r0 * dim, (int)(nr * dim), (int)nr,
+                                           d_off.get(), d_off + 1, st) != cudaSuccess)
       rc = SDB_ECUDA;
     count_launch(ctx);
   }
@@ -269,8 +273,6 @@ sdb_status jaccard_prepare(Ctx* ctx, const K* keys, uint64_t rows, uint32_t dim,
     distinct_sorted_kernel<<<(unsigned)((rows + 127) / 128), 128, 0, st>>>(bits, dim, rows, nbits);
     count_launch(ctx);
   }
-  cudaFreeAsync(d_tmp, st);
-  cudaFreeAsync(d_off, st);
   if (rc != SDB_OK) set_error("hnsw jaccard: segmented sort failed: %s", cudaGetErrorString(cudaGetLastError()));
   return rc;
 }
@@ -284,16 +286,14 @@ sdb_status jaccard_prepare_typed(Ctx* ctx, sdb_vector_type vt, const void* d_vec
   if (vt != SDB_VT_I16)
     return jaccard_prepare(ctx, static_cast<const uint32_t*>(d_vec), rows, dim, static_cast<uint32_t*>(bits), nbits, st);
   if (!rows) return SDB_OK;
-  uint32_t* keys = nullptr;
-  if (cudaMallocAsync(&keys, sizeof(uint32_t) * rows * dim, st) != cudaSuccess) {
+  AsyncBuf<uint32_t> keys;
+  if (keys.reserve(rows * dim, st) != cudaSuccess) {
     set_error("hnsw jaccard: %llu bytes of key scratch could not be allocated", (unsigned long long)(4 * rows * dim));
     return SDB_ENOMEM;
   }
   widen_keys_kernel<<<(unsigned)((rows * dim + 255) / 256), 256, 0, st>>>(static_cast<const short*>(d_vec), rows * dim, keys);
   count_launch(ctx);
-  const sdb_status rc = jaccard_prepare(ctx, static_cast<const uint32_t*>(keys), rows, dim, static_cast<uint32_t*>(bits), nbits, st);
-  cudaFreeAsync(keys, st);
-  return rc;
+  return jaccard_prepare(ctx, static_cast<const uint32_t*>(keys), rows, dim, static_cast<uint32_t*>(bits), nbits, st);
 }
 
 // per-query operands of the metrics that carry state (staged once per query, the same arithmetic as the elements')
@@ -1372,8 +1372,8 @@ __global__ void csr_validate_kernel(const uint64_t* __restrict__ rp, const uint3
 
 sdb_status csr_check(Ctx* ctx, const uint64_t* d_rp, const uint32_t* d_ci, uint64_t n_rows, uint64_t n_edges,
                      uint64_t id_limit, unsigned long long counts[2], const char* what, cudaStream_t st) {
-  unsigned long long* d_bad = nullptr;
-  SDB_CUDA(cudaMallocAsync(&d_bad, 16, st));
+  AsyncBuf<unsigned long long> d_bad;
+  SDB_CUDA(d_bad.reserve(2, st));
   cudaMemsetAsync(d_bad, 0, 16, st);
   const uint64_t work = n_rows > n_edges ? n_rows : n_edges;
   const unsigned grid = (unsigned)std::min<uint64_t>((work + 255) / 256 + 1, (uint64_t)ctx->sm_count * 16);
@@ -1382,7 +1382,7 @@ sdb_status csr_check(Ctx* ctx, const uint64_t* d_rp, const uint32_t* d_ci, uint6
   unsigned long long h_bad[2] = {0, 0};
   cudaError_t e = cudaMemcpyAsync(h_bad, d_bad, 16, cudaMemcpyDeviceToHost, st);
   if (e == cudaSuccess) e = cudaStreamSynchronize(st);
-  cudaFreeAsync(d_bad, st);
+  d_bad.reset();
   if (e != cudaSuccess) {
     set_error("%s: validation failed to run: %s", what, cudaGetErrorString(e));
     return SDB_ECUDA;
@@ -1497,29 +1497,21 @@ static sdb_hnsw* new_hnsw(Ctx* ctx, uint32_t dim, sdb_metric metric, sdb_vector_
   return h;
 }
 
-// Whose per-vector state it is, which fixes how it is allocated.  ELEMENTS: an index's elements, cudaMalloc'd and freed
-// with the index.  BATCH: the queries or pending vectors of one call, from the stream's pool and freed on the stream
-// once the call's kernels are queued.
-enum class VecSet { ELEMENTS, BATCH };
-
 // The state `metric` needs for rows x dim vectors d_v of type vt, allocated into s and computed on st: COSINE the norms
-// (none for an F32 BATCH: the walk computes the query's own, typed_distance_kernel both), PEARSON the mean and sx2,
-// JACCARD the sorted distinct keys.  What was allocated stays in s for vec_state_free, also on failure.
-static sdb_status vec_state_make(Ctx* ctx, VecSet set, sdb_metric metric, sdb_vector_type vt, const void* d_v,
-                                 uint64_t rows, uint32_t dim, VecState& s, cudaStream_t st) {
+// (none for an F32 batch: the walk computes the query's own, typed_distance_kernel both), PEARSON the mean and sx2,
+// JACCARD the sorted distinct keys.
+template <Mem K>
+static sdb_status vec_state_make(Ctx* ctx, sdb_metric metric, sdb_vector_type vt, const void* d_v, uint64_t rows,
+                                 uint32_t dim, VecState<K>& s, cudaStream_t st) {
   if (!rows) return SDB_OK;
-  auto alloc = [&](auto** p, size_t bytes) {
-    if ((set == VecSet::BATCH ? cudaMallocAsync(p, bytes, st) : cudaMalloc(p, bytes)) == cudaSuccess) return true;
-    *p = nullptr;
-    return false;
-  };
+  cudaError_t e = cudaSuccess;
   auto oom = [&](const char* what, size_t bytes) {
-    set_error("hnsw: %s (%zu bytes) could not be allocated: %s", what, bytes, cudaGetErrorString(cudaGetLastError()));
-    return set == VecSet::BATCH ? SDB_ECUDA : SDB_ENOMEM;
+    set_error("hnsw: %s (%zu bytes) could not be allocated: %s", what, bytes, cudaGetErrorString(e));
+    return K == Mem::Async ? SDB_ECUDA : SDB_ENOMEM;
   };
   const unsigned grid = (unsigned)((rows + 127) / 128);
-  if (metric == SDB_COSINE && !(vt == SDB_VT_F32 && set == VecSet::BATCH)) {
-    if (!alloc(&s.norm, sizeof(double) * rows)) return oom("cosine norms", sizeof(double) * rows);
+  if (metric == SDB_COSINE && !(vt == SDB_VT_F32 && K == Mem::Async)) {
+    if ((e = s.norm.reserve(rows, st)) != cudaSuccess) return oom("cosine norms", sizeof(double) * rows);
     with_vt(vt, [&](auto tag) {
       using T = decltype(tag);
       if constexpr (is_f32_v<T>)
@@ -1530,7 +1522,7 @@ static sdb_status vec_state_make(Ctx* ctx, VecSet set, sdb_metric metric, sdb_ve
     });
     count_launch(ctx);
   } else if (metric == SDB_PEARSON) {
-    if (!alloc(&s.mean, sizeof(double) * rows) || !alloc(&s.sx2, sizeof(double) * rows))
+    if ((e = s.mean.reserve(rows, st)) != cudaSuccess || (e = s.sx2.reserve(rows, st)) != cudaSuccess)
       return oom("pearson state", 2 * sizeof(double) * rows);
     with_vt(vt, [&](auto tag) {
       using T = decltype(tag);
@@ -1539,31 +1531,22 @@ static sdb_status vec_state_make(Ctx* ctx, VecSet set, sdb_metric metric, sdb_ve
     count_launch(ctx);
   } else if (metric == SDB_JACCARD) {  // key bytes * rows * dim: the sorted distinct keys of every vector
     const size_t kb = jkey_size(vt) * rows * dim;
-    if (!alloc(&s.bits, kb) || !alloc(&s.nbits, sizeof(uint32_t) * rows))
+    if ((e = s.bits.reserve(kb, st)) != cudaSuccess || (e = s.nbits.reserve(rows, st)) != cudaSuccess)
       return oom("jaccard state", kb + sizeof(uint32_t) * rows);
     return jaccard_prepare_typed(ctx, vt, d_v, rows, dim, s.bits, s.nbits, st);
   }
   return SDB_OK;
 }
-static void vec_state_free(VecState& s, VecSet set, cudaStream_t st) {
-  for (void* p : {(void*)s.norm, (void*)s.mean, (void*)s.sx2, s.bits, (void*)s.nbits}) {
-    if (!p) continue;
-    if (set == VecSet::BATCH) cudaFreeAsync(p, st);
-    else cudaFree(p);
-  }
-  s = VecState();
-}
 
 // the device tables of per-layer CSR pointers (h->rp, h->ci), (re)allocated for h->n_layers; the copy is queued on st
 static sdb_status upload_layer_tables(sdb_hnsw* h, cudaStream_t st) {
   const uint32_t n_layers = h->n_layers;
-  cudaFree(h->d_rp);
-  cudaFree(h->d_ci);
-  h->d_rp = nullptr;
-  h->d_ci = nullptr;
-  if (cudaMalloc(&h->d_rp, sizeof(void*) * n_layers) != cudaSuccess ||
-      cudaMalloc(&h->d_ci, sizeof(void*) * n_layers) != cudaSuccess) {
-    set_error("hnsw: layer table allocation failed: %s", cudaGetErrorString(cudaGetLastError()));
+  h->d_rp.reset();
+  h->d_ci.reset();
+  cudaError_t e = h->d_rp.reserve(n_layers);
+  if (e == cudaSuccess) e = h->d_ci.reserve(n_layers);
+  if (e != cudaSuccess) {
+    set_error("hnsw: layer table allocation failed: %s", cudaGetErrorString(e));
     return SDB_ENOMEM;
   }
   if (cudaMemcpyAsync(h->d_rp, h->rp.data(), sizeof(void*) * n_layers, cudaMemcpyHostToDevice, st) != cudaSuccess ||
@@ -1588,7 +1571,7 @@ static sdb_status hnsw_finish(sdb_hnsw* h, sdb_hnsw** out) {
     sdb_hnsw_destroy(h);
     return rc;
   }
-  rc = vec_state_make(ctx, VecSet::ELEMENTS, h->metric, h->vt, h->d_vec, h->n, h->dim, h->elems, st);
+  rc = vec_state_make(ctx, h->metric, h->vt, h->d_vec, h->n, h->dim, h->elems, st);
   if (rc != SDB_OK) {
     sdb_hnsw_destroy(h);
     return rc;
@@ -1642,15 +1625,6 @@ extern "C" {
 void sdb_hnsw_destroy(sdb_hnsw* h) {
   if (!h) return;
   cudaSetDevice(h->ctx->device);
-  if (!h->borrowed) {
-    cudaFree(h->d_vec);
-    for (auto p : h->rp) cudaFree(p);
-    for (auto p : h->ci) cudaFree(p);
-  }
-  vec_state_free(h->elems, VecSet::ELEMENTS, nullptr);
-  cudaFree(h->d_rp);
-  cudaFree(h->d_ci);
-  cudaFree(h->d_visited);
   delete h;
 }
 
@@ -1669,30 +1643,36 @@ sdb_status sdb_hnsw_load_typed(sdb_ctx* ctx, uint32_t dim, sdb_metric metric, sd
   SDB_CUDA(cudaSetDevice(ctx->device));
   sdb_hnsw* h = new_hnsw(ctx, dim, metric, vt, n_elems, n_layers, entry_point);
   cudaStream_t st = ctx->stream;
-  auto fail = [&](const char* what) {
-    set_error("hnsw load: %s failed: %s", what, cudaGetErrorString(cudaGetLastError()));
-    sdb_hnsw_destroy(h);
-    return SDB_ENOMEM;
-  };
-  const uint64_t nn = n_elems ? n_elems : 1;
-  const size_t esz = vt_size(vt);
-  if (cudaMalloc(&h->d_vec, esz * nn * dim) != cudaSuccess) return fail("vectors");
-  if (n_elems) SDB_CUDA(cudaMemcpyAsync(h->d_vec, vectors, esz * n_elems * dim, cudaMemcpyHostToDevice, st));
-  for (uint32_t l = 0; l < n_layers; l++) {
-    const uint64_t e = n_elems ? row_ptr[l][n_elems] : 0;
-    uint64_t* drp = nullptr;
-    uint32_t* dci = nullptr;
-    if (cudaMalloc(&drp, sizeof(uint64_t) * (n_elems + 1)) != cudaSuccess) return fail("row_ptr");
-    h->rp.push_back(drp);
-    if (cudaMalloc(&dci, sizeof(uint32_t) * (e ? e : 1)) != cudaSuccess) return fail("col_idx");
-    h->ci.push_back(dci);
-    SDB_CUDA(cudaMemcpyAsync(drp, row_ptr[l], sizeof(uint64_t) * (n_elems + 1), cudaMemcpyHostToDevice, st));
-    if (e) SDB_CUDA(cudaMemcpyAsync(dci, col_idx[l], sizeof(uint32_t) * e, cudaMemcpyHostToDevice, st));
-    const sdb_status vrc = csr_validate(ctx, drp, dci, n_elems, e, n_elems, "sdb_hnsw_load", st);
-    if (vrc != SDB_OK) {
-      sdb_hnsw_destroy(h);
-      return vrc;
+  const sdb_status rc = [&]() -> sdb_status {
+    auto fail = [&](const char* what, cudaError_t e) {
+      set_error("hnsw load: %s failed: %s", what, cudaGetErrorString(e));
+      return SDB_ENOMEM;
+    };
+    const uint64_t nn = n_elems ? n_elems : 1;
+    const size_t esz = vt_size(vt);
+    cudaError_t e = h->own_vec.reserve(esz * nn * dim);
+    if (e != cudaSuccess) return fail("vectors", e);
+    h->d_vec = h->own_vec;
+    if (n_elems) SDB_CUDA(cudaMemcpyAsync(h->d_vec, vectors, esz * n_elems * dim, cudaMemcpyHostToDevice, st));
+    for (uint32_t l = 0; l < n_layers; l++) {
+      const uint64_t ne = n_elems ? row_ptr[l][n_elems] : 0;
+      DevBuf<uint64_t> drp;
+      DevBuf<uint32_t> dci;
+      if ((e = drp.reserve(n_elems + 1)) != cudaSuccess) return fail("row_ptr", e);
+      if ((e = dci.reserve(ne ? ne : 1)) != cudaSuccess) return fail("col_idx", e);
+      h->rp.push_back(drp);
+      h->ci.push_back(dci);
+      h->own_rp.push_back(std::move(drp));
+      h->own_ci.push_back(std::move(dci));
+      SDB_CUDA(cudaMemcpyAsync(h->rp[l], row_ptr[l], sizeof(uint64_t) * (n_elems + 1), cudaMemcpyHostToDevice, st));
+      if (ne) SDB_CUDA(cudaMemcpyAsync(h->ci[l], col_idx[l], sizeof(uint32_t) * ne, cudaMemcpyHostToDevice, st));
+      SDB_TRY(csr_validate(ctx, h->rp[l], h->ci[l], n_elems, ne, n_elems, "sdb_hnsw_load", st));
     }
+    return SDB_OK;
+  }();
+  if (rc != SDB_OK) {
+    sdb_hnsw_destroy(h);
+    return rc;
   }
   return hnsw_finish(h, out);
 }
@@ -1775,16 +1755,19 @@ static sdb_status hnsw_load_staged_impl(sdb_ctx* ctx, uint32_t dim, sdb_metric m
   const uint64_t nn = n_elems ? n_elems : 1;
   uint64_t bad_total = 0, bad = 0;
   sdb_status rc = SDB_OK;
-  uint8_t* d_present = nullptr;
-  if (cudaMalloc(&d_present, nn) != cudaSuccess || cudaMemsetAsync(d_present, 0, nn, st) != cudaSuccess) {
-    set_error("hnsw load: present-mask allocation failed: %s", cudaGetErrorString(cudaGetLastError()));
+  DevBuf<uint8_t> d_present;
+  cudaError_t e = d_present.reserve(nn);
+  if (e == cudaSuccess) e = cudaMemsetAsync(d_present, 0, nn, st);
+  if (e != cudaSuccess) {
+    set_error("hnsw load: present-mask allocation failed: %s", cudaGetErrorString(e));
     rc = SDB_ENOMEM;
   }
   const size_t esz = vt_size(vt);
-  if (cudaMalloc(&h->d_vec, esz * nn * dim) != cudaSuccess) {
-    set_error("hnsw load: vector allocation failed: %s", cudaGetErrorString(cudaGetLastError()));
+  if ((e = h->own_vec.reserve(esz * nn * dim)) != cudaSuccess) {
+    set_error("hnsw load: vector allocation failed: %s", cudaGetErrorString(e));
     rc = SDB_ENOMEM;
   }
+  h->d_vec = h->own_vec;
   // elements without an He value keep all-zero vectors; they are unreachable unless an Hn value names them
   if (rc == SDB_OK && cudaMemsetAsync(h->d_vec, 0, esz * nn * dim, st) != cudaSuccess) rc = SDB_ECUDA;
   if (rc == SDB_OK)
@@ -1793,19 +1776,19 @@ static sdb_status hnsw_load_staged_impl(sdb_ctx* ctx, uint32_t dim, sdb_metric m
   bad_total += bad;
   uint64_t n_dropped = 0;
   for (uint32_t l = 0; l < n_layers && rc == SDB_OK; l++) {
-    uint64_t* drp = nullptr;
-    uint32_t* dci = nullptr;
+    DevBuf<uint64_t> drp;
+    DevBuf<uint32_t> dci;
     uint64_t ne = 0;
     bad = 0;
     rc = stage_decode_nodes(ctx, node_blob[l], node_off[l], node_ids[l], n_nodes[l], n_elems, &drp, &dci, &ne, &bad, st);
     if (rc == SDB_OK) {
       bad_total += bad;
       // drop edges from / to elements that have no He value ("edge to an unknown element")
-      uint64_t *rp2 = nullptr, *d_tot = nullptr;
-      uint32_t* ci2 = nullptr;
+      DevBuf<uint64_t> rp2, d_tot;
+      DevBuf<uint32_t> ci2;
       uint64_t kept = 0;
       const unsigned g1 = (unsigned)((n_elems + 1 + 255) / 256);
-      if (cudaMalloc(&rp2, 8 * (n_elems + 1)) != cudaSuccess || cudaMalloc(&d_tot, 8) != cudaSuccess) rc = SDB_ENOMEM;
+      if (rp2.reserve(n_elems + 1) != cudaSuccess || d_tot.reserve(1) != cudaSuccess) rc = SDB_ENOMEM;
       if (rc == SDB_OK) {
         csr_present_degree_kernel<<<g1, 256, 0, st>>>(drp, dci, d_present, n_elems, rp2);
         count_launch(ctx);
@@ -1814,25 +1797,20 @@ static sdb_status hnsw_load_staged_impl(sdb_ctx* ctx, uint32_t dim, sdb_metric m
       if (rc == SDB_OK && (cudaMemcpyAsync(&kept, d_tot, 8, cudaMemcpyDeviceToHost, st) != cudaSuccess ||
                            cudaStreamSynchronize(st) != cudaSuccess))
         rc = SDB_ECUDA;
-      if (rc == SDB_OK && cudaMalloc(&ci2, 4 * (kept ? kept : 1)) != cudaSuccess) rc = SDB_ENOMEM;
+      if (rc == SDB_OK && ci2.reserve(kept ? kept : 1) != cudaSuccess) rc = SDB_ENOMEM;
       if (rc == SDB_OK && n_elems) {
         csr_present_fill_kernel<<<g1, 256, 0, st>>>(drp, dci, d_present, n_elems, rp2, ci2);
         count_launch(ctx);
         if (cudaStreamSynchronize(st) != cudaSuccess) rc = SDB_ECUDA;
       }
-      cudaFree(d_tot);
       if (rc == SDB_OK) {
         n_dropped += ne - kept;
-        cudaFree(drp);
-        cudaFree(dci);
         h->rp.push_back(rp2);
         h->ci.push_back(ci2);
-      } else {
-        if (rc == SDB_ENOMEM) set_error("hnsw load: CSR filter allocation failed");
-        cudaFree(rp2);
-        cudaFree(ci2);
-        cudaFree(drp);
-        cudaFree(dci);
+        h->own_rp.push_back(std::move(rp2));
+        h->own_ci.push_back(std::move(ci2));
+      } else if (rc == SDB_ENOMEM) {
+        set_error("hnsw load: CSR filter allocation failed");
       }
     }
   }
@@ -1842,7 +1820,7 @@ static sdb_status hnsw_load_staged_impl(sdb_ctx* ctx, uint32_t dim, sdb_metric m
   if (rc == SDB_OK && entry_point >= 0 && n_elems &&
       cudaMemcpy(&ep_present, d_present + entry_point, 1, cudaMemcpyDeviceToHost) != cudaSuccess)
     rc = SDB_ECUDA;
-  cudaFree(d_present);
+  d_present.reset();
   if (rc == SDB_OK && !ep_present) {
     set_error("sdb_hnsw_load_staged: the entry point %lld has no He value", (long long)entry_point);
     rc = SDB_EINVAL;
@@ -1919,18 +1897,18 @@ sdb_status sdb_hnsw_knn_exact_device(sdb_hnsw* h, const void* d_queries, uint32_
   std::lock_guard<std::mutex> guard(h->mu);
   SDB_CUDA(cudaSetDevice(ctx->device));
   cudaStream_t st = ctx->stream;
-  uint32_t* sorted = nullptr;
-  unsigned int* d_max = nullptr;
-  void* d_tmp = nullptr;
-  VecState qs;
-  auto run = [&]() -> sdb_status {
+  auto run = [&]() -> sdb_status {  // the temporaries are released on every path, before the synchronisation below
+    AsyncBuf<uint32_t> sorted;
+    AsyncBuf<unsigned int> d_max;
+    AsyncBuf<char> d_tmp;
+    VecState<Mem::Async> qs;
     if (d_members && n_members) {  // ascending ids: ties are then ranked by id; every id must name an element
       size_t tmp_bytes = 0;
-      SDB_CUDA(cub::DeviceRadixSort::SortKeys(nullptr, tmp_bytes, d_members, sorted, n_members, 0, 32, st));
-      SDB_CUDA(cudaMallocAsync(&sorted, sizeof(uint32_t) * n_members, st));
-      SDB_CUDA(cudaMallocAsync(&d_tmp, tmp_bytes ? tmp_bytes : 1, st));
-      SDB_CUDA(cudaMallocAsync(&d_max, sizeof(unsigned int), st));
-      SDB_CUDA(cub::DeviceRadixSort::SortKeys(d_tmp, tmp_bytes, d_members, sorted, n_members, 0, 32, st));
+      SDB_CUDA(cub::DeviceRadixSort::SortKeys(nullptr, tmp_bytes, d_members, sorted.get(), n_members, 0, 32, st));
+      SDB_CUDA(sorted.reserve(n_members, st));
+      SDB_CUDA(d_tmp.reserve(tmp_bytes ? tmp_bytes : 1, st));
+      SDB_CUDA(d_max.reserve(1, st));
+      SDB_CUDA(cub::DeviceRadixSort::SortKeys(d_tmp.get(), tmp_bytes, d_members, sorted.get(), n_members, 0, 32, st));
       count_launch(ctx);
       SDB_CUDA(cudaMemsetAsync(d_max, 0, sizeof(unsigned int), st));
       members_max_kernel<<<(unsigned)((n_members + 255) / 256), 256, 0, st>>>(sorted, n_members, d_max);
@@ -1943,7 +1921,7 @@ sdb_status sdb_hnsw_knn_exact_device(sdb_hnsw* h, const void* d_queries, uint32_
         return SDB_EINVAL;
       }
     }
-    SDB_TRY(vec_state_make(ctx, VecSet::BATCH, h->metric, h->vt, d_queries, nq, h->dim, qs, st));
+    SDB_TRY(vec_state_make(ctx, h->metric, h->vt, d_queries, nq, h->dim, qs, st));
     HnswParams P = element_params(h);
     P.queries = d_queries;
     P.nq = nq;
@@ -1957,7 +1935,7 @@ sdb_status sdb_hnsw_knn_exact_device(sdb_hnsw* h, const void* d_queries, uint32_
     P.q_nbits = qs.nbits;
     P.q_norm = qs.norm;
     const size_t per_warp = hn_stage_bytes(h->dim, h->metric, h->vt) + 12 * ((size_t)k + 1) + 64;
-    const uint32_t* mem = d_members ? sorted : nullptr;
+    const uint32_t* mem = d_members ? sorted.get() : nullptr;
     return with_vt(h->vt, [&](auto tag) {
       using T = decltype(tag);
       return with_metric(h->metric, [&](auto met) {
@@ -1967,9 +1945,6 @@ sdb_status sdb_hnsw_knn_exact_device(sdb_hnsw* h, const void* d_queries, uint32_
     });
   };
   sdb_status rc = run();
-  vec_state_free(qs, VecSet::BATCH, st);
-  for (void* p : {(void*)sorted, (void*)d_max, d_tmp})
-    if (p) cudaFreeAsync(p, st);
   if (cudaStreamSynchronize(st) != cudaSuccess && rc == SDB_OK) {
     set_error("sdb_hnsw_knn_exact_device: %s", cudaGetErrorString(cudaGetLastError()));
     rc = SDB_ECUDA;
@@ -2078,9 +2053,8 @@ static sdb_status hnsw_search_impl(sdb_hnsw* h, const void* queries, uint32_t nq
   if (truthy) tl = tl + 3 > 18 ? (tl > 18 ? tl : 18) : tl + 3;  // filtered walks visit ~1/selectivity more elements
   const uint32_t n_tables = grid * HN_WARPS;
   if (!h->d_visited || h->table_log2 != tl || h->n_tables < n_tables) {
-    cudaFree(h->d_visited);
-    h->d_visited = nullptr;
-    SDB_CUDA(cudaMalloc(&h->d_visited, sizeof(uint64_t) * ((size_t)n_tables << tl)));
+    h->d_visited.reset();
+    SDB_CUDA(h->d_visited.reserve((size_t)n_tables << tl));
     SDB_CUDA(cudaMemsetAsync(h->d_visited, 0, sizeof(uint64_t) * ((size_t)n_tables << tl), st));
     h->table_log2 = tl;
     h->n_tables = n_tables;
@@ -2093,35 +2067,33 @@ static sdb_status hnsw_search_impl(sdb_hnsw* h, const void* queries, uint32_t nq
     h->gen = 1;
   }
   const size_t esz = vt_size(h->vt);
-  void* d_q = nullptr;
-  uint64_t* d_elems = nullptr;
-  double* d_dist = nullptr;
-  uint32_t* d_cnt = nullptr;
-  uint64_t* d_ctr = nullptr;
-  uint32_t* d_ovf = nullptr;
-  if (device_io) {  // queries and outputs already live on the device (index construction): no staging
-    d_q = const_cast<void*>(queries);
-    d_elems = out_elems;
-    d_dist = out_dist;
-    d_cnt = out_count;
-  } else {
-    SDB_CUDA(cudaMallocAsync(&d_q, esz * (size_t)nq * h->dim, st));
-    SDB_CUDA(cudaMallocAsync(&d_elems, sizeof(uint64_t) * (size_t)nq * k, st));
-    SDB_CUDA(cudaMallocAsync(&d_dist, sizeof(double) * (size_t)nq * k, st));
-    SDB_CUDA(cudaMallocAsync(&d_cnt, sizeof(uint32_t) * nq, st));
+  // device_io: queries and outputs already live on the device (index construction), no staging
+  AsyncBuf<char> q_buf;
+  AsyncBuf<uint64_t> elems_buf, d_ctr;
+  AsyncBuf<double> dist_buf;
+  AsyncBuf<uint32_t> cnt_buf, d_ovf;
+  AsyncBuf<uint8_t> d_noexp, d_truthy;
+  void* d_q = const_cast<void*>(queries);
+  uint64_t* d_elems = out_elems;
+  double* d_dist = out_dist;
+  uint32_t* d_cnt = out_count;
+  if (!device_io) {
+    SDB_CUDA(q_buf.reserve(esz * (size_t)nq * h->dim, st));
+    SDB_CUDA(elems_buf.reserve((size_t)nq * k, st));
+    SDB_CUDA(dist_buf.reserve((size_t)nq * k, st));
+    SDB_CUDA(cnt_buf.reserve(nq, st));
+    d_q = q_buf, d_elems = elems_buf, d_dist = dist_buf, d_cnt = cnt_buf;
     SDB_CUDA(cudaMemcpyAsync(d_q, queries, esz * (size_t)nq * h->dim, cudaMemcpyHostToDevice, st));
   }
-  SDB_CUDA(cudaMallocAsync(&d_ctr, sizeof(uint64_t) * 2 * nq, st));
-  SDB_CUDA(cudaMallocAsync(&d_ovf, 4, st));
+  SDB_CUDA(d_ctr.reserve(2 * (size_t)nq, st));
+  SDB_CUDA(d_ovf.reserve(1, st));
   SDB_CUDA(cudaMemsetAsync(d_ovf, 0, 4, st));
-  uint8_t* d_noexp = nullptr;
   if (noexp) {
-    SDB_CUDA(cudaMallocAsync(&d_noexp, h->n ? h->n : 1, st));
+    SDB_CUDA(d_noexp.reserve(h->n ? h->n : 1, st));
     SDB_CUDA(cudaMemcpyAsync(d_noexp, noexp, h->n, cudaMemcpyHostToDevice, st));
   }
-  uint8_t* d_truthy = nullptr;
   if (truthy) {
-    SDB_CUDA(cudaMallocAsync(&d_truthy, h->n ? h->n : 1, st));
+    SDB_CUDA(d_truthy.reserve(h->n ? h->n : 1, st));
     SDB_CUDA(cudaMemcpyAsync(d_truthy, truthy, h->n, cudaMemcpyHostToDevice, st));
   }
   HnswParams P;
@@ -2154,8 +2126,8 @@ static sdb_status hnsw_search_impl(sdb_hnsw* h, const void* queries, uint32_t nq
   P.e_sx2 = h->elems.sx2;
   P.e_bits = h->elems.bits;
   P.e_nbits = h->elems.nbits;
-  VecState qs;
-  const sdb_status qrc = vec_state_make(ctx, VecSet::BATCH, h->metric, h->vt, d_q, nq, h->dim, qs, st);
+  VecState<Mem::Async> qs;
+  const sdb_status qrc = vec_state_make(ctx, h->metric, h->vt, d_q, nq, h->dim, qs, st);
   P.q_mean = qs.mean;
   P.q_sx2 = qs.sx2;
   P.q_bits = qs.bits;
@@ -2165,7 +2137,6 @@ static sdb_status hnsw_search_impl(sdb_hnsw* h, const void* queries, uint32_t nq
     kern<<<grid, HN_WARPS * 32, smem, st>>>(P);
     count_launch(ctx);
   }
-  vec_state_free(qs, VecSet::BATCH, st);
   h->gen += gens_per_warp * n_tables;
   uint32_t ovf = 0;
   if (!device_io) {
@@ -2176,16 +2147,6 @@ static sdb_status hnsw_search_impl(sdb_hnsw* h, const void* queries, uint32_t nq
   if (out_counters)
     SDB_CUDA(cudaMemcpyAsync(out_counters, d_ctr, sizeof(uint64_t) * 2 * nq, device_io ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost, st));
   SDB_CUDA(cudaMemcpyAsync(&ovf, d_ovf, 4, cudaMemcpyDeviceToHost, st));
-  if (!device_io) {
-    cudaFreeAsync(d_q, st);
-    cudaFreeAsync(d_elems, st);
-    cudaFreeAsync(d_dist, st);
-    cudaFreeAsync(d_cnt, st);
-  }
-  cudaFreeAsync(d_ctr, st);
-  cudaFreeAsync(d_ovf, st);
-  if (d_truthy) cudaFreeAsync(d_truthy, st);
-  if (d_noexp) cudaFreeAsync(d_noexp, st);
   SDB_CUDA(cudaStreamSynchronize(st));
   SDB_CUDA(cudaGetLastError());
   if (qrc != SDB_OK) return qrc;
@@ -2210,20 +2171,20 @@ static sdb_status typed_distances(Ctx* ctx, sdb_metric metric, sdb_vector_type v
                                   const void* query, const void* vectors, uint64_t n, double* out, const char* what) {
   cudaStream_t st = ctx->stream;
   const size_t esz = vt_size(vt);
-  void *d_q = nullptr, *d_v = nullptr;
-  double* d_o = nullptr;
-  VecState qs, vs;
-  auto run = [&]() -> sdb_status {
-    SDB_CUDA(cudaMallocAsync(&d_q, esz * dim, st));
-    SDB_CUDA(cudaMallocAsync(&d_v, esz * n * dim, st));
-    SDB_CUDA(cudaMallocAsync(&d_o, sizeof(double) * n, st));
+  auto run = [&]() -> sdb_status {  // the temporaries are released on every path, before the synchronisation below
+    AsyncBuf<char> d_q, d_v;
+    AsyncBuf<double> d_o;
+    VecState<Mem::Async> qs, vs;
+    SDB_CUDA(d_q.reserve(esz * dim, st));
+    SDB_CUDA(d_v.reserve(esz * n * dim, st));
+    SDB_CUDA(d_o.reserve(n, st));
     SDB_CUDA(cudaMemcpyAsync(d_q, query, esz * dim, cudaMemcpyHostToDevice, st));
     SDB_CUDA(cudaMemcpyAsync(d_v, vectors, esz * n * dim, cudaMemcpyHostToDevice, st));
-    SDB_TRY(vec_state_make(ctx, VecSet::BATCH, metric, vt, d_q, 1, dim, qs, st));
-    SDB_TRY(vec_state_make(ctx, VecSet::BATCH, metric, vt, d_v, n, dim, vs, st));
+    SDB_TRY(vec_state_make(ctx, metric, vt, d_q, 1, dim, qs, st));
+    SDB_TRY(vec_state_make(ctx, metric, vt, d_v, n, dim, vs, st));
     TypedArgs A;
-    A.q = static_cast<const float*>(d_q);
-    A.vecs = static_cast<const float*>(d_v);
+    A.q = reinterpret_cast<const float*>(d_q.get());
+    A.vecs = reinterpret_cast<const float*>(d_v.get());
     A.dim = dim;
     A.n = n;
     A.out = d_o;
@@ -2255,11 +2216,6 @@ static sdb_status typed_distances(Ctx* ctx, sdb_metric metric, sdb_vector_type v
     return SDB_OK;
   };
   const sdb_status rc = run();
-  vec_state_free(qs, VecSet::BATCH, st);
-  vec_state_free(vs, VecSet::BATCH, st);
-  if (d_q) cudaFreeAsync(d_q, st);
-  if (d_v) cudaFreeAsync(d_v, st);
-  if (d_o) cudaFreeAsync(d_o, st);
   if (cudaStreamSynchronize(st) != cudaSuccess && rc == SDB_OK) {
     set_error("%s: %s", what, cudaGetErrorString(cudaGetLastError()));
     return SDB_ECUDA;

@@ -3,6 +3,7 @@
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
 
+#include <atomic>
 #include <cstdarg>
 #include <cstdint>
 #include <cstdio>
@@ -30,6 +31,83 @@ void set_error(const char* fmt, ...);
     sdb_status s__ = (call);           \
     if (s__ != SDB_OK) return s__;     \
   } while (0)
+
+// ---- owned buffers --------------------------------------------------------------------------------
+// Every device and pinned buffer of the library is held by a Buf: move-only, freed by its destructor (on the device
+// that is current then: the destroy entry points select the owner's device first).  reserve() only grows, and frees the
+// old buffer before it allocates the larger one, so the peak is the new size alone; a failed reserve leaves it empty.
+// A Buf converts to T*, so kernel launches and copies take it like the raw pointer.
+enum class Mem { Device, Async, Pinned };  // cudaMalloc / cudaMallocAsync on a stream / cudaHostAlloc
+inline std::atomic<uint64_t> g_live_bufs{0}, g_live_bytes{0};  // sdb_debug_live_allocations
+template <class T, Mem K>
+class Buf {
+ public:
+  Buf() = default;
+  Buf(Buf&& o) noexcept : p_(o.p_), n_(o.n_), st_(o.st_) { o.p_ = nullptr, o.n_ = 0; }
+  Buf& operator=(Buf&& o) noexcept {
+    if (this != &o) reset(), p_ = o.p_, n_ = o.n_, st_ = o.st_, o.p_ = nullptr, o.n_ = 0;
+    return *this;
+  }
+  ~Buf() { reset(); }
+  T* get() const { return p_; }
+  operator T*() const { return p_; }
+  size_t size() const { return n_; }  // elements
+  // st: the stream of a Mem::Async buffer (it is freed there too); flags: cudaHostAlloc flags of a Mem::Pinned one
+  cudaError_t reserve(size_t n, cudaStream_t st = nullptr, unsigned flags = cudaHostAllocDefault) {
+    if (n <= n_) return cudaSuccess;
+    reset();
+    void* p = nullptr;
+    const cudaError_t e = K == Mem::Device ? cudaMalloc(&p, sizeof(T) * n)
+                          : K == Mem::Async ? cudaMallocAsync(&p, sizeof(T) * n, st)
+                                            : cudaHostAlloc(&p, sizeof(T) * n, flags);
+    if (e != cudaSuccess) {
+      cudaGetLastError();  // reported through the return value: the next launch check must not see it
+      return e;
+    }
+    p_ = (T*)p, n_ = n, st_ = st;
+    g_live_bufs++, g_live_bytes += sizeof(T) * n;
+    return cudaSuccess;
+  }
+  void reset() {
+    if (p_) free_released((void*)p_, st_);
+    drop();
+  }
+  T* release() {  // hands the buffer to the caller, who frees it with free_released
+    T* p = p_;
+    drop();
+    return p;
+  }
+  static void free_released(void* p, cudaStream_t st = nullptr) {
+    if (K == Mem::Device) cudaFree(p);
+    else if (K == Mem::Async) cudaFreeAsync(p, st);
+    else cudaFreeHost(p);
+  }
+
+ private:
+  void drop() {
+    if (p_) g_live_bufs--, g_live_bytes -= sizeof(T) * n_;
+    p_ = nullptr, n_ = 0;
+  }
+  T* p_ = nullptr;
+  size_t n_ = 0;
+  cudaStream_t st_ = nullptr;
+};
+template <class T> using DevBuf = Buf<T, Mem::Device>;
+template <class T> using AsyncBuf = Buf<T, Mem::Async>;
+template <class T> using PinnedBuf = Buf<T, Mem::Pinned>;
+
+// rows / distances / counts of a batch's results (nq queries, n_out = nq x k entries), grow-only
+struct ResultBufs {
+  DevBuf<uint64_t> rows;
+  DevBuf<double> dist;
+  DevBuf<uint32_t> count;
+  cudaError_t reserve(size_t n_out, size_t nq) {
+    cudaError_t e = rows.reserve(n_out);
+    if (e == cudaSuccess) e = dist.reserve(n_out);
+    if (e == cudaSuccess) e = count.reserve(nq);
+    return e;
+  }
+};
 
 constexpr int TILE_ROWS = 256;    // screening tile = 256 corpus rows (one wgmma N=256 MMA tile)
 constexpr int PASS_RATIO = 8;     // default geometric threshold-refinement ratio (api.cu:pass_ratio picks per batch size)
@@ -126,15 +204,14 @@ struct Ctx {
   uint64_t launches = 0;
   std::mutex mu;
   void* encode_tiled = nullptr;  // cuTensorMapEncodeTiled (driver entry point), resolved lazily
-  void* h_stage = nullptr;       // pinned staging buffer for large device->host results (grow-only)
-  size_t h_stage_bytes = 0;
+  PinnedBuf<uint8_t> h_stage;    // pinned staging buffer for large device->host results (grow-only)
   Comm* comm = nullptr;
   // cancellation (sdb_ctx_cancel): one int in pinned memory that the host side polls between kernel phases, mirrored
   // into a word in DEVICE memory (copied on its own stream by sdb_ctx_cancel) that long-running kernels (the HNSW walk)
   // poll per query -- polling the pinned word itself from thousands of warps is a PCIe read each (ncu r2: 8 % of the
   // walk's stall samples)
-  volatile int* h_cancel = nullptr;
-  int* d_cancel = nullptr;
+  PinnedBuf<volatile int> h_cancel;
+  DevBuf<int> d_cancel;
   cudaStream_t cancel_stream = nullptr;
   int prio_high = 0;  // greatest launch priority of the device (cudaDeviceGetStreamPriorityRange)
   int tc_pair_ctas = 0;  // CTAs of the int8 streaming screen launched as resident 2-CTA clusters (0: no pair launch)
@@ -178,16 +255,13 @@ struct Ticket {
   uint32_t n_passes = 0;
   uint64_t launches0 = 0;
   cudaEvent_t ev_begin = nullptr, ev_screen0 = nullptr, ev_screen1 = nullptr, ev_end = nullptr;
-  uint32_t* h_flags = nullptr;   // pinned: per query, bit0 overflow, bit1 proof failed
+  PinnedBuf<uint32_t> h_flags;   // per query, bit0 overflow, bit1 proof failed
   uint32_t* h_qflags = nullptr;  // pinned: per query, bit0 needs the exact path, bit1 NaN input
   uint32_t* h_stat = nullptr;    // pinned: [0] queries flagged, [1] candidates re-ranked, [2] max per query, [3] survivors gathered
   uint32_t h_cap = 0;
   // host-buffer entry points: per-slot device staging
-  double* d_in_q = nullptr;
-  uint64_t* d_res_rows = nullptr;
-  double* d_res_dist = nullptr;
-  uint32_t* d_res_count = nullptr;
-  size_t in_cap = 0, res_cap = 0, res_cap_q = 0;
+  DevBuf<double> d_in_q;
+  ResultBufs res;
   cudaEvent_t ev_h2d = nullptr, ev_out = nullptr;
   cudaEvent_t ev_main = nullptr;  // recorded after this batch's last screen launch (the next batch's screen waits for it)
   bool wait_h2d = false;  // the batch's stream still has to wait for ev_h2d (queries travelling on the copy stream)
@@ -207,39 +281,38 @@ void trace_host(Ctx* ctx, uint32_t ticket, const char* name);  // host-side time
 // anything, and every launch captures the pointers by value.
 struct Scratch {
   uint32_t sc_nq = 0, sc_cap = 0;
-  double* d_q64 = nullptr;
-  float* d_q32 = nullptr;
-  __nv_bfloat16* d_qbf16 = nullptr;
-  double* d_qmag = nullptr;
-  uint32_t* d_qflags = nullptr;  // bit0: query needs the exact path; bit1: query has NaN input
-  float* d_qbferr = nullptr;     // |q - bf16(q)| / |q| per query
-  int8_t* d_q8 = nullptr;        // int8 queries nq_pad x dim_pad8
-  float* d_q8scale = nullptr;    // max|q|/127 per query
-  float* d_q8err = nullptr;      // |q - dequant(q)| / |q| per query
-  Cand* d_sub = nullptr;         // thread-private candidate sub-lists of the tensor-core screens
-  uint32_t* d_sub_cnt = nullptr; // [nq][sub_slots]
+  DevBuf<double> d_q64;
+  DevBuf<float> d_q32;
+  DevBuf<__nv_bfloat16> d_qbf16;
+  DevBuf<double> d_qmag;
+  DevBuf<uint32_t> d_qflags;  // bit0: query needs the exact path; bit1: query has NaN input
+  DevBuf<float> d_qbferr;     // |q - bf16(q)| / |q| per query
+  DevBuf<int8_t> d_q8;        // int8 queries nq_pad x dim_pad8
+  DevBuf<float> d_q8scale;    // max|q|/127 per query
+  DevBuf<float> d_q8err;      // |q - dequant(q)| / |q| per query
+  DevBuf<Cand> d_sub;         // thread-private candidate sub-lists of the tensor-core screens
+  DevBuf<uint32_t> d_sub_cnt; // [nq][sub_slots]
   uint32_t sub_slots = 0, sub_cap = 0, last_slots = 0;
-  float* d_bscale = nullptr;     // per query: factor that turns tau into similarity*|q| units (1 or q8scale * i8_scale)
-  float* d_beps = nullptr;       // per query: rigorous screen error bound (cosine units / relative dot error)
-  float* d_margin = nullptr;     // per query: 2.1 x that bound in score units (0 in approximate mode)
-  float* d_margin2 = nullptr;    // stage B (f32 re-score of the candidates): margin, error bound, threshold
-  float* d_beps2 = nullptr;
-  float* d_tau2 = nullptr;
-  float* d_qlow = nullptr;       // per query: lower / upper bound of any score (histogram geometry)
-  float* d_qcap = nullptr;
-  HistParam* d_hparam = nullptr; // per query histogram geometry of the streaming screen
-  uint32_t* d_hist = nullptr;    // [nq][HIST_BINS]
-  float* d_probe = nullptr;      // [nq][PROBE_STRIDE] chunk maxima of the probe launch
-  float* d_tau = nullptr;
-  Cand* d_cand = nullptr;
-  uint32_t* d_cand_cnt = nullptr;
-  uint32_t* d_flags = nullptr;   // per query: bit0 overflow, bit1 verification failed
-  uint32_t* d_stat = nullptr;    // [0] queries flagged by cand_final, [1] candidates re-ranked, [2] max per query, [3] gathered
-  uint64_t* d_rr_key = nullptr;  // re-rank results: nq x rr_stride
-  double* d_rr_dist = nullptr;
-  uint32_t* d_rr_row = nullptr;
+  DevBuf<float> d_bscale;     // per query: factor that turns tau into similarity*|q| units (1 or q8scale * i8_scale)
+  DevBuf<float> d_beps;       // per query: rigorous screen error bound (cosine units / relative dot error)
+  DevBuf<float> d_margin;     // per query: 2.1 x that bound in score units (0 in approximate mode)
+  DevBuf<float> d_margin2;    // stage B (f32 re-score of the candidates): margin, error bound, threshold
+  DevBuf<float> d_beps2;
+  DevBuf<float> d_tau2;
+  DevBuf<float> d_qlow;       // per query: lower / upper bound of any score (histogram geometry)
+  DevBuf<float> d_qcap;
+  DevBuf<HistParam> d_hparam; // per query histogram geometry of the streaming screen
+  DevBuf<uint32_t> d_hist;    // [nq][HIST_BINS]
+  DevBuf<float> d_probe;      // [nq][PROBE_STRIDE] chunk maxima of the probe launch
+  DevBuf<float> d_tau;
+  DevBuf<Cand> d_cand;
+  DevBuf<uint32_t> d_cand_cnt;
+  DevBuf<uint32_t> d_flags;   // per query: bit0 overflow, bit1 verification failed
+  DevBuf<uint32_t> d_stat;    // [0] queries flagged by cand_final, [1] candidates re-ranked, [2] max per query, [3] gathered
+  DevBuf<uint64_t> d_rr_key;  // re-rank results: nq x rr_stride
+  DevBuf<double> d_rr_dist;
+  DevBuf<uint32_t> d_rr_row;
   uint32_t rr_stride = 0;
-  uint32_t sc_gen = 0;           // bumped whenever this set is reallocated
 };
 
 // Test-only snapshot of one batch's stage-A candidate lists (sdb_debug_screen_batch).  enqueue_batch fills it when
@@ -267,46 +340,38 @@ struct Corpus : Scratch {
   uint64_t cap = 0, n = 0;
   uint64_t row_base = 0;            // global id of row 0 (row-sharded corpora)
   bool finalized = false;
-  void* d_rows = nullptr;           // master copy, cap x dim (f32 or f64)
-  double* d_mag = nullptr;          // exact f64 magnitude per row (reference arithmetic)
-  float* d_snorm = nullptr;         // cosine: 1/|x| ; euclid: |x|^2 ; NaN = never a screen candidate
-  __nv_bfloat16* d_bf16 = nullptr;  // screen copy cap_pad x dim_pad (rows padded to TILE_ROWS)
+  DevBuf<char> d_rows;              // master copy, cap x dim (f32 or f64)
+  DevBuf<double> d_mag;          // exact f64 magnitude per row (reference arithmetic)
+  DevBuf<float> d_snorm;         // cosine: 1/|x| ; euclid: |x|^2 ; NaN = never a screen candidate
+  DevBuf<__nv_bfloat16> d_bf16;  // screen copy cap_pad x dim_pad (rows padded to TILE_ROWS)
   float bf16_rel_err = 0.00390625f; // max over rows of |x - bf16(x)| / |x| (measured at finalize, rounded up)
-  int8_t* d_i8 = nullptr;           // int8 screen copy cap_pad x dim_pad8 of the normalised rows (one global scale), cosine only
+  DevBuf<int8_t> d_i8;           // int8 screen copy cap_pad x dim_pad8 of the normalised rows (one global scale), cosine only
   uint32_t dim_pad8 = 0;            // multiple of 128
   float max_rel_qerr = 0.f;         // max over rows of |x/|x| - s * x8|
   float i8_scale = 1.f;             // global scale s of the int8 copy
-  uint8_t* d_skip = nullptr;        // optional skip mask
-  uint8_t* d_removed = nullptr;     // tombstones (sdb_corpus_remove); OR-ed with the skip mask at finalize
+  DevBuf<uint8_t> d_skip;        // optional skip mask
+  DevBuf<uint8_t> d_removed;     // tombstones (sdb_corpus_remove); OR-ed with the skip mask at finalize
   uint64_t n_removed = 0;
-  uint32_t* d_special = nullptr;    // rows ranked exactly on every query
+  DevBuf<uint32_t> d_special;    // rows ranked exactly on every query
   uint32_t n_special = 0;
   uint32_t n_outliers = 0;          // of those: rows made special because one component dominates (int8 scale)
   bool special_overflow = false;
   float max_norm = 0.f;
   // exact path scratch
-  uint64_t* d_ex_key = nullptr;  // N keys
-  double* d_ex_val = nullptr;    // N distances (the key maps -0.0 to 0.0; the result returns the value itself)
-  uint32_t* d_sel = nullptr;     // radix-select state
-  uint64_t ex_cap = 0;
-  double* d_fb_q = nullptr;      // fallback query scratch (one query: f64 copy, |q|, flags)
-  double* d_rp_q = nullptr;      // repair sub-batch: the failed queries of a batch, gathered, and their results
-  uint64_t* d_rp_rows = nullptr;
-  double* d_rp_dist = nullptr;
-  uint32_t* d_rp_cnt = nullptr;
-  size_t rp_cap_q = 0, rp_cap_o = 0, rp_cap_n = 0;
-  double* d_fb_qmag = nullptr;
-  uint32_t* d_fb_qflags = nullptr;
-  Scratch sets[2];  // the inactive set's fields are parked here (see Scratch)
+  DevBuf<uint64_t> d_ex_key;  // N keys
+  DevBuf<double> d_ex_val;    // N distances (the key maps -0.0 to 0.0; the result returns the value itself)
+  DevBuf<uint32_t> d_sel;     // radix-select state
+  DevBuf<double> d_fb_q;      // fallback query scratch (one query: f64 copy, |q|, flags)
+  DevBuf<double> d_rp_q;      // repair sub-batch: the failed queries of a batch, gathered, and their results
+  ResultBufs rp;
+  DevBuf<double> d_fb_qmag;
+  DevBuf<uint32_t> d_fb_qflags;
+  Scratch parked;  // the inactive set (see Scratch)
   int active_set = 0;
   cudaEvent_t last_main = nullptr;  // ev_main of the batch whose screen was enqueued last
   // asynchronous batches
   Ticket tickets[N_TICKETS];
   uint32_t next_ticket = 1;
-  // sharded search (comm.cu): this rank's result block + the all-gathered blocks
-  uint8_t* d_block = nullptr;
-  uint8_t* d_gather = nullptr;
-  size_t block_cap = 0, gather_cap = 0;
   sdb_knn_stats stats{};
   std::mutex mu;
 };
@@ -364,8 +429,8 @@ sdb_status stage_decode_vectors(Ctx* ctx, const uint8_t* blob, const uint64_t* o
                                 uint32_t dim, sdb_dtype out_dtype, uint64_t n_rows, void* d_out, uint8_t* d_present,
                                 uint64_t* n_bad, cudaStream_t st, int native = -1);  // native: see stage_vectors_kernel
 sdb_status stage_decode_nodes(Ctx* ctx, const uint8_t* blob, const uint64_t* off, const uint64_t* node_ids, uint64_t n,
-                              uint64_t n_elems, uint64_t** d_row_ptr_out, uint32_t** d_col_idx_out, uint64_t* n_edges,
-                              uint64_t* n_bad, cudaStream_t st);
+                              uint64_t n_elems, DevBuf<uint64_t>* d_row_ptr_out, DevBuf<uint32_t>* d_col_idx_out,
+                              uint64_t* n_edges, uint64_t* n_bad, cudaStream_t st);
 
 inline void count_launch(Ctx* ctx, uint64_t n = 1) { ctx->launches += n; }
 

@@ -230,7 +230,7 @@ static sdb_status launch_ring_q(Corpus* c, uint32_t nq, const PassDesc& p, cudaS
   if (grid > p.count) grid = p.count;
   for (uint32_t q0 = 0; q0 < nq; q0 += QB) {
     const uint32_t nqb = nq - q0 < (uint32_t)QB ? nq - q0 : (uint32_t)QB;
-    kern<<<grid, SIMT_THREADS, smem, st>>>((const float*)c->d_rows, c->d_snorm, c->dim, c->n, c->d_q32, q0, nqb,
+    kern<<<grid, SIMT_THREADS, smem, st>>>((const float*)c->d_rows.get(), c->d_snorm, c->dim, c->n, c->d_q32, q0, nqb,
                                            (int)c->metric, p, c->d_tau, c->d_cand, c->d_cand_cnt, c->sc_cap);
     count_launch(ctx);
   }
@@ -270,7 +270,7 @@ sdb_status screen_simt_pass(Corpus* c, uint32_t nq, const PassDesc& p, cudaStrea
   if (grid > p.count) grid = p.count;
   for (uint32_t q0 = 0; q0 < nq; q0 += SIMT_QB) {
     const uint32_t nqb = nq - q0 < (uint32_t)SIMT_QB ? nq - q0 : (uint32_t)SIMT_QB;
-    screen_simt_generic_kernel<<<grid, 256, q_bytes, st>>>((const float*)c->d_rows, c->d_snorm, c->dim, c->n, c->d_q32, q0,
+    screen_simt_generic_kernel<<<grid, 256, q_bytes, st>>>((const float*)c->d_rows.get(), c->d_snorm, c->dim, c->n, c->d_q32, q0,
                                                           nqb, (int)c->metric, p, c->d_tau, c->d_cand, c->d_cand_cnt,
                                                           c->sc_cap);
     count_launch(ctx);

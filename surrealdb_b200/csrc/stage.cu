@@ -162,52 +162,41 @@ __global__ void __launch_bounds__(256) stage_nodes_kernel(const uint8_t* __restr
 }
 
 // host blob (any memory) -> padded device copy
-static sdb_status blob_to_device(const uint8_t* blob, uint64_t bytes, uint8_t** d_out, cudaStream_t st) {
-  uint8_t* d = nullptr;
-  cudaError_t e = cudaMalloc(&d, bytes + 16);
+static sdb_status blob_to_device(const uint8_t* blob, uint64_t bytes, DevBuf<uint8_t>* d_out, cudaStream_t st) {
+  DevBuf<uint8_t>& d = *d_out;
+  cudaError_t e = d.reserve(bytes + 16);
   if (e != cudaSuccess) {
     set_error("staging: cannot allocate %llu bytes for the value blob: %s", (unsigned long long)bytes, cudaGetErrorString(e));
     return SDB_ENOMEM;
   }
   if (bytes) SDB_CUDA(cudaMemcpyAsync(d, blob, bytes, cudaMemcpyHostToDevice, st));
   SDB_CUDA(cudaMemsetAsync(d + bytes, 0, 16, st));
-  *d_out = d;
   return SDB_OK;
 }
 
 sdb_status stage_decode_vectors(Ctx* ctx, const uint8_t* blob, const uint64_t* off, const uint64_t* ids, uint64_t n,
                                 uint32_t dim, sdb_dtype out_dtype, uint64_t n_rows, void* d_out, uint8_t* d_present,
                                 uint64_t* n_bad, cudaStream_t st, int native) {
-  unsigned long long* d_bad = nullptr;
-  SDB_CUDA(cudaMalloc(&d_bad, 8));
+  DevBuf<unsigned long long> d_bad;
+  SDB_CUDA(d_bad.reserve(1));
   SDB_CUDA(cudaMemsetAsync(d_bad, 0, 8, st));
   // chunked so that the staging copy stays small next to a 10M x 768 index (30 GB of He values)
   const uint64_t CHUNK_BYTES = 512ull << 20, CHUNK_VALS = 4ull << 20;
-  uint8_t* d_blob = nullptr;
-  uint64_t *d_off = nullptr, *d_ids = nullptr;
-  uint64_t cap_bytes = 0, cap_vals = 0;
+  DevBuf<uint8_t> d_blob;
+  DevBuf<uint64_t> d_off, d_ids;
   sdb_status rc = SDB_OK;
   for (uint64_t v0 = 0; v0 < n && rc == SDB_OK;) {
     uint64_t v1 = v0 + 1;
     while (v1 < n && v1 - v0 < CHUNK_VALS && off[v1 + 1] - off[v0] <= CHUNK_BYTES) v1++;
     const uint64_t bytes = off[v1] - off[v0], nv = v1 - v0;
-    if (bytes + 16 > cap_bytes) {
-      cudaFree(d_blob);
-      cap_bytes = bytes + 16;
-      if (cudaMalloc(&d_blob, cap_bytes) != cudaSuccess) {
-        set_error("staging: cannot allocate the %llu-byte staging chunk", (unsigned long long)cap_bytes);
-        rc = SDB_ENOMEM;
-        break;
-      }
+    if (d_blob.reserve(bytes + 16) != cudaSuccess) {
+      set_error("staging: cannot allocate the %llu-byte staging chunk", (unsigned long long)(bytes + 16));
+      rc = SDB_ENOMEM;
+      break;
     }
-    if (nv > cap_vals) {
-      cudaFree(d_off);
-      cudaFree(d_ids);
-      cap_vals = nv;
-      if (cudaMalloc(&d_off, 8 * (cap_vals + 1)) != cudaSuccess || cudaMalloc(&d_ids, 8 * cap_vals) != cudaSuccess) {
-        rc = SDB_ENOMEM;
-        break;
-      }
+    if (d_off.reserve(nv + 1) != cudaSuccess || d_ids.reserve(nv) != cudaSuccess) {
+      rc = SDB_ENOMEM;
+      break;
     }
     auto chk = [&](cudaError_t e) {
       if (e != cudaSuccess && rc == SDB_OK) {
@@ -221,7 +210,7 @@ sdb_status stage_decode_vectors(Ctx* ctx, const uint8_t* blob, const uint64_t* o
     if (ids) chk(cudaMemcpyAsync(d_ids, ids + v0, 8 * nv, cudaMemcpyHostToDevice, st));
     if (rc != SDB_OK) break;
     const unsigned grid = (unsigned)std::min<uint64_t>((nv + 7) / 8, (uint64_t)ctx->sm_count * 16);
-    const uint64_t* d_ids_or_null = ids ? d_ids : nullptr;
+    const uint64_t* d_ids_or_null = ids ? d_ids.get() : nullptr;
     switch (native) {  // sdb_vector_type numbers = SerializedVector variants
       case 0: stage_vectors_kernel<double, 0><<<grid, 256, 0, st>>>(d_blob, off[v0], d_off, d_ids_or_null, v0, nv, dim, n_rows, (double*)d_out, d_present, d_bad); break;
       case 1: stage_vectors_kernel<float, 1><<<grid, 256, 0, st>>>(d_blob, off[v0], d_off, d_ids_or_null, v0, nv, dim, n_rows, (float*)d_out, d_present, d_bad); break;
@@ -230,10 +219,10 @@ sdb_status stage_decode_vectors(Ctx* ctx, const uint8_t* blob, const uint64_t* o
       case 4: stage_vectors_kernel<short, 4><<<grid, 256, 0, st>>>(d_blob, off[v0], d_off, d_ids_or_null, v0, nv, dim, n_rows, (short*)d_out, d_present, d_bad); break;
       default:
         if (out_dtype == SDB_F32)
-          stage_vectors_kernel<float><<<grid, 256, 0, st>>>(d_blob, off[v0], d_off, ids ? d_ids : nullptr, v0, nv, dim, n_rows,
+          stage_vectors_kernel<float><<<grid, 256, 0, st>>>(d_blob, off[v0], d_off, ids ? d_ids.get() : nullptr, v0, nv, dim, n_rows,
                                                             (float*)d_out, d_present, d_bad);
         else
-          stage_vectors_kernel<double><<<grid, 256, 0, st>>>(d_blob, off[v0], d_off, ids ? d_ids : nullptr, v0, nv, dim,
+          stage_vectors_kernel<double><<<grid, 256, 0, st>>>(d_blob, off[v0], d_off, ids ? d_ids.get() : nullptr, v0, nv, dim,
                                                              n_rows, (double*)d_out, d_present, d_bad);
     }
     count_launch(ctx);
@@ -243,83 +232,60 @@ sdb_status stage_decode_vectors(Ctx* ctx, const uint8_t* blob, const uint64_t* o
   }
   unsigned long long h_bad = 0;
   if (rc == SDB_OK && cudaMemcpy(&h_bad, d_bad, 8, cudaMemcpyDeviceToHost) != cudaSuccess) rc = SDB_ECUDA;
-  cudaFree(d_blob);
-  cudaFree(d_off);
-  cudaFree(d_ids);
-  cudaFree(d_bad);
   if (n_bad) *n_bad = h_bad;
   return rc;
 }
 
 sdb_status stage_decode_nodes(Ctx* ctx, const uint8_t* blob, const uint64_t* off, const uint64_t* node_ids, uint64_t n,
-                              uint64_t n_elems, uint64_t** d_row_ptr_out, uint32_t** d_col_idx_out, uint64_t* n_edges,
-                              uint64_t* n_bad, cudaStream_t st) {
-  uint8_t* d_blob = nullptr;
-  uint64_t *d_off = nullptr, *d_ids = nullptr, *d_rp = nullptr, *d_tot = nullptr;
-  uint32_t* d_ci = nullptr;
-  unsigned long long* d_bad = nullptr;
-  sdb_status rc = SDB_OK;
-  auto done = [&](sdb_status s) {
-    cudaFree(d_blob);
-    cudaFree(d_off);
-    cudaFree(d_ids);
-    cudaFree(d_tot);
-    cudaFree(d_bad);
-    if (s != SDB_OK) {
-      cudaFree(d_rp);
-      cudaFree(d_ci);
-    }
-    return s;
-  };
+                              uint64_t n_elems, DevBuf<uint64_t>* d_row_ptr_out, DevBuf<uint32_t>* d_col_idx_out,
+                              uint64_t* n_edges, uint64_t* n_bad, cudaStream_t st) {
+  DevBuf<uint8_t> d_blob;
+  DevBuf<uint64_t> d_off, d_ids, d_rp, d_tot;
+  DevBuf<uint32_t> d_ci;
+  DevBuf<unsigned long long> d_bad;
   const uint64_t bytes = n ? off[n] : 0;
-  if ((rc = blob_to_device(blob, bytes, &d_blob, st)) != SDB_OK) return done(rc);
-  if (cudaMalloc(&d_off, 8 * (n + 1)) != cudaSuccess || cudaMalloc(&d_ids, 8 * (n ? n : 1)) != cudaSuccess ||
-      cudaMalloc(&d_rp, 8 * (n_elems + 1)) != cudaSuccess || cudaMalloc(&d_tot, 8) != cudaSuccess ||
-      cudaMalloc(&d_bad, 8) != cudaSuccess) {
-    set_error("staging: device allocation failed: %s", cudaGetErrorString(cudaGetLastError()));
-    return done(SDB_ENOMEM);
+  SDB_TRY(blob_to_device(blob, bytes, &d_blob, st));
+  cudaError_t e = d_off.reserve(n + 1);
+  if (e == cudaSuccess) e = d_ids.reserve(n ? n : 1);
+  if (e == cudaSuccess) e = d_rp.reserve(n_elems + 1);
+  if (e == cudaSuccess) e = d_tot.reserve(1);
+  if (e == cudaSuccess) e = d_bad.reserve(1);
+  if (e != cudaSuccess) {
+    set_error("staging: device allocation failed: %s", cudaGetErrorString(e));
+    return SDB_ENOMEM;
   }
-#define ST_CUDA(call)                                                          \
-  do {                                                                         \
-    cudaError_t e__ = (call);                                                  \
-    if (e__ != cudaSuccess) {                                                  \
-      set_error("%s:%d: %s -> %s", __FILE__, __LINE__, #call, cudaGetErrorString(e__)); \
-      return done(SDB_ECUDA);                                                  \
-    }                                                                          \
-  } while (0)
   if (n) {
-    ST_CUDA(cudaMemcpyAsync(d_off, off, 8 * (n + 1), cudaMemcpyHostToDevice, st));
-    ST_CUDA(cudaMemcpyAsync(d_ids, node_ids, 8 * n, cudaMemcpyHostToDevice, st));
+    SDB_CUDA(cudaMemcpyAsync(d_off, off, 8 * (n + 1), cudaMemcpyHostToDevice, st));
+    SDB_CUDA(cudaMemcpyAsync(d_ids, node_ids, 8 * n, cudaMemcpyHostToDevice, st));
   }
-  ST_CUDA(cudaMemsetAsync(d_rp, 0, 8 * (n_elems + 1), st));
-  ST_CUDA(cudaMemsetAsync(d_bad, 0, 8, st));
+  SDB_CUDA(cudaMemsetAsync(d_rp, 0, 8 * (n_elems + 1), st));
+  SDB_CUDA(cudaMemsetAsync(d_bad, 0, 8, st));
   const unsigned grid = (unsigned)std::min<uint64_t>((n + 7) / 8 + 1, (uint64_t)ctx->sm_count * 16);
   if (n) {
     stage_nodes_kernel<false><<<grid, 256, 0, st>>>(d_blob, d_off, d_ids, n, n_elems, d_rp, nullptr, d_bad);
     count_launch(ctx);
   }
-  if ((rc = exclusive_scan(ctx, d_rp, d_rp, n_elems + 1, d_tot, st)) != SDB_OK) return done(rc);
+  SDB_TRY(exclusive_scan(ctx, d_rp, d_rp, n_elems + 1, d_tot, st));
   uint64_t total = 0;
-  ST_CUDA(cudaMemcpyAsync(&total, d_tot, 8, cudaMemcpyDeviceToHost, st));
-  ST_CUDA(cudaStreamSynchronize(st));
-  if (cudaMalloc(&d_ci, 4 * (total ? total : 1)) != cudaSuccess) {
+  SDB_CUDA(cudaMemcpyAsync(&total, d_tot, 8, cudaMemcpyDeviceToHost, st));
+  SDB_CUDA(cudaStreamSynchronize(st));
+  if (d_ci.reserve(total ? total : 1) != cudaSuccess) {
     set_error("staging: cannot allocate col_idx for %llu edges", (unsigned long long)total);
-    return done(SDB_ENOMEM);
+    return SDB_ENOMEM;
   }
   if (n) {
     stage_nodes_kernel<true><<<grid, 256, 0, st>>>(d_blob, d_off, d_ids, n, n_elems, d_rp, d_ci, d_bad);
     count_launch(ctx);
   }
   unsigned long long h_bad = 0;
-  ST_CUDA(cudaMemcpyAsync(&h_bad, d_bad, 8, cudaMemcpyDeviceToHost, st));
-  ST_CUDA(cudaStreamSynchronize(st));
-  ST_CUDA(cudaGetLastError());
-#undef ST_CUDA
-  *d_row_ptr_out = d_rp;
-  *d_col_idx_out = d_ci;
+  SDB_CUDA(cudaMemcpyAsync(&h_bad, d_bad, 8, cudaMemcpyDeviceToHost, st));
+  SDB_CUDA(cudaStreamSynchronize(st));
+  SDB_CUDA(cudaGetLastError());
+  *d_row_ptr_out = std::move(d_rp);
+  *d_col_idx_out = std::move(d_ci);
   if (n_edges) *n_edges = total;
   if (n_bad) *n_bad = h_bad;
-  return done(SDB_OK);
+  return SDB_OK;
 }
 
 }  // namespace sdb
@@ -350,8 +316,8 @@ sdb_status sdb_stage_decode_nodes(sdb_ctx* ctx, const uint8_t* blob, const uint6
   }
   std::lock_guard<std::mutex> guard(ctx->mu);
   SDB_CUDA(cudaSetDevice(ctx->device));
-  uint64_t* d_rp = nullptr;
-  uint32_t* d_ci = nullptr;
+  DevBuf<uint64_t> d_rp;
+  DevBuf<uint32_t> d_ci;
   uint64_t total = 0;
   SDB_TRY(stage_decode_nodes(ctx, blob, off, node_ids, n, n_elems, &d_rp, &d_ci, &total, n_bad, ctx->stream));
   uint64_t* h_rp = (uint64_t*)malloc(8 * (n_elems + 1));
@@ -361,8 +327,6 @@ sdb_status sdb_stage_decode_nodes(sdb_ctx* ctx, const uint8_t* blob, const uint6
     e = cudaMemcpy(h_rp, d_rp, 8 * (n_elems + 1), cudaMemcpyDeviceToHost);
     if (e == cudaSuccess && total) e = cudaMemcpy(h_ci, d_ci, 4 * total, cudaMemcpyDeviceToHost);
   }
-  cudaFree(d_rp);
-  cudaFree(d_ci);
   if (!h_rp || !h_ci || e != cudaSuccess) {
     free(h_rp);
     free(h_ci);

@@ -81,3 +81,8 @@ assert S.decode_vectors(ctx, items, 7, out.data_ptr(), 4, "F64") == 0
 torch.cuda.synchronize()
 assert out.cpu().numpy()[3].tolist() == [3, 4, 5, 6, 7, 8, 9]
 print("filtered walk / staging ok", flush=True)
+# every handle and the context are closed, so that --leak-check full sees what the library failed to release
+for handle in (col, big, idx, idx2, gr):
+    handle.close()
+ctx.close()
+print("closed", flush=True)
