@@ -468,6 +468,35 @@ void sdb_device_free(sdb_ctx*, void* d_ptr);
 /* +collect BFS: first-seen dedup, emits from min_depth, start only marked seen when inclusive. */
 sdb_status sdb_graph_collect(sdb_graph*, const uint32_t* start, uint64_t n_start, uint32_t min_depth,
                              uint32_t max_depth, int inclusive, uint32_t** out_ids, uint64_t* out_n);
+
+/* ---- WHERE-filtered hops: `->(edge WHERE c1)->(node WHERE c2)`, which the reference plans as GraphScanOutput::FullEdge
+ *      followed by a Filter (exec/planner/source.rs, plan_lookup_with_input).  The caller evaluates each condition into a
+ *      bitmap (bit i = bit i % 32 of word i / 32):
+ *        edge_bits    one bit per CSR position p (ceil(n_edges / 32) words): the edge record behind p satisfies the
+ *                     hop's edge condition.  A `<->` CSR holds each edge record at two positions per endpoint; set both.
+ *        target_bits  one bit per node id (ceil(n_rows / 32) words): node v satisfies the target condition.  Needs every
+ *                     target id below n_rows (SDB_EINVAL otherwise).
+ *      Position p passes iff (edge_bits == NULL || bit p) && (target_bits == NULL || bit col_idx[p]).  The result is the
+ *      unfiltered call's, order and duplicates included, with the failing positions removed; per_source_limit = n > 0
+ *      keeps each source's first n PASSING positions.  A NULL filter array, or a hop whose two bitmaps are NULL, runs
+ *      that hop unfiltered.  Shard handles are refused (SDB_EUNSUPPORTED). */
+typedef struct {
+  const uint32_t* edge_bits;
+  const uint32_t* target_bits;
+} sdb_hop_filter;
+/* filters: n_hops entries or NULL; the bitmaps are host memory, copied for this call */
+sdb_status sdb_graph_expand_filtered(sdb_graph* const* hops, const sdb_hop_filter* filters, uint32_t n_hops,
+                                     const uint32_t* frontier, uint64_t n_frontier, uint32_t per_source_limit,
+                                     uint32_t** out_ids, uint64_t* out_n);
+/* device-resident variant: the bitmaps (the filters array itself is host memory), d_frontier and *d_out_ids are device
+ * pointers; *d_out_ids is library-owned (sdb_device_free) */
+sdb_status sdb_graph_expand_filtered_device(sdb_graph* const* hops, const sdb_hop_filter* filters, uint32_t n_hops,
+                                            const uint32_t* d_frontier, uint64_t n_frontier, uint32_t per_source_limit,
+                                            uint32_t** d_out_ids, uint64_t* out_n);
+/* +collect whose every BFS level is the filtered hop (host bitmaps); the start set itself is not filtered */
+sdb_status sdb_graph_collect_filtered(sdb_graph*, const sdb_hop_filter* filter, const uint32_t* start, uint64_t n_start,
+                                      uint32_t min_depth, uint32_t max_depth, int inclusive, uint32_t** out_ids,
+                                      uint64_t* out_n);
 void sdb_free(void*);
 
 #ifdef __cplusplus

@@ -10,6 +10,7 @@
 // `+collect` (exec/operators/recursion/collect.rs:74-143) adds a first-seen de-duplication per BFS level.
 //
 // Algorithmic bytes per hop: 16|F| (two row_ptr reads per source) + 4|E_h| (col_idx) + 4|E_h| (output).
+// A WHERE-filtered hop (filter_kernel, below) scans every candidate edge of its sources, even with a per-source limit.
 #include "internal.cuh"
 
 namespace sdb {
@@ -271,6 +272,207 @@ __global__ void collect_compact_kernel(const uint32_t* __restrict__ lvl, uint64_
   }
 }
 
+// ---- filtered hop: a WHERE condition on the edge records and/or the target records, evaluated by the caller ----------
+// into bitmaps (bit i = bit i % 32 of word i / 32).  CSR position p with target t passes iff
+// (edge_bits == nullptr || bit p of edge_bits) && (target_bits == nullptr || bit t of target_bits); the result is the
+// unfiltered hop's with the failing positions removed, and a per-source limit keeps each source's first n PASSING ones.
+//
+// The candidate space is the unfiltered hop's output [0, T) (degree_kernel without a limit + exclusive_scan).  It is
+// split into equal runs of EXP_TILE-candidate tiles, one run per block of a fixed grid, and filter_kernel walks each run
+// twice: the COUNT pass counts the passing candidates per block (and per source when a limit is set), the WRITE pass
+// recomputes the flags and writes the passing targets compacted, in order.  T stays on the device, so a hop synchronises
+// with the host once, for its output size, and the unfiltered level is never written.
+using HopFilter = sdb_hop_filter;  // with device bitmaps; nullptr = no condition on that side
+
+__device__ __forceinline__ bool bit_set(const uint32_t* bits, uint64_t i) { return (__ldg(bits + (i >> 5)) >> (i & 31)) & 1u; }
+// the pass flag of CSR position p whose target is t: the one definition every filtered hop and +collect level uses
+__device__ __forceinline__ bool hop_pass(const HopFilter& f, uint64_t p, uint32_t t) {
+  return (!f.edge_bits || bit_set(f.edge_bits, p)) && (!f.target_bits || bit_set(f.target_bits, t));
+}
+
+// COUNT: blk[b] = passing candidates of block b's run; with a limit also src_cnt[i] += passing candidates of source i.
+// WRITE: blk = exclusive scan of the COUNT blk (so blk[b] + the passing candidates before a candidate in b's run = its
+//        rank among all passing ones); with a limit, src_cnt = exclusive scan of the per-source passing counts and
+//        src_out = exclusive scan of min(count, limit): the r-th passing candidate of source i goes to src_out[i] + r
+//        when r < limit.
+template <bool WRITE>
+__global__ void __launch_bounds__(EXP_THREADS) filter_kernel(const uint64_t* __restrict__ row_ptr,
+                                                             const uint32_t* __restrict__ col_idx, uint64_t n_rows,
+                                                             const uint32_t* __restrict__ frontier, uint64_t n_f,
+                                                             const uint64_t* __restrict__ off /* n_f + 1, off[n_f] = T */,
+                                                             HopFilter f, uint32_t limit, uint64_t* __restrict__ blk,
+                                                             uint64_t* __restrict__ src_cnt,
+                                                             const uint64_t* __restrict__ src_out, uint32_t* __restrict__ out) {
+  __shared__ uint64_t s_off[EXP_SRC_MAX];
+  __shared__ uint64_t s_row[EXP_SRC_MAX];
+  __shared__ uint32_t s_cnt[WRITE ? 1 : EXP_SRC_MAX];  // COUNT with a limit: passing candidates per source of the tile
+  __shared__ uint64_t s_warp[EXP_THREADS / 32];
+  __shared__ uint64_t s_i0, s_i1;
+  const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const uint64_t T = off[n_f];
+  const uint64_t n_tiles = (T + EXP_TILE - 1) / EXP_TILE;
+  const uint64_t t_end = n_tiles * (blockIdx.x + 1) / gridDim.x;
+  uint64_t base = WRITE ? blk[blockIdx.x] : 0;  // WRITE: passing candidates before the current round (block-uniform)
+  uint64_t mine = 0;                            // COUNT: passing candidates this thread saw
+  for (uint64_t tile = n_tiles * blockIdx.x / gridDim.x; tile < t_end; tile++) {
+    const uint64_t o0 = tile * EXP_TILE;
+    const uint64_t o1 = o0 + EXP_TILE < T ? o0 + EXP_TILE : T;
+    if (threadIdx.x == 0) {
+      s_i0 = upper_bound_minus1(off, 0, n_f + 1, o0);
+      s_i1 = upper_bound_minus1(off, 0, n_f + 1, o1 - 1);
+    }
+    __syncthreads();
+    const uint64_t i0 = s_i0, i1 = s_i1;
+    const bool in_smem = (i1 - i0 + 2) <= (uint64_t)EXP_SRC_MAX;
+    if (in_smem) {
+      for (uint64_t t = threadIdx.x; t < i1 - i0 + 2; t += EXP_THREADS) {
+        const uint64_t i = i0 + t;
+        s_off[t] = off[i];
+        // a frontier id out of range has degree 0 (degree_kernel flagged it; the hop fails after this pass): never read
+        s_row[t] = i < n_f && frontier[i] < n_rows ? row_ptr[frontier[i]] : 0;
+        if (!WRITE) s_cnt[t] = 0;
+      }
+    }
+    __syncthreads();
+#pragma unroll
+    for (int u = 0; u < EXP_PER_THREAD; u++) {  // every thread runs every round: the warp votes below need all lanes
+      const uint64_t o = o0 + (uint64_t)u * EXP_THREADS + threadIdx.x;
+      uint64_t src = 0, p = 0;
+      uint32_t t = 0;
+      bool pass = false;
+      if (o < o1) {
+        uint64_t start, rbeg;
+        if (in_smem) {
+          const uint64_t k = upper_bound_minus1(s_off, 0, i1 - i0 + 2, o);
+          src = i0 + k;
+          start = s_off[k];
+          rbeg = s_row[k];
+        } else {  // pathological: thousands of zero-degree sources inside this tile
+          src = upper_bound_minus1(off, i0, i1 + 2, o);
+          start = off[src];
+          rbeg = row_ptr[frontier[src]];  // src owns candidate o, so its id is in range
+        }
+        p = rbeg + (o - start);
+        if (f.target_bits) t = __ldg(col_idx + p);
+        pass = hop_pass(f, p, t);
+      }
+      if (!WRITE) {
+        mine += pass;
+        if (limit) {  // one atomic per (warp, source): a hub's candidates fill whole warps
+          const uint32_t peers = __match_any_sync(0xFFFFFFFFu, pass ? src : ~0ull);
+          if (pass && lane == (uint32_t)(__ffs(peers) - 1)) {
+            if (in_smem) atomicAdd(&s_cnt[src - i0], (uint32_t)__popc(peers));
+            else atomicAdd((unsigned long long*)&src_cnt[src], (unsigned long long)__popc(peers));
+          }
+        }
+      } else {
+        const uint32_t vote = __ballot_sync(0xFFFFFFFFu, pass);
+        if (lane == 0) s_warp[warp] = __popc(vote);
+        __syncthreads();
+        uint64_t rank = base + __popc(vote & ((1u << lane) - 1u)), round = 0;
+        for (uint32_t w = 0; w < EXP_THREADS / 32; w++) {
+          if (w < warp) rank += s_warp[w];
+          round += s_warp[w];
+        }
+        if (pass) {
+          const uint64_t r = limit ? rank - src_cnt[src] : 0;
+          if (r < limit || !limit) {
+            // an edge condition alone reads only the targets it writes (a limit drops most passing ones)
+            if (!f.target_bits) t = __ldg(col_idx + p);
+            out[limit ? src_out[src] + r : rank] = t;
+          }
+        }
+        base += round;
+        __syncthreads();  // s_warp is rewritten by the next round
+      }
+    }
+    if (!WRITE && limit && in_smem) {
+      __syncthreads();
+      for (uint64_t t = threadIdx.x; t < i1 - i0 + 1; t += EXP_THREADS)
+        if (s_cnt[t]) atomicAdd((unsigned long long*)&src_cnt[i0 + t], (unsigned long long)s_cnt[t]);
+    }
+    __syncthreads();  // the next tile rewrites the shared tables
+  }
+  if (!WRITE) {
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) mine += __shfl_down_sync(0xFFFFFFFFu, mine, o);
+    if (lane == 0) s_warp[warp] = mine;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+      uint64_t s = 0;
+      for (int w = 0; w < EXP_THREADS / 32; w++) s += s_warp[w];
+      blk[blockIdx.x] = s;
+    }
+  }
+}
+
+__global__ void clamp_kernel(const uint64_t* __restrict__ cnt, uint64_t n, uint32_t limit, uint64_t* __restrict__ out) {
+  const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n) out[i] = cnt[i] < limit ? cnt[i] : limit;
+}
+
+// the filtered counterpart of hop_device (same contract); the graph is unsharded and f's bitmaps are device memory
+static sdb_status hop_filtered(Graph* g, const HopFilter& f, const uint32_t* d_frontier, uint64_t n_f, uint32_t limit,
+                               AsyncBuf<uint32_t>* d_out, uint64_t* n_out, cudaStream_t st) {
+  Ctx* ctx = g->ctx;
+  *n_out = 0;
+  if (n_f == 0) return SDB_OK;
+  // one run of tiles per resident block; both passes must use the same grid
+  int occ_count = 0, occ_write = 0;
+  SDB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_count, filter_kernel<false>, EXP_THREADS, 0));
+  SDB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_write, filter_kernel<true>, EXP_THREADS, 0));
+  const uint64_t grid = (uint64_t)ctx->sm_count * std::max(1, std::min(occ_count, occ_write));
+  AsyncBuf<uint64_t> d_off, d_blk, d_src, d_src_out;
+  AsyncBuf<uint32_t> d_err;
+  SDB_CUDA(d_off.reserve(n_f + 2, st));
+  SDB_CUDA(d_blk.reserve(grid + 1, st));
+  SDB_CUDA(d_err.reserve(1, st));
+  SDB_CUDA(cudaMemsetAsync(d_err, 0, 4, st));
+  if (limit) {
+    SDB_CUDA(d_src.reserve(n_f + 1, st));
+    SDB_CUDA(d_src_out.reserve(n_f + 1, st));
+    SDB_CUDA(cudaMemsetAsync(d_src, 0, sizeof(uint64_t) * n_f, st));
+  }
+  degree_kernel<<<(unsigned)((n_f + 255) / 256), 256, 0, st>>>(g->d_row_ptr, g->n_rows, 0, g->n_rows, d_frontier, n_f, 0,
+                                                               d_off, d_err);
+  count_launch(ctx);
+  SDB_TRY(exclusive_scan(ctx, d_off, d_off, n_f, d_off + n_f, st));
+  filter_kernel<false><<<(unsigned)grid, EXP_THREADS, 0, st>>>(g->d_row_ptr, g->d_col_idx, g->n_rows, d_frontier, n_f, d_off,
+                                                                f, limit, d_blk, d_src, nullptr, nullptr);
+  count_launch(ctx);
+  SDB_TRY(exclusive_scan(ctx, d_blk, d_blk, grid, d_blk + grid, st));
+  const uint64_t* d_total = d_blk + grid;
+  if (limit) {
+    clamp_kernel<<<(unsigned)((n_f + 255) / 256), 256, 0, st>>>(d_src, n_f, limit, d_src_out);
+    count_launch(ctx);
+    SDB_TRY(exclusive_scan(ctx, d_src, d_src, n_f, d_src + n_f, st));
+    SDB_TRY(exclusive_scan(ctx, d_src_out, d_src_out, n_f, d_src_out + n_f, st));
+    d_total = d_src_out + n_f;
+  }
+  uint64_t total = 0;
+  uint32_t err = 0;
+  SDB_CUDA(cudaMemcpyAsync(&total, d_total, 8, cudaMemcpyDeviceToHost, st));
+  SDB_CUDA(cudaMemcpyAsync(&err, d_err, 4, cudaMemcpyDeviceToHost, st));
+  SDB_CUDA(cudaStreamSynchronize(st));
+  if (err) {
+    set_error("graph expand: frontier id out of range (graph has %llu rows)", (unsigned long long)g->n_rows);
+    return SDB_EINVAL;
+  }
+  if (total > 0xFFFFFFF0ull) {
+    set_error("graph expand: %llu results exceed the 2^32 frontier limit", (unsigned long long)total);
+    return SDB_EOVERFLOW;
+  }
+  if (total) {
+    SDB_CUDA(d_out->reserve(total, st));
+    filter_kernel<true><<<(unsigned)grid, EXP_THREADS, 0, st>>>(g->d_row_ptr, g->d_col_idx, g->n_rows, d_frontier, n_f,
+                                                                 d_off, f, limit, d_blk, d_src, d_src_out, *d_out);
+    count_launch(ctx);
+  }
+  SDB_CUDA(cudaGetLastError());
+  *n_out = total;
+  return SDB_OK;
+}
+
 }  // namespace sdb
 
 struct sdb_graph : sdb::Graph {};
@@ -351,9 +553,13 @@ void sdb_graph_destroy(sdb_graph* g) {
   delete g;
 }
 
-// device-resident core: frontier and result stay in HBM (sdb_graph_expand_device hands the result to the caller)
+static bool has_filter(const HopFilter* f) { return f && (f->edge_bits || f->target_bits); }
+
+// device-resident core: frontier and result stay in HBM (sdb_graph_expand_device hands the result to the caller).
+// filters: nullptr, or one per hop (device bitmaps); a hop without bitmaps runs the unfiltered hop
 static sdb_status graph_expand_dev(sdb_graph* const* hops, uint32_t n_hops, const uint32_t* d_frontier, uint64_t n_frontier,
-                                   uint32_t per_source_limit, AsyncBuf<uint32_t>* d_out, uint64_t* out_n, cudaStream_t st) {
+                                   uint32_t per_source_limit, AsyncBuf<uint32_t>* d_out, uint64_t* out_n, cudaStream_t st,
+                                   const HopFilter* filters = nullptr) {
   AsyncBuf<uint32_t> d_f;
   uint64_t n_f = n_frontier;
   bool owned = false;  // the caller's frontier is never freed
@@ -364,7 +570,11 @@ static sdb_status graph_expand_dev(sdb_graph* const* hops, uint32_t n_hops, cons
       set_error("query cancelled");
       return SDB_ECANCELLED;
     }
-    SDB_TRY(hop_device(hops[h], owned ? d_f.get() : d_frontier, n_f, per_source_limit, &d_next, &n_next, st));
+    const uint32_t* d_in = owned ? d_f.get() : d_frontier;
+    if (filters && has_filter(&filters[h]))
+      SDB_TRY(hop_filtered(hops[h], filters[h], d_in, n_f, per_source_limit, &d_next, &n_next, st));
+    else
+      SDB_TRY(hop_device(hops[h], d_in, n_f, per_source_limit, &d_next, &n_next, st));
     d_f = std::move(d_next);
     owned = true;
     n_f = n_next;
@@ -378,6 +588,55 @@ static sdb_status graph_expand_dev(sdb_graph* const* hops, uint32_t n_hops, cons
   return SDB_OK;
 }
 
+// what the filtered entry points refuse: shard handles, and a target condition on a CSR whose targets leave its rows
+// (target_bits has one bit per row)
+static sdb_status check_filtered(const sdb_graph* g, const sdb_hop_filter* f, const char* fn) {
+  if (g->sharded) {
+    set_error("%s: filtered hops are not served on shard handles (sdb_graph_load_csr_shard)", fn);
+    return SDB_EUNSUPPORTED;
+  }
+  if (f && f->target_bits && !g->targets_in_rows) {
+    set_error("%s: a target condition needs every target id below the graph's row count", fn);
+    return SDB_EINVAL;
+  }
+  return SDB_OK;
+}
+
+// copies host bitmaps to the device: ceil(n_edges / 32) words of edge bits and ceil(n_rows / 32) of target bits per
+// graph.  dev[i] holds the device copies of host[i]; bufs owns them.
+static sdb_status upload_filters(sdb_graph* const* graphs, const sdb_hop_filter* host, uint32_t n,
+                                 std::vector<AsyncBuf<uint32_t>>* bufs, std::vector<HopFilter>* dev, cudaStream_t st) {
+  bufs->resize(2 * (size_t)n);
+  dev->assign(n, HopFilter{nullptr, nullptr});
+  for (uint32_t h = 0; h < n; h++) {
+    const uint32_t* src[2] = {host[h].edge_bits, host[h].target_bits};
+    const uint64_t words[2] = {(graphs[h]->n_edges + 31) / 32, (graphs[h]->n_rows + 31) / 32};
+    const uint32_t* dst[2] = {nullptr, nullptr};
+    for (int k = 0; k < 2; k++) {
+      if (!src[k] || !words[k]) continue;  // no positions (or no rows) to test: no bitmap needed
+      AsyncBuf<uint32_t>& b = (*bufs)[2 * (size_t)h + k];
+      SDB_CUDA(b.reserve(words[k], st));
+      SDB_CUDA(cudaMemcpyAsync(b, src[k], sizeof(uint32_t) * words[k], cudaMemcpyHostToDevice, st));
+      dst[k] = b;
+    }
+    (*dev)[h] = HopFilter{dst[0], dst[1]};
+  }
+  return SDB_OK;
+}
+
+static sdb_status expand_device_call(sdb_graph* const* hops, const sdb_hop_filter* d_filters, uint32_t n_hops,
+                                     const uint32_t* d_frontier, uint64_t n_frontier, uint32_t per_source_limit,
+                                     uint32_t** d_out_ids, uint64_t* out_n) {
+  Ctx* ctx = hops[0]->ctx;
+  std::lock_guard<std::mutex> guard(ctx->mu);
+  SDB_CUDA(cudaSetDevice(ctx->device));
+  AsyncBuf<uint32_t> d_out;
+  SDB_TRY(graph_expand_dev(hops, n_hops, d_frontier, n_frontier, per_source_limit, &d_out, out_n, ctx->stream, d_filters));
+  *d_out_ids = d_out.release();
+  SDB_CUDA(cudaStreamSynchronize(ctx->stream));
+  return SDB_OK;
+}
+
 sdb_status sdb_graph_expand_device(sdb_graph* const* hops, uint32_t n_hops, const uint32_t* d_frontier, uint64_t n_frontier,
                                    uint32_t per_source_limit, uint32_t** d_out_ids, uint64_t* out_n) {
   if (!hops || !n_hops || !d_out_ids || !out_n || (n_frontier && !d_frontier)) return SDB_EINVAL;
@@ -385,14 +644,20 @@ sdb_status sdb_graph_expand_device(sdb_graph* const* hops, uint32_t n_hops, cons
   *out_n = 0;
   for (uint32_t h = 0; h < n_hops; h++)
     if (!hops[h]) return SDB_EINVAL;
-  Ctx* ctx = hops[0]->ctx;
-  std::lock_guard<std::mutex> guard(ctx->mu);
-  SDB_CUDA(cudaSetDevice(ctx->device));
-  AsyncBuf<uint32_t> d_out;
-  SDB_TRY(graph_expand_dev(hops, n_hops, d_frontier, n_frontier, per_source_limit, &d_out, out_n, ctx->stream));
-  *d_out_ids = d_out.release();
-  SDB_CUDA(cudaStreamSynchronize(ctx->stream));
-  return SDB_OK;
+  return expand_device_call(hops, nullptr, n_hops, d_frontier, n_frontier, per_source_limit, d_out_ids, out_n);
+}
+
+sdb_status sdb_graph_expand_filtered_device(sdb_graph* const* hops, const sdb_hop_filter* filters, uint32_t n_hops,
+                                            const uint32_t* d_frontier, uint64_t n_frontier, uint32_t per_source_limit,
+                                            uint32_t** d_out_ids, uint64_t* out_n) {
+  if (!hops || !n_hops || !d_out_ids || !out_n || (n_frontier && !d_frontier)) return SDB_EINVAL;
+  *d_out_ids = nullptr;
+  *out_n = 0;
+  for (uint32_t h = 0; h < n_hops; h++) {
+    if (!hops[h]) return SDB_EINVAL;
+    SDB_TRY(check_filtered(hops[h], filters ? &filters[h] : nullptr, "sdb_graph_expand_filtered_device"));
+  }
+  return expand_device_call(hops, filters, n_hops, d_frontier, n_frontier, per_source_limit, d_out_ids, out_n);
 }
 
 void sdb_device_free(sdb_ctx* ctx, void* d_ptr) {
@@ -401,17 +666,17 @@ void sdb_device_free(sdb_ctx* ctx, void* d_ptr) {
   AsyncBuf<uint32_t>::free_released(d_ptr, ctx->stream);
 }
 
-sdb_status sdb_graph_expand(sdb_graph* const* hops, uint32_t n_hops, const uint32_t* frontier, uint64_t n_frontier,
-                            uint32_t per_source_limit, uint32_t** out_ids, uint64_t* out_n) {
-  if (!hops || !n_hops || !out_ids || !out_n || (n_frontier && !frontier)) return SDB_EINVAL;
-  *out_ids = nullptr;
-  *out_n = 0;
-  for (uint32_t h = 0; h < n_hops; h++)
-    if (!hops[h]) return SDB_EINVAL;
+// host frontier and result; filters: nullptr or one per hop, host bitmaps (copied for this call)
+static sdb_status expand_host_call(sdb_graph* const* hops, const sdb_hop_filter* filters, uint32_t n_hops,
+                                   const uint32_t* frontier, uint64_t n_frontier, uint32_t per_source_limit,
+                                   uint32_t** out_ids, uint64_t* out_n) {
   Ctx* ctx = hops[0]->ctx;
   std::lock_guard<std::mutex> guard(ctx->mu);
   SDB_CUDA(cudaSetDevice(ctx->device));
   cudaStream_t st = ctx->stream;
+  std::vector<AsyncBuf<uint32_t>> bits;
+  std::vector<HopFilter> d_filters;
+  if (filters) SDB_TRY(upload_filters(hops, filters, n_hops, &bits, &d_filters, st));
   AsyncBuf<uint32_t> d_in;
   if (n_frontier) {
     SDB_CUDA(d_in.reserve(n_frontier, st));
@@ -419,7 +684,8 @@ sdb_status sdb_graph_expand(sdb_graph* const* hops, uint32_t n_hops, const uint3
   }
   AsyncBuf<uint32_t> d_f;
   uint64_t n_f = 0;
-  SDB_TRY(graph_expand_dev(hops, n_hops, d_in, n_frontier, per_source_limit, &d_f, &n_f, st));
+  SDB_TRY(graph_expand_dev(hops, n_hops, d_in, n_frontier, per_source_limit, &d_f, &n_f, st,
+                           filters ? d_filters.data() : nullptr));
   d_in.reset();
   if (n_f) {
     uint32_t* h_out = (uint32_t*)malloc(sizeof(uint32_t) * n_f);
@@ -440,11 +706,32 @@ sdb_status sdb_graph_expand(sdb_graph* const* hops, uint32_t n_hops, const uint3
   return SDB_OK;
 }
 
-sdb_status sdb_graph_collect(sdb_graph* g, const uint32_t* start, uint64_t n_start, uint32_t min_depth,
-                             uint32_t max_depth, int inclusive, uint32_t** out_ids, uint64_t* out_n) {
-  if (!g || !out_ids || !out_n || (n_start && !start)) return SDB_EINVAL;
+sdb_status sdb_graph_expand(sdb_graph* const* hops, uint32_t n_hops, const uint32_t* frontier, uint64_t n_frontier,
+                            uint32_t per_source_limit, uint32_t** out_ids, uint64_t* out_n) {
+  if (!hops || !n_hops || !out_ids || !out_n || (n_frontier && !frontier)) return SDB_EINVAL;
   *out_ids = nullptr;
   *out_n = 0;
+  for (uint32_t h = 0; h < n_hops; h++)
+    if (!hops[h]) return SDB_EINVAL;
+  return expand_host_call(hops, nullptr, n_hops, frontier, n_frontier, per_source_limit, out_ids, out_n);
+}
+
+sdb_status sdb_graph_expand_filtered(sdb_graph* const* hops, const sdb_hop_filter* filters, uint32_t n_hops,
+                                     const uint32_t* frontier, uint64_t n_frontier, uint32_t per_source_limit,
+                                     uint32_t** out_ids, uint64_t* out_n) {
+  if (!hops || !n_hops || !out_ids || !out_n || (n_frontier && !frontier)) return SDB_EINVAL;
+  *out_ids = nullptr;
+  *out_n = 0;
+  for (uint32_t h = 0; h < n_hops; h++) {
+    if (!hops[h]) return SDB_EINVAL;
+    SDB_TRY(check_filtered(hops[h], filters ? &filters[h] : nullptr, "sdb_graph_expand_filtered"));
+  }
+  return expand_host_call(hops, filters, n_hops, frontier, n_frontier, per_source_limit, out_ids, out_n);
+}
+
+// +collect; filter: nullptr, or host bitmaps applied at every BFS level (the start set is not filtered)
+static sdb_status collect_call(sdb_graph* g, const sdb_hop_filter* filter, const uint32_t* start, uint64_t n_start,
+                               uint32_t min_depth, uint32_t max_depth, int inclusive, uint32_t** out_ids, uint64_t* out_n) {
   Ctx* ctx = g->ctx;
   std::lock_guard<std::mutex> guard(ctx->mu);
   SDB_CUDA(cudaSetDevice(ctx->device));
@@ -459,6 +746,11 @@ sdb_status sdb_graph_collect(sdb_graph* g, const uint32_t* start, uint64_t n_sta
       set_error("graph collect: start id out of range");
       return SDB_EINVAL;
     }
+  std::vector<AsyncBuf<uint32_t>> bits;
+  std::vector<HopFilter> d_filter;
+  sdb_graph* graphs[1] = {g};
+  if (filter) SDB_TRY(upload_filters(graphs, filter, 1, &bits, &d_filter, st));
+  const bool filtered = filter && has_filter(&d_filter[0]);
   // the stream-ordered temporaries below are released on every return path, then the stream is drained
   struct Drain {
     cudaStream_t st;
@@ -497,7 +789,10 @@ sdb_status sdb_graph_collect(sdb_graph* g, const uint32_t* start, uint64_t n_sta
     }
     AsyncBuf<uint32_t> d_lvl;
     uint64_t n_lvl = 0;
-    SDB_TRY(hop_device(g, d_f, n_f, 0, &d_lvl, &n_lvl, st));
+    if (filtered)
+      SDB_TRY(hop_filtered(g, d_filter[0], d_f, n_f, 0, &d_lvl, &n_lvl, st));
+    else
+      SDB_TRY(hop_device(g, d_f, n_f, 0, &d_lvl, &n_lvl, st));
     d_f.reset();
     n_f = 0;
     if (n_lvl) {
@@ -553,6 +848,24 @@ sdb_status sdb_graph_collect(sdb_graph* g, const uint32_t* start, uint64_t n_sta
     *out_n = n_res;
   }
   return SDB_OK;
+}
+
+sdb_status sdb_graph_collect(sdb_graph* g, const uint32_t* start, uint64_t n_start, uint32_t min_depth,
+                             uint32_t max_depth, int inclusive, uint32_t** out_ids, uint64_t* out_n) {
+  if (!g || !out_ids || !out_n || (n_start && !start)) return SDB_EINVAL;
+  *out_ids = nullptr;
+  *out_n = 0;
+  return collect_call(g, nullptr, start, n_start, min_depth, max_depth, inclusive, out_ids, out_n);
+}
+
+sdb_status sdb_graph_collect_filtered(sdb_graph* g, const sdb_hop_filter* filter, const uint32_t* start, uint64_t n_start,
+                                      uint32_t min_depth, uint32_t max_depth, int inclusive, uint32_t** out_ids,
+                                      uint64_t* out_n) {
+  if (!g || !out_ids || !out_n || (n_start && !start)) return SDB_EINVAL;
+  *out_ids = nullptr;
+  *out_n = 0;
+  SDB_TRY(check_filtered(g, filter, "sdb_graph_collect_filtered"));
+  return collect_call(g, filter, start, n_start, min_depth, max_depth, inclusive, out_ids, out_n);
 }
 
 }  // extern "C"

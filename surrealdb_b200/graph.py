@@ -8,6 +8,9 @@
                       exec/planner/idiom.rs:161-193): multiset, order-preserving
   GraphStore.collect  `.{min..max+collect[+inclusive]}` (exec/operators/recursion/collect.rs:74-143)
   GraphStore.recurse  default `.{min..max}` recursion (exec/operators/recursion/default.rs:75-133)
+  GraphStore.lookup_filtered / collect_filtered / recurse_filtered
+                      the same with WHERE conditions on the edge and target records, evaluated into bitmaps
+                      (hop_masks) for sdb_graph_expand_filtered / sdb_graph_collect_filtered
   GraphEdgeScan       the operator itself: new(input, direction, edge_tables, output_mode, version).with_limit(n)
                       (exec/operators/scan/graph.rs:89-147) -- name(), attrs(), execute()
 """
@@ -99,6 +102,75 @@ def collect(graph, start, min_depth=1, max_depth=0, inclusive=False):
     return _take(out, n)
 
 
+class HopFilter(C.Structure):
+    """sdb_hop_filter"""
+    _fields_ = [("edge_bits", C.c_void_p), ("target_bits", C.c_void_p)]
+
+
+def pack_bits(mask):
+    """a bitmap for the filtered calls: uint32 words (bit i = bit i % 32 of word i // 32) are taken as they are, a bool
+    array (one entry per CSR position or node id) is packed"""
+    a = np.asarray(mask)
+    if a.dtype == np.uint32:
+        return np.ascontiguousarray(a)
+    if a.dtype != np.bool_:
+        raise TypeError(f"bitmap: expected uint32 words or a bool mask, got {a.dtype}")
+    b = np.packbits(a, bitorder="little")
+    b = np.concatenate([b, np.zeros(-b.size % 4, np.uint8)])
+    return b.view("<u4").astype(np.uint32)
+
+
+def _filters(filters, n, on_device):
+    """(edge_bits, target_bits) or None per hop -> (sdb_hop_filter array, the packed host arrays it points into)"""
+    if len(filters) != n:
+        raise ValueError(f"{len(filters)} filters for {n} hops")
+    arr, keep = (HopFilter * n)(), []
+    for h, f in enumerate(filters):
+        for name, m in zip(("edge_bits", "target_bits"), f or (None, None)):
+            if m is None:
+                continue
+            if on_device:  # a device pointer (int) or a tensor
+                setattr(arr[h], name, int(m.data_ptr()) if hasattr(m, "data_ptr") else int(m))
+            else:
+                w = pack_bits(m)
+                keep.append(w)
+                setattr(arr[h], name, w.ctypes.data if w.size else None)
+    return arr, keep
+
+
+def expand_filtered(hops, filters, frontier, per_source_limit=0):
+    """sdb_graph_expand_filtered: expand() with a WHERE condition per hop.  filters: per hop None or (edge_bits,
+    target_bits), each None, a bool mask (per CSR position / per node id) or packed uint32 words."""
+    fr = np.ascontiguousarray(frontier, np.uint32)
+    arr = (C.c_void_p * len(hops))(*[g.h for g in hops])
+    farr, _keep = _filters(filters, len(hops), False)
+    out, n = C.c_void_p(), C.c_uint64()
+    L.check(L.lib().sdb_graph_expand_filtered(arr, farr, len(hops), C.c_void_p(fr.ctypes.data) if fr.size else None, fr.size,
+                                              int(per_source_limit), C.byref(out), C.byref(n)))
+    return _take(out, n)
+
+
+def expand_filtered_device(ctx, hops, filters, d_frontier, n_frontier, per_source_limit=0):
+    """sdb_graph_expand_filtered_device: filters hold DEVICE bitmaps (pointers or tensors of packed uint32 words).
+    -> (device pointer (int), count); free with device_free(ctx, ptr)."""
+    arr = (C.c_void_p * len(hops))(*[g.h for g in hops])
+    farr, _keep = _filters(filters, len(hops), True)
+    out, n = C.c_void_p(), C.c_uint64()
+    L.check(L.lib().sdb_graph_expand_filtered_device(arr, farr, len(hops), C.c_void_p(d_frontier), int(n_frontier),
+                                                     int(per_source_limit), C.byref(out), C.byref(n)))
+    return (out.value or 0), n.value
+
+
+def collect_filtered(graph, filt, start, min_depth=1, max_depth=0, inclusive=False):
+    """sdb_graph_collect_filtered: collect() whose every level is the filtered hop; filt = (edge_bits, target_bits)"""
+    st = np.ascontiguousarray(start, np.uint32)
+    farr, _keep = _filters([filt], 1, False)
+    out, n = C.c_void_p(), C.c_uint64()
+    L.check(L.lib().sdb_graph_collect_filtered(graph.h, farr, C.c_void_p(st.ctypes.data) if st.size else None, st.size,
+                                               int(min_depth), int(max_depth), int(bool(inclusive)), C.byref(out), C.byref(n)))
+    return _take(out, n)
+
+
 def _key_order(rid_key):
     """storekey order of a RecordIdKey (val/record_id.rs:181-192): numbers (numeric) before strings (bytes)"""
     if isinstance(rid_key, (int, np.integer)):
@@ -108,17 +180,29 @@ def _key_order(rid_key):
 
 class GraphStore:
     """CSR snapshots of a set of RELATE edges: relations = iterable of (src, edge_table, edge_id, dst) with
-    record ids like 'person:alice'."""
+    record ids like 'person:alice'.  For WHERE-filtered hops, edge_props maps an edge record id ('works_on:alice_db')
+    and node_props a node record id to its fields (a dict); records without an entry have no fields."""
 
-    def __init__(self, ctx, relations):
+    def __init__(self, ctx, relations, edge_props=None, node_props=None):
         self.ctx = ctx
         rel = list(relations)
         self.names = sorted({r[0] for r in rel} | {r[3] for r in rel})
         self.idx = {n: i for i, n in enumerate(self.names)}
         self._rel = rel
         self._csr = {}
+        self.edge_props = dict(edge_props or {})
+        self.node_props = dict(node_props or {})
 
     def csr_arrays(self, edge_table, direction):
+        return self._csr_build(edge_table, direction)[:2]
+
+    def edge_records(self, edge_table, direction):
+        """the edge record id behind every CSR position of csr_arrays(edge_table, direction), from the same sort (a
+        `<->` CSR lists each edge record at two positions of each endpoint's row)"""
+        rel = self._csr_build(edge_table, direction)[2]
+        return [f"{self._rel[r][1]}:{self._rel[r][2]}" for r in rel]
+
+    def _csr_build(self, edge_table, direction):
         """(row_ptr, col_idx) of one `node <dir> edge_table <dir> node` step, neighbours in the order the reference's
         KV scan yields them: per source the graph keys sort by (direction, edge table, edge record key)
         (key/graph/mod.rs:122-137).  edge_table=None is the `?` wildcard (all edge tables, scan/graph.rs:303-311); a tuple of
@@ -126,7 +210,7 @@ class GraphStore:
         Out (exec/operators/scan/graph.rs:203-207), and the second `<->` of the pair yields both endpoints of every
         edge record, In pointer (the edge's source node) first."""
         adj = [[] for _ in self.names]
-        for src, tb, eid, dst in self._rel:
+        for ri, (src, tb, eid, dst) in enumerate(self._rel):
             if edge_table is None:  # the `?` wildcard: one range over every edge table, i.e. key order by table name
                 tkey = tb.encode()
             elif isinstance(edge_table, (tuple, list)):  # one range per listed table, scanned in the listed order
@@ -140,22 +224,23 @@ class GraphStore:
             ek = (tkey, _key_order(eid))  # `ft` (the edge table) sorts before `fk` (the edge record key)
             s, d = self.idx[src], self.idx[dst]
             if direction == "out":
-                adj[s].append(((1, ek, 0), d))
+                adj[s].append(((1, ek, 0), d, ri))
             elif direction == "in":
-                adj[d].append(((0, ek, 0), s))
+                adj[d].append(((0, ek, 0), s, ri))
             elif direction == "both":
-                adj[d].append(((0, ek, 0), s))  # edges pointing at d: [source, d]
-                adj[d].append(((0, ek, 1), d))
-                adj[s].append(((1, ek, 0), s))  # edges leaving s: [s, target]
-                adj[s].append(((1, ek, 1), d))
+                adj[d].append(((0, ek, 0), s, ri))  # edges pointing at d: [source, d]
+                adj[d].append(((0, ek, 1), d, ri))
+                adj[s].append(((1, ek, 0), s, ri))  # edges leaving s: [s, target]
+                adj[s].append(((1, ek, 1), d, ri))
             else:
                 raise ValueError(f"direction {direction!r}: expected 'out', 'in' or 'both'")
-        rp, ci = [0], []
+        rp, ci, rel = [0], [], []
         for a in adj:
-            a.sort()
-            ci += [t for _, t in a]
+            a.sort()  # (key, target) first: the relation index only breaks ties between identical keys and targets
+            ci += [t for _, t, _r in a]
+            rel += [r for _, _t, r in a]
             rp.append(len(ci))
-        return np.asarray(rp, np.uint64), np.asarray(ci, np.uint32)
+        return np.asarray(rp, np.uint64), np.asarray(ci, np.uint32), rel
 
     def csr(self, edge_table, direction):
         key = (tuple(edge_table) if isinstance(edge_table, list) else edge_table, direction)
@@ -189,6 +274,48 @@ class GraphStore:
         depth = 0
         while depth < max_depth:
             nxt = expand([g], cur)
+            depth += 1
+            if nxt.size == 0 or (nxt.size == cur.size and np.array_equal(nxt, cur)):
+                return self.to_names(cur) if depth > min_depth else None
+            cur = nxt
+        return self.to_names(cur) if depth >= min_depth else None
+
+    def hop_masks(self, edge_table, direction, edge_pred=None, target_pred=None):
+        """what the shim evaluates a hop's WHERE conditions into: (edge mask per CSR position or None, target mask per
+        node id or None).  The predicates take a record's fields (a dict with its `id`).  This costs O(E) on the host per
+        condition, so on a real table the bitmap is cached or comes from an index."""
+        em = tm = None
+        if edge_pred is not None:
+            em = np.fromiter((bool(edge_pred({**self.edge_props.get(r, {}), "id": r}))
+                              for r in self.edge_records(edge_table, direction)), bool)
+        if target_pred is not None:
+            tm = np.fromiter((bool(target_pred({**self.node_props.get(n, {}), "id": n})) for n in self.names), bool,
+                             len(self.names))
+        return em, tm
+
+    def lookup_filtered(self, start, hops, limit=0):
+        """start: record ids; hops: [(direction, edge_table, edge_pred | None, target_pred | None), ...], i.e.
+        `->(edge_table WHERE edge_pred)->(node WHERE target_pred)` -> record ids, order and duplicates as the
+        reference returns them"""
+        graphs = [self.csr(tb, d) for d, tb, _e, _t in hops]
+        masks = [self.hop_masks(tb, d, e, t) for d, tb, e, t in hops]
+        return self.to_names(expand_filtered(graphs, masks, self.ids(start), limit))
+
+    def collect_filtered(self, start, direction, edge_table, edge_pred=None, target_pred=None, min_depth=1, max_depth=0,
+                         inclusive=False):
+        """`.{min..max+collect}->(edge_table WHERE ..)->(node WHERE ..)`: every BFS level is the filtered hop"""
+        masks = self.hop_masks(edge_table, direction, edge_pred, target_pred)
+        return self.to_names(collect_filtered(self.csr(edge_table, direction), masks, self.ids([start]), min_depth,
+                                              max_depth, inclusive))
+
+    def recurse_filtered(self, start, direction, edge_table, edge_pred, target_pred, min_depth, max_depth):
+        """default recursion over the filtered hop"""
+        g = self.csr(edge_table, direction)
+        masks = self.hop_masks(edge_table, direction, edge_pred, target_pred)
+        cur = self.ids([start])
+        depth = 0
+        while depth < max_depth:
+            nxt = expand_filtered([g], [masks], cur)
             depth += 1
             if nxt.size == 0 or (nxt.size == cur.size and np.array_equal(nxt, cur)):
                 return self.to_names(cur) if depth > min_depth else None
