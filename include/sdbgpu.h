@@ -59,7 +59,9 @@ typedef enum {
 
 /* element type of the rows handed to sdb_corpus_append (catalog VectorType, index.rs:321-334).
  * Brute-force KnnTopK holds Vec<Number>: F64 covers arbitrary Number::Float rows, F32 covers rows whose
- * values are f32-representable (the BASELINE configs) and enables the low-precision screen. */
+ * values are f32-representable (the BASELINE configs).  COSINE / EUCLIDEAN corpora of either type are screened on the
+ * tensor cores (F64: when the bf16 / int8 copies, 3 bytes per element, fit beside the rows at creation; otherwise the
+ * corpus is ranked by the exact kernel alone).  The f32 SIMT screen needs F32 rows: on F64 it means the exact kernel. */
 typedef enum { SDB_F32 = 0, SDB_F64 = 1 } sdb_dtype;
 
 /* element type of an HNSW index: catalog::VectorType (catalog/schema/index.rs:321-335), numbered as the SerializedVector
@@ -120,7 +122,8 @@ sdb_status sdb_debug_schedule(uint64_t n_rows, uint32_t cand_cap, uint32_t k, ui
                               uint32_t cap_probe, uint32_t* out_n_probe);
 /* Test-only diagnostics of the brute-force screens (no reference seam): the state the exactness proof rests on, so that
  * tests can compare every intermediate with a plain reference.  Every output may be NULL.
- * sdb_debug_corpus_state, on a finalized F32 corpus (n_pad = rows rounded up to 256):
+ * sdb_debug_corpus_state, on a finalized F32 corpus or an F64 one that has screen copies (n_pad = rows rounded up to
+ * 256):
  *   out_f[4]    i8_scale, max_rel_qerr, bf16_rel_err, max_norm
  *   out_u[5]    n_special, n_outliers, dim_pad, dim_pad8, n_pad
  *   out_i8      [n_pad][dim_pad8] int8 copy of the normalised rows (cosine corpora only)
@@ -131,7 +134,8 @@ sdb_status sdb_debug_corpus_state(sdb_corpus*, float* out_f, uint32_t* out_u, in
                                   float* out_snorm, uint32_t* out_special);
 /* sdb_debug_screen_batch: one batch of nq host queries screened with `screen` (TC_INT8, TC_BF16 or SIMT_F32) at the
  * first rung of the ladder, through the production sequence (streaming = 0: the multi-pass schedule), with exactly
- * cand_cap (>= 4096) candidate slots per query.  The ladder and the exact fallback do not run: flags are as the batch
+ * cand_cap (>= 4096) candidate slots per query (F64 corpora with screen copies: TC_INT8 or TC_BF16 only).  The ladder
+ * and the exact fallback do not run: flags are as the batch
  * left them.  score_all != 0 instead runs one pass-0 launch over every tile (SIMT: tau = -inf) with max(cand_cap,
  * n_pad) slots and selects nothing: out_a then holds every score of that kernel, and out_b / out_rr are untouched.
  * Let cap be the slots per query.

@@ -109,7 +109,9 @@ static std::vector<Rung> build_rungs(Corpus* c, uint32_t k, sdb_screen* first) {
   if (scr == SDB_SCREEN_TC_INT8 && !int8_ok) scr = SDB_SCREEN_TC_BF16;
   if (scr == SDB_SCREEN_TC_BF16 && (!screen_tc_available() || !c->d_bf16)) scr = SDB_SCREEN_SIMT_F32;
   const bool screenable = c->metric == SDB_COSINE || c->metric == SDB_EUCLIDEAN;
-  if (c->dtype == SDB_F64 || c->special_overflow || k > 256 || !screenable) scr = SDB_SCREEN_NONE_EXACT;
+  // the SIMT screen streams f32 rows: an f64 corpus is screened on the tensor cores or not at all
+  if (c->dtype == SDB_F64 && scr == SDB_SCREEN_SIMT_F32) scr = SDB_SCREEN_NONE_EXACT;
+  if (c->special_overflow || k > 256 || !screenable) scr = SDB_SCREEN_NONE_EXACT;
   *first = scr;
   std::vector<Rung> r;
   if (scr == SDB_SCREEN_TC_INT8)
@@ -311,7 +313,7 @@ static sdb_status enqueue_batch(Corpus* c, Ticket& t) {
   // stage B: the coarse screens' candidates are re-scored in f32 and narrowed before the (FP64-bound) exact re-rank
   static const bool no_refine = getenv("SDB_NO_REFINE") != nullptr;
   bool refined = false;
-  if (tc && c->exact && c->dtype == SDB_F32 && !no_refine) {
+  if (tc && c->exact && !no_refine) {
     SDB_TRY(cand_refine(c, nq, st));
     if (c->tap) SDB_TRY(tap_list(c, nq, &c->tap->list_r, nullptr, st));
     SDB_TRY(cand_select(c, nq, k, false, 0u, false, st, 1));
@@ -914,6 +916,16 @@ sdb_status sdb_corpus_create(sdb_ctx* ctx, uint32_t dim, sdb_dtype dt, sdb_metri
     sdb_corpus_destroy(c);
     return SDB_ENOMEM;
   }
+  // f64 rows get the same screen copies (3 more bytes per element beside their 8), but only when they fit: an f64
+  // corpus without them is still served, by the exact kernel alone, as before they existed
+  if (dt == SDB_F64 && screenable) {
+    cudaError_t e2 = c->d_bf16.reserve(cap_pad * c->dim_pad);
+    if (e2 == cudaSuccess && m == SDB_COSINE) e2 = c->d_i8.reserve((size_t)cap_pad * c->dim_pad8);
+    if (e2 != cudaSuccess) {
+      c->d_bf16.reset();
+      c->d_i8.reset();
+    }
+  }
   *out = c;
   return SDB_OK;
 }
@@ -1137,8 +1149,8 @@ sdb_status sdb_debug_corpus_state(sdb_corpus* c, float* out_f, uint32_t* out_u, 
                                   float* out_snorm, uint32_t* out_special) {
   if (!c) return SDB_EINVAL;
   std::lock_guard<std::mutex> g(c->mu);
-  if (!c->finalized || c->dtype != SDB_F32 || (out_i8 && !c->d_i8) || (out_bf16 && !c->d_bf16)) {
-    set_error("sdb_debug_corpus_state: needs a finalized F32 corpus (int8 copy: cosine only)");
+  if (!c->finalized || (c->dtype != SDB_F32 && !c->d_bf16) || (out_i8 && !c->d_i8) || (out_bf16 && !c->d_bf16)) {
+    set_error("sdb_debug_corpus_state: needs a finalized F32 corpus or a screened F64 one (int8 copy: cosine only)");
     return SDB_EINVAL;
   }
   SDB_CUDA(cudaSetDevice(c->ctx->device));
@@ -1179,9 +1191,11 @@ sdb_status sdb_debug_screen_batch(sdb_corpus* c, const double* queries, uint32_t
   }
   std::lock_guard<std::mutex> g(c->mu);
   const bool int8 = screen == SDB_SCREEN_TC_INT8;
-  if (!c->finalized || c->dtype != SDB_F32 || (c->metric != SDB_COSINE && c->metric != SDB_EUCLIDEAN) ||
+  const bool f64_ok = c->dtype == SDB_F64 && tc && c->d_bf16;  // f64 rows: tensor-core screens only
+  if (!c->finalized || (c->dtype != SDB_F32 && !f64_ok) || (c->metric != SDB_COSINE && c->metric != SDB_EUCLIDEAN) ||
       (int8 && !c->d_i8) || c->special_overflow || !c->n) {
-    set_error("sdb_debug_screen_batch: needs a finalized, non-empty F32 cosine / euclidean corpus (int8: cosine)");
+    set_error("sdb_debug_screen_batch: needs a finalized, non-empty F32 cosine / euclidean corpus, or an F64 one with "
+              "screen copies and a tensor-core screen (int8: cosine)");
     return SDB_EINVAL;
   }
   Ctx* ctx = c->ctx;

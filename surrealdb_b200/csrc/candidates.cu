@@ -4,6 +4,8 @@
 //   cand_rerank  : exact f64 distances (the reference's arithmetic, op for op) of the survivors
 //   cand_final   : order by (distance, scan position), emit top-k, PROVE that no unscreened row could
 //                  belong to it (error-bound check) or flag the query for the exact kernel.
+#include <type_traits>
+
 #include "exactmath.cuh"
 #include "internal.cuh"
 #include "rowwalk.cuh"
@@ -128,7 +130,7 @@ __global__ void cand_begin_kernel(float* __restrict__ tau, uint32_t* __restrict_
                                   const double* __restrict__ qmag, const float* __restrict__ q8scale,
                                   const float* __restrict__ q8err, const float* __restrict__ qbferr, uint32_t nq,
                                   int screen, int metric, uint32_t dim, float max_rel_qerr, float i8_scale,
-                                  float bf16_rel_err, float max_norm, int exact) {
+                                  float bf16_rel_err, float max_norm, int exact, int f64_rows) {
   const uint32_t q = blockIdx.x * blockDim.x + threadIdx.x;
   if (q == 0) {
     stat[0] = 0;
@@ -141,6 +143,11 @@ __global__ void cand_begin_kernel(float* __restrict__ tau, uint32_t* __restrict_
   cnt[q] = 0;
   flags[q] = 0;
   const double qm = qmag[q];
+  // f64 rows, cosine: products q_i x_i below 2^-126 may be flushed by the tensor cores (and lose their low bits in
+  // stage B's f32 FMA chain), an ABSOLUTE dot error of at most D 2^-126 that no relative term covers.  Screened f64
+  // rows have |x| >= 2^-100 (finalize_rows_kernel), so in similarity units it is at most D 2^-26 / |q|: nothing for
+  // ordinary queries, while a query so small that it matters gets a bound too wide to prove anything (exact kernel).
+  const double u_abs = (f64_rows && metric == SDB_COSINE) ? dim * 0x1p-26 / qm : 0.0;
   double eps_rel, bs = 1.0;
   if (screen == SDB_SCREEN_TC_INT8) {
     const double eq = q8err[q];
@@ -148,7 +155,7 @@ __global__ void cand_begin_kernel(float* __restrict__ tau, uint32_t* __restrict_
     bs = (double)q8scale[q] * (double)i8_scale * 1.000001;
   } else if (screen == SDB_SCREEN_TC_BF16) {
     const double eq = qbferr[q], ex = bf16_rel_err;
-    eps_rel = ex + eq + ex * eq + dim * 4.76837158e-7 + 1e-5;
+    eps_rel = ex + eq + ex * eq + dim * 4.76837158e-7 + 1e-5 + u_abs;
   } else {
     eps_rel = (dim / 16.0 + 16.0) * 1.1920929e-7;
   }
@@ -173,8 +180,10 @@ __global__ void cand_begin_kernel(float* __restrict__ tau, uint32_t* __restrict_
   }
   // stage B (cand_refine: f32 re-score of the candidates with the f32 rows and the f32 query): any summation order of
   // D products in f32 with FMA stays within (D + 16) * 2^-24 of sum |q_i x_i| <= |q||x| (the +16 covers the f64 -> f32
-  // rounding of the query, the f32 screening norm and the final scaling)
-  const double e2_rel = (dim + 16.0) * 5.9604645e-8;
+  // rounding of the query, the f32 screening norm and the final scaling).  f64 rows are rounded to f32 as they are
+  // gathered, which moves the dot product by at most 2^-24 sum |q_i x_i| more, plus the underflow term above
+  double e2_rel = (dim + 16.0) * 5.9604645e-8;
+  if (f64_rows) e2_rel += 5.9604644775390625e-8 + u_abs;
   double e2, mg2;
   if (metric == SDB_COSINE) {
     e2 = e2_rel;
@@ -200,7 +209,7 @@ sdb_status cand_begin(Corpus* c, uint32_t nq, int screen, cudaStream_t st) {
                                                       c->d_qmag, c->d_q8scale,
                                                       c->d_q8err, c->d_qbferr, nq, screen, (int)c->metric, c->dim,
                                                       c->max_rel_qerr, c->i8_scale, c->bf16_rel_err, c->max_norm,
-                                                      c->exact ? 1 : 0);
+                                                      c->exact ? 1 : 0, c->dtype == SDB_F64 ? 1 : 0);
   count_launch(c->ctx);
   SDB_CUDA(cudaGetLastError());
   return SDB_OK;
@@ -574,8 +583,10 @@ sdb_status cand_select(Corpus* c, uint32_t nq, uint32_t k, bool drop_invalid, ui
 // shuffle reduction.  The error of that score is bounded rigorously (cand_begin_kernel: beps2), so the same rule
 // "keep everything within 2.1 x the bound of the k-th best" (cand_select, stage 1) shrinks the set to k plus a few
 // near-ties, and only those reach the f64 kernel.
-template <bool COSINE>
-__global__ void __launch_bounds__(128) cand_refine_f32_kernel(const float* __restrict__ rows, uint32_t dim,
+// f64 rows: gathered as f64 (16-byte loads when the row length is even) and rounded to f32 element by element before
+// the same FMA chain; no f32 copy of the corpus is kept (cand_begin_kernel adds the rounding to beps2).
+template <typename T, bool COSINE>
+__global__ void __launch_bounds__(128) cand_refine_f32_kernel(const T* __restrict__ rows, uint32_t dim,
                                                                const float* __restrict__ snorm,
                                                                const float* __restrict__ q32, Cand* __restrict__ cand,
                                                                const uint32_t* __restrict__ cnt, uint32_t cap) {
@@ -589,10 +600,27 @@ __global__ void __launch_bounds__(128) cand_refine_f32_kernel(const float* __res
     const uint32_t r0 = cq[e0].row;
     const bool has1 = e0 + 1 < n_c;
     const uint32_t r1 = has1 ? cq[e0 + 1].row : r0;
-    const float* x0 = rows + (size_t)r0 * dim;
-    const float* x1 = rows + (size_t)r1 * dim;
+    const T* x0 = rows + (size_t)r0 * dim;
+    const T* x1 = rows + (size_t)r1 * dim;
     float a0 = 0.f, a1 = 0.f;
-    if (vec4) {
+    if constexpr (std::is_same<T, double>::value) {
+      if ((dim & 1u) == 0) {
+#pragma unroll 2
+        for (uint32_t c = lane * 2; c < dim; c += 64) {
+          const double2 u = __ldg(reinterpret_cast<const double2*>(x0 + c));
+          const double2 v = __ldg(reinterpret_cast<const double2*>(x1 + c));
+          const float2 w = __ldg(reinterpret_cast<const float2*>(qv + c));
+          a0 = fmaf(__double2float_rn(u.x), w.x, a0); a0 = fmaf(__double2float_rn(u.y), w.y, a0);
+          a1 = fmaf(__double2float_rn(v.x), w.x, a1); a1 = fmaf(__double2float_rn(v.y), w.y, a1);
+        }
+      } else {
+        for (uint32_t c = lane; c < dim; c += 32) {
+          const float w = __ldg(qv + c);
+          a0 = fmaf(__double2float_rn(__ldg(x0 + c)), w, a0);
+          a1 = fmaf(__double2float_rn(__ldg(x1 + c)), w, a1);
+        }
+      }
+    } else if (vec4) {
       for (uint32_t c = lane * 4; c < dim; c += 128) {
         const float4 u = __ldg(reinterpret_cast<const float4*>(x0 + c));
         const float4 v = __ldg(reinterpret_cast<const float4*>(x1 + c));
@@ -623,14 +651,21 @@ __global__ void __launch_bounds__(128) cand_refine_f32_kernel(const float* __res
   }
 }
 sdb_status cand_refine(Corpus* c, uint32_t nq, cudaStream_t st) {
-  if (c->dtype != SDB_F32) return SDB_OK;
   const dim3 grid(nq, 8);  // 128-thread blocks (register budget beside a resident screen CTA)
-  if (c->metric == SDB_COSINE)
-    cand_refine_f32_kernel<true><<<grid, 128, 0, st>>>((const float*)c->d_rows.get(), c->dim, c->d_snorm, c->d_q32, c->d_cand,
-                                                       c->d_cand_cnt, c->sc_cap);
+  const float* f32_rows = (const float*)c->d_rows.get();
+  const double* f64_rows = (const double*)c->d_rows.get();
+  if (c->dtype == SDB_F32 && c->metric == SDB_COSINE)
+    cand_refine_f32_kernel<float, true><<<grid, 128, 0, st>>>(f32_rows, c->dim, c->d_snorm, c->d_q32, c->d_cand,
+                                                              c->d_cand_cnt, c->sc_cap);
+  else if (c->dtype == SDB_F32)
+    cand_refine_f32_kernel<float, false><<<grid, 128, 0, st>>>(f32_rows, c->dim, c->d_snorm, c->d_q32, c->d_cand,
+                                                               c->d_cand_cnt, c->sc_cap);
+  else if (c->metric == SDB_COSINE)
+    cand_refine_f32_kernel<double, true><<<grid, 128, 0, st>>>(f64_rows, c->dim, c->d_snorm, c->d_q32, c->d_cand,
+                                                               c->d_cand_cnt, c->sc_cap);
   else
-    cand_refine_f32_kernel<false><<<grid, 128, 0, st>>>((const float*)c->d_rows.get(), c->dim, c->d_snorm, c->d_q32, c->d_cand,
-                                                        c->d_cand_cnt, c->sc_cap);
+    cand_refine_f32_kernel<double, false><<<grid, 128, 0, st>>>(f64_rows, c->dim, c->d_snorm, c->d_q32, c->d_cand,
+                                                                c->d_cand_cnt, c->sc_cap);
   count_launch(c->ctx);
   SDB_CUDA(cudaGetLastError());
   return SDB_OK;
@@ -806,9 +841,10 @@ constexpr size_t RRV_SMEM = sizeof(double) * QCHUNK + sizeof(float) * 4 * 32 * R
 // (the staged variant's 6 KB per warp let only two warps per SM in, and the re-rank took 0.58 ms instead of 0.1 ms
 // whenever it overlapped a screen -- SDB_TRACE timeline, round 2).  Every lane streams its own row (16-byte loads; the
 // second half of each 32-byte sector comes from L1) and reads the query from global memory (one address per half-warp).
-template <bool COSINE>
+// f64 rows stream as double2 (16-byte) loads when the row length is even.
+template <typename T, bool COSINE>
 __global__ void __launch_bounds__(128) cand_rerank_packed_kernel(
-    const float* __restrict__ rows, uint32_t dim, const double* __restrict__ mag, const double* __restrict__ q64,
+    const T* __restrict__ rows, uint32_t dim, const double* __restrict__ mag, const double* __restrict__ q64,
     const double* __restrict__ qmag, const uint32_t* __restrict__ qflags, const Cand* __restrict__ cand,
     const uint32_t* __restrict__ cnt, uint32_t cap, const uint32_t* __restrict__ special, uint32_t n_special, uint32_t nq,
     uint64_t* __restrict__ rr_key, double* __restrict__ rr_dist, uint32_t* __restrict__ rr_row, uint32_t rr_stride) {
@@ -823,9 +859,29 @@ __global__ void __launch_bounds__(128) cand_rerank_packed_kernel(
   const bool vec4 = (dim & 3u) == 0;
   for (uint32_t e = l16; e < n_e; e += 16) {
     const uint32_t my_row = e < n_c ? cand[(size_t)q * cap + e].row : special[e - n_c];
-    const float* x = rows + (size_t)my_row * dim;
+    const T* x = rows + (size_t)my_row * dim;
     ExactAcc acc;
-    if (vec4) {
+    if constexpr (std::is_same<T, double>::value) {
+      if ((dim & 1u) == 0) {
+#pragma unroll 2
+        for (uint32_t j = 0; j < dim; j += 2) {
+          const double2 v = __ldg(reinterpret_cast<const double2*>(x + j));
+          const double2 qa = __ldg(reinterpret_cast<const double2*>(qv + j));
+          if (COSINE) {
+            acc.cosine_step(v.x, qa.x);
+            acc.cosine_step(v.y, qa.y);
+          } else {
+            acc.euclid_step(v.x, qa.x);
+            acc.euclid_step(v.y, qa.y);
+          }
+        }
+      } else {
+        for (uint32_t j = 0; j < dim; j++) {
+          if (COSINE) acc.cosine_step(__ldg(x + j), __ldg(qv + j));
+          else acc.euclid_step(__ldg(x + j), __ldg(qv + j));
+        }
+      }
+    } else if (vec4) {
 #pragma unroll 2
       for (uint32_t j = 0; j < dim; j += 4) {
         const float4 v = __ldg(reinterpret_cast<const float4*>(x + j));
@@ -861,16 +917,26 @@ sdb_status cand_rerank(Corpus* c, uint32_t nq, cudaStream_t st, bool small_sets)
   const dim3 grid(nq, RR_GROUPS_Y);
   static const bool no_v4 = getenv("SDB_RERANK_SCALAR") != nullptr;
   static const bool no_packed = getenv("SDB_RERANK_STAGED") != nullptr;
-  if (small_sets && c->dtype == SDB_F32 && !no_packed && (c->metric == SDB_COSINE || c->metric == SDB_EUCLIDEAN)) {
+  if (small_sets && !no_packed && (c->metric == SDB_COSINE || c->metric == SDB_EUCLIDEAN)) {
     const unsigned g = (nq + 7) / 8;
-    if (c->metric == SDB_COSINE)
-      cand_rerank_packed_kernel<true><<<g, 128, 0, st>>>((const float*)c->d_rows.get(), c->dim, c->d_mag, c->d_q64, c->d_qmag, c->d_qflags,
-                                                        c->d_cand, c->d_cand_cnt, c->sc_cap, c->d_special, c->n_special, nq,
-                                                        c->d_rr_key, c->d_rr_dist, c->d_rr_row, c->rr_stride);
+    const float* f32_rows = (const float*)c->d_rows.get();
+    const double* f64_rows = (const double*)c->d_rows.get();
+    if (c->dtype == SDB_F32 && c->metric == SDB_COSINE)
+      cand_rerank_packed_kernel<float, true><<<g, 128, 0, st>>>(f32_rows, c->dim, c->d_mag, c->d_q64, c->d_qmag, c->d_qflags,
+                                                               c->d_cand, c->d_cand_cnt, c->sc_cap, c->d_special, c->n_special,
+                                                               nq, c->d_rr_key, c->d_rr_dist, c->d_rr_row, c->rr_stride);
+    else if (c->dtype == SDB_F32)
+      cand_rerank_packed_kernel<float, false><<<g, 128, 0, st>>>(f32_rows, c->dim, c->d_mag, c->d_q64, c->d_qmag, c->d_qflags,
+                                                                c->d_cand, c->d_cand_cnt, c->sc_cap, c->d_special, c->n_special,
+                                                                nq, c->d_rr_key, c->d_rr_dist, c->d_rr_row, c->rr_stride);
+    else if (c->metric == SDB_COSINE)
+      cand_rerank_packed_kernel<double, true><<<g, 128, 0, st>>>(f64_rows, c->dim, c->d_mag, c->d_q64, c->d_qmag, c->d_qflags,
+                                                                c->d_cand, c->d_cand_cnt, c->sc_cap, c->d_special, c->n_special,
+                                                                nq, c->d_rr_key, c->d_rr_dist, c->d_rr_row, c->rr_stride);
     else
-      cand_rerank_packed_kernel<false><<<g, 128, 0, st>>>((const float*)c->d_rows.get(), c->dim, c->d_mag, c->d_q64, c->d_qmag, c->d_qflags,
-                                                         c->d_cand, c->d_cand_cnt, c->sc_cap, c->d_special, c->n_special, nq,
-                                                         c->d_rr_key, c->d_rr_dist, c->d_rr_row, c->rr_stride);
+      cand_rerank_packed_kernel<double, false><<<g, 128, 0, st>>>(f64_rows, c->dim, c->d_mag, c->d_q64, c->d_qmag, c->d_qflags,
+                                                                 c->d_cand, c->d_cand_cnt, c->sc_cap, c->d_special, c->n_special,
+                                                                 nq, c->d_rr_key, c->d_rr_dist, c->d_rr_row, c->rr_stride);
   } else if (small_sets && c->dtype == SDB_F32)
     // (kept for A/B: one warp per query, rows transposed through 6 KB of shared memory)
     cand_rerank_kernel<float, 1, 32, 256><<<grid, 32, 0, st>>>((const float*)c->d_rows.get(), c->dim, (int)c->metric, c->d_mag,

@@ -1,10 +1,11 @@
 // corpus.cu -- device-resident vector column: per-row exact magnitudes, screening norms, bf16 screen
 // copy, special-row list.  Data layout in HBM (DESIGN.md section 4):
 //   rows   [cap][dim]        f32|f64  master copy (exact re-rank reads it; the SIMT screen streams it)
-//   bf16   [cap][dim_pad]    bf16     screen copy, K-major rows = wgmma "B" operand via TMA
+//   bf16   [cap][dim_pad]    bf16     screen copy, K-major rows = wgmma "B" operand via TMA (f32 and f64 rows alike)
 //   mag    [cap]             f64      sqrt(sum x^2), the reference's `magnitude()` arithmetic
 //   snorm  [cap]             f32      cosine: 1/|x|, euclid: |x|^2, NaN => row never screened in
 #include <algorithm>
+#include <type_traits>
 
 #include "internal.cuh"
 #include "rowwalk.cuh"
@@ -25,9 +26,11 @@ __global__ void __launch_bounds__(WARPS * 32) finalize_rows_kernel(const T* __re
     const uint64_t r = base + lane;
     const uint32_t my_row = r < n ? (uint32_t)r : NO_ROW;
     double s = 0.0;
+    double amax = 0.0;  // f64 rows: largest |x_i| (an NaN element makes s NaN, which is special anyway)
     warp_walk_rows<T>(rows, dim, my_row, tile[warp], [&](uint32_t, T x) {
       const double xd = (double)x;
       s = __dadd_rn(s, __dmul_rn(xd, xd));
+      if constexpr (std::is_same<T, double>::value) amax = fmax(amax, fabs(xd));
     });
     if (my_row == NO_ROW) continue;
     const double m = __dsqrt_rn(s);
@@ -42,6 +45,22 @@ __global__ void __launch_bounds__(WARPS * 32) finalize_rows_kernel(const T* __re
       is_special = !isfinite(s);
       sn = (float)s;
       if (!isfinite(sn)) is_special = true;  // |x|^2 overflows f32: rank exactly
+    }
+    if constexpr (std::is_same<T, double>::value) {
+      // f64 rows the f32 / bf16 operands cannot stand for (the screens and stage B see them only through those):
+      //  - an element beyond f32 range (its f32 / bf16 copy is inf);
+      //  - |x| or the screening norm (1/|x|, |x|^2) not a finite normal f32: the bounds scale by them in f32;
+      //  - a non-zero row with |x| < 2^-100 (f64 subnormals, whose squares vanish, included).  Flushing an element to
+      //    f32 / bf16 zero or a subnormal errs by at most 2^-150 (f32) or 2^-134 (bf16) absolutely.  The bf16 and
+      //    int8 residuals are measured in f64 and include it; stage B's bound is relative (2^-24 per element), and
+      //    sqrt(D) 2^-150 |q| <= 2^-142 |q| stays below 2^-42 |q||x| for |x| >= 2^-100 -- far inside the +16 2^-24
+      //    slack of beps2.  An all-zero row is exact in every copy (euclidean screens it; cosine never does).
+      const bool nonzero = amax > 0.0;
+      const float mf = (float)m;
+      const bool m_normal = mf >= 1.17549435e-38f && mf <= 3.40282347e38f;
+      const bool sn_normal = fabsf(sn) >= 1.17549435e-38f && fabsf(sn) <= 3.40282347e38f;
+      if (!(amax <= 3.4028234663852886e38)) is_special = true;
+      if (nonzero && (m < 0x1p-100 || !m_normal || !sn_normal)) is_special = true;
     }
     if (skipped) {
       sn = __int_as_float(0x7fc00000);
@@ -64,29 +83,45 @@ __global__ void pad_snorm_kernel(float* __restrict__ snorm, uint64_t n, uint64_t
 
 // bf16 screen copy, one warp per row; also measures e_x = max over valid rows of |x - bf16(x)| / |x| (the residual
 // norm that enters the screen's error bound; at most 2^-8 by construction of round-to-nearest, usually ~0.6 of that)
-__global__ void __launch_bounds__(256) to_bf16_kernel(const float* __restrict__ rows, uint32_t dim, uint32_t dim_pad, uint64_t n,
+// f64 rows are rounded to bf16 in one step (cvt.rn.bf16.f64: no double rounding through f32), and their residual is
+// measured in f64 against the f64 values, then rounded up to f32.
+template <typename T>
+__global__ void __launch_bounds__(256) to_bf16_kernel(const T* __restrict__ rows, uint32_t dim, uint32_t dim_pad, uint64_t n,
                                                       uint64_t n_pad, const double* __restrict__ mag,
                                                       const float* __restrict__ snorm, __nv_bfloat16* __restrict__ out,
                                                       uint32_t* max_rel_bits) {
+  using Acc = typename std::conditional<std::is_same<T, double>::value, double, float>::type;
   const uint32_t lane = threadIdx.x & 31;
   const uint64_t warps = (uint64_t)gridDim.x * 8;
   for (uint64_t r = (uint64_t)blockIdx.x * 8 + (threadIdx.x >> 5); r < n_pad; r += warps) {
     __nv_bfloat16* o = out + r * dim_pad;
-    float err2 = 0.f;
+    Acc err2 = 0;
     for (uint32_t c = lane; c < dim_pad; c += 32) {
-      const float v = (r < n && c < dim) ? rows[r * dim + c] : 0.f;
-      const __nv_bfloat16 h = __float2bfloat16_rn(v);
-      o[c] = h;
-      const float d = v - __bfloat162float(h);
-      if (d == d) err2 = fmaf(d, d, err2);
+      if constexpr (std::is_same<T, double>::value) {
+        const double v = (r < n && c < dim) ? rows[r * dim + c] : 0.0;
+        const __nv_bfloat16 h = __double2bfloat16(v);
+        o[c] = h;
+        const double d = v - (double)__bfloat162float(h);
+        if (d == d) err2 = fma(d, d, err2);
+      } else {
+        const float v = (r < n && c < dim) ? rows[r * dim + c] : 0.f;
+        const __nv_bfloat16 h = __float2bfloat16_rn(v);
+        o[c] = h;
+        const float d = v - __bfloat162float(h);
+        if (d == d) err2 = fmaf(d, d, err2);
+      }
     }
 #pragma unroll
     for (int o2 = 16; o2 > 0; o2 >>= 1) err2 += __shfl_xor_sync(0xffffffffu, err2, o2);
     if (lane == 0 && r < n) {
       const float sn = snorm[r];
       const double m = mag[r];
-      if (sn == sn && m > 0.0 && isfinite(m) && isfinite(err2))  // skipped / special rows never reach the screen
-        atomicMax(max_rel_bits, __float_as_uint((sqrtf(err2) / (float)m) * 1.0001f + 1e-9f));
+      if (sn == sn && m > 0.0 && isfinite(m) && isfinite(err2)) {  // skipped / special rows never reach the screen
+        if constexpr (std::is_same<T, double>::value)  // (1 + 2^-30) covers the f64 rounding of the figure itself
+          atomicMax(max_rel_bits, __float_as_uint(__double2float_ru(sqrt(err2) / m * (1.0 + 0x1p-30))));
+        else
+          atomicMax(max_rel_bits, __float_as_uint((sqrtf(err2) / (float)m) * 1.0001f + 1e-9f));
+      }
     }
   }
 }
@@ -108,7 +143,9 @@ __device__ __host__ inline uint32_t rmax_bin(float v) {  // v > 0
 #endif
   return (u >> 19) & (RMAX_BINS - 1);
 }
-__global__ void __launch_bounds__(256) quantize_scan_kernel(const float* __restrict__ rows, uint32_t dim, uint64_t n,
+// (f64 rows: max_i |x_i| / |x| in f64, rounded up to f32)
+template <typename T>
+__global__ void __launch_bounds__(256) quantize_scan_kernel(const T* __restrict__ rows, uint32_t dim, uint64_t n,
                                                             const double* __restrict__ mag, const float* __restrict__ snorm,
                                                             uint32_t* gmax_bits, float* __restrict__ rmax,
                                                             uint32_t* __restrict__ hist) {
@@ -124,12 +161,21 @@ __global__ void __launch_bounds__(256) quantize_scan_kernel(const float* __restr
       if (lane == 0) rmax[r] = 0.f;
       continue;
     }
-    const float* x = rows + r * dim;
-    float mx = 0.f;
-    for (uint32_t c = lane; c < dim; c += 32) mx = fmaxf(mx, fabsf(x[c]));
+    const T* x = rows + r * dim;
+    float v;
+    if constexpr (std::is_same<T, double>::value) {
+      double mx = 0.0;
+      for (uint32_t c = lane; c < dim; c += 32) mx = fmax(mx, fabs(x[c]));
 #pragma unroll
-    for (int o2 = 16; o2 > 0; o2 >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o2));
-    const float v = mx / (float)mag[r];
+      for (int o2 = 16; o2 > 0; o2 >>= 1) mx = fmax(mx, __shfl_xor_sync(0xffffffffu, mx, o2));
+      v = __double2float_ru(mx / mag[r]);
+    } else {
+      float mx = 0.f;
+      for (uint32_t c = lane; c < dim; c += 32) mx = fmaxf(mx, fabsf(x[c]));
+#pragma unroll
+      for (int o2 = 16; o2 > 0; o2 >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o2));
+      v = mx / (float)mag[r];
+    }
     best = fmaxf(best, v);
     if (lane == 0) {
       rmax[r] = v;
@@ -157,7 +203,9 @@ __global__ void mark_outliers_kernel(const float* __restrict__ rmax, uint64_t n,
   }
 }
 // pass 2: x8 = clamp(rn(x / (|x| s)), +-127), e_x accumulated exactly as the residual norm (clipping included)
-__global__ void __launch_bounds__(256) quantize_rows_kernel(const float* __restrict__ rows, uint32_t dim, uint32_t dim_pad8,
+// f64 rows: xn = x / |x| and xn / s in f64 (each correctly rounded), the residual xn - s x8 in f64, rounded up to f32
+template <typename T>
+__global__ void __launch_bounds__(256) quantize_rows_kernel(const T* __restrict__ rows, uint32_t dim, uint32_t dim_pad8,
                                                             uint64_t n, uint64_t n_pad, const double* __restrict__ mag,
                                                             const float* __restrict__ snorm, const uint32_t* gmax_bits,
                                                             int8_t* __restrict__ out, uint32_t* max_rel_bits) {
@@ -173,25 +221,45 @@ __global__ void __launch_bounds__(256) quantize_rows_kernel(const float* __restr
       for (uint32_t c = lane; c < dim_pad8; c += 32) o[c] = 0;
       continue;
     }
-    const float* x = rows + r * dim;
-    const float inv_norm = 1.f / (float)mag[r];
-    const float inv = 1.f / s;
-    float err2 = 0.f;
-    for (uint32_t c = lane; c < dim_pad8; c += 32) {
-      int q = 0;
-      if (c < dim) {
-        const float xn = x[c] * inv_norm;
-        q = __float2int_rn(xn * inv);
-        q = q > 127 ? 127 : (q < -127 ? -127 : q);
-        const float d = xn - (float)q * s;
-        err2 = fmaf(d, d, err2);
+    const T* x = rows + r * dim;
+    if constexpr (std::is_same<T, double>::value) {
+      const double m = mag[r], sd = (double)s;
+      double err2 = 0.0;
+      for (uint32_t c = lane; c < dim_pad8; c += 32) {
+        int q = 0;
+        if (c < dim) {
+          const double xn = x[c] / m;
+          q = __double2int_rn(xn / sd);
+          q = q > 127 ? 127 : (q < -127 ? -127 : q);
+          const double d = xn - (double)q * sd;  // q * s is exact (7 x 24 bits)
+          err2 = fma(d, d, err2);
+        }
+        o[c] = (int8_t)q;
       }
-      o[c] = (int8_t)q;
-    }
 #pragma unroll
-    for (int o2 = 16; o2 > 0; o2 >>= 1) err2 += __shfl_xor_sync(0xffffffffu, err2, o2);
-    // + 2^-22: the f32 normalisation x * (1/|x|) is itself rounded; the whole figure is rounded up
-    if (lane == 0) atomicMax(max_rel_bits, __float_as_uint(sqrtf(err2) * 1.0001f + 5e-7f));
+      for (int o2 = 16; o2 > 0; o2 >>= 1) err2 += __shfl_xor_sync(0xffffffffu, err2, o2);
+      // + 2^-40: the f64 normalisation x / |x| is itself rounded (at most 2^-53 in norm); the whole figure rounded up
+      if (lane == 0) atomicMax(max_rel_bits, __float_as_uint(__double2float_ru(sqrt(err2) * (1.0 + 0x1p-30) + 0x1p-40)));
+    } else {
+      const float inv_norm = 1.f / (float)mag[r];
+      const float inv = 1.f / s;
+      float err2 = 0.f;
+      for (uint32_t c = lane; c < dim_pad8; c += 32) {
+        int q = 0;
+        if (c < dim) {
+          const float xn = x[c] * inv_norm;
+          q = __float2int_rn(xn * inv);
+          q = q > 127 ? 127 : (q < -127 ? -127 : q);
+          const float d = xn - (float)q * s;
+          err2 = fmaf(d, d, err2);
+        }
+        o[c] = (int8_t)q;
+      }
+#pragma unroll
+      for (int o2 = 16; o2 > 0; o2 >>= 1) err2 += __shfl_xor_sync(0xffffffffu, err2, o2);
+      // + 2^-22: the f32 normalisation x * (1/|x|) is itself rounded; the whole figure is rounded up
+      if (lane == 0) atomicMax(max_rel_bits, __float_as_uint(sqrtf(err2) * 1.0001f + 5e-7f));
+    }
   }
 }
 
@@ -292,24 +360,32 @@ sdb_status corpus_finalize_device(Corpus* c) {
                                                          d_tmp + 1);
     count_launch(ctx);
     SDB_CUDA(cudaGetLastError());
-    if (c->dtype == SDB_F32 && c->d_bf16) {
+    if (c->d_bf16) {
       const uint64_t n_pad = (c->n + TILE_ROWS - 1) / TILE_ROWS * TILE_ROWS;
-      to_bf16_kernel<<<ctx->sm_count * 16, 256, 0, st>>>((const float*)c->d_rows.get(), c->dim, c->dim_pad, c->n, n_pad,
-                                                         c->d_mag, c->d_snorm, c->d_bf16, d_tmp + 4);
+      if (c->dtype == SDB_F32)
+        to_bf16_kernel<float><<<ctx->sm_count * 16, 256, 0, st>>>((const float*)c->d_rows.get(), c->dim, c->dim_pad, c->n,
+                                                                  n_pad, c->d_mag, c->d_snorm, c->d_bf16, d_tmp + 4);
+      else
+        to_bf16_kernel<double><<<ctx->sm_count * 16, 256, 0, st>>>((const double*)c->d_rows.get(), c->dim, c->dim_pad,
+                                                                   c->n, n_pad, c->d_mag, c->d_snorm, c->d_bf16, d_tmp + 4);
       count_launch(ctx);
       SDB_CUDA(cudaGetLastError());
     }
   }
   c->n_outliers = 0;
-  if (c->n && c->dtype == SDB_F32 && c->d_i8 && c->metric == SDB_COSINE) {
+  if (c->n && c->d_i8 && c->metric == SDB_COSINE) {
     const uint64_t n_pad = (c->n + TILE_ROWS - 1) / TILE_ROWS * TILE_ROWS;
     AsyncBuf<float> d_rmax;
     AsyncBuf<uint32_t> d_hist;
     SDB_CUDA(d_rmax.reserve(c->n, st));
     SDB_CUDA(d_hist.reserve(RMAX_BINS, st));
     SDB_CUDA(cudaMemsetAsync(d_hist, 0, sizeof(uint32_t) * RMAX_BINS, st));
-    quantize_scan_kernel<<<ctx->sm_count * 8, 256, 0, st>>>((const float*)c->d_rows.get(), c->dim, c->n, c->d_mag, c->d_snorm,
-                                                            d_tmp + 3, d_rmax, d_hist);
+    if (c->dtype == SDB_F32)
+      quantize_scan_kernel<float><<<ctx->sm_count * 8, 256, 0, st>>>((const float*)c->d_rows.get(), c->dim, c->n, c->d_mag,
+                                                                     c->d_snorm, d_tmp + 3, d_rmax, d_hist);
+    else
+      quantize_scan_kernel<double><<<ctx->sm_count * 8, 256, 0, st>>>((const double*)c->d_rows.get(), c->dim, c->n, c->d_mag,
+                                                                      c->d_snorm, d_tmp + 3, d_rmax, d_hist);
     count_launch(ctx);
     // ---- pick the scale: if at most 64 rows sit far above the rest (their largest normalised component is more
     //      than 1.5 x that of the 65th), make THEM special rows and quantise for the others ----
@@ -360,8 +436,13 @@ sdb_status corpus_finalize_device(Corpus* c) {
         }
       }
     }
-    quantize_rows_kernel<<<ctx->sm_count * 8, 256, 0, st>>>((const float*)c->d_rows.get(), c->dim, c->dim_pad8, c->n, n_pad,
-                                                            c->d_mag, c->d_snorm, d_tmp + 3, c->d_i8, d_tmp + 2);
+    if (c->dtype == SDB_F32)
+      quantize_rows_kernel<float><<<ctx->sm_count * 8, 256, 0, st>>>((const float*)c->d_rows.get(), c->dim, c->dim_pad8, c->n,
+                                                                     n_pad, c->d_mag, c->d_snorm, d_tmp + 3, c->d_i8, d_tmp + 2);
+    else
+      quantize_rows_kernel<double><<<ctx->sm_count * 8, 256, 0, st>>>((const double*)c->d_rows.get(), c->dim, c->dim_pad8,
+                                                                      c->n, n_pad, c->d_mag, c->d_snorm, d_tmp + 3, c->d_i8,
+                                                                      d_tmp + 2);
     count_launch(ctx);
     SDB_CUDA(cudaGetLastError());
   }
