@@ -230,6 +230,37 @@ sdb_status sdb_knn_submit_device(sdb_corpus*, const double* d_queries, uint32_t 
                                  uint64_t* d_out_rows, double* d_out_dist, uint32_t* d_out_count, uint32_t* ticket);
 sdb_status sdb_knn_wait(sdb_corpus*, uint32_t ticket);
 
+/* ---- filtered brute force: `WHERE emb <|k|> $q AND cond`, the condition applied before ranking, per statement, with
+ * no change to the corpus (a filtered call is a search: the screen copies, the skip mask and the special rows stay as
+ * sdb_corpus_finalize left them, so one finalized column serves any number of predicates).
+ * filters: n_filters bitmaps of W = ceil(sdb_corpus_rows / 32) uint32 words each; bit r = bit r % 32 of word r / 32
+ * (the sdb_hop_filter convention).  No word past W - 1 of a bitmap is read.
+ * query_filter: ALWAYS host memory, nq indices < n_filters (checked, and copied before the call returns); NULL = every
+ * query uses filter 0.
+ * Query q ranks exactly the rows whose bit is set in its filter and that are neither skipped (sdb_corpus_set_skip) nor
+ * removed (sdb_corpus_remove): a set bit never brings a skipped or removed row back.  The result equals the unfiltered
+ * call's after set_skip(skip | ~filter) + finalize -- same rows, same order, bit-identical distances, same counts
+ * (out_count[q] < k when fewer rows pass, 0 when none does).  Everything else is as in the unfiltered calls: every
+ * metric, F32 and F64, k <= 4096, cancellation, sdb_knn_last_stats, up to 4 tickets in flight (filtered and unfiltered
+ * mixed), completion through sdb_knn_wait.  SDB_EINVAL: n_filters == 0 with nq > 0, filters == NULL, or an index >=
+ * n_filters.
+ * A query whose bitmap has at most 4096 set bits skips the screen (its passing rows are ranked directly; results are
+ * the same); sdb_knn_last_stats then reports screen_used = SDB_SCREEN_NONE_EXACT and n_passes = 0 for a batch of such
+ * queries only.
+ * Host variants: `filters` is host memory, staged per batch on the copy stream (submit: `queries`, `filters` and the
+ * outputs stay valid until the wait returns).  Device variant: d_filters is device memory. */
+sdb_status sdb_knn_bruteforce_filtered(sdb_corpus*, const double* queries, uint32_t nq, uint32_t k,
+                                       const uint32_t* filters, uint32_t n_filters, const uint32_t* query_filter,
+                                       uint64_t* out_rows, double* out_dist, uint32_t* out_count,
+                                       const volatile int* cancel_flag);
+sdb_status sdb_knn_bruteforce_filtered_device(sdb_corpus*, const double* d_queries, uint32_t nq, uint32_t k,
+                                              const uint32_t* d_filters, uint32_t n_filters,
+                                              const uint32_t* query_filter, uint64_t row_base, uint64_t* d_out_rows,
+                                              double* d_out_dist, uint32_t* d_out_count);
+sdb_status sdb_knn_submit_filtered(sdb_corpus*, const double* queries, uint32_t nq, uint32_t k,
+                                   const uint32_t* filters, uint32_t n_filters, const uint32_t* query_filter,
+                                   uint64_t* out_rows, double* out_dist, uint32_t* out_count, uint32_t* ticket);
+
 /* ---- multi-GPU brute force (SURVEY 8e): the corpus is row-sharded, every shard searches its rows, ONE NCCL
  * all-gather moves the per-shard top-k blocks and a merge kernel on every rank produces the global top-k by
  * (distance, global row).  NCCL lives inside the library (bound at run time with dlopen, so single-GPU users need

@@ -5,8 +5,9 @@ HnswIndex.knn_search, GraphEdgeScan) on top of the C ABI in include/sdbgpu.h; al
 hand-written sm_90a CUDA in surrealdb_b200/csrc.
 """
 from ._lib import SdbError, SO_PATH  # noqa: F401
-from .engine import Context, VectorColumn  # noqa: F401
-from .operators import Distance, KnnBruteForceLegacy, KnnContext, KnnScan, KnnTopK  # noqa: F401
+from .engine import Context, VectorColumn, pack_row_filter  # noqa: F401
+from .operators import (Distance, Filter, KnnBruteForceLegacy, KnnContext, KnnScan, KnnTopK, TableScan,  # noqa: F401
+                        Union)
 from .graph import CsrGraph, GraphEdgeScan, GraphStore  # noqa: F401
 from .hnsw import HnswIndex  # noqa: F401
 

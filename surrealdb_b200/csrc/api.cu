@@ -225,10 +225,93 @@ static sdb_status tap_list(Corpus* c, uint32_t nq, std::vector<Cand>* list, std:
   return SDB_OK;
 }
 
+// ---- direct regime of filtered batches: the queries whose filter passes at most DIRECT_MAX_ROWS rows ------------------
+// mixed batches run permuted (screened queries first, then the direct ones): gather of the queries, scatter of the results
+__global__ void gather_queries_kernel(const double* __restrict__ src, const uint32_t* __restrict__ perm, uint32_t dim,
+                                      double* __restrict__ dst) {
+  const uint32_t i = blockIdx.x;
+  const double* s = src + (size_t)perm[i] * dim;
+  for (uint32_t j = threadIdx.x; j < dim; j += blockDim.x) dst[(size_t)i * dim + j] = s[j];
+}
+__global__ void scatter_results_kernel(const uint32_t* __restrict__ perm, uint32_t k, const uint64_t* __restrict__ rows,
+                                       const double* __restrict__ dist, const uint32_t* __restrict__ cnt,
+                                       uint64_t* __restrict__ out_rows, double* __restrict__ out_dist,
+                                       uint32_t* __restrict__ out_cnt) {
+  const uint32_t i = blockIdx.x, d = perm[i];
+  const uint32_t n = cnt[i] < k ? cnt[i] : k;
+  for (uint32_t j = threadIdx.x; j < n; j += blockDim.x) {
+    out_rows[(size_t)d * k + j] = rows[(size_t)i * k + j];
+    out_dist[(size_t)d * k + j] = dist[(size_t)i * k + j];
+  }
+  if (threadIdx.x == 0) out_cnt[d] = cnt[i];
+}
+static sdb_status scatter_results(Corpus* c, Ticket& t) {
+  if (!t.permuted || !t.nq) return SDB_OK;
+  scatter_results_kernel<<<t.nq, 128, 0, t.stream>>>(t.d_perm, t.k, t.d_out_rows, t.d_out_dist, t.d_out_count,
+                                                     t.d_fin_rows, t.d_fin_dist, t.d_fin_count);
+  count_launch(c->ctx);
+  SDB_CUDA(cudaGetLastError());
+  return SDB_OK;
+}
+
+// queries q0 .. q0 + nd - 1 of the batch: no screen.  Each list holds exactly the query's passing rows, so tau stays
+// -inf and cand_final's proof holds trivially; the exact re-rank and cand_final order them as any candidate list.
+static sdb_status enqueue_direct(Corpus* c, Ticket& t, uint32_t q0, uint32_t nd, bool whole) {
+  cudaStream_t st = t.stream;
+  const uint32_t k = t.k;
+  SDB_TRY(scratch_for(c, nd, DIRECT_MAX_ROWS));
+  SDB_TRY(prep_queries(c, t.d_queries + (size_t)q0 * c->dim, nd, st));
+  SDB_TRY(cand_begin(c, nd, SDB_SCREEN_NONE_EXACT, st));
+  c->filt = t.filt;
+  c->filt.qf += q0;
+  SDB_TRY(cand_direct(c, nd, st));
+  SDB_TRY(cand_rerank(c, nd, st, false));
+  SDB_TRY(cand_final(c, nd, k, t.row_base, t.d_out_rows + (size_t)q0 * k, t.d_out_dist + (size_t)q0 * k,
+                     t.d_out_count + q0, st));
+  c->filt = t.filt;
+  SDB_CUDA(cudaMemcpyAsync(t.h_flags + q0, c->d_flags, sizeof(uint32_t) * nd, cudaMemcpyDeviceToHost, st));
+  SDB_CUDA(cudaMemcpyAsync(t.h_qflags + q0, c->d_qflags, sizeof(uint32_t) * nd, cudaMemcpyDeviceToHost, st));
+  if (whole) SDB_CUDA(cudaMemcpyAsync(t.h_stat, c->d_stat, sizeof(uint32_t) * 4, cudaMemcpyDeviceToHost, st));
+  return SDB_OK;
+}
+
+static sdb_status enqueue_screened(Corpus* c, Ticket& t);
 static sdb_status enqueue_batch(Corpus* c, Ticket& t) {
+  activate_set(c, t.set);
+  // the batch's row filter is visible to the launches below only (every launch copies it)
+  struct FiltScope {
+    Corpus* c;
+    ~FiltScope() { c->filt = FiltArg(); }
+  } filt_scope{c};
+  c->filt = t.filt;
+  const uint32_t nd = t.n_direct;
+  if (nd == 0) return enqueue_screened(c, t);
+  cudaStream_t st = t.stream;
+  if (nd == t.nq) {  // every query is direct: no screen at all
+    t.n_passes = 0;
+    t.screen = SDB_SCREEN_NONE_EXACT;
+    SDB_CUDA(cudaEventRecord(t.ev_begin, st));
+    SDB_CUDA(cudaEventRecord(t.ev_screen0, st));
+    SDB_CUDA(cudaEventRecord(t.ev_screen1, st));
+    SDB_TRY(enqueue_direct(c, t, 0, nd, true));
+    SDB_CUDA(cudaEventRecord(t.ev_end, st));
+    return SDB_OK;
+  }
+  // mixed (permuted) batch: the screened sub-batch, then the direct one behind it on the same stream and scratch set
+  SDB_TRY(scratch_for(c, t.nq, DIRECT_MAX_ROWS));  // sized for both, so that the direct part does not reallocate
+  const uint32_t ns = t.nq - nd;
+  t.nq = ns;
+  const sdb_status rc = enqueue_screened(c, t);
+  t.nq = ns + nd;
+  SDB_TRY(rc);
+  SDB_TRY(enqueue_direct(c, t, ns, nd, false));
+  SDB_CUDA(cudaEventRecord(t.ev_end, st));
+  return SDB_OK;
+}
+
+static sdb_status enqueue_screened(Corpus* c, Ticket& t) {
   Ctx* ctx = c->ctx;
   cudaStream_t st = t.stream;
-  activate_set(c, t.set);
   const uint32_t nq = t.nq, k = t.k;
   sdb_screen first;
   const std::vector<Rung> rungs = build_rungs(c, k, &first);
@@ -320,6 +403,7 @@ static sdb_status enqueue_batch(Corpus* c, Ticket& t) {
     refined = true;
     trace_mark(ctx, t, "refined", st);
   }
+  if (c->filt.bits) SDB_TRY(cand_add_specials(c, nq, st));  // each query re-ranks its own passing special rows
   SDB_TRY(cand_rerank(c, nq, st, refined));
   trace_mark(ctx, t, "reranked", st);
   SDB_TRY(cand_final(c, nq, k, t.row_base, t.d_out_rows, t.d_out_dist, t.d_out_count, st));
@@ -336,10 +420,10 @@ static sdb_status copy_out(Corpus* c, Ticket& t) {  // host-buffer entry points:
   cudaStream_t st = t.stream;
   if (!t.h_out_count) return SDB_OK;
   if (t.k) {
-    SDB_CUDA(cudaMemcpyAsync(t.h_out_rows, t.d_out_rows, sizeof(uint64_t) * (size_t)t.nq * t.k, cudaMemcpyDeviceToHost, st));
-    SDB_CUDA(cudaMemcpyAsync(t.h_out_dist, t.d_out_dist, sizeof(double) * (size_t)t.nq * t.k, cudaMemcpyDeviceToHost, st));
+    SDB_CUDA(cudaMemcpyAsync(t.h_out_rows, t.d_fin_rows, sizeof(uint64_t) * (size_t)t.nq * t.k, cudaMemcpyDeviceToHost, st));
+    SDB_CUDA(cudaMemcpyAsync(t.h_out_dist, t.d_fin_dist, sizeof(double) * (size_t)t.nq * t.k, cudaMemcpyDeviceToHost, st));
   }
-  SDB_CUDA(cudaMemcpyAsync(t.h_out_count, t.d_out_count, sizeof(uint32_t) * t.nq, cudaMemcpyDeviceToHost, st));
+  SDB_CUDA(cudaMemcpyAsync(t.h_out_count, t.d_fin_count, sizeof(uint32_t) * t.nq, cudaMemcpyDeviceToHost, st));
   SDB_CUDA(cudaEventRecord(t.ev_out, st));  // wait() blocks on THIS batch's copies, not on whatever was queued behind it
   return SDB_OK;
 }
@@ -387,6 +471,9 @@ static sdb_status finish_local(Corpus* c, Ticket& t, uint32_t* n_fallback, bool*
     const uint32_t save_rung = t.rung, save_nq = t.nq, save_passes = t.n_passes;
     const int save_screen = t.screen;
     const double* save_q = t.d_queries;
+    const uint32_t* save_qf = t.filt.qf;
+    const uint32_t save_nd = t.n_direct;
+    t.n_direct = 0;  // the failing queries are screened ones (a direct query's proof cannot fail)
     uint64_t* save_rows = t.d_out_rows;
     double* save_dist = t.d_out_dist;
     uint32_t* save_cnt = t.d_out_count;
@@ -405,6 +492,19 @@ static sdb_status finish_local(Corpus* c, Ticket& t, uint32_t* n_fallback, bool*
       }
       for (uint32_t i = 0; i < nf; i++)
         cudaMemcpyAsync(c->d_rp_q + (size_t)i * c->dim, save_q + (size_t)fails[i] * c->dim, sizeof(double) * c->dim, cudaMemcpyDeviceToDevice, st);
+      std::vector<uint32_t> rp_qf;  // filtered batch: each gathered query keeps its own filter
+      if (t.filt.bits) {
+        rp_qf.resize(nf);
+        for (uint32_t i = 0; i < nf; i++) rp_qf[i] = t.h_qf[fails[i]];
+        e = c->d_rp_qf.reserve(nf);
+        if (e == cudaSuccess) e = cudaMemcpyAsync(c->d_rp_qf, rp_qf.data(), sizeof(uint32_t) * nf, cudaMemcpyHostToDevice, st);
+        if (e != cudaSuccess) {
+          set_error("repair filter indices: %s", cudaGetErrorString(e));
+          rc = SDB_ECUDA;
+          break;
+        }
+        t.filt.qf = c->d_rp_qf;
+      }
       t.d_queries = c->d_rp_q;
       t.nq = nf;
       t.d_out_rows = c->rp.rows;
@@ -431,6 +531,8 @@ static sdb_status finish_local(Corpus* c, Ticket& t, uint32_t* n_fallback, bool*
       *repaired = true;
     }
     t.d_queries = save_q;
+    t.filt.qf = save_qf;
+    t.n_direct = save_nd;
     t.nq = save_nq;
     t.d_out_rows = save_rows;
     t.d_out_dist = save_dist;
@@ -450,12 +552,16 @@ static sdb_status finish_local(Corpus* c, Ticket& t, uint32_t* n_fallback, bool*
       return SDB_ECANCELLED;
     }
     SDB_TRY(prep_fallback_query(c, t.d_queries + (size_t)q * c->dim, st));
+    const uint32_t* q_filter = t.filt.bits ? t.filt.bits + (size_t)t.h_qf[q] * t.filt.words : nullptr;
     SDB_TRY(exact_query(c, c->d_fb_q, c->d_fb_qmag, c->d_fb_qflags, k, t.row_base, t.d_out_rows + (size_t)q * k,
-                        t.d_out_dist + (size_t)q * k, t.d_out_count + q, st));
+                        t.d_out_dist + (size_t)q * k, t.d_out_count + q, st, q_filter, t.filt.words));
     (*n_fallback)++;
     *repaired = true;
   }
-  if (*repaired) SDB_CUDA(cudaStreamSynchronize(st));
+  if (*repaired) {
+    SDB_TRY(scatter_results(c, t));  // a permuted batch: the repaired results to the caller's positions
+    SDB_CUDA(cudaStreamSynchronize(st));
+  }
   return SDB_OK;
 }
 
@@ -491,7 +597,8 @@ static Ticket* free_ticket(Corpus* c) {
 
 static sdb_status submit_locked(Corpus* c, Ticket* t, const double* d_queries, uint32_t nq, uint32_t k, uint64_t row_base,
                                 uint64_t* d_out_rows, double* d_out_dist, uint32_t* d_out_count,
-                                const volatile int* cancel) {
+                                const volatile int* cancel, const uint32_t* d_filters = nullptr,
+                                const uint32_t* query_filter = nullptr, const uint64_t* filter_rows = nullptr) {
   if (!c->finalized) {
     set_error("corpus not finalized (call sdb_corpus_finalize after the last append)");
     return SDB_EINVAL;
@@ -515,9 +622,53 @@ static sdb_status submit_locked(Corpus* c, Ticket* t, const double* d_queries, u
   t->nq = nq;
   t->k = k;
   t->row_base = row_base;
-  t->d_out_rows = d_out_rows;
-  t->d_out_dist = d_out_dist;
-  t->d_out_count = d_out_count;
+  t->d_fin_rows = t->d_out_rows = d_out_rows;
+  t->d_fin_dist = t->d_out_dist = d_out_dist;
+  t->d_fin_count = t->d_out_count = d_out_count;
+  t->filt = FiltArg();
+  t->n_direct = 0;
+  t->permuted = false;
+  if (d_filters) {  // filtered batch: per query filter index on the host (exact fallbacks, repairs) and the device
+    t->h_qf.assign(nq, 0u);
+    if (query_filter) std::copy(query_filter, query_filter + nq, t->h_qf.begin());
+    t->filt.bits = d_filters;
+    t->filt.words = (uint32_t)((c->n + 31) / 32);
+    // direct regime: a query whose filter passes at most DIRECT_MAX_ROWS rows (filter_rows: set bits, an upper bound
+    // of the rows it passes) skips the screen; the re-rank and cand_final serve the two screenable metrics, k <= 256
+    std::vector<uint32_t> scr, dir;
+    const bool direct_ok = filter_rows && k > 0 && k <= 256 && (c->metric == SDB_COSINE || c->metric == SDB_EUCLIDEAN);
+    for (uint32_t q = 0; q < nq; q++) {
+      const uint64_t rows_q = filter_rows ? filter_rows[t->h_qf[q]] : ~0ull;
+      if (direct_ok && rows_q <= DIRECT_MAX_ROWS) dir.push_back(q);
+      else {
+        scr.push_back(q);
+        if (rows_q < c->n / MASK_HITS_DIV) t->filt.mask_hits = 1;  // a selective filter among the screened queries
+      }
+    }
+    t->n_direct = (uint32_t)dir.size();
+    if (!dir.empty() && !scr.empty()) {  // mixed: run permuted, screened queries first (see Ticket::permuted)
+      std::vector<uint32_t> perm(scr);
+      perm.insert(perm.end(), dir.begin(), dir.end());
+      std::vector<uint32_t> qf(nq);
+      for (uint32_t i = 0; i < nq; i++) qf[i] = t->h_qf[perm[i]];
+      t->h_qf.swap(qf);
+      SDB_CUDA(t->d_perm.reserve(nq));
+      SDB_CUDA(t->d_pq.reserve((size_t)nq * c->dim));
+      SDB_CUDA(t->pres.reserve((size_t)nq * k, nq));
+      SDB_CUDA(cudaMemcpyAsync(t->d_perm, perm.data(), sizeof(uint32_t) * nq, cudaMemcpyHostToDevice, t->stream));
+      gather_queries_kernel<<<nq, 128, 0, t->stream>>>(d_queries, t->d_perm, c->dim, t->d_pq);
+      count_launch(c->ctx);
+      SDB_CUDA(cudaGetLastError());
+      t->permuted = true;
+      t->d_queries = t->d_pq;
+      t->d_out_rows = t->pres.rows;
+      t->d_out_dist = t->pres.dist;
+      t->d_out_count = t->pres.count;
+    }
+    SDB_CUDA(t->d_qf.reserve(nq ? nq : 1));
+    if (nq) SDB_CUDA(cudaMemcpyAsync(t->d_qf, t->h_qf.data(), sizeof(uint32_t) * nq, cudaMemcpyHostToDevice, t->stream));
+    t->filt.qf = t->d_qf;
+  }
   t->cancel = cancel;
   t->launches0 = c->ctx->launches;
   t->n_repaired = 0;
@@ -541,7 +692,8 @@ static sdb_status submit_locked(Corpus* c, Ticket* t, const double* d_queries, u
     t->busy = true;
     return SDB_OK;
   }
-  const sdb_status rc = enqueue_batch(c, *t);
+  sdb_status rc = enqueue_batch(c, *t);
+  if (rc == SDB_OK) rc = scatter_results(c, *t);
   if (rc == SDB_OK) t->busy = true;
   trace_host(c->ctx, t->id, "submitted");
   return rc;
@@ -1075,8 +1227,46 @@ sdb_status sdb_knn_submit_device(sdb_corpus* c, const double* d_queries, uint32_
   return SDB_OK;
 }
 
+// per filter used by the batch, on the host, as far as the two decisions need it: the exact number of set bits while
+// it is at most DIRECT_MAX_ROWS (direct regime; the count stops at the first bit beyond, after ~T / 32 / density words,
+// and all-zero words cost one compare), else an estimate from 4096 evenly spaced words, which only decides
+// FiltArg::mask_hits (a speed switch; either value gives the same results)
+static std::vector<uint64_t> count_filter_rows_host(const Corpus* c, const uint32_t* filters, uint32_t n_filters,
+                                                    const uint32_t* query_filter, uint32_t nq) {
+  const uint64_t words = (c->n + 31) / 32;
+  std::vector<uint64_t> cnt(n_filters, ~0ull);
+  for (uint32_t q = 0; q < nq; q++) {
+    const uint32_t f = query_filter ? query_filter[q] : 0u;
+    if (cnt[f] != ~0ull) continue;
+    const uint32_t* b = filters + (size_t)f * words;
+    uint64_t n = 0;
+    for (uint64_t w = 0; w < words && n <= DIRECT_MAX_ROWS; w++)
+      if (b[w]) n += (uint64_t)__builtin_popcount(b[w]);
+    if (n > DIRECT_MAX_ROWS) {
+      const uint64_t samples = std::min<uint64_t>(words, 4096), step = words / samples;
+      uint64_t s = 0;
+      for (uint64_t i = 0; i < samples; i++) s += (uint64_t)__builtin_popcount(b[i * step]);
+      n = std::max<uint64_t>(DIRECT_MAX_ROWS + 1, s * step);  // estimate, never below the direct bound
+    }
+    cnt[f] = n;
+  }
+  return cnt;
+}
+__global__ void count_filter_rows_kernel(const uint32_t* __restrict__ bits, uint64_t words,
+                                         unsigned long long* __restrict__ cnt) {
+  const uint32_t* b = bits + (size_t)blockIdx.y * words;
+  unsigned long long n = 0;
+  for (uint64_t w = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; w < words; w += (uint64_t)gridDim.x * blockDim.x)
+    n += (unsigned long long)__popc(__ldg(b + w));
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) n += __shfl_xor_sync(0xffffffffu, n, o);
+  if ((threadIdx.x & 31u) == 0 && n) atomicAdd(cnt + blockIdx.y, n);
+}
+
 static sdb_status submit_host_locked(sdb_corpus* c, const double* queries, uint32_t nq, uint32_t k, uint64_t* out_rows,
-                                     double* out_dist, uint32_t* out_count, const volatile int* cancel, Ticket** out_t) {
+                                     double* out_dist, uint32_t* out_count, const volatile int* cancel, Ticket** out_t,
+                                     const uint32_t* filters = nullptr, uint32_t n_filters = 0,
+                                     const uint32_t* query_filter = nullptr) {
   Ticket* t = free_ticket(c);
   if (!t) {
     set_error("too many batches in flight (%d): call sdb_knn_wait first", N_TICKETS);
@@ -1088,9 +1278,18 @@ static sdb_status submit_host_locked(sdb_corpus* c, const double* queries, uint3
   // the queries travel on the copy stream, so the transfer of batch i+1 overlaps the kernels of batch i
   cudaStream_t cs = c->ctx->copy_stream;
   SDB_CUDA(cudaMemcpyAsync(t->d_in_q, queries, sizeof(double) * (size_t)nq * c->dim, cudaMemcpyHostToDevice, cs));
+  if (filters) {  // ... and so do the row filters, into the slot's own copy
+    const size_t words = (size_t)n_filters * ((c->n + 31) / 32);
+    SDB_CUDA(t->d_in_filt.reserve(words ? words : 1));
+    if (words) SDB_CUDA(cudaMemcpyAsync(t->d_in_filt, filters, sizeof(uint32_t) * words, cudaMemcpyHostToDevice, cs));
+  }
   SDB_CUDA(cudaEventRecord(t->ev_h2d, cs));
   t->wait_h2d = true;  // submit_locked makes the batch's stream wait for the transfer
-  SDB_TRY(submit_locked(c, t, t->d_in_q, nq, k, c->row_base, t->res.rows, t->res.dist, t->res.count, cancel));
+  std::vector<uint64_t> rows_per_filter;
+  if (filters) rows_per_filter = count_filter_rows_host(c, filters, n_filters, query_filter, nq);
+  SDB_TRY(submit_locked(c, t, t->d_in_q, nq, k, c->row_base, t->res.rows, t->res.dist, t->res.count, cancel,
+                        filters ? t->d_in_filt.get() : nullptr, query_filter,
+                        filters ? rows_per_filter.data() : nullptr));
   t->h_out_rows = out_rows;
   t->h_out_dist = out_dist;
   t->h_out_count = out_count;
@@ -1247,6 +1446,7 @@ sdb_status sdb_debug_screen_batch(sdb_corpus* c, const double* queries, uint32_t
     t->d_out_count = out.count;
     t->cancel = nullptr;
     t->rung = 0;
+    t->filt = FiltArg();
     c->tap = &tap;
     const sdb_status rc = enqueue_batch(c, *t);
     c->tap = nullptr;
@@ -1389,6 +1589,87 @@ sdb_status sdb_knn_bruteforce(sdb_corpus* c, const double* queries, uint32_t nq,
   Ticket* t = nullptr;
   SDB_TRY(submit_host_locked(c, queries, nq, k, out_rows, out_dist, out_count, cancel_flag, &t));
   return wait_locked(c, t);
+}
+
+// ---- filtered brute-force KNN: per-query row bitmaps (see the header) ----------------------------------------------
+static sdb_status check_filters(uint32_t nq, const uint32_t* filters, uint32_t n_filters, const uint32_t* query_filter) {
+  if (nq && (n_filters == 0 || !filters)) {
+    set_error("filtered KNN: %s", n_filters == 0 ? "no filter given (n_filters == 0)" : "filters is NULL");
+    return SDB_EINVAL;
+  }
+  if (query_filter)
+    for (uint32_t q = 0; q < nq; q++)
+      if (query_filter[q] >= n_filters) {
+        set_error("filtered KNN: query %u uses filter %u of %u", q, query_filter[q], n_filters);
+        return SDB_EINVAL;
+      }
+  return SDB_OK;
+}
+
+sdb_status sdb_knn_bruteforce_filtered(sdb_corpus* c, const double* queries, uint32_t nq, uint32_t k,
+                                       const uint32_t* filters, uint32_t n_filters, const uint32_t* query_filter,
+                                       uint64_t* out_rows, double* out_dist, uint32_t* out_count,
+                                       const volatile int* cancel_flag) {
+  if (!c || (nq && (!queries || !out_count || (k && (!out_rows || !out_dist))))) return SDB_EINVAL;
+  SDB_TRY(check_filters(nq, filters, n_filters, query_filter));
+  if (nq == 0) return SDB_OK;
+  if (cancel_flag && *cancel_flag) {
+    set_error("query cancelled");
+    return SDB_ECANCELLED;
+  }
+  std::lock_guard<std::mutex> g(c->mu);
+  SDB_CUDA(cudaSetDevice(c->ctx->device));
+  Ticket* t = nullptr;
+  SDB_TRY(submit_host_locked(c, queries, nq, k, out_rows, out_dist, out_count, cancel_flag, &t, filters, n_filters,
+                             query_filter));
+  return wait_locked(c, t);
+}
+
+sdb_status sdb_knn_bruteforce_filtered_device(sdb_corpus* c, const double* d_queries, uint32_t nq, uint32_t k,
+                                              const uint32_t* d_filters, uint32_t n_filters,
+                                              const uint32_t* query_filter, uint64_t row_base, uint64_t* d_out_rows,
+                                              double* d_out_dist, uint32_t* d_out_count) {
+  if (!c || (nq && (!d_queries || !d_out_count || (k && (!d_out_rows || !d_out_dist))))) return SDB_EINVAL;
+  SDB_TRY(check_filters(nq, d_filters, n_filters, query_filter));
+  if (nq == 0) return SDB_OK;
+  std::lock_guard<std::mutex> g(c->mu);
+  SDB_CUDA(cudaSetDevice(c->ctx->device));
+  Ticket* t = free_ticket(c);
+  if (!t) {
+    set_error("too many batches in flight (%d): call sdb_knn_wait first", N_TICKETS);
+    return SDB_EOVERFLOW;
+  }
+  std::vector<uint64_t> rows_per_filter(n_filters, 0);
+  if (c->finalized && c->n) {  // a blocking call anyway: count the bitmaps' set bits on the device and read them back
+    const uint64_t words = (c->n + 31) / 32;
+    AsyncBuf<unsigned long long> d_cnt;
+    cudaStream_t st = c->ctx->stream;
+    SDB_CUDA(d_cnt.reserve(n_filters, st));
+    SDB_CUDA(cudaMemsetAsync(d_cnt, 0, sizeof(unsigned long long) * n_filters, st));
+    const uint32_t gx = (uint32_t)std::min<uint64_t>((words + 255) / 256, 64);
+    count_filter_rows_kernel<<<dim3(gx, n_filters), 256, 0, st>>>(d_filters, words, d_cnt);
+    count_launch(c->ctx);
+    SDB_CUDA(cudaGetLastError());
+    SDB_CUDA(cudaMemcpyAsync(rows_per_filter.data(), d_cnt, sizeof(uint64_t) * n_filters, cudaMemcpyDeviceToHost, st));
+    SDB_CUDA(cudaStreamSynchronize(st));
+  }
+  SDB_TRY(submit_locked(c, t, d_queries, nq, k, row_base, d_out_rows, d_out_dist, d_out_count, nullptr, d_filters,
+                        query_filter, rows_per_filter.data()));
+  return wait_locked(c, t);
+}
+
+sdb_status sdb_knn_submit_filtered(sdb_corpus* c, const double* queries, uint32_t nq, uint32_t k,
+                                   const uint32_t* filters, uint32_t n_filters, const uint32_t* query_filter,
+                                   uint64_t* out_rows, double* out_dist, uint32_t* out_count, uint32_t* ticket) {
+  if (!c || !ticket || !nq || !queries || !out_count || (k && (!out_rows || !out_dist))) return SDB_EINVAL;
+  SDB_TRY(check_filters(nq, filters, n_filters, query_filter));
+  std::lock_guard<std::mutex> g(c->mu);
+  SDB_CUDA(cudaSetDevice(c->ctx->device));
+  Ticket* t = nullptr;
+  SDB_TRY(submit_host_locked(c, queries, nq, k, out_rows, out_dist, out_count, nullptr, &t, filters, n_filters,
+                             query_filter));
+  *ticket = t->id;
+  return SDB_OK;
 }
 
 sdb_status sdb_corpus_project(sdb_corpus* c, const double* query, int fn, double* out) {

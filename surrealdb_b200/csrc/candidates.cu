@@ -313,6 +313,87 @@ sdb_status cand_set_count(Corpus* c, uint32_t nq, uint32_t value, cudaStream_t s
   return SDB_OK;
 }
 
+// filtered batches: a pass-0 launch wrote every row of its tiles to fixed slots; the rows a query's filter rejects get
+// a NaN score, and cand_select drops them with the invalid rows
+__global__ void __launch_bounds__(256) cand_filter_list_kernel(Cand* __restrict__ cand, const uint32_t* __restrict__ cnt,
+                                                                uint32_t cap, FiltArg filt) {
+  const uint32_t q = blockIdx.x;
+  const uint32_t n = cnt[q] < cap ? cnt[q] : cap;
+  Cand* cq = cand + (size_t)q * cap;
+  for (uint32_t i = threadIdx.x; i < n; i += blockDim.x)
+    if (!filt_pass(filt, q, cq[i].row)) cq[i].score = __int_as_float(0x7fc00000);
+}
+sdb_status cand_filter_list(Corpus* c, uint32_t nq, cudaStream_t st) {
+  cand_filter_list_kernel<<<nq, 256, 0, st>>>(c->d_cand, c->d_cand_cnt, c->sc_cap, c->filt);
+  count_launch(c->ctx);
+  SDB_CUDA(cudaGetLastError());
+  return SDB_OK;
+}
+
+// filtered batches: the special rows (ranked exactly on every query of an unfiltered batch) join the list of each query
+// whose filter passes them, so that the re-rank and the final ordering see exactly the query's own row set
+__global__ void __launch_bounds__(256) cand_add_specials_kernel(Cand* __restrict__ cand, uint32_t* __restrict__ cnt,
+                                                                 uint32_t* __restrict__ flags, uint32_t cap,
+                                                                 const uint32_t* __restrict__ special, uint32_t n_special,
+                                                                 FiltArg filt) {
+  const uint32_t q = blockIdx.x;
+  for (uint32_t i = threadIdx.x; i < n_special; i += blockDim.x) {
+    const uint32_t row = special[i];
+    if (!filt_pass(filt, q, row)) continue;
+    const uint32_t pos = atomicAdd(cnt + q, 1u);
+    if (pos < cap) {
+      Cand cd;
+      cd.score = __int_as_float(0x7f800000);
+      cd.row = row;
+      cand[(size_t)q * cap + pos] = cd;
+    } else {
+      atomicOr(flags + q, 1u);  // no room: the query is re-run
+    }
+  }
+}
+sdb_status cand_add_specials(Corpus* c, uint32_t nq, cudaStream_t st) {
+  if (!c->n_special) return SDB_OK;
+  cand_add_specials_kernel<<<nq, 256, 0, st>>>(c->d_cand, c->d_cand_cnt, c->d_flags, c->sc_cap, c->d_special,
+                                               c->n_special, c->filt);
+  count_launch(c->ctx);
+  SDB_CUDA(cudaGetLastError());
+  return SDB_OK;
+}
+
+// direct regime: the query's bitmap words, set bit by set bit; rows past the corpus and skipped / removed rows (the
+// tombstones are in the skip mask) are left out.  List order does not matter: cand_final orders by (distance, row).
+__global__ void __launch_bounds__(256) cand_direct_kernel(Cand* __restrict__ cand, uint32_t* __restrict__ cnt,
+                                                           uint32_t* __restrict__ flags, uint32_t cap, FiltArg filt,
+                                                           const uint8_t* __restrict__ skip, uint64_t n) {
+  const uint32_t q = blockIdx.x;
+  const uint64_t need = (n + 31) / 32;
+  const uint32_t nw = need < filt.words ? (uint32_t)need : filt.words;
+  const uint32_t* b = filt.bits + (size_t)__ldg(filt.qf + q) * filt.words;
+  for (uint32_t w = threadIdx.x; w < nw; w += blockDim.x) {
+    uint32_t x = __ldg(b + w);
+    while (x) {
+      const uint32_t r = w * 32u + (uint32_t)(__ffs(x) - 1);
+      x &= x - 1u;
+      if (r >= n || (skip && skip[r])) continue;
+      const uint32_t pos = atomicAdd(cnt + q, 1u);
+      if (pos < cap) {
+        Cand cd;
+        cd.score = __int_as_float(0x7f800000);
+        cd.row = r;
+        cand[(size_t)q * cap + pos] = cd;
+      } else {
+        atomicOr(flags + q, 1u);  // more rows than the list holds: the query is re-run (cannot happen below cap)
+      }
+    }
+  }
+}
+sdb_status cand_direct(Corpus* c, uint32_t nq, cudaStream_t st) {
+  cand_direct_kernel<<<nq, 256, 0, st>>>(c->d_cand, c->d_cand_cnt, c->d_flags, c->sc_cap, c->filt, c->d_skip, c->n);
+  count_launch(c->ctx);
+  SDB_CUDA(cudaGetLastError());
+  return SDB_OK;
+}
+
 constexpr uint32_t SEL_SMEM_KEYS = 1408;  // 11 KB: cand_select fits beside a resident screen CTA (15 KB are free)
 
 __device__ __forceinline__ Cand key_to_cand(uint64_t key) {
@@ -917,46 +998,47 @@ sdb_status cand_rerank(Corpus* c, uint32_t nq, cudaStream_t st, bool small_sets)
   const dim3 grid(nq, RR_GROUPS_Y);
   static const bool no_v4 = getenv("SDB_RERANK_SCALAR") != nullptr;
   static const bool no_packed = getenv("SDB_RERANK_STAGED") != nullptr;
+  const uint32_t n_sp = c->filt.bits ? 0u : c->n_special;  // filtered: the passing special rows are in the lists
   if (small_sets && !no_packed && (c->metric == SDB_COSINE || c->metric == SDB_EUCLIDEAN)) {
     const unsigned g = (nq + 7) / 8;
     const float* f32_rows = (const float*)c->d_rows.get();
     const double* f64_rows = (const double*)c->d_rows.get();
     if (c->dtype == SDB_F32 && c->metric == SDB_COSINE)
       cand_rerank_packed_kernel<float, true><<<g, 128, 0, st>>>(f32_rows, c->dim, c->d_mag, c->d_q64, c->d_qmag, c->d_qflags,
-                                                               c->d_cand, c->d_cand_cnt, c->sc_cap, c->d_special, c->n_special,
+                                                               c->d_cand, c->d_cand_cnt, c->sc_cap, c->d_special, n_sp,
                                                                nq, c->d_rr_key, c->d_rr_dist, c->d_rr_row, c->rr_stride);
     else if (c->dtype == SDB_F32)
       cand_rerank_packed_kernel<float, false><<<g, 128, 0, st>>>(f32_rows, c->dim, c->d_mag, c->d_q64, c->d_qmag, c->d_qflags,
-                                                                c->d_cand, c->d_cand_cnt, c->sc_cap, c->d_special, c->n_special,
+                                                                c->d_cand, c->d_cand_cnt, c->sc_cap, c->d_special, n_sp,
                                                                 nq, c->d_rr_key, c->d_rr_dist, c->d_rr_row, c->rr_stride);
     else if (c->metric == SDB_COSINE)
       cand_rerank_packed_kernel<double, true><<<g, 128, 0, st>>>(f64_rows, c->dim, c->d_mag, c->d_q64, c->d_qmag, c->d_qflags,
-                                                                c->d_cand, c->d_cand_cnt, c->sc_cap, c->d_special, c->n_special,
+                                                                c->d_cand, c->d_cand_cnt, c->sc_cap, c->d_special, n_sp,
                                                                 nq, c->d_rr_key, c->d_rr_dist, c->d_rr_row, c->rr_stride);
     else
       cand_rerank_packed_kernel<double, false><<<g, 128, 0, st>>>(f64_rows, c->dim, c->d_mag, c->d_q64, c->d_qmag, c->d_qflags,
-                                                                 c->d_cand, c->d_cand_cnt, c->sc_cap, c->d_special, c->n_special,
+                                                                 c->d_cand, c->d_cand_cnt, c->sc_cap, c->d_special, n_sp,
                                                                  nq, c->d_rr_key, c->d_rr_dist, c->d_rr_row, c->rr_stride);
   } else if (small_sets && c->dtype == SDB_F32)
     // (kept for A/B: one warp per query, rows transposed through 6 KB of shared memory)
     cand_rerank_kernel<float, 1, 32, 256><<<grid, 32, 0, st>>>((const float*)c->d_rows.get(), c->dim, (int)c->metric, c->d_mag,
                                                                c->d_q64, c->d_qmag, c->d_qflags, c->d_cand, c->d_cand_cnt,
-                                                               c->sc_cap, c->d_special, c->n_special, c->d_rr_key,
+                                                               c->sc_cap, c->d_special, n_sp, c->d_rr_key,
                                                                c->d_rr_dist, c->d_rr_row, c->rr_stride);
   else if (c->dtype == SDB_F32 && c->dim % 4 == 0 && !no_v4)
     cand_rerank_v4_kernel<4><<<grid, 128, RRV_SMEM, st>>>((const float*)c->d_rows.get(), c->dim, (int)c->metric, c->d_mag, c->d_q64,
                                                           c->d_qmag, c->d_qflags, c->d_cand, c->d_cand_cnt, c->sc_cap,
-                                                          c->d_special, c->n_special, c->d_rr_key, c->d_rr_dist,
+                                                          c->d_special, n_sp, c->d_rr_key, c->d_rr_dist,
                                                           c->d_rr_row, c->rr_stride);
   else if (c->dtype == SDB_F32)
     cand_rerank_kernel<float, 4, 32><<<grid, 128, 0, st>>>((const float*)c->d_rows.get(), c->dim, (int)c->metric, c->d_mag,
                                                            c->d_q64, c->d_qmag, c->d_qflags, c->d_cand, c->d_cand_cnt,
-                                                           c->sc_cap, c->d_special, c->n_special, c->d_rr_key,
+                                                           c->sc_cap, c->d_special, n_sp, c->d_rr_key,
                                                            c->d_rr_dist, c->d_rr_row, c->rr_stride);
   else
     cand_rerank_kernel<double, 4, 32><<<grid, 128, 0, st>>>((const double*)c->d_rows.get(), c->dim, (int)c->metric, c->d_mag,
                                                             c->d_q64, c->d_qmag, c->d_qflags, c->d_cand, c->d_cand_cnt,
-                                                            c->sc_cap, c->d_special, c->n_special, c->d_rr_key,
+                                                            c->sc_cap, c->d_special, n_sp, c->d_rr_key,
                                                             c->d_rr_dist, c->d_rr_row, c->rr_stride);
   count_launch(c->ctx);
   SDB_CUDA(cudaGetLastError());
@@ -1091,8 +1173,9 @@ sdb_status cand_final(Corpus* c, uint32_t nq, uint32_t k, uint64_t row_base, uin
     return SDB_EINVAL;
   }
   static const int debug = getenv("SDB_DEBUG") != nullptr;
+  const uint32_t n_sp = c->filt.bits ? 0u : c->n_special;  // filtered: the passing special rows are in the lists
   cand_final_kernel<<<nq, 256, 0, st>>>(c->d_rr_key, c->d_rr_dist, c->d_rr_row, c->rr_stride, c->d_cand_cnt, c->sc_cap,
-                                        c->n_special, c->d_tau, c->d_qmag, c->d_bscale, c->d_beps, c->d_tau2, c->d_beps2, c->d_flags, c->d_qflags, c->d_stat,
+                                        n_sp, c->d_tau, c->d_qmag, c->d_bscale, c->d_beps, c->d_tau2, c->d_beps2, c->d_flags, c->d_qflags, c->d_stat,
                                         (int)c->metric, k, row_base, d_out_rows, d_out_dist, d_out_count, debug);
   count_launch(c->ctx);
   SDB_CUDA(cudaGetLastError());

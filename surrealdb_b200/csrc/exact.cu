@@ -358,6 +358,13 @@ __global__ void __launch_bounds__(1024) sel_emit_kernel(const SelState* st, cons
   if (threadIdx.x == 0) *out_count = n;
 }
 
+// filtered queries: rows the query's bitmap rejects leave the selection like skipped rows
+__global__ void __launch_bounds__(256) exact_filter_keys_kernel(uint64_t* __restrict__ keys, uint64_t n,
+                                                                const uint32_t* __restrict__ bits) {
+  for (uint64_t r = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; r < n; r += (uint64_t)gridDim.x * blockDim.x)
+    if (!((__ldg(bits + (r >> 5)) >> (r & 31u)) & 1u)) keys[r] = KEY_SKIPPED;
+}
+
 sdb_status exact_init_device() {
   SDB_CUDA(cudaFuncSetAttribute(sel_emit_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 16 * 4096));
   return SDB_OK;
@@ -366,7 +373,7 @@ sdb_status exact_init_device() {
 // d_out_rows / d_out_dist / d_out_count point at THIS query's output row
 sdb_status exact_query(Corpus* c, const double* d_q64, const double* d_qmag, const uint32_t* d_qflags, uint32_t k,
                        uint64_t row_base, uint64_t* d_out_rows, double* d_out_dist, uint32_t* d_out_count,
-                       cudaStream_t st) {
+                       cudaStream_t st, const uint32_t* filter, uint32_t filter_words) {
   Ctx* ctx = c->ctx;
   {
     const uint64_t cap = c->cap > c->n ? c->cap : c->n;
@@ -394,6 +401,15 @@ sdb_status exact_query(Corpus* c, const double* d_q64, const double* d_qmag, con
       exact_keys_kernel<double, 4><<<grid, 128, 0, st>>>((const double*)c->d_rows.get(), c->dim, n, (int)c->metric,
                                                          c->d_mag, c->d_skip, d_q64, d_qmag, d_qflags, c->d_ex_key,
                                                          c->d_ex_val, c->minkowski_p);
+    count_launch(ctx);
+  }
+  if (n && filter) {
+    if ((n + 31) / 32 > filter_words) {
+      set_error("exact path: the row filter has %u words, the corpus needs %llu", filter_words,
+                (unsigned long long)((n + 31) / 32));
+      return SDB_EINVAL;
+    }
+    exact_filter_keys_kernel<<<ctx->sm_count * 4, 256, 0, st>>>(c->d_ex_key, n, filter);
     count_launch(ctx);
   }
   sel_init_kernel<<<1, 256, 0, st>>>(sel, k);

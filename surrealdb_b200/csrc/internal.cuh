@@ -193,6 +193,28 @@ __host__ __device__ inline uint32_t pass_tile(const PassDesc& p, uint32_t w) {
   return i * p.stride;
 }
 
+// ---- per-query row filters (sdb_knn_*_filtered) --------------------------------------------------------------------
+// bits: n_filters bitmaps of `words` uint32 words each (bit r = bit r % 32 of word r / 32); qf: the filter index of each
+// query of the launch (offset like every other per-query array of a query-chunked launch).  bits == nullptr: no filter.
+struct FiltArg {
+  const uint32_t* bits = nullptr;
+  const uint32_t* qf = nullptr;
+  uint32_t words = 0;
+  // int8 screens: also clear rejected rows from the consumers' hit masks (set when some query of the batch has a
+  // selective filter, which keeps its threshold low; with dense filters the drain warp's test alone is cheaper)
+  uint32_t mask_hits = 0;
+};
+// filtered batches: a query whose filter passes at most this many rows skips the screen (the direct regime): its
+// passing rows are compacted into its candidate list and ranked by the exact re-rank (DESIGN.md section 5)
+constexpr uint32_t DIRECT_MAX_ROWS = 4096;
+// ... and a filter passing fewer than 1/MASK_HITS_DIV of the rows switches FiltArg::mask_hits on
+constexpr uint64_t MASK_HITS_DIV = 20;
+// does query q rank corpus row `row`?  Rows past the bitmap (the screen copies' padding) never pass.
+__device__ __forceinline__ bool filt_pass(const FiltArg& f, uint32_t q, uint32_t row) {
+  const uint32_t w = row >> 5;
+  return w < f.words && ((__ldg(f.bits + (size_t)__ldg(f.qf + q) * f.words + w) >> (row & 31u)) & 1u) != 0;
+}
+
 struct Comm;  // comm.cu: NCCL communicator attached to a context (nullptr = single shard)
 
 struct Ctx {
@@ -265,6 +287,22 @@ struct Ticket {
   cudaEvent_t ev_h2d = nullptr, ev_out = nullptr;
   cudaEvent_t ev_main = nullptr;  // recorded after this batch's last screen launch (the next batch's screen waits for it)
   bool wait_h2d = false;  // the batch's stream still has to wait for ev_h2d (queries travelling on the copy stream)
+  // filtered batches: filt.bits = the caller's device bitmaps or d_in_filt (host bitmaps staged per slot), filt.qf =
+  // d_qf (per query filter index, also kept on the host in h_qf); unfiltered batches: filt.bits == nullptr
+  FiltArg filt;
+  std::vector<uint32_t> h_qf;
+  DevBuf<uint32_t> d_qf, d_in_filt;
+  // direct regime: the last n_direct queries of the batch skip the screen.  A batch that mixes both kinds runs
+  // permuted (screened queries first): d_queries / d_out_* / h_qf are then the permuted copies (d_pq, pres) and the
+  // results are scattered through d_perm (permuted position -> caller's query) to d_fin_*, the caller's outputs
+  uint32_t n_direct = 0;
+  bool permuted = false;
+  DevBuf<double> d_pq;
+  DevBuf<uint32_t> d_perm;
+  ResultBufs pres;
+  uint64_t* d_fin_rows = nullptr;
+  double* d_fin_dist = nullptr;
+  uint32_t* d_fin_count = nullptr;
   // SDB_TRACE=1: named timestamps of this batch on its stream, printed at wait time relative to the context's epoch
   std::vector<std::pair<const char*, cudaEvent_t>> trace;
 };
@@ -363,7 +401,9 @@ struct Corpus : Scratch {
   DevBuf<uint32_t> d_sel;     // radix-select state
   DevBuf<double> d_fb_q;      // fallback query scratch (one query: f64 copy, |q|, flags)
   DevBuf<double> d_rp_q;      // repair sub-batch: the failed queries of a batch, gathered, and their results
+  DevBuf<uint32_t> d_rp_qf;   // ... and their filter indices (filtered batches)
   ResultBufs rp;
+  FiltArg filt;               // row filter of the batch being enqueued (enqueue_batch sets it; launches copy it)
   DevBuf<double> d_fb_qmag;
   DevBuf<uint32_t> d_fb_qflags;
   Scratch parked;  // the inactive set (see Scratch)
@@ -406,13 +446,22 @@ sdb_status cand_select(Corpus* c, uint32_t nq, uint32_t k, bool drop_invalid, ui
 sdb_status cand_refine(Corpus* c, uint32_t nq, cudaStream_t st);
 // after a probe launch over n_tiles tiles: tau = (k-th largest chunk maximum) - margin, histogram geometry, empty lists
 sdb_status cand_seed_from_probe(Corpus* c, uint32_t nq, uint32_t k, uint32_t n_tiles, cudaStream_t st);
+// filtered batches (c->filt set): after a pass-0 launch, give the entries of rows a query's filter rejects a NaN score,
+// which cand_select drops like any invalid row
+sdb_status cand_filter_list(Corpus* c, uint32_t nq, cudaStream_t st);
+// filtered batches: append each query's passing special rows to its list (the re-rank and cand_final then run without
+// the shared special-row tail); a list that has no room is flagged as overflowed
+sdb_status cand_add_specials(Corpus* c, uint32_t nq, cudaStream_t st);
+// direct regime (c->filt set): each query's list = the rows its filter passes that are neither skipped nor removed
+sdb_status cand_direct(Corpus* c, uint32_t nq, cudaStream_t st);
 sdb_status cand_rerank(Corpus* c, uint32_t nq, cudaStream_t st, bool small_sets = false);
 sdb_status cand_final(Corpus* c, uint32_t nq, uint32_t k, uint64_t row_base, uint64_t* d_out_rows, double* d_out_dist,
                       uint32_t* d_out_count, cudaStream_t st);
-// exact.cu: query vector / |q| / flags are passed explicitly (batch scratch row or the fallback scratch)
+// exact.cu: query vector / |q| / flags are passed explicitly (batch scratch row or the fallback scratch).
+// filter: nullptr, or the query's bitmap (c->filt.words words): rows whose bit is clear are not ranked.
 sdb_status exact_query(Corpus* c, const double* d_q64, const double* d_qmag, const uint32_t* d_qflags, uint32_t k,
                        uint64_t row_base, uint64_t* d_out_rows, double* d_out_dist, uint32_t* d_out_count,
-                       cudaStream_t st);
+                       cudaStream_t st, const uint32_t* filter = nullptr, uint32_t filter_words = 0);
 // gen.cu
 sdb_status exact_project(Corpus* c, int fn, double* d_vals, cudaStream_t st);
 sdb_status gen_fill_f32(Ctx* ctx, float* d_out, uint64_t seed, uint64_t first, uint64_t n, cudaStream_t st);

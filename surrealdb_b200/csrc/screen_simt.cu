@@ -49,11 +49,13 @@ __device__ __forceinline__ void bulk_load(uint32_t dst, const void* src, uint32_
 
 // RPW = rows per consumer warp per stage (4, 2 or 1; chosen so that 2 stages + the queries fit shared memory)
 // QB  = queries per launch (1, 4 or 8): fewer queries = less shared-memory read traffic per row
-template <int RPW, int QB>
+// FILT: filtered batch -- a row the query's filter rejects is never appended (filt.qf is indexed by q0 + query)
+template <int RPW, int QB, bool FILT>
 __global__ void __launch_bounds__(SIMT_THREADS, 1) screen_simt_kernel(
     const float* __restrict__ rows, const float* __restrict__ snorm, uint32_t dim, uint64_t n_rows,
     const float* __restrict__ q32, uint32_t q0, uint32_t nqb, int metric, PassDesc pass,
-    const float* __restrict__ tau, Cand* __restrict__ cand, uint32_t* __restrict__ cand_cnt, uint32_t cap) {
+    const float* __restrict__ tau, Cand* __restrict__ cand, uint32_t* __restrict__ cand_cnt, uint32_t cap,
+    FiltArg filt) {
   constexpr int RPS = RPW * SIMT_CWARPS;  // rows per stage
   extern __shared__ __align__(128) uint8_t smem_raw[];
   float* s_q = reinterpret_cast<float*>(smem_raw);                 // [QB][dim]
@@ -152,7 +154,7 @@ __global__ void __launch_bounds__(SIMT_THREADS, 1) screen_simt_kernel(
           if (lane < nqb && row < n_rows) {
             const float sn = __ldg(snorm + row);
             const float sc = metric == SDB_COSINE ? mine * sn : fmaf(2.f, mine, -sn);
-            if (sc >= my_tau) {  // NaN (skipped / special rows) never passes
+            if (sc >= my_tau && (!FILT || filt_pass(filt, q0 + lane, (uint32_t)row))) {  // NaN (skipped / special rows) never passes
               const uint32_t pos = atomicAdd(cand_cnt + q0 + lane, 1u);
               if (pos < cap) {
                 Cand cd;
@@ -169,10 +171,12 @@ __global__ void __launch_bounds__(SIMT_THREADS, 1) screen_simt_kernel(
 }
 
 // generic fallback for dimensions that are not a multiple of 4 (rows not 16-byte aligned): plain coalesced loads
+template <bool FILT>
 __global__ void __launch_bounds__(256) screen_simt_generic_kernel(
     const float* __restrict__ rows, const float* __restrict__ snorm, uint32_t dim, uint64_t n_rows,
     const float* __restrict__ q32, uint32_t q0, uint32_t nqb, int metric, PassDesc pass,
-    const float* __restrict__ tau, Cand* __restrict__ cand, uint32_t* __restrict__ cand_cnt, uint32_t cap) {
+    const float* __restrict__ tau, Cand* __restrict__ cand, uint32_t* __restrict__ cand_cnt, uint32_t cap,
+    FiltArg filt) {
   extern __shared__ __align__(16) uint8_t smem_raw[];
   float* s_q = reinterpret_cast<float*>(smem_raw);
   const uint32_t warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -207,7 +211,7 @@ __global__ void __launch_bounds__(256) screen_simt_generic_kernel(
       if (lane < nqb) {
         const float sn = __ldg(snorm + row);
         const float sc = metric == SDB_COSINE ? mine * sn : fmaf(2.f, mine, -sn);
-        if (sc >= my_tau) {
+        if (sc >= my_tau && (!FILT || filt_pass(filt, q0 + lane, (uint32_t)row))) {
           const uint32_t pos = atomicAdd(cand_cnt + q0 + lane, 1u);
           if (pos < cap) {
             Cand cd;
@@ -224,14 +228,14 @@ __global__ void __launch_bounds__(256) screen_simt_generic_kernel(
 template <int RPW, int QB>
 static sdb_status launch_ring_q(Corpus* c, uint32_t nq, const PassDesc& p, cudaStream_t st, size_t smem) {
   Ctx* ctx = c->ctx;
-  auto kern = screen_simt_kernel<RPW, QB>;
+  auto kern = c->filt.bits ? screen_simt_kernel<RPW, QB, true> : screen_simt_kernel<RPW, QB, false>;
   SDB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   uint32_t grid = (uint32_t)ctx->sm_count;
   if (grid > p.count) grid = p.count;
   for (uint32_t q0 = 0; q0 < nq; q0 += QB) {
     const uint32_t nqb = nq - q0 < (uint32_t)QB ? nq - q0 : (uint32_t)QB;
     kern<<<grid, SIMT_THREADS, smem, st>>>((const float*)c->d_rows.get(), c->d_snorm, c->dim, c->n, c->d_q32, q0, nqb,
-                                           (int)c->metric, p, c->d_tau, c->d_cand, c->d_cand_cnt, c->sc_cap);
+                                           (int)c->metric, p, c->d_tau, c->d_cand, c->d_cand_cnt, c->sc_cap, c->filt);
     count_launch(ctx);
   }
   SDB_CUDA(cudaGetLastError());
@@ -262,17 +266,17 @@ sdb_status screen_simt_pass(Corpus* c, uint32_t nq, const PassDesc& p, cudaStrea
     set_error("screen_simt: dim %u too large for the shared-memory query tile", c->dim);
     return SDB_EUNSUPPORTED;
   }
-  SDB_CUDA(cudaFuncSetAttribute(screen_simt_generic_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)q_bytes));
+  auto kern = c->filt.bits ? screen_simt_generic_kernel<true> : screen_simt_generic_kernel<false>;
+  SDB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)q_bytes));
   int per_sm = 1;
-  SDB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, screen_simt_generic_kernel, 256, q_bytes));
+  SDB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, 256, q_bytes));
   if (per_sm < 1) per_sm = 1;
   uint32_t grid = (uint32_t)(ctx->sm_count * per_sm);
   if (grid > p.count) grid = p.count;
   for (uint32_t q0 = 0; q0 < nq; q0 += SIMT_QB) {
     const uint32_t nqb = nq - q0 < (uint32_t)SIMT_QB ? nq - q0 : (uint32_t)SIMT_QB;
-    screen_simt_generic_kernel<<<grid, 256, q_bytes, st>>>((const float*)c->d_rows.get(), c->d_snorm, c->dim, c->n, c->d_q32, q0,
-                                                          nqb, (int)c->metric, p, c->d_tau, c->d_cand, c->d_cand_cnt,
-                                                          c->sc_cap);
+    kern<<<grid, 256, q_bytes, st>>>((const float*)c->d_rows.get(), c->d_snorm, c->dim, c->n, c->d_q32, q0, nqb,
+                                     (int)c->metric, p, c->d_tau, c->d_cand, c->d_cand_cnt, c->sc_cap, c->filt);
     count_launch(ctx);
   }
   SDB_CUDA(cudaGetLastError());

@@ -281,14 +281,18 @@ __device__ __forceinline__ void push_survivors(const uint32_t (&acc)[128], int i
 //         (probe[q][tile * 8 + chunk]).  The chunk maxima belong to DISJOINT row sets, so the k-th largest of them is a
 //         lower bound of the k-th best score of the corpus: the seed of the streaming pass's thresholds, at the cost
 //         of one round of MMAs and no candidate traffic.
-template <bool COSINE, bool INT8, int MODE>
+// FILT: filtered batch -- rows a query's filter rejects never reach its lists, its histogram or its chunk maxima.  The
+// test sits where a survivor is appended (bf16: the consumer's append; int8: the drain warp, next to the screening-norm
+// look-up) and, in the probe, on the one bitmap word of every 32-row chunk.  Pass 0 writes every row; cand_filter_list
+// drops the rejected ones there.
+template <bool COSINE, bool INT8, int MODE, bool FILT>
 __global__ void __launch_bounds__(threads<INT8, MODE>(), 1)
 screen_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b,
                  const float* __restrict__ snorm, uint32_t k_blocks, uint32_t n_mblocks, uint32_t nq,
                  PassDesc pass, float* tau, Cand* __restrict__ cand,
                  uint32_t* __restrict__ cand_cnt, uint32_t cap, Cand* __restrict__ sub, uint32_t* __restrict__ sub_cnt,
                  uint32_t k, const HistParam* __restrict__ hparam, uint32_t* hist, float* __restrict__ probe,
-                 uint32_t probe_stride, uint32_t sleep_min_ns, uint32_t sleep_max_ns, uint32_t pair) {
+                 uint32_t probe_stride, uint32_t sleep_min_ns, uint32_t sleep_max_ns, uint32_t pair, FiltArg filt) {
   extern __shared__ uint8_t smem_raw[];
   // SWIZZLE_128B operand tiles need 1024-byte alignment
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -451,13 +455,27 @@ screen_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constan
         const uint32_t q = mb * BLOCK_M + row;
         if (MODE == 3) {
           // maximum of every 32-column chunk: 8 values per lane, the quad of lanes sharing the row covers the chunk
+          // FILT: chunk h's 32 rows are word h of the tile's 8 words of the query's bitmap (row0 is a multiple of 256);
+          // lane j of the quad holds words j and j + 4, and the quad exchanges them per chunk
+          uint32_t fw_lo = 0u, fw_hi = 0u;
+          if constexpr (FILT) {
+            const uint32_t w = (row0 >> 5) + (lane & 3u);
+            if (q < nq) {
+              const uint32_t* fb = filt.bits + (size_t)__ldg(filt.qf + q) * filt.words;
+              if (w < filt.words) fw_lo = __ldg(fb + w);
+              if (w + 4 < filt.words) fw_hi = __ldg(fb + w + 4);
+            }
+          }
 #pragma unroll
           for (int h = 0; h < 8; h++) {
             float m = __int_as_float(0xff800000);  // -inf: no valid row in the chunk
+            uint32_t fw = 0xffffffffu;
+            if constexpr (FILT) fw = __shfl_sync(0xffffffffu, h < 4 ? fw_lo : fw_hi, (lane & ~3u) | (uint32_t)(h & 3));
 #pragma unroll
             for (int jj = 4 * h; jj < 4 * h + 4; jj++) {
 #pragma unroll
               for (int c = 0; c < 2; c++) {
+                if (FILT && !((fw >> (8 * (jj - 4 * h) + col_l + c)) & 1u)) continue;
                 if constexpr (INT8) {
                   // invalid rows (NaN screening norm) score 0 in the integer screen: they must not pose as a score
                   const float snv = sn[8 * jj + col_l + c];
@@ -505,6 +523,26 @@ screen_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constan
 #pragma unroll
                 for (int t = 0; t < 64; t++)
                   if ((int)acc_at(acc, i, t) >= tau_i) hits |= 1ull << t;
+                if constexpr (FILT) {
+                  // rejected rows never reach the ring: while a selective filter keeps tau low, they would flood it.
+                  // Values 8h .. 8h+7 lie in the tile's 32-row chunk h (word h of the query's 8 bitmap words), at bits
+                  // col_l + {0, 1, 8, 9, 16, 17, 24, 25} of it.
+                  // Only for batches with selective filters (filt.mask_hits): with dense ones the drain warp's test is
+                  // cheaper.
+                  if (filt.mask_hits && hits && q < nq) {
+                    const uint32_t* fb = filt.bits + (size_t)__ldg(filt.qf + q) * filt.words + (row0 >> 5);
+                    const uint32_t nw = filt.words > (row0 >> 5) ? filt.words - (row0 >> 5) : 0u;
+                    uint64_t keep = 0;
+#pragma unroll 1
+                    for (uint32_t h = 0; h < 8; h++) {
+                      if (h >= nw || !((hits >> (8 * h)) & 0xFFull)) continue;
+                      const uint32_t g = __ldg(fb + h) >> col_l;
+                      const uint32_t m8 = (g & 3u) | ((g >> 6) & 0xCu) | ((g >> 12) & 0x30u) | ((g >> 18) & 0xC0u);
+                      keep |= (uint64_t)m8 << (8 * h);
+                    }
+                    hits &= keep;
+                  }
+                }
               }
               push_survivors(acc, i, hits, q, row0, col_l, lane, r_val, r_row, r_tag, s_ring_tail, s_ring_head);
             }
@@ -518,7 +556,7 @@ screen_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constan
 #pragma unroll
                 for (int c = 0; c < 2; c++) {
                   const float v = acc[4 * jj + 2 * i + c];
-                  if (v >= my_tau[i])  // NaN scores never pass
+                  if (v >= my_tau[i] && (!FILT || filt_pass(filt, q, row0 + 8 * jj + col_l + c)))  // NaN never passes
                     append_survivor<MODE>(v, q, row, 8 * jj + col_l + c, row0, my_hp[i], s_cnt_mb, cand, cand_cnt,
                                           cap, sub, hist);
                 }
@@ -574,7 +612,7 @@ screen_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constan
           const uint32_t col = grow % BLOCK_N, row = q % BLOCK_M;
           // invalid rows (skipped / special / padding) are all-zero in the int8 copy and score exactly 0: only a
           // zero score needs the look-up of the row's screening norm
-          if (v != 0 || __ldg(snorm + grow) == __ldg(snorm + grow)) {
+          if ((v != 0 || __ldg(snorm + grow) == __ldg(snorm + grow)) && (!FILT || filt_pass(filt, q, grow))) {
             const float2 hpv = MODE == 2 ? __ldg(reinterpret_cast<const float2*>(hparam + q)) : make_float2(0.f, 0.f);
             append_survivor<MODE>(__int2float_rn(v), q, row, col, grow - col, hpv, s_cnt + q / BLOCK_M * 256, cand,
                                   cand_cnt, cap, sub, hist);
@@ -698,12 +736,14 @@ static sdb_status make_map(Ctx* ctx, CUtensorMap* map, const void* base, uint64_
 bool screen_tc_available() { return true; }
 
 sdb_status screen_tc_init_device(Ctx* ctx) {
-#define SET_SMEM(COS, I8, MODE) \
-  SDB_CUDA(cudaFuncSetAttribute(tc::screen_tc_kernel<COS, I8, MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tc::SMEM_BYTES))
+#define SET_SMEM1(COS, I8, MODE, F) \
+  SDB_CUDA(cudaFuncSetAttribute(tc::screen_tc_kernel<COS, I8, MODE, F>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tc::SMEM_BYTES))
+#define SET_SMEM(COS, I8, MODE) SET_SMEM1(COS, I8, MODE, false); SET_SMEM1(COS, I8, MODE, true)
   SET_SMEM(true, false, 0); SET_SMEM(true, false, 1); SET_SMEM(true, false, 2); SET_SMEM(true, false, 3);
   SET_SMEM(false, false, 0); SET_SMEM(false, false, 1); SET_SMEM(false, false, 2); SET_SMEM(false, false, 3);
   SET_SMEM(true, true, 0); SET_SMEM(true, true, 1); SET_SMEM(true, true, 2); SET_SMEM(true, true, 3);
 #undef SET_SMEM
+#undef SET_SMEM1
   // how many 2-CTA clusters of the int8 streaming screen are resident at once (pairs must share a GPC, so this can be
   // fewer than half the SMs): the pair launch is persistent only if its grid is all resident
   cudaLaunchConfig_t cfg = {};
@@ -718,7 +758,7 @@ sdb_status screen_tc_init_device(Ctx* ctx) {
   cfg.attrs = attr;
   cfg.numAttrs = 1;
   int clusters = 0;
-  SDB_CUDA(cudaOccupancyMaxActiveClusters(&clusters, tc::screen_tc_kernel<true, true, 2>, &cfg));
+  SDB_CUDA(cudaOccupancyMaxActiveClusters(&clusters, tc::screen_tc_kernel<true, true, 2, false>, &cfg));
   ctx->tc_pair_ctas = 2 * clusters;
   return SDB_OK;
 }
@@ -801,12 +841,17 @@ sdb_status screen_tc_pass(Corpus* c, uint32_t nq, uint32_t k, const PassDesc& p,
     float* probe_ptr = c->d_probe + (size_t)q0 * PROBE_STRIDE;
     const uint32_t probe_stride = PROBE_STRIDE, cap_arg = c->sc_cap;
     const float* snorm_arg = c->d_snorm;
-#define LAUNCH_TC1(COS, I8, MODE)                                                                                    \
-  do {                                                                                                               \
-    cfg.blockDim = dim3(tc::threads<I8, MODE>());                                                                    \
-    SDB_CUDA(cudaLaunchKernelEx(&cfg, tc::screen_tc_kernel<COS, I8, MODE>, map_a, map_b, snorm_arg, k_blocks,        \
-                                n_mblocks, nqc, p, tau, cand, ccnt, cap_arg, sub, scnt, k, hp, hist, probe_ptr,      \
-                                probe_stride, sleep_min, sleep_max, pair));                                          \
+    FiltArg filt = c->filt;
+    if (filt.bits) filt.qf += q0;
+#define LAUNCH_TC2(COS, I8, MODE, F)                                                                                 \
+  SDB_CUDA(cudaLaunchKernelEx(&cfg, tc::screen_tc_kernel<COS, I8, MODE, F>, map_a, map_b, snorm_arg, k_blocks,       \
+                              n_mblocks, nqc, p, tau, cand, ccnt, cap_arg, sub, scnt, k, hp, hist, probe_ptr,        \
+                              probe_stride, sleep_min, sleep_max, pair, filt))
+#define LAUNCH_TC1(COS, I8, MODE)                      \
+  do {                                                 \
+    cfg.blockDim = dim3(tc::threads<I8, MODE>());      \
+    if (filt.bits) LAUNCH_TC2(COS, I8, MODE, true);    \
+    else LAUNCH_TC2(COS, I8, MODE, false);             \
   } while (0)
 #define LAUNCH_TC(COS, I8)                   \
   do {                                       \
@@ -820,11 +865,13 @@ sdb_status screen_tc_pass(Corpus* c, uint32_t nq, uint32_t k, const PassDesc& p,
     else LAUNCH_TC(false, false);
 #undef LAUNCH_TC
 #undef LAUNCH_TC1
+#undef LAUNCH_TC2
     count_launch(ctx);
   }
   if (mode == 0) {
     SDB_TRY(cand_set_count(c, nq, p.count * TILE_ROWS, st));  // pass 0 wrote fixed slots of the main lists
     c->last_slots = 0;                                         // ... and no private sub-lists
+    if (c->filt.bits) SDB_TRY(cand_filter_list(c, nq, st));   // ... of every row, the filtered-out ones included
   }
   SDB_CUDA(cudaGetLastError());
   return SDB_OK;

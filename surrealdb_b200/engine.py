@@ -10,6 +10,40 @@ def _ptr(a):
     return C.c_void_p(a.ctypes.data)
 
 
+def pack_row_filter(mask):
+    """bool mask over the corpus rows (or a 2-D stack of masks) -> uint32 words of the filtered KNN bitmaps:
+    bit r = bit r % 32 of word r // 32, ceil(rows / 32) words per mask."""
+    m = np.asarray(mask, dtype=bool)
+    flat = m.reshape(-1, m.shape[-1]) if m.ndim else m.reshape(1, 1)
+    n = flat.shape[1]
+    words = (n + 31) // 32
+    padded = np.zeros((flat.shape[0], words * 32), bool)
+    padded[:, :n] = flat
+    packed = np.packbits(padded, axis=1, bitorder="little").view("<u4").astype(np.uint32)
+    return packed.reshape(m.shape[:-1] + (words,)) if m.ndim else packed[0]
+
+
+def _filter_args(filters, query_filter, nq, n_rows):
+    """(uint32 bitmaps (n_filters, W), uint32 indices (nq,) or None) -- contiguous, ready for the C calls.  The
+    library reads W = ceil(n_rows / 32) words per bitmap, so a bitmap of any other width is refused."""
+    f = np.ascontiguousarray(filters, np.uint32)
+    if f.ndim == 1:
+        f = f[None, :]
+    if f.ndim != 2 or f.shape[1] != (n_rows + 31) // 32:
+        raise L.SdbError(L.SDB_EINVAL, f"filters must be (n_filters, {(n_rows + 31) // 32}) uint32 words for "
+                                       f"{n_rows} rows, got {f.shape}")
+    return f, _query_filter(query_filter, nq)
+
+
+def _query_filter(query_filter, nq):
+    if query_filter is None:
+        return None
+    qf = np.ascontiguousarray(query_filter, np.uint32).reshape(-1)
+    if qf.size != nq:
+        raise L.SdbError(L.SDB_EINVAL, f"query_filter has {qf.size} entries for {nq} queries")
+    return qf
+
+
 class Context:
     """sdb_ctx: one CUDA device."""
 
@@ -129,8 +163,10 @@ class VectorColumn:
         """False = opt-in approximate mode (no proof, no exact fallback)"""
         L.check(L.lib().sdb_corpus_set_exact(self.h, int(bool(exact))))
 
-    def knn(self, queries, k, cancel_flag=None):
-        """queries (nq, dim) float64 -> (rows u64 (nq,k), dist f64 (nq,k), count u32 (nq,))"""
+    def knn(self, queries, k, cancel_flag=None, filters=None, query_filter=None):
+        """queries (nq, dim) float64 -> (rows u64 (nq,k), dist f64 (nq,k), count u32 (nq,)).
+        filters: optional uint32 bitmaps (n_filters, ceil(rows/32)) from pack_row_filter; query q then ranks only
+        the rows of filters[query_filter[q]] (query_filter None: every query uses filters[0])."""
         q = np.ascontiguousarray(queries, np.float64)
         if q.ndim == 1:
             q = q[None, :]
@@ -143,8 +179,25 @@ class VectorColumn:
         dist = np.zeros((nq, max(k, 1)), np.float64)
         cnt = np.zeros(nq, np.uint32)
         cf = None if cancel_flag is None else C.c_void_p(cancel_flag.ctypes.data)
-        L.check(L.lib().sdb_knn_bruteforce(self.h, _ptr(q), nq, int(k), _ptr(rows), _ptr(dist), _ptr(cnt), cf))
+        if filters is None:
+            L.check(L.lib().sdb_knn_bruteforce(self.h, _ptr(q), nq, int(k), _ptr(rows), _ptr(dist), _ptr(cnt), cf))
+        else:
+            f, qf = _filter_args(filters, query_filter, nq, len(self))
+            L.check(L.lib().sdb_knn_bruteforce_filtered(self.h, _ptr(q), nq, int(k), _ptr(f), f.shape[0],
+                                                        None if qf is None else _ptr(qf), _ptr(rows), _ptr(dist),
+                                                        _ptr(cnt), cf))
         return rows[:, :k], dist[:, :k], cnt
+
+    def knn_device_filtered(self, d_queries, nq, k, d_filters, n_filters, query_filter, row_base, d_out_rows,
+                            d_out_dist, d_out_count):
+        """device pointers (ints) for queries, bitmaps and outputs; query_filter is a host array (or None).  d_filters
+        must hold n_filters x ceil(len(self) / 32) uint32 words (the library reads exactly that many)."""
+        qf = _query_filter(query_filter, nq)
+        L.check(L.lib().sdb_knn_bruteforce_filtered_device(self.h, C.c_void_p(d_queries), int(nq), int(k),
+                                                           C.c_void_p(d_filters), int(n_filters),
+                                                           None if qf is None else _ptr(qf), int(row_base),
+                                                           C.c_void_p(d_out_rows), C.c_void_p(d_out_dist),
+                                                           C.c_void_p(d_out_count)))
 
     def knn_device(self, d_queries, nq, k, row_base, d_out_rows, d_out_dist, d_out_count):
         """all arguments are raw device pointers (ints); results complete on return."""
@@ -165,6 +218,18 @@ class VectorColumn:
         t = C.c_uint32()
         L.check(L.lib().sdb_knn_submit(self.h, C.c_void_p(h_queries), int(nq), int(k), C.c_void_p(h_out_rows),
                                        C.c_void_p(h_out_dist), C.c_void_p(h_out_count), C.byref(t)))
+        return t.value
+
+    def submit_host_filtered(self, h_queries, nq, k, h_filters, n_filters, query_filter, h_out_rows, h_out_dist,
+                             h_out_count):
+        """raw host pointers (ints) like submit_host, plus the host bitmaps (valid until wait); query_filter is a host
+        array (or None), copied before the call returns.  h_filters must hold n_filters x ceil(len(self) / 32) words."""
+        qf = _query_filter(query_filter, nq)
+        t = C.c_uint32()
+        L.check(L.lib().sdb_knn_submit_filtered(self.h, C.c_void_p(h_queries), int(nq), int(k), C.c_void_p(h_filters),
+                                                int(n_filters), None if qf is None else _ptr(qf),
+                                                C.c_void_p(h_out_rows), C.c_void_p(h_out_dist),
+                                                C.c_void_p(h_out_count), C.byref(t)))
         return t.value
 
     def wait(self, ticket):

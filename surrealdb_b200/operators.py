@@ -12,10 +12,16 @@ meaning and error behaviour, on top of the same C ABI:
 
 Records are dicts with an "id"; `input` is any iterable yielding them in scan (record-key) order, i.e.
 what TableScan yields.
+
+  TableScan(table, records, version) / Union(*inputs) / Filter(input, predicate)
+      the sources of `WHERE emb <|k|> $q AND cond`, planned as KnnTopK(Filter(TableScan))
+      (exec/planner/select.rs:1642-1652).  KnnTopK over a Filter ranks the source's column with the predicate's
+      row bitmap (sdb_knn_bruteforce_filtered) and keeps that column cached per (tables, table versions), so
+      statements with different predicates share one staged column (INTEGRATION.md section 8).
 """
 import numpy as np
 
-from .engine import Context, VectorColumn
+from .engine import Context, VectorColumn, pack_row_filter
 
 
 class Distance:
@@ -61,9 +67,70 @@ def extract_vector(value, field):
     return out
 
 
+class TableScan:
+    """The records of one table in scan (record-key) order.  `version` changes whenever the table does: a staged
+    column is reused only for the version it was staged from."""
+
+    def __init__(self, table, records, version=0):
+        self.table, self.records, self.version = table, records, version
+
+    def name(self):
+        return "TableScan"
+
+    def source_key(self):
+        return ("TableScan", self.table), self.version
+
+    def __iter__(self):
+        return iter(self.records)
+
+
+class Union:
+    """Several sources one after the other (`FROM a, b`)."""
+
+    def __init__(self, *inputs):
+        self.inputs = inputs
+
+    def name(self):
+        return "Union"
+
+    def source_key(self):
+        keys = [_source_key(i) for i in self.inputs]
+        if any(k is None for k in keys):
+            return None
+        return ("Union",) + tuple(k[0] for k in keys), tuple(k[1] for k in keys)
+
+    def __iter__(self):
+        for i in self.inputs:
+            yield from i
+
+
+class Filter:
+    """exec Filter operator: the records of `input` for which `predicate(record)` is truthy, in input order."""
+
+    def __init__(self, input, predicate):
+        self.input, self.predicate = input, predicate
+
+    def name(self):
+        return "Filter"
+
+    def __iter__(self):
+        return (rec for rec in self.input if self.predicate(rec))
+
+
+def _source_key(src):
+    """(identity, version) of a cacheable source, None for a plain iterable"""
+    fn = getattr(src, "source_key", None)
+    return fn() if fn is not None else None
+
+
 class KnnTopK:
     """Brute-force KNN operator backed by the GPU column.  Pipeline-breaking: consumes the whole input,
     returns the k nearest records ordered by (distance, scan position)."""
+
+    # staged columns of cacheable sources: (source identity, field, dimension, distance) -> (version, column, records).
+    # One entry per source and field: a new table version replaces the entry.  Nothing else evicts (the Rust shim owns
+    # the column cache and its memory budget, INTEGRATION.md section 8); clear_column_cache() releases everything.
+    _column_cache = {}
 
     def __init__(self, input, field, query_vector, k, distance, ctx=None):
         self.input = input
@@ -87,11 +154,11 @@ class KnnTopK:
         return [("field", self.field), ("k", str(self.k)), ("distance", self.distance),
                 ("dimension", str(len(self.query_vector)))]
 
-    def _stage(self):
+    def _stage(self, source=None):
         """TableScan -> pinned rows -> HBM column (the staging a Rust shim caches per table version)."""
         dim = len(self.query_vector)
         recs, rows, skip = [], [], []
-        for rec in self.input:
+        for rec in (self.input if source is None else source):
             vec = extract_vector(rec, self.field)
             recs.append(rec)
             if vec is None or len(vec) != dim:  # extract_vector None, or compute() Err on dimension mismatch
@@ -115,12 +182,41 @@ class KnnTopK:
         col.finalize()
         return col
 
+    def _source_column(self, source):
+        """the staged column of `source` (cached per source identity and version when the source has one)"""
+        key = _source_key(source)
+        if key is None:
+            return self._stage(source)
+        ident, version = key
+        ck = (ident, self.field, len(self.query_vector), self.distance)
+        hit = KnnTopK._column_cache.get(ck)
+        if hit is not None and hit[0] == version and (self._ctx is None or hit[1].ctx is self._ctx):
+            self._records = hit[2]
+            return hit[1]
+        col = self._stage(source)
+        KnnTopK._column_cache[ck] = (version, col, self._records)
+        return col
+
+    @classmethod
+    def clear_column_cache(cls):
+        cls._column_cache.clear()
+
     def execute(self):
+        filt = None
         if self._column is None:
-            self._column = self._stage()
+            if isinstance(self.input, Filter):
+                # KnnTopK(Filter(source)): rank the source's column with the predicate's row bitmap
+                self._column = self._source_column(self.input.input)
+            else:
+                self._column = self._stage()
         if self._column is None or self.k == 0:
             return []
-        rows, dist, cnt = self._column.knn(np.asarray([self.query_vector], np.float64), self.k)
+        q = np.asarray([self.query_vector], np.float64)
+        if isinstance(self.input, Filter):
+            filt = pack_row_filter([bool(self.input.predicate(rec)) for rec in self._records])
+            rows, dist, cnt = self._column.knn(q, self.k, filters=filt)
+        else:
+            rows, dist, cnt = self._column.knn(q, self.k)
         out = []
         for j in range(int(cnt[0])):
             rec = self._records[int(rows[0, j])]
