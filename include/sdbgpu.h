@@ -360,6 +360,33 @@ void sdb_hnsw_destroy(sdb_hnsw*);
 sdb_status sdb_hnsw_search_filtered(sdb_hnsw*, const void* queries, uint32_t nq, uint32_t k, uint32_t ef,
                                     const uint8_t* truthy, uint64_t* out_elems, double* out_dist, uint32_t* out_count,
                                     uint64_t* out_counters);
+/* Filtered search of any selectivity, one bitmap per query: `WHERE cond AND emb <|k,ef|> $q` for a batch of statements
+ * with different conditions.  Query q is exactly Hnsw::knn_search_with_filter with truthy[e] = bit e of its bitmap --
+ * same ids, f64 distances and both counters as the reference, for any selectivity, none and all included.  The descent
+ * through the upper layers is unfiltered.
+ * filters: n_filters bitmaps of W = ceil(n_elems / 32) uint32 words each; bit e = bit e % 32 of word e / 32 (the
+ * sdb_hop_filter convention); bits past n_elems in the last word are ignored.
+ * query_filter: ALWAYS host memory, nq indices < n_filters (checked, and copied before the call returns); NULL = every
+ * query uses filter 0.
+ * These calls never return SDB_EOVERFLOW.  A query that outgrows the on-chip candidate window or the visited table is
+ * walked again by the spill tier: its candidate queue in device memory (a heap of 16 bytes per element) with an exact
+ * visited set (4 bytes per element), in a pool of such slots sized to the free device memory; queries wait for a slot
+ * and none fails for capacity.  SDB_ENOMEM only when not even one slot fits.  The other queries of the batch are not
+ * affected.  SDB_EINVAL: n_filters == 0 with nq > 0, filters == NULL with nq > 0, or an index >= n_filters.  Every
+ * metric and vector type, ef <= 4096, the Minkowski order, SDB_ECANCELLED and the handle's lock as in sdb_hnsw_search.
+ * Pending documents: clear their elements' bits (add_if_truthy ignores such elements, as for the byte mask above).
+ * Host variant: queries, filters and the outputs are host memory.  Device variant: d_queries, d_filters and the
+ * outputs are device memory (d_out_counters nullable). */
+sdb_status sdb_hnsw_search_filtered_batch(sdb_hnsw*, const void* queries, uint32_t nq, uint32_t k, uint32_t ef,
+                                          const uint32_t* filters, uint32_t n_filters, const uint32_t* query_filter,
+                                          uint64_t* out_elems, double* out_dist, uint32_t* out_count,
+                                          uint64_t* out_counters);
+sdb_status sdb_hnsw_search_filtered_batch_device(sdb_hnsw*, const void* d_queries, uint32_t nq, uint32_t k, uint32_t ef,
+                                                 const uint32_t* d_filters, uint32_t n_filters,
+                                                 const uint32_t* query_filter, uint64_t* d_out_elems,
+                                                 double* d_out_dist, uint32_t* d_out_count, uint64_t* d_out_counters);
+/* how many queries of the handle's last sdb_hnsw_search_filtered_batch[_device] call the spill tier finished */
+uint32_t sdb_hnsw_last_spilled(const sdb_hnsw*);
 
 /* Search while pending updates exist: Hnsw::knn_search(.., pending_docs = Some(bitmap)) (hnsw/mod.rs:459-482).
  * all_docs_pending[e] != 0 iff EVERY document of element e is in the pending bitmap that

@@ -37,6 +37,7 @@ ABI_SYMBOLS = [
     "sdb_graph_load_csr", "sdb_graph_load_csr_shard", "sdb_graph_destroy", "sdb_graph_expand", "sdb_graph_expand_device", "sdb_device_free", "sdb_graph_collect", "sdb_free",
     "sdb_graph_expand_filtered", "sdb_graph_expand_filtered_device", "sdb_graph_collect_filtered",
     "sdb_knn_bruteforce_filtered", "sdb_knn_bruteforce_filtered_device", "sdb_knn_submit_filtered",
+    "sdb_hnsw_search_filtered_batch", "sdb_hnsw_search_filtered_batch_device", "sdb_hnsw_last_spilled",
 ]
 
 
@@ -140,6 +141,10 @@ def lib():
     L.sdb_hnsw_search.argtypes = [vp, vp, u32, u32, u32, vp, vp, vp, vp]
     L.sdb_hnsw_search_filtered.argtypes = [vp, vp, u32, u32, u32, vp, vp, vp, vp, vp]
     L.sdb_hnsw_search_pending.argtypes = [vp, vp, u32, u32, u32, vp, vp, vp, vp, vp]
+    L.sdb_hnsw_search_filtered_batch.argtypes = [vp, vp, u32, u32, u32, vp, u32, vp, vp, vp, vp, vp]
+    L.sdb_hnsw_search_filtered_batch_device.argtypes = [vp, vp, u32, u32, u32, vp, u32, vp, vp, vp, vp, vp]
+    L.sdb_hnsw_last_spilled.argtypes = [vp]
+    L.sdb_hnsw_last_spilled.restype = u32
     L.sdb_vec_distance_f32.argtypes = [vp, i32, u32, vp, vp, u64, vp]
     L.sdb_hnsw_distance.argtypes = [vp, vp, vp, u64, vp]
     L.sdb_hnsw_set_minkowski_order.argtypes = [vp, C.c_double]

@@ -60,6 +60,7 @@ struct Hnsw {
   DevBuf<uint64_t> d_visited;
   uint32_t table_log2 = 0, n_tables = 0;
   uint32_t gen = 1;  // generations consumed so far (each warp uses gen_base + its own counter)
+  uint32_t last_spilled = 0;  // queries of the last batch-filtered call that the spill tier finished
   bool borrowed = false;  // sdb_hnsw_load_device: vectors and CSR arrays belong to the caller
   std::mutex mu;
 };
@@ -814,7 +815,20 @@ struct HnswParams {
   const void* q_bits;
   const uint32_t* q_nbits;
   const double* q_norm;       // COSINE of the types other than F32: per query norm (the elements' are `norm`)
+  // the batch-filtered walk (hnsw_search_kernel<.., BITS = true>, hnsw_spill_kernel): per-query element bitmaps
+  const uint32_t* filters;       // bitmaps of fwords words: element e passes iff bit e % 32 of word e / 32 is set
+  const uint32_t* query_filter;  // nq bitmap indices (null: every query uses bitmap 0)
+  uint32_t fwords;
+  uint32_t* spill_list;  // the queries the on-chip walk gave up on (candidate window or visited table full) ...
+  uint32_t* n_spill;     // ... and how many there are
 };
+
+// bit e of a filter bitmap
+__device__ __forceinline__ bool filter_bit(const uint32_t* bits, uint32_t e) { return (__ldg(bits + (e >> 5)) >> (e & 31u)) & 1u; }
+// the bitmap query q tests
+__device__ __forceinline__ const uint32_t* query_bits(const HnswParams& P, uint32_t q) {
+  return P.filters + (size_t)(P.query_filter ? P.query_filter[q] : 0u) * P.fwords;
+}
 
 // Stages vector r of a set (the queries of a walk, or an element) in shared memory as the distance functions above read
 // it: F32 COSINE transposed (hn_q_stride) with its 8-lane norm computed here (the same arithmetic as the elements'
@@ -880,7 +894,10 @@ __device__ __forceinline__ double walk_distance(const HnswParams& P, uint32_t my
 }
 
 // T: the element type of the index (float = F32; double, long long, int, short = F64, I64, I32, I16)
-template <int MET, int MINB, typename T>
+// BITS: the batch-filtered walk.  Layer 0 tests bit e of the query's own bitmap (query_bits) where the single-mask walk
+// reads truthy[e], and a query that fills its candidate window or its visited table stops at once and is appended to
+// the spill list (hnsw_spill_kernel walks it again and writes its outputs) instead of raising the batch's overflow word.
+template <int MET, int MINB, typename T, bool BITS = false>
 __global__ void __launch_bounds__(HN_WARPS * 32, MINB) hnsw_search_kernel(HnswParams P) {
   constexpr bool COSINE = MET == SDB_COSINE && is_f32_v<T>;  // the 8-lane transposed path of F32 cosine
   constexpr size_t ELEM = MET == SDB_JACCARD ? sizeof(JKey<T>) : sizeof(T);  // bytes of a staged query element
@@ -949,6 +966,8 @@ __global__ void __launch_bounds__(HN_WARPS * 32, MINB) hnsw_search_kernel(HnswPa
     }
     uint64_t n_visited = 0, n_expanded = 0;
     uint32_t n_out = 0;
+    const uint32_t* qbits = BITS ? query_bits(P, q) : nullptr;
+    bool spill = false;  // BITS: this query goes to the spill tier (warp-uniform once set)
     if (P.entry >= 0) {
       uint32_t ep = (uint32_t)P.entry;
       double ep_d = walk_distance<MET, T>(P, lane == 0 ? ep : NO_ROW, s_q, q_norm, mq, tile);
@@ -974,7 +993,7 @@ __global__ void __launch_bounds__(HN_WARPS * 32, MINB) hnsw_search_kernel(HnswPa
         const uint8_t* truthy = layer == 0 ? P.truthy : nullptr;
         cn = sorted_insert(c_key, c_id, head, cn, walk_key(ep_d), ep);
         double fd = 1.7976931348623157e308;  // w.peek_last_dist().unwrap_or(f64::MAX)
-        if (!truthy || truthy[ep]) {
+        if (BITS ? layer != 0 || filter_bit(qbits, ep) : !truthy || truthy[ep]) {
           wn = sorted_insert(w_key, w_id, 0, wn, walk_key(ep_d), ep);
           fd = ep_d;
         }
@@ -1005,13 +1024,18 @@ __global__ void __launch_bounds__(HN_WARPS * 32, MINB) hnsw_search_kernel(HnswPa
                   if ((uint32_t)(old >> 32) != gen) continue;
                 }
                 if (probes > mask) {  // table full: report, treat as visited
-                  *P.overflow = 1;
+                  if (BITS) spill = true;
+                  else *P.overflow = 1;
                   break;
                 }
                 slot = (slot + 1) & mask;
               }
             }
             const uint32_t new_mask = __ballot_sync(0xffffffffu, is_new);
+            if (BITS && __any_sync(0xffffffffu, spill)) {
+              spill = true;
+              break;
+            }
             if (!new_mask) continue;
             n_visited += __popc(new_mask);
             const double d = walk_distance<MET, T>(P, is_new ? nb : NO_ROW, s_q, q_norm, mq, tile);
@@ -1039,12 +1063,16 @@ __global__ void __launch_bounds__(HN_WARPS * 32, MINB) hnsw_search_kernel(HnswPa
                     head = 0;
                   }
                   if (cn >= ccap) {
+                    if (BITS) {
+                      spill = true;
+                      break;
+                    }
                     cn = ccap - 1;
                     *P.overflow = 2;
                   }
                 }
                 if (!P.noexp || !P.noexp[idi]) cn = sorted_insert(c_key, c_id, head, cn, key, idi);
-                if (!truthy || truthy[idi]) {  // add_if_truthy  layer.rs:277-306
+                if (BITS ? layer != 0 || filter_bit(qbits, idi) : !truthy || truthy[idi]) {  // add_if_truthy  layer.rs:277-306
                   wn = sorted_insert(w_key, w_id, 0, wn, key, idi);
                   if (wn > ef) wn--;  // pop_last
                   fd = key_to_double(w_key[wn - 1]);
@@ -1056,8 +1084,11 @@ __global__ void __launch_bounds__(HN_WARPS * 32, MINB) hnsw_search_kernel(HnswPa
                 }
               }
             }
+            if (BITS && spill) break;
           }
+          if (BITS && spill) break;
         }
+        if (BITS && spill) break;
         // next layer starts from w.peek_first()                                mod.rs:530-538
         if (wn) {
           ep = w_id[0];
@@ -1072,6 +1103,10 @@ __global__ void __launch_bounds__(HN_WARPS * 32, MINB) hnsw_search_kernel(HnswPa
         }
         __syncwarp();
       }
+    }
+    if (BITS && spill) {  // outputs and counters come from the spill tier
+      if (lane == 0) P.spill_list[atomicAdd(P.n_spill, 1u)] = q;
+      continue;
     }
     if (lane == 0) {
       P.out_count[q] = n_out;
@@ -1098,6 +1133,191 @@ __device__ __forceinline__ void hn_warp_layout(uint8_t* base, uint32_t dim, floa
   tile = reinterpret_cast<float(*)[33]>(is_f32_v<T> ? s_q + ((hn_q_floats(dim, COSINE) + 3) & ~size_t(3))
                                                     : reinterpret_cast<float*>(base + hn_q_bytes(dim, false, false, ELEM)));
   rest = reinterpret_cast<uint8_t*>(tile) + hn_tile_bytes(COSINE);
+}
+
+// ---- spill tier of the batch-filtered walk: the queries hnsw_search_kernel<.., BITS> gave up on, walked again from the
+// top layer with no capacity limit.  One warp per slot; a slot is
+//   heap:  a binary min-heap of (walk_key, tag = insertion sequence << 32 | element) in global memory, n entries: an
+//          element enters a layer's candidates at most once (it is visited once), so n is a hard bound.  Popping by
+//          (key, sequence) is sorted_insert's order -- nearest first, FIFO among equal keys -- without the window.
+//   stamp: one u32 per element, the slot's layer generation that last visited it (an exact visited set; 0 = never).
+// w (ef + 2 entries) stays in shared memory, as in the on-chip walk.  Lane 0 owns the heap; the other lanes wait.
+struct SpillSlots {
+  ulonglong2* heap;   // n_slots x n
+  uint32_t* stamp;    // n_slots x n
+  uint64_t n;
+  uint32_t n_slots;
+  uint32_t* next;     // the next spill-list entry to take
+};
+
+__device__ __forceinline__ bool heap_less(ulonglong2 a, ulonglong2 b) { return a.x < b.x || (a.x == b.x && a.y < b.y); }
+// adds v to the heap of hn entries (the caller counts it)
+__device__ __forceinline__ void heap_push(ulonglong2* hp, uint32_t hn, ulonglong2 v) {
+  uint32_t i = hn;
+  while (i) {
+    const uint32_t p = (i - 1) >> 1;
+    const ulonglong2 pv = hp[p];
+    if (!heap_less(v, pv)) break;
+    hp[i] = pv;
+    i = p;
+  }
+  hp[i] = v;
+}
+// removes and returns the smallest entry; hn = the number of entries left (the caller has counted the removal)
+__device__ __forceinline__ ulonglong2 heap_pop(ulonglong2* hp, uint32_t hn) {
+  const ulonglong2 top = hp[0];
+  const ulonglong2 last = hp[hn];
+  uint32_t i = 0;
+  for (;;) {
+    uint32_t c = 2 * i + 1;
+    if (c >= hn) break;
+    ulonglong2 cv = hp[c];
+    if (c + 1 < hn) {
+      const ulonglong2 rv = hp[c + 1];
+      if (heap_less(rv, cv)) cv = rv, c++;
+    }
+    if (!heap_less(cv, last)) break;
+    hp[i] = cv;
+    i = c;
+  }
+  if (hn) hp[i] = last;
+  return top;
+}
+
+// The same walk as hnsw_search_kernel<MET, .., T, true> (layer 0 filtered by the query's bitmap, the descent above
+// unfiltered), for the queries of P.spill_list: each warp takes the next one until the list is done.  The cancel word is
+// polled per query and every 32 expansions, since one walk may cover the whole reachable layer 0.
+template <int MET, typename T>
+__global__ void __launch_bounds__(HN_WARPS * 32, 1) hnsw_spill_kernel(HnswParams P, SpillSlots S, uint32_t per_warp) {
+  extern __shared__ uint8_t smem_raw[];
+  const uint32_t warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const uint32_t slot = blockIdx.x * HN_WARPS + warp;
+  if (slot >= S.n_slots) return;
+  float* s_q;
+  float(*tile)[33];
+  uint8_t* rest;
+  hn_warp_layout<MET, T>(smem_raw + (size_t)warp * per_warp, P.dim, s_q, tile, rest);
+  const uint32_t wcap = P.ef + 2;
+  uint64_t* w_key = reinterpret_cast<uint64_t*>(rest);
+  uint32_t* w_id = reinterpret_cast<uint32_t*>(w_key + wcap);
+  ulonglong2* hp = S.heap + slot * S.n;
+  uint32_t* stamp = S.stamp + slot * S.n;
+  const volatile int* cancel = reinterpret_cast<const volatile int*>(P.cancel);
+  const uint32_t n_spill = *P.n_spill;
+  uint32_t gen = 0;
+  // lane 0 reads the cancel word for the warp, so that every lane takes the same branch
+  auto cancelled = [&]() { return __shfl_sync(0xffffffffu, lane == 0 ? *cancel : 0, 0) != 0; };
+  for (;;) {
+    uint32_t i = 0;
+    if (lane == 0) i = atomicAdd(S.next, 1u);
+    i = __shfl_sync(0xffffffffu, i, 0);
+    if (i >= n_spill || cancelled()) break;
+    const uint32_t q = P.spill_list[i];
+    double q_norm = 0.0;
+    MetricQ mq;
+    stage_vector<MET, T>(P.dim, P.queries, P.q_norm, P.q_mean, P.q_sx2, P.q_bits, P.q_nbits, P.mink_p, q, s_q, q_norm, mq);
+    const uint32_t* qbits = query_bits(P, q);
+    uint64_t n_visited = 0, n_expanded = 0;
+    uint32_t n_out = 0;
+    bool stop = false;
+    if (P.entry >= 0) {
+      uint32_t ep = (uint32_t)P.entry;
+      double ep_d = walk_distance<MET, T>(P, lane == 0 ? ep : NO_ROW, s_q, q_norm, mq, tile);
+      ep_d = __shfl_sync(0xffffffffu, ep_d, 0);
+      n_visited++;
+      for (int32_t layer = (int32_t)P.n_layers - 1; layer >= 0; layer--) {
+        const uint32_t ef = layer == 0 ? P.ef : 1u;
+        const uint64_t* rp = P.rp[layer];
+        const uint32_t* ci = P.ci[layer];
+        if (++gen == 0) {  // the generations wrapped: forget every stamp
+          for (uint64_t e = lane; e < S.n; e += 32) stamp[e] = 0;
+          gen = 1;
+        }
+        __syncwarp();
+        // search_single(_with_filter): visited = {ep}; candidates = {(ep_d, ep)}; w = {(ep_d, ep)} if ep passes
+        uint32_t wn = 0;
+        if (lane == 0) {
+          stamp[ep] = gen;
+          heap_push(hp, 0, make_ulonglong2(walk_key(ep_d), ep));
+        }
+        uint32_t hn = 1, seq = 1;  // heap entries, insertions so far
+        __syncwarp();
+        double fd = 1.7976931348623157e308;
+        if (layer != 0 || filter_bit(qbits, ep)) {
+          wn = sorted_insert(w_key, w_id, 0, wn, walk_key(ep_d), ep);
+          fd = ep_d;
+        }
+        while (hn) {
+          hn--;
+          ulonglong2 top = make_ulonglong2(0, 0);
+          if (lane == 0) top = heap_pop(hp, hn);
+          const uint64_t ckey = __shfl_sync(0xffffffffu, top.x, 0);
+          const uint32_t cid = (uint32_t)__shfl_sync(0xffffffffu, top.y, 0);
+          if (key_to_double(ckey) > fd) break;  // cq_dist > fq_dist
+          n_expanded++;
+          if ((n_expanded & 31) == 0 && cancelled()) {
+            stop = true;
+            break;
+          }
+          const uint64_t beg = rp[cid], end = rp[cid + 1];
+          for (uint64_t b0 = beg; b0 < end; b0 += 32) {
+            const uint32_t nb = b0 + lane < end ? __ldg(ci + b0 + lane) : NO_ROW;
+            // visited.insert in stored order: of repeats inside the chunk only the first can be new
+            const uint32_t dup = __match_any_sync(0xffffffffu, nb);
+            bool is_new = false;
+            if (nb != NO_ROW && (dup & ((1u << lane) - 1u)) == 0 && stamp[nb] != gen) {
+              stamp[nb] = gen;
+              is_new = true;
+            }
+            __syncwarp();  // the stamps are seen by every lane of the next chunk
+            const uint32_t new_mask = __ballot_sync(0xffffffffu, is_new);
+            if (!new_mask) continue;
+            n_visited += __popc(new_mask);
+            const double d = walk_distance<MET, T>(P, is_new ? nb : NO_ROW, s_q, q_norm, mq, tile);
+            uint32_t m = new_mask;
+            while (m) {  // admission in stored order                      layer.rs:205-217,277-306
+              const int j = __ffs(m) - 1;
+              m &= m - 1;
+              const double dj = __shfl_sync(0xffffffffu, d, j);
+              const uint32_t idj = __shfl_sync(0xffffffffu, nb, j);
+              if (dj < fd || wn < ef) {
+                const uint64_t key = walk_key(dj);
+                if (lane == 0) heap_push(hp, hn, make_ulonglong2(key, ((uint64_t)seq << 32) | idj));
+                hn++, seq++;
+                if (layer != 0 || filter_bit(qbits, idj)) {
+                  wn = sorted_insert(w_key, w_id, 0, wn, key, idj);
+                  if (wn > ef) wn--;  // pop_last
+                  fd = key_to_double(w_key[wn - 1]);
+                }
+              }
+            }
+          }
+        }
+        __syncwarp();
+        if (stop) break;
+        if (wn) {
+          ep = w_id[0];
+          ep_d = key_to_double(w_key[0]);
+        }
+        if (layer == 0) {
+          n_out = wn < P.k ? wn : P.k;
+          for (uint32_t o = lane; o < n_out; o += 32) {
+            P.out_elems[(size_t)q * P.k + o] = w_id[o];
+            P.out_dist[(size_t)q * P.k + o] = key_to_double(w_key[o]);
+          }
+        }
+        __syncwarp();
+      }
+    }
+    if (stop) break;  // cancelled: the caller reports SDB_ECANCELLED
+    if (lane == 0) {
+      P.out_count[q] = n_out;
+      if (P.out_counters) {
+        P.out_counters[2 * (size_t)q] = n_visited;
+        P.out_counters[2 * (size_t)q + 1] = n_expanded;
+      }
+    }
+  }
 }
 
 // ---- exact kNN over the elements in the walk's arithmetic (TestCollection::knn, idx/trees/hnsw/mod.rs:1186-1197) ----
@@ -1978,22 +2198,99 @@ sdb_status sdb_hnsw_select_device(sdb_hnsw* h, const uint32_t* d_elem_ids, uint6
 }
 
 using WalkKernel = void (*)(HnswParams);
-static WalkKernel walk_kernel(sdb_metric metric, sdb_vector_type vt, int occ) {
-  if (vt == SDB_VT_F32 && metric == SDB_COSINE)
+static WalkKernel walk_kernel(sdb_metric metric, sdb_vector_type vt, int occ, bool bits) {
+  if (vt == SDB_VT_F32 && metric == SDB_COSINE) {
+    if (bits) return hnsw_search_kernel<SDB_COSINE, 4, float, true>;  // 123 registers: no spills (6 blocks spill)
     return occ >= 8 ? hnsw_search_kernel<SDB_COSINE, 8, float> : occ <= 4 ? hnsw_search_kernel<SDB_COSINE, 4, float> : hnsw_search_kernel<SDB_COSINE, 6, float>;
+  }
   return with_vt(vt, [&](auto tag) {
     using T = decltype(tag);
     return with_metric(metric, [&](auto met) -> WalkKernel {
       constexpr int MET = decltype(met)::value;
-      return hnsw_search_kernel<MET, MET == SDB_COSINE && is_f32_v<T> ? 6 : 1, T>;  // (F32 cosine: returned above)
+      constexpr bool COS32 = MET == SDB_COSINE && is_f32_v<T>;  // (F32 cosine: returned above)
+      return bits ? hnsw_search_kernel<MET, COS32 ? 4 : 1, T, true> : hnsw_search_kernel<MET, COS32 ? 6 : 1, T>;
+    });
+  });
+}
+
+// the bitmaps of sdb_hnsw_search_filtered_batch[_device] (see the header)
+struct BatchFilter {
+  const uint32_t* filters;
+  uint32_t n_filters;
+  const uint32_t* query_filter;  // host
+  bool on_device;                // filters is device memory
+};
+
+// The spill tier of a batch-filtered call: n_sp queries of P.spill_list walked by hnsw_spill_kernel, in as many slots
+// as free device memory holds (at most one per resident warp, at most one per query).  Queued on the context's stream.
+static sdb_status hnsw_spill(sdb_hnsw* h, const HnswParams& P, uint32_t n_sp, DevBuf<ulonglong2>& heap,
+                             DevBuf<uint32_t>& stamp, AsyncBuf<uint32_t>& next) {
+  Ctx* ctx = h->ctx;
+  cudaStream_t st = ctx->stream;
+  const size_t per_warp = (hn_stage_bytes(h->dim, h->metric, h->vt) + 12 * ((size_t)P.ef + 2) + 64 + 15) & ~size_t(15);
+  const size_t smem = per_warp * HN_WARPS;
+  if (smem > 220 * 1024) {
+    set_error("hnsw: dim %u / ef %u need %zu bytes of shared memory per block in the spill tier", h->dim, P.ef, smem);
+    return SDB_EUNSUPPORTED;
+  }
+  return with_vt(h->vt, [&](auto tag) -> sdb_status {
+    using T = decltype(tag);
+    return with_metric(h->metric, [&](auto met) -> sdb_status {
+      const auto kern = hnsw_spill_kernel<decltype(met)::value, T>;
+      SDB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+      int per_sm = 1;
+      SDB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, HN_WARPS * 32, smem));
+      const uint64_t resident = (uint64_t)ctx->sm_count * std::max(per_sm, 1) * HN_WARPS;
+      // a slot: the heap (16 bytes per element) and the visited stamps (4 bytes per element); the pool takes at most
+      // half of the free memory, from cudaMalloc, so that it goes back to the device when the call returns (the stream
+      // pool would keep it cached)
+      const uint64_t slot_bytes = 20 * std::max<uint64_t>(h->n, 1);
+      size_t free_b = 0, total_b = 0;
+      SDB_CUDA(cudaMemGetInfo(&free_b, &total_b));
+      uint64_t slots = std::min<uint64_t>({(uint64_t)n_sp, resident, free_b / 2 / slot_bytes});
+      for (;; slots /= 2) {  // memory can be taken in between: halve until it fits
+        if (slots == 0) {
+          set_error("hnsw: not even one spill slot (%llu bytes) fits in device memory",
+                    (unsigned long long)slot_bytes);
+          return SDB_ENOMEM;
+        }
+        if (heap.reserve(slots * h->n) == cudaSuccess && stamp.reserve(slots * h->n) == cudaSuccess) break;
+        heap.reset(), stamp.reset();
+      }
+      SDB_CUDA(next.reserve(1, st));
+      SDB_CUDA(cudaMemsetAsync(stamp, 0, sizeof(uint32_t) * slots * h->n, st));
+      SDB_CUDA(cudaMemsetAsync(next, 0, sizeof(uint32_t), st));
+      SpillSlots S;
+      S.heap = heap;
+      S.stamp = stamp;
+      S.n = h->n;
+      S.n_slots = (uint32_t)slots;
+      S.next = next;
+      kern<<<(unsigned)((slots + HN_WARPS - 1) / HN_WARPS), HN_WARPS * 32, smem, st>>>(P, S, (uint32_t)per_warp);
+      count_launch(ctx);
+      SDB_CUDA(cudaGetLastError());
+      return SDB_OK;
     });
   });
 }
 
 static sdb_status hnsw_search_impl(sdb_hnsw* h, const void* queries, uint32_t nq, uint32_t k, uint32_t ef,
                                    const uint8_t* truthy, const uint8_t* noexp, uint64_t* out_elems, double* out_dist,
-                                   uint32_t* out_count, uint64_t* out_counters, bool device_io = false) {
+                                   uint32_t* out_count, uint64_t* out_counters, bool device_io = false,
+                                   const BatchFilter* bf = nullptr) {
   if (!h || (nq && (!queries || !out_count)) || (nq && k && (!out_elems || !out_dist))) return SDB_EINVAL;
+  if (bf && nq) {
+    if (bf->n_filters == 0 || !bf->filters) {
+      set_error("filtered hnsw: %s", bf->n_filters == 0 ? "no filter given (n_filters == 0)" : "filters is NULL");
+      return SDB_EINVAL;
+    }
+    if (bf->query_filter)
+      for (uint32_t q = 0; q < nq; q++)
+        if (bf->query_filter[q] >= bf->n_filters) {
+          set_error("filtered hnsw: query %u uses filter %u of %u", q, bf->query_filter[q], bf->n_filters);
+          return SDB_EINVAL;
+        }
+  }
   if (nq == 0) return SDB_OK;
   if (k == 0 || ef == 0) {  // to_vec_limit(0) underflows in the reference; we return nothing
     if (device_io) {
@@ -2014,14 +2311,16 @@ static sdb_status hnsw_search_impl(sdb_hnsw* h, const void* queries, uint32_t nq
   SDB_CUDA(cudaSetDevice(ctx->device));
   cudaStream_t st = ctx->stream;
   // unfiltered: live candidates are a subset of w plus ties, 2*ef+34 is ample.  Filtered: every admitted element is a
-  // candidate but only truthy ones enter w, so the window is sized for a selectivity down to ~1/16 (more = EOVERFLOW)
+  // candidate but only truthy ones enter w, so the window is sized for a selectivity down to ~1/16 (more = EOVERFLOW,
+  // or the spill tier for the batch-filtered calls)
+  const bool filtered = truthy || bf;
   uint32_t ccap = 2 * ef + 34;
   const uint32_t wcap = ef + 2;
   // bytes of a staged query and of the distance scratch (the kernel's per-warp layout)
   const size_t q_tile = hn_q_bytes(h->dim, h->vt == SDB_VT_F32, h->metric == SDB_COSINE,
                                    h->metric == SDB_JACCARD ? jkey_size(h->vt) : vt_size(h->vt)) +
                         hn_tile_bytes(h->vt == SDB_VT_F32 && h->metric == SDB_COSINE);
-  if (truthy) {
+  if (filtered) {
     ccap = 16 * ef + 34;
     if (ccap < 1024) ccap = 1024;
     const size_t fixed = q_tile + 12 * (size_t)wcap + 64 + 16;
@@ -2037,7 +2336,7 @@ static sdb_status hnsw_search_impl(sdb_hnsw* h, const void* queries, uint32_t nq
   }
   // cosine: 8 lanes per row keep ~16 loads in flight per lane; 80 registers (6 blocks per SM) holds that without spills
   const int occ = getenv("SDB_HNSW_OCC") ? atoi(getenv("SDB_HNSW_OCC")) : 6;  // measured r2 (1M x 768, ef 64): 6 -> 1.40M QPS, 4 -> 1.32M, 8 -> 1.02M (spills)
-  const WalkKernel kern = walk_kernel(h->metric, h->vt, occ);
+  const WalkKernel kern = walk_kernel(h->metric, h->vt, occ, bf != nullptr);
   SDB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   // the walk gets nothing from L1 (0.7 % hit rate): give the whole array to shared memory, or the driver's default
   // carve-out (135 KB) caps the kernel at 5 blocks per SM
@@ -2050,7 +2349,7 @@ static sdb_status hnsw_search_impl(sdb_hnsw* h, const void* queries, uint32_t nq
   // visited tables: one per resident warp; 16 x the worst-case expansion of a typical walk, >= 2^13 slots
   uint32_t tl = 13;
   while ((1u << tl) < ef * 64u * 4u && tl < 20) tl++;
-  if (truthy) tl = tl + 3 > 18 ? (tl > 18 ? tl : 18) : tl + 3;  // filtered walks visit ~1/selectivity more elements
+  if (filtered) tl = tl + 3 > 18 ? (tl > 18 ? tl : 18) : tl + 3;  // filtered walks visit ~1/selectivity more elements
   const uint32_t n_tables = grid * HN_WARPS;
   if (!h->d_visited || h->table_log2 != tl || h->n_tables < n_tables) {
     h->d_visited.reset();
@@ -2073,6 +2372,10 @@ static sdb_status hnsw_search_impl(sdb_hnsw* h, const void* queries, uint32_t nq
   AsyncBuf<double> dist_buf;
   AsyncBuf<uint32_t> cnt_buf, d_ovf;
   AsyncBuf<uint8_t> d_noexp, d_truthy;
+  AsyncBuf<uint32_t> d_filters, d_qf, d_spill;
+  DevBuf<ulonglong2> spill_heap;
+  DevBuf<uint32_t> spill_stamp;
+  AsyncBuf<uint32_t> spill_next;
   void* d_q = const_cast<void*>(queries);
   uint64_t* d_elems = out_elems;
   double* d_dist = out_dist;
@@ -2096,7 +2399,30 @@ static sdb_status hnsw_search_impl(sdb_hnsw* h, const void* queries, uint32_t nq
     SDB_CUDA(d_truthy.reserve(h->n ? h->n : 1, st));
     SDB_CUDA(cudaMemcpyAsync(d_truthy, truthy, h->n, cudaMemcpyHostToDevice, st));
   }
+  const uint32_t fwords = (uint32_t)((h->n + 31) / 32);
+  const uint32_t* filters = nullptr;
+  if (bf) {
+    filters = bf->filters;
+    if (!bf->on_device) {
+      const size_t words = (size_t)fwords * bf->n_filters;
+      SDB_CUDA(d_filters.reserve(words ? words : 1, st));
+      SDB_CUDA(cudaMemcpyAsync(d_filters, bf->filters, sizeof(uint32_t) * words, cudaMemcpyHostToDevice, st));
+      filters = d_filters;
+    }
+    if (bf->query_filter) {  // copied before the call returns (the synchronisation below)
+      SDB_CUDA(d_qf.reserve(nq, st));
+      SDB_CUDA(cudaMemcpyAsync(d_qf, bf->query_filter, sizeof(uint32_t) * nq, cudaMemcpyHostToDevice, st));
+    }
+    h->last_spilled = 0;
+    SDB_CUDA(d_spill.reserve((size_t)nq + 1, st));  // the spill list, then its length
+    SDB_CUDA(cudaMemsetAsync(d_spill.get() + nq, 0, sizeof(uint32_t), st));
+  }
   HnswParams P;
+  P.filters = filters;
+  P.query_filter = d_qf;
+  P.fwords = fwords;
+  P.spill_list = d_spill;
+  P.n_spill = bf ? d_spill.get() + nq : nullptr;
   P.ccap = ccap;
   P.truthy = d_truthy;
   P.noexp = d_noexp;
@@ -2138,6 +2464,14 @@ static sdb_status hnsw_search_impl(sdb_hnsw* h, const void* queries, uint32_t nq
     count_launch(ctx);
   }
   h->gen += gens_per_warp * n_tables;
+  if (bf && qrc == SDB_OK) {  // the queries the on-chip walk gave up on go to the spill tier
+    uint32_t n_sp = 0;
+    SDB_CUDA(cudaMemcpyAsync(&n_sp, P.n_spill, sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
+    SDB_CUDA(cudaStreamSynchronize(st));
+    SDB_CUDA(cudaGetLastError());
+    h->last_spilled = n_sp;
+    if (n_sp && !ctx_cancelled(ctx)) SDB_TRY(hnsw_spill(h, P, n_sp, spill_heap, spill_stamp, spill_next));
+  }
   uint32_t ovf = 0;
   if (!device_io) {
     SDB_CUDA(cudaMemcpyAsync(out_elems, d_elems, sizeof(uint64_t) * (size_t)nq * k, cudaMemcpyDeviceToHost, st));
@@ -2280,5 +2614,25 @@ sdb_status sdb_hnsw_search_filtered(sdb_hnsw* h, const void* queries, uint32_t n
   }
   return hnsw_search_impl(h, queries, nq, k, ef, truthy, nullptr, out_elems, out_dist, out_count, out_counters);
 }
+
+sdb_status sdb_hnsw_search_filtered_batch(sdb_hnsw* h, const void* queries, uint32_t nq, uint32_t k, uint32_t ef,
+                                          const uint32_t* filters, uint32_t n_filters, const uint32_t* query_filter,
+                                          uint64_t* out_elems, double* out_dist, uint32_t* out_count,
+                                          uint64_t* out_counters) {
+  const BatchFilter bf{filters, n_filters, query_filter, false};
+  return hnsw_search_impl(h, queries, nq, k, ef, nullptr, nullptr, out_elems, out_dist, out_count, out_counters, false,
+                          &bf);
+}
+
+sdb_status sdb_hnsw_search_filtered_batch_device(sdb_hnsw* h, const void* d_queries, uint32_t nq, uint32_t k, uint32_t ef,
+                                                 const uint32_t* d_filters, uint32_t n_filters,
+                                                 const uint32_t* query_filter, uint64_t* d_out_elems,
+                                                 double* d_out_dist, uint32_t* d_out_count, uint64_t* d_out_counters) {
+  const BatchFilter bf{d_filters, n_filters, query_filter, true};
+  return hnsw_search_impl(h, d_queries, nq, k, ef, nullptr, nullptr, d_out_elems, d_out_dist, d_out_count, d_out_counters,
+                          true, &bf);
+}
+
+uint32_t sdb_hnsw_last_spilled(const sdb_hnsw* h) { return h ? h->last_spilled : 0; }
 
 }  // extern "C"

@@ -3,6 +3,7 @@
   HnswIndex.load(...)                 what the Rust shim hands over after HnswFlavor::check_state
                                       (idx/trees/hnsw/mod.rs:187-224): element vectors + per-layer adjacency
   HnswIndex.search_graph(q, k, ef)    Hnsw::knn_search (hnsw/mod.rs:459-482) -> [(dist, element)] ascending
+  HnswIndex.search_graph_filtered(..) Hnsw::knn_search_with_filter with one element bitmap per query, any selectivity
   HnswIndex.knn_search(q, k, ef)      HnswIndex::knn_search (hnsw/index.rs:270-335): pending updates first
                                       (search_pendings, :372-420), then the graph with the pending-docs bitmap,
                                       element -> docs expansion through KnnResultBuilder semantics
@@ -268,6 +269,46 @@ class HnswIndex:
             return ids, dist, cnt, ctr
         return ids, dist, cnt
 
+    def filter_words(self, filters):
+        """bool masks (n,) or (n_filters, n) over the elements, or their packed uint32 words (engine.pack_row_filter)
+        -> contiguous (n_filters, ceil(n / 32)) uint32 words"""
+        from .engine import _filter_args, pack_row_filter
+        f = np.asarray(filters)
+        if f.dtype == np.bool_:
+            if f.shape[-1] != self.n:
+                raise L.SdbError(L.SDB_EINVAL, f"filter masks must have one entry per element ({self.n})")
+            f = pack_row_filter(f)
+        return _filter_args(f, None, 0, self.n)[0]
+
+    def search_graph_filtered(self, queries, k, ef, filters, query_filter=None, counters=False):
+        """Hnsw::knn_search_with_filter for a batch whose queries each pick one of several predicates
+        (sdb_hnsw_search_filtered_batch): filters = bool masks (n,) / (n_filters, n) or packed uint32 words
+        (filter_words); query_filter = one filter index per query (None: filter 0 for every query).  Any selectivity
+        is served on the GPU: queries that outgrow the on-chip candidate window finish in the spill tier."""
+        from .engine import _query_filter
+        q = to_vector_type(queries, self.vector_type)
+        if q.ndim == 1:
+            q = q[None, :]
+        if q.shape[1] != self.dim:  # Error::InvalidVectorDimension  idx/trees/vector.rs:643-652
+            raise L.SdbError(L.SDB_EDIM, f"Incorrect vector dimension ({q.shape[1]}). Expected a vector of {self.dim} dimension.")
+        nq = q.shape[0]
+        f = self.filter_words(filters)
+        qf = _query_filter(query_filter, nq)
+        ids = np.zeros((nq, max(k, 1)), np.uint64)
+        dist = np.zeros((nq, max(k, 1)), np.float64)
+        cnt = np.zeros(nq, np.uint32)
+        ctr = np.zeros((nq, 2), np.uint64)
+        L.check(L.lib().sdb_hnsw_search_filtered_batch(self.h, C.c_void_p(q.ctypes.data), nq, int(k), int(ef),
+                                                       C.c_void_p(f.ctypes.data), f.shape[0],
+                                                       None if qf is None else C.c_void_p(qf.ctypes.data),
+                                                       C.c_void_p(ids.ctypes.data), C.c_void_p(dist.ctypes.data),
+                                                       C.c_void_p(cnt.ctypes.data), C.c_void_p(ctr.ctypes.data)))
+        return (ids, dist, cnt, ctr) if counters else (ids, dist, cnt)
+
+    def last_spilled(self):
+        """queries of the last search_graph_filtered call that the spill tier finished"""
+        return int(L.lib().sdb_hnsw_last_spilled(self.h))
+
     def knn_search(self, query, k, ef, truthy_docs=None):
         """-> [(vector id, distance)] ordered by (distance, VectorId), at most k  (one query).  Mirrors
         HnswIndex::knn_search (hnsw/index.rs:270-335):
@@ -314,8 +355,13 @@ class HnswIndex:
             for e in range(self.n):
                 dl = docs_of(e)
                 all_pending[e] = all(int(d) in pending_docs for d in dl)  # an element without docs counts as pending
-        ids, dist, cnt = self.search_graph(to_vector_type(query, self.vector_type)[None, :], k, ef, truthy=truthy,
-                                           all_docs_pending=all_pending)
+        q = to_vector_type(query, self.vector_type)[None, :]
+        if truthy is not None:  # any selectivity on the GPU; add_if_truthy ignores all-pending elements (layer.rs:287-296)
+            if all_pending is not None:
+                truthy &= all_pending == 0
+            ids, dist, cnt = self.search_graph_filtered(q, k, ef, truthy.astype(bool))
+        else:
+            ids, dist, cnt = self.search_graph(q, k, ef, all_docs_pending=all_pending)
         for j in range(int(cnt[0])):
             d, e = float(dist[0, j]), int(ids[0, j])
             if builder.check_add(d):
