@@ -45,7 +45,9 @@ typedef enum {
 } sdb_status;
 
 /* catalog::Distance (catalog/schema/index.rs:247-284).  COSINE and EUCLIDEAN are screened on the tensor cores and
- * re-ranked exactly; the other six run through the exact kernel (sequential f64, Distance::compute op for op). */
+ * re-ranked exactly; MANHATTAN and CHEBYSHEV are screened by the f32 L1 / L-infinity SIMT screen (SDB_SCREEN_SIMT_F32)
+ * and re-ranked exactly; HAMMING, JACCARD, MINKOWSKI and PEARSON run through the exact kernel (sequential f64,
+ * Distance::compute op for op). */
 typedef enum {
   SDB_CHEBYSHEV = 0,
   SDB_COSINE = 1,
@@ -61,7 +63,9 @@ typedef enum {
  * Brute-force KnnTopK holds Vec<Number>: F64 covers arbitrary Number::Float rows, F32 covers rows whose
  * values are f32-representable (the BASELINE configs).  COSINE / EUCLIDEAN corpora of either type are screened on the
  * tensor cores (F64: when the bf16 / int8 copies, 3 bytes per element, fit beside the rows at creation; otherwise the
- * corpus is ranked by the exact kernel alone).  The f32 SIMT screen needs F32 rows: on F64 it means the exact kernel. */
+ * corpus is ranked by the exact kernel alone).  The f32 SIMT screen of COSINE / EUCLIDEAN needs F32 rows: on F64 it
+ * means the exact kernel.  MANHATTAN / CHEBYSHEV corpora of either type are screened by the f32 L1 / L-infinity screen
+ * (f64 rows rounded to f32 as the screen reads them; rows with an element beyond f32 range are ranked exactly). */
 typedef enum { SDB_F32 = 0, SDB_F64 = 1 } sdb_dtype;
 
 /* element type of an HNSW index: catalog::VectorType (catalog/schema/index.rs:321-335), numbered as the SerializedVector
@@ -72,10 +76,13 @@ typedef enum { SDB_VT_F64 = 0, SDB_VT_F32 = 1, SDB_VT_I64 = 2, SDB_VT_I32 = 3, S
 /* which screening kernel sdb_knn_bruteforce uses (results are identical for all; this only moves the performance
  * point).  AUTO: cosine corpora whose normalised rows quantise well (largest relative int8 error <= 0.02 once the few
  * outlier rows are set aside) start on the int8 tensor-core screen, everything else on the bf16 one; queries whose
- * proof fails climb to finer screens (bf16, then the f32 stream) before the exact kernel. */
+ * proof fails climb to finer screens (bf16, then the f32 stream) before the exact kernel.  MANHATTAN / CHEBYSHEV corpora
+ * (k <= 256) are screened by SDB_SCREEN_SIMT_F32 for AUTO and every TC request (4096, then 16384 candidates per query,
+ * then the exact kernel), except that AUTO ranks a batch of one query with the exact kernel (faster for a single query);
+ * NONE_EXACT keeps them on the exact kernel. */
 typedef enum {
   SDB_SCREEN_AUTO = 0,
-  SDB_SCREEN_SIMT_F32 = 1,   /* f32 streaming SIMT kernel                                             */
+  SDB_SCREEN_SIMT_F32 = 1,   /* f32 SIMT screen: streaming dot products; MANHATTAN / CHEBYSHEV: L1 / L-inf */
   SDB_SCREEN_TC_BF16 = 2,    /* wgmma bf16 operands, f32 accumulation                                    */
   SDB_SCREEN_NONE_EXACT = 3, /* no screen: exact f64 kernel for every query                              */
   SDB_SCREEN_TC_INT8 = 4     /* wgmma s8, int8 copy         of the normalised rows (cosine); falls back to bf16 */
@@ -134,7 +141,8 @@ sdb_status sdb_debug_corpus_state(sdb_corpus*, float* out_f, uint32_t* out_u, in
                                   float* out_snorm, uint32_t* out_special);
 /* sdb_debug_screen_batch: one batch of nq host queries screened with `screen` (TC_INT8, TC_BF16 or SIMT_F32) at the
  * first rung of the ladder, through the production sequence (streaming = 0: the multi-pass schedule), with exactly
- * cand_cap (>= 4096) candidate slots per query (F64 corpora with screen copies: TC_INT8 or TC_BF16 only).  The ladder
+ * cand_cap (>= 4096) candidate slots per query (F64 corpora with screen copies: TC_INT8 or TC_BF16 only; MANHATTAN / CHEBYSHEV corpora, F32 or F64: SIMT_F32, where
+ * beps bounds |s~ - d| and the score is -s~).  The ladder
  * and the exact fallback do not run: flags are as the batch
  * left them.  score_all != 0 instead runs one pass-0 launch over every tile (SIMT: tau = -inf) with max(cand_cap,
  * n_pad) slots and selects nothing: out_a then holds every score of that kernel, and out_b / out_rr are untouched.
@@ -244,7 +252,8 @@ sdb_status sdb_knn_wait(sdb_corpus*, uint32_t ticket);
  * metric, F32 and F64, k <= 4096, cancellation, sdb_knn_last_stats, up to 4 tickets in flight (filtered and unfiltered
  * mixed), completion through sdb_knn_wait.  SDB_EINVAL: n_filters == 0 with nq > 0, filters == NULL, or an index >=
  * n_filters.
- * A query whose bitmap has at most 4096 set bits skips the screen (its passing rows are ranked directly; results are
+ * A query whose bitmap has at most 4096 set bits (COSINE, EUCLIDEAN, MANHATTAN, CHEBYSHEV; k <= 256) skips the screen
+ * (its passing rows are ranked directly; results are
  * the same); sdb_knn_last_stats then reports screen_used = SDB_SCREEN_NONE_EXACT and n_passes = 0 for a batch of such
  * queries only.
  * Host variants: `filters` is host memory, staged per batch on the copy stream (submit: `queries`, `filters` and the

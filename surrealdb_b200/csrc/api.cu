@@ -100,7 +100,7 @@ struct Rung {
 // cluster on tightly packed data); a rung fails for a query only when that set overflows the list.  When that happens
 // to more than a handful of queries the batch is re-screened with a tighter screen / longer lists instead of paying
 // one exact pass over the corpus per failed query; the rung that worked is remembered per corpus and k.
-static std::vector<Rung> build_rungs(Corpus* c, uint32_t k, sdb_screen* first) {
+static std::vector<Rung> build_rungs(Corpus* c, uint32_t k, uint32_t nq, sdb_screen* first) {
   const bool int8_ok = c->d_i8 && c->metric == SDB_COSINE && screen_tc_available();
   sdb_screen scr = c->screen;
   if (scr == SDB_SCREEN_AUTO)
@@ -108,15 +108,21 @@ static std::vector<Rung> build_rungs(Corpus* c, uint32_t k, sdb_screen* first) {
                                  : (int8_ok && c->max_rel_qerr <= 0.02f ? SDB_SCREEN_TC_INT8 : SDB_SCREEN_TC_BF16);
   if (scr == SDB_SCREEN_TC_INT8 && !int8_ok) scr = SDB_SCREEN_TC_BF16;
   if (scr == SDB_SCREEN_TC_BF16 && (!screen_tc_available() || !c->d_bf16)) scr = SDB_SCREEN_SIMT_F32;
-  const bool screenable = c->metric == SDB_COSINE || c->metric == SDB_EUCLIDEAN;
-  // the SIMT screen streams f32 rows: an f64 corpus is screened on the tensor cores or not at all
-  if (c->dtype == SDB_F64 && scr == SDB_SCREEN_SIMT_F32) scr = SDB_SCREEN_NONE_EXACT;
+  // MANHATTAN / CHEBYSHEV: the f32 L1 / L-infinity screen (screen_lp.cu) is their only screen, for f32 and f64 rows
+  const bool lp = c->metric == SDB_MANHATTAN || c->metric == SDB_CHEBYSHEV;
+  const bool screenable = c->metric == SDB_COSINE || c->metric == SDB_EUCLIDEAN || lp;
+  // the SIMT screen streams f32 rows: an f64 cosine / euclidean corpus is screened on the tensor cores or not at all
+  if (c->dtype == SDB_F64 && scr == SDB_SCREEN_SIMT_F32 && !lp) scr = SDB_SCREEN_NONE_EXACT;
   if (c->special_overflow || k > 256 || !screenable) scr = SDB_SCREEN_NONE_EXACT;
+  // a single query streams the rows once either way, and the exact kernel does it at the higher HBM rate (DESIGN.md
+  // section 5): AUTO ranks it there; an explicit SIMT_F32 request is kept
+  if (lp && nq == 1 && c->screen == SDB_SCREEN_AUTO) scr = SDB_SCREEN_NONE_EXACT;
   *first = scr;
   std::vector<Rung> r;
   if (scr == SDB_SCREEN_TC_INT8)
     r = {{SDB_SCREEN_TC_INT8, 4096}, {SDB_SCREEN_TC_INT8, 16384}, {SDB_SCREEN_TC_BF16, 4096}, {SDB_SCREEN_TC_BF16, 16384}};
   else if (scr == SDB_SCREEN_TC_BF16) r = {{SDB_SCREEN_TC_BF16, 4096}, {SDB_SCREEN_TC_BF16, 16384}};
+  else if (scr == SDB_SCREEN_SIMT_F32 && lp) r = {{SDB_SCREEN_SIMT_F32, 4096}, {SDB_SCREEN_SIMT_F32, 16384}};
   else if (scr == SDB_SCREEN_SIMT_F32) r = {{SDB_SCREEN_SIMT_F32, 4096}};
   // the f32 stream (error bound ~500x tighter than bf16) as the last rung before the exact kernel -- only ever used
   // for the few queries of a batch that every tensor-core rung failed to prove (finish_local), never for a whole batch
@@ -125,7 +131,8 @@ static std::vector<Rung> build_rungs(Corpus* c, uint32_t k, sdb_screen* first) {
 }
 static uint32_t n_batch_rungs(const std::vector<Rung>& r) {  // rungs a WHOLE batch may be re-screened on
   uint32_t n = (uint32_t)r.size();
-  if (n > 1 && r.back().scr == SDB_SCREEN_SIMT_F32) n--;
+  // (the f32 stream behind tensor-core rungs is for single queries; an all-SIMT ladder re-screens whole batches)
+  if (n > 1 && r.back().scr == SDB_SCREEN_SIMT_F32 && r[n - 2].scr != SDB_SCREEN_SIMT_F32) n--;
   return n;
 }
 
@@ -314,7 +321,7 @@ static sdb_status enqueue_screened(Corpus* c, Ticket& t) {
   cudaStream_t st = t.stream;
   const uint32_t nq = t.nq, k = t.k;
   sdb_screen first;
-  const std::vector<Rung> rungs = build_rungs(c, k, &first);
+  const std::vector<Rung> rungs = build_rungs(c, k, nq, &first);
   t.n_rungs = (uint32_t)rungs.size();
   t.n_passes = 0;
   SDB_CUDA(cudaEventRecord(t.ev_begin, st));
@@ -451,7 +458,7 @@ static sdb_status finish_local(Corpus* c, Ticket& t, uint32_t* n_fallback, bool*
   }
   if (t.n_rungs) {
     sdb_screen first;
-    build_rungs(c, k, &first);
+    build_rungs(c, k, nq, &first);
     c->rung_scr = first;
     c->rung_k = k;
     c->rung = t.rung;
@@ -468,7 +475,8 @@ static sdb_status finish_local(Corpus* c, Ticket& t, uint32_t* n_fallback, bool*
   // corpus costs about as much for 60 queries as for 1, and far less than one sequential-f64 pass per query); the f32
   // stream is the last rung.  Whatever is still unproven after that goes to the exact kernel.
   if (!fails.empty() && t.screen != SDB_SCREEN_NONE_EXACT && c->exact && k) {
-    const uint32_t save_rung = t.rung, save_nq = t.nq, save_passes = t.n_passes;
+    // (save_rungs: a one-query MANHATTAN / CHEBYSHEV repair has no rungs of its own, build_rungs)
+    const uint32_t save_rung = t.rung, save_nq = t.nq, save_passes = t.n_passes, save_rungs = t.n_rungs;
     const int save_screen = t.screen;
     const double* save_q = t.d_queries;
     const uint32_t* save_qf = t.filt.qf;
@@ -479,7 +487,7 @@ static sdb_status finish_local(Corpus* c, Ticket& t, uint32_t* n_fallback, bool*
     uint32_t* save_cnt = t.d_out_count;
     uint32_t save_stat[4] = {t.h_stat[0], t.h_stat[1], t.h_stat[2], t.h_stat[3]};
     sdb_status rc = SDB_OK;
-    for (uint32_t rung = save_rung + 1; rung < t.n_rungs && !fails.empty() && rc == SDB_OK; rung++) {
+    for (uint32_t rung = save_rung + 1; rung < save_rungs && !fails.empty() && rc == SDB_OK; rung++) {
       if ((t.cancel && *t.cancel) || ctx_cancelled(ctx)) break;
       const uint32_t nf = (uint32_t)fails.size();
       const size_t need_q = (size_t)nf * c->dim, need_o = (size_t)nf * k;
@@ -538,6 +546,7 @@ static sdb_status finish_local(Corpus* c, Ticket& t, uint32_t* n_fallback, bool*
     t.d_out_dist = save_dist;
     t.d_out_count = save_cnt;
     t.rung = save_rung;
+    t.n_rungs = save_rungs;
     t.screen = save_screen;
     t.n_passes = save_passes;
     for (int i = 0; i < 4; i++) t.h_stat[i] = save_stat[i];
@@ -634,9 +643,11 @@ static sdb_status submit_locked(Corpus* c, Ticket* t, const double* d_queries, u
     t->filt.bits = d_filters;
     t->filt.words = (uint32_t)((c->n + 31) / 32);
     // direct regime: a query whose filter passes at most DIRECT_MAX_ROWS rows (filter_rows: set bits, an upper bound
-    // of the rows it passes) skips the screen; the re-rank and cand_final serve the two screenable metrics, k <= 256
+    // of the rows it passes) skips the screen; the re-rank and cand_final serve the four screenable metrics, k <= 256
     std::vector<uint32_t> scr, dir;
-    const bool direct_ok = filter_rows && k > 0 && k <= 256 && (c->metric == SDB_COSINE || c->metric == SDB_EUCLIDEAN);
+    const bool direct_ok = filter_rows && k > 0 && k <= 256 &&
+                           (c->metric == SDB_COSINE || c->metric == SDB_EUCLIDEAN || c->metric == SDB_MANHATTAN ||
+                            c->metric == SDB_CHEBYSHEV);
     for (uint32_t q = 0; q < nq; q++) {
       const uint64_t rows_q = filter_rows ? filter_rows[t->h_qf[q]] : ~0ull;
       if (direct_ok && rows_q <= DIRECT_MAX_ROWS) dir.push_back(q);
@@ -673,7 +684,7 @@ static sdb_status submit_locked(Corpus* c, Ticket* t, const double* d_queries, u
   t->launches0 = c->ctx->launches;
   t->n_repaired = 0;
   sdb_screen first;
-  const std::vector<Rung> rungs = build_rungs(c, k, &first);
+  const std::vector<Rung> rungs = build_rungs(c, k, nq, &first);
   t->rung = (c->rung_scr == first && c->rung_k == k && c->rung < n_batch_rungs(rungs)) ? c->rung : 0;
   t->n_rungs = (uint32_t)rungs.size();
   t->n_batch_rungs = n_batch_rungs(rungs);
@@ -1037,8 +1048,8 @@ sdb_status sdb_corpus_create(sdb_ctx* ctx, uint32_t dim, sdb_dtype dt, sdb_metri
     set_error("sdb_corpus_create: bad argument (dim 1..65535, 0 < capacity < 2^32)");
     return SDB_EINVAL;
   }
-  // COSINE / EUCLIDEAN: screened (K1/K2) + exact re-rank.  MANHATTAN / CHEBYSHEV / HAMMING / PEARSON / JACCARD /
-  // MINKOWSKI: served by the exact kernel alone (sequential f64, Distance::compute op for op).  MINKOWSKI goes through
+  // COSINE / EUCLIDEAN: screened (K1/K2) + exact re-rank.  MANHATTAN / CHEBYSHEV: the f32 L1 / L-infinity screen
+  // (screen_lp.cu) + exact re-rank.  HAMMING / PEARSON / JACCARD / MINKOWSKI: served by the exact kernel alone (sequential f64, Distance::compute op for op).  MINKOWSKI goes through
   // pow(), which CUDA's libm and Rust's (the platform libm) implement separately: within 1 ulp of each other per term,
   // so its distances are compared with a 1e-12 relative tolerance instead of bit equality (tests/test_gpu_knn.py).
   const bool screenable = m == SDB_COSINE || m == SDB_EUCLIDEAN;
@@ -1348,7 +1359,8 @@ sdb_status sdb_debug_corpus_state(sdb_corpus* c, float* out_f, uint32_t* out_u, 
                                   float* out_snorm, uint32_t* out_special) {
   if (!c) return SDB_EINVAL;
   std::lock_guard<std::mutex> g(c->mu);
-  if (!c->finalized || (c->dtype != SDB_F32 && !c->d_bf16) || (out_i8 && !c->d_i8) || (out_bf16 && !c->d_bf16)) {
+  const bool lp = c->metric == SDB_MANHATTAN || c->metric == SDB_CHEBYSHEV;
+  if (!c->finalized || (c->dtype != SDB_F32 && !c->d_bf16 && !lp) || (out_i8 && !c->d_i8) || (out_bf16 && !c->d_bf16)) {
     set_error("sdb_debug_corpus_state: needs a finalized F32 corpus or a screened F64 one (int8 copy: cosine only)");
     return SDB_EINVAL;
   }
@@ -1390,11 +1402,15 @@ sdb_status sdb_debug_screen_batch(sdb_corpus* c, const double* queries, uint32_t
   }
   std::lock_guard<std::mutex> g(c->mu);
   const bool int8 = screen == SDB_SCREEN_TC_INT8;
-  const bool f64_ok = c->dtype == SDB_F64 && tc && c->d_bf16;  // f64 rows: tensor-core screens only
-  if (!c->finalized || (c->dtype != SDB_F32 && !f64_ok) || (c->metric != SDB_COSINE && c->metric != SDB_EUCLIDEAN) ||
-      (int8 && !c->d_i8) || c->special_overflow || !c->n) {
-    set_error("sdb_debug_screen_batch: needs a finalized, non-empty F32 cosine / euclidean corpus, or an F64 one with "
-              "screen copies and a tensor-core screen (int8: cosine)");
+  // MANHATTAN / CHEBYSHEV: the SIMT_F32 (L1 / L-infinity) screen, f32 and f64 rows
+  const bool lp = (c->metric == SDB_MANHATTAN || c->metric == SDB_CHEBYSHEV) && screen == SDB_SCREEN_SIMT_F32;
+  // f64 rows: tensor-core screens only (cosine / euclidean)
+  const bool f64_ok = c->dtype == SDB_F64 && ((tc && c->d_bf16) || lp);
+  if (!c->finalized || (c->dtype != SDB_F32 && !f64_ok) ||
+      (c->metric != SDB_COSINE && c->metric != SDB_EUCLIDEAN && !lp) || (int8 && !c->d_i8) || c->special_overflow ||
+      !c->n) {
+    set_error("sdb_debug_screen_batch: needs a finalized, non-empty F32 cosine / euclidean corpus, an F64 one with "
+              "screen copies and a tensor-core screen (int8: cosine), or a MANHATTAN / CHEBYSHEV one with SIMT_F32");
     return SDB_EINVAL;
   }
   Ctx* ctx = c->ctx;

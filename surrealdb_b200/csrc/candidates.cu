@@ -203,7 +203,87 @@ __global__ void cand_begin_kernel(float* __restrict__ tau, uint32_t* __restrict_
   qlow[q] = __double2float_rd(lo);
   qcap[q] = __double2float_ru(hi);
 }
+// The same for MANHATTAN / CHEBYSHEV corpora (screen_lp.cu: score = -s~), one warp per query.  beps bounds |s~ - d|
+// for every screened row, d = the reference's distance (sequential f64 over the f64 values).  With u = 2^-24,
+// Q = sum_i |q^_i|, Qm = max_i |q^_i| (q^ = fl32(q)) and M = max_norm (largest sum_i |x^_i| resp. max_i |x^_i| of a
+// screened row; x^ = fl32(x), so x^ = x for f32 rows):
+//  - q^_i = q_i (1 + d1) + a1, |d1| <= u, |a1| <= 2^-150 (f32 underflow); the same for x^_i of f64 rows;
+//  - t_i = fl32(x^_i - q^_i) = (x^_i - q^_i)(1 + d2), |d2| <= u (an f32 difference in the subnormal range is exact);
+//  - MANHATTAN: f32 sums of D non-negative terms in any order err by at most (D-1) u / (1 - (D-1) u) relative (f32
+//    additions of non-negative numbers never lose more to underflow); the reference's sequential f64 sum and its f64
+//    differences by at most D 2^-53 relative.  Every term is bounded by W = M + Q: sum_i |x^_i - q^_i| <= M + Q, and
+//    sum_i |x_i| + |q_i| <= (1 + u) W + D 2^-149.  Summed: |s~ - d| <= (D + 3) u (1 + 2 (D + 3) u) W + D 2^-52 W
+//    + D 2^-147;
+//  - CHEBYSHEV: a maximum adds no error; |t_i - |x_i - q_i|| <= u (|x^_i| + |q^_i|) (1 + u) + u |q_i| + u |x_i| + 2^-149
+//    and the reference's f64 difference adds 2^-53 relative: |s~ - d| <= (3 u + 2^-52) (M + Qm) (1 + 2^-20) + 2^-147.
+// A query or a corpus whose W is not a finite f32 gets an infinite bound (tau then proves nothing: exact fallback).
+// Stage B (cand_refine) does not run for these metrics: tau2 stays -inf.
+__global__ void __launch_bounds__(128) cand_begin_lp_kernel(float* __restrict__ tau, uint32_t* __restrict__ cnt,
+                                                            uint32_t* __restrict__ flags, uint32_t* __restrict__ stat,
+                                                            float* __restrict__ bscale, float* __restrict__ beps,
+                                                            float* __restrict__ margin, float* __restrict__ margin2,
+                                                            float* __restrict__ beps2, float* __restrict__ tau2,
+                                                            float* __restrict__ qlow, float* __restrict__ qcap,
+                                                            const float* __restrict__ q32, uint32_t nq, int metric,
+                                                            uint32_t dim, float max_norm, int exact) {
+  const uint32_t lane = threadIdx.x & 31u, q = blockIdx.x * 4 + (threadIdx.x >> 5);
+  if (blockIdx.x == 0 && threadIdx.x < 4) stat[threadIdx.x] = 0;
+  if (q >= nq) return;
+  double l1 = 0.0;
+  float amax = 0.f;
+  for (uint32_t c = lane; c < dim; c += 32) {
+    const float v = fabsf(q32[(size_t)q * dim + c]);
+    l1 += (double)v;
+    amax = fmaxf(amax, v);
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    l1 += __shfl_xor_sync(0xffffffffu, l1, o);
+    amax = fmaxf(amax, __shfl_xor_sync(0xffffffffu, amax, o));
+  }
+  if (lane != 0) return;
+  const double D = (double)dim, u = 0x1p-24;
+  double eps, w;
+  if (metric == SDB_MANHATTAN) {
+    w = (double)max_norm + l1 * (1.0 + 0x1p-30);
+    eps = ((D + 3.0) * u * (1.0 + 2.0 * (D + 3.0) * u) + D * 0x1p-52) * w + D * 0x1p-147;
+  } else {
+    w = (double)max_norm + (double)amax;
+    eps = (3.0 * u + 0x1p-52) * w * (1.0 + 0x1p-20) + 0x1p-147;
+  }
+  double mg = 2.1 * eps, hi = eps + 1e-30, lo = -(w * 1.01 + eps) - 1e-30;
+  if (!(w <= 3.4028234663852886e38) || !isfinite(eps)) {  // s~ may overflow f32: no bound
+    eps = INFINITY;
+    mg = 0.0;
+    hi = 1.0;
+    lo = -1.0;
+  }
+  if (!exact) mg = 0.0;
+  tau[q] = __int_as_float(0xff800000);  // -inf
+  cnt[q] = 0;
+  flags[q] = 0;
+  bscale[q] = 1.f;
+  beps[q] = __double2float_ru(eps);
+  margin[q] = __double2float_ru(mg);
+  margin2[q] = 0.f;
+  beps2[q] = 0.f;
+  tau2[q] = __int_as_float(0xff800000);
+  qlow[q] = __double2float_rd(lo);
+  qcap[q] = __double2float_ru(hi);
+}
+
+static bool lp_metric(const Corpus* c) { return c->metric == SDB_MANHATTAN || c->metric == SDB_CHEBYSHEV; }
+
 sdb_status cand_begin(Corpus* c, uint32_t nq, int screen, cudaStream_t st) {
+  if (lp_metric(c)) {
+    cand_begin_lp_kernel<<<(nq + 3) / 4, 128, 0, st>>>(c->d_tau, c->d_cand_cnt, c->d_flags, c->d_stat, c->d_bscale,
+                                                       c->d_beps, c->d_margin, c->d_margin2, c->d_beps2, c->d_tau2,
+                                                       c->d_qlow, c->d_qcap, c->d_q32, nq, (int)c->metric, c->dim,
+                                                       c->max_norm, c->exact ? 1 : 0);
+    count_launch(c->ctx);
+    SDB_CUDA(cudaGetLastError());
+    return SDB_OK;
+  }
   cand_begin_kernel<<<(nq + 255) / 256, 256, 0, st>>>(c->d_tau, c->d_cand_cnt, c->d_flags, c->d_stat, c->d_bscale, c->d_beps,
                                                       c->d_margin, c->d_margin2, c->d_beps2, c->d_tau2, c->d_qlow, c->d_qcap,
                                                       c->d_qmag, c->d_q8scale,
@@ -994,8 +1074,54 @@ __global__ void __launch_bounds__(128) cand_rerank_packed_kernel(
   }
 }
 
+// MANHATTAN / CHEBYSHEV re-rank: the exact kernel's arithmetic (ExactAcc::manhattan_step / chebyshev_step, canon_nan)
+// per candidate, one thread per list entry and its row streamed left to right (the query's elements are the same
+// address across the warp).  Blocks (x = query, y = 0 .. RR_GROUPS_Y - 1) stride over the query's entries.
+template <typename T, int METRIC>
+__global__ void __launch_bounds__(128) cand_rerank_lp_kernel(
+    const T* __restrict__ rows, uint32_t dim, const double* __restrict__ q64, const uint32_t* __restrict__ qflags,
+    const Cand* __restrict__ cand, const uint32_t* __restrict__ cnt, uint32_t cap, const uint32_t* __restrict__ special,
+    uint32_t n_special, uint64_t* __restrict__ rr_key, double* __restrict__ rr_dist, uint32_t* __restrict__ rr_row,
+    uint32_t rr_stride) {
+  const uint32_t q = blockIdx.x;
+  const uint32_t n_c = cnt[q] < cap ? cnt[q] : cap;
+  const uint32_t n_e = n_c + n_special;
+  const bool q_nan = (qflags[q] & 2u) != 0;
+  const double* qv = q64 + (size_t)q * dim;
+  for (uint32_t e = blockIdx.y * blockDim.x + threadIdx.x; e < n_e; e += gridDim.y * blockDim.x) {
+    const uint32_t my_row = e < n_c ? cand[(size_t)q * cap + e].row : special[e - n_c];
+    const T* x = rows + (size_t)my_row * dim;
+    ExactAcc acc;
+    if (METRIC == SDB_CHEBYSHEV) acc.acc = -1.7976931348623157e308;  // f64::MIN
+    for (uint32_t j = 0; j < dim; j++) {
+      if (METRIC == SDB_MANHATTAN) acc.manhattan_step((double)__ldg(x + j), __ldg(qv + j));
+      else acc.chebyshev_step((double)__ldg(x + j), __ldg(qv + j));
+    }
+    const double d = METRIC == SDB_MANHATTAN ? canon_nan(acc.acc, acc.nan_in || q_nan) : acc.acc;
+    const size_t o = (size_t)q * rr_stride + e;
+    rr_key[o] = dist_key(d);
+    rr_dist[o] = d;
+    rr_row[o] = my_row;
+  }
+}
+template <typename T>
+static void launch_rerank_lp(Corpus* c, uint32_t nq, uint32_t n_sp, cudaStream_t st) {
+  const dim3 grid(nq, RR_GROUPS_Y);
+  auto kern = c->metric == SDB_MANHATTAN ? cand_rerank_lp_kernel<T, SDB_MANHATTAN> : cand_rerank_lp_kernel<T, SDB_CHEBYSHEV>;
+  kern<<<grid, 128, 0, st>>>((const T*)c->d_rows.get(), c->dim, c->d_q64, c->d_qflags, c->d_cand, c->d_cand_cnt,
+                             c->sc_cap, c->d_special, n_sp, c->d_rr_key, c->d_rr_dist, c->d_rr_row, c->rr_stride);
+}
+
 sdb_status cand_rerank(Corpus* c, uint32_t nq, cudaStream_t st, bool small_sets) {
   const dim3 grid(nq, RR_GROUPS_Y);
+  if (lp_metric(c)) {
+    const uint32_t n_sp = c->filt.bits ? 0u : c->n_special;
+    if (c->dtype == SDB_F32) launch_rerank_lp<float>(c, nq, n_sp, st);
+    else launch_rerank_lp<double>(c, nq, n_sp, st);
+    count_launch(c->ctx);
+    SDB_CUDA(cudaGetLastError());
+    return SDB_OK;
+  }
   static const bool no_v4 = getenv("SDB_RERANK_SCALAR") != nullptr;
   static const bool no_packed = getenv("SDB_RERANK_STAGED") != nullptr;
   const uint32_t n_sp = c->filt.bits ? 0u : c->n_special;  // filtered: the passing special rows are in the lists
@@ -1073,14 +1199,17 @@ __device__ __forceinline__ void bitonic_pairs(uint64_t* s_key, uint64_t* s_idx, 
   }
 }
 
-__global__ void __launch_bounds__(256) cand_final_kernel(
-    const uint64_t* __restrict__ rr_key, const double* __restrict__ rr_dist, const uint32_t* __restrict__ rr_row,
-    uint32_t rr_stride, const uint32_t* __restrict__ cnt, uint32_t cap, uint32_t n_special,
-    const float* __restrict__ tau, const double* __restrict__ qmag, const float* __restrict__ bscale,
-    const float* __restrict__ beps, const float* __restrict__ tau2, const float* __restrict__ beps2,
-    uint32_t* __restrict__ flags, const uint32_t* __restrict__ qflags, uint32_t* __restrict__ stat, int metric,
-    uint32_t k, uint64_t row_base, uint64_t* __restrict__ out_rows,
-    double* __restrict__ out_dist, uint32_t* __restrict__ out_count, int debug) {
+// LP: the MANHATTAN / CHEBYSHEV proof (cand_final_lp_kernel); otherwise cosine / euclidean (cand_final_kernel)
+#define SDB_FINAL_PARAMS                                                                                               \
+  const uint64_t *__restrict__ rr_key, const double *__restrict__ rr_dist, const uint32_t *__restrict__ rr_row,       \
+      uint32_t rr_stride, const uint32_t *__restrict__ cnt, uint32_t cap, uint32_t n_special,                          \
+      const float *__restrict__ tau, const double *__restrict__ qmag, const float *__restrict__ bscale,                \
+      const float *__restrict__ beps, const float *__restrict__ tau2, const float *__restrict__ beps2,                 \
+      uint32_t *__restrict__ flags, const uint32_t *__restrict__ qflags, uint32_t *__restrict__ stat, int metric,      \
+      uint32_t k, uint64_t row_base, uint64_t *__restrict__ out_rows, double *__restrict__ out_dist,                   \
+      uint32_t *__restrict__ out_count, int debug
+template <bool LP>
+__device__ __forceinline__ void cand_final_body(SDB_FINAL_PARAMS) {
   __shared__ uint64_t s_key[FIN_WIN];  // distance key
   __shared__ uint64_t s_idx[FIN_WIN];  // (row << 32 | entry): secondary order by row (unique), entry = index into rr_*
   const uint32_t q = blockIdx.x;
@@ -1133,7 +1262,12 @@ __global__ void __launch_bounds__(256) cand_final_kernel(
       const double qm = qmag[q];
       const uint64_t kth = s_key[k - 1];
       bool ok;
-      if (metric == SDB_COSINE) {
+      if (LP) {
+        // score = -s~ < tau for a non-candidate, so s~ > -tau and d >= s~ - beps > -tau - beps: the row cannot reach
+        // the top k if that bound (rounded down) is strictly above the k-th exact key.  No stage B ran (tau2 = -inf).
+        const double L = (-(double)t - (double)beps[q]) * (1.0 - 1e-12);
+        ok = dist_key(L) > kth;
+      } else if (metric == SDB_COSINE) {
         // non-candidate: score <= tau  =>  sim <= tau * bscale / |q| + eps  =>  dist >= 1 - tau * bscale / |q| - eps
         const double bound = 1.0 - (double)t * (double)bscale[q] / qm - (double)beps[q] - 1e-9;
         ok = dist_key(bound) > kth;
@@ -1165,6 +1299,13 @@ __global__ void __launch_bounds__(256) cand_final_kernel(
     atomicMax(stat + 2, n_e);
   }
 }
+#define SDB_FINAL_ARGS                                                                                                 \
+  rr_key, rr_dist, rr_row, rr_stride, cnt, cap, n_special, tau, qmag, bscale, beps, tau2, beps2, flags, qflags, stat, \
+      metric, k, row_base, out_rows, out_dist, out_count, debug
+__global__ void __launch_bounds__(256) cand_final_kernel(SDB_FINAL_PARAMS) { cand_final_body<false>(SDB_FINAL_ARGS); }
+__global__ void __launch_bounds__(256) cand_final_lp_kernel(SDB_FINAL_PARAMS) { cand_final_body<true>(SDB_FINAL_ARGS); }
+#undef SDB_FINAL_ARGS
+#undef SDB_FINAL_PARAMS
 
 sdb_status cand_final(Corpus* c, uint32_t nq, uint32_t k, uint64_t row_base, uint64_t* d_out_rows, double* d_out_dist,
                       uint32_t* d_out_count, cudaStream_t st) {
@@ -1174,7 +1315,8 @@ sdb_status cand_final(Corpus* c, uint32_t nq, uint32_t k, uint64_t row_base, uin
   }
   static const int debug = getenv("SDB_DEBUG") != nullptr;
   const uint32_t n_sp = c->filt.bits ? 0u : c->n_special;  // filtered: the passing special rows are in the lists
-  cand_final_kernel<<<nq, 256, 0, st>>>(c->d_rr_key, c->d_rr_dist, c->d_rr_row, c->rr_stride, c->d_cand_cnt, c->sc_cap,
+  auto fin = lp_metric(c) ? cand_final_lp_kernel : cand_final_kernel;
+  fin<<<nq, 256, 0, st>>>(c->d_rr_key, c->d_rr_dist, c->d_rr_row, c->rr_stride, c->d_cand_cnt, c->sc_cap,
                                         n_sp, c->d_tau, c->d_qmag, c->d_bscale, c->d_beps, c->d_tau2, c->d_beps2, c->d_flags, c->d_qflags, c->d_stat,
                                         (int)c->metric, k, row_base, d_out_rows, d_out_dist, d_out_count, debug);
   count_launch(c->ctx);

@@ -75,6 +75,53 @@ __global__ void __launch_bounds__(WARPS * 32) finalize_rows_kernel(const T* __re
   }
 }
 
+// MANHATTAN / CHEBYSHEV corpora (screen_lp.cu).  The screen sees every row through its f32 copy x^ = fl32(x), so a
+// row with an element whose f32 copy is not finite (NaN, +-inf, or, in f64 rows, beyond f32 range) is special: ranked
+// exactly on every query.  snorm is 0 for screened rows (the score is -(s~ + snorm)) and NaN for skipped / special
+// ones.  max_norm = the largest norm of the metric over the screened rows, sum_i |x^_i| (MANHATTAN) or max_i |x^_i|
+// (CHEBYSHEV), summed in f64 and rounded up: the error bound of cand_begin_lp_kernel scales with it.  mag keeps the
+// reference's magnitude() arithmetic, as finalize_rows_kernel computes it.
+template <typename T, int WARPS>
+__global__ void __launch_bounds__(WARPS * 32) finalize_lp_kernel(const T* __restrict__ rows, uint32_t dim, uint64_t n,
+                                                                 int metric, const uint8_t* __restrict__ skip,
+                                                                 double* __restrict__ mag, float* __restrict__ snorm,
+                                                                 uint32_t* __restrict__ special, uint32_t* special_cnt,
+                                                                 uint32_t* max_norm_bits) {
+  __shared__ T tile[WARPS][32][33];
+  const uint32_t warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const uint64_t warps_total = (uint64_t)gridDim.x * WARPS;
+  for (uint64_t base = ((uint64_t)blockIdx.x * WARPS + warp) * 32; base < n; base += warps_total * 32) {
+    const uint64_t r = base + lane;
+    const uint32_t my_row = r < n ? (uint32_t)r : NO_ROW;
+    double s = 0.0, l1 = 0.0, amax = 0.0;
+    bool bad = false;
+    warp_walk_rows<T>(rows, dim, my_row, tile[warp], [&](uint32_t, T x) {
+      const double xd = (double)x;
+      s = __dadd_rn(s, __dmul_rn(xd, xd));
+      const float f = (float)x;
+      bad |= !isfinite(f);
+      const double a = fabs((double)f);
+      l1 += a;
+      amax = fmax(amax, a);
+    });
+    if (my_row == NO_ROW) continue;
+    mag[r] = __dsqrt_rn(s);
+    float sn = 0.f;
+    if (skip && skip[r]) {
+      sn = __int_as_float(0x7fc00000);
+    } else if (bad) {
+      sn = __int_as_float(0x7fc00000);
+      const uint32_t pos = atomicAdd(special_cnt, 1u);
+      if (pos < (uint32_t)SPECIAL_CAP) special[pos] = (uint32_t)r;
+    } else {
+      // the f64 sum of dim f32 magnitudes errs by at most dim 2^-53 relative: (1 + 2^-30) covers it up to dim 2^23
+      const double nrm = metric == SDB_MANHATTAN ? l1 * (1.0 + 0x1p-30) : amax;
+      atomicMax(max_norm_bits, __float_as_uint(__double2float_ru(nrm)));
+    }
+    snorm[r] = sn;
+  }
+}
+
 // rows in [n, cap_pad) are TMA padding of the last screening tile: NaN norm => never a candidate
 __global__ void pad_snorm_kernel(float* __restrict__ snorm, uint64_t n, uint64_t n_pad) {
   const uint64_t i = n + (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -350,7 +397,16 @@ sdb_status corpus_finalize_device(Corpus* c) {
   }
   if (c->n) {
     const int grid = ctx->sm_count * 8;
-    if (c->dtype == SDB_F32)
+    if (c->metric == SDB_MANHATTAN || c->metric == SDB_CHEBYSHEV) {
+      if (c->dtype == SDB_F32)
+        finalize_lp_kernel<float, 8><<<grid, 256, 0, st>>>((const float*)c->d_rows.get(), c->dim, c->n, (int)c->metric,
+                                                           c->d_skip, c->d_mag, c->d_snorm, c->d_special, d_tmp,
+                                                           d_tmp + 1);
+      else
+        finalize_lp_kernel<double, 4><<<grid * 2, 128, 0, st>>>((const double*)c->d_rows.get(), c->dim, c->n,
+                                                                (int)c->metric, c->d_skip, c->d_mag, c->d_snorm,
+                                                                c->d_special, d_tmp, d_tmp + 1);
+    } else if (c->dtype == SDB_F32)
       finalize_rows_kernel<float, 8><<<grid, 256, 0, st>>>((const float*)c->d_rows.get(), c->dim, c->n, (int)c->metric,
                                                         c->d_skip, c->d_mag, c->d_snorm, c->d_special, d_tmp,
                                                         d_tmp + 1);

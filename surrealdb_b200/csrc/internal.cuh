@@ -421,8 +421,10 @@ struct Corpus : Scratch {
 sdb_status corpus_finalize_device(Corpus* c);
 sdb_status corpus_remove_device(Corpus* c, const uint64_t* h_ids, uint64_t n);
 sdb_status corpus_reapply_tombstones(Corpus* c, cudaStream_t st);
-// screen_simt.cu
+// screen_simt.cu (the SIMT_F32 screen; MANHATTAN / CHEBYSHEV corpora go to screen_lp_pass)
 sdb_status screen_simt_pass(Corpus* c, uint32_t nq, const PassDesc& p, cudaStream_t st);
+// screen_lp.cu: f32 L1 / L-infinity screen (score = -s~), f32 and f64 rows
+sdb_status screen_lp_pass(Corpus* c, uint32_t nq, const PassDesc& p, cudaStream_t st);
 // screen_tc.cu
 // mode 0: pass 0 (every score of the pass's tiles written to fixed slots), 1: threshold pass, 2: streaming pass with
 // in-kernel threshold refinement (histogram + refiner warp), 3: probe (chunk maxima of a few tiles, no candidates)
