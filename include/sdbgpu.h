@@ -498,8 +498,10 @@ sdb_status sdb_hnsw_select_device(sdb_hnsw*, const uint32_t* d_elem_ids, uint64_
  * row.  For every element: if it has <= m_max candidates all are taken, otherwise candidates are visited nearest-first
  * and e is accepted iff no already accepted r is closer to e than the element is (e_dist > dist(e,r) rejects), until
  * m_max are accepted.  presorted = 0: the candidates are first ordered by their distance to the element
- * (build_priority_list, layer.rs:389-405 -- the re-selection of an over-full node).  d_out: n x m_max member indices,
- * d_out_cnt: accepted count.  All pointers are device pointers. */
+ * (build_priority_list, layer.rs:389-405 -- the re-selection of an over-full node), equal distances in list order; a
+ * NaN distance (a zero row under cosine, a NaN or infinite element) comes after every number, NaNs in list order.  A
+ * NaN distance never rejects and is never rejected.  d_out: n x m_max member indices, d_out_cnt: accepted count.  All
+ * pointers are device pointers.  dim + kc > 7264 (more than 227 KB of shared memory per block): SDB_EUNSUPPORTED. */
 sdb_status sdb_hnsw_select_neighbors(sdb_ctx*, const float* d_vectors, uint32_t dim, sdb_metric, uint64_t row0, uint64_t n,
                                      const uint64_t* d_cand, const uint32_t* d_cand_cnt, uint32_t kc, uint32_t m_max,
                                      int presorted, uint32_t* d_out, uint32_t* d_out_cnt);

@@ -1533,10 +1533,16 @@ __global__ void __launch_bounds__(128) hnsw_select_kernel(const float* __restric
       if (lane == 0) s_d[j] = d;
     }
     __syncwarp();
+    // a total order, so that the ranks are a permutation: numbers by value, equal ones in list order; NaN (a zero
+    // row under cosine, a NaN or inf element) after every number and the self marker, NaNs in list order
     for (uint32_t j = lane; j < nc; j += 32) {
       const float dj = s_d[j];
+      const bool nj = dj != dj;
       uint32_t rank = 0;
-      for (uint32_t t = 0; t < nc; t++) rank += (s_d[t] < dj) || (s_d[t] == dj && t < j);
+      for (uint32_t t = 0; t < nc; t++) {
+        const float dt = s_d[t];
+        rank += (dt != dt) != nj ? nj : (dt < dj || ((dt == dj || nj) && t < j));
+      }
       s_ord[rank] = j;
     }
   }
@@ -2078,9 +2084,13 @@ static sdb_status select_neighbors(sdb_ctx* ctx, const float* d_vectors, uint32_
   if (!ctx || !d_vectors || !d_cand || !d_cand_cnt || !d_out || !d_out_cnt || !dim || !kc || !m_max) return SDB_EINVAL;
   if (metric != SDB_COSINE && metric != SDB_EUCLIDEAN) return SDB_EUNSUPPORTED;
   if (n == 0) return SDB_OK;
+  const size_t smem = sizeof(float) * (2 * (size_t)dim + 2 * kc) * 4;
+  if (smem > 227 * 1024) {  // the opt-in limit of dynamic shared memory per block
+    set_error("sdb_hnsw_select_neighbors: %zu bytes of shared memory per block needed (dimension + kc > 7264)", smem);
+    return SDB_EUNSUPPORTED;
+  }
   std::lock_guard<std::mutex> guard(ctx->mu);
   SDB_CUDA(cudaSetDevice(ctx->device));
-  const size_t smem = sizeof(float) * (2 * (size_t)dim + 2 * kc) * 4;
   auto kern = metric == SDB_COSINE ? hnsw_select_kernel<true> : hnsw_select_kernel<false>;
   SDB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   kern<<<(unsigned)((n + 3) / 4), 128, smem, ctx->stream>>>(d_vectors, dim, row0, n, d_elem_ids, d_cand, d_cand_cnt, kc, m_max, presorted, d_out, d_out_cnt);

@@ -11,7 +11,9 @@ data-parallel algorithm, so instead of porting it this builder works layer by la
     links early elements get in the incremental algorithm;
   * Heuristic::select (heuristic.rs:61-81,201-216) on the GPU (sdb_hnsw_select_neighbors) picks <= m_max of them;
   * every selected edge is mirrored (graph.rs:52-64) and a node that ends up with more than m_max edges is re-selected
-    among its own picks plus up to (rev_factor-1)*m_max reverse edges ordered by distance (layer.rs:362-378).
+    among its own picks plus up to (rev_factor-1)*m_max reverse edges ordered by distance (layer.rs:362-378);
+  * a candidate at a NaN distance (a zero row under cosine, a row with a NaN) is dropped before the selection, in every
+    builder: nothing links to such a row, because a NaN neighbour is never rejected and stalls the searches that meet it.
 
 The result is a valid input for the layer-walk kernel (the same CSR the reference's Hn records decode to).  It is NOT
 the graph the reference would have built, so parity claims apply to the walk on a given graph; quality is measured as
@@ -59,6 +61,24 @@ def _merge_reverse(fwd, cnt, m_max, cap=None):
     out = np.take_along_axis(allc, order2, axis=1)
     out_cnt = np.minimum(ok.sum(1), cap)
     return out, out_cnt
+
+
+def _drop_nan(cand, dist, cnt, also=None):
+    """candidate lists (CUDA (b, kc) ids and f64 distances, cnt valid entries per row) without the entries at a NaN
+    distance (a zero row under cosine, a row with a NaN) or marked in `also`, order kept -> (cand, cnt).  The selection
+    never rejects a NaN candidate (no comparison with NaN holds), and a linked one stops every search whose result set
+    fills up with it last (no distance is < NaN): such a row is left unlinked."""
+    import torch
+    kc = cand.shape[1]
+    pos = torch.arange(kc, device=cand.device)[None, :]
+    live = pos < cnt[:, None]
+    out = torch.isnan(dist) & live
+    if also is not None:
+        out |= also & live
+    elif not bool(out.any()):
+        return cand, cnt
+    cand = torch.gather(cand, 1, torch.argsort(pos + out.to(torch.int64) * kc, dim=1, stable=True)).contiguous()
+    return cand, (cnt - out.sum(1).to(cnt.dtype)).contiguous()
 
 
 VT_TORCH = {"F64": "float64", "F32": "float32", "I64": "int64", "I32": "int32", "I16": "int16"}
@@ -179,7 +199,8 @@ def _build_layers_typed(ctx, x, n, dim, metric, vector_type, minkowski_order, le
                 for b0 in range(seg_lo, seg_hi, batch):
                     b1 = min(seg_hi, b0 + batch)
                     q = x.index_select(0, mem_dev[b0:b1].to(torch.int64))
-                    ids, _, cnt = knn_exact(h, q, kc, mem_dev[:seg_hi])
+                    ids, dist, cnt = knn_exact(h, q, kc, mem_dev[:seg_hi])
+                    ids, cnt = _drop_nan(ids, dist, cnt)
                     if heuristic:
                         s_o, s_c = select(h, ids, cnt, k_nb, 1, elem_ids=mem_dev[b0:b1])
                         sel, sc = s_o.cpu().numpy().astype(np.int64), s_c.cpu().numpy().astype(np.int64)
@@ -279,15 +300,17 @@ def build_layers(ctx, vectors_dev, n, dim, metric="EUCLIDEAN", m=16, m0=32, seed
                 o_rv = o_r.view(-1)[: batch * kc].view(batch, kc)
                 o_dv = o_d.view(-1)[: batch * kc].view(batch, kc)
                 col.knn_device(q.data_ptr(), b1 - b0, kc, 0, o_rv.data_ptr(), o_dv.data_ptr(), o_c.data_ptr())
+                c_r, c_c = _drop_nan(o_rv[: b1 - b0], o_dv[: b1 - b0], o_c[: b1 - b0])
+                torch.cuda.current_stream().synchronize()
                 if heuristic:
                     L.check(L.lib().sdb_hnsw_select_neighbors(ctx.h, C.c_void_p(sub.data_ptr()), dim, L.METRIC[metric.upper()],
-                                                              b0, b1 - b0, C.c_void_p(o_rv.data_ptr()), C.c_void_p(o_c.data_ptr()),
+                                                              b0, b1 - b0, C.c_void_p(c_r.data_ptr()), C.c_void_p(c_c.data_ptr()),
                                                               kc, k_nb, 1, C.c_void_p(s_o.data_ptr()), C.c_void_p(s_c.data_ptr())))
                     nbrs[b0:b1] = s_o[: b1 - b0].cpu().numpy()
                     counts[b0:b1] = s_c[: b1 - b0].cpu().numpy()
                 else:
-                    r = o_rv[: b1 - b0].cpu().numpy()
-                    cnt = o_c[: b1 - b0].cpu().numpy().astype(np.int64)
+                    r = c_r.cpu().numpy()
+                    cnt = c_c.cpu().numpy().astype(np.int64)
                     valid = np.arange(kc)[None, :] < cnt[:, None]
                     keep = valid & (r != (b0 + np.arange(b1 - b0))[:, None])  # drop self, keep nearest-first order
                     order = np.argsort(~keep, axis=1, kind="stable")[:, :k_nb]
@@ -426,14 +449,11 @@ def build_incremental(ctx, x, metric="COSINE", m=16, m0=32, efc=150, seed=1, gro
                 L.check(L.lib().sdb_hnsw_search_device(h, C.c_void_p(x[lo + c0].data_ptr()), nqc, efc, efc,
                                                        C.c_void_p(cand.data_ptr()), C.c_void_p(cdist.data_ptr()),
                                                        C.c_void_p(ccnt.data_ptr())))
-                if drop_self:  # the element is part of the graph by now: take it out of its own candidate list (order kept)
-                    me = torch.arange(lo + c0, lo + c1, device=dev, dtype=torch.int64)[:, None]
-                    live = torch.arange(efc, device=dev)[None, :] < ccnt[:, None]
-                    is_me = (cand == me) & live
-                    key = torch.arange(efc, device=dev)[None, :] + is_me.to(torch.int64) * efc  # self goes last
-                    cand = torch.gather(cand, 1, torch.argsort(key, dim=1, stable=True)).contiguous()
-                    ccnt = (ccnt - is_me.sum(1).to(torch.int32)).contiguous()
-                    torch.cuda.synchronize()
+                # candidates at a NaN distance leave the list (_drop_nan); second pass: the element is part of the graph
+                # by now and leaves its own list too
+                me = torch.arange(lo + c0, lo + c1, device=dev, dtype=torch.int64)[:, None]
+                cand, ccnt = _drop_nan(cand, cdist, ccnt, (cand == me) if drop_self else None)
+                torch.cuda.synchronize()
                 if typed:
                     L.check(L.lib().sdb_hnsw_select_device(h, None, lo + c0, nqc, C.c_void_p(cand.data_ptr()),
                                                            C.c_void_p(ccnt.data_ptr()), efc, m0, 1,
