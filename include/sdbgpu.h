@@ -45,9 +45,10 @@ typedef enum {
 } sdb_status;
 
 /* catalog::Distance (catalog/schema/index.rs:247-284).  COSINE and EUCLIDEAN are screened on the tensor cores and
- * re-ranked exactly; MANHATTAN and CHEBYSHEV are screened by the f32 L1 / L-infinity SIMT screen (SDB_SCREEN_SIMT_F32)
- * and re-ranked exactly; HAMMING, JACCARD, MINKOWSKI and PEARSON run through the exact kernel (sequential f64,
- * Distance::compute op for op). */
+ * re-ranked exactly; PEARSON is screened on the tensor cores as the cosine of the rows and the query centred on their
+ * own means, and re-ranked exactly; MANHATTAN and CHEBYSHEV are screened by the f32 L1 / L-infinity SIMT screen
+ * (SDB_SCREEN_SIMT_F32) and re-ranked exactly; HAMMING, JACCARD and MINKOWSKI run through the exact kernel (sequential
+ * f64, Distance::compute op for op). */
 typedef enum {
   SDB_CHEBYSHEV = 0,
   SDB_COSINE = 1,
@@ -65,7 +66,9 @@ typedef enum {
  * tensor cores (F64: when the bf16 / int8 copies, 3 bytes per element, fit beside the rows at creation; otherwise the
  * corpus is ranked by the exact kernel alone).  The f32 SIMT screen of COSINE / EUCLIDEAN needs F32 rows: on F64 it
  * means the exact kernel.  MANHATTAN / CHEBYSHEV corpora of either type are screened by the f32 L1 / L-infinity screen
- * (f64 rows rounded to f32 as the screen reads them; rows with an element beyond f32 range are ranked exactly). */
+ * (f64 rows rounded to f32 as the screen reads them; rows with an element beyond f32 range are ranked exactly).
+ * PEARSON corpora of either type are screened on the tensor cores when the bf16 / int8 copies of the centred rows and
+ * 16 bytes of moments per row fit beside the rows at creation; otherwise the exact kernel ranks them. */
 typedef enum { SDB_F32 = 0, SDB_F64 = 1 } sdb_dtype;
 
 /* element type of an HNSW index: catalog::VectorType (catalog/schema/index.rs:321-335), numbered as the SerializedVector
@@ -79,13 +82,14 @@ typedef enum { SDB_VT_F64 = 0, SDB_VT_F32 = 1, SDB_VT_I64 = 2, SDB_VT_I32 = 3, S
  * proof fails climb to finer screens (bf16, then the f32 stream) before the exact kernel.  MANHATTAN / CHEBYSHEV corpora
  * (k <= 256) are screened by SDB_SCREEN_SIMT_F32 for AUTO and every TC request (4096, then 16384 candidates per query,
  * then the exact kernel), except that AUTO ranks a batch of one query with the exact kernel (faster for a single query);
- * NONE_EXACT keeps them on the exact kernel. */
+ * NONE_EXACT keeps them on the exact kernel.  PEARSON corpora (k <= 256) follow the cosine ladder on the centred rows
+ * (int8, then bf16, then the exact kernel; no f32 stream): SIMT_F32 and NONE_EXACT mean the exact kernel. */
 typedef enum {
   SDB_SCREEN_AUTO = 0,
   SDB_SCREEN_SIMT_F32 = 1,   /* f32 SIMT screen: streaming dot products; MANHATTAN / CHEBYSHEV: L1 / L-inf */
   SDB_SCREEN_TC_BF16 = 2,    /* wgmma bf16 operands, f32 accumulation                                    */
   SDB_SCREEN_NONE_EXACT = 3, /* no screen: exact f64 kernel for every query                              */
-  SDB_SCREEN_TC_INT8 = 4     /* wgmma s8, int8 copy         of the normalised rows (cosine); falls back to bf16 */
+  SDB_SCREEN_TC_INT8 = 4     /* wgmma s8, int8 copy of the normalised (pearson: centred) rows; falls back to bf16 */
 } sdb_screen;
 
 /* counters of the last brute-force call on a corpus (diagnostics / bench roofline arithmetic) */
@@ -133,16 +137,18 @@ sdb_status sdb_debug_schedule(uint64_t n_rows, uint32_t cand_cap, uint32_t k, ui
  * 256):
  *   out_f[4]    i8_scale, max_rel_qerr, bf16_rel_err, max_norm
  *   out_u[5]    n_special, n_outliers, dim_pad, dim_pad8, n_pad
- *   out_i8      [n_pad][dim_pad8] int8 copy of the normalised rows (cosine corpora only)
- *   out_bf16    [n_pad][dim_pad] bf16 copy (bit patterns)
- *   out_snorm   [n_pad] screening norm (cosine 1/|x|, euclidean |x|^2; NaN: never a screen candidate)
- *   out_special [n_special] rows ranked exactly on every query */
+ *   out_i8      [n_pad][dim_pad8] int8 copy of the normalised rows (cosine corpora; PEARSON: of dx / |dx|)
+ *   out_bf16    [n_pad][dim_pad] bf16 copy (bit patterns; PEARSON: of the centred rows dx = x - mean(x))
+ *   out_snorm   [n_pad] screening norm (cosine 1/|x|, euclidean |x|^2, pearson 1/|dx|; NaN: never a screen candidate)
+ *   out_special [n_special] rows ranked exactly on every query
+ * PEARSON corpora qualify when they hold their screen copies. */
 sdb_status sdb_debug_corpus_state(sdb_corpus*, float* out_f, uint32_t* out_u, int8_t* out_i8, uint16_t* out_bf16,
                                   float* out_snorm, uint32_t* out_special);
 /* sdb_debug_screen_batch: one batch of nq host queries screened with `screen` (TC_INT8, TC_BF16 or SIMT_F32) at the
  * first rung of the ladder, through the production sequence (streaming = 0: the multi-pass schedule), with exactly
  * cand_cap (>= 4096) candidate slots per query (F64 corpora with screen copies: TC_INT8 or TC_BF16 only; MANHATTAN / CHEBYSHEV corpora, F32 or F64: SIMT_F32, where
- * beps bounds |s~ - d| and the score is -s~).  The ladder
+ * beps bounds |s~ - d| and the score is -s~; PEARSON corpora with screen copies, F32 or F64: TC_INT8 or TC_BF16, where
+ * the scores are those of the unit query -dq/|dq| against dx, qmag is 1 and the proof adds eps_ref).  The ladder
  * and the exact fallback do not run: flags are as the batch
  * left them.  score_all != 0 instead runs one pass-0 launch over every tile (SIMT: tau = -inf) with max(cand_cap,
  * n_pad) slots and selects nothing: out_a then holds every score of that kernel, and out_b / out_rr are untouched.
@@ -252,7 +258,7 @@ sdb_status sdb_knn_wait(sdb_corpus*, uint32_t ticket);
  * metric, F32 and F64, k <= 4096, cancellation, sdb_knn_last_stats, up to 4 tickets in flight (filtered and unfiltered
  * mixed), completion through sdb_knn_wait.  SDB_EINVAL: n_filters == 0 with nq > 0, filters == NULL, or an index >=
  * n_filters.
- * A query whose bitmap has at most 4096 set bits (COSINE, EUCLIDEAN, MANHATTAN, CHEBYSHEV; k <= 256) skips the screen
+ * A query whose bitmap has at most 4096 set bits (COSINE, EUCLIDEAN, MANHATTAN, CHEBYSHEV, PEARSON; k <= 256) skips the screen
  * (its passing rows are ranked directly; results are
  * the same); sdb_knn_last_stats then reports screen_used = SDB_SCREEN_NONE_EXACT and n_passes = 0 for a batch of such
  * queries only.

@@ -101,7 +101,9 @@ struct Rung {
 // to more than a handful of queries the batch is re-screened with a tighter screen / longer lists instead of paying
 // one exact pass over the corpus per failed query; the rung that worked is remembered per corpus and k.
 static std::vector<Rung> build_rungs(Corpus* c, uint32_t k, uint32_t nq, sdb_screen* first) {
-  const bool int8_ok = c->d_i8 && c->metric == SDB_COSINE && screen_tc_available();
+  // PEARSON: the cosine screens on the centred rows when the corpus holds their copies and moments (sdb_corpus_create)
+  const bool pearson = c->metric == SDB_PEARSON && c->d_mom;
+  const bool int8_ok = c->d_i8 && (c->metric == SDB_COSINE || pearson) && screen_tc_available();
   sdb_screen scr = c->screen;
   if (scr == SDB_SCREEN_AUTO)
     scr = !screen_tc_available() ? SDB_SCREEN_SIMT_F32
@@ -110,9 +112,10 @@ static std::vector<Rung> build_rungs(Corpus* c, uint32_t k, uint32_t nq, sdb_scr
   if (scr == SDB_SCREEN_TC_BF16 && (!screen_tc_available() || !c->d_bf16)) scr = SDB_SCREEN_SIMT_F32;
   // MANHATTAN / CHEBYSHEV: the f32 L1 / L-infinity screen (screen_lp.cu) is their only screen, for f32 and f64 rows
   const bool lp = c->metric == SDB_MANHATTAN || c->metric == SDB_CHEBYSHEV;
-  const bool screenable = c->metric == SDB_COSINE || c->metric == SDB_EUCLIDEAN || lp;
-  // the SIMT screen streams f32 rows: an f64 cosine / euclidean corpus is screened on the tensor cores or not at all
-  if (c->dtype == SDB_F64 && scr == SDB_SCREEN_SIMT_F32 && !lp) scr = SDB_SCREEN_NONE_EXACT;
+  const bool screenable = c->metric == SDB_COSINE || c->metric == SDB_EUCLIDEAN || lp || pearson;
+  // the SIMT screen streams f32 rows: an f64 cosine / euclidean corpus is screened on the tensor cores or not at all,
+  // and so is a PEARSON one of either type (the SIMT screen would need the centred rows)
+  if ((c->dtype == SDB_F64 || pearson) && scr == SDB_SCREEN_SIMT_F32 && !lp) scr = SDB_SCREEN_NONE_EXACT;
   if (c->special_overflow || k > 256 || !screenable) scr = SDB_SCREEN_NONE_EXACT;
   // a single query streams the rows once either way, and the exact kernel does it at the higher HBM rate (DESIGN.md
   // section 5): AUTO ranks it there; an explicit SIMT_F32 request is kept
@@ -126,7 +129,8 @@ static std::vector<Rung> build_rungs(Corpus* c, uint32_t k, uint32_t nq, sdb_scr
   else if (scr == SDB_SCREEN_SIMT_F32) r = {{SDB_SCREEN_SIMT_F32, 4096}};
   // the f32 stream (error bound ~500x tighter than bf16) as the last rung before the exact kernel -- only ever used
   // for the few queries of a batch that every tensor-core rung failed to prove (finish_local), never for a whole batch
-  if (!r.empty() && r.back().scr != SDB_SCREEN_SIMT_F32 && c->dtype == SDB_F32) r.push_back({SDB_SCREEN_SIMT_F32, 4096});
+  if (!r.empty() && r.back().scr != SDB_SCREEN_SIMT_F32 && c->dtype == SDB_F32 && !pearson)
+    r.push_back({SDB_SCREEN_SIMT_F32, 4096});
   return r;
 }
 static uint32_t n_batch_rungs(const std::vector<Rung>& r) {  // rungs a WHOLE batch may be re-screened on
@@ -643,11 +647,11 @@ static sdb_status submit_locked(Corpus* c, Ticket* t, const double* d_queries, u
     t->filt.bits = d_filters;
     t->filt.words = (uint32_t)((c->n + 31) / 32);
     // direct regime: a query whose filter passes at most DIRECT_MAX_ROWS rows (filter_rows: set bits, an upper bound
-    // of the rows it passes) skips the screen; the re-rank and cand_final serve the four screenable metrics, k <= 256
+    // of the rows it passes) skips the screen; the re-rank and cand_final serve the five screenable metrics, k <= 256
     std::vector<uint32_t> scr, dir;
     const bool direct_ok = filter_rows && k > 0 && k <= 256 &&
                            (c->metric == SDB_COSINE || c->metric == SDB_EUCLIDEAN || c->metric == SDB_MANHATTAN ||
-                            c->metric == SDB_CHEBYSHEV);
+                            c->metric == SDB_CHEBYSHEV || (c->metric == SDB_PEARSON && c->d_mom));
     for (uint32_t q = 0; q < nq; q++) {
       const uint64_t rows_q = filter_rows ? filter_rows[t->h_qf[q]] : ~0ull;
       if (direct_ok && rows_q <= DIRECT_MAX_ROWS) dir.push_back(q);
@@ -1049,7 +1053,8 @@ sdb_status sdb_corpus_create(sdb_ctx* ctx, uint32_t dim, sdb_dtype dt, sdb_metri
     return SDB_EINVAL;
   }
   // COSINE / EUCLIDEAN: screened (K1/K2) + exact re-rank.  MANHATTAN / CHEBYSHEV: the f32 L1 / L-infinity screen
-  // (screen_lp.cu) + exact re-rank.  HAMMING / PEARSON / JACCARD / MINKOWSKI: served by the exact kernel alone (sequential f64, Distance::compute op for op).  MINKOWSKI goes through
+  // (screen_lp.cu) + exact re-rank.  PEARSON: the cosine tensor-core screens on the centred rows + exact re-rank.
+  // HAMMING / JACCARD / MINKOWSKI: served by the exact kernel alone (sequential f64, Distance::compute op for op).  MINKOWSKI goes through
   // pow(), which CUDA's libm and Rust's (the platform libm) implement separately: within 1 ulp of each other per term,
   // so its distances are compared with a 1e-12 relative tolerance instead of bit equality (tests/test_gpu_knn.py).
   const bool screenable = m == SDB_COSINE || m == SDB_EUCLIDEAN;
@@ -1087,6 +1092,18 @@ sdb_status sdb_corpus_create(sdb_ctx* ctx, uint32_t dim, sdb_dtype dt, sdb_metri
     if (e2 != cudaSuccess) {
       c->d_bf16.reset();
       c->d_i8.reset();
+    }
+  }
+  // PEARSON (f32 and f64 rows): the cosine screens run on the centred rows, which takes the bf16 and int8 copies and
+  // 16 bytes of moments per row -- again only when they fit
+  if (m == SDB_PEARSON) {
+    cudaError_t e2 = c->d_bf16.reserve(cap_pad * c->dim_pad);
+    if (e2 == cudaSuccess) e2 = c->d_i8.reserve((size_t)cap_pad * c->dim_pad8);
+    if (e2 == cudaSuccess) e2 = c->d_mom.reserve(cap);
+    if (e2 != cudaSuccess) {
+      c->d_bf16.reset();
+      c->d_i8.reset();
+      c->d_mom.reset();
     }
   }
   *out = c;
@@ -1360,8 +1377,10 @@ sdb_status sdb_debug_corpus_state(sdb_corpus* c, float* out_f, uint32_t* out_u, 
   if (!c) return SDB_EINVAL;
   std::lock_guard<std::mutex> g(c->mu);
   const bool lp = c->metric == SDB_MANHATTAN || c->metric == SDB_CHEBYSHEV;
-  if (!c->finalized || (c->dtype != SDB_F32 && !c->d_bf16 && !lp) || (out_i8 && !c->d_i8) || (out_bf16 && !c->d_bf16)) {
-    set_error("sdb_debug_corpus_state: needs a finalized F32 corpus or a screened F64 one (int8 copy: cosine only)");
+  if (!c->finalized || (c->dtype != SDB_F32 && !c->d_bf16 && !lp) || (c->metric == SDB_PEARSON && !c->d_mom) ||
+      (out_i8 && !c->d_i8) || (out_bf16 && !c->d_bf16)) {
+    set_error("sdb_debug_corpus_state: needs a finalized F32 corpus or a screened F64 / PEARSON one (int8 copy: "
+              "cosine and pearson only)");
     return SDB_EINVAL;
   }
   SDB_CUDA(cudaSetDevice(c->ctx->device));
@@ -1406,11 +1425,14 @@ sdb_status sdb_debug_screen_batch(sdb_corpus* c, const double* queries, uint32_t
   const bool lp = (c->metric == SDB_MANHATTAN || c->metric == SDB_CHEBYSHEV) && screen == SDB_SCREEN_SIMT_F32;
   // f64 rows: tensor-core screens only (cosine / euclidean)
   const bool f64_ok = c->dtype == SDB_F64 && ((tc && c->d_bf16) || lp);
+  // PEARSON (f32 and f64 rows): the cosine tensor-core screens on the centred rows
+  const bool pearson = c->metric == SDB_PEARSON && c->d_mom && tc;
   if (!c->finalized || (c->dtype != SDB_F32 && !f64_ok) ||
-      (c->metric != SDB_COSINE && c->metric != SDB_EUCLIDEAN && !lp) || (int8 && !c->d_i8) || c->special_overflow ||
-      !c->n) {
+      (c->metric != SDB_COSINE && c->metric != SDB_EUCLIDEAN && !lp && !pearson) ||
+      (c->metric == SDB_PEARSON && !pearson) || (int8 && !c->d_i8) || c->special_overflow || !c->n) {
     set_error("sdb_debug_screen_batch: needs a finalized, non-empty F32 cosine / euclidean corpus, an F64 one with "
-              "screen copies and a tensor-core screen (int8: cosine), or a MANHATTAN / CHEBYSHEV one with SIMT_F32");
+              "screen copies and a tensor-core screen (int8: cosine), a PEARSON one with screen copies and a "
+              "tensor-core screen, or a MANHATTAN / CHEBYSHEV one with SIMT_F32");
     return SDB_EINVAL;
   }
   Ctx* ctx = c->ctx;

@@ -12,6 +12,9 @@
 
 namespace sdb {
 
+// PEARSON corpora that hold the centred screen copies and the row moments (sdb_corpus_create reserves them if they fit)
+static bool pearson_screened(const Corpus* c) { return c->metric == SDB_PEARSON && c->d_mom; }
+
 // ------------------------------------------------------------------------------------------------
 __global__ void prep_queries_kernel(const double* __restrict__ q64, uint32_t dim, uint32_t dim_pad, int metric,
                                     float* __restrict__ q32, __nv_bfloat16* __restrict__ qbf, double* __restrict__ qmag,
@@ -61,6 +64,74 @@ __global__ void prep_queries_kernel(const double* __restrict__ q64, uint32_t dim
     qflags[q] = f;
     // |q - bf16(q)| / |q|, rounded up; + 2^-23 for the f64 -> f32 rounding of the query itself
     if (qbferr) qbferr[q] = (m > 0.0 && isfinite(m)) ? (sqrtf(s_err2) / (float)m) * 1.0001f + 2.4e-7f : 1.f;
+  }
+}
+
+// PEARSON: the query's mean m2 and S2 = sum (q_i - m2)^2 in the exact kernel's arithmetic (sequential f64), then the
+// screen copies of the NEGATED centred query scaled to unit norm, -dq / |dq| with dq_i = q_i - m2 and |dq| = sqrt(S2)
+// in f64: the cosine screens score cos(dx, -dq), which is largest for the smallest pearson (DESIGN.md section 2).  The
+// unit norm keeps every f32 product and partial sum of the screens and of stage B below |dx| <= 2^126 (no overflow
+// for rows of any magnitude) and, for the screened rows' |dx| >= 2^-100, far above the f32 underflow.  q64 keeps the
+// raw query (exact kernel, re-rank); qmag = 1, the norm of the screens' query.  The exact kernel takes a query that is
+// constant (S2 = 0), not finite, has an element of dq beyond f32 range, or whose |dq| is below 2^-100 or not a normal
+// f32 -- the rules of the rows (finalize_pearson_kernel).
+__global__ void prep_queries_pearson_kernel(const double* __restrict__ q64, uint32_t dim, uint32_t dim_pad,
+                                            float* __restrict__ q32, __nv_bfloat16* __restrict__ qbf,
+                                            double* __restrict__ qmag, double2* __restrict__ qmom,
+                                            uint32_t* __restrict__ qflags, float* __restrict__ qbferr, uint32_t nq) {
+  const uint32_t q = blockIdx.x;
+  __shared__ uint32_t s_flags;
+  __shared__ float s_err2;
+  __shared__ double s_m2, s_nrm;
+  if (threadIdx.x == 0) {
+    s_flags = 0;
+    s_err2 = 0.f;
+    double s = 0.0, s2 = 0.0;
+    if (q < nq) {
+      for (uint32_t c = 0; c < dim; c++) s = __dadd_rn(s, q64[(size_t)q * dim + c]);
+      const double m2 = __ddiv_rn(s, (double)dim);
+      for (uint32_t c = 0; c < dim; c++) {  // ExactAcc::pearson_step's acc2, as exact_keys_kernel's deviation
+        const double d = __dsub_rn(q64[(size_t)q * dim + c], m2);
+        s2 = __dadd_rn(s2, __dmul_rn(d, d));
+      }
+      qmom[q] = make_double2(m2, s2);
+      s_m2 = m2;
+    }
+    s_nrm = __dsqrt_rn(s2);
+  }
+  __syncthreads();
+  const double m2 = s_m2, nrm = s_nrm;
+  uint32_t fl = 0;
+  float err2 = 0.f;
+  if (q < nq) {
+    for (uint32_t c = threadIdx.x; c < dim_pad; c += blockDim.x) {
+      const double x = c < dim ? q64[(size_t)q * dim + c] : 0.0;
+      const double dq = c < dim ? __dsub_rn(x, m2) : 0.0;
+      const float f = (float)__ddiv_rn(-dq, nrm);
+      if (c < dim) q32[(size_t)q * dim + c] = f;
+      const __nv_bfloat16 h = __float2bfloat16_rn(f);
+      qbf[(size_t)q * dim_pad + c] = h;
+      const float d = f - __bfloat162float(h);
+      if (d == d) err2 = fmaf(d, d, err2);
+      if (x != x) fl |= 3u;                           // NaN input: exact path, positive-NaN propagation
+      else if (!isfinite((float)dq) || f != f) fl |= 1u;  // inf, or dq beyond f32 range
+    }
+  } else {  // padding queries of the bf16 operand tile
+    for (uint32_t c = threadIdx.x; c < dim_pad; c += blockDim.x) qbf[(size_t)q * dim_pad + c] = __float2bfloat16_rn(0.f);
+  }
+  if (fl) atomicOr(&s_flags, fl);
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) err2 += __shfl_xor_sync(0xffffffffu, err2, o);
+  if ((threadIdx.x & 31) == 0 && err2 > 0.f) atomicAdd(&s_err2, err2);
+  __syncthreads();
+  if (threadIdx.x == 0 && q < nq) {
+    qmag[q] = 1.0;
+    uint32_t f = s_flags;
+    const float mf = (float)nrm;
+    if (!(nrm > 0.0) || !isfinite(nrm) || nrm < 0x1p-100 || !(mf >= 1.17549435e-38f && mf <= 3.40282347e38f)) f |= 1u;
+    qflags[q] = f;
+    // |q^ - bf16(q^)| for the unit query, rounded up; + 2^-23 for its f64 -> f32 rounding (and the f64 division)
+    qbferr[q] = (f & 1u) ? 1.f : sqrtf(s_err2) * 1.0001f + 2.4e-7f;
   }
 }
 
@@ -275,6 +346,19 @@ __global__ void __launch_bounds__(128) cand_begin_lp_kernel(float* __restrict__ 
 static bool lp_metric(const Corpus* c) { return c->metric == SDB_MANHATTAN || c->metric == SDB_CHEBYSHEV; }
 
 sdb_status cand_begin(Corpus* c, uint32_t nq, int screen, cudaStream_t st) {
+  if (pearson_screened(c)) {
+    // the cosine bounds of the centred operands with the F64 terms (the rows are centred in f64, whatever their type);
+    // the gap between their cosine and the reference's pearson is cand_final's eps_ref
+    cand_begin_kernel<<<(nq + 255) / 256, 256, 0, st>>>(c->d_tau, c->d_cand_cnt, c->d_flags, c->d_stat, c->d_bscale,
+                                                        c->d_beps, c->d_margin, c->d_margin2, c->d_beps2, c->d_tau2,
+                                                        c->d_qlow, c->d_qcap, c->d_qmag, c->d_q8scale, c->d_q8err,
+                                                        c->d_qbferr, nq, screen, (int)SDB_COSINE, c->dim,
+                                                        c->max_rel_qerr, c->i8_scale, c->bf16_rel_err, c->max_norm,
+                                                        c->exact ? 1 : 0, 1);
+    count_launch(c->ctx);
+    SDB_CUDA(cudaGetLastError());
+    return SDB_OK;
+  }
   if (lp_metric(c)) {
     cand_begin_lp_kernel<<<(nq + 3) / 4, 128, 0, st>>>(c->d_tau, c->d_cand_cnt, c->d_flags, c->d_stat, c->d_bscale,
                                                        c->d_beps, c->d_margin, c->d_margin2, c->d_beps2, c->d_tau2,
@@ -308,6 +392,7 @@ static sdb_status ensure_scratch(Corpus* c, uint32_t nq, uint32_t cap) {
     SDB_CUDA(s.d_q32.reserve((size_t)nqa * c->dim));
     SDB_CUDA(s.d_qbf16.reserve((size_t)nqa * c->dim_pad));
     SDB_CUDA(s.d_qmag.reserve(nqa));
+    if (pearson_screened(c)) SDB_CUDA(s.d_qmom.reserve(nqa));
     SDB_CUDA(s.d_qflags.reserve(nqa));
     SDB_CUDA(s.d_qbferr.reserve(nqa));
     SDB_CUDA(s.d_tau.reserve(nqa));
@@ -355,8 +440,12 @@ sdb_status prep_queries(Corpus* c, const double* d_queries, uint32_t nq, cudaStr
   if (d_queries != c->d_q64)
     SDB_CUDA(cudaMemcpyAsync(c->d_q64, d_queries, sizeof(double) * (size_t)nq * c->dim, cudaMemcpyDeviceToDevice, st));
   const uint32_t nq_pad = (nq + 127) / 128 * 128;
-  prep_queries_kernel<<<nq_pad, 128, 0, st>>>(c->d_q64, c->dim, c->dim_pad, (int)c->metric, c->d_q32, c->d_qbf16,
-                                              c->d_qmag, c->d_qflags, c->d_qbferr, nq);
+  if (pearson_screened(c))
+    prep_queries_pearson_kernel<<<nq_pad, 128, 0, st>>>(c->d_q64, c->dim, c->dim_pad, c->d_q32, c->d_qbf16, c->d_qmag,
+                                                        c->d_qmom, c->d_qflags, c->d_qbferr, nq);
+  else
+    prep_queries_kernel<<<nq_pad, 128, 0, st>>>(c->d_q64, c->dim, c->dim_pad, (int)c->metric, c->d_q32, c->d_qbf16,
+                                                c->d_qmag, c->d_qflags, c->d_qbferr, nq);
   count_launch(c->ctx);
   if (c->d_i8) {
     prep_queries_i8_kernel<<<nq_pad, 128, 0, st>>>(c->d_q32, c->d_qmag, c->dim, c->dim_pad8, nq, c->d_q8, c->d_q8scale,
@@ -746,11 +835,16 @@ sdb_status cand_select(Corpus* c, uint32_t nq, uint32_t k, bool drop_invalid, ui
 // near-ties, and only those reach the f64 kernel.
 // f64 rows: gathered as f64 (16-byte loads when the row length is even) and rounded to f32 element by element before
 // the same FMA chain; no f32 copy of the corpus is kept (cand_begin_kernel adds the rounding to beps2).
-template <typename T, bool COSINE>
+// CENTRED (PEARSON, f32 and f64 rows): every element is centred in f64 with the row's own mean and then rounded to f32,
+// fl32(x_i - m1), against the f32 copy of -dq: the rounding is relative per element, as for f64 cosine rows, so the
+// same stage-B bound holds for dx.  (Subtracting fl32(m1) in f32 would err by 2^-24 |m1| per element, absolutely:
+// unbounded relative to |dx| for rows whose offset dwarfs their spread.)
+template <typename T, bool COSINE, bool CENTRED = false>
 __global__ void __launch_bounds__(128) cand_refine_f32_kernel(const T* __restrict__ rows, uint32_t dim,
                                                                const float* __restrict__ snorm,
                                                                const float* __restrict__ q32, Cand* __restrict__ cand,
-                                                               const uint32_t* __restrict__ cnt, uint32_t cap) {
+                                                               const uint32_t* __restrict__ cnt, uint32_t cap,
+                                                               const double2* __restrict__ mom) {
   const uint32_t q = blockIdx.x, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const uint32_t n_c = cnt[q] < cap ? cnt[q] : cap;
   const float* qv = q32 + (size_t)q * dim;
@@ -764,7 +858,14 @@ __global__ void __launch_bounds__(128) cand_refine_f32_kernel(const T* __restric
     const T* x0 = rows + (size_t)r0 * dim;
     const T* x1 = rows + (size_t)r1 * dim;
     float a0 = 0.f, a1 = 0.f;
-    if constexpr (std::is_same<T, double>::value) {
+    if constexpr (CENTRED) {
+      const double m0 = __ldg(&mom[r0].x), m1 = __ldg(&mom[r1].x);
+      for (uint32_t c = lane; c < dim; c += 32) {
+        const float w = __ldg(qv + c);
+        a0 = fmaf(__double2float_rn(__dsub_rn((double)__ldg(x0 + c), m0)), w, a0);
+        a1 = fmaf(__double2float_rn(__dsub_rn((double)__ldg(x1 + c), m1)), w, a1);
+      }
+    } else if constexpr (std::is_same<T, double>::value) {
       if ((dim & 1u) == 0) {
 #pragma unroll 2
         for (uint32_t c = lane * 2; c < dim; c += 64) {
@@ -815,18 +916,24 @@ sdb_status cand_refine(Corpus* c, uint32_t nq, cudaStream_t st) {
   const dim3 grid(nq, 8);  // 128-thread blocks (register budget beside a resident screen CTA)
   const float* f32_rows = (const float*)c->d_rows.get();
   const double* f64_rows = (const double*)c->d_rows.get();
-  if (c->dtype == SDB_F32 && c->metric == SDB_COSINE)
+  if (pearson_screened(c) && c->dtype == SDB_F32)
+    cand_refine_f32_kernel<float, true, true><<<grid, 128, 0, st>>>(f32_rows, c->dim, c->d_snorm, c->d_q32, c->d_cand,
+                                                                    c->d_cand_cnt, c->sc_cap, c->d_mom);
+  else if (pearson_screened(c))
+    cand_refine_f32_kernel<double, true, true><<<grid, 128, 0, st>>>(f64_rows, c->dim, c->d_snorm, c->d_q32, c->d_cand,
+                                                                     c->d_cand_cnt, c->sc_cap, c->d_mom);
+  else if (c->dtype == SDB_F32 && c->metric == SDB_COSINE)
     cand_refine_f32_kernel<float, true><<<grid, 128, 0, st>>>(f32_rows, c->dim, c->d_snorm, c->d_q32, c->d_cand,
-                                                              c->d_cand_cnt, c->sc_cap);
+                                                              c->d_cand_cnt, c->sc_cap, nullptr);
   else if (c->dtype == SDB_F32)
     cand_refine_f32_kernel<float, false><<<grid, 128, 0, st>>>(f32_rows, c->dim, c->d_snorm, c->d_q32, c->d_cand,
-                                                               c->d_cand_cnt, c->sc_cap);
+                                                               c->d_cand_cnt, c->sc_cap, nullptr);
   else if (c->metric == SDB_COSINE)
     cand_refine_f32_kernel<double, true><<<grid, 128, 0, st>>>(f64_rows, c->dim, c->d_snorm, c->d_q32, c->d_cand,
-                                                               c->d_cand_cnt, c->sc_cap);
+                                                               c->d_cand_cnt, c->sc_cap, nullptr);
   else
     cand_refine_f32_kernel<double, false><<<grid, 128, 0, st>>>(f64_rows, c->dim, c->d_snorm, c->d_q32, c->d_cand,
-                                                                c->d_cand_cnt, c->sc_cap);
+                                                                c->d_cand_cnt, c->sc_cap, nullptr);
   count_launch(c->ctx);
   SDB_CUDA(cudaGetLastError());
   return SDB_OK;
@@ -1104,6 +1211,44 @@ __global__ void __launch_bounds__(128) cand_rerank_lp_kernel(
     rr_row[o] = my_row;
   }
 }
+// PEARSON re-rank: exact_keys_kernel's two passes in one, from the stored means -- pass A's m1 = mom[row].x (finalize)
+// and the query's m2 (prep_queries_pearson_kernel) -- then one chain covar = sum (x_i - m1)(q_i - m2) in
+// ExactAcc::pearson_step, and pass B's finish with S1 = mom[row].y and S2, which are that kernel's deviation sums
+// bit for bit.  nan_in: a NaN element of the row (pass A's rule) or of the query; a row holding +inf and -inf has a
+// generated NaN mean and sorts first.  Special rows (constant ones included) go through here too.
+template <typename T>
+__global__ void __launch_bounds__(128) cand_rerank_pearson_kernel(
+    const T* __restrict__ rows, uint32_t dim, const double2* __restrict__ mom, const double* __restrict__ q64,
+    const double2* __restrict__ qmom, const uint32_t* __restrict__ qflags, const Cand* __restrict__ cand,
+    const uint32_t* __restrict__ cnt, uint32_t cap, const uint32_t* __restrict__ special, uint32_t n_special,
+    uint64_t* __restrict__ rr_key, double* __restrict__ rr_dist, uint32_t* __restrict__ rr_row, uint32_t rr_stride) {
+  const uint32_t q = blockIdx.x;
+  const uint32_t n_c = cnt[q] < cap ? cnt[q] : cap;
+  const uint32_t n_e = n_c + n_special;
+  const bool q_nan = (qflags[q] & 2u) != 0;
+  const double* qv = q64 + (size_t)q * dim;
+  const double2 qm = qmom[q];
+  const double sd2 = dim == 1 ? 0.0 : __dsqrt_rn(__ddiv_rn(qm.y, (double)dim));
+  for (uint32_t e = blockIdx.y * blockDim.x + threadIdx.x; e < n_e; e += gridDim.y * blockDim.x) {
+    const uint32_t my_row = e < n_c ? cand[(size_t)q * cap + e].row : special[e - n_c];
+    const T* x = rows + (size_t)my_row * dim;
+    const double2 rm = mom[my_row];
+    ExactAcc acc;
+    for (uint32_t j = 0; j < dim; j++) {
+      const double xd = (double)__ldg(x + j);
+      acc.nan_in |= (xd != xd);
+      acc.pearson_step(xd, __ldg(qv + j), rm.x, qm.x);
+    }
+    const double covar = __ddiv_rn(acc.acc, (double)dim);
+    const double sd1 = dim == 1 ? 0.0 : __dsqrt_rn(__ddiv_rn(rm.y, (double)dim));
+    const double d = canon_nan(__ddiv_rn(covar, __dmul_rn(sd1, sd2)), acc.nan_in || q_nan);
+    const size_t o = (size_t)q * rr_stride + e;
+    rr_key[o] = dist_key(d);
+    rr_dist[o] = d;
+    rr_row[o] = my_row;
+  }
+}
+
 template <typename T>
 static void launch_rerank_lp(Corpus* c, uint32_t nq, uint32_t n_sp, cudaStream_t st) {
   const dim3 grid(nq, RR_GROUPS_Y);
@@ -1118,6 +1263,22 @@ sdb_status cand_rerank(Corpus* c, uint32_t nq, cudaStream_t st, bool small_sets)
     const uint32_t n_sp = c->filt.bits ? 0u : c->n_special;
     if (c->dtype == SDB_F32) launch_rerank_lp<float>(c, nq, n_sp, st);
     else launch_rerank_lp<double>(c, nq, n_sp, st);
+    count_launch(c->ctx);
+    SDB_CUDA(cudaGetLastError());
+    return SDB_OK;
+  }
+  if (pearson_screened(c)) {  // one kernel for small (after stage B) and large (direct regime, no stage B) sets
+    const uint32_t n_sp = c->filt.bits ? 0u : c->n_special;
+    if (c->dtype == SDB_F32)
+      cand_rerank_pearson_kernel<float><<<grid, 128, 0, st>>>((const float*)c->d_rows.get(), c->dim, c->d_mom, c->d_q64,
+                                                              c->d_qmom, c->d_qflags, c->d_cand, c->d_cand_cnt,
+                                                              c->sc_cap, c->d_special, n_sp, c->d_rr_key, c->d_rr_dist,
+                                                              c->d_rr_row, c->rr_stride);
+    else
+      cand_rerank_pearson_kernel<double><<<grid, 128, 0, st>>>((const double*)c->d_rows.get(), c->dim, c->d_mom,
+                                                               c->d_q64, c->d_qmom, c->d_qflags, c->d_cand,
+                                                               c->d_cand_cnt, c->sc_cap, c->d_special, n_sp,
+                                                               c->d_rr_key, c->d_rr_dist, c->d_rr_row, c->rr_stride);
     count_launch(c->ctx);
     SDB_CUDA(cudaGetLastError());
     return SDB_OK;
@@ -1208,8 +1369,10 @@ __device__ __forceinline__ void bitonic_pairs(uint64_t* s_key, uint64_t* s_idx, 
       uint32_t *__restrict__ flags, const uint32_t *__restrict__ qflags, uint32_t *__restrict__ stat, int metric,      \
       uint32_t k, uint64_t row_base, uint64_t *__restrict__ out_rows, double *__restrict__ out_dist,                   \
       uint32_t *__restrict__ out_count, int debug
-template <bool LP>
-__device__ __forceinline__ void cand_final_body(SDB_FINAL_PARAMS) {
+// PEARSON: the cosine proof on the centred operands (cand_final_pearson_kernel), eps_ref = the gap between their cosine
+// and the reference's pearson (DESIGN.md section 2)
+template <bool LP, bool PEARSON = false>
+__device__ __forceinline__ void cand_final_body(SDB_FINAL_PARAMS, double eps_ref = 0.0) {
   __shared__ uint64_t s_key[FIN_WIN];  // distance key
   __shared__ uint64_t s_idx[FIN_WIN];  // (row << 32 | entry): secondary order by row (unique), entry = index into rr_*
   const uint32_t q = blockIdx.x;
@@ -1267,6 +1430,13 @@ __device__ __forceinline__ void cand_final_body(SDB_FINAL_PARAMS) {
         // the top k if that bound (rounded down) is strictly above the k-th exact key.  No stage B ran (tau2 = -inf).
         const double L = (-(double)t - (double)beps[q]) * (1.0 - 1e-12);
         ok = dist_key(L) > kth;
+      } else if (PEARSON) {
+        // the screen scored s = cos(dx, -dq) |dq| / bscale.  Non-candidate: score <= tau  =>  cos(dx, dq) >= -tau
+        // bscale / |dq| - beps  =>  pearson >= -tau bscale / |dq| - beps - eps_ref, evaluated with directed rounding
+        // so that the bound itself is rounded down
+        const double a = __ddiv_ru(__dmul_ru((double)t, (double)bscale[q]), qm);
+        const double L = __dsub_rd(__dsub_rd(-a, (double)beps[q]), eps_ref);
+        ok = dist_key(L) > kth;
       } else if (metric == SDB_COSINE) {
         // non-candidate: score <= tau  =>  sim <= tau * bscale / |q| + eps  =>  dist >= 1 - tau * bscale / |q| - eps
         const double bound = 1.0 - (double)t * (double)bscale[q] / qm - (double)beps[q] - 1e-9;
@@ -1279,7 +1449,10 @@ __device__ __forceinline__ void cand_final_body(SDB_FINAL_PARAMS) {
       // stage B dropped candidates whose f32 score is below tau2: the same proof with the f32 bound
       const float t2 = tau2[q];
       if (ok && t2 > __int_as_float(0xff800000)) {
-        if (metric == SDB_COSINE) {
+        if (PEARSON) {  // stage B scores in the same units with bscale 1
+          const double L2 = __dsub_rd(__dsub_rd(-__ddiv_ru((double)t2, qm), (double)beps2[q]), eps_ref);
+          ok = dist_key(L2) > kth;
+        } else if (metric == SDB_COSINE) {
           const double bound2 = 1.0 - (double)t2 / qm - (double)beps2[q] - 1e-9;
           ok = dist_key(bound2) > kth;
         } else {
@@ -1304,6 +1477,9 @@ __device__ __forceinline__ void cand_final_body(SDB_FINAL_PARAMS) {
       metric, k, row_base, out_rows, out_dist, out_count, debug
 __global__ void __launch_bounds__(256) cand_final_kernel(SDB_FINAL_PARAMS) { cand_final_body<false>(SDB_FINAL_ARGS); }
 __global__ void __launch_bounds__(256) cand_final_lp_kernel(SDB_FINAL_PARAMS) { cand_final_body<true>(SDB_FINAL_ARGS); }
+__global__ void __launch_bounds__(256) cand_final_pearson_kernel(SDB_FINAL_PARAMS, double eps_ref) {
+  cand_final_body<false, true>(SDB_FINAL_ARGS, eps_ref);
+}
 #undef SDB_FINAL_ARGS
 #undef SDB_FINAL_PARAMS
 
@@ -1315,6 +1491,18 @@ sdb_status cand_final(Corpus* c, uint32_t nq, uint32_t k, uint64_t row_base, uin
   }
   static const int debug = getenv("SDB_DEBUG") != nullptr;
   const uint32_t n_sp = c->filt.bits ? 0u : c->n_special;  // filtered: the passing special rows are in the lists
+  if (pearson_screened(c)) {
+    // |pearson - cos(dx, dq)| <= (2 D + 6) 2^-53 to first order (DESIGN.md section 2); +2 covers the rest
+    const double eps_ref = (2.0 * c->dim + 8.0) * 0x1p-53;
+    cand_final_pearson_kernel<<<nq, 256, 0, st>>>(c->d_rr_key, c->d_rr_dist, c->d_rr_row, c->rr_stride, c->d_cand_cnt,
+                                                  c->sc_cap, n_sp, c->d_tau, c->d_qmag, c->d_bscale, c->d_beps,
+                                                  c->d_tau2, c->d_beps2, c->d_flags, c->d_qflags, c->d_stat,
+                                                  (int)c->metric, k, row_base, d_out_rows, d_out_dist, d_out_count,
+                                                  debug, eps_ref);
+    count_launch(c->ctx);
+    SDB_CUDA(cudaGetLastError());
+    return SDB_OK;
+  }
   auto fin = lp_metric(c) ? cand_final_lp_kernel : cand_final_kernel;
   fin<<<nq, 256, 0, st>>>(c->d_rr_key, c->d_rr_dist, c->d_rr_row, c->rr_stride, c->d_cand_cnt, c->sc_cap,
                                         n_sp, c->d_tau, c->d_qmag, c->d_bscale, c->d_beps, c->d_tau2, c->d_beps2, c->d_flags, c->d_qflags, c->d_stat,

@@ -122,6 +122,64 @@ __global__ void __launch_bounds__(WARPS * 32) finalize_lp_kernel(const T* __rest
   }
 }
 
+// PEARSON corpora: the reference ranks pearson = covar / (sd1 sd2) of the rows centred in f64 with their own mean, which
+// is the cosine of the centred vectors dx_i = x_i - m1 up to f64 rounding (DESIGN.md section 2, "PEARSON screen").
+// So the cosine screens run on dx (f32 and f64 rows alike), and this kernel keeps per row, in the exact kernel's own
+// arithmetic (ExactAcc::sum_step, then pearson_step's acc2): mom[r] = {m1 = (sum x) / D, S1 = sum (x_i - m1)^2}, both
+// sequential f64, and snorm = fl32(1/sqrt(S1)).  mag stays the magnitude (sdb_corpus_project reads it).  Special rows
+// (ranked exactly on every query):
+//  - S1 = 0: constant rows (zero and -0.0 rows too, every row when D = 1): pearson is a generated NaN (0/0);
+//  - m1 or S1 not finite (a NaN or infinite element);
+//  - an element of dx beyond f32 range (its f32 / bf16 copy would be infinite);
+//  - sqrt(S1) or 1/sqrt(S1) not a normal f32, or sqrt(S1) < 2^-100: the F64 cosine rules of finalize_rows_kernel,
+//    applied to dx.
+template <typename T, int WARPS>
+__global__ void __launch_bounds__(WARPS * 32) finalize_pearson_kernel(const T* __restrict__ rows, uint32_t dim,
+                                                                      uint64_t n, const uint8_t* __restrict__ skip,
+                                                                      double* __restrict__ mag, double2* __restrict__ mom,
+                                                                      float* __restrict__ snorm,
+                                                                      uint32_t* __restrict__ special,
+                                                                      uint32_t* special_cnt) {
+  __shared__ T tile[WARPS][32][33];
+  const uint32_t warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const uint64_t warps_total = (uint64_t)gridDim.x * WARPS;
+  for (uint64_t base = ((uint64_t)blockIdx.x * WARPS + warp) * 32; base < n; base += warps_total * 32) {
+    const uint64_t r = base + lane;
+    const uint32_t my_row = r < n ? (uint32_t)r : NO_ROW;
+    double s = 0.0, sum = 0.0;
+    warp_walk_rows<T>(rows, dim, my_row, tile[warp], [&](uint32_t, T x) {
+      const double xd = (double)x;
+      s = __dadd_rn(s, __dmul_rn(xd, xd));
+      sum = __dadd_rn(sum, xd);
+    });
+    const double m1 = __ddiv_rn(sum, (double)dim);
+    double s1 = 0.0, amax = 0.0;
+    warp_walk_rows<T>(rows, dim, my_row, tile[warp], [&](uint32_t, T x) {
+      const double dx = __dsub_rn((double)x, m1);
+      s1 = __dadd_rn(s1, __dmul_rn(dx, dx));
+      amax = fmax(amax, fabs(dx));
+    });
+    if (my_row == NO_ROW) continue;
+    mag[r] = __dsqrt_rn(s);
+    mom[r] = make_double2(m1, s1);
+    const double nrm = __dsqrt_rn(s1);
+    float sn = (float)(1.0 / nrm);
+    const float nf = (float)nrm;
+    const bool n_normal = nf >= 1.17549435e-38f && nf <= 3.40282347e38f;
+    const bool sn_normal = fabsf(sn) >= 1.17549435e-38f && fabsf(sn) <= 3.40282347e38f;
+    const bool is_special = !(s1 > 0.0) || !isfinite(s1) || !isfinite(m1) || !(amax <= 3.4028234663852886e38) ||
+                            nrm < 0x1p-100 || !n_normal || !sn_normal;
+    if (skip && skip[r]) {
+      sn = __int_as_float(0x7fc00000);
+    } else if (is_special) {
+      sn = __int_as_float(0x7fc00000);
+      const uint32_t pos = atomicAdd(special_cnt, 1u);
+      if (pos < (uint32_t)SPECIAL_CAP) special[pos] = (uint32_t)r;
+    }
+    snorm[r] = sn;
+  }
+}
+
 // rows in [n, cap_pad) are TMA padding of the last screening tile: NaN norm => never a candidate
 __global__ void pad_snorm_kernel(float* __restrict__ snorm, uint64_t n, uint64_t n_pad) {
   const uint64_t i = n + (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -132,19 +190,29 @@ __global__ void pad_snorm_kernel(float* __restrict__ snorm, uint64_t n, uint64_t
 // norm that enters the screen's error bound; at most 2^-8 by construction of round-to-nearest, usually ~0.6 of that)
 // f64 rows are rounded to bf16 in one step (cvt.rn.bf16.f64: no double rounding through f32), and their residual is
 // measured in f64 against the f64 values, then rounded up to f32.
-template <typename T>
+// CENTRED (PEARSON corpora): the copy holds bf16(dx_i), dx_i = x_i - m1 in f64 for f32 and f64 rows alike, and `mag`
+// points at the rows' moments {m1, S1} (finalize_pearson_kernel): the residual is measured in f64 against dx, relative
+// to |dx| = sqrt(S1).
+template <typename T, bool CENTRED = false>
 __global__ void __launch_bounds__(256) to_bf16_kernel(const T* __restrict__ rows, uint32_t dim, uint32_t dim_pad, uint64_t n,
                                                       uint64_t n_pad, const double* __restrict__ mag,
                                                       const float* __restrict__ snorm, __nv_bfloat16* __restrict__ out,
                                                       uint32_t* max_rel_bits) {
-  using Acc = typename std::conditional<std::is_same<T, double>::value, double, float>::type;
+  using Acc = typename std::conditional<std::is_same<T, double>::value || CENTRED, double, float>::type;
   const uint32_t lane = threadIdx.x & 31;
   const uint64_t warps = (uint64_t)gridDim.x * 8;
   for (uint64_t r = (uint64_t)blockIdx.x * 8 + (threadIdx.x >> 5); r < n_pad; r += warps) {
     __nv_bfloat16* o = out + r * dim_pad;
     Acc err2 = 0;
+    const double m1 = (CENTRED && r < n) ? mag[2 * r] : 0.0;
     for (uint32_t c = lane; c < dim_pad; c += 32) {
-      if constexpr (std::is_same<T, double>::value) {
+      if constexpr (CENTRED) {
+        const double v = (r < n && c < dim) ? __dsub_rn((double)rows[r * dim + c], m1) : 0.0;
+        const __nv_bfloat16 h = __double2bfloat16(v);
+        o[c] = h;
+        const double d = v - (double)__bfloat162float(h);
+        if (d == d) err2 = fma(d, d, err2);
+      } else if constexpr (std::is_same<T, double>::value) {
         const double v = (r < n && c < dim) ? rows[r * dim + c] : 0.0;
         const __nv_bfloat16 h = __double2bfloat16(v);
         o[c] = h;
@@ -162,9 +230,9 @@ __global__ void __launch_bounds__(256) to_bf16_kernel(const T* __restrict__ rows
     for (int o2 = 16; o2 > 0; o2 >>= 1) err2 += __shfl_xor_sync(0xffffffffu, err2, o2);
     if (lane == 0 && r < n) {
       const float sn = snorm[r];
-      const double m = mag[r];
+      const double m = CENTRED ? __dsqrt_rn(mag[2 * r + 1]) : mag[r];
       if (sn == sn && m > 0.0 && isfinite(m) && isfinite(err2)) {  // skipped / special rows never reach the screen
-        if constexpr (std::is_same<T, double>::value)  // (1 + 2^-30) covers the f64 rounding of the figure itself
+        if constexpr (std::is_same<T, double>::value || CENTRED)  // (1 + 2^-30): the f64 rounding of the figure itself
           atomicMax(max_rel_bits, __float_as_uint(__double2float_ru(sqrt(err2) / m * (1.0 + 0x1p-30))));
         else
           atomicMax(max_rel_bits, __float_as_uint((sqrtf(err2) / (float)m) * 1.0001f + 1e-9f));
@@ -190,8 +258,8 @@ __device__ __host__ inline uint32_t rmax_bin(float v) {  // v > 0
 #endif
   return (u >> 19) & (RMAX_BINS - 1);
 }
-// (f64 rows: max_i |x_i| / |x| in f64, rounded up to f32)
-template <typename T>
+// (f64 rows: max_i |x_i| / |x| in f64, rounded up to f32; CENTRED: max_i |dx_i| / sqrt(S1), as to_bf16_kernel)
+template <typename T, bool CENTRED = false>
 __global__ void __launch_bounds__(256) quantize_scan_kernel(const T* __restrict__ rows, uint32_t dim, uint64_t n,
                                                             const double* __restrict__ mag, const float* __restrict__ snorm,
                                                             uint32_t* gmax_bits, float* __restrict__ rmax,
@@ -210,7 +278,14 @@ __global__ void __launch_bounds__(256) quantize_scan_kernel(const T* __restrict_
     }
     const T* x = rows + r * dim;
     float v;
-    if constexpr (std::is_same<T, double>::value) {
+    if constexpr (CENTRED) {
+      const double m1 = mag[2 * r];
+      double mx = 0.0;
+      for (uint32_t c = lane; c < dim; c += 32) mx = fmax(mx, fabs(__dsub_rn((double)x[c], m1)));
+#pragma unroll
+      for (int o2 = 16; o2 > 0; o2 >>= 1) mx = fmax(mx, __shfl_xor_sync(0xffffffffu, mx, o2));
+      v = __double2float_ru(mx / __dsqrt_rn(mag[2 * r + 1]));
+    } else if constexpr (std::is_same<T, double>::value) {
       double mx = 0.0;
       for (uint32_t c = lane; c < dim; c += 32) mx = fmax(mx, fabs(x[c]));
 #pragma unroll
@@ -251,7 +326,8 @@ __global__ void mark_outliers_kernel(const float* __restrict__ rmax, uint64_t n,
 }
 // pass 2: x8 = clamp(rn(x / (|x| s)), +-127), e_x accumulated exactly as the residual norm (clipping included)
 // f64 rows: xn = x / |x| and xn / s in f64 (each correctly rounded), the residual xn - s x8 in f64, rounded up to f32
-template <typename T>
+// CENTRED (PEARSON): the same in f64 with xn = dx / sqrt(S1), dx_i = x_i - m1 (`mag` = the moments, as to_bf16_kernel)
+template <typename T, bool CENTRED = false>
 __global__ void __launch_bounds__(256) quantize_rows_kernel(const T* __restrict__ rows, uint32_t dim, uint32_t dim_pad8,
                                                             uint64_t n, uint64_t n_pad, const double* __restrict__ mag,
                                                             const float* __restrict__ snorm, const uint32_t* gmax_bits,
@@ -269,13 +345,14 @@ __global__ void __launch_bounds__(256) quantize_rows_kernel(const T* __restrict_
       continue;
     }
     const T* x = rows + r * dim;
-    if constexpr (std::is_same<T, double>::value) {
-      const double m = mag[r], sd = (double)s;
+    if constexpr (std::is_same<T, double>::value || CENTRED) {
+      const double m = CENTRED ? __dsqrt_rn(mag[2 * r + 1]) : mag[r], sd = (double)s;
+      const double m1 = CENTRED ? mag[2 * r] : 0.0;
       double err2 = 0.0;
       for (uint32_t c = lane; c < dim_pad8; c += 32) {
         int q = 0;
         if (c < dim) {
-          const double xn = x[c] / m;
+          const double xn = (CENTRED ? __dsub_rn((double)x[c], m1) : (double)x[c]) / m;
           q = __double2int_rn(xn / sd);
           q = q > 127 ? 127 : (q < -127 ? -127 : q);
           const double d = xn - (double)q * sd;  // q * s is exact (7 x 24 bits)
@@ -395,9 +472,20 @@ sdb_status corpus_finalize_device(Corpus* c) {
       count_launch(ctx);
     }
   }
+  // PEARSON corpora with their screen copies (sdb_corpus_create): moments, centred copies; without them the exact
+  // kernel serves every query and the corpus is finalized as before
+  const bool centred = c->metric == SDB_PEARSON && c->d_mom;
   if (c->n) {
     const int grid = ctx->sm_count * 8;
-    if (c->metric == SDB_MANHATTAN || c->metric == SDB_CHEBYSHEV) {
+    if (centred) {
+      if (c->dtype == SDB_F32)
+        finalize_pearson_kernel<float, 8><<<grid, 256, 0, st>>>((const float*)c->d_rows.get(), c->dim, c->n, c->d_skip,
+                                                                c->d_mag, c->d_mom, c->d_snorm, c->d_special, d_tmp);
+      else
+        finalize_pearson_kernel<double, 4><<<grid * 2, 128, 0, st>>>((const double*)c->d_rows.get(), c->dim, c->n,
+                                                                     c->d_skip, c->d_mag, c->d_mom, c->d_snorm,
+                                                                     c->d_special, d_tmp);
+    } else if (c->metric == SDB_MANHATTAN || c->metric == SDB_CHEBYSHEV) {
       if (c->dtype == SDB_F32)
         finalize_lp_kernel<float, 8><<<grid, 256, 0, st>>>((const float*)c->d_rows.get(), c->dim, c->n, (int)c->metric,
                                                            c->d_skip, c->d_mag, c->d_snorm, c->d_special, d_tmp,
@@ -418,7 +506,15 @@ sdb_status corpus_finalize_device(Corpus* c) {
     SDB_CUDA(cudaGetLastError());
     if (c->d_bf16) {
       const uint64_t n_pad = (c->n + TILE_ROWS - 1) / TILE_ROWS * TILE_ROWS;
-      if (c->dtype == SDB_F32)
+      const double* mom = (const double*)c->d_mom.get();
+      if (centred && c->dtype == SDB_F32)
+        to_bf16_kernel<float, true><<<ctx->sm_count * 16, 256, 0, st>>>((const float*)c->d_rows.get(), c->dim, c->dim_pad,
+                                                                        c->n, n_pad, mom, c->d_snorm, c->d_bf16, d_tmp + 4);
+      else if (centred)
+        to_bf16_kernel<double, true><<<ctx->sm_count * 16, 256, 0, st>>>((const double*)c->d_rows.get(), c->dim,
+                                                                         c->dim_pad, c->n, n_pad, mom, c->d_snorm,
+                                                                         c->d_bf16, d_tmp + 4);
+      else if (c->dtype == SDB_F32)
         to_bf16_kernel<float><<<ctx->sm_count * 16, 256, 0, st>>>((const float*)c->d_rows.get(), c->dim, c->dim_pad, c->n,
                                                                   n_pad, c->d_mag, c->d_snorm, c->d_bf16, d_tmp + 4);
       else
@@ -429,14 +525,21 @@ sdb_status corpus_finalize_device(Corpus* c) {
     }
   }
   c->n_outliers = 0;
-  if (c->n && c->d_i8 && c->metric == SDB_COSINE) {
+  if (c->n && c->d_i8 && (c->metric == SDB_COSINE || centred)) {
     const uint64_t n_pad = (c->n + TILE_ROWS - 1) / TILE_ROWS * TILE_ROWS;
+    const double* mom = (const double*)c->d_mom.get();
     AsyncBuf<float> d_rmax;
     AsyncBuf<uint32_t> d_hist;
     SDB_CUDA(d_rmax.reserve(c->n, st));
     SDB_CUDA(d_hist.reserve(RMAX_BINS, st));
     SDB_CUDA(cudaMemsetAsync(d_hist, 0, sizeof(uint32_t) * RMAX_BINS, st));
-    if (c->dtype == SDB_F32)
+    if (centred && c->dtype == SDB_F32)
+      quantize_scan_kernel<float, true><<<ctx->sm_count * 8, 256, 0, st>>>((const float*)c->d_rows.get(), c->dim, c->n,
+                                                                           mom, c->d_snorm, d_tmp + 3, d_rmax, d_hist);
+    else if (centred)
+      quantize_scan_kernel<double, true><<<ctx->sm_count * 8, 256, 0, st>>>((const double*)c->d_rows.get(), c->dim, c->n,
+                                                                            mom, c->d_snorm, d_tmp + 3, d_rmax, d_hist);
+    else if (c->dtype == SDB_F32)
       quantize_scan_kernel<float><<<ctx->sm_count * 8, 256, 0, st>>>((const float*)c->d_rows.get(), c->dim, c->n, c->d_mag,
                                                                      c->d_snorm, d_tmp + 3, d_rmax, d_hist);
     else
@@ -492,7 +595,15 @@ sdb_status corpus_finalize_device(Corpus* c) {
         }
       }
     }
-    if (c->dtype == SDB_F32)
+    if (centred && c->dtype == SDB_F32)
+      quantize_rows_kernel<float, true><<<ctx->sm_count * 8, 256, 0, st>>>((const float*)c->d_rows.get(), c->dim,
+                                                                           c->dim_pad8, c->n, n_pad, mom, c->d_snorm,
+                                                                           d_tmp + 3, c->d_i8, d_tmp + 2);
+    else if (centred)
+      quantize_rows_kernel<double, true><<<ctx->sm_count * 8, 256, 0, st>>>((const double*)c->d_rows.get(), c->dim,
+                                                                            c->dim_pad8, c->n, n_pad, mom, c->d_snorm,
+                                                                            d_tmp + 3, c->d_i8, d_tmp + 2);
+    else if (c->dtype == SDB_F32)
       quantize_rows_kernel<float><<<ctx->sm_count * 8, 256, 0, st>>>((const float*)c->d_rows.get(), c->dim, c->dim_pad8, c->n,
                                                                      n_pad, c->d_mag, c->d_snorm, d_tmp + 3, c->d_i8, d_tmp + 2);
     else

@@ -323,6 +323,7 @@ struct Scratch {
   DevBuf<float> d_q32;
   DevBuf<__nv_bfloat16> d_qbf16;
   DevBuf<double> d_qmag;
+  DevBuf<double2> d_qmom;     // PEARSON: {m2, S2} per query (mean and sum of squared deviations, the exact kernel's)
   DevBuf<uint32_t> d_qflags;  // bit0: query needs the exact path; bit1: query has NaN input
   DevBuf<float> d_qbferr;     // |q - bf16(q)| / |q| per query
   DevBuf<int8_t> d_q8;        // int8 queries nq_pad x dim_pad8
@@ -380,7 +381,8 @@ struct Corpus : Scratch {
   bool finalized = false;
   DevBuf<char> d_rows;              // master copy, cap x dim (f32 or f64)
   DevBuf<double> d_mag;          // exact f64 magnitude per row (reference arithmetic)
-  DevBuf<float> d_snorm;         // cosine: 1/|x| ; euclid: |x|^2 ; NaN = never a screen candidate
+  DevBuf<float> d_snorm;         // cosine: 1/|x| ; euclid: |x|^2 ; pearson: 1/|x - m1| ; NaN = never a screen candidate
+  DevBuf<double2> d_mom;         // PEARSON corpora with screen copies: {m1, S1} per row (finalize_pearson_kernel)
   DevBuf<__nv_bfloat16> d_bf16;  // screen copy cap_pad x dim_pad (rows padded to TILE_ROWS)
   float bf16_rel_err = 0.00390625f; // max over rows of |x - bf16(x)| / |x| (measured at finalize, rounded up)
   DevBuf<int8_t> d_i8;           // int8 screen copy cap_pad x dim_pad8 of the normalised rows (one global scale), cosine only

@@ -766,8 +766,11 @@ sdb_status screen_tc_init_device(Ctx* ctx) {
 sdb_status screen_tc_pass(Corpus* c, uint32_t nq, uint32_t k, const PassDesc& p, bool int8, int mode, cudaStream_t st) {
   if (p.count == 0) return SDB_OK;
   Ctx* ctx = c->ctx;
-  if (int8 ? (!c->d_i8 || c->metric != SDB_COSINE) : !c->d_bf16) {
-    set_error("tensor-core screen: the %s screen copy is not available for this corpus", int8 ? "int8 (cosine only)" : "bf16");
+  // PEARSON corpora hold centred copies (corpus.cu) and centred, negated queries (prep_queries): their cosine screen
+  const bool cosine = c->metric == SDB_COSINE || (c->metric == SDB_PEARSON && c->d_mom);
+  if (int8 ? (!c->d_i8 || !cosine) : !c->d_bf16) {
+    set_error("tensor-core screen: the %s screen copy is not available for this corpus",
+              int8 ? "int8 (cosine and pearson only)" : "bf16");
     return SDB_EUNSUPPORTED;
   }
   const uint64_t n_pad = (c->n + TILE_ROWS - 1) / TILE_ROWS * TILE_ROWS;
@@ -861,7 +864,7 @@ sdb_status screen_tc_pass(Corpus* c, uint32_t nq, uint32_t k, const PassDesc& p,
     else LAUNCH_TC1(COS, I8, 3);             \
   } while (0)
     if (int8) LAUNCH_TC(true, true);
-    else if (c->metric == SDB_COSINE) LAUNCH_TC(true, false);
+    else if (cosine) LAUNCH_TC(true, false);
     else LAUNCH_TC(false, false);
 #undef LAUNCH_TC
 #undef LAUNCH_TC1

@@ -26,12 +26,12 @@ from .engine import Context, VectorColumn, pack_row_filter
 
 class Distance:
     """catalog::Distance (catalog/schema/index.rs:247-284); Debug names as printed by EXPLAIN."""
-    Cosine = "Cosine"
-    Euclidean = "Euclidean"
-    Manhattan = "Manhattan"      # the next four are ranked by the exact kernel only (no screen)
+    Cosine = "Cosine"            # int8 / bf16 tensor-core screens + exact re-rank
+    Euclidean = "Euclidean"      # bf16 tensor-core screen + exact re-rank
+    Manhattan = "Manhattan"      # this and Chebyshev: the f32 L1 / L-infinity screen + exact re-rank
     Chebyshev = "Chebyshev"
-    Hamming = "Hamming"
-    Pearson = "Pearson"
+    Hamming = "Hamming"          # exact kernel only (no screen)
+    Pearson = "Pearson"          # the cosine screens on the centred rows + exact re-rank
     Minkowski = "Minkowski"      # exact kernel, order via VectorColumn.set_minkowski_order (pow(): ~1e-14 relative)
     Jaccard = "Jaccard"          # exact kernel, set semantics over the values
 
