@@ -167,6 +167,23 @@ sdb_status sdb_debug_screen_batch(sdb_corpus*, const double* queries, uint32_t n
                                   int streaming, uint32_t cand_cap, int score_all, float* out_qf, double* out_qmag,
                                   uint32_t* out_qu, int8_t* out_q8, uint16_t* out_qbf16, uint32_t* out_a,
                                   uint32_t* out_b, uint32_t* out_rr);
+/* sdb_debug_screen_batch_filtered: the same batch with a row filter per query (filters, n_filters, query_filter as in
+ * sdb_knn_bruteforce_filtered; sdb_debug_screen_batch is this call with filters = NULL).  The queries are classified as
+ * sdb_knn_bruteforce_filtered classifies them (direct regime or screened, FiltArg mask_hits); mask_hits = -1 keeps that
+ * rule's choice, 0 and 1 force the int8 consumers' hit-mask filtering off or on.  A batch that mixes direct and
+ * screened queries returns SDB_EUNSUPPORTED (unless score_all).  What the lists hold with a filter:
+ *   score_all   pass 0 with the filter: the tensor-core screens write every row and NaN the scores of the rows the
+ *               query's filter rejects (cand_filter_list); SIMT_F32 never appends a rejected row
+ *   out_b       the passing special rows follow the stage-B rows in the query's list (score +inf), so n_e = n_b and
+ *               out_rr holds no special rows beyond them
+ *   all-direct  no screen pass runs (n_passes = 0): out_a and out_b are the direct list (every passing row that is
+ *               neither skipped nor removed, score +inf), tau is -inf and the gathered count is 0 */
+sdb_status sdb_debug_screen_batch_filtered(sdb_corpus*, const double* queries, uint32_t nq, uint32_t k,
+                                           sdb_screen screen, int streaming, uint32_t cand_cap, int score_all,
+                                           float* out_qf, double* out_qmag, uint32_t* out_qu, int8_t* out_q8,
+                                           uint16_t* out_qbf16, uint32_t* out_a, uint32_t* out_b, uint32_t* out_rr,
+                                           const uint32_t* filters, uint32_t n_filters, const uint32_t* query_filter,
+                                           int mask_hits);
 /* Test-only: device and pinned buffers the library holds right now, process-wide (count and bytes).  Buffers handed to
  * the caller (sdb_pinned_alloc, sdb_graph_expand_device) are not counted.  Either output may be NULL. */
 void sdb_debug_live_allocations(uint64_t* count, uint64_t* bytes);

@@ -608,6 +608,31 @@ static Ticket* free_ticket(Corpus* c) {
   return nullptr;
 }
 
+// filtered batch (submit_locked, sdb_debug_screen_batch_filtered): the per query filter index on the host (exact
+// fallbacks, repairs), the direct / screened split (query indices in batch order) and FiltArg::mask_hits
+static void plan_filtered(const Corpus* c, Ticket& t, uint32_t nq, uint32_t k, const uint32_t* d_filters,
+                          const uint32_t* query_filter, const uint64_t* filter_rows, std::vector<uint32_t>* scr,
+                          std::vector<uint32_t>* dir) {
+  t.h_qf.assign(nq, 0u);
+  if (query_filter) std::copy(query_filter, query_filter + nq, t.h_qf.begin());
+  t.filt.bits = d_filters;
+  t.filt.words = (uint32_t)((c->n + 31) / 32);
+  // direct regime: a query whose filter passes at most DIRECT_MAX_ROWS rows (filter_rows: set bits, an upper bound
+  // of the rows it passes) skips the screen; the re-rank and cand_final serve the five screenable metrics, k <= 256
+  const bool direct_ok = filter_rows && k > 0 && k <= 256 &&
+                         (c->metric == SDB_COSINE || c->metric == SDB_EUCLIDEAN || c->metric == SDB_MANHATTAN ||
+                          c->metric == SDB_CHEBYSHEV || (c->metric == SDB_PEARSON && c->d_mom));
+  for (uint32_t q = 0; q < nq; q++) {
+    const uint64_t rows_q = filter_rows ? filter_rows[t.h_qf[q]] : ~0ull;
+    if (direct_ok && rows_q <= DIRECT_MAX_ROWS) dir->push_back(q);
+    else {
+      scr->push_back(q);
+      if (rows_q < c->n / MASK_HITS_DIV) t.filt.mask_hits = 1;  // a selective filter among the screened queries
+    }
+  }
+  t.n_direct = (uint32_t)dir->size();
+}
+
 static sdb_status submit_locked(Corpus* c, Ticket* t, const double* d_queries, uint32_t nq, uint32_t k, uint64_t row_base,
                                 uint64_t* d_out_rows, double* d_out_dist, uint32_t* d_out_count,
                                 const volatile int* cancel, const uint32_t* d_filters = nullptr,
@@ -641,26 +666,9 @@ static sdb_status submit_locked(Corpus* c, Ticket* t, const double* d_queries, u
   t->filt = FiltArg();
   t->n_direct = 0;
   t->permuted = false;
-  if (d_filters) {  // filtered batch: per query filter index on the host (exact fallbacks, repairs) and the device
-    t->h_qf.assign(nq, 0u);
-    if (query_filter) std::copy(query_filter, query_filter + nq, t->h_qf.begin());
-    t->filt.bits = d_filters;
-    t->filt.words = (uint32_t)((c->n + 31) / 32);
-    // direct regime: a query whose filter passes at most DIRECT_MAX_ROWS rows (filter_rows: set bits, an upper bound
-    // of the rows it passes) skips the screen; the re-rank and cand_final serve the five screenable metrics, k <= 256
+  if (d_filters) {
     std::vector<uint32_t> scr, dir;
-    const bool direct_ok = filter_rows && k > 0 && k <= 256 &&
-                           (c->metric == SDB_COSINE || c->metric == SDB_EUCLIDEAN || c->metric == SDB_MANHATTAN ||
-                            c->metric == SDB_CHEBYSHEV || (c->metric == SDB_PEARSON && c->d_mom));
-    for (uint32_t q = 0; q < nq; q++) {
-      const uint64_t rows_q = filter_rows ? filter_rows[t->h_qf[q]] : ~0ull;
-      if (direct_ok && rows_q <= DIRECT_MAX_ROWS) dir.push_back(q);
-      else {
-        scr.push_back(q);
-        if (rows_q < c->n / MASK_HITS_DIV) t->filt.mask_hits = 1;  // a selective filter among the screened queries
-      }
-    }
-    t->n_direct = (uint32_t)dir.size();
+    plan_filtered(c, *t, nq, k, d_filters, query_filter, filter_rows, &scr, &dir);
     if (!dir.empty() && !scr.empty()) {  // mixed: run permuted, screened queries first (see Ticket::permuted)
       std::vector<uint32_t> perm(scr);
       perm.insert(perm.end(), dir.begin(), dir.end());
@@ -1414,11 +1422,26 @@ sdb_status sdb_debug_screen_batch(sdb_corpus* c, const double* queries, uint32_t
                                   int streaming, uint32_t cand_cap, int score_all, float* out_qf, double* out_qmag,
                                   uint32_t* out_qu, int8_t* out_q8, uint16_t* out_qbf16, uint32_t* out_a,
                                   uint32_t* out_b, uint32_t* out_rr) {
+  return sdb_debug_screen_batch_filtered(c, queries, nq, k, screen, streaming, cand_cap, score_all, out_qf, out_qmag,
+                                         out_qu, out_q8, out_qbf16, out_a, out_b, out_rr, nullptr, 0, nullptr, -1);
+}
+
+static sdb_status check_filters(uint32_t nq, const uint32_t* filters, uint32_t n_filters, const uint32_t* query_filter);
+
+sdb_status sdb_debug_screen_batch_filtered(sdb_corpus* c, const double* queries, uint32_t nq, uint32_t k,
+                                           sdb_screen screen, int streaming, uint32_t cand_cap, int score_all,
+                                           float* out_qf, double* out_qmag, uint32_t* out_qu, int8_t* out_q8,
+                                           uint16_t* out_qbf16, uint32_t* out_a, uint32_t* out_b, uint32_t* out_rr,
+                                           const uint32_t* filters, uint32_t n_filters, const uint32_t* query_filter,
+                                           int mask_hits) {
   const bool tc = screen == SDB_SCREEN_TC_INT8 || screen == SDB_SCREEN_TC_BF16;
-  if (!c || !queries || !nq || !k || k > 256 || cand_cap < 4096 || (!tc && screen != SDB_SCREEN_SIMT_F32)) {
-    set_error("sdb_debug_screen_batch: bad argument (1 <= k <= 256, cand_cap >= 4096, a TC_INT8 / TC_BF16 / SIMT_F32 screen)");
+  if (!c || !queries || !nq || !k || k > 256 || cand_cap < 4096 || (!tc && screen != SDB_SCREEN_SIMT_F32) ||
+      mask_hits < -1 || mask_hits > 1) {
+    set_error("sdb_debug_screen_batch: bad argument (1 <= k <= 256, cand_cap >= 4096, a TC_INT8 / TC_BF16 / SIMT_F32 "
+              "screen, mask_hits -1, 0 or 1)");
     return SDB_EINVAL;
   }
+  if (filters) SDB_TRY(check_filters(nq, filters, n_filters, query_filter));
   std::lock_guard<std::mutex> g(c->mu);
   const bool int8 = screen == SDB_SCREEN_TC_INT8;
   // MANHATTAN / CHEBYSHEV: the SIMT_F32 (L1 / L-infinity) screen, f32 and f64 rows
@@ -1451,6 +1474,29 @@ sdb_status sdb_debug_screen_batch(sdb_corpus* c, const double* queries, uint32_t
   c->sc_nq = c->sc_cap = 0;
   SDB_TRY(scratch_for(c, nq, cap));
   cudaStream_t st = ctx->stream;
+  // the batch's filter, classified as ticket submission classifies it
+  t->filt = FiltArg();
+  t->n_direct = 0;
+  t->permuted = false;
+  if (filters) {
+    const size_t words = (size_t)n_filters * ((c->n + 31) / 32);
+    SDB_CUDA(t->d_in_filt.reserve(words));
+    SDB_CUDA(cudaMemcpyAsync(t->d_in_filt, filters, sizeof(uint32_t) * words, cudaMemcpyHostToDevice, st));
+    const std::vector<uint64_t> rows_per_filter = count_filter_rows_host(c, filters, n_filters, query_filter, nq);
+    std::vector<uint32_t> scr, dir;
+    plan_filtered(c, *t, nq, k, t->d_in_filt, query_filter, rows_per_filter.data(), &scr, &dir);
+    if (!score_all && !scr.empty() && !dir.empty()) {
+      t->filt = FiltArg();
+      t->n_direct = 0;
+      set_error("sdb_debug_screen_batch_filtered: a batch that mixes direct and screened queries has no readable lists");
+      return SDB_EUNSUPPORTED;
+    }
+    if (mask_hits >= 0) t->filt.mask_hits = (uint32_t)mask_hits;
+    SDB_CUDA(t->d_qf.reserve(nq));
+    SDB_CUDA(cudaMemcpyAsync(t->d_qf, t->h_qf.data(), sizeof(uint32_t) * nq, cudaMemcpyHostToDevice, st));
+    t->filt.qf = t->d_qf;
+  }
+  const bool direct = !score_all && t->n_direct == nq;
   DevBuf<double> d_q;
   ResultBufs out;
   ScreenTap tap;
@@ -1464,8 +1510,10 @@ sdb_status sdb_debug_screen_batch(sdb_corpus* c, const double* queries, uint32_t
       const PassDesc all{1u, 0u, (uint32_t)(n_pad / TILE_ROWS), 0u};
       SDB_TRY(prep_queries(c, d_q, nq, st));
       SDB_TRY(cand_begin(c, nq, (int)screen, st));
-      if (tc) SDB_TRY(screen_tc_pass(c, nq, k, all, int8, 0, st));
-      else SDB_TRY(screen_simt_pass(c, nq, all, st));
+      c->filt = t->filt;
+      sdb_status rc = tc ? screen_tc_pass(c, nq, k, all, int8, 0, st) : screen_simt_pass(c, nq, all, st);
+      c->filt = FiltArg();
+      SDB_TRY(rc);
       SDB_TRY(tap_list(c, nq, &tap.list_a, &tap.cnt_a, st));
       tap.gathered = tap.cnt_a;
       return SDB_OK;
@@ -1484,12 +1532,12 @@ sdb_status sdb_debug_screen_batch(sdb_corpus* c, const double* queries, uint32_t
     t->d_out_count = out.count;
     t->cancel = nullptr;
     t->rung = 0;
-    t->filt = FiltArg();
     c->tap = &tap;
     const sdb_status rc = enqueue_batch(c, *t);
     c->tap = nullptr;
     SDB_TRY(rc);
     SDB_CUDA(cudaStreamSynchronize(st));
+    if (direct) return tap_list(c, nq, &tap.list_a, &tap.cnt_a, st);  // no screen ran: the lists are the direct ones
     if (t->screen != (int)screen) {
       set_error("sdb_debug_screen_batch: the corpus does not offer screen %d", (int)screen);
       return SDB_EINVAL;
@@ -1533,7 +1581,8 @@ sdb_status sdb_debug_screen_batch(sdb_corpus* c, const double* queries, uint32_t
     }
     if (rc == SDB_OK && cudaStreamSynchronize(st) != cudaSuccess) rc = SDB_ECUDA;
     if (rc == SDB_OK) {
-      const uint32_t n_special = score_all ? 0u : c->n_special;
+      // (filtered: the passing special rows are in the stage-B list)
+      const uint32_t n_special = score_all || filters ? 0u : c->n_special;
       auto bits = [](float v) {
         uint32_t u;
         memcpy(&u, &v, 4);
