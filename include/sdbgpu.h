@@ -47,8 +47,9 @@ typedef enum {
 /* catalog::Distance (catalog/schema/index.rs:247-284).  COSINE and EUCLIDEAN are screened on the tensor cores and
  * re-ranked exactly; PEARSON is screened on the tensor cores as the cosine of the rows and the query centred on their
  * own means, and re-ranked exactly; MANHATTAN and CHEBYSHEV are screened by the f32 L1 / L-infinity SIMT screen
- * (SDB_SCREEN_SIMT_F32) and re-ranked exactly; HAMMING, JACCARD and MINKOWSKI run through the exact kernel (sequential
- * f64, Distance::compute op for op). */
+ * (SDB_SCREEN_SIMT_F32) and re-ranked exactly, and so is MINKOWSKI of an integer order 1 .. 8 (f32 Lp screen); HAMMING,
+ * JACCARD and MINKOWSKI of any other order run through the exact kernel (sequential f64, Distance::compute op for
+ * op). */
 typedef enum {
   SDB_CHEBYSHEV = 0,
   SDB_COSINE = 1,
@@ -66,7 +67,8 @@ typedef enum {
  * tensor cores (F64: when the bf16 / int8 copies, 3 bytes per element, fit beside the rows at creation; otherwise the
  * corpus is ranked by the exact kernel alone).  The f32 SIMT screen of COSINE / EUCLIDEAN needs F32 rows: on F64 it
  * means the exact kernel.  MANHATTAN / CHEBYSHEV corpora of either type are screened by the f32 L1 / L-infinity screen
- * (f64 rows rounded to f32 as the screen reads them; rows with an element beyond f32 range are ranked exactly).
+ * (f64 rows rounded to f32 as the screen reads them; rows with an element beyond f32 range are ranked exactly), and
+ * MINKOWSKI corpora of an integer order 1 .. 8 by the f32 Lp screen in the same way.
  * PEARSON corpora of either type are screened on the tensor cores when the bf16 / int8 copies of the centred rows and
  * 16 bytes of moments per row fit beside the rows at creation; otherwise the exact kernel ranks them. */
 typedef enum { SDB_F32 = 0, SDB_F64 = 1 } sdb_dtype;
@@ -82,11 +84,12 @@ typedef enum { SDB_VT_F64 = 0, SDB_VT_F32 = 1, SDB_VT_I64 = 2, SDB_VT_I32 = 3, S
  * proof fails climb to finer screens (bf16, then the f32 stream) before the exact kernel.  MANHATTAN / CHEBYSHEV corpora
  * (k <= 256) are screened by SDB_SCREEN_SIMT_F32 for AUTO and every TC request (4096, then 16384 candidates per query,
  * then the exact kernel), except that AUTO ranks a batch of one query with the exact kernel (faster for a single query);
- * NONE_EXACT keeps them on the exact kernel.  PEARSON corpora (k <= 256) follow the cosine ladder on the centred rows
+ * NONE_EXACT keeps them on the exact kernel.  MINKOWSKI corpora of an integer order 1 .. 8 take the same ladder, a
+ * single query included (their exact kernel is bound by a pow() per element); other orders keep the exact kernel.  PEARSON corpora (k <= 256) follow the cosine ladder on the centred rows
  * (int8, then bf16, then the exact kernel; no f32 stream): SIMT_F32 and NONE_EXACT mean the exact kernel. */
 typedef enum {
   SDB_SCREEN_AUTO = 0,
-  SDB_SCREEN_SIMT_F32 = 1,   /* f32 SIMT screen: streaming dot products; MANHATTAN / CHEBYSHEV: L1 / L-inf */
+  SDB_SCREEN_SIMT_F32 = 1,   /* f32 SIMT screen: streaming dot products; MANHATTAN / CHEBYSHEV / MINKOWSKI: Lp */
   SDB_SCREEN_TC_BF16 = 2,    /* wgmma bf16 operands, f32 accumulation                                    */
   SDB_SCREEN_NONE_EXACT = 3, /* no screen: exact f64 kernel for every query                              */
   SDB_SCREEN_TC_INT8 = 4     /* wgmma s8, int8 copy of the normalised (pearson: centred) rows; falls back to bf16 */
@@ -133,9 +136,10 @@ sdb_status sdb_debug_schedule(uint64_t n_rows, uint32_t cand_cap, uint32_t k, ui
                               uint32_t cap_probe, uint32_t* out_n_probe);
 /* Test-only diagnostics of the brute-force screens (no reference seam): the state the exactness proof rests on, so that
  * tests can compare every intermediate with a plain reference.  Every output may be NULL.
- * sdb_debug_corpus_state, on a finalized F32 corpus or an F64 one that has screen copies (n_pad = rows rounded up to
- * 256):
- *   out_f[4]    i8_scale, max_rel_qerr, bf16_rel_err, max_norm
+ * sdb_debug_corpus_state, on a finalized F32 corpus, an F64 one that has screen copies, or an F64 MANHATTAN /
+ * CHEBYSHEV / MINKOWSKI one (n_pad = rows rounded up to 256):
+ *   out_f[4]    i8_scale, max_rel_qerr, bf16_rel_err, max_norm (MANHATTAN: the largest sum_i |x^_i| of a screened
+ *               row; CHEBYSHEV and MINKOWSKI of any order: the largest |x^_i|)
  *   out_u[5]    n_special, n_outliers, dim_pad, dim_pad8, n_pad
  *   out_i8      [n_pad][dim_pad8] int8 copy of the normalised rows (cosine corpora; PEARSON: of dx / |dx|)
  *   out_bf16    [n_pad][dim_pad] bf16 copy (bit patterns; PEARSON: of the centred rows dx = x - mean(x))
@@ -147,7 +151,8 @@ sdb_status sdb_debug_corpus_state(sdb_corpus*, float* out_f, uint32_t* out_u, in
 /* sdb_debug_screen_batch: one batch of nq host queries screened with `screen` (TC_INT8, TC_BF16 or SIMT_F32) at the
  * first rung of the ladder, through the production sequence (streaming = 0: the multi-pass schedule), with exactly
  * cand_cap (>= 4096) candidate slots per query (F64 corpora with screen copies: TC_INT8 or TC_BF16 only; MANHATTAN / CHEBYSHEV corpora, F32 or F64: SIMT_F32, where
- * beps bounds |s~ - d| and the score is -s~; PEARSON corpora with screen copies, F32 or F64: TC_INT8 or TC_BF16, where
+ * beps bounds |s~ - d| and the score is -s~; MINKOWSKI corpora of an integer order 1 .. 8, F32 or F64: SIMT_F32, where
+ * the score is the f32 norm -n~ of the batch's scaled power sum and beps bounds |n~ - d|; PEARSON corpora with screen copies, F32 or F64: TC_INT8 or TC_BF16, where
  * the scores are those of the unit query -dq/|dq| against dx, qmag is 1 and the proof adds eps_ref).  The ladder
  * and the exact fallback do not run: flags are as the batch
  * left them.  score_all != 0 instead runs one pass-0 launch over every tile (SIMT: tau = -inf) with max(cand_cap,
@@ -224,7 +229,8 @@ sdb_status sdb_corpus_read_rows(sdb_corpus*, uint64_t first_row, uint64_t n, voi
 /* order p of Distance::Minkowski(p) (catalog/schema/index.rs:247-284; fnc/util/math/vector.rs:163-174); default 3.
  * MINKOWSKI goes through pow(): CUDA's libm here, the platform libm in the reference -- each call agrees to within an
  * ulp or two, so Minkowski distances are equal to ~1e-14 relative rather than bit for bit (every other metric is
- * bit-exact). */
+ * bit-exact).  Integer orders 1 .. 8 are screened (f32 Lp screen + exact re-rank), every other order is ranked by the
+ * exact kernel; the order may change after finalize. */
 sdb_status sdb_corpus_set_minkowski_order(sdb_corpus*, double order);
 sdb_status sdb_corpus_set_screen(sdb_corpus*, sdb_screen);
 /* schedule of the tensor-core screens (results are identical; tuning / A-B only).  streaming = 1 (default): a scored
@@ -275,7 +281,8 @@ sdb_status sdb_knn_wait(sdb_corpus*, uint32_t ticket);
  * metric, F32 and F64, k <= 4096, cancellation, sdb_knn_last_stats, up to 4 tickets in flight (filtered and unfiltered
  * mixed), completion through sdb_knn_wait.  SDB_EINVAL: n_filters == 0 with nq > 0, filters == NULL, or an index >=
  * n_filters.
- * A query whose bitmap has at most 4096 set bits (COSINE, EUCLIDEAN, MANHATTAN, CHEBYSHEV, PEARSON; k <= 256) skips the screen
+ * A query whose bitmap has at most 4096 set bits (COSINE, EUCLIDEAN, MANHATTAN, CHEBYSHEV, PEARSON, MINKOWSKI of
+ * an integer order 1 .. 8; k <= 256) skips the screen
  * (its passing rows are ranked directly; results are
  * the same); sdb_knn_last_stats then reports screen_used = SDB_SCREEN_NONE_EXACT and n_passes = 0 for a batch of such
  * queries only.

@@ -110,16 +110,18 @@ static std::vector<Rung> build_rungs(Corpus* c, uint32_t k, uint32_t nq, sdb_scr
                                  : (int8_ok && c->max_rel_qerr <= 0.02f ? SDB_SCREEN_TC_INT8 : SDB_SCREEN_TC_BF16);
   if (scr == SDB_SCREEN_TC_INT8 && !int8_ok) scr = SDB_SCREEN_TC_BF16;
   if (scr == SDB_SCREEN_TC_BF16 && (!screen_tc_available() || !c->d_bf16)) scr = SDB_SCREEN_SIMT_F32;
-  // MANHATTAN / CHEBYSHEV: the f32 L1 / L-infinity screen (screen_lp.cu) is their only screen, for f32 and f64 rows
-  const bool lp = c->metric == SDB_MANHATTAN || c->metric == SDB_CHEBYSHEV;
+  // MANHATTAN / CHEBYSHEV / MINKOWSKI of an integer order 1 .. 8: the f32 Lp screen (screen_lp.cu) is their only
+  // screen, for f32 and f64 rows; MINKOWSKI of any other order stays on the exact kernel (!screenable below)
+  const bool lp = lp_screened(c);
   const bool screenable = c->metric == SDB_COSINE || c->metric == SDB_EUCLIDEAN || lp || pearson;
   // the SIMT screen streams f32 rows: an f64 cosine / euclidean corpus is screened on the tensor cores or not at all,
   // and so is a PEARSON one of either type (the SIMT screen would need the centred rows)
   if ((c->dtype == SDB_F64 || pearson) && scr == SDB_SCREEN_SIMT_F32 && !lp) scr = SDB_SCREEN_NONE_EXACT;
   if (c->special_overflow || k > 256 || !screenable) scr = SDB_SCREEN_NONE_EXACT;
-  // a single query streams the rows once either way, and the exact kernel does it at the higher HBM rate (DESIGN.md
-  // section 5): AUTO ranks it there; an explicit SIMT_F32 request is kept
-  if (lp && nq == 1 && c->screen == SDB_SCREEN_AUTO) scr = SDB_SCREEN_NONE_EXACT;
+  // MANHATTAN / CHEBYSHEV: a single query streams the rows once either way, and the exact kernel does it at the higher
+  // HBM rate (DESIGN.md section 5): AUTO ranks it there; an explicit SIMT_F32 request is kept.  MINKOWSKI's exact
+  // kernel is bound by its f64 pow() calls, not by HBM, and the screen is faster for a single query too (section 5).
+  if (lp && c->metric != SDB_MINKOWSKI && nq == 1 && c->screen == SDB_SCREEN_AUTO) scr = SDB_SCREEN_NONE_EXACT;
   *first = scr;
   std::vector<Rung> r;
   if (scr == SDB_SCREEN_TC_INT8)
@@ -618,10 +620,10 @@ static void plan_filtered(const Corpus* c, Ticket& t, uint32_t nq, uint32_t k, c
   t.filt.bits = d_filters;
   t.filt.words = (uint32_t)((c->n + 31) / 32);
   // direct regime: a query whose filter passes at most DIRECT_MAX_ROWS rows (filter_rows: set bits, an upper bound
-  // of the rows it passes) skips the screen; the re-rank and cand_final serve the five screenable metrics, k <= 256
+  // of the rows it passes) skips the screen; the re-rank and cand_final serve the screenable metrics, k <= 256
   const bool direct_ok = filter_rows && k > 0 && k <= 256 &&
-                         (c->metric == SDB_COSINE || c->metric == SDB_EUCLIDEAN || c->metric == SDB_MANHATTAN ||
-                          c->metric == SDB_CHEBYSHEV || (c->metric == SDB_PEARSON && c->d_mom));
+                         (c->metric == SDB_COSINE || c->metric == SDB_EUCLIDEAN || lp_screened(c) ||
+                          (c->metric == SDB_PEARSON && c->d_mom));
   for (uint32_t q = 0; q < nq; q++) {
     const uint64_t rows_q = filter_rows ? filter_rows[t.h_qf[q]] : ~0ull;
     if (direct_ok && rows_q <= DIRECT_MAX_ROWS) dir->push_back(q);
@@ -1062,7 +1064,8 @@ sdb_status sdb_corpus_create(sdb_ctx* ctx, uint32_t dim, sdb_dtype dt, sdb_metri
   }
   // COSINE / EUCLIDEAN: screened (K1/K2) + exact re-rank.  MANHATTAN / CHEBYSHEV: the f32 L1 / L-infinity screen
   // (screen_lp.cu) + exact re-rank.  PEARSON: the cosine tensor-core screens on the centred rows + exact re-rank.
-  // HAMMING / JACCARD / MINKOWSKI: served by the exact kernel alone (sequential f64, Distance::compute op for op).  MINKOWSKI goes through
+  // MINKOWSKI of integer order 1 .. 8: the f32 Lp screen + exact re-rank; of any other order, like HAMMING / JACCARD:
+  // served by the exact kernel alone (sequential f64, Distance::compute op for op).  MINKOWSKI goes through
   // pow(), which CUDA's libm and Rust's (the platform libm) implement separately: within 1 ulp of each other per term,
   // so its distances are compared with a 1e-12 relative tolerance instead of bit equality (tests/test_gpu_knn.py).
   const bool screenable = m == SDB_COSINE || m == SDB_EUCLIDEAN;
@@ -1384,7 +1387,7 @@ sdb_status sdb_debug_corpus_state(sdb_corpus* c, float* out_f, uint32_t* out_u, 
                                   float* out_snorm, uint32_t* out_special) {
   if (!c) return SDB_EINVAL;
   std::lock_guard<std::mutex> g(c->mu);
-  const bool lp = c->metric == SDB_MANHATTAN || c->metric == SDB_CHEBYSHEV;
+  const bool lp = c->metric == SDB_MANHATTAN || c->metric == SDB_CHEBYSHEV || c->metric == SDB_MINKOWSKI;
   if (!c->finalized || (c->dtype != SDB_F32 && !c->d_bf16 && !lp) || (c->metric == SDB_PEARSON && !c->d_mom) ||
       (out_i8 && !c->d_i8) || (out_bf16 && !c->d_bf16)) {
     set_error("sdb_debug_corpus_state: needs a finalized F32 corpus or a screened F64 / PEARSON one (int8 copy: "
@@ -1444,8 +1447,8 @@ sdb_status sdb_debug_screen_batch_filtered(sdb_corpus* c, const double* queries,
   if (filters) SDB_TRY(check_filters(nq, filters, n_filters, query_filter));
   std::lock_guard<std::mutex> g(c->mu);
   const bool int8 = screen == SDB_SCREEN_TC_INT8;
-  // MANHATTAN / CHEBYSHEV: the SIMT_F32 (L1 / L-infinity) screen, f32 and f64 rows
-  const bool lp = (c->metric == SDB_MANHATTAN || c->metric == SDB_CHEBYSHEV) && screen == SDB_SCREEN_SIMT_F32;
+  // MANHATTAN / CHEBYSHEV / MINKOWSKI of a screened order: the SIMT_F32 (L1 / L-infinity / Lp) screen, f32 and f64
+  const bool lp = lp_screened(c) && screen == SDB_SCREEN_SIMT_F32;
   // f64 rows: tensor-core screens only (cosine / euclidean)
   const bool f64_ok = c->dtype == SDB_F64 && ((tc && c->d_bf16) || lp);
   // PEARSON (f32 and f64 rows): the cosine tensor-core screens on the centred rows
@@ -1455,7 +1458,7 @@ sdb_status sdb_debug_screen_batch_filtered(sdb_corpus* c, const double* queries,
       (c->metric == SDB_PEARSON && !pearson) || (int8 && !c->d_i8) || c->special_overflow || !c->n) {
     set_error("sdb_debug_screen_batch: needs a finalized, non-empty F32 cosine / euclidean corpus, an F64 one with "
               "screen copies and a tensor-core screen (int8: cosine), a PEARSON one with screen copies and a "
-              "tensor-core screen, or a MANHATTAN / CHEBYSHEV one with SIMT_F32");
+              "tensor-core screen, or a MANHATTAN / CHEBYSHEV / MINKOWSKI (integer order 1 .. 8) one with SIMT_F32");
     return SDB_EINVAL;
   }
   Ctx* ctx = c->ctx;

@@ -343,7 +343,108 @@ __global__ void __launch_bounds__(128) cand_begin_lp_kernel(float* __restrict__ 
   qcap[q] = __double2float_ru(hi);
 }
 
-static bool lp_metric(const Corpus* c) { return c->metric == SDB_MANHATTAN || c->metric == SDB_CHEBYSHEV; }
+// MINKOWSKI of integer order p (1 .. 8, minkowski_screen_order): the launch's scale first.  The screen multiplies
+// every staged element by s = 2^-e, with 2^e > M + Qb: M = max_norm (the largest |x^_i| of a screened row), Qb = the
+// largest |q^_i| of the batch's queries that the screen can bound (qflags bit 0 clear).  Then every |s x^_i - s q^_i|
+// <= 1, so no product of minkowski_fma and no power sum of at most 65535 terms overflows.  One warp per query folds
+// its largest |q^_i| into mscale[0] (non-negative f32 bits order as integers); cand_begin_minkowski_kernel reads it.
+__global__ void __launch_bounds__(128) minkowski_batch_max_kernel(const float* __restrict__ q32,
+                                                                  const uint32_t* __restrict__ qflags, uint32_t nq,
+                                                                  uint32_t dim, uint32_t* __restrict__ mscale) {
+  const uint32_t lane = threadIdx.x & 31u, q = blockIdx.x * 4 + (threadIdx.x >> 5);
+  if (q >= nq || (qflags[q] & 1u)) return;
+  float amax = 0.f;
+  for (uint32_t c = lane; c < dim; c += 32) amax = fmaxf(amax, fabsf(q32[(size_t)q * dim + c]));
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) amax = fmaxf(amax, __shfl_xor_sync(0xffffffffu, amax, o));
+  if (lane == 0) atomicMax(mscale, __float_as_uint(amax));
+}
+
+// The bound of the MINKOWSKI screen (screen_lp.cu, score = -n~, n~ = fl32(S~^(1/p) 2^e)), one warp per query.  beps
+// bounds |n~ - d| for every screened row, d = the exact kernel's distance (pow(sum_i pow(|x_i - q_i|, p), 1/p) in f64,
+// sequentially).  With u = 2^-24, R = D^(1/p), M = max_norm, |q^|_p = the query's f32 copy's p-norm and
+// W = (R M + |q^|_p + R 2^-148)(1 + 2u) >= |x|_p + |q|_p (the f64 values), by the triangle inequality of the p-norm:
+//  - rounding x and q to f32: u W, plus R 2^-149 for the elements that land in or below f32's subnormal range (each
+//    moves by up to 2^-150 there, whatever the launch's scale: this term is not multiplied by 2^e);
+//  - the f32 subtraction (u W) and the final rounding of n~ (u W, 2^-149 subnormal);
+//  - the multiplication chain and the sequential FFMA sum: a relative error g = (D + p - 1) u / (1 - (D + p - 1) u) of
+//    the power sum, g / (p (1 - g)) of its root;
+//  - underflow under the scale: staging products that land below 2^-126 (2^-150 each, R 2^-149 in norm, times 2^e),
+//    and chain / sum roundings below 2^-126 (at most D (p^2 + 1) 2^-149 in the power sum: its p-th root, times 2^e);
+//  - the root in f64: CUDA's pow() is within 2 ulp (CUDA C++ Programming Guide, double-precision mathematical functions)
+//    and 1/p is rounded (|ln S~| / p 2^-53 relative, S~ >= 2^-149): 2^-44 relative;
+//  - the exact kernel: its f64 differences, pow() calls (2 ulp each), sequential sum and final pow() with a rounded 1/p
+//    err by at most (D + 2p + 810) 2^-53 relative, and its f64 underflow by (D 2^-1073)^(1/p) absolute.
+// beps = (3u + g / (p (1 - g)) + 2^-44 + (D + 2p + 810) 2^-53) W (1 + 2^-20) + R 2^-149 + R 2^-149 2^e
+//        + (D (p^2 + 1) 2^-149)^(1/p) 2^e + (D 2^-1073)^(1/p) + 2^-149.
+// A query or corpus whose W is not a finite f32, or whose W^p could overflow the exact kernel's f64 sum, gets an
+// infinite bound (tau then proves nothing: exact fallback).  Stage B does not run: tau2 stays -inf.
+__global__ void __launch_bounds__(128) cand_begin_minkowski_kernel(
+    float* __restrict__ tau, uint32_t* __restrict__ cnt, uint32_t* __restrict__ flags, uint32_t* __restrict__ stat,
+    float* __restrict__ bscale, float* __restrict__ beps, float* __restrict__ margin, float* __restrict__ margin2,
+    float* __restrict__ beps2, float* __restrict__ tau2, float* __restrict__ qlow, float* __restrict__ qcap,
+    const float* __restrict__ q32, uint32_t nq, uint32_t dim, int p, float max_norm, uint32_t* __restrict__ mscale,
+    int exact) {
+  const uint32_t lane = threadIdx.x & 31u, q = blockIdx.x * 4 + (threadIdx.x >> 5);
+  if (blockIdx.x == 0 && threadIdx.x < 4) stat[threadIdx.x] = 0;
+  // the launch's scale exponent: M + Qb < 2^e (frexp), at least -126 so that s = 2^-e is a finite f32
+  const double v = (double)max_norm + (double)__uint_as_float(mscale[0]);
+  int e = -126;
+  if (v > 0.0) {
+    frexp(v, &e);
+    if (e < -126) e = -126;
+  }
+  if (blockIdx.x == 0 && threadIdx.x == 0) mscale[1] = (uint32_t)e;
+  if (q >= nq) return;
+  float amax = 0.f;
+  for (uint32_t c = lane; c < dim; c += 32) amax = fmaxf(amax, fabsf(q32[(size_t)q * dim + c]));
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) amax = fmaxf(amax, __shfl_xor_sync(0xffffffffu, amax, o));
+  // |q^|_p = amax (sum_i (|q^_i| / amax)^p)^(1/p): no overflow for any finite query
+  double sp = 0.0;
+  if (amax > 0.f && isfinite(amax)) {
+    const double inv = 1.0 / (double)amax;
+    for (uint32_t c = lane; c < dim; c += 32) {
+      const double r = (double)fabsf(q32[(size_t)q * dim + c]) * inv;
+      double t = r;
+      for (int i = 1; i < p; i++) t *= r;
+      sp += t;
+    }
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) sp += __shfl_xor_sync(0xffffffffu, sp, o);
+  if (lane != 0) return;
+  const double D = (double)dim, u = 0x1p-24, P = (double)p, up = 1.0 + 0x1p-40;
+  const double R = pow(D, 1.0 / P) * up, se = ldexp(1.0, e);
+  const double qn = amax > 0.f ? (double)amax * pow(sp, 1.0 / P) * up : (double)amax;
+  const double w = (R * (double)max_norm + qn + R * 0x1p-148) * (1.0 + 2.0 * u);
+  const double gn = (D + P - 1.0) * u, g = gn / (1.0 - gn);
+  const double rel = 3.0 * u + g / (P * (1.0 - g)) + 0x1p-44 + (D + 2.0 * P + 810.0) * 0x1p-53;
+  double eps = rel * w * (1.0 + 0x1p-20) + R * 0x1p-149 + R * 0x1p-149 * se + pow(D * (P * P + 1.0) * 0x1p-149, 1.0 / P) * up * se +
+               pow(D * 0x1p-1073, 1.0 / P) * up + 0x1p-149;
+  double mg = 2.1 * eps, hi = eps + 1e-30, lo = -(w * 1.01 + eps) - 1e-30;
+  if (!(w <= 3.4028234663852886e38) || !(pow(w, P) <= 1e307) || !isfinite(eps)) {  // no bound
+    eps = INFINITY;
+    mg = 0.0;
+    hi = 1.0;
+    lo = -1.0;
+  }
+  if (!exact) mg = 0.0;
+  tau[q] = __int_as_float(0xff800000);  // -inf
+  cnt[q] = 0;
+  flags[q] = 0;
+  bscale[q] = 1.f;
+  beps[q] = __double2float_ru(eps);
+  margin[q] = __double2float_ru(mg);
+  margin2[q] = 0.f;
+  beps2[q] = 0.f;
+  tau2[q] = __int_as_float(0xff800000);
+  qlow[q] = __double2float_rd(lo);
+  qcap[q] = __double2float_ru(hi);
+}
+
+// MANHATTAN / CHEBYSHEV / screened MINKOWSKI: the f32 Lp screen's bound, re-rank and proof
+static bool lp_metric(const Corpus* c) { return lp_screened(c); }
 
 sdb_status cand_begin(Corpus* c, uint32_t nq, int screen, cudaStream_t st) {
   if (pearson_screened(c)) {
@@ -356,6 +457,17 @@ sdb_status cand_begin(Corpus* c, uint32_t nq, int screen, cudaStream_t st) {
                                                         c->max_rel_qerr, c->i8_scale, c->bf16_rel_err, c->max_norm,
                                                         c->exact ? 1 : 0, 1);
     count_launch(c->ctx);
+    SDB_CUDA(cudaGetLastError());
+    return SDB_OK;
+  }
+  if (const int p = minkowski_screen_order(c)) {
+    SDB_CUDA(cudaMemsetAsync(c->d_mscale, 0, sizeof(uint32_t), st));
+    minkowski_batch_max_kernel<<<(nq + 3) / 4, 128, 0, st>>>(c->d_q32, c->d_qflags, nq, c->dim, c->d_mscale);
+    cand_begin_minkowski_kernel<<<(nq + 3) / 4, 128, 0, st>>>(c->d_tau, c->d_cand_cnt, c->d_flags, c->d_stat,
+                                                              c->d_bscale, c->d_beps, c->d_margin, c->d_margin2,
+                                                              c->d_beps2, c->d_tau2, c->d_qlow, c->d_qcap, c->d_q32, nq,
+                                                              c->dim, p, c->max_norm, c->d_mscale, c->exact ? 1 : 0);
+    count_launch(c->ctx, 2);
     SDB_CUDA(cudaGetLastError());
     return SDB_OK;
   }
@@ -406,6 +518,7 @@ static sdb_status ensure_scratch(Corpus* c, uint32_t nq, uint32_t cap) {
     SDB_CUDA(s.d_q8.reserve((size_t)nqa * (c->dim_pad8 ? c->dim_pad8 : 128)));
     SDB_CUDA(s.d_q8scale.reserve(nqa));
     SDB_CUDA(s.d_q8err.reserve(nqa));
+    SDB_CUDA(s.d_mscale.reserve(2));
     SDB_CUDA(s.d_bscale.reserve(nqa));
     SDB_CUDA(s.d_beps.reserve(nqa));
     SDB_CUDA(s.d_margin.reserve(nqa));
@@ -1181,15 +1294,15 @@ __global__ void __launch_bounds__(128) cand_rerank_packed_kernel(
   }
 }
 
-// MANHATTAN / CHEBYSHEV re-rank: the exact kernel's arithmetic (ExactAcc::manhattan_step / chebyshev_step, canon_nan)
-// per candidate, one thread per list entry and its row streamed left to right (the query's elements are the same
+// MANHATTAN / CHEBYSHEV / MINKOWSKI re-rank: the exact kernel's arithmetic (ExactAcc::manhattan_step / chebyshev_step /
+// minkowski_step, canon_nan; MINKOWSKI's order mink_p a run-time argument there and here) per candidate, one thread per list entry and its row streamed left to right (the query's elements are the same
 // address across the warp).  Blocks (x = query, y = 0 .. RR_GROUPS_Y - 1) stride over the query's entries.
 template <typename T, int METRIC>
 __global__ void __launch_bounds__(128) cand_rerank_lp_kernel(
     const T* __restrict__ rows, uint32_t dim, const double* __restrict__ q64, const uint32_t* __restrict__ qflags,
     const Cand* __restrict__ cand, const uint32_t* __restrict__ cnt, uint32_t cap, const uint32_t* __restrict__ special,
     uint32_t n_special, uint64_t* __restrict__ rr_key, double* __restrict__ rr_dist, uint32_t* __restrict__ rr_row,
-    uint32_t rr_stride) {
+    uint32_t rr_stride, double mink_p) {
   const uint32_t q = blockIdx.x;
   const uint32_t n_c = cnt[q] < cap ? cnt[q] : cap;
   const uint32_t n_e = n_c + n_special;
@@ -1202,9 +1315,13 @@ __global__ void __launch_bounds__(128) cand_rerank_lp_kernel(
     if (METRIC == SDB_CHEBYSHEV) acc.acc = -1.7976931348623157e308;  // f64::MIN
     for (uint32_t j = 0; j < dim; j++) {
       if (METRIC == SDB_MANHATTAN) acc.manhattan_step((double)__ldg(x + j), __ldg(qv + j));
+      else if (METRIC == SDB_MINKOWSKI) acc.minkowski_step((double)__ldg(x + j), __ldg(qv + j), mink_p);
       else acc.chebyshev_step((double)__ldg(x + j), __ldg(qv + j));
     }
-    const double d = METRIC == SDB_MANHATTAN ? canon_nan(acc.acc, acc.nan_in || q_nan) : acc.acc;
+    double d;
+    if (METRIC == SDB_MANHATTAN) d = canon_nan(acc.acc, acc.nan_in || q_nan);
+    else if (METRIC == SDB_MINKOWSKI) d = canon_nan(pow(acc.acc, __ddiv_rn(1.0, mink_p)), acc.nan_in || q_nan);
+    else d = acc.acc;
     const size_t o = (size_t)q * rr_stride + e;
     rr_key[o] = dist_key(d);
     rr_dist[o] = d;
@@ -1252,9 +1369,12 @@ __global__ void __launch_bounds__(128) cand_rerank_pearson_kernel(
 template <typename T>
 static void launch_rerank_lp(Corpus* c, uint32_t nq, uint32_t n_sp, cudaStream_t st) {
   const dim3 grid(nq, RR_GROUPS_Y);
-  auto kern = c->metric == SDB_MANHATTAN ? cand_rerank_lp_kernel<T, SDB_MANHATTAN> : cand_rerank_lp_kernel<T, SDB_CHEBYSHEV>;
+  auto kern = c->metric == SDB_MANHATTAN   ? cand_rerank_lp_kernel<T, SDB_MANHATTAN>
+              : c->metric == SDB_MINKOWSKI ? cand_rerank_lp_kernel<T, SDB_MINKOWSKI>
+                                           : cand_rerank_lp_kernel<T, SDB_CHEBYSHEV>;
   kern<<<grid, 128, 0, st>>>((const T*)c->d_rows.get(), c->dim, c->d_q64, c->d_qflags, c->d_cand, c->d_cand_cnt,
-                             c->sc_cap, c->d_special, n_sp, c->d_rr_key, c->d_rr_dist, c->d_rr_row, c->rr_stride);
+                             c->sc_cap, c->d_special, n_sp, c->d_rr_key, c->d_rr_dist, c->d_rr_row, c->rr_stride,
+                             c->minkowski_p);
 }
 
 sdb_status cand_rerank(Corpus* c, uint32_t nq, cudaStream_t st, bool small_sets) {
@@ -1360,7 +1480,7 @@ __device__ __forceinline__ void bitonic_pairs(uint64_t* s_key, uint64_t* s_idx, 
   }
 }
 
-// LP: the MANHATTAN / CHEBYSHEV proof (cand_final_lp_kernel); otherwise cosine / euclidean (cand_final_kernel)
+// LP: the MANHATTAN / CHEBYSHEV / MINKOWSKI proof (cand_final_lp_kernel); otherwise cosine / euclidean (cand_final_kernel)
 #define SDB_FINAL_PARAMS                                                                                               \
   const uint64_t *__restrict__ rr_key, const double *__restrict__ rr_dist, const uint32_t *__restrict__ rr_row,       \
       uint32_t rr_stride, const uint32_t *__restrict__ cnt, uint32_t cap, uint32_t n_special,                          \

@@ -75,11 +75,12 @@ __global__ void __launch_bounds__(WARPS * 32) finalize_rows_kernel(const T* __re
   }
 }
 
-// MANHATTAN / CHEBYSHEV corpora (screen_lp.cu).  The screen sees every row through its f32 copy x^ = fl32(x), so a
+// MANHATTAN / CHEBYSHEV / MINKOWSKI corpora (screen_lp.cu).  The screen sees every row through its f32 copy x^ = fl32(x), so a
 // row with an element whose f32 copy is not finite (NaN, +-inf, or, in f64 rows, beyond f32 range) is special: ranked
 // exactly on every query.  snorm is 0 for screened rows (the score is -(s~ + snorm)) and NaN for skipped / special
 // ones.  max_norm = the largest norm of the metric over the screened rows, sum_i |x^_i| (MANHATTAN) or max_i |x^_i|
-// (CHEBYSHEV), summed in f64 and rounded up: the error bound of cand_begin_lp_kernel scales with it.  mag keeps the
+// (CHEBYSHEV, and MINKOWSKI of any order: its bound and scale need the largest element, which no order change moves),
+// summed in f64 and rounded up: the error bound of cand_begin_lp_kernel scales with it.  mag keeps the
 // reference's magnitude() arithmetic, as finalize_rows_kernel computes it.
 template <typename T, int WARPS>
 __global__ void __launch_bounds__(WARPS * 32) finalize_lp_kernel(const T* __restrict__ rows, uint32_t dim, uint64_t n,
@@ -485,7 +486,8 @@ sdb_status corpus_finalize_device(Corpus* c) {
         finalize_pearson_kernel<double, 4><<<grid * 2, 128, 0, st>>>((const double*)c->d_rows.get(), c->dim, c->n,
                                                                      c->d_skip, c->d_mag, c->d_mom, c->d_snorm,
                                                                      c->d_special, d_tmp);
-    } else if (c->metric == SDB_MANHATTAN || c->metric == SDB_CHEBYSHEV) {
+    } else if (c->metric == SDB_MANHATTAN || c->metric == SDB_CHEBYSHEV || c->metric == SDB_MINKOWSKI) {
+      // (MINKOWSKI of every order: the order may change after finalize, sdb_corpus_set_minkowski_order)
       if (c->dtype == SDB_F32)
         finalize_lp_kernel<float, 8><<<grid, 256, 0, st>>>((const float*)c->d_rows.get(), c->dim, c->n, (int)c->metric,
                                                            c->d_skip, c->d_mag, c->d_snorm, c->d_special, d_tmp,

@@ -329,6 +329,7 @@ struct Scratch {
   DevBuf<int8_t> d_q8;        // int8 queries nq_pad x dim_pad8
   DevBuf<float> d_q8scale;    // max|q|/127 per query
   DevBuf<float> d_q8err;      // |q - dequant(q)| / |q| per query
+  DevBuf<uint32_t> d_mscale;  // MINKOWSKI screen: [0] the batch's largest |q^_i| (f32 bits), [1] its scale exponent e
   DevBuf<Cand> d_sub;         // thread-private candidate sub-lists of the tensor-core screens
   DevBuf<uint32_t> d_sub_cnt; // [nq][sub_slots]
   uint32_t sub_slots = 0, sub_cap = 0, last_slots = 0;
@@ -418,14 +419,27 @@ struct Corpus : Scratch {
   std::mutex mu;
 };
 
+// The order of a MINKOWSKI corpus that the f32 screen serves (screen_lp.cu): an integer 1 .. 8, whose |t|^p is a short
+// chain of f32 multiplications.  0 for every other metric and order (non-integers, p < 1, p > 8, +-inf): those stay on
+// the exact kernel, which calls pow() per element.
+inline int minkowski_screen_order(const Corpus* c) {
+  if (c->metric != SDB_MINKOWSKI) return 0;
+  const double p = c->minkowski_p;
+  return (p >= 1.0 && p <= 8.0 && p == (double)(int)p) ? (int)p : 0;
+}
+// MANHATTAN / CHEBYSHEV and MINKOWSKI of a screened order: the f32 Lp screen, its bound, proof and re-rank
+inline bool lp_screened(const Corpus* c) {
+  return c->metric == SDB_MANHATTAN || c->metric == SDB_CHEBYSHEV || minkowski_screen_order(c) > 0;
+}
+
 // ---- launch wrappers (defined in the .cu files) ---------------------------------------------------
 // corpus.cu
 sdb_status corpus_finalize_device(Corpus* c);
 sdb_status corpus_remove_device(Corpus* c, const uint64_t* h_ids, uint64_t n);
 sdb_status corpus_reapply_tombstones(Corpus* c, cudaStream_t st);
-// screen_simt.cu (the SIMT_F32 screen; MANHATTAN / CHEBYSHEV corpora go to screen_lp_pass)
+// screen_simt.cu (the SIMT_F32 screen; MANHATTAN / CHEBYSHEV / screened MINKOWSKI corpora go to screen_lp_pass)
 sdb_status screen_simt_pass(Corpus* c, uint32_t nq, const PassDesc& p, cudaStream_t st);
-// screen_lp.cu: f32 L1 / L-infinity screen (score = -s~), f32 and f64 rows
+// screen_lp.cu: f32 L1 / L-infinity / Lp screen (score = -s~), f32 and f64 rows
 sdb_status screen_lp_pass(Corpus* c, uint32_t nq, const PassDesc& p, cudaStream_t st);
 // screen_tc.cu
 // mode 0: pass 0 (every score of the pass's tiles written to fixed slots), 1: threshold pass, 2: streaming pass with

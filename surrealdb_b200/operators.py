@@ -32,7 +32,8 @@ class Distance:
     Chebyshev = "Chebyshev"
     Hamming = "Hamming"          # exact kernel only (no screen)
     Pearson = "Pearson"          # the cosine screens on the centred rows + exact re-rank
-    Minkowski = "Minkowski"      # exact kernel, order via VectorColumn.set_minkowski_order (pow(): ~1e-14 relative)
+    Minkowski = "Minkowski"      # order via VectorColumn.set_minkowski_order: integer orders 1-8 on the f32 Lp screen
+                                 # + exact re-rank, every other order on the exact kernel (pow(): ~1e-14 relative)
     Jaccard = "Jaccard"          # exact kernel, set semantics over the values
 
 
