@@ -47,9 +47,10 @@ typedef enum {
 /* catalog::Distance (catalog/schema/index.rs:247-284).  COSINE and EUCLIDEAN are screened on the tensor cores and
  * re-ranked exactly; PEARSON is screened on the tensor cores as the cosine of the rows and the query centred on their
  * own means, and re-ranked exactly; MANHATTAN and CHEBYSHEV are screened by the f32 L1 / L-infinity SIMT screen
- * (SDB_SCREEN_SIMT_F32) and re-ranked exactly, and so is MINKOWSKI of an integer order 1 .. 8 (f32 Lp screen); HAMMING,
- * JACCARD and MINKOWSKI of any other order run through the exact kernel (sequential f64, Distance::compute op for
- * op). */
+ * (SDB_SCREEN_SIMT_F32) and re-ranked exactly, and so is MINKOWSKI of an integer order 1 .. 8 (f32 Lp screen);
+ * HAMMING and JACCARD (k <= 256) are ranked by exact counts of every row, batched over the queries (the count path,
+ * no screen and no proof: mismatches for HAMMING, distinct and shared values for JACCARD); MINKOWSKI of any other
+ * order and HAMMING / JACCARD with k > 256 run through the exact kernel (sequential f64, Distance::compute op for op). */
 typedef enum {
   SDB_CHEBYSHEV = 0,
   SDB_COSINE = 1,
@@ -69,6 +70,10 @@ typedef enum {
  * means the exact kernel.  MANHATTAN / CHEBYSHEV corpora of either type are screened by the f32 L1 / L-infinity screen
  * (f64 rows rounded to f32 as the screen reads them; rows with an element beyond f32 range are ranked exactly), and
  * MINKOWSKI corpora of an integer order 1 .. 8 by the f32 Lp screen in the same way.
+ * HAMMING corpora of either type take the count path: f64 rows are compared on all 64 bits, f32 rows as the exact
+ * kernel widens them to f64; no row is special (zero, NaN and +-inf are ordinary values for equality).  JACCARD
+ * corpora take it the same way when their first-occurrence state (one bit per element and 4 bytes per row) fits
+ * beside the rows at creation; otherwise the exact kernel ranks them.
  * PEARSON corpora of either type are screened on the tensor cores when the bf16 / int8 copies of the centred rows and
  * 16 bytes of moments per row fit beside the rows at creation; otherwise the exact kernel ranks them. */
 typedef enum { SDB_F32 = 0, SDB_F64 = 1 } sdb_dtype;
@@ -85,11 +90,16 @@ typedef enum { SDB_VT_F64 = 0, SDB_VT_F32 = 1, SDB_VT_I64 = 2, SDB_VT_I32 = 3, S
  * (k <= 256) are screened by SDB_SCREEN_SIMT_F32 for AUTO and every TC request (4096, then 16384 candidates per query,
  * then the exact kernel), except that AUTO ranks a batch of one query with the exact kernel (faster for a single query);
  * NONE_EXACT keeps them on the exact kernel.  MINKOWSKI corpora of an integer order 1 .. 8 take the same ladder, a
- * single query included (their exact kernel is bound by a pow() per element); other orders keep the exact kernel.  PEARSON corpora (k <= 256) follow the cosine ladder on the centred rows
+ * single query included (their exact kernel is bound by a pow() per element); other orders keep the exact kernel.
+ * HAMMING corpora (1 <= k <= 256) take the count path for AUTO and every screen request but NONE_EXACT, which keeps the
+ * exact kernel, except that AUTO ranks a batch of one query with the exact kernel (faster for a single query);
+ * JACCARD corpora with their first-occurrence state take the same path, a single query included (their exact kernel
+ * is O(D^2) per row); sdb_knn_last_stats reports it as screen_used = SDB_SCREEN_SIMT_F32, n_passes = 1, n_fallback = 0.  PEARSON corpora (k <= 256) follow the cosine ladder on the centred rows
  * (int8, then bf16, then the exact kernel; no f32 stream): SIMT_F32 and NONE_EXACT mean the exact kernel. */
 typedef enum {
   SDB_SCREEN_AUTO = 0,
-  SDB_SCREEN_SIMT_F32 = 1,   /* f32 SIMT screen: streaming dot products; MANHATTAN / CHEBYSHEV / MINKOWSKI: Lp */
+  SDB_SCREEN_SIMT_F32 = 1,   /* f32 SIMT screen: streaming dot products; MANHATTAN / CHEBYSHEV / MINKOWSKI: Lp;
+                                HAMMING / JACCARD: the count path                                           */
   SDB_SCREEN_TC_BF16 = 2,    /* wgmma bf16 operands, f32 accumulation                                    */
   SDB_SCREEN_NONE_EXACT = 3, /* no screen: exact f64 kernel for every query                              */
   SDB_SCREEN_TC_INT8 = 4     /* wgmma s8, int8 copy of the normalised (pearson: centred) rows; falls back to bf16 */
@@ -282,7 +292,7 @@ sdb_status sdb_knn_wait(sdb_corpus*, uint32_t ticket);
  * mixed), completion through sdb_knn_wait.  SDB_EINVAL: n_filters == 0 with nq > 0, filters == NULL, or an index >=
  * n_filters.
  * A query whose bitmap has at most 4096 set bits (COSINE, EUCLIDEAN, MANHATTAN, CHEBYSHEV, PEARSON, MINKOWSKI of
- * an integer order 1 .. 8; k <= 256) skips the screen
+ * an integer order 1 .. 8, HAMMING and JACCARD on the count path; k <= 256) skips the screen
  * (its passing rows are ranked directly; results are
  * the same); sdb_knn_last_stats then reports screen_used = SDB_SCREEN_NONE_EXACT and n_passes = 0 for a batch of such
  * queries only.

@@ -322,10 +322,50 @@ static sdb_status enqueue_batch(Corpus* c, Ticket& t) {
   return SDB_OK;
 }
 
+// HAMMING / JACCARD (count_ranked): exact counts of every row in one launch, ranked per row range; each query's list
+// is the union of its ranges' best k with their exact distances, so cand_final orders it with tau = -inf and nothing
+// is left to prove or repair.  Reported as one SIMT_F32 pass.
+static sdb_status enqueue_counted(Corpus* c, Ticket& t) {
+  Ctx* ctx = c->ctx;
+  cudaStream_t st = t.stream;
+  const uint32_t nq = t.nq, k = t.k;
+  t.screen = SDB_SCREEN_SIMT_F32;
+  t.n_passes = 1;
+  SDB_CUDA(cudaEventRecord(t.ev_begin, st));
+  trace_mark(ctx, t, "begin", st);
+  SDB_TRY(scratch_for(c, nq, std::max(4096u, count_ranges(c, nq, k) * k)));
+  SDB_TRY(prep_queries(c, t.d_queries, nq, st));
+  SDB_TRY(cand_begin(c, nq, SDB_SCREEN_NONE_EXACT, st));
+  if (c->last_main && c->last_main != t.ev_main) SDB_CUDA(cudaStreamWaitEvent(st, c->last_main, 0));
+  SDB_CUDA(cudaEventRecord(t.ev_screen0, st));
+  if ((t.cancel && *t.cancel) || ctx_cancelled(ctx)) {
+    cudaStreamSynchronize(st);
+    set_error("query cancelled");
+    return SDB_ECANCELLED;
+  }
+  SDB_TRY(count_pass(c, nq, k, st));
+  SDB_CUDA(cudaEventRecord(t.ev_main, st));
+  c->last_main = t.ev_main;
+  SDB_CUDA(cudaEventRecord(t.ev_screen1, st));
+  trace_mark(ctx, t, "counted", st);
+  SDB_TRY(cand_final(c, nq, k, t.row_base, t.d_out_rows, t.d_out_dist, t.d_out_count, st));
+  SDB_CUDA(cudaMemcpyAsync(t.h_flags, c->d_flags, sizeof(uint32_t) * nq, cudaMemcpyDeviceToHost, st));
+  SDB_CUDA(cudaMemcpyAsync(t.h_qflags, c->d_qflags, sizeof(uint32_t) * nq, cudaMemcpyDeviceToHost, st));
+  SDB_CUDA(cudaMemcpyAsync(t.h_stat, c->d_stat, sizeof(uint32_t) * 4, cudaMemcpyDeviceToHost, st));
+  SDB_CUDA(cudaEventRecord(t.ev_end, st));
+  trace_mark(ctx, t, "end", st);
+  return SDB_OK;
+}
+
 static sdb_status enqueue_screened(Corpus* c, Ticket& t) {
   Ctx* ctx = c->ctx;
   cudaStream_t st = t.stream;
   const uint32_t nq = t.nq, k = t.k;
+  // HAMMING: AUTO ranks a batch of one query with the exact kernel, which streams the rows once at the higher rate
+  // (DESIGN.md section 5); an explicit screen request still counts it.  JACCARD's exact kernel is O(D^2) per row: the
+  // count path takes a single query too
+  if (count_ranked(c, k) && (nq > 1 || c->screen != SDB_SCREEN_AUTO || c->metric == SDB_JACCARD))
+    return enqueue_counted(c, t);
   sdb_screen first;
   const std::vector<Rung> rungs = build_rungs(c, k, nq, &first);
   t.n_rungs = (uint32_t)rungs.size();
@@ -620,10 +660,11 @@ static void plan_filtered(const Corpus* c, Ticket& t, uint32_t nq, uint32_t k, c
   t.filt.bits = d_filters;
   t.filt.words = (uint32_t)((c->n + 31) / 32);
   // direct regime: a query whose filter passes at most DIRECT_MAX_ROWS rows (filter_rows: set bits, an upper bound
-  // of the rows it passes) skips the screen; the re-rank and cand_final serve the screenable metrics, k <= 256
+  // of the rows it passes) skips the screen; the re-rank and cand_final serve the screenable metrics and the HAMMING
+  // count path, k <= 256
   const bool direct_ok = filter_rows && k > 0 && k <= 256 &&
                          (c->metric == SDB_COSINE || c->metric == SDB_EUCLIDEAN || lp_screened(c) ||
-                          (c->metric == SDB_PEARSON && c->d_mom));
+                          (c->metric == SDB_PEARSON && c->d_mom) || count_ranked(c, k));
   for (uint32_t q = 0; q < nq; q++) {
     const uint64_t rows_q = filter_rows ? filter_rows[t.h_qf[q]] : ~0ull;
     if (direct_ok && rows_q <= DIRECT_MAX_ROWS) dir->push_back(q);
@@ -1115,6 +1156,16 @@ sdb_status sdb_corpus_create(sdb_ctx* ctx, uint32_t dim, sdb_dtype dt, sdb_metri
       c->d_bf16.reset();
       c->d_i8.reset();
       c->d_mom.reset();
+    }
+  }
+  // JACCARD: the count path's first-occurrence bitmask (one bit per element) and distinct-value count per row, 4 bytes
+  // per 32 elements plus 4 per row -- only when they fit; without them the exact kernel ranks the corpus
+  if (m == SDB_JACCARD) {
+    cudaError_t e2 = c->d_jfirst.reserve((size_t)cap * ((dim + 31) / 32));
+    if (e2 == cudaSuccess) e2 = c->d_jux.reserve(cap);
+    if (e2 != cudaSuccess) {
+      c->d_jfirst.reset();
+      c->d_jux.reset();
     }
   }
   *out = c;

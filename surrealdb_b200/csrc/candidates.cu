@@ -61,6 +61,7 @@ __global__ void prep_queries_kernel(const double* __restrict__ q64, uint32_t dim
     uint32_t f = s_flags;
     if (metric == SDB_COSINE && (!(m > 0.0) || !isfinite(m))) f |= 1u;
     if (metric != SDB_COSINE && !isfinite(m)) f |= 1u;
+    if (metric == SDB_HAMMING || metric == SDB_JACCARD) f &= ~1u;  // counts are exact for any value: zero, inf, NaN
     qflags[q] = f;
     // |q - bf16(q)| / |q|, rounded up; + 2^-23 for the f64 -> f32 rounding of the query itself
     if (qbferr) qbferr[q] = (m > 0.0 && isfinite(m)) ? (sqrtf(s_err2) / (float)m) * 1.0001f + 2.4e-7f : 1.f;
@@ -519,6 +520,8 @@ static sdb_status ensure_scratch(Corpus* c, uint32_t nq, uint32_t cap) {
     SDB_CUDA(s.d_q8scale.reserve(nqa));
     SDB_CUDA(s.d_q8err.reserve(nqa));
     SDB_CUDA(s.d_mscale.reserve(2));
+    if (count_metric(c)) SDB_CUDA(s.d_qkey.reserve((size_t)nqa * c->dim * (c->dtype == SDB_F64 ? 2 : 1)));
+    if (c->metric == SDB_JACCARD && c->d_jfirst) SDB_CUDA(s.d_qjac.reserve((size_t)nqa * (2 + c->dim)));
     SDB_CUDA(s.d_bscale.reserve(nqa));
     SDB_CUDA(s.d_beps.reserve(nqa));
     SDB_CUDA(s.d_margin.reserve(nqa));
@@ -560,6 +563,7 @@ sdb_status prep_queries(Corpus* c, const double* d_queries, uint32_t nq, cudaStr
     prep_queries_kernel<<<nq_pad, 128, 0, st>>>(c->d_q64, c->dim, c->dim_pad, (int)c->metric, c->d_q32, c->d_qbf16,
                                                 c->d_qmag, c->d_qflags, c->d_qbferr, nq);
   count_launch(c->ctx);
+  if (count_metric(c)) SDB_TRY(count_prep_queries(c, nq, st));
   if (c->d_i8) {
     prep_queries_i8_kernel<<<nq_pad, 128, 0, st>>>(c->d_q32, c->d_qmag, c->dim, c->dim_pad8, nq, c->d_q8, c->d_q8scale,
                                                    c->d_q8err);
@@ -1294,8 +1298,8 @@ __global__ void __launch_bounds__(128) cand_rerank_packed_kernel(
   }
 }
 
-// MANHATTAN / CHEBYSHEV / MINKOWSKI re-rank: the exact kernel's arithmetic (ExactAcc::manhattan_step / chebyshev_step /
-// minkowski_step, canon_nan; MINKOWSKI's order mink_p a run-time argument there and here) per candidate, one thread per list entry and its row streamed left to right (the query's elements are the same
+// MANHATTAN / CHEBYSHEV / MINKOWSKI / HAMMING re-rank: the exact kernel's arithmetic (ExactAcc::manhattan_step /
+// chebyshev_step / minkowski_step / hamming_step, canon_nan; HAMMING only in the direct regime of filtered batches; MINKOWSKI's order mink_p a run-time argument there and here) per candidate, one thread per list entry and its row streamed left to right (the query's elements are the same
 // address across the warp).  Blocks (x = query, y = 0 .. RR_GROUPS_Y - 1) stride over the query's entries.
 template <typename T, int METRIC>
 __global__ void __launch_bounds__(128) cand_rerank_lp_kernel(
@@ -1315,6 +1319,7 @@ __global__ void __launch_bounds__(128) cand_rerank_lp_kernel(
     if (METRIC == SDB_CHEBYSHEV) acc.acc = -1.7976931348623157e308;  // f64::MIN
     for (uint32_t j = 0; j < dim; j++) {
       if (METRIC == SDB_MANHATTAN) acc.manhattan_step((double)__ldg(x + j), __ldg(qv + j));
+      else if (METRIC == SDB_HAMMING) acc.hamming_step((double)__ldg(x + j), __ldg(qv + j));
       else if (METRIC == SDB_MINKOWSKI) acc.minkowski_step((double)__ldg(x + j), __ldg(qv + j), mink_p);
       else acc.chebyshev_step((double)__ldg(x + j), __ldg(qv + j));
     }
@@ -1366,11 +1371,34 @@ __global__ void __launch_bounds__(128) cand_rerank_pearson_kernel(
   }
 }
 
+// JACCARD re-rank (direct regime of filtered batches): jaccard_counts per list entry, one thread each, from the
+// corpus's first-occurrence state and the batch's query state (count_prep_queries)
+template <typename T>
+__global__ void __launch_bounds__(128) cand_rerank_jaccard_kernel(
+    const T* __restrict__ rows, uint32_t dim, const uint32_t* __restrict__ jfirst, const uint32_t* __restrict__ jux,
+    const EqKey<T>* __restrict__ qkey, const uint32_t* __restrict__ qjac, const Cand* __restrict__ cand,
+    const uint32_t* __restrict__ cnt, uint32_t cap, uint64_t* __restrict__ rr_key, double* __restrict__ rr_dist,
+    uint32_t* __restrict__ rr_row, uint32_t rr_stride) {
+  const uint32_t q = blockIdx.x;
+  const uint32_t n_c = cnt[q] < cap ? cnt[q] : cap;
+  const uint32_t words = (dim + 31) / 32;
+  for (uint32_t e = blockIdx.y * blockDim.x + threadIdx.x; e < n_c; e += gridDim.y * blockDim.x) {
+    const uint32_t row = cand[(size_t)q * cap + e].row;
+    const double d = jaccard_counts(rows + (size_t)row * dim, dim, jfirst + (size_t)row * words, jux[row],
+                                    qkey + (size_t)q * dim, qjac[2 * q + 1], qjac[2 * q]);
+    const size_t o = (size_t)q * rr_stride + e;
+    rr_key[o] = dist_key(d);
+    rr_dist[o] = d;
+    rr_row[o] = row;
+  }
+}
+
 template <typename T>
 static void launch_rerank_lp(Corpus* c, uint32_t nq, uint32_t n_sp, cudaStream_t st) {
   const dim3 grid(nq, RR_GROUPS_Y);
   auto kern = c->metric == SDB_MANHATTAN   ? cand_rerank_lp_kernel<T, SDB_MANHATTAN>
               : c->metric == SDB_MINKOWSKI ? cand_rerank_lp_kernel<T, SDB_MINKOWSKI>
+              : c->metric == SDB_HAMMING   ? cand_rerank_lp_kernel<T, SDB_HAMMING>
                                            : cand_rerank_lp_kernel<T, SDB_CHEBYSHEV>;
   kern<<<grid, 128, 0, st>>>((const T*)c->d_rows.get(), c->dim, c->d_q64, c->d_qflags, c->d_cand, c->d_cand_cnt,
                              c->sc_cap, c->d_special, n_sp, c->d_rr_key, c->d_rr_dist, c->d_rr_row, c->rr_stride,
@@ -1379,7 +1407,22 @@ static void launch_rerank_lp(Corpus* c, uint32_t nq, uint32_t n_sp, cudaStream_t
 
 sdb_status cand_rerank(Corpus* c, uint32_t nq, cudaStream_t st, bool small_sets) {
   const dim3 grid(nq, RR_GROUPS_Y);
-  if (lp_metric(c)) {
+  if (c->metric == SDB_JACCARD && c->d_jfirst) {  // the direct regime only: no special rows
+    if (c->dtype == SDB_F32)
+      cand_rerank_jaccard_kernel<float><<<grid, 128, 0, st>>>((const float*)c->d_rows.get(), c->dim, c->d_jfirst,
+                                                              c->d_jux, c->d_qkey.get(), c->d_qjac, c->d_cand,
+                                                              c->d_cand_cnt, c->sc_cap, c->d_rr_key, c->d_rr_dist,
+                                                              c->d_rr_row, c->rr_stride);
+    else
+      cand_rerank_jaccard_kernel<double><<<grid, 128, 0, st>>>((const double*)c->d_rows.get(), c->dim, c->d_jfirst,
+                                                               c->d_jux, (const unsigned long long*)c->d_qkey.get(),
+                                                               c->d_qjac, c->d_cand, c->d_cand_cnt, c->sc_cap,
+                                                               c->d_rr_key, c->d_rr_dist, c->d_rr_row, c->rr_stride);
+    count_launch(c->ctx);
+    SDB_CUDA(cudaGetLastError());
+    return SDB_OK;
+  }
+  if (lp_metric(c) || c->metric == SDB_HAMMING) {
     const uint32_t n_sp = c->filt.bits ? 0u : c->n_special;
     if (c->dtype == SDB_F32) launch_rerank_lp<float>(c, nq, n_sp, st);
     else launch_rerank_lp<double>(c, nq, n_sp, st);

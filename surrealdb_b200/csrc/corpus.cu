@@ -7,6 +7,7 @@
 #include <algorithm>
 #include <type_traits>
 
+#include "exactmath.cuh"
 #include "internal.cuh"
 #include "rowwalk.cuh"
 
@@ -178,6 +179,33 @@ __global__ void __launch_bounds__(WARPS * 32) finalize_pearson_kernel(const T* _
       if (pos < (uint32_t)SPECIAL_CAP) special[pos] = (uint32_t)r;
     }
     snorm[r] = sn;
+  }
+}
+
+// JACCARD corpora with the count path's state (sdb_corpus_create): per row the first-occurrence bitmask (bit i of word
+// i / 32 set when no earlier element equals x_i under num_eq_f64, compared through eq_key_row) and the number of
+// distinct values u_x.  One warp per row, O(D^2 / 32) compares per lane (early exit on the first equal element).
+template <typename T>
+__global__ void __launch_bounds__(256) finalize_jaccard_kernel(const T* __restrict__ rows, uint32_t dim, uint64_t n,
+                                                               uint32_t* __restrict__ first, uint32_t* __restrict__ ux) {
+  const uint32_t lane = threadIdx.x & 31u, words = (dim + 31) / 32;
+  const uint64_t n_warps = ((uint64_t)gridDim.x * blockDim.x) >> 5;
+  for (uint64_t r = ((uint64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5; r < n; r += n_warps) {
+    const T* x = rows + r * dim;
+    uint32_t u = 0;
+    for (uint32_t w = 0; w < words; w++) {
+      const uint32_t i = w * 32 + lane;
+      bool f = false;
+      if (i < dim) {
+        const auto key = eq_key_row(x[i]);
+        f = true;
+        for (uint32_t j = 0; j < i && f; j++) f = eq_key_row(x[j]) != key;
+      }
+      const uint32_t bits = __ballot_sync(0xffffffffu, f);
+      if (lane == 0) first[r * words + w] = bits;
+      u += __popc(bits);
+    }
+    if (lane == 0) ux[r] = u;
   }
 }
 
@@ -526,6 +554,16 @@ sdb_status corpus_finalize_device(Corpus* c) {
       SDB_CUDA(cudaGetLastError());
     }
   }
+  if (c->n && c->metric == SDB_JACCARD && c->d_jfirst) {
+    if (c->dtype == SDB_F32)
+      finalize_jaccard_kernel<float><<<ctx->sm_count * 8, 256, 0, st>>>((const float*)c->d_rows.get(), c->dim, c->n,
+                                                                       c->d_jfirst, c->d_jux);
+    else
+      finalize_jaccard_kernel<double><<<ctx->sm_count * 8, 256, 0, st>>>((const double*)c->d_rows.get(), c->dim, c->n,
+                                                                        c->d_jfirst, c->d_jux);
+    count_launch(ctx);
+    SDB_CUDA(cudaGetLastError());
+  }
   c->n_outliers = 0;
   if (c->n && c->d_i8 && (c->metric == SDB_COSINE || centred)) {
     const uint64_t n_pad = (c->n + TILE_ROWS - 1) / TILE_ROWS * TILE_ROWS;
@@ -618,6 +656,8 @@ sdb_status corpus_finalize_device(Corpus* c) {
   uint32_t h[8] = {0, 0, 0, 0, 0, 0, 0, 0};
   SDB_CUDA(cudaMemcpyAsync(h, d_tmp, 32, cudaMemcpyDeviceToHost, st));
   SDB_CUDA(cudaStreamSynchronize(st));
+  // no special rows: zero, NaN and +-inf are ordinary values for equality
+  if (c->metric == SDB_HAMMING || c->metric == SDB_JACCARD) h[0] = 0;
   c->special_overflow = h[0] > (uint32_t)SPECIAL_CAP;
   c->n_special = h[0] > (uint32_t)SPECIAL_CAP ? (uint32_t)SPECIAL_CAP : h[0];
   float mn;

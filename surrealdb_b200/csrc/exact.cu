@@ -154,9 +154,7 @@ __global__ void __launch_bounds__(WARPS * 32) exact_keys_kernel(const T* __restr
 //   inter = #{j : in_row[j] or dup[j]}                  union = distinct(row) + #{j : not in_row[j] and not dup[j]}
 // Number equality on floats: same bits, or both zero (val/number.rs PartialEq; NaN == NaN when the payloads agree).
 // One warp per row, O(dim^2 / 32) comparisons per lane: a niche metric served for completeness, not for speed.
-__device__ __forceinline__ bool num_eq_f64(double a, double b) {
-  return __double_as_longlong(a) == __double_as_longlong(b) || (a == 0.0 && b == 0.0);
-}
+// (num_eq_f64: exactmath.cuh)
 __global__ void jaccard_qdup_kernel(const double* __restrict__ q64, uint32_t dim, uint8_t* __restrict__ dup) {
   for (uint32_t j = blockIdx.x * blockDim.x + threadIdx.x; j < dim; j += gridDim.x * blockDim.x) {
     bool d = false;

@@ -9,8 +9,78 @@
 // as a positive NaN and sorts LAST.  Mixed cases are unpinned (DESIGN.md section 3).
 #pragma once
 #include <cstdint>
+#include <type_traits>
 
 namespace sdb {
+
+// Number equality of two elements after the widening to f64 (val/number.rs PartialEq): the same bits, or both zero, so
+// 0.0 == -0.0 and NaN == NaN exactly when the bits agree.  HAMMING and JACCARD count with it everywhere.
+__device__ __forceinline__ bool num_eq_f64(double a, double b) {
+  return __double_as_longlong(a) == __double_as_longlong(b) || (a == 0.0 && b == 0.0);
+}
+// Keys that turn num_eq_f64 into one integer compare (the HAMMING count kernel, screen_lp.cu).
+//  - f64 rows and queries: the bits, -0.0 folded onto 0.0.
+//  - f32 rows: the key of (double)x, the exact kernel's widening, in 32 bits: x's own bits for a number (the widening
+//    is exact; -0.0 folded onto 0.0), sign | 0x7f800000 | fraction bits 51..29 of the widened value for a NaN, so that
+//    two NaNs get one key exactly when the device widens them to the same bits.
+//  - an f64 query element against f32 rows: the key of the f32 that widens to it bit for bit, or EQ_KEY_NONE when no
+//    f32 does; EQ_KEY_NONE is -0.0's pattern, which no row key takes.
+constexpr uint32_t EQ_KEY_NONE = 0x80000000u;
+__device__ __forceinline__ unsigned long long eq_key_f64(double x) {
+  const unsigned long long b = (unsigned long long)__double_as_longlong(x);
+  return (b << 1) == 0 ? 0ull : b;
+}
+__device__ __forceinline__ uint32_t eq_key_f32(float x) {
+  const double w = (double)x;
+  const unsigned long long b = (unsigned long long)__double_as_longlong(w);
+  if ((b << 1) == 0) return 0u;
+  if (w != w) return ((uint32_t)(b >> 32) & 0x80000000u) | 0x7f800000u | ((uint32_t)(b >> 29) & 0x7fffffu);
+  return __float_as_uint(x);
+}
+__device__ __forceinline__ uint32_t eq_qkey_f32(double q) {
+  const unsigned long long b = (unsigned long long)__double_as_longlong(q);
+  if ((b << 1) == 0) return 0u;
+  // the only f32 that can widen to q: q rounded for a number, q's sign and top fraction bits for a NaN
+  const uint32_t fb = q != q ? ((uint32_t)(b >> 32) & 0x80000000u) | 0x7f800000u | ((uint32_t)(b >> 29) & 0x7fffffu)
+                             : __float_as_uint(__double2float_rn(q));
+  const float f = __uint_as_float(fb);
+  if ((unsigned long long)__double_as_longlong((double)f) != b) return EQ_KEY_NONE;
+  return eq_key_f32(f);
+}
+
+template <typename T>
+using EqKey = typename std::conditional<sizeof(T) == 8, unsigned long long, uint32_t>::type;
+__device__ __forceinline__ uint32_t eq_key_row(float x) { return eq_key_f32(x); }
+__device__ __forceinline__ unsigned long long eq_key_row(double x) { return eq_key_f64(x); }
+
+// JACCARD (vector.rs:121-127 with v1 = the row, v2 = the query) from counts, as jaccard_keys_kernel computes it:
+// u_x / u_q = distinct values of the row / the query, m = values both share; inter = D - u_q + m,
+// union = u_x + u_q - m, result inter / union in one f64 division.  first: the row's first-occurrence bitmask (bit i
+// set when x_i is the first element of its value; popcount = u_x, finalize_jaccard_kernel); qk: the query's distinct
+// keys that some row element can have, sorted ascending (n_look of them).  m = first-occurrence elements of the row
+// whose key is among them: O(u_x log u_q) per pair.
+template <typename T>
+__device__ __forceinline__ double jaccard_counts(const T* __restrict__ x, uint32_t dim, const uint32_t* __restrict__ first,
+                                                 uint32_t ux, const EqKey<T>* __restrict__ qk, uint32_t n_look,
+                                                 uint32_t uq) {
+  uint32_t m = 0;
+  for (uint32_t w = 0; w * 32 < dim; w++) {
+    uint32_t b = __ldg(first + w);
+    while (b) {
+      const uint32_t i = w * 32 + (uint32_t)(__ffs(b) - 1);
+      b &= b - 1;
+      const EqKey<T> key = eq_key_row(__ldg(x + i));
+      uint32_t lo = 0, hi = n_look;
+      while (lo < hi) {
+        const uint32_t mid = (lo + hi) >> 1;
+        if (__ldg(qk + mid) < key) lo = mid + 1;
+        else hi = mid;
+      }
+      m += (lo < n_look && __ldg(qk + lo) == key) ? 1u : 0u;
+    }
+  }
+  return __ddiv_rn((double)(dim - uq + m), (double)(ux + uq - m));
+}
 
 struct ExactAcc {
   double acc = 0.0;
@@ -34,8 +104,7 @@ struct ExactAcc {
   __device__ __forceinline__ void chebyshev_step(double x, double q) { acc = fmax(acc, fabs(__dsub_rn(x, q))); }
   //   hamming  : vector.rs:111-116   count of a != b under Number's PartialEq (0.0 == -0.0, NaN == NaN bitwise)
   __device__ __forceinline__ void hamming_step(double x, double q) {
-    const bool eq = (__double_as_longlong(x) == __double_as_longlong(q)) || (x == 0.0 && q == 0.0);
-    acc = __dadd_rn(acc, eq ? 0.0 : 1.0);  // exact: an integer count below 2^53
+    acc = __dadd_rn(acc, num_eq_f64(x, q) ? 0.0 : 1.0);  // exact: an integer count below 2^53
   }
   //   minkowski: vector.rs:163-174   acc = acc + |x - q|^p ; finish: acc^(1/p).  pow() is CUDA's libm here and the
   //              platform libm in the reference: each call agrees to within an ulp or two, not bit for bit.

@@ -329,6 +329,9 @@ struct Scratch {
   DevBuf<int8_t> d_q8;        // int8 queries nq_pad x dim_pad8
   DevBuf<float> d_q8scale;    // max|q|/127 per query
   DevBuf<float> d_q8err;      // |q - dequant(q)| / |q| per query
+  DevBuf<uint32_t> d_qkey;    // count path, u32 keys for f32 rows, u64 for f64 rows: HAMMING: the queries' equality
+                              // keys; JACCARD: each query's distinct keys, sorted (count_prep_queries)
+  DevBuf<uint32_t> d_qjac;    // JACCARD count path: per query {u_q, n_look}, then scratch flags [nq][dim]
   DevBuf<uint32_t> d_mscale;  // MINKOWSKI screen: [0] the batch's largest |q^_i| (f32 bits), [1] its scale exponent e
   DevBuf<Cand> d_sub;         // thread-private candidate sub-lists of the tensor-core screens
   DevBuf<uint32_t> d_sub_cnt; // [nq][sub_slots]
@@ -384,6 +387,8 @@ struct Corpus : Scratch {
   DevBuf<double> d_mag;          // exact f64 magnitude per row (reference arithmetic)
   DevBuf<float> d_snorm;         // cosine: 1/|x| ; euclid: |x|^2 ; pearson: 1/|x - m1| ; NaN = never a screen candidate
   DevBuf<double2> d_mom;         // PEARSON corpora with screen copies: {m1, S1} per row (finalize_pearson_kernel)
+  DevBuf<uint32_t> d_jfirst;     // JACCARD corpora (when it fits): first-occurrence bitmask [cap][ceil(dim / 32)]
+  DevBuf<uint32_t> d_jux;        // ... and the number of distinct values per row
   DevBuf<__nv_bfloat16> d_bf16;  // screen copy cap_pad x dim_pad (rows padded to TILE_ROWS)
   float bf16_rel_err = 0.00390625f; // max over rows of |x - bf16(x)| / |x| (measured at finalize, rounded up)
   DevBuf<int8_t> d_i8;           // int8 screen copy cap_pad x dim_pad8 of the normalised rows (one global scale), cosine only
@@ -432,6 +437,18 @@ inline bool lp_screened(const Corpus* c) {
   return c->metric == SDB_MANHATTAN || c->metric == SDB_CHEBYSHEV || minkowski_screen_order(c) > 0;
 }
 
+// HAMMING, and JACCARD corpora that hold their first-occurrence state: the count path's per-batch query state
+// (count_prep_queries) and re-rank.  With 1 <= k <= 256 and any screen but NONE_EXACT they are ranked by exact counts
+// of every row, per row range (count_pass), then cand_final with tau = -inf.  NONE_EXACT and k > 256 keep the exact
+// kernel.
+constexpr uint32_t COUNT_CAP_MAX = 16384;  // candidate entries per query of the count path: n_ranges k at most
+inline bool count_metric(const Corpus* c) {
+  return c->metric == SDB_HAMMING || (c->metric == SDB_JACCARD && c->d_jfirst);
+}
+inline bool count_ranked(const Corpus* c, uint32_t k) {
+  return count_metric(c) && k >= 1 && k <= 256 && c->screen != SDB_SCREEN_NONE_EXACT;
+}
+
 // ---- launch wrappers (defined in the .cu files) ---------------------------------------------------
 // corpus.cu
 sdb_status corpus_finalize_device(Corpus* c);
@@ -441,6 +458,12 @@ sdb_status corpus_reapply_tombstones(Corpus* c, cudaStream_t st);
 sdb_status screen_simt_pass(Corpus* c, uint32_t nq, const PassDesc& p, cudaStream_t st);
 // screen_lp.cu: f32 L1 / L-infinity / Lp screen (score = -s~), f32 and f64 rows
 sdb_status screen_lp_pass(Corpus* c, uint32_t nq, const PassDesc& p, cudaStream_t st);
+// ... and the HAMMING / JACCARD count path: rows split into count_ranges() ranges, each query's candidate entries
+// (cnt, rr_*) = the union of its ranges' k best (distance, row) pairs with their exact distances; needs prep_queries
+// (which runs count_prep_queries for count_metric corpora) and cand_begin
+uint32_t count_ranges(const Corpus* c, uint32_t nq, uint32_t k);
+sdb_status count_prep_queries(Corpus* c, uint32_t nq, cudaStream_t st);
+sdb_status count_pass(Corpus* c, uint32_t nq, uint32_t k, cudaStream_t st);
 // screen_tc.cu
 // mode 0: pass 0 (every score of the pass's tiles written to fixed slots), 1: threshold pass, 2: streaming pass with
 // in-kernel threshold refinement (histogram + refiner warp), 3: probe (chunk maxima of a few tiles, no candidates)

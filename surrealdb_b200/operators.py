@@ -30,11 +30,12 @@ class Distance:
     Euclidean = "Euclidean"      # bf16 tensor-core screen + exact re-rank
     Manhattan = "Manhattan"      # this and Chebyshev: the f32 L1 / L-infinity screen + exact re-rank
     Chebyshev = "Chebyshev"
-    Hamming = "Hamming"          # exact kernel only (no screen)
+    Hamming = "Hamming"          # exact mismatch counts batched over the queries (k <= 256); k > 256: exact kernel
     Pearson = "Pearson"          # the cosine screens on the centred rows + exact re-rank
     Minkowski = "Minkowski"      # order via VectorColumn.set_minkowski_order: integer orders 1-8 on the f32 Lp screen
                                  # + exact re-rank, every other order on the exact kernel (pow(): ~1e-14 relative)
-    Jaccard = "Jaccard"          # exact kernel, set semantics over the values
+    Jaccard = "Jaccard"          # set semantics over the values: exact distinct / shared counts batched over the
+                                 # queries (k <= 256); k > 256: exact kernel
 
 
 class KnnContext(dict):
