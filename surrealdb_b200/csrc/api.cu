@@ -101,37 +101,36 @@ struct Rung {
 // to more than a handful of queries the batch is re-screened with a tighter screen / longer lists instead of paying
 // one exact pass over the corpus per failed query; the rung that worked is remembered per corpus and k.
 static std::vector<Rung> build_rungs(Corpus* c, uint32_t k, uint32_t nq, sdb_screen* first) {
-  // PEARSON: the cosine screens on the centred rows when the corpus holds their copies and moments (sdb_corpus_create)
-  const bool pearson = c->metric == SDB_PEARSON && c->d_mom;
-  const bool int8_ok = c->d_i8 && (c->metric == SDB_COSINE || pearson) && screen_tc_available();
+  const Family f = family(c);
+  const bool int8_ok = c->d_i8 && screen_tc_available();  // (COSINE and Centred corpora hold an int8 copy)
   sdb_screen scr = c->screen;
   if (scr == SDB_SCREEN_AUTO)
     scr = !screen_tc_available() ? SDB_SCREEN_SIMT_F32
                                  : (int8_ok && c->max_rel_qerr <= 0.02f ? SDB_SCREEN_TC_INT8 : SDB_SCREEN_TC_BF16);
   if (scr == SDB_SCREEN_TC_INT8 && !int8_ok) scr = SDB_SCREEN_TC_BF16;
+  // (Lp corpora hold no bf16 copy: the f32 Lp screen, screen_lp.cu, is their only screen, for f32 and f64 rows)
   if (scr == SDB_SCREEN_TC_BF16 && (!screen_tc_available() || !c->d_bf16)) scr = SDB_SCREEN_SIMT_F32;
-  // MANHATTAN / CHEBYSHEV / MINKOWSKI of an integer order 1 .. 8: the f32 Lp screen (screen_lp.cu) is their only
-  // screen, for f32 and f64 rows; MINKOWSKI of any other order stays on the exact kernel (!screenable below)
-  const bool lp = lp_screened(c);
-  const bool screenable = c->metric == SDB_COSINE || c->metric == SDB_EUCLIDEAN || lp || pearson;
-  // the SIMT screen streams f32 rows: an f64 cosine / euclidean corpus is screened on the tensor cores or not at all,
-  // and so is a PEARSON one of either type (the SIMT screen would need the centred rows)
-  if ((c->dtype == SDB_F64 || pearson) && scr == SDB_SCREEN_SIMT_F32 && !lp) scr = SDB_SCREEN_NONE_EXACT;
-  if (c->special_overflow || k > 256 || !screenable) scr = SDB_SCREEN_NONE_EXACT;
+  // the SIMT screen streams f32 rows: an f64 Dot corpus is screened on the tensor cores or not at all, and so is a
+  // Centred one of either type (the SIMT screen would need the centred rows)
+  if ((f == Family::Centred || (f == Family::Dot && c->dtype == SDB_F64)) && scr == SDB_SCREEN_SIMT_F32)
+    scr = SDB_SCREEN_NONE_EXACT;
+  // (Count: the count path, enqueue_counted, or the exact kernel)
+  if (c->special_overflow || k > 256 || f == Family::Count || f == Family::Exact) scr = SDB_SCREEN_NONE_EXACT;
   // MANHATTAN / CHEBYSHEV: a single query streams the rows once either way, and the exact kernel does it at the higher
   // HBM rate (DESIGN.md section 5): AUTO ranks it there; an explicit SIMT_F32 request is kept.  MINKOWSKI's exact
   // kernel is bound by its f64 pow() calls, not by HBM, and the screen is faster for a single query too (section 5).
-  if (lp && c->metric != SDB_MINKOWSKI && nq == 1 && c->screen == SDB_SCREEN_AUTO) scr = SDB_SCREEN_NONE_EXACT;
+  if (f == Family::Lp && c->metric != SDB_MINKOWSKI && nq == 1 && c->screen == SDB_SCREEN_AUTO)
+    scr = SDB_SCREEN_NONE_EXACT;
   *first = scr;
   std::vector<Rung> r;
   if (scr == SDB_SCREEN_TC_INT8)
     r = {{SDB_SCREEN_TC_INT8, 4096}, {SDB_SCREEN_TC_INT8, 16384}, {SDB_SCREEN_TC_BF16, 4096}, {SDB_SCREEN_TC_BF16, 16384}};
   else if (scr == SDB_SCREEN_TC_BF16) r = {{SDB_SCREEN_TC_BF16, 4096}, {SDB_SCREEN_TC_BF16, 16384}};
-  else if (scr == SDB_SCREEN_SIMT_F32 && lp) r = {{SDB_SCREEN_SIMT_F32, 4096}, {SDB_SCREEN_SIMT_F32, 16384}};
+  else if (scr == SDB_SCREEN_SIMT_F32 && f == Family::Lp) r = {{SDB_SCREEN_SIMT_F32, 4096}, {SDB_SCREEN_SIMT_F32, 16384}};
   else if (scr == SDB_SCREEN_SIMT_F32) r = {{SDB_SCREEN_SIMT_F32, 4096}};
   // the f32 stream (error bound ~500x tighter than bf16) as the last rung before the exact kernel -- only ever used
   // for the few queries of a batch that every tensor-core rung failed to prove (finish_local), never for a whole batch
-  if (!r.empty() && r.back().scr != SDB_SCREEN_SIMT_F32 && c->dtype == SDB_F32 && !pearson)
+  if (!r.empty() && r.back().scr != SDB_SCREEN_SIMT_F32 && c->dtype == SDB_F32 && f == Family::Dot)
     r.push_back({SDB_SCREEN_SIMT_F32, 4096});
   return r;
 }
@@ -433,8 +432,9 @@ static sdb_status enqueue_screened(Corpus* c, Ticket& t) {
         set_error("query cancelled");
         return SDB_ECANCELLED;
       }
-      if (!tc) SDB_TRY(screen_simt_pass(c, nq, p, st));
-      else SDB_TRY(screen_tc_pass(c, nq, k, p, int8, first_pass ? 0 : 1, st));
+      if (tc) SDB_TRY(screen_tc_pass(c, nq, k, p, int8, first_pass ? 0 : 1, st));
+      else if (family(c) == Family::Lp) SDB_TRY(screen_lp_pass(c, nq, p, st));
+      else SDB_TRY(screen_simt_pass(c, nq, p, st));
       if (c->tap) SDB_TRY(tap_gathered(c, nq, tc ? c->last_slots : 0u, st));
       SDB_TRY(cand_select(c, nq, k, int8, tc ? c->last_slots : 0u, false, st));
       first_pass = false;
@@ -660,11 +660,11 @@ static void plan_filtered(const Corpus* c, Ticket& t, uint32_t nq, uint32_t k, c
   t.filt.bits = d_filters;
   t.filt.words = (uint32_t)((c->n + 31) / 32);
   // direct regime: a query whose filter passes at most DIRECT_MAX_ROWS rows (filter_rows: set bits, an upper bound
-  // of the rows it passes) skips the screen; the re-rank and cand_final serve the screenable metrics and the HAMMING
-  // count path, k <= 256
+  // of the rows it passes) skips the screen; the re-rank and cand_final serve every family but Exact (Count: when the
+  // count path would rank the batch), k <= 256
+  const Family f = family(c);
   const bool direct_ok = filter_rows && k > 0 && k <= 256 &&
-                         (c->metric == SDB_COSINE || c->metric == SDB_EUCLIDEAN || lp_screened(c) ||
-                          (c->metric == SDB_PEARSON && c->d_mom) || count_ranked(c, k));
+                         (f == Family::Dot || f == Family::Centred || f == Family::Lp || count_ranked(c, k));
   for (uint32_t q = 0; q < nq; q++) {
     const uint64_t rows_q = filter_rows ? filter_rows[t.h_qf[q]] : ~0ull;
     if (direct_ok && rows_q <= DIRECT_MAX_ROWS) dir->push_back(q);
@@ -1103,12 +1103,11 @@ sdb_status sdb_corpus_create(sdb_ctx* ctx, uint32_t dim, sdb_dtype dt, sdb_metri
     set_error("sdb_corpus_create: bad argument (dim 1..65535, 0 < capacity < 2^32)");
     return SDB_EINVAL;
   }
-  // COSINE / EUCLIDEAN: screened (K1/K2) + exact re-rank.  MANHATTAN / CHEBYSHEV: the f32 L1 / L-infinity screen
-  // (screen_lp.cu) + exact re-rank.  PEARSON: the cosine tensor-core screens on the centred rows + exact re-rank.
-  // MINKOWSKI of integer order 1 .. 8: the f32 Lp screen + exact re-rank; of any other order, like HAMMING / JACCARD:
-  // served by the exact kernel alone (sequential f64, Distance::compute op for op).  MINKOWSKI goes through
-  // pow(), which CUDA's libm and Rust's (the platform libm) implement separately: within 1 ulp of each other per term,
-  // so its distances are compared with a 1e-12 relative tolerance instead of bit equality (tests/test_gpu_knn.py).
+  // The buffers of each metric's family (Family, internal.cuh): COSINE / EUCLIDEAN the screen copies, PEARSON also
+  // the moments, JACCARD the count path's first-occurrence state; the Lp screen and HAMMING's count path read the rows.
+  // MINKOWSKI goes through pow(), which CUDA's libm and Rust's (the platform libm) implement separately: within 1 ulp of
+  // each other per term, so its distances are compared with a 1e-12 relative tolerance instead of bit equality with the
+  // CPU oracle (tests/test_gpu_knn.py).
   const bool screenable = m == SDB_COSINE || m == SDB_EUCLIDEAN;
   if ((int)m < 0 || (int)m > (int)SDB_PEARSON) {
     set_error("unknown metric %d", (int)m);
@@ -1438,8 +1437,10 @@ sdb_status sdb_debug_corpus_state(sdb_corpus* c, float* out_f, uint32_t* out_u, 
                                   float* out_snorm, uint32_t* out_special) {
   if (!c) return SDB_EINVAL;
   std::lock_guard<std::mutex> g(c->mu);
+  // MINKOWSKI of every order, not only Family::Lp: finalize prepares its state for every order (it may change later)
   const bool lp = c->metric == SDB_MANHATTAN || c->metric == SDB_CHEBYSHEV || c->metric == SDB_MINKOWSKI;
-  if (!c->finalized || (c->dtype != SDB_F32 && !c->d_bf16 && !lp) || (c->metric == SDB_PEARSON && !c->d_mom) ||
+  if (!c->finalized || (c->dtype != SDB_F32 && !c->d_bf16 && !lp) ||
+      (c->metric == SDB_PEARSON && family(c) != Family::Centred) ||
       (out_i8 && !c->d_i8) || (out_bf16 && !c->d_bf16)) {
     set_error("sdb_debug_corpus_state: needs a finalized F32 corpus or a screened F64 / PEARSON one (int8 copy: "
               "cosine and pearson only)");
@@ -1498,15 +1499,13 @@ sdb_status sdb_debug_screen_batch_filtered(sdb_corpus* c, const double* queries,
   if (filters) SDB_TRY(check_filters(nq, filters, n_filters, query_filter));
   std::lock_guard<std::mutex> g(c->mu);
   const bool int8 = screen == SDB_SCREEN_TC_INT8;
-  // MANHATTAN / CHEBYSHEV / MINKOWSKI of a screened order: the SIMT_F32 (L1 / L-infinity / Lp) screen, f32 and f64
-  const bool lp = lp_screened(c) && screen == SDB_SCREEN_SIMT_F32;
-  // f64 rows: tensor-core screens only (cosine / euclidean)
-  const bool f64_ok = c->dtype == SDB_F64 && ((tc && c->d_bf16) || lp);
-  // PEARSON (f32 and f64 rows): the cosine tensor-core screens on the centred rows
-  const bool pearson = c->metric == SDB_PEARSON && c->d_mom && tc;
-  if (!c->finalized || (c->dtype != SDB_F32 && !f64_ok) ||
-      (c->metric != SDB_COSINE && c->metric != SDB_EUCLIDEAN && !lp && !pearson) ||
-      (c->metric == SDB_PEARSON && !pearson) || (int8 && !c->d_i8) || c->special_overflow || !c->n) {
+  // Dot: any screen on f32 rows, the tensor cores on f64 ones; Centred: the tensor cores; Lp: SIMT_F32 (the Lp screen)
+  const Family f = family(c);
+  const bool served = f == Family::Dot       ? c->dtype == SDB_F32 || (tc && c->d_bf16)
+                      : f == Family::Centred ? tc
+                      : f == Family::Lp      ? screen == SDB_SCREEN_SIMT_F32
+                                             : false;
+  if (!c->finalized || !served || (int8 && !c->d_i8) || c->special_overflow || !c->n) {
     set_error("sdb_debug_screen_batch: needs a finalized, non-empty F32 cosine / euclidean corpus, an F64 one with "
               "screen copies and a tensor-core screen (int8: cosine), a PEARSON one with screen copies and a "
               "tensor-core screen, or a MANHATTAN / CHEBYSHEV / MINKOWSKI (integer order 1 .. 8) one with SIMT_F32");
@@ -1565,7 +1564,9 @@ sdb_status sdb_debug_screen_batch_filtered(sdb_corpus* c, const double* queries,
       SDB_TRY(prep_queries(c, d_q, nq, st));
       SDB_TRY(cand_begin(c, nq, (int)screen, st));
       c->filt = t->filt;
-      sdb_status rc = tc ? screen_tc_pass(c, nq, k, all, int8, 0, st) : screen_simt_pass(c, nq, all, st);
+      sdb_status rc = tc                ? screen_tc_pass(c, nq, k, all, int8, 0, st)
+                      : f == Family::Lp ? screen_lp_pass(c, nq, all, st)
+                                        : screen_simt_pass(c, nq, all, st);
       c->filt = FiltArg();
       SDB_TRY(rc);
       SDB_TRY(tap_list(c, nq, &tap.list_a, &tap.cnt_a, st));

@@ -12,9 +12,6 @@
 
 namespace sdb {
 
-// PEARSON corpora that hold the centred screen copies and the row moments (sdb_corpus_create reserves them if they fit)
-static bool pearson_screened(const Corpus* c) { return c->metric == SDB_PEARSON && c->d_mom; }
-
 // ------------------------------------------------------------------------------------------------
 __global__ void prep_queries_kernel(const double* __restrict__ q64, uint32_t dim, uint32_t dim_pad, int metric,
                                     float* __restrict__ q32, __nv_bfloat16* __restrict__ qbf, double* __restrict__ qmag,
@@ -61,7 +58,8 @@ __global__ void prep_queries_kernel(const double* __restrict__ q64, uint32_t dim
     uint32_t f = s_flags;
     if (metric == SDB_COSINE && (!(m > 0.0) || !isfinite(m))) f |= 1u;
     if (metric != SDB_COSINE && !isfinite(m)) f |= 1u;
-    if (metric == SDB_HAMMING || metric == SDB_JACCARD) f &= ~1u;  // counts are exact for any value: zero, inf, NaN
+    // counts are exact for any value: zero, inf, NaN (a fact of the metric: JACCARD's exact kernel relies on it too)
+    if (metric == SDB_HAMMING || metric == SDB_JACCARD) f &= ~1u;
     qflags[q] = f;
     // |q - bf16(q)| / |q|, rounded up; + 2^-23 for the f64 -> f32 rounding of the query itself
     if (qbferr) qbferr[q] = (m > 0.0 && isfinite(m)) ? (sqrtf(s_err2) / (float)m) * 1.0001f + 2.4e-7f : 1.f;
@@ -195,6 +193,25 @@ __global__ void __launch_bounds__(128) prep_queries_i8_kernel(const float* __res
 // e_x = max_rows |x - bf16(x)|/|x| (finalize) and e_q = |q - bf16(q)|/|q| (prep) -- at most 2^-8 each -- plus fp32
 // accumulation D * 2^-21 and 1e-5 for the f32 screening norm; int8  (1 + e_q) e_x + e_q  (integer accumulation is
 // exact); f32 SIMT (D/16 + 16) * 2^-23.
+// begin_query: what every cand_begin_* kernel leaves per query -- tau = -inf, an empty list, no flags, the bounds above
+// (stage B's margin2 / beps2, tau2 = -inf) and the score range qlow .. qcap
+__device__ __forceinline__ void begin_query(
+    uint32_t q, float* __restrict__ tau, uint32_t* __restrict__ cnt, uint32_t* __restrict__ flags,
+    float* __restrict__ bscale, float* __restrict__ beps, float* __restrict__ margin, float* __restrict__ margin2,
+    float* __restrict__ beps2, float* __restrict__ tau2, float* __restrict__ qlow, float* __restrict__ qcap, float bs,
+    float eps, float mg, float mg2, float e2, float lo, float hi) {
+  tau[q] = __int_as_float(0xff800000);  // -inf
+  cnt[q] = 0;
+  flags[q] = 0;
+  bscale[q] = bs;
+  beps[q] = eps;
+  margin[q] = mg;
+  margin2[q] = mg2;
+  beps2[q] = e2;
+  tau2[q] = __int_as_float(0xff800000);
+  qlow[q] = lo;
+  qcap[q] = hi;
+}
 __global__ void cand_begin_kernel(float* __restrict__ tau, uint32_t* __restrict__ cnt, uint32_t* __restrict__ flags,
                                   uint32_t* __restrict__ stat, float* __restrict__ bscale, float* __restrict__ beps,
                                   float* __restrict__ margin, float* __restrict__ margin2, float* __restrict__ beps2,
@@ -211,9 +228,6 @@ __global__ void cand_begin_kernel(float* __restrict__ tau, uint32_t* __restrict_
     stat[3] = 0;
   }
   if (q >= nq) return;
-  tau[q] = __int_as_float(0xff800000);  // -inf
-  cnt[q] = 0;
-  flags[q] = 0;
   const double qm = qmag[q];
   // f64 rows, cosine: products q_i x_i below 2^-126 may be flushed by the tensor cores (and lose their low bits in
   // stage B's f32 FMA chain), an ABSOLUTE dot error of at most D 2^-126 that no relative term covers.  Screened f64
@@ -266,14 +280,9 @@ __global__ void cand_begin_kernel(float* __restrict__ tau, uint32_t* __restrict_
     mg2 = 2.1 * e2;
   }
   if (!exact || !(qm > 0.0) || !isfinite(qm) || !isfinite(mg2)) mg2 = 0.0;
-  bscale[q] = (float)bs;
-  beps[q] = __double2float_ru(eps);
-  margin[q] = __double2float_ru(mg);
-  margin2[q] = __double2float_ru(mg2);
-  beps2[q] = __double2float_ru(e2);
-  tau2[q] = __int_as_float(0xff800000);
-  qlow[q] = __double2float_rd(lo);
-  qcap[q] = __double2float_ru(hi);
+  begin_query(q, tau, cnt, flags, bscale, beps, margin, margin2, beps2, tau2, qlow, qcap, (float)bs,
+              __double2float_ru(eps), __double2float_ru(mg), __double2float_ru(mg2), __double2float_ru(e2),
+              __double2float_rd(lo), __double2float_ru(hi));
 }
 // The same for MANHATTAN / CHEBYSHEV corpora (screen_lp.cu: score = -s~), one warp per query.  beps bounds |s~ - d|
 // for every screened row, d = the reference's distance (sequential f64 over the f64 values).  With u = 2^-24,
@@ -331,17 +340,8 @@ __global__ void __launch_bounds__(128) cand_begin_lp_kernel(float* __restrict__ 
     lo = -1.0;
   }
   if (!exact) mg = 0.0;
-  tau[q] = __int_as_float(0xff800000);  // -inf
-  cnt[q] = 0;
-  flags[q] = 0;
-  bscale[q] = 1.f;
-  beps[q] = __double2float_ru(eps);
-  margin[q] = __double2float_ru(mg);
-  margin2[q] = 0.f;
-  beps2[q] = 0.f;
-  tau2[q] = __int_as_float(0xff800000);
-  qlow[q] = __double2float_rd(lo);
-  qcap[q] = __double2float_ru(hi);
+  begin_query(q, tau, cnt, flags, bscale, beps, margin, margin2, beps2, tau2, qlow, qcap, 1.f, __double2float_ru(eps),
+              __double2float_ru(mg), 0.f, 0.f, __double2float_rd(lo), __double2float_ru(hi));
 }
 
 // MINKOWSKI of integer order p (1 .. 8, minkowski_screen_order): the launch's scale first.  The screen multiplies
@@ -431,62 +431,50 @@ __global__ void __launch_bounds__(128) cand_begin_minkowski_kernel(
     lo = -1.0;
   }
   if (!exact) mg = 0.0;
-  tau[q] = __int_as_float(0xff800000);  // -inf
-  cnt[q] = 0;
-  flags[q] = 0;
-  bscale[q] = 1.f;
-  beps[q] = __double2float_ru(eps);
-  margin[q] = __double2float_ru(mg);
-  margin2[q] = 0.f;
-  beps2[q] = 0.f;
-  tau2[q] = __int_as_float(0xff800000);
-  qlow[q] = __double2float_rd(lo);
-  qcap[q] = __double2float_ru(hi);
+  begin_query(q, tau, cnt, flags, bscale, beps, margin, margin2, beps2, tau2, qlow, qcap, 1.f, __double2float_ru(eps),
+              __double2float_ru(mg), 0.f, 0.f, __double2float_rd(lo), __double2float_ru(hi));
 }
 
-// MANHATTAN / CHEBYSHEV / screened MINKOWSKI: the f32 Lp screen's bound, re-rank and proof
-static bool lp_metric(const Corpus* c) { return lp_screened(c); }
-
 sdb_status cand_begin(Corpus* c, uint32_t nq, int screen, cudaStream_t st) {
-  if (pearson_screened(c)) {
-    // the cosine bounds of the centred operands with the F64 terms (the rows are centred in f64, whatever their type);
-    // the gap between their cosine and the reference's pearson is cand_final's eps_ref
-    cand_begin_kernel<<<(nq + 255) / 256, 256, 0, st>>>(c->d_tau, c->d_cand_cnt, c->d_flags, c->d_stat, c->d_bscale,
-                                                        c->d_beps, c->d_margin, c->d_margin2, c->d_beps2, c->d_tau2,
-                                                        c->d_qlow, c->d_qcap, c->d_qmag, c->d_q8scale, c->d_q8err,
-                                                        c->d_qbferr, nq, screen, (int)SDB_COSINE, c->dim,
-                                                        c->max_rel_qerr, c->i8_scale, c->bf16_rel_err, c->max_norm,
-                                                        c->exact ? 1 : 0, 1);
-    count_launch(c->ctx);
-    SDB_CUDA(cudaGetLastError());
-    return SDB_OK;
+  switch (family(c)) {
+    case Family::Lp:
+      if (const int p = minkowski_screen_order(c)) {
+        SDB_CUDA(cudaMemsetAsync(c->d_mscale, 0, sizeof(uint32_t), st));
+        minkowski_batch_max_kernel<<<(nq + 3) / 4, 128, 0, st>>>(c->d_q32, c->d_qflags, nq, c->dim, c->d_mscale);
+        cand_begin_minkowski_kernel<<<(nq + 3) / 4, 128, 0, st>>>(c->d_tau, c->d_cand_cnt, c->d_flags, c->d_stat,
+                                                                  c->d_bscale, c->d_beps, c->d_margin, c->d_margin2,
+                                                                  c->d_beps2, c->d_tau2, c->d_qlow, c->d_qcap, c->d_q32,
+                                                                  nq, c->dim, p, c->max_norm, c->d_mscale,
+                                                                  c->exact ? 1 : 0);
+        count_launch(c->ctx);
+      } else {
+        cand_begin_lp_kernel<<<(nq + 3) / 4, 128, 0, st>>>(c->d_tau, c->d_cand_cnt, c->d_flags, c->d_stat,
+                                                           c->d_bscale, c->d_beps, c->d_margin, c->d_margin2,
+                                                           c->d_beps2, c->d_tau2, c->d_qlow, c->d_qcap, c->d_q32, nq,
+                                                           (int)c->metric, c->dim, c->max_norm, c->exact ? 1 : 0);
+      }
+      break;
+    case Family::Centred:
+      // the cosine bounds of the centred operands with the F64 terms (the rows are centred in f64, whatever their
+      // type); the gap between their cosine and the reference's pearson is cand_final's eps_ref
+      cand_begin_kernel<<<(nq + 255) / 256, 256, 0, st>>>(c->d_tau, c->d_cand_cnt, c->d_flags, c->d_stat, c->d_bscale,
+                                                          c->d_beps, c->d_margin, c->d_margin2, c->d_beps2, c->d_tau2,
+                                                          c->d_qlow, c->d_qcap, c->d_qmag, c->d_q8scale, c->d_q8err,
+                                                          c->d_qbferr, nq, screen, (int)SDB_COSINE, c->dim,
+                                                          c->max_rel_qerr, c->i8_scale, c->bf16_rel_err, c->max_norm,
+                                                          c->exact ? 1 : 0, 1);
+      break;
+    case Family::Dot:
+    case Family::Count:  // (Count, Exact: the reset of tau, counts, flags and stat; their bounds go unused)
+    case Family::Exact:
+      cand_begin_kernel<<<(nq + 255) / 256, 256, 0, st>>>(c->d_tau, c->d_cand_cnt, c->d_flags, c->d_stat, c->d_bscale,
+                                                          c->d_beps, c->d_margin, c->d_margin2, c->d_beps2, c->d_tau2,
+                                                          c->d_qlow, c->d_qcap, c->d_qmag, c->d_q8scale, c->d_q8err,
+                                                          c->d_qbferr, nq, screen, (int)c->metric, c->dim,
+                                                          c->max_rel_qerr, c->i8_scale, c->bf16_rel_err, c->max_norm,
+                                                          c->exact ? 1 : 0, c->dtype == SDB_F64 ? 1 : 0);
+      break;
   }
-  if (const int p = minkowski_screen_order(c)) {
-    SDB_CUDA(cudaMemsetAsync(c->d_mscale, 0, sizeof(uint32_t), st));
-    minkowski_batch_max_kernel<<<(nq + 3) / 4, 128, 0, st>>>(c->d_q32, c->d_qflags, nq, c->dim, c->d_mscale);
-    cand_begin_minkowski_kernel<<<(nq + 3) / 4, 128, 0, st>>>(c->d_tau, c->d_cand_cnt, c->d_flags, c->d_stat,
-                                                              c->d_bscale, c->d_beps, c->d_margin, c->d_margin2,
-                                                              c->d_beps2, c->d_tau2, c->d_qlow, c->d_qcap, c->d_q32, nq,
-                                                              c->dim, p, c->max_norm, c->d_mscale, c->exact ? 1 : 0);
-    count_launch(c->ctx, 2);
-    SDB_CUDA(cudaGetLastError());
-    return SDB_OK;
-  }
-  if (lp_metric(c)) {
-    cand_begin_lp_kernel<<<(nq + 3) / 4, 128, 0, st>>>(c->d_tau, c->d_cand_cnt, c->d_flags, c->d_stat, c->d_bscale,
-                                                       c->d_beps, c->d_margin, c->d_margin2, c->d_beps2, c->d_tau2,
-                                                       c->d_qlow, c->d_qcap, c->d_q32, nq, (int)c->metric, c->dim,
-                                                       c->max_norm, c->exact ? 1 : 0);
-    count_launch(c->ctx);
-    SDB_CUDA(cudaGetLastError());
-    return SDB_OK;
-  }
-  cand_begin_kernel<<<(nq + 255) / 256, 256, 0, st>>>(c->d_tau, c->d_cand_cnt, c->d_flags, c->d_stat, c->d_bscale, c->d_beps,
-                                                      c->d_margin, c->d_margin2, c->d_beps2, c->d_tau2, c->d_qlow, c->d_qcap,
-                                                      c->d_qmag, c->d_q8scale,
-                                                      c->d_q8err, c->d_qbferr, nq, screen, (int)c->metric, c->dim,
-                                                      c->max_rel_qerr, c->i8_scale, c->bf16_rel_err, c->max_norm,
-                                                      c->exact ? 1 : 0, c->dtype == SDB_F64 ? 1 : 0);
   count_launch(c->ctx);
   SDB_CUDA(cudaGetLastError());
   return SDB_OK;
@@ -505,7 +493,6 @@ static sdb_status ensure_scratch(Corpus* c, uint32_t nq, uint32_t cap) {
     SDB_CUDA(s.d_q32.reserve((size_t)nqa * c->dim));
     SDB_CUDA(s.d_qbf16.reserve((size_t)nqa * c->dim_pad));
     SDB_CUDA(s.d_qmag.reserve(nqa));
-    if (pearson_screened(c)) SDB_CUDA(s.d_qmom.reserve(nqa));
     SDB_CUDA(s.d_qflags.reserve(nqa));
     SDB_CUDA(s.d_qbferr.reserve(nqa));
     SDB_CUDA(s.d_tau.reserve(nqa));
@@ -520,8 +507,14 @@ static sdb_status ensure_scratch(Corpus* c, uint32_t nq, uint32_t cap) {
     SDB_CUDA(s.d_q8scale.reserve(nqa));
     SDB_CUDA(s.d_q8err.reserve(nqa));
     SDB_CUDA(s.d_mscale.reserve(2));
-    if (count_metric(c)) SDB_CUDA(s.d_qkey.reserve((size_t)nqa * c->dim * (c->dtype == SDB_F64 ? 2 : 1)));
-    if (c->metric == SDB_JACCARD && c->d_jfirst) SDB_CUDA(s.d_qjac.reserve((size_t)nqa * (2 + c->dim)));
+    switch (family(c)) {
+      case Family::Centred: SDB_CUDA(s.d_qmom.reserve(nqa)); break;
+      case Family::Count:
+        SDB_CUDA(s.d_qkey.reserve((size_t)nqa * c->dim * (c->dtype == SDB_F64 ? 2 : 1)));
+        if (c->metric == SDB_JACCARD) SDB_CUDA(s.d_qjac.reserve((size_t)nqa * (2 + c->dim)));
+        break;
+      default: break;
+    }
     SDB_CUDA(s.d_bscale.reserve(nqa));
     SDB_CUDA(s.d_beps.reserve(nqa));
     SDB_CUDA(s.d_margin.reserve(nqa));
@@ -556,14 +549,15 @@ sdb_status prep_queries(Corpus* c, const double* d_queries, uint32_t nq, cudaStr
   if (d_queries != c->d_q64)
     SDB_CUDA(cudaMemcpyAsync(c->d_q64, d_queries, sizeof(double) * (size_t)nq * c->dim, cudaMemcpyDeviceToDevice, st));
   const uint32_t nq_pad = (nq + 127) / 128 * 128;
-  if (pearson_screened(c))
+  const Family f = family(c);
+  if (f == Family::Centred)
     prep_queries_pearson_kernel<<<nq_pad, 128, 0, st>>>(c->d_q64, c->dim, c->dim_pad, c->d_q32, c->d_qbf16, c->d_qmag,
                                                         c->d_qmom, c->d_qflags, c->d_qbferr, nq);
   else
     prep_queries_kernel<<<nq_pad, 128, 0, st>>>(c->d_q64, c->dim, c->dim_pad, (int)c->metric, c->d_q32, c->d_qbf16,
                                                 c->d_qmag, c->d_qflags, c->d_qbferr, nq);
   count_launch(c->ctx);
-  if (count_metric(c)) SDB_TRY(count_prep_queries(c, nq, st));
+  if (f == Family::Count) SDB_TRY(count_prep_queries(c, nq, st));
   if (c->d_i8) {
     prep_queries_i8_kernel<<<nq_pad, 128, 0, st>>>(c->d_q32, c->d_qmag, c->dim, c->dim_pad8, nq, c->d_q8, c->d_q8scale,
                                                    c->d_q8err);
@@ -1033,24 +1027,31 @@ sdb_status cand_refine(Corpus* c, uint32_t nq, cudaStream_t st) {
   const dim3 grid(nq, 8);  // 128-thread blocks (register budget beside a resident screen CTA)
   const float* f32_rows = (const float*)c->d_rows.get();
   const double* f64_rows = (const double*)c->d_rows.get();
-  if (pearson_screened(c) && c->dtype == SDB_F32)
-    cand_refine_f32_kernel<float, true, true><<<grid, 128, 0, st>>>(f32_rows, c->dim, c->d_snorm, c->d_q32, c->d_cand,
-                                                                    c->d_cand_cnt, c->sc_cap, c->d_mom);
-  else if (pearson_screened(c))
-    cand_refine_f32_kernel<double, true, true><<<grid, 128, 0, st>>>(f64_rows, c->dim, c->d_snorm, c->d_q32, c->d_cand,
-                                                                     c->d_cand_cnt, c->sc_cap, c->d_mom);
-  else if (c->dtype == SDB_F32 && c->metric == SDB_COSINE)
-    cand_refine_f32_kernel<float, true><<<grid, 128, 0, st>>>(f32_rows, c->dim, c->d_snorm, c->d_q32, c->d_cand,
-                                                              c->d_cand_cnt, c->sc_cap, nullptr);
-  else if (c->dtype == SDB_F32)
-    cand_refine_f32_kernel<float, false><<<grid, 128, 0, st>>>(f32_rows, c->dim, c->d_snorm, c->d_q32, c->d_cand,
-                                                               c->d_cand_cnt, c->sc_cap, nullptr);
-  else if (c->metric == SDB_COSINE)
-    cand_refine_f32_kernel<double, true><<<grid, 128, 0, st>>>(f64_rows, c->dim, c->d_snorm, c->d_q32, c->d_cand,
-                                                               c->d_cand_cnt, c->sc_cap, nullptr);
-  else
-    cand_refine_f32_kernel<double, false><<<grid, 128, 0, st>>>(f64_rows, c->dim, c->d_snorm, c->d_q32, c->d_cand,
-                                                                c->d_cand_cnt, c->sc_cap, nullptr);
+  switch (family(c)) {
+    case Family::Centred:
+      if (c->dtype == SDB_F32)
+        cand_refine_f32_kernel<float, true, true><<<grid, 128, 0, st>>>(f32_rows, c->dim, c->d_snorm, c->d_q32,
+                                                                        c->d_cand, c->d_cand_cnt, c->sc_cap, c->d_mom);
+      else
+        cand_refine_f32_kernel<double, true, true><<<grid, 128, 0, st>>>(f64_rows, c->dim, c->d_snorm, c->d_q32,
+                                                                         c->d_cand, c->d_cand_cnt, c->sc_cap, c->d_mom);
+      break;
+    case Family::Dot:
+      if (c->dtype == SDB_F32 && c->metric == SDB_COSINE)
+        cand_refine_f32_kernel<float, true><<<grid, 128, 0, st>>>(f32_rows, c->dim, c->d_snorm, c->d_q32, c->d_cand,
+                                                                  c->d_cand_cnt, c->sc_cap, nullptr);
+      else if (c->dtype == SDB_F32)
+        cand_refine_f32_kernel<float, false><<<grid, 128, 0, st>>>(f32_rows, c->dim, c->d_snorm, c->d_q32, c->d_cand,
+                                                                   c->d_cand_cnt, c->sc_cap, nullptr);
+      else if (c->metric == SDB_COSINE)
+        cand_refine_f32_kernel<double, true><<<grid, 128, 0, st>>>(f64_rows, c->dim, c->d_snorm, c->d_q32, c->d_cand,
+                                                                   c->d_cand_cnt, c->sc_cap, nullptr);
+      else
+        cand_refine_f32_kernel<double, false><<<grid, 128, 0, st>>>(f64_rows, c->dim, c->d_snorm, c->d_q32, c->d_cand,
+                                                                    c->d_cand_cnt, c->sc_cap, nullptr);
+      break;
+    default: break;  // stage B follows the tensor-core screens (Dot, Centred) only
+  }
   count_launch(c->ctx);
   SDB_CUDA(cudaGetLastError());
   return SDB_OK;
@@ -1405,51 +1406,12 @@ static void launch_rerank_lp(Corpus* c, uint32_t nq, uint32_t n_sp, cudaStream_t
                              c->minkowski_p);
 }
 
-sdb_status cand_rerank(Corpus* c, uint32_t nq, cudaStream_t st, bool small_sets) {
+// COSINE / EUCLIDEAN: the packed kernel for the small sets stage B leaves, the vectorised one for f32 rows otherwise
+static void rerank_dot(Corpus* c, uint32_t nq, bool small_sets, uint32_t n_sp, cudaStream_t st) {
   const dim3 grid(nq, RR_GROUPS_Y);
-  if (c->metric == SDB_JACCARD && c->d_jfirst) {  // the direct regime only: no special rows
-    if (c->dtype == SDB_F32)
-      cand_rerank_jaccard_kernel<float><<<grid, 128, 0, st>>>((const float*)c->d_rows.get(), c->dim, c->d_jfirst,
-                                                              c->d_jux, c->d_qkey.get(), c->d_qjac, c->d_cand,
-                                                              c->d_cand_cnt, c->sc_cap, c->d_rr_key, c->d_rr_dist,
-                                                              c->d_rr_row, c->rr_stride);
-    else
-      cand_rerank_jaccard_kernel<double><<<grid, 128, 0, st>>>((const double*)c->d_rows.get(), c->dim, c->d_jfirst,
-                                                               c->d_jux, (const unsigned long long*)c->d_qkey.get(),
-                                                               c->d_qjac, c->d_cand, c->d_cand_cnt, c->sc_cap,
-                                                               c->d_rr_key, c->d_rr_dist, c->d_rr_row, c->rr_stride);
-    count_launch(c->ctx);
-    SDB_CUDA(cudaGetLastError());
-    return SDB_OK;
-  }
-  if (lp_metric(c) || c->metric == SDB_HAMMING) {
-    const uint32_t n_sp = c->filt.bits ? 0u : c->n_special;
-    if (c->dtype == SDB_F32) launch_rerank_lp<float>(c, nq, n_sp, st);
-    else launch_rerank_lp<double>(c, nq, n_sp, st);
-    count_launch(c->ctx);
-    SDB_CUDA(cudaGetLastError());
-    return SDB_OK;
-  }
-  if (pearson_screened(c)) {  // one kernel for small (after stage B) and large (direct regime, no stage B) sets
-    const uint32_t n_sp = c->filt.bits ? 0u : c->n_special;
-    if (c->dtype == SDB_F32)
-      cand_rerank_pearson_kernel<float><<<grid, 128, 0, st>>>((const float*)c->d_rows.get(), c->dim, c->d_mom, c->d_q64,
-                                                              c->d_qmom, c->d_qflags, c->d_cand, c->d_cand_cnt,
-                                                              c->sc_cap, c->d_special, n_sp, c->d_rr_key, c->d_rr_dist,
-                                                              c->d_rr_row, c->rr_stride);
-    else
-      cand_rerank_pearson_kernel<double><<<grid, 128, 0, st>>>((const double*)c->d_rows.get(), c->dim, c->d_mom,
-                                                               c->d_q64, c->d_qmom, c->d_qflags, c->d_cand,
-                                                               c->d_cand_cnt, c->sc_cap, c->d_special, n_sp,
-                                                               c->d_rr_key, c->d_rr_dist, c->d_rr_row, c->rr_stride);
-    count_launch(c->ctx);
-    SDB_CUDA(cudaGetLastError());
-    return SDB_OK;
-  }
   static const bool no_v4 = getenv("SDB_RERANK_SCALAR") != nullptr;
   static const bool no_packed = getenv("SDB_RERANK_STAGED") != nullptr;
-  const uint32_t n_sp = c->filt.bits ? 0u : c->n_special;  // filtered: the passing special rows are in the lists
-  if (small_sets && !no_packed && (c->metric == SDB_COSINE || c->metric == SDB_EUCLIDEAN)) {
+  if (small_sets && !no_packed) {
     const unsigned g = (nq + 7) / 8;
     const float* f32_rows = (const float*)c->d_rows.get();
     const double* f64_rows = (const double*)c->d_rows.get();
@@ -1490,6 +1452,49 @@ sdb_status cand_rerank(Corpus* c, uint32_t nq, cudaStream_t st, bool small_sets)
                                                             c->d_q64, c->d_qmag, c->d_qflags, c->d_cand, c->d_cand_cnt,
                                                             c->sc_cap, c->d_special, n_sp, c->d_rr_key,
                                                             c->d_rr_dist, c->d_rr_row, c->rr_stride);
+}
+
+sdb_status cand_rerank(Corpus* c, uint32_t nq, cudaStream_t st, bool small_sets) {
+  const dim3 grid(nq, RR_GROUPS_Y);
+  const uint32_t n_sp = c->filt.bits ? 0u : c->n_special;  // filtered: the passing special rows are in the lists
+  switch (family(c)) {
+    case Family::Count:  // the direct regime only (the count path's lists carry exact distances): no special rows
+      if (c->metric == SDB_HAMMING) {
+        if (c->dtype == SDB_F32) launch_rerank_lp<float>(c, nq, n_sp, st);
+        else launch_rerank_lp<double>(c, nq, n_sp, st);
+      } else if (c->dtype == SDB_F32) {
+        cand_rerank_jaccard_kernel<float><<<grid, 128, 0, st>>>((const float*)c->d_rows.get(), c->dim, c->d_jfirst,
+                                                                c->d_jux, c->d_qkey.get(), c->d_qjac, c->d_cand,
+                                                                c->d_cand_cnt, c->sc_cap, c->d_rr_key, c->d_rr_dist,
+                                                                c->d_rr_row, c->rr_stride);
+      } else {
+        cand_rerank_jaccard_kernel<double><<<grid, 128, 0, st>>>((const double*)c->d_rows.get(), c->dim, c->d_jfirst,
+                                                                 c->d_jux, (const unsigned long long*)c->d_qkey.get(),
+                                                                 c->d_qjac, c->d_cand, c->d_cand_cnt, c->sc_cap,
+                                                                 c->d_rr_key, c->d_rr_dist, c->d_rr_row, c->rr_stride);
+      }
+      break;
+    case Family::Lp:
+      if (c->dtype == SDB_F32) launch_rerank_lp<float>(c, nq, n_sp, st);
+      else launch_rerank_lp<double>(c, nq, n_sp, st);
+      break;
+    case Family::Centred:  // one kernel for small (after stage B) and large (direct regime, no stage B) sets
+      if (c->dtype == SDB_F32)
+        cand_rerank_pearson_kernel<float><<<grid, 128, 0, st>>>((const float*)c->d_rows.get(), c->dim, c->d_mom,
+                                                                c->d_q64, c->d_qmom, c->d_qflags, c->d_cand,
+                                                                c->d_cand_cnt, c->sc_cap, c->d_special, n_sp,
+                                                                c->d_rr_key, c->d_rr_dist, c->d_rr_row, c->rr_stride);
+      else
+        cand_rerank_pearson_kernel<double><<<grid, 128, 0, st>>>((const double*)c->d_rows.get(), c->dim, c->d_mom,
+                                                                 c->d_q64, c->d_qmom, c->d_qflags, c->d_cand,
+                                                                 c->d_cand_cnt, c->sc_cap, c->d_special, n_sp,
+                                                                 c->d_rr_key, c->d_rr_dist, c->d_rr_row, c->rr_stride);
+      break;
+    case Family::Dot:
+    case Family::Exact:  // (never reaches the re-rank: the exact kernel alone ranks it)
+      rerank_dot(c, nq, small_sets, n_sp, st);
+      break;
+  }
   count_launch(c->ctx);
   SDB_CUDA(cudaGetLastError());
   return SDB_OK;
@@ -1523,19 +1528,19 @@ __device__ __forceinline__ void bitonic_pairs(uint64_t* s_key, uint64_t* s_idx, 
   }
 }
 
-// LP: the MANHATTAN / CHEBYSHEV / MINKOWSKI proof (cand_final_lp_kernel); otherwise cosine / euclidean (cand_final_kernel)
-#define SDB_FINAL_PARAMS                                                                                               \
-  const uint64_t *__restrict__ rr_key, const double *__restrict__ rr_dist, const uint32_t *__restrict__ rr_row,       \
-      uint32_t rr_stride, const uint32_t *__restrict__ cnt, uint32_t cap, uint32_t n_special,                          \
-      const float *__restrict__ tau, const double *__restrict__ qmag, const float *__restrict__ bscale,                \
-      const float *__restrict__ beps, const float *__restrict__ tau2, const float *__restrict__ beps2,                 \
-      uint32_t *__restrict__ flags, const uint32_t *__restrict__ qflags, uint32_t *__restrict__ stat, int metric,      \
-      uint32_t k, uint64_t row_base, uint64_t *__restrict__ out_rows, double *__restrict__ out_dist,                   \
-      uint32_t *__restrict__ out_count, int debug
-// PEARSON: the cosine proof on the centred operands (cand_final_pearson_kernel), eps_ref = the gap between their cosine
-// and the reference's pearson (DESIGN.md section 2)
-template <bool LP, bool PEARSON = false>
-__device__ __forceinline__ void cand_final_body(SDB_FINAL_PARAMS, double eps_ref = 0.0) {
+// The proof of the family F's bound: Dot (cosine / euclidean, also the count path's lists, whose tau stays -inf), Lp, or
+// Centred (the cosine proof on the centred operands, eps_ref = the gap between their cosine and the reference's
+// pearson, DESIGN.md section 2; 0 for the other families)
+template <Family F>
+__global__ void __launch_bounds__(256)
+    cand_final_kernel(const uint64_t* __restrict__ rr_key, const double* __restrict__ rr_dist,
+                      const uint32_t* __restrict__ rr_row, uint32_t rr_stride, const uint32_t* __restrict__ cnt,
+                      uint32_t cap, uint32_t n_special, const float* __restrict__ tau, const double* __restrict__ qmag,
+                      const float* __restrict__ bscale, const float* __restrict__ beps, const float* __restrict__ tau2,
+                      const float* __restrict__ beps2, uint32_t* __restrict__ flags, const uint32_t* __restrict__ qflags,
+                      uint32_t* __restrict__ stat, int metric, uint32_t k, uint64_t row_base,
+                      uint64_t* __restrict__ out_rows, double* __restrict__ out_dist, uint32_t* __restrict__ out_count,
+                      int debug, double eps_ref) {
   __shared__ uint64_t s_key[FIN_WIN];  // distance key
   __shared__ uint64_t s_idx[FIN_WIN];  // (row << 32 | entry): secondary order by row (unique), entry = index into rr_*
   const uint32_t q = blockIdx.x;
@@ -1588,12 +1593,12 @@ __device__ __forceinline__ void cand_final_body(SDB_FINAL_PARAMS, double eps_ref
       const double qm = qmag[q];
       const uint64_t kth = s_key[k - 1];
       bool ok;
-      if (LP) {
+      if (F == Family::Lp) {
         // score = -s~ < tau for a non-candidate, so s~ > -tau and d >= s~ - beps > -tau - beps: the row cannot reach
         // the top k if that bound (rounded down) is strictly above the k-th exact key.  No stage B ran (tau2 = -inf).
         const double L = (-(double)t - (double)beps[q]) * (1.0 - 1e-12);
         ok = dist_key(L) > kth;
-      } else if (PEARSON) {
+      } else if (F == Family::Centred) {
         // the screen scored s = cos(dx, -dq) |dq| / bscale.  Non-candidate: score <= tau  =>  cos(dx, dq) >= -tau
         // bscale / |dq| - beps  =>  pearson >= -tau bscale / |dq| - beps - eps_ref, evaluated with directed rounding
         // so that the bound itself is rounded down
@@ -1612,7 +1617,7 @@ __device__ __forceinline__ void cand_final_body(SDB_FINAL_PARAMS, double eps_ref
       // stage B dropped candidates whose f32 score is below tau2: the same proof with the f32 bound
       const float t2 = tau2[q];
       if (ok && t2 > __int_as_float(0xff800000)) {
-        if (PEARSON) {  // stage B scores in the same units with bscale 1
+        if (F == Family::Centred) {  // stage B scores in the same units with bscale 1
           const double L2 = __dsub_rd(__dsub_rd(-__ddiv_ru((double)t2, qm), (double)beps2[q]), eps_ref);
           ok = dist_key(L2) > kth;
         } else if (metric == SDB_COSINE) {
@@ -1635,16 +1640,6 @@ __device__ __forceinline__ void cand_final_body(SDB_FINAL_PARAMS, double eps_ref
     atomicMax(stat + 2, n_e);
   }
 }
-#define SDB_FINAL_ARGS                                                                                                 \
-  rr_key, rr_dist, rr_row, rr_stride, cnt, cap, n_special, tau, qmag, bscale, beps, tau2, beps2, flags, qflags, stat, \
-      metric, k, row_base, out_rows, out_dist, out_count, debug
-__global__ void __launch_bounds__(256) cand_final_kernel(SDB_FINAL_PARAMS) { cand_final_body<false>(SDB_FINAL_ARGS); }
-__global__ void __launch_bounds__(256) cand_final_lp_kernel(SDB_FINAL_PARAMS) { cand_final_body<true>(SDB_FINAL_ARGS); }
-__global__ void __launch_bounds__(256) cand_final_pearson_kernel(SDB_FINAL_PARAMS, double eps_ref) {
-  cand_final_body<false, true>(SDB_FINAL_ARGS, eps_ref);
-}
-#undef SDB_FINAL_ARGS
-#undef SDB_FINAL_PARAMS
 
 sdb_status cand_final(Corpus* c, uint32_t nq, uint32_t k, uint64_t row_base, uint64_t* d_out_rows, double* d_out_dist,
                       uint32_t* d_out_count, cudaStream_t st) {
@@ -1654,22 +1649,25 @@ sdb_status cand_final(Corpus* c, uint32_t nq, uint32_t k, uint64_t row_base, uin
   }
   static const int debug = getenv("SDB_DEBUG") != nullptr;
   const uint32_t n_sp = c->filt.bits ? 0u : c->n_special;  // filtered: the passing special rows are in the lists
-  if (pearson_screened(c)) {
-    // |pearson - cos(dx, dq)| <= (2 D + 6) 2^-53 to first order (DESIGN.md section 2); +2 covers the rest
-    const double eps_ref = (2.0 * c->dim + 8.0) * 0x1p-53;
-    cand_final_pearson_kernel<<<nq, 256, 0, st>>>(c->d_rr_key, c->d_rr_dist, c->d_rr_row, c->rr_stride, c->d_cand_cnt,
-                                                  c->sc_cap, n_sp, c->d_tau, c->d_qmag, c->d_bscale, c->d_beps,
-                                                  c->d_tau2, c->d_beps2, c->d_flags, c->d_qflags, c->d_stat,
-                                                  (int)c->metric, k, row_base, d_out_rows, d_out_dist, d_out_count,
-                                                  debug, eps_ref);
-    count_launch(c->ctx);
-    SDB_CUDA(cudaGetLastError());
-    return SDB_OK;
+  auto fin = cand_final_kernel<Family::Dot>;
+  double eps_ref = 0.0;
+  switch (family(c)) {
+    case Family::Dot:
+    case Family::Count:  // (tau = -inf: nothing to prove)
+    case Family::Exact:  // (never reaches cand_final)
+      break;
+    case Family::Centred:
+      fin = cand_final_kernel<Family::Centred>;
+      // |pearson - cos(dx, dq)| <= (2 D + 6) 2^-53 to first order (DESIGN.md section 2); +2 covers the rest
+      eps_ref = (2.0 * c->dim + 8.0) * 0x1p-53;
+      break;
+    case Family::Lp:
+      fin = cand_final_kernel<Family::Lp>;
+      break;
   }
-  auto fin = lp_metric(c) ? cand_final_lp_kernel : cand_final_kernel;
-  fin<<<nq, 256, 0, st>>>(c->d_rr_key, c->d_rr_dist, c->d_rr_row, c->rr_stride, c->d_cand_cnt, c->sc_cap,
-                                        n_sp, c->d_tau, c->d_qmag, c->d_bscale, c->d_beps, c->d_tau2, c->d_beps2, c->d_flags, c->d_qflags, c->d_stat,
-                                        (int)c->metric, k, row_base, d_out_rows, d_out_dist, d_out_count, debug);
+  fin<<<nq, 256, 0, st>>>(c->d_rr_key, c->d_rr_dist, c->d_rr_row, c->rr_stride, c->d_cand_cnt, c->sc_cap, n_sp,
+                          c->d_tau, c->d_qmag, c->d_bscale, c->d_beps, c->d_tau2, c->d_beps2, c->d_flags, c->d_qflags,
+                          c->d_stat, (int)c->metric, k, row_base, d_out_rows, d_out_dist, d_out_count, debug, eps_ref);
   count_launch(c->ctx);
   SDB_CUDA(cudaGetLastError());
   return SDB_OK;

@@ -501,9 +501,9 @@ sdb_status corpus_finalize_device(Corpus* c) {
       count_launch(ctx);
     }
   }
-  // PEARSON corpora with their screen copies (sdb_corpus_create): moments, centred copies; without them the exact
-  // kernel serves every query and the corpus is finalized as before
-  const bool centred = c->metric == SDB_PEARSON && c->d_mom;
+  // Centred corpora (PEARSON with their screen copies, sdb_corpus_create): moments, centred copies; without them the
+  // exact kernel serves every query and the corpus is finalized as before
+  const bool centred = family(c) == Family::Centred;
   if (c->n) {
     const int grid = ctx->sm_count * 8;
     if (centred) {
@@ -515,7 +515,7 @@ sdb_status corpus_finalize_device(Corpus* c) {
                                                                      c->d_skip, c->d_mag, c->d_mom, c->d_snorm,
                                                                      c->d_special, d_tmp);
     } else if (c->metric == SDB_MANHATTAN || c->metric == SDB_CHEBYSHEV || c->metric == SDB_MINKOWSKI) {
-      // (MINKOWSKI of every order: the order may change after finalize, sdb_corpus_set_minkowski_order)
+      // (MINKOWSKI of every order, not only Family::Lp: the order may change after finalize)
       if (c->dtype == SDB_F32)
         finalize_lp_kernel<float, 8><<<grid, 256, 0, st>>>((const float*)c->d_rows.get(), c->dim, c->n, (int)c->metric,
                                                            c->d_skip, c->d_mag, c->d_snorm, c->d_special, d_tmp,
@@ -554,7 +554,7 @@ sdb_status corpus_finalize_device(Corpus* c) {
       SDB_CUDA(cudaGetLastError());
     }
   }
-  if (c->n && c->metric == SDB_JACCARD && c->d_jfirst) {
+  if (c->n && c->d_jfirst) {  // JACCARD corpora that hold their first-occurrence state
     if (c->dtype == SDB_F32)
       finalize_jaccard_kernel<float><<<ctx->sm_count * 8, 256, 0, st>>>((const float*)c->d_rows.get(), c->dim, c->n,
                                                                        c->d_jfirst, c->d_jux);
@@ -656,7 +656,7 @@ sdb_status corpus_finalize_device(Corpus* c) {
   uint32_t h[8] = {0, 0, 0, 0, 0, 0, 0, 0};
   SDB_CUDA(cudaMemcpyAsync(h, d_tmp, 32, cudaMemcpyDeviceToHost, st));
   SDB_CUDA(cudaStreamSynchronize(st));
-  // no special rows: zero, NaN and +-inf are ordinary values for equality
+  // no special rows: zero, NaN and +-inf are ordinary values for equality (a fact of the metric, whatever the family)
   if (c->metric == SDB_HAMMING || c->metric == SDB_JACCARD) h[0] = 0;
   c->special_overflow = h[0] > (uint32_t)SPECIAL_CAP;
   c->n_special = h[0] > (uint32_t)SPECIAL_CAP ? (uint32_t)SPECIAL_CAP : h[0];

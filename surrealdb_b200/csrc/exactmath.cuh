@@ -18,7 +18,7 @@ namespace sdb {
 __device__ __forceinline__ bool num_eq_f64(double a, double b) {
   return __double_as_longlong(a) == __double_as_longlong(b) || (a == 0.0 && b == 0.0);
 }
-// Keys that turn num_eq_f64 into one integer compare (the HAMMING count kernel, screen_lp.cu).
+// Keys that turn num_eq_f64 into one integer compare (the HAMMING count kernel, count.cu).
 //  - f64 rows and queries: the bits, -0.0 folded onto 0.0.
 //  - f32 rows: the key of (double)x, the exact kernel's widening, in 32 bits: x's own bits for a number (the widening
 //    is exact; -0.0 folded onto 0.0), sign | 0x7f800000 | fraction bits 51..29 of the widened value for a NaN, so that

@@ -432,35 +432,47 @@ inline int minkowski_screen_order(const Corpus* c) {
   const double p = c->minkowski_p;
   return (p >= 1.0 && p <= 8.0 && p == (double)(int)p) ? (int)p : 0;
 }
-// MANHATTAN / CHEBYSHEV and MINKOWSKI of a screened order: the f32 Lp screen, its bound, proof and re-rank
-inline bool lp_screened(const Corpus* c) {
-  return c->metric == SDB_MANHATTAN || c->metric == SDB_CHEBYSHEV || minkowski_screen_order(c) > 0;
+// The scoring family of a corpus: the per-query bound, candidate re-rank and proof that serve its brute-force searches,
+// on which every stage of a batch switches.  Evaluated per batch, never stored: sdb_corpus_set_minkowski_order may move
+// a finalized MINKOWSKI corpus between Lp and Exact.  Dot: COSINE, EUCLIDEAN.  Centred: PEARSON with its moments
+// (d_mom).  Lp: MANHATTAN, CHEBYSHEV, MINKOWSKI of a screened order.  Count: HAMMING, JACCARD with its first-occurrence
+// state (d_jfirst); count_ranked batches take the count path (exact counts of every row per row range, count.cu,
+// then cand_final with tau = -inf), the others the exact kernel.  Exact: the exact kernel alone.
+enum class Family { Dot, Centred, Lp, Count, Exact };
+inline Family family(const Corpus* c) {
+  switch (c->metric) {
+    case SDB_COSINE: case SDB_EUCLIDEAN: return Family::Dot;
+    case SDB_PEARSON: return c->d_mom ? Family::Centred : Family::Exact;
+    case SDB_MANHATTAN: case SDB_CHEBYSHEV: return Family::Lp;
+    case SDB_MINKOWSKI: return minkowski_screen_order(c) > 0 ? Family::Lp : Family::Exact;
+    case SDB_HAMMING: return Family::Count;
+    default: return c->d_jfirst ? Family::Count : Family::Exact;  // SDB_JACCARD
+  }
+}
+constexpr uint32_t COUNT_CAP_MAX = 16384;  // candidate entries per query of the count path: n_ranges k at most
+inline bool count_ranked(const Corpus* c, uint32_t k) {
+  return family(c) == Family::Count && k >= 1 && k <= 256 && c->screen != SDB_SCREEN_NONE_EXACT;
 }
 
-// HAMMING, and JACCARD corpora that hold their first-occurrence state: the count path's per-batch query state
-// (count_prep_queries) and re-rank.  With 1 <= k <= 256 and any screen but NONE_EXACT they are ranked by exact counts
-// of every row, per row range (count_pass), then cand_final with tau = -inf.  NONE_EXACT and k > 256 keep the exact
-// kernel.
-constexpr uint32_t COUNT_CAP_MAX = 16384;  // candidate entries per query of the count path: n_ranges k at most
-inline bool count_metric(const Corpus* c) {
-  return c->metric == SDB_HAMMING || (c->metric == SDB_JACCARD && c->d_jfirst);
-}
-inline bool count_ranked(const Corpus* c, uint32_t k) {
-  return count_metric(c) && k >= 1 && k <= 256 && c->screen != SDB_SCREEN_NONE_EXACT;
-}
+// tiling shared by the f32 Lp screen (screen_lp.cu) and the count path (count.cu)
+constexpr int LP_THREADS = 256;
+constexpr int LP_RB = 128;          // rows per CTA step (a pass tile is two steps)
+constexpr int LP_KC = 32;           // columns per shared-memory chunk
+constexpr int LP_STRIDE = LP_KC + 4;
+constexpr int LP_TQ = 4;            // queries per thread
 
 // ---- launch wrappers (defined in the .cu files) ---------------------------------------------------
 // corpus.cu
 sdb_status corpus_finalize_device(Corpus* c);
 sdb_status corpus_remove_device(Corpus* c, const uint64_t* h_ids, uint64_t n);
 sdb_status corpus_reapply_tombstones(Corpus* c, cudaStream_t st);
-// screen_simt.cu (the SIMT_F32 screen; MANHATTAN / CHEBYSHEV / screened MINKOWSKI corpora go to screen_lp_pass)
+// screen_simt.cu: the SIMT_F32 screen of Dot corpora (f32 rows)
 sdb_status screen_simt_pass(Corpus* c, uint32_t nq, const PassDesc& p, cudaStream_t st);
-// screen_lp.cu: f32 L1 / L-infinity / Lp screen (score = -s~), f32 and f64 rows
+// screen_lp.cu: the SIMT_F32 screen of Lp corpora, f32 L1 / L-infinity / Lp (score = -s~), f32 and f64 rows
 sdb_status screen_lp_pass(Corpus* c, uint32_t nq, const PassDesc& p, cudaStream_t st);
-// ... and the HAMMING / JACCARD count path: rows split into count_ranges() ranges, each query's candidate entries
+// count.cu: the count path of Count corpora: rows split into count_ranges() ranges, each query's candidate entries
 // (cnt, rr_*) = the union of its ranges' k best (distance, row) pairs with their exact distances; needs prep_queries
-// (which runs count_prep_queries for count_metric corpora) and cand_begin
+// (which runs count_prep_queries for Count corpora) and cand_begin
 uint32_t count_ranges(const Corpus* c, uint32_t nq, uint32_t k);
 sdb_status count_prep_queries(Corpus* c, uint32_t nq, cudaStream_t st);
 sdb_status count_pass(Corpus* c, uint32_t nq, uint32_t k, cudaStream_t st);

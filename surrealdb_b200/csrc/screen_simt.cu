@@ -251,7 +251,6 @@ static sdb_status launch_ring(Corpus* c, uint32_t nq, const PassDesc& p, cudaStr
 }
 
 sdb_status screen_simt_pass(Corpus* c, uint32_t nq, const PassDesc& p, cudaStream_t st) {
-  if (lp_screened(c)) return screen_lp_pass(c, nq, p, st);
   if (p.count == 0) return SDB_OK;
   Ctx* ctx = c->ctx;
   const size_t q_bytes = sizeof(float) * SIMT_QB * c->dim;

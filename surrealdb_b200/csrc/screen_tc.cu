@@ -767,7 +767,7 @@ sdb_status screen_tc_pass(Corpus* c, uint32_t nq, uint32_t k, const PassDesc& p,
   if (p.count == 0) return SDB_OK;
   Ctx* ctx = c->ctx;
   // PEARSON corpora hold centred copies (corpus.cu) and centred, negated queries (prep_queries): their cosine screen
-  const bool cosine = c->metric == SDB_COSINE || (c->metric == SDB_PEARSON && c->d_mom);
+  const bool cosine = c->metric == SDB_COSINE || family(c) == Family::Centred;
   if (int8 ? (!c->d_i8 || !cosine) : !c->d_bf16) {
     set_error("tensor-core screen: the %s screen copy is not available for this corpus",
               int8 ? "int8 (cosine and pearson only)" : "bf16");

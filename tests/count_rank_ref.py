@@ -1,4 +1,4 @@
-"""Numpy restatement of the count path (screen_lp.cu: count_hamming_kernel, count_jaccard_kernel; exactmath.cuh: the keys).
+"""Numpy restatement of the count path (count.cu: count_hamming_kernel, count_jaccard_kernel; exactmath.cuh: the keys).
 
 - Number equality of two elements widened to f64: same bits, or both zero (num_eq_f64).
 - The keys that make it one integer compare: eq_key_f64, eq_key_f32 (f32 rows) and eq_qkey_f32 (an f64 query element

@@ -1,4 +1,4 @@
-"""Brute-force KNN of HAMMING and JACCARD columns through the count path (count_pass in screen_lp.cu, then cand_final):
+"""Brute-force KNN of HAMMING and JACCARD columns through the count path (count_pass in count.cu, then cand_final):
 exact counts of every row, ranked per row range.  Every answer is compared bit for bit (rows, their order, f64
 distances, counts) with the CPU oracle and with the same column under NONE_EXACT, the exact kernel."""
 import zlib
