@@ -85,16 +85,12 @@ __global__ void prep_queries_pearson_kernel(const double* __restrict__ q64, uint
   if (threadIdx.x == 0) {
     s_flags = 0;
     s_err2 = 0.f;
-    double s = 0.0, s2 = 0.0;
+    double s2 = 0.0;
     if (q < nq) {
-      for (uint32_t c = 0; c < dim; c++) s = __dadd_rn(s, q64[(size_t)q * dim + c]);
-      const double m2 = __ddiv_rn(s, (double)dim);
-      for (uint32_t c = 0; c < dim; c++) {  // ExactAcc::pearson_step's acc2, as exact_keys_kernel's deviation
-        const double d = __dsub_rn(q64[(size_t)q * dim + c], m2);
-        s2 = __dadd_rn(s2, __dmul_rn(d, d));
-      }
-      qmom[q] = make_double2(m2, s2);
-      s_m2 = m2;
+      const double2 mom = pearson_moments(q64 + (size_t)q * dim, dim);
+      qmom[q] = mom;
+      s_m2 = mom.x;
+      s2 = mom.y;
     }
     s_nrm = __dsqrt_rn(s2);
   }
@@ -1058,79 +1054,89 @@ sdb_status cand_refine(Corpus* c, uint32_t nq, cudaStream_t st) {
 }
 
 // ------------------------------------------------------------------------------------------------
-// exact re-rank.  Work unit = (query, group of 128 entries): blocks (x = query, y = 0..3) stride over the groups of
-// their query; each warp takes 32 entries (candidates first, then the special rows) and walks their rows 64 columns at
-// a time: 64 coalesced 128-byte row segments are requested back to back (all in flight before the first is consumed --
-// the kernel is bound by the latency of these gathers, not by the f64 arithmetic), transposed through shared memory,
-// and every lane then accumulates ITS row strictly left to right in the reference's arithmetic.  Candidate counts
-// vary per query by orders of magnitude (a handful ... a whole cluster).
+// exact re-rank: per query, every list entry (candidates first, then the special rows) gets the reference's distance
+// (RefAcc, exactmath.cuh) and is stored at its entry index for cand_final.  Candidate counts vary per query by orders
+// of magnitude (a handful ... a whole cluster).  COSINE / EUCLIDEAN have three load schemes (packed, v4, staged below);
+// the other metrics give each entry to one thread (cand_rerank_entry_kernel).
 constexpr uint32_t QCHUNK = 1024;  // query columns staged in shared memory per step
 
 constexpr uint32_t RR_GROUPS_Y = 4;  // blocks per query; block y takes the groups y, y + 4, ... of its query
 
-template <typename T, int WARPS, int COLS, int QC = QCHUNK>
-__global__ void __launch_bounds__(WARPS * 32) cand_rerank_kernel(
+struct RerankOut {  // nq x stride results: the distance's key, the distance, the row
+  uint64_t* key;
+  double* dist;
+  uint32_t* row;
+  uint32_t stride;
+};
+__device__ __forceinline__ void rr_store(const RerankOut& out, uint32_t q, uint32_t e, uint32_t row, double d) {
+  const size_t o = (size_t)q * out.stride + e;
+  out.key[o] = dist_key(d);
+  out.dist[o] = d;
+  out.row[o] = row;
+}
+static RerankOut rr_out(const Corpus* c) { return RerankOut{c->d_rr_key, c->d_rr_dist, c->d_rr_row, c->rr_stride}; }
+
+// the COSINE / EUCLIDEAN finish of one entry
+__device__ __forceinline__ double dot_finish(bool cosine, const RefSum& s, const double* mag, uint32_t row, double qm,
+                                             bool q_nan) {
+  return cosine ? RefAcc<SDB_COSINE>{}.finish(s, mag[row], qm, q_nan) : RefAcc<SDB_EUCLIDEAN>{}.finish(s, q_nan);
+}
+
+// Staged: blocks (x = query, y = 0..3) stride over groups of 128 entries; each warp takes 32 entries and walks their
+// rows 32 columns at a time: 32 coalesced 128-byte row segments are requested back to back (all in flight before the
+// first is consumed -- the kernel is bound by the latency of these gathers, not by the f64 arithmetic), transposed
+// through shared memory, and every lane then accumulates ITS row strictly left to right.
+constexpr uint32_t RR_WARPS = 4, RR_COLS = 32;
+template <typename T>
+__global__ void __launch_bounds__(RR_WARPS * 32) cand_rerank_kernel(
     const T* __restrict__ rows, uint32_t dim, int metric, const double* __restrict__ mag,
     const double* __restrict__ q64, const double* __restrict__ qmag, const uint32_t* __restrict__ qflags,
     const Cand* __restrict__ cand, const uint32_t* __restrict__ cnt, uint32_t cap, const uint32_t* __restrict__ special,
-    uint32_t n_special, uint64_t* __restrict__ rr_key, double* __restrict__ rr_dist, uint32_t* __restrict__ rr_row,
-    uint32_t rr_stride) {
-  constexpr int NL = COLS / 32;  // 128-byte segments per row and step
-  __shared__ T tile[WARPS][32][COLS + 1];
-  __shared__ double s_q[QC];
+    uint32_t n_special, RerankOut out) {
+  __shared__ T tile[RR_WARPS][32][RR_COLS + 1];
+  __shared__ double s_q[QCHUNK];
   const uint32_t q = blockIdx.x, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const uint32_t n_c = cnt[q] < cap ? cnt[q] : cap;
   const uint32_t n_e = n_c + n_special;
   const bool q_nan = (qflags[q] & 2u) != 0;
   const double qm = qmag[q];
-  for (uint32_t e_first = blockIdx.y * (WARPS * 32); e_first < n_e; e_first += gridDim.y * (WARPS * 32)) {  // uniform per block
+  for (uint32_t e_first = blockIdx.y * (RR_WARPS * 32); e_first < n_e; e_first += gridDim.y * (RR_WARPS * 32)) {  // uniform per block
     const uint32_t e = e_first + warp * 32 + lane;
     uint32_t my_row = NO_ROW;
     if (e < n_c) my_row = cand[(size_t)q * cap + e].row;
     else if (e < n_e) my_row = special[e - n_c];
     const bool warp_active = e_first + warp * 32 < n_e;
-    ExactAcc acc;
-    for (uint32_t cb = 0; cb < dim; cb += QC) {
-      const uint32_t cw = dim - cb < (uint32_t)QC ? dim - cb : (uint32_t)QC;
+    RefSum acc;
+    for (uint32_t cb = 0; cb < dim; cb += QCHUNK) {
+      const uint32_t cw = dim - cb < QCHUNK ? dim - cb : QCHUNK;
       __syncthreads();
       for (uint32_t i = threadIdx.x; i < cw; i += blockDim.x) s_q[i] = q64[(size_t)q * dim + cb + i];
       __syncthreads();
       if (!warp_active) continue;
       const T* base = rows + cb;
-      for (uint32_t c0 = 0; c0 < cw; c0 += COLS) {
-        T vals[32 * NL];
+      for (uint32_t c0 = 0; c0 < cw; c0 += RR_COLS) {
+        T vals[32];
 #pragma unroll
-        for (int r = 0; r < 32; r++) {  // 32 x NL independent 128-byte gathers in flight
+        for (int r = 0; r < 32; r++) {  // 32 independent 128-byte gathers in flight
           const uint32_t row = __shfl_sync(0xffffffffu, my_row, r);
-#pragma unroll
-          for (int h = 0; h < NL; h++) {
-            const uint32_t c = c0 + h * 32 + lane;
-            vals[r * NL + h] = (row != NO_ROW && c < cw) ? __ldg(base + (size_t)row * dim + c) : T(0);
-          }
+          const uint32_t c = c0 + lane;
+          vals[r] = (row != NO_ROW && c < cw) ? __ldg(base + (size_t)row * dim + c) : T(0);
         }
 #pragma unroll
-        for (int r = 0; r < 32; r++)
-#pragma unroll
-          for (int h = 0; h < NL; h++) tile[warp][r][h * 32 + lane] = vals[r * NL + h];
+        for (int r = 0; r < 32; r++) tile[warp][r][lane] = vals[r];
         __syncwarp();
         if (my_row != NO_ROW) {
-          const uint32_t lim = cw - c0 < (uint32_t)COLS ? cw - c0 : (uint32_t)COLS;
+          const uint32_t lim = cw - c0 < RR_COLS ? cw - c0 : RR_COLS;
           if (metric == SDB_COSINE) {
-            for (uint32_t j = 0; j < lim; j++) acc.cosine_step((double)tile[warp][lane][j], s_q[c0 + j]);
+            for (uint32_t j = 0; j < lim; j++) RefAcc<SDB_COSINE>{}.step(acc, (double)tile[warp][lane][j], s_q[c0 + j]);
           } else {
-            for (uint32_t j = 0; j < lim; j++) acc.euclid_step((double)tile[warp][lane][j], s_q[c0 + j]);
+            for (uint32_t j = 0; j < lim; j++) RefAcc<SDB_EUCLIDEAN>{}.step(acc, (double)tile[warp][lane][j], s_q[c0 + j]);
           }
         }
         __syncwarp();
       }
     }
-    if (my_row != NO_ROW) {
-      const double d = metric == SDB_COSINE ? cosine_finish(acc, mag[my_row], qm, q_nan) : euclid_finish(acc, q_nan);
-      const size_t o = (size_t)q * rr_stride + e;
-      rr_key[o] = dist_key(d);
-      rr_dist[o] = d;
-      rr_row[o] = my_row;
-    }
+    if (my_row != NO_ROW) rr_store(out, q, e, my_row, dot_finish(metric == SDB_COSINE, acc, mag, my_row, qm, q_nan));
   }
 }
 
@@ -1139,29 +1145,27 @@ __global__ void __launch_bounds__(WARPS * 32) cand_rerank_kernel(
 // 128-byte pieces of 32 different rows (random 128-byte gathers reach ~2 TB/s on HBM3e, page-friendly ones several
 // times that).  The 32 x 128 tile is then walked per lane with conflict-free LDS.128 (row stride 132 floats).
 constexpr uint32_t RRV_COLS = 128, RRV_STRIDE = RRV_COLS + 4;
-template <int WARPS>
-__global__ void __launch_bounds__(WARPS * 32) cand_rerank_v4_kernel(
+__global__ void __launch_bounds__(RR_WARPS * 32) cand_rerank_v4_kernel(
     const float* __restrict__ rows, uint32_t dim, int metric, const double* __restrict__ mag,
     const double* __restrict__ q64, const double* __restrict__ qmag, const uint32_t* __restrict__ qflags,
     const Cand* __restrict__ cand, const uint32_t* __restrict__ cnt, uint32_t cap, const uint32_t* __restrict__ special,
-    uint32_t n_special, uint64_t* __restrict__ rr_key, double* __restrict__ rr_dist, uint32_t* __restrict__ rr_row,
-    uint32_t rr_stride) {
+    uint32_t n_special, RerankOut out) {
   extern __shared__ __align__(16) uint8_t rr_smem[];
   double* s_q = reinterpret_cast<double*>(rr_smem);                                   // [QCHUNK]
-  float* tiles = reinterpret_cast<float*>(rr_smem + sizeof(double) * QCHUNK);          // [WARPS][32][RRV_STRIDE]
+  float* tiles = reinterpret_cast<float*>(rr_smem + sizeof(double) * QCHUNK);          // [RR_WARPS][32][RRV_STRIDE]
   const uint32_t q = blockIdx.x, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   float* tile = tiles + (size_t)warp * 32 * RRV_STRIDE;
   const uint32_t n_c = cnt[q] < cap ? cnt[q] : cap;
   const uint32_t n_e = n_c + n_special;
   const bool q_nan = (qflags[q] & 2u) != 0;
   const double qm = qmag[q];
-  for (uint32_t e_first = blockIdx.y * (WARPS * 32); e_first < n_e; e_first += gridDim.y * (WARPS * 32)) {  // uniform per block
+  for (uint32_t e_first = blockIdx.y * (RR_WARPS * 32); e_first < n_e; e_first += gridDim.y * (RR_WARPS * 32)) {  // uniform per block
     const uint32_t e = e_first + warp * 32 + lane;
     uint32_t my_row = NO_ROW;
     if (e < n_c) my_row = cand[(size_t)q * cap + e].row;
     else if (e < n_e) my_row = special[e - n_c];
     const bool warp_active = e_first + warp * 32 < n_e;
-    ExactAcc acc;
+    RefSum acc;
     for (uint32_t cb = 0; cb < dim; cb += QCHUNK) {
       const uint32_t cw = dim - cb < QCHUNK ? dim - cb : QCHUNK;  // multiple of 4
       __syncthreads();
@@ -1188,36 +1192,32 @@ __global__ void __launch_bounds__(WARPS * 32) cand_rerank_v4_kernel(
           const uint32_t lim = cw - c0 < RRV_COLS ? cw - c0 : RRV_COLS;  // multiple of 4
           const float* mine = tile + (size_t)lane * RRV_STRIDE;
           if (metric == SDB_COSINE) {
+            const RefAcc<SDB_COSINE> ref;
             for (uint32_t j = 0; j < lim; j += 4) {
               const float4 v = *reinterpret_cast<const float4*>(mine + j);
-              acc.cosine_step((double)v.x, s_q[c0 + j]);
-              acc.cosine_step((double)v.y, s_q[c0 + j + 1]);
-              acc.cosine_step((double)v.z, s_q[c0 + j + 2]);
-              acc.cosine_step((double)v.w, s_q[c0 + j + 3]);
+              ref.step(acc, (double)v.x, s_q[c0 + j]);
+              ref.step(acc, (double)v.y, s_q[c0 + j + 1]);
+              ref.step(acc, (double)v.z, s_q[c0 + j + 2]);
+              ref.step(acc, (double)v.w, s_q[c0 + j + 3]);
             }
           } else {
+            const RefAcc<SDB_EUCLIDEAN> ref;
             for (uint32_t j = 0; j < lim; j += 4) {
               const float4 v = *reinterpret_cast<const float4*>(mine + j);
-              acc.euclid_step((double)v.x, s_q[c0 + j]);
-              acc.euclid_step((double)v.y, s_q[c0 + j + 1]);
-              acc.euclid_step((double)v.z, s_q[c0 + j + 2]);
-              acc.euclid_step((double)v.w, s_q[c0 + j + 3]);
+              ref.step(acc, (double)v.x, s_q[c0 + j]);
+              ref.step(acc, (double)v.y, s_q[c0 + j + 1]);
+              ref.step(acc, (double)v.z, s_q[c0 + j + 2]);
+              ref.step(acc, (double)v.w, s_q[c0 + j + 3]);
             }
           }
         }
         __syncwarp();
       }
     }
-    if (my_row != NO_ROW) {
-      const double d = metric == SDB_COSINE ? cosine_finish(acc, mag[my_row], qm, q_nan) : euclid_finish(acc, q_nan);
-      const size_t o = (size_t)q * rr_stride + e;
-      rr_key[o] = dist_key(d);
-      rr_dist[o] = d;
-      rr_row[o] = my_row;
-    }
+    if (my_row != NO_ROW) rr_store(out, q, e, my_row, dot_finish(metric == SDB_COSINE, acc, mag, my_row, qm, q_nan));
   }
 }
-constexpr size_t RRV_SMEM = sizeof(double) * QCHUNK + sizeof(float) * 4 * 32 * RRV_STRIDE;  // 4 warps: 75.8 KB
+constexpr size_t RRV_SMEM = sizeof(double) * QCHUNK + sizeof(float) * RR_WARPS * 32 * RRV_STRIDE;  // 75.8 KB
 
 
 // After the f32 stage a query keeps k candidates plus a few near-ties (about 10 at k = 10), and the exact re-rank is one
@@ -1227,13 +1227,13 @@ constexpr size_t RRV_SMEM = sizeof(double) * QCHUNK + sizeof(float) * 4 * 32 * R
 // (the staged variant's 6 KB per warp let only two warps per SM in, and the re-rank took 0.58 ms instead of 0.1 ms
 // whenever it overlapped a screen -- SDB_TRACE timeline, round 2).  Every lane streams its own row (16-byte loads; the
 // second half of each 32-byte sector comes from L1) and reads the query from global memory (one address per half-warp).
-// f64 rows stream as double2 (16-byte) loads when the row length is even.
-template <typename T, bool COSINE>
+// f64 rows stream as double2 (16-byte) loads when the row length is even.  M: SDB_COSINE or SDB_EUCLIDEAN.
+template <typename T, int M>
 __global__ void __launch_bounds__(128) cand_rerank_packed_kernel(
     const T* __restrict__ rows, uint32_t dim, const double* __restrict__ mag, const double* __restrict__ q64,
     const double* __restrict__ qmag, const uint32_t* __restrict__ qflags, const Cand* __restrict__ cand,
     const uint32_t* __restrict__ cnt, uint32_t cap, const uint32_t* __restrict__ special, uint32_t n_special, uint32_t nq,
-    uint64_t* __restrict__ rr_key, double* __restrict__ rr_dist, uint32_t* __restrict__ rr_row, uint32_t rr_stride) {
+    RerankOut out) {
   const uint32_t warp = threadIdx.x >> 5, lane = threadIdx.x & 31u;
   const uint32_t q = (blockIdx.x * 4 + warp) * 2 + (lane >> 4), l16 = lane & 15u;
   if (q >= nq) return;
@@ -1243,29 +1243,22 @@ __global__ void __launch_bounds__(128) cand_rerank_packed_kernel(
   const double qm = qmag[q];
   const double* qv = q64 + (size_t)q * dim;
   const bool vec4 = (dim & 3u) == 0;
+  const RefAcc<M> ref;
   for (uint32_t e = l16; e < n_e; e += 16) {
     const uint32_t my_row = e < n_c ? cand[(size_t)q * cap + e].row : special[e - n_c];
     const T* x = rows + (size_t)my_row * dim;
-    ExactAcc acc;
+    RefSum acc;
     if constexpr (std::is_same<T, double>::value) {
       if ((dim & 1u) == 0) {
 #pragma unroll 2
         for (uint32_t j = 0; j < dim; j += 2) {
           const double2 v = __ldg(reinterpret_cast<const double2*>(x + j));
           const double2 qa = __ldg(reinterpret_cast<const double2*>(qv + j));
-          if (COSINE) {
-            acc.cosine_step(v.x, qa.x);
-            acc.cosine_step(v.y, qa.y);
-          } else {
-            acc.euclid_step(v.x, qa.x);
-            acc.euclid_step(v.y, qa.y);
-          }
+          ref.step(acc, v.x, qa.x);
+          ref.step(acc, v.y, qa.y);
         }
       } else {
-        for (uint32_t j = 0; j < dim; j++) {
-          if (COSINE) acc.cosine_step(__ldg(x + j), __ldg(qv + j));
-          else acc.euclid_step(__ldg(x + j), __ldg(qv + j));
-        }
+        for (uint32_t j = 0; j < dim; j++) ref.step(acc, __ldg(x + j), __ldg(qv + j));
       }
     } else if (vec4) {
 #pragma unroll 2
@@ -1273,222 +1266,133 @@ __global__ void __launch_bounds__(128) cand_rerank_packed_kernel(
         const float4 v = __ldg(reinterpret_cast<const float4*>(x + j));
         const double2 qa = __ldg(reinterpret_cast<const double2*>(qv + j));
         const double2 qb = __ldg(reinterpret_cast<const double2*>(qv + j + 2));
-        if (COSINE) {
-          acc.cosine_step((double)v.x, qa.x);
-          acc.cosine_step((double)v.y, qa.y);
-          acc.cosine_step((double)v.z, qb.x);
-          acc.cosine_step((double)v.w, qb.y);
-        } else {
-          acc.euclid_step((double)v.x, qa.x);
-          acc.euclid_step((double)v.y, qa.y);
-          acc.euclid_step((double)v.z, qb.x);
-          acc.euclid_step((double)v.w, qb.y);
-        }
+        ref.step(acc, (double)v.x, qa.x);
+        ref.step(acc, (double)v.y, qa.y);
+        ref.step(acc, (double)v.z, qb.x);
+        ref.step(acc, (double)v.w, qb.y);
       }
     } else {
-      for (uint32_t j = 0; j < dim; j++) {
-        if (COSINE) acc.cosine_step((double)__ldg(x + j), __ldg(qv + j));
-        else acc.euclid_step((double)__ldg(x + j), __ldg(qv + j));
-      }
+      for (uint32_t j = 0; j < dim; j++) ref.step(acc, (double)__ldg(x + j), __ldg(qv + j));
     }
-    const double d = COSINE ? cosine_finish(acc, mag[my_row], qm, q_nan) : euclid_finish(acc, q_nan);
-    const size_t o = (size_t)q * rr_stride + e;
-    rr_key[o] = dist_key(d);
-    rr_dist[o] = d;
-    rr_row[o] = my_row;
+    rr_store(out, q, e, my_row, dot_finish(M == SDB_COSINE, acc, mag, my_row, qm, q_nan));
   }
 }
 
-// MANHATTAN / CHEBYSHEV / MINKOWSKI / HAMMING re-rank: the exact kernel's arithmetic (ExactAcc::manhattan_step /
-// chebyshev_step / minkowski_step / hamming_step, canon_nan; HAMMING only in the direct regime of filtered batches; MINKOWSKI's order mink_p a run-time argument there and here) per candidate, one thread per list entry and its row streamed left to right (the query's elements are the same
-// address across the warp).  Blocks (x = query, y = 0 .. RR_GROUPS_Y - 1) stride over the query's entries.
-template <typename T, int METRIC>
-__global__ void __launch_bounds__(128) cand_rerank_lp_kernel(
+// The per-metric inputs of cand_rerank_entry_kernel
+struct EntryArgs {
+  double mink_p;        // MINKOWSKI: the order
+  const double2* mom;   // PEARSON: {m1, S1} per row (finalize_pearson_kernel)
+  const double2* qmom;  // ... and {m2, S2} per query (prep_queries_pearson_kernel)
+  const uint32_t* jfirst;  // JACCARD: the rows' first-occurrence bitmasks and distinct counts (finalize) ...
+  const uint32_t* jux;
+  const void* qkey;        // ... and the batch's sorted query keys, EqKey<T>, and {u_q, n_look} (count_prep_queries)
+  const uint32_t* qjac;
+};
+
+// Every metric but COSINE / EUCLIDEAN: one thread per list entry, its row streamed left to right (the query's elements
+// are the same address across the warp); blocks (x = query, y = 0 .. RR_GROUPS_Y - 1) stride over the query's entries.
+//  - MANHATTAN / CHEBYSHEV / MINKOWSKI: screened and in the direct regime of filtered batches; HAMMING / JACCARD: the
+//    direct regime only (the count path's lists carry exact distances).
+//  - PEARSON runs exact_keys_kernel's two passes in one, from the stored means: the row's m1 and S1 and the query's m2
+//    and S2 are that kernel's mean and deviation sums bit for bit.
+//  - JACCARD: jaccard_counts from the corpus's first-occurrence state and the batch's query keys.
+template <typename T, int M>
+__global__ void __launch_bounds__(128) cand_rerank_entry_kernel(
     const T* __restrict__ rows, uint32_t dim, const double* __restrict__ q64, const uint32_t* __restrict__ qflags,
     const Cand* __restrict__ cand, const uint32_t* __restrict__ cnt, uint32_t cap, const uint32_t* __restrict__ special,
-    uint32_t n_special, uint64_t* __restrict__ rr_key, double* __restrict__ rr_dist, uint32_t* __restrict__ rr_row,
-    uint32_t rr_stride, double mink_p) {
+    uint32_t n_special, RerankOut out, EntryArgs a) {
   const uint32_t q = blockIdx.x;
   const uint32_t n_c = cnt[q] < cap ? cnt[q] : cap;
   const uint32_t n_e = n_c + n_special;
   const bool q_nan = (qflags[q] & 2u) != 0;
   const double* qv = q64 + (size_t)q * dim;
+  double2 qm = make_double2(0.0, 0.0);
+  double sd2 = 0.0;
+  if constexpr (M == SDB_PEARSON) {
+    qm = __ldg(a.qmom + q);
+    sd2 = RefAcc<SDB_PEARSON>::sd(qm.y, dim);
+  }
   for (uint32_t e = blockIdx.y * blockDim.x + threadIdx.x; e < n_e; e += gridDim.y * blockDim.x) {
-    const uint32_t my_row = e < n_c ? cand[(size_t)q * cap + e].row : special[e - n_c];
-    const T* x = rows + (size_t)my_row * dim;
-    ExactAcc acc;
-    if (METRIC == SDB_CHEBYSHEV) acc.acc = -1.7976931348623157e308;  // f64::MIN
-    for (uint32_t j = 0; j < dim; j++) {
-      if (METRIC == SDB_MANHATTAN) acc.manhattan_step((double)__ldg(x + j), __ldg(qv + j));
-      else if (METRIC == SDB_HAMMING) acc.hamming_step((double)__ldg(x + j), __ldg(qv + j));
-      else if (METRIC == SDB_MINKOWSKI) acc.minkowski_step((double)__ldg(x + j), __ldg(qv + j), mink_p);
-      else acc.chebyshev_step((double)__ldg(x + j), __ldg(qv + j));
-    }
+    const uint32_t row = e < n_c ? cand[(size_t)q * cap + e].row : special[e - n_c];
+    const T* x = rows + (size_t)row * dim;
     double d;
-    if (METRIC == SDB_MANHATTAN) d = canon_nan(acc.acc, acc.nan_in || q_nan);
-    else if (METRIC == SDB_MINKOWSKI) d = canon_nan(pow(acc.acc, __ddiv_rn(1.0, mink_p)), acc.nan_in || q_nan);
-    else d = acc.acc;
-    const size_t o = (size_t)q * rr_stride + e;
-    rr_key[o] = dist_key(d);
-    rr_dist[o] = d;
-    rr_row[o] = my_row;
-  }
-}
-// PEARSON re-rank: exact_keys_kernel's two passes in one, from the stored means -- pass A's m1 = mom[row].x (finalize)
-// and the query's m2 (prep_queries_pearson_kernel) -- then one chain covar = sum (x_i - m1)(q_i - m2) in
-// ExactAcc::pearson_step, and pass B's finish with S1 = mom[row].y and S2, which are that kernel's deviation sums
-// bit for bit.  nan_in: a NaN element of the row (pass A's rule) or of the query; a row holding +inf and -inf has a
-// generated NaN mean and sorts first.  Special rows (constant ones included) go through here too.
-template <typename T>
-__global__ void __launch_bounds__(128) cand_rerank_pearson_kernel(
-    const T* __restrict__ rows, uint32_t dim, const double2* __restrict__ mom, const double* __restrict__ q64,
-    const double2* __restrict__ qmom, const uint32_t* __restrict__ qflags, const Cand* __restrict__ cand,
-    const uint32_t* __restrict__ cnt, uint32_t cap, const uint32_t* __restrict__ special, uint32_t n_special,
-    uint64_t* __restrict__ rr_key, double* __restrict__ rr_dist, uint32_t* __restrict__ rr_row, uint32_t rr_stride) {
-  const uint32_t q = blockIdx.x;
-  const uint32_t n_c = cnt[q] < cap ? cnt[q] : cap;
-  const uint32_t n_e = n_c + n_special;
-  const bool q_nan = (qflags[q] & 2u) != 0;
-  const double* qv = q64 + (size_t)q * dim;
-  const double2 qm = qmom[q];
-  const double sd2 = dim == 1 ? 0.0 : __dsqrt_rn(__ddiv_rn(qm.y, (double)dim));
-  for (uint32_t e = blockIdx.y * blockDim.x + threadIdx.x; e < n_e; e += gridDim.y * blockDim.x) {
-    const uint32_t my_row = e < n_c ? cand[(size_t)q * cap + e].row : special[e - n_c];
-    const T* x = rows + (size_t)my_row * dim;
-    const double2 rm = mom[my_row];
-    ExactAcc acc;
-    for (uint32_t j = 0; j < dim; j++) {
-      const double xd = (double)__ldg(x + j);
-      acc.nan_in |= (xd != xd);
-      acc.pearson_step(xd, __ldg(qv + j), rm.x, qm.x);
+    if constexpr (M == SDB_JACCARD) {
+      const uint32_t words = (dim + 31) / 32;
+      d = jaccard_counts(x, dim, a.jfirst + (size_t)row * words, __ldg(a.jux + row),
+                         static_cast<const EqKey<T>*>(a.qkey) + (size_t)q * dim, __ldg(a.qjac + 2 * q + 1),
+                         __ldg(a.qjac + 2 * q));
+    } else if constexpr (M == SDB_PEARSON) {
+      const double2 rm = __ldg(a.mom + row);
+      const RefAcc<SDB_PEARSON> ref{rm.x, qm.x};
+      RefSum acc;
+      for (uint32_t j = 0; j < dim; j++) ref.step(acc, (double)__ldg(x + j), __ldg(qv + j));
+      d = ref.finish(acc, dim, RefAcc<SDB_PEARSON>::sd(rm.y, dim), sd2, q_nan);
+    } else {
+      RefAcc<M> ref;
+      if constexpr (M == SDB_MINKOWSKI) ref.p = a.mink_p;
+      RefSum acc{RefAcc<M>::start};
+      for (uint32_t j = 0; j < dim; j++) ref.step(acc, (double)__ldg(x + j), __ldg(qv + j));
+      d = ref.finish(acc, q_nan);
     }
-    const double covar = __ddiv_rn(acc.acc, (double)dim);
-    const double sd1 = dim == 1 ? 0.0 : __dsqrt_rn(__ddiv_rn(rm.y, (double)dim));
-    const double d = canon_nan(__ddiv_rn(covar, __dmul_rn(sd1, sd2)), acc.nan_in || q_nan);
-    const size_t o = (size_t)q * rr_stride + e;
-    rr_key[o] = dist_key(d);
-    rr_dist[o] = d;
-    rr_row[o] = my_row;
+    rr_store(out, q, e, row, d);
   }
 }
 
-// JACCARD re-rank (direct regime of filtered batches): jaccard_counts per list entry, one thread each, from the
-// corpus's first-occurrence state and the batch's query state (count_prep_queries)
-template <typename T>
-__global__ void __launch_bounds__(128) cand_rerank_jaccard_kernel(
-    const T* __restrict__ rows, uint32_t dim, const uint32_t* __restrict__ jfirst, const uint32_t* __restrict__ jux,
-    const EqKey<T>* __restrict__ qkey, const uint32_t* __restrict__ qjac, const Cand* __restrict__ cand,
-    const uint32_t* __restrict__ cnt, uint32_t cap, uint64_t* __restrict__ rr_key, double* __restrict__ rr_dist,
-    uint32_t* __restrict__ rr_row, uint32_t rr_stride) {
-  const uint32_t q = blockIdx.x;
-  const uint32_t n_c = cnt[q] < cap ? cnt[q] : cap;
-  const uint32_t words = (dim + 31) / 32;
-  for (uint32_t e = blockIdx.y * blockDim.x + threadIdx.x; e < n_c; e += gridDim.y * blockDim.x) {
-    const uint32_t row = cand[(size_t)q * cap + e].row;
-    const double d = jaccard_counts(rows + (size_t)row * dim, dim, jfirst + (size_t)row * words, jux[row],
-                                    qkey + (size_t)q * dim, qjac[2 * q + 1], qjac[2 * q]);
-    const size_t o = (size_t)q * rr_stride + e;
-    rr_key[o] = dist_key(d);
-    rr_dist[o] = d;
-    rr_row[o] = row;
-  }
-}
-
-template <typename T>
-static void launch_rerank_lp(Corpus* c, uint32_t nq, uint32_t n_sp, cudaStream_t st) {
+template <int M>
+static void rerank_entry(Corpus* c, uint32_t nq, uint32_t n_sp, cudaStream_t st) {
   const dim3 grid(nq, RR_GROUPS_Y);
-  auto kern = c->metric == SDB_MANHATTAN   ? cand_rerank_lp_kernel<T, SDB_MANHATTAN>
-              : c->metric == SDB_MINKOWSKI ? cand_rerank_lp_kernel<T, SDB_MINKOWSKI>
-              : c->metric == SDB_HAMMING   ? cand_rerank_lp_kernel<T, SDB_HAMMING>
-                                           : cand_rerank_lp_kernel<T, SDB_CHEBYSHEV>;
-  kern<<<grid, 128, 0, st>>>((const T*)c->d_rows.get(), c->dim, c->d_q64, c->d_qflags, c->d_cand, c->d_cand_cnt,
-                             c->sc_cap, c->d_special, n_sp, c->d_rr_key, c->d_rr_dist, c->d_rr_row, c->rr_stride,
-                             c->minkowski_p);
+  const EntryArgs a{c->minkowski_p, c->d_mom, c->d_qmom, c->d_jfirst, c->d_jux, c->d_qkey.get(), c->d_qjac};
+  if (c->dtype == SDB_F32)
+    cand_rerank_entry_kernel<float, M><<<grid, 128, 0, st>>>((const float*)c->d_rows.get(), c->dim, c->d_q64, c->d_qflags,
+                                                             c->d_cand, c->d_cand_cnt, c->sc_cap, c->d_special, n_sp,
+                                                             rr_out(c), a);
+  else
+    cand_rerank_entry_kernel<double, M><<<grid, 128, 0, st>>>((const double*)c->d_rows.get(), c->dim, c->d_q64,
+                                                              c->d_qflags, c->d_cand, c->d_cand_cnt, c->sc_cap,
+                                                              c->d_special, n_sp, rr_out(c), a);
 }
 
-// COSINE / EUCLIDEAN: the packed kernel for the small sets stage B leaves, the vectorised one for f32 rows otherwise
+template <typename T>
+static void rerank_packed(Corpus* c, uint32_t nq, uint32_t n_sp, cudaStream_t st) {
+  auto kern = c->metric == SDB_COSINE ? cand_rerank_packed_kernel<T, SDB_COSINE> : cand_rerank_packed_kernel<T, SDB_EUCLIDEAN>;
+  kern<<<(nq + 7) / 8, 128, 0, st>>>((const T*)c->d_rows.get(), c->dim, c->d_mag, c->d_q64, c->d_qmag, c->d_qflags,
+                                     c->d_cand, c->d_cand_cnt, c->sc_cap, c->d_special, n_sp, nq, rr_out(c));
+}
+
+// COSINE / EUCLIDEAN: the packed kernel for the small sets stage B leaves; otherwise the vectorised one for f32 rows
+// of a length divisible by 4, the staged one for the rest
 static void rerank_dot(Corpus* c, uint32_t nq, bool small_sets, uint32_t n_sp, cudaStream_t st) {
   const dim3 grid(nq, RR_GROUPS_Y);
-  static const bool no_v4 = getenv("SDB_RERANK_SCALAR") != nullptr;
-  static const bool no_packed = getenv("SDB_RERANK_STAGED") != nullptr;
-  if (small_sets && !no_packed) {
-    const unsigned g = (nq + 7) / 8;
-    const float* f32_rows = (const float*)c->d_rows.get();
-    const double* f64_rows = (const double*)c->d_rows.get();
-    if (c->dtype == SDB_F32 && c->metric == SDB_COSINE)
-      cand_rerank_packed_kernel<float, true><<<g, 128, 0, st>>>(f32_rows, c->dim, c->d_mag, c->d_q64, c->d_qmag, c->d_qflags,
-                                                               c->d_cand, c->d_cand_cnt, c->sc_cap, c->d_special, n_sp,
-                                                               nq, c->d_rr_key, c->d_rr_dist, c->d_rr_row, c->rr_stride);
-    else if (c->dtype == SDB_F32)
-      cand_rerank_packed_kernel<float, false><<<g, 128, 0, st>>>(f32_rows, c->dim, c->d_mag, c->d_q64, c->d_qmag, c->d_qflags,
-                                                                c->d_cand, c->d_cand_cnt, c->sc_cap, c->d_special, n_sp,
-                                                                nq, c->d_rr_key, c->d_rr_dist, c->d_rr_row, c->rr_stride);
-    else if (c->metric == SDB_COSINE)
-      cand_rerank_packed_kernel<double, true><<<g, 128, 0, st>>>(f64_rows, c->dim, c->d_mag, c->d_q64, c->d_qmag, c->d_qflags,
-                                                                c->d_cand, c->d_cand_cnt, c->sc_cap, c->d_special, n_sp,
-                                                                nq, c->d_rr_key, c->d_rr_dist, c->d_rr_row, c->rr_stride);
-    else
-      cand_rerank_packed_kernel<double, false><<<g, 128, 0, st>>>(f64_rows, c->dim, c->d_mag, c->d_q64, c->d_qmag, c->d_qflags,
-                                                                 c->d_cand, c->d_cand_cnt, c->sc_cap, c->d_special, n_sp,
-                                                                 nq, c->d_rr_key, c->d_rr_dist, c->d_rr_row, c->rr_stride);
-  } else if (small_sets && c->dtype == SDB_F32)
-    // (kept for A/B: one warp per query, rows transposed through 6 KB of shared memory)
-    cand_rerank_kernel<float, 1, 32, 256><<<grid, 32, 0, st>>>((const float*)c->d_rows.get(), c->dim, (int)c->metric, c->d_mag,
-                                                               c->d_q64, c->d_qmag, c->d_qflags, c->d_cand, c->d_cand_cnt,
-                                                               c->sc_cap, c->d_special, n_sp, c->d_rr_key,
-                                                               c->d_rr_dist, c->d_rr_row, c->rr_stride);
-  else if (c->dtype == SDB_F32 && c->dim % 4 == 0 && !no_v4)
-    cand_rerank_v4_kernel<4><<<grid, 128, RRV_SMEM, st>>>((const float*)c->d_rows.get(), c->dim, (int)c->metric, c->d_mag, c->d_q64,
-                                                          c->d_qmag, c->d_qflags, c->d_cand, c->d_cand_cnt, c->sc_cap,
-                                                          c->d_special, n_sp, c->d_rr_key, c->d_rr_dist,
-                                                          c->d_rr_row, c->rr_stride);
+  if (small_sets && c->dtype == SDB_F32) rerank_packed<float>(c, nq, n_sp, st);
+  else if (small_sets) rerank_packed<double>(c, nq, n_sp, st);
+  else if (c->dtype == SDB_F32 && c->dim % 4 == 0)
+    cand_rerank_v4_kernel<<<grid, RR_WARPS * 32, RRV_SMEM, st>>>((const float*)c->d_rows.get(), c->dim, (int)c->metric,
+                                                                c->d_mag, c->d_q64, c->d_qmag, c->d_qflags, c->d_cand,
+                                                                c->d_cand_cnt, c->sc_cap, c->d_special, n_sp, rr_out(c));
   else if (c->dtype == SDB_F32)
-    cand_rerank_kernel<float, 4, 32><<<grid, 128, 0, st>>>((const float*)c->d_rows.get(), c->dim, (int)c->metric, c->d_mag,
-                                                           c->d_q64, c->d_qmag, c->d_qflags, c->d_cand, c->d_cand_cnt,
-                                                           c->sc_cap, c->d_special, n_sp, c->d_rr_key,
-                                                           c->d_rr_dist, c->d_rr_row, c->rr_stride);
+    cand_rerank_kernel<float><<<grid, RR_WARPS * 32, 0, st>>>((const float*)c->d_rows.get(), c->dim, (int)c->metric,
+                                                             c->d_mag, c->d_q64, c->d_qmag, c->d_qflags, c->d_cand,
+                                                             c->d_cand_cnt, c->sc_cap, c->d_special, n_sp, rr_out(c));
   else
-    cand_rerank_kernel<double, 4, 32><<<grid, 128, 0, st>>>((const double*)c->d_rows.get(), c->dim, (int)c->metric, c->d_mag,
-                                                            c->d_q64, c->d_qmag, c->d_qflags, c->d_cand, c->d_cand_cnt,
-                                                            c->sc_cap, c->d_special, n_sp, c->d_rr_key,
-                                                            c->d_rr_dist, c->d_rr_row, c->rr_stride);
+    cand_rerank_kernel<double><<<grid, RR_WARPS * 32, 0, st>>>((const double*)c->d_rows.get(), c->dim, (int)c->metric,
+                                                              c->d_mag, c->d_q64, c->d_qmag, c->d_qflags, c->d_cand,
+                                                              c->d_cand_cnt, c->sc_cap, c->d_special, n_sp, rr_out(c));
 }
 
 sdb_status cand_rerank(Corpus* c, uint32_t nq, cudaStream_t st, bool small_sets) {
-  const dim3 grid(nq, RR_GROUPS_Y);
   const uint32_t n_sp = c->filt.bits ? 0u : c->n_special;  // filtered: the passing special rows are in the lists
   switch (family(c)) {
-    case Family::Count:  // the direct regime only (the count path's lists carry exact distances): no special rows
-      if (c->metric == SDB_HAMMING) {
-        if (c->dtype == SDB_F32) launch_rerank_lp<float>(c, nq, n_sp, st);
-        else launch_rerank_lp<double>(c, nq, n_sp, st);
-      } else if (c->dtype == SDB_F32) {
-        cand_rerank_jaccard_kernel<float><<<grid, 128, 0, st>>>((const float*)c->d_rows.get(), c->dim, c->d_jfirst,
-                                                                c->d_jux, c->d_qkey.get(), c->d_qjac, c->d_cand,
-                                                                c->d_cand_cnt, c->sc_cap, c->d_rr_key, c->d_rr_dist,
-                                                                c->d_rr_row, c->rr_stride);
-      } else {
-        cand_rerank_jaccard_kernel<double><<<grid, 128, 0, st>>>((const double*)c->d_rows.get(), c->dim, c->d_jfirst,
-                                                                 c->d_jux, (const unsigned long long*)c->d_qkey.get(),
-                                                                 c->d_qjac, c->d_cand, c->d_cand_cnt, c->sc_cap,
-                                                                 c->d_rr_key, c->d_rr_dist, c->d_rr_row, c->rr_stride);
-      }
+    case Family::Count:  // (the direct regime only; no special rows)
+      if (c->metric == SDB_HAMMING) rerank_entry<SDB_HAMMING>(c, nq, n_sp, st);
+      else rerank_entry<SDB_JACCARD>(c, nq, n_sp, st);
       break;
     case Family::Lp:
-      if (c->dtype == SDB_F32) launch_rerank_lp<float>(c, nq, n_sp, st);
-      else launch_rerank_lp<double>(c, nq, n_sp, st);
+      if (c->metric == SDB_MANHATTAN) rerank_entry<SDB_MANHATTAN>(c, nq, n_sp, st);
+      else if (c->metric == SDB_MINKOWSKI) rerank_entry<SDB_MINKOWSKI>(c, nq, n_sp, st);
+      else rerank_entry<SDB_CHEBYSHEV>(c, nq, n_sp, st);
       break;
     case Family::Centred:  // one kernel for small (after stage B) and large (direct regime, no stage B) sets
-      if (c->dtype == SDB_F32)
-        cand_rerank_pearson_kernel<float><<<grid, 128, 0, st>>>((const float*)c->d_rows.get(), c->dim, c->d_mom,
-                                                                c->d_q64, c->d_qmom, c->d_qflags, c->d_cand,
-                                                                c->d_cand_cnt, c->sc_cap, c->d_special, n_sp,
-                                                                c->d_rr_key, c->d_rr_dist, c->d_rr_row, c->rr_stride);
-      else
-        cand_rerank_pearson_kernel<double><<<grid, 128, 0, st>>>((const double*)c->d_rows.get(), c->dim, c->d_mom,
-                                                                 c->d_q64, c->d_qmom, c->d_qflags, c->d_cand,
-                                                                 c->d_cand_cnt, c->sc_cap, c->d_special, n_sp,
-                                                                 c->d_rr_key, c->d_rr_dist, c->d_rr_row, c->rr_stride);
+      rerank_entry<SDB_PEARSON>(c, nq, n_sp, st);
       break;
     case Family::Dot:
     case Family::Exact:  // (never reaches the re-rank: the exact kernel alone ranks it)
@@ -1674,7 +1578,7 @@ sdb_status cand_final(Corpus* c, uint32_t nq, uint32_t k, uint64_t row_base, uin
 }
 
 sdb_status candidates_init_device() {
-  SDB_CUDA(cudaFuncSetAttribute(cand_rerank_v4_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)RRV_SMEM));
+  SDB_CUDA(cudaFuncSetAttribute(cand_rerank_v4_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)RRV_SMEM));
   return SDB_OK;
 }
 

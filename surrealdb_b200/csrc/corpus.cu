@@ -127,7 +127,7 @@ __global__ void __launch_bounds__(WARPS * 32) finalize_lp_kernel(const T* __rest
 // PEARSON corpora: the reference ranks pearson = covar / (sd1 sd2) of the rows centred in f64 with their own mean, which
 // is the cosine of the centred vectors dx_i = x_i - m1 up to f64 rounding (DESIGN.md section 2, "PEARSON screen").
 // So the cosine screens run on dx (f32 and f64 rows alike), and this kernel keeps per row, in the exact kernel's own
-// arithmetic (ExactAcc::sum_step, then pearson_step's acc2): mom[r] = {m1 = (sum x) / D, S1 = sum (x_i - m1)^2}, both
+// arithmetic (RefAcc<SDB_PEARSON>::mean_step, then step_dev's acc2): mom[r] = {m1 = (sum x) / D, S1 = sum (x_i - m1)^2}, both
 // sequential f64, and snorm = fl32(1/sqrt(S1)).  mag stays the magnitude (sdb_corpus_project reads it).  Special rows
 // (ranked exactly on every query):
 //  - S1 = 0: constant rows (zero and -0.0 rows too, every row when D = 1): pearson is a generated NaN (0/0);

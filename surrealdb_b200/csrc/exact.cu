@@ -1,5 +1,5 @@
 // exact.cu -- KX: exact brute force for ONE query over the whole corpus, in the reference's own f64
-// arithmetic (fnc/util/math/vector.rs:65-83,279-314), followed by an exact radix selection of the k
+// arithmetic (RefAcc, exactmath.cuh), followed by an exact radix selection of the k
 // smallest (distance key, scan position) pairs.  Used for
 //   * F64 corpora and SDB_SCREEN_NONE_EXACT,
 //   * queries the screens cannot bound (zero / non-finite query norm),
@@ -32,17 +32,9 @@ __global__ void __launch_bounds__(WARPS * 32) exact_keys_kernel(const T* __restr
   const double qm = *qmag_p;
   // `metric` also takes the projection-only ids SDB_FN_SIMILARITY_COSINE / SDB_FN_DOT / SDB_FN_MAGNITUDE
   if (metric == SDB_PEARSON && threadIdx.x == 0) {
-    // mean: fnc/util/math/mod.rs:54-69 ; deviation(sample=false): vector.rs:9-21 -- sequential, as the reference
-    double s = 0.0;
-    for (uint32_t i = 0; i < dim; i++) s = __dadd_rn(s, q64[i]);
-    const double m2 = __ddiv_rn(s, (double)dim);
-    double dv = 0.0;
-    for (uint32_t i = 0; i < dim; i++) {
-      const double x = __dsub_rn(q64[i], m2);
-      dv = __dadd_rn(dv, __dmul_rn(x, x));
-    }
-    s_qstat[0] = m2;
-    s_qstat[1] = dim == 1 ? 0.0 : __dsqrt_rn(__ddiv_rn(dv, (double)dim));
+    const double2 mom = pearson_moments(q64, dim);
+    s_qstat[0] = mom.x;
+    s_qstat[1] = RefAcc<SDB_PEARSON>::sd(mom.y, dim);
   }
   __syncthreads();
   const int n_phase = metric == SDB_PEARSON ? 2 : 1;
@@ -50,10 +42,9 @@ __global__ void __launch_bounds__(WARPS * 32) exact_keys_kernel(const T* __restr
   for (uint64_t b0 = (uint64_t)blockIdx.x * rows_per_block; b0 < n; b0 += (uint64_t)gridDim.x * rows_per_block) {
     const uint64_t r = b0 + warp * 32 + lane;
     const uint32_t my_row = r < n ? (uint32_t)r : NO_ROW;
-    ExactAcc acc;
+    RefSum acc;
     double m1 = 0.0;
-    bool nan_in = false;
-    if (metric == SDB_CHEBYSHEV) acc.acc = -1.7976931348623157e308;  // f64::MIN
+    if (metric == SDB_CHEBYSHEV) acc.acc = RefAcc<SDB_CHEBYSHEV>::start;
     for (int phase = 0; phase < n_phase; phase++) {
       for (uint32_t cb = 0; cb < dim; cb += EX_QCHUNK) {
         const uint32_t cw = dim - cb < EX_QCHUNK ? dim - cb : EX_QCHUNK;
@@ -78,29 +69,30 @@ __global__ void __launch_bounds__(WARPS * 32) exact_keys_kernel(const T* __restr
               case SDB_COSINE:
               case SDB_FN_SIMILARITY_COSINE:
               case SDB_FN_DOT:
-                for (uint32_t j = 0; j < lim; j++) acc.cosine_step((double)t[j], s_q[c0 + j]);
+                for (uint32_t j = 0; j < lim; j++) RefAcc<SDB_COSINE>{}.step(acc, (double)t[j], s_q[c0 + j]);
                 break;
               case SDB_FN_MAGNITUDE: break;  // precomputed at finalize
               case SDB_EUCLIDEAN:
-                for (uint32_t j = 0; j < lim; j++) acc.euclid_step((double)t[j], s_q[c0 + j]);
+                for (uint32_t j = 0; j < lim; j++) RefAcc<SDB_EUCLIDEAN>{}.step(acc, (double)t[j], s_q[c0 + j]);
                 break;
               case SDB_MANHATTAN:
-                for (uint32_t j = 0; j < lim; j++) acc.manhattan_step((double)t[j], s_q[c0 + j]);
+                for (uint32_t j = 0; j < lim; j++) RefAcc<SDB_MANHATTAN>{}.step(acc, (double)t[j], s_q[c0 + j]);
                 break;
               case SDB_CHEBYSHEV:
-                for (uint32_t j = 0; j < lim; j++) acc.chebyshev_step((double)t[j], s_q[c0 + j]);
+                for (uint32_t j = 0; j < lim; j++) RefAcc<SDB_CHEBYSHEV>{}.step(acc, (double)t[j], s_q[c0 + j]);
                 break;
               case SDB_HAMMING:
-                for (uint32_t j = 0; j < lim; j++) acc.hamming_step((double)t[j], s_q[c0 + j]);
+                for (uint32_t j = 0; j < lim; j++) RefAcc<SDB_HAMMING>{}.step(acc, (double)t[j], s_q[c0 + j]);
                 break;
               case SDB_MINKOWSKI:
-                for (uint32_t j = 0; j < lim; j++) acc.minkowski_step((double)t[j], s_q[c0 + j], mink_p);
+                for (uint32_t j = 0; j < lim; j++) RefAcc<SDB_MINKOWSKI>{mink_p}.step(acc, (double)t[j], s_q[c0 + j]);
                 break;
               default:  // SDB_PEARSON
                 if (phase == 0) {
-                  for (uint32_t j = 0; j < lim; j++) acc.sum_step((double)t[j]);
+                  for (uint32_t j = 0; j < lim; j++) RefAcc<SDB_PEARSON>::mean_step(acc, (double)t[j]);
                 } else {
-                  for (uint32_t j = 0; j < lim; j++) acc.pearson_step((double)t[j], s_q[c0 + j], m1, s_qstat[0]);
+                  const RefAcc<SDB_PEARSON> pe{m1, s_qstat[0]};
+                  for (uint32_t j = 0; j < lim; j++) pe.step_dev(acc, (double)t[j], s_q[c0 + j]);
                 }
                 break;
             }
@@ -110,7 +102,6 @@ __global__ void __launch_bounds__(WARPS * 32) exact_keys_kernel(const T* __restr
       }
       if (metric == SDB_PEARSON && phase == 0) {
         m1 = __ddiv_rn(acc.acc, (double)dim);
-        nan_in = acc.nan_in;
         acc.acc = 0.0;
       }
     }
@@ -122,22 +113,17 @@ __global__ void __launch_bounds__(WARPS * 32) exact_keys_kernel(const T* __restr
       } else {
         double d;
         switch (metric) {
-          case SDB_COSINE: d = cosine_finish(acc, mag[r], qm, q_nan); break;
-          case SDB_FN_SIMILARITY_COSINE:  // vector.rs:65-71
-            d = canon_nan(__ddiv_rn(acc.acc, __dmul_rn(mag[r], qm)), acc.nan_in || q_nan);
-            break;
-          case SDB_FN_DOT: d = canon_nan(acc.acc, acc.nan_in || q_nan); break;  // vector.rs:279-281
-          case SDB_FN_MAGNITUDE: d = mag[r]; break;                             // vector.rs:301-314
-          case SDB_EUCLIDEAN: d = euclid_finish(acc, q_nan); break;
-          case SDB_MANHATTAN: d = canon_nan(acc.acc, acc.nan_in || q_nan); break;
-          case SDB_MINKOWSKI: d = canon_nan(pow(acc.acc, __ddiv_rn(1.0, mink_p)), acc.nan_in || q_nan); break;
-          case SDB_CHEBYSHEV:
-          case SDB_HAMMING: d = acc.acc; break;
-          default: {  // pearson: covar/len / (sd1 * sd2)
-            const double covar = __ddiv_rn(acc.acc, (double)dim);
-            const double sd1 = dim == 1 ? 0.0 : __dsqrt_rn(__ddiv_rn(acc.acc2, (double)dim));
-            d = canon_nan(__ddiv_rn(covar, __dmul_rn(sd1, s_qstat[1])), nan_in || q_nan);
-          }
+          case SDB_COSINE: d = RefAcc<SDB_COSINE>{}.finish(acc, mag[r], qm, q_nan); break;
+          case SDB_FN_SIMILARITY_COSINE: d = RefAcc<SDB_FN_SIMILARITY_COSINE>{}.finish(acc, mag[r], qm, q_nan); break;
+          case SDB_FN_DOT: d = RefAcc<SDB_FN_DOT>{}.finish(acc, q_nan); break;
+          case SDB_FN_MAGNITUDE: d = RefAcc<SDB_FN_MAGNITUDE>{}.finish(mag[r]); break;
+          case SDB_EUCLIDEAN: d = RefAcc<SDB_EUCLIDEAN>{}.finish(acc, q_nan); break;
+          case SDB_MANHATTAN: d = RefAcc<SDB_MANHATTAN>{}.finish(acc, q_nan); break;
+          case SDB_MINKOWSKI: d = RefAcc<SDB_MINKOWSKI>{mink_p}.finish(acc, q_nan); break;
+          case SDB_CHEBYSHEV: d = RefAcc<SDB_CHEBYSHEV>{}.finish(acc, q_nan); break;
+          case SDB_HAMMING: d = RefAcc<SDB_HAMMING>{}.finish(acc, q_nan); break;
+          default:  // SDB_PEARSON
+            d = RefAcc<SDB_PEARSON>::finish(acc, dim, RefAcc<SDB_PEARSON>::sd(acc.acc2, dim), s_qstat[1], q_nan);
         }
         key = dist_key(d);
         if (vals) vals[r] = d;
