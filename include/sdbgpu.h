@@ -297,7 +297,12 @@ sdb_status sdb_knn_wait(sdb_corpus*, uint32_t ticket);
  * the same); sdb_knn_last_stats then reports screen_used = SDB_SCREEN_NONE_EXACT and n_passes = 0 for a batch of such
  * queries only.
  * Host variants: `filters` is host memory, staged per batch on the copy stream (submit: `queries`, `filters` and the
- * outputs stay valid until the wait returns).  Device variant: d_filters is device memory. */
+ * outputs stay valid until the wait returns).  Device variants: d_filters is device memory, read in place (submit: it
+ * stays valid and unchanged until the wait returns).
+ * sdb_knn_submit_filtered_device is the asynchronous device variant (row_base as in sdb_knn_submit_device).  The
+ * direct / screened split needs each bitmap's set bits on the host, so before it returns the call counts them on the
+ * device and waits for that count alone: one short host wait for a kernel that reads the bitmaps once, on a stream
+ * that carries no batch, never for the batches already in flight. */
 sdb_status sdb_knn_bruteforce_filtered(sdb_corpus*, const double* queries, uint32_t nq, uint32_t k,
                                        const uint32_t* filters, uint32_t n_filters, const uint32_t* query_filter,
                                        uint64_t* out_rows, double* out_dist, uint32_t* out_count,
@@ -309,6 +314,10 @@ sdb_status sdb_knn_bruteforce_filtered_device(sdb_corpus*, const double* d_queri
 sdb_status sdb_knn_submit_filtered(sdb_corpus*, const double* queries, uint32_t nq, uint32_t k,
                                    const uint32_t* filters, uint32_t n_filters, const uint32_t* query_filter,
                                    uint64_t* out_rows, double* out_dist, uint32_t* out_count, uint32_t* ticket);
+sdb_status sdb_knn_submit_filtered_device(sdb_corpus*, const double* d_queries, uint32_t nq, uint32_t k,
+                                          const uint32_t* d_filters, uint32_t n_filters, const uint32_t* query_filter,
+                                          uint64_t row_base, uint64_t* d_out_rows, double* d_out_dist,
+                                          uint32_t* d_out_count, uint32_t* ticket);
 
 /* ---- multi-GPU brute force (SURVEY 8e): the corpus is row-sharded, every shard searches its rows, ONE NCCL
  * all-gather moves the per-shard top-k blocks and a merge kernel on every rank produces the global top-k by
@@ -339,6 +348,32 @@ sdb_status sdb_knn_sharded_wait(sdb_corpus*, uint32_t ticket);
 /* one process, N GPUs: shards[i] lives on the i-th context of sdb_ctx_create_multi; queries / out_* are host buffers */
 sdb_status sdb_knn_sharded_multi(sdb_corpus* const* shards, int n_shards, const double* queries, uint32_t nq, uint32_t k,
                                  uint64_t* out_rows, double* out_dist, uint32_t* out_count);
+/* Filtered brute force on a row-sharded column: `WHERE emb <|k|> $q AND cond` when the column spans several GPUs.
+ * The bitmaps cover the GLOBAL rows: n_filters bitmaps of W = ceil(n_rows_total / 32) uint32 words each, bit r = bit
+ * r % 32 of word r / 32 (the sdb_hop_filter convention), query_filter as in sdb_knn_bruteforce_filtered (host memory,
+ * NULL = filter 0).  Collective like the calls above: every rank passes the same queries, bitmaps and query_filter.
+ * Each shard reads only its span of each bitmap (words row_base / 32 .. (row_base + rows) / 32 + 1, the host variants
+ * copy just that span) and shifts it to its own rows on the device; any row_base works, aligned or not.  Query q
+ * returns exactly what sdb_knn_bruteforce_filtered returns on the unsharded column with the same bitmaps: the same
+ * global rows in the same order, bit-identical distances, the same counts.  Completion through sdb_knn_sharded_wait;
+ * filtered and unfiltered sharded tickets mix, up to 4 in flight.  Refusals: those of sdb_knn_bruteforce_filtered,
+ * and SDB_EINVAL when row_base + sdb_corpus_rows > n_rows_total; the column keeps answering after one.  Device
+ * variant: d_filters is device memory, read in place until the wait returns; before it returns the call counts the
+ * slice's set bits on the device and waits for that count alone (see sdb_knn_submit_filtered_device). */
+sdb_status sdb_knn_sharded_submit_filtered(sdb_corpus*, const double* queries, uint32_t nq, uint32_t k,
+                                           const uint32_t* filters, uint32_t n_filters, const uint32_t* query_filter,
+                                           uint64_t n_rows_total, uint64_t* out_rows, double* out_dist,
+                                           uint32_t* out_count, uint32_t* ticket);
+sdb_status sdb_knn_sharded_submit_filtered_device(sdb_corpus*, const double* d_queries, uint32_t nq, uint32_t k,
+                                                  const uint32_t* d_filters, uint32_t n_filters,
+                                                  const uint32_t* query_filter, uint64_t n_rows_total,
+                                                  uint64_t* d_out_rows, double* d_out_dist, uint32_t* d_out_count,
+                                                  uint32_t* ticket);
+/* one process, N GPUs: every shard slices the same host bitmaps */
+sdb_status sdb_knn_sharded_multi_filtered(sdb_corpus* const* shards, int n_shards, const double* queries, uint32_t nq,
+                                          uint32_t k, const uint32_t* filters, uint32_t n_filters,
+                                          const uint32_t* query_filter, uint64_t n_rows_total, uint64_t* out_rows,
+                                          double* out_dist, uint32_t* out_count);
 /* ---- projected scalar vector functions over a whole column (SURVEY 8f-4): replaces a per-row evaluation of
  *      vector::distance::* / vector::similarity::* / vector::dot / vector::magnitude (fnc/vector.rs:25-143,
  *      fnc/util/math/vector.rs:61-314) in `SELECT vector::similarity::cosine(emb, $q) FROM t`.

@@ -37,6 +37,8 @@ ABI_SYMBOLS = [
     "sdb_graph_load_csr", "sdb_graph_load_csr_shard", "sdb_graph_destroy", "sdb_graph_expand", "sdb_graph_expand_device", "sdb_device_free", "sdb_graph_collect", "sdb_free",
     "sdb_graph_expand_filtered", "sdb_graph_expand_filtered_device", "sdb_graph_collect_filtered",
     "sdb_knn_bruteforce_filtered", "sdb_knn_bruteforce_filtered_device", "sdb_knn_submit_filtered",
+    "sdb_knn_submit_filtered_device", "sdb_knn_sharded_submit_filtered", "sdb_knn_sharded_submit_filtered_device",
+    "sdb_knn_sharded_multi_filtered",
     "sdb_hnsw_search_filtered_batch", "sdb_hnsw_search_filtered_batch_device", "sdb_hnsw_last_spilled",
 ]
 
@@ -111,6 +113,7 @@ def lib():
     L.sdb_knn_bruteforce_filtered.argtypes = [vp, vp, u32, u32, vp, u32, vp, vp, vp, vp, vp]
     L.sdb_knn_bruteforce_filtered_device.argtypes = [vp, vp, u32, u32, vp, u32, vp, u64, vp, vp, vp]
     L.sdb_knn_submit_filtered.argtypes = [vp, vp, u32, u32, vp, u32, vp, vp, vp, vp, C.POINTER(u32)]
+    L.sdb_knn_submit_filtered_device.argtypes = [vp, vp, u32, u32, vp, u32, vp, u64, vp, vp, vp, C.POINTER(u32)]
     L.sdb_comm_unique_id.argtypes = [vp]
     L.sdb_comm_init_rank.argtypes = [vp, i32, i32, vp]
     L.sdb_comm_size.argtypes = [vp]
@@ -121,6 +124,10 @@ def lib():
     L.sdb_knn_sharded_submit_device.argtypes = [vp, vp, u32, u32, vp, vp, vp, C.POINTER(u32)]
     L.sdb_knn_sharded_wait.argtypes = [vp, u32]
     L.sdb_knn_sharded_multi.argtypes = [vp, i32, vp, u32, u32, vp, vp, vp]
+    L.sdb_knn_sharded_submit_filtered.argtypes = [vp, vp, u32, u32, vp, u32, vp, u64, vp, vp, vp, C.POINTER(u32)]
+    L.sdb_knn_sharded_submit_filtered_device.argtypes = [vp, vp, u32, u32, vp, u32, vp, u64, vp, vp, vp,
+                                                         C.POINTER(u32)]
+    L.sdb_knn_sharded_multi_filtered.argtypes = [vp, i32, vp, u32, u32, vp, u32, vp, u64, vp, vp, vp]
     L.sdb_corpus_project.argtypes = [vp, vp, i32, vp]
     L.sdb_knn_last_stats.argtypes = [vp, C.POINTER(KnnStats)]
     L.sdb_topk_merge_device.argtypes = [vp, u32, u32, u32, vp, vp, vp, u64, u64, u64, vp, vp, vp]

@@ -316,6 +316,8 @@ static sdb_status enqueue_batch(Corpus* c, Ticket& t) {
   const sdb_status rc = enqueue_screened(c, t);
   t.nq = ns + nd;
   SDB_TRY(rc);
+  SDB_CUDA(t.d_stat_scr.reserve(4));  // (the block header of a sharded batch adds both parts' flagged queries)
+  SDB_CUDA(cudaMemcpyAsync(t.d_stat_scr, c->d_stat, sizeof(uint32_t) * 4, cudaMemcpyDeviceToDevice, st));
   SDB_TRY(enqueue_direct(c, t, ns, nd, false));
   SDB_CUDA(cudaEventRecord(t.ev_end, st));
   return SDB_OK;
@@ -784,29 +786,49 @@ static sdb_status wait_locked(Corpus* c, Ticket* t) {
   return rc;
 }
 
+}  // namespace sdb
+extern "C" {  // (defined with the entry points below)
+static sdb_status check_filters(uint32_t nq, const uint32_t* filters, uint32_t n_filters, const uint32_t* query_filter);
+static sdb_status stage_filters(sdb::Corpus* c, sdb::Ticket& t, const sdb::RowFilters& rf, bool host, uint32_t nq,
+                                const uint32_t** bits, std::vector<uint64_t>* rows);
+}
+namespace sdb {
+
 // ---- hooks for comm.cu (sharded search).  The caller holds c->mu. ---------------------------------------------------
+// rf: the call's global bitmaps (rf.bits == nullptr: unfiltered), host memory with h_queries, else device memory
 sdb_status knn_submit_for_shard(Corpus* c, const double* d_queries, const double* h_queries, uint32_t nq, uint32_t k,
-                                uint64_t* d_out_rows, double* d_out_dist, uint32_t* d_out_count, int* slot_index,
-                                uint32_t* ticket, const double** d_queries_used) {
+                                const RowFilters& rf, uint64_t* d_out_rows, double* d_out_dist, uint32_t* d_out_count,
+                                int* slot_index, uint32_t* ticket, const double** d_queries_used) {
+  if (rf.bits) {  // refused before anything is enqueued
+    SDB_TRY(check_filters(nq, rf.bits, rf.n_filters, rf.query_filter));
+    if (c->row_base + c->n > rf.n_rows_total) {
+      set_error("sharded filtered KNN: shard rows %llu..%llu outside the bitmaps' %llu rows",
+                (unsigned long long)c->row_base, (unsigned long long)(c->row_base + c->n),
+                (unsigned long long)rf.n_rows_total);
+      return SDB_EINVAL;
+    }
+  }
   Ticket* t = free_ticket(c);
   if (!t) {
     set_error("too many batches in flight (%d): call the matching wait first", N_TICKETS);
     return SDB_EOVERFLOW;
   }
   *slot_index = (int)(t - c->tickets);
-  bool h2d_pending = false;
+  SDB_TRY(ticket_prepare(c, *t, nq));
+  cudaStream_t cs = c->ctx->copy_stream;
   if (h_queries) {  // host queries: staged through the slot's device buffer on the copy stream
-    SDB_TRY(ticket_prepare(c, *t, nq));
     const size_t need_q = (size_t)nq * c->dim;
     SDB_CUDA(t->d_in_q.reserve(need_q));
-    cudaStream_t cs = c->ctx->copy_stream;
     SDB_CUDA(cudaMemcpyAsync(t->d_in_q, h_queries, sizeof(double) * need_q, cudaMemcpyHostToDevice, cs));
-    SDB_CUDA(cudaEventRecord(t->ev_h2d, cs));
     d_queries = t->d_in_q;
-    h2d_pending = true;
   }
-  t->wait_h2d = h2d_pending;
-  SDB_TRY(submit_locked(c, t, d_queries, nq, k, c->row_base, d_out_rows, d_out_dist, d_out_count, nullptr));
+  const uint32_t* bits = nullptr;
+  std::vector<uint64_t> rows_per_filter;
+  if (rf.bits) SDB_TRY(stage_filters(c, *t, rf, h_queries != nullptr, nq, &bits, &rows_per_filter));
+  t->wait_h2d = h_queries || rf.bits;
+  if (t->wait_h2d) SDB_CUDA(cudaEventRecord(t->ev_h2d, cs));
+  SDB_TRY(submit_locked(c, t, d_queries, nq, k, c->row_base, d_out_rows, d_out_dist, d_out_count, nullptr, bits,
+                        rf.query_filter, rf.bits ? rows_per_filter.data() : nullptr));
   *ticket = t->id;
   *d_queries_used = d_queries;
   return SDB_OK;
@@ -835,11 +857,27 @@ sdb_status knn_release_ticket(Corpus* c, uint32_t ticket) {
   t->h_out_count = nullptr;
   return SDB_OK;
 }
-const uint32_t* knn_ticket_stat_host(Corpus* c, uint32_t ticket, int* exact_only) {
+// a permuted batch's counters: queries flagged by both sub-batches, the rest as the direct sub-batch left them
+__global__ void sum_flagged_kernel(const uint32_t* __restrict__ direct, const uint32_t* __restrict__ screened,
+                                   uint32_t* __restrict__ out) {
+  if (threadIdx.x < 4) out[threadIdx.x] = direct[threadIdx.x] + (threadIdx.x == 0 ? screened[0] : 0u);
+}
+// the 16-byte block header of a sharded batch, enqueued on its stream: [0] = queries this shard must still repair on
+// the host (failed proof, special queries), [1..3] the batch's other counters (d_stat)
+sdb_status knn_shard_header(Corpus* c, uint32_t ticket, void* d_hdr) {
   Ticket* t = find_ticket(c, ticket);
-  if (!t) return nullptr;
-  *exact_only = (t->n_rungs == 0) ? 1 : 0;
-  return t->h_stat;
+  if (!t) return SDB_EINVAL;
+  cudaStream_t st = t->stream;
+  if (t->n_rungs == 0) {  // exact-only or counted batch: the counters the host holds
+    SDB_CUDA(cudaMemcpyAsync(d_hdr, t->h_stat, 16, cudaMemcpyHostToDevice, st));
+  } else if (t->permuted) {
+    sum_flagged_kernel<<<1, 32, 0, st>>>(c->d_stat, t->d_stat_scr, (uint32_t*)d_hdr);
+    count_launch(c->ctx);
+    SDB_CUDA(cudaGetLastError());
+  } else {
+    SDB_CUDA(cudaMemcpyAsync(d_hdr, c->d_stat, 16, cudaMemcpyDeviceToDevice, st));
+  }
+  return SDB_OK;
 }
 
 // ---- global top-k merge of per-shard lists (after the NCCL all-gather) -----------------------------
@@ -1316,25 +1354,31 @@ sdb_status sdb_knn_submit_device(sdb_corpus* c, const double* d_queries, uint32_
   return SDB_OK;
 }
 
-// per filter used by the batch, on the host, as far as the two decisions need it: the exact number of set bits while
-// it is at most DIRECT_MAX_ROWS (direct regime; the count stops at the first bit beyond, after ~T / 32 / density words,
-// and all-zero words cost one compare), else an estimate from 4096 evenly spaced words, which only decides
-// FiltArg::mask_hits (a speed switch; either value gives the same results)
-static std::vector<uint64_t> count_filter_rows_host(const Corpus* c, const uint32_t* filters, uint32_t n_filters,
-                                                    const uint32_t* query_filter, uint32_t nq) {
-  const uint64_t words = (c->n + 31) / 32;
+// per filter used by the batch, on the host, as far as the two decisions need it, over the bits [first, first + n_rows)
+// of bitmaps of `words` words (a shard's rows of global bitmaps; unsharded calls: 0 and the corpus' rows): the exact
+// number of set bits while it is at most DIRECT_MAX_ROWS (direct regime; the count stops at the first bit beyond, after
+// ~T / 32 / density words, and all-zero words cost one compare), else an estimate from 4096 evenly spaced words, which
+// only decides FiltArg::mask_hits (a speed switch; either value gives the same results)
+static std::vector<uint64_t> count_filter_rows_host(const uint32_t* filters, uint64_t words, uint64_t first,
+                                                    uint64_t n_rows, uint32_t n_filters, const uint32_t* query_filter,
+                                                    uint32_t nq) {
+  const uint64_t w0 = first / 32, w1 = (first + n_rows + 31) / 32;  // the words holding the range
+  const uint32_t end = (uint32_t)((first + n_rows) & 31u);
+  const uint32_t m0 = ~0u << (first & 31u), m1 = end ? ~0u >> (32u - end) : ~0u;  // its bits in the first / last word
   std::vector<uint64_t> cnt(n_filters, ~0ull);
   for (uint32_t q = 0; q < nq; q++) {
     const uint32_t f = query_filter ? query_filter[q] : 0u;
     if (cnt[f] != ~0ull) continue;
     const uint32_t* b = filters + (size_t)f * words;
     uint64_t n = 0;
-    for (uint64_t w = 0; w < words && n <= DIRECT_MAX_ROWS; w++)
-      if (b[w]) n += (uint64_t)__builtin_popcount(b[w]);
+    for (uint64_t w = w0; w < w1 && n <= DIRECT_MAX_ROWS; w++) {
+      const uint32_t v = b[w] & (w == w0 ? m0 : ~0u) & (w == w1 - 1 ? m1 : ~0u);
+      if (v) n += (uint64_t)__builtin_popcount(v);
+    }
     if (n > DIRECT_MAX_ROWS) {
-      const uint64_t samples = std::min<uint64_t>(words, 4096), step = words / samples;
+      const uint64_t samples = std::min<uint64_t>(w1 - w0, 4096), step = (w1 - w0) / samples;
       uint64_t s = 0;
-      for (uint64_t i = 0; i < samples; i++) s += (uint64_t)__builtin_popcount(b[i * step]);
+      for (uint64_t i = 0; i < samples; i++) s += (uint64_t)__builtin_popcount(b[w0 + i * step]);
       n = std::max<uint64_t>(DIRECT_MAX_ROWS + 1, s * step);  // estimate, never below the direct bound
     }
     cnt[f] = n;
@@ -1351,11 +1395,102 @@ __global__ void count_filter_rows_kernel(const uint32_t* __restrict__ bits, uint
   for (int o = 16; o > 0; o >>= 1) n += __shfl_xor_sync(0xffffffffu, n, o);
   if ((threadIdx.x & 31u) == 0 && n) atomicAdd(cnt + blockIdx.y, n);
 }
+// A shard's part of global bitmaps (sharded filtered calls): bits [row_base, row_base + n) of each as a local bitmap of
+// ceil(n / 32) words, bit r = the shard's row r.  src: word row_base / 32 of filter 0's bitmap, filters `pitch` words
+// apart, `avail` words of each readable from there; shift = row_base % 32.  The bits past the shard's last row belong
+// to the next shard's rows and are cleared: the screens' padding rows must never pass.  cnt (nullable, zeroed): set
+// bits per filter.
+__global__ void slice_filter_rows_kernel(const uint32_t* __restrict__ src, uint64_t pitch, uint64_t avail,
+                                         uint32_t shift, uint64_t n, uint32_t n_filters, uint32_t* __restrict__ dst,
+                                         unsigned long long* __restrict__ cnt) {
+  const uint64_t words = (n + 31) / 32;
+  const uint32_t tail = (uint32_t)(n & 31u);
+  for (uint32_t f = blockIdx.y; f < n_filters; f += gridDim.y) {
+    const uint32_t* s = src + (size_t)f * pitch;
+    unsigned long long c = 0;
+    for (uint64_t w = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; w < words; w += (uint64_t)gridDim.x * blockDim.x) {
+      const uint32_t lo = __ldg(s + w), hi = w + 1 < avail ? __ldg(s + w + 1) : 0u;
+      uint32_t v = __funnelshift_r(lo, hi, shift);
+      if (tail && w == words - 1) v &= (1u << tail) - 1u;
+      dst[(size_t)f * words + w] = v;
+      c += (unsigned long long)__popc(v);
+    }
+    if (cnt) {
+#pragma unroll
+      for (int o = 16; o > 0; o >>= 1) c += __shfl_xor_sync(0xffffffffu, c, o);
+      if ((threadIdx.x & 31u) == 0 && c) atomicAdd(cnt + f, c);
+    }
+  }
+}
+
+// The bitmaps of a filtered batch as its kernels read them (*bits: ceil(c->n / 32) words per filter, bit r = the
+// corpus' row r) and the set bits of each for plan_filtered (*rows), enqueued on the copy stream, which carries no batch.
+//   unsharded call: host bitmaps are copied whole into the slot's d_in_filt; device bitmaps are read in place
+//   sharded call: only the shard's span of each global bitmap is read, words row_base / 32 .. (row_base + n) / 32 + 1
+//     (host bitmaps: one strided copy into d_in_span), and slice_filter_rows_kernel shifts it into d_in_filt
+// Host bitmaps are counted on the host.  Device bitmaps are counted on the device, and the host waits for that count
+// alone -- an event on the copy stream, never a batch stream, so a batch in flight keeps running.  The caller records
+// ev_h2d on the copy stream afterwards; submit_locked makes the batch's stream wait for it.
+static sdb_status stage_filters(Corpus* c, Ticket& t, const RowFilters& rf, bool host, uint32_t nq,
+                                const uint32_t** bits, std::vector<uint64_t>* rows) {
+  cudaStream_t cs = c->ctx->copy_stream;
+  const uint32_t nf = rf.n_filters;
+  const bool sharded = rf.n_rows_total != 0;
+  const uint64_t words = (c->n + 31) / 32;
+  const uint64_t W = sharded ? (rf.n_rows_total + 31) / 32 : words;  // words of each bitmap the caller holds
+  const uint64_t first = sharded ? c->row_base : 0;
+  *bits = rf.bits;
+  if (host || sharded) {
+    SDB_CUDA(t.d_in_filt.reserve(std::max<size_t>(1, (size_t)nf * words)));
+    *bits = t.d_in_filt;
+  }
+  rows->assign(nf, 0);
+  if (!words || !nf || !c->finalized) return SDB_OK;  // (submit_locked refuses a corpus that is not finalized)
+  if (host && !sharded) {
+    SDB_CUDA(cudaMemcpyAsync(t.d_in_filt, rf.bits, sizeof(uint32_t) * nf * words, cudaMemcpyHostToDevice, cs));
+    *rows = count_filter_rows_host(rf.bits, W, first, c->n, nf, rf.query_filter, nq);  // while the copy runs
+    return SDB_OK;
+  }
+  unsigned long long* d_cnt = nullptr;
+  if (!host) {
+    SDB_CUDA(t.d_fcnt.reserve(nf));
+    SDB_CUDA(t.h_fcnt.reserve(nf));
+    SDB_CUDA(cudaMemsetAsync(t.d_fcnt, 0, sizeof(unsigned long long) * nf, cs));
+    d_cnt = t.d_fcnt;
+  }
+  const uint32_t gx = (uint32_t)std::min<uint64_t>((words + 255) / 256, 64);
+  if (sharded) {
+    const uint64_t w0 = first / 32, span = std::min(words + 1, W - w0);  // (the last row's word is below W)
+    const uint32_t* src = rf.bits + w0;
+    uint64_t pitch = W;
+    if (host) {  // per rank and batch about 1 / R of the bytes an unsharded filtered call moves
+      SDB_CUDA(t.d_in_span.reserve((size_t)nf * span));
+      SDB_CUDA(cudaMemcpy2DAsync(t.d_in_span, sizeof(uint32_t) * span, src, sizeof(uint32_t) * W,
+                                 sizeof(uint32_t) * span, nf, cudaMemcpyHostToDevice, cs));
+      src = t.d_in_span;
+      pitch = span;
+    }
+    slice_filter_rows_kernel<<<dim3(gx, std::min(nf, 65535u)), 256, 0, cs>>>(src, pitch, span, (uint32_t)(first & 31u),
+                                                                           c->n, nf, t.d_in_filt, d_cnt);
+  } else {
+    count_filter_rows_kernel<<<dim3(gx, nf), 256, 0, cs>>>(rf.bits, words, d_cnt);
+  }
+  count_launch(c->ctx);
+  SDB_CUDA(cudaGetLastError());
+  if (host) {
+    *rows = count_filter_rows_host(rf.bits, W, first, c->n, nf, rf.query_filter, nq);  // while the slice runs
+    return SDB_OK;
+  }
+  SDB_CUDA(cudaMemcpyAsync(t.h_fcnt, t.d_fcnt, sizeof(unsigned long long) * nf, cudaMemcpyDeviceToHost, cs));
+  SDB_CUDA(cudaEventRecord(t.ev_h2d, cs));
+  SDB_CUDA(cudaEventSynchronize(t.ev_h2d));
+  for (uint32_t f = 0; f < nf; f++) (*rows)[f] = t.h_fcnt[f];
+  return SDB_OK;
+}
 
 static sdb_status submit_host_locked(sdb_corpus* c, const double* queries, uint32_t nq, uint32_t k, uint64_t* out_rows,
                                      double* out_dist, uint32_t* out_count, const volatile int* cancel, Ticket** out_t,
-                                     const uint32_t* filters = nullptr, uint32_t n_filters = 0,
-                                     const uint32_t* query_filter = nullptr) {
+                                     const RowFilters& rf = RowFilters()) {
   Ticket* t = free_ticket(c);
   if (!t) {
     set_error("too many batches in flight (%d): call sdb_knn_wait first", N_TICKETS);
@@ -1367,18 +1502,13 @@ static sdb_status submit_host_locked(sdb_corpus* c, const double* queries, uint3
   // the queries travel on the copy stream, so the transfer of batch i+1 overlaps the kernels of batch i
   cudaStream_t cs = c->ctx->copy_stream;
   SDB_CUDA(cudaMemcpyAsync(t->d_in_q, queries, sizeof(double) * (size_t)nq * c->dim, cudaMemcpyHostToDevice, cs));
-  if (filters) {  // ... and so do the row filters, into the slot's own copy
-    const size_t words = (size_t)n_filters * ((c->n + 31) / 32);
-    SDB_CUDA(t->d_in_filt.reserve(words ? words : 1));
-    if (words) SDB_CUDA(cudaMemcpyAsync(t->d_in_filt, filters, sizeof(uint32_t) * words, cudaMemcpyHostToDevice, cs));
-  }
+  const uint32_t* bits = nullptr;  // ... and so do the row filters, into the slot's own copy
+  std::vector<uint64_t> rows_per_filter;
+  if (rf.bits) SDB_TRY(stage_filters(c, *t, rf, true, nq, &bits, &rows_per_filter));
   SDB_CUDA(cudaEventRecord(t->ev_h2d, cs));
   t->wait_h2d = true;  // submit_locked makes the batch's stream wait for the transfer
-  std::vector<uint64_t> rows_per_filter;
-  if (filters) rows_per_filter = count_filter_rows_host(c, filters, n_filters, query_filter, nq);
-  SDB_TRY(submit_locked(c, t, t->d_in_q, nq, k, c->row_base, t->res.rows, t->res.dist, t->res.count, cancel,
-                        filters ? t->d_in_filt.get() : nullptr, query_filter,
-                        filters ? rows_per_filter.data() : nullptr));
+  SDB_TRY(submit_locked(c, t, t->d_in_q, nq, k, c->row_base, t->res.rows, t->res.dist, t->res.count, cancel, bits,
+                        rf.query_filter, rf.bits ? rows_per_filter.data() : nullptr));
   t->h_out_rows = out_rows;
   t->h_out_dist = out_dist;
   t->h_out_count = out_count;
@@ -1481,8 +1611,6 @@ sdb_status sdb_debug_screen_batch(sdb_corpus* c, const double* queries, uint32_t
                                          out_qu, out_q8, out_qbf16, out_a, out_b, out_rr, nullptr, 0, nullptr, -1);
 }
 
-static sdb_status check_filters(uint32_t nq, const uint32_t* filters, uint32_t n_filters, const uint32_t* query_filter);
-
 sdb_status sdb_debug_screen_batch_filtered(sdb_corpus* c, const double* queries, uint32_t nq, uint32_t k,
                                            sdb_screen screen, int streaming, uint32_t cand_cap, int score_all,
                                            float* out_qf, double* out_qmag, uint32_t* out_qu, int8_t* out_q8,
@@ -1535,7 +1663,8 @@ sdb_status sdb_debug_screen_batch_filtered(sdb_corpus* c, const double* queries,
     const size_t words = (size_t)n_filters * ((c->n + 31) / 32);
     SDB_CUDA(t->d_in_filt.reserve(words));
     SDB_CUDA(cudaMemcpyAsync(t->d_in_filt, filters, sizeof(uint32_t) * words, cudaMemcpyHostToDevice, st));
-    const std::vector<uint64_t> rows_per_filter = count_filter_rows_host(c, filters, n_filters, query_filter, nq);
+    const std::vector<uint64_t> rows_per_filter =
+        count_filter_rows_host(filters, (c->n + 31) / 32, 0, c->n, n_filters, query_filter, nq);
     std::vector<uint32_t> scr, dir;
     plan_filtered(c, *t, nq, k, t->d_in_filt, query_filter, rows_per_filter.data(), &scr, &dir);
     if (!score_all && !scr.empty() && !dir.empty()) {
@@ -1762,9 +1891,30 @@ sdb_status sdb_knn_bruteforce_filtered(sdb_corpus* c, const double* queries, uin
   std::lock_guard<std::mutex> g(c->mu);
   SDB_CUDA(cudaSetDevice(c->ctx->device));
   Ticket* t = nullptr;
-  SDB_TRY(submit_host_locked(c, queries, nq, k, out_rows, out_dist, out_count, cancel_flag, &t, filters, n_filters,
-                             query_filter));
+  SDB_TRY(submit_host_locked(c, queries, nq, k, out_rows, out_dist, out_count, cancel_flag, &t,
+                             RowFilters{filters, n_filters, query_filter, 0}));
   return wait_locked(c, t);
+}
+
+// device bitmaps, read in place: counted on the copy stream (stage_filters), then the batch
+static sdb_status submit_device_filtered_locked(sdb_corpus* c, const double* d_queries, uint32_t nq, uint32_t k,
+                                                const RowFilters& rf, uint64_t row_base, uint64_t* d_out_rows,
+                                                double* d_out_dist, uint32_t* d_out_count, Ticket** out_t) {
+  Ticket* t = free_ticket(c);
+  if (!t) {
+    set_error("too many batches in flight (%d): call sdb_knn_wait first", N_TICKETS);
+    return SDB_EOVERFLOW;
+  }
+  SDB_TRY(ticket_prepare(c, *t, nq ? nq : 1));
+  const uint32_t* bits = nullptr;
+  std::vector<uint64_t> rows_per_filter;
+  SDB_TRY(stage_filters(c, *t, rf, false, nq, &bits, &rows_per_filter));
+  SDB_CUDA(cudaEventRecord(t->ev_h2d, c->ctx->copy_stream));
+  t->wait_h2d = true;
+  SDB_TRY(submit_locked(c, t, d_queries, nq, k, row_base, d_out_rows, d_out_dist, d_out_count, nullptr, bits,
+                        rf.query_filter, rows_per_filter.data()));
+  *out_t = t;
+  return SDB_OK;
 }
 
 sdb_status sdb_knn_bruteforce_filtered_device(sdb_corpus* c, const double* d_queries, uint32_t nq, uint32_t k,
@@ -1776,28 +1926,25 @@ sdb_status sdb_knn_bruteforce_filtered_device(sdb_corpus* c, const double* d_que
   if (nq == 0) return SDB_OK;
   std::lock_guard<std::mutex> g(c->mu);
   SDB_CUDA(cudaSetDevice(c->ctx->device));
-  Ticket* t = free_ticket(c);
-  if (!t) {
-    set_error("too many batches in flight (%d): call sdb_knn_wait first", N_TICKETS);
-    return SDB_EOVERFLOW;
-  }
-  std::vector<uint64_t> rows_per_filter(n_filters, 0);
-  if (c->finalized && c->n) {  // a blocking call anyway: count the bitmaps' set bits on the device and read them back
-    const uint64_t words = (c->n + 31) / 32;
-    AsyncBuf<unsigned long long> d_cnt;
-    cudaStream_t st = c->ctx->stream;
-    SDB_CUDA(d_cnt.reserve(n_filters, st));
-    SDB_CUDA(cudaMemsetAsync(d_cnt, 0, sizeof(unsigned long long) * n_filters, st));
-    const uint32_t gx = (uint32_t)std::min<uint64_t>((words + 255) / 256, 64);
-    count_filter_rows_kernel<<<dim3(gx, n_filters), 256, 0, st>>>(d_filters, words, d_cnt);
-    count_launch(c->ctx);
-    SDB_CUDA(cudaGetLastError());
-    SDB_CUDA(cudaMemcpyAsync(rows_per_filter.data(), d_cnt, sizeof(uint64_t) * n_filters, cudaMemcpyDeviceToHost, st));
-    SDB_CUDA(cudaStreamSynchronize(st));
-  }
-  SDB_TRY(submit_locked(c, t, d_queries, nq, k, row_base, d_out_rows, d_out_dist, d_out_count, nullptr, d_filters,
-                        query_filter, rows_per_filter.data()));
+  Ticket* t = nullptr;
+  SDB_TRY(submit_device_filtered_locked(c, d_queries, nq, k, RowFilters{d_filters, n_filters, query_filter, 0},
+                                        row_base, d_out_rows, d_out_dist, d_out_count, &t));
   return wait_locked(c, t);
+}
+
+sdb_status sdb_knn_submit_filtered_device(sdb_corpus* c, const double* d_queries, uint32_t nq, uint32_t k,
+                                          const uint32_t* d_filters, uint32_t n_filters, const uint32_t* query_filter,
+                                          uint64_t row_base, uint64_t* d_out_rows, double* d_out_dist,
+                                          uint32_t* d_out_count, uint32_t* ticket) {
+  if (!c || !ticket || (nq && (!d_queries || !d_out_count || (k && (!d_out_rows || !d_out_dist))))) return SDB_EINVAL;
+  SDB_TRY(check_filters(nq, d_filters, n_filters, query_filter));
+  std::lock_guard<std::mutex> g(c->mu);
+  SDB_CUDA(cudaSetDevice(c->ctx->device));
+  Ticket* t = nullptr;
+  SDB_TRY(submit_device_filtered_locked(c, d_queries, nq, k, RowFilters{d_filters, n_filters, query_filter, 0},
+                                        row_base, d_out_rows, d_out_dist, d_out_count, &t));
+  *ticket = t->id;
+  return SDB_OK;
 }
 
 sdb_status sdb_knn_submit_filtered(sdb_corpus* c, const double* queries, uint32_t nq, uint32_t k,
@@ -1808,8 +1955,8 @@ sdb_status sdb_knn_submit_filtered(sdb_corpus* c, const double* queries, uint32_
   std::lock_guard<std::mutex> g(c->mu);
   SDB_CUDA(cudaSetDevice(c->ctx->device));
   Ticket* t = nullptr;
-  SDB_TRY(submit_host_locked(c, queries, nq, k, out_rows, out_dist, out_count, nullptr, &t, filters, n_filters,
-                             query_filter));
+  SDB_TRY(submit_host_locked(c, queries, nq, k, out_rows, out_dist, out_count, nullptr, &t,
+                             RowFilters{filters, n_filters, query_filter, 0}));
   *ticket = t->id;
   return SDB_OK;
 }

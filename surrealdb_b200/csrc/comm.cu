@@ -147,11 +147,11 @@ using namespace sdb;
 // the brute-force driver of api.cu
 namespace sdb {
 sdb_status knn_submit_for_shard(Corpus* c, const double* d_queries, const double* h_queries, uint32_t nq, uint32_t k,
-                                uint64_t* d_out_rows, double* d_out_dist, uint32_t* d_out_count, int* slot_index,
-                                uint32_t* ticket, const double** d_queries_used);
+                                const RowFilters& rf, uint64_t* d_out_rows, double* d_out_dist, uint32_t* d_out_count,
+                                int* slot_index, uint32_t* ticket, const double** d_queries_used);
 sdb_status knn_finish_for_shard(Corpus* c, uint32_t ticket, bool* repaired);
 sdb_status knn_release_ticket(Corpus* c, uint32_t ticket);
-const uint32_t* knn_ticket_stat_host(Corpus* c, uint32_t ticket, int* exact_only);
+sdb_status knn_shard_header(Corpus* c, uint32_t ticket, void* d_hdr);
 cudaStream_t knn_ticket_stream(Corpus* c, uint32_t ticket);
 void knn_trace_mark(Corpus* c, uint32_t ticket, const char* name);
 sdb_status topk_merge_launch(Ctx* ctx, uint32_t n_lists, uint32_t nq, uint32_t k, const uint64_t* d_rows,
@@ -483,10 +483,11 @@ static bool use_p2p(Corpus* c, ShardState* ss) {
   return c->ctx->comm && c->ctx->comm->nranks > 1 && ss->arena && ss->arena->ok && !exchange_forced_nccl();
 }
 
-// phase A: the local search into this rank's block, header = number of queries this rank must repair on the host
+// phase A: the local search into this rank's block, header = number of queries this rank must repair on the host.
+// rf: the call's global row filters (rf.bits == nullptr: unfiltered); the driver slices this shard's rows out of them.
 sdb_status phase_local(Corpus* c, const double* d_queries, const double* h_queries, uint32_t nq, uint32_t k,
-                       uint64_t* d_out_rows, double* d_out_dist, uint32_t* d_out_count, uint64_t* h_out_rows,
-                       double* h_out_dist, uint32_t* h_out_count, Pending* p) {
+                       const RowFilters& rf, uint64_t* d_out_rows, double* d_out_dist, uint32_t* d_out_count,
+                       uint64_t* h_out_rows, double* h_out_dist, uint32_t* h_out_count, Pending* p) {
   ShardState* ss = state_of(c);
   const BlockLayout bl = block_layout(nq, k);
   // the slot index follows the brute-force driver's ticket slot, so slot buffers are free exactly when the ticket is
@@ -510,18 +511,14 @@ sdb_status phase_local(Corpus* c, const double* d_queries, const double* h_queri
   const bool host_out = h_out_count != nullptr;
   SDB_TRY(slot_reserve(c, s, nq, k, host_out));
   int used = -1;
-  SDB_TRY(knn_submit_for_shard(c, d_queries, h_queries, nq, k, (uint64_t*)(s.d_block + bl.off_rows),
+  SDB_TRY(knn_submit_for_shard(c, d_queries, h_queries, nq, k, rf, (uint64_t*)(s.d_block + bl.off_rows),
                                (double*)(s.d_block + bl.off_dist), (uint32_t*)(s.d_block + bl.off_cnt), &used, &ticket,
                                &dq));
   if (used != slot) {
     set_error("internal: ticket slot mismatch (%d vs %d)", used, slot);
     return SDB_EINVAL;
   }
-  cudaStream_t st = knn_ticket_stream(c, ticket);
-  int exact_only = 0;
-  const uint32_t* h_stat = knn_ticket_stat_host(c, ticket, &exact_only);
-  if (exact_only) SDB_CUDA(cudaMemcpyAsync(s.d_block + bl.off_hdr, h_stat, 16, cudaMemcpyHostToDevice, st));
-  else SDB_CUDA(cudaMemcpyAsync(s.d_block + bl.off_hdr, c->d_stat, 16, cudaMemcpyDeviceToDevice, st));
+  SDB_TRY(knn_shard_header(c, ticket, s.d_block + bl.off_hdr));
   s.d_out_rows = host_out ? s.res.rows : d_out_rows;
   s.d_out_dist = host_out ? s.res.dist : d_out_dist;
   s.d_out_count = host_out ? s.res.count : d_out_count;
@@ -751,8 +748,8 @@ sdb_status sdb_corpus_set_row_base(sdb_corpus* c, uint64_t row_base) {
 }
 
 static sdb_status sharded_submit(sdb_corpus* c, const double* d_queries, const double* h_queries, uint32_t nq, uint32_t k,
-                                 uint64_t* d_out_rows, double* d_out_dist, uint32_t* d_out_count, uint64_t* h_out_rows,
-                                 double* h_out_dist, uint32_t* h_out_count, uint32_t* ticket) {
+                                 const RowFilters& rf, uint64_t* d_out_rows, double* d_out_dist, uint32_t* d_out_count,
+                                 uint64_t* h_out_rows, double* h_out_dist, uint32_t* h_out_count, uint32_t* ticket) {
   if (!c || !ticket || !nq) return SDB_EINVAL;
   if (c->ctx->comm && c->ctx->comm->nranks > 1) SDB_TRY(nccl_load());
   Pending p;
@@ -766,8 +763,8 @@ static sdb_status sharded_submit(sdb_corpus* c, const double* d_queries, const d
       }
       SDB_TRY(arena_ensure_ipc(c, state_of(c), block_layout(nq, k).bytes));
     }
-    SDB_TRY(phase_local(c, d_queries, h_queries, nq, k, d_out_rows, d_out_dist, d_out_count, h_out_rows, h_out_dist,
-                        h_out_count, &p));
+    SDB_TRY(phase_local(c, d_queries, h_queries, nq, k, rf, d_out_rows, d_out_dist, d_out_count, h_out_rows,
+                        h_out_dist, h_out_count, &p));
     sdb_status rc = phase_gather(p);
     if (rc == SDB_OK) rc = phase_merge(p);
     if (rc != SDB_OK) {
@@ -789,13 +786,34 @@ sdb_status sdb_knn_sharded_submit_device(sdb_corpus* c, const double* d_queries,
                                          uint64_t* d_out_rows, double* d_out_dist, uint32_t* d_out_count,
                                          uint32_t* ticket) {
   if (!d_queries || !d_out_count || (k && (!d_out_rows || !d_out_dist))) return SDB_EINVAL;
-  return sharded_submit(c, d_queries, nullptr, nq, k, d_out_rows, d_out_dist, d_out_count, nullptr, nullptr, nullptr, ticket);
+  return sharded_submit(c, d_queries, nullptr, nq, k, RowFilters(), d_out_rows, d_out_dist, d_out_count, nullptr, nullptr,
+                        nullptr, ticket);
 }
 
 sdb_status sdb_knn_sharded_submit(sdb_corpus* c, const double* queries, uint32_t nq, uint32_t k, uint64_t* out_rows,
                                   double* out_dist, uint32_t* out_count, uint32_t* ticket) {
   if (!queries || !out_count || (k && (!out_rows || !out_dist))) return SDB_EINVAL;
-  return sharded_submit(c, nullptr, queries, nq, k, nullptr, nullptr, nullptr, out_rows, out_dist, out_count, ticket);
+  return sharded_submit(c, nullptr, queries, nq, k, RowFilters(), nullptr, nullptr, nullptr, out_rows, out_dist, out_count,
+                        ticket);
+}
+
+sdb_status sdb_knn_sharded_submit_filtered(sdb_corpus* c, const double* queries, uint32_t nq, uint32_t k,
+                                           const uint32_t* filters, uint32_t n_filters, const uint32_t* query_filter,
+                                           uint64_t n_rows_total, uint64_t* out_rows, double* out_dist,
+                                           uint32_t* out_count, uint32_t* ticket) {
+  if (!filters || !queries || !out_count || (k && (!out_rows || !out_dist))) return SDB_EINVAL;
+  return sharded_submit(c, nullptr, queries, nq, k, RowFilters{filters, n_filters, query_filter, n_rows_total}, nullptr,
+                        nullptr, nullptr, out_rows, out_dist, out_count, ticket);
+}
+
+sdb_status sdb_knn_sharded_submit_filtered_device(sdb_corpus* c, const double* d_queries, uint32_t nq, uint32_t k,
+                                                  const uint32_t* d_filters, uint32_t n_filters,
+                                                  const uint32_t* query_filter, uint64_t n_rows_total,
+                                                  uint64_t* d_out_rows, double* d_out_dist, uint32_t* d_out_count,
+                                                  uint32_t* ticket) {
+  if (!d_filters || !d_queries || !d_out_count || (k && (!d_out_rows || !d_out_dist))) return SDB_EINVAL;
+  return sharded_submit(c, d_queries, nullptr, nq, k, RowFilters{d_filters, n_filters, query_filter, n_rows_total},
+                        d_out_rows, d_out_dist, d_out_count, nullptr, nullptr, nullptr, ticket);
 }
 
 sdb_status sdb_knn_sharded_wait(sdb_corpus* c, uint32_t ticket) {
@@ -817,8 +835,8 @@ sdb_status sdb_knn_sharded_wait(sdb_corpus* c, uint32_t ticket) {
   return finish_all(&p, 1);
 }
 
-sdb_status sdb_knn_sharded_multi(sdb_corpus* const* shards, int n, const double* queries, uint32_t nq, uint32_t k,
-                                 uint64_t* out_rows, double* out_dist, uint32_t* out_count) {
+static sdb_status sharded_multi(sdb_corpus* const* shards, int n, const double* queries, uint32_t nq, uint32_t k,
+                                const RowFilters& rf, uint64_t* out_rows, double* out_dist, uint32_t* out_count) {
   if (!shards || n < 1 || n > 64 || !queries || !nq || !out_count || (k && (!out_rows || !out_dist))) return SDB_EINVAL;
   if (n > 1) SDB_TRY(nccl_load());
   std::vector<Pending> ps((size_t)n);
@@ -835,10 +853,10 @@ sdb_status sdb_knn_sharded_multi(sdb_corpus* const* shards, int n, const double*
     cudaSetDevice(shards[i]->ctx->device);
     ShardState* ss = state_of(shards[i]);
     (void)ss;
-    if (i == 0) rc = phase_local(shards[i], nullptr, queries, nq, k, nullptr, nullptr, nullptr, out_rows, out_dist, out_count, &ps[i]);
+    if (i == 0) rc = phase_local(shards[i], nullptr, queries, nq, k, rf, nullptr, nullptr, nullptr, out_rows, out_dist, out_count, &ps[i]);
     else {
       // the other shards keep their merged copy on the device (slot staging buffers)
-      rc = phase_local(shards[i], nullptr, queries, nq, k, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, &ps[i]);
+      rc = phase_local(shards[i], nullptr, queries, nq, k, rf, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, &ps[i]);
       if (rc == SDB_OK) {
         ShardSlot& s = *ps[i].s;
         rc = slot_reserve(shards[i], s, nq, k, true);
@@ -869,6 +887,20 @@ sdb_status sdb_knn_sharded_multi(sdb_corpus* const* shards, int n, const double*
     knn_release_ticket(shards[i], ps[i].ticket);
   }
   return rc;
+}
+
+sdb_status sdb_knn_sharded_multi(sdb_corpus* const* shards, int n, const double* queries, uint32_t nq, uint32_t k,
+                                 uint64_t* out_rows, double* out_dist, uint32_t* out_count) {
+  return sharded_multi(shards, n, queries, nq, k, RowFilters(), out_rows, out_dist, out_count);
+}
+
+sdb_status sdb_knn_sharded_multi_filtered(sdb_corpus* const* shards, int n, const double* queries, uint32_t nq,
+                                          uint32_t k, const uint32_t* filters, uint32_t n_filters,
+                                          const uint32_t* query_filter, uint64_t n_rows_total, uint64_t* out_rows,
+                                          double* out_dist, uint32_t* out_count) {
+  if (!filters) return SDB_EINVAL;
+  return sharded_multi(shards, n, queries, nq, k, RowFilters{filters, n_filters, query_filter, n_rows_total}, out_rows,
+                       out_dist, out_count);
 }
 
 }  // extern "C"

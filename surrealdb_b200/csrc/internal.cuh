@@ -214,6 +214,16 @@ __device__ __forceinline__ bool filt_pass(const FiltArg& f, uint32_t q, uint32_t
   const uint32_t w = row >> 5;
   return w < f.words && ((__ldg(f.bits + (size_t)__ldg(f.qf + q) * f.words + w) >> (row & 31u)) & 1u) != 0;
 }
+// the row filters of one filtered call as the caller hands them over: n_filters bitmaps (host or device memory, where
+// the call's queries are), query_filter on the host (NULL: every query uses filter 0).  n_rows_total: the global rows
+// the bitmaps of a sharded call cover (ceil(n_rows_total / 32) words each, bit r = global row r); 0 for an unsharded
+// call, whose bitmaps cover the corpus' own rows.  bits == nullptr: an unfiltered call.
+struct RowFilters {
+  const uint32_t* bits = nullptr;
+  uint32_t n_filters = 0;
+  const uint32_t* query_filter = nullptr;
+  uint64_t n_rows_total = 0;
+};
 
 struct Comm;  // comm.cu: NCCL communicator attached to a context (nullptr = single shard)
 
@@ -292,6 +302,12 @@ struct Ticket {
   FiltArg filt;
   std::vector<uint32_t> h_qf;
   DevBuf<uint32_t> d_qf, d_in_filt;
+  // stage_filters: a sharded call's span of its host bitmaps (before the slice), and the set bits of device bitmaps
+  DevBuf<uint32_t> d_in_span;
+  DevBuf<unsigned long long> d_fcnt;
+  PinnedBuf<unsigned long long> h_fcnt;
+  // a permuted batch: the screened sub-batch's counters (d_stat), which the direct sub-batch's cand_begin resets
+  DevBuf<uint32_t> d_stat_scr;
   // direct regime: the last n_direct queries of the batch skip the screen.  A batch that mixes both kinds runs
   // permuted (screened queries first): d_queries / d_out_* / h_qf are then the permuted copies (d_pq, pres) and the
   // results are scattered through d_perm (permuted position -> caller's query) to d_fin_*, the caller's outputs

@@ -108,6 +108,7 @@ class VectorColumn:
 
     def __init__(self, ctx, dim, metric="COSINE", dtype="F32", capacity=1 << 20):
         self.ctx, self.dim, self.metric, self.dtype = ctx, int(dim), metric.upper(), dtype.upper()
+        self.row_base = 0  # global id of row 0 (set_row_base)
         self.h = C.c_void_p()
         L.check(L.lib().sdb_corpus_create(ctx.h, self.dim, L.DTYPE[self.dtype], L.METRIC[self.metric],
                                           int(capacity), C.byref(self.h)))
@@ -232,12 +233,26 @@ class VectorColumn:
                                                 C.c_void_p(h_out_count), C.byref(t)))
         return t.value
 
+    def submit_device_filtered(self, d_queries, nq, k, d_filters, n_filters, query_filter, row_base, d_out_rows,
+                               d_out_dist, d_out_count):
+        """asynchronous knn_device_filtered: device pointers (ints) valid until wait; query_filter is a host array (or
+        None), copied before the call returns"""
+        qf = _query_filter(query_filter, nq)
+        t = C.c_uint32()
+        L.check(L.lib().sdb_knn_submit_filtered_device(self.h, C.c_void_p(d_queries), int(nq), int(k),
+                                                       C.c_void_p(d_filters), int(n_filters),
+                                                       None if qf is None else _ptr(qf), int(row_base),
+                                                       C.c_void_p(d_out_rows), C.c_void_p(d_out_dist),
+                                                       C.c_void_p(d_out_count), C.byref(t)))
+        return t.value
+
     def wait(self, ticket):
         L.check(L.lib().sdb_knn_wait(self.h, int(ticket)))
 
     # ---- row-sharded search (collective over the context's communicator) ----
     def set_row_base(self, row_base):
         L.check(L.lib().sdb_corpus_set_row_base(self.h, int(row_base)))
+        self.row_base = int(row_base)
 
     def sharded_submit_device(self, d_queries, nq, k, d_out_rows, d_out_dist, d_out_count):
         t = C.c_uint32()
@@ -250,6 +265,31 @@ class VectorColumn:
         t = C.c_uint32()
         L.check(L.lib().sdb_knn_sharded_submit(self.h, C.c_void_p(h_queries), int(nq), int(k), C.c_void_p(h_out_rows),
                                                C.c_void_p(h_out_dist), C.c_void_p(h_out_count), C.byref(t)))
+        return t.value
+
+    def sharded_submit_filtered_host(self, h_queries, nq, k, h_filters, n_filters, query_filter, n_rows_total,
+                                     h_out_rows, h_out_dist, h_out_count):
+        """raw host pointers (ints) like sharded_submit_host, plus the host bitmaps over the GLOBAL rows: n_filters x
+        ceil(n_rows_total / 32) words, valid until sharded_wait; query_filter is a host array (or None)"""
+        qf = _query_filter(query_filter, nq)
+        t = C.c_uint32()
+        L.check(L.lib().sdb_knn_sharded_submit_filtered(self.h, C.c_void_p(h_queries), int(nq), int(k),
+                                                        C.c_void_p(h_filters), int(n_filters),
+                                                        None if qf is None else _ptr(qf), int(n_rows_total),
+                                                        C.c_void_p(h_out_rows), C.c_void_p(h_out_dist),
+                                                        C.c_void_p(h_out_count), C.byref(t)))
+        return t.value
+
+    def sharded_submit_filtered_device(self, d_queries, nq, k, d_filters, n_filters, query_filter, n_rows_total,
+                                       d_out_rows, d_out_dist, d_out_count):
+        """device pointers (ints) like sharded_submit_device, plus the device bitmaps over the GLOBAL rows"""
+        qf = _query_filter(query_filter, nq)
+        t = C.c_uint32()
+        L.check(L.lib().sdb_knn_sharded_submit_filtered_device(self.h, C.c_void_p(d_queries), int(nq), int(k),
+                                                               C.c_void_p(d_filters), int(n_filters),
+                                                               None if qf is None else _ptr(qf), int(n_rows_total),
+                                                               C.c_void_p(d_out_rows), C.c_void_p(d_out_dist),
+                                                               C.c_void_p(d_out_count), C.byref(t)))
         return t.value
 
     def sharded_wait(self, ticket):
@@ -303,13 +343,23 @@ def shard_block_layout(nq, k):
     return off_rows, off_dist, off_cnt, size
 
 
-def knn_sharded_multi(shards, queries, k):
-    """one process, N GPUs: shards[i] is the VectorColumn on the i-th context of Context.create_multi"""
+def knn_sharded_multi(shards, queries, k, filters=None, query_filter=None, n_rows_total=None):
+    """one process, N GPUs: shards[i] is the VectorColumn on the i-th context of Context.create_multi.
+    filters: optional uint32 bitmaps (n_filters, ceil(n_rows_total / 32)) over the GLOBAL rows (pack_row_filter of
+    global masks), as in VectorColumn.knn; n_rows_total defaults to the largest row_base + len over the shards."""
     q = np.ascontiguousarray(queries, np.float64)
     nq = q.shape[0]
     rows = np.zeros((nq, max(k, 1)), np.uint64)
     dist = np.zeros((nq, max(k, 1)), np.float64)
     cnt = np.zeros(nq, np.uint32)
     hs = (C.c_void_p * len(shards))(*[s.h for s in shards])
-    L.check(L.lib().sdb_knn_sharded_multi(hs, len(shards), _ptr(q), nq, int(k), _ptr(rows), _ptr(dist), _ptr(cnt)))
+    if filters is None:
+        L.check(L.lib().sdb_knn_sharded_multi(hs, len(shards), _ptr(q), nq, int(k), _ptr(rows), _ptr(dist), _ptr(cnt)))
+    else:
+        if n_rows_total is None:
+            n_rows_total = max(s.row_base + len(s) for s in shards)
+        f, qf = _filter_args(filters, query_filter, nq, int(n_rows_total))
+        L.check(L.lib().sdb_knn_sharded_multi_filtered(hs, len(shards), _ptr(q), nq, int(k), _ptr(f), f.shape[0],
+                                                       None if qf is None else _ptr(qf), int(n_rows_total),
+                                                       _ptr(rows), _ptr(dist), _ptr(cnt)))
     return rows[:, :k], dist[:, :k], cnt
