@@ -469,8 +469,48 @@ sdb_status sdb_hnsw_search_filtered_batch_device(sdb_hnsw*, const void* d_querie
                                                  const uint32_t* d_filters, uint32_t n_filters,
                                                  const uint32_t* query_filter, uint64_t* d_out_elems,
                                                  double* d_out_dist, uint32_t* d_out_count, uint64_t* d_out_counters);
-/* how many queries of the handle's last sdb_hnsw_search_filtered_batch[_device] call the spill tier finished */
+/* how many queries of the handle's last sdb_hnsw_search_filtered_batch[_device] call the spill tier finished; after
+ * sdb_hnsw_wait(t) on a filtered ticket, t's */
 uint32_t sdb_hnsw_last_spilled(const sdb_hnsw*);
+
+/* Asynchronous HNSW search: submit queues a whole batch without a host synchronisation and returns a ticket;
+ * sdb_hnsw_wait(ticket) completes it.  Up to 4 tickets per handle are in flight (a fifth submit: SDB_EOVERFLOW, and the
+ * handle keeps answering); they complete in any order, filtered and unfiltered mixed, and blocking searches on the
+ * handle may run between them.  After the wait returns SDB_OK a ticket's outputs are byte for byte those of the
+ * matching blocking call on the same handle (ids, f64 distances, counts, both counters):
+ *   sdb_hnsw_submit                      = sdb_hnsw_search (all_docs_pending NULL) or sdb_hnsw_search_pending,
+ *   sdb_hnsw_submit_device               = sdb_hnsw_search_device (d_out_counters nullable),
+ *   sdb_hnsw_submit_filtered[_device]    = sdb_hnsw_search_filtered_batch[_device].
+ * Submit refuses what the blocking call refuses before it walks (SDB_EINVAL, SDB_EUNSUPPORTED), and returns
+ * SDB_ECANCELLED, with no ticket, when the context's cancel flag is up.  The wait returns what the blocking call finds
+ * after its walk: SDB_EOVERFLOW (unfiltered visited table), the spill tier's SDB_ENOMEM / SDB_EUNSUPPORTED, and
+ * SDB_ECANCELLED when the flag went up while the ticket was in flight (outputs undefined; the spill tier does not run).
+ * The wait releases the ticket whatever it returns; an unknown or completed ticket is SDB_EINVAL.  nq, k or ef = 0 get
+ * a ticket whose wait leaves zero counts.  sdb_hnsw_last_spilled after the wait of a filtered ticket reports its spill.
+ * Buffers: query_filter (host) is checked and copied before submit returns; queries, filters, all_docs_pending and the
+ * outputs stay valid (d_filters also unchanged) until the wait returns.  Pinned host buffers overlap with the walk;
+ * pageable ones work, with host copies the driver makes synchronous.  The Minkowski order is the one at submit.
+ * While a ticket is in flight sdb_hnsw_set_layers_device returns SDB_EINVAL (the spill tier at the wait reads the
+ * layers the ticket was submitted against); sdb_hnsw_destroy waits for the tickets' work and frees their buffers.
+ * Submit holds the handle's lock only while it queues; the wait releases it while it waits for the device.  Tickets
+ * alternate the context's two streams, each with its own visited tables, so one batch's walk fills the SMs another's
+ * tail and spill tier leave idle. */
+sdb_status sdb_hnsw_submit(sdb_hnsw*, const void* queries, uint32_t nq, uint32_t k, uint32_t ef,
+                           const uint8_t* all_docs_pending /* nullable */, uint64_t* out_elems, double* out_dist,
+                           uint32_t* out_count, uint64_t* out_counters /* nullable */, uint32_t* ticket);
+sdb_status sdb_hnsw_submit_device(sdb_hnsw*, const void* d_queries, uint32_t nq, uint32_t k, uint32_t ef,
+                                  uint64_t* d_out_elems, double* d_out_dist, uint32_t* d_out_count,
+                                  uint64_t* d_out_counters /* nullable */, uint32_t* ticket);
+sdb_status sdb_hnsw_submit_filtered(sdb_hnsw*, const void* queries, uint32_t nq, uint32_t k, uint32_t ef,
+                                    const uint32_t* filters, uint32_t n_filters, const uint32_t* query_filter,
+                                    uint64_t* out_elems, double* out_dist, uint32_t* out_count,
+                                    uint64_t* out_counters, uint32_t* ticket);
+sdb_status sdb_hnsw_submit_filtered_device(sdb_hnsw*, const void* d_queries, uint32_t nq, uint32_t k, uint32_t ef,
+                                           const uint32_t* d_filters, uint32_t n_filters,
+                                           const uint32_t* query_filter /* host */, uint64_t* d_out_elems,
+                                           double* d_out_dist, uint32_t* d_out_count, uint64_t* d_out_counters,
+                                           uint32_t* ticket);
+sdb_status sdb_hnsw_wait(sdb_hnsw*, uint32_t ticket);
 
 /* Search while pending updates exist: Hnsw::knn_search(.., pending_docs = Some(bitmap)) (hnsw/mod.rs:459-482).
  * all_docs_pending[e] != 0 iff EVERY document of element e is in the pending bitmap that

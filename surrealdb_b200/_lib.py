@@ -40,6 +40,8 @@ ABI_SYMBOLS = [
     "sdb_knn_submit_filtered_device", "sdb_knn_sharded_submit_filtered", "sdb_knn_sharded_submit_filtered_device",
     "sdb_knn_sharded_multi_filtered",
     "sdb_hnsw_search_filtered_batch", "sdb_hnsw_search_filtered_batch_device", "sdb_hnsw_last_spilled",
+    "sdb_hnsw_submit", "sdb_hnsw_submit_device", "sdb_hnsw_submit_filtered", "sdb_hnsw_submit_filtered_device",
+    "sdb_hnsw_wait",
 ]
 
 
@@ -154,6 +156,11 @@ def lib():
     L.sdb_hnsw_search_filtered_batch_device.argtypes = [vp, vp, u32, u32, u32, vp, u32, vp, vp, vp, vp, vp]
     L.sdb_hnsw_last_spilled.argtypes = [vp]
     L.sdb_hnsw_last_spilled.restype = u32
+    L.sdb_hnsw_submit.argtypes = [vp, vp, u32, u32, u32, vp, vp, vp, vp, vp, C.POINTER(u32)]
+    L.sdb_hnsw_submit_device.argtypes = [vp, vp, u32, u32, u32, vp, vp, vp, vp, C.POINTER(u32)]
+    L.sdb_hnsw_submit_filtered.argtypes = [vp, vp, u32, u32, u32, vp, u32, vp, vp, vp, vp, vp, C.POINTER(u32)]
+    L.sdb_hnsw_submit_filtered_device.argtypes = [vp, vp, u32, u32, u32, vp, u32, vp, vp, vp, vp, vp, C.POINTER(u32)]
+    L.sdb_hnsw_wait.argtypes = [vp, u32]
     L.sdb_vec_distance_f32.argtypes = [vp, i32, u32, vp, vp, u64, vp]
     L.sdb_hnsw_distance.argtypes = [vp, vp, vp, u64, vp]
     L.sdb_hnsw_set_minkowski_order.argtypes = [vp, C.c_double]

@@ -39,32 +39,6 @@ struct VecState {
   Buf<uint32_t, K> nbits;   // ... and how many there are (vector.rs:316-356)
 };
 
-struct Hnsw {
-  Ctx* ctx = nullptr;
-  uint32_t dim = 0;
-  sdb_metric metric = SDB_EUCLIDEAN;
-  sdb_vector_type vt = SDB_VT_F32;  // element type of the vectors (and of the queries a search takes)
-  uint64_t n = 0;
-  uint32_t n_layers = 0;
-  int64_t entry = -1;
-  void* d_vec = nullptr;     // n x dim elements of type vt (own_vec's, or the caller's for a borrowed handle)
-  double minkowski_p = 3.0;  // order of SDB_MINKOWSKI (sdb_hnsw_set_minkowski_order)
-  VecState<Mem::Device> elems;  // the elements' metric state
-  std::vector<uint64_t*> rp;    // per layer CSR (own_rp / own_ci's, or the caller's for a borrowed handle)
-  std::vector<uint32_t*> ci;
-  DevBuf<char> own_vec;         // empty for a borrowed handle
-  std::vector<DevBuf<uint64_t>> own_rp;
-  std::vector<DevBuf<uint32_t>> own_ci;
-  DevBuf<const uint64_t*> d_rp;  // device tables of the rp / ci pointers
-  DevBuf<const uint32_t*> d_ci;
-  DevBuf<uint64_t> d_visited;
-  uint32_t table_log2 = 0, n_tables = 0;
-  uint32_t gen = 1;  // generations consumed so far (each warp uses gen_base + its own counter)
-  uint32_t last_spilled = 0;  // queries of the last batch-filtered call that the spill tier finished
-  bool borrowed = false;  // sdb_hnsw_load_device: vectors and CSR arrays belong to the caller
-  std::mutex mu;
-};
-
 constexpr int HN_WARPS = 4;
 
 // The queues' order (FloatKey, idx/trees/knn.rs:129-160): f64::total_cmp, so -0.0 sorts before 0.0.  Unlike the
@@ -1653,6 +1627,90 @@ __global__ void csr_present_fill_kernel(const uint64_t* __restrict__ rp, const u
   }
 }
 
+// The visited tables of the walks queued on one stream (one table per resident warp) and their generation counter.
+// Each of the context's two streams has its own set, so a re-size or a generation wrap is ordered after the walks
+// already queued on that set by the stream itself: the table is an AsyncBuf of that stream, freed there.
+struct VisitSet {
+  AsyncBuf<uint64_t> tab;
+  uint32_t table_log2 = 0, n_tables = 0;
+  uint32_t gen = 1;  // generations consumed so far (each warp uses gen_base + its own counter)
+};
+
+// One search between the two halves of the walk driver (hnsw_enqueue, hnsw_complete): an asynchronous ticket of
+// sdb_hnsw_submit* or a blocking call.  It owns everything the completion half still reads: the staged queries and
+// their metric state, the staged bitmaps or pending mask, the copied query_filter, the device outputs of the host
+// variants, the counters, the spill list and the spill tier's slots.
+struct HnswTicket {
+  bool busy = false;
+  bool waiting = false;  // a sdb_hnsw_wait has taken it
+  uint32_t id = 0;
+  cudaStream_t st = nullptr;
+  VisitSet* vis = nullptr;  // the visited-table set of st
+  HnswParams P{};
+  bool walked = false;      // the walk was launched (false: an empty batch)
+  bool batch_filter = false;
+  bool device_io = false;
+  uint32_t nq = 0, k = 0;
+  uint64_t* out_elems = nullptr;  // the caller's outputs
+  double* out_dist = nullptr;
+  uint32_t* out_count = nullptr;
+  uint64_t* out_counters = nullptr;
+  uint32_t* h_word = nullptr;  // pinned, 2 words: [0] the spill count, [1] the overflow flag, copied after the walk
+  cudaEvent_t ev = nullptr;    // the last work of the search queued so far
+  AsyncBuf<char> q_buf;
+  AsyncBuf<uint64_t> elems_buf, d_ctr;
+  AsyncBuf<double> dist_buf;
+  AsyncBuf<uint32_t> cnt_buf, d_ovf;
+  AsyncBuf<uint8_t> d_noexp, d_truthy;
+  AsyncBuf<uint32_t> d_filters, d_qf, d_spill;
+  VecState<Mem::Async> qs;
+  std::vector<uint32_t> h_qf;  // the caller's query_filter, copied at submit
+  DevBuf<ulonglong2> spill_heap;
+  DevBuf<uint32_t> spill_stamp;
+  AsyncBuf<uint32_t> spill_next;
+  // frees the per-search buffers (the AsyncBufs on the stream, after the search's own work) and frees the slot
+  void release() {
+    q_buf.reset(), elems_buf.reset(), d_ctr.reset(), dist_buf.reset(), cnt_buf.reset(), d_ovf.reset();
+    d_noexp.reset(), d_truthy.reset(), d_filters.reset(), d_qf.reset(), d_spill.reset();
+    qs = VecState<Mem::Async>();
+    h_qf = std::vector<uint32_t>();
+    spill_heap.reset(), spill_stamp.reset(), spill_next.reset();
+    busy = waiting = walked = false;
+  }
+  ~HnswTicket() {
+    if (ev) cudaEventDestroy(ev);
+  }
+};
+
+struct Hnsw {
+  Ctx* ctx = nullptr;
+  uint32_t dim = 0;
+  sdb_metric metric = SDB_EUCLIDEAN;
+  sdb_vector_type vt = SDB_VT_F32;  // element type of the vectors (and of the queries a search takes)
+  uint64_t n = 0;
+  uint32_t n_layers = 0;
+  int64_t entry = -1;
+  void* d_vec = nullptr;     // n x dim elements of type vt (own_vec's, or the caller's for a borrowed handle)
+  double minkowski_p = 3.0;  // order of SDB_MINKOWSKI (sdb_hnsw_set_minkowski_order)
+  VecState<Mem::Device> elems;  // the elements' metric state
+  std::vector<uint64_t*> rp;    // per layer CSR (own_rp / own_ci's, or the caller's for a borrowed handle)
+  std::vector<uint32_t*> ci;
+  DevBuf<char> own_vec;         // empty for a borrowed handle
+  std::vector<DevBuf<uint64_t>> own_rp;
+  std::vector<DevBuf<uint32_t>> own_ci;
+  DevBuf<const uint64_t*> d_rp;  // device tables of the rp / ci pointers
+  DevBuf<const uint32_t*> d_ci;
+  VisitSet vis[2];             // the walks of the context's stream / stream2
+  uint32_t last_spilled = 0;  // queries of the last batch-filtered call (or waited ticket) that the spill tier finished
+  // slots 0 .. N_TICKETS - 1: the asynchronous tickets (even slots on the context's stream, odd ones on stream2);
+  // slot N_TICKETS: the blocking calls, which hold `mu` from their enqueue to their completion
+  HnswTicket slots[N_TICKETS + 1];
+  PinnedBuf<uint32_t> h_words;  // 2 words per slot (HnswTicket::h_word), allocated with the first search
+  uint32_t next_ticket = 1;
+  bool borrowed = false;  // sdb_hnsw_load_device: vectors and CSR arrays belong to the caller
+  std::mutex mu;
+};
+
 }  // namespace sdb
 
 struct sdb_hnsw : sdb::Hnsw {};
@@ -1851,6 +1909,8 @@ extern "C" {
 void sdb_hnsw_destroy(sdb_hnsw* h) {
   if (!h) return;
   cudaSetDevice(h->ctx->device);
+  for (const HnswTicket& t : h->slots)  // tickets never waited for: their work ends before their buffers go
+    if (t.busy) cudaEventSynchronize(t.ev);
   delete h;
 }
 
@@ -1935,7 +1995,12 @@ sdb_status sdb_hnsw_set_layers_device(sdb_hnsw* h, uint32_t n_layers, const uint
               "swap its adjacency)");
     return SDB_EINVAL;
   }
-  std::lock_guard<std::mutex> guard(h->mu);  // searches hold it for their whole run
+  std::lock_guard<std::mutex> guard(h->mu);  // blocking searches hold it for their whole run
+  for (const HnswTicket& t : h->slots)  // a ticket's spill tier reads the layers it was submitted against
+    if (t.busy) {
+      set_error("sdb_hnsw_set_layers_device: tickets in flight (call sdb_hnsw_wait first)");
+      return SDB_EINVAL;
+    }
   SDB_CUDA(cudaSetDevice(h->ctx->device));
   h->rp.clear();
   h->ci.clear();
@@ -2232,11 +2297,10 @@ struct BatchFilter {
 };
 
 // The spill tier of a batch-filtered call: n_sp queries of P.spill_list walked by hnsw_spill_kernel, in as many slots
-// as free device memory holds (at most one per resident warp, at most one per query).  Queued on the context's stream.
+// as free device memory holds (at most one per resident warp, at most one per query).  Queued on st, the walk's stream.
 static sdb_status hnsw_spill(sdb_hnsw* h, const HnswParams& P, uint32_t n_sp, DevBuf<ulonglong2>& heap,
-                             DevBuf<uint32_t>& stamp, AsyncBuf<uint32_t>& next) {
+                             DevBuf<uint32_t>& stamp, AsyncBuf<uint32_t>& next, cudaStream_t st) {
   Ctx* ctx = h->ctx;
-  cudaStream_t st = ctx->stream;
   const size_t per_warp = (hn_stage_bytes(h->dim, h->metric, h->vt) + 12 * ((size_t)P.ef + 2) + 64 + 15) & ~size_t(15);
   const size_t smem = per_warp * HN_WARPS;
   if (smem > 220 * 1024) {
@@ -2284,10 +2348,16 @@ static sdb_status hnsw_spill(sdb_hnsw* h, const HnswParams& P, uint32_t n_sp, De
   });
 }
 
-static sdb_status hnsw_search_impl(sdb_hnsw* h, const void* queries, uint32_t nq, uint32_t k, uint32_t ef,
-                                   const uint8_t* truthy, const uint8_t* noexp, uint64_t* out_elems, double* out_dist,
-                                   uint32_t* out_count, uint64_t* out_counters, bool device_io = false,
-                                   const BatchFilter* bf = nullptr) {
+// ---- the walk driver, in two halves.  hnsw_enqueue sizes and stages everything, launches the walk and queues the
+// copies of its results, of the spill count and of the overflow flag, then records the search's event; hnsw_complete
+// waits for that event, runs the spill tier when queries spilled (and copies the results again), and maps the flags to a
+// status.  A blocking call runs both back to back in the handle's blocking slot, holding h->mu throughout; a ticket runs
+// the first in sdb_hnsw_submit* and the second in sdb_hnsw_wait, which releases h->mu whenever it waits for the device.
+
+// the argument checks of every search, before anything is queued
+static sdb_status hnsw_check(const sdb_hnsw* h, const void* queries, uint32_t nq, uint32_t k, uint32_t ef,
+                             const uint64_t* out_elems, const double* out_dist, const uint32_t* out_count,
+                             const BatchFilter* bf) {
   if (!h || (nq && (!queries || !out_count)) || (nq && k && (!out_elems || !out_dist))) return SDB_EINVAL;
   if (bf && nq) {
     if (bf->n_filters == 0 || !bf->filters) {
@@ -2301,25 +2371,49 @@ static sdb_status hnsw_search_impl(sdb_hnsw* h, const void* queries, uint32_t nq
           return SDB_EINVAL;
         }
   }
-  if (nq == 0) return SDB_OK;
-  if (k == 0 || ef == 0) {  // to_vec_limit(0) underflows in the reference; we return nothing
-    if (device_io) {
-      SDB_CUDA(cudaSetDevice(h->ctx->device));
-      SDB_CUDA(cudaMemsetAsync(out_count, 0, sizeof(uint32_t) * nq, h->ctx->stream));
-      SDB_CUDA(cudaStreamSynchronize(h->ctx->stream));
-    } else {
-      memset(out_count, 0, sizeof(uint32_t) * nq);
-    }
-    return SDB_OK;
-  }
-  if (ef > 4096) {
+  if (nq && k && ef > 4096) {  // (k == 0 or ef == 0: an empty answer for any ef)
     set_error("hnsw: ef %u > 4096 unsupported", ef);
     return SDB_EUNSUPPORTED;
   }
+  return SDB_OK;
+}
+
+// the result copies of a search: the outputs of a host variant, and the counters
+static sdb_status copy_results(HnswTicket& t) {
+  const size_t nk = (size_t)t.nq * t.k;
+  if (!t.device_io) {
+    SDB_CUDA(cudaMemcpyAsync(t.out_elems, t.P.out_elems, sizeof(uint64_t) * nk, cudaMemcpyDeviceToHost, t.st));
+    SDB_CUDA(cudaMemcpyAsync(t.out_dist, t.P.out_dist, sizeof(double) * nk, cudaMemcpyDeviceToHost, t.st));
+    SDB_CUDA(cudaMemcpyAsync(t.out_count, t.P.out_count, sizeof(uint32_t) * t.nq, cudaMemcpyDeviceToHost, t.st));
+  }
+  if (t.out_counters)
+    SDB_CUDA(cudaMemcpyAsync(t.out_counters, t.P.out_counters, sizeof(uint64_t) * 2 * t.nq,
+                             t.device_io ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost, t.st));
+  return SDB_OK;
+}
+
+// The first half: everything up to the walk and its result copies, queued on t.st (the caller has set t.st and t.vis,
+// holds h->mu and has checked the arguments with hnsw_check).
+static sdb_status hnsw_enqueue(sdb_hnsw* h, HnswTicket& t, const void* queries, uint32_t nq, uint32_t k, uint32_t ef,
+                               const uint8_t* truthy, const uint8_t* noexp, uint64_t* out_elems, double* out_dist,
+                               uint32_t* out_count, uint64_t* out_counters, bool device_io, const BatchFilter* bf) {
   Ctx* ctx = h->ctx;
-  std::lock_guard<std::mutex> guard(h->mu);
-  SDB_CUDA(cudaSetDevice(ctx->device));
-  cudaStream_t st = ctx->stream;
+  cudaStream_t st = t.st;
+  t.nq = nq, t.k = k;
+  t.device_io = device_io;
+  t.batch_filter = bf != nullptr;
+  t.out_elems = out_elems, t.out_dist = out_dist, t.out_count = out_count, t.out_counters = out_counters;
+  t.walked = false;
+  if (!t.ev) SDB_CUDA(cudaEventCreateWithFlags(&t.ev, cudaEventDisableTiming));
+  if (!h->h_words) SDB_CUDA(h->h_words.reserve(2 * (N_TICKETS + 1)));
+  t.h_word = h->h_words.get() + 2 * (&t - h->slots);
+  t.h_word[0] = t.h_word[1] = 0;
+  if (nq == 0 || k == 0 || ef == 0) {  // to_vec_limit(0) underflows in the reference; we return nothing
+    if (nq && device_io) SDB_CUDA(cudaMemsetAsync(out_count, 0, sizeof(uint32_t) * nq, st));
+    else if (nq) memset(out_count, 0, sizeof(uint32_t) * nq);
+    SDB_CUDA(cudaEventRecord(t.ev, st));
+    return SDB_OK;
+  }
   // unfiltered: live candidates are a subset of w plus ties, 2*ef+34 is ample.  Filtered: every admitted element is a
   // candidate but only truthy ones enter w, so the window is sized for a selectivity down to ~1/16 (more = EOVERFLOW,
   // or the spill tier for the batch-filtered calls)
@@ -2361,53 +2455,45 @@ static sdb_status hnsw_search_impl(sdb_hnsw* h, const void* queries, uint32_t nq
   while ((1u << tl) < ef * 64u * 4u && tl < 20) tl++;
   if (filtered) tl = tl + 3 > 18 ? (tl > 18 ? tl : 18) : tl + 3;  // filtered walks visit ~1/selectivity more elements
   const uint32_t n_tables = grid * HN_WARPS;
-  if (!h->d_visited || h->table_log2 != tl || h->n_tables < n_tables) {
-    h->d_visited.reset();
-    SDB_CUDA(h->d_visited.reserve((size_t)n_tables << tl));
-    SDB_CUDA(cudaMemsetAsync(h->d_visited, 0, sizeof(uint64_t) * ((size_t)n_tables << tl), st));
-    h->table_log2 = tl;
-    h->n_tables = n_tables;
-    h->gen = 1;
+  VisitSet& vs = *t.vis;
+  if (!vs.tab || vs.table_log2 != tl || vs.n_tables < n_tables) {
+    vs.tab.reset();  // a free on st: after the walks already queued on this set
+    SDB_CUDA(vs.tab.reserve((size_t)n_tables << tl, st));
+    SDB_CUDA(cudaMemsetAsync(vs.tab, 0, sizeof(uint64_t) * ((size_t)n_tables << tl), st));
+    vs.table_log2 = tl;
+    vs.n_tables = n_tables;
+    vs.gen = 1;
   }
   const uint32_t q_per_warp = (nq + n_tables - 1) / n_tables;
   const uint32_t gens_per_warp = q_per_warp * h->n_layers + 1;
-  if ((uint64_t)h->gen + (uint64_t)gens_per_warp * n_tables >= 0xFFFFFFF0ull) {  // generation counter wrap
-    SDB_CUDA(cudaMemsetAsync(h->d_visited, 0, sizeof(uint64_t) * ((size_t)h->n_tables << tl), st));
-    h->gen = 1;
+  if ((uint64_t)vs.gen + (uint64_t)gens_per_warp * n_tables >= 0xFFFFFFF0ull) {  // generation counter wrap
+    SDB_CUDA(cudaMemsetAsync(vs.tab, 0, sizeof(uint64_t) * ((size_t)vs.n_tables << tl), st));
+    vs.gen = 1;
   }
   const size_t esz = vt_size(h->vt);
   // device_io: queries and outputs already live on the device (index construction), no staging
-  AsyncBuf<char> q_buf;
-  AsyncBuf<uint64_t> elems_buf, d_ctr;
-  AsyncBuf<double> dist_buf;
-  AsyncBuf<uint32_t> cnt_buf, d_ovf;
-  AsyncBuf<uint8_t> d_noexp, d_truthy;
-  AsyncBuf<uint32_t> d_filters, d_qf, d_spill;
-  DevBuf<ulonglong2> spill_heap;
-  DevBuf<uint32_t> spill_stamp;
-  AsyncBuf<uint32_t> spill_next;
   void* d_q = const_cast<void*>(queries);
   uint64_t* d_elems = out_elems;
   double* d_dist = out_dist;
   uint32_t* d_cnt = out_count;
   if (!device_io) {
-    SDB_CUDA(q_buf.reserve(esz * (size_t)nq * h->dim, st));
-    SDB_CUDA(elems_buf.reserve((size_t)nq * k, st));
-    SDB_CUDA(dist_buf.reserve((size_t)nq * k, st));
-    SDB_CUDA(cnt_buf.reserve(nq, st));
-    d_q = q_buf, d_elems = elems_buf, d_dist = dist_buf, d_cnt = cnt_buf;
+    SDB_CUDA(t.q_buf.reserve(esz * (size_t)nq * h->dim, st));
+    SDB_CUDA(t.elems_buf.reserve((size_t)nq * k, st));
+    SDB_CUDA(t.dist_buf.reserve((size_t)nq * k, st));
+    SDB_CUDA(t.cnt_buf.reserve(nq, st));
+    d_q = t.q_buf, d_elems = t.elems_buf, d_dist = t.dist_buf, d_cnt = t.cnt_buf;
     SDB_CUDA(cudaMemcpyAsync(d_q, queries, esz * (size_t)nq * h->dim, cudaMemcpyHostToDevice, st));
   }
-  SDB_CUDA(d_ctr.reserve(2 * (size_t)nq, st));
-  SDB_CUDA(d_ovf.reserve(1, st));
-  SDB_CUDA(cudaMemsetAsync(d_ovf, 0, 4, st));
+  SDB_CUDA(t.d_ctr.reserve(2 * (size_t)nq, st));
+  SDB_CUDA(t.d_ovf.reserve(1, st));
+  SDB_CUDA(cudaMemsetAsync(t.d_ovf, 0, 4, st));
   if (noexp) {
-    SDB_CUDA(d_noexp.reserve(h->n ? h->n : 1, st));
-    SDB_CUDA(cudaMemcpyAsync(d_noexp, noexp, h->n, cudaMemcpyHostToDevice, st));
+    SDB_CUDA(t.d_noexp.reserve(h->n ? h->n : 1, st));
+    SDB_CUDA(cudaMemcpyAsync(t.d_noexp, noexp, h->n, cudaMemcpyHostToDevice, st));
   }
   if (truthy) {
-    SDB_CUDA(d_truthy.reserve(h->n ? h->n : 1, st));
-    SDB_CUDA(cudaMemcpyAsync(d_truthy, truthy, h->n, cudaMemcpyHostToDevice, st));
+    SDB_CUDA(t.d_truthy.reserve(h->n ? h->n : 1, st));
+    SDB_CUDA(cudaMemcpyAsync(t.d_truthy, truthy, h->n, cudaMemcpyHostToDevice, st));
   }
   const uint32_t fwords = (uint32_t)((h->n + 31) / 32);
   const uint32_t* filters = nullptr;
@@ -2415,27 +2501,29 @@ static sdb_status hnsw_search_impl(sdb_hnsw* h, const void* queries, uint32_t nq
     filters = bf->filters;
     if (!bf->on_device) {
       const size_t words = (size_t)fwords * bf->n_filters;
-      SDB_CUDA(d_filters.reserve(words ? words : 1, st));
-      SDB_CUDA(cudaMemcpyAsync(d_filters, bf->filters, sizeof(uint32_t) * words, cudaMemcpyHostToDevice, st));
-      filters = d_filters;
+      SDB_CUDA(t.d_filters.reserve(words ? words : 1, st));
+      SDB_CUDA(cudaMemcpyAsync(t.d_filters, bf->filters, sizeof(uint32_t) * words, cudaMemcpyHostToDevice, st));
+      filters = t.d_filters;
     }
-    if (bf->query_filter) {  // copied before the call returns (the synchronisation below)
-      SDB_CUDA(d_qf.reserve(nq, st));
-      SDB_CUDA(cudaMemcpyAsync(d_qf, bf->query_filter, sizeof(uint32_t) * nq, cudaMemcpyHostToDevice, st));
+    if (bf->query_filter) {  // copied first: the caller may reuse its array as soon as the call returns
+      t.h_qf.assign(bf->query_filter, bf->query_filter + nq);
+      SDB_CUDA(t.d_qf.reserve(nq, st));
+      SDB_CUDA(cudaMemcpyAsync(t.d_qf, t.h_qf.data(), sizeof(uint32_t) * nq, cudaMemcpyHostToDevice, st));
     }
     h->last_spilled = 0;
-    SDB_CUDA(d_spill.reserve((size_t)nq + 1, st));  // the spill list, then its length
-    SDB_CUDA(cudaMemsetAsync(d_spill.get() + nq, 0, sizeof(uint32_t), st));
+    SDB_CUDA(t.d_spill.reserve((size_t)nq + 1, st));  // the spill list, then its length
+    SDB_CUDA(cudaMemsetAsync(t.d_spill.get() + nq, 0, sizeof(uint32_t), st));
   }
-  HnswParams P;
+  HnswParams& P = t.P;
+  P = HnswParams{};
   P.filters = filters;
-  P.query_filter = d_qf;
+  P.query_filter = t.d_qf;
   P.fwords = fwords;
-  P.spill_list = d_spill;
-  P.n_spill = bf ? d_spill.get() + nq : nullptr;
+  P.spill_list = t.d_spill;
+  P.n_spill = bf ? t.d_spill.get() + nq : nullptr;
   P.ccap = ccap;
-  P.truthy = d_truthy;
-  P.noexp = d_noexp;
+  P.truthy = t.d_truthy;
+  P.noexp = t.d_noexp;
   P.vec = h->d_vec;
   P.norm = h->elems.norm;
   P.rp = h->d_rp;
@@ -2447,65 +2535,135 @@ static sdb_status hnsw_search_impl(sdb_hnsw* h, const void* queries, uint32_t nq
   P.nq = nq;
   P.k = k;
   P.ef = ef;
-  P.visited = h->d_visited;
+  P.visited = vs.tab;
   P.table_log2 = tl;
-  P.gen_base = h->gen;
+  P.gen_base = vs.gen;
   P.gens_per_warp = gens_per_warp;
   P.cancel = ctx->d_cancel;
   P.out_elems = d_elems;
   P.out_dist = d_dist;
   P.out_count = d_cnt;
-  P.out_counters = d_ctr;
-  P.overflow = d_ovf;
-  P.mink_p = h->minkowski_p;
+  P.out_counters = t.d_ctr;
+  P.overflow = t.d_ovf;
+  P.mink_p = h->minkowski_p;  // the spill tier at completion keeps the order of the submit
   P.e_mean = h->elems.mean;
   P.e_sx2 = h->elems.sx2;
   P.e_bits = h->elems.bits;
   P.e_nbits = h->elems.nbits;
-  VecState<Mem::Async> qs;
-  const sdb_status qrc = vec_state_make(ctx, h->metric, h->vt, d_q, nq, h->dim, qs, st);
-  P.q_mean = qs.mean;
-  P.q_sx2 = qs.sx2;
-  P.q_bits = qs.bits;
-  P.q_nbits = qs.nbits;
-  P.q_norm = qs.norm;
-  if (qrc == SDB_OK) {
-    kern<<<grid, HN_WARPS * 32, smem, st>>>(P);
-    count_launch(ctx);
-  }
-  h->gen += gens_per_warp * n_tables;
-  if (bf && qrc == SDB_OK) {  // the queries the on-chip walk gave up on go to the spill tier
-    uint32_t n_sp = 0;
-    SDB_CUDA(cudaMemcpyAsync(&n_sp, P.n_spill, sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
-    SDB_CUDA(cudaStreamSynchronize(st));
-    SDB_CUDA(cudaGetLastError());
-    h->last_spilled = n_sp;
-    if (n_sp && !ctx_cancelled(ctx)) SDB_TRY(hnsw_spill(h, P, n_sp, spill_heap, spill_stamp, spill_next));
-  }
-  uint32_t ovf = 0;
-  if (!device_io) {
-    SDB_CUDA(cudaMemcpyAsync(out_elems, d_elems, sizeof(uint64_t) * (size_t)nq * k, cudaMemcpyDeviceToHost, st));
-    SDB_CUDA(cudaMemcpyAsync(out_dist, d_dist, sizeof(double) * (size_t)nq * k, cudaMemcpyDeviceToHost, st));
-    SDB_CUDA(cudaMemcpyAsync(out_count, d_cnt, sizeof(uint32_t) * nq, cudaMemcpyDeviceToHost, st));
-  }
-  if (out_counters)
-    SDB_CUDA(cudaMemcpyAsync(out_counters, d_ctr, sizeof(uint64_t) * 2 * nq, device_io ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost, st));
-  SDB_CUDA(cudaMemcpyAsync(&ovf, d_ovf, 4, cudaMemcpyDeviceToHost, st));
-  SDB_CUDA(cudaStreamSynchronize(st));
+  SDB_TRY(vec_state_make(ctx, h->metric, h->vt, d_q, nq, h->dim, t.qs, st));
+  P.q_mean = t.qs.mean;
+  P.q_sx2 = t.qs.sx2;
+  P.q_bits = t.qs.bits;
+  P.q_nbits = t.qs.nbits;
+  P.q_norm = t.qs.norm;
+  kern<<<grid, HN_WARPS * 32, smem, st>>>(P);
+  count_launch(ctx);
   SDB_CUDA(cudaGetLastError());
-  if (qrc != SDB_OK) return qrc;
+  t.walked = true;
+  vs.gen += gens_per_warp * n_tables;
+  if (bf) SDB_CUDA(cudaMemcpyAsync(&t.h_word[0], P.n_spill, sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
+  SDB_TRY(copy_results(t));
+  SDB_CUDA(cudaMemcpyAsync(&t.h_word[1], t.d_ovf, sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
+  SDB_CUDA(cudaEventRecord(t.ev, st));
+  return SDB_OK;
+}
+
+// The second half: waits for the search's event, runs the spill tier for the queries the walk gave up on, maps the
+// flags to a status.  lk: a ticket's hold of h->mu, released while this waits for the device (the spill tier can take
+// seconds at 0 % selectivity and must not stall the handle's other submits); null for a blocking call.
+static sdb_status hnsw_complete(sdb_hnsw* h, HnswTicket& t, std::unique_lock<std::mutex>* lk) {
+  Ctx* ctx = h->ctx;
+  auto wait_event = [&](bool drop_spill) {
+    if (lk) lk->unlock();
+    const cudaError_t e = cudaEventSynchronize(t.ev);
+    if (drop_spill) t.spill_heap.reset(), t.spill_stamp.reset();  // cudaFree may wait for the device: not under h->mu
+    if (lk) lk->lock();
+    return e;
+  };
+  SDB_CUDA(wait_event(false));
+  if (!t.walked) return SDB_OK;
+  if (t.batch_filter) {  // the queries the on-chip walk gave up on go to the spill tier
+    const uint32_t n_sp = t.h_word[0];
+    h->last_spilled = n_sp;
+    if (n_sp && !ctx_cancelled(ctx)) {
+      SDB_TRY(hnsw_spill(h, t.P, n_sp, t.spill_heap, t.spill_stamp, t.spill_next, t.st));
+      SDB_TRY(copy_results(t));  // the copies queued with the walk predate the spilled queries' results
+      SDB_CUDA(cudaEventRecord(t.ev, t.st));
+      SDB_CUDA(wait_event(true));
+    }
+  }
+  SDB_CUDA(cudaGetLastError());
   if (ctx_cancelled(ctx)) {  // warps stop taking new queries once the flag is up: the outputs are incomplete
     set_error("query cancelled");
     return SDB_ECANCELLED;
   }
+  const uint32_t ovf = t.h_word[1];
   if (ovf == 1) {
     set_error("hnsw: visited table overflow (ef too large, or filter too selective, for the per-query table)");
     return SDB_EOVERFLOW;
   }
   if (ovf == 2) {
-    set_error("hnsw: candidate window overflow (filter too selective for ef %u): use the CPU path for this query", ef);
+    set_error("hnsw: candidate window overflow (filter too selective for ef %u): use the CPU path for this query", t.P.ef);
     return SDB_EOVERFLOW;
   }
+  return SDB_OK;
+}
+
+// a blocking search: both halves in the blocking slot, on the context's stream, under h->mu throughout
+static sdb_status hnsw_search_impl(sdb_hnsw* h, const void* queries, uint32_t nq, uint32_t k, uint32_t ef,
+                                   const uint8_t* truthy, const uint8_t* noexp, uint64_t* out_elems, double* out_dist,
+                                   uint32_t* out_count, uint64_t* out_counters, bool device_io = false,
+                                   const BatchFilter* bf = nullptr) {
+  SDB_TRY(hnsw_check(h, queries, nq, k, ef, out_elems, out_dist, out_count, bf));
+  if (nq == 0) return SDB_OK;
+  std::lock_guard<std::mutex> guard(h->mu);
+  SDB_CUDA(cudaSetDevice(h->ctx->device));
+  HnswTicket& t = h->slots[N_TICKETS];
+  t.st = h->ctx->stream;
+  t.vis = &h->vis[0];
+  sdb_status rc = hnsw_enqueue(h, t, queries, nq, k, ef, truthy, noexp, out_elems, out_dist, out_count, out_counters,
+                               device_io, bf);
+  if (rc == SDB_OK) rc = hnsw_complete(h, t, nullptr);
+  else cudaStreamSynchronize(t.st);  // what the failed call queued no longer reads the caller's buffers
+  t.release();
+  return rc;
+}
+
+// an asynchronous search: the first half in a free ticket slot (even slots on the context's stream, odd ones on stream2,
+// each stream with its own visited tables), completed by sdb_hnsw_wait
+static sdb_status hnsw_submit_impl(sdb_hnsw* h, const void* queries, uint32_t nq, uint32_t k, uint32_t ef,
+                                   const uint8_t* noexp, uint64_t* out_elems, double* out_dist, uint32_t* out_count,
+                                   uint64_t* out_counters, bool device_io, const BatchFilter* bf, uint32_t* ticket) {
+  if (!ticket) return SDB_EINVAL;
+  SDB_TRY(hnsw_check(h, queries, nq, k, ef, out_elems, out_dist, out_count, bf));
+  Ctx* ctx = h->ctx;
+  if (ctx_cancelled(ctx)) {
+    set_error("query cancelled");
+    return SDB_ECANCELLED;
+  }
+  std::lock_guard<std::mutex> guard(h->mu);
+  SDB_CUDA(cudaSetDevice(ctx->device));
+  HnswTicket* t = nullptr;
+  for (int i = 0; i < N_TICKETS && !t; i++)
+    if (!h->slots[i].busy) t = &h->slots[i];
+  if (!t) {
+    set_error("too many batches in flight (%d): call the matching wait first", N_TICKETS);
+    return SDB_EOVERFLOW;
+  }
+  const int slot = (int)(t - h->slots);
+  t->st = slot & 1 ? ctx->stream2 : ctx->stream;
+  t->vis = &h->vis[slot & 1];
+  const sdb_status rc = hnsw_enqueue(h, *t, queries, nq, k, ef, nullptr, noexp, out_elems, out_dist, out_count,
+                                     out_counters, device_io, bf);
+  if (rc != SDB_OK) {
+    cudaStreamSynchronize(t->st);  // what the failed submit queued no longer reads the caller's buffers
+    t->release();
+    return rc;
+  }
+  t->busy = true;
+  t->id = h->next_ticket++;
+  if (h->next_ticket == 0) h->next_ticket = 1;
+  *ticket = t->id;
   return SDB_OK;
 }
 
@@ -2590,7 +2748,7 @@ sdb_status sdb_hnsw_distance(sdb_hnsw* h, const void* query, const void* vectors
 
 sdb_status sdb_hnsw_set_minkowski_order(sdb_hnsw* h, double order) {
   if (!h || !(order == order)) return SDB_EINVAL;
-  std::lock_guard<std::mutex> guard(h->mu);  // searches hold it for their whole run
+  std::lock_guard<std::mutex> guard(h->mu);  // blocking searches hold it for their whole run; tickets keep their order
   h->minkowski_p = order;
   return SDB_OK;
 }
@@ -2641,6 +2799,55 @@ sdb_status sdb_hnsw_search_filtered_batch_device(sdb_hnsw* h, const void* d_quer
   const BatchFilter bf{d_filters, n_filters, query_filter, true};
   return hnsw_search_impl(h, d_queries, nq, k, ef, nullptr, nullptr, d_out_elems, d_out_dist, d_out_count, d_out_counters,
                           true, &bf);
+}
+
+sdb_status sdb_hnsw_submit(sdb_hnsw* h, const void* queries, uint32_t nq, uint32_t k, uint32_t ef,
+                           const uint8_t* all_docs_pending, uint64_t* out_elems, double* out_dist, uint32_t* out_count,
+                           uint64_t* out_counters, uint32_t* ticket) {
+  return hnsw_submit_impl(h, queries, nq, k, ef, all_docs_pending, out_elems, out_dist, out_count, out_counters, false,
+                          nullptr, ticket);
+}
+
+sdb_status sdb_hnsw_submit_device(sdb_hnsw* h, const void* d_queries, uint32_t nq, uint32_t k, uint32_t ef,
+                                  uint64_t* d_out_elems, double* d_out_dist, uint32_t* d_out_count,
+                                  uint64_t* d_out_counters, uint32_t* ticket) {
+  return hnsw_submit_impl(h, d_queries, nq, k, ef, nullptr, d_out_elems, d_out_dist, d_out_count, d_out_counters, true,
+                          nullptr, ticket);
+}
+
+sdb_status sdb_hnsw_submit_filtered(sdb_hnsw* h, const void* queries, uint32_t nq, uint32_t k, uint32_t ef,
+                                    const uint32_t* filters, uint32_t n_filters, const uint32_t* query_filter,
+                                    uint64_t* out_elems, double* out_dist, uint32_t* out_count, uint64_t* out_counters,
+                                    uint32_t* ticket) {
+  const BatchFilter bf{filters, n_filters, query_filter, false};
+  return hnsw_submit_impl(h, queries, nq, k, ef, nullptr, out_elems, out_dist, out_count, out_counters, false, &bf,
+                          ticket);
+}
+
+sdb_status sdb_hnsw_submit_filtered_device(sdb_hnsw* h, const void* d_queries, uint32_t nq, uint32_t k, uint32_t ef,
+                                           const uint32_t* d_filters, uint32_t n_filters, const uint32_t* query_filter,
+                                           uint64_t* d_out_elems, double* d_out_dist, uint32_t* d_out_count,
+                                           uint64_t* d_out_counters, uint32_t* ticket) {
+  const BatchFilter bf{d_filters, n_filters, query_filter, true};
+  return hnsw_submit_impl(h, d_queries, nq, k, ef, nullptr, d_out_elems, d_out_dist, d_out_count, d_out_counters, true,
+                          &bf, ticket);
+}
+
+sdb_status sdb_hnsw_wait(sdb_hnsw* h, uint32_t ticket) {
+  if (!h) return SDB_EINVAL;
+  std::unique_lock<std::mutex> lk(h->mu);
+  SDB_CUDA(cudaSetDevice(h->ctx->device));
+  HnswTicket* t = nullptr;
+  for (int i = 0; i < N_TICKETS && !t; i++)
+    if (h->slots[i].busy && !h->slots[i].waiting && h->slots[i].id == ticket) t = &h->slots[i];
+  if (!t) {
+    set_error("sdb_hnsw_wait: unknown or already completed ticket %u", ticket);
+    return SDB_EINVAL;
+  }
+  t->waiting = true;  // a second wait on the same ticket, while this one has released the lock, is refused
+  const sdb_status rc = hnsw_complete(h, *t, &lk);
+  t->release();
+  return rc;
 }
 
 uint32_t sdb_hnsw_last_spilled(const sdb_hnsw* h) { return h ? h->last_spilled : 0; }

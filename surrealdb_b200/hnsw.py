@@ -226,28 +226,40 @@ class HnswIndex:
                                           C.c_void_p(out.ctypes.data)))
         return out
 
-    def search_graph(self, queries, k, ef, counters=False, truthy=None, all_docs_pending=None):
-        """truthy: optional predicate mask, one byte per element (Hnsw::knn_search_with_filter, hnsw/mod.rs:488-515).
-        all_docs_pending: optional mask, one byte per element: every document of the element has a pending update
-        (the pending_docs argument of Hnsw::knn_search evaluated per element, hnsw/layer.rs:209,320-339).
-        queries are converted to the index's vector type (to_vector_type)."""
+    def _queries(self, queries):
+        """queries as a contiguous (nq, dim) array of the index's vector type (to_vector_type)"""
         q = to_vector_type(queries, self.vector_type)
         if q.ndim == 1:
             q = q[None, :]
         if q.shape[1] != self.dim:  # Error::InvalidVectorDimension  idx/trees/vector.rs:643-652
             raise L.SdbError(L.SDB_EDIM, f"Incorrect vector dimension ({q.shape[1]}). Expected a vector of {self.dim} dimension.")
+        return q
+
+    @staticmethod
+    def _outputs(nq, k):
+        """host outputs of a search: ids, distances, counts, counters"""
+        return (np.zeros((nq, max(k, 1)), np.uint64), np.zeros((nq, max(k, 1)), np.float64), np.zeros(nq, np.uint32),
+                np.zeros((nq, 2), np.uint64))
+
+    def _pending_mask(self, all_docs_pending):
+        m = np.ascontiguousarray(all_docs_pending, np.uint8)
+        if m.shape != (self.n,):
+            raise L.SdbError(L.SDB_EINVAL, f"pending mask must have one byte per element ({self.n})")
+        return m
+
+    def search_graph(self, queries, k, ef, counters=False, truthy=None, all_docs_pending=None):
+        """truthy: optional predicate mask, one byte per element (Hnsw::knn_search_with_filter, hnsw/mod.rs:488-515).
+        all_docs_pending: optional mask, one byte per element: every document of the element has a pending update
+        (the pending_docs argument of Hnsw::knn_search evaluated per element, hnsw/layer.rs:209,320-339).
+        queries are converted to the index's vector type (to_vector_type)."""
+        q = self._queries(queries)
         nq = q.shape[0]
-        ids = np.zeros((nq, max(k, 1)), np.uint64)
-        dist = np.zeros((nq, max(k, 1)), np.float64)
-        cnt = np.zeros(nq, np.uint32)
-        ctr = np.zeros((nq, 2), np.uint64)
+        ids, dist, cnt, ctr = self._outputs(nq, k)
         if truthy is not None and all_docs_pending is not None:
             # add_if_truthy ignores an element whose documents are all pending (layer.rs:287-296)
             truthy = np.asarray(truthy, np.uint8) & (np.asarray(all_docs_pending, np.uint8) == 0)
         elif all_docs_pending is not None:
-            m = np.ascontiguousarray(all_docs_pending, np.uint8)
-            if m.shape != (self.n,):
-                raise L.SdbError(L.SDB_EINVAL, f"pending mask must have one byte per element ({self.n})")
+            m = self._pending_mask(all_docs_pending)
             L.check(L.lib().sdb_hnsw_search_pending(self.h, C.c_void_p(q.ctypes.data), nq, int(k), int(ef),
                                                     C.c_void_p(m.ctypes.data), C.c_void_p(ids.ctypes.data),
                                                     C.c_void_p(dist.ctypes.data), C.c_void_p(cnt.ctypes.data),
@@ -286,18 +298,11 @@ class HnswIndex:
         (filter_words); query_filter = one filter index per query (None: filter 0 for every query).  Any selectivity
         is served on the GPU: queries that outgrow the on-chip candidate window finish in the spill tier."""
         from .engine import _query_filter
-        q = to_vector_type(queries, self.vector_type)
-        if q.ndim == 1:
-            q = q[None, :]
-        if q.shape[1] != self.dim:  # Error::InvalidVectorDimension  idx/trees/vector.rs:643-652
-            raise L.SdbError(L.SDB_EDIM, f"Incorrect vector dimension ({q.shape[1]}). Expected a vector of {self.dim} dimension.")
+        q = self._queries(queries)
         nq = q.shape[0]
         f = self.filter_words(filters)
         qf = _query_filter(query_filter, nq)
-        ids = np.zeros((nq, max(k, 1)), np.uint64)
-        dist = np.zeros((nq, max(k, 1)), np.float64)
-        cnt = np.zeros(nq, np.uint32)
-        ctr = np.zeros((nq, 2), np.uint64)
+        ids, dist, cnt, ctr = self._outputs(nq, k)
         L.check(L.lib().sdb_hnsw_search_filtered_batch(self.h, C.c_void_p(q.ctypes.data), nq, int(k), int(ef),
                                                        C.c_void_p(f.ctypes.data), f.shape[0],
                                                        None if qf is None else C.c_void_p(qf.ctypes.data),
@@ -306,8 +311,83 @@ class HnswIndex:
         return (ids, dist, cnt, ctr) if counters else (ids, dist, cnt)
 
     def last_spilled(self):
-        """queries of the last search_graph_filtered call that the spill tier finished"""
+        """queries of the last search_graph_filtered call (or waited filtered ticket) that the spill tier finished"""
         return int(L.lib().sdb_hnsw_last_spilled(self.h))
+
+    # ---- asynchronous search: up to 4 tickets in flight per index, completed by wait() in any order -----------------
+    def submit_graph(self, queries, k, ef, counters=False, all_docs_pending=None):
+        """search_graph (without truthy) queued without a host synchronisation (sdb_hnsw_submit): -> a ticket, whose
+        wait() returns what search_graph would have returned"""
+        q = self._queries(queries)
+        nq = q.shape[0]
+        m = None if all_docs_pending is None else self._pending_mask(all_docs_pending)
+        out = self._outputs(nq, k)
+        ids, dist, cnt, ctr = out
+        t = C.c_uint32()
+        L.check(L.lib().sdb_hnsw_submit(self.h, C.c_void_p(q.ctypes.data), nq, int(k), int(ef),
+                                        None if m is None else C.c_void_p(m.ctypes.data), C.c_void_p(ids.ctypes.data),
+                                        C.c_void_p(dist.ctypes.data), C.c_void_p(cnt.ctypes.data),
+                                        C.c_void_p(ctr.ctypes.data), C.byref(t)))
+        self._tickets()[t.value] = ((q, m) + out, counters)
+        return t.value
+
+    def submit_graph_filtered(self, queries, k, ef, filters, query_filter=None, counters=False):
+        """search_graph_filtered queued without a host synchronisation (sdb_hnsw_submit_filtered): -> a ticket, whose
+        wait() returns what search_graph_filtered would have returned"""
+        from .engine import _query_filter
+        q = self._queries(queries)
+        nq = q.shape[0]
+        f = self.filter_words(filters)
+        qf = _query_filter(query_filter, nq)
+        out = self._outputs(nq, k)
+        ids, dist, cnt, ctr = out
+        t = C.c_uint32()
+        L.check(L.lib().sdb_hnsw_submit_filtered(self.h, C.c_void_p(q.ctypes.data), nq, int(k), int(ef),
+                                                 C.c_void_p(f.ctypes.data), f.shape[0],
+                                                 None if qf is None else C.c_void_p(qf.ctypes.data),
+                                                 C.c_void_p(ids.ctypes.data), C.c_void_p(dist.ctypes.data),
+                                                 C.c_void_p(cnt.ctypes.data), C.c_void_p(ctr.ctypes.data), C.byref(t)))
+        self._tickets()[t.value] = ((q, f) + out, counters)
+        return t.value
+
+    def submit_device(self, d_queries, nq, k, ef, d_out_elems, d_out_dist, d_out_count, d_out_counters=None):
+        """sdb_hnsw_submit_device: device pointers (ints), valid until wait(ticket), which then returns None"""
+        t = C.c_uint32()
+        L.check(L.lib().sdb_hnsw_submit_device(self.h, C.c_void_p(d_queries), int(nq), int(k), int(ef),
+                                               C.c_void_p(d_out_elems), C.c_void_p(d_out_dist), C.c_void_p(d_out_count),
+                                               C.c_void_p(d_out_counters), C.byref(t)))
+        return t.value
+
+    def submit_filtered_device(self, d_queries, nq, k, ef, d_filters, n_filters, query_filter, d_out_elems, d_out_dist,
+                               d_out_count, d_out_counters=None):
+        """sdb_hnsw_submit_filtered_device: device pointers (ints) valid, and d_filters unchanged, until wait(ticket),
+        which then returns None; query_filter is a host array (or None), copied before the call returns"""
+        from .engine import _query_filter
+        qf = _query_filter(query_filter, nq)
+        t = C.c_uint32()
+        L.check(L.lib().sdb_hnsw_submit_filtered_device(self.h, C.c_void_p(d_queries), int(nq), int(k), int(ef),
+                                                        C.c_void_p(d_filters), int(n_filters),
+                                                        None if qf is None else C.c_void_p(qf.ctypes.data),
+                                                        C.c_void_p(d_out_elems), C.c_void_p(d_out_dist),
+                                                        C.c_void_p(d_out_count), C.c_void_p(d_out_counters), C.byref(t)))
+        return t.value
+
+    def wait(self, ticket):
+        """completes a ticket (sdb_hnsw_wait): the tuple search_graph / search_graph_filtered would have returned for a
+        ticket of submit_graph / submit_graph_filtered, None for the raw device submits.  The ticket is released (and
+        its arrays with it) whether or not the wait succeeds."""
+        kept = self._tickets().pop(int(ticket), None)
+        L.check(L.lib().sdb_hnsw_wait(self.h, int(ticket)))
+        if kept is None:
+            return None
+        (_, _, ids, dist, cnt, ctr), counters = kept
+        return (ids, dist, cnt, ctr) if counters else (ids, dist, cnt)
+
+    def _tickets(self):
+        """ticket -> the arrays the library reads or writes until its wait (and whether it reports counters)"""
+        if not hasattr(self, "_inflight"):
+            self._inflight = {}
+        return self._inflight
 
     def knn_search(self, query, k, ef, truthy_docs=None):
         """-> [(vector id, distance)] ordered by (distance, VectorId), at most k  (one query).  Mirrors
@@ -371,8 +451,9 @@ class HnswIndex:
 
     def close(self):
         if self.h:
-            L.lib().sdb_hnsw_destroy(self.h)
+            L.lib().sdb_hnsw_destroy(self.h)  # waits for the tickets in flight: their arrays go after it
             self.h = C.c_void_p()
+            self._tickets().clear()
 
     def __del__(self):
         try:
