@@ -685,6 +685,45 @@ sdb_status sdb_graph_expand_filtered_device(sdb_graph* const* hops, const sdb_ho
 sdb_status sdb_graph_collect_filtered(sdb_graph*, const sdb_hop_filter* filter, const uint32_t* start, uint64_t n_start,
                                       uint32_t min_depth, uint32_t max_depth, int inclusive, uint32_t** out_ids,
                                       uint64_t* out_n);
+
+/* ---- batches of documents: LookupPart::evaluate_batch (exec/parts/lookup.rs:96-112) and the per-row +collect
+ *      (exec/operators/recursion/collect.rs:74-143) over a ValueBatch of rows, in one call.  Document d is the segment
+ *      frontier[doc_off[d] .. doc_off[d + 1]) (the record ids of one row's value; an array value is flattened).  doc_off
+ *      has n_docs + 1 entries: doc_off[0] == 0, non-decreasing, doc_off[n_docs] == n_frontier, n_docs < 2^32; anything
+ *      else is SDB_EINVAL.  Empty documents and n_docs == 0 are valid.  The result is every document's result
+ *      concatenated; out_doc_off (n_docs + 1 entries, the caller's buffer) marks where each one starts and ends.
+ *      filters / filter: NULL (unfiltered) or as in the filtered calls above.  Unfiltered calls on shard handles are
+ *      collective like the flat ones (every rank receives the complete output and identical offsets); filters on shard
+ *      handles are refused (SDB_EUNSUPPORTED).  Cancellation is polled once per hop / level. */
+/* Segment d of the output is exactly sdb_graph_expand[_filtered] on document d: same order, same duplicates, the limit
+ * per source and per hop.  So the concatenated output is the flat call's on the whole frontier, byte for byte.  Host
+ * frontier, offsets, bitmaps and result (*out_ids: sdb_free; NULL when empty). */
+sdb_status sdb_graph_expand_batch(sdb_graph* const* hops, const sdb_hop_filter* filters, uint32_t n_hops,
+                                  const uint32_t* frontier, uint64_t n_frontier, const uint64_t* doc_off, uint64_t n_docs,
+                                  uint32_t per_source_limit, uint32_t** out_ids, uint64_t* out_doc_off, uint64_t* out_n);
+/* device-resident variant: d_frontier, d_doc_off, the bitmaps (the filters array itself is host memory), *d_out_ids and
+ * d_out_doc_off are device memory; *d_out_ids is library-owned (sdb_device_free).  d_doc_off is checked on the device,
+ * and the verdict is read back before the first hop (one 4-byte copy). */
+sdb_status sdb_graph_expand_batch_device(sdb_graph* const* hops, const sdb_hop_filter* filters, uint32_t n_hops,
+                                         const uint32_t* d_frontier, uint64_t n_frontier, const uint64_t* d_doc_off,
+                                         uint64_t n_docs, uint32_t per_source_limit, uint32_t** d_out_ids,
+                                         uint64_t* d_out_doc_off, uint64_t* out_n);
+/* Segment d of the output is exactly sdb_graph_collect[_filtered] on document d's start ids: its own first-seen set,
+ * in level order (with inclusive its start ids first).  The de-duplication state is sized by the (document, node)
+ * pairs the call visits, not by n_docs x n_rows.  The documents of a level are expanded together; a run of documents
+ * whose level (before de-duplication) would exceed 2^32 ids, or, on an unsharded handle, does not fit on the device,
+ * is served as two halves, down to single documents.  So SDB_EOVERFLOW means the whole result or one document's level
+ * exceeds the limit, as for the single-document call, and SDB_ENOMEM that one document does not fit.  Host memory.
+ * On shard handles every rank splits alike (level sizes are global), but an allocation failure is per rank: a rank
+ * that returns SDB_ENOMEM or SDB_ECUDA leaves its peers in a collective, and the communicator is not usable after it. */
+sdb_status sdb_graph_collect_batch(sdb_graph*, const sdb_hop_filter* filter, const uint32_t* start, uint64_t n_start,
+                                   const uint64_t* doc_off, uint64_t n_docs, uint32_t min_depth, uint32_t max_depth,
+                                   int inclusive, uint32_t** out_ids, uint64_t* out_doc_off, uint64_t* out_n);
+/* Diagnostics of the last sdb_graph_collect_batch on this handle (for measurement, not for control flow): the pair
+ * table's peak device bytes (the transient of a growth included), how many times it grew, how many level passes were
+ * repeated because the level overflowed it, and how many runs of documents were split in two.  Any output may be NULL. */
+void sdb_graph_last_collect_table(const sdb_graph*, uint64_t* peak_bytes, uint32_t* grows, uint32_t* repeated_passes,
+                                  uint32_t* splits);
 void sdb_free(void*);
 
 #ifdef __cplusplus

@@ -36,6 +36,7 @@ ABI_SYMBOLS = [
     "sdb_corpus_project", "sdb_topk_merge_device", "sdb_hnsw_load", "sdb_hnsw_load_typed", "sdb_hnsw_load_device", "sdb_hnsw_load_device_typed", "sdb_hnsw_set_layers_device", "sdb_hnsw_search_device", "sdb_hnsw_knn_exact_device", "sdb_hnsw_select_device", "sdb_hnsw_select_neighbors_ids", "sdb_hnsw_destroy", "sdb_stage_decode_vectors", "sdb_stage_decode_nodes", "sdb_hnsw_load_staged", "sdb_hnsw_load_staged_typed", "sdb_hnsw_search", "sdb_hnsw_search_filtered", "sdb_hnsw_search_pending", "sdb_vec_distance_f32", "sdb_hnsw_distance", "sdb_hnsw_set_minkowski_order", "sdb_hnsw_select_neighbors",
     "sdb_graph_load_csr", "sdb_graph_load_csr_shard", "sdb_graph_destroy", "sdb_graph_expand", "sdb_graph_expand_device", "sdb_device_free", "sdb_graph_collect", "sdb_free",
     "sdb_graph_expand_filtered", "sdb_graph_expand_filtered_device", "sdb_graph_collect_filtered",
+    "sdb_graph_expand_batch", "sdb_graph_expand_batch_device", "sdb_graph_collect_batch", "sdb_graph_last_collect_table",
     "sdb_knn_bruteforce_filtered", "sdb_knn_bruteforce_filtered_device", "sdb_knn_submit_filtered",
     "sdb_knn_submit_filtered_device", "sdb_knn_sharded_submit_filtered", "sdb_knn_sharded_submit_filtered_device",
     "sdb_knn_sharded_multi_filtered",
@@ -175,6 +176,11 @@ def lib():
     L.sdb_graph_expand_filtered.argtypes = [vp, vp, u32, vp, u64, u32, C.POINTER(vp), C.POINTER(u64)]
     L.sdb_graph_expand_filtered_device.argtypes = [vp, vp, u32, vp, u64, u32, C.POINTER(vp), C.POINTER(u64)]
     L.sdb_graph_collect_filtered.argtypes = [vp, vp, vp, u64, u32, u32, i32, C.POINTER(vp), C.POINTER(u64)]
+    L.sdb_graph_expand_batch.argtypes = [vp, vp, u32, vp, u64, vp, u64, u32, C.POINTER(vp), vp, C.POINTER(u64)]
+    L.sdb_graph_expand_batch_device.argtypes = [vp, vp, u32, vp, u64, vp, u64, u32, C.POINTER(vp), vp, C.POINTER(u64)]
+    L.sdb_graph_collect_batch.argtypes = [vp, vp, vp, u64, vp, u64, u32, u32, i32, C.POINTER(vp), vp, C.POINTER(u64)]
+    L.sdb_graph_last_collect_table.argtypes = [vp, C.POINTER(u64), C.POINTER(u32), C.POINTER(u32), C.POINTER(u32)]
+    L.sdb_graph_last_collect_table.restype = None
     L.sdb_free.argtypes = [vp]
     _lib = L
     return L

@@ -29,6 +29,10 @@ struct Graph {
   DevBuf<uint8_t> d_seen;
   DevBuf<uint32_t> d_first;
   DevBuf<uint32_t> d_res;
+  // diagnostics of the last sdb_graph_collect_batch (sdb_graph_last_collect_table): the pair table's peak bytes, its
+  // growths, the level passes an overflow repeated, and the runs of documents split in two
+  uint64_t table_peak_bytes = 0;
+  uint32_t table_grows = 0, table_repeats = 0, collect_splits = 0;
   std::mutex mu;
 };
 
@@ -195,9 +199,24 @@ __global__ void __launch_bounds__(EXP_THREADS) expand_kernel(const uint64_t* __r
   }
 }
 
-// *d_out: an empty buffer, which receives the next frontier (stays empty when it has no elements)
+// ---- document boundaries of a batch (sdb_graph_expand_batch / sdb_graph_collect_batch) ------------------------------
+// seg[0..n_seg) are positions into a level whose output positions are given by the exclusive scan off (off[n] = total):
+// the boundaries move to the next level by one gather.  Each thread reads and writes its own entry, so in place is safe.
+__global__ void seg_gather_kernel(const uint64_t* __restrict__ off, uint64_t* seg, uint64_t n_seg) {
+  const uint64_t d = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (d < n_seg) seg[d] = off[seg[d]];
+}
+static sdb_status seg_gather(Ctx* ctx, const uint64_t* d_off, uint64_t* d_seg, uint64_t n_seg, cudaStream_t st) {
+  seg_gather_kernel<<<(unsigned)((n_seg + 255) / 256), 256, 0, st>>>(d_off, d_seg, n_seg);
+  count_launch(ctx);
+  SDB_CUDA(cudaGetLastError());
+  return SDB_OK;
+}
+
+// *d_out: an empty buffer, which receives the next frontier (stays empty when it has no elements).
+// d_seg: nullptr, or n_seg document boundaries into the frontier, moved to the output's boundaries
 static sdb_status hop_device(Graph* g, const uint32_t* d_frontier, uint64_t n_f, uint32_t limit, AsyncBuf<uint32_t>* d_out,
-                             uint64_t* n_out, cudaStream_t st) {
+                             uint64_t* n_out, cudaStream_t st, uint64_t* d_seg = nullptr, uint64_t n_seg = 0) {
   Ctx* ctx = g->ctx;
   *n_out = 0;
   if (n_f == 0) return SDB_OK;
@@ -214,6 +233,7 @@ static sdb_status hop_device(Graph* g, const uint32_t* d_frontier, uint64_t n_f,
   const bool multi = g->sharded && comm_size(ctx) > 1;
   if (multi) SDB_TRY(comm_allreduce_sum(ctx, d_off, n_f, 8, st));
   SDB_TRY(exclusive_scan(ctx, d_off, d_off, n_f, d_total, st));
+  if (d_seg) SDB_TRY(seg_gather(ctx, d_off, d_seg, n_seg, st));
   uint64_t total = 0;
   uint32_t err = 0;
   SDB_CUDA(cudaMemcpyAsync(&total, d_total, 8, cudaMemcpyDeviceToHost, st));
@@ -411,12 +431,17 @@ __global__ void clamp_kernel(const uint64_t* __restrict__ cnt, uint64_t n, uint3
   if (i < n) out[i] = cnt[i] < limit ? cnt[i] : limit;
 }
 
-// the filtered counterpart of hop_device (same contract); the graph is unsharded and f's bitmaps are device memory
+// the filtered counterpart of hop_device (same contract); the graph is unsharded and f's bitmaps are device memory.
+// Document boundaries need the output offset of every source, which only the per-source path has (src_out): with
+// d_seg and no limit the hop takes that path with an unbounded limit, i.e. one per-source count per passing candidate
+// group and two more scans over the frontier.
 static sdb_status hop_filtered(Graph* g, const HopFilter& f, const uint32_t* d_frontier, uint64_t n_f, uint32_t limit,
-                               AsyncBuf<uint32_t>* d_out, uint64_t* n_out, cudaStream_t st) {
+                               AsyncBuf<uint32_t>* d_out, uint64_t* n_out, cudaStream_t st, uint64_t* d_seg = nullptr,
+                               uint64_t n_seg = 0) {
   Ctx* ctx = g->ctx;
   *n_out = 0;
   if (n_f == 0) return SDB_OK;
+  if (d_seg && !limit) limit = 0xFFFFFFFFu;
   // one run of tiles per resident block; both passes must use the same grid
   int occ_count = 0, occ_write = 0;
   SDB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_count, filter_kernel<false>, EXP_THREADS, 0));
@@ -448,6 +473,7 @@ static sdb_status hop_filtered(Graph* g, const HopFilter& f, const uint32_t* d_f
     SDB_TRY(exclusive_scan(ctx, d_src, d_src, n_f, d_src + n_f, st));
     SDB_TRY(exclusive_scan(ctx, d_src_out, d_src_out, n_f, d_src_out + n_f, st));
     d_total = d_src_out + n_f;
+    if (d_seg) SDB_TRY(seg_gather(ctx, d_src_out, d_seg, n_seg, st));
   }
   uint64_t total = 0;
   uint32_t err = 0;
@@ -471,6 +497,133 @@ static sdb_status hop_filtered(Graph* g, const HopFilter& f, const uint32_t* d_f
   SDB_CUDA(cudaGetLastError());
   *n_out = total;
   return SDB_OK;
+}
+
+// ---- batch +collect: first-seen de-duplication per (document, node) pair ----------------------------------------------
+// An open-addressing table keyed on (doc << 32) | node holds every pair the call has visited, so its size follows the
+// visited pairs, never n_docs x n_rows.  A slot's value is the first level position of its pair while the level is
+// marked (PAIR_NONE before any), then PAIR_SEEN once the pair has been kept; level positions stay below 0xFFFFFFF0.
+// Insertions reserve a unit of `fill` first and fail (setting the overflow flag) past max_fill < capacity, so probing
+// always finds a free slot; the host then grows the table and repeats the pass, which is idempotent.
+constexpr unsigned long long PAIR_EMPTY = ~0ull;  // node ids are < 2^32 - 16: no pair has this key
+constexpr uint32_t PAIR_NONE = 0xFFFFFFFFu, PAIR_SEEN = 0xFFFFFFFEu;
+
+struct PairTable {
+  unsigned long long* keys;
+  uint32_t* vals;
+  uint64_t mask;                 // capacity - 1 (a power of two)
+  unsigned long long* fill;      // [0] reserved slots, [1] overflow flag
+  unsigned long long max_fill;
+};
+
+__device__ __forceinline__ uint64_t pair_hash(uint64_t k) {  // splitmix64 finaliser
+  k ^= k >> 30;
+  k *= 0xbf58476d1ce4e5b9ull;
+  k ^= k >> 27;
+  k *= 0x94d049bb133111ebull;
+  return k ^ (k >> 31);
+}
+// slot of `key`, inserted if absent; ~0 when the table is too full (the overflow flag is set)
+__device__ uint64_t pair_insert(const PairTable& t, unsigned long long key) {
+  uint64_t s = pair_hash(key) & t.mask;
+  for (uint64_t i = 0; i <= t.mask; i++, s = (s + 1) & t.mask) {
+    unsigned long long k = __ldcg(t.keys + s);
+    if (k == PAIR_EMPTY) {
+      if (*(volatile unsigned long long*)(t.fill + 1)) return ~0ull;  // the pass repeats anyway: no more fill atomics
+      if (atomicAdd(t.fill, 1ull) >= t.max_fill) {
+        atomicAdd(t.fill, ~0ull);  // give the unit back
+        t.fill[1] = 1;
+        return ~0ull;
+      }
+      k = atomicCAS(t.keys + s, PAIR_EMPTY, key);
+      if (k == PAIR_EMPTY) return s;
+      atomicAdd(t.fill, ~0ull);  // another thread took the slot
+    }
+    if (k == key) return s;
+  }
+  t.fill[1] = 1;
+  return ~0ull;
+}
+// slot of a pair that was inserted, ~0 if absent
+__device__ uint64_t pair_find(const PairTable& t, unsigned long long key) {
+  uint64_t s = pair_hash(key) & t.mask;
+  for (uint64_t i = 0; i <= t.mask; i++, s = (s + 1) & t.mask) {
+    const unsigned long long k = t.keys[s];
+    if (k == key) return s;
+    if (k == PAIR_EMPTY) return ~0ull;
+  }
+  return ~0ull;
+}
+// the document of level position p: seg holds n_docs + 1 boundaries and p < seg[n_docs]
+__device__ __forceinline__ unsigned long long pair_key(const uint64_t* seg, uint64_t n_docs, uint64_t p, uint32_t v) {
+  return (upper_bound_minus1(seg, 0, n_docs + 1, p) << 32) | v;
+}
+
+// +inclusive: the start ids are emitted and marked seen in their own document
+__global__ void pair_seed_kernel(const uint32_t* __restrict__ ids, uint64_t n, const uint64_t* __restrict__ seg,
+                                 uint64_t n_docs, PairTable t) {
+  const uint64_t p = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (p >= n) return;
+  const uint64_t s = pair_insert(t, pair_key(seg, n_docs, p, ids[p]));
+  if (s != ~0ull) t.vals[s] = PAIR_SEEN;
+}
+__global__ void pair_mark_kernel(const uint32_t* __restrict__ lvl, uint64_t n, const uint64_t* __restrict__ seg,
+                                 uint64_t n_docs, PairTable t) {
+  const uint64_t p = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (p >= n) return;
+  const uint64_t s = pair_insert(t, pair_key(seg, n_docs, p, lvl[p]));
+  if (s == ~0ull) return;
+  const uint32_t v = __ldcg(t.vals + s);  // PAIR_SEEN is only written between levels
+  if (v != PAIR_SEEN && v > (uint32_t)p) atomicMin(t.vals + s, (uint32_t)p);
+}
+__global__ void pair_flag_kernel(const uint32_t* __restrict__ lvl, uint64_t n, const uint64_t* __restrict__ seg,
+                                 uint64_t n_docs, PairTable t, uint64_t* __restrict__ keep) {
+  const uint64_t p = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (p >= n) return;
+  const uint64_t s = pair_find(t, pair_key(seg, n_docs, p, lvl[p]));
+  keep[p] = s != ~0ull && t.vals[s] == (uint32_t)p;
+}
+__global__ void pair_compact_kernel(const uint32_t* __restrict__ lvl, uint64_t n, const uint64_t* __restrict__ seg,
+                                    uint64_t n_docs, PairTable t, const uint64_t* __restrict__ pos /* n+1 */,
+                                    uint32_t* __restrict__ next) {
+  const uint64_t p = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (p >= n || pos[p + 1] == pos[p]) return;
+  const uint32_t v = lvl[p];
+  next[pos[p]] = v;
+  t.vals[pair_find(t, pair_key(seg, n_docs, p, v))] = PAIR_SEEN;  // kept, so present
+}
+// re-inserts the pairs of a smaller table (with their values) into a grown one
+__global__ void pair_rehash_kernel(const unsigned long long* __restrict__ keys, const uint32_t* __restrict__ vals,
+                                   uint64_t cap, PairTable t) {
+  const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= cap || keys[i] == PAIR_EMPTY) return;
+  const uint64_t s = pair_insert(t, keys[i]);
+  if (s != ~0ull) t.vals[s] = vals[i];
+}
+
+// ---- per-document assembly of a batch result ------------------------------------------------------------------------
+// cnt[d] += seg[d + 1] - seg[d]
+__global__ void seg_count_kernel(const uint64_t* __restrict__ seg, uint64_t n_docs, uint64_t* __restrict__ cnt) {
+  const uint64_t d = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (d < n_docs) cnt[d] += seg[d + 1] - seg[d];
+}
+// writes a level's segment d after what earlier levels wrote for document d: out[out_off[d] + done[d] + (p - seg[d])]
+__global__ void seg_scatter_kernel(const uint32_t* __restrict__ ids, uint64_t n, const uint64_t* __restrict__ seg,
+                                   uint64_t n_docs, const uint64_t* __restrict__ out_off,
+                                   const uint64_t* __restrict__ done, uint32_t* __restrict__ out) {
+  const uint64_t p = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (p >= n) return;
+  const uint64_t d = upper_bound_minus1(seg, 0, n_docs + 1, p);
+  out[out_off[d] + done[d] + (p - seg[d])] = ids[p];
+}
+// device doc_off check: seg = doc_off clamped to [0, n], *bad = 1 unless doc_off[0] == 0, non-decreasing, doc_off[n_docs] == n
+__global__ void seg_check_kernel(const uint64_t* __restrict__ doc_off, uint64_t n_docs, uint64_t n,
+                                 uint64_t* __restrict__ seg, uint32_t* __restrict__ bad) {
+  const uint64_t d = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (d > n_docs) return;
+  const uint64_t v = doc_off[d];
+  if ((d == 0 && v != 0) || (d == n_docs && v != n) || (d > 0 && v < doc_off[d - 1]) || v > n) *bad = 1;
+  seg[d] = v < n ? v : n;
 }
 
 }  // namespace sdb
@@ -556,10 +709,11 @@ void sdb_graph_destroy(sdb_graph* g) {
 static bool has_filter(const HopFilter* f) { return f && (f->edge_bits || f->target_bits); }
 
 // device-resident core: frontier and result stay in HBM (sdb_graph_expand_device hands the result to the caller).
-// filters: nullptr, or one per hop (device bitmaps); a hop without bitmaps runs the unfiltered hop
+// filters: nullptr, or one per hop (device bitmaps); a hop without bitmaps runs the unfiltered hop.
+// d_seg: nullptr, or n_seg document boundaries into the frontier, moved hop by hop to the result's boundaries
 static sdb_status graph_expand_dev(sdb_graph* const* hops, uint32_t n_hops, const uint32_t* d_frontier, uint64_t n_frontier,
                                    uint32_t per_source_limit, AsyncBuf<uint32_t>* d_out, uint64_t* out_n, cudaStream_t st,
-                                   const HopFilter* filters = nullptr) {
+                                   const HopFilter* filters = nullptr, uint64_t* d_seg = nullptr, uint64_t n_seg = 0) {
   AsyncBuf<uint32_t> d_f;
   uint64_t n_f = n_frontier;
   bool owned = false;  // the caller's frontier is never freed
@@ -572,9 +726,9 @@ static sdb_status graph_expand_dev(sdb_graph* const* hops, uint32_t n_hops, cons
     }
     const uint32_t* d_in = owned ? d_f.get() : d_frontier;
     if (filters && has_filter(&filters[h]))
-      SDB_TRY(hop_filtered(hops[h], filters[h], d_in, n_f, per_source_limit, &d_next, &n_next, st));
+      SDB_TRY(hop_filtered(hops[h], filters[h], d_in, n_f, per_source_limit, &d_next, &n_next, st, d_seg, n_seg));
     else
-      SDB_TRY(hop_device(hops[h], d_in, n_f, per_source_limit, &d_next, &n_next, st));
+      SDB_TRY(hop_device(hops[h], d_in, n_f, per_source_limit, &d_next, &n_next, st, d_seg, n_seg));
     d_f = std::move(d_next);
     owned = true;
     n_f = n_next;
@@ -624,16 +778,41 @@ static sdb_status upload_filters(sdb_graph* const* graphs, const sdb_hop_filter*
   return SDB_OK;
 }
 
+// d_doc_off: nullptr, or n_docs + 1 document boundaries into d_frontier (device), checked on the device; the result's
+// boundaries go to d_out_doc_off (device)
 static sdb_status expand_device_call(sdb_graph* const* hops, const sdb_hop_filter* d_filters, uint32_t n_hops,
                                      const uint32_t* d_frontier, uint64_t n_frontier, uint32_t per_source_limit,
-                                     uint32_t** d_out_ids, uint64_t* out_n) {
+                                     uint32_t** d_out_ids, uint64_t* out_n, const uint64_t* d_doc_off = nullptr,
+                                     uint64_t n_docs = 0, uint64_t* d_out_doc_off = nullptr) {
   Ctx* ctx = hops[0]->ctx;
   std::lock_guard<std::mutex> guard(ctx->mu);
   SDB_CUDA(cudaSetDevice(ctx->device));
+  cudaStream_t st = ctx->stream;
+  AsyncBuf<uint64_t> d_seg;
+  AsyncBuf<uint32_t> d_bad;
+  if (d_doc_off) {
+    SDB_CUDA(d_seg.reserve(n_docs + 1, st));
+    SDB_CUDA(d_bad.reserve(1, st));
+    SDB_CUDA(cudaMemsetAsync(d_bad, 0, 4, st));
+    seg_check_kernel<<<(unsigned)((n_docs + 256) / 256), 256, 0, st>>>(d_doc_off, n_docs, n_frontier, d_seg, d_bad);
+    count_launch(ctx);
+    SDB_CUDA(cudaGetLastError());
+    // the verdict comes first: a malformed d_doc_off runs no hop, and no hop's status can hide it
+    uint32_t bad = 0;
+    SDB_CUDA(cudaMemcpyAsync(&bad, d_bad, 4, cudaMemcpyDeviceToHost, st));
+    SDB_CUDA(cudaStreamSynchronize(st));
+    if (bad) {
+      set_error("graph expand batch: doc_off must start at 0, not decrease and end at n_frontier");
+      return SDB_EINVAL;
+    }
+  }
   AsyncBuf<uint32_t> d_out;
-  SDB_TRY(graph_expand_dev(hops, n_hops, d_frontier, n_frontier, per_source_limit, &d_out, out_n, ctx->stream, d_filters));
+  SDB_TRY(graph_expand_dev(hops, n_hops, d_frontier, n_frontier, per_source_limit, &d_out, out_n, st, d_filters, d_seg,
+                           n_docs + 1));
+  if (d_doc_off)
+    SDB_CUDA(cudaMemcpyAsync(d_out_doc_off, d_seg, sizeof(uint64_t) * (n_docs + 1), cudaMemcpyDeviceToDevice, st));
   *d_out_ids = d_out.release();
-  SDB_CUDA(cudaStreamSynchronize(ctx->stream));
+  SDB_CUDA(cudaStreamSynchronize(st));
   return SDB_OK;
 }
 
@@ -666,10 +845,12 @@ void sdb_device_free(sdb_ctx* ctx, void* d_ptr) {
   AsyncBuf<uint32_t>::free_released(d_ptr, ctx->stream);
 }
 
-// host frontier and result; filters: nullptr or one per hop, host bitmaps (copied for this call)
+// host frontier and result; filters: nullptr or one per hop, host bitmaps (copied for this call).  doc_off: nullptr, or
+// n_docs + 1 checked document boundaries into frontier (host); the result's boundaries go to out_doc_off (host)
 static sdb_status expand_host_call(sdb_graph* const* hops, const sdb_hop_filter* filters, uint32_t n_hops,
                                    const uint32_t* frontier, uint64_t n_frontier, uint32_t per_source_limit,
-                                   uint32_t** out_ids, uint64_t* out_n) {
+                                   uint32_t** out_ids, uint64_t* out_n, const uint64_t* doc_off = nullptr,
+                                   uint64_t n_docs = 0, uint64_t* out_doc_off = nullptr) {
   Ctx* ctx = hops[0]->ctx;
   std::lock_guard<std::mutex> guard(ctx->mu);
   SDB_CUDA(cudaSetDevice(ctx->device));
@@ -682,11 +863,18 @@ static sdb_status expand_host_call(sdb_graph* const* hops, const sdb_hop_filter*
     SDB_CUDA(d_in.reserve(n_frontier, st));
     SDB_CUDA(cudaMemcpyAsync(d_in, frontier, sizeof(uint32_t) * n_frontier, cudaMemcpyHostToDevice, st));
   }
+  AsyncBuf<uint64_t> d_seg;
+  if (doc_off) {
+    SDB_CUDA(d_seg.reserve(n_docs + 1, st));
+    SDB_CUDA(cudaMemcpyAsync(d_seg, doc_off, sizeof(uint64_t) * (n_docs + 1), cudaMemcpyHostToDevice, st));
+  }
   AsyncBuf<uint32_t> d_f;
   uint64_t n_f = 0;
   SDB_TRY(graph_expand_dev(hops, n_hops, d_in, n_frontier, per_source_limit, &d_f, &n_f, st,
-                           filters ? d_filters.data() : nullptr));
+                           filters ? d_filters.data() : nullptr, d_seg, n_docs + 1));
   d_in.reset();
+  if (doc_off)  // pageable: complete when the synchronisation below returns
+    SDB_CUDA(cudaMemcpyAsync(out_doc_off, d_seg, sizeof(uint64_t) * (n_docs + 1), cudaMemcpyDeviceToHost, st));
   if (n_f) {
     uint32_t* h_out = (uint32_t*)malloc(sizeof(uint32_t) * n_f);
     if (!h_out) return SDB_ENOMEM;
@@ -866,6 +1054,371 @@ sdb_status sdb_graph_collect_filtered(sdb_graph* g, const sdb_hop_filter* filter
   *out_n = 0;
   SDB_TRY(check_filtered(g, filter, "sdb_graph_collect_filtered"));
   return collect_call(g, filter, start, n_start, min_depth, max_depth, inclusive, out_ids, out_n);
+}
+
+// ---- batches of documents: document d is frontier[doc_off[d] .. doc_off[d + 1]) -----------------------------------------
+static sdb_status check_doc_off(const uint64_t* doc_off, uint64_t n_docs, uint64_t n, const char* fn) {
+  if (n_docs >= (1ull << 32)) {
+    set_error("%s: %llu documents exceed the 2^32 limit", fn, (unsigned long long)n_docs);
+    return SDB_EINVAL;
+  }
+  bool ok = doc_off[0] == 0 && doc_off[n_docs] == n;
+  for (uint64_t d = 0; ok && d < n_docs; d++) ok = doc_off[d + 1] >= doc_off[d];
+  if (!ok) {
+    set_error("%s: doc_off must start at 0, not decrease and end at %llu", fn, (unsigned long long)n);
+    return SDB_EINVAL;
+  }
+  return SDB_OK;
+}
+
+// the checks every batch expand shares; filters on shard handles are refused as by the filtered calls
+static sdb_status check_expand_batch(sdb_graph* const* hops, const sdb_hop_filter* filters, uint32_t n_hops, const char* fn) {
+  for (uint32_t h = 0; h < n_hops; h++) {
+    if (!hops[h]) return SDB_EINVAL;
+    if (filters) SDB_TRY(check_filtered(hops[h], &filters[h], fn));
+  }
+  return SDB_OK;
+}
+
+sdb_status sdb_graph_expand_batch(sdb_graph* const* hops, const sdb_hop_filter* filters, uint32_t n_hops,
+                                  const uint32_t* frontier, uint64_t n_frontier, const uint64_t* doc_off, uint64_t n_docs,
+                                  uint32_t per_source_limit, uint32_t** out_ids, uint64_t* out_doc_off, uint64_t* out_n) {
+  if (!hops || !n_hops || !out_ids || !out_n || !doc_off || !out_doc_off || (n_frontier && !frontier)) return SDB_EINVAL;
+  *out_ids = nullptr;
+  *out_n = 0;
+  SDB_TRY(check_expand_batch(hops, filters, n_hops, "sdb_graph_expand_batch"));
+  SDB_TRY(check_doc_off(doc_off, n_docs, n_frontier, "sdb_graph_expand_batch"));
+  return expand_host_call(hops, filters, n_hops, frontier, n_frontier, per_source_limit, out_ids, out_n, doc_off, n_docs,
+                          out_doc_off);
+}
+
+sdb_status sdb_graph_expand_batch_device(sdb_graph* const* hops, const sdb_hop_filter* filters, uint32_t n_hops,
+                                         const uint32_t* d_frontier, uint64_t n_frontier, const uint64_t* d_doc_off,
+                                         uint64_t n_docs, uint32_t per_source_limit, uint32_t** d_out_ids,
+                                         uint64_t* d_out_doc_off, uint64_t* out_n) {
+  if (!hops || !n_hops || !d_out_ids || !out_n || !d_doc_off || !d_out_doc_off || (n_frontier && !d_frontier))
+    return SDB_EINVAL;
+  *d_out_ids = nullptr;
+  *out_n = 0;
+  SDB_TRY(check_expand_batch(hops, filters, n_hops, "sdb_graph_expand_batch_device"));
+  if (n_docs >= (1ull << 32)) {
+    set_error("sdb_graph_expand_batch_device: %llu documents exceed the 2^32 limit", (unsigned long long)n_docs);
+    return SDB_EINVAL;
+  }
+  return expand_device_call(hops, filters, n_hops, d_frontier, n_frontier, per_source_limit, d_out_ids, out_n, d_doc_off,
+                            n_docs, d_out_doc_off);
+}
+
+}  // extern "C"
+
+// the pair table of a batch +collect (PairTable), with the buffers behind it
+struct PairTableBufs {
+  AsyncBuf<unsigned long long> keys, fill;
+  AsyncBuf<uint32_t> vals;
+  uint64_t cap = 0;
+  PairTable view() { return PairTable{keys, vals, cap - 1, fill, cap / 2}; }
+  uint64_t bytes() const { return cap * (sizeof(unsigned long long) + sizeof(uint32_t)); }
+};
+// a failed device allocation of a batch +collect: SDB_ENOMEM when the device has no room, SDB_ECUDA otherwise
+static sdb_status room(cudaError_t e, const char* what) {
+  if (e == cudaSuccess) return SDB_OK;
+  set_error("graph collect batch: no room for %s: %s", what, cudaGetErrorString(e));
+  return e == cudaErrorMemoryAllocation ? SDB_ENOMEM : SDB_ECUDA;
+}
+static sdb_status table_alloc(PairTableBufs* t, uint64_t cap, cudaStream_t st) {
+  SDB_TRY(room(t->keys.reserve(cap, st), "the pair table"));
+  SDB_TRY(room(t->vals.reserve(cap, st), "the pair table"));
+  SDB_TRY(room(t->fill.reserve(2, st), "the pair table"));
+  t->cap = cap;
+  SDB_CUDA(cudaMemsetAsync(t->keys, 0xFF, sizeof(unsigned long long) * cap, st));                  // PAIR_EMPTY
+  SDB_CUDA(cudaMemsetAsync(t->vals, (int)(PAIR_NONE & 0xFF), sizeof(uint32_t) * cap, st));  // every byte of PAIR_NONE
+  SDB_CUDA(cudaMemsetAsync(t->fill, 0, 2 * sizeof(unsigned long long), st));
+  return SDB_OK;
+}
+// a table of cap slots (a larger power of two) holding the same pairs and values
+static sdb_status table_grow(Graph* g, PairTableBufs* t, uint64_t cap, cudaStream_t st) {
+  PairTableBufs n;
+  SDB_TRY(table_alloc(&n, cap, st));
+  g->table_peak_bytes = std::max(g->table_peak_bytes, t->bytes() + n.bytes());
+  pair_rehash_kernel<<<(unsigned)((t->cap + 255) / 256), 256, 0, st>>>(t->keys, t->vals, t->cap, n.view());
+  count_launch(g->ctx);
+  SDB_CUDA(cudaGetLastError());
+  *t = std::move(n);
+  g->table_grows++;
+  return SDB_OK;
+}
+// runs `pass` (idempotent insertions into t) until it fits: a pass that overflows doubles the table and runs again.
+// read: extra 8-byte device words copied back with the overflow flag (the level's size), in the same synchronisation
+template <class Pass>
+static sdb_status table_pass(Graph* g, PairTableBufs* t, cudaStream_t st, Pass pass, const uint64_t* d_read = nullptr,
+                             uint64_t* h_read = nullptr) {
+  for (;;) {
+    SDB_CUDA(cudaMemsetAsync(t->fill.get() + 1, 0, sizeof(unsigned long long), st));
+    SDB_TRY(pass(t->view()));
+    unsigned long long overflow = 0;
+    SDB_CUDA(cudaMemcpyAsync(&overflow, t->fill.get() + 1, 8, cudaMemcpyDeviceToHost, st));
+    if (d_read) SDB_CUDA(cudaMemcpyAsync(h_read, d_read, 8, cudaMemcpyDeviceToHost, st));
+    SDB_CUDA(cudaStreamSynchronize(st));
+    if (!overflow) return SDB_OK;
+    g->table_repeats++;
+    SDB_TRY(table_grow(g, t, 2 * t->cap, st));
+  }
+}
+// SDB_DEBUG_PAIR_TABLE_SLOTS=n caps the table's size before a level (diagnostics: it makes the levels overflow and
+// exercises the doubling above); unset, the size before a level is bounded by the device's free memory only
+static uint64_t table_size_cap() {
+  const char* s = getenv("SDB_DEBUG_PAIR_TABLE_SLOTS");
+  const unsigned long long v = s ? strtoull(s, nullptr, 10) : 0;
+  return v >= 64 ? (uint64_t)v : ~0ull;
+}
+
+struct CollectArgs {
+  Graph* g;
+  const HopFilter* f;  // device bitmaps, nullptr = unfiltered
+  uint32_t min_depth, max_depth;
+  int inclusive;
+  cudaStream_t st;
+};
+
+// +collect of one run of documents: the levels of its documents run together, each document with its own first-seen
+// set.  Appends the run's ids to *ids and writes its n_docs + 1 offsets (from 0) to run_off.  The 2^32-id limit holds
+// for the whole batch: res_before ids precede this run; *total_overflow says the batch's result exceeded it.
+static sdb_status collect_run(const CollectArgs& a, const uint32_t* start, const uint64_t* doc_off, uint64_t n_docs,
+                              std::vector<uint32_t>* ids, uint64_t* run_off, uint64_t res_before, bool* total_overflow) {
+  Graph* g = a.g;
+  Ctx* ctx = g->ctx;
+  cudaStream_t st = a.st;
+  struct Drain {  // the stream-ordered temporaries below are released on every return path, then the stream is drained
+    cudaStream_t st;
+    ~Drain() { cudaStreamSynchronize(st); }
+  } drain{st};
+  const uint64_t n_start = doc_off[n_docs], n_seg = n_docs + 1;
+  AsyncBuf<uint64_t> d_seg;  // the current frontier's document boundaries
+  SDB_TRY(room(d_seg.reserve(n_seg, st), "the document offsets"));
+  SDB_CUDA(cudaMemcpyAsync(d_seg, doc_off, sizeof(uint64_t) * n_seg, cudaMemcpyHostToDevice, st));
+  AsyncBuf<uint32_t> d_f;
+  uint64_t n_f = n_start;
+  if (n_f) {
+    SDB_TRY(room(d_f.reserve(n_f, st), "the start ids"));
+    SDB_CUDA(cudaMemcpyAsync(d_f, start, sizeof(uint32_t) * n_f, cudaMemcpyHostToDevice, st));
+  }
+  const uint64_t size_cap = table_size_cap();
+  PairTableBufs tab;
+  uint64_t cap = 4096;
+  while (cap < 4 * n_start && cap < size_cap) cap *= 2;
+  SDB_TRY(table_alloc(&tab, cap, st));
+  g->table_peak_bytes = std::max(g->table_peak_bytes, tab.bytes());
+  // the emitted levels with their document boundaries, assembled per document at the end
+  struct Level {
+    AsyncBuf<uint32_t> ids;
+    AsyncBuf<uint64_t> seg;
+    uint64_t n;
+  };
+  std::vector<Level> levels;
+  uint64_t n_res = 0;
+  uint64_t n_pairs = a.inclusive ? n_start : 0;  // an upper bound of the pairs in the table
+  auto emit = [&](const uint32_t* d_ids, uint64_t n) -> sdb_status {
+    if (res_before + n_res + n > 0xFFFFFFF0ull) {
+      set_error("graph collect batch: %llu results exceed the 2^32 limit", (unsigned long long)(res_before + n_res + n));
+      *total_overflow = true;
+      return SDB_EOVERFLOW;
+    }
+    Level l;
+    l.n = n;
+    SDB_TRY(room(l.ids.reserve(n, st), "a level's result"));
+    SDB_TRY(room(l.seg.reserve(n_seg, st), "a level's result"));
+    SDB_CUDA(cudaMemcpyAsync(l.ids, d_ids, sizeof(uint32_t) * n, cudaMemcpyDeviceToDevice, st));
+    SDB_CUDA(cudaMemcpyAsync(l.seg, d_seg, sizeof(uint64_t) * n_seg, cudaMemcpyDeviceToDevice, st));
+    levels.push_back(std::move(l));
+    n_res += n;
+    return SDB_OK;
+  };
+  if (a.inclusive && n_start) {  // collect.rs:83-86: the start values are emitted and marked seen only when inclusive
+    SDB_TRY(table_pass(g, &tab, st, [&](PairTable t) -> sdb_status {
+      pair_seed_kernel<<<(unsigned)((n_start + 255) / 256), 256, 0, st>>>(d_f, n_start, d_seg, n_docs, t);
+      count_launch(ctx);
+      SDB_CUDA(cudaGetLastError());
+      return SDB_OK;
+    }));
+    SDB_TRY(emit(d_f, n_start));
+  }
+  uint32_t depth = 0;
+  while (n_f && (a.max_depth == 0 || depth < a.max_depth)) {
+    if (ctx_cancelled(ctx)) {  // polled once per BFS level
+      set_error("query cancelled");
+      return SDB_ECANCELLED;
+    }
+    AsyncBuf<uint32_t> d_lvl;
+    uint64_t n_lvl = 0;
+    if (a.f)
+      SDB_TRY(hop_filtered(g, *a.f, d_f, n_f, 0, &d_lvl, &n_lvl, st, d_seg, n_seg));
+    else
+      SDB_TRY(hop_device(g, d_f, n_f, 0, &d_lvl, &n_lvl, st, d_seg, n_seg));
+    d_f.reset();
+    n_f = 0;
+    if (n_lvl) {
+      // within the level the first position of each (document, node) pair not seen before is kept
+      AsyncBuf<uint64_t> d_pos;
+      SDB_TRY(room(d_pos.reserve(n_lvl + 2, st), "a level's positions"));
+      const unsigned grid = (unsigned)((n_lvl + 255) / 256);
+      // between levels the table grows to hold every pair the level could add at half load, as far as half of the
+      // device's free memory allows (the rest is for the next frontier and the emitted levels) -- the largest power of
+      // two that fits; a level whose distinct pairs still overflow it doubles it in table_pass
+      uint64_t want = tab.cap;
+      while (want / 2 < n_pairs + n_lvl && want < size_cap) want *= 2;
+      size_t free_b = 0, total_b = 0;
+      SDB_CUDA(cudaMemGetInfo(&free_b, &total_b));
+      while (want > tab.cap && (want + tab.cap) * (sizeof(unsigned long long) + sizeof(uint32_t)) > free_b / 2) want /= 2;
+      while (want > tab.cap) {
+        const sdb_status rc = table_grow(g, &tab, want, st);
+        if (rc != SDB_ENOMEM) {
+          SDB_TRY(rc);
+          break;
+        }
+        want /= 2;
+      }
+      uint64_t n_next = 0;
+      SDB_TRY(table_pass(g, &tab, st, [&](PairTable t) -> sdb_status {
+        pair_mark_kernel<<<grid, 256, 0, st>>>(d_lvl, n_lvl, d_seg, n_docs, t);
+        pair_flag_kernel<<<grid, 256, 0, st>>>(d_lvl, n_lvl, d_seg, n_docs, t, d_pos);
+        count_launch(ctx, 2);
+        SDB_CUDA(cudaGetLastError());
+        return exclusive_scan(ctx, d_pos, d_pos, n_lvl, d_pos + n_lvl, st);
+      }, d_pos + n_lvl, &n_next));
+      if (n_next) {
+        SDB_TRY(room(d_f.reserve(n_next, st), "the next frontier"));
+        pair_compact_kernel<<<grid, 256, 0, st>>>(d_lvl, n_lvl, d_seg, n_docs, tab.view(), d_pos, d_f);
+        count_launch(ctx);
+        SDB_CUDA(cudaGetLastError());
+      }
+      SDB_TRY(seg_gather(ctx, d_pos, d_seg, n_seg, st));  // the kept positions' boundaries: the next frontier's
+      n_f = n_next;
+      n_pairs += n_next;
+      if (n_next && depth + 1 >= a.min_depth) SDB_TRY(emit(d_f, n_next));  // below min_depth: traversed, not emitted
+    }
+    depth++;
+  }
+  tab = PairTableBufs();
+  // per document in level order: out_off = exclusive scan of the per-document totals, then each level's segment d
+  // after what the levels before it wrote for d
+  AsyncBuf<uint64_t> d_off, d_done;
+  AsyncBuf<uint32_t> d_res;
+  SDB_TRY(room(d_off.reserve(n_seg, st), "the result offsets"));
+  SDB_TRY(room(d_done.reserve(n_seg, st), "the result offsets"));
+  SDB_CUDA(cudaMemsetAsync(d_off, 0, sizeof(uint64_t) * n_seg, st));
+  SDB_CUDA(cudaMemsetAsync(d_done, 0, sizeof(uint64_t) * n_seg, st));
+  const unsigned dgrid = (unsigned)((n_docs + 255) / 256);
+  if (n_docs)
+    for (const Level& l : levels) seg_count_kernel<<<dgrid, 256, 0, st>>>(l.seg, n_docs, d_off);
+  count_launch(ctx, levels.size());
+  SDB_TRY(exclusive_scan(ctx, d_off, d_off, n_docs, d_off + n_docs, st));
+  if (n_res) {
+    SDB_TRY(room(d_res.reserve(n_res, st), "the result"));
+    for (Level& l : levels) {
+      seg_scatter_kernel<<<(unsigned)((l.n + 255) / 256), 256, 0, st>>>(l.ids, l.n, l.seg, n_docs, d_off, d_done, d_res);
+      seg_count_kernel<<<dgrid, 256, 0, st>>>(l.seg, n_docs, d_done);
+      count_launch(ctx, 2);
+      l.ids.reset();
+      l.seg.reset();
+    }
+  }
+  SDB_CUDA(cudaGetLastError());
+  const uint64_t base = ids->size();
+  ids->resize(base + n_res);
+  const size_t bytes = sizeof(uint32_t) * n_res;
+  uint8_t* stage = bytes >= (1u << 20) ? stage_buffer(ctx, bytes) : nullptr;
+  SDB_CUDA(cudaMemcpyAsync(run_off, d_off, sizeof(uint64_t) * n_seg, cudaMemcpyDeviceToHost, st));
+  if (n_res) SDB_CUDA(cudaMemcpyAsync(stage ? (void*)stage : (void*)(ids->data() + base), d_res, bytes, cudaMemcpyDeviceToHost, st));
+  SDB_CUDA(cudaStreamSynchronize(st));
+  if (stage) memcpy(ids->data() + base, stage, bytes);
+  return SDB_OK;
+}
+
+// documents [d0, d1) of the batch (doc_off: the batch's offsets); their offsets go to out_off[d0 .. d1] (the batch's).
+// Documents are independent: a run that a hop refuses because its level exceeds 2^32 ids, or (unsharded) that finds no
+// room on the device, is served as two halves.  On shard handles the level's size is the same on every rank, so every
+// rank splits alike; a per-rank allocation failure is not split.
+static sdb_status collect_split(const CollectArgs& a, const uint32_t* start, const uint64_t* doc_off, uint64_t d0,
+                                uint64_t d1, std::vector<uint32_t>* ids, uint64_t* out_off) {
+  std::vector<uint64_t> off(d1 - d0 + 1), run_off(d1 - d0 + 1);
+  for (uint64_t i = 0; i <= d1 - d0; i++) off[i] = doc_off[d0 + i] - doc_off[d0];
+  const uint64_t base = ids->size();
+  bool total_overflow = false;
+  const sdb_status rc = collect_run(a, start + doc_off[d0], off.data(), d1 - d0, ids, run_off.data(), base, &total_overflow);
+  if (rc == SDB_OK) {
+    for (uint64_t i = 0; i <= d1 - d0; i++) out_off[d0 + i] = base + run_off[i];
+    return SDB_OK;
+  }
+  if (d1 - d0 < 2 || total_overflow || !(rc == SDB_EOVERFLOW || (rc == SDB_ENOMEM && !a.g->sharded))) return rc;
+  a.g->collect_splits++;
+  const uint64_t dm = d0 + (d1 - d0) / 2;
+  SDB_TRY(collect_split(a, start, doc_off, d0, dm, ids, out_off));
+  return collect_split(a, start, doc_off, dm, d1, ids, out_off);
+}
+
+extern "C" {
+
+static sdb_status collect_batch_call(sdb_graph* g, const sdb_hop_filter* filter, const uint32_t* start, uint64_t n_start,
+                                     const uint64_t* doc_off, uint64_t n_docs, uint32_t min_depth, uint32_t max_depth,
+                                     int inclusive, uint32_t** out_ids, uint64_t* out_doc_off, uint64_t* out_n) {
+  Ctx* ctx = g->ctx;
+  std::lock_guard<std::mutex> guard(ctx->mu);
+  SDB_CUDA(cudaSetDevice(ctx->device));
+  cudaStream_t st = ctx->stream;
+  if (!g->targets_in_rows) {
+    set_error("graph collect batch: this CSR has targets outside its own rows (an edge table into another node table); "
+              "+collect needs source and target ids in one id space");
+    return SDB_EINVAL;
+  }
+  for (uint64_t i = 0; i < n_start; i++)
+    if (start[i] >= g->n_rows) {
+      set_error("graph collect batch: start id out of range");
+      return SDB_EINVAL;
+    }
+  std::vector<AsyncBuf<uint32_t>> bits;
+  std::vector<HopFilter> d_filter;
+  sdb_graph* graphs[1] = {g};
+  if (filter) SDB_TRY(upload_filters(graphs, filter, 1, &bits, &d_filter, st));
+  g->table_peak_bytes = 0;
+  g->table_grows = g->table_repeats = g->collect_splits = 0;
+  const CollectArgs args{g, filter && has_filter(&d_filter[0]) ? &d_filter[0] : nullptr, min_depth, max_depth, inclusive, st};
+  std::vector<uint32_t> ids;
+  SDB_TRY(collect_split(args, start, doc_off, 0, n_docs, &ids, out_doc_off));
+  if (!ids.empty()) {
+    uint32_t* h_out = (uint32_t*)malloc(sizeof(uint32_t) * ids.size());
+    if (!h_out) return SDB_ENOMEM;
+    memcpy(h_out, ids.data(), sizeof(uint32_t) * ids.size());
+    *out_ids = h_out;
+    *out_n = ids.size();
+  }
+  return SDB_OK;
+}
+
+sdb_status sdb_graph_collect_batch(sdb_graph* g, const sdb_hop_filter* filter, const uint32_t* start, uint64_t n_start,
+                                   const uint64_t* doc_off, uint64_t n_docs, uint32_t min_depth, uint32_t max_depth,
+                                   int inclusive, uint32_t** out_ids, uint64_t* out_doc_off, uint64_t* out_n) {
+  if (!g || !out_ids || !out_n || !doc_off || !out_doc_off || (n_start && !start)) return SDB_EINVAL;
+  *out_ids = nullptr;
+  *out_n = 0;
+  if (filter) SDB_TRY(check_filtered(g, filter, "sdb_graph_collect_batch"));
+  SDB_TRY(check_doc_off(doc_off, n_docs, n_start, "sdb_graph_collect_batch"));
+  return collect_batch_call(g, filter, start, n_start, doc_off, n_docs, min_depth, max_depth, inclusive, out_ids,
+                            out_doc_off, out_n);
+}
+
+void sdb_graph_last_collect_table(const sdb_graph* g, uint64_t* peak_bytes, uint32_t* grows, uint32_t* repeated_passes,
+                                  uint32_t* splits) {
+  uint64_t b = 0;
+  uint32_t n[3] = {0, 0, 0};
+  if (g) {
+    std::lock_guard<std::mutex> guard(g->ctx->mu);  // sdb_graph_collect_batch writes them under the same lock
+    b = g->table_peak_bytes;
+    n[0] = g->table_grows, n[1] = g->table_repeats, n[2] = g->collect_splits;
+  }
+  if (peak_bytes) *peak_bytes = b;
+  if (grows) *grows = n[0];
+  if (repeated_passes) *repeated_passes = n[1];
+  if (splits) *splits = n[2];
 }
 
 }  // extern "C"

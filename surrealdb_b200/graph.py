@@ -11,6 +11,9 @@
   GraphStore.lookup_filtered / collect_filtered / recurse_filtered
                       the same with WHERE conditions on the edge and target records, evaluated into bitmaps
                       (hop_masks) for sdb_graph_expand_filtered / sdb_graph_collect_filtered
+  GraphStore.lookup_batch / collect_batch
+                      LookupPart::evaluate_batch (exec/parts/lookup.rs:96-112): lookup / collect of every row of a
+                      ValueBatch, optionally filtered, in one sdb_graph_expand_batch / sdb_graph_collect_batch call
   GraphEdgeScan       the operator itself: new(input, direction, edge_tables, output_mode, version).with_limit(n)
                       (exec/operators/scan/graph.rs:89-147) -- name(), attrs(), execute()
 """
@@ -171,6 +174,74 @@ def collect_filtered(graph, filt, start, min_depth=1, max_depth=0, inclusive=Fal
     return _take(out, n)
 
 
+def _docs(docs):
+    """a batch of documents: a list of per-document id arrays, or (ids, doc_off) -> (ids uint32, doc_off uint64)"""
+    if isinstance(docs, tuple):
+        ids, off = docs
+        return np.ascontiguousarray(ids, np.uint32), np.ascontiguousarray(off, np.uint64)
+    parts = [np.asarray(d, np.uint32).ravel() for d in docs]
+    off = np.zeros(len(parts) + 1, np.uint64)
+    off[1:] = np.cumsum([p.size for p in parts], dtype=np.uint64)
+    ids = np.concatenate(parts) if parts else np.zeros(0, np.uint32)
+    return np.ascontiguousarray(ids, np.uint32), off
+
+
+def _split(ids, off):
+    return [ids[int(off[d]):int(off[d + 1])] for d in range(off.size - 1)]
+
+
+def _ptr(a):
+    return C.c_void_p(a.ctypes.data) if a.size else None
+
+
+def expand_batch(hops, docs, per_source_limit=0, filters=None):
+    """sdb_graph_expand_batch: expand() of every document of the batch in one call.  docs: a list of per-document id
+    arrays or (ids, doc_off); filters: None or, per hop, as in expand_filtered.  -> one array per document"""
+    ids, off = _docs(docs)
+    arr = (C.c_void_p * len(hops))(*[g.h for g in hops])
+    farr, _keep = _filters(filters, len(hops), False) if filters is not None else (None, None)
+    out, n = C.c_void_p(), C.c_uint64()
+    out_off = np.zeros(off.size, np.uint64)
+    L.check(L.lib().sdb_graph_expand_batch(arr, farr, len(hops), _ptr(ids), ids.size, C.c_void_p(off.ctypes.data),
+                                           off.size - 1, int(per_source_limit), C.byref(out),
+                                           C.c_void_p(out_off.ctypes.data), C.byref(n)))
+    return _split(_take(out, n), out_off)
+
+
+def expand_batch_device(ctx, hops, d_frontier, n_frontier, d_doc_off, n_docs, d_out_doc_off, per_source_limit=0,
+                        filters=None):
+    """sdb_graph_expand_batch_device: frontier, doc_off (n_docs + 1 uint64), the bitmaps and the result in HBM; the
+    result's boundaries are written to d_out_doc_off (n_docs + 1 uint64).  -> (device pointer (int), count); free with
+    device_free(ctx, ptr)."""
+    arr = (C.c_void_p * len(hops))(*[g.h for g in hops])
+    farr, _keep = _filters(filters, len(hops), True) if filters is not None else (None, None)
+    out, n = C.c_void_p(), C.c_uint64()
+    L.check(L.lib().sdb_graph_expand_batch_device(arr, farr, len(hops), C.c_void_p(d_frontier), int(n_frontier),
+                                                  C.c_void_p(d_doc_off), int(n_docs), int(per_source_limit), C.byref(out),
+                                                  C.c_void_p(d_out_doc_off), C.byref(n)))
+    return (out.value or 0), n.value
+
+
+def collect_batch(graph, docs, min_depth=1, max_depth=0, inclusive=False, filt=None):
+    """sdb_graph_collect_batch: collect() of every document's start ids, each with its own first-seen set, in one
+    call; filt: None or (edge_bits, target_bits) as in collect_filtered.  -> one array per document"""
+    ids, off = _docs(docs)
+    farr, _keep = _filters([filt], 1, False) if filt is not None else (None, None)
+    out, n = C.c_void_p(), C.c_uint64()
+    out_off = np.zeros(off.size, np.uint64)
+    L.check(L.lib().sdb_graph_collect_batch(graph.h, farr, _ptr(ids), ids.size, C.c_void_p(off.ctypes.data), off.size - 1,
+                                            int(min_depth), int(max_depth), int(bool(inclusive)), C.byref(out),
+                                            C.c_void_p(out_off.ctypes.data), C.byref(n)))
+    return _split(_take(out, n), out_off)
+
+
+def last_collect_table(graph):
+    """diagnostics of the last collect_batch on this graph: {peak_bytes, grows, repeated_passes, splits}"""
+    b, g, r, s = C.c_uint64(), C.c_uint32(), C.c_uint32(), C.c_uint32()
+    L.lib().sdb_graph_last_collect_table(graph.h, C.byref(b), C.byref(g), C.byref(r), C.byref(s))
+    return {"peak_bytes": b.value, "grows": g.value, "repeated_passes": r.value, "splits": s.value}
+
+
 def _key_order(rid_key):
     """storekey order of a RecordIdKey (val/record_id.rs:181-192): numbers (numeric) before strings (bytes)"""
     if isinstance(rid_key, (int, np.integer)):
@@ -307,6 +378,28 @@ class GraphStore:
         masks = self.hop_masks(edge_table, direction, edge_pred, target_pred)
         return self.to_names(collect_filtered(self.csr(edge_table, direction), masks, self.ids([start]), min_depth,
                                               max_depth, inclusive))
+
+    def lookup_batch(self, docs, hops, limit=0):
+        """LookupPart::evaluate_batch (exec/parts/lookup.rs:96-112): docs = one list of record ids per row; hops =
+        [(direction, edge_table), ...] or [(direction, edge_table, edge_pred | None, target_pred | None), ...] ->
+        per row its record ids, as lookup / lookup_filtered returns them, from one batch call"""
+        graphs = [self.csr(h[1], h[0]) for h in hops]
+        filters = None
+        if any(len(h) > 2 and (h[2] is not None or h[3] is not None) for h in hops):
+            filters = [self.hop_masks(h[1], h[0], h[2], h[3]) if len(h) > 2 else None for h in hops]
+        out = expand_batch(graphs, [self.ids(d) for d in docs], limit, filters)
+        return [self.to_names(o) for o in out]
+
+    def collect_batch(self, docs, direction, edge_table, edge_pred=None, target_pred=None, min_depth=1, max_depth=0,
+                      inclusive=False):
+        """`.{min..max+collect}` per row: docs = one list of start record ids per row -> per row its collected record
+        ids, as collect / collect_filtered returns them, from one batch call"""
+        filt = None
+        if edge_pred is not None or target_pred is not None:
+            filt = self.hop_masks(edge_table, direction, edge_pred, target_pred)
+        out = collect_batch(self.csr(edge_table, direction), [self.ids(d) for d in docs], min_depth, max_depth, inclusive,
+                            filt)
+        return [self.to_names(o) for o in out]
 
     def recurse_filtered(self, start, direction, edge_table, edge_pred, target_pred, min_depth, max_depth):
         """default recursion over the filtered hop"""
