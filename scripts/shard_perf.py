@@ -22,9 +22,7 @@ stream = torch.cuda.ExternalStream(ctx.stream(), device=dev)
 torch.cuda.synchronize()
 
 
-def run(label, env=None, schedule=True, screen="AUTO", depth=2):
-    for kk, vv in (env or {}).items():
-        os.environ[kk] = vv
+def run(label, schedule=True, screen="AUTO", depth=2):
     col.set_schedule(schedule)
     col.set_screen(screen)
     def loop(first, last, stats):
@@ -51,12 +49,9 @@ def run(label, env=None, schedule=True, screen="AUTO", depth=2):
     scr = np.mean([s["screen_ms"] for s in st]); tot = np.mean([s["total_ms"] for s in st])
     print(f"{label:34s} step {best:7.3f} ms  lib_total {tot:6.3f}  screen {scr:6.3f}  tail {tot-scr:6.3f}  surv/q {np.mean([s['n_survivors'] for s in st])/nq:7.1f}"
           f"  rerank/q {np.mean([s['n_reranked'] for s in st])/nq:6.1f}  passes {st[-1]['n_passes']} fb {sum(s['n_fallback'] for s in st)}", flush=True)
-    for kk in (env or {}):
-        os.environ.pop(kk, None)
 
 
 run("streaming, 2 streams (default)")
-run("one stream", env={"SDB_ONE_STREAM": "1"})
 run("2 streams depth 3", depth=3)
 run("2 streams depth 1", depth=1)
 run("multipass", schedule=False)

@@ -646,10 +646,17 @@ static Ticket* find_ticket(Corpus* c, uint32_t id) {
     if (t.busy && t.id == id) return &t;
   return nullptr;
 }
-static Ticket* free_ticket(Corpus* c) {
+Ticket* claim_ticket(Corpus* c) {
   for (Ticket& t : c->tickets)
     if (!t.busy) return &t;
+  set_error("too many batches in flight (%d): call the matching wait first", N_TICKETS);
   return nullptr;
+}
+static void release_ticket(Ticket& t) {
+  t.busy = false;
+  t.h_out_rows = nullptr;
+  t.h_out_dist = nullptr;
+  t.h_out_count = nullptr;
 }
 
 // filtered batch (submit_locked, sdb_debug_screen_batch_filtered): the per query filter index on the host (exact
@@ -678,10 +685,11 @@ static void plan_filtered(const Corpus* c, Ticket& t, uint32_t nq, uint32_t k, c
   t.n_direct = (uint32_t)dir->size();
 }
 
+// the batch itself, on a ticket that submit_call has prepared and whose inputs it has staged
 static sdb_status submit_locked(Corpus* c, Ticket* t, const double* d_queries, uint32_t nq, uint32_t k, uint64_t row_base,
                                 uint64_t* d_out_rows, double* d_out_dist, uint32_t* d_out_count,
-                                const volatile int* cancel, const uint32_t* d_filters = nullptr,
-                                const uint32_t* query_filter = nullptr, const uint64_t* filter_rows = nullptr) {
+                                const volatile int* cancel, const uint32_t* d_filters, const uint32_t* query_filter,
+                                const uint64_t* filter_rows) {
   if (!c->finalized) {
     set_error("corpus not finalized (call sdb_corpus_finalize after the last append)");
     return SDB_EINVAL;
@@ -690,11 +698,8 @@ static sdb_status submit_locked(Corpus* c, Ticket* t, const double* d_queries, u
     set_error("query cancelled");
     return SDB_ECANCELLED;
   }
-  SDB_TRY(ticket_prepare(c, *t, nq ? nq : 1));
   {  // slot parity picks the stream and the scratch set: consecutive batches overlap (screen of i+1 || tail of i)
-    const int slot = (int)(t - c->tickets);
-    const bool one_stream = getenv("SDB_ONE_STREAM") != nullptr;  // (A/B knob)
-    t->set = one_stream ? 0 : (slot & 1);
+    t->set = (int)(t - c->tickets) & 1;
     t->stream = t->set ? c->ctx->stream2 : c->ctx->stream;
     if (t->wait_h2d) SDB_CUDA(cudaStreamWaitEvent(t->stream, t->ev_h2d, 0));
     t->wait_h2d = false;
@@ -779,60 +784,11 @@ static sdb_status wait_locked(Corpus* c, Ticket* t) {
     }
   }
   if (rc == SDB_OK) rc = finish_stats(c, *t, n_fb);
-  t->busy = false;
-  t->h_out_rows = nullptr;
-  t->h_out_dist = nullptr;
-  t->h_out_count = nullptr;
+  release_ticket(*t);
   return rc;
 }
 
-}  // namespace sdb
-extern "C" {  // (defined with the entry points below)
-static sdb_status check_filters(uint32_t nq, const uint32_t* filters, uint32_t n_filters, const uint32_t* query_filter);
-static sdb_status stage_filters(sdb::Corpus* c, sdb::Ticket& t, const sdb::RowFilters& rf, bool host, uint32_t nq,
-                                const uint32_t** bits, std::vector<uint64_t>* rows);
-}
-namespace sdb {
-
 // ---- hooks for comm.cu (sharded search).  The caller holds c->mu. ---------------------------------------------------
-// rf: the call's global bitmaps (rf.bits == nullptr: unfiltered), host memory with h_queries, else device memory
-sdb_status knn_submit_for_shard(Corpus* c, const double* d_queries, const double* h_queries, uint32_t nq, uint32_t k,
-                                const RowFilters& rf, uint64_t* d_out_rows, double* d_out_dist, uint32_t* d_out_count,
-                                int* slot_index, uint32_t* ticket, const double** d_queries_used) {
-  if (rf.bits) {  // refused before anything is enqueued
-    SDB_TRY(check_filters(nq, rf.bits, rf.n_filters, rf.query_filter));
-    if (c->row_base + c->n > rf.n_rows_total) {
-      set_error("sharded filtered KNN: shard rows %llu..%llu outside the bitmaps' %llu rows",
-                (unsigned long long)c->row_base, (unsigned long long)(c->row_base + c->n),
-                (unsigned long long)rf.n_rows_total);
-      return SDB_EINVAL;
-    }
-  }
-  Ticket* t = free_ticket(c);
-  if (!t) {
-    set_error("too many batches in flight (%d): call the matching wait first", N_TICKETS);
-    return SDB_EOVERFLOW;
-  }
-  *slot_index = (int)(t - c->tickets);
-  SDB_TRY(ticket_prepare(c, *t, nq));
-  cudaStream_t cs = c->ctx->copy_stream;
-  if (h_queries) {  // host queries: staged through the slot's device buffer on the copy stream
-    const size_t need_q = (size_t)nq * c->dim;
-    SDB_CUDA(t->d_in_q.reserve(need_q));
-    SDB_CUDA(cudaMemcpyAsync(t->d_in_q, h_queries, sizeof(double) * need_q, cudaMemcpyHostToDevice, cs));
-    d_queries = t->d_in_q;
-  }
-  const uint32_t* bits = nullptr;
-  std::vector<uint64_t> rows_per_filter;
-  if (rf.bits) SDB_TRY(stage_filters(c, *t, rf, h_queries != nullptr, nq, &bits, &rows_per_filter));
-  t->wait_h2d = h_queries || rf.bits;
-  if (t->wait_h2d) SDB_CUDA(cudaEventRecord(t->ev_h2d, cs));
-  SDB_TRY(submit_locked(c, t, d_queries, nq, k, c->row_base, d_out_rows, d_out_dist, d_out_count, nullptr, bits,
-                        rf.query_filter, rf.bits ? rows_per_filter.data() : nullptr));
-  *ticket = t->id;
-  *d_queries_used = d_queries;
-  return SDB_OK;
-}
 void knn_trace_mark(Corpus* c, uint32_t ticket, const char* name) {
   Ticket* t = find_ticket(c, ticket);
   if (t) trace_mark(c->ctx, *t, name, t->stream);
@@ -851,10 +807,7 @@ sdb_status knn_finish_for_shard(Corpus* c, uint32_t ticket, bool* repaired) {
 sdb_status knn_release_ticket(Corpus* c, uint32_t ticket) {
   Ticket* t = find_ticket(c, ticket);
   if (!t) return SDB_EINVAL;
-  t->busy = false;
-  t->h_out_rows = nullptr;
-  t->h_out_dist = nullptr;
-  t->h_out_count = nullptr;
+  release_ticket(*t);
   return SDB_OK;
 }
 // a permuted batch's counters: queries flagged by both sub-batches, the rest as the direct sub-batch left them
@@ -1338,22 +1291,7 @@ sdb_status sdb_knn_last_stats(const sdb_corpus* c, sdb_knn_stats* out) {
   return SDB_OK;
 }
 
-// ---- asynchronous batches ------------------------------------------------------------------------------------------
-sdb_status sdb_knn_submit_device(sdb_corpus* c, const double* d_queries, uint32_t nq, uint32_t k, uint64_t row_base,
-                                 uint64_t* d_out_rows, double* d_out_dist, uint32_t* d_out_count, uint32_t* ticket) {
-  if (!c || !ticket || (nq && (!d_queries || !d_out_count || (k && (!d_out_rows || !d_out_dist))))) return SDB_EINVAL;
-  std::lock_guard<std::mutex> g(c->mu);
-  SDB_CUDA(cudaSetDevice(c->ctx->device));
-  Ticket* t = free_ticket(c);
-  if (!t) {
-    set_error("too many batches in flight (%d): call sdb_knn_wait first", N_TICKETS);
-    return SDB_EOVERFLOW;
-  }
-  SDB_TRY(submit_locked(c, t, d_queries, nq, k, row_base, d_out_rows, d_out_dist, d_out_count, nullptr));
-  *ticket = t->id;
-  return SDB_OK;
-}
-
+// ---- staging of a batch's inputs -----------------------------------------------------------------------------------
 // per filter used by the batch, on the host, as far as the two decisions need it, over the bits [first, first + n_rows)
 // of bitmaps of `words` words (a shard's rows of global bitmaps; unsharded calls: 0 and the corpus' rows): the exact
 // number of set bits while it is at most DIRECT_MAX_ROWS (direct regime; the count stops at the first bit beyond, after
@@ -1423,6 +1361,23 @@ __global__ void slice_filter_rows_kernel(const uint32_t* __restrict__ src, uint6
   }
 }
 
+}  // extern "C"
+namespace sdb {
+
+sdb_status check_filters(uint32_t nq, const uint32_t* filters, uint32_t n_filters, const uint32_t* query_filter) {
+  if (nq && (n_filters == 0 || !filters)) {
+    set_error("filtered KNN: %s", n_filters == 0 ? "no filter given (n_filters == 0)" : "filters is NULL");
+    return SDB_EINVAL;
+  }
+  if (query_filter)
+    for (uint32_t q = 0; q < nq; q++)
+      if (query_filter[q] >= n_filters) {
+        set_error("filtered KNN: query %u uses filter %u of %u", q, query_filter[q], n_filters);
+        return SDB_EINVAL;
+      }
+  return SDB_OK;
+}
+
 // The bitmaps of a filtered batch as its kernels read them (*bits: ceil(c->n / 32) words per filter, bit r = the
 // corpus' row r) and the set bits of each for plan_filtered (*rows), enqueued on the copy stream, which carries no batch.
 //   unsharded call: host bitmaps are copied whole into the slot's d_in_filt; device bitmaps are read in place
@@ -1430,7 +1385,7 @@ __global__ void slice_filter_rows_kernel(const uint32_t* __restrict__ src, uint6
 //     (host bitmaps: one strided copy into d_in_span), and slice_filter_rows_kernel shifts it into d_in_filt
 // Host bitmaps are counted on the host.  Device bitmaps are counted on the device, and the host waits for that count
 // alone -- an event on the copy stream, never a batch stream, so a batch in flight keeps running.  The caller records
-// ev_h2d on the copy stream afterwards; submit_locked makes the batch's stream wait for it.
+// ev_h2d on the copy stream afterwards; the batch's stream waits for it.
 static sdb_status stage_filters(Corpus* c, Ticket& t, const RowFilters& rf, bool host, uint32_t nq,
                                 const uint32_t** bits, std::vector<uint64_t>* rows) {
   cudaStream_t cs = c->ctx->copy_stream;
@@ -1488,39 +1443,67 @@ static sdb_status stage_filters(Corpus* c, Ticket& t, const RowFilters& rf, bool
   return SDB_OK;
 }
 
-static sdb_status submit_host_locked(sdb_corpus* c, const double* queries, uint32_t nq, uint32_t k, uint64_t* out_rows,
-                                     double* out_dist, uint32_t* out_count, const volatile int* cancel, Ticket** out_t,
-                                     const RowFilters& rf = RowFilters()) {
-  Ticket* t = free_ticket(c);
-  if (!t) {
-    set_error("too many batches in flight (%d): call sdb_knn_wait first", N_TICKETS);
-    return SDB_EOVERFLOW;
-  }
-  SDB_TRY(ticket_prepare(c, *t, nq));
-  SDB_CUDA(t->d_in_q.reserve((size_t)nq * c->dim));
-  SDB_CUDA(t->res.reserve((size_t)nq * (k ? k : 1), nq));
-  // the queries travel on the copy stream, so the transfer of batch i+1 overlaps the kernels of batch i
+sdb_status submit_call(Corpus* c, Ticket* t, uint32_t nq, uint32_t k, const KnnCall& call) {
+  SDB_TRY(ticket_prepare(c, *t, nq ? nq : 1));
+  // host inputs travel on the copy stream, so the transfer of batch i+1 overlaps the kernels of batch i
   cudaStream_t cs = c->ctx->copy_stream;
-  SDB_CUDA(cudaMemcpyAsync(t->d_in_q, queries, sizeof(double) * (size_t)nq * c->dim, cudaMemcpyHostToDevice, cs));
-  const uint32_t* bits = nullptr;  // ... and so do the row filters, into the slot's own copy
+  const double* d_queries = call.queries;
+  if (call.host_in) {
+    SDB_CUDA(t->d_in_q.reserve((size_t)nq * c->dim));
+    SDB_CUDA(cudaMemcpyAsync(t->d_in_q, call.queries, sizeof(double) * (size_t)nq * c->dim, cudaMemcpyHostToDevice, cs));
+    d_queries = t->d_in_q;
+  }
+  const uint32_t* bits = nullptr;
   std::vector<uint64_t> rows_per_filter;
-  if (rf.bits) SDB_TRY(stage_filters(c, *t, rf, true, nq, &bits, &rows_per_filter));
-  SDB_CUDA(cudaEventRecord(t->ev_h2d, cs));
-  t->wait_h2d = true;  // submit_locked makes the batch's stream wait for the transfer
-  SDB_TRY(submit_locked(c, t, t->d_in_q, nq, k, c->row_base, t->res.rows, t->res.dist, t->res.count, cancel, bits,
-                        rf.query_filter, rf.bits ? rows_per_filter.data() : nullptr));
-  t->h_out_rows = out_rows;
-  t->h_out_dist = out_dist;
-  t->h_out_count = out_count;
+  if (call.rf.bits) SDB_TRY(stage_filters(c, *t, call.rf, call.host_in, nq, &bits, &rows_per_filter));
+  t->wait_h2d = call.host_in || call.rf.bits;
+  if (t->wait_h2d) SDB_CUDA(cudaEventRecord(t->ev_h2d, cs));
+  uint64_t* d_rows = call.out_rows;
+  double* d_dist = call.out_dist;
+  uint32_t* d_count = call.out_count;
+  if (call.host_out) {
+    SDB_CUDA(t->res.reserve((size_t)nq * (k ? k : 1), nq));
+    d_rows = t->res.rows;
+    d_dist = t->res.dist;
+    d_count = t->res.count;
+  }
+  SDB_TRY(submit_locked(c, t, d_queries, nq, k, call.row_base, d_rows, d_dist, d_count, call.cancel, bits,
+                        call.rf.query_filter, call.rf.bits ? rows_per_filter.data() : nullptr));
+  if (!call.host_out) return SDB_OK;
+  t->h_out_rows = call.out_rows;
+  t->h_out_dist = call.out_dist;
+  t->h_out_count = call.out_count;
   const sdb_status rc = copy_out(c, *t);
   if (rc != SDB_OK) {
     cudaStreamSynchronize(t->stream);
-    t->busy = false;
-    return rc;
+    release_ticket(*t);
   }
-  *out_t = t;
+  return rc;
+}
+
+// the sdb_knn_{bruteforce,submit}* entry points after their own argument checks: one batch, then its wait (blocking
+// calls: ticket == nullptr) or its ticket id
+static sdb_status knn_call(Corpus* c, uint32_t nq, uint32_t k, const KnnCall& call, uint32_t* ticket) {
+  std::lock_guard<std::mutex> g(c->mu);
+  SDB_CUDA(cudaSetDevice(c->ctx->device));
+  Ticket* t = claim_ticket(c);
+  if (!t) return SDB_EOVERFLOW;
+  SDB_TRY(submit_call(c, t, nq, k, call));
+  if (!ticket) return wait_locked(c, t);
+  *ticket = t->id;
   return SDB_OK;
 }
+static KnnCall host_call(Corpus* c, const double* queries, const RowFilters& rf, uint64_t* out_rows, double* out_dist,
+                         uint32_t* out_count, const volatile int* cancel) {
+  return KnnCall{queries, true, rf, c->row_base, out_rows, out_dist, out_count, true, cancel};
+}
+static KnnCall device_call(const double* d_queries, const RowFilters& rf, uint64_t row_base, uint64_t* d_out_rows,
+                           double* d_out_dist, uint32_t* d_out_count) {
+  return KnnCall{d_queries, false, rf, row_base, d_out_rows, d_out_dist, d_out_count, false, nullptr};
+}
+
+}  // namespace sdb
+extern "C" {
 
 // Host-only diagnostic (no GPU needed): the corpus tiles (TILE_ROWS rows each) a screened search visits, in order.
 // Every row that is not visited can never become a candidate and the exactness proof would not know, so "every tile
@@ -1642,11 +1625,8 @@ sdb_status sdb_debug_screen_batch_filtered(sdb_corpus* c, const double* queries,
   Ctx* ctx = c->ctx;
   SDB_CUDA(cudaSetDevice(ctx->device));
   SDB_CUDA(drain(ctx));
-  Ticket* t = free_ticket(c);
-  if (!t) {
-    set_error("too many batches in flight (%d): call sdb_knn_wait first", N_TICKETS);
-    return SDB_EOVERFLOW;
-  }
+  Ticket* t = claim_ticket(c);
+  if (!t) return SDB_EOVERFLOW;
   SDB_TRY(ticket_prepare(c, *t, nq));
   const uint64_t n_pad = (c->n + TILE_ROWS - 1) / TILE_ROWS * TILE_ROWS;
   const uint32_t cap = score_all ? (uint32_t)std::max<uint64_t>(cand_cap, n_pad) : cand_cap;
@@ -1660,13 +1640,13 @@ sdb_status sdb_debug_screen_batch_filtered(sdb_corpus* c, const double* queries,
   t->n_direct = 0;
   t->permuted = false;
   if (filters) {
-    const size_t words = (size_t)n_filters * ((c->n + 31) / 32);
-    SDB_CUDA(t->d_in_filt.reserve(words));
-    SDB_CUDA(cudaMemcpyAsync(t->d_in_filt, filters, sizeof(uint32_t) * words, cudaMemcpyHostToDevice, st));
-    const std::vector<uint64_t> rows_per_filter =
-        count_filter_rows_host(filters, (c->n + 31) / 32, 0, c->n, n_filters, query_filter, nq);
+    const uint32_t* bits = nullptr;
+    std::vector<uint64_t> rows_per_filter;
+    SDB_TRY(stage_filters(c, *t, RowFilters{filters, n_filters, query_filter, 0}, true, nq, &bits, &rows_per_filter));
+    SDB_CUDA(cudaEventRecord(t->ev_h2d, ctx->copy_stream));
+    SDB_CUDA(cudaStreamWaitEvent(st, t->ev_h2d, 0));
     std::vector<uint32_t> scr, dir;
-    plan_filtered(c, *t, nq, k, t->d_in_filt, query_filter, rows_per_filter.data(), &scr, &dir);
+    plan_filtered(c, *t, nq, k, bits, query_filter, rows_per_filter.data(), &scr, &dir);
     if (!score_all && !scr.empty() && !dir.empty()) {
       t->filt = FiltArg();
       t->n_direct = 0;
@@ -1811,12 +1791,13 @@ sdb_status sdb_debug_screen_batch_filtered(sdb_corpus* c, const double* queries,
 sdb_status sdb_knn_submit(sdb_corpus* c, const double* queries, uint32_t nq, uint32_t k, uint64_t* out_rows,
                           double* out_dist, uint32_t* out_count, uint32_t* ticket) {
   if (!c || !ticket || !nq || !queries || !out_count || (k && (!out_rows || !out_dist))) return SDB_EINVAL;
-  std::lock_guard<std::mutex> g(c->mu);
-  SDB_CUDA(cudaSetDevice(c->ctx->device));
-  Ticket* t = nullptr;
-  SDB_TRY(submit_host_locked(c, queries, nq, k, out_rows, out_dist, out_count, nullptr, &t));
-  *ticket = t->id;
-  return SDB_OK;
+  return knn_call(c, nq, k, host_call(c, queries, RowFilters(), out_rows, out_dist, out_count, nullptr), ticket);
+}
+
+sdb_status sdb_knn_submit_device(sdb_corpus* c, const double* d_queries, uint32_t nq, uint32_t k, uint64_t row_base,
+                                 uint64_t* d_out_rows, double* d_out_dist, uint32_t* d_out_count, uint32_t* ticket) {
+  if (!c || !ticket || (nq && (!d_queries || !d_out_count || (k && (!d_out_rows || !d_out_dist))))) return SDB_EINVAL;
+  return knn_call(c, nq, k, device_call(d_queries, RowFilters(), row_base, d_out_rows, d_out_dist, d_out_count), ticket);
 }
 
 sdb_status sdb_knn_wait(sdb_corpus* c, uint32_t ticket) {
@@ -1836,15 +1817,7 @@ sdb_status sdb_knn_bruteforce_device(sdb_corpus* c, const double* d_queries, uin
                                      uint32_t* d_out_count) {
   if (!c || (nq && (!d_queries || !d_out_count || (k && (!d_out_rows || !d_out_dist))))) return SDB_EINVAL;
   if (nq == 0) return SDB_OK;
-  std::lock_guard<std::mutex> g(c->mu);
-  SDB_CUDA(cudaSetDevice(c->ctx->device));
-  Ticket* t = free_ticket(c);
-  if (!t) {
-    set_error("too many batches in flight (%d): call sdb_knn_wait first", N_TICKETS);
-    return SDB_EOVERFLOW;
-  }
-  SDB_TRY(submit_locked(c, t, d_queries, nq, k, row_base, d_out_rows, d_out_dist, d_out_count, nullptr));
-  return wait_locked(c, t);
+  return knn_call(c, nq, k, device_call(d_queries, RowFilters(), row_base, d_out_rows, d_out_dist, d_out_count), nullptr);
 }
 
 sdb_status sdb_knn_bruteforce(sdb_corpus* c, const double* queries, uint32_t nq, uint32_t k, uint64_t* out_rows,
@@ -1855,28 +1828,10 @@ sdb_status sdb_knn_bruteforce(sdb_corpus* c, const double* queries, uint32_t nq,
     set_error("query cancelled");
     return SDB_ECANCELLED;
   }
-  std::lock_guard<std::mutex> g(c->mu);
-  SDB_CUDA(cudaSetDevice(c->ctx->device));
-  Ticket* t = nullptr;
-  SDB_TRY(submit_host_locked(c, queries, nq, k, out_rows, out_dist, out_count, cancel_flag, &t));
-  return wait_locked(c, t);
+  return knn_call(c, nq, k, host_call(c, queries, RowFilters(), out_rows, out_dist, out_count, cancel_flag), nullptr);
 }
 
 // ---- filtered brute-force KNN: per-query row bitmaps (see the header) ----------------------------------------------
-static sdb_status check_filters(uint32_t nq, const uint32_t* filters, uint32_t n_filters, const uint32_t* query_filter) {
-  if (nq && (n_filters == 0 || !filters)) {
-    set_error("filtered KNN: %s", n_filters == 0 ? "no filter given (n_filters == 0)" : "filters is NULL");
-    return SDB_EINVAL;
-  }
-  if (query_filter)
-    for (uint32_t q = 0; q < nq; q++)
-      if (query_filter[q] >= n_filters) {
-        set_error("filtered KNN: query %u uses filter %u of %u", q, query_filter[q], n_filters);
-        return SDB_EINVAL;
-      }
-  return SDB_OK;
-}
-
 sdb_status sdb_knn_bruteforce_filtered(sdb_corpus* c, const double* queries, uint32_t nq, uint32_t k,
                                        const uint32_t* filters, uint32_t n_filters, const uint32_t* query_filter,
                                        uint64_t* out_rows, double* out_dist, uint32_t* out_count,
@@ -1888,35 +1843,11 @@ sdb_status sdb_knn_bruteforce_filtered(sdb_corpus* c, const double* queries, uin
     set_error("query cancelled");
     return SDB_ECANCELLED;
   }
-  std::lock_guard<std::mutex> g(c->mu);
-  SDB_CUDA(cudaSetDevice(c->ctx->device));
-  Ticket* t = nullptr;
-  SDB_TRY(submit_host_locked(c, queries, nq, k, out_rows, out_dist, out_count, cancel_flag, &t,
-                             RowFilters{filters, n_filters, query_filter, 0}));
-  return wait_locked(c, t);
+  const RowFilters rf{filters, n_filters, query_filter, 0};
+  return knn_call(c, nq, k, host_call(c, queries, rf, out_rows, out_dist, out_count, cancel_flag), nullptr);
 }
 
-// device bitmaps, read in place: counted on the copy stream (stage_filters), then the batch
-static sdb_status submit_device_filtered_locked(sdb_corpus* c, const double* d_queries, uint32_t nq, uint32_t k,
-                                                const RowFilters& rf, uint64_t row_base, uint64_t* d_out_rows,
-                                                double* d_out_dist, uint32_t* d_out_count, Ticket** out_t) {
-  Ticket* t = free_ticket(c);
-  if (!t) {
-    set_error("too many batches in flight (%d): call sdb_knn_wait first", N_TICKETS);
-    return SDB_EOVERFLOW;
-  }
-  SDB_TRY(ticket_prepare(c, *t, nq ? nq : 1));
-  const uint32_t* bits = nullptr;
-  std::vector<uint64_t> rows_per_filter;
-  SDB_TRY(stage_filters(c, *t, rf, false, nq, &bits, &rows_per_filter));
-  SDB_CUDA(cudaEventRecord(t->ev_h2d, c->ctx->copy_stream));
-  t->wait_h2d = true;
-  SDB_TRY(submit_locked(c, t, d_queries, nq, k, row_base, d_out_rows, d_out_dist, d_out_count, nullptr, bits,
-                        rf.query_filter, rows_per_filter.data()));
-  *out_t = t;
-  return SDB_OK;
-}
-
+// device bitmaps are read in place: counted on the copy stream (stage_filters), then the batch
 sdb_status sdb_knn_bruteforce_filtered_device(sdb_corpus* c, const double* d_queries, uint32_t nq, uint32_t k,
                                               const uint32_t* d_filters, uint32_t n_filters,
                                               const uint32_t* query_filter, uint64_t row_base, uint64_t* d_out_rows,
@@ -1924,12 +1855,8 @@ sdb_status sdb_knn_bruteforce_filtered_device(sdb_corpus* c, const double* d_que
   if (!c || (nq && (!d_queries || !d_out_count || (k && (!d_out_rows || !d_out_dist))))) return SDB_EINVAL;
   SDB_TRY(check_filters(nq, d_filters, n_filters, query_filter));
   if (nq == 0) return SDB_OK;
-  std::lock_guard<std::mutex> g(c->mu);
-  SDB_CUDA(cudaSetDevice(c->ctx->device));
-  Ticket* t = nullptr;
-  SDB_TRY(submit_device_filtered_locked(c, d_queries, nq, k, RowFilters{d_filters, n_filters, query_filter, 0},
-                                        row_base, d_out_rows, d_out_dist, d_out_count, &t));
-  return wait_locked(c, t);
+  const RowFilters rf{d_filters, n_filters, query_filter, 0};
+  return knn_call(c, nq, k, device_call(d_queries, rf, row_base, d_out_rows, d_out_dist, d_out_count), nullptr);
 }
 
 sdb_status sdb_knn_submit_filtered_device(sdb_corpus* c, const double* d_queries, uint32_t nq, uint32_t k,
@@ -1938,13 +1865,8 @@ sdb_status sdb_knn_submit_filtered_device(sdb_corpus* c, const double* d_queries
                                           uint32_t* d_out_count, uint32_t* ticket) {
   if (!c || !ticket || (nq && (!d_queries || !d_out_count || (k && (!d_out_rows || !d_out_dist))))) return SDB_EINVAL;
   SDB_TRY(check_filters(nq, d_filters, n_filters, query_filter));
-  std::lock_guard<std::mutex> g(c->mu);
-  SDB_CUDA(cudaSetDevice(c->ctx->device));
-  Ticket* t = nullptr;
-  SDB_TRY(submit_device_filtered_locked(c, d_queries, nq, k, RowFilters{d_filters, n_filters, query_filter, 0},
-                                        row_base, d_out_rows, d_out_dist, d_out_count, &t));
-  *ticket = t->id;
-  return SDB_OK;
+  const RowFilters rf{d_filters, n_filters, query_filter, 0};
+  return knn_call(c, nq, k, device_call(d_queries, rf, row_base, d_out_rows, d_out_dist, d_out_count), ticket);
 }
 
 sdb_status sdb_knn_submit_filtered(sdb_corpus* c, const double* queries, uint32_t nq, uint32_t k,
@@ -1952,13 +1874,8 @@ sdb_status sdb_knn_submit_filtered(sdb_corpus* c, const double* queries, uint32_
                                    uint64_t* out_rows, double* out_dist, uint32_t* out_count, uint32_t* ticket) {
   if (!c || !ticket || !nq || !queries || !out_count || (k && (!out_rows || !out_dist))) return SDB_EINVAL;
   SDB_TRY(check_filters(nq, filters, n_filters, query_filter));
-  std::lock_guard<std::mutex> g(c->mu);
-  SDB_CUDA(cudaSetDevice(c->ctx->device));
-  Ticket* t = nullptr;
-  SDB_TRY(submit_host_locked(c, queries, nq, k, out_rows, out_dist, out_count, nullptr, &t,
-                             RowFilters{filters, n_filters, query_filter, 0}));
-  *ticket = t->id;
-  return SDB_OK;
+  const RowFilters rf{filters, n_filters, query_filter, 0};
+  return knn_call(c, nq, k, host_call(c, queries, rf, out_rows, out_dist, out_count, nullptr), ticket);
 }
 
 sdb_status sdb_corpus_project(sdb_corpus* c, const double* query, int fn, double* out) {

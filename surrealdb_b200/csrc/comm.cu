@@ -144,22 +144,6 @@ struct ShardSlot {  // per in-flight ticket: this rank's block, the gathered blo
 
 using namespace sdb;
 
-// the brute-force driver of api.cu
-namespace sdb {
-sdb_status knn_submit_for_shard(Corpus* c, const double* d_queries, const double* h_queries, uint32_t nq, uint32_t k,
-                                const RowFilters& rf, uint64_t* d_out_rows, double* d_out_dist, uint32_t* d_out_count,
-                                int* slot_index, uint32_t* ticket, const double** d_queries_used);
-sdb_status knn_finish_for_shard(Corpus* c, uint32_t ticket, bool* repaired);
-sdb_status knn_release_ticket(Corpus* c, uint32_t ticket);
-sdb_status knn_shard_header(Corpus* c, uint32_t ticket, void* d_hdr);
-cudaStream_t knn_ticket_stream(Corpus* c, uint32_t ticket);
-void knn_trace_mark(Corpus* c, uint32_t ticket, const char* name);
-sdb_status topk_merge_launch(Ctx* ctx, uint32_t n_lists, uint32_t nq, uint32_t k, const uint64_t* d_rows,
-                             const double* d_dist, const uint32_t* d_counts, uint64_t stride_rows, uint64_t stride_dist,
-                             uint64_t stride_counts, uint64_t* d_out_rows, double* d_out_dist, uint32_t* d_out_count,
-                             cudaStream_t st);
-}  // namespace sdb
-
 namespace {
 
 struct Arena;
@@ -485,40 +469,31 @@ static bool use_p2p(Corpus* c, ShardState* ss) {
 
 // phase A: the local search into this rank's block, header = number of queries this rank must repair on the host.
 // rf: the call's global row filters (rf.bits == nullptr: unfiltered); the driver slices this shard's rows out of them.
+// The slot's buffers belong to the batch's ticket slot, so they are free exactly when the ticket is.
 sdb_status phase_local(Corpus* c, const double* d_queries, const double* h_queries, uint32_t nq, uint32_t k,
                        const RowFilters& rf, uint64_t* d_out_rows, double* d_out_dist, uint32_t* d_out_count,
                        uint64_t* h_out_rows, double* h_out_dist, uint32_t* h_out_count, Pending* p) {
-  ShardState* ss = state_of(c);
-  const BlockLayout bl = block_layout(nq, k);
-  // the slot index follows the brute-force driver's ticket slot, so slot buffers are free exactly when the ticket is
-  int slot = -1;
-  uint32_t ticket = 0;
-  // reserve with a provisional slot: the driver tells us which ticket slot it used
-  // (buffers are per slot; reserve all lazily below)
-  const double* dq = nullptr;
-  // block pointers are only known once the slot is; the driver lets us pass them through a callback-free two-step:
-  // first pick the slot (free_ticket order is deterministic), then reserve, then submit.
-  for (int i = 0; i < N_TICKETS; i++)
-    if (!c->tickets[i].busy) {
-      slot = i;
-      break;
+  if (rf.bits) {  // refused before anything is enqueued
+    SDB_TRY(check_filters(nq, rf.bits, rf.n_filters, rf.query_filter));
+    if (c->row_base + c->n > rf.n_rows_total) {
+      set_error("sharded filtered KNN: shard rows %llu..%llu outside the bitmaps' %llu rows",
+                (unsigned long long)c->row_base, (unsigned long long)(c->row_base + c->n),
+                (unsigned long long)rf.n_rows_total);
+      return SDB_EINVAL;
     }
-  if (slot < 0) {
-    set_error("too many batches in flight (%d): call the matching wait first", N_TICKETS);
-    return SDB_EOVERFLOW;
   }
-  ShardSlot& s = ss->slots[slot];
+  Ticket* t = claim_ticket(c);
+  if (!t) return SDB_EOVERFLOW;
+  const int slot = (int)(t - c->tickets);
+  ShardSlot& s = state_of(c)->slots[slot];
+  const BlockLayout bl = block_layout(nq, k);
   const bool host_out = h_out_count != nullptr;
   SDB_TRY(slot_reserve(c, s, nq, k, host_out));
-  int used = -1;
-  SDB_TRY(knn_submit_for_shard(c, d_queries, h_queries, nq, k, rf, (uint64_t*)(s.d_block + bl.off_rows),
-                               (double*)(s.d_block + bl.off_dist), (uint32_t*)(s.d_block + bl.off_cnt), &used, &ticket,
-                               &dq));
-  if (used != slot) {
-    set_error("internal: ticket slot mismatch (%d vs %d)", used, slot);
-    return SDB_EINVAL;
-  }
-  SDB_TRY(knn_shard_header(c, ticket, s.d_block + bl.off_hdr));
+  const KnnCall call{h_queries ? h_queries : d_queries, h_queries != nullptr, rf, c->row_base,
+                     (uint64_t*)(s.d_block + bl.off_rows), (double*)(s.d_block + bl.off_dist),
+                     (uint32_t*)(s.d_block + bl.off_cnt), false, nullptr};
+  SDB_TRY(submit_call(c, t, nq, k, call));
+  SDB_TRY(knn_shard_header(c, t->id, s.d_block + bl.off_hdr));
   s.d_out_rows = host_out ? s.res.rows : d_out_rows;
   s.d_out_dist = host_out ? s.res.dist : d_out_dist;
   s.d_out_count = host_out ? s.res.count : d_out_count;
@@ -527,7 +502,7 @@ sdb_status phase_local(Corpus* c, const double* d_queries, const double* h_queri
   s.h_out_count = h_out_count;
   p->c = c;
   p->s = &s;
-  p->ticket = ticket;
+  p->ticket = t->id;
   p->nq = nq;
   p->k = k;
   p->slot = slot;

@@ -296,7 +296,7 @@ struct Ticket {
   ResultBufs res;
   cudaEvent_t ev_h2d = nullptr, ev_out = nullptr;
   cudaEvent_t ev_main = nullptr;  // recorded after this batch's last screen launch (the next batch's screen waits for it)
-  bool wait_h2d = false;  // the batch's stream still has to wait for ev_h2d (queries travelling on the copy stream)
+  bool wait_h2d = false;  // the batch's stream still has to wait for ev_h2d (inputs travelling on the copy stream)
   // filtered batches: filt.bits = the caller's device bitmaps or d_in_filt (host bitmaps staged per slot), filt.qf =
   // d_qf (per query filter index, also kept on the host in h_qf); unfiltered batches: filt.bits == nullptr
   FiltArg filt;
@@ -469,6 +469,37 @@ constexpr uint32_t COUNT_CAP_MAX = 16384;  // candidate entries per query of the
 inline bool count_ranked(const Corpus* c, uint32_t k) {
   return family(c) == Family::Count && k >= 1 && k <= 256 && c->screen != SDB_SCREEN_NONE_EXACT;
 }
+
+// ---- the brute-force driver (api.cu), as its entry points and the sharded search (comm.cu) use it ------------------
+// one batch as a caller hands it over: queries and row filters on the host (host_in) or the device; outputs on the host
+// (host_out: the batch writes the slot's res buffers and copy_out copies them) or the device
+struct KnnCall {
+  const double* queries = nullptr;
+  bool host_in = false;
+  RowFilters rf;  // rf.bits == nullptr: unfiltered; rf.n_rows_total != 0: a shard's part of global bitmaps
+  uint64_t row_base = 0;
+  uint64_t* out_rows = nullptr;
+  double* out_dist = nullptr;
+  uint32_t* out_count = nullptr;
+  bool host_out = false;
+  const volatile int* cancel = nullptr;
+};
+// a free ticket slot, or nullptr with the "too many batches in flight" error (the caller returns SDB_EOVERFLOW)
+Ticket* claim_ticket(Corpus* c);
+// stages the call's host inputs on the copy stream and enqueues the batch on the claimed ticket t; the caller holds c->mu
+sdb_status submit_call(Corpus* c, Ticket* t, uint32_t nq, uint32_t k, const KnnCall& call);
+sdb_status check_filters(uint32_t nq, const uint32_t* filters, uint32_t n_filters, const uint32_t* query_filter);
+// by ticket id, for a sharded batch: completion (ladder re-runs, exact fallbacks, statistics), release, the 16-byte
+// block header enqueued into d_hdr, the batch's stream and a trace mark on it
+sdb_status knn_finish_for_shard(Corpus* c, uint32_t ticket, bool* repaired);
+sdb_status knn_release_ticket(Corpus* c, uint32_t ticket);
+sdb_status knn_shard_header(Corpus* c, uint32_t ticket, void* d_hdr);
+cudaStream_t knn_ticket_stream(Corpus* c, uint32_t ticket);
+void knn_trace_mark(Corpus* c, uint32_t ticket, const char* name);
+sdb_status topk_merge_launch(Ctx* ctx, uint32_t n_lists, uint32_t nq, uint32_t k, const uint64_t* d_rows,
+                             const double* d_dist, const uint32_t* d_counts, uint64_t stride_rows, uint64_t stride_dist,
+                             uint64_t stride_counts, uint64_t* d_out_rows, double* d_out_dist, uint32_t* d_out_count,
+                             cudaStream_t st);
 
 // tiling shared by the f32 Lp screen (screen_lp.cu) and the count path (count.cu)
 constexpr int LP_THREADS = 256;
