@@ -100,10 +100,11 @@ struct Rung {
 // cluster on tightly packed data); a rung fails for a query only when that set overflows the list.  When that happens
 // to more than a handful of queries the batch is re-screened with a tighter screen / longer lists instead of paying
 // one exact pass over the corpus per failed query; the rung that worked is remembered per corpus and k.
-static std::vector<Rung> build_rungs(Corpus* c, uint32_t k, uint32_t nq, sdb_screen* first) {
+// screen: the corpus' screen choice (Corpus::screen, or the one a debug batch asks for)
+static std::vector<Rung> build_rungs(const Corpus* c, sdb_screen screen, uint32_t k, uint32_t nq, sdb_screen* first) {
   const Family f = family(c);
   const bool int8_ok = c->d_i8 && screen_tc_available();  // (COSINE and Centred corpora hold an int8 copy)
-  sdb_screen scr = c->screen;
+  sdb_screen scr = screen;
   if (scr == SDB_SCREEN_AUTO)
     scr = !screen_tc_available() ? SDB_SCREEN_SIMT_F32
                                  : (int8_ok && c->max_rel_qerr <= 0.02f ? SDB_SCREEN_TC_INT8 : SDB_SCREEN_TC_BF16);
@@ -119,7 +120,7 @@ static std::vector<Rung> build_rungs(Corpus* c, uint32_t k, uint32_t nq, sdb_scr
   // MANHATTAN / CHEBYSHEV: a single query streams the rows once either way, and the exact kernel does it at the higher
   // HBM rate (DESIGN.md section 5): AUTO ranks it there; an explicit SIMT_F32 request is kept.  MINKOWSKI's exact
   // kernel is bound by its f64 pow() calls, not by HBM, and the screen is faster for a single query too (section 5).
-  if (f == Family::Lp && c->metric != SDB_MINKOWSKI && nq == 1 && c->screen == SDB_SCREEN_AUTO)
+  if (f == Family::Lp && c->metric != SDB_MINKOWSKI && nq == 1 && screen == SDB_SCREEN_AUTO)
     scr = SDB_SCREEN_NONE_EXACT;
   *first = scr;
   std::vector<Rung> r;
@@ -141,12 +142,6 @@ static uint32_t n_batch_rungs(const std::vector<Rung>& r) {  // rungs a WHOLE ba
   return n;
 }
 
-// swap the ticket's scratch set into the corpus' active fields (see Scratch in internal.cuh)
-static void activate_set(Corpus* c, int set) {
-  if (c->active_set == set) return;
-  std::swap(static_cast<Scratch&>(*c), c->parked);
-  c->active_set = set;
-}
 static cudaError_t drain(Ctx* ctx) {  // both batch streams idle
   cudaError_t e = cudaStreamSynchronize(ctx->stream);
   const cudaError_t e2 = cudaStreamSynchronize(ctx->stream2);
@@ -210,28 +205,29 @@ void trace_dump(Ctx* ctx, Ticket& t) {
 }
 
 // ScreenTap (test-only): what a stage-A selection is about to gather -- main list and private sub-lists, before capping
-static sdb_status tap_gathered(Corpus* c, uint32_t nq, uint32_t n_slots, cudaStream_t st) {
+static sdb_status tap_gathered(const Scratch& s, ScreenTap* tap, uint32_t nq, uint32_t n_slots, cudaStream_t st) {
   std::vector<uint32_t> cnt(nq), sub((size_t)nq * n_slots);
-  SDB_CUDA(cudaMemcpyAsync(cnt.data(), c->d_cand_cnt, sizeof(uint32_t) * nq, cudaMemcpyDeviceToHost, st));
+  SDB_CUDA(cudaMemcpyAsync(cnt.data(), s.d_cand_cnt, sizeof(uint32_t) * nq, cudaMemcpyDeviceToHost, st));
   if (n_slots)
-    SDB_CUDA(cudaMemcpyAsync(sub.data(), c->d_sub_cnt, sizeof(uint32_t) * sub.size(), cudaMemcpyDeviceToHost, st));
+    SDB_CUDA(cudaMemcpyAsync(sub.data(), s.d_sub_cnt, sizeof(uint32_t) * sub.size(), cudaMemcpyDeviceToHost, st));
   SDB_CUDA(cudaStreamSynchronize(st));
-  std::vector<uint32_t>& g = c->tap->gathered;
+  std::vector<uint32_t>& g = tap->gathered;
   g.resize(nq, 0u);
   for (uint32_t q = 0; q < nq; q++) {
     uint64_t n = cnt[q];
-    for (uint32_t s = 0; s < n_slots; s++) n += std::min(sub[(size_t)q * n_slots + s], c->sub_cap);
+    for (uint32_t j = 0; j < n_slots; j++) n += std::min(sub[(size_t)q * n_slots + j], s.sub_cap);
     g[q] = std::max(g[q], (uint32_t)std::min<uint64_t>(n, 0xFFFFFFFFu));
   }
   return SDB_OK;
 }
 // ScreenTap: the candidate lists as they stand (cnt: their counts, optional)
-static sdb_status tap_list(Corpus* c, uint32_t nq, std::vector<Cand>* list, std::vector<uint32_t>* cnt, cudaStream_t st) {
-  list->resize((size_t)nq * c->sc_cap);
-  SDB_CUDA(cudaMemcpyAsync(list->data(), c->d_cand, sizeof(Cand) * list->size(), cudaMemcpyDeviceToHost, st));
+static sdb_status tap_list(const Scratch& s, uint32_t nq, std::vector<Cand>* list, std::vector<uint32_t>* cnt,
+                           cudaStream_t st) {
+  list->resize((size_t)nq * s.sc_cap);
+  SDB_CUDA(cudaMemcpyAsync(list->data(), s.d_cand, sizeof(Cand) * list->size(), cudaMemcpyDeviceToHost, st));
   if (cnt) {
     cnt->resize(nq);
-    SDB_CUDA(cudaMemcpyAsync(cnt->data(), c->d_cand_cnt, sizeof(uint32_t) * nq, cudaMemcpyDeviceToHost, st));
+    SDB_CUDA(cudaMemcpyAsync(cnt->data(), s.d_cand_cnt, sizeof(uint32_t) * nq, cudaMemcpyDeviceToHost, st));
   }
   SDB_CUDA(cudaStreamSynchronize(st));
   return SDB_OK;
@@ -266,59 +262,83 @@ static sdb_status scatter_results(Corpus* c, Ticket& t) {
   return SDB_OK;
 }
 
-// queries q0 .. q0 + nd - 1 of the batch: no screen.  Each list holds exactly the query's passing rows, so tau stays
-// -inf and cand_final's proof holds trivially; the exact re-rank and cand_final order them as any candidate list.
-static sdb_status enqueue_direct(Corpus* c, Ticket& t, uint32_t q0, uint32_t nd, bool whole) {
-  cudaStream_t st = t.stream;
-  const uint32_t k = t.k;
-  SDB_TRY(scratch_for(c, nd, DIRECT_MAX_ROWS));
-  SDB_TRY(prep_queries(c, t.d_queries + (size_t)q0 * c->dim, nd, st));
-  SDB_TRY(cand_begin(c, nd, SDB_SCREEN_NONE_EXACT, st));
-  c->filt = t.filt;
-  c->filt.qf += q0;
-  SDB_TRY(cand_direct(c, nd, st));
-  SDB_TRY(cand_rerank(c, nd, st, false));
-  SDB_TRY(cand_final(c, nd, k, t.row_base, t.d_out_rows + (size_t)q0 * k, t.d_out_dist + (size_t)q0 * k,
-                     t.d_out_count + q0, st));
-  c->filt = t.filt;
-  SDB_CUDA(cudaMemcpyAsync(t.h_flags + q0, c->d_flags, sizeof(uint32_t) * nd, cudaMemcpyDeviceToHost, st));
-  SDB_CUDA(cudaMemcpyAsync(t.h_qflags + q0, c->d_qflags, sizeof(uint32_t) * nd, cudaMemcpyDeviceToHost, st));
-  if (whole) SDB_CUDA(cudaMemcpyAsync(t.h_stat, c->d_stat, sizeof(uint32_t) * 4, cudaMemcpyDeviceToHost, st));
+// One run of the enqueue functions: a whole batch, the screened head or the direct tail of a mixed one, or the failed
+// queries of a per-query repair.  The ticket holds what every run of the batch shares: stream, scratch set, k,
+// row_base, events and cancel flag.
+struct Run {
+  const double* d_queries;
+  uint32_t nq;
+  uint64_t* d_out_rows; double* d_out_dist; uint32_t* d_out_count;
+  FiltArg filt;
+  uint32_t rung;
+  sdb_screen screen;   // the screen asked for (Corpus::screen, or a debug batch's)
+  bool stream_refine;  // ... and the tensor-core schedule (Corpus::stream_refine)
+  ScreenTap* tap;      // test-only (see ScreenTap)
+  uint32_t *h_flags, *h_qflags;  // pinned: where the run's per-query flags go
+  uint32_t* h_stat;              // pinned: where its counters go (nullptr: nowhere)
+};
+// what a run decided: the screen it used and its screen launches
+struct Enqueued {
+  int screen = SDB_SCREEN_NONE_EXACT;
+  uint32_t n_passes = 0;
+};
+
+static sdb_status copy_flags(const Scratch& s, const Run& r, cudaStream_t st) {
+  SDB_CUDA(cudaMemcpyAsync(r.h_flags, s.d_flags, sizeof(uint32_t) * r.nq, cudaMemcpyDeviceToHost, st));
+  SDB_CUDA(cudaMemcpyAsync(r.h_qflags, s.d_qflags, sizeof(uint32_t) * r.nq, cudaMemcpyDeviceToHost, st));
+  if (r.h_stat) SDB_CUDA(cudaMemcpyAsync(r.h_stat, s.d_stat, sizeof(uint32_t) * 4, cudaMemcpyDeviceToHost, st));
   return SDB_OK;
 }
 
-static sdb_status enqueue_screened(Corpus* c, Ticket& t);
-static sdb_status enqueue_batch(Corpus* c, Ticket& t) {
-  activate_set(c, t.set);
-  // the batch's row filter is visible to the launches below only (every launch copies it)
-  struct FiltScope {
-    Corpus* c;
-    ~FiltScope() { c->filt = FiltArg(); }
-  } filt_scope{c};
-  c->filt = t.filt;
-  const uint32_t nd = t.n_direct;
-  if (nd == 0) return enqueue_screened(c, t);
+// direct queries: no screen.  Each list holds exactly the query's passing rows, so tau stays -inf and cand_final's
+// proof holds trivially; the exact re-rank and cand_final order them as any candidate list.
+static sdb_status enqueue_direct(Corpus* c, Ticket& t, const Run& r) {
   cudaStream_t st = t.stream;
-  if (nd == t.nq) {  // every query is direct: no screen at all
-    t.n_passes = 0;
-    t.screen = SDB_SCREEN_NONE_EXACT;
+  Scratch& s = c->sets[t.set];
+  SDB_TRY(scratch_for(c, s, r.nq, DIRECT_MAX_ROWS));
+  SDB_TRY(prep_queries(c, s, r.d_queries, r.nq, st));
+  SDB_TRY(cand_begin(c, s, r.nq, SDB_SCREEN_NONE_EXACT, st));
+  SDB_TRY(cand_direct(c, s, r.filt, r.nq, st));
+  SDB_TRY(cand_rerank(c, s, r.filt, r.nq, st, false));
+  SDB_TRY(cand_final(c, s, r.filt, r.nq, t.k, t.row_base, r.d_out_rows, r.d_out_dist, r.d_out_count, st));
+  return copy_flags(s, r, st);
+}
+
+static sdb_status enqueue_screened(Corpus* c, Ticket& t, const Run& r, Enqueued* e);
+// a whole batch: its last t.n_direct queries are direct, the others screened
+static sdb_status enqueue_batch(Corpus* c, Ticket& t, const Run& r, Enqueued* e) {
+  const uint32_t nd = t.n_direct;
+  if (nd == 0) return enqueue_screened(c, t, r, e);
+  cudaStream_t st = t.stream;
+  if (nd == r.nq) {  // every query is direct: no screen at all
+    *e = Enqueued();
     SDB_CUDA(cudaEventRecord(t.ev_begin, st));
     SDB_CUDA(cudaEventRecord(t.ev_screen0, st));
     SDB_CUDA(cudaEventRecord(t.ev_screen1, st));
-    SDB_TRY(enqueue_direct(c, t, 0, nd, true));
+    SDB_TRY(enqueue_direct(c, t, r));
     SDB_CUDA(cudaEventRecord(t.ev_end, st));
     return SDB_OK;
   }
-  // mixed (permuted) batch: the screened sub-batch, then the direct one behind it on the same stream and scratch set
-  SDB_TRY(scratch_for(c, t.nq, DIRECT_MAX_ROWS));  // sized for both, so that the direct part does not reallocate
-  const uint32_t ns = t.nq - nd;
-  t.nq = ns;
-  const sdb_status rc = enqueue_screened(c, t);
-  t.nq = ns + nd;
-  SDB_TRY(rc);
+  // mixed (permuted) batch: the screened head, then the direct tail behind it on the same stream and scratch set
+  Scratch& s = c->sets[t.set];
+  SDB_TRY(scratch_for(c, s, r.nq, DIRECT_MAX_ROWS));  // sized for both, so that the tail does not reallocate
+  const uint32_t ns = r.nq - nd;
+  Run head = r;
+  head.nq = ns;
+  SDB_TRY(enqueue_screened(c, t, head, e));
   SDB_CUDA(t.d_stat_scr.reserve(4));  // (the block header of a sharded batch adds both parts' flagged queries)
-  SDB_CUDA(cudaMemcpyAsync(t.d_stat_scr, c->d_stat, sizeof(uint32_t) * 4, cudaMemcpyDeviceToDevice, st));
-  SDB_TRY(enqueue_direct(c, t, ns, nd, false));
+  SDB_CUDA(cudaMemcpyAsync(t.d_stat_scr, s.d_stat, sizeof(uint32_t) * 4, cudaMemcpyDeviceToDevice, st));
+  Run tail = r;
+  tail.d_queries += (size_t)ns * c->dim;
+  tail.nq = nd;
+  tail.d_out_rows += (size_t)ns * t.k;
+  tail.d_out_dist += (size_t)ns * t.k;
+  tail.d_out_count += ns;
+  tail.filt.qf += ns;
+  tail.h_flags += ns;
+  tail.h_qflags += ns;
+  tail.h_stat = nullptr;  // (the batch's counters are the head's)
+  SDB_TRY(enqueue_direct(c, t, tail));
   SDB_CUDA(cudaEventRecord(t.ev_end, st));
   return SDB_OK;
 }
@@ -326,17 +346,18 @@ static sdb_status enqueue_batch(Corpus* c, Ticket& t) {
 // HAMMING / JACCARD (count_ranked): exact counts of every row in one launch, ranked per row range; each query's list
 // is the union of its ranges' best k with their exact distances, so cand_final orders it with tau = -inf and nothing
 // is left to prove or repair.  Reported as one SIMT_F32 pass.
-static sdb_status enqueue_counted(Corpus* c, Ticket& t) {
+static sdb_status enqueue_counted(Corpus* c, Ticket& t, const Run& r, Enqueued* e) {
   Ctx* ctx = c->ctx;
   cudaStream_t st = t.stream;
-  const uint32_t nq = t.nq, k = t.k;
-  t.screen = SDB_SCREEN_SIMT_F32;
-  t.n_passes = 1;
+  Scratch& s = c->sets[t.set];
+  const uint32_t nq = r.nq, k = t.k;
+  e->screen = SDB_SCREEN_SIMT_F32;
+  e->n_passes = 1;
   SDB_CUDA(cudaEventRecord(t.ev_begin, st));
   trace_mark(ctx, t, "begin", st);
-  SDB_TRY(scratch_for(c, nq, std::max(4096u, count_ranges(c, nq, k) * k)));
-  SDB_TRY(prep_queries(c, t.d_queries, nq, st));
-  SDB_TRY(cand_begin(c, nq, SDB_SCREEN_NONE_EXACT, st));
+  SDB_TRY(scratch_for(c, s, nq, std::max(4096u, count_ranges(c, nq, k) * k)));
+  SDB_TRY(prep_queries(c, s, r.d_queries, nq, st));
+  SDB_TRY(cand_begin(c, s, nq, SDB_SCREEN_NONE_EXACT, st));
   if (c->last_main && c->last_main != t.ev_main) SDB_CUDA(cudaStreamWaitEvent(st, c->last_main, 0));
   SDB_CUDA(cudaEventRecord(t.ev_screen0, st));
   if ((t.cancel && *t.cancel) || ctx_cancelled(ctx)) {
@@ -344,86 +365,83 @@ static sdb_status enqueue_counted(Corpus* c, Ticket& t) {
     set_error("query cancelled");
     return SDB_ECANCELLED;
   }
-  SDB_TRY(count_pass(c, nq, k, st));
+  SDB_TRY(count_pass(c, s, r.filt, nq, k, st));
   SDB_CUDA(cudaEventRecord(t.ev_main, st));
   c->last_main = t.ev_main;
   SDB_CUDA(cudaEventRecord(t.ev_screen1, st));
   trace_mark(ctx, t, "counted", st);
-  SDB_TRY(cand_final(c, nq, k, t.row_base, t.d_out_rows, t.d_out_dist, t.d_out_count, st));
-  SDB_CUDA(cudaMemcpyAsync(t.h_flags, c->d_flags, sizeof(uint32_t) * nq, cudaMemcpyDeviceToHost, st));
-  SDB_CUDA(cudaMemcpyAsync(t.h_qflags, c->d_qflags, sizeof(uint32_t) * nq, cudaMemcpyDeviceToHost, st));
-  SDB_CUDA(cudaMemcpyAsync(t.h_stat, c->d_stat, sizeof(uint32_t) * 4, cudaMemcpyDeviceToHost, st));
+  SDB_TRY(cand_final(c, s, r.filt, nq, k, t.row_base, r.d_out_rows, r.d_out_dist, r.d_out_count, st));
+  SDB_TRY(copy_flags(s, r, st));
   SDB_CUDA(cudaEventRecord(t.ev_end, st));
   trace_mark(ctx, t, "end", st);
   return SDB_OK;
 }
 
-static sdb_status enqueue_screened(Corpus* c, Ticket& t) {
+static sdb_status enqueue_screened(Corpus* c, Ticket& t, const Run& r, Enqueued* e) {
   Ctx* ctx = c->ctx;
   cudaStream_t st = t.stream;
-  const uint32_t nq = t.nq, k = t.k;
+  Scratch& s = c->sets[t.set];
+  const uint32_t nq = r.nq, k = t.k;
   // HAMMING: AUTO ranks a batch of one query with the exact kernel, which streams the rows once at the higher rate
   // (DESIGN.md section 5); an explicit screen request still counts it.  JACCARD's exact kernel is O(D^2) per row: the
   // count path takes a single query too
-  if (count_ranked(c, k) && (nq > 1 || c->screen != SDB_SCREEN_AUTO || c->metric == SDB_JACCARD))
-    return enqueue_counted(c, t);
+  if (count_ranked(c, k) && (nq > 1 || r.screen != SDB_SCREEN_AUTO || c->metric == SDB_JACCARD))
+    return enqueue_counted(c, t, r, e);
   sdb_screen first;
-  const std::vector<Rung> rungs = build_rungs(c, k, nq, &first);
-  t.n_rungs = (uint32_t)rungs.size();
-  t.n_passes = 0;
+  const std::vector<Rung> rungs = build_rungs(c, r.screen, k, nq, &first);
+  e->n_passes = 0;
   SDB_CUDA(cudaEventRecord(t.ev_begin, st));
   trace_mark(ctx, t, "begin", st);
   if (rungs.empty()) {  // exact-only: the exact kernel needs the prepared queries (f64 copy, |q|, flags)
-    t.screen = SDB_SCREEN_NONE_EXACT;
-    SDB_TRY(scratch_for(c, nq, 4096));
-    SDB_TRY(prep_queries(c, t.d_queries, nq, st));
+    e->screen = SDB_SCREEN_NONE_EXACT;
+    SDB_TRY(scratch_for(c, s, nq, 4096));
+    SDB_TRY(prep_queries(c, s, r.d_queries, nq, st));
     SDB_CUDA(cudaEventRecord(t.ev_screen0, st));
     SDB_CUDA(cudaEventRecord(t.ev_screen1, st));
-    SDB_CUDA(cudaMemsetAsync(t.d_out_count, 0, sizeof(uint32_t) * nq, st));
-    SDB_CUDA(cudaMemcpyAsync(t.h_qflags, c->d_qflags, sizeof(uint32_t) * nq, cudaMemcpyDeviceToHost, st));
-    for (uint32_t q = 0; q < nq; q++) t.h_flags[q] = 2u;  // every query takes the exact kernel
-    t.h_stat[0] = nq;
-    t.h_stat[1] = t.h_stat[2] = t.h_stat[3] = 0;
+    SDB_CUDA(cudaMemsetAsync(r.d_out_count, 0, sizeof(uint32_t) * nq, st));
+    SDB_CUDA(cudaMemcpyAsync(r.h_qflags, s.d_qflags, sizeof(uint32_t) * nq, cudaMemcpyDeviceToHost, st));
+    for (uint32_t q = 0; q < nq; q++) r.h_flags[q] = 2u;  // every query takes the exact kernel
+    const uint32_t stat[4] = {nq, 0u, 0u, 0u};
+    if (r.h_stat) std::copy(stat, stat + 4, r.h_stat);
     SDB_CUDA(cudaEventRecord(t.ev_end, st));
     return SDB_OK;
   }
-  if (t.rung >= rungs.size()) t.rung = (uint32_t)rungs.size() - 1;
-  const Rung rg = rungs[t.rung];
+  const Rung rg = rungs[std::min<size_t>(r.rung, rungs.size() - 1)];
   const sdb_screen rs = rg.scr;
-  t.screen = (int)rs;
+  e->screen = (int)rs;
   const bool tc = rs == SDB_SCREEN_TC_INT8 || rs == SDB_SCREEN_TC_BF16;
   const bool int8 = rs == SDB_SCREEN_TC_INT8;
-  SDB_TRY(scratch_for(c, nq, rg.cap));
-  const uint32_t cap = c->sc_cap;
-  SDB_TRY(prep_queries(c, t.d_queries, nq, st));
-  SDB_TRY(cand_begin(c, nq, (int)rs, st));
+  SDB_TRY(scratch_for(c, s, nq, rg.cap));
+  const uint32_t cap = s.sc_cap;
+  SDB_TRY(prep_queries(c, s, r.d_queries, nq, st));
+  SDB_TRY(cand_begin(c, s, nq, (int)rs, st));
   // Screens are persistent one-CTA-per-SM kernels: two of them in flight on different streams would split the SMs,
   // run in two waves and starve the refiners of the CTAs that are not resident yet.  So the screen of this batch waits
   // for the end of the previous batch's screen -- only the TAIL of the previous batch overlaps with it.
   if (c->last_main && c->last_main != t.ev_main) SDB_CUDA(cudaStreamWaitEvent(st, c->last_main, 0));
   SDB_CUDA(cudaEventRecord(t.ev_screen0, st));  // after the wait: screen_ms is this batch's screen, not the queueing
   trace_mark(ctx, t, "screen0", st);
-  if (tc && c->stream_refine) {
+  if (tc && r.stream_refine) {
     PassDesc p0, pm;
     build_stream_passes(c->n, cap, k, &p0, &pm);
     if (p0.count && !pm.count) {  // the whole corpus fits the lists: score everything once
-      SDB_TRY(screen_tc_pass(c, nq, k, p0, int8, 0, st));
+      SDB_TRY(screen_tc_pass(c, s, r.filt, nq, k, p0, int8, 0, st));
       SDB_CUDA(cudaEventRecord(t.ev_main, st));
       c->last_main = t.ev_main;
-      if (c->tap) SDB_TRY(tap_gathered(c, nq, 0u, st));
-      SDB_TRY(cand_select(c, nq, k, int8, 0u, false, st));
-      t.n_passes++;
+      if (r.tap) SDB_TRY(tap_gathered(s, r.tap, nq, 0u, st));
+      SDB_TRY(cand_select(c, s, nq, k, int8, 0u, false, st));
+      e->n_passes++;
     } else if (pm.count) {
-      SDB_TRY(screen_tc_pass(c, nq, k, p0, int8, 3, st));           // probe: chunk maxima of a few tiles
-      SDB_TRY(cand_seed_from_probe(c, nq, k, p0.count, st));         // thresholds + histogram geometry
+      SDB_TRY(screen_tc_pass(c, s, r.filt, nq, k, p0, int8, 3, st));  // probe: chunk maxima of a few tiles
+      SDB_TRY(cand_seed_from_probe(c, s, nq, k, p0.count, st));       // thresholds + histogram geometry
       trace_mark(ctx, t, "seeded", st);
-      SDB_TRY(screen_tc_pass(c, nq, k, pm, int8, 2, st));           // the streaming launch over every tile
+      SDB_TRY(screen_tc_pass(c, s, r.filt, nq, k, pm, int8, 2, st));  // the streaming launch over every tile
       trace_mark(ctx, t, "main_end", st);
       SDB_CUDA(cudaEventRecord(t.ev_main, st));
       c->last_main = t.ev_main;
-      if (c->tap) SDB_TRY(tap_gathered(c, nq, c->last_slots, st));
-      SDB_TRY(cand_select(c, nq, k, int8, c->last_slots, false, st));
-      t.n_passes += 2;
+      if (r.tap) SDB_TRY(tap_gathered(s, r.tap, nq, s.last_slots, st));
+      SDB_TRY(cand_select(c, s, nq, k, int8, s.last_slots, false, st));
+      e->n_passes += 2;
     }
   } else {
     const std::vector<PassDesc> passes = build_passes(c->n, cap, nq);
@@ -434,40 +452,49 @@ static sdb_status enqueue_screened(Corpus* c, Ticket& t) {
         set_error("query cancelled");
         return SDB_ECANCELLED;
       }
-      if (tc) SDB_TRY(screen_tc_pass(c, nq, k, p, int8, first_pass ? 0 : 1, st));
-      else if (family(c) == Family::Lp) SDB_TRY(screen_lp_pass(c, nq, p, st));
-      else SDB_TRY(screen_simt_pass(c, nq, p, st));
-      if (c->tap) SDB_TRY(tap_gathered(c, nq, tc ? c->last_slots : 0u, st));
-      SDB_TRY(cand_select(c, nq, k, int8, tc ? c->last_slots : 0u, false, st));
+      if (tc) SDB_TRY(screen_tc_pass(c, s, r.filt, nq, k, p, int8, first_pass ? 0 : 1, st));
+      else if (family(c) == Family::Lp) SDB_TRY(screen_lp_pass(c, s, r.filt, nq, p, st));
+      else SDB_TRY(screen_simt_pass(c, s, r.filt, nq, p, st));
+      if (r.tap) SDB_TRY(tap_gathered(s, r.tap, nq, tc ? s.last_slots : 0u, st));
+      SDB_TRY(cand_select(c, s, nq, k, int8, tc ? s.last_slots : 0u, false, st));
       first_pass = false;
-      t.n_passes++;
+      e->n_passes++;
     }
     SDB_CUDA(cudaEventRecord(t.ev_main, st));
     c->last_main = t.ev_main;
   }
-  if (c->tap) SDB_TRY(tap_list(c, nq, &c->tap->list_a, &c->tap->cnt_a, st));
+  if (r.tap) SDB_TRY(tap_list(s, nq, &r.tap->list_a, &r.tap->cnt_a, st));
   SDB_CUDA(cudaEventRecord(t.ev_screen1, st));
   trace_mark(ctx, t, "selected", st);
   // stage B: the coarse screens' candidates are re-scored in f32 and narrowed before the (FP64-bound) exact re-rank
   static const bool no_refine = getenv("SDB_NO_REFINE") != nullptr;
   bool refined = false;
   if (tc && c->exact && !no_refine) {
-    SDB_TRY(cand_refine(c, nq, st));
-    if (c->tap) SDB_TRY(tap_list(c, nq, &c->tap->list_r, nullptr, st));
-    SDB_TRY(cand_select(c, nq, k, false, 0u, false, st, 1));
+    SDB_TRY(cand_refine(c, s, nq, st));
+    if (r.tap) SDB_TRY(tap_list(s, nq, &r.tap->list_r, nullptr, st));
+    SDB_TRY(cand_select(c, s, nq, k, false, 0u, false, st, 1));
     refined = true;
     trace_mark(ctx, t, "refined", st);
   }
-  if (c->filt.bits) SDB_TRY(cand_add_specials(c, nq, st));  // each query re-ranks its own passing special rows
-  SDB_TRY(cand_rerank(c, nq, st, refined));
+  if (r.filt.bits) SDB_TRY(cand_add_specials(c, s, r.filt, nq, st));  // each query re-ranks its passing special rows
+  SDB_TRY(cand_rerank(c, s, r.filt, nq, st, refined));
   trace_mark(ctx, t, "reranked", st);
-  SDB_TRY(cand_final(c, nq, k, t.row_base, t.d_out_rows, t.d_out_dist, t.d_out_count, st));
+  SDB_TRY(cand_final(c, s, r.filt, nq, k, t.row_base, r.d_out_rows, r.d_out_dist, r.d_out_count, st));
   trace_mark(ctx, t, "final", st);
-  SDB_CUDA(cudaMemcpyAsync(t.h_flags, c->d_flags, sizeof(uint32_t) * nq, cudaMemcpyDeviceToHost, st));
-  SDB_CUDA(cudaMemcpyAsync(t.h_qflags, c->d_qflags, sizeof(uint32_t) * nq, cudaMemcpyDeviceToHost, st));
-  SDB_CUDA(cudaMemcpyAsync(t.h_stat, c->d_stat, sizeof(uint32_t) * 4, cudaMemcpyDeviceToHost, st));
+  SDB_TRY(copy_flags(s, r, st));
   SDB_CUDA(cudaEventRecord(t.ev_end, st));
   trace_mark(ctx, t, "end", st);
+  return SDB_OK;
+}
+
+// the whole batch at its rung, with what it decided recorded on the ticket
+static sdb_status enqueue_ticket(Corpus* c, Ticket& t) {
+  const Run r{t.d_queries, t.nq, t.d_out_rows, t.d_out_dist, t.d_out_count, t.filt, t.rung, c->screen,
+              c->stream_refine, nullptr, t.h_flags, t.h_qflags, t.h_stat};
+  Enqueued e;
+  SDB_TRY(enqueue_batch(c, t, r, &e));
+  t.screen = e.screen;
+  t.n_passes = e.n_passes;
   return SDB_OK;
 }
 
@@ -499,14 +526,14 @@ static sdb_status finish_local(Corpus* c, Ticket& t, uint32_t* n_fallback, bool*
       if (n_fail <= 2 + nq / 64) break;
       SDB_CUDA(drain(ctx));  // later batches in flight share scratch sets and the ladder state: drain them first
       t.rung++;
-      SDB_TRY(enqueue_batch(c, t));
+      SDB_TRY(enqueue_ticket(c, t));
       SDB_CUDA(cudaEventSynchronize(t.ev_end));
       *repaired = true;
     }
   }
   if (t.n_rungs) {
     sdb_screen first;
-    build_rungs(c, k, nq, &first);
+    build_rungs(c, c->screen, k, nq, &first);
     c->rung_scr = first;
     c->rung_k = k;
     c->rung = t.rung;
@@ -523,19 +550,7 @@ static sdb_status finish_local(Corpus* c, Ticket& t, uint32_t* n_fallback, bool*
   // corpus costs about as much for 60 queries as for 1, and far less than one sequential-f64 pass per query); the f32
   // stream is the last rung.  Whatever is still unproven after that goes to the exact kernel.
   if (!fails.empty() && t.screen != SDB_SCREEN_NONE_EXACT && c->exact && k) {
-    // (save_rungs: a one-query MANHATTAN / CHEBYSHEV repair has no rungs of its own, build_rungs)
-    const uint32_t save_rung = t.rung, save_nq = t.nq, save_passes = t.n_passes, save_rungs = t.n_rungs;
-    const int save_screen = t.screen;
-    const double* save_q = t.d_queries;
-    const uint32_t* save_qf = t.filt.qf;
-    const uint32_t save_nd = t.n_direct;
-    t.n_direct = 0;  // the failing queries are screened ones (a direct query's proof cannot fail)
-    uint64_t* save_rows = t.d_out_rows;
-    double* save_dist = t.d_out_dist;
-    uint32_t* save_cnt = t.d_out_count;
-    uint32_t save_stat[4] = {t.h_stat[0], t.h_stat[1], t.h_stat[2], t.h_stat[3]};
-    sdb_status rc = SDB_OK;
-    for (uint32_t rung = save_rung + 1; rung < save_rungs && !fails.empty() && rc == SDB_OK; rung++) {
+    for (uint32_t rung = t.rung + 1; rung < t.n_rungs && !fails.empty(); rung++) {
       if ((t.cancel && *t.cancel) || ctx_cancelled(ctx)) break;
       const uint32_t nf = (uint32_t)fails.size();
       const size_t need_q = (size_t)nf * c->dim, need_o = (size_t)nf * k;
@@ -543,12 +558,12 @@ static sdb_status finish_local(Corpus* c, Ticket& t, uint32_t* n_fallback, bool*
       if (e == cudaSuccess) e = c->rp.reserve(need_o, nf);
       if (e != cudaSuccess) {
         set_error("repair buffers: %s", cudaGetErrorString(e));
-        rc = SDB_ENOMEM;
-        break;
+        return SDB_ENOMEM;
       }
       for (uint32_t i = 0; i < nf; i++)
-        cudaMemcpyAsync(c->d_rp_q + (size_t)i * c->dim, save_q + (size_t)fails[i] * c->dim, sizeof(double) * c->dim, cudaMemcpyDeviceToDevice, st);
+        cudaMemcpyAsync(c->d_rp_q + (size_t)i * c->dim, t.d_queries + (size_t)fails[i] * c->dim, sizeof(double) * c->dim, cudaMemcpyDeviceToDevice, st);
       std::vector<uint32_t> rp_qf;  // filtered batch: each gathered query keeps its own filter
+      FiltArg filt = t.filt;
       if (t.filt.bits) {
         rp_qf.resize(nf);
         for (uint32_t i = 0; i < nf; i++) rp_qf[i] = t.h_qf[fails[i]];
@@ -556,20 +571,17 @@ static sdb_status finish_local(Corpus* c, Ticket& t, uint32_t* n_fallback, bool*
         if (e == cudaSuccess) e = cudaMemcpyAsync(c->d_rp_qf, rp_qf.data(), sizeof(uint32_t) * nf, cudaMemcpyHostToDevice, st);
         if (e != cudaSuccess) {
           set_error("repair filter indices: %s", cudaGetErrorString(e));
-          rc = SDB_ECUDA;
-          break;
+          return SDB_ECUDA;
         }
-        t.filt.qf = c->d_rp_qf;
+        filt.qf = c->d_rp_qf;
       }
-      t.d_queries = c->d_rp_q;
-      t.nq = nf;
-      t.d_out_rows = c->rp.rows;
-      t.d_out_dist = c->rp.dist;
-      t.d_out_count = c->rp.count;
-      t.rung = rung;
-      rc = enqueue_batch(c, t);
-      if (rc == SDB_OK && cudaEventSynchronize(t.ev_end) != cudaSuccess) rc = SDB_ECUDA;
-      if (rc != SDB_OK) break;
+      // the failed queries are screened ones (a direct query's proof cannot fail); their flags go to the batch's first
+      // entries, which were read above
+      const Run rp{c->d_rp_q, nf, c->rp.rows, c->rp.dist, c->rp.count, filt, rung, c->screen, c->stream_refine,
+                   nullptr, t.h_flags, t.h_qflags, nullptr};
+      Enqueued ignored;
+      SDB_TRY(enqueue_screened(c, t, rp, &ignored));
+      SDB_CUDA(cudaEventSynchronize(t.ev_end));
       std::vector<uint32_t> still;
       for (uint32_t i = 0; i < nf; i++) {
         const uint32_t q = fails[i];
@@ -577,28 +589,15 @@ static sdb_status finish_local(Corpus* c, Ticket& t, uint32_t* n_fallback, bool*
           still.push_back(q);
           continue;
         }
-        cudaMemcpyAsync(save_rows + (size_t)q * k, c->rp.rows + (size_t)i * k, sizeof(uint64_t) * k, cudaMemcpyDeviceToDevice, st);
-        cudaMemcpyAsync(save_dist + (size_t)q * k, c->rp.dist + (size_t)i * k, sizeof(double) * k, cudaMemcpyDeviceToDevice, st);
-        cudaMemcpyAsync(save_cnt + q, c->rp.count + i, sizeof(uint32_t), cudaMemcpyDeviceToDevice, st);
+        cudaMemcpyAsync(t.d_out_rows + (size_t)q * k, c->rp.rows + (size_t)i * k, sizeof(uint64_t) * k, cudaMemcpyDeviceToDevice, st);
+        cudaMemcpyAsync(t.d_out_dist + (size_t)q * k, c->rp.dist + (size_t)i * k, sizeof(double) * k, cudaMemcpyDeviceToDevice, st);
+        cudaMemcpyAsync(t.d_out_count + q, c->rp.count + i, sizeof(uint32_t), cudaMemcpyDeviceToDevice, st);
         t.n_repaired++;
       }
       SDB_CUDA(cudaStreamSynchronize(st));
       fails.swap(still);
       *repaired = true;
     }
-    t.d_queries = save_q;
-    t.filt.qf = save_qf;
-    t.n_direct = save_nd;
-    t.nq = save_nq;
-    t.d_out_rows = save_rows;
-    t.d_out_dist = save_dist;
-    t.d_out_count = save_cnt;
-    t.rung = save_rung;
-    t.n_rungs = save_rungs;
-    t.screen = save_screen;
-    t.n_passes = save_passes;
-    for (int i = 0; i < 4; i++) t.h_stat[i] = save_stat[i];
-    SDB_TRY(rc);
   }
   // ---- exact kernel: special queries and whatever no screen could prove ----
   exacts.insert(exacts.end(), fails.begin(), fails.end());
@@ -745,11 +744,13 @@ static sdb_status submit_locked(Corpus* c, Ticket* t, const double* d_queries, u
   t->cancel = cancel;
   t->launches0 = c->ctx->launches;
   t->n_repaired = 0;
-  sdb_screen first;
-  const std::vector<Rung> rungs = build_rungs(c, k, nq, &first);
+  sdb_screen first, first_scr;
+  const std::vector<Rung> rungs = build_rungs(c, c->screen, k, nq, &first);
   t->rung = (c->rung_scr == first && c->rung_k == k && c->rung < n_batch_rungs(rungs)) ? c->rung : 0;
-  t->n_rungs = (uint32_t)rungs.size();
   t->n_batch_rungs = n_batch_rungs(rungs);
+  // the ladder of its screened queries, which a mixed batch screens on their own (one Lp query has none, build_rungs)
+  const uint32_t n_scr = t->n_direct < nq ? nq - t->n_direct : nq;
+  t->n_rungs = (uint32_t)build_rungs(c, c->screen, k, n_scr, &first_scr).size();
   if (nq == 0 || k == 0) {  // nothing to search: counts are zero
     cudaStream_t st = t->stream;
     SDB_CUDA(cudaEventRecord(t->ev_begin, st));
@@ -765,7 +766,7 @@ static sdb_status submit_locked(Corpus* c, Ticket* t, const double* d_queries, u
     t->busy = true;
     return SDB_OK;
   }
-  sdb_status rc = enqueue_batch(c, *t);
+  sdb_status rc = enqueue_ticket(c, *t);
   if (rc == SDB_OK) rc = scatter_results(c, *t);
   if (rc == SDB_OK) t->busy = true;
   trace_host(c->ctx, t->id, "submitted");
@@ -824,11 +825,11 @@ sdb_status knn_shard_header(Corpus* c, uint32_t ticket, void* d_hdr) {
   if (t->n_rungs == 0) {  // exact-only or counted batch: the counters the host holds
     SDB_CUDA(cudaMemcpyAsync(d_hdr, t->h_stat, 16, cudaMemcpyHostToDevice, st));
   } else if (t->permuted) {
-    sum_flagged_kernel<<<1, 32, 0, st>>>(c->d_stat, t->d_stat_scr, (uint32_t*)d_hdr);
+    sum_flagged_kernel<<<1, 32, 0, st>>>(c->sets[t->set].d_stat, t->d_stat_scr, (uint32_t*)d_hdr);
     count_launch(c->ctx);
     SDB_CUDA(cudaGetLastError());
   } else {
-    SDB_CUDA(cudaMemcpyAsync(d_hdr, c->d_stat, 16, cudaMemcpyDeviceToDevice, st));
+    SDB_CUDA(cudaMemcpyAsync(d_hdr, c->sets[t->set].d_stat, 16, cudaMemcpyDeviceToDevice, st));
   }
   return SDB_OK;
 }
@@ -1630,11 +1631,14 @@ sdb_status sdb_debug_screen_batch_filtered(sdb_corpus* c, const double* queries,
   SDB_TRY(ticket_prepare(c, *t, nq));
   const uint64_t n_pad = (c->n + TILE_ROWS - 1) / TILE_ROWS * TILE_ROWS;
   const uint32_t cap = score_all ? (uint32_t)std::max<uint64_t>(cand_cap, n_pad) : cand_cap;
-  // exactly `cap` slots per query: drop the batch scratch so that ensure_scratch allocates it at this size
-  activate_set(c, 0);
-  c->sc_nq = c->sc_cap = 0;
-  SDB_TRY(scratch_for(c, nq, cap));
+  // the batch runs on set 0 and the first stream; exactly `cap` slots per query: drop the set so that scratch_for
+  // allocates it at this size
+  Scratch& s = c->sets[0];
+  s.sc_nq = s.sc_cap = 0;
+  SDB_TRY(scratch_for(c, s, nq, cap));
   cudaStream_t st = ctx->stream;
+  t->set = 0;
+  t->stream = st;
   // the batch's filter, classified as ticket submission classifies it
   t->filt = FiltArg();
   t->n_direct = 0;
@@ -1662,56 +1666,38 @@ sdb_status sdb_debug_screen_batch_filtered(sdb_corpus* c, const double* queries,
   DevBuf<double> d_q;
   ResultBufs out;
   ScreenTap tap;
-  const sdb_screen save_screen = c->screen;
-  const bool save_stream = c->stream_refine;
   auto run = [&]() -> sdb_status {
     SDB_CUDA(d_q.reserve((size_t)nq * c->dim));
     SDB_CUDA(out.reserve((size_t)nq * k, nq));
     SDB_CUDA(cudaMemcpyAsync(d_q, queries, sizeof(double) * (size_t)nq * c->dim, cudaMemcpyHostToDevice, st));
     if (score_all) {  // one pass-0 launch over every tile (SIMT: tau stays -inf), nothing selected
       const PassDesc all{1u, 0u, (uint32_t)(n_pad / TILE_ROWS), 0u};
-      SDB_TRY(prep_queries(c, d_q, nq, st));
-      SDB_TRY(cand_begin(c, nq, (int)screen, st));
-      c->filt = t->filt;
-      sdb_status rc = tc                ? screen_tc_pass(c, nq, k, all, int8, 0, st)
-                      : f == Family::Lp ? screen_lp_pass(c, nq, all, st)
-                                        : screen_simt_pass(c, nq, all, st);
-      c->filt = FiltArg();
-      SDB_TRY(rc);
-      SDB_TRY(tap_list(c, nq, &tap.list_a, &tap.cnt_a, st));
+      SDB_TRY(prep_queries(c, s, d_q, nq, st));
+      SDB_TRY(cand_begin(c, s, nq, (int)screen, st));
+      SDB_TRY(tc                ? screen_tc_pass(c, s, t->filt, nq, k, all, int8, 0, st)
+              : f == Family::Lp ? screen_lp_pass(c, s, t->filt, nq, all, st)
+                                : screen_simt_pass(c, s, t->filt, nq, all, st));
+      SDB_TRY(tap_list(s, nq, &tap.list_a, &tap.cnt_a, st));
       tap.gathered = tap.cnt_a;
       return SDB_OK;
     }
     // the production sequence of one batch at rung 0 of `screen` (no ladder, no exact fallback)
-    c->screen = screen;
-    c->stream_refine = streaming != 0;
-    t->set = 0;
-    t->stream = st;
-    t->d_queries = d_q;
-    t->nq = nq;
     t->k = k;
     t->row_base = 0;
-    t->d_out_rows = out.rows;
-    t->d_out_dist = out.dist;
-    t->d_out_count = out.count;
     t->cancel = nullptr;
-    t->rung = 0;
-    c->tap = &tap;
-    const sdb_status rc = enqueue_batch(c, *t);
-    c->tap = nullptr;
-    SDB_TRY(rc);
+    const Run r{d_q, nq, out.rows, out.dist, out.count, t->filt, 0u, screen, streaming != 0, &tap,
+                t->h_flags, t->h_qflags, t->h_stat};
+    Enqueued e;
+    SDB_TRY(enqueue_batch(c, *t, r, &e));
     SDB_CUDA(cudaStreamSynchronize(st));
-    if (direct) return tap_list(c, nq, &tap.list_a, &tap.cnt_a, st);  // no screen ran: the lists are the direct ones
-    if (t->screen != (int)screen) {
+    if (direct) return tap_list(s, nq, &tap.list_a, &tap.cnt_a, st);  // no screen ran: the lists are the direct ones
+    if (e.screen != (int)screen) {
       set_error("sdb_debug_screen_batch: the corpus does not offer screen %d", (int)screen);
       return SDB_EINVAL;
     }
     return SDB_OK;
   };
   sdb_status rc = run();
-  c->tap = nullptr;
-  c->screen = save_screen;
-  c->stream_refine = save_stream;
   if (rc == SDB_OK) {  // per-query figures and lists (columns documented in the header)
     auto rd = [&](void* dst, const void* src, size_t bytes) {
       if (rc == SDB_OK && cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToHost, st) != cudaSuccess) {
@@ -1721,8 +1707,8 @@ sdb_status sdb_debug_screen_batch_filtered(sdb_corpus* c, const double* queries,
     };
     const size_t cap_sz = (size_t)nq * cap;
     std::vector<float> f[9];
-    const float* srcf[9] = {c->d_tau, c->d_margin, c->d_bscale, c->d_beps, c->d_tau2, c->d_beps2,
-                            c->d_i8 ? c->d_q8scale.get() : nullptr, c->d_i8 ? c->d_q8err.get() : nullptr, c->d_qbferr};
+    const float* srcf[9] = {s.d_tau, s.d_margin, s.d_bscale, s.d_beps, s.d_tau2, s.d_beps2,
+                            c->d_i8 ? s.d_q8scale.get() : nullptr, c->d_i8 ? s.d_q8err.get() : nullptr, s.d_qbferr};
     for (int j = 0; j < 9; j++) {
       f[j].assign(nq, NAN);
       if (srcf[j]) rd(f[j].data(), srcf[j], sizeof(float) * nq);
@@ -1730,17 +1716,17 @@ sdb_status sdb_debug_screen_batch_filtered(sdb_corpus* c, const double* queries,
     std::vector<uint32_t> flags(nq), qflags(nq), cnt_b(nq);
     std::vector<Cand> list_b(score_all ? 0 : cap_sz);
     std::vector<uint32_t> rr;
-    rd(flags.data(), c->d_flags, sizeof(uint32_t) * nq);
-    rd(qflags.data(), c->d_qflags, sizeof(uint32_t) * nq);
-    if (out_qmag) rd(out_qmag, c->d_qmag, sizeof(double) * nq);
-    if (out_q8 && c->d_i8) rd(out_q8, c->d_q8, (size_t)nq * c->dim_pad8);
-    if (out_qbf16) rd(out_qbf16, c->d_qbf16, 2 * (size_t)nq * c->dim_pad);
+    rd(flags.data(), s.d_flags, sizeof(uint32_t) * nq);
+    rd(qflags.data(), s.d_qflags, sizeof(uint32_t) * nq);
+    if (out_qmag) rd(out_qmag, s.d_qmag, sizeof(double) * nq);
+    if (out_q8 && c->d_i8) rd(out_q8, s.d_q8, (size_t)nq * c->dim_pad8);
+    if (out_qbf16) rd(out_qbf16, s.d_qbf16, 2 * (size_t)nq * c->dim_pad);
     if (!score_all) {
-      rd(cnt_b.data(), c->d_cand_cnt, sizeof(uint32_t) * nq);
-      rd(list_b.data(), c->d_cand, sizeof(Cand) * cap_sz);
+      rd(cnt_b.data(), s.d_cand_cnt, sizeof(uint32_t) * nq);
+      rd(list_b.data(), s.d_cand, sizeof(Cand) * cap_sz);
       if (out_rr) {
-        rr.resize((size_t)nq * c->rr_stride);
-        rd(rr.data(), c->d_rr_row, sizeof(uint32_t) * rr.size());
+        rr.resize((size_t)nq * s.rr_stride);
+        rd(rr.data(), s.d_rr_row, sizeof(uint32_t) * rr.size());
       }
     }
     if (rc == SDB_OK && cudaStreamSynchronize(st) != cudaSuccess) rc = SDB_ECUDA;
@@ -1781,7 +1767,7 @@ sdb_status sdb_debug_screen_batch_filtered(sdb_corpus* c, const double* queries,
         }
         if (out_rr && !score_all)
           for (uint32_t e = 0; e < cap + SPECIAL_CAP; e++)
-            out_rr[(size_t)q * (cap + SPECIAL_CAP) + e] = e < n_b + n_special ? rr[(size_t)q * c->rr_stride + e] : 0xFFFFFFFFu;
+            out_rr[(size_t)q * (cap + SPECIAL_CAP) + e] = e < n_b + n_special ? rr[(size_t)q * s.rr_stride + e] : 0xFFFFFFFFu;
       }
     }
   }
@@ -1893,17 +1879,18 @@ sdb_status sdb_corpus_project(sdb_corpus* c, const double* query, int fn, double
   }
   if (c->n == 0) return SDB_OK;
   SDB_CUDA(cudaSetDevice(c->ctx->device));
-  SDB_CUDA(drain(c->ctx));  // borrows the active scratch set for the prepared query
+  SDB_CUDA(drain(c->ctx));  // borrows scratch set 0 for the prepared query
   cudaStream_t st = c->ctx->stream;
+  Scratch& s = c->sets[0];
   auto run = [&]() -> sdb_status {  // the temporaries are released on every path, before the synchronisation below
     AsyncBuf<double> d_q, d_vals;
     SDB_CUDA(d_q.reserve(c->dim, st));
     SDB_CUDA(d_vals.reserve(c->n, st));
     if (query) SDB_CUDA(cudaMemcpyAsync(d_q, query, sizeof(double) * c->dim, cudaMemcpyHostToDevice, st));
     else SDB_CUDA(cudaMemsetAsync(d_q, 0, sizeof(double) * c->dim, st));
-    SDB_TRY(scratch_for(c, 1, 4096));
-    SDB_TRY(prep_queries(c, d_q, 1, st));
-    SDB_TRY(exact_project(c, fn, d_vals, st));
+    SDB_TRY(scratch_for(c, s, 1, 4096));
+    SDB_TRY(prep_queries(c, s, d_q, 1, st));
+    SDB_TRY(exact_project(c, fn, s.d_q64, s.d_qmag, s.d_qflags, d_vals, st));
     SDB_CUDA(cudaMemcpyAsync(out, d_vals, sizeof(double) * c->n, cudaMemcpyDeviceToHost, st));
     return SDB_OK;
   };

@@ -431,42 +431,42 @@ __global__ void __launch_bounds__(128) cand_begin_minkowski_kernel(
               __double2float_ru(mg), 0.f, 0.f, __double2float_rd(lo), __double2float_ru(hi));
 }
 
-sdb_status cand_begin(Corpus* c, uint32_t nq, int screen, cudaStream_t st) {
+sdb_status cand_begin(const Corpus* c, Scratch& s, uint32_t nq, int screen, cudaStream_t st) {
   switch (family(c)) {
     case Family::Lp:
       if (const int p = minkowski_screen_order(c)) {
-        SDB_CUDA(cudaMemsetAsync(c->d_mscale, 0, sizeof(uint32_t), st));
-        minkowski_batch_max_kernel<<<(nq + 3) / 4, 128, 0, st>>>(c->d_q32, c->d_qflags, nq, c->dim, c->d_mscale);
-        cand_begin_minkowski_kernel<<<(nq + 3) / 4, 128, 0, st>>>(c->d_tau, c->d_cand_cnt, c->d_flags, c->d_stat,
-                                                                  c->d_bscale, c->d_beps, c->d_margin, c->d_margin2,
-                                                                  c->d_beps2, c->d_tau2, c->d_qlow, c->d_qcap, c->d_q32,
-                                                                  nq, c->dim, p, c->max_norm, c->d_mscale,
+        SDB_CUDA(cudaMemsetAsync(s.d_mscale, 0, sizeof(uint32_t), st));
+        minkowski_batch_max_kernel<<<(nq + 3) / 4, 128, 0, st>>>(s.d_q32, s.d_qflags, nq, c->dim, s.d_mscale);
+        cand_begin_minkowski_kernel<<<(nq + 3) / 4, 128, 0, st>>>(s.d_tau, s.d_cand_cnt, s.d_flags, s.d_stat,
+                                                                  s.d_bscale, s.d_beps, s.d_margin, s.d_margin2,
+                                                                  s.d_beps2, s.d_tau2, s.d_qlow, s.d_qcap, s.d_q32,
+                                                                  nq, c->dim, p, c->max_norm, s.d_mscale,
                                                                   c->exact ? 1 : 0);
         count_launch(c->ctx);
       } else {
-        cand_begin_lp_kernel<<<(nq + 3) / 4, 128, 0, st>>>(c->d_tau, c->d_cand_cnt, c->d_flags, c->d_stat,
-                                                           c->d_bscale, c->d_beps, c->d_margin, c->d_margin2,
-                                                           c->d_beps2, c->d_tau2, c->d_qlow, c->d_qcap, c->d_q32, nq,
+        cand_begin_lp_kernel<<<(nq + 3) / 4, 128, 0, st>>>(s.d_tau, s.d_cand_cnt, s.d_flags, s.d_stat,
+                                                           s.d_bscale, s.d_beps, s.d_margin, s.d_margin2,
+                                                           s.d_beps2, s.d_tau2, s.d_qlow, s.d_qcap, s.d_q32, nq,
                                                            (int)c->metric, c->dim, c->max_norm, c->exact ? 1 : 0);
       }
       break;
     case Family::Centred:
       // the cosine bounds of the centred operands with the F64 terms (the rows are centred in f64, whatever their
       // type); the gap between their cosine and the reference's pearson is cand_final's eps_ref
-      cand_begin_kernel<<<(nq + 255) / 256, 256, 0, st>>>(c->d_tau, c->d_cand_cnt, c->d_flags, c->d_stat, c->d_bscale,
-                                                          c->d_beps, c->d_margin, c->d_margin2, c->d_beps2, c->d_tau2,
-                                                          c->d_qlow, c->d_qcap, c->d_qmag, c->d_q8scale, c->d_q8err,
-                                                          c->d_qbferr, nq, screen, (int)SDB_COSINE, c->dim,
+      cand_begin_kernel<<<(nq + 255) / 256, 256, 0, st>>>(s.d_tau, s.d_cand_cnt, s.d_flags, s.d_stat, s.d_bscale,
+                                                          s.d_beps, s.d_margin, s.d_margin2, s.d_beps2, s.d_tau2,
+                                                          s.d_qlow, s.d_qcap, s.d_qmag, s.d_q8scale, s.d_q8err,
+                                                          s.d_qbferr, nq, screen, (int)SDB_COSINE, c->dim,
                                                           c->max_rel_qerr, c->i8_scale, c->bf16_rel_err, c->max_norm,
                                                           c->exact ? 1 : 0, 1);
       break;
     case Family::Dot:
     case Family::Count:  // (Count, Exact: the reset of tau, counts, flags and stat; their bounds go unused)
     case Family::Exact:
-      cand_begin_kernel<<<(nq + 255) / 256, 256, 0, st>>>(c->d_tau, c->d_cand_cnt, c->d_flags, c->d_stat, c->d_bscale,
-                                                          c->d_beps, c->d_margin, c->d_margin2, c->d_beps2, c->d_tau2,
-                                                          c->d_qlow, c->d_qcap, c->d_qmag, c->d_q8scale, c->d_q8err,
-                                                          c->d_qbferr, nq, screen, (int)c->metric, c->dim,
+      cand_begin_kernel<<<(nq + 255) / 256, 256, 0, st>>>(s.d_tau, s.d_cand_cnt, s.d_flags, s.d_stat, s.d_bscale,
+                                                          s.d_beps, s.d_margin, s.d_margin2, s.d_beps2, s.d_tau2,
+                                                          s.d_qlow, s.d_qcap, s.d_qmag, s.d_q8scale, s.d_q8err,
+                                                          s.d_qbferr, nq, screen, (int)c->metric, c->dim,
                                                           c->max_rel_qerr, c->i8_scale, c->bf16_rel_err, c->max_norm,
                                                           c->exact ? 1 : 0, c->dtype == SDB_F64 ? 1 : 0);
       break;
@@ -476,12 +476,11 @@ sdb_status cand_begin(Corpus* c, uint32_t nq, int screen, cudaStream_t st) {
   return SDB_OK;
 }
 
-static sdb_status ensure_scratch(Corpus* c, uint32_t nq, uint32_t cap) {
+sdb_status scratch_for(const Corpus* c, Scratch& s, uint32_t nq, uint32_t cap) {
   const uint32_t nq_pad = (nq + 127) / 128 * 128;
-  if (c->sc_nq >= nq_pad && c->sc_cap >= cap) return SDB_OK;
-  const uint32_t nqa = nq_pad > c->sc_nq ? nq_pad : c->sc_nq;
-  const uint32_t capa = cap > c->sc_cap ? cap : c->sc_cap;
-  Scratch& s = *c;
+  if (s.sc_nq >= nq_pad && s.sc_cap >= cap) return SDB_OK;
+  const uint32_t nqa = nq_pad > s.sc_nq ? nq_pad : s.sc_nq;
+  const uint32_t capa = cap > s.sc_cap ? cap : s.sc_cap;
   s = Scratch();  // everything below is reallocated: prepared queries, candidate lists ... are gone
   auto alloc = [&]() -> sdb_status {
     s.rr_stride = capa + SPECIAL_CAP;
@@ -496,9 +495,9 @@ static sdb_status ensure_scratch(Corpus* c, uint32_t nq, uint32_t cap) {
     SDB_CUDA(s.d_cand_cnt.reserve(nqa));
     SDB_CUDA(s.d_flags.reserve(nqa));
     SDB_CUDA(s.d_stat.reserve(4));
-    SDB_CUDA(s.d_rr_key.reserve((size_t)nqa * c->rr_stride));
-    SDB_CUDA(s.d_rr_dist.reserve((size_t)nqa * c->rr_stride));
-    SDB_CUDA(s.d_rr_row.reserve((size_t)nqa * c->rr_stride));
+    SDB_CUDA(s.d_rr_key.reserve((size_t)nqa * s.rr_stride));
+    SDB_CUDA(s.d_rr_dist.reserve((size_t)nqa * s.rr_stride));
+    SDB_CUDA(s.d_rr_row.reserve((size_t)nqa * s.rr_stride));
     SDB_CUDA(s.d_q8.reserve((size_t)nqa * (c->dim_pad8 ? c->dim_pad8 : 128)));
     SDB_CUDA(s.d_q8scale.reserve(nqa));
     SDB_CUDA(s.d_q8err.reserve(nqa));
@@ -524,8 +523,8 @@ static sdb_status ensure_scratch(Corpus* c, uint32_t nq, uint32_t cap) {
     SDB_CUDA(s.d_probe.reserve((size_t)nqa * PROBE_STRIDE));
     s.sub_slots = 2 * (uint32_t)c->ctx->sm_count;
     s.sub_cap = 16;
-    SDB_CUDA(s.d_sub.reserve((size_t)nqa * c->sub_slots * c->sub_cap));
-    SDB_CUDA(s.d_sub_cnt.reserve((size_t)nqa * c->sub_slots));
+    SDB_CUDA(s.d_sub.reserve((size_t)nqa * s.sub_slots * s.sub_cap));
+    SDB_CUDA(s.d_sub_cnt.reserve((size_t)nqa * s.sub_slots));
     return SDB_OK;
   };
   const sdb_status rc = alloc();
@@ -538,25 +537,23 @@ static sdb_status ensure_scratch(Corpus* c, uint32_t nq, uint32_t cap) {
   return SDB_OK;
 }
 
-sdb_status scratch_for(Corpus* c, uint32_t nq, uint32_t cap) { return ensure_scratch(c, nq, cap); }
-
-sdb_status prep_queries(Corpus* c, const double* d_queries, uint32_t nq, cudaStream_t st) {
-  // d_queries may alias c->d_q64
-  if (d_queries != c->d_q64)
-    SDB_CUDA(cudaMemcpyAsync(c->d_q64, d_queries, sizeof(double) * (size_t)nq * c->dim, cudaMemcpyDeviceToDevice, st));
+sdb_status prep_queries(const Corpus* c, Scratch& s, const double* d_queries, uint32_t nq, cudaStream_t st) {
+  // d_queries may alias s.d_q64
+  if (d_queries != s.d_q64)
+    SDB_CUDA(cudaMemcpyAsync(s.d_q64, d_queries, sizeof(double) * (size_t)nq * c->dim, cudaMemcpyDeviceToDevice, st));
   const uint32_t nq_pad = (nq + 127) / 128 * 128;
   const Family f = family(c);
   if (f == Family::Centred)
-    prep_queries_pearson_kernel<<<nq_pad, 128, 0, st>>>(c->d_q64, c->dim, c->dim_pad, c->d_q32, c->d_qbf16, c->d_qmag,
-                                                        c->d_qmom, c->d_qflags, c->d_qbferr, nq);
+    prep_queries_pearson_kernel<<<nq_pad, 128, 0, st>>>(s.d_q64, c->dim, c->dim_pad, s.d_q32, s.d_qbf16, s.d_qmag,
+                                                        s.d_qmom, s.d_qflags, s.d_qbferr, nq);
   else
-    prep_queries_kernel<<<nq_pad, 128, 0, st>>>(c->d_q64, c->dim, c->dim_pad, (int)c->metric, c->d_q32, c->d_qbf16,
-                                                c->d_qmag, c->d_qflags, c->d_qbferr, nq);
+    prep_queries_kernel<<<nq_pad, 128, 0, st>>>(s.d_q64, c->dim, c->dim_pad, (int)c->metric, s.d_q32, s.d_qbf16,
+                                                s.d_qmag, s.d_qflags, s.d_qbferr, nq);
   count_launch(c->ctx);
-  if (f == Family::Count) SDB_TRY(count_prep_queries(c, nq, st));
+  if (f == Family::Count) SDB_TRY(count_prep_queries(c, s, nq, st));
   if (c->d_i8) {
-    prep_queries_i8_kernel<<<nq_pad, 128, 0, st>>>(c->d_q32, c->d_qmag, c->dim, c->dim_pad8, nq, c->d_q8, c->d_q8scale,
-                                                   c->d_q8err);
+    prep_queries_i8_kernel<<<nq_pad, 128, 0, st>>>(s.d_q32, s.d_qmag, c->dim, c->dim_pad8, nq, s.d_q8, s.d_q8scale,
+                                                   s.d_q8err);
     count_launch(c->ctx);
   }
   SDB_CUDA(cudaGetLastError());
@@ -582,8 +579,8 @@ __global__ void cand_set_count_kernel(uint32_t* cnt, uint32_t nq, uint32_t value
   const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i < nq) cnt[i] = value;
 }
-sdb_status cand_set_count(Corpus* c, uint32_t nq, uint32_t value, cudaStream_t st) {
-  cand_set_count_kernel<<<(nq + 255) / 256, 256, 0, st>>>(c->d_cand_cnt, nq, value);
+sdb_status cand_set_count(const Corpus* c, Scratch& s, uint32_t nq, uint32_t value, cudaStream_t st) {
+  cand_set_count_kernel<<<(nq + 255) / 256, 256, 0, st>>>(s.d_cand_cnt, nq, value);
   count_launch(c->ctx);
   SDB_CUDA(cudaGetLastError());
   return SDB_OK;
@@ -599,8 +596,8 @@ __global__ void __launch_bounds__(256) cand_filter_list_kernel(Cand* __restrict_
   for (uint32_t i = threadIdx.x; i < n; i += blockDim.x)
     if (!filt_pass(filt, q, cq[i].row)) cq[i].score = __int_as_float(0x7fc00000);
 }
-sdb_status cand_filter_list(Corpus* c, uint32_t nq, cudaStream_t st) {
-  cand_filter_list_kernel<<<nq, 256, 0, st>>>(c->d_cand, c->d_cand_cnt, c->sc_cap, c->filt);
+sdb_status cand_filter_list(const Corpus* c, Scratch& s, const FiltArg& filt, uint32_t nq, cudaStream_t st) {
+  cand_filter_list_kernel<<<nq, 256, 0, st>>>(s.d_cand, s.d_cand_cnt, s.sc_cap, filt);
   count_launch(c->ctx);
   SDB_CUDA(cudaGetLastError());
   return SDB_OK;
@@ -627,10 +624,10 @@ __global__ void __launch_bounds__(256) cand_add_specials_kernel(Cand* __restrict
     }
   }
 }
-sdb_status cand_add_specials(Corpus* c, uint32_t nq, cudaStream_t st) {
+sdb_status cand_add_specials(const Corpus* c, Scratch& s, const FiltArg& filt, uint32_t nq, cudaStream_t st) {
   if (!c->n_special) return SDB_OK;
-  cand_add_specials_kernel<<<nq, 256, 0, st>>>(c->d_cand, c->d_cand_cnt, c->d_flags, c->sc_cap, c->d_special,
-                                               c->n_special, c->filt);
+  cand_add_specials_kernel<<<nq, 256, 0, st>>>(s.d_cand, s.d_cand_cnt, s.d_flags, s.sc_cap, c->d_special,
+                                               c->n_special, filt);
   count_launch(c->ctx);
   SDB_CUDA(cudaGetLastError());
   return SDB_OK;
@@ -663,8 +660,8 @@ __global__ void __launch_bounds__(256) cand_direct_kernel(Cand* __restrict__ can
     }
   }
 }
-sdb_status cand_direct(Corpus* c, uint32_t nq, cudaStream_t st) {
-  cand_direct_kernel<<<nq, 256, 0, st>>>(c->d_cand, c->d_cand_cnt, c->d_flags, c->sc_cap, c->filt, c->d_skip, c->n);
+sdb_status cand_direct(const Corpus* c, Scratch& s, const FiltArg& filt, uint32_t nq, cudaStream_t st) {
+  cand_direct_kernel<<<nq, 256, 0, st>>>(s.d_cand, s.d_cand_cnt, s.d_flags, s.sc_cap, filt, c->d_skip, c->n);
   count_launch(c->ctx);
   SDB_CUDA(cudaGetLastError());
   return SDB_OK;
@@ -737,9 +734,10 @@ __global__ void __launch_bounds__(128) cand_seed_probe_kernel(const float* __res
     cnt[q] = 0;
   }
 }
-sdb_status cand_seed_from_probe(Corpus* c, uint32_t nq, uint32_t k, uint32_t n_tiles, cudaStream_t st) {
-  cand_seed_probe_kernel<<<nq, 128, 0, st>>>(c->d_probe, n_tiles * 8, k, c->d_margin, c->d_qlow, c->d_qcap, c->d_tau,
-                                             c->d_cand_cnt, c->d_hparam, c->d_hist);
+sdb_status cand_seed_from_probe(const Corpus* c, Scratch& s, uint32_t nq, uint32_t k, uint32_t n_tiles,
+                                cudaStream_t st) {
+  cand_seed_probe_kernel<<<nq, 128, 0, st>>>(s.d_probe, n_tiles * 8, k, s.d_margin, s.d_qlow, s.d_qcap, s.d_tau,
+                                             s.d_cand_cnt, s.d_hparam, s.d_hist);
   count_launch(c->ctx);
   SDB_CUDA(cudaGetLastError());
   return SDB_OK;
@@ -913,20 +911,20 @@ __global__ void __launch_bounds__(256) cand_select_kernel(Cand* __restrict__ can
   if (hparam) hist[(size_t)q * HIST_BINS + threadIdx.x] = s_hist[threadIdx.x];
 }
 
-sdb_status cand_select(Corpus* c, uint32_t nq, uint32_t k, bool drop_invalid, uint32_t n_slots, bool seed_hist,
-                       cudaStream_t st, int stage) {
+sdb_status cand_select(const Corpus* c, Scratch& s, uint32_t nq, uint32_t k, bool drop_invalid, uint32_t n_slots,
+                       bool seed_hist, cudaStream_t st, int stage) {
   if (stage == 1) {  // stage B: the lists hold f32 scores now; own threshold / margin, nothing else to gather
-    cand_select_kernel<<<nq, 256, 0, st>>>(c->d_cand, c->d_cand_cnt, c->d_tau2, c->d_flags, c->sc_cap, k, c->d_margin2,
-                                           nullptr, c->d_sub, c->d_sub_cnt, 0u, c->sub_cap, nullptr, c->d_hist, c->d_qlow,
-                                           c->d_qcap, nullptr, c->d_rr_key, c->rr_stride);
+    cand_select_kernel<<<nq, 256, 0, st>>>(s.d_cand, s.d_cand_cnt, s.d_tau2, s.d_flags, s.sc_cap, k, s.d_margin2,
+                                           nullptr, s.d_sub, s.d_sub_cnt, 0u, s.sub_cap, nullptr, s.d_hist, s.d_qlow,
+                                           s.d_qcap, nullptr, s.d_rr_key, s.rr_stride);
     count_launch(c->ctx);
     SDB_CUDA(cudaGetLastError());
     return SDB_OK;
   }
   cand_select_kernel<<<nq, 256, 0, st>>>(  // 256 threads: several blocks per SM, the whole batch is one wave
-      c->d_cand, c->d_cand_cnt, c->d_tau, c->d_flags, c->sc_cap, k, c->d_margin, drop_invalid ? c->d_snorm.get() : nullptr,
-      c->d_sub, c->d_sub_cnt, n_slots, c->sub_cap, seed_hist ? c->d_hparam.get() : nullptr, c->d_hist, c->d_qlow, c->d_qcap,
-      c->d_stat, c->d_rr_key, c->rr_stride);
+      s.d_cand, s.d_cand_cnt, s.d_tau, s.d_flags, s.sc_cap, k, s.d_margin, drop_invalid ? c->d_snorm.get() : nullptr,
+      s.d_sub, s.d_sub_cnt, n_slots, s.sub_cap, seed_hist ? s.d_hparam.get() : nullptr, s.d_hist, s.d_qlow, s.d_qcap,
+      s.d_stat, s.d_rr_key, s.rr_stride);
   count_launch(c->ctx);
   SDB_CUDA(cudaGetLastError());
   return SDB_OK;
@@ -1019,32 +1017,32 @@ __global__ void __launch_bounds__(128) cand_refine_f32_kernel(const T* __restric
     }
   }
 }
-sdb_status cand_refine(Corpus* c, uint32_t nq, cudaStream_t st) {
+sdb_status cand_refine(const Corpus* c, Scratch& s, uint32_t nq, cudaStream_t st) {
   const dim3 grid(nq, 8);  // 128-thread blocks (register budget beside a resident screen CTA)
   const float* f32_rows = (const float*)c->d_rows.get();
   const double* f64_rows = (const double*)c->d_rows.get();
   switch (family(c)) {
     case Family::Centred:
       if (c->dtype == SDB_F32)
-        cand_refine_f32_kernel<float, true, true><<<grid, 128, 0, st>>>(f32_rows, c->dim, c->d_snorm, c->d_q32,
-                                                                        c->d_cand, c->d_cand_cnt, c->sc_cap, c->d_mom);
+        cand_refine_f32_kernel<float, true, true><<<grid, 128, 0, st>>>(f32_rows, c->dim, c->d_snorm, s.d_q32,
+                                                                        s.d_cand, s.d_cand_cnt, s.sc_cap, c->d_mom);
       else
-        cand_refine_f32_kernel<double, true, true><<<grid, 128, 0, st>>>(f64_rows, c->dim, c->d_snorm, c->d_q32,
-                                                                         c->d_cand, c->d_cand_cnt, c->sc_cap, c->d_mom);
+        cand_refine_f32_kernel<double, true, true><<<grid, 128, 0, st>>>(f64_rows, c->dim, c->d_snorm, s.d_q32,
+                                                                         s.d_cand, s.d_cand_cnt, s.sc_cap, c->d_mom);
       break;
     case Family::Dot:
       if (c->dtype == SDB_F32 && c->metric == SDB_COSINE)
-        cand_refine_f32_kernel<float, true><<<grid, 128, 0, st>>>(f32_rows, c->dim, c->d_snorm, c->d_q32, c->d_cand,
-                                                                  c->d_cand_cnt, c->sc_cap, nullptr);
+        cand_refine_f32_kernel<float, true><<<grid, 128, 0, st>>>(f32_rows, c->dim, c->d_snorm, s.d_q32, s.d_cand,
+                                                                  s.d_cand_cnt, s.sc_cap, nullptr);
       else if (c->dtype == SDB_F32)
-        cand_refine_f32_kernel<float, false><<<grid, 128, 0, st>>>(f32_rows, c->dim, c->d_snorm, c->d_q32, c->d_cand,
-                                                                   c->d_cand_cnt, c->sc_cap, nullptr);
+        cand_refine_f32_kernel<float, false><<<grid, 128, 0, st>>>(f32_rows, c->dim, c->d_snorm, s.d_q32, s.d_cand,
+                                                                   s.d_cand_cnt, s.sc_cap, nullptr);
       else if (c->metric == SDB_COSINE)
-        cand_refine_f32_kernel<double, true><<<grid, 128, 0, st>>>(f64_rows, c->dim, c->d_snorm, c->d_q32, c->d_cand,
-                                                                   c->d_cand_cnt, c->sc_cap, nullptr);
+        cand_refine_f32_kernel<double, true><<<grid, 128, 0, st>>>(f64_rows, c->dim, c->d_snorm, s.d_q32, s.d_cand,
+                                                                   s.d_cand_cnt, s.sc_cap, nullptr);
       else
-        cand_refine_f32_kernel<double, false><<<grid, 128, 0, st>>>(f64_rows, c->dim, c->d_snorm, c->d_q32, c->d_cand,
-                                                                    c->d_cand_cnt, c->sc_cap, nullptr);
+        cand_refine_f32_kernel<double, false><<<grid, 128, 0, st>>>(f64_rows, c->dim, c->d_snorm, s.d_q32, s.d_cand,
+                                                                    s.d_cand_cnt, s.sc_cap, nullptr);
       break;
     default: break;  // stage B follows the tensor-core screens (Dot, Centred) only
   }
@@ -1074,7 +1072,7 @@ __device__ __forceinline__ void rr_store(const RerankOut& out, uint32_t q, uint3
   out.dist[o] = d;
   out.row[o] = row;
 }
-static RerankOut rr_out(const Corpus* c) { return RerankOut{c->d_rr_key, c->d_rr_dist, c->d_rr_row, c->rr_stride}; }
+static RerankOut rr_out(const Scratch& s) { return RerankOut{s.d_rr_key, s.d_rr_dist, s.d_rr_row, s.rr_stride}; }
 
 // the COSINE / EUCLIDEAN finish of one entry
 __device__ __forceinline__ double dot_finish(bool cosine, const RefSum& s, const double* mag, uint32_t row, double qm,
@@ -1339,64 +1337,65 @@ __global__ void __launch_bounds__(128) cand_rerank_entry_kernel(
 }
 
 template <int M>
-static void rerank_entry(Corpus* c, uint32_t nq, uint32_t n_sp, cudaStream_t st) {
+static void rerank_entry(const Corpus* c, Scratch& s, uint32_t nq, uint32_t n_sp, cudaStream_t st) {
   const dim3 grid(nq, RR_GROUPS_Y);
-  const EntryArgs a{c->minkowski_p, c->d_mom, c->d_qmom, c->d_jfirst, c->d_jux, c->d_qkey.get(), c->d_qjac};
+  const EntryArgs a{c->minkowski_p, c->d_mom, s.d_qmom, c->d_jfirst, c->d_jux, s.d_qkey.get(), s.d_qjac};
   if (c->dtype == SDB_F32)
-    cand_rerank_entry_kernel<float, M><<<grid, 128, 0, st>>>((const float*)c->d_rows.get(), c->dim, c->d_q64, c->d_qflags,
-                                                             c->d_cand, c->d_cand_cnt, c->sc_cap, c->d_special, n_sp,
-                                                             rr_out(c), a);
+    cand_rerank_entry_kernel<float, M><<<grid, 128, 0, st>>>((const float*)c->d_rows.get(), c->dim, s.d_q64, s.d_qflags,
+                                                             s.d_cand, s.d_cand_cnt, s.sc_cap, c->d_special, n_sp,
+                                                             rr_out(s), a);
   else
-    cand_rerank_entry_kernel<double, M><<<grid, 128, 0, st>>>((const double*)c->d_rows.get(), c->dim, c->d_q64,
-                                                              c->d_qflags, c->d_cand, c->d_cand_cnt, c->sc_cap,
-                                                              c->d_special, n_sp, rr_out(c), a);
+    cand_rerank_entry_kernel<double, M><<<grid, 128, 0, st>>>((const double*)c->d_rows.get(), c->dim, s.d_q64,
+                                                              s.d_qflags, s.d_cand, s.d_cand_cnt, s.sc_cap,
+                                                              c->d_special, n_sp, rr_out(s), a);
 }
 
 template <typename T>
-static void rerank_packed(Corpus* c, uint32_t nq, uint32_t n_sp, cudaStream_t st) {
+static void rerank_packed(const Corpus* c, Scratch& s, uint32_t nq, uint32_t n_sp, cudaStream_t st) {
   auto kern = c->metric == SDB_COSINE ? cand_rerank_packed_kernel<T, SDB_COSINE> : cand_rerank_packed_kernel<T, SDB_EUCLIDEAN>;
-  kern<<<(nq + 7) / 8, 128, 0, st>>>((const T*)c->d_rows.get(), c->dim, c->d_mag, c->d_q64, c->d_qmag, c->d_qflags,
-                                     c->d_cand, c->d_cand_cnt, c->sc_cap, c->d_special, n_sp, nq, rr_out(c));
+  kern<<<(nq + 7) / 8, 128, 0, st>>>((const T*)c->d_rows.get(), c->dim, c->d_mag, s.d_q64, s.d_qmag, s.d_qflags,
+                                     s.d_cand, s.d_cand_cnt, s.sc_cap, c->d_special, n_sp, nq, rr_out(s));
 }
 
 // COSINE / EUCLIDEAN: the packed kernel for the small sets stage B leaves; otherwise the vectorised one for f32 rows
 // of a length divisible by 4, the staged one for the rest
-static void rerank_dot(Corpus* c, uint32_t nq, bool small_sets, uint32_t n_sp, cudaStream_t st) {
+static void rerank_dot(const Corpus* c, Scratch& s, uint32_t nq, bool small_sets, uint32_t n_sp, cudaStream_t st) {
   const dim3 grid(nq, RR_GROUPS_Y);
-  if (small_sets && c->dtype == SDB_F32) rerank_packed<float>(c, nq, n_sp, st);
-  else if (small_sets) rerank_packed<double>(c, nq, n_sp, st);
+  if (small_sets && c->dtype == SDB_F32) rerank_packed<float>(c, s, nq, n_sp, st);
+  else if (small_sets) rerank_packed<double>(c, s, nq, n_sp, st);
   else if (c->dtype == SDB_F32 && c->dim % 4 == 0)
     cand_rerank_v4_kernel<<<grid, RR_WARPS * 32, RRV_SMEM, st>>>((const float*)c->d_rows.get(), c->dim, (int)c->metric,
-                                                                c->d_mag, c->d_q64, c->d_qmag, c->d_qflags, c->d_cand,
-                                                                c->d_cand_cnt, c->sc_cap, c->d_special, n_sp, rr_out(c));
+                                                                c->d_mag, s.d_q64, s.d_qmag, s.d_qflags, s.d_cand,
+                                                                s.d_cand_cnt, s.sc_cap, c->d_special, n_sp, rr_out(s));
   else if (c->dtype == SDB_F32)
     cand_rerank_kernel<float><<<grid, RR_WARPS * 32, 0, st>>>((const float*)c->d_rows.get(), c->dim, (int)c->metric,
-                                                             c->d_mag, c->d_q64, c->d_qmag, c->d_qflags, c->d_cand,
-                                                             c->d_cand_cnt, c->sc_cap, c->d_special, n_sp, rr_out(c));
+                                                             c->d_mag, s.d_q64, s.d_qmag, s.d_qflags, s.d_cand,
+                                                             s.d_cand_cnt, s.sc_cap, c->d_special, n_sp, rr_out(s));
   else
     cand_rerank_kernel<double><<<grid, RR_WARPS * 32, 0, st>>>((const double*)c->d_rows.get(), c->dim, (int)c->metric,
-                                                              c->d_mag, c->d_q64, c->d_qmag, c->d_qflags, c->d_cand,
-                                                              c->d_cand_cnt, c->sc_cap, c->d_special, n_sp, rr_out(c));
+                                                              c->d_mag, s.d_q64, s.d_qmag, s.d_qflags, s.d_cand,
+                                                              s.d_cand_cnt, s.sc_cap, c->d_special, n_sp, rr_out(s));
 }
 
-sdb_status cand_rerank(Corpus* c, uint32_t nq, cudaStream_t st, bool small_sets) {
-  const uint32_t n_sp = c->filt.bits ? 0u : c->n_special;  // filtered: the passing special rows are in the lists
+sdb_status cand_rerank(const Corpus* c, Scratch& s, const FiltArg& filt, uint32_t nq, cudaStream_t st,
+                       bool small_sets) {
+  const uint32_t n_sp = filt.bits ? 0u : c->n_special;  // filtered: the passing special rows are in the lists
   switch (family(c)) {
     case Family::Count:  // (the direct regime only; no special rows)
-      if (c->metric == SDB_HAMMING) rerank_entry<SDB_HAMMING>(c, nq, n_sp, st);
-      else rerank_entry<SDB_JACCARD>(c, nq, n_sp, st);
+      if (c->metric == SDB_HAMMING) rerank_entry<SDB_HAMMING>(c, s, nq, n_sp, st);
+      else rerank_entry<SDB_JACCARD>(c, s, nq, n_sp, st);
       break;
     case Family::Lp:
-      if (c->metric == SDB_MANHATTAN) rerank_entry<SDB_MANHATTAN>(c, nq, n_sp, st);
-      else if (c->metric == SDB_MINKOWSKI) rerank_entry<SDB_MINKOWSKI>(c, nq, n_sp, st);
-      else rerank_entry<SDB_CHEBYSHEV>(c, nq, n_sp, st);
+      if (c->metric == SDB_MANHATTAN) rerank_entry<SDB_MANHATTAN>(c, s, nq, n_sp, st);
+      else if (c->metric == SDB_MINKOWSKI) rerank_entry<SDB_MINKOWSKI>(c, s, nq, n_sp, st);
+      else rerank_entry<SDB_CHEBYSHEV>(c, s, nq, n_sp, st);
       break;
     case Family::Centred:  // one kernel for small (after stage B) and large (direct regime, no stage B) sets
-      rerank_entry<SDB_PEARSON>(c, nq, n_sp, st);
+      rerank_entry<SDB_PEARSON>(c, s, nq, n_sp, st);
       break;
     case Family::Dot:
     case Family::Exact:  // (never reaches the re-rank: the exact kernel alone ranks it)
-      rerank_dot(c, nq, small_sets, n_sp, st);
+      rerank_dot(c, s, nq, small_sets, n_sp, st);
       break;
   }
   count_launch(c->ctx);
@@ -1545,14 +1544,14 @@ __global__ void __launch_bounds__(256)
   }
 }
 
-sdb_status cand_final(Corpus* c, uint32_t nq, uint32_t k, uint64_t row_base, uint64_t* d_out_rows, double* d_out_dist,
-                      uint32_t* d_out_count, cudaStream_t st) {
+sdb_status cand_final(const Corpus* c, Scratch& s, const FiltArg& filt, uint32_t nq, uint32_t k, uint64_t row_base,
+                      uint64_t* d_out_rows, double* d_out_dist, uint32_t* d_out_count, cudaStream_t st) {
   if (k > FIN_KEEP) {
     set_error("cand_final: k = %u exceeds the screened path's limit of %u", k, FIN_KEEP);
     return SDB_EINVAL;
   }
   static const int debug = getenv("SDB_DEBUG") != nullptr;
-  const uint32_t n_sp = c->filt.bits ? 0u : c->n_special;  // filtered: the passing special rows are in the lists
+  const uint32_t n_sp = filt.bits ? 0u : c->n_special;  // filtered: the passing special rows are in the lists
   auto fin = cand_final_kernel<Family::Dot>;
   double eps_ref = 0.0;
   switch (family(c)) {
@@ -1569,9 +1568,9 @@ sdb_status cand_final(Corpus* c, uint32_t nq, uint32_t k, uint64_t row_base, uin
       fin = cand_final_kernel<Family::Lp>;
       break;
   }
-  fin<<<nq, 256, 0, st>>>(c->d_rr_key, c->d_rr_dist, c->d_rr_row, c->rr_stride, c->d_cand_cnt, c->sc_cap, n_sp,
-                          c->d_tau, c->d_qmag, c->d_bscale, c->d_beps, c->d_tau2, c->d_beps2, c->d_flags, c->d_qflags,
-                          c->d_stat, (int)c->metric, k, row_base, d_out_rows, d_out_dist, d_out_count, debug, eps_ref);
+  fin<<<nq, 256, 0, st>>>(s.d_rr_key, s.d_rr_dist, s.d_rr_row, s.rr_stride, s.d_cand_cnt, s.sc_cap, n_sp,
+                          s.d_tau, s.d_qmag, s.d_bscale, s.d_beps, s.d_tau2, s.d_beps2, s.d_flags, s.d_qflags,
+                          s.d_stat, (int)c->metric, k, row_base, d_out_rows, d_out_dist, d_out_count, debug, eps_ref);
   count_launch(c->ctx);
   SDB_CUDA(cudaGetLastError());
   return SDB_OK;

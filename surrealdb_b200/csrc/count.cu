@@ -338,7 +338,8 @@ __global__ void count_qkeys_kernel(const double* __restrict__ q64, uint32_t nq, 
 // (query block, queries per thread) by batch size, as launch_lp_qb: a block larger than the batch counts padding
 // queries.  f64 keys stop at 32-query blocks, whose staging stays within the 48 KB of static shared memory.
 template <typename T, bool FILT, int QB, int TQ>
-static sdb_status launch_count(Corpus* c, uint32_t nq, uint32_t k, uint32_t n_ranges, cudaStream_t st) {
+static sdb_status launch_count(const Corpus* c, Scratch& s, const FiltArg& filt, uint32_t nq, uint32_t k,
+                               uint32_t n_ranges, cudaStream_t st) {
   auto kern = count_hamming_kernel<T, FILT, QB, TQ>;
   const size_t smem = sizeof(uint64_t) * QB * k;
   SDB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(sizeof(uint64_t) * QB * 256)));
@@ -351,23 +352,19 @@ static sdb_status launch_count(Corpus* c, uint32_t nq, uint32_t k, uint32_t n_ra
   uint64_t grid = (uint64_t)c->ctx->sm_count * per_sm;
   if (grid > items) grid = items;
   kern<<<(unsigned)grid, LP_THREADS, smem, st>>>((const T*)c->d_rows.get(), c->dim, c->n, c->d_skip,
-                                                 (const CountKey<T>*)c->d_qkey.get(), nq, k, n_ranges, c->d_cand_cnt,
-                                                 c->d_rr_key, c->d_rr_dist, c->d_rr_row, c->rr_stride, c->filt);
+                                                 (const CountKey<T>*)s.d_qkey.get(), nq, k, n_ranges, s.d_cand_cnt,
+                                                 s.d_rr_key, s.d_rr_dist, s.d_rr_row, s.rr_stride, filt);
   count_launch(c->ctx);
   SDB_CUDA(cudaGetLastError());
   return SDB_OK;
 }
 template <typename T, bool FILT>
-static sdb_status launch_count_qb(Corpus* c, uint32_t nq, uint32_t k, uint32_t n_ranges, cudaStream_t st) {
-  if (nq <= 8) return launch_count<T, FILT, 8, 1>(c, nq, k, n_ranges, st);
-  if constexpr (sizeof(T) == 8) return launch_count<T, FILT, 32, 4>(c, nq, k, n_ranges, st);
-  else return nq <= 32 ? launch_count<T, FILT, 32, 4>(c, nq, k, n_ranges, st)
-                       : launch_count<T, FILT, 64, 4>(c, nq, k, n_ranges, st);
-}
-template <typename T>
-static sdb_status launch_count_type(Corpus* c, uint32_t nq, uint32_t k, uint32_t n_ranges, cudaStream_t st) {
-  return c->filt.bits ? launch_count_qb<T, true>(c, nq, k, n_ranges, st)
-                      : launch_count_qb<T, false>(c, nq, k, n_ranges, st);
+static sdb_status launch_count_qb(const Corpus* c, Scratch& s, const FiltArg& filt, uint32_t nq, uint32_t k,
+                                  uint32_t n_ranges, cudaStream_t st) {
+  if (nq <= 8) return launch_count<T, FILT, 8, 1>(c, s, filt, nq, k, n_ranges, st);
+  if constexpr (sizeof(T) == 8) return launch_count<T, FILT, 32, 4>(c, s, filt, nq, k, n_ranges, st);
+  else return nq <= 32 ? launch_count<T, FILT, 32, 4>(c, s, filt, nq, k, n_ranges, st)
+                       : launch_count<T, FILT, 64, 4>(c, s, filt, nq, k, n_ranges, st);
 }
 
 uint32_t count_ranges(const Corpus* c, uint32_t nq, uint32_t k) {
@@ -384,20 +381,20 @@ uint32_t count_ranges(const Corpus* c, uint32_t nq, uint32_t k) {
   return s < 1 ? 1u : (uint32_t)s;
 }
 
-sdb_status count_prep_queries(Corpus* c, uint32_t nq, cudaStream_t st) {
+sdb_status count_prep_queries(const Corpus* c, Scratch& s, uint32_t nq, cudaStream_t st) {
   if (nq == 0) return SDB_OK;
   if (c->metric == SDB_JACCARD) {
     if (c->dtype == SDB_F32)
-      count_jaccard_qprep_kernel<uint32_t><<<nq, 256, 0, st>>>(c->d_q64, nq, c->dim, c->d_qkey.get(), c->d_qjac,
-                                                               c->d_qjac + 2 * (size_t)c->sc_nq);
+      count_jaccard_qprep_kernel<uint32_t><<<nq, 256, 0, st>>>(s.d_q64, nq, c->dim, s.d_qkey.get(), s.d_qjac,
+                                                               s.d_qjac + 2 * (size_t)s.sc_nq);
     else
       count_jaccard_qprep_kernel<unsigned long long><<<nq, 256, 0, st>>>(
-          c->d_q64, nq, c->dim, (unsigned long long*)c->d_qkey.get(), c->d_qjac, c->d_qjac + 2 * (size_t)c->sc_nq);
+          s.d_q64, nq, c->dim, (unsigned long long*)s.d_qkey.get(), s.d_qjac, s.d_qjac + 2 * (size_t)s.sc_nq);
   } else if (c->dtype == SDB_F32) {
-    count_qkeys_kernel<uint32_t><<<nq, 128, 0, st>>>(c->d_q64, nq, c->dim, c->d_qkey.get());
+    count_qkeys_kernel<uint32_t><<<nq, 128, 0, st>>>(s.d_q64, nq, c->dim, s.d_qkey.get());
   } else {
-    count_qkeys_kernel<unsigned long long><<<nq, 128, 0, st>>>(c->d_q64, nq, c->dim,
-                                                               (unsigned long long*)c->d_qkey.get());
+    count_qkeys_kernel<unsigned long long><<<nq, 128, 0, st>>>(s.d_q64, nq, c->dim,
+                                                               (unsigned long long*)s.d_qkey.get());
   }
   count_launch(c->ctx);
   SDB_CUDA(cudaGetLastError());
@@ -405,7 +402,8 @@ sdb_status count_prep_queries(Corpus* c, uint32_t nq, cudaStream_t st) {
 }
 
 template <typename T, bool FILT>
-static sdb_status launch_count_jaccard(Corpus* c, uint32_t nq, uint32_t k, uint32_t n_ranges, cudaStream_t st) {
+static sdb_status launch_count_jaccard(const Corpus* c, Scratch& s, const FiltArg& filt, uint32_t nq, uint32_t k,
+                                       uint32_t n_ranges, cudaStream_t st) {
   auto kern = count_jaccard_kernel<T, FILT>;
   const size_t smem = sizeof(JEntry) * JQ_QB * k;  // at most 32 KB
   int per_sm = 1;
@@ -417,26 +415,29 @@ static sdb_status launch_count_jaccard(Corpus* c, uint32_t nq, uint32_t k, uint3
   uint64_t grid = (uint64_t)c->ctx->sm_count * per_sm;
   if (grid > items) grid = items;
   kern<<<(unsigned)grid, JQ_QB * 32, smem, st>>>((const T*)c->d_rows.get(), c->dim, c->n, c->d_skip, c->d_jfirst,
-                                                 c->d_jux, (const EqKey<T>*)c->d_qkey.get(), c->d_qjac, nq, k,
-                                                 n_ranges, c->d_cand_cnt, c->d_rr_key, c->d_rr_dist, c->d_rr_row,
-                                                 c->rr_stride, c->filt);
+                                                 c->d_jux, (const EqKey<T>*)s.d_qkey.get(), s.d_qjac, nq, k,
+                                                 n_ranges, s.d_cand_cnt, s.d_rr_key, s.d_rr_dist, s.d_rr_row,
+                                                 s.rr_stride, filt);
   count_launch(c->ctx);
   SDB_CUDA(cudaGetLastError());
   return SDB_OK;
 }
 
-sdb_status count_pass(Corpus* c, uint32_t nq, uint32_t k, cudaStream_t st) {
+sdb_status count_pass(const Corpus* c, Scratch& s, const FiltArg& filt, uint32_t nq, uint32_t k, cudaStream_t st) {
   if (nq == 0 || k == 0 || c->n == 0) return SDB_OK;
   const uint32_t n_ranges = count_ranges(c, nq, k);
   if (c->metric == SDB_JACCARD) {
     if (c->dtype == SDB_F32)
-      return c->filt.bits ? launch_count_jaccard<float, true>(c, nq, k, n_ranges, st)
-                          : launch_count_jaccard<float, false>(c, nq, k, n_ranges, st);
-    return c->filt.bits ? launch_count_jaccard<double, true>(c, nq, k, n_ranges, st)
-                        : launch_count_jaccard<double, false>(c, nq, k, n_ranges, st);
+      return filt.bits ? launch_count_jaccard<float, true>(c, s, filt, nq, k, n_ranges, st)
+                       : launch_count_jaccard<float, false>(c, s, filt, nq, k, n_ranges, st);
+    return filt.bits ? launch_count_jaccard<double, true>(c, s, filt, nq, k, n_ranges, st)
+                     : launch_count_jaccard<double, false>(c, s, filt, nq, k, n_ranges, st);
   }
-  return c->dtype == SDB_F32 ? launch_count_type<float>(c, nq, k, n_ranges, st)
-                             : launch_count_type<double>(c, nq, k, n_ranges, st);
+  if (c->dtype == SDB_F32)
+    return filt.bits ? launch_count_qb<float, true>(c, s, filt, nq, k, n_ranges, st)
+                     : launch_count_qb<float, false>(c, s, filt, nq, k, n_ranges, st);
+  return filt.bits ? launch_count_qb<double, true>(c, s, filt, nq, k, n_ranges, st)
+                   : launch_count_qb<double, false>(c, s, filt, nq, k, n_ranges, st);
 }
 
 }  // namespace sdb

@@ -192,7 +192,8 @@ __global__ void __launch_bounds__(128) jaccard_keys_kernel(const T* __restrict__
     }
   }
 }
-static sdb_status jaccard_launch(Corpus* c, const double* d_q64, uint64_t* d_keys, double* d_vals, cudaStream_t st) {
+static sdb_status jaccard_launch(const Corpus* c, const double* d_q64, uint64_t* d_keys, double* d_vals,
+                                 cudaStream_t st) {
   Ctx* ctx = c->ctx;
   AsyncBuf<uint8_t> d_dup;
   SDB_CUDA(d_dup.reserve(c->dim, st));
@@ -416,18 +417,19 @@ sdb_status exact_query(Corpus* c, const double* d_q64, const double* d_qmag, con
 
 
 // one reference-arithmetic value per row (SURVEY 8f-4: projected scalar vector functions)
-sdb_status exact_project(Corpus* c, int fn, double* d_vals, cudaStream_t st) {
+sdb_status exact_project(const Corpus* c, int fn, const double* d_q64, const double* d_qmag, const uint32_t* d_qflags,
+                         double* d_vals, cudaStream_t st) {
   Ctx* ctx = c->ctx;
   const uint64_t n = c->n;
   if (!n) return SDB_OK;
-  if (fn == SDB_JACCARD) return jaccard_launch(c, c->d_q64, nullptr, d_vals, st);
+  if (fn == SDB_JACCARD) return jaccard_launch(c, d_q64, nullptr, d_vals, st);
   const int grid = ctx->sm_count * 8;
   if (c->dtype == SDB_F32)
     exact_keys_kernel<float, 4><<<grid, 128, 0, st>>>((const float*)c->d_rows.get(), c->dim, n, fn, c->d_mag, c->d_skip,
-                                                      c->d_q64, c->d_qmag, c->d_qflags, nullptr, d_vals, c->minkowski_p);
+                                                      d_q64, d_qmag, d_qflags, nullptr, d_vals, c->minkowski_p);
   else
     exact_keys_kernel<double, 4><<<grid, 128, 0, st>>>((const double*)c->d_rows.get(), c->dim, n, fn, c->d_mag, c->d_skip,
-                                                       c->d_q64, c->d_qmag, c->d_qflags, nullptr, d_vals, c->minkowski_p);
+                                                       d_q64, d_qmag, d_qflags, nullptr, d_vals, c->minkowski_p);
   count_launch(ctx);
   SDB_CUDA(cudaGetLastError());
   return SDB_OK;

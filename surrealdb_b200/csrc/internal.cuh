@@ -328,11 +328,10 @@ void trace_mark(Ctx* ctx, Ticket& t, const char* name, cudaStream_t st);  // api
 void trace_dump(Ctx* ctx, Ticket& t);
 void trace_host(Ctx* ctx, uint32_t ticket, const char* name);  // host-side timestamp on the same time base
 
-// Per-batch search scratch.  Two sets exist per corpus: consecutive batches alternate between them (and between the
-// context's two streams), so the screen of batch i+1 can run while the tail of batch i (candidate selection, f32
-// re-score, exact re-rank, final ordering, all-gather + merge) is still in flight.  The Corpus object itself carries
-// the ACTIVE set's fields (it derives from Scratch): enqueue_batch swaps the ticket's set in before it launches
-// anything, and every launch captures the pointers by value.
+// Per-batch search scratch.  Each corpus holds two sets (Corpus::sets): a ticket's slot parity names its set (and its
+// stream), so consecutive batches alternate between them and the screen of batch i+1 can run while the tail of batch i
+// (candidate selection, f32 re-score, exact re-rank, final ordering, all-gather + merge) is still in flight.  Every
+// stage of a batch takes its set explicitly; what the corpus holds beside the sets is shared by every batch.
 struct Scratch {
   uint32_t sc_nq = 0, sc_cap = 0;
   DevBuf<double> d_q64;
@@ -374,8 +373,8 @@ struct Scratch {
   uint32_t rr_stride = 0;
 };
 
-// Test-only snapshot of one batch's stage-A candidate lists (sdb_debug_screen_batch).  enqueue_batch fills it when
-// Corpus::tap is set, which is never the case in production.
+// Test-only snapshot of one batch's stage-A candidate lists (sdb_debug_screen_batch).  The enqueue functions fill it
+// when the batch they run carries one, which is never the case in production.
 struct ScreenTap {
   std::vector<uint32_t> gathered;  // per query: most entries any stage-A selection gathered, before capping
   std::vector<Cand> list_a;        // [nq][cap]: kept list after the last stage-A selection
@@ -383,9 +382,8 @@ struct ScreenTap {
   std::vector<Cand> list_r;        // [nq][cap]: the same list after cand_refine re-scored it in f32 (empty if it did not run)
 };
 
-struct Corpus : Scratch {
+struct Corpus {
   Ctx* ctx = nullptr;
-  ScreenTap* tap = nullptr;  // test-only (see ScreenTap)
   uint32_t dim = 0, dim_pad = 0;  // dim_pad: bf16 screen copy row length (multiple of 64)
   sdb_dtype dtype = SDB_F32;
   sdb_metric metric = SDB_COSINE;
@@ -427,11 +425,9 @@ struct Corpus : Scratch {
   DevBuf<double> d_rp_q;      // repair sub-batch: the failed queries of a batch, gathered, and their results
   DevBuf<uint32_t> d_rp_qf;   // ... and their filter indices (filtered batches)
   ResultBufs rp;
-  FiltArg filt;               // row filter of the batch being enqueued (enqueue_batch sets it; launches copy it)
   DevBuf<double> d_fb_qmag;
   DevBuf<uint32_t> d_fb_qflags;
-  Scratch parked;  // the inactive set (see Scratch)
-  int active_set = 0;
+  Scratch sets[2];  // per-batch scratch (see Scratch); Ticket::set names a batch's
   cudaEvent_t last_main = nullptr;  // ev_main of the batch whose screen was enqueued last
   // asynchronous batches
   Ticket tickets[N_TICKETS];
@@ -513,57 +509,65 @@ constexpr int LP_TQ = 4;            // queries per thread
 sdb_status corpus_finalize_device(Corpus* c);
 sdb_status corpus_remove_device(Corpus* c, const uint64_t* h_ids, uint64_t n);
 sdb_status corpus_reapply_tombstones(Corpus* c, cudaStream_t st);
+// The stages of a batch take its scratch set s and, where rows are screened or ranked, its row filter filt.
 // screen_simt.cu: the SIMT_F32 screen of Dot corpora (f32 rows)
-sdb_status screen_simt_pass(Corpus* c, uint32_t nq, const PassDesc& p, cudaStream_t st);
+sdb_status screen_simt_pass(const Corpus* c, Scratch& s, const FiltArg& filt, uint32_t nq, const PassDesc& p,
+                            cudaStream_t st);
 // screen_lp.cu: the SIMT_F32 screen of Lp corpora, f32 L1 / L-infinity / Lp (score = -s~), f32 and f64 rows
-sdb_status screen_lp_pass(Corpus* c, uint32_t nq, const PassDesc& p, cudaStream_t st);
+sdb_status screen_lp_pass(const Corpus* c, Scratch& s, const FiltArg& filt, uint32_t nq, const PassDesc& p,
+                          cudaStream_t st);
 // count.cu: the count path of Count corpora: rows split into count_ranges() ranges, each query's candidate entries
 // (cnt, rr_*) = the union of its ranges' k best (distance, row) pairs with their exact distances; needs prep_queries
 // (which runs count_prep_queries for Count corpora) and cand_begin
 uint32_t count_ranges(const Corpus* c, uint32_t nq, uint32_t k);
-sdb_status count_prep_queries(Corpus* c, uint32_t nq, cudaStream_t st);
-sdb_status count_pass(Corpus* c, uint32_t nq, uint32_t k, cudaStream_t st);
+sdb_status count_prep_queries(const Corpus* c, Scratch& s, uint32_t nq, cudaStream_t st);
+sdb_status count_pass(const Corpus* c, Scratch& s, const FiltArg& filt, uint32_t nq, uint32_t k, cudaStream_t st);
 // screen_tc.cu
 // mode 0: pass 0 (every score of the pass's tiles written to fixed slots), 1: threshold pass, 2: streaming pass with
 // in-kernel threshold refinement (histogram + refiner warp), 3: probe (chunk maxima of a few tiles, no candidates)
-sdb_status screen_tc_pass(Corpus* c, uint32_t nq, uint32_t k, const PassDesc& p, bool int8, int mode, cudaStream_t st);
+sdb_status screen_tc_pass(const Corpus* c, Scratch& s, const FiltArg& filt, uint32_t nq, uint32_t k, const PassDesc& p,
+                          bool int8, int mode, cudaStream_t st);
 bool screen_tc_available();
 // candidates.cu
-sdb_status scratch_for(Corpus* c, uint32_t nq, uint32_t cap);
-sdb_status prep_queries(Corpus* c, const double* d_queries, uint32_t nq, cudaStream_t st);
+// grows s to nq queries x cap candidates (a set that grows loses its contents)
+sdb_status scratch_for(const Corpus* c, Scratch& s, uint32_t nq, uint32_t cap);
+sdb_status prep_queries(const Corpus* c, Scratch& s, const double* d_queries, uint32_t nq, cudaStream_t st);
 // one query prepared into the fallback scratch (d_fb_*), independent of the batch scratch
 sdb_status prep_fallback_query(Corpus* c, const double* d_query, cudaStream_t st);
 // resets tau / counts / flags and derives, per query, the screen's error bound, the selection margin and the score range
-sdb_status cand_begin(Corpus* c, uint32_t nq, int screen, cudaStream_t st);
-sdb_status cand_set_count(Corpus* c, uint32_t nq, uint32_t value, cudaStream_t st);
+sdb_status cand_begin(const Corpus* c, Scratch& s, uint32_t nq, int screen, cudaStream_t st);
+sdb_status cand_set_count(const Corpus* c, Scratch& s, uint32_t nq, uint32_t value, cudaStream_t st);
 // per query: gather the main list + the private sub-lists, find the k-th best score s_k, keep every candidate with
 // score >= tau = s_k - margin (all of them while fewer than k exist), publish tau.  seed_hist: also (re)build the
 // query's histogram (geometry + counts of the kept candidates) for the streaming pass that follows.
-sdb_status cand_select(Corpus* c, uint32_t nq, uint32_t k, bool drop_invalid, uint32_t n_slots, bool seed_hist,
-                       cudaStream_t st, int stage = 0);
+sdb_status cand_select(const Corpus* c, Scratch& s, uint32_t nq, uint32_t k, bool drop_invalid, uint32_t n_slots,
+                       bool seed_hist, cudaStream_t st, int stage = 0);
 // stage B: re-score every kept candidate in f32 (master rows x f32 query) so that cand_select(stage 1) can shrink the
 // set before the FP64-bound exact re-rank
-sdb_status cand_refine(Corpus* c, uint32_t nq, cudaStream_t st);
+sdb_status cand_refine(const Corpus* c, Scratch& s, uint32_t nq, cudaStream_t st);
 // after a probe launch over n_tiles tiles: tau = (k-th largest chunk maximum) - margin, histogram geometry, empty lists
-sdb_status cand_seed_from_probe(Corpus* c, uint32_t nq, uint32_t k, uint32_t n_tiles, cudaStream_t st);
-// filtered batches (c->filt set): after a pass-0 launch, give the entries of rows a query's filter rejects a NaN score,
-// which cand_select drops like any invalid row
-sdb_status cand_filter_list(Corpus* c, uint32_t nq, cudaStream_t st);
+sdb_status cand_seed_from_probe(const Corpus* c, Scratch& s, uint32_t nq, uint32_t k, uint32_t n_tiles,
+                                cudaStream_t st);
+// filtered batches: after a pass-0 launch, give the entries of rows a query's filter rejects a NaN score, which
+// cand_select drops like any invalid row
+sdb_status cand_filter_list(const Corpus* c, Scratch& s, const FiltArg& filt, uint32_t nq, cudaStream_t st);
 // filtered batches: append each query's passing special rows to its list (the re-rank and cand_final then run without
 // the shared special-row tail); a list that has no room is flagged as overflowed
-sdb_status cand_add_specials(Corpus* c, uint32_t nq, cudaStream_t st);
-// direct regime (c->filt set): each query's list = the rows its filter passes that are neither skipped nor removed
-sdb_status cand_direct(Corpus* c, uint32_t nq, cudaStream_t st);
-sdb_status cand_rerank(Corpus* c, uint32_t nq, cudaStream_t st, bool small_sets = false);
-sdb_status cand_final(Corpus* c, uint32_t nq, uint32_t k, uint64_t row_base, uint64_t* d_out_rows, double* d_out_dist,
-                      uint32_t* d_out_count, cudaStream_t st);
-// exact.cu: query vector / |q| / flags are passed explicitly (batch scratch row or the fallback scratch).
-// filter: nullptr, or the query's bitmap (c->filt.words words): rows whose bit is clear are not ranked.
+sdb_status cand_add_specials(const Corpus* c, Scratch& s, const FiltArg& filt, uint32_t nq, cudaStream_t st);
+// direct regime (filtered): each query's list = the rows its filter passes that are neither skipped nor removed
+sdb_status cand_direct(const Corpus* c, Scratch& s, const FiltArg& filt, uint32_t nq, cudaStream_t st);
+sdb_status cand_rerank(const Corpus* c, Scratch& s, const FiltArg& filt, uint32_t nq, cudaStream_t st,
+                       bool small_sets = false);
+sdb_status cand_final(const Corpus* c, Scratch& s, const FiltArg& filt, uint32_t nq, uint32_t k, uint64_t row_base,
+                      uint64_t* d_out_rows, double* d_out_dist, uint32_t* d_out_count, cudaStream_t st);
+// exact.cu: query vector / |q| / flags are passed explicitly (a batch scratch row or the fallback scratch).
+// filter: nullptr, or the query's bitmap (filter_words words): rows whose bit is clear are not ranked.
 sdb_status exact_query(Corpus* c, const double* d_q64, const double* d_qmag, const uint32_t* d_qflags, uint32_t k,
                        uint64_t row_base, uint64_t* d_out_rows, double* d_out_dist, uint32_t* d_out_count,
                        cudaStream_t st, const uint32_t* filter = nullptr, uint32_t filter_words = 0);
+sdb_status exact_project(const Corpus* c, int fn, const double* d_q64, const double* d_qmag, const uint32_t* d_qflags,
+                         double* d_vals, cudaStream_t st);
 // gen.cu
-sdb_status exact_project(Corpus* c, int fn, double* d_vals, cudaStream_t st);
 sdb_status gen_fill_f32(Ctx* ctx, float* d_out, uint64_t seed, uint64_t first, uint64_t n, cudaStream_t st);
 
 // hnsw.cu: range / monotonicity check of a device CSR handed over the ABI (SDB_EINVAL with a message on violation)

@@ -240,7 +240,8 @@ __global__ void __launch_bounds__(LP_THREADS, QB >= 32 || sizeof(T) == 8 ? 1 : 2
 }
 
 template <int METRIC, int P, typename T, bool FILT, int QB>
-static sdb_status launch_lp(Corpus* c, uint32_t nq, const PassDesc& p, cudaStream_t st) {
+static sdb_status launch_lp(const Corpus* c, Scratch& s, const FiltArg& filt, uint32_t nq, const PassDesc& p,
+                            cudaStream_t st) {
   // P = 0: MANHATTAN / CHEBYSHEV; P = 1 .. 8: MINKOWSKI of that order
   auto kern = [] {
     if constexpr (P == 0) return screen_lp_kernel<METRIC, T, FILT, QB>;
@@ -259,11 +260,11 @@ static sdb_status launch_lp(Corpus* c, uint32_t nq, const PassDesc& p, cudaStrea
   uint64_t grid = (uint64_t)c->ctx->sm_count * per_sm;
   if (grid > items) grid = items;
   if constexpr (P == 0)
-    kern<<<(unsigned)grid, LP_THREADS, 0, st>>>((const T*)c->d_rows.get(), c->d_snorm, c->dim, c->n, c->d_q32, nq, p,
-                                                c->d_tau, c->d_cand, c->d_cand_cnt, c->sc_cap, c->filt);
+    kern<<<(unsigned)grid, LP_THREADS, 0, st>>>((const T*)c->d_rows.get(), c->d_snorm, c->dim, c->n, s.d_q32, nq, p,
+                                                s.d_tau, s.d_cand, s.d_cand_cnt, s.sc_cap, filt);
   else
-    kern<<<(unsigned)grid, LP_THREADS, 0, st>>>((const T*)c->d_rows.get(), c->d_snorm, c->dim, c->n, c->d_q32, nq, p,
-                                                c->d_tau, c->d_cand, c->d_cand_cnt, c->sc_cap, c->filt, c->d_mscale);
+    kern<<<(unsigned)grid, LP_THREADS, 0, st>>>((const T*)c->d_rows.get(), c->d_snorm, c->dim, c->n, s.d_q32, nq, p,
+                                                s.d_tau, s.d_cand, s.d_cand_cnt, s.sc_cap, filt, s.d_mscale);
   count_launch(c->ctx);
   SDB_CUDA(cudaGetLastError());
   return SDB_OK;
@@ -272,36 +273,38 @@ static sdb_status launch_lp(Corpus* c, uint32_t nq, const PassDesc& p, cudaStrea
 // the query block follows the batch: small batches are HBM-bound, and a block larger than the batch spends FP32 work
 // on padding queries (an 8-query block at most 7 / 8 of it, a 32-query block for 17-32 queries at most 15 / 32)
 template <int METRIC, int P, typename T, bool FILT>
-static sdb_status launch_lp_qb(Corpus* c, uint32_t nq, const PassDesc& p, cudaStream_t st) {
-  if (nq <= 16) return launch_lp<METRIC, P, T, FILT, 8>(c, nq, p, st);
-  if (nq <= 32) return launch_lp<METRIC, P, T, FILT, 32>(c, nq, p, st);
-  return launch_lp<METRIC, P, T, FILT, 64>(c, nq, p, st);
-}
-template <int METRIC, int P, typename T>
-static sdb_status launch_lp_filt(Corpus* c, uint32_t nq, const PassDesc& p, cudaStream_t st) {
-  return c->filt.bits ? launch_lp_qb<METRIC, P, T, true>(c, nq, p, st) : launch_lp_qb<METRIC, P, T, false>(c, nq, p, st);
+static sdb_status launch_lp_qb(const Corpus* c, Scratch& s, const FiltArg& filt, uint32_t nq, const PassDesc& p,
+                               cudaStream_t st) {
+  if (nq <= 16) return launch_lp<METRIC, P, T, FILT, 8>(c, s, filt, nq, p, st);
+  if (nq <= 32) return launch_lp<METRIC, P, T, FILT, 32>(c, s, filt, nq, p, st);
+  return launch_lp<METRIC, P, T, FILT, 64>(c, s, filt, nq, p, st);
 }
 template <int METRIC, int P = 0>
-static sdb_status launch_lp_type(Corpus* c, uint32_t nq, const PassDesc& p, cudaStream_t st) {
-  return c->dtype == SDB_F32 ? launch_lp_filt<METRIC, P, float>(c, nq, p, st)
-                             : launch_lp_filt<METRIC, P, double>(c, nq, p, st);
+static sdb_status launch_lp_type(const Corpus* c, Scratch& s, const FiltArg& filt, uint32_t nq, const PassDesc& p,
+                                 cudaStream_t st) {
+  if (c->dtype == SDB_F32)
+    return filt.bits ? launch_lp_qb<METRIC, P, float, true>(c, s, filt, nq, p, st)
+                     : launch_lp_qb<METRIC, P, float, false>(c, s, filt, nq, p, st);
+  return filt.bits ? launch_lp_qb<METRIC, P, double, true>(c, s, filt, nq, p, st)
+                   : launch_lp_qb<METRIC, P, double, false>(c, s, filt, nq, p, st);
 }
 
-sdb_status screen_lp_pass(Corpus* c, uint32_t nq, const PassDesc& p, cudaStream_t st) {
+sdb_status screen_lp_pass(const Corpus* c, Scratch& s, const FiltArg& filt, uint32_t nq, const PassDesc& p,
+                          cudaStream_t st) {
   if (p.count == 0 || nq == 0) return SDB_OK;
   switch (minkowski_screen_order(c)) {
-    case 1: return launch_lp_type<SDB_MINKOWSKI, 1>(c, nq, p, st);
-    case 2: return launch_lp_type<SDB_MINKOWSKI, 2>(c, nq, p, st);
-    case 3: return launch_lp_type<SDB_MINKOWSKI, 3>(c, nq, p, st);
-    case 4: return launch_lp_type<SDB_MINKOWSKI, 4>(c, nq, p, st);
-    case 5: return launch_lp_type<SDB_MINKOWSKI, 5>(c, nq, p, st);
-    case 6: return launch_lp_type<SDB_MINKOWSKI, 6>(c, nq, p, st);
-    case 7: return launch_lp_type<SDB_MINKOWSKI, 7>(c, nq, p, st);
-    case 8: return launch_lp_type<SDB_MINKOWSKI, 8>(c, nq, p, st);
+    case 1: return launch_lp_type<SDB_MINKOWSKI, 1>(c, s, filt, nq, p, st);
+    case 2: return launch_lp_type<SDB_MINKOWSKI, 2>(c, s, filt, nq, p, st);
+    case 3: return launch_lp_type<SDB_MINKOWSKI, 3>(c, s, filt, nq, p, st);
+    case 4: return launch_lp_type<SDB_MINKOWSKI, 4>(c, s, filt, nq, p, st);
+    case 5: return launch_lp_type<SDB_MINKOWSKI, 5>(c, s, filt, nq, p, st);
+    case 6: return launch_lp_type<SDB_MINKOWSKI, 6>(c, s, filt, nq, p, st);
+    case 7: return launch_lp_type<SDB_MINKOWSKI, 7>(c, s, filt, nq, p, st);
+    case 8: return launch_lp_type<SDB_MINKOWSKI, 8>(c, s, filt, nq, p, st);
     default: break;
   }
-  return c->metric == SDB_MANHATTAN ? launch_lp_type<SDB_MANHATTAN>(c, nq, p, st)
-                                    : launch_lp_type<SDB_CHEBYSHEV>(c, nq, p, st);
+  return c->metric == SDB_MANHATTAN ? launch_lp_type<SDB_MANHATTAN>(c, s, filt, nq, p, st)
+                                    : launch_lp_type<SDB_CHEBYSHEV>(c, s, filt, nq, p, st);
 }
 
 }  // namespace sdb

@@ -226,16 +226,17 @@ __global__ void __launch_bounds__(256) screen_simt_generic_kernel(
 }
 
 template <int RPW, int QB>
-static sdb_status launch_ring_q(Corpus* c, uint32_t nq, const PassDesc& p, cudaStream_t st, size_t smem) {
+static sdb_status launch_ring_q(const Corpus* c, Scratch& s, const FiltArg& filt, uint32_t nq, const PassDesc& p,
+                                cudaStream_t st, size_t smem) {
   Ctx* ctx = c->ctx;
-  auto kern = c->filt.bits ? screen_simt_kernel<RPW, QB, true> : screen_simt_kernel<RPW, QB, false>;
+  auto kern = filt.bits ? screen_simt_kernel<RPW, QB, true> : screen_simt_kernel<RPW, QB, false>;
   SDB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   uint32_t grid = (uint32_t)ctx->sm_count;
   if (grid > p.count) grid = p.count;
   for (uint32_t q0 = 0; q0 < nq; q0 += QB) {
     const uint32_t nqb = nq - q0 < (uint32_t)QB ? nq - q0 : (uint32_t)QB;
-    kern<<<grid, SIMT_THREADS, smem, st>>>((const float*)c->d_rows.get(), c->d_snorm, c->dim, c->n, c->d_q32, q0, nqb,
-                                           (int)c->metric, p, c->d_tau, c->d_cand, c->d_cand_cnt, c->sc_cap, c->filt);
+    kern<<<grid, SIMT_THREADS, smem, st>>>((const float*)c->d_rows.get(), c->d_snorm, c->dim, c->n, s.d_q32, q0, nqb,
+                                           (int)c->metric, p, s.d_tau, s.d_cand, s.d_cand_cnt, s.sc_cap, filt);
     count_launch(ctx);
   }
   SDB_CUDA(cudaGetLastError());
@@ -243,14 +244,16 @@ static sdb_status launch_ring_q(Corpus* c, uint32_t nq, const PassDesc& p, cudaS
 }
 
 template <int RPW>
-static sdb_status launch_ring(Corpus* c, uint32_t nq, const PassDesc& p, cudaStream_t st, size_t q_bytes8, size_t ring) {
+static sdb_status launch_ring(const Corpus* c, Scratch& s, const FiltArg& filt, uint32_t nq, const PassDesc& p,
+                              cudaStream_t st, size_t q_bytes8, size_t ring) {
   // the shared-memory query tile shrinks with QB; the row ring keeps its size
-  if (nq == 1) return launch_ring_q<RPW, 1>(c, nq, p, st, q_bytes8 / 8 + ring);
-  if (nq <= 4) return launch_ring_q<RPW, 4>(c, nq, p, st, q_bytes8 / 2 + ring);
-  return launch_ring_q<RPW, 8>(c, nq, p, st, q_bytes8 + ring);
+  if (nq == 1) return launch_ring_q<RPW, 1>(c, s, filt, nq, p, st, q_bytes8 / 8 + ring);
+  if (nq <= 4) return launch_ring_q<RPW, 4>(c, s, filt, nq, p, st, q_bytes8 / 2 + ring);
+  return launch_ring_q<RPW, 8>(c, s, filt, nq, p, st, q_bytes8 + ring);
 }
 
-sdb_status screen_simt_pass(Corpus* c, uint32_t nq, const PassDesc& p, cudaStream_t st) {
+sdb_status screen_simt_pass(const Corpus* c, Scratch& s, const FiltArg& filt, uint32_t nq, const PassDesc& p,
+                            cudaStream_t st) {
   if (p.count == 0) return SDB_OK;
   Ctx* ctx = c->ctx;
   const size_t q_bytes = sizeof(float) * SIMT_QB * c->dim;
@@ -258,15 +261,15 @@ sdb_status screen_simt_pass(Corpus* c, uint32_t nq, const PassDesc& p, cudaStrea
   auto ring_only = [&](int rpw) { return sizeof(float) * SIMT_STAGES * rpw * SIMT_CWARPS * (size_t)c->dim + 64; };
   auto ring_bytes = [&](int rpw) { return q_bytes + ring_only(rpw); };
   if (c->dim % 4 == 0 && ring_bytes(1) <= budget) {
-    if (ring_bytes(4) <= budget) return launch_ring<4>(c, nq, p, st, q_bytes, ring_only(4));
-    if (ring_bytes(2) <= budget) return launch_ring<2>(c, nq, p, st, q_bytes, ring_only(2));
-    return launch_ring<1>(c, nq, p, st, q_bytes, ring_only(1));
+    if (ring_bytes(4) <= budget) return launch_ring<4>(c, s, filt, nq, p, st, q_bytes, ring_only(4));
+    if (ring_bytes(2) <= budget) return launch_ring<2>(c, s, filt, nq, p, st, q_bytes, ring_only(2));
+    return launch_ring<1>(c, s, filt, nq, p, st, q_bytes, ring_only(1));
   }
   if (q_bytes > 200 * 1024) {
     set_error("screen_simt: dim %u too large for the shared-memory query tile", c->dim);
     return SDB_EUNSUPPORTED;
   }
-  auto kern = c->filt.bits ? screen_simt_generic_kernel<true> : screen_simt_generic_kernel<false>;
+  auto kern = filt.bits ? screen_simt_generic_kernel<true> : screen_simt_generic_kernel<false>;
   SDB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)q_bytes));
   int per_sm = 1;
   SDB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, 256, q_bytes));
@@ -275,8 +278,8 @@ sdb_status screen_simt_pass(Corpus* c, uint32_t nq, const PassDesc& p, cudaStrea
   if (grid > p.count) grid = p.count;
   for (uint32_t q0 = 0; q0 < nq; q0 += SIMT_QB) {
     const uint32_t nqb = nq - q0 < (uint32_t)SIMT_QB ? nq - q0 : (uint32_t)SIMT_QB;
-    kern<<<grid, 256, q_bytes, st>>>((const float*)c->d_rows.get(), c->d_snorm, c->dim, c->n, c->d_q32, q0, nqb,
-                                     (int)c->metric, p, c->d_tau, c->d_cand, c->d_cand_cnt, c->sc_cap, c->filt);
+    kern<<<grid, 256, q_bytes, st>>>((const float*)c->d_rows.get(), c->d_snorm, c->dim, c->n, s.d_q32, q0, nqb,
+                                     (int)c->metric, p, s.d_tau, s.d_cand, s.d_cand_cnt, s.sc_cap, filt);
     count_launch(ctx);
   }
   SDB_CUDA(cudaGetLastError());

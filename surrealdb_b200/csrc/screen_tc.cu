@@ -763,7 +763,8 @@ sdb_status screen_tc_init_device(Ctx* ctx) {
   return SDB_OK;
 }
 
-sdb_status screen_tc_pass(Corpus* c, uint32_t nq, uint32_t k, const PassDesc& p, bool int8, int mode, cudaStream_t st) {
+sdb_status screen_tc_pass(const Corpus* c, Scratch& s, const FiltArg& filt, uint32_t nq, uint32_t k, const PassDesc& p,
+                          bool int8, int mode, cudaStream_t st) {
   if (p.count == 0) return SDB_OK;
   Ctx* ctx = c->ctx;
   // PEARSON corpora hold centred copies (corpus.cu) and centred, negated queries (prep_queries): their cosine screen
@@ -809,22 +810,22 @@ sdb_status screen_tc_pass(Corpus* c, uint32_t nq, uint32_t k, const PassDesc& p,
     set_error("screen_tc_pass: probe of %u tiles exceeds the probe buffer", p.count);
     return SDB_EINVAL;
   }
-  if (mode != 3) c->last_slots = grid * 2;
+  if (mode != 3) s.last_slots = grid * 2;
   const uint32_t slots = grid * 2;
   for (uint32_t q0 = 0; q0 < nq; q0 += chunk_q) {
     const uint32_t nqc = nq - q0 < chunk_q ? nq - q0 : chunk_q;
     const uint32_t nq_pad = (nqc + tc::BLOCK_M - 1) / tc::BLOCK_M * tc::BLOCK_M;
     const uint32_t n_mblocks = nq_pad / tc::BLOCK_M;
     CUtensorMap map_a;
-    if (int8) SDB_TRY(make_map(ctx, &map_a, c->d_q8 + (size_t)q0 * c->dim_pad8, nq_pad, c->dim_pad8, tc::BLOCK_M, false, true));
-    else SDB_TRY(make_map(ctx, &map_a, c->d_qbf16 + (size_t)q0 * c->dim_pad, nq_pad, c->dim_pad, tc::BLOCK_M, false));
-    float* tau = c->d_tau + q0;
-    Cand* cand = c->d_cand + (size_t)q0 * c->sc_cap;
-    uint32_t* ccnt = c->d_cand_cnt + q0;
-    Cand* sub = c->d_sub + (size_t)q0 * slots * tc::SUBCAP;
-    uint32_t* scnt = c->d_sub_cnt + (size_t)q0 * slots;
-    const HistParam* hp = c->d_hparam + q0;
-    uint32_t* hist = c->d_hist + (size_t)q0 * HIST_BINS;
+    if (int8) SDB_TRY(make_map(ctx, &map_a, s.d_q8 + (size_t)q0 * c->dim_pad8, nq_pad, c->dim_pad8, tc::BLOCK_M, false, true));
+    else SDB_TRY(make_map(ctx, &map_a, s.d_qbf16 + (size_t)q0 * c->dim_pad, nq_pad, c->dim_pad, tc::BLOCK_M, false));
+    float* tau = s.d_tau + q0;
+    Cand* cand = s.d_cand + (size_t)q0 * s.sc_cap;
+    uint32_t* ccnt = s.d_cand_cnt + q0;
+    Cand* sub = s.d_sub + (size_t)q0 * slots * tc::SUBCAP;
+    uint32_t* scnt = s.d_sub_cnt + (size_t)q0 * slots;
+    const HistParam* hp = s.d_hparam + q0;
+    uint32_t* hist = s.d_hist + (size_t)q0 * HIST_BINS;
     // the screen is launched at the highest priority: when the previous batch's screen retires, the blocks of THIS
     // launch are placed before the queued blocks of that batch's tail kernels (which fit beside a screen CTA anyway),
     // instead of waiting behind two 13 KB selection blocks per SM
@@ -841,19 +842,19 @@ sdb_status screen_tc_pass(Corpus* c, uint32_t nq, uint32_t k, const PassDesc& p,
     attr[1].val.clusterDim.z = 1;
     cfg.attrs = attr;
     cfg.numAttrs = pair ? 2 : 1;
-    float* probe_ptr = c->d_probe + (size_t)q0 * PROBE_STRIDE;
-    const uint32_t probe_stride = PROBE_STRIDE, cap_arg = c->sc_cap;
+    float* probe_ptr = s.d_probe + (size_t)q0 * PROBE_STRIDE;
+    const uint32_t probe_stride = PROBE_STRIDE, cap_arg = s.sc_cap;
     const float* snorm_arg = c->d_snorm;
-    FiltArg filt = c->filt;
-    if (filt.bits) filt.qf += q0;
+    FiltArg filt_q = filt;
+    if (filt_q.bits) filt_q.qf += q0;
 #define LAUNCH_TC2(COS, I8, MODE, F)                                                                                 \
   SDB_CUDA(cudaLaunchKernelEx(&cfg, tc::screen_tc_kernel<COS, I8, MODE, F>, map_a, map_b, snorm_arg, k_blocks,       \
                               n_mblocks, nqc, p, tau, cand, ccnt, cap_arg, sub, scnt, k, hp, hist, probe_ptr,        \
-                              probe_stride, sleep_min, sleep_max, pair, filt))
+                              probe_stride, sleep_min, sleep_max, pair, filt_q))
 #define LAUNCH_TC1(COS, I8, MODE)                      \
   do {                                                 \
     cfg.blockDim = dim3(tc::threads<I8, MODE>());      \
-    if (filt.bits) LAUNCH_TC2(COS, I8, MODE, true);    \
+    if (filt_q.bits) LAUNCH_TC2(COS, I8, MODE, true);  \
     else LAUNCH_TC2(COS, I8, MODE, false);             \
   } while (0)
 #define LAUNCH_TC(COS, I8)                   \
@@ -872,9 +873,9 @@ sdb_status screen_tc_pass(Corpus* c, uint32_t nq, uint32_t k, const PassDesc& p,
     count_launch(ctx);
   }
   if (mode == 0) {
-    SDB_TRY(cand_set_count(c, nq, p.count * TILE_ROWS, st));  // pass 0 wrote fixed slots of the main lists
-    c->last_slots = 0;                                         // ... and no private sub-lists
-    if (c->filt.bits) SDB_TRY(cand_filter_list(c, nq, st));   // ... of every row, the filtered-out ones included
+    SDB_TRY(cand_set_count(c, s, nq, p.count * TILE_ROWS, st));    // pass 0 wrote fixed slots of the main lists
+    s.last_slots = 0;                                              // ... and no private sub-lists
+    if (filt.bits) SDB_TRY(cand_filter_list(c, s, filt, nq, st));  // ... of every row, the filtered-out ones included
   }
   SDB_CUDA(cudaGetLastError());
   return SDB_OK;
