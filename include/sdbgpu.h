@@ -383,6 +383,45 @@ sdb_status sdb_knn_sharded_multi_filtered(sdb_corpus* const* shards, int n_shard
  * (ignored for SDB_FN_MAGNITUDE). */
 typedef enum { SDB_FN_SIMILARITY_COSINE = 16, SDB_FN_DOT = 17, SDB_FN_MAGNITUDE = 18 } sdb_vector_fn;
 sdb_status sdb_corpus_project(sdb_corpus*, const double* query, int fn, double* out);
+/* ---- ORDER BY a projected vector function: replaces Compute + SortTopK (exec/operators/sort/topk.rs) in
+ *      `SELECT id, vector::similarity::cosine(emb, $q) AS score FROM t ORDER BY score DESC LIMIT k` on a cached column.
+ * fn: as in sdb_corpus_project (an sdb_metric id or an sdb_vector_fn); each row's value is exactly what
+ * sdb_corpus_project returns for that row (MINKOWSKI: the same pow() caveat).  SDB_FN_MAGNITUDE ignores the queries,
+ * which may then be NULL.  Query q returns the k rows SortTopK keeps over the rows its filter passes (filters,
+ * n_filters, query_filter exactly as in sdb_knn_bruteforce_filtered; filters == NULL: every row) that are neither
+ * skipped nor removed: ordered by Number::cmp of the value (-0.0 == 0.0, otherwise total_cmp, so NaNs by sign and
+ * payload), reversed as a whole for SDB_ORDER_DESC, then by ascending scan position.  out_value is the computed f64
+ * (a -0.0 stays -0.0); out_count[q] = min(k, ranked rows).  k <= 4096 (SDB_EUNSUPPORTED beyond); k = 0 gives zero
+ * counts.  Above k = 1000 the reference sorts with an unstable sort instead of its top-k heap, so rows of equal value
+ * may come back in any order there: scan order is one valid answer.
+ * Routing: fn = the corpus metric with SDB_ORDER_ASC is the KNN ranking and takes the KNN path unchanged (the results
+ * equal sdb_knn_bruteforce[_filtered] byte for byte); SDB_FN_SIMILARITY_COSINE DESC on a COSINE corpus is screened
+ * like KNN (k <= 256) and proven with the similarity's bound, vector::similarity::pearson DESC on a PEARSON corpus
+ * on the same screens with the query's centred copy un-negated (k <= 256), HAMMING / JACCARD DESC on their own corpus
+ * on the count path (k <= 256, exact counts); every other (fn, order) is ranked by the exact kernel.
+ * Refusals: an unknown fn or order, or nq > 0 with NULL queries for a function that takes a query: SDB_EINVAL.
+ * Tickets share the corpus' four slots with KNN tickets; sdb_knn_wait completes them; cancellation and
+ * sdb_knn_last_stats work as for KNN.  Row-sharded columns are not served. */
+/* order: an sdb_order value, passed as int (like fn) so that any other value can be refused without first being
+ * converted to the enum */
+typedef enum { SDB_ORDER_ASC = 0, SDB_ORDER_DESC = 1 } sdb_order;
+sdb_status sdb_corpus_order_topk(sdb_corpus*, const double* queries, uint32_t nq, int fn, int order, uint32_t k,
+                                 const uint32_t* filters, uint32_t n_filters, const uint32_t* query_filter,
+                                 uint64_t* out_rows, double* out_value, uint32_t* out_count);
+/* device queries, bitmaps and outputs (query_filter stays host memory); row_base is added to every returned row */
+sdb_status sdb_corpus_order_topk_device(sdb_corpus*, const double* d_queries, uint32_t nq, int fn, int order,
+                                        uint32_t k, const uint32_t* d_filters, uint32_t n_filters,
+                                        const uint32_t* query_filter, uint64_t row_base, uint64_t* d_out_rows,
+                                        double* d_out_value, uint32_t* d_out_count);
+/* asynchronous variants (buffers valid until sdb_knn_wait returns, as for sdb_knn_submit[_filtered][_device]) */
+sdb_status sdb_corpus_order_submit(sdb_corpus*, const double* queries, uint32_t nq, int fn, int order,
+                                   uint32_t k, const uint32_t* filters, uint32_t n_filters,
+                                   const uint32_t* query_filter, uint64_t* out_rows, double* out_value,
+                                   uint32_t* out_count, uint32_t* ticket);
+sdb_status sdb_corpus_order_submit_device(sdb_corpus*, const double* d_queries, uint32_t nq, int fn, int order,
+                                          uint32_t k, const uint32_t* d_filters, uint32_t n_filters,
+                                          const uint32_t* query_filter, uint64_t row_base, uint64_t* d_out_rows,
+                                          double* d_out_value, uint32_t* d_out_count, uint32_t* ticket);
 
 /* merges `n_lists` per-shard result lists (each nq x k; list l's entry j of query q is valid iff
  * j < d_counts[l*stride_counts + q]) into the global top-k by (distance, row); all pointers are device

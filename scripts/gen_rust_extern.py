@@ -10,7 +10,7 @@ protos = re.findall(r"^\s*((?:const\s+)?[A-Za-z_][A-Za-z0-9_]*\s*\**)\s*(sdb_[a-
 HANDLES = {"sdb_ctx": "SdbCtx", "sdb_corpus": "SdbCorpus", "sdb_hnsw": "SdbHnsw", "sdb_graph": "SdbGraph"}
 PRIM = {"uint64_t": "u64", "uint32_t": "u32", "uint16_t": "u16", "uint8_t": "u8", "int8_t": "i8", "int64_t": "i64", "int32_t": "i32", "double": "f64",
         "float": "f32", "int": "i32", "size_t": "usize", "char": "c_char", "void": "c_void", "sdb_status": "i32",
-        "sdb_metric": "i32", "sdb_dtype": "i32", "sdb_vector_type": "i32", "sdb_screen": "i32", "sdb_knn_stats": "SdbKnnStats", "sdb_hop_filter": "SdbHopFilter"}
+        "sdb_metric": "i32", "sdb_order": "i32", "sdb_dtype": "i32", "sdb_vector_type": "i32", "sdb_screen": "i32", "sdb_knn_stats": "SdbKnnStats", "sdb_hop_filter": "SdbHopFilter"}
 
 
 def conv(t):

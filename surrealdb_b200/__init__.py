@@ -6,8 +6,8 @@ hand-written sm_90a CUDA in surrealdb_b200/csrc.
 """
 from ._lib import SdbError, SO_PATH  # noqa: F401
 from .engine import Context, VectorColumn, pack_row_filter  # noqa: F401
-from .operators import (Distance, Filter, KnnBruteForceLegacy, KnnContext, KnnScan, KnnTopK, TableScan,  # noqa: F401
-                        Union)
+from .operators import (Distance, Filter, KnnBruteForceLegacy, KnnContext, KnnScan, KnnTopK, SortTopK,  # noqa: F401
+                        TableScan, Union)
 from .graph import CsrGraph, GraphEdgeScan, GraphStore  # noqa: F401
 from .hnsw import HnswIndex  # noqa: F401
 

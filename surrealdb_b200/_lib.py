@@ -21,6 +21,7 @@ DTYPE = {"F32": 0, "F64": 1}
 VTYPE = {"F64": 0, "F32": 1, "I64": 2, "I32": 3, "I16": 4}
 VECTOR_FN = {"SIMILARITY_COSINE": 16, "DOT": 17, "MAGNITUDE": 18}
 SCREEN = {"AUTO": 0, "SIMT_F32": 1, "TC_BF16": 2, "NONE_EXACT": 3, "TC_INT8": 4}
+ORDER = {"ASC": 0, "DESC": 1}
 
 # every symbol include/sdbgpu.h declares (tests/test_abi_symbols.py cross-checks this list with the header)
 ABI_SYMBOLS = [
@@ -33,7 +34,8 @@ ABI_SYMBOLS = [
     "sdb_knn_last_stats", "sdb_knn_submit", "sdb_knn_submit_device", "sdb_knn_wait", "sdb_comm_unique_id",
     "sdb_comm_init_rank", "sdb_comm_size", "sdb_comm_rank", "sdb_ctx_create_multi", "sdb_corpus_set_row_base",
     "sdb_knn_sharded_submit", "sdb_knn_sharded_submit_device", "sdb_knn_sharded_wait", "sdb_knn_sharded_multi",
-    "sdb_corpus_project", "sdb_topk_merge_device", "sdb_hnsw_load", "sdb_hnsw_load_typed", "sdb_hnsw_load_device", "sdb_hnsw_load_device_typed", "sdb_hnsw_set_layers_device", "sdb_hnsw_search_device", "sdb_hnsw_knn_exact_device", "sdb_hnsw_select_device", "sdb_hnsw_select_neighbors_ids", "sdb_hnsw_destroy", "sdb_stage_decode_vectors", "sdb_stage_decode_nodes", "sdb_hnsw_load_staged", "sdb_hnsw_load_staged_typed", "sdb_hnsw_search", "sdb_hnsw_search_filtered", "sdb_hnsw_search_pending", "sdb_vec_distance_f32", "sdb_hnsw_distance", "sdb_hnsw_set_minkowski_order", "sdb_hnsw_select_neighbors",
+    "sdb_corpus_project", "sdb_corpus_order_topk", "sdb_corpus_order_topk_device", "sdb_corpus_order_submit",
+    "sdb_corpus_order_submit_device", "sdb_topk_merge_device", "sdb_hnsw_load", "sdb_hnsw_load_typed", "sdb_hnsw_load_device", "sdb_hnsw_load_device_typed", "sdb_hnsw_set_layers_device", "sdb_hnsw_search_device", "sdb_hnsw_knn_exact_device", "sdb_hnsw_select_device", "sdb_hnsw_select_neighbors_ids", "sdb_hnsw_destroy", "sdb_stage_decode_vectors", "sdb_stage_decode_nodes", "sdb_hnsw_load_staged", "sdb_hnsw_load_staged_typed", "sdb_hnsw_search", "sdb_hnsw_search_filtered", "sdb_hnsw_search_pending", "sdb_vec_distance_f32", "sdb_hnsw_distance", "sdb_hnsw_set_minkowski_order", "sdb_hnsw_select_neighbors",
     "sdb_graph_load_csr", "sdb_graph_load_csr_shard", "sdb_graph_destroy", "sdb_graph_expand", "sdb_graph_expand_device", "sdb_device_free", "sdb_graph_collect", "sdb_free",
     "sdb_graph_expand_filtered", "sdb_graph_expand_filtered_device", "sdb_graph_collect_filtered",
     "sdb_graph_expand_batch", "sdb_graph_expand_batch_device", "sdb_graph_collect_batch", "sdb_graph_last_collect_table",
@@ -132,6 +134,11 @@ def lib():
                                                          C.POINTER(u32)]
     L.sdb_knn_sharded_multi_filtered.argtypes = [vp, i32, vp, u32, u32, vp, u32, vp, u64, vp, vp, vp]
     L.sdb_corpus_project.argtypes = [vp, vp, i32, vp]
+    L.sdb_corpus_order_topk.argtypes = [vp, vp, u32, i32, i32, u32, vp, u32, vp, vp, vp, vp]
+    L.sdb_corpus_order_topk_device.argtypes = [vp, vp, u32, i32, i32, u32, vp, u32, vp, u64, vp, vp, vp]
+    L.sdb_corpus_order_submit.argtypes = [vp, vp, u32, i32, i32, u32, vp, u32, vp, vp, vp, vp, C.POINTER(u32)]
+    L.sdb_corpus_order_submit_device.argtypes = [vp, vp, u32, i32, i32, u32, vp, u32, vp, u64, vp, vp, vp,
+                                                 C.POINTER(u32)]
     L.sdb_knn_last_stats.argtypes = [vp, C.POINTER(KnnStats)]
     L.sdb_topk_merge_device.argtypes = [vp, u32, u32, u32, vp, vp, vp, u64, u64, u64, vp, vp, vp]
     L.sdb_hnsw_load.argtypes = [vp, u32, i32, u64, vp, u32, vp, vp, C.c_int64, C.POINTER(vp)]

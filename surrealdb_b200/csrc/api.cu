@@ -101,7 +101,8 @@ struct Rung {
 // to more than a handful of queries the batch is re-screened with a tighter screen / longer lists instead of paying
 // one exact pass over the corpus per failed query; the rung that worked is remembered per corpus and k.
 // screen: the corpus' screen choice (Corpus::screen, or the one a debug batch asks for)
-static std::vector<Rung> build_rungs(const Corpus* c, sdb_screen screen, uint32_t k, uint32_t nq, sdb_screen* first) {
+static std::vector<Rung> build_rungs(const Corpus* c, sdb_screen screen, uint32_t k, uint32_t nq, const Ranking& rank,
+                                     sdb_screen* first) {
   const Family f = family(c);
   const bool int8_ok = c->d_i8 && screen_tc_available();  // (COSINE and Centred corpora hold an int8 copy)
   sdb_screen scr = screen;
@@ -117,6 +118,8 @@ static std::vector<Rung> build_rungs(const Corpus* c, sdb_screen screen, uint32_
     scr = SDB_SCREEN_NONE_EXACT;
   // (Count: the count path, enqueue_counted, or the exact kernel)
   if (c->special_overflow || k > 256 || f == Family::Count || f == Family::Exact) scr = SDB_SCREEN_NONE_EXACT;
+  // a ranking the screens do not serve (screened_ranking): the exact kernel
+  if (!screened_ranking(c, rank)) scr = SDB_SCREEN_NONE_EXACT;
   // MANHATTAN / CHEBYSHEV: a single query streams the rows once either way, and the exact kernel does it at the higher
   // HBM rate (DESIGN.md section 5): AUTO ranks it there; an explicit SIMT_F32 request is kept.  MINKOWSKI's exact
   // kernel is bound by its f64 pow() calls, not by HBM, and the screen is faster for a single query too (section 5).
@@ -299,8 +302,9 @@ static sdb_status enqueue_direct(Corpus* c, Ticket& t, const Run& r) {
   SDB_TRY(prep_queries(c, s, r.d_queries, r.nq, st));
   SDB_TRY(cand_begin(c, s, r.nq, SDB_SCREEN_NONE_EXACT, st));
   SDB_TRY(cand_direct(c, s, r.filt, r.nq, st));
-  SDB_TRY(cand_rerank(c, s, r.filt, r.nq, st, false));
-  SDB_TRY(cand_final(c, s, r.filt, r.nq, t.k, t.row_base, r.d_out_rows, r.d_out_dist, r.d_out_count, st));
+  SDB_TRY(cand_rerank(c, s, r.filt, r.nq, st, false, t.rank.desc));
+  SDB_TRY(cand_final(c, s, r.filt, r.nq, t.k, t.row_base, r.d_out_rows, r.d_out_dist, r.d_out_count, st,
+                     t.rank.desc));
   return copy_flags(s, r, st);
 }
 
@@ -365,12 +369,12 @@ static sdb_status enqueue_counted(Corpus* c, Ticket& t, const Run& r, Enqueued* 
     set_error("query cancelled");
     return SDB_ECANCELLED;
   }
-  SDB_TRY(count_pass(c, s, r.filt, nq, k, st));
+  SDB_TRY(count_pass(c, s, r.filt, nq, k, st, t.rank.desc));
   SDB_CUDA(cudaEventRecord(t.ev_main, st));
   c->last_main = t.ev_main;
   SDB_CUDA(cudaEventRecord(t.ev_screen1, st));
   trace_mark(ctx, t, "counted", st);
-  SDB_TRY(cand_final(c, s, r.filt, nq, k, t.row_base, r.d_out_rows, r.d_out_dist, r.d_out_count, st));
+  SDB_TRY(cand_final(c, s, r.filt, nq, k, t.row_base, r.d_out_rows, r.d_out_dist, r.d_out_count, st, t.rank.desc));
   SDB_TRY(copy_flags(s, r, st));
   SDB_CUDA(cudaEventRecord(t.ev_end, st));
   trace_mark(ctx, t, "end", st);
@@ -385,10 +389,11 @@ static sdb_status enqueue_screened(Corpus* c, Ticket& t, const Run& r, Enqueued*
   // HAMMING: AUTO ranks a batch of one query with the exact kernel, which streams the rows once at the higher rate
   // (DESIGN.md section 5); an explicit screen request still counts it.  JACCARD's exact kernel is O(D^2) per row: the
   // count path takes a single query too
-  if (count_ranked(c, k) && (nq > 1 || r.screen != SDB_SCREEN_AUTO || c->metric == SDB_JACCARD))
+  if (screened_ranking(c, t.rank) && count_ranked(c, k) &&
+      (nq > 1 || r.screen != SDB_SCREEN_AUTO || c->metric == SDB_JACCARD))
     return enqueue_counted(c, t, r, e);
   sdb_screen first;
-  const std::vector<Rung> rungs = build_rungs(c, r.screen, k, nq, &first);
+  const std::vector<Rung> rungs = build_rungs(c, r.screen, k, nq, t.rank, &first);
   e->n_passes = 0;
   SDB_CUDA(cudaEventRecord(t.ev_begin, st));
   trace_mark(ctx, t, "begin", st);
@@ -413,7 +418,7 @@ static sdb_status enqueue_screened(Corpus* c, Ticket& t, const Run& r, Enqueued*
   const bool int8 = rs == SDB_SCREEN_TC_INT8;
   SDB_TRY(scratch_for(c, s, nq, rg.cap));
   const uint32_t cap = s.sc_cap;
-  SDB_TRY(prep_queries(c, s, r.d_queries, nq, st));
+  SDB_TRY(prep_queries(c, s, r.d_queries, nq, st, t.rank.desc));
   SDB_TRY(cand_begin(c, s, nq, (int)rs, st));
   // Screens are persistent one-CTA-per-SM kernels: two of them in flight on different streams would split the SMs,
   // run in two waves and starve the refiners of the CTAs that are not resident yet.  So the screen of this batch waits
@@ -477,9 +482,9 @@ static sdb_status enqueue_screened(Corpus* c, Ticket& t, const Run& r, Enqueued*
     trace_mark(ctx, t, "refined", st);
   }
   if (r.filt.bits) SDB_TRY(cand_add_specials(c, s, r.filt, nq, st));  // each query re-ranks its passing special rows
-  SDB_TRY(cand_rerank(c, s, r.filt, nq, st, refined));
+  SDB_TRY(cand_rerank(c, s, r.filt, nq, st, refined, t.rank.desc));
   trace_mark(ctx, t, "reranked", st);
-  SDB_TRY(cand_final(c, s, r.filt, nq, k, t.row_base, r.d_out_rows, r.d_out_dist, r.d_out_count, st));
+  SDB_TRY(cand_final(c, s, r.filt, nq, k, t.row_base, r.d_out_rows, r.d_out_dist, r.d_out_count, st, t.rank.desc));
   trace_mark(ctx, t, "final", st);
   SDB_TRY(copy_flags(s, r, st));
   SDB_CUDA(cudaEventRecord(t.ev_end, st));
@@ -533,7 +538,7 @@ static sdb_status finish_local(Corpus* c, Ticket& t, uint32_t* n_fallback, bool*
   }
   if (t.n_rungs) {
     sdb_screen first;
-    build_rungs(c, c->screen, k, nq, &first);
+    build_rungs(c, c->screen, k, nq, t.rank, &first);
     c->rung_scr = first;
     c->rung_k = k;
     c->rung = t.rung;
@@ -610,7 +615,7 @@ static sdb_status finish_local(Corpus* c, Ticket& t, uint32_t* n_fallback, bool*
     SDB_TRY(prep_fallback_query(c, t.d_queries + (size_t)q * c->dim, st));
     const uint32_t* q_filter = t.filt.bits ? t.filt.bits + (size_t)t.h_qf[q] * t.filt.words : nullptr;
     SDB_TRY(exact_query(c, c->d_fb_q, c->d_fb_qmag, c->d_fb_qflags, k, t.row_base, t.d_out_rows + (size_t)q * k,
-                        t.d_out_dist + (size_t)q * k, t.d_out_count + q, st, q_filter, t.filt.words));
+                        t.d_out_dist + (size_t)q * k, t.d_out_count + q, st, q_filter, t.filt.words, t.rank));
     (*n_fallback)++;
     *repaired = true;
   }
@@ -671,7 +676,7 @@ static void plan_filtered(const Corpus* c, Ticket& t, uint32_t nq, uint32_t k, c
   // of the rows it passes) skips the screen; the re-rank and cand_final serve every family but Exact (Count: when the
   // count path would rank the batch), k <= 256
   const Family f = family(c);
-  const bool direct_ok = filter_rows && k > 0 && k <= 256 &&
+  const bool direct_ok = filter_rows && k > 0 && k <= 256 && screened_ranking(c, t.rank) &&
                          (f == Family::Dot || f == Family::Centred || f == Family::Lp || count_ranked(c, k));
   for (uint32_t q = 0; q < nq; q++) {
     const uint64_t rows_q = filter_rows ? filter_rows[t.h_qf[q]] : ~0ull;
@@ -688,7 +693,7 @@ static void plan_filtered(const Corpus* c, Ticket& t, uint32_t nq, uint32_t k, c
 static sdb_status submit_locked(Corpus* c, Ticket* t, const double* d_queries, uint32_t nq, uint32_t k, uint64_t row_base,
                                 uint64_t* d_out_rows, double* d_out_dist, uint32_t* d_out_count,
                                 const volatile int* cancel, const uint32_t* d_filters, const uint32_t* query_filter,
-                                const uint64_t* filter_rows) {
+                                const uint64_t* filter_rows, const Ranking& rank) {
   if (!c->finalized) {
     set_error("corpus not finalized (call sdb_corpus_finalize after the last append)");
     return SDB_EINVAL;
@@ -715,6 +720,7 @@ static sdb_status submit_locked(Corpus* c, Ticket* t, const double* d_queries, u
   t->filt = FiltArg();
   t->n_direct = 0;
   t->permuted = false;
+  t->rank = rank;
   if (d_filters) {
     std::vector<uint32_t> scr, dir;
     plan_filtered(c, *t, nq, k, d_filters, query_filter, filter_rows, &scr, &dir);
@@ -745,12 +751,12 @@ static sdb_status submit_locked(Corpus* c, Ticket* t, const double* d_queries, u
   t->launches0 = c->ctx->launches;
   t->n_repaired = 0;
   sdb_screen first, first_scr;
-  const std::vector<Rung> rungs = build_rungs(c, c->screen, k, nq, &first);
+  const std::vector<Rung> rungs = build_rungs(c, c->screen, k, nq, rank, &first);
   t->rung = (c->rung_scr == first && c->rung_k == k && c->rung < n_batch_rungs(rungs)) ? c->rung : 0;
   t->n_batch_rungs = n_batch_rungs(rungs);
   // the ladder of its screened queries, which a mixed batch screens on their own (one Lp query has none, build_rungs)
   const uint32_t n_scr = t->n_direct < nq ? nq - t->n_direct : nq;
-  t->n_rungs = (uint32_t)build_rungs(c, c->screen, k, n_scr, &first_scr).size();
+  t->n_rungs = (uint32_t)build_rungs(c, c->screen, k, n_scr, rank, &first_scr).size();
   if (nq == 0 || k == 0) {  // nothing to search: counts are zero
     cudaStream_t st = t->stream;
     SDB_CUDA(cudaEventRecord(t->ev_begin, st));
@@ -1449,15 +1455,19 @@ sdb_status submit_call(Corpus* c, Ticket* t, uint32_t nq, uint32_t k, const KnnC
   // host inputs travel on the copy stream, so the transfer of batch i+1 overlaps the kernels of batch i
   cudaStream_t cs = c->ctx->copy_stream;
   const double* d_queries = call.queries;
-  if (call.host_in) {
-    SDB_CUDA(t->d_in_q.reserve((size_t)nq * c->dim));
-    SDB_CUDA(cudaMemcpyAsync(t->d_in_q, call.queries, sizeof(double) * (size_t)nq * c->dim, cudaMemcpyHostToDevice, cs));
+  const bool zero_q = !call.queries && nq;  // an SDB_FN_MAGNITUDE ranking without queries: it reads zero vectors
+  if (call.host_in || zero_q) {
+    SDB_CUDA(t->d_in_q.reserve(std::max<size_t>(1, (size_t)nq * c->dim)));
+    if (call.queries)
+      SDB_CUDA(cudaMemcpyAsync(t->d_in_q, call.queries, sizeof(double) * (size_t)nq * c->dim, cudaMemcpyHostToDevice, cs));
+    else
+      SDB_CUDA(cudaMemsetAsync(t->d_in_q, 0, sizeof(double) * (size_t)nq * c->dim, cs));
     d_queries = t->d_in_q;
   }
   const uint32_t* bits = nullptr;
   std::vector<uint64_t> rows_per_filter;
   if (call.rf.bits) SDB_TRY(stage_filters(c, *t, call.rf, call.host_in, nq, &bits, &rows_per_filter));
-  t->wait_h2d = call.host_in || call.rf.bits;
+  t->wait_h2d = call.host_in || zero_q || call.rf.bits;
   if (t->wait_h2d) SDB_CUDA(cudaEventRecord(t->ev_h2d, cs));
   uint64_t* d_rows = call.out_rows;
   double* d_dist = call.out_dist;
@@ -1469,7 +1479,7 @@ sdb_status submit_call(Corpus* c, Ticket* t, uint32_t nq, uint32_t k, const KnnC
     d_count = t->res.count;
   }
   SDB_TRY(submit_locked(c, t, d_queries, nq, k, call.row_base, d_rows, d_dist, d_count, call.cancel, bits,
-                        call.rf.query_filter, call.rf.bits ? rows_per_filter.data() : nullptr));
+                        call.rf.query_filter, call.rf.bits ? rows_per_filter.data() : nullptr, call.rank));
   if (!call.host_out) return SDB_OK;
   t->h_out_rows = call.out_rows;
   t->h_out_dist = call.out_dist;
@@ -1643,6 +1653,7 @@ sdb_status sdb_debug_screen_batch_filtered(sdb_corpus* c, const double* queries,
   t->filt = FiltArg();
   t->n_direct = 0;
   t->permuted = false;
+  t->rank = Ranking();
   if (filters) {
     const uint32_t* bits = nullptr;
     std::vector<uint64_t> rows_per_filter;
@@ -1862,6 +1873,93 @@ sdb_status sdb_knn_submit_filtered(sdb_corpus* c, const double* queries, uint32_
   SDB_TRY(check_filters(nq, filters, n_filters, query_filter));
   const RowFilters rf{filters, n_filters, query_filter, 0};
   return knn_call(c, nq, k, host_call(c, queries, rf, out_rows, out_dist, out_count, nullptr), ticket);
+}
+
+// ---- ORDER BY vector::<fn>(field, $q) ASC|DESC LIMIT k: the brute-force driver with another ranking -----------------
+static bool vector_fn_known(int fn) {
+  return (fn >= (int)SDB_CHEBYSHEV && fn <= (int)SDB_PEARSON) || fn == SDB_FN_SIMILARITY_COSINE || fn == SDB_FN_DOT ||
+         fn == SDB_FN_MAGNITUDE;
+}
+// the checks every sdb_corpus_order_* call shares; host: queries and outputs are host memory
+static sdb_status order_args(sdb_corpus* c, const double* queries, uint32_t nq, int fn, int order, uint32_t k,
+                             const uint32_t* filters, uint32_t n_filters, const uint32_t* query_filter,
+                             const uint64_t* out_rows, const double* out_value, const uint32_t* out_count,
+                             Ranking* rank) {
+  if (!c) return SDB_EINVAL;
+  if (!vector_fn_known(fn)) {
+    set_error("sdb_corpus_order: unknown vector function %d", fn);
+    return SDB_EINVAL;
+  }
+  if (order != SDB_ORDER_ASC && order != SDB_ORDER_DESC) {
+    set_error("sdb_corpus_order: unknown order %d", order);
+    return SDB_EINVAL;
+  }
+  if (nq && ((!queries && fn != SDB_FN_MAGNITUDE) || !out_count || (k && (!out_rows || !out_value)))) {
+    set_error("sdb_corpus_order: NULL queries (only SDB_FN_MAGNITUDE takes none) or outputs");
+    return SDB_EINVAL;
+  }
+  if (k > 4096) {
+    set_error("sdb_corpus_order: k = %u exceeds 4096", k);
+    return SDB_EUNSUPPORTED;
+  }
+  if (filters) SDB_TRY(check_filters(nq, filters, n_filters, query_filter));
+  *rank = Ranking{fn, order == SDB_ORDER_DESC};
+  return SDB_OK;
+}
+
+sdb_status sdb_corpus_order_topk(sdb_corpus* c, const double* queries, uint32_t nq, int fn, int order, uint32_t k,
+                                 const uint32_t* filters, uint32_t n_filters, const uint32_t* query_filter,
+                                 uint64_t* out_rows, double* out_value, uint32_t* out_count) {
+  Ranking rank;
+  SDB_TRY(order_args(c, queries, nq, fn, order, k, filters, n_filters, query_filter, out_rows, out_value, out_count,
+                     &rank));
+  if (nq == 0) return SDB_OK;
+  KnnCall call = host_call(c, queries, RowFilters{filters, n_filters, query_filter, 0}, out_rows, out_value, out_count,
+                           nullptr);
+  call.rank = rank;
+  return knn_call(c, nq, k, call, nullptr);
+}
+
+sdb_status sdb_corpus_order_topk_device(sdb_corpus* c, const double* d_queries, uint32_t nq, int fn, int order,
+                                        uint32_t k, const uint32_t* d_filters, uint32_t n_filters,
+                                        const uint32_t* query_filter, uint64_t row_base, uint64_t* d_out_rows,
+                                        double* d_out_value, uint32_t* d_out_count) {
+  Ranking rank;
+  SDB_TRY(order_args(c, d_queries, nq, fn, order, k, d_filters, n_filters, query_filter, d_out_rows, d_out_value,
+                     d_out_count, &rank));
+  if (nq == 0) return SDB_OK;
+  KnnCall call = device_call(d_queries, RowFilters{d_filters, n_filters, query_filter, 0}, row_base, d_out_rows,
+                             d_out_value, d_out_count);
+  call.rank = rank;
+  return knn_call(c, nq, k, call, nullptr);
+}
+
+sdb_status sdb_corpus_order_submit(sdb_corpus* c, const double* queries, uint32_t nq, int fn, int order,
+                                   uint32_t k, const uint32_t* filters, uint32_t n_filters,
+                                   const uint32_t* query_filter, uint64_t* out_rows, double* out_value,
+                                   uint32_t* out_count, uint32_t* ticket) {
+  Ranking rank;
+  if (!ticket || !nq) return SDB_EINVAL;
+  SDB_TRY(order_args(c, queries, nq, fn, order, k, filters, n_filters, query_filter, out_rows, out_value, out_count,
+                     &rank));
+  KnnCall call = host_call(c, queries, RowFilters{filters, n_filters, query_filter, 0}, out_rows, out_value, out_count,
+                           nullptr);
+  call.rank = rank;
+  return knn_call(c, nq, k, call, ticket);
+}
+
+sdb_status sdb_corpus_order_submit_device(sdb_corpus* c, const double* d_queries, uint32_t nq, int fn,
+                                          int order, uint32_t k, const uint32_t* d_filters, uint32_t n_filters,
+                                          const uint32_t* query_filter, uint64_t row_base, uint64_t* d_out_rows,
+                                          double* d_out_value, uint32_t* d_out_count, uint32_t* ticket) {
+  Ranking rank;
+  if (!ticket) return SDB_EINVAL;
+  SDB_TRY(order_args(c, d_queries, nq, fn, order, k, d_filters, n_filters, query_filter, d_out_rows, d_out_value,
+                     d_out_count, &rank));
+  KnnCall call = device_call(d_queries, RowFilters{d_filters, n_filters, query_filter, 0}, row_base, d_out_rows,
+                             d_out_value, d_out_count);
+  call.rank = rank;
+  return knn_call(c, nq, k, call, ticket);
 }
 
 sdb_status sdb_corpus_project(sdb_corpus* c, const double* query, int fn, double* out) {

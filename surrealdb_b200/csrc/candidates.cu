@@ -77,7 +77,8 @@ __global__ void prep_queries_kernel(const double* __restrict__ q64, uint32_t dim
 __global__ void prep_queries_pearson_kernel(const double* __restrict__ q64, uint32_t dim, uint32_t dim_pad,
                                             float* __restrict__ q32, __nv_bfloat16* __restrict__ qbf,
                                             double* __restrict__ qmag, double2* __restrict__ qmom,
-                                            uint32_t* __restrict__ qflags, float* __restrict__ qbferr, uint32_t nq) {
+                                            uint32_t* __restrict__ qflags, float* __restrict__ qbferr, uint32_t nq,
+                                            bool desc) {
   const uint32_t q = blockIdx.x;
   __shared__ uint32_t s_flags;
   __shared__ float s_err2;
@@ -102,7 +103,7 @@ __global__ void prep_queries_pearson_kernel(const double* __restrict__ q64, uint
     for (uint32_t c = threadIdx.x; c < dim_pad; c += blockDim.x) {
       const double x = c < dim ? q64[(size_t)q * dim + c] : 0.0;
       const double dq = c < dim ? __dsub_rn(x, m2) : 0.0;
-      const float f = (float)__ddiv_rn(-dq, nrm);
+      const float f = (float)__ddiv_rn(desc ? dq : -dq, nrm);  // (desc: PEARSON DESC, largest pearson first)
       if (c < dim) q32[(size_t)q * dim + c] = f;
       const __nv_bfloat16 h = __float2bfloat16_rn(f);
       qbf[(size_t)q * dim_pad + c] = h;
@@ -537,7 +538,8 @@ sdb_status scratch_for(const Corpus* c, Scratch& s, uint32_t nq, uint32_t cap) {
   return SDB_OK;
 }
 
-sdb_status prep_queries(const Corpus* c, Scratch& s, const double* d_queries, uint32_t nq, cudaStream_t st) {
+sdb_status prep_queries(const Corpus* c, Scratch& s, const double* d_queries, uint32_t nq, cudaStream_t st,
+                        bool desc) {
   // d_queries may alias s.d_q64
   if (d_queries != s.d_q64)
     SDB_CUDA(cudaMemcpyAsync(s.d_q64, d_queries, sizeof(double) * (size_t)nq * c->dim, cudaMemcpyDeviceToDevice, st));
@@ -545,7 +547,7 @@ sdb_status prep_queries(const Corpus* c, Scratch& s, const double* d_queries, ui
   const Family f = family(c);
   if (f == Family::Centred)
     prep_queries_pearson_kernel<<<nq_pad, 128, 0, st>>>(s.d_q64, c->dim, c->dim_pad, s.d_q32, s.d_qbf16, s.d_qmag,
-                                                        s.d_qmom, s.d_qflags, s.d_qbferr, nq);
+                                                        s.d_qmom, s.d_qflags, s.d_qbferr, nq, desc);
   else
     prep_queries_kernel<<<nq_pad, 128, 0, st>>>(s.d_q64, c->dim, c->dim_pad, (int)c->metric, s.d_q32, s.d_qbf16,
                                                 s.d_qmag, s.d_qflags, s.d_qbferr, nq);
@@ -1060,24 +1062,29 @@ constexpr uint32_t QCHUNK = 1024;  // query columns staged in shared memory per 
 
 constexpr uint32_t RR_GROUPS_Y = 4;  // blocks per query; block y takes the groups y, y + 4, ... of its query
 
-struct RerankOut {  // nq x stride results: the distance's key, the distance, the row
+struct RerankOut {  // nq x stride results: the value's key, the value, the row
   uint64_t* key;
   double* dist;
   uint32_t* row;
   uint32_t stride;
+  bool desc;  // cosine_desc batches: the value is the cosine similarity, keyed descending
 };
 __device__ __forceinline__ void rr_store(const RerankOut& out, uint32_t q, uint32_t e, uint32_t row, double d) {
   const size_t o = (size_t)q * out.stride + e;
-  out.key[o] = dist_key(d);
+  out.key[o] = order_key(d, out.desc);
   out.dist[o] = d;
   out.row[o] = row;
 }
-static RerankOut rr_out(const Scratch& s) { return RerankOut{s.d_rr_key, s.d_rr_dist, s.d_rr_row, s.rr_stride}; }
+static RerankOut rr_out(const Scratch& s, bool desc = false) {
+  return RerankOut{s.d_rr_key, s.d_rr_dist, s.d_rr_row, s.rr_stride, desc};
+}
 
-// the COSINE / EUCLIDEAN finish of one entry
-__device__ __forceinline__ double dot_finish(bool cosine, const RefSum& s, const double* mag, uint32_t row, double qm,
-                                             bool q_nan) {
-  return cosine ? RefAcc<SDB_COSINE>{}.finish(s, mag[row], qm, q_nan) : RefAcc<SDB_EUCLIDEAN>{}.finish(s, q_nan);
+// the COSINE / EUCLIDEAN finish of one entry (sim: COSINE's similarity instead of its distance)
+__device__ __forceinline__ double dot_finish(bool cosine, bool sim, const RefSum& s, const double* mag, uint32_t row,
+                                             double qm, bool q_nan) {
+  if (!cosine) return RefAcc<SDB_EUCLIDEAN>{}.finish(s, q_nan);
+  return sim ? RefAcc<SDB_FN_SIMILARITY_COSINE>{}.finish(s, mag[row], qm, q_nan)
+             : RefAcc<SDB_COSINE>{}.finish(s, mag[row], qm, q_nan);
 }
 
 // Staged: blocks (x = query, y = 0..3) stride over groups of 128 entries; each warp takes 32 entries and walks their
@@ -1134,7 +1141,7 @@ __global__ void __launch_bounds__(RR_WARPS * 32) cand_rerank_kernel(
         __syncwarp();
       }
     }
-    if (my_row != NO_ROW) rr_store(out, q, e, my_row, dot_finish(metric == SDB_COSINE, acc, mag, my_row, qm, q_nan));
+    if (my_row != NO_ROW) rr_store(out, q, e, my_row, dot_finish(metric == SDB_COSINE, out.desc, acc, mag, my_row, qm, q_nan));
   }
 }
 
@@ -1212,7 +1219,7 @@ __global__ void __launch_bounds__(RR_WARPS * 32) cand_rerank_v4_kernel(
         __syncwarp();
       }
     }
-    if (my_row != NO_ROW) rr_store(out, q, e, my_row, dot_finish(metric == SDB_COSINE, acc, mag, my_row, qm, q_nan));
+    if (my_row != NO_ROW) rr_store(out, q, e, my_row, dot_finish(metric == SDB_COSINE, out.desc, acc, mag, my_row, qm, q_nan));
   }
 }
 constexpr size_t RRV_SMEM = sizeof(double) * QCHUNK + sizeof(float) * RR_WARPS * 32 * RRV_STRIDE;  // 75.8 KB
@@ -1272,7 +1279,7 @@ __global__ void __launch_bounds__(128) cand_rerank_packed_kernel(
     } else {
       for (uint32_t j = 0; j < dim; j++) ref.step(acc, (double)__ldg(x + j), __ldg(qv + j));
     }
-    rr_store(out, q, e, my_row, dot_finish(M == SDB_COSINE, acc, mag, my_row, qm, q_nan));
+    rr_store(out, q, e, my_row, dot_finish(M == SDB_COSINE, out.desc, acc, mag, my_row, qm, q_nan));
   }
 }
 
@@ -1337,65 +1344,67 @@ __global__ void __launch_bounds__(128) cand_rerank_entry_kernel(
 }
 
 template <int M>
-static void rerank_entry(const Corpus* c, Scratch& s, uint32_t nq, uint32_t n_sp, cudaStream_t st) {
+static void rerank_entry(const Corpus* c, Scratch& s, uint32_t nq, uint32_t n_sp, bool desc, cudaStream_t st) {
   const dim3 grid(nq, RR_GROUPS_Y);
   const EntryArgs a{c->minkowski_p, c->d_mom, s.d_qmom, c->d_jfirst, c->d_jux, s.d_qkey.get(), s.d_qjac};
   if (c->dtype == SDB_F32)
     cand_rerank_entry_kernel<float, M><<<grid, 128, 0, st>>>((const float*)c->d_rows.get(), c->dim, s.d_q64, s.d_qflags,
                                                              s.d_cand, s.d_cand_cnt, s.sc_cap, c->d_special, n_sp,
-                                                             rr_out(s), a);
+                                                             rr_out(s, desc), a);
   else
     cand_rerank_entry_kernel<double, M><<<grid, 128, 0, st>>>((const double*)c->d_rows.get(), c->dim, s.d_q64,
                                                               s.d_qflags, s.d_cand, s.d_cand_cnt, s.sc_cap,
-                                                              c->d_special, n_sp, rr_out(s), a);
+                                                              c->d_special, n_sp, rr_out(s, desc), a);
 }
 
 template <typename T>
-static void rerank_packed(const Corpus* c, Scratch& s, uint32_t nq, uint32_t n_sp, cudaStream_t st) {
+static void rerank_packed(const Corpus* c, Scratch& s, uint32_t nq, uint32_t n_sp, bool desc, cudaStream_t st) {
   auto kern = c->metric == SDB_COSINE ? cand_rerank_packed_kernel<T, SDB_COSINE> : cand_rerank_packed_kernel<T, SDB_EUCLIDEAN>;
   kern<<<(nq + 7) / 8, 128, 0, st>>>((const T*)c->d_rows.get(), c->dim, c->d_mag, s.d_q64, s.d_qmag, s.d_qflags,
-                                     s.d_cand, s.d_cand_cnt, s.sc_cap, c->d_special, n_sp, nq, rr_out(s));
+                                     s.d_cand, s.d_cand_cnt, s.sc_cap, c->d_special, n_sp, nq, rr_out(s, desc));
 }
 
 // COSINE / EUCLIDEAN: the packed kernel for the small sets stage B leaves; otherwise the vectorised one for f32 rows
 // of a length divisible by 4, the staged one for the rest
-static void rerank_dot(const Corpus* c, Scratch& s, uint32_t nq, bool small_sets, uint32_t n_sp, cudaStream_t st) {
+static void rerank_dot(const Corpus* c, Scratch& s, uint32_t nq, bool small_sets, uint32_t n_sp, bool desc,
+                       cudaStream_t st) {
   const dim3 grid(nq, RR_GROUPS_Y);
-  if (small_sets && c->dtype == SDB_F32) rerank_packed<float>(c, s, nq, n_sp, st);
-  else if (small_sets) rerank_packed<double>(c, s, nq, n_sp, st);
+  const RerankOut out = rr_out(s, desc);
+  if (small_sets && c->dtype == SDB_F32) rerank_packed<float>(c, s, nq, n_sp, desc, st);
+  else if (small_sets) rerank_packed<double>(c, s, nq, n_sp, desc, st);
   else if (c->dtype == SDB_F32 && c->dim % 4 == 0)
     cand_rerank_v4_kernel<<<grid, RR_WARPS * 32, RRV_SMEM, st>>>((const float*)c->d_rows.get(), c->dim, (int)c->metric,
                                                                 c->d_mag, s.d_q64, s.d_qmag, s.d_qflags, s.d_cand,
-                                                                s.d_cand_cnt, s.sc_cap, c->d_special, n_sp, rr_out(s));
+                                                                s.d_cand_cnt, s.sc_cap, c->d_special, n_sp, out);
   else if (c->dtype == SDB_F32)
     cand_rerank_kernel<float><<<grid, RR_WARPS * 32, 0, st>>>((const float*)c->d_rows.get(), c->dim, (int)c->metric,
                                                              c->d_mag, s.d_q64, s.d_qmag, s.d_qflags, s.d_cand,
-                                                             s.d_cand_cnt, s.sc_cap, c->d_special, n_sp, rr_out(s));
+                                                             s.d_cand_cnt, s.sc_cap, c->d_special, n_sp, out);
   else
     cand_rerank_kernel<double><<<grid, RR_WARPS * 32, 0, st>>>((const double*)c->d_rows.get(), c->dim, (int)c->metric,
                                                               c->d_mag, s.d_q64, s.d_qmag, s.d_qflags, s.d_cand,
-                                                              s.d_cand_cnt, s.sc_cap, c->d_special, n_sp, rr_out(s));
+                                                              s.d_cand_cnt, s.sc_cap, c->d_special, n_sp, out);
 }
 
 sdb_status cand_rerank(const Corpus* c, Scratch& s, const FiltArg& filt, uint32_t nq, cudaStream_t st,
-                       bool small_sets) {
+                       bool small_sets, bool desc) {
   const uint32_t n_sp = filt.bits ? 0u : c->n_special;  // filtered: the passing special rows are in the lists
   switch (family(c)) {
     case Family::Count:  // (the direct regime only; no special rows)
-      if (c->metric == SDB_HAMMING) rerank_entry<SDB_HAMMING>(c, s, nq, n_sp, st);
-      else rerank_entry<SDB_JACCARD>(c, s, nq, n_sp, st);
+      if (c->metric == SDB_HAMMING) rerank_entry<SDB_HAMMING>(c, s, nq, n_sp, desc, st);
+      else rerank_entry<SDB_JACCARD>(c, s, nq, n_sp, desc, st);
       break;
     case Family::Lp:
-      if (c->metric == SDB_MANHATTAN) rerank_entry<SDB_MANHATTAN>(c, s, nq, n_sp, st);
-      else if (c->metric == SDB_MINKOWSKI) rerank_entry<SDB_MINKOWSKI>(c, s, nq, n_sp, st);
-      else rerank_entry<SDB_CHEBYSHEV>(c, s, nq, n_sp, st);
+      if (c->metric == SDB_MANHATTAN) rerank_entry<SDB_MANHATTAN>(c, s, nq, n_sp, desc, st);
+      else if (c->metric == SDB_MINKOWSKI) rerank_entry<SDB_MINKOWSKI>(c, s, nq, n_sp, desc, st);
+      else rerank_entry<SDB_CHEBYSHEV>(c, s, nq, n_sp, desc, st);
       break;
     case Family::Centred:  // one kernel for small (after stage B) and large (direct regime, no stage B) sets
-      rerank_entry<SDB_PEARSON>(c, s, nq, n_sp, st);
+      rerank_entry<SDB_PEARSON>(c, s, nq, n_sp, desc, st);
       break;
     case Family::Dot:
     case Family::Exact:  // (never reaches the re-rank: the exact kernel alone ranks it)
-      rerank_dot(c, s, nq, small_sets, n_sp, st);
+      rerank_dot(c, s, nq, small_sets, n_sp, desc, st);
       break;
   }
   count_launch(c->ctx);
@@ -1405,7 +1414,8 @@ sdb_status cand_rerank(const Corpus* c, Scratch& s, const FiltArg& filt, uint32_
 
 // ------------------------------------------------------------------------------------------------
 // final ordering + proof.  Entries sorted ascending by (Number::cmp key, row) -- exactly the
-// DistanceEntry order of KnnTopK (knn_topk.rs:61-73): nearest first, earlier scan position wins ties.
+// DistanceEntry order of KnnTopK (knn_topk.rs:61-73): nearest first, earlier scan position wins ties.  A cosine_desc
+// batch's keys are order_key(similarity, desc): most similar first, ties again by scan position (SortTopK's order).
 // The candidate count varies per query (a handful on spread-out data, thousands inside a tight cluster), so the sort
 // works on a fixed 512-entry window: up to 512 entries are sorted in one go; longer lists are folded in chunks of
 // 256 into the running best 256 (k <= 256 on the screened path).
@@ -1443,7 +1453,7 @@ __global__ void __launch_bounds__(256)
                       const float* __restrict__ beps2, uint32_t* __restrict__ flags, const uint32_t* __restrict__ qflags,
                       uint32_t* __restrict__ stat, int metric, uint32_t k, uint64_t row_base,
                       uint64_t* __restrict__ out_rows, double* __restrict__ out_dist, uint32_t* __restrict__ out_count,
-                      int debug, double eps_ref) {
+                      int debug, double eps_ref, bool desc) {
   __shared__ uint64_t s_key[FIN_WIN];  // distance key
   __shared__ uint64_t s_idx[FIN_WIN];  // (row << 32 | entry): secondary order by row (unique), entry = index into rr_*
   const uint32_t q = blockIdx.x;
@@ -1501,6 +1511,13 @@ __global__ void __launch_bounds__(256)
         // the top k if that bound (rounded down) is strictly above the k-th exact key.  No stage B ran (tau2 = -inf).
         const double L = (-(double)t - (double)beps[q]) * (1.0 - 1e-12);
         ok = dist_key(L) > kth;
+      } else if (F == Family::Centred && desc) {
+        // PEARSON DESC: the screen scored s = cos(dx, +dq) |dq| / bscale and the entries are pearsons keyed descending.
+        // Non-candidate: cos(dx, dq) <= tau bscale / |dq| + beps  =>  pearson <= tau bscale / |dq| + beps + eps_ref,
+        // rounded up; proven when that upper bound sorts strictly after the k-th entry
+        const double a = __ddiv_ru(__dmul_ru((double)t, (double)bscale[q]), qm);
+        const double U = __dadd_ru(__dadd_ru(a, (double)beps[q]), eps_ref);
+        ok = order_key(U, true) > kth;
       } else if (F == Family::Centred) {
         // the screen scored s = cos(dx, -dq) |dq| / bscale.  Non-candidate: score <= tau  =>  cos(dx, dq) >= -tau
         // bscale / |dq| - beps  =>  pearson >= -tau bscale / |dq| - beps - eps_ref, evaluated with directed rounding
@@ -1508,6 +1525,11 @@ __global__ void __launch_bounds__(256)
         const double a = __ddiv_ru(__dmul_ru((double)t, (double)bscale[q]), qm);
         const double L = __dsub_rd(__dsub_rd(-a, (double)beps[q]), eps_ref);
         ok = dist_key(L) > kth;
+      } else if (metric == SDB_COSINE && desc) {
+        // cosine_desc: the entries are similarities keyed descending.  Non-candidate: sim <= tau * bscale / |q| + eps,
+        // so it cannot reach the top k if that upper bound sorts strictly after the k-th entry
+        const double upper = (double)t * (double)bscale[q] / qm + (double)beps[q] + 1e-9;
+        ok = order_key(upper, true) > kth;
       } else if (metric == SDB_COSINE) {
         // non-candidate: score <= tau  =>  sim <= tau * bscale / |q| + eps  =>  dist >= 1 - tau * bscale / |q| - eps
         const double bound = 1.0 - (double)t * (double)bscale[q] / qm - (double)beps[q] - 1e-9;
@@ -1520,9 +1542,15 @@ __global__ void __launch_bounds__(256)
       // stage B dropped candidates whose f32 score is below tau2: the same proof with the f32 bound
       const float t2 = tau2[q];
       if (ok && t2 > __int_as_float(0xff800000)) {
-        if (F == Family::Centred) {  // stage B scores in the same units with bscale 1
+        if (F == Family::Centred && desc) {
+          const double U2 = __dadd_ru(__dadd_ru(__ddiv_ru((double)t2, qm), (double)beps2[q]), eps_ref);
+          ok = order_key(U2, true) > kth;
+        } else if (F == Family::Centred) {  // stage B scores in the same units with bscale 1
           const double L2 = __dsub_rd(__dsub_rd(-__ddiv_ru((double)t2, qm), (double)beps2[q]), eps_ref);
           ok = dist_key(L2) > kth;
+        } else if (metric == SDB_COSINE && desc) {
+          const double upper2 = (double)t2 / qm + (double)beps2[q] + 1e-9;
+          ok = order_key(upper2, true) > kth;
         } else if (metric == SDB_COSINE) {
           const double bound2 = 1.0 - (double)t2 / qm - (double)beps2[q] - 1e-9;
           ok = dist_key(bound2) > kth;
@@ -1545,7 +1573,7 @@ __global__ void __launch_bounds__(256)
 }
 
 sdb_status cand_final(const Corpus* c, Scratch& s, const FiltArg& filt, uint32_t nq, uint32_t k, uint64_t row_base,
-                      uint64_t* d_out_rows, double* d_out_dist, uint32_t* d_out_count, cudaStream_t st) {
+                      uint64_t* d_out_rows, double* d_out_dist, uint32_t* d_out_count, cudaStream_t st, bool desc) {
   if (k > FIN_KEEP) {
     set_error("cand_final: k = %u exceeds the screened path's limit of %u", k, FIN_KEEP);
     return SDB_EINVAL;
@@ -1570,7 +1598,8 @@ sdb_status cand_final(const Corpus* c, Scratch& s, const FiltArg& filt, uint32_t
   }
   fin<<<nq, 256, 0, st>>>(s.d_rr_key, s.d_rr_dist, s.d_rr_row, s.rr_stride, s.d_cand_cnt, s.sc_cap, n_sp,
                           s.d_tau, s.d_qmag, s.d_bscale, s.d_beps, s.d_tau2, s.d_beps2, s.d_flags, s.d_qflags,
-                          s.d_stat, (int)c->metric, k, row_base, d_out_rows, d_out_dist, d_out_count, debug, eps_ref);
+                          s.d_stat, (int)c->metric, k, row_base, d_out_rows, d_out_dist, d_out_count, debug, eps_ref,
+                          desc);
   count_launch(c->ctx);
   SDB_CUDA(cudaGetLastError());
   return SDB_OK;

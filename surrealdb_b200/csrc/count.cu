@@ -30,7 +30,10 @@ template <typename T>
 using CountKey = EqKey<T>;
 
 // List entries: HAMMING packs (count << 32 | row) into one integer; JACCARD's distance is a ratio, so its entries are
-// (dist_key(d), row) pairs.  Both order as (distance, row), which is unique per list.
+// (dist_key(d), row) pairs.  Both order as (distance, row), which is unique per list.  A descending batch (desc) keeps
+// the complement of the value's half instead -- ~count, order_key(d, true) -- so the same lists and the same merge keep
+// the k largest values, earlier rows first: the union of every range's k best still holds the query's k best, ties
+// included, in either direction.
 struct JEntry {
   unsigned long long key;
   uint32_t row;
@@ -88,7 +91,7 @@ __global__ void __launch_bounds__(LP_THREADS, 1) count_hamming_kernel(
     const T* __restrict__ rows, uint32_t dim, uint64_t n_rows, const uint8_t* __restrict__ skip,
     const CountKey<T>* __restrict__ qkey, uint32_t nq, uint32_t k, uint32_t n_ranges, uint32_t* __restrict__ cnt,
     uint64_t* __restrict__ rr_key, double* __restrict__ rr_dist, uint32_t* __restrict__ rr_row, uint32_t rr_stride,
-    FiltArg filt) {
+    FiltArg filt, bool desc) {
   using K = CountKey<T>;
   constexpr int NTQ = QB / TQ, NTR = LP_THREADS / NTQ, TR = LP_RB / NTR;
   constexpr int XL = LP_RB * LP_KC / LP_THREADS, QL = QB * LP_KC / LP_THREADS;
@@ -185,7 +188,7 @@ __global__ void __launch_bounds__(LP_THREADS, 1) count_hamming_kernel(
 #pragma unroll
           for (int i = 0; i < TR; i++) {
             const uint32_t row = (uint32_t)(row0 + tr + NTR * i);
-            const uint64_t e = ((uint64_t)acc[i][j] << 32) | row;
+            const uint64_t e = ((uint64_t)(desc ? ~acc[i][j] : acc[i][j]) << 32) | row;
             const bool want = mine && row_ok[i] && e < s_max[ql] && (!FILT || filt_pass(filt, q, row));
             uint32_t m = __ballot_sync(0xffffffffu, want);
             while (m) {
@@ -212,9 +215,10 @@ __global__ void __launch_bounds__(LP_THREADS, 1) count_hamming_kernel(
         const uint64_t* L = s_list + (size_t)ql * k;
         for (uint32_t p = lane; p < fill; p += 32) {
           const uint64_t v = L[p];
-          const double d = (double)(uint32_t)(v >> 32);
+          const uint32_t cv = (uint32_t)(v >> 32);
+          const double d = (double)(desc ? ~cv : cv);
           const size_t o = (size_t)q * rr_stride + base + p;
-          rr_key[o] = dist_key(d);
+          rr_key[o] = order_key(d, desc);
           rr_dist[o] = d;
           rr_row[o] = (uint32_t)v;
         }
@@ -278,7 +282,7 @@ __global__ void __launch_bounds__(JQ_QB * 32) count_jaccard_kernel(
     const uint32_t* __restrict__ jfirst, const uint32_t* __restrict__ jux, const EqKey<T>* __restrict__ qkey,
     const uint32_t* __restrict__ qjac, uint32_t nq, uint32_t k, uint32_t n_ranges, uint32_t* __restrict__ cnt,
     uint64_t* __restrict__ rr_key, double* __restrict__ rr_dist, uint32_t* __restrict__ rr_row, uint32_t rr_stride,
-    FiltArg filt) {
+    FiltArg filt, bool desc) {
   __shared__ JEntry s_max[JQ_QB];
   __shared__ uint32_t s_pos[JQ_QB], s_fill[JQ_QB];
   extern __shared__ __align__(16) unsigned char s_raw[];
@@ -299,7 +303,9 @@ __global__ void __launch_bounds__(JQ_QB * 32) count_jaccard_kernel(
       const uint64_t row = r0 + lane;
       const bool ok = row < r_end && !(skip && __ldg(skip + row)) && (!FILT || filt_pass(filt, q, (uint32_t)row));
       JEntry e{~0ull, (uint32_t)row};
-      if (ok) e.key = dist_key(jaccard_counts(rows + row * dim, dim, jfirst + row * words, __ldg(jux + row), qk, n_look, uq));
+      if (ok)
+        e.key = order_key(jaccard_counts(rows + row * dim, dim, jfirst + row * words, __ldg(jux + row), qk, n_look, uq),
+                          desc);
       uint32_t m = __ballot_sync(0xffffffffu, ok && e < s_max[ql]);
       while (m) {
         const int src = __ffs(m) - 1;
@@ -316,7 +322,7 @@ __global__ void __launch_bounds__(JQ_QB * 32) count_jaccard_kernel(
       const JEntry v = L[p];
       const size_t o = (size_t)q * rr_stride + base + p;
       rr_key[o] = v.key;
-      rr_dist[o] = __longlong_as_double((long long)(v.key ^ 0x8000000000000000ull));
+      rr_dist[o] = __longlong_as_double((long long)((desc ? ~v.key : v.key) ^ 0x8000000000000000ull));
       rr_row[o] = v.row;
     }
     __syncwarp();
@@ -339,7 +345,7 @@ __global__ void count_qkeys_kernel(const double* __restrict__ q64, uint32_t nq, 
 // queries.  f64 keys stop at 32-query blocks, whose staging stays within the 48 KB of static shared memory.
 template <typename T, bool FILT, int QB, int TQ>
 static sdb_status launch_count(const Corpus* c, Scratch& s, const FiltArg& filt, uint32_t nq, uint32_t k,
-                               uint32_t n_ranges, cudaStream_t st) {
+                               uint32_t n_ranges, bool desc, cudaStream_t st) {
   auto kern = count_hamming_kernel<T, FILT, QB, TQ>;
   const size_t smem = sizeof(uint64_t) * QB * k;
   SDB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(sizeof(uint64_t) * QB * 256)));
@@ -353,18 +359,18 @@ static sdb_status launch_count(const Corpus* c, Scratch& s, const FiltArg& filt,
   if (grid > items) grid = items;
   kern<<<(unsigned)grid, LP_THREADS, smem, st>>>((const T*)c->d_rows.get(), c->dim, c->n, c->d_skip,
                                                  (const CountKey<T>*)s.d_qkey.get(), nq, k, n_ranges, s.d_cand_cnt,
-                                                 s.d_rr_key, s.d_rr_dist, s.d_rr_row, s.rr_stride, filt);
+                                                 s.d_rr_key, s.d_rr_dist, s.d_rr_row, s.rr_stride, filt, desc);
   count_launch(c->ctx);
   SDB_CUDA(cudaGetLastError());
   return SDB_OK;
 }
 template <typename T, bool FILT>
 static sdb_status launch_count_qb(const Corpus* c, Scratch& s, const FiltArg& filt, uint32_t nq, uint32_t k,
-                                  uint32_t n_ranges, cudaStream_t st) {
-  if (nq <= 8) return launch_count<T, FILT, 8, 1>(c, s, filt, nq, k, n_ranges, st);
-  if constexpr (sizeof(T) == 8) return launch_count<T, FILT, 32, 4>(c, s, filt, nq, k, n_ranges, st);
-  else return nq <= 32 ? launch_count<T, FILT, 32, 4>(c, s, filt, nq, k, n_ranges, st)
-                       : launch_count<T, FILT, 64, 4>(c, s, filt, nq, k, n_ranges, st);
+                                  uint32_t n_ranges, bool desc, cudaStream_t st) {
+  if (nq <= 8) return launch_count<T, FILT, 8, 1>(c, s, filt, nq, k, n_ranges, desc, st);
+  if constexpr (sizeof(T) == 8) return launch_count<T, FILT, 32, 4>(c, s, filt, nq, k, n_ranges, desc, st);
+  else return nq <= 32 ? launch_count<T, FILT, 32, 4>(c, s, filt, nq, k, n_ranges, desc, st)
+                       : launch_count<T, FILT, 64, 4>(c, s, filt, nq, k, n_ranges, desc, st);
 }
 
 uint32_t count_ranges(const Corpus* c, uint32_t nq, uint32_t k) {
@@ -403,7 +409,7 @@ sdb_status count_prep_queries(const Corpus* c, Scratch& s, uint32_t nq, cudaStre
 
 template <typename T, bool FILT>
 static sdb_status launch_count_jaccard(const Corpus* c, Scratch& s, const FiltArg& filt, uint32_t nq, uint32_t k,
-                                       uint32_t n_ranges, cudaStream_t st) {
+                                       uint32_t n_ranges, bool desc, cudaStream_t st) {
   auto kern = count_jaccard_kernel<T, FILT>;
   const size_t smem = sizeof(JEntry) * JQ_QB * k;  // at most 32 KB
   int per_sm = 1;
@@ -417,27 +423,28 @@ static sdb_status launch_count_jaccard(const Corpus* c, Scratch& s, const FiltAr
   kern<<<(unsigned)grid, JQ_QB * 32, smem, st>>>((const T*)c->d_rows.get(), c->dim, c->n, c->d_skip, c->d_jfirst,
                                                  c->d_jux, (const EqKey<T>*)s.d_qkey.get(), s.d_qjac, nq, k,
                                                  n_ranges, s.d_cand_cnt, s.d_rr_key, s.d_rr_dist, s.d_rr_row,
-                                                 s.rr_stride, filt);
+                                                 s.rr_stride, filt, desc);
   count_launch(c->ctx);
   SDB_CUDA(cudaGetLastError());
   return SDB_OK;
 }
 
-sdb_status count_pass(const Corpus* c, Scratch& s, const FiltArg& filt, uint32_t nq, uint32_t k, cudaStream_t st) {
+sdb_status count_pass(const Corpus* c, Scratch& s, const FiltArg& filt, uint32_t nq, uint32_t k, cudaStream_t st,
+                      bool desc) {
   if (nq == 0 || k == 0 || c->n == 0) return SDB_OK;
   const uint32_t n_ranges = count_ranges(c, nq, k);
   if (c->metric == SDB_JACCARD) {
     if (c->dtype == SDB_F32)
-      return filt.bits ? launch_count_jaccard<float, true>(c, s, filt, nq, k, n_ranges, st)
-                       : launch_count_jaccard<float, false>(c, s, filt, nq, k, n_ranges, st);
-    return filt.bits ? launch_count_jaccard<double, true>(c, s, filt, nq, k, n_ranges, st)
-                     : launch_count_jaccard<double, false>(c, s, filt, nq, k, n_ranges, st);
+      return filt.bits ? launch_count_jaccard<float, true>(c, s, filt, nq, k, n_ranges, desc, st)
+                       : launch_count_jaccard<float, false>(c, s, filt, nq, k, n_ranges, desc, st);
+    return filt.bits ? launch_count_jaccard<double, true>(c, s, filt, nq, k, n_ranges, desc, st)
+                     : launch_count_jaccard<double, false>(c, s, filt, nq, k, n_ranges, desc, st);
   }
   if (c->dtype == SDB_F32)
-    return filt.bits ? launch_count_qb<float, true>(c, s, filt, nq, k, n_ranges, st)
-                     : launch_count_qb<float, false>(c, s, filt, nq, k, n_ranges, st);
-  return filt.bits ? launch_count_qb<double, true>(c, s, filt, nq, k, n_ranges, st)
-                   : launch_count_qb<double, false>(c, s, filt, nq, k, n_ranges, st);
+    return filt.bits ? launch_count_qb<float, true>(c, s, filt, nq, k, n_ranges, desc, st)
+                     : launch_count_qb<float, false>(c, s, filt, nq, k, n_ranges, desc, st);
+  return filt.bits ? launch_count_qb<double, true>(c, s, filt, nq, k, n_ranges, desc, st)
+                   : launch_count_qb<double, false>(c, s, filt, nq, k, n_ranges, desc, st);
 }
 
 }  // namespace sdb

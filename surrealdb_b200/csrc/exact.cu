@@ -4,7 +4,8 @@
 //   * F64 corpora and SDB_SCREEN_NONE_EXACT,
 //   * queries the screens cannot bound (zero / non-finite query norm),
 //   * queries whose screened result failed the error-bound proof or overflowed its candidate buffer.
-// It never approximates, so the library's answer does not depend on the screens being right.
+// It never approximates, so the library's answer does not depend on the screens being right.  It also ranks every
+// vector function in either direction (sdb_corpus_order_*): the keys are order_key(value, desc).
 #include "exactmath.cuh"
 #include "internal.cuh"
 #include "rowwalk.cuh"
@@ -23,7 +24,7 @@ __global__ void __launch_bounds__(WARPS * 32) exact_keys_kernel(const T* __restr
                                                                 const uint32_t* __restrict__ qflags_p,
                                                                 uint64_t* __restrict__ keys,
                                                                 double* __restrict__ vals /* non-null: every row's value */,
-                                                                double mink_p) {
+                                                                double mink_p, bool desc) {
   __shared__ T tile[WARPS][32][33];
   __shared__ double s_q[EX_QCHUNK];
   __shared__ double s_qstat[2];  // pearson: mean and (population) deviation of the query
@@ -125,7 +126,7 @@ __global__ void __launch_bounds__(WARPS * 32) exact_keys_kernel(const T* __restr
           default:  // SDB_PEARSON
             d = RefAcc<SDB_PEARSON>::finish(acc, dim, RefAcc<SDB_PEARSON>::sd(acc.acc2, dim), s_qstat[1], q_nan);
         }
-        key = dist_key(d);
+        key = order_key(d, desc);
         if (vals) vals[r] = d;
       }
       if (keys) keys[r] = key;
@@ -152,7 +153,8 @@ template <typename T>
 __global__ void __launch_bounds__(128) jaccard_keys_kernel(const T* __restrict__ rows, uint32_t dim, uint64_t n,
                                                            const uint8_t* __restrict__ skip,
                                                            const double* __restrict__ q64, const uint8_t* __restrict__ qdup,
-                                                           uint64_t* __restrict__ keys, double* __restrict__ vals) {
+                                                           uint64_t* __restrict__ keys, double* __restrict__ vals,
+                                                           bool desc) {
   const uint32_t lane = threadIdx.x & 31;
   const uint64_t warp0 = ((uint64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   const uint64_t n_warps = ((uint64_t)gridDim.x * blockDim.x) >> 5;
@@ -187,22 +189,22 @@ __global__ void __launch_bounds__(128) jaccard_keys_kernel(const T* __restrict__
     }
     if (lane == 0) {
       const double d = __ddiv_rn((double)inter, (double)(distinct + fresh));  // (intersection_size / union.len() as f64)
-      if (keys) keys[r] = dist_key(d);
+      if (keys) keys[r] = order_key(d, desc);
       if (vals) vals[r] = d;
     }
   }
 }
 static sdb_status jaccard_launch(const Corpus* c, const double* d_q64, uint64_t* d_keys, double* d_vals,
-                                 cudaStream_t st) {
+                                 cudaStream_t st, bool desc = false) {
   Ctx* ctx = c->ctx;
   AsyncBuf<uint8_t> d_dup;
   SDB_CUDA(d_dup.reserve(c->dim, st));
   jaccard_qdup_kernel<<<(c->dim + 127) / 128, 128, 0, st>>>(d_q64, c->dim, d_dup);
   const int grid = ctx->sm_count * 16;
   if (c->dtype == SDB_F32)
-    jaccard_keys_kernel<float><<<grid, 128, 0, st>>>((const float*)c->d_rows.get(), c->dim, c->n, c->d_skip, d_q64, d_dup, d_keys, d_vals);
+    jaccard_keys_kernel<float><<<grid, 128, 0, st>>>((const float*)c->d_rows.get(), c->dim, c->n, c->d_skip, d_q64, d_dup, d_keys, d_vals, desc);
   else
-    jaccard_keys_kernel<double><<<grid, 128, 0, st>>>((const double*)c->d_rows.get(), c->dim, c->n, c->d_skip, d_q64, d_dup, d_keys, d_vals);
+    jaccard_keys_kernel<double><<<grid, 128, 0, st>>>((const double*)c->d_rows.get(), c->dim, c->n, c->d_skip, d_q64, d_dup, d_keys, d_vals, desc);
   count_launch(ctx, 2);
   SDB_CUDA(cudaGetLastError());
   return SDB_OK;
@@ -358,7 +360,7 @@ sdb_status exact_init_device() {
 // d_out_rows / d_out_dist / d_out_count point at THIS query's output row
 sdb_status exact_query(Corpus* c, const double* d_q64, const double* d_qmag, const uint32_t* d_qflags, uint32_t k,
                        uint64_t row_base, uint64_t* d_out_rows, double* d_out_dist, uint32_t* d_out_count,
-                       cudaStream_t st, const uint32_t* filter, uint32_t filter_words) {
+                       cudaStream_t st, const uint32_t* filter, uint32_t filter_words, const Ranking& rank) {
   Ctx* ctx = c->ctx;
   {
     const uint64_t cap = c->cap > c->n ? c->cap : c->n;
@@ -375,17 +377,19 @@ sdb_status exact_query(Corpus* c, const double* d_q64, const double* d_qmag, con
   uint64_t* g_key = reinterpret_cast<uint64_t*>(reinterpret_cast<char*>(c->d_sel.get()) + ((sizeof(SelState) + 63) / 64) * 64);
   uint32_t* g_row = reinterpret_cast<uint32_t*>(g_key + 4096);
   const uint64_t n = c->n;
-  if (n && c->metric == SDB_JACCARD) {
-    SDB_TRY(jaccard_launch(c, d_q64, c->d_ex_key, c->d_ex_val, st));
+  const int fn = rank.fn < 0 ? (int)c->metric : rank.fn;
+  if (n && fn == SDB_JACCARD) {
+    SDB_TRY(jaccard_launch(c, d_q64, c->d_ex_key, c->d_ex_val, st, rank.desc));
   } else if (n) {
     const int grid = ctx->sm_count * 8;
     if (c->dtype == SDB_F32)
-      exact_keys_kernel<float, 4><<<grid, 128, 0, st>>>((const float*)c->d_rows.get(), c->dim, n, (int)c->metric, c->d_mag,
-                                                        c->d_skip, d_q64, d_qmag, d_qflags, c->d_ex_key, c->d_ex_val, c->minkowski_p);
+      exact_keys_kernel<float, 4><<<grid, 128, 0, st>>>((const float*)c->d_rows.get(), c->dim, n, fn, c->d_mag,
+                                                        c->d_skip, d_q64, d_qmag, d_qflags, c->d_ex_key, c->d_ex_val,
+                                                        c->minkowski_p, rank.desc);
     else
-      exact_keys_kernel<double, 4><<<grid, 128, 0, st>>>((const double*)c->d_rows.get(), c->dim, n, (int)c->metric,
-                                                         c->d_mag, c->d_skip, d_q64, d_qmag, d_qflags, c->d_ex_key,
-                                                         c->d_ex_val, c->minkowski_p);
+      exact_keys_kernel<double, 4><<<grid, 128, 0, st>>>((const double*)c->d_rows.get(), c->dim, n, fn, c->d_mag,
+                                                         c->d_skip, d_q64, d_qmag, d_qflags, c->d_ex_key, c->d_ex_val,
+                                                         c->minkowski_p, rank.desc);
     count_launch(ctx);
   }
   if (n && filter) {
@@ -426,10 +430,10 @@ sdb_status exact_project(const Corpus* c, int fn, const double* d_q64, const dou
   const int grid = ctx->sm_count * 8;
   if (c->dtype == SDB_F32)
     exact_keys_kernel<float, 4><<<grid, 128, 0, st>>>((const float*)c->d_rows.get(), c->dim, n, fn, c->d_mag, c->d_skip,
-                                                      d_q64, d_qmag, d_qflags, nullptr, d_vals, c->minkowski_p);
+                                                      d_q64, d_qmag, d_qflags, nullptr, d_vals, c->minkowski_p, false);
   else
     exact_keys_kernel<double, 4><<<grid, 128, 0, st>>>((const double*)c->d_rows.get(), c->dim, n, fn, c->d_mag, c->d_skip,
-                                                       d_q64, d_qmag, d_qflags, nullptr, d_vals, c->minkowski_p);
+                                                       d_q64, d_qmag, d_qflags, nullptr, d_vals, c->minkowski_p, false);
   count_launch(ctx);
   SDB_CUDA(cudaGetLastError());
   return SDB_OK;

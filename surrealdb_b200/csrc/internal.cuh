@@ -132,6 +132,13 @@ __host__ __device__ inline uint64_t dist_key(double d) {
   if ((b << 1) == 0) b = 0;  // canonicalise -0.0
   return (b >> 63) ? ~b : (b | 0x8000000000000000ull);
 }
+// the key of a value in a ranking's direction: dist_key ascending, its complement descending (the whole total order
+// reversed, NaNs included).  ~dist_key(d) is ~0 -- the key the exact kernel reserves for skipped rows and the sorters
+// for padding -- only for the NaN whose bits are all set; that NaN takes the next key down and ties with 0xFFF...FE.
+__host__ __device__ inline uint64_t order_key(double d, bool desc) {
+  const uint64_t k = dist_key(d);
+  return !desc ? k : (k ? ~k : ~1ull);
+}
 __host__ __device__ inline uint32_t f32_key(float f) {  // ascending key of a float (total order)
   uint32_t b;
 #ifdef __CUDA_ARCH__
@@ -223,6 +230,13 @@ struct RowFilters {
   uint32_t n_filters = 0;
   const uint32_t* query_filter = nullptr;
   uint64_t n_rows_total = 0;
+};
+
+// What a batch ranks (sdb_corpus_order_*): the value of vector function fn per row (an sdb_metric id or an
+// sdb_vector_fn), ascending or descending.  KNN batches rank the corpus metric ascending (fn = -1).
+struct Ranking {
+  int fn = -1;
+  bool desc = false;
 };
 
 struct Comm;  // comm.cu: NCCL communicator attached to a context (nullptr = single shard)
@@ -319,6 +333,7 @@ struct Ticket {
   uint64_t* d_fin_rows = nullptr;
   double* d_fin_dist = nullptr;
   uint32_t* d_fin_count = nullptr;
+  Ranking rank;  // what the batch ranks (KNN: the corpus metric ascending)
   // SDB_TRACE=1: named timestamps of this batch on its stream, printed at wait time relative to the context's epoch
   std::vector<std::pair<const char*, cudaEvent_t>> trace;
 };
@@ -465,6 +480,29 @@ constexpr uint32_t COUNT_CAP_MAX = 16384;  // candidate entries per query of the
 inline bool count_ranked(const Corpus* c, uint32_t k) {
   return family(c) == Family::Count && k >= 1 && k <= 256 && c->screen != SDB_SCREEN_NONE_EXACT;
 }
+// The ranking of KNN itself, the corpus metric ascending: KnnTopK's DistanceEntry order and SortTopK's are both
+// Number::cmp and then scan position, so it takes the KNN path unchanged.
+inline bool knn_ranking(const Corpus* c, const Ranking& r) { return !r.desc && (r.fn < 0 || r.fn == (int)c->metric); }
+// vector::similarity::cosine descending on a COSINE corpus: the distance 1 - s is computed from the same s and does not
+// increase as s grows, so the Dot screens' candidate sets hold its top k; the re-rank keys s descending and cand_final
+// proves the result with the similarity's upper bound (DESIGN.md section 5, ORDER BY).
+inline bool cosine_desc(const Corpus* c, const Ranking& r) {
+  return r.desc && r.fn == SDB_FN_SIMILARITY_COSINE && c->metric == SDB_COSINE;
+}
+// The corpus metric descending where that needs no new screen:
+//  - HAMMING / JACCARD on the count path: it computes every row's value exactly, so the direction is a key transform
+//    of its per-range top-k and of the merge after it (count.cu), with nothing to prove;
+//  - PEARSON with its moments (Centred): the screens score cos(dx, +dq) instead of cos(dx, -dq), largest for the
+//    largest pearson, and cand_final mirrors the proof (DESIGN.md section 5, ORDER BY).
+inline bool metric_desc(const Corpus* c, const Ranking& r) {
+  const Family f = family(c);
+  return r.desc && r.fn == (int)c->metric && (f == Family::Count || f == Family::Centred);
+}
+// the rankings the screens (and the count path) serve; every other one is ranked by the exact kernel alone.  Those
+// that are descending are cosine_desc and metric_desc, and every stage takes Ranking::desc as it is.
+inline bool screened_ranking(const Corpus* c, const Ranking& r) {
+  return knn_ranking(c, r) || cosine_desc(c, r) || metric_desc(c, r);
+}
 
 // ---- the brute-force driver (api.cu), as its entry points and the sharded search (comm.cu) use it ------------------
 // one batch as a caller hands it over: queries and row filters on the host (host_in) or the device; outputs on the host
@@ -479,6 +517,7 @@ struct KnnCall {
   uint32_t* out_count = nullptr;
   bool host_out = false;
   const volatile int* cancel = nullptr;
+  Ranking rank;  // sdb_corpus_order_*: queries == nullptr for SDB_FN_MAGNITUDE, which takes no query
 };
 // a free ticket slot, or nullptr with the "too many batches in flight" error (the caller returns SDB_EOVERFLOW)
 Ticket* claim_ticket(Corpus* c);
@@ -521,7 +560,9 @@ sdb_status screen_lp_pass(const Corpus* c, Scratch& s, const FiltArg& filt, uint
 // (which runs count_prep_queries for Count corpora) and cand_begin
 uint32_t count_ranges(const Corpus* c, uint32_t nq, uint32_t k);
 sdb_status count_prep_queries(const Corpus* c, Scratch& s, uint32_t nq, cudaStream_t st);
-sdb_status count_pass(const Corpus* c, Scratch& s, const FiltArg& filt, uint32_t nq, uint32_t k, cudaStream_t st);
+// desc: the k largest (value, -row) per range instead of the k smallest (metric_desc batches)
+sdb_status count_pass(const Corpus* c, Scratch& s, const FiltArg& filt, uint32_t nq, uint32_t k, cudaStream_t st,
+                      bool desc = false);
 // screen_tc.cu
 // mode 0: pass 0 (every score of the pass's tiles written to fixed slots), 1: threshold pass, 2: streaming pass with
 // in-kernel threshold refinement (histogram + refiner warp), 3: probe (chunk maxima of a few tiles, no candidates)
@@ -531,7 +572,9 @@ bool screen_tc_available();
 // candidates.cu
 // grows s to nq queries x cap candidates (a set that grows loses its contents)
 sdb_status scratch_for(const Corpus* c, Scratch& s, uint32_t nq, uint32_t cap);
-sdb_status prep_queries(const Corpus* c, Scratch& s, const double* d_queries, uint32_t nq, cudaStream_t st);
+// desc: PEARSON's screen copies of +dq / |dq| (a metric_desc batch) instead of -dq / |dq|
+sdb_status prep_queries(const Corpus* c, Scratch& s, const double* d_queries, uint32_t nq, cudaStream_t st,
+                        bool desc = false);
 // one query prepared into the fallback scratch (d_fb_*), independent of the batch scratch
 sdb_status prep_fallback_query(Corpus* c, const double* d_query, cudaStream_t st);
 // resets tau / counts / flags and derives, per query, the screen's error bound, the selection margin and the score range
@@ -556,15 +599,20 @@ sdb_status cand_filter_list(const Corpus* c, Scratch& s, const FiltArg& filt, ui
 sdb_status cand_add_specials(const Corpus* c, Scratch& s, const FiltArg& filt, uint32_t nq, cudaStream_t st);
 // direct regime (filtered): each query's list = the rows its filter passes that are neither skipped nor removed
 sdb_status cand_direct(const Corpus* c, Scratch& s, const FiltArg& filt, uint32_t nq, cudaStream_t st);
+// desc (the descending screened rankings): the re-rank keys its values descending (cosine_desc: it computes the
+// cosine similarity), and cand_final proves that order
 sdb_status cand_rerank(const Corpus* c, Scratch& s, const FiltArg& filt, uint32_t nq, cudaStream_t st,
-                       bool small_sets = false);
+                       bool small_sets = false, bool desc = false);
 sdb_status cand_final(const Corpus* c, Scratch& s, const FiltArg& filt, uint32_t nq, uint32_t k, uint64_t row_base,
-                      uint64_t* d_out_rows, double* d_out_dist, uint32_t* d_out_count, cudaStream_t st);
+                      uint64_t* d_out_rows, double* d_out_dist, uint32_t* d_out_count, cudaStream_t st,
+                      bool desc = false);
 // exact.cu: query vector / |q| / flags are passed explicitly (a batch scratch row or the fallback scratch).
 // filter: nullptr, or the query's bitmap (filter_words words): rows whose bit is clear are not ranked.
+// rank: the value ranked (any vector function) and its direction; the default is the corpus metric ascending (KNN).
 sdb_status exact_query(Corpus* c, const double* d_q64, const double* d_qmag, const uint32_t* d_qflags, uint32_t k,
                        uint64_t row_base, uint64_t* d_out_rows, double* d_out_dist, uint32_t* d_out_count,
-                       cudaStream_t st, const uint32_t* filter = nullptr, uint32_t filter_words = 0);
+                       cudaStream_t st, const uint32_t* filter = nullptr, uint32_t filter_words = 0,
+                       const Ranking& rank = Ranking());
 sdb_status exact_project(const Corpus* c, int fn, const double* d_q64, const double* d_qmag, const uint32_t* d_qflags,
                          double* d_vals, cudaStream_t st);
 // gen.cu

@@ -299,8 +299,7 @@ class VectorColumn:
         """One value per row of `vector::<fn>(row, query)` in the reference's f64 arithmetic (fnc/vector.rs): fn is a
         metric name ("EUCLIDEAN", "MANHATTAN", ... = vector::distance::*, "COSINE" = 1 - similarity, "PEARSON" =
         vector::similarity::pearson) or "SIMILARITY_COSINE" / "DOT" / "MAGNITUDE"."""
-        fn = fn.upper()
-        code = L.VECTOR_FN[fn] if fn in L.VECTOR_FN else L.METRIC[fn]
+        code = self._fn_code(fn)
         out = np.zeros(len(self), np.float64)
         q = None
         if query is not None:
@@ -309,6 +308,78 @@ class VectorColumn:
                 raise L.SdbError(L.SDB_EDIM, "The two vectors must be of the same dimension.")
         L.check(L.lib().sdb_corpus_project(self.h, _ptr(q) if q is not None else None, code, _ptr(out)))
         return out
+
+    @staticmethod
+    def _fn_code(fn):
+        """a project() function name, or its integer id as is (unknown ids reach the library, which refuses them)"""
+        if isinstance(fn, (int, np.integer)):
+            return int(fn)
+        fn = fn.upper()
+        return L.VECTOR_FN[fn] if fn in L.VECTOR_FN else L.METRIC[fn]
+
+    @staticmethod
+    def _order_code(order):
+        return int(order) if isinstance(order, (int, np.integer)) else L.ORDER[order.upper()]
+
+    def order_topk(self, queries, k, fn, order, filters=None, query_filter=None):
+        """`ORDER BY vector::<fn>(field, $q) ASC|DESC LIMIT k` (SortTopK over project()'s values): fn as in project(),
+        order "ASC" / "DESC".  queries (nq, dim) float64, or None for "MAGNITUDE" with nq = 1.  filters / query_filter
+        as in knn().  -> (rows u64 (nq,k), values f64 (nq,k), count u32 (nq,))"""
+        code = self._fn_code(fn)
+        if queries is None:
+            q = None
+            nq = 1
+        else:
+            q = np.ascontiguousarray(queries, np.float64)
+            if q.ndim == 1:
+                q = q[None, :]
+            if q.shape[1] != self.dim:  # check_same_dimension  fnc/util/math/vector.rs:23-32
+                raise L.SdbError(L.SDB_EDIM, "The two vectors must be of the same dimension.")
+            nq = q.shape[0]
+        rows = np.zeros((nq, max(k, 1)), np.uint64)
+        vals = np.zeros((nq, max(k, 1)), np.float64)
+        cnt = np.zeros(nq, np.uint32)
+        f, qf = (None, None) if filters is None else _filter_args(filters, query_filter, nq, len(self))
+        L.check(L.lib().sdb_corpus_order_topk(self.h, None if q is None else _ptr(q), nq, code, self._order_code(order),
+                                              int(k), None if f is None else _ptr(f), 0 if f is None else f.shape[0],
+                                              None if qf is None else _ptr(qf), _ptr(rows), _ptr(vals), _ptr(cnt)))
+        return rows[:, :k], vals[:, :k], cnt
+
+    def order_topk_device(self, d_queries, nq, k, fn, order, row_base, d_out_rows, d_out_values, d_out_count,
+                          d_filters=None, n_filters=0, query_filter=None):
+        """order_topk on device pointers (ints; d_queries 0 for MAGNITUDE); query_filter is a host array (or None)"""
+        qf = _query_filter(query_filter, nq)
+        L.check(L.lib().sdb_corpus_order_topk_device(self.h, C.c_void_p(d_queries or None), int(nq),
+                                                     self._fn_code(fn), self._order_code(order), int(k),
+                                                     C.c_void_p(d_filters or None), int(n_filters),
+                                                     None if qf is None else _ptr(qf), int(row_base),
+                                                     C.c_void_p(d_out_rows), C.c_void_p(d_out_values),
+                                                     C.c_void_p(d_out_count)))
+
+    def order_submit_host(self, h_queries, nq, k, fn, order, h_out_rows, h_out_values, h_out_count, h_filters=None,
+                          n_filters=0, query_filter=None):
+        """asynchronous order_topk on raw host pointers (ints, valid until wait), like submit_host_filtered"""
+        qf = _query_filter(query_filter, nq)
+        t = C.c_uint32()
+        L.check(L.lib().sdb_corpus_order_submit(self.h, C.c_void_p(h_queries or None), int(nq), self._fn_code(fn),
+                                                self._order_code(order), int(k), C.c_void_p(h_filters or None),
+                                                int(n_filters), None if qf is None else _ptr(qf),
+                                                C.c_void_p(h_out_rows), C.c_void_p(h_out_values),
+                                                C.c_void_p(h_out_count), C.byref(t)))
+        return t.value
+
+    def order_submit_device(self, d_queries, nq, k, fn, order, row_base, d_out_rows, d_out_values, d_out_count,
+                            d_filters=None, n_filters=0, query_filter=None):
+        """asynchronous order_topk_device (device pointers valid until wait)"""
+        qf = _query_filter(query_filter, nq)
+        t = C.c_uint32()
+        L.check(L.lib().sdb_corpus_order_submit_device(self.h, C.c_void_p(d_queries or None), int(nq),
+                                                       self._fn_code(fn), self._order_code(order), int(k),
+                                                       C.c_void_p(d_filters or None), int(n_filters),
+                                                       None if qf is None else _ptr(qf), int(row_base),
+                                                       C.c_void_p(d_out_rows), C.c_void_p(d_out_values),
+                                                       C.c_void_p(d_out_count), C.byref(t)))
+        return t.value
 
     def stats(self):
         s = L.KnnStats()

@@ -9,6 +9,9 @@ meaning and error behaviour, on top of the same C ABI:
       .name() / .attrs()                              knn_topk.rs:133-144   (EXPLAIN output)
   KnnScan(index, vector, k, ef, table_name, ...)      core/exec/operators/scan/knn.rs:68-118,135-347 (HNSW-backed)
   KnnContext: record id -> distance hand-back         core/exec/function/index.rs:289-314
+  SortTopK(input, field, fn, query_vector, limit, direction)   core/exec/operators/sort/topk.rs:100-118
+      Compute(vector::<fn>(field, $q)) + SortTopK with that single ORDER BY key (planner/select.rs:782-789)
+      .execute()  -> records best first, each with the computed value under `alias`
 
 Records are dicts with an "id"; `input` is any iterable yielding them in scan (record-key) order, i.e.
 what TableScan yields.
@@ -225,6 +228,73 @@ class KnnTopK:
             if self.knn_context is not None and isinstance(rec, dict) and "id" in rec:
                 self.knn_context.insert(rec["id"], float(dist[0, j]))
             out.append(rec)
+        return out
+
+
+# vector functions SortTopK ranks on the GPU: SurrealQL name -> (sdb function name, the metric of the staged column).
+# The column's metric only picks its screen copies: vector::similarity::cosine DESC is screened on a COSINE column.
+VECTOR_FUNCTIONS = {
+    "vector::similarity::cosine": ("SIMILARITY_COSINE", "COSINE"),
+    "vector::similarity::pearson": ("PEARSON", "PEARSON"),
+    "vector::similarity::jaccard": ("JACCARD", "JACCARD"),
+    "vector::dot": ("DOT", "COSINE"),
+    "vector::magnitude": ("MAGNITUDE", "COSINE"),
+    "vector::distance::euclidean": ("EUCLIDEAN", "EUCLIDEAN"),
+    "vector::distance::manhattan": ("MANHATTAN", "MANHATTAN"),
+    "vector::distance::chebyshev": ("CHEBYSHEV", "CHEBYSHEV"),
+    "vector::distance::hamming": ("HAMMING", "HAMMING"),
+}  # (vector::distance::minkowski takes its order as a third argument; a cached column holds one: left to the reference)
+
+
+class SortTopK(KnnTopK):
+    """`SELECT .., vector::<fn>(field, $q) AS alias FROM .. ORDER BY alias ASC|DESC LIMIT k`: the reference plans
+    Compute + SortTopK (a heap over Value::compare of the key, earlier rows winning ties) when start + limit <= 1000;
+    this operator ranks the staged column with sdb_corpus_order_topk instead, cached like KnnTopK's.  fn is one of
+    VECTOR_FUNCTIONS (vector::magnitude takes no query: pass query_vector=None and dim).  A Filter input ranks the
+    source's column with the predicate's row bitmap.  The reference raises an error when a ranked row has no vector of
+    the query's dimension; this operator does not rank such a statement (SdbError, SDB_EINVAL), the shim leaves it to
+    the reference."""
+
+    def __init__(self, input, field, fn, query_vector, limit, direction="ASC", alias=None, order_expr=None,
+                 dim=None, ctx=None):
+        if fn not in VECTOR_FUNCTIONS:
+            from . import _lib as L
+            raise L.SdbError(L.SDB_EINVAL, f"SortTopK: {fn} is not ranked on the GPU")
+        self.fn, self.direction = fn, direction.upper()
+        qv = query_vector if query_vector is not None else [0.0] * int(dim)
+        super().__init__(input, field, qv, limit, VECTOR_FUNCTIONS[fn][1], ctx=ctx)
+        self.limit, self.alias = int(limit), alias
+        self.order_expr = order_expr or (f"{fn}({field})" if query_vector is None else f"{fn}({field}, $q)")
+        self._has_query = query_vector is not None
+
+    def name(self):
+        return "SortTopK"
+
+    def attrs(self):  # topk.rs:100-118
+        return [("order_by", f"{self.order_expr} {self.direction}"), ("limit", str(self.limit))]
+
+    def execute(self):
+        from . import _lib as L
+        filtered = isinstance(self.input, Filter)
+        if self._column is None:
+            self._column = self._source_column(self.input.input) if filtered else self._stage()
+        if self._column is None or self.limit == 0:
+            return []
+        dim = len(self.query_vector)
+        passes = [bool(self.input.predicate(rec)) for rec in self._records] if filtered else None
+        for j, rec in enumerate(self._records):
+            vec = extract_vector(rec, self.field)
+            if (passes is None or passes[j]) and (vec is None or len(vec) != dim):
+                raise L.SdbError(L.SDB_EINVAL, "SortTopK: a ranked row has no vector of the query's dimension "
+                                               "(the reference raises an error; not ranked on the GPU)")
+        q = np.asarray([self.query_vector], np.float64) if self._has_query else None
+        filt = pack_row_filter(passes) if filtered else None
+        rows, vals, cnt = self._column.order_topk(q, self.limit, VECTOR_FUNCTIONS[self.fn][0], self.direction,
+                                                  filters=filt)
+        out = []
+        for j in range(int(cnt[0])):
+            rec = self._records[int(rows[0, j])]
+            out.append(dict(rec, **{self.alias: float(vals[0, j])}) if self.alias else rec)
         return out
 
 
