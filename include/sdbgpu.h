@@ -199,6 +199,17 @@ sdb_status sdb_debug_screen_batch_filtered(sdb_corpus*, const double* queries, u
                                            uint16_t* out_qbf16, uint32_t* out_a, uint32_t* out_b, uint32_t* out_rr,
                                            const uint32_t* filters, uint32_t n_filters, const uint32_t* query_filter,
                                            int mask_hits);
+/* sdb_debug_screen_batch_ranked: sdb_debug_screen_batch_filtered for the ranking (fn, order) of sdb_corpus_order_topk
+ * instead of KNN's; SDB_EINVAL for a ranking the screens do not serve on the corpus.  SDB_FN_DOT on a COSINE or
+ * EUCLIDEAN corpus (TC_BF16, or SIMT_F32 on F32 rows): the scores are the dots of the rows with the query (DESC) or
+ * with its negation (ASC), out_qbf16 is the bf16 copy of that query, bscale is 1 and beps bounds the score's
+ * distance from the exact dot; the exact re-rank still ranks the query itself. */
+sdb_status sdb_debug_screen_batch_ranked(sdb_corpus*, const double* queries, uint32_t nq, uint32_t k,
+                                         sdb_screen screen, int streaming, uint32_t cand_cap, int score_all,
+                                         float* out_qf, double* out_qmag, uint32_t* out_qu, int8_t* out_q8,
+                                         uint16_t* out_qbf16, uint32_t* out_a, uint32_t* out_b, uint32_t* out_rr,
+                                         const uint32_t* filters, uint32_t n_filters, const uint32_t* query_filter,
+                                         int mask_hits, int fn, int order);
 /* Test-only: device and pinned buffers the library holds right now, process-wide (count and bytes).  Buffers handed to
  * the caller (sdb_pinned_alloc, sdb_graph_expand_device) are not counted.  Either output may be NULL. */
 void sdb_debug_live_allocations(uint64_t* count, uint64_t* bytes);
@@ -397,8 +408,11 @@ sdb_status sdb_corpus_project(sdb_corpus*, const double* query, int fn, double* 
  * Routing: fn = the corpus metric with SDB_ORDER_ASC is the KNN ranking and takes the KNN path unchanged (the results
  * equal sdb_knn_bruteforce[_filtered] byte for byte); SDB_FN_SIMILARITY_COSINE DESC on a COSINE corpus is screened
  * like KNN (k <= 256) and proven with the similarity's bound, vector::similarity::pearson DESC on a PEARSON corpus
- * on the same screens with the query's centred copy un-negated (k <= 256), HAMMING / JACCARD DESC on their own corpus
- * on the count path (k <= 256, exact counts); every other (fn, order) is ranked by the exact kernel.
+ * on the same screens with the query's centred copy un-negated (k <= 256), SDB_FN_DOT in either direction on a COSINE
+ * or EUCLIDEAN corpus on the bf16 tensor-core screen (maximum / minimum inner product, k <= 256: the screens score the
+ * dot with q for DESC and with -q for ASC, never on the int8 copy, with the F32 stream as the ladder's last rung),
+ * HAMMING / JACCARD DESC on their own corpus on the count path (k <= 256, exact counts); every other (fn, order) is
+ * ranked by the exact kernel.
  * Refusals: an unknown fn or order, or nq > 0 with NULL queries for a function that takes a query: SDB_EINVAL.
  * Tickets share the corpus' four slots with KNN tickets; sdb_knn_wait completes them; cancellation and
  * sdb_knn_last_stats work as for KNN.  Row-sharded columns are not served. */

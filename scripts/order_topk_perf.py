@@ -5,11 +5,15 @@
     on the same column and batch;
   * vector::similarity::pearson DESC on a PEARSON column (the exact kernel) against the exact kernel's KNN ranking
     (sdb_knn_bruteforce with NONE_EXACT) on the same column;
+  * vector::dot DESC (maximum inner product, the bf16 screen + the dot proof) on the COSINE column and on a EUCLIDEAN
+    one, each against sdb_knn_bruteforce on the same column and against the exact kernel (NONE_EXACT, --exact-max
+    queries), with the survivors per query and the repaired / fallback counts;
   * the route without this call: sdb_corpus_project per query (every row's value copied to the host) and a host top-k
     (numpy argpartition + sort), timed on --project-max queries and scaled.
 
   python scripts/order_topk_perf.py [--n 10000000 --dim 768 --k 10 --batch 1024 --reps 3 --exact-max 4
-                                     --project-max 4 --pearson-n 10000000 --out order_topk_perf.json]
+                                     --project-max 4 --pearson-n 10000000 --dot-euclid-n 10000000
+                                     --out order_topk_perf.json]
 
 The rows are the library's synthetic rows (append_synthetic), the queries gen_f32 values of another seed.  Each rate
 is the batch over the median of --reps synchronous calls after one warm-up call.  10 queries of the batch are checked
@@ -66,6 +70,7 @@ def main():
     ap.add_argument("--exact-max", type=int, default=4)
     ap.add_argument("--project-max", type=int, default=4)
     ap.add_argument("--pearson-n", type=int, default=10_000_000)
+    ap.add_argument("--dot-euclid-n", type=int, default=10_000_000)
     ap.add_argument("--out", default="")
     a = ap.parse_args()
     import torch
@@ -85,6 +90,25 @@ def main():
         lines.append(line)
 
     summary = {"config": f"{a.n}x{a.dim} F32 synthetic", "k": k, "batch": B, "gpu": gpu_info()}
+
+    def dot_rows(col, column, t_knn):
+        """vector::dot DESC on col: the screened batch, the exact kernel on a few queries, parity on 10"""
+        t_dot, sp_dot = timed(lambda: col.order_topk(Q, k, "DOT", "DESC"), a.reps)
+        st = col.stats()
+        Be = min(B, a.exact_max)
+        col.set_screen("NONE_EXACT")
+        t_ex, sp_ex = timed(lambda: col.order_topk(Q[:Be], k, "DOT", "DESC"), a.reps)
+        ref = col.order_topk(Q[:10], k, "DOT", "DESC")
+        col.set_screen("AUTO")
+        got = col.order_topk(Q[:10], k, "DOT", "DESC")
+        summary[f"dot_desc_{column.lower()}_parity_10_vs_exact"] = all(u.tobytes() == v.tobytes()
+                                                                       for u, v in zip(got, ref))
+        emit({"fn": "DOT", "order": "DESC", "column": column, "batch": B, "order_qps": B / t_dot,
+              "knn_qps": B / t_knn, "order_over_knn_time": t_dot / t_knn, "order_spread_ms": sp_dot,
+              "exact_timed_queries": Be, "exact_qps": Be / t_ex, "exact_spread_ms": sp_ex,
+              "screen_used": st["screen_used"], "screen_ms": st["screen_ms"], "total_ms": st["total_ms"],
+              "survivors_per_query": st["n_survivors"] / B, "largest_candidate_set": st["n_candidates"],
+              "n_fallback": st["n_fallback"], "n_repaired": st["n_repaired"]})
 
     col = VectorColumn(ctx, a.dim, "COSINE", "F32", capacity=a.n)
     col.append_synthetic(seed=0x5DB0, first_row=0, n=a.n)
@@ -108,7 +132,18 @@ def main():
     ref = col.order_topk(Qp, k, "SIMILARITY_COSINE", "DESC")
     col.set_screen("AUTO")
     summary["cosine_desc_parity_10_vs_exact"] = all(u.tobytes() == v.tobytes() for u, v in zip(got, ref))
+    dot_rows(col, "COSINE", t_knn)
     col.close()
+    del col
+    torch.cuda.empty_cache()
+
+    if a.dot_euclid_n:
+        col = VectorColumn(ctx, a.dim, "EUCLIDEAN", "F32", capacity=a.dot_euclid_n)
+        col.append_synthetic(seed=0x5DB0, first_row=0, n=a.dot_euclid_n)
+        col.finalize()
+        t_knn, _ = timed(lambda: col.knn(Q, k), a.reps)
+        dot_rows(col, "EUCLIDEAN", t_knn)
+        col.close()
     del col
     torch.cuda.empty_cache()
 

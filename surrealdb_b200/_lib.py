@@ -27,7 +27,7 @@ ORDER = {"ASC": 0, "DESC": 1}
 ABI_SYMBOLS = [
     "sdb_ctx_create", "sdb_ctx_destroy", "sdb_last_error", "sdb_version", "sdb_pinned_alloc", "sdb_pinned_free",
     "sdb_ctx_cancel", "sdb_ctx_cancel_reset", "sdb_debug_schedule", "sdb_debug_corpus_state", "sdb_debug_screen_batch",
-    "sdb_debug_screen_batch_filtered", "sdb_debug_live_allocations",
+    "sdb_debug_screen_batch_filtered", "sdb_debug_screen_batch_ranked", "sdb_debug_live_allocations",
     "sdb_ctx_kernel_launches", "sdb_ctx_stream", "sdb_corpus_create", "sdb_corpus_destroy", "sdb_corpus_append",
     "sdb_corpus_append_device", "sdb_corpus_append_synthetic", "sdb_corpus_set_skip", "sdb_corpus_remove", "sdb_corpus_finalize",
     "sdb_corpus_rows", "sdb_corpus_read_rows", "sdb_corpus_set_minkowski_order", "sdb_corpus_set_screen", "sdb_corpus_set_schedule", "sdb_corpus_set_exact", "sdb_knn_bruteforce", "sdb_knn_bruteforce_device",
@@ -93,6 +93,8 @@ def lib():
     L.sdb_debug_screen_batch.argtypes = [vp, vp, u32, u32, i32, i32, u32, i32, vp, vp, vp, vp, vp, vp, vp, vp]
     L.sdb_debug_screen_batch_filtered.argtypes = [vp, vp, u32, u32, i32, i32, u32, i32, vp, vp, vp, vp, vp, vp, vp, vp,
                                                   vp, u32, vp, i32]
+    L.sdb_debug_screen_batch_ranked.argtypes = [vp, vp, u32, u32, i32, i32, u32, i32, vp, vp, vp, vp, vp, vp, vp, vp,
+                                                vp, u32, vp, i32, i32, i32]
     L.sdb_debug_live_allocations.argtypes = [vp, vp]
     L.sdb_debug_live_allocations.restype = None
     L.sdb_corpus_create.argtypes = [vp, u32, i32, i32, u64, C.POINTER(vp)]

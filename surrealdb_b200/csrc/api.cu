@@ -110,6 +110,8 @@ static std::vector<Rung> build_rungs(const Corpus* c, sdb_screen screen, uint32_
     scr = !screen_tc_available() ? SDB_SCREEN_SIMT_F32
                                  : (int8_ok && c->max_rel_qerr <= 0.02f ? SDB_SCREEN_TC_INT8 : SDB_SCREEN_TC_BF16);
   if (scr == SDB_SCREEN_TC_INT8 && !int8_ok) scr = SDB_SCREEN_TC_BF16;
+  // the int8 copy holds x / |x| and its integer threshold compare takes no per-row scale: dot batches start on bf16
+  if (scr == SDB_SCREEN_TC_INT8 && score_kind(c, rank) == Score::Dot) scr = SDB_SCREEN_TC_BF16;
   // (Lp corpora hold no bf16 copy: the f32 Lp screen, screen_lp.cu, is their only screen, for f32 and f64 rows)
   if (scr == SDB_SCREEN_TC_BF16 && (!screen_tc_available() || !c->d_bf16)) scr = SDB_SCREEN_SIMT_F32;
   // the SIMT screen streams f32 rows: an f64 Dot corpus is screened on the tensor cores or not at all, and so is a
@@ -298,13 +300,14 @@ static sdb_status copy_flags(const Scratch& s, const Run& r, cudaStream_t st) {
 static sdb_status enqueue_direct(Corpus* c, Ticket& t, const Run& r) {
   cudaStream_t st = t.stream;
   Scratch& s = c->sets[t.set];
+  const Score sc = score_kind(c, t.rank);
   SDB_TRY(scratch_for(c, s, r.nq, DIRECT_MAX_ROWS));
-  SDB_TRY(prep_queries(c, s, r.d_queries, r.nq, st));
-  SDB_TRY(cand_begin(c, s, r.nq, SDB_SCREEN_NONE_EXACT, st));
+  SDB_TRY(prep_queries(c, s, r.d_queries, r.nq, st, sc, t.rank.desc));
+  SDB_TRY(cand_begin(c, s, r.nq, SDB_SCREEN_NONE_EXACT, st, sc));
   SDB_TRY(cand_direct(c, s, r.filt, r.nq, st));
-  SDB_TRY(cand_rerank(c, s, r.filt, r.nq, st, false, t.rank.desc));
+  SDB_TRY(cand_rerank(c, s, r.filt, r.nq, st, false, t.rank.desc, sc));
   SDB_TRY(cand_final(c, s, r.filt, r.nq, t.k, t.row_base, r.d_out_rows, r.d_out_dist, r.d_out_count, st,
-                     t.rank.desc));
+                     t.rank.desc, sc));
   return copy_flags(s, r, st);
 }
 
@@ -359,9 +362,10 @@ static sdb_status enqueue_counted(Corpus* c, Ticket& t, const Run& r, Enqueued* 
   e->n_passes = 1;
   SDB_CUDA(cudaEventRecord(t.ev_begin, st));
   trace_mark(ctx, t, "begin", st);
+  const Score sc = score_kind(c, t.rank);
   SDB_TRY(scratch_for(c, s, nq, std::max(4096u, count_ranges(c, nq, k) * k)));
-  SDB_TRY(prep_queries(c, s, r.d_queries, nq, st));
-  SDB_TRY(cand_begin(c, s, nq, SDB_SCREEN_NONE_EXACT, st));
+  SDB_TRY(prep_queries(c, s, r.d_queries, nq, st, sc, t.rank.desc));
+  SDB_TRY(cand_begin(c, s, nq, SDB_SCREEN_NONE_EXACT, st, sc));
   if (c->last_main && c->last_main != t.ev_main) SDB_CUDA(cudaStreamWaitEvent(st, c->last_main, 0));
   SDB_CUDA(cudaEventRecord(t.ev_screen0, st));
   if ((t.cancel && *t.cancel) || ctx_cancelled(ctx)) {
@@ -374,7 +378,8 @@ static sdb_status enqueue_counted(Corpus* c, Ticket& t, const Run& r, Enqueued* 
   c->last_main = t.ev_main;
   SDB_CUDA(cudaEventRecord(t.ev_screen1, st));
   trace_mark(ctx, t, "counted", st);
-  SDB_TRY(cand_final(c, s, r.filt, nq, k, t.row_base, r.d_out_rows, r.d_out_dist, r.d_out_count, st, t.rank.desc));
+  SDB_TRY(cand_final(c, s, r.filt, nq, k, t.row_base, r.d_out_rows, r.d_out_dist, r.d_out_count, st, t.rank.desc,
+                     sc));
   SDB_TRY(copy_flags(s, r, st));
   SDB_CUDA(cudaEventRecord(t.ev_end, st));
   trace_mark(ctx, t, "end", st);
@@ -386,6 +391,7 @@ static sdb_status enqueue_screened(Corpus* c, Ticket& t, const Run& r, Enqueued*
   cudaStream_t st = t.stream;
   Scratch& s = c->sets[t.set];
   const uint32_t nq = r.nq, k = t.k;
+  const Score sc = score_kind(c, t.rank);
   // HAMMING: AUTO ranks a batch of one query with the exact kernel, which streams the rows once at the higher rate
   // (DESIGN.md section 5); an explicit screen request still counts it.  JACCARD's exact kernel is O(D^2) per row: the
   // count path takes a single query too
@@ -400,7 +406,7 @@ static sdb_status enqueue_screened(Corpus* c, Ticket& t, const Run& r, Enqueued*
   if (rungs.empty()) {  // exact-only: the exact kernel needs the prepared queries (f64 copy, |q|, flags)
     e->screen = SDB_SCREEN_NONE_EXACT;
     SDB_TRY(scratch_for(c, s, nq, 4096));
-    SDB_TRY(prep_queries(c, s, r.d_queries, nq, st));
+    SDB_TRY(prep_queries(c, s, r.d_queries, nq, st, sc, t.rank.desc));
     SDB_CUDA(cudaEventRecord(t.ev_screen0, st));
     SDB_CUDA(cudaEventRecord(t.ev_screen1, st));
     SDB_CUDA(cudaMemsetAsync(r.d_out_count, 0, sizeof(uint32_t) * nq, st));
@@ -418,8 +424,8 @@ static sdb_status enqueue_screened(Corpus* c, Ticket& t, const Run& r, Enqueued*
   const bool int8 = rs == SDB_SCREEN_TC_INT8;
   SDB_TRY(scratch_for(c, s, nq, rg.cap));
   const uint32_t cap = s.sc_cap;
-  SDB_TRY(prep_queries(c, s, r.d_queries, nq, st, t.rank.desc));
-  SDB_TRY(cand_begin(c, s, nq, (int)rs, st));
+  SDB_TRY(prep_queries(c, s, r.d_queries, nq, st, sc, t.rank.desc));
+  SDB_TRY(cand_begin(c, s, nq, (int)rs, st, sc));
   // Screens are persistent one-CTA-per-SM kernels: two of them in flight on different streams would split the SMs,
   // run in two waves and starve the refiners of the CTAs that are not resident yet.  So the screen of this batch waits
   // for the end of the previous batch's screen -- only the TAIL of the previous batch overlaps with it.
@@ -430,17 +436,17 @@ static sdb_status enqueue_screened(Corpus* c, Ticket& t, const Run& r, Enqueued*
     PassDesc p0, pm;
     build_stream_passes(c->n, cap, k, &p0, &pm);
     if (p0.count && !pm.count) {  // the whole corpus fits the lists: score everything once
-      SDB_TRY(screen_tc_pass(c, s, r.filt, nq, k, p0, int8, 0, st));
+      SDB_TRY(screen_tc_pass(c, s, r.filt, nq, k, p0, int8, 0, st, sc));
       SDB_CUDA(cudaEventRecord(t.ev_main, st));
       c->last_main = t.ev_main;
       if (r.tap) SDB_TRY(tap_gathered(s, r.tap, nq, 0u, st));
       SDB_TRY(cand_select(c, s, nq, k, int8, 0u, false, st));
       e->n_passes++;
     } else if (pm.count) {
-      SDB_TRY(screen_tc_pass(c, s, r.filt, nq, k, p0, int8, 3, st));  // probe: chunk maxima of a few tiles
+      SDB_TRY(screen_tc_pass(c, s, r.filt, nq, k, p0, int8, 3, st, sc));  // probe: chunk maxima of a few tiles
       SDB_TRY(cand_seed_from_probe(c, s, nq, k, p0.count, st));       // thresholds + histogram geometry
       trace_mark(ctx, t, "seeded", st);
-      SDB_TRY(screen_tc_pass(c, s, r.filt, nq, k, pm, int8, 2, st));  // the streaming launch over every tile
+      SDB_TRY(screen_tc_pass(c, s, r.filt, nq, k, pm, int8, 2, st, sc));  // the streaming launch over every tile
       trace_mark(ctx, t, "main_end", st);
       SDB_CUDA(cudaEventRecord(t.ev_main, st));
       c->last_main = t.ev_main;
@@ -457,9 +463,9 @@ static sdb_status enqueue_screened(Corpus* c, Ticket& t, const Run& r, Enqueued*
         set_error("query cancelled");
         return SDB_ECANCELLED;
       }
-      if (tc) SDB_TRY(screen_tc_pass(c, s, r.filt, nq, k, p, int8, first_pass ? 0 : 1, st));
+      if (tc) SDB_TRY(screen_tc_pass(c, s, r.filt, nq, k, p, int8, first_pass ? 0 : 1, st, sc));
       else if (family(c) == Family::Lp) SDB_TRY(screen_lp_pass(c, s, r.filt, nq, p, st));
-      else SDB_TRY(screen_simt_pass(c, s, r.filt, nq, p, st));
+      else SDB_TRY(screen_simt_pass(c, s, r.filt, nq, p, st, sc));
       if (r.tap) SDB_TRY(tap_gathered(s, r.tap, nq, tc ? s.last_slots : 0u, st));
       SDB_TRY(cand_select(c, s, nq, k, int8, tc ? s.last_slots : 0u, false, st));
       first_pass = false;
@@ -475,16 +481,17 @@ static sdb_status enqueue_screened(Corpus* c, Ticket& t, const Run& r, Enqueued*
   static const bool no_refine = getenv("SDB_NO_REFINE") != nullptr;
   bool refined = false;
   if (tc && c->exact && !no_refine) {
-    SDB_TRY(cand_refine(c, s, nq, st));
+    SDB_TRY(cand_refine(c, s, nq, st, sc));
     if (r.tap) SDB_TRY(tap_list(s, nq, &r.tap->list_r, nullptr, st));
     SDB_TRY(cand_select(c, s, nq, k, false, 0u, false, st, 1));
     refined = true;
     trace_mark(ctx, t, "refined", st);
   }
   if (r.filt.bits) SDB_TRY(cand_add_specials(c, s, r.filt, nq, st));  // each query re-ranks its passing special rows
-  SDB_TRY(cand_rerank(c, s, r.filt, nq, st, refined, t.rank.desc));
+  SDB_TRY(cand_rerank(c, s, r.filt, nq, st, refined, t.rank.desc, sc));
   trace_mark(ctx, t, "reranked", st);
-  SDB_TRY(cand_final(c, s, r.filt, nq, k, t.row_base, r.d_out_rows, r.d_out_dist, r.d_out_count, st, t.rank.desc));
+  SDB_TRY(cand_final(c, s, r.filt, nq, k, t.row_base, r.d_out_rows, r.d_out_dist, r.d_out_count, st, t.rank.desc,
+                     sc));
   trace_mark(ctx, t, "final", st);
   SDB_TRY(copy_flags(s, r, st));
   SDB_CUDA(cudaEventRecord(t.ev_end, st));
@@ -524,6 +531,12 @@ static sdb_status finish_local(Corpus* c, Ticket& t, uint32_t* n_fallback, bool*
   *repaired = false;
   *n_fallback = 0;
   SDB_CUDA(cudaEventSynchronize(t.ev_end));
+  // vector::dot batches were ranked by the exact kernel, which reports a cancel raised while a batch is in flight (it
+  // polls before every query); on the screens they still report it, here
+  if (dot_ranking(c, t.rank) && nq && k && ((t.cancel && *t.cancel) || ctx_cancelled(ctx))) {
+    set_error("query cancelled");
+    return SDB_ECANCELLED;
+  }
   if (t.screen != SDB_SCREEN_NONE_EXACT && c->exact) {
     while (t.rung + 1 < t.n_batch_rungs) {  // many failures: the whole batch moves up one rung (and stays there)
       uint32_t n_fail = 0;
@@ -541,6 +554,7 @@ static sdb_status finish_local(Corpus* c, Ticket& t, uint32_t* n_fallback, bool*
     build_rungs(c, c->screen, k, nq, t.rank, &first);
     c->rung_scr = first;
     c->rung_k = k;
+    c->rung_score = (int)score_kind(c, t.rank);
     c->rung = t.rung;
   }
   // ---- what the batch's rung could not prove ----
@@ -752,7 +766,10 @@ static sdb_status submit_locked(Corpus* c, Ticket* t, const double* d_queries, u
   t->n_repaired = 0;
   sdb_screen first, first_scr;
   const std::vector<Rung> rungs = build_rungs(c, c->screen, k, nq, rank, &first);
-  t->rung = (c->rung_scr == first && c->rung_k == k && c->rung < n_batch_rungs(rungs)) ? c->rung : 0;
+  t->rung = (c->rung_scr == first && c->rung_k == k && c->rung_score == (int)score_kind(c, rank) &&
+             c->rung < n_batch_rungs(rungs))
+                ? c->rung
+                : 0;
   t->n_batch_rungs = n_batch_rungs(rungs);
   // the ladder of its screened queries, which a mixed batch screens on their own (one Lp query has none, build_rungs)
   const uint32_t n_scr = t->n_direct < nq ? nq - t->n_direct : nq;
@@ -1605,12 +1622,12 @@ sdb_status sdb_debug_screen_batch(sdb_corpus* c, const double* queries, uint32_t
                                          out_qu, out_q8, out_qbf16, out_a, out_b, out_rr, nullptr, 0, nullptr, -1);
 }
 
-sdb_status sdb_debug_screen_batch_filtered(sdb_corpus* c, const double* queries, uint32_t nq, uint32_t k,
-                                           sdb_screen screen, int streaming, uint32_t cand_cap, int score_all,
-                                           float* out_qf, double* out_qmag, uint32_t* out_qu, int8_t* out_q8,
-                                           uint16_t* out_qbf16, uint32_t* out_a, uint32_t* out_b, uint32_t* out_rr,
-                                           const uint32_t* filters, uint32_t n_filters, const uint32_t* query_filter,
-                                           int mask_hits) {
+// sdb_debug_screen_batch_filtered with the ranking `rank` (sdb_debug_screen_batch_ranked; the others rank KNN's)
+static sdb_status debug_screen_batch(sdb_corpus* c, const double* queries, uint32_t nq, uint32_t k, sdb_screen screen,
+                                     int streaming, uint32_t cand_cap, int score_all, float* out_qf, double* out_qmag,
+                                     uint32_t* out_qu, int8_t* out_q8, uint16_t* out_qbf16, uint32_t* out_a,
+                                     uint32_t* out_b, uint32_t* out_rr, const uint32_t* filters, uint32_t n_filters,
+                                     const uint32_t* query_filter, int mask_hits, const Ranking& rank) {
   const bool tc = screen == SDB_SCREEN_TC_INT8 || screen == SDB_SCREEN_TC_BF16;
   if (!c || !queries || !nq || !k || k > 256 || cand_cap < 4096 || (!tc && screen != SDB_SCREEN_SIMT_F32) ||
       mask_hits < -1 || mask_hits > 1) {
@@ -1653,7 +1670,8 @@ sdb_status sdb_debug_screen_batch_filtered(sdb_corpus* c, const double* queries,
   t->filt = FiltArg();
   t->n_direct = 0;
   t->permuted = false;
-  t->rank = Ranking();
+  t->rank = rank;
+  const Score sc = score_kind(c, rank);
   if (filters) {
     const uint32_t* bits = nullptr;
     std::vector<uint64_t> rows_per_filter;
@@ -1683,11 +1701,11 @@ sdb_status sdb_debug_screen_batch_filtered(sdb_corpus* c, const double* queries,
     SDB_CUDA(cudaMemcpyAsync(d_q, queries, sizeof(double) * (size_t)nq * c->dim, cudaMemcpyHostToDevice, st));
     if (score_all) {  // one pass-0 launch over every tile (SIMT: tau stays -inf), nothing selected
       const PassDesc all{1u, 0u, (uint32_t)(n_pad / TILE_ROWS), 0u};
-      SDB_TRY(prep_queries(c, s, d_q, nq, st));
-      SDB_TRY(cand_begin(c, s, nq, (int)screen, st));
-      SDB_TRY(tc                ? screen_tc_pass(c, s, t->filt, nq, k, all, int8, 0, st)
+      SDB_TRY(prep_queries(c, s, d_q, nq, st, sc, rank.desc));
+      SDB_TRY(cand_begin(c, s, nq, (int)screen, st, sc));
+      SDB_TRY(tc                ? screen_tc_pass(c, s, t->filt, nq, k, all, int8, 0, st, sc)
               : f == Family::Lp ? screen_lp_pass(c, s, t->filt, nq, all, st)
-                                : screen_simt_pass(c, s, t->filt, nq, all, st));
+                                : screen_simt_pass(c, s, t->filt, nq, all, st, sc));
       SDB_TRY(tap_list(s, nq, &tap.list_a, &tap.cnt_a, st));
       tap.gathered = tap.cnt_a;
       return SDB_OK;
@@ -1783,6 +1801,36 @@ sdb_status sdb_debug_screen_batch_filtered(sdb_corpus* c, const double* queries,
     }
   }
   return rc;
+}
+
+sdb_status sdb_debug_screen_batch_filtered(sdb_corpus* c, const double* queries, uint32_t nq, uint32_t k,
+                                           sdb_screen screen, int streaming, uint32_t cand_cap, int score_all,
+                                           float* out_qf, double* out_qmag, uint32_t* out_qu, int8_t* out_q8,
+                                           uint16_t* out_qbf16, uint32_t* out_a, uint32_t* out_b, uint32_t* out_rr,
+                                           const uint32_t* filters, uint32_t n_filters, const uint32_t* query_filter,
+                                           int mask_hits) {
+  return debug_screen_batch(c, queries, nq, k, screen, streaming, cand_cap, score_all, out_qf, out_qmag, out_qu, out_q8,
+                            out_qbf16, out_a, out_b, out_rr, filters, n_filters, query_filter, mask_hits, Ranking());
+}
+
+sdb_status sdb_debug_screen_batch_ranked(sdb_corpus* c, const double* queries, uint32_t nq, uint32_t k,
+                                         sdb_screen screen, int streaming, uint32_t cand_cap, int score_all,
+                                         float* out_qf, double* out_qmag, uint32_t* out_qu, int8_t* out_q8,
+                                         uint16_t* out_qbf16, uint32_t* out_a, uint32_t* out_b, uint32_t* out_rr,
+                                         const uint32_t* filters, uint32_t n_filters, const uint32_t* query_filter,
+                                         int mask_hits, int fn, int order) {
+  if (c && !screened_ranking(c, Ranking{fn, order == SDB_ORDER_DESC})) {
+    set_error("sdb_debug_screen_batch_ranked: (fn %d, order %d) is not a ranking the screens serve on this corpus", fn,
+              order);
+    return SDB_EINVAL;
+  }
+  if (order != SDB_ORDER_ASC && order != SDB_ORDER_DESC) {
+    set_error("sdb_debug_screen_batch_ranked: unknown order %d", order);
+    return SDB_EINVAL;
+  }
+  return debug_screen_batch(c, queries, nq, k, screen, streaming, cand_cap, score_all, out_qf, out_qmag, out_qu, out_q8,
+                            out_qbf16, out_a, out_b, out_rr, filters, n_filters, query_filter, mask_hits,
+                            Ranking{fn, order == SDB_ORDER_DESC});
 }
 
 sdb_status sdb_knn_submit(sdb_corpus* c, const double* queries, uint32_t nq, uint32_t k, uint64_t* out_rows,
@@ -1987,7 +2035,7 @@ sdb_status sdb_corpus_project(sdb_corpus* c, const double* query, int fn, double
     if (query) SDB_CUDA(cudaMemcpyAsync(d_q, query, sizeof(double) * c->dim, cudaMemcpyHostToDevice, st));
     else SDB_CUDA(cudaMemsetAsync(d_q, 0, sizeof(double) * c->dim, st));
     SDB_TRY(scratch_for(c, s, 1, 4096));
-    SDB_TRY(prep_queries(c, s, d_q, 1, st));
+    SDB_TRY(prep_queries(c, s, d_q, 1, st, score_kind(c, Ranking()), false));
     SDB_TRY(exact_project(c, fn, s.d_q64, s.d_qmag, s.d_qflags, d_vals, st));
     SDB_CUDA(cudaMemcpyAsync(out, d_vals, sizeof(double) * c->n, cudaMemcpyDeviceToHost, st));
     return SDB_OK;

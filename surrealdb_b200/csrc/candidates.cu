@@ -13,6 +13,9 @@
 namespace sdb {
 
 // ------------------------------------------------------------------------------------------------
+// NEG: the f32 / bf16 screen copies (and the measured residual qbferr) are those of -q, negated in f64 before any
+// rounding (Score::Dot, ascending); qmag and the flags are those of q, which the negation does not change
+template <bool NEG = false>
 __global__ void prep_queries_kernel(const double* __restrict__ q64, uint32_t dim, uint32_t dim_pad, int metric,
                                     float* __restrict__ q32, __nv_bfloat16* __restrict__ qbf, double* __restrict__ qmag,
                                     uint32_t* __restrict__ qflags, float* __restrict__ qbferr, uint32_t nq) {
@@ -28,7 +31,7 @@ __global__ void prep_queries_kernel(const double* __restrict__ q64, uint32_t dim
   float err2 = 0.f;
   if (q < nq) {
     for (uint32_t c = threadIdx.x; c < dim_pad; c += blockDim.x) {
-      const double v = c < dim ? q64[(size_t)q * dim + c] : 0.0;
+      const double v = c < dim ? (NEG ? -q64[(size_t)q * dim + c] : q64[(size_t)q * dim + c]) : 0.0;
       const float f = (float)v;
       if (q32 && c < dim) q32[(size_t)q * dim + c] = f;
       const __nv_bfloat16 h = __float2bfloat16_rn(f);
@@ -432,7 +435,66 @@ __global__ void __launch_bounds__(128) cand_begin_minkowski_kernel(
               __double2float_ru(mg), 0.f, 0.f, __double2float_rd(lo), __double2float_ru(hi));
 }
 
-sdb_status cand_begin(const Corpus* c, Scratch& s, uint32_t nq, int screen, cudaStream_t st) {
+// Score::Dot (dot_ranking batches): the screens score s~ = x~.q~, with q~ the screen copy of q (DESC) or of -q (ASC),
+// and beps bounds |s~ - x.(+-q)| for every screened row.  M = max_norm >= |x| of every screened row (f32, rounded up).
+//  - Operand rounding: x~.q~ - x.q = (x~ - x).q~ + x.(q~ - q), so |.| <= (e_x (1 + e_q) + e_q) |x||q| with the measured
+//    residuals e_x (bf16_rel_err) and e_q (qbferr: of the copy actually used, -q for ASC) of cand_begin_kernel.
+//  - f32 accumulation: at most D 2^-21 of sum |x~_i q~_i| <= |x~||q~| <= 1.01 |x||q| (bf16); the SIMT f32 screen's
+//    whole relative term is (D/16 + 16) 2^-23 as above.  So e_rel = e_x + e_q + e_x e_q + 1.01 D 2^-21 (bf16).
+//  - Absolute terms, which no relative one covers: an element of the f32 query or of a stage-B row in f32's subnormal
+//    range rounds by up to 2^-150 (at most D 2^-150 (|q| + M) over the dot), and the tensor cores or the f32 chains may
+//    flush operands, products and partial sums below 2^-126 (at most D 2^-126 (1 + |q| + M) in all); also the
+//    reference's own f64 underflow (D 2^-1074; cand_final's eps_ref is relative).  All are inside
+//    e_abs = D 2^-120 (1 + |q| + M), for f32 and f64 rows alike.
+// beps = e_rel |q| M + e_abs, margin = 2.1 beps in score (= dot) units, bscale = 1, every score lies in
+// +-(|q| M 1.01 + beps) (histogram range).  Stage B (cand_refine: f32 rows, or f64 rows rounded to f32 (+2^-24),
+// against the f32 copy): beps2 = e2_rel |q| M + e_abs with cand_begin_kernel's e2_rel.  A zero or non-finite |q| takes
+// the exact kernel (prep_queries' flags); a bound or score range that is not a finite f32 becomes an infinite bound
+// (tau then proves nothing: exact fallback).
+__global__ void cand_begin_dot_kernel(float* __restrict__ tau, uint32_t* __restrict__ cnt, uint32_t* __restrict__ flags,
+                                      uint32_t* __restrict__ stat, float* __restrict__ bscale, float* __restrict__ beps,
+                                      float* __restrict__ margin, float* __restrict__ margin2,
+                                      float* __restrict__ beps2, float* __restrict__ tau2, float* __restrict__ qlow,
+                                      float* __restrict__ qcap, const double* __restrict__ qmag,
+                                      const float* __restrict__ qbferr, uint32_t nq, int screen, uint32_t dim,
+                                      float bf16_rel_err, float max_norm, int exact, int f64_rows) {
+  const uint32_t q = blockIdx.x * blockDim.x + threadIdx.x;
+  if (blockIdx.x == 0 && threadIdx.x < 4) stat[threadIdx.x] = 0;
+  if (q >= nq) return;
+  const double qm = qmag[q], mn = (double)max_norm, D = (double)dim;
+  double e_rel;
+  if (screen == SDB_SCREEN_TC_BF16) {
+    const double eq = qbferr[q], ex = bf16_rel_err;
+    e_rel = ex + eq + ex * eq + 1.01 * D * 0x1p-21;
+  } else {
+    e_rel = (D / 16.0 + 16.0) * 0x1p-23;
+  }
+  const double e_abs = D * 0x1p-120 * (1.0 + qm + mn);
+  double eps = e_rel * qm * mn + e_abs;
+  double e2 = ((D + 16.0) * 0x1p-24 + (f64_rows ? 0x1p-24 : 0.0)) * qm * mn + e_abs;
+  double mg = 2.1 * eps, mg2 = 2.1 * e2, hi = qm * mn * 1.01 + eps + 1e-30;
+  if (!(qm > 0.0) || !(hi <= 3.4028234663852886e38) || !(mg <= 3.4028234663852886e38)) {  // no bound
+    eps = e2 = INFINITY;
+    mg = mg2 = 0.0;
+    hi = 1.0;
+  }
+  if (!exact) mg = mg2 = 0.0;
+  begin_query(q, tau, cnt, flags, bscale, beps, margin, margin2, beps2, tau2, qlow, qcap, 1.f, __double2float_ru(eps),
+              __double2float_ru(mg), __double2float_ru(mg2), __double2float_ru(e2), __double2float_rd(-hi),
+              __double2float_ru(hi));
+}
+
+sdb_status cand_begin(const Corpus* c, Scratch& s, uint32_t nq, int screen, cudaStream_t st, Score sc) {
+  if (sc == Score::Dot) {
+    cand_begin_dot_kernel<<<(nq + 255) / 256, 256, 0, st>>>(s.d_tau, s.d_cand_cnt, s.d_flags, s.d_stat, s.d_bscale,
+                                                            s.d_beps, s.d_margin, s.d_margin2, s.d_beps2, s.d_tau2,
+                                                            s.d_qlow, s.d_qcap, s.d_qmag, s.d_qbferr, nq, screen,
+                                                            c->dim, c->bf16_rel_err, c->max_norm, c->exact ? 1 : 0,
+                                                            c->dtype == SDB_F64 ? 1 : 0);
+    count_launch(c->ctx);
+    SDB_CUDA(cudaGetLastError());
+    return SDB_OK;
+  }
   switch (family(c)) {
     case Family::Lp:
       if (const int p = minkowski_screen_order(c)) {
@@ -538,7 +600,7 @@ sdb_status scratch_for(const Corpus* c, Scratch& s, uint32_t nq, uint32_t cap) {
   return SDB_OK;
 }
 
-sdb_status prep_queries(const Corpus* c, Scratch& s, const double* d_queries, uint32_t nq, cudaStream_t st,
+sdb_status prep_queries(const Corpus* c, Scratch& s, const double* d_queries, uint32_t nq, cudaStream_t st, Score sc,
                         bool desc) {
   // d_queries may alias s.d_q64
   if (d_queries != s.d_q64)
@@ -548,7 +610,11 @@ sdb_status prep_queries(const Corpus* c, Scratch& s, const double* d_queries, ui
   if (f == Family::Centred)
     prep_queries_pearson_kernel<<<nq_pad, 128, 0, st>>>(s.d_q64, c->dim, c->dim_pad, s.d_q32, s.d_qbf16, s.d_qmag,
                                                         s.d_qmom, s.d_qflags, s.d_qbferr, nq, desc);
-  else
+  else if (sc == Score::Dot) {  // (COSINE's query rule: a zero or non-finite |q| takes the exact kernel)
+    auto prep = desc ? prep_queries_kernel<false> : prep_queries_kernel<true>;
+    prep<<<nq_pad, 128, 0, st>>>(s.d_q64, c->dim, c->dim_pad, (int)SDB_COSINE, s.d_q32, s.d_qbf16, s.d_qmag,
+                                 s.d_qflags, s.d_qbferr, nq);
+  } else
     prep_queries_kernel<<<nq_pad, 128, 0, st>>>(s.d_q64, c->dim, c->dim_pad, (int)c->metric, s.d_q32, s.d_qbf16,
                                                 s.d_qmag, s.d_qflags, s.d_qbferr, nq);
   count_launch(c->ctx);
@@ -946,7 +1012,8 @@ sdb_status cand_select(const Corpus* c, Scratch& s, uint32_t nq, uint32_t k, boo
 // fl32(x_i - m1), against the f32 copy of -dq: the rounding is relative per element, as for f64 cosine rows, so the
 // same stage-B bound holds for dx.  (Subtracting fl32(m1) in f32 would err by 2^-24 |m1| per element, absolutely:
 // unbounded relative to |dx| for rows whose offset dwarfs their spread.)
-template <typename T, bool COSINE, bool CENTRED = false>
+// S: the score (score_kind), from the f32 dot a: a / |x|, 2 a - |x|^2 or a itself
+template <typename T, Score S, bool CENTRED = false>
 __global__ void __launch_bounds__(128) cand_refine_f32_kernel(const T* __restrict__ rows, uint32_t dim,
                                                                const float* __restrict__ snorm,
                                                                const float* __restrict__ q32, Cand* __restrict__ cand,
@@ -1010,41 +1077,47 @@ __global__ void __launch_bounds__(128) cand_refine_f32_kernel(const T* __restric
       a1 += __shfl_xor_sync(0xffffffffu, a1, o);
     }
     if (lane == 0) {
-      const float s0 = __ldg(snorm + r0);
-      cq[e0].score = COSINE ? a0 * s0 : fmaf(2.f, a0, -s0);
-      if (has1) {
-        const float s1 = __ldg(snorm + r1);
-        cq[e0 + 1].score = COSINE ? a1 * s1 : fmaf(2.f, a1, -s1);
+      if constexpr (S == Score::Dot) {
+        cq[e0].score = a0;
+        if (has1) cq[e0 + 1].score = a1;
+      } else {
+        const float s0 = __ldg(snorm + r0);
+        cq[e0].score = S == Score::Cosine ? a0 * s0 : fmaf(2.f, a0, -s0);
+        if (has1) {
+          const float s1 = __ldg(snorm + r1);
+          cq[e0 + 1].score = S == Score::Cosine ? a1 * s1 : fmaf(2.f, a1, -s1);
+        }
       }
     }
   }
 }
-sdb_status cand_refine(const Corpus* c, Scratch& s, uint32_t nq, cudaStream_t st) {
+template <Score S>
+static void refine_dot(const Corpus* c, Scratch& s, uint32_t nq, cudaStream_t st) {
+  const dim3 grid(nq, 8);
+  if (c->dtype == SDB_F32)
+    cand_refine_f32_kernel<float, S><<<grid, 128, 0, st>>>((const float*)c->d_rows.get(), c->dim, c->d_snorm, s.d_q32,
+                                                           s.d_cand, s.d_cand_cnt, s.sc_cap, nullptr);
+  else
+    cand_refine_f32_kernel<double, S><<<grid, 128, 0, st>>>((const double*)c->d_rows.get(), c->dim, c->d_snorm,
+                                                            s.d_q32, s.d_cand, s.d_cand_cnt, s.sc_cap, nullptr);
+}
+sdb_status cand_refine(const Corpus* c, Scratch& s, uint32_t nq, cudaStream_t st, Score sc) {
   const dim3 grid(nq, 8);  // 128-thread blocks (register budget beside a resident screen CTA)
   const float* f32_rows = (const float*)c->d_rows.get();
   const double* f64_rows = (const double*)c->d_rows.get();
   switch (family(c)) {
     case Family::Centred:
       if (c->dtype == SDB_F32)
-        cand_refine_f32_kernel<float, true, true><<<grid, 128, 0, st>>>(f32_rows, c->dim, c->d_snorm, s.d_q32,
-                                                                        s.d_cand, s.d_cand_cnt, s.sc_cap, c->d_mom);
+        cand_refine_f32_kernel<float, Score::Cosine, true><<<grid, 128, 0, st>>>(
+            f32_rows, c->dim, c->d_snorm, s.d_q32, s.d_cand, s.d_cand_cnt, s.sc_cap, c->d_mom);
       else
-        cand_refine_f32_kernel<double, true, true><<<grid, 128, 0, st>>>(f64_rows, c->dim, c->d_snorm, s.d_q32,
-                                                                         s.d_cand, s.d_cand_cnt, s.sc_cap, c->d_mom);
+        cand_refine_f32_kernel<double, Score::Cosine, true><<<grid, 128, 0, st>>>(
+            f64_rows, c->dim, c->d_snorm, s.d_q32, s.d_cand, s.d_cand_cnt, s.sc_cap, c->d_mom);
       break;
     case Family::Dot:
-      if (c->dtype == SDB_F32 && c->metric == SDB_COSINE)
-        cand_refine_f32_kernel<float, true><<<grid, 128, 0, st>>>(f32_rows, c->dim, c->d_snorm, s.d_q32, s.d_cand,
-                                                                  s.d_cand_cnt, s.sc_cap, nullptr);
-      else if (c->dtype == SDB_F32)
-        cand_refine_f32_kernel<float, false><<<grid, 128, 0, st>>>(f32_rows, c->dim, c->d_snorm, s.d_q32, s.d_cand,
-                                                                   s.d_cand_cnt, s.sc_cap, nullptr);
-      else if (c->metric == SDB_COSINE)
-        cand_refine_f32_kernel<double, true><<<grid, 128, 0, st>>>(f64_rows, c->dim, c->d_snorm, s.d_q32, s.d_cand,
-                                                                   s.d_cand_cnt, s.sc_cap, nullptr);
-      else
-        cand_refine_f32_kernel<double, false><<<grid, 128, 0, st>>>(f64_rows, c->dim, c->d_snorm, s.d_q32, s.d_cand,
-                                                                    s.d_cand_cnt, s.sc_cap, nullptr);
+      if (sc == Score::Cosine) refine_dot<Score::Cosine>(c, s, nq, st);
+      else if (sc == Score::Euclid) refine_dot<Score::Euclid>(c, s, nq, st);
+      else refine_dot<Score::Dot>(c, s, nq, st);
       break;
     default: break;  // stage B follows the tensor-core screens (Dot, Centred) only
   }
@@ -1067,7 +1140,7 @@ struct RerankOut {  // nq x stride results: the value's key, the value, the row
   double* dist;
   uint32_t* row;
   uint32_t stride;
-  bool desc;  // cosine_desc batches: the value is the cosine similarity, keyed descending
+  bool desc;  // the descending rankings (cosine_desc: the value is the cosine similarity): keyed descending
 };
 __device__ __forceinline__ void rr_store(const RerankOut& out, uint32_t q, uint32_t e, uint32_t row, double d) {
   const size_t o = (size_t)q * out.stride + e;
@@ -1079,9 +1152,12 @@ static RerankOut rr_out(const Scratch& s, bool desc = false) {
   return RerankOut{s.d_rr_key, s.d_rr_dist, s.d_rr_row, s.rr_stride, desc};
 }
 
-// the COSINE / EUCLIDEAN finish of one entry (sim: COSINE's similarity instead of its distance)
+// the COSINE / EUCLIDEAN finish of one entry (sim: COSINE's similarity instead of its distance; DOT: vector::dot, whose
+// entries accumulated the cosine steps on either metric)
+template <bool DOT = false>
 __device__ __forceinline__ double dot_finish(bool cosine, bool sim, const RefSum& s, const double* mag, uint32_t row,
                                              double qm, bool q_nan) {
+  if (DOT) return RefAcc<SDB_FN_DOT>{}.finish(s, q_nan);
   if (!cosine) return RefAcc<SDB_EUCLIDEAN>{}.finish(s, q_nan);
   return sim ? RefAcc<SDB_FN_SIMILARITY_COSINE>{}.finish(s, mag[row], qm, q_nan)
              : RefAcc<SDB_COSINE>{}.finish(s, mag[row], qm, q_nan);
@@ -1091,8 +1167,9 @@ __device__ __forceinline__ double dot_finish(bool cosine, bool sim, const RefSum
 // rows 32 columns at a time: 32 coalesced 128-byte row segments are requested back to back (all in flight before the
 // first is consumed -- the kernel is bound by the latency of these gathers, not by the f64 arithmetic), transposed
 // through shared memory, and every lane then accumulates ITS row strictly left to right.
+// DOT (Score::Dot): metric is SDB_COSINE (the dot's steps) and the entries finish as vector::dot; so in the others.
 constexpr uint32_t RR_WARPS = 4, RR_COLS = 32;
-template <typename T>
+template <typename T, bool DOT = false>
 __global__ void __launch_bounds__(RR_WARPS * 32) cand_rerank_kernel(
     const T* __restrict__ rows, uint32_t dim, int metric, const double* __restrict__ mag,
     const double* __restrict__ q64, const double* __restrict__ qmag, const uint32_t* __restrict__ qflags,
@@ -1141,7 +1218,7 @@ __global__ void __launch_bounds__(RR_WARPS * 32) cand_rerank_kernel(
         __syncwarp();
       }
     }
-    if (my_row != NO_ROW) rr_store(out, q, e, my_row, dot_finish(metric == SDB_COSINE, out.desc, acc, mag, my_row, qm, q_nan));
+    if (my_row != NO_ROW) rr_store(out, q, e, my_row, dot_finish<DOT>(metric == SDB_COSINE, out.desc, acc, mag, my_row, qm, q_nan));
   }
 }
 
@@ -1150,6 +1227,7 @@ __global__ void __launch_bounds__(RR_WARPS * 32) cand_rerank_kernel(
 // 128-byte pieces of 32 different rows (random 128-byte gathers reach ~2 TB/s on HBM3e, page-friendly ones several
 // times that).  The 32 x 128 tile is then walked per lane with conflict-free LDS.128 (row stride 132 floats).
 constexpr uint32_t RRV_COLS = 128, RRV_STRIDE = RRV_COLS + 4;
+template <bool DOT = false>
 __global__ void __launch_bounds__(RR_WARPS * 32) cand_rerank_v4_kernel(
     const float* __restrict__ rows, uint32_t dim, int metric, const double* __restrict__ mag,
     const double* __restrict__ q64, const double* __restrict__ qmag, const uint32_t* __restrict__ qflags,
@@ -1219,7 +1297,7 @@ __global__ void __launch_bounds__(RR_WARPS * 32) cand_rerank_v4_kernel(
         __syncwarp();
       }
     }
-    if (my_row != NO_ROW) rr_store(out, q, e, my_row, dot_finish(metric == SDB_COSINE, out.desc, acc, mag, my_row, qm, q_nan));
+    if (my_row != NO_ROW) rr_store(out, q, e, my_row, dot_finish<DOT>(metric == SDB_COSINE, out.desc, acc, mag, my_row, qm, q_nan));
   }
 }
 constexpr size_t RRV_SMEM = sizeof(double) * QCHUNK + sizeof(float) * RR_WARPS * 32 * RRV_STRIDE;  // 75.8 KB
@@ -1232,7 +1310,8 @@ constexpr size_t RRV_SMEM = sizeof(double) * QCHUNK + sizeof(float) * RR_WARPS *
 // (the staged variant's 6 KB per warp let only two warps per SM in, and the re-rank took 0.58 ms instead of 0.1 ms
 // whenever it overlapped a screen -- SDB_TRACE timeline, round 2).  Every lane streams its own row (16-byte loads; the
 // second half of each 32-byte sector comes from L1) and reads the query from global memory (one address per half-warp).
-// f64 rows stream as double2 (16-byte) loads when the row length is even.  M: SDB_COSINE or SDB_EUCLIDEAN.
+// f64 rows stream as double2 (16-byte) loads when the row length is even.  M: SDB_COSINE, SDB_EUCLIDEAN or SDB_FN_DOT
+// (Score::Dot on either metric).
 template <typename T, int M>
 __global__ void __launch_bounds__(128) cand_rerank_packed_kernel(
     const T* __restrict__ rows, uint32_t dim, const double* __restrict__ mag, const double* __restrict__ q64,
@@ -1279,7 +1358,7 @@ __global__ void __launch_bounds__(128) cand_rerank_packed_kernel(
     } else {
       for (uint32_t j = 0; j < dim; j++) ref.step(acc, (double)__ldg(x + j), __ldg(qv + j));
     }
-    rr_store(out, q, e, my_row, dot_finish(M == SDB_COSINE, out.desc, acc, mag, my_row, qm, q_nan));
+    rr_store(out, q, e, my_row, dot_finish<M == SDB_FN_DOT>(M == SDB_COSINE, out.desc, acc, mag, my_row, qm, q_nan));
   }
 }
 
@@ -1358,36 +1437,45 @@ static void rerank_entry(const Corpus* c, Scratch& s, uint32_t nq, uint32_t n_sp
 }
 
 template <typename T>
-static void rerank_packed(const Corpus* c, Scratch& s, uint32_t nq, uint32_t n_sp, bool desc, cudaStream_t st) {
-  auto kern = c->metric == SDB_COSINE ? cand_rerank_packed_kernel<T, SDB_COSINE> : cand_rerank_packed_kernel<T, SDB_EUCLIDEAN>;
+static void rerank_packed(const Corpus* c, Scratch& s, uint32_t nq, uint32_t n_sp, bool desc, Score sc,
+                          cudaStream_t st) {
+  auto kern = sc == Score::Dot            ? cand_rerank_packed_kernel<T, SDB_FN_DOT>
+              : c->metric == SDB_COSINE ? cand_rerank_packed_kernel<T, SDB_COSINE>
+                                          : cand_rerank_packed_kernel<T, SDB_EUCLIDEAN>;
   kern<<<(nq + 7) / 8, 128, 0, st>>>((const T*)c->d_rows.get(), c->dim, c->d_mag, s.d_q64, s.d_qmag, s.d_qflags,
                                      s.d_cand, s.d_cand_cnt, s.sc_cap, c->d_special, n_sp, nq, rr_out(s, desc));
 }
 
 // COSINE / EUCLIDEAN: the packed kernel for the small sets stage B leaves; otherwise the vectorised one for f32 rows
 // of a length divisible by 4, the staged one for the rest
-static void rerank_dot(const Corpus* c, Scratch& s, uint32_t nq, bool small_sets, uint32_t n_sp, bool desc,
-                       cudaStream_t st) {
+template <bool DOT>
+static void rerank_wide(const Corpus* c, Scratch& s, uint32_t nq, uint32_t n_sp, bool desc, cudaStream_t st) {
   const dim3 grid(nq, RR_GROUPS_Y);
   const RerankOut out = rr_out(s, desc);
-  if (small_sets && c->dtype == SDB_F32) rerank_packed<float>(c, s, nq, n_sp, desc, st);
-  else if (small_sets) rerank_packed<double>(c, s, nq, n_sp, desc, st);
-  else if (c->dtype == SDB_F32 && c->dim % 4 == 0)
-    cand_rerank_v4_kernel<<<grid, RR_WARPS * 32, RRV_SMEM, st>>>((const float*)c->d_rows.get(), c->dim, (int)c->metric,
-                                                                c->d_mag, s.d_q64, s.d_qmag, s.d_qflags, s.d_cand,
-                                                                s.d_cand_cnt, s.sc_cap, c->d_special, n_sp, out);
+  const int metric = DOT ? (int)SDB_COSINE : (int)c->metric;
+  if (c->dtype == SDB_F32 && c->dim % 4 == 0)
+    cand_rerank_v4_kernel<DOT><<<grid, RR_WARPS * 32, RRV_SMEM, st>>>((const float*)c->d_rows.get(), c->dim, metric,
+                                                                     c->d_mag, s.d_q64, s.d_qmag, s.d_qflags, s.d_cand,
+                                                                     s.d_cand_cnt, s.sc_cap, c->d_special, n_sp, out);
   else if (c->dtype == SDB_F32)
-    cand_rerank_kernel<float><<<grid, RR_WARPS * 32, 0, st>>>((const float*)c->d_rows.get(), c->dim, (int)c->metric,
-                                                             c->d_mag, s.d_q64, s.d_qmag, s.d_qflags, s.d_cand,
-                                                             s.d_cand_cnt, s.sc_cap, c->d_special, n_sp, out);
+    cand_rerank_kernel<float, DOT><<<grid, RR_WARPS * 32, 0, st>>>((const float*)c->d_rows.get(), c->dim, metric,
+                                                                  c->d_mag, s.d_q64, s.d_qmag, s.d_qflags, s.d_cand,
+                                                                  s.d_cand_cnt, s.sc_cap, c->d_special, n_sp, out);
   else
-    cand_rerank_kernel<double><<<grid, RR_WARPS * 32, 0, st>>>((const double*)c->d_rows.get(), c->dim, (int)c->metric,
-                                                              c->d_mag, s.d_q64, s.d_qmag, s.d_qflags, s.d_cand,
-                                                              s.d_cand_cnt, s.sc_cap, c->d_special, n_sp, out);
+    cand_rerank_kernel<double, DOT><<<grid, RR_WARPS * 32, 0, st>>>((const double*)c->d_rows.get(), c->dim, metric,
+                                                                   c->d_mag, s.d_q64, s.d_qmag, s.d_qflags, s.d_cand,
+                                                                   s.d_cand_cnt, s.sc_cap, c->d_special, n_sp, out);
+}
+static void rerank_dot(const Corpus* c, Scratch& s, uint32_t nq, bool small_sets, uint32_t n_sp, bool desc, Score sc,
+                       cudaStream_t st) {
+  if (small_sets && c->dtype == SDB_F32) rerank_packed<float>(c, s, nq, n_sp, desc, sc, st);
+  else if (small_sets) rerank_packed<double>(c, s, nq, n_sp, desc, sc, st);
+  else if (sc == Score::Dot) rerank_wide<true>(c, s, nq, n_sp, desc, st);
+  else rerank_wide<false>(c, s, nq, n_sp, desc, st);
 }
 
 sdb_status cand_rerank(const Corpus* c, Scratch& s, const FiltArg& filt, uint32_t nq, cudaStream_t st,
-                       bool small_sets, bool desc) {
+                       bool small_sets, bool desc, Score sc) {
   const uint32_t n_sp = filt.bits ? 0u : c->n_special;  // filtered: the passing special rows are in the lists
   switch (family(c)) {
     case Family::Count:  // (the direct regime only; no special rows)
@@ -1404,7 +1492,7 @@ sdb_status cand_rerank(const Corpus* c, Scratch& s, const FiltArg& filt, uint32_
       break;
     case Family::Dot:
     case Family::Exact:  // (never reaches the re-rank: the exact kernel alone ranks it)
-      rerank_dot(c, s, nq, small_sets, n_sp, desc, st);
+      rerank_dot(c, s, nq, small_sets, n_sp, desc, sc, st);
       break;
   }
   count_launch(c->ctx);
@@ -1443,8 +1531,9 @@ __device__ __forceinline__ void bitonic_pairs(uint64_t* s_key, uint64_t* s_idx, 
 
 // The proof of the family F's bound: Dot (cosine / euclidean, also the count path's lists, whose tau stays -inf), Lp, or
 // Centred (the cosine proof on the centred operands, eps_ref = the gap between their cosine and the reference's
-// pearson, DESIGN.md section 2; 0 for the other families)
-template <Family F>
+// pearson, DESIGN.md section 2; 0 for the other families).  DOT: Score::Dot batches of Dot corpora, whose eps_ref is the
+// reference's relative rounding times max_norm (per unit of |q|)
+template <Family F, bool DOT = false>
 __global__ void __launch_bounds__(256)
     cand_final_kernel(const uint64_t* __restrict__ rr_key, const double* __restrict__ rr_dist,
                       const uint32_t* __restrict__ rr_row, uint32_t rr_stride, const uint32_t* __restrict__ cnt,
@@ -1506,7 +1595,14 @@ __global__ void __launch_bounds__(256)
       const double qm = qmag[q];
       const uint64_t kth = s_key[k - 1];
       bool ok;
-      if (F == Family::Lp) {
+      if (DOT) {
+        // Score::Dot (cand_begin_dot_kernel): a non-candidate's screened score is below tau, so its dot with the
+        // screened query (q DESC, -q ASC) is at most tau + beps, and the reference's sequential f64 dot -- the value
+        // keyed -- is within eps_ref |q| of the real one.  DESC: value <= U = tau + beps + eps_ref |q|; ASC: value >= -U.
+        // U is rounded up (so -U down); proven when that bound sorts strictly after the k-th entry
+        const double U = __dadd_ru(__dadd_ru((double)t, (double)beps[q]), __dmul_ru(eps_ref, qm));
+        ok = U == U && order_key(desc ? U : -U, desc) > kth;
+      } else if (F == Family::Lp) {
         // score = -s~ < tau for a non-candidate, so s~ > -tau and d >= s~ - beps > -tau - beps: the row cannot reach
         // the top k if that bound (rounded down) is strictly above the k-th exact key.  No stage B ran (tau2 = -inf).
         const double L = (-(double)t - (double)beps[q]) * (1.0 - 1e-12);
@@ -1542,7 +1638,10 @@ __global__ void __launch_bounds__(256)
       // stage B dropped candidates whose f32 score is below tau2: the same proof with the f32 bound
       const float t2 = tau2[q];
       if (ok && t2 > __int_as_float(0xff800000)) {
-        if (F == Family::Centred && desc) {
+        if (DOT) {
+          const double U2 = __dadd_ru(__dadd_ru((double)t2, (double)beps2[q]), __dmul_ru(eps_ref, qm));
+          ok = U2 == U2 && order_key(desc ? U2 : -U2, desc) > kth;
+        } else if (F == Family::Centred && desc) {
           const double U2 = __dadd_ru(__dadd_ru(__ddiv_ru((double)t2, qm), (double)beps2[q]), eps_ref);
           ok = order_key(U2, true) > kth;
         } else if (F == Family::Centred) {  // stage B scores in the same units with bscale 1
@@ -1573,7 +1672,8 @@ __global__ void __launch_bounds__(256)
 }
 
 sdb_status cand_final(const Corpus* c, Scratch& s, const FiltArg& filt, uint32_t nq, uint32_t k, uint64_t row_base,
-                      uint64_t* d_out_rows, double* d_out_dist, uint32_t* d_out_count, cudaStream_t st, bool desc) {
+                      uint64_t* d_out_rows, double* d_out_dist, uint32_t* d_out_count, cudaStream_t st, bool desc,
+                      Score sc) {
   if (k > FIN_KEEP) {
     set_error("cand_final: k = %u exceeds the screened path's limit of %u", k, FIN_KEEP);
     return SDB_EINVAL;
@@ -1584,6 +1684,14 @@ sdb_status cand_final(const Corpus* c, Scratch& s, const FiltArg& filt, uint32_t
   double eps_ref = 0.0;
   switch (family(c)) {
     case Family::Dot:
+      if (sc == Score::Dot) {
+        fin = cand_final_kernel<Family::Dot, true>;
+        // the reference's sequential f64 dot of D terms errs by at most gamma_D sum |x_i q_i| <= gamma_D |x||q|,
+        // gamma_D = D 2^-53 / (1 - D 2^-53) <= (D + 2) 2^-53; |x| <= max_norm; (1 + 2^-20) covers the rounding of
+        // |q| (qmag) and of this figure
+        eps_ref = (c->dim + 2.0) * 0x1p-53 * (double)c->max_norm * (1.0 + 0x1p-20);
+      }
+      break;
     case Family::Count:  // (tau = -inf: nothing to prove)
     case Family::Exact:  // (never reaches cand_final)
       break;
@@ -1606,7 +1714,8 @@ sdb_status cand_final(const Corpus* c, Scratch& s, const FiltArg& filt, uint32_t
 }
 
 sdb_status candidates_init_device() {
-  SDB_CUDA(cudaFuncSetAttribute(cand_rerank_v4_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)RRV_SMEM));
+  SDB_CUDA(cudaFuncSetAttribute(cand_rerank_v4_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)RRV_SMEM));
+  SDB_CUDA(cudaFuncSetAttribute(cand_rerank_v4_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)RRV_SMEM));
   return SDB_OK;
 }
 

@@ -408,7 +408,8 @@ struct Corpus {
   double minkowski_p = 3.0;   // order of SDB_MINKOWSKI
   sdb_screen rung_scr = SDB_SCREEN_AUTO;  // the first-choice screen the remembered rung belongs to
   uint32_t rung_k = 0;                    // ... and the k it was learnt for
-  uint32_t rung = 0;                      // rung of the precision ladder the last batch settled on (api.cu)
+  int rung_score = 0;                     // ... and the Score of its batch (dot batches' candidate sets are not KNN's)
+  uint32_t rung = 0;                     // rung of the precision ladder the last batch settled on (api.cu)
   uint64_t cap = 0, n = 0;
   uint64_t row_base = 0;            // global id of row 0 (row-sharded corpora)
   bool finalized = false;
@@ -498,10 +499,25 @@ inline bool metric_desc(const Corpus* c, const Ranking& r) {
   const Family f = family(c);
   return r.desc && r.fn == (int)c->metric && (f == Family::Count || f == Family::Centred);
 }
+// vector::dot in either direction on a Dot corpus (COSINE or EUCLIDEAN with its bf16 copy): maximum (DESC) or minimum
+// (ASC) inner product.  The screens score x.q (DESC) or x.(-q) (ASC) with no norm term, the re-rank computes the
+// reference's dot and cand_final proves the order with the dot's bound (DESIGN.md sections 2 and 5, ORDER BY).
+inline bool dot_ranking(const Corpus* c, const Ranking& r) { return r.fn == SDB_FN_DOT && family(c) == Family::Dot; }
 // the rankings the screens (and the count path) serve; every other one is ranked by the exact kernel alone.  Those
-// that are descending are cosine_desc and metric_desc, and every stage takes Ranking::desc as it is.
+// that are descending are cosine_desc, metric_desc and dot_ranking, and every stage takes Ranking::desc as it is.
 inline bool screened_ranking(const Corpus* c, const Ranking& r) {
-  return knn_ranking(c, r) || cosine_desc(c, r) || metric_desc(c, r);
+  return knn_ranking(c, r) || cosine_desc(c, r) || metric_desc(c, r) || dot_ranking(c, r);
+}
+// What the Dot and Centred screens score per row, decided once per batch and handed to every stage that depends on it
+// (prep_queries, cand_begin, the screens, cand_refine, the re-rank, cand_final):
+//   Cosine  acc / |x|          COSINE corpora and the centred operands of PEARSON ones
+//   Euclid  2 acc - |x|^2      EUCLIDEAN corpora
+//   Dot     acc                dot_ranking batches on either Dot metric
+// acc = x~.q~, the dot of the screen copies.  (Lp / Count / Exact corpora: Euclid, which none of their stages reads.)
+enum class Score { Cosine, Euclid, Dot };
+inline Score score_kind(const Corpus* c, const Ranking& r) {
+  if (dot_ranking(c, r)) return Score::Dot;
+  return c->metric == SDB_COSINE || family(c) == Family::Centred ? Score::Cosine : Score::Euclid;
 }
 
 // ---- the brute-force driver (api.cu), as its entry points and the sharded search (comm.cu) use it ------------------
@@ -549,9 +565,9 @@ sdb_status corpus_finalize_device(Corpus* c);
 sdb_status corpus_remove_device(Corpus* c, const uint64_t* h_ids, uint64_t n);
 sdb_status corpus_reapply_tombstones(Corpus* c, cudaStream_t st);
 // The stages of a batch take its scratch set s and, where rows are screened or ranked, its row filter filt.
-// screen_simt.cu: the SIMT_F32 screen of Dot corpora (f32 rows)
+// screen_simt.cu: the SIMT_F32 screen of Dot corpora (f32 rows), scoring sc
 sdb_status screen_simt_pass(const Corpus* c, Scratch& s, const FiltArg& filt, uint32_t nq, const PassDesc& p,
-                            cudaStream_t st);
+                            cudaStream_t st, Score sc);
 // screen_lp.cu: the SIMT_F32 screen of Lp corpora, f32 L1 / L-infinity / Lp (score = -s~), f32 and f64 rows
 sdb_status screen_lp_pass(const Corpus* c, Scratch& s, const FiltArg& filt, uint32_t nq, const PassDesc& p,
                           cudaStream_t st);
@@ -566,19 +582,21 @@ sdb_status count_pass(const Corpus* c, Scratch& s, const FiltArg& filt, uint32_t
 // screen_tc.cu
 // mode 0: pass 0 (every score of the pass's tiles written to fixed slots), 1: threshold pass, 2: streaming pass with
 // in-kernel threshold refinement (histogram + refiner warp), 3: probe (chunk maxima of a few tiles, no candidates)
+// sc: the batch's score_kind (the int8 screen serves Score::Cosine only)
 sdb_status screen_tc_pass(const Corpus* c, Scratch& s, const FiltArg& filt, uint32_t nq, uint32_t k, const PassDesc& p,
-                          bool int8, int mode, cudaStream_t st);
+                          bool int8, int mode, cudaStream_t st, Score sc);
 bool screen_tc_available();
 // candidates.cu
 // grows s to nq queries x cap candidates (a set that grows loses its contents)
 sdb_status scratch_for(const Corpus* c, Scratch& s, uint32_t nq, uint32_t cap);
-// desc: PEARSON's screen copies of +dq / |dq| (a metric_desc batch) instead of -dq / |dq|
-sdb_status prep_queries(const Corpus* c, Scratch& s, const double* d_queries, uint32_t nq, cudaStream_t st,
-                        bool desc = false);
+// sc, desc: the batch's score_kind and direction.  Centred: desc takes the screen copies of +dq / |dq| (a metric_desc
+// batch) instead of -dq / |dq|; Score::Dot: ascending batches take the screen copies of -q (the re-rank keeps q)
+sdb_status prep_queries(const Corpus* c, Scratch& s, const double* d_queries, uint32_t nq, cudaStream_t st, Score sc,
+                        bool desc);
 // one query prepared into the fallback scratch (d_fb_*), independent of the batch scratch
 sdb_status prep_fallback_query(Corpus* c, const double* d_query, cudaStream_t st);
 // resets tau / counts / flags and derives, per query, the screen's error bound, the selection margin and the score range
-sdb_status cand_begin(const Corpus* c, Scratch& s, uint32_t nq, int screen, cudaStream_t st);
+sdb_status cand_begin(const Corpus* c, Scratch& s, uint32_t nq, int screen, cudaStream_t st, Score sc);
 sdb_status cand_set_count(const Corpus* c, Scratch& s, uint32_t nq, uint32_t value, cudaStream_t st);
 // per query: gather the main list + the private sub-lists, find the k-th best score s_k, keep every candidate with
 // score >= tau = s_k - margin (all of them while fewer than k exist), publish tau.  seed_hist: also (re)build the
@@ -587,7 +605,7 @@ sdb_status cand_select(const Corpus* c, Scratch& s, uint32_t nq, uint32_t k, boo
                        bool seed_hist, cudaStream_t st, int stage = 0);
 // stage B: re-score every kept candidate in f32 (master rows x f32 query) so that cand_select(stage 1) can shrink the
 // set before the FP64-bound exact re-rank
-sdb_status cand_refine(const Corpus* c, Scratch& s, uint32_t nq, cudaStream_t st);
+sdb_status cand_refine(const Corpus* c, Scratch& s, uint32_t nq, cudaStream_t st, Score sc);
 // after a probe launch over n_tiles tiles: tau = (k-th largest chunk maximum) - margin, histogram geometry, empty lists
 sdb_status cand_seed_from_probe(const Corpus* c, Scratch& s, uint32_t nq, uint32_t k, uint32_t n_tiles,
                                 cudaStream_t st);
@@ -600,12 +618,13 @@ sdb_status cand_add_specials(const Corpus* c, Scratch& s, const FiltArg& filt, u
 // direct regime (filtered): each query's list = the rows its filter passes that are neither skipped nor removed
 sdb_status cand_direct(const Corpus* c, Scratch& s, const FiltArg& filt, uint32_t nq, cudaStream_t st);
 // desc (the descending screened rankings): the re-rank keys its values descending (cosine_desc: it computes the
-// cosine similarity), and cand_final proves that order
+// cosine similarity), and cand_final proves that order.  sc = Score::Dot: the re-rank computes the reference's dot and
+// cand_final proves the order with the dot's bound, in either direction
 sdb_status cand_rerank(const Corpus* c, Scratch& s, const FiltArg& filt, uint32_t nq, cudaStream_t st,
-                       bool small_sets = false, bool desc = false);
+                       bool small_sets, bool desc, Score sc);
 sdb_status cand_final(const Corpus* c, Scratch& s, const FiltArg& filt, uint32_t nq, uint32_t k, uint64_t row_base,
-                      uint64_t* d_out_rows, double* d_out_dist, uint32_t* d_out_count, cudaStream_t st,
-                      bool desc = false);
+                      uint64_t* d_out_rows, double* d_out_dist, uint32_t* d_out_count, cudaStream_t st, bool desc,
+                      Score sc);
 // exact.cu: query vector / |q| / flags are passed explicitly (a batch scratch row or the fallback scratch).
 // filter: nullptr, or the query's bitmap (filter_words words): rows whose bit is clear are not ranked.
 // rank: the value ranked (any vector function) and its direction; the default is the corpus metric ascending (KNN).

@@ -285,7 +285,8 @@ __device__ __forceinline__ void push_survivors(const uint32_t (&acc)[128], int i
 // test sits where a survivor is appended (bf16: the consumer's append; int8: the drain warp, next to the screening-norm
 // look-up) and, in the probe, on the one bitmap word of every 32-row chunk.  Pass 0 writes every row; cand_filter_list
 // drops the rejected ones there.
-template <bool COSINE, bool INT8, int MODE, bool FILT>
+// S: the score of the bf16 epilogue (score_kind); the int8 screen scores Score::Cosine alone.
+template <Score S, bool INT8, int MODE, bool FILT>
 __global__ void __launch_bounds__(threads<INT8, MODE>(), 1)
 screen_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b,
                  const float* __restrict__ snorm, uint32_t k_blocks, uint32_t n_mblocks, uint32_t nq,
@@ -444,8 +445,15 @@ screen_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constan
           for (int i = 0; i < 2; i++) {
             float& a0 = acc[4 * jj + 2 * i];
             float& a1 = acc[4 * jj + 2 * i + 1];
-            a0 = COSINE ? a0 * n2.x : fmaf(2.f, a0, -n2.x);
-            a1 = COSINE ? a1 * n2.y : fmaf(2.f, a1, -n2.y);
+            if constexpr (S == Score::Dot) {
+              // the dot itself; the staged norm still marks invalid rows (NaN: skipped, special, padding), whose score
+              // becomes that NaN.  (A select, not acc + (n - n): a valid COSINE row's 1/|x| may be +inf in f32.)
+              a0 = n2.x == n2.x ? a0 : n2.x;
+              a1 = n2.y == n2.y ? a1 : n2.y;
+            } else {
+              a0 = S == Score::Cosine ? a0 * n2.x : fmaf(2.f, a0, -n2.x);
+              a1 = S == Score::Cosine ? a1 * n2.y : fmaf(2.f, a1, -n2.y);
+            }
           }
         }
       }
@@ -736,12 +744,13 @@ static sdb_status make_map(Ctx* ctx, CUtensorMap* map, const void* base, uint64_
 bool screen_tc_available() { return true; }
 
 sdb_status screen_tc_init_device(Ctx* ctx) {
-#define SET_SMEM1(COS, I8, MODE, F) \
-  SDB_CUDA(cudaFuncSetAttribute(tc::screen_tc_kernel<COS, I8, MODE, F>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tc::SMEM_BYTES))
-#define SET_SMEM(COS, I8, MODE) SET_SMEM1(COS, I8, MODE, false); SET_SMEM1(COS, I8, MODE, true)
-  SET_SMEM(true, false, 0); SET_SMEM(true, false, 1); SET_SMEM(true, false, 2); SET_SMEM(true, false, 3);
-  SET_SMEM(false, false, 0); SET_SMEM(false, false, 1); SET_SMEM(false, false, 2); SET_SMEM(false, false, 3);
-  SET_SMEM(true, true, 0); SET_SMEM(true, true, 1); SET_SMEM(true, true, 2); SET_SMEM(true, true, 3);
+#define SET_SMEM1(SC, I8, MODE, F) \
+  SDB_CUDA(cudaFuncSetAttribute(tc::screen_tc_kernel<SC, I8, MODE, F>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tc::SMEM_BYTES))
+#define SET_SMEM(SC, I8, MODE) SET_SMEM1(SC, I8, MODE, false); SET_SMEM1(SC, I8, MODE, true)
+  SET_SMEM(Score::Cosine, false, 0); SET_SMEM(Score::Cosine, false, 1); SET_SMEM(Score::Cosine, false, 2); SET_SMEM(Score::Cosine, false, 3);
+  SET_SMEM(Score::Euclid, false, 0); SET_SMEM(Score::Euclid, false, 1); SET_SMEM(Score::Euclid, false, 2); SET_SMEM(Score::Euclid, false, 3);
+  SET_SMEM(Score::Dot, false, 0); SET_SMEM(Score::Dot, false, 1); SET_SMEM(Score::Dot, false, 2); SET_SMEM(Score::Dot, false, 3);
+  SET_SMEM(Score::Cosine, true, 0); SET_SMEM(Score::Cosine, true, 1); SET_SMEM(Score::Cosine, true, 2); SET_SMEM(Score::Cosine, true, 3);
 #undef SET_SMEM
 #undef SET_SMEM1
   // how many 2-CTA clusters of the int8 streaming screen are resident at once (pairs must share a GPC, so this can be
@@ -758,20 +767,19 @@ sdb_status screen_tc_init_device(Ctx* ctx) {
   cfg.attrs = attr;
   cfg.numAttrs = 1;
   int clusters = 0;
-  SDB_CUDA(cudaOccupancyMaxActiveClusters(&clusters, tc::screen_tc_kernel<true, true, 2, false>, &cfg));
+  SDB_CUDA(cudaOccupancyMaxActiveClusters(&clusters, tc::screen_tc_kernel<Score::Cosine, true, 2, false>, &cfg));
   ctx->tc_pair_ctas = 2 * clusters;
   return SDB_OK;
 }
 
 sdb_status screen_tc_pass(const Corpus* c, Scratch& s, const FiltArg& filt, uint32_t nq, uint32_t k, const PassDesc& p,
-                          bool int8, int mode, cudaStream_t st) {
+                          bool int8, int mode, cudaStream_t st, Score sc) {
   if (p.count == 0) return SDB_OK;
   Ctx* ctx = c->ctx;
-  // PEARSON corpora hold centred copies (corpus.cu) and centred, negated queries (prep_queries): their cosine screen
-  const bool cosine = c->metric == SDB_COSINE || family(c) == Family::Centred;
-  if (int8 ? (!c->d_i8 || !cosine) : !c->d_bf16) {
+  // (PEARSON corpora hold centred copies (corpus.cu) and centred, negated queries (prep_queries): Score::Cosine)
+  if (int8 ? (!c->d_i8 || sc != Score::Cosine) : !c->d_bf16) {
     set_error("tensor-core screen: the %s screen copy is not available for this corpus",
-              int8 ? "int8 (cosine and pearson only)" : "bf16");
+              int8 ? "int8 (cosine and pearson scores only)" : "bf16");
     return SDB_EUNSUPPORTED;
   }
   const uint64_t n_pad = (c->n + TILE_ROWS - 1) / TILE_ROWS * TILE_ROWS;
@@ -847,26 +855,27 @@ sdb_status screen_tc_pass(const Corpus* c, Scratch& s, const FiltArg& filt, uint
     const float* snorm_arg = c->d_snorm;
     FiltArg filt_q = filt;
     if (filt_q.bits) filt_q.qf += q0;
-#define LAUNCH_TC2(COS, I8, MODE, F)                                                                                 \
-  SDB_CUDA(cudaLaunchKernelEx(&cfg, tc::screen_tc_kernel<COS, I8, MODE, F>, map_a, map_b, snorm_arg, k_blocks,       \
+#define LAUNCH_TC2(SC, I8, MODE, F)                                                                                  \
+  SDB_CUDA(cudaLaunchKernelEx(&cfg, tc::screen_tc_kernel<SC, I8, MODE, F>, map_a, map_b, snorm_arg, k_blocks,        \
                               n_mblocks, nqc, p, tau, cand, ccnt, cap_arg, sub, scnt, k, hp, hist, probe_ptr,        \
                               probe_stride, sleep_min, sleep_max, pair, filt_q))
-#define LAUNCH_TC1(COS, I8, MODE)                      \
-  do {                                                 \
-    cfg.blockDim = dim3(tc::threads<I8, MODE>());      \
-    if (filt_q.bits) LAUNCH_TC2(COS, I8, MODE, true);  \
-    else LAUNCH_TC2(COS, I8, MODE, false);             \
+#define LAUNCH_TC1(SC, I8, MODE)                      \
+  do {                                                \
+    cfg.blockDim = dim3(tc::threads<I8, MODE>());     \
+    if (filt_q.bits) LAUNCH_TC2(SC, I8, MODE, true);  \
+    else LAUNCH_TC2(SC, I8, MODE, false);             \
   } while (0)
-#define LAUNCH_TC(COS, I8)                   \
-  do {                                       \
-    if (mode == 0) LAUNCH_TC1(COS, I8, 0);   \
-    else if (mode == 1) LAUNCH_TC1(COS, I8, 1); \
-    else if (mode == 2) LAUNCH_TC1(COS, I8, 2); \
-    else LAUNCH_TC1(COS, I8, 3);             \
+#define LAUNCH_TC(SC, I8)                   \
+  do {                                      \
+    if (mode == 0) LAUNCH_TC1(SC, I8, 0);   \
+    else if (mode == 1) LAUNCH_TC1(SC, I8, 1); \
+    else if (mode == 2) LAUNCH_TC1(SC, I8, 2); \
+    else LAUNCH_TC1(SC, I8, 3);             \
   } while (0)
-    if (int8) LAUNCH_TC(true, true);
-    else if (cosine) LAUNCH_TC(true, false);
-    else LAUNCH_TC(false, false);
+    if (int8) LAUNCH_TC(Score::Cosine, true);
+    else if (sc == Score::Cosine) LAUNCH_TC(Score::Cosine, false);
+    else if (sc == Score::Euclid) LAUNCH_TC(Score::Euclid, false);
+    else LAUNCH_TC(Score::Dot, false);
 #undef LAUNCH_TC
 #undef LAUNCH_TC1
 #undef LAUNCH_TC2
