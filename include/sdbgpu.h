@@ -203,7 +203,11 @@ sdb_status sdb_debug_screen_batch_filtered(sdb_corpus*, const double* queries, u
  * instead of KNN's; SDB_EINVAL for a ranking the screens do not serve on the corpus.  SDB_FN_DOT on a COSINE or
  * EUCLIDEAN corpus (TC_BF16, or SIMT_F32 on F32 rows): the scores are the dots of the rows with the query (DESC) or
  * with its negation (ASC), out_qbf16 is the bf16 copy of that query, bscale is 1 and beps bounds the score's
- * distance from the exact dot; the exact re-rank still ranks the query itself. */
+ * distance from the exact dot; the exact re-rank still ranks the query itself.  The cross views of a COSINE or
+ * EUCLIDEAN corpus (cosine distance / similarity in the order KNN does not take, euclidean distance ASC on COSINE and
+ * DESC on either): the scores, the query copy (q or -q), bscale and beps are the view's -- cosine acc/|x| in
+ * similarity x |q| units, euclidean 2 acc - |x|^2 or farthest-first 2 acc + |x|^2 in squared-distance units -- and the
+ * special rows of out_rr are the view's (the cross special list where the view reads the other metric's norm). */
 sdb_status sdb_debug_screen_batch_ranked(sdb_corpus*, const double* queries, uint32_t nq, uint32_t k,
                                          sdb_screen screen, int streaming, uint32_t cand_cap, int score_all,
                                          float* out_qf, double* out_qmag, uint32_t* out_qu, int8_t* out_q8,
@@ -411,8 +415,13 @@ sdb_status sdb_corpus_project(sdb_corpus*, const double* query, int fn, double* 
  * on the same screens with the query's centred copy un-negated (k <= 256), SDB_FN_DOT in either direction on a COSINE
  * or EUCLIDEAN corpus on the bf16 tensor-core screen (maximum / minimum inner product, k <= 256: the screens score the
  * dot with q for DESC and with -q for ASC, never on the int8 copy, with the F32 stream as the ladder's last rung),
- * HAMMING / JACCARD DESC on their own corpus on the count path (k <= 256, exact counts); every other (fn, order) is
- * ranked by the exact kernel.
+ * SDB_COSINE / SDB_FN_SIMILARITY_COSINE / SDB_EUCLIDEAN in the other orders on a COSINE or EUCLIDEAN corpus with its
+ * bf16 copy (cosine distance DESC and similarity ASC on either; cosine distance ASC and similarity DESC on EUCLIDEAN;
+ * euclidean ASC on COSINE; euclidean DESC, farthest first, on either; k <= 256) on the screens in the view of the
+ * ranked function: the cosine score towards q or -q (the COSINE corpus' int8 copy included) or the euclidean score
+ * with the other metric's per-row norm and special rows, which finalize keeps beside the corpus' own (past 1024 such
+ * rows those views take the exact kernel), HAMMING / JACCARD DESC on their own corpus on the count path (k <= 256,
+ * exact counts); every other (fn, order) is ranked by the exact kernel.
  * Refusals: an unknown fn or order, or nq > 0 with NULL queries for a function that takes a query: SDB_EINVAL.
  * Tickets share the corpus' four slots with KNN tickets; sdb_knn_wait completes them; cancellation and
  * sdb_knn_last_stats work as for KNN.  Row-sharded columns are not served. */

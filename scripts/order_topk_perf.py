@@ -8,6 +8,8 @@
   * vector::dot DESC (maximum inner product, the bf16 screen + the dot proof) on the COSINE column and on a EUCLIDEAN
     one, each against sdb_knn_bruteforce on the same column and against the exact kernel (NONE_EXACT, --exact-max
     queries), with the survivors per query and the repaired / fallback counts;
+  * the cross views, each against the same column's KNN and the exact kernel like the dot rows: cosine distance DESC
+    and euclidean DESC (farthest first) on the COSINE column, similarity DESC and euclidean DESC on the EUCLIDEAN one;
   * the route without this call: sdb_corpus_project per query (every row's value copied to the host) and a host top-k
     (numpy argpartition + sort), timed on --project-max queries and scaled.
 
@@ -91,19 +93,20 @@ def main():
 
     summary = {"config": f"{a.n}x{a.dim} F32 synthetic", "k": k, "batch": B, "gpu": gpu_info()}
 
-    def dot_rows(col, column, t_knn):
-        """vector::dot DESC on col: the screened batch, the exact kernel on a few queries, parity on 10"""
-        t_dot, sp_dot = timed(lambda: col.order_topk(Q, k, "DOT", "DESC"), a.reps)
+    def dot_rows(col, column, t_knn, fn="DOT", order="DESC"):
+        """fn / order (vector::dot DESC by default) on col: the screened batch, the exact kernel on a few queries,
+        parity on 10"""
+        t_dot, sp_dot = timed(lambda: col.order_topk(Q, k, fn, order), a.reps)
         st = col.stats()
         Be = min(B, a.exact_max)
         col.set_screen("NONE_EXACT")
-        t_ex, sp_ex = timed(lambda: col.order_topk(Q[:Be], k, "DOT", "DESC"), a.reps)
-        ref = col.order_topk(Q[:10], k, "DOT", "DESC")
+        t_ex, sp_ex = timed(lambda: col.order_topk(Q[:Be], k, fn, order), a.reps)
+        ref = col.order_topk(Q[:10], k, fn, order)
         col.set_screen("AUTO")
-        got = col.order_topk(Q[:10], k, "DOT", "DESC")
-        summary[f"dot_desc_{column.lower()}_parity_10_vs_exact"] = all(u.tobytes() == v.tobytes()
-                                                                       for u, v in zip(got, ref))
-        emit({"fn": "DOT", "order": "DESC", "column": column, "batch": B, "order_qps": B / t_dot,
+        got = col.order_topk(Q[:10], k, fn, order)
+        summary[f"{fn.lower()}_{order.lower()}_{column.lower()}_parity_10_vs_exact"] = all(
+            u.tobytes() == v.tobytes() for u, v in zip(got, ref))
+        emit({"fn": fn, "order": order, "column": column, "batch": B, "order_qps": B / t_dot,
               "knn_qps": B / t_knn, "order_over_knn_time": t_dot / t_knn, "order_spread_ms": sp_dot,
               "exact_timed_queries": Be, "exact_qps": Be / t_ex, "exact_spread_ms": sp_ex,
               "screen_used": st["screen_used"], "screen_ms": st["screen_ms"], "total_ms": st["total_ms"],
@@ -133,6 +136,8 @@ def main():
     col.set_screen("AUTO")
     summary["cosine_desc_parity_10_vs_exact"] = all(u.tobytes() == v.tobytes() for u, v in zip(got, ref))
     dot_rows(col, "COSINE", t_knn)
+    dot_rows(col, "COSINE", t_knn, "COSINE", "DESC")
+    dot_rows(col, "COSINE", t_knn, "EUCLIDEAN", "DESC")
     col.close()
     del col
     torch.cuda.empty_cache()
@@ -143,6 +148,8 @@ def main():
         col.finalize()
         t_knn, _ = timed(lambda: col.knn(Q, k), a.reps)
         dot_rows(col, "EUCLIDEAN", t_knn)
+        dot_rows(col, "EUCLIDEAN", t_knn, "SIMILARITY_COSINE", "DESC")
+        dot_rows(col, "EUCLIDEAN", t_knn, "EUCLIDEAN", "DESC")
         col.close()
     del col
     torch.cuda.empty_cache()

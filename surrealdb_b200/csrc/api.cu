@@ -110,8 +110,11 @@ static std::vector<Rung> build_rungs(const Corpus* c, sdb_screen screen, uint32_
     scr = !screen_tc_available() ? SDB_SCREEN_SIMT_F32
                                  : (int8_ok && c->max_rel_qerr <= 0.02f ? SDB_SCREEN_TC_INT8 : SDB_SCREEN_TC_BF16);
   if (scr == SDB_SCREEN_TC_INT8 && !int8_ok) scr = SDB_SCREEN_TC_BF16;
-  // the int8 copy holds x / |x| and its integer threshold compare takes no per-row scale: dot batches start on bf16
-  if (scr == SDB_SCREEN_TC_INT8 && score_kind(c, rank) == Score::Dot) scr = SDB_SCREEN_TC_BF16;
+  // the int8 copy holds x / |x| and its integer threshold compare takes no per-row scale: only the cosine score on the
+  // own screening norm runs on it (towards q or -q, whose int8 copy is the negation of q's); dot batches and the
+  // other views start on bf16
+  const View v = view_of(c, rank);
+  if (scr == SDB_SCREEN_TC_INT8 && (v.sc != Score::Cosine || v.cross)) scr = SDB_SCREEN_TC_BF16;
   // (Lp corpora hold no bf16 copy: the f32 Lp screen, screen_lp.cu, is their only screen, for f32 and f64 rows)
   if (scr == SDB_SCREEN_TC_BF16 && (!screen_tc_available() || !c->d_bf16)) scr = SDB_SCREEN_SIMT_F32;
   // the SIMT screen streams f32 rows: an f64 Dot corpus is screened on the tensor cores or not at all, and so is a
@@ -120,6 +123,8 @@ static std::vector<Rung> build_rungs(const Corpus* c, sdb_screen screen, uint32_
     scr = SDB_SCREEN_NONE_EXACT;
   // (Count: the count path, enqueue_counted, or the exact kernel)
   if (c->special_overflow || k > 256 || f == Family::Count || f == Family::Exact) scr = SDB_SCREEN_NONE_EXACT;
+  // a view on the cross state whose special list overflowed
+  if (v.cross && c->xspecial_overflow) scr = SDB_SCREEN_NONE_EXACT;
   // a ranking the screens do not serve (screened_ranking): the exact kernel
   if (!screened_ranking(c, rank)) scr = SDB_SCREEN_NONE_EXACT;
   // MANHATTAN / CHEBYSHEV: a single query streams the rows once either way, and the exact kernel does it at the higher
@@ -300,14 +305,14 @@ static sdb_status copy_flags(const Scratch& s, const Run& r, cudaStream_t st) {
 static sdb_status enqueue_direct(Corpus* c, Ticket& t, const Run& r) {
   cudaStream_t st = t.stream;
   Scratch& s = c->sets[t.set];
-  const Score sc = score_kind(c, t.rank);
+  const View v = view_of(c, t.rank);
   SDB_TRY(scratch_for(c, s, r.nq, DIRECT_MAX_ROWS));
-  SDB_TRY(prep_queries(c, s, r.d_queries, r.nq, st, sc, t.rank.desc));
-  SDB_TRY(cand_begin(c, s, r.nq, SDB_SCREEN_NONE_EXACT, st, sc));
+  SDB_TRY(prep_queries(c, s, r.d_queries, r.nq, st, v, t.rank.desc));
+  SDB_TRY(cand_begin(c, s, r.nq, SDB_SCREEN_NONE_EXACT, st, v));
   SDB_TRY(cand_direct(c, s, r.filt, r.nq, st));
-  SDB_TRY(cand_rerank(c, s, r.filt, r.nq, st, false, t.rank.desc, sc));
+  SDB_TRY(cand_rerank(c, s, r.filt, r.nq, st, false, t.rank.desc, v));
   SDB_TRY(cand_final(c, s, r.filt, r.nq, t.k, t.row_base, r.d_out_rows, r.d_out_dist, r.d_out_count, st,
-                     t.rank.desc, sc));
+                     t.rank.desc, v));
   return copy_flags(s, r, st);
 }
 
@@ -362,10 +367,10 @@ static sdb_status enqueue_counted(Corpus* c, Ticket& t, const Run& r, Enqueued* 
   e->n_passes = 1;
   SDB_CUDA(cudaEventRecord(t.ev_begin, st));
   trace_mark(ctx, t, "begin", st);
-  const Score sc = score_kind(c, t.rank);
+  const View v = view_of(c, t.rank);
   SDB_TRY(scratch_for(c, s, nq, std::max(4096u, count_ranges(c, nq, k) * k)));
-  SDB_TRY(prep_queries(c, s, r.d_queries, nq, st, sc, t.rank.desc));
-  SDB_TRY(cand_begin(c, s, nq, SDB_SCREEN_NONE_EXACT, st, sc));
+  SDB_TRY(prep_queries(c, s, r.d_queries, nq, st, v, t.rank.desc));
+  SDB_TRY(cand_begin(c, s, nq, SDB_SCREEN_NONE_EXACT, st, v));
   if (c->last_main && c->last_main != t.ev_main) SDB_CUDA(cudaStreamWaitEvent(st, c->last_main, 0));
   SDB_CUDA(cudaEventRecord(t.ev_screen0, st));
   if ((t.cancel && *t.cancel) || ctx_cancelled(ctx)) {
@@ -379,7 +384,7 @@ static sdb_status enqueue_counted(Corpus* c, Ticket& t, const Run& r, Enqueued* 
   SDB_CUDA(cudaEventRecord(t.ev_screen1, st));
   trace_mark(ctx, t, "counted", st);
   SDB_TRY(cand_final(c, s, r.filt, nq, k, t.row_base, r.d_out_rows, r.d_out_dist, r.d_out_count, st, t.rank.desc,
-                     sc));
+                     v));
   SDB_TRY(copy_flags(s, r, st));
   SDB_CUDA(cudaEventRecord(t.ev_end, st));
   trace_mark(ctx, t, "end", st);
@@ -391,7 +396,7 @@ static sdb_status enqueue_screened(Corpus* c, Ticket& t, const Run& r, Enqueued*
   cudaStream_t st = t.stream;
   Scratch& s = c->sets[t.set];
   const uint32_t nq = r.nq, k = t.k;
-  const Score sc = score_kind(c, t.rank);
+  const View v = view_of(c, t.rank);
   // HAMMING: AUTO ranks a batch of one query with the exact kernel, which streams the rows once at the higher rate
   // (DESIGN.md section 5); an explicit screen request still counts it.  JACCARD's exact kernel is O(D^2) per row: the
   // count path takes a single query too
@@ -406,7 +411,7 @@ static sdb_status enqueue_screened(Corpus* c, Ticket& t, const Run& r, Enqueued*
   if (rungs.empty()) {  // exact-only: the exact kernel needs the prepared queries (f64 copy, |q|, flags)
     e->screen = SDB_SCREEN_NONE_EXACT;
     SDB_TRY(scratch_for(c, s, nq, 4096));
-    SDB_TRY(prep_queries(c, s, r.d_queries, nq, st, sc, t.rank.desc));
+    SDB_TRY(prep_queries(c, s, r.d_queries, nq, st, v, t.rank.desc));
     SDB_CUDA(cudaEventRecord(t.ev_screen0, st));
     SDB_CUDA(cudaEventRecord(t.ev_screen1, st));
     SDB_CUDA(cudaMemsetAsync(r.d_out_count, 0, sizeof(uint32_t) * nq, st));
@@ -424,8 +429,8 @@ static sdb_status enqueue_screened(Corpus* c, Ticket& t, const Run& r, Enqueued*
   const bool int8 = rs == SDB_SCREEN_TC_INT8;
   SDB_TRY(scratch_for(c, s, nq, rg.cap));
   const uint32_t cap = s.sc_cap;
-  SDB_TRY(prep_queries(c, s, r.d_queries, nq, st, sc, t.rank.desc));
-  SDB_TRY(cand_begin(c, s, nq, (int)rs, st, sc));
+  SDB_TRY(prep_queries(c, s, r.d_queries, nq, st, v, t.rank.desc));
+  SDB_TRY(cand_begin(c, s, nq, (int)rs, st, v));
   // Screens are persistent one-CTA-per-SM kernels: two of them in flight on different streams would split the SMs,
   // run in two waves and starve the refiners of the CTAs that are not resident yet.  So the screen of this batch waits
   // for the end of the previous batch's screen -- only the TAIL of the previous batch overlaps with it.
@@ -436,17 +441,17 @@ static sdb_status enqueue_screened(Corpus* c, Ticket& t, const Run& r, Enqueued*
     PassDesc p0, pm;
     build_stream_passes(c->n, cap, k, &p0, &pm);
     if (p0.count && !pm.count) {  // the whole corpus fits the lists: score everything once
-      SDB_TRY(screen_tc_pass(c, s, r.filt, nq, k, p0, int8, 0, st, sc));
+      SDB_TRY(screen_tc_pass(c, s, r.filt, nq, k, p0, int8, 0, st, v));
       SDB_CUDA(cudaEventRecord(t.ev_main, st));
       c->last_main = t.ev_main;
       if (r.tap) SDB_TRY(tap_gathered(s, r.tap, nq, 0u, st));
       SDB_TRY(cand_select(c, s, nq, k, int8, 0u, false, st));
       e->n_passes++;
     } else if (pm.count) {
-      SDB_TRY(screen_tc_pass(c, s, r.filt, nq, k, p0, int8, 3, st, sc));  // probe: chunk maxima of a few tiles
+      SDB_TRY(screen_tc_pass(c, s, r.filt, nq, k, p0, int8, 3, st, v));  // probe: chunk maxima of a few tiles
       SDB_TRY(cand_seed_from_probe(c, s, nq, k, p0.count, st));       // thresholds + histogram geometry
       trace_mark(ctx, t, "seeded", st);
-      SDB_TRY(screen_tc_pass(c, s, r.filt, nq, k, pm, int8, 2, st, sc));  // the streaming launch over every tile
+      SDB_TRY(screen_tc_pass(c, s, r.filt, nq, k, pm, int8, 2, st, v));  // the streaming launch over every tile
       trace_mark(ctx, t, "main_end", st);
       SDB_CUDA(cudaEventRecord(t.ev_main, st));
       c->last_main = t.ev_main;
@@ -463,9 +468,9 @@ static sdb_status enqueue_screened(Corpus* c, Ticket& t, const Run& r, Enqueued*
         set_error("query cancelled");
         return SDB_ECANCELLED;
       }
-      if (tc) SDB_TRY(screen_tc_pass(c, s, r.filt, nq, k, p, int8, first_pass ? 0 : 1, st, sc));
+      if (tc) SDB_TRY(screen_tc_pass(c, s, r.filt, nq, k, p, int8, first_pass ? 0 : 1, st, v));
       else if (family(c) == Family::Lp) SDB_TRY(screen_lp_pass(c, s, r.filt, nq, p, st));
-      else SDB_TRY(screen_simt_pass(c, s, r.filt, nq, p, st, sc));
+      else SDB_TRY(screen_simt_pass(c, s, r.filt, nq, p, st, v));
       if (r.tap) SDB_TRY(tap_gathered(s, r.tap, nq, tc ? s.last_slots : 0u, st));
       SDB_TRY(cand_select(c, s, nq, k, int8, tc ? s.last_slots : 0u, false, st));
       first_pass = false;
@@ -481,17 +486,17 @@ static sdb_status enqueue_screened(Corpus* c, Ticket& t, const Run& r, Enqueued*
   static const bool no_refine = getenv("SDB_NO_REFINE") != nullptr;
   bool refined = false;
   if (tc && c->exact && !no_refine) {
-    SDB_TRY(cand_refine(c, s, nq, st, sc));
+    SDB_TRY(cand_refine(c, s, nq, st, v));
     if (r.tap) SDB_TRY(tap_list(s, nq, &r.tap->list_r, nullptr, st));
     SDB_TRY(cand_select(c, s, nq, k, false, 0u, false, st, 1));
     refined = true;
     trace_mark(ctx, t, "refined", st);
   }
-  if (r.filt.bits) SDB_TRY(cand_add_specials(c, s, r.filt, nq, st));  // each query re-ranks its passing special rows
-  SDB_TRY(cand_rerank(c, s, r.filt, nq, st, refined, t.rank.desc, sc));
+  if (r.filt.bits) SDB_TRY(cand_add_specials(c, s, r.filt, nq, st, v));  // each query re-ranks its passing special rows
+  SDB_TRY(cand_rerank(c, s, r.filt, nq, st, refined, t.rank.desc, v));
   trace_mark(ctx, t, "reranked", st);
   SDB_TRY(cand_final(c, s, r.filt, nq, k, t.row_base, r.d_out_rows, r.d_out_dist, r.d_out_count, st, t.rank.desc,
-                     sc));
+                     v));
   trace_mark(ctx, t, "final", st);
   SDB_TRY(copy_flags(s, r, st));
   SDB_CUDA(cudaEventRecord(t.ev_end, st));
@@ -531,9 +536,9 @@ static sdb_status finish_local(Corpus* c, Ticket& t, uint32_t* n_fallback, bool*
   *repaired = false;
   *n_fallback = 0;
   SDB_CUDA(cudaEventSynchronize(t.ev_end));
-  // vector::dot batches were ranked by the exact kernel, which reports a cancel raised while a batch is in flight (it
-  // polls before every query); on the screens they still report it, here
-  if (dot_ranking(c, t.rank) && nq && k && ((t.cancel && *t.cancel) || ctx_cancelled(ctx))) {
+  // vector::dot and the cross views were ranked by the exact kernel, which reports a cancel raised while a batch is in
+  // flight (it polls before every query); on the screens they still report it, here
+  if ((dot_ranking(c, t.rank) || cross_ranking(c, t.rank)) && nq && k && ((t.cancel && *t.cancel) || ctx_cancelled(ctx))) {
     set_error("query cancelled");
     return SDB_ECANCELLED;
   }
@@ -554,7 +559,7 @@ static sdb_status finish_local(Corpus* c, Ticket& t, uint32_t* n_fallback, bool*
     build_rungs(c, c->screen, k, nq, t.rank, &first);
     c->rung_scr = first;
     c->rung_k = k;
-    c->rung_score = (int)score_kind(c, t.rank);
+    c->rung_view = view_key(view_of(c, t.rank));
     c->rung = t.rung;
   }
   // ---- what the batch's rung could not prove ----
@@ -766,7 +771,7 @@ static sdb_status submit_locked(Corpus* c, Ticket* t, const double* d_queries, u
   t->n_repaired = 0;
   sdb_screen first, first_scr;
   const std::vector<Rung> rungs = build_rungs(c, c->screen, k, nq, rank, &first);
-  t->rung = (c->rung_scr == first && c->rung_k == k && c->rung_score == (int)score_kind(c, rank) &&
+  t->rung = (c->rung_scr == first && c->rung_k == k && c->rung_view == view_key(view_of(c, rank)) &&
              c->rung < n_batch_rungs(rungs))
                 ? c->rung
                 : 0;
@@ -1644,7 +1649,8 @@ static sdb_status debug_screen_batch(sdb_corpus* c, const double* queries, uint3
                       : f == Family::Centred ? tc
                       : f == Family::Lp      ? screen == SDB_SCREEN_SIMT_F32
                                              : false;
-  if (!c->finalized || !served || (int8 && !c->d_i8) || c->special_overflow || !c->n) {
+  if (!c->finalized || !served || (int8 && !c->d_i8) || c->special_overflow || !c->n ||
+      (view_of(c, rank).cross && c->xspecial_overflow)) {
     set_error("sdb_debug_screen_batch: needs a finalized, non-empty F32 cosine / euclidean corpus, an F64 one with "
               "screen copies and a tensor-core screen (int8: cosine), a PEARSON one with screen copies and a "
               "tensor-core screen, or a MANHATTAN / CHEBYSHEV / MINKOWSKI (integer order 1 .. 8) one with SIMT_F32");
@@ -1671,7 +1677,7 @@ static sdb_status debug_screen_batch(sdb_corpus* c, const double* queries, uint3
   t->n_direct = 0;
   t->permuted = false;
   t->rank = rank;
-  const Score sc = score_kind(c, rank);
+  const View v = view_of(c, rank);
   if (filters) {
     const uint32_t* bits = nullptr;
     std::vector<uint64_t> rows_per_filter;
@@ -1701,11 +1707,11 @@ static sdb_status debug_screen_batch(sdb_corpus* c, const double* queries, uint3
     SDB_CUDA(cudaMemcpyAsync(d_q, queries, sizeof(double) * (size_t)nq * c->dim, cudaMemcpyHostToDevice, st));
     if (score_all) {  // one pass-0 launch over every tile (SIMT: tau stays -inf), nothing selected
       const PassDesc all{1u, 0u, (uint32_t)(n_pad / TILE_ROWS), 0u};
-      SDB_TRY(prep_queries(c, s, d_q, nq, st, sc, rank.desc));
-      SDB_TRY(cand_begin(c, s, nq, (int)screen, st, sc));
-      SDB_TRY(tc                ? screen_tc_pass(c, s, t->filt, nq, k, all, int8, 0, st, sc)
+      SDB_TRY(prep_queries(c, s, d_q, nq, st, v, rank.desc));
+      SDB_TRY(cand_begin(c, s, nq, (int)screen, st, v));
+      SDB_TRY(tc                ? screen_tc_pass(c, s, t->filt, nq, k, all, int8, 0, st, v)
               : f == Family::Lp ? screen_lp_pass(c, s, t->filt, nq, all, st)
-                                : screen_simt_pass(c, s, t->filt, nq, all, st, sc));
+                                : screen_simt_pass(c, s, t->filt, nq, all, st, v));
       SDB_TRY(tap_list(s, nq, &tap.list_a, &tap.cnt_a, st));
       tap.gathered = tap.cnt_a;
       return SDB_OK;
@@ -1761,7 +1767,7 @@ static sdb_status debug_screen_batch(sdb_corpus* c, const double* queries, uint3
     if (rc == SDB_OK && cudaStreamSynchronize(st) != cudaSuccess) rc = SDB_ECUDA;
     if (rc == SDB_OK) {
       // (filtered: the passing special rows are in the stage-B list)
-      const uint32_t n_special = score_all || filters ? 0u : c->n_special;
+      const uint32_t n_special = score_all || filters ? 0u : view_n_special(c, view_of(c, rank));
       auto bits = [](float v) {
         uint32_t u;
         memcpy(&u, &v, 4);
@@ -2035,7 +2041,7 @@ sdb_status sdb_corpus_project(sdb_corpus* c, const double* query, int fn, double
     if (query) SDB_CUDA(cudaMemcpyAsync(d_q, query, sizeof(double) * c->dim, cudaMemcpyHostToDevice, st));
     else SDB_CUDA(cudaMemsetAsync(d_q, 0, sizeof(double) * c->dim, st));
     SDB_TRY(scratch_for(c, s, 1, 4096));
-    SDB_TRY(prep_queries(c, s, d_q, 1, st, score_kind(c, Ranking()), false));
+    SDB_TRY(prep_queries(c, s, d_q, 1, st, view_of(c, Ranking()), false));
     SDB_TRY(exact_project(c, fn, s.d_q64, s.d_qmag, s.d_qflags, d_vals, st));
     SDB_CUDA(cudaMemcpyAsync(out, d_vals, sizeof(double) * c->n, cudaMemcpyDeviceToHost, st));
     return SDB_OK;

@@ -14,7 +14,7 @@ namespace sdb {
 
 // ------------------------------------------------------------------------------------------------
 // NEG: the f32 / bf16 screen copies (and the measured residual qbferr) are those of -q, negated in f64 before any
-// rounding (Score::Dot, ascending); qmag and the flags are those of q, which the negation does not change
+// rounding (View::neg); qmag and the flags are those of q, which the negation does not change
 template <bool NEG = false>
 __global__ void prep_queries_kernel(const double* __restrict__ q64, uint32_t dim, uint32_t dim_pad, int metric,
                                     float* __restrict__ q32, __nv_bfloat16* __restrict__ qbf, double* __restrict__ qmag,
@@ -219,7 +219,7 @@ __global__ void cand_begin_kernel(float* __restrict__ tau, uint32_t* __restrict_
                                   const double* __restrict__ qmag, const float* __restrict__ q8scale,
                                   const float* __restrict__ q8err, const float* __restrict__ qbferr, uint32_t nq,
                                   int screen, int metric, uint32_t dim, float max_rel_qerr, float i8_scale,
-                                  float bf16_rel_err, float max_norm, int exact, int f64_rows) {
+                                  float bf16_rel_err, float max_norm, int exact, int f64_rows, int far) {
   const uint32_t q = blockIdx.x * blockDim.x + threadIdx.x;
   if (q == 0) {
     stat[0] = 0;
@@ -257,6 +257,13 @@ __global__ void cand_begin_kernel(float* __restrict__ tau, uint32_t* __restrict_
     mg = 2.1 * eps;
     hi = qm * qm * 1.01 + eps + 1e-30;
     lo = -(mn * mn + 2.0 * qm * mn) * 1.01 - eps - 1e-30;
+    // EuclidFar: |x|^2 - 2 x.q = d^2 - |q|^2 lies in [-|q|^2, M^2 + 2 |q| M], and its error is Euclid's (the same two
+    // terms, 2 acc and |x|^2, with the sign of one flipped)
+    if (far) {
+      const double t = hi;
+      hi = -lo;
+      lo = -t;
+    }
   }
   if (!exact) mg = 0.0;
   if (!(qm > 0.0) || !isfinite(qm) || !isfinite(mg) || !isfinite(hi) || !isfinite(lo)) {  // exact path anyway (qflags)
@@ -484,8 +491,8 @@ __global__ void cand_begin_dot_kernel(float* __restrict__ tau, uint32_t* __restr
               __double2float_ru(hi));
 }
 
-sdb_status cand_begin(const Corpus* c, Scratch& s, uint32_t nq, int screen, cudaStream_t st, Score sc) {
-  if (sc == Score::Dot) {
+sdb_status cand_begin(const Corpus* c, Scratch& s, uint32_t nq, int screen, cudaStream_t st, const View& v) {
+  if (v.sc == Score::Dot) {
     cand_begin_dot_kernel<<<(nq + 255) / 256, 256, 0, st>>>(s.d_tau, s.d_cand_cnt, s.d_flags, s.d_stat, s.d_bscale,
                                                             s.d_beps, s.d_margin, s.d_margin2, s.d_beps2, s.d_tau2,
                                                             s.d_qlow, s.d_qcap, s.d_qmag, s.d_qbferr, nq, screen,
@@ -521,9 +528,21 @@ sdb_status cand_begin(const Corpus* c, Scratch& s, uint32_t nq, int screen, cuda
                                                           s.d_qlow, s.d_qcap, s.d_qmag, s.d_q8scale, s.d_q8err,
                                                           s.d_qbferr, nq, screen, (int)SDB_COSINE, c->dim,
                                                           c->max_rel_qerr, c->i8_scale, c->bf16_rel_err, c->max_norm,
-                                                          c->exact ? 1 : 0, 1);
+                                                          c->exact ? 1 : 0, 1, 0);
       break;
-    case Family::Dot:
+    case Family::Dot: {
+      // the bound's form is the view's score, not the corpus metric: Cosine (relative, with the F64 rows' underflow
+      // term), or Euclid / EuclidFar (absolute, with max_norm -- an upper bound of |x| over the own screened rows,
+      // which include the cross view's)
+      const int form = v.sc == Score::Cosine ? (int)SDB_COSINE : (int)SDB_EUCLIDEAN;
+      cand_begin_kernel<<<(nq + 255) / 256, 256, 0, st>>>(s.d_tau, s.d_cand_cnt, s.d_flags, s.d_stat, s.d_bscale,
+                                                          s.d_beps, s.d_margin, s.d_margin2, s.d_beps2, s.d_tau2,
+                                                          s.d_qlow, s.d_qcap, s.d_qmag, s.d_q8scale, s.d_q8err,
+                                                          s.d_qbferr, nq, screen, form, c->dim, c->max_rel_qerr,
+                                                          c->i8_scale, c->bf16_rel_err, c->max_norm, c->exact ? 1 : 0,
+                                                          c->dtype == SDB_F64 ? 1 : 0, v.sc == Score::EuclidFar);
+      break;
+    }
     case Family::Count:  // (Count, Exact: the reset of tau, counts, flags and stat; their bounds go unused)
     case Family::Exact:
       cand_begin_kernel<<<(nq + 255) / 256, 256, 0, st>>>(s.d_tau, s.d_cand_cnt, s.d_flags, s.d_stat, s.d_bscale,
@@ -531,7 +550,7 @@ sdb_status cand_begin(const Corpus* c, Scratch& s, uint32_t nq, int screen, cuda
                                                           s.d_qlow, s.d_qcap, s.d_qmag, s.d_q8scale, s.d_q8err,
                                                           s.d_qbferr, nq, screen, (int)c->metric, c->dim,
                                                           c->max_rel_qerr, c->i8_scale, c->bf16_rel_err, c->max_norm,
-                                                          c->exact ? 1 : 0, c->dtype == SDB_F64 ? 1 : 0);
+                                                          c->exact ? 1 : 0, c->dtype == SDB_F64 ? 1 : 0, 0);
       break;
   }
   count_launch(c->ctx);
@@ -600,8 +619,8 @@ sdb_status scratch_for(const Corpus* c, Scratch& s, uint32_t nq, uint32_t cap) {
   return SDB_OK;
 }
 
-sdb_status prep_queries(const Corpus* c, Scratch& s, const double* d_queries, uint32_t nq, cudaStream_t st, Score sc,
-                        bool desc) {
+sdb_status prep_queries(const Corpus* c, Scratch& s, const double* d_queries, uint32_t nq, cudaStream_t st,
+                        const View& v, bool desc) {
   // d_queries may alias s.d_q64
   if (d_queries != s.d_q64)
     SDB_CUDA(cudaMemcpyAsync(s.d_q64, d_queries, sizeof(double) * (size_t)nq * c->dim, cudaMemcpyDeviceToDevice, st));
@@ -610,10 +629,13 @@ sdb_status prep_queries(const Corpus* c, Scratch& s, const double* d_queries, ui
   if (f == Family::Centred)
     prep_queries_pearson_kernel<<<nq_pad, 128, 0, st>>>(s.d_q64, c->dim, c->dim_pad, s.d_q32, s.d_qbf16, s.d_qmag,
                                                         s.d_qmom, s.d_qflags, s.d_qbferr, nq, desc);
-  else if (sc == Score::Dot) {  // (COSINE's query rule: a zero or non-finite |q| takes the exact kernel)
-    auto prep = desc ? prep_queries_kernel<false> : prep_queries_kernel<true>;
-    prep<<<nq_pad, 128, 0, st>>>(s.d_q64, c->dim, c->dim_pad, (int)SDB_COSINE, s.d_q32, s.d_qbf16, s.d_qmag,
-                                 s.d_qflags, s.d_qbferr, nq);
+  else if (v.neg || v.sc == Score::Dot || v.cross) {
+    // the query rule of the view's score: Cosine and Dot (COSINE's) send a zero or non-finite |q| to the exact kernel
+    // -- a cosine view of a EUCLIDEAN corpus with |q| = 0 is NaN for every row --, Euclid / EuclidFar a non-finite one
+    auto prep = v.neg ? prep_queries_kernel<true> : prep_queries_kernel<false>;
+    const int rule = v.sc == Score::Euclid || v.sc == Score::EuclidFar ? (int)SDB_EUCLIDEAN : (int)SDB_COSINE;
+    prep<<<nq_pad, 128, 0, st>>>(s.d_q64, c->dim, c->dim_pad, rule, s.d_q32, s.d_qbf16, s.d_qmag, s.d_qflags,
+                                 s.d_qbferr, nq);
   } else
     prep_queries_kernel<<<nq_pad, 128, 0, st>>>(s.d_q64, c->dim, c->dim_pad, (int)c->metric, s.d_q32, s.d_qbf16,
                                                 s.d_qmag, s.d_qflags, s.d_qbferr, nq);
@@ -692,10 +714,12 @@ __global__ void __launch_bounds__(256) cand_add_specials_kernel(Cand* __restrict
     }
   }
 }
-sdb_status cand_add_specials(const Corpus* c, Scratch& s, const FiltArg& filt, uint32_t nq, cudaStream_t st) {
-  if (!c->n_special) return SDB_OK;
-  cand_add_specials_kernel<<<nq, 256, 0, st>>>(s.d_cand, s.d_cand_cnt, s.d_flags, s.sc_cap, c->d_special,
-                                               c->n_special, filt);
+sdb_status cand_add_specials(const Corpus* c, Scratch& s, const FiltArg& filt, uint32_t nq, cudaStream_t st,
+                             const View& v) {
+  const uint32_t n_sp = view_n_special(c, v);
+  if (!n_sp) return SDB_OK;
+  cand_add_specials_kernel<<<nq, 256, 0, st>>>(s.d_cand, s.d_cand_cnt, s.d_flags, s.sc_cap, view_special(c, v), n_sp,
+                                               filt);
   count_launch(c->ctx);
   SDB_CUDA(cudaGetLastError());
   return SDB_OK;
@@ -1012,7 +1036,7 @@ sdb_status cand_select(const Corpus* c, Scratch& s, uint32_t nq, uint32_t k, boo
 // fl32(x_i - m1), against the f32 copy of -dq: the rounding is relative per element, as for f64 cosine rows, so the
 // same stage-B bound holds for dx.  (Subtracting fl32(m1) in f32 would err by 2^-24 |m1| per element, absolutely:
 // unbounded relative to |dx| for rows whose offset dwarfs their spread.)
-// S: the score (score_kind), from the f32 dot a: a / |x|, 2 a - |x|^2 or a itself
+// S: the score (View::sc), from the f32 dot a: a / |x|, 2 a - |x|^2, a itself or 2 a + |x|^2
 template <typename T, Score S, bool CENTRED = false>
 __global__ void __launch_bounds__(128) cand_refine_f32_kernel(const T* __restrict__ rows, uint32_t dim,
                                                                const float* __restrict__ snorm,
@@ -1080,6 +1104,9 @@ __global__ void __launch_bounds__(128) cand_refine_f32_kernel(const T* __restric
       if constexpr (S == Score::Dot) {
         cq[e0].score = a0;
         if (has1) cq[e0 + 1].score = a1;
+      } else if constexpr (S == Score::EuclidFar) {
+        cq[e0].score = fmaf(2.f, a0, __ldg(snorm + r0));
+        if (has1) cq[e0 + 1].score = fmaf(2.f, a1, __ldg(snorm + r1));
       } else {
         const float s0 = __ldg(snorm + r0);
         cq[e0].score = S == Score::Cosine ? a0 * s0 : fmaf(2.f, a0, -s0);
@@ -1092,16 +1119,16 @@ __global__ void __launch_bounds__(128) cand_refine_f32_kernel(const T* __restric
   }
 }
 template <Score S>
-static void refine_dot(const Corpus* c, Scratch& s, uint32_t nq, cudaStream_t st) {
+static void refine_dot(const Corpus* c, Scratch& s, uint32_t nq, cudaStream_t st, const float* snorm) {
   const dim3 grid(nq, 8);
   if (c->dtype == SDB_F32)
-    cand_refine_f32_kernel<float, S><<<grid, 128, 0, st>>>((const float*)c->d_rows.get(), c->dim, c->d_snorm, s.d_q32,
+    cand_refine_f32_kernel<float, S><<<grid, 128, 0, st>>>((const float*)c->d_rows.get(), c->dim, snorm, s.d_q32,
                                                            s.d_cand, s.d_cand_cnt, s.sc_cap, nullptr);
   else
-    cand_refine_f32_kernel<double, S><<<grid, 128, 0, st>>>((const double*)c->d_rows.get(), c->dim, c->d_snorm,
-                                                            s.d_q32, s.d_cand, s.d_cand_cnt, s.sc_cap, nullptr);
+    cand_refine_f32_kernel<double, S><<<grid, 128, 0, st>>>((const double*)c->d_rows.get(), c->dim, snorm, s.d_q32,
+                                                            s.d_cand, s.d_cand_cnt, s.sc_cap, nullptr);
 }
-sdb_status cand_refine(const Corpus* c, Scratch& s, uint32_t nq, cudaStream_t st, Score sc) {
+sdb_status cand_refine(const Corpus* c, Scratch& s, uint32_t nq, cudaStream_t st, const View& v) {
   const dim3 grid(nq, 8);  // 128-thread blocks (register budget beside a resident screen CTA)
   const float* f32_rows = (const float*)c->d_rows.get();
   const double* f64_rows = (const double*)c->d_rows.get();
@@ -1115,9 +1142,13 @@ sdb_status cand_refine(const Corpus* c, Scratch& s, uint32_t nq, cudaStream_t st
             f64_rows, c->dim, c->d_snorm, s.d_q32, s.d_cand, s.d_cand_cnt, s.sc_cap, c->d_mom);
       break;
     case Family::Dot:
-      if (sc == Score::Cosine) refine_dot<Score::Cosine>(c, s, nq, st);
-      else if (sc == Score::Euclid) refine_dot<Score::Euclid>(c, s, nq, st);
-      else refine_dot<Score::Dot>(c, s, nq, st);
+    {
+      const float* sn = view_snorm(c, v);
+      if (v.sc == Score::Cosine) refine_dot<Score::Cosine>(c, s, nq, st, sn);
+      else if (v.sc == Score::Euclid) refine_dot<Score::Euclid>(c, s, nq, st, sn);
+      else if (v.sc == Score::EuclidFar) refine_dot<Score::EuclidFar>(c, s, nq, st, sn);
+      else refine_dot<Score::Dot>(c, s, nq, st, sn);
+    }
       break;
     default: break;  // stage B follows the tensor-core screens (Dot, Centred) only
   }
@@ -1140,7 +1171,8 @@ struct RerankOut {  // nq x stride results: the value's key, the value, the row
   double* dist;
   uint32_t* row;
   uint32_t stride;
-  bool desc;  // the descending rankings (cosine_desc: the value is the cosine similarity): keyed descending
+  bool desc;  // the descending rankings: keyed descending
+  bool sim;   // COSINE steps: the value is the cosine similarity, not the distance (View::sim)
 };
 __device__ __forceinline__ void rr_store(const RerankOut& out, uint32_t q, uint32_t e, uint32_t row, double d) {
   const size_t o = (size_t)q * out.stride + e;
@@ -1148,12 +1180,13 @@ __device__ __forceinline__ void rr_store(const RerankOut& out, uint32_t q, uint3
   out.dist[o] = d;
   out.row[o] = row;
 }
-static RerankOut rr_out(const Scratch& s, bool desc = false) {
-  return RerankOut{s.d_rr_key, s.d_rr_dist, s.d_rr_row, s.rr_stride, desc};
+static RerankOut rr_out(const Scratch& s, bool desc = false, bool sim = false) {
+  return RerankOut{s.d_rr_key, s.d_rr_dist, s.d_rr_row, s.rr_stride, desc, sim};
 }
 
-// the COSINE / EUCLIDEAN finish of one entry (sim: COSINE's similarity instead of its distance; DOT: vector::dot, whose
-// entries accumulated the cosine steps on either metric)
+// the COSINE / EUCLIDEAN finish of one entry (sim: the cosine similarity instead of the distance; DOT: vector::dot,
+// whose entries accumulated the cosine steps).  cosine: the entries accumulated the cosine steps, whatever the corpus
+// metric (a cosine view of a EUCLIDEAN corpus finishes with its |x|, d_mag, as a COSINE corpus does)
 template <bool DOT = false>
 __device__ __forceinline__ double dot_finish(bool cosine, bool sim, const RefSum& s, const double* mag, uint32_t row,
                                              double qm, bool q_nan) {
@@ -1167,7 +1200,8 @@ __device__ __forceinline__ double dot_finish(bool cosine, bool sim, const RefSum
 // rows 32 columns at a time: 32 coalesced 128-byte row segments are requested back to back (all in flight before the
 // first is consumed -- the kernel is bound by the latency of these gathers, not by the f64 arithmetic), transposed
 // through shared memory, and every lane then accumulates ITS row strictly left to right.
-// DOT (Score::Dot): metric is SDB_COSINE (the dot's steps) and the entries finish as vector::dot; so in the others.
+// metric: the view's steps (SDB_COSINE or SDB_EUCLIDEAN), not the corpus metric.  DOT (Score::Dot): metric is
+// SDB_COSINE (the dot's steps) and the entries finish as vector::dot; so in the others.
 constexpr uint32_t RR_WARPS = 4, RR_COLS = 32;
 template <typename T, bool DOT = false>
 __global__ void __launch_bounds__(RR_WARPS * 32) cand_rerank_kernel(
@@ -1218,7 +1252,7 @@ __global__ void __launch_bounds__(RR_WARPS * 32) cand_rerank_kernel(
         __syncwarp();
       }
     }
-    if (my_row != NO_ROW) rr_store(out, q, e, my_row, dot_finish<DOT>(metric == SDB_COSINE, out.desc, acc, mag, my_row, qm, q_nan));
+    if (my_row != NO_ROW) rr_store(out, q, e, my_row, dot_finish<DOT>(metric == SDB_COSINE, out.sim, acc, mag, my_row, qm, q_nan));
   }
 }
 
@@ -1297,7 +1331,7 @@ __global__ void __launch_bounds__(RR_WARPS * 32) cand_rerank_v4_kernel(
         __syncwarp();
       }
     }
-    if (my_row != NO_ROW) rr_store(out, q, e, my_row, dot_finish<DOT>(metric == SDB_COSINE, out.desc, acc, mag, my_row, qm, q_nan));
+    if (my_row != NO_ROW) rr_store(out, q, e, my_row, dot_finish<DOT>(metric == SDB_COSINE, out.sim, acc, mag, my_row, qm, q_nan));
   }
 }
 constexpr size_t RRV_SMEM = sizeof(double) * QCHUNK + sizeof(float) * RR_WARPS * 32 * RRV_STRIDE;  // 75.8 KB
@@ -1310,8 +1344,8 @@ constexpr size_t RRV_SMEM = sizeof(double) * QCHUNK + sizeof(float) * RR_WARPS *
 // (the staged variant's 6 KB per warp let only two warps per SM in, and the re-rank took 0.58 ms instead of 0.1 ms
 // whenever it overlapped a screen -- SDB_TRACE timeline, round 2).  Every lane streams its own row (16-byte loads; the
 // second half of each 32-byte sector comes from L1) and reads the query from global memory (one address per half-warp).
-// f64 rows stream as double2 (16-byte) loads when the row length is even.  M: SDB_COSINE, SDB_EUCLIDEAN or SDB_FN_DOT
-// (Score::Dot on either metric).
+// f64 rows stream as double2 (16-byte) loads when the row length is even.  M: the view's steps, SDB_COSINE,
+// SDB_EUCLIDEAN or SDB_FN_DOT (Score::Dot on either metric).
 template <typename T, int M>
 __global__ void __launch_bounds__(128) cand_rerank_packed_kernel(
     const T* __restrict__ rows, uint32_t dim, const double* __restrict__ mag, const double* __restrict__ q64,
@@ -1358,7 +1392,7 @@ __global__ void __launch_bounds__(128) cand_rerank_packed_kernel(
     } else {
       for (uint32_t j = 0; j < dim; j++) ref.step(acc, (double)__ldg(x + j), __ldg(qv + j));
     }
-    rr_store(out, q, e, my_row, dot_finish<M == SDB_FN_DOT>(M == SDB_COSINE, out.desc, acc, mag, my_row, qm, q_nan));
+    rr_store(out, q, e, my_row, dot_finish<M == SDB_FN_DOT>(M == SDB_COSINE, out.sim, acc, mag, my_row, qm, q_nan));
   }
 }
 
@@ -1437,46 +1471,49 @@ static void rerank_entry(const Corpus* c, Scratch& s, uint32_t nq, uint32_t n_sp
 }
 
 template <typename T>
-static void rerank_packed(const Corpus* c, Scratch& s, uint32_t nq, uint32_t n_sp, bool desc, Score sc,
+static void rerank_packed(const Corpus* c, Scratch& s, uint32_t nq, uint32_t n_sp, bool desc, const View& v,
                           cudaStream_t st) {
-  auto kern = sc == Score::Dot            ? cand_rerank_packed_kernel<T, SDB_FN_DOT>
-              : c->metric == SDB_COSINE ? cand_rerank_packed_kernel<T, SDB_COSINE>
-                                          : cand_rerank_packed_kernel<T, SDB_EUCLIDEAN>;
+  auto kern = v.steps == SDB_FN_DOT ? cand_rerank_packed_kernel<T, SDB_FN_DOT>
+              : v.steps == SDB_COSINE ? cand_rerank_packed_kernel<T, SDB_COSINE>
+                                      : cand_rerank_packed_kernel<T, SDB_EUCLIDEAN>;
   kern<<<(nq + 7) / 8, 128, 0, st>>>((const T*)c->d_rows.get(), c->dim, c->d_mag, s.d_q64, s.d_qmag, s.d_qflags,
-                                     s.d_cand, s.d_cand_cnt, s.sc_cap, c->d_special, n_sp, nq, rr_out(s, desc));
+                                     s.d_cand, s.d_cand_cnt, s.sc_cap, view_special(c, v), n_sp, nq,
+                                     rr_out(s, desc, v.sim));
 }
 
 // COSINE / EUCLIDEAN: the packed kernel for the small sets stage B leaves; otherwise the vectorised one for f32 rows
 // of a length divisible by 4, the staged one for the rest
 template <bool DOT>
-static void rerank_wide(const Corpus* c, Scratch& s, uint32_t nq, uint32_t n_sp, bool desc, cudaStream_t st) {
+static void rerank_wide(const Corpus* c, Scratch& s, uint32_t nq, uint32_t n_sp, bool desc, const View& v,
+                        cudaStream_t st) {
   const dim3 grid(nq, RR_GROUPS_Y);
-  const RerankOut out = rr_out(s, desc);
-  const int metric = DOT ? (int)SDB_COSINE : (int)c->metric;
+  const RerankOut out = rr_out(s, desc, v.sim);
+  const int metric = DOT ? (int)SDB_COSINE : v.steps;
+  const uint32_t* sp = view_special(c, v);
   if (c->dtype == SDB_F32 && c->dim % 4 == 0)
     cand_rerank_v4_kernel<DOT><<<grid, RR_WARPS * 32, RRV_SMEM, st>>>((const float*)c->d_rows.get(), c->dim, metric,
                                                                      c->d_mag, s.d_q64, s.d_qmag, s.d_qflags, s.d_cand,
-                                                                     s.d_cand_cnt, s.sc_cap, c->d_special, n_sp, out);
+                                                                     s.d_cand_cnt, s.sc_cap, sp, n_sp, out);
   else if (c->dtype == SDB_F32)
     cand_rerank_kernel<float, DOT><<<grid, RR_WARPS * 32, 0, st>>>((const float*)c->d_rows.get(), c->dim, metric,
                                                                   c->d_mag, s.d_q64, s.d_qmag, s.d_qflags, s.d_cand,
-                                                                  s.d_cand_cnt, s.sc_cap, c->d_special, n_sp, out);
+                                                                  s.d_cand_cnt, s.sc_cap, sp, n_sp, out);
   else
     cand_rerank_kernel<double, DOT><<<grid, RR_WARPS * 32, 0, st>>>((const double*)c->d_rows.get(), c->dim, metric,
                                                                    c->d_mag, s.d_q64, s.d_qmag, s.d_qflags, s.d_cand,
-                                                                   s.d_cand_cnt, s.sc_cap, c->d_special, n_sp, out);
+                                                                   s.d_cand_cnt, s.sc_cap, sp, n_sp, out);
 }
-static void rerank_dot(const Corpus* c, Scratch& s, uint32_t nq, bool small_sets, uint32_t n_sp, bool desc, Score sc,
-                       cudaStream_t st) {
-  if (small_sets && c->dtype == SDB_F32) rerank_packed<float>(c, s, nq, n_sp, desc, sc, st);
-  else if (small_sets) rerank_packed<double>(c, s, nq, n_sp, desc, sc, st);
-  else if (sc == Score::Dot) rerank_wide<true>(c, s, nq, n_sp, desc, st);
-  else rerank_wide<false>(c, s, nq, n_sp, desc, st);
+static void rerank_dot(const Corpus* c, Scratch& s, uint32_t nq, bool small_sets, uint32_t n_sp, bool desc,
+                       const View& v, cudaStream_t st) {
+  if (small_sets && c->dtype == SDB_F32) rerank_packed<float>(c, s, nq, n_sp, desc, v, st);
+  else if (small_sets) rerank_packed<double>(c, s, nq, n_sp, desc, v, st);
+  else if (v.sc == Score::Dot) rerank_wide<true>(c, s, nq, n_sp, desc, v, st);
+  else rerank_wide<false>(c, s, nq, n_sp, desc, v, st);
 }
 
 sdb_status cand_rerank(const Corpus* c, Scratch& s, const FiltArg& filt, uint32_t nq, cudaStream_t st,
-                       bool small_sets, bool desc, Score sc) {
-  const uint32_t n_sp = filt.bits ? 0u : c->n_special;  // filtered: the passing special rows are in the lists
+                       bool small_sets, bool desc, const View& v) {
+  const uint32_t n_sp = filt.bits ? 0u : view_n_special(c, v);  // filtered: the passing special rows are in the lists
   switch (family(c)) {
     case Family::Count:  // (the direct regime only; no special rows)
       if (c->metric == SDB_HAMMING) rerank_entry<SDB_HAMMING>(c, s, nq, n_sp, desc, st);
@@ -1492,7 +1529,7 @@ sdb_status cand_rerank(const Corpus* c, Scratch& s, const FiltArg& filt, uint32_
       break;
     case Family::Dot:
     case Family::Exact:  // (never reaches the re-rank: the exact kernel alone ranks it)
-      rerank_dot(c, s, nq, small_sets, n_sp, desc, sc, st);
+      rerank_dot(c, s, nq, small_sets, n_sp, desc, v, st);
       break;
   }
   count_launch(c->ctx);
@@ -1532,7 +1569,9 @@ __device__ __forceinline__ void bitonic_pairs(uint64_t* s_key, uint64_t* s_idx, 
 // The proof of the family F's bound: Dot (cosine / euclidean, also the count path's lists, whose tau stays -inf), Lp, or
 // Centred (the cosine proof on the centred operands, eps_ref = the gap between their cosine and the reference's
 // pearson, DESIGN.md section 2; 0 for the other families).  DOT: Score::Dot batches of Dot corpora, whose eps_ref is the
-// reference's relative rounding times max_norm (per unit of |q|)
+// reference's relative rounding times max_norm (per unit of |q|).  kind, neg: the view's score (View::sc as an int) and
+// query sign, on which the Dot family's other proofs switch; EuclidFar's eps_ref is the reference's relative rounding
+// of the euclidean distance
 template <Family F, bool DOT = false>
 __global__ void __launch_bounds__(256)
     cand_final_kernel(const uint64_t* __restrict__ rr_key, const double* __restrict__ rr_dist,
@@ -1542,7 +1581,7 @@ __global__ void __launch_bounds__(256)
                       const float* __restrict__ beps2, uint32_t* __restrict__ flags, const uint32_t* __restrict__ qflags,
                       uint32_t* __restrict__ stat, int metric, uint32_t k, uint64_t row_base,
                       uint64_t* __restrict__ out_rows, double* __restrict__ out_dist, uint32_t* __restrict__ out_count,
-                      int debug, double eps_ref, bool desc) {
+                      int debug, double eps_ref, bool desc, int kind, bool neg) {
   __shared__ uint64_t s_key[FIN_WIN];  // distance key
   __shared__ uint64_t s_idx[FIN_WIN];  // (row << 32 | entry): secondary order by row (unique), entry = index into rr_*
   const uint32_t q = blockIdx.x;
@@ -1621,12 +1660,25 @@ __global__ void __launch_bounds__(256)
         const double a = __ddiv_ru(__dmul_ru((double)t, (double)bscale[q]), qm);
         const double L = __dsub_rd(__dsub_rd(-a, (double)beps[q]), eps_ref);
         ok = dist_key(L) > kth;
-      } else if (metric == SDB_COSINE && desc) {
-        // cosine_desc: the entries are similarities keyed descending.  Non-candidate: sim <= tau * bscale / |q| + eps,
-        // so it cannot reach the top k if that upper bound sorts strictly after the k-th entry
+      } else if (kind == (int)Score::Cosine && neg) {
+        // the copy of -q (cosine distance DESC, similarity ASC): a non-candidate has cos(x, -q) <= U = tau bscale / |q|
+        // + beps, and the reference's value is within 1e-9 of the real one: sim >= -U, dist = 1 - sim <= 1 + U.  U is
+        // rounded up; proven when that bound sorts strictly after the k-th entry in the batch's direction
+        const double U = __dadd_ru(__dadd_ru(__ddiv_ru(__dmul_ru((double)t, (double)bscale[q]), qm), (double)beps[q]), 1e-9);
+        ok = U == U && (desc ? order_key(__dadd_ru(1.0, U), true) : dist_key(-U)) > kth;
+      } else if (kind == (int)Score::EuclidFar) {
+        // 2 x.(-q)~ + |x|^2~ < tau for a non-candidate, so d^2 - |q|^2 = |x|^2 - 2 x.q <= tau + beps: d^2 <= U = tau + beps
+        // + |q|^2 (+ the reference's f64 underflow), rounded up, and the reference's distance is at most
+        // sqrt(U) (1 + eps_ref), rounded up; proven when that bound sorts strictly after the k-th entry (descending)
+        const double U = __dadd_ru(__dadd_ru(__dadd_ru((double)t, (double)beps[q]), __dmul_ru(qm, qm)), 0x1p-1000);
+        const double d = __dmul_ru(__dsqrt_ru(fmax(U, 0.0)), 1.0 + eps_ref);
+        ok = U == U && order_key(d, true) > kth;
+      } else if (kind == (int)Score::Cosine && desc) {
+        // similarity descending: the entries are similarities keyed descending.  Non-candidate: sim <= tau * bscale /
+        // |q| + eps, so it cannot reach the top k if that upper bound sorts strictly after the k-th entry
         const double upper = (double)t * (double)bscale[q] / qm + (double)beps[q] + 1e-9;
         ok = order_key(upper, true) > kth;
-      } else if (metric == SDB_COSINE) {
+      } else if (kind == (int)Score::Cosine) {
         // non-candidate: score <= tau  =>  sim <= tau * bscale / |q| + eps  =>  dist >= 1 - tau * bscale / |q| - eps
         const double bound = 1.0 - (double)t * (double)bscale[q] / qm - (double)beps[q] - 1e-9;
         ok = dist_key(bound) > kth;
@@ -1647,10 +1699,17 @@ __global__ void __launch_bounds__(256)
         } else if (F == Family::Centred) {  // stage B scores in the same units with bscale 1
           const double L2 = __dsub_rd(__dsub_rd(-__ddiv_ru((double)t2, qm), (double)beps2[q]), eps_ref);
           ok = dist_key(L2) > kth;
-        } else if (metric == SDB_COSINE && desc) {
+        } else if (kind == (int)Score::Cosine && neg) {  // stage B scores in similarity x |q| units (bscale 1)
+          const double U2 = __dadd_ru(__dadd_ru(__ddiv_ru((double)t2, qm), (double)beps2[q]), 1e-9);
+          ok = U2 == U2 && (desc ? order_key(__dadd_ru(1.0, U2), true) : dist_key(-U2)) > kth;
+        } else if (kind == (int)Score::EuclidFar) {
+          const double U2 = __dadd_ru(__dadd_ru(__dadd_ru((double)t2, (double)beps2[q]), __dmul_ru(qm, qm)), 0x1p-1000);
+          const double d2 = __dmul_ru(__dsqrt_ru(fmax(U2, 0.0)), 1.0 + eps_ref);
+          ok = U2 == U2 && order_key(d2, true) > kth;
+        } else if (kind == (int)Score::Cosine && desc) {
           const double upper2 = (double)t2 / qm + (double)beps2[q] + 1e-9;
           ok = order_key(upper2, true) > kth;
-        } else if (metric == SDB_COSINE) {
+        } else if (kind == (int)Score::Cosine) {
           const double bound2 = 1.0 - (double)t2 / qm - (double)beps2[q] - 1e-9;
           ok = dist_key(bound2) > kth;
         } else {
@@ -1673,18 +1732,22 @@ __global__ void __launch_bounds__(256)
 
 sdb_status cand_final(const Corpus* c, Scratch& s, const FiltArg& filt, uint32_t nq, uint32_t k, uint64_t row_base,
                       uint64_t* d_out_rows, double* d_out_dist, uint32_t* d_out_count, cudaStream_t st, bool desc,
-                      Score sc) {
+                      const View& v) {
   if (k > FIN_KEEP) {
     set_error("cand_final: k = %u exceeds the screened path's limit of %u", k, FIN_KEEP);
     return SDB_EINVAL;
   }
   static const int debug = getenv("SDB_DEBUG") != nullptr;
-  const uint32_t n_sp = filt.bits ? 0u : c->n_special;  // filtered: the passing special rows are in the lists
+  const uint32_t n_sp = filt.bits ? 0u : view_n_special(c, v);  // filtered: the passing special rows are in the lists
   auto fin = cand_final_kernel<Family::Dot>;
   double eps_ref = 0.0;
   switch (family(c)) {
     case Family::Dot:
-      if (sc == Score::Dot) {
+      if (v.sc == Score::EuclidFar) {
+        // the reference's distance sqrt(sum (x_i - q_i)^2) in sequential f64: D roundings of differences, squares and
+        // sums err by at most (D + 2) 2^-53 relative on the sum (gamma_D), the square root halves that and adds 2^-53
+        eps_ref = (c->dim + 4.0) * 0x1p-53;
+      } else if (v.sc == Score::Dot) {
         fin = cand_final_kernel<Family::Dot, true>;
         // the reference's sequential f64 dot of D terms errs by at most gamma_D sum |x_i q_i| <= gamma_D |x||q|,
         // gamma_D = D 2^-53 / (1 - D 2^-53) <= (D + 2) 2^-53; |x| <= max_norm; (1 + 2^-20) covers the rounding of
@@ -1707,7 +1770,7 @@ sdb_status cand_final(const Corpus* c, Scratch& s, const FiltArg& filt, uint32_t
   fin<<<nq, 256, 0, st>>>(s.d_rr_key, s.d_rr_dist, s.d_rr_row, s.rr_stride, s.d_cand_cnt, s.sc_cap, n_sp,
                           s.d_tau, s.d_qmag, s.d_bscale, s.d_beps, s.d_tau2, s.d_beps2, s.d_flags, s.d_qflags,
                           s.d_stat, (int)c->metric, k, row_base, d_out_rows, d_out_dist, d_out_count, debug, eps_ref,
-                          desc);
+                          desc, (int)v.sc, v.neg);
   count_launch(c->ctx);
   SDB_CUDA(cudaGetLastError());
   return SDB_OK;

@@ -4,6 +4,7 @@
 //   bf16   [cap][dim_pad]    bf16     screen copy, K-major rows = wgmma "B" operand via TMA (f32 and f64 rows alike)
 //   mag    [cap]             f64      sqrt(sum x^2), the reference's `magnitude()` arithmetic
 //   snorm  [cap]             f32      cosine: 1/|x|, euclid: |x|^2, NaN => row never screened in
+//   xnorm  [cap]             f32      the other metric's screening norm (cross views), NaN wherever snorm is
 #include <algorithm>
 #include <type_traits>
 
@@ -416,8 +417,53 @@ __global__ void __launch_bounds__(256) quantize_rows_kernel(const T* __restrict_
   }
 }
 
+// The cross state of a COSINE or EUCLIDEAN corpus with a bf16 copy, after the own state is final (outliers included):
+// per row the other metric's screening norm and special rule, from the exact magnitude m = mag alone (no pass over the
+// rows), as finalize_rows_kernel applies them to that metric:
+//  - COSINE corpora, for the euclidean views: fl32(m m).  m m is not the reference's sum of squares s, only m = sqrt(s)
+//    is stored: m = sqrt(s) (1 + d1) and fl64(m m) = s (1 + d1)^2 (1 + d2), |d1|, |d2| <= 2^-53, so fl32(m m) is within
+//    2^-24 + 3.01 2^-53 of s relatively -- inside the 8 2^-24 |x|^2 (stage A) and 4 2^-24 |x|^2 (stage B) that the
+//    euclidean bounds give the screening norm (cand_begin_kernel).  Special: m m or its f32 copy not finite;
+//  - EUCLIDEAN corpora, for the cosine views: fl32(1 / m), exactly the COSINE corpus' d_snorm.  Special: m not finite or
+//    not above 0 (zero rows: their cosine is the generated NaN, which sorts first in the ascending orders);
+//  - f64 rows, either metric: a non-zero row whose |x| or screening norm is not a normal f32 or whose |x| < 2^-100.
+// xnorm is NaN wherever snorm is (skipped, removed, own special and outlier rows, padding up to n_pad), and the cross
+// special list is the own list (already in xspecial[0, n_own)) plus the rows only the cross rule makes special.
+template <bool F64>
+__global__ void finalize_cross_kernel(const double* __restrict__ mag, const float* __restrict__ snorm, uint64_t n,
+                                      uint64_t n_pad, int metric, float* __restrict__ xnorm,
+                                      uint32_t* __restrict__ xspecial, uint32_t* xcnt) {
+  const uint64_t r = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (r >= n_pad) return;
+  float xn = __int_as_float(0x7fc00000);
+  if (r < n && snorm[r] == snorm[r]) {
+    const double m = mag[r];
+    bool special;
+    if (metric == SDB_COSINE) {
+      const double s = __dmul_rn(m, m);
+      xn = (float)s;
+      special = !isfinite(s) || !isfinite(xn);
+    } else {
+      special = !(m > 0.0) || !isfinite(m);
+      xn = (float)(1.0 / m);
+    }
+    if (F64) {
+      const float mf = (float)m;
+      const bool m_normal = mf >= 1.17549435e-38f && mf <= 3.40282347e38f;
+      const bool xn_normal = fabsf(xn) >= 1.17549435e-38f && fabsf(xn) <= 3.40282347e38f;
+      if (m > 0.0 && (m < 0x1p-100 || !m_normal || !xn_normal)) special = true;
+    }
+    if (special) {
+      xn = __int_as_float(0x7fc00000);
+      const uint32_t pos = atomicAdd(xcnt, 1u);
+      if (pos < (uint32_t)SPECIAL_CAP) xspecial[pos] = (uint32_t)r;
+    }
+  }
+  xnorm[r] = xn;
+}
+
 // tombstones (sdb_corpus_remove): the row is skipped by every path from now on -- skip mask for the exact kernel, NaN
-// screening norm for the screens and the re-rank's special list, and an all-zero int8 row so that the integer screen
+// screening norms (own and cross) for the screens and the re-rank's special lists, and an all-zero int8 row so that the integer screen
 // scores it exactly 0 (the only score for which that screen looks up a row's validity).  No re-finalize needed.
 __global__ void or_mask_kernel(uint8_t* __restrict__ dst, const uint8_t* __restrict__ src, uint64_t n) {
   const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -435,8 +481,8 @@ sdb_status corpus_reapply_tombstones(Corpus* c, cudaStream_t st) {  // after the
   return SDB_OK;
 }
 __global__ void remove_rows_kernel(const uint64_t* __restrict__ ids, uint64_t n, uint8_t* __restrict__ skip,
-                                   uint8_t* __restrict__ removed, float* __restrict__ snorm, int8_t* __restrict__ i8,
-                                   uint32_t dim_pad8) {
+                                   uint8_t* __restrict__ removed, float* __restrict__ snorm, float* __restrict__ xnorm,
+                                   int8_t* __restrict__ i8, uint32_t dim_pad8) {
   const uint32_t lane = threadIdx.x & 31;
   const uint64_t w = ((uint64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   if (w >= n) return;
@@ -445,6 +491,7 @@ __global__ void remove_rows_kernel(const uint64_t* __restrict__ ids, uint64_t n,
     skip[r] = 1;
     removed[r] = 1;
     if (snorm) snorm[r] = __int_as_float(0x7fc00000);
+    if (xnorm) xnorm[r] = __int_as_float(0x7fc00000);
   }
   if (i8)
     for (uint32_t c = lane; c < dim_pad8; c += 32) i8[r * dim_pad8 + c] = 0;
@@ -463,25 +510,32 @@ sdb_status corpus_remove_device(Corpus* c, const uint64_t* h_ids, uint64_t n) {
   AsyncBuf<uint64_t> d_ids;
   SDB_CUDA(d_ids.reserve(n, st));
   SDB_CUDA(cudaMemcpyAsync(d_ids, h_ids, sizeof(uint64_t) * n, cudaMemcpyHostToDevice, st));
-  remove_rows_kernel<<<(unsigned)((n * 32 + 255) / 256), 256, 0, st>>>(d_ids, n, c->d_skip, c->d_removed, c->finalized ? c->d_snorm.get() : nullptr,
-                                                                       c->finalized ? c->d_i8.get() : nullptr, c->dim_pad8);
+  remove_rows_kernel<<<(unsigned)((n * 32 + 255) / 256), 256, 0, st>>>(
+      d_ids, n, c->d_skip, c->d_removed, c->finalized ? c->d_snorm.get() : nullptr,
+      c->finalized && c->d_xnorm ? c->d_xnorm.get() : nullptr, c->finalized ? c->d_i8.get() : nullptr, c->dim_pad8);
   count_launch(ctx);
   d_ids.reset();
-  if (c->finalized && c->n_special) {  // a removed special row leaves the always-exact list
-    std::vector<uint32_t> sp(c->n_special);
-    SDB_CUDA(cudaMemcpyAsync(sp.data(), c->d_special, sizeof(uint32_t) * c->n_special, cudaMemcpyDeviceToHost, st));
+  std::vector<uint64_t> sorted(h_ids, h_ids + n);
+  std::sort(sorted.begin(), sorted.end());
+  // a removed special row leaves the always-exact lists (own and cross)
+  auto compact = [&](DevBuf<uint32_t>& d_list, uint32_t& n_list) -> sdb_status {
+    if (!c->finalized || !n_list) return SDB_OK;
+    std::vector<uint32_t> sp(n_list);
+    SDB_CUDA(cudaMemcpyAsync(sp.data(), d_list, sizeof(uint32_t) * n_list, cudaMemcpyDeviceToHost, st));
     SDB_CUDA(cudaStreamSynchronize(st));
-    std::vector<uint64_t> sorted(h_ids, h_ids + n);
-    std::sort(sorted.begin(), sorted.end());
     std::vector<uint32_t> keep;
     for (uint32_t r : sp)
       if (!std::binary_search(sorted.begin(), sorted.end(), (uint64_t)r)) keep.push_back(r);
     if (keep.size() != sp.size()) {
       if (!keep.empty())
-        SDB_CUDA(cudaMemcpyAsync(c->d_special, keep.data(), sizeof(uint32_t) * keep.size(), cudaMemcpyHostToDevice, st));
-      c->n_special = (uint32_t)keep.size();
+        SDB_CUDA(cudaMemcpyAsync(d_list, keep.data(), sizeof(uint32_t) * keep.size(), cudaMemcpyHostToDevice, st));
+      SDB_CUDA(cudaStreamSynchronize(st));  // `keep` lives in this frame
+      n_list = (uint32_t)keep.size();
     }
-  }
+    return SDB_OK;
+  };
+  SDB_TRY(compact(c->d_special, c->n_special));
+  if (c->d_xnorm) SDB_TRY(compact(c->d_xspecial, c->n_xspecial));
   SDB_CUDA(cudaStreamSynchronize(st));
   SDB_CUDA(cudaGetLastError());
   return SDB_OK;
@@ -674,6 +728,35 @@ sdb_status corpus_finalize_device(Corpus* c) {
     float gmax;
     memcpy(&gmax, &h[3], 4);
     c->i8_scale = gmax > 0.f ? gmax / 127.f : 1.f;
+  }
+  // the cross state (cross_ranking): after the own state is final, so that it follows every own NaN norm and special
+  // row; the union overflowing SPECIAL_CAP sends the cross views to the exact kernel, and KNN keeps its own state
+  c->n_xspecial = 0;
+  c->xspecial_overflow = false;
+  if (family(c) == Family::Dot && c->d_bf16) {
+    const uint64_t n_pad = (c->n + TILE_ROWS - 1) / TILE_ROWS * TILE_ROWS;
+    const uint64_t cap_pad = (c->cap + TILE_ROWS - 1) / TILE_ROWS * TILE_ROWS;
+    if (c->d_xnorm.reserve(cap_pad) != cudaSuccess || c->d_xspecial.reserve(SPECIAL_CAP) != cudaSuccess) {
+      c->d_xnorm.reset();  // no cross state: the cross views take the exact kernel
+      c->d_xspecial.reset();
+    } else {
+      if (c->n_special)
+        SDB_CUDA(cudaMemcpyAsync(c->d_xspecial, c->d_special, sizeof(uint32_t) * c->n_special, cudaMemcpyDeviceToDevice, st));
+      const uint32_t own = c->special_overflow ? (uint32_t)SPECIAL_CAP + 1u : c->n_special;
+      SDB_CUDA(cudaMemcpyAsync(d_tmp, &own, 4, cudaMemcpyHostToDevice, st));
+      if (n_pad) {
+        auto kern = c->dtype == SDB_F64 ? finalize_cross_kernel<true> : finalize_cross_kernel<false>;
+        kern<<<(unsigned)((n_pad + 255) / 256), 256, 0, st>>>(c->d_mag, c->d_snorm, c->n, n_pad, (int)c->metric,
+                                                              c->d_xnorm, c->d_xspecial, d_tmp);
+        count_launch(ctx);
+        SDB_CUDA(cudaGetLastError());
+      }
+      uint32_t nx = 0;
+      SDB_CUDA(cudaMemcpyAsync(&nx, d_tmp, 4, cudaMemcpyDeviceToHost, st));
+      SDB_CUDA(cudaStreamSynchronize(st));  // (`own` and `nx` live in this frame)
+      c->xspecial_overflow = nx > (uint32_t)SPECIAL_CAP;
+      c->n_xspecial = nx > (uint32_t)SPECIAL_CAP ? (uint32_t)SPECIAL_CAP : nx;
+    }
   }
   c->finalized = true;
   return SDB_OK;

@@ -408,7 +408,7 @@ struct Corpus {
   double minkowski_p = 3.0;   // order of SDB_MINKOWSKI
   sdb_screen rung_scr = SDB_SCREEN_AUTO;  // the first-choice screen the remembered rung belongs to
   uint32_t rung_k = 0;                    // ... and the k it was learnt for
-  int rung_score = 0;                     // ... and the Score of its batch (dot batches' candidate sets are not KNN's)
+  int rung_view = 0;                      // ... and the view_key of its batch (dot batches' candidate sets are not KNN's)
   uint32_t rung = 0;                     // rung of the precision ladder the last batch settled on (api.cu)
   uint64_t cap = 0, n = 0;
   uint64_t row_base = 0;            // global id of row 0 (row-sharded corpora)
@@ -432,6 +432,13 @@ struct Corpus {
   uint32_t n_special = 0;
   uint32_t n_outliers = 0;          // of those: rows made special because one component dominates (int8 scale)
   bool special_overflow = false;
+  // cross state of a COSINE / EUCLIDEAN corpus with a bf16 copy (finalize_cross_kernel), read by the views that rank the
+  // other metric (View::cross): the other metric's screening norm -- |x|^2 on COSINE corpora, 1/|x| on EUCLIDEAN ones,
+  // NaN wherever d_snorm is NaN -- and the union of the own special rows with those the other metric's rule adds
+  DevBuf<float> d_xnorm;
+  DevBuf<uint32_t> d_xspecial;
+  uint32_t n_xspecial = 0;
+  bool xspecial_overflow = false;  // more than SPECIAL_CAP: the cross views take the exact kernel (KNN does not)
   float max_norm = 0.f;
   // exact path scratch
   DevBuf<uint64_t> d_ex_key;  // N keys
@@ -503,22 +510,61 @@ inline bool metric_desc(const Corpus* c, const Ranking& r) {
 // (ASC) inner product.  The screens score x.q (DESC) or x.(-q) (ASC) with no norm term, the re-rank computes the
 // reference's dot and cand_final proves the order with the dot's bound (DESIGN.md sections 2 and 5, ORDER BY).
 inline bool dot_ranking(const Corpus* c, const Ranking& r) { return r.fn == SDB_FN_DOT && family(c) == Family::Dot; }
+// The other cosine and euclidean rankings of a Dot corpus with its cross state (d_xnorm): vector::distance::cosine or
+// vector::similarity::cosine in the order KNN / cosine_desc do not take (farthest first, least similar first), on either
+// metric, and vector::distance::euclidean in either order on COSINE corpora and descending (farthest first) on
+// EUCLIDEAN ones.  The screens score the cosine or the euclidean form of the ranked function towards q or -q, with the
+// per-row array of that form (view_of), and cand_final proves the order with that form's bound (DESIGN.md sections 2
+// and 5, ORDER BY).
+inline bool cross_ranking(const Corpus* c, const Ranking& r) {
+  const bool cos_fn = r.fn == SDB_COSINE || r.fn == SDB_FN_SIMILARITY_COSINE;
+  if (family(c) != Family::Dot || !c->d_xnorm || (!cos_fn && r.fn != SDB_EUCLIDEAN)) return false;
+  return !knn_ranking(c, r) && !cosine_desc(c, r);
+}
 // the rankings the screens (and the count path) serve; every other one is ranked by the exact kernel alone.  Those
-// that are descending are cosine_desc, metric_desc and dot_ranking, and every stage takes Ranking::desc as it is.
+// that are descending are cosine_desc, metric_desc, dot_ranking and cross_ranking, and every stage takes
+// Ranking::desc as it is.
 inline bool screened_ranking(const Corpus* c, const Ranking& r) {
-  return knn_ranking(c, r) || cosine_desc(c, r) || metric_desc(c, r) || dot_ranking(c, r);
+  return knn_ranking(c, r) || cosine_desc(c, r) || metric_desc(c, r) || dot_ranking(c, r) || cross_ranking(c, r);
 }
-// What the Dot and Centred screens score per row, decided once per batch and handed to every stage that depends on it
-// (prep_queries, cand_begin, the screens, cand_refine, the re-rank, cand_final):
-//   Cosine  acc / |x|          COSINE corpora and the centred operands of PEARSON ones
-//   Euclid  2 acc - |x|^2      EUCLIDEAN corpora
-//   Dot     acc                dot_ranking batches on either Dot metric
+// What the Dot and Centred screens score per row:
+//   Cosine     acc / |x|          (own: COSINE corpora and the centred operands of PEARSON ones; cross: EUCLIDEAN ones)
+//   Euclid     2 acc - |x|^2      (own: EUCLIDEAN corpora; cross: COSINE ones)
+//   Dot        acc                dot_ranking batches on either Dot metric
+//   EuclidFar  2 acc + |x|^2      euclidean descending, acc against -q: |x|^2 - 2 x.q = d^2 - |q|^2
 // acc = x~.q~, the dot of the screen copies.  (Lp / Count / Exact corpora: Euclid, which none of their stages reads.)
-enum class Score { Cosine, Euclid, Dot };
-inline Score score_kind(const Corpus* c, const Ranking& r) {
-  if (dot_ranking(c, r)) return Score::Dot;
-  return c->metric == SDB_COSINE || family(c) == Family::Centred ? Score::Cosine : Score::Euclid;
+enum class Score { Cosine, Euclid, Dot, EuclidFar };
+// A batch's view of a Dot or Centred corpus, decided once per batch (view_of) and handed to every stage that depends on
+// it (prep_queries, cand_begin, the screens, cand_refine, cand_add_specials, the re-rank, cand_final).
+struct View {
+  Score sc = Score::Euclid;
+  bool neg = false;    // the screen copies are those of -q (the re-rank keeps q)
+  bool cross = false;  // per-row array and special list: the cross state (d_xnorm, d_xspecial), else d_snorm, d_special
+  int steps = SDB_EUCLIDEAN;  // the re-rank's accumulation: SDB_COSINE (x.q), SDB_EUCLIDEAN ((x - q)^2), SDB_FN_DOT
+  bool sim = false;    // ... and its finish: the cosine similarity instead of the cosine distance
+};
+inline View view_of(const Corpus* c, const Ranking& r) {
+  View v;
+  if (dot_ranking(c, r)) {
+    v.sc = Score::Dot, v.neg = !r.desc, v.steps = SDB_FN_DOT;
+  } else if (cross_ranking(c, r) && r.fn != SDB_EUCLIDEAN) {
+    // cosine distance ascending and similarity descending look towards q; the other two orders towards -q
+    v.sc = Score::Cosine, v.neg = (r.fn == SDB_COSINE) == r.desc, v.cross = c->metric != SDB_COSINE;
+    v.steps = SDB_COSINE, v.sim = r.fn == SDB_FN_SIMILARITY_COSINE;
+  } else if (cross_ranking(c, r)) {
+    v.sc = r.desc ? Score::EuclidFar : Score::Euclid, v.neg = r.desc, v.cross = c->metric != SDB_EUCLIDEAN;
+  } else if (c->metric == SDB_COSINE || family(c) == Family::Centred) {
+    v.sc = Score::Cosine, v.steps = SDB_COSINE, v.sim = cosine_desc(c, r);
+  }
+  return v;
 }
+// the remembered ladder rung belongs to what the screens select: score, query sign and per-row array
+inline int view_key(const View& v) { return (int)v.sc | (v.neg ? 8 : 0) | (v.cross ? 16 : 0); }
+inline const float* view_snorm(const Corpus* c, const View& v) { return v.cross ? c->d_xnorm.get() : c->d_snorm.get(); }
+inline const uint32_t* view_special(const Corpus* c, const View& v) {
+  return v.cross ? c->d_xspecial.get() : c->d_special.get();
+}
+inline uint32_t view_n_special(const Corpus* c, const View& v) { return v.cross ? c->n_xspecial : c->n_special; }
 
 // ---- the brute-force driver (api.cu), as its entry points and the sharded search (comm.cu) use it ------------------
 // one batch as a caller hands it over: queries and row filters on the host (host_in) or the device; outputs on the host
@@ -565,9 +611,9 @@ sdb_status corpus_finalize_device(Corpus* c);
 sdb_status corpus_remove_device(Corpus* c, const uint64_t* h_ids, uint64_t n);
 sdb_status corpus_reapply_tombstones(Corpus* c, cudaStream_t st);
 // The stages of a batch take its scratch set s and, where rows are screened or ranked, its row filter filt.
-// screen_simt.cu: the SIMT_F32 screen of Dot corpora (f32 rows), scoring sc
+// screen_simt.cu: the SIMT_F32 screen of Dot corpora (f32 rows), scoring the view v
 sdb_status screen_simt_pass(const Corpus* c, Scratch& s, const FiltArg& filt, uint32_t nq, const PassDesc& p,
-                            cudaStream_t st, Score sc);
+                            cudaStream_t st, const View& v);
 // screen_lp.cu: the SIMT_F32 screen of Lp corpora, f32 L1 / L-infinity / Lp (score = -s~), f32 and f64 rows
 sdb_status screen_lp_pass(const Corpus* c, Scratch& s, const FiltArg& filt, uint32_t nq, const PassDesc& p,
                           cudaStream_t st);
@@ -582,21 +628,21 @@ sdb_status count_pass(const Corpus* c, Scratch& s, const FiltArg& filt, uint32_t
 // screen_tc.cu
 // mode 0: pass 0 (every score of the pass's tiles written to fixed slots), 1: threshold pass, 2: streaming pass with
 // in-kernel threshold refinement (histogram + refiner warp), 3: probe (chunk maxima of a few tiles, no candidates)
-// sc: the batch's score_kind (the int8 screen serves Score::Cosine only)
+// v: the batch's view (the int8 screen serves Score::Cosine on the own screening norm only)
 sdb_status screen_tc_pass(const Corpus* c, Scratch& s, const FiltArg& filt, uint32_t nq, uint32_t k, const PassDesc& p,
-                          bool int8, int mode, cudaStream_t st, Score sc);
+                          bool int8, int mode, cudaStream_t st, const View& v);
 bool screen_tc_available();
 // candidates.cu
 // grows s to nq queries x cap candidates (a set that grows loses its contents)
 sdb_status scratch_for(const Corpus* c, Scratch& s, uint32_t nq, uint32_t cap);
-// sc, desc: the batch's score_kind and direction.  Centred: desc takes the screen copies of +dq / |dq| (a metric_desc
-// batch) instead of -dq / |dq|; Score::Dot: ascending batches take the screen copies of -q (the re-rank keeps q)
-sdb_status prep_queries(const Corpus* c, Scratch& s, const double* d_queries, uint32_t nq, cudaStream_t st, Score sc,
-                        bool desc);
+// v, desc: the batch's view and direction.  Centred: desc takes the screen copies of +dq / |dq| (a metric_desc batch)
+// instead of -dq / |dq|; Dot corpora: View::neg takes the screen copies of -q (the re-rank keeps q)
+sdb_status prep_queries(const Corpus* c, Scratch& s, const double* d_queries, uint32_t nq, cudaStream_t st,
+                        const View& v, bool desc);
 // one query prepared into the fallback scratch (d_fb_*), independent of the batch scratch
 sdb_status prep_fallback_query(Corpus* c, const double* d_query, cudaStream_t st);
 // resets tau / counts / flags and derives, per query, the screen's error bound, the selection margin and the score range
-sdb_status cand_begin(const Corpus* c, Scratch& s, uint32_t nq, int screen, cudaStream_t st, Score sc);
+sdb_status cand_begin(const Corpus* c, Scratch& s, uint32_t nq, int screen, cudaStream_t st, const View& v);
 sdb_status cand_set_count(const Corpus* c, Scratch& s, uint32_t nq, uint32_t value, cudaStream_t st);
 // per query: gather the main list + the private sub-lists, find the k-th best score s_k, keep every candidate with
 // score >= tau = s_k - margin (all of them while fewer than k exist), publish tau.  seed_hist: also (re)build the
@@ -605,7 +651,7 @@ sdb_status cand_select(const Corpus* c, Scratch& s, uint32_t nq, uint32_t k, boo
                        bool seed_hist, cudaStream_t st, int stage = 0);
 // stage B: re-score every kept candidate in f32 (master rows x f32 query) so that cand_select(stage 1) can shrink the
 // set before the FP64-bound exact re-rank
-sdb_status cand_refine(const Corpus* c, Scratch& s, uint32_t nq, cudaStream_t st, Score sc);
+sdb_status cand_refine(const Corpus* c, Scratch& s, uint32_t nq, cudaStream_t st, const View& v);
 // after a probe launch over n_tiles tiles: tau = (k-th largest chunk maximum) - margin, histogram geometry, empty lists
 sdb_status cand_seed_from_probe(const Corpus* c, Scratch& s, uint32_t nq, uint32_t k, uint32_t n_tiles,
                                 cudaStream_t st);
@@ -614,17 +660,18 @@ sdb_status cand_seed_from_probe(const Corpus* c, Scratch& s, uint32_t nq, uint32
 sdb_status cand_filter_list(const Corpus* c, Scratch& s, const FiltArg& filt, uint32_t nq, cudaStream_t st);
 // filtered batches: append each query's passing special rows to its list (the re-rank and cand_final then run without
 // the shared special-row tail); a list that has no room is flagged as overflowed
-sdb_status cand_add_specials(const Corpus* c, Scratch& s, const FiltArg& filt, uint32_t nq, cudaStream_t st);
+sdb_status cand_add_specials(const Corpus* c, Scratch& s, const FiltArg& filt, uint32_t nq, cudaStream_t st,
+                             const View& v);
 // direct regime (filtered): each query's list = the rows its filter passes that are neither skipped nor removed
 sdb_status cand_direct(const Corpus* c, Scratch& s, const FiltArg& filt, uint32_t nq, cudaStream_t st);
-// desc (the descending screened rankings): the re-rank keys its values descending (cosine_desc: it computes the
-// cosine similarity), and cand_final proves that order.  sc = Score::Dot: the re-rank computes the reference's dot and
-// cand_final proves the order with the dot's bound, in either direction
+// desc (the descending screened rankings): the re-rank keys its values descending, and cand_final proves that order.
+// v (Dot corpora): the re-rank computes the view's function (View::steps, View::sim) over its special list, and
+// cand_final proves the order with the bound of the view's score
 sdb_status cand_rerank(const Corpus* c, Scratch& s, const FiltArg& filt, uint32_t nq, cudaStream_t st,
-                       bool small_sets, bool desc, Score sc);
+                       bool small_sets, bool desc, const View& v);
 sdb_status cand_final(const Corpus* c, Scratch& s, const FiltArg& filt, uint32_t nq, uint32_t k, uint64_t row_base,
                       uint64_t* d_out_rows, double* d_out_dist, uint32_t* d_out_count, cudaStream_t st, bool desc,
-                      Score sc);
+                      const View& v);
 // exact.cu: query vector / |q| / flags are passed explicitly (a batch scratch row or the fallback scratch).
 // filter: nullptr, or the query's bitmap (filter_words words): rows whose bit is clear are not ranked.
 // rank: the value ranked (any vector function) and its direction; the default is the corpus metric ascending (KNN).

@@ -50,9 +50,9 @@ __device__ __forceinline__ void bulk_load(uint32_t dst, const void* src, uint32_
 // RPW = rows per consumer warp per stage (4, 2 or 1; chosen so that 2 stages + the queries fit shared memory)
 // QB  = queries per launch (1, 4 or 8): fewer queries = less shared-memory read traffic per row
 // FILT: filtered batch -- a row the query's filter rejects is never appended (filt.qf is indexed by q0 + query)
-// DOT: Score::Dot -- the score is the dot itself, NaN for the rows whose screening norm is NaN; otherwise the metric's
-// score (cosine / euclidean)
-template <int RPW, int QB, bool FILT, bool DOT = false>
+// DOT: Score::Dot -- the score is the dot itself, NaN for the rows whose screening norm is NaN; FAR: Score::EuclidFar,
+// 2 acc + |x|^2; otherwise the score of `metric` (SDB_COSINE: cosine, else euclidean)
+template <int RPW, int QB, bool FILT, bool DOT = false, bool FAR = false>
 __global__ void __launch_bounds__(SIMT_THREADS, 1) screen_simt_kernel(
     const float* __restrict__ rows, const float* __restrict__ snorm, uint32_t dim, uint64_t n_rows,
     const float* __restrict__ q32, uint32_t q0, uint32_t nqb, int metric, PassDesc pass,
@@ -155,7 +155,9 @@ __global__ void __launch_bounds__(SIMT_THREADS, 1) screen_simt_kernel(
           }
           if (lane < nqb && row < n_rows) {
             const float sn = __ldg(snorm + row);
-            const float sc = DOT ? (sn == sn ? mine : sn) : metric == SDB_COSINE ? mine * sn : fmaf(2.f, mine, -sn);
+            const float sc = DOT   ? (sn == sn ? mine : sn)
+                           : FAR ? fmaf(2.f, mine, sn)
+                                 : metric == SDB_COSINE ? mine * sn : fmaf(2.f, mine, -sn);
             if (sc >= my_tau && (!FILT || filt_pass(filt, q0 + lane, (uint32_t)row))) {  // NaN (skipped / special rows) never passes
               const uint32_t pos = atomicAdd(cand_cnt + q0 + lane, 1u);
               if (pos < cap) {
@@ -173,7 +175,7 @@ __global__ void __launch_bounds__(SIMT_THREADS, 1) screen_simt_kernel(
 }
 
 // generic fallback for dimensions that are not a multiple of 4 (rows not 16-byte aligned): plain coalesced loads
-template <bool FILT, bool DOT = false>
+template <bool FILT, bool DOT = false, bool FAR = false>
 __global__ void __launch_bounds__(256) screen_simt_generic_kernel(
     const float* __restrict__ rows, const float* __restrict__ snorm, uint32_t dim, uint64_t n_rows,
     const float* __restrict__ q32, uint32_t q0, uint32_t nqb, int metric, PassDesc pass,
@@ -212,7 +214,9 @@ __global__ void __launch_bounds__(256) screen_simt_generic_kernel(
       }
       if (lane < nqb) {
         const float sn = __ldg(snorm + row);
-        const float sc = DOT ? (sn == sn ? mine : sn) : metric == SDB_COSINE ? mine * sn : fmaf(2.f, mine, -sn);
+        const float sc = DOT   ? (sn == sn ? mine : sn)
+                           : FAR ? fmaf(2.f, mine, sn)
+                                 : metric == SDB_COSINE ? mine * sn : fmaf(2.f, mine, -sn);
         if (sc >= my_tau && (!FILT || filt_pass(filt, q0 + lane, (uint32_t)row))) {
           const uint32_t pos = atomicAdd(cand_cnt + q0 + lane, 1u);
           if (pos < cap) {
@@ -227,19 +231,24 @@ __global__ void __launch_bounds__(256) screen_simt_generic_kernel(
   }
 }
 
+// the kernels' runtime `metric`: the form of the view's score (SDB_COSINE: acc / |x|), not the corpus metric
+static int simt_metric(const View& v) { return v.sc == Score::Cosine ? (int)SDB_COSINE : (int)SDB_EUCLIDEAN; }
+
 template <int RPW, int QB>
 static sdb_status launch_ring_q(const Corpus* c, Scratch& s, const FiltArg& filt, uint32_t nq, const PassDesc& p,
-                                cudaStream_t st, size_t smem, Score sc) {
+                                cudaStream_t st, size_t smem, const View& v) {
   Ctx* ctx = c->ctx;
-  auto kern = sc == Score::Dot ? (filt.bits ? screen_simt_kernel<RPW, QB, true, true> : screen_simt_kernel<RPW, QB, false, true>)
-                               : (filt.bits ? screen_simt_kernel<RPW, QB, true> : screen_simt_kernel<RPW, QB, false>);
+  auto kern = v.sc == Score::Dot ? (filt.bits ? screen_simt_kernel<RPW, QB, true, true> : screen_simt_kernel<RPW, QB, false, true>)
+              : v.sc == Score::EuclidFar
+                  ? (filt.bits ? screen_simt_kernel<RPW, QB, true, false, true> : screen_simt_kernel<RPW, QB, false, false, true>)
+                  : (filt.bits ? screen_simt_kernel<RPW, QB, true> : screen_simt_kernel<RPW, QB, false>);
   SDB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   uint32_t grid = (uint32_t)ctx->sm_count;
   if (grid > p.count) grid = p.count;
   for (uint32_t q0 = 0; q0 < nq; q0 += QB) {
     const uint32_t nqb = nq - q0 < (uint32_t)QB ? nq - q0 : (uint32_t)QB;
-    kern<<<grid, SIMT_THREADS, smem, st>>>((const float*)c->d_rows.get(), c->d_snorm, c->dim, c->n, s.d_q32, q0, nqb,
-                                           (int)c->metric, p, s.d_tau, s.d_cand, s.d_cand_cnt, s.sc_cap, filt);
+    kern<<<grid, SIMT_THREADS, smem, st>>>((const float*)c->d_rows.get(), view_snorm(c, v), c->dim, c->n, s.d_q32, q0,
+                                           nqb, simt_metric(v), p, s.d_tau, s.d_cand, s.d_cand_cnt, s.sc_cap, filt);
     count_launch(ctx);
   }
   SDB_CUDA(cudaGetLastError());
@@ -248,15 +257,15 @@ static sdb_status launch_ring_q(const Corpus* c, Scratch& s, const FiltArg& filt
 
 template <int RPW>
 static sdb_status launch_ring(const Corpus* c, Scratch& s, const FiltArg& filt, uint32_t nq, const PassDesc& p,
-                              cudaStream_t st, size_t q_bytes8, size_t ring, Score sc) {
+                              cudaStream_t st, size_t q_bytes8, size_t ring, const View& v) {
   // the shared-memory query tile shrinks with QB; the row ring keeps its size
-  if (nq == 1) return launch_ring_q<RPW, 1>(c, s, filt, nq, p, st, q_bytes8 / 8 + ring, sc);
-  if (nq <= 4) return launch_ring_q<RPW, 4>(c, s, filt, nq, p, st, q_bytes8 / 2 + ring, sc);
-  return launch_ring_q<RPW, 8>(c, s, filt, nq, p, st, q_bytes8 + ring, sc);
+  if (nq == 1) return launch_ring_q<RPW, 1>(c, s, filt, nq, p, st, q_bytes8 / 8 + ring, v);
+  if (nq <= 4) return launch_ring_q<RPW, 4>(c, s, filt, nq, p, st, q_bytes8 / 2 + ring, v);
+  return launch_ring_q<RPW, 8>(c, s, filt, nq, p, st, q_bytes8 + ring, v);
 }
 
 sdb_status screen_simt_pass(const Corpus* c, Scratch& s, const FiltArg& filt, uint32_t nq, const PassDesc& p,
-                            cudaStream_t st, Score sc) {
+                            cudaStream_t st, const View& v) {
   if (p.count == 0) return SDB_OK;
   Ctx* ctx = c->ctx;
   const size_t q_bytes = sizeof(float) * SIMT_QB * c->dim;
@@ -264,16 +273,18 @@ sdb_status screen_simt_pass(const Corpus* c, Scratch& s, const FiltArg& filt, ui
   auto ring_only = [&](int rpw) { return sizeof(float) * SIMT_STAGES * rpw * SIMT_CWARPS * (size_t)c->dim + 64; };
   auto ring_bytes = [&](int rpw) { return q_bytes + ring_only(rpw); };
   if (c->dim % 4 == 0 && ring_bytes(1) <= budget) {
-    if (ring_bytes(4) <= budget) return launch_ring<4>(c, s, filt, nq, p, st, q_bytes, ring_only(4), sc);
-    if (ring_bytes(2) <= budget) return launch_ring<2>(c, s, filt, nq, p, st, q_bytes, ring_only(2), sc);
-    return launch_ring<1>(c, s, filt, nq, p, st, q_bytes, ring_only(1), sc);
+    if (ring_bytes(4) <= budget) return launch_ring<4>(c, s, filt, nq, p, st, q_bytes, ring_only(4), v);
+    if (ring_bytes(2) <= budget) return launch_ring<2>(c, s, filt, nq, p, st, q_bytes, ring_only(2), v);
+    return launch_ring<1>(c, s, filt, nq, p, st, q_bytes, ring_only(1), v);
   }
   if (q_bytes > 200 * 1024) {
     set_error("screen_simt: dim %u too large for the shared-memory query tile", c->dim);
     return SDB_EUNSUPPORTED;
   }
-  auto kern = sc == Score::Dot ? (filt.bits ? screen_simt_generic_kernel<true, true> : screen_simt_generic_kernel<false, true>)
-                               : (filt.bits ? screen_simt_generic_kernel<true> : screen_simt_generic_kernel<false>);
+  auto kern = v.sc == Score::Dot ? (filt.bits ? screen_simt_generic_kernel<true, true> : screen_simt_generic_kernel<false, true>)
+              : v.sc == Score::EuclidFar
+                  ? (filt.bits ? screen_simt_generic_kernel<true, false, true> : screen_simt_generic_kernel<false, false, true>)
+                  : (filt.bits ? screen_simt_generic_kernel<true> : screen_simt_generic_kernel<false>);
   SDB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)q_bytes));
   int per_sm = 1;
   SDB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, 256, q_bytes));
@@ -282,8 +293,8 @@ sdb_status screen_simt_pass(const Corpus* c, Scratch& s, const FiltArg& filt, ui
   if (grid > p.count) grid = p.count;
   for (uint32_t q0 = 0; q0 < nq; q0 += SIMT_QB) {
     const uint32_t nqb = nq - q0 < (uint32_t)SIMT_QB ? nq - q0 : (uint32_t)SIMT_QB;
-    kern<<<grid, 256, q_bytes, st>>>((const float*)c->d_rows.get(), c->d_snorm, c->dim, c->n, s.d_q32, q0, nqb,
-                                     (int)c->metric, p, s.d_tau, s.d_cand, s.d_cand_cnt, s.sc_cap, filt);
+    kern<<<grid, 256, q_bytes, st>>>((const float*)c->d_rows.get(), view_snorm(c, v), c->dim, c->n, s.d_q32, q0, nqb,
+                                     simt_metric(v), p, s.d_tau, s.d_cand, s.d_cand_cnt, s.sc_cap, filt);
     count_launch(ctx);
   }
   SDB_CUDA(cudaGetLastError());

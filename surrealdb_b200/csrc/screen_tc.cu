@@ -285,7 +285,7 @@ __device__ __forceinline__ void push_survivors(const uint32_t (&acc)[128], int i
 // test sits where a survivor is appended (bf16: the consumer's append; int8: the drain warp, next to the screening-norm
 // look-up) and, in the probe, on the one bitmap word of every 32-row chunk.  Pass 0 writes every row; cand_filter_list
 // drops the rejected ones there.
-// S: the score of the bf16 epilogue (score_kind); the int8 screen scores Score::Cosine alone.
+// S: the score of the bf16 epilogue (View::sc); the int8 screen scores Score::Cosine alone.
 template <Score S, bool INT8, int MODE, bool FILT>
 __global__ void __launch_bounds__(threads<INT8, MODE>(), 1)
 screen_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b,
@@ -450,6 +450,9 @@ screen_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constan
               // becomes that NaN.  (A select, not acc + (n - n): a valid COSINE row's 1/|x| may be +inf in f32.)
               a0 = n2.x == n2.x ? a0 : n2.x;
               a1 = n2.y == n2.y ? a1 : n2.y;
+            } else if constexpr (S == Score::EuclidFar) {
+              a0 = fmaf(2.f, a0, n2.x);  // |x|^2 - 2 x.q against the copy of -q (NaN norm: NaN score)
+              a1 = fmaf(2.f, a1, n2.y);
             } else {
               a0 = S == Score::Cosine ? a0 * n2.x : fmaf(2.f, a0, -n2.x);
               a1 = S == Score::Cosine ? a1 * n2.y : fmaf(2.f, a1, -n2.y);
@@ -750,6 +753,8 @@ sdb_status screen_tc_init_device(Ctx* ctx) {
   SET_SMEM(Score::Cosine, false, 0); SET_SMEM(Score::Cosine, false, 1); SET_SMEM(Score::Cosine, false, 2); SET_SMEM(Score::Cosine, false, 3);
   SET_SMEM(Score::Euclid, false, 0); SET_SMEM(Score::Euclid, false, 1); SET_SMEM(Score::Euclid, false, 2); SET_SMEM(Score::Euclid, false, 3);
   SET_SMEM(Score::Dot, false, 0); SET_SMEM(Score::Dot, false, 1); SET_SMEM(Score::Dot, false, 2); SET_SMEM(Score::Dot, false, 3);
+  SET_SMEM(Score::EuclidFar, false, 0); SET_SMEM(Score::EuclidFar, false, 1); SET_SMEM(Score::EuclidFar, false, 2);
+  SET_SMEM(Score::EuclidFar, false, 3);
   SET_SMEM(Score::Cosine, true, 0); SET_SMEM(Score::Cosine, true, 1); SET_SMEM(Score::Cosine, true, 2); SET_SMEM(Score::Cosine, true, 3);
 #undef SET_SMEM
 #undef SET_SMEM1
@@ -773,11 +778,12 @@ sdb_status screen_tc_init_device(Ctx* ctx) {
 }
 
 sdb_status screen_tc_pass(const Corpus* c, Scratch& s, const FiltArg& filt, uint32_t nq, uint32_t k, const PassDesc& p,
-                          bool int8, int mode, cudaStream_t st, Score sc) {
+                          bool int8, int mode, cudaStream_t st, const View& v) {
   if (p.count == 0) return SDB_OK;
   Ctx* ctx = c->ctx;
+  const Score sc = v.sc;
   // (PEARSON corpora hold centred copies (corpus.cu) and centred, negated queries (prep_queries): Score::Cosine)
-  if (int8 ? (!c->d_i8 || sc != Score::Cosine) : !c->d_bf16) {
+  if (int8 ? (!c->d_i8 || sc != Score::Cosine || v.cross) : !c->d_bf16) {
     set_error("tensor-core screen: the %s screen copy is not available for this corpus",
               int8 ? "int8 (cosine and pearson scores only)" : "bf16");
     return SDB_EUNSUPPORTED;
@@ -852,7 +858,7 @@ sdb_status screen_tc_pass(const Corpus* c, Scratch& s, const FiltArg& filt, uint
     cfg.numAttrs = pair ? 2 : 1;
     float* probe_ptr = s.d_probe + (size_t)q0 * PROBE_STRIDE;
     const uint32_t probe_stride = PROBE_STRIDE, cap_arg = s.sc_cap;
-    const float* snorm_arg = c->d_snorm;
+    const float* snorm_arg = view_snorm(c, v);
     FiltArg filt_q = filt;
     if (filt_q.bits) filt_q.qf += q0;
 #define LAUNCH_TC2(SC, I8, MODE, F)                                                                                  \
@@ -875,6 +881,7 @@ sdb_status screen_tc_pass(const Corpus* c, Scratch& s, const FiltArg& filt, uint
     if (int8) LAUNCH_TC(Score::Cosine, true);
     else if (sc == Score::Cosine) LAUNCH_TC(Score::Cosine, false);
     else if (sc == Score::Euclid) LAUNCH_TC(Score::Euclid, false);
+    else if (sc == Score::EuclidFar) LAUNCH_TC(Score::EuclidFar, false);
     else LAUNCH_TC(Score::Dot, false);
 #undef LAUNCH_TC
 #undef LAUNCH_TC1
