@@ -424,7 +424,7 @@ sdb_status sdb_corpus_project(sdb_corpus*, const double* query, int fn, double* 
  * exact counts); every other (fn, order) is ranked by the exact kernel.
  * Refusals: an unknown fn or order, or nq > 0 with NULL queries for a function that takes a query: SDB_EINVAL.
  * Tickets share the corpus' four slots with KNN tickets; sdb_knn_wait completes them; cancellation and
- * sdb_knn_last_stats work as for KNN.  Row-sharded columns are not served. */
+ * sdb_knn_last_stats work as for KNN.  Row-sharded columns: sdb_corpus_order_sharded_* below. */
 /* order: an sdb_order value, passed as int (like fn) so that any other value can be refused without first being
  * converted to the enum */
 typedef enum { SDB_ORDER_ASC = 0, SDB_ORDER_DESC = 1 } sdb_order;
@@ -446,6 +446,35 @@ sdb_status sdb_corpus_order_submit_device(sdb_corpus*, const double* d_queries, 
                                           const uint32_t* query_filter, uint64_t row_base, uint64_t* d_out_rows,
                                           double* d_out_value, uint32_t* d_out_count, uint32_t* ticket);
 
+/* ORDER BY on a row-sharded column: the collective counterpart of sdb_corpus_order_submit[_device], like
+ * sdb_knn_sharded_submit[_filtered][_device].  Every shard ranks its rows by (fn, order) on its own route (screens,
+ * count path or exact kernel, as sdb_corpus_order_topk would on that shard) and returns its top-k by (value, global
+ * row); the blocks are exchanged as for KNN and merged in the ranking's direction, so query q returns exactly what
+ * sdb_corpus_order_topk returns on the unsharded column: the same global rows in the same order (above k = 1000, rows
+ * of equal value in one valid order, as there), bit-identical values, the same counts.  filters == NULL: unfiltered
+ * (n_rows_total ignored); otherwise the bitmaps cover the GLOBAL rows exactly as in sdb_knn_sharded_submit_filtered.
+ * COLLECTIVE: every rank passes the same queries, fn, order, k, bitmaps and query_filter, in the same order of calls.
+ * For SDB_MINKOWSKI every shard must also hold the same order (sdb_corpus_set_minkowski_order); the library cannot
+ * check either without another collective.  Completion through sdb_knn_sharded_wait; order and KNN sharded tickets
+ * share the four slots and mix.  Refusals: those of sdb_corpus_order_topk (unknown fn or order, NULL queries for a
+ * function that takes one: SDB_EINVAL; k > 4096: SDB_EUNSUPPORTED) and SDB_EINVAL when filters are given and
+ * row_base + sdb_corpus_rows > n_rows_total; no ticket stays claimed and the column keeps answering after one. */
+sdb_status sdb_corpus_order_sharded_submit(sdb_corpus*, const double* queries, uint32_t nq, int fn, int order,
+                                           uint32_t k, const uint32_t* filters, uint32_t n_filters,
+                                           const uint32_t* query_filter, uint64_t n_rows_total, uint64_t* out_rows,
+                                           double* out_value, uint32_t* out_count, uint32_t* ticket);
+/* device queries, bitmaps and outputs (query_filter stays host memory) */
+sdb_status sdb_corpus_order_sharded_submit_device(sdb_corpus*, const double* d_queries, uint32_t nq, int fn,
+                                                  int order, uint32_t k, const uint32_t* d_filters,
+                                                  uint32_t n_filters, const uint32_t* query_filter,
+                                                  uint64_t n_rows_total, uint64_t* d_out_rows, double* d_out_value,
+                                                  uint32_t* d_out_count, uint32_t* ticket);
+/* one process, N GPUs (like sdb_knn_sharded_multi[_filtered]); host buffers, blocking */
+sdb_status sdb_corpus_order_sharded_multi(sdb_corpus* const* shards, int n_shards, const double* queries, uint32_t nq,
+                                          int fn, int order, uint32_t k, const uint32_t* filters, uint32_t n_filters,
+                                          const uint32_t* query_filter, uint64_t n_rows_total, uint64_t* out_rows,
+                                          double* out_value, uint32_t* out_count);
+
 /* merges `n_lists` per-shard result lists (each nq x k; list l's entry j of query q is valid iff
  * j < d_counts[l*stride_counts + q]) into the global top-k by (distance, row); all pointers are device
  * pointers.  stride_* = distance in ELEMENTS between consecutive lists (0 = dense: nq*k, nq*k, nq), so the
@@ -455,6 +484,14 @@ sdb_status sdb_topk_merge_device(sdb_ctx*, uint32_t n_lists, uint32_t nq, uint32
                                  const double* d_dist, const uint32_t* d_counts, uint64_t stride_rows,
                                  uint64_t stride_dist, uint64_t stride_counts, uint64_t* d_out_rows,
                                  double* d_out_dist, uint32_t* d_out_count);
+/* sdb_topk_merge_device for an ORDER BY ranking: the lists are in (value, row) order for `order` (an sdb_order value:
+ * Number::cmp of the value, reversed as a whole for SDB_ORDER_DESC, then ascending row) and so is the merged list;
+ * values are carried through unchanged (a -0.0 stays -0.0).  SDB_ORDER_ASC merges exactly as sdb_topk_merge_device.
+ * k <= 4096 (SDB_EUNSUPPORTED beyond); more than 32 lists share the sorter's limit. */
+sdb_status sdb_order_merge_device(sdb_ctx*, uint32_t n_lists, uint32_t nq, uint32_t k, int order, const uint64_t* d_rows,
+                                  const double* d_value, const uint32_t* d_counts, uint64_t stride_rows,
+                                  uint64_t stride_value, uint64_t stride_counts, uint64_t* d_out_rows,
+                                  double* d_out_value, uint32_t* d_out_count);
 
 /* ---- HNSW search: replaces Hnsw::knn_search (idx/trees/hnsw/mod.rs:459-482) called from
  *      HnswIndex::search_graph (idx/trees/hnsw/index.rs:341-364) ------------------------------- */

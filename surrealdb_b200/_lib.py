@@ -41,7 +41,8 @@ ABI_SYMBOLS = [
     "sdb_graph_expand_batch", "sdb_graph_expand_batch_device", "sdb_graph_collect_batch", "sdb_graph_last_collect_table",
     "sdb_knn_bruteforce_filtered", "sdb_knn_bruteforce_filtered_device", "sdb_knn_submit_filtered",
     "sdb_knn_submit_filtered_device", "sdb_knn_sharded_submit_filtered", "sdb_knn_sharded_submit_filtered_device",
-    "sdb_knn_sharded_multi_filtered",
+    "sdb_knn_sharded_multi_filtered", "sdb_corpus_order_sharded_submit", "sdb_corpus_order_sharded_submit_device",
+    "sdb_corpus_order_sharded_multi", "sdb_order_merge_device",
     "sdb_hnsw_search_filtered_batch", "sdb_hnsw_search_filtered_batch_device", "sdb_hnsw_last_spilled",
     "sdb_hnsw_submit", "sdb_hnsw_submit_device", "sdb_hnsw_submit_filtered", "sdb_hnsw_submit_filtered_device",
     "sdb_hnsw_wait",
@@ -141,8 +142,14 @@ def lib():
     L.sdb_corpus_order_submit.argtypes = [vp, vp, u32, i32, i32, u32, vp, u32, vp, vp, vp, vp, C.POINTER(u32)]
     L.sdb_corpus_order_submit_device.argtypes = [vp, vp, u32, i32, i32, u32, vp, u32, vp, u64, vp, vp, vp,
                                                  C.POINTER(u32)]
+    L.sdb_corpus_order_sharded_submit.argtypes = [vp, vp, u32, i32, i32, u32, vp, u32, vp, u64, vp, vp, vp,
+                                                  C.POINTER(u32)]
+    L.sdb_corpus_order_sharded_submit_device.argtypes = [vp, vp, u32, i32, i32, u32, vp, u32, vp, u64, vp, vp, vp,
+                                                         C.POINTER(u32)]
+    L.sdb_corpus_order_sharded_multi.argtypes = [vp, i32, vp, u32, i32, i32, u32, vp, u32, vp, u64, vp, vp, vp]
     L.sdb_knn_last_stats.argtypes = [vp, C.POINTER(KnnStats)]
     L.sdb_topk_merge_device.argtypes = [vp, u32, u32, u32, vp, vp, vp, u64, u64, u64, vp, vp, vp]
+    L.sdb_order_merge_device.argtypes = [vp, u32, u32, u32, i32, vp, vp, vp, u64, u64, u64, vp, vp, vp]
     L.sdb_hnsw_load.argtypes = [vp, u32, i32, u64, vp, u32, vp, vp, C.c_int64, C.POINTER(vp)]
     L.sdb_hnsw_load_typed.argtypes = [vp, u32, i32, i32, u64, vp, u32, vp, vp, C.c_int64, C.POINTER(vp)]
     L.sdb_hnsw_load_device.argtypes = [vp, u32, i32, u64, vp, u32, vp, vp, C.c_int64, C.POINTER(vp)]

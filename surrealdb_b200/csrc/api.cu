@@ -863,6 +863,12 @@ sdb_status knn_shard_header(Corpus* c, uint32_t ticket, void* d_hdr) {
 }
 
 // ---- global top-k merge of per-shard lists (after the NCCL all-gather) -----------------------------
+// Both merges order the entries by (order_key(value, DESC), global row): DESC = false is KNN's (distance, row) order and
+// the ascending ORDER BY ranking, DESC = true the descending one (sdb_corpus_order_sharded_*).  Each list must already
+// be in that order.  Padding and exhausted lists take key ~0 and row ~0: order_key never yields ~0 for DESC, and for
+// ASC the row still sets the sentinel apart from the all-ones NaN.  The value carried through is the one the shard
+// returned, so -0.0 stays -0.0.
+template <bool DESC>
 __global__ void __launch_bounds__(1024) topk_merge_kernel(uint32_t n_lists, uint32_t nq, uint32_t k,
                                                           const uint64_t* __restrict__ rows,
                                                           const double* __restrict__ dist,
@@ -889,7 +895,7 @@ __global__ void __launch_bounds__(1024) topk_merge_kernel(uint32_t n_lists, uint
       if (j < counts[(size_t)l * st_cnt + q]) {
         const size_t o = (size_t)q * k + j;
         d = dist[(size_t)l * st_dist + o];
-        key = dist_key(d);
+        key = order_key(d, DESC);
         row = rows[(size_t)l * st_rows + o];
         atomicAdd(&s_n, 1u);
       }
@@ -927,9 +933,10 @@ __global__ void __launch_bounds__(1024) topk_merge_kernel(uint32_t n_lists, uint
 }
 
 
-// <= 32 lists: one warp per query, lane l walks list l (each list is already in (distance, row) order).  Every step takes
-// the warp-wide minimum head.  No shared memory and 128-thread blocks, so the merge runs beside the resident screen of
-// the next batch (the sorter above needs 24 bytes of shared memory per entry and up to 1024 threads).
+// <= 32 lists: one warp per query, lane l walks list l (each list is already in (order key, row) order).  Every step
+// takes the warp-wide minimum head.  No shared memory and 128-thread blocks, so the merge runs beside the resident screen
+// of the next batch (the sorter above needs 24 bytes of shared memory per entry and up to 1024 threads).
+template <bool DESC>
 __global__ void __launch_bounds__(128) topk_kway_merge_kernel(uint32_t n_lists, uint32_t nq, uint32_t k,
                                                               const uint64_t* __restrict__ rows,
                                                               const double* __restrict__ dist,
@@ -952,7 +959,7 @@ __global__ void __launch_bounds__(128) topk_kway_merge_kernel(uint32_t n_lists, 
   double d = 0.0;
   if (pos < cnt) {
     d = ld[0];
-    key = dist_key(d);
+    key = order_key(d, DESC);
     row = lr[0];
   }
   uint32_t n_out = 0;
@@ -976,7 +983,7 @@ __global__ void __launch_bounds__(128) topk_kway_merge_kernel(uint32_t n_lists, 
       pos++;
       if (pos < cnt) {
         d = ld[pos];
-        key = dist_key(d);
+        key = order_key(d, DESC);
         row = lr[pos];
       } else {
         key = ~0ull;
@@ -990,13 +997,14 @@ __global__ void __launch_bounds__(128) topk_kway_merge_kernel(uint32_t n_lists, 
 sdb_status topk_merge_launch(Ctx* ctx, uint32_t n_lists, uint32_t nq, uint32_t k, const uint64_t* d_rows,
                              const double* d_dist, const uint32_t* d_counts, uint64_t stride_rows, uint64_t stride_dist,
                              uint64_t stride_counts, uint64_t* d_out_rows, double* d_out_dist, uint32_t* d_out_count,
-                             cudaStream_t st) {
+                             bool desc, cudaStream_t st) {
   if (!stride_rows) stride_rows = (uint64_t)nq * k;
   if (!stride_dist) stride_dist = (uint64_t)nq * k;
   if (!stride_counts) stride_counts = nq;
   if (n_lists <= 32) {
-    topk_kway_merge_kernel<<<(nq + 3) / 4, 128, 0, st>>>(n_lists, nq, k, d_rows, d_dist, d_counts, stride_rows, stride_dist,
-                                                       stride_counts, d_out_rows, d_out_dist, d_out_count);
+    auto kway = desc ? topk_kway_merge_kernel<true> : topk_kway_merge_kernel<false>;
+    kway<<<(nq + 3) / 4, 128, 0, st>>>(n_lists, nq, k, d_rows, d_dist, d_counts, stride_rows, stride_dist, stride_counts,
+                                       d_out_rows, d_out_dist, d_out_count);
     count_launch(ctx);
     SDB_CUDA(cudaGetLastError());
     return SDB_OK;
@@ -1009,8 +1017,9 @@ sdb_status topk_merge_launch(Ctx* ctx, uint32_t n_lists, uint32_t nq, uint32_t k
     return SDB_EUNSUPPORTED;
   }
   const uint32_t threads = p2 >= 1024 ? 1024 : (p2 < 64 ? 64 : p2);
-  topk_merge_kernel<<<nq, threads, smem, st>>>(n_lists, nq, k, d_rows, d_dist, d_counts, stride_rows, stride_dist,
-                                               stride_counts, d_out_rows, d_out_dist, d_out_count);
+  auto sorter = desc ? topk_merge_kernel<true> : topk_merge_kernel<false>;
+  sorter<<<nq, threads, smem, st>>>(n_lists, nq, k, d_rows, d_dist, d_counts, stride_rows, stride_dist, stride_counts,
+                                    d_out_rows, d_out_dist, d_out_count);
   count_launch(ctx);
   SDB_CUDA(cudaGetLastError());
   return SDB_OK;
@@ -1066,7 +1075,8 @@ sdb_status sdb_ctx_create(int device, sdb_ctx** out) {
   SDB_TRY(screen_tc_init_device(c));
   SDB_TRY(candidates_init_device());
   SDB_TRY(exact_init_device());
-  SDB_CUDA(cudaFuncSetAttribute(topk_merge_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+  SDB_CUDA(cudaFuncSetAttribute(topk_merge_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+  SDB_CUDA(cudaFuncSetAttribute(topk_merge_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
   {  // keep stream-ordered allocations cached in the pool instead of returning them to the OS at every sync
     cudaMemPool_t pool;
     if (cudaDeviceGetDefaultMemPool(&pool, device) == cudaSuccess) {
@@ -1535,6 +1545,37 @@ static KnnCall device_call(const double* d_queries, const RowFilters& rf, uint64
   return KnnCall{d_queries, false, rf, row_base, d_out_rows, d_out_dist, d_out_count, false, nullptr};
 }
 
+// ---- ORDER BY vector::<fn>(field, $q) ASC|DESC LIMIT k: the argument checks of sdb_corpus_order_* (unsharded and
+// sharded alike)
+static bool vector_fn_known(int fn) {
+  return (fn >= (int)SDB_CHEBYSHEV && fn <= (int)SDB_PEARSON) || fn == SDB_FN_SIMILARITY_COSINE || fn == SDB_FN_DOT ||
+         fn == SDB_FN_MAGNITUDE;
+}
+sdb_status order_args(Corpus* c, const double* queries, uint32_t nq, int fn, int order, uint32_t k,
+                      const uint32_t* filters, uint32_t n_filters, const uint32_t* query_filter, const uint64_t* out_rows,
+                      const double* out_value, const uint32_t* out_count, Ranking* rank) {
+  if (!c) return SDB_EINVAL;
+  if (!vector_fn_known(fn)) {
+    set_error("sdb_corpus_order: unknown vector function %d", fn);
+    return SDB_EINVAL;
+  }
+  if (order != SDB_ORDER_ASC && order != SDB_ORDER_DESC) {
+    set_error("sdb_corpus_order: unknown order %d", order);
+    return SDB_EINVAL;
+  }
+  if (nq && ((!queries && fn != SDB_FN_MAGNITUDE) || !out_count || (k && (!out_rows || !out_value)))) {
+    set_error("sdb_corpus_order: NULL queries (only SDB_FN_MAGNITUDE takes none) or outputs");
+    return SDB_EINVAL;
+  }
+  if (k > 4096) {
+    set_error("sdb_corpus_order: k = %u exceeds 4096", k);
+    return SDB_EUNSUPPORTED;
+  }
+  if (filters) SDB_TRY(check_filters(nq, filters, n_filters, query_filter));
+  *rank = Ranking{fn, order == SDB_ORDER_DESC};
+  return SDB_OK;
+}
+
 }  // namespace sdb
 extern "C" {
 
@@ -1930,37 +1971,6 @@ sdb_status sdb_knn_submit_filtered(sdb_corpus* c, const double* queries, uint32_
 }
 
 // ---- ORDER BY vector::<fn>(field, $q) ASC|DESC LIMIT k: the brute-force driver with another ranking -----------------
-static bool vector_fn_known(int fn) {
-  return (fn >= (int)SDB_CHEBYSHEV && fn <= (int)SDB_PEARSON) || fn == SDB_FN_SIMILARITY_COSINE || fn == SDB_FN_DOT ||
-         fn == SDB_FN_MAGNITUDE;
-}
-// the checks every sdb_corpus_order_* call shares; host: queries and outputs are host memory
-static sdb_status order_args(sdb_corpus* c, const double* queries, uint32_t nq, int fn, int order, uint32_t k,
-                             const uint32_t* filters, uint32_t n_filters, const uint32_t* query_filter,
-                             const uint64_t* out_rows, const double* out_value, const uint32_t* out_count,
-                             Ranking* rank) {
-  if (!c) return SDB_EINVAL;
-  if (!vector_fn_known(fn)) {
-    set_error("sdb_corpus_order: unknown vector function %d", fn);
-    return SDB_EINVAL;
-  }
-  if (order != SDB_ORDER_ASC && order != SDB_ORDER_DESC) {
-    set_error("sdb_corpus_order: unknown order %d", order);
-    return SDB_EINVAL;
-  }
-  if (nq && ((!queries && fn != SDB_FN_MAGNITUDE) || !out_count || (k && (!out_rows || !out_value)))) {
-    set_error("sdb_corpus_order: NULL queries (only SDB_FN_MAGNITUDE takes none) or outputs");
-    return SDB_EINVAL;
-  }
-  if (k > 4096) {
-    set_error("sdb_corpus_order: k = %u exceeds 4096", k);
-    return SDB_EUNSUPPORTED;
-  }
-  if (filters) SDB_TRY(check_filters(nq, filters, n_filters, query_filter));
-  *rank = Ranking{fn, order == SDB_ORDER_DESC};
-  return SDB_OK;
-}
-
 sdb_status sdb_corpus_order_topk(sdb_corpus* c, const double* queries, uint32_t nq, int fn, int order, uint32_t k,
                                  const uint32_t* filters, uint32_t n_filters, const uint32_t* query_filter,
                                  uint64_t* out_rows, double* out_value, uint32_t* out_count) {
@@ -2064,7 +2074,30 @@ sdb_status sdb_topk_merge_device(sdb_ctx* ctx, uint32_t n_lists, uint32_t nq, ui
   std::lock_guard<std::mutex> g(ctx->mu);
   SDB_CUDA(cudaSetDevice(ctx->device));
   SDB_TRY(topk_merge_launch(ctx, n_lists, nq, k, d_rows, d_dist, d_counts, stride_rows, stride_dist, stride_counts,
-                            d_out_rows, d_out_dist, d_out_count, ctx->stream));
+                            d_out_rows, d_out_dist, d_out_count, false, ctx->stream));
+  SDB_CUDA(cudaStreamSynchronize(ctx->stream));
+  return SDB_OK;
+}
+
+sdb_status sdb_order_merge_device(sdb_ctx* ctx, uint32_t n_lists, uint32_t nq, uint32_t k, int order,
+                                  const uint64_t* d_rows, const double* d_value, const uint32_t* d_counts,
+                                  uint64_t stride_rows, uint64_t stride_value, uint64_t stride_counts,
+                                  uint64_t* d_out_rows, double* d_out_value, uint32_t* d_out_count) {
+  if (!ctx || !n_lists || !k || !d_rows || !d_value || !d_counts || !d_out_rows || !d_out_value || !d_out_count)
+    return SDB_EINVAL;
+  if (order != SDB_ORDER_ASC && order != SDB_ORDER_DESC) {
+    set_error("sdb_order_merge_device: unknown order %d", order);
+    return SDB_EINVAL;
+  }
+  if (k > 4096) {
+    set_error("sdb_order_merge_device: k = %u exceeds 4096", k);
+    return SDB_EUNSUPPORTED;
+  }
+  if (nq == 0) return SDB_OK;
+  std::lock_guard<std::mutex> g(ctx->mu);
+  SDB_CUDA(cudaSetDevice(ctx->device));
+  SDB_TRY(topk_merge_launch(ctx, n_lists, nq, k, d_rows, d_value, d_counts, stride_rows, stride_value, stride_counts,
+                            d_out_rows, d_out_value, d_out_count, order == SDB_ORDER_DESC, ctx->stream));
   SDB_CUDA(cudaStreamSynchronize(ctx->stream));
   return SDB_OK;
 }

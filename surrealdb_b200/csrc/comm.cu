@@ -275,6 +275,7 @@ struct Pending {  // one shard's in-flight sharded batch
   ShardSlot* s = nullptr;
   uint32_t ticket = 0, nq = 0, k = 0;
   int slot = -1;
+  Ranking rank;  // what the batch ranks: the merges (first and repair round) order the blocks in its direction
 };
 
 
@@ -469,14 +470,16 @@ static bool use_p2p(Corpus* c, ShardState* ss) {
 
 // phase A: the local search into this rank's block, header = number of queries this rank must repair on the host.
 // rf: the call's global row filters (rf.bits == nullptr: unfiltered); the driver slices this shard's rows out of them.
+// rank: what the batch ranks (KNN: the default Ranking); the shard's list is its top-k by (order key, global row).
+// host_in: queries and bitmaps are host memory (queries may be NULL for SDB_FN_MAGNITUDE, so their pointer cannot tell).
 // The slot's buffers belong to the batch's ticket slot, so they are free exactly when the ticket is.
-sdb_status phase_local(Corpus* c, const double* d_queries, const double* h_queries, uint32_t nq, uint32_t k,
-                       const RowFilters& rf, uint64_t* d_out_rows, double* d_out_dist, uint32_t* d_out_count,
+sdb_status phase_local(Corpus* c, const double* queries, bool host_in, uint32_t nq, uint32_t k, const RowFilters& rf,
+                       const Ranking& rank, uint64_t* d_out_rows, double* d_out_dist, uint32_t* d_out_count,
                        uint64_t* h_out_rows, double* h_out_dist, uint32_t* h_out_count, Pending* p) {
   if (rf.bits) {  // refused before anything is enqueued
     SDB_TRY(check_filters(nq, rf.bits, rf.n_filters, rf.query_filter));
     if (c->row_base + c->n > rf.n_rows_total) {
-      set_error("sharded filtered KNN: shard rows %llu..%llu outside the bitmaps' %llu rows",
+      set_error("sharded filtered search: shard rows %llu..%llu outside the bitmaps' %llu rows",
                 (unsigned long long)c->row_base, (unsigned long long)(c->row_base + c->n),
                 (unsigned long long)rf.n_rows_total);
       return SDB_EINVAL;
@@ -489,9 +492,9 @@ sdb_status phase_local(Corpus* c, const double* d_queries, const double* h_queri
   const BlockLayout bl = block_layout(nq, k);
   const bool host_out = h_out_count != nullptr;
   SDB_TRY(slot_reserve(c, s, nq, k, host_out));
-  const KnnCall call{h_queries ? h_queries : d_queries, h_queries != nullptr, rf, c->row_base,
+  const KnnCall call{queries, host_in, rf, c->row_base,
                      (uint64_t*)(s.d_block + bl.off_rows), (double*)(s.d_block + bl.off_dist),
-                     (uint32_t*)(s.d_block + bl.off_cnt), false, nullptr};
+                     (uint32_t*)(s.d_block + bl.off_cnt), false, nullptr, rank};
   SDB_TRY(submit_call(c, t, nq, k, call));
   SDB_TRY(knn_shard_header(c, t->id, s.d_block + bl.off_hdr));
   s.d_out_rows = host_out ? s.res.rows : d_out_rows;
@@ -506,6 +509,7 @@ sdb_status phase_local(Corpus* c, const double* d_queries, const double* h_queri
   p->nq = nq;
   p->k = k;
   p->slot = slot;
+  p->rank = rank;
   return SDB_OK;
 }
 
@@ -562,7 +566,8 @@ sdb_status phase_merge(const Pending& p) {
   if (p.k)
     SDB_TRY(topk_merge_launch(c->ctx, (uint32_t)nranks, p.nq, p.k, (const uint64_t*)(s.gather + bl.off_rows),
                               (const double*)(s.gather + bl.off_dist), (const uint32_t*)(s.gather + bl.off_cnt),
-                              s.stride / 8, s.stride / 8, s.stride / 4, s.d_out_rows, s.d_out_dist, s.d_out_count, st));
+                              s.stride / 8, s.stride / 8, s.stride / 4, s.d_out_rows, s.d_out_dist, s.d_out_count,
+                              p.rank.desc, st));
   else SDB_CUDA(cudaMemsetAsync(s.d_out_count, 0, sizeof(uint32_t) * p.nq, st));
   SDB_CUDA(cudaMemcpy2DAsync(s.h_hdr, 16, s.gather + bl.off_hdr, s.stride, 16, (size_t)nranks, cudaMemcpyDeviceToHost, st));
   if (use_p2p(c, ss)) {  // the slot's blocks have been consumed: peers may overwrite them (four batches from now)
@@ -723,8 +728,9 @@ sdb_status sdb_corpus_set_row_base(sdb_corpus* c, uint64_t row_base) {
 }
 
 static sdb_status sharded_submit(sdb_corpus* c, const double* d_queries, const double* h_queries, uint32_t nq, uint32_t k,
-                                 const RowFilters& rf, uint64_t* d_out_rows, double* d_out_dist, uint32_t* d_out_count,
-                                 uint64_t* h_out_rows, double* h_out_dist, uint32_t* h_out_count, uint32_t* ticket) {
+                                 const RowFilters& rf, const Ranking& rank, uint64_t* d_out_rows, double* d_out_dist,
+                                 uint32_t* d_out_count, uint64_t* h_out_rows, double* h_out_dist,
+                                 uint32_t* h_out_count, uint32_t* ticket) {
   if (!c || !ticket || !nq) return SDB_EINVAL;
   if (c->ctx->comm && c->ctx->comm->nranks > 1) SDB_TRY(nccl_load());
   Pending p;
@@ -738,8 +744,9 @@ static sdb_status sharded_submit(sdb_corpus* c, const double* d_queries, const d
       }
       SDB_TRY(arena_ensure_ipc(c, state_of(c), block_layout(nq, k).bytes));
     }
-    SDB_TRY(phase_local(c, d_queries, h_queries, nq, k, rf, d_out_rows, d_out_dist, d_out_count, h_out_rows,
-                        h_out_dist, h_out_count, &p));
+    // the host entry points hand over host outputs, the device ones device outputs
+    SDB_TRY(phase_local(c, h_queries ? h_queries : d_queries, h_out_count != nullptr, nq, k, rf, rank, d_out_rows,
+                        d_out_dist, d_out_count, h_out_rows, h_out_dist, h_out_count, &p));
     sdb_status rc = phase_gather(p);
     if (rc == SDB_OK) rc = phase_merge(p);
     if (rc != SDB_OK) {
@@ -761,14 +768,14 @@ sdb_status sdb_knn_sharded_submit_device(sdb_corpus* c, const double* d_queries,
                                          uint64_t* d_out_rows, double* d_out_dist, uint32_t* d_out_count,
                                          uint32_t* ticket) {
   if (!d_queries || !d_out_count || (k && (!d_out_rows || !d_out_dist))) return SDB_EINVAL;
-  return sharded_submit(c, d_queries, nullptr, nq, k, RowFilters(), d_out_rows, d_out_dist, d_out_count, nullptr, nullptr,
+  return sharded_submit(c, d_queries, nullptr, nq, k, RowFilters(), Ranking(), d_out_rows, d_out_dist, d_out_count, nullptr, nullptr,
                         nullptr, ticket);
 }
 
 sdb_status sdb_knn_sharded_submit(sdb_corpus* c, const double* queries, uint32_t nq, uint32_t k, uint64_t* out_rows,
                                   double* out_dist, uint32_t* out_count, uint32_t* ticket) {
   if (!queries || !out_count || (k && (!out_rows || !out_dist))) return SDB_EINVAL;
-  return sharded_submit(c, nullptr, queries, nq, k, RowFilters(), nullptr, nullptr, nullptr, out_rows, out_dist, out_count,
+  return sharded_submit(c, nullptr, queries, nq, k, RowFilters(), Ranking(), nullptr, nullptr, nullptr, out_rows, out_dist, out_count,
                         ticket);
 }
 
@@ -777,8 +784,8 @@ sdb_status sdb_knn_sharded_submit_filtered(sdb_corpus* c, const double* queries,
                                            uint64_t n_rows_total, uint64_t* out_rows, double* out_dist,
                                            uint32_t* out_count, uint32_t* ticket) {
   if (!filters || !queries || !out_count || (k && (!out_rows || !out_dist))) return SDB_EINVAL;
-  return sharded_submit(c, nullptr, queries, nq, k, RowFilters{filters, n_filters, query_filter, n_rows_total}, nullptr,
-                        nullptr, nullptr, out_rows, out_dist, out_count, ticket);
+  return sharded_submit(c, nullptr, queries, nq, k, RowFilters{filters, n_filters, query_filter, n_rows_total}, Ranking(),
+                        nullptr, nullptr, nullptr, out_rows, out_dist, out_count, ticket);
 }
 
 sdb_status sdb_knn_sharded_submit_filtered_device(sdb_corpus* c, const double* d_queries, uint32_t nq, uint32_t k,
@@ -788,7 +795,7 @@ sdb_status sdb_knn_sharded_submit_filtered_device(sdb_corpus* c, const double* d
                                                   uint32_t* ticket) {
   if (!d_filters || !d_queries || !d_out_count || (k && (!d_out_rows || !d_out_dist))) return SDB_EINVAL;
   return sharded_submit(c, d_queries, nullptr, nq, k, RowFilters{d_filters, n_filters, query_filter, n_rows_total},
-                        d_out_rows, d_out_dist, d_out_count, nullptr, nullptr, nullptr, ticket);
+                        Ranking(), d_out_rows, d_out_dist, d_out_count, nullptr, nullptr, nullptr, ticket);
 }
 
 sdb_status sdb_knn_sharded_wait(sdb_corpus* c, uint32_t ticket) {
@@ -810,9 +817,13 @@ sdb_status sdb_knn_sharded_wait(sdb_corpus* c, uint32_t ticket) {
   return finish_all(&p, 1);
 }
 
+// rank: what the batch ranks; queries may be NULL only for SDB_FN_MAGNITUDE, which takes none
 static sdb_status sharded_multi(sdb_corpus* const* shards, int n, const double* queries, uint32_t nq, uint32_t k,
-                                const RowFilters& rf, uint64_t* out_rows, double* out_dist, uint32_t* out_count) {
-  if (!shards || n < 1 || n > 64 || !queries || !nq || !out_count || (k && (!out_rows || !out_dist))) return SDB_EINVAL;
+                                const RowFilters& rf, const Ranking& rank, uint64_t* out_rows, double* out_dist,
+                                uint32_t* out_count) {
+  if (!shards || n < 1 || n > 64 || (!queries && rank.fn != SDB_FN_MAGNITUDE) || !nq || !out_count ||
+      (k && (!out_rows || !out_dist)))
+    return SDB_EINVAL;
   if (n > 1) SDB_TRY(nccl_load());
   std::vector<Pending> ps((size_t)n);
   std::vector<std::unique_lock<std::mutex>> locks;
@@ -828,10 +839,13 @@ static sdb_status sharded_multi(sdb_corpus* const* shards, int n, const double* 
     cudaSetDevice(shards[i]->ctx->device);
     ShardState* ss = state_of(shards[i]);
     (void)ss;
-    if (i == 0) rc = phase_local(shards[i], nullptr, queries, nq, k, rf, nullptr, nullptr, nullptr, out_rows, out_dist, out_count, &ps[i]);
+    if (i == 0)
+      rc = phase_local(shards[i], queries, true, nq, k, rf, rank, nullptr, nullptr, nullptr, out_rows, out_dist,
+                       out_count, &ps[i]);
     else {
       // the other shards keep their merged copy on the device (slot staging buffers)
-      rc = phase_local(shards[i], nullptr, queries, nq, k, rf, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, &ps[i]);
+      rc = phase_local(shards[i], queries, true, nq, k, rf, rank, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr,
+                       &ps[i]);
       if (rc == SDB_OK) {
         ShardSlot& s = *ps[i].s;
         rc = slot_reserve(shards[i], s, nq, k, true);
@@ -866,7 +880,7 @@ static sdb_status sharded_multi(sdb_corpus* const* shards, int n, const double* 
 
 sdb_status sdb_knn_sharded_multi(sdb_corpus* const* shards, int n, const double* queries, uint32_t nq, uint32_t k,
                                  uint64_t* out_rows, double* out_dist, uint32_t* out_count) {
-  return sharded_multi(shards, n, queries, nq, k, RowFilters(), out_rows, out_dist, out_count);
+  return sharded_multi(shards, n, queries, nq, k, RowFilters(), Ranking(), out_rows, out_dist, out_count);
 }
 
 sdb_status sdb_knn_sharded_multi_filtered(sdb_corpus* const* shards, int n, const double* queries, uint32_t nq,
@@ -874,8 +888,49 @@ sdb_status sdb_knn_sharded_multi_filtered(sdb_corpus* const* shards, int n, cons
                                           const uint32_t* query_filter, uint64_t n_rows_total, uint64_t* out_rows,
                                           double* out_dist, uint32_t* out_count) {
   if (!filters) return SDB_EINVAL;
-  return sharded_multi(shards, n, queries, nq, k, RowFilters{filters, n_filters, query_filter, n_rows_total}, out_rows,
-                       out_dist, out_count);
+  return sharded_multi(shards, n, queries, nq, k, RowFilters{filters, n_filters, query_filter, n_rows_total}, Ranking(),
+                       out_rows, out_dist, out_count);
+}
+
+// ---- ORDER BY vector::<fn>(field, $q) ASC|DESC LIMIT k on a row-sharded column: the sharded driver with the ranking
+// (fn, order).  Every shard returns its top-k by (order key, global row) -- its own order, since a shard's global rows
+// are row_base + its scan positions -- so the union of the blocks holds the global top-k, and the merge in the
+// ranking's direction returns what sdb_corpus_order_topk returns on the unsharded column.
+sdb_status sdb_corpus_order_sharded_submit(sdb_corpus* c, const double* queries, uint32_t nq, int fn, int order,
+                                           uint32_t k, const uint32_t* filters, uint32_t n_filters,
+                                           const uint32_t* query_filter, uint64_t n_rows_total, uint64_t* out_rows,
+                                           double* out_value, uint32_t* out_count, uint32_t* ticket) {
+  Ranking rank;
+  if (!ticket) return SDB_EINVAL;
+  SDB_TRY(order_args(c, queries, nq, fn, order, k, filters, n_filters, query_filter, out_rows, out_value, out_count,
+                     &rank));
+  return sharded_submit(c, nullptr, queries, nq, k, RowFilters{filters, n_filters, query_filter, n_rows_total}, rank,
+                        nullptr, nullptr, nullptr, out_rows, out_value, out_count, ticket);
+}
+
+sdb_status sdb_corpus_order_sharded_submit_device(sdb_corpus* c, const double* d_queries, uint32_t nq, int fn,
+                                                  int order, uint32_t k, const uint32_t* d_filters,
+                                                  uint32_t n_filters, const uint32_t* query_filter,
+                                                  uint64_t n_rows_total, uint64_t* d_out_rows, double* d_out_value,
+                                                  uint32_t* d_out_count, uint32_t* ticket) {
+  Ranking rank;
+  if (!ticket) return SDB_EINVAL;
+  SDB_TRY(order_args(c, d_queries, nq, fn, order, k, d_filters, n_filters, query_filter, d_out_rows, d_out_value,
+                     d_out_count, &rank));
+  return sharded_submit(c, d_queries, nullptr, nq, k, RowFilters{d_filters, n_filters, query_filter, n_rows_total},
+                        rank, d_out_rows, d_out_value, d_out_count, nullptr, nullptr, nullptr, ticket);
+}
+
+sdb_status sdb_corpus_order_sharded_multi(sdb_corpus* const* shards, int n_shards, const double* queries, uint32_t nq,
+                                          int fn, int order, uint32_t k, const uint32_t* filters, uint32_t n_filters,
+                                          const uint32_t* query_filter, uint64_t n_rows_total, uint64_t* out_rows,
+                                          double* out_value, uint32_t* out_count) {
+  Ranking rank;
+  if (!shards || n_shards < 1) return SDB_EINVAL;
+  SDB_TRY(order_args(shards[0], queries, nq, fn, order, k, filters, n_filters, query_filter, out_rows, out_value,
+                     out_count, &rank));
+  return sharded_multi(shards, n_shards, queries, nq, k, RowFilters{filters, n_filters, query_filter, n_rows_total},
+                       rank, out_rows, out_value, out_count);
 }
 
 }  // extern "C"

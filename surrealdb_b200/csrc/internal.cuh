@@ -586,6 +586,11 @@ Ticket* claim_ticket(Corpus* c);
 // stages the call's host inputs on the copy stream and enqueues the batch on the claimed ticket t; the caller holds c->mu
 sdb_status submit_call(Corpus* c, Ticket* t, uint32_t nq, uint32_t k, const KnnCall& call);
 sdb_status check_filters(uint32_t nq, const uint32_t* filters, uint32_t n_filters, const uint32_t* query_filter);
+// the checks every sdb_corpus_order_* call shares (fn, order, NULL queries or outputs, k <= 4096, the filters); *rank is
+// the batch's ranking
+sdb_status order_args(Corpus* c, const double* queries, uint32_t nq, int fn, int order, uint32_t k,
+                      const uint32_t* filters, uint32_t n_filters, const uint32_t* query_filter, const uint64_t* out_rows,
+                      const double* out_value, const uint32_t* out_count, Ranking* rank);
 // by ticket id, for a sharded batch: completion (ladder re-runs, exact fallbacks, statistics), release, the 16-byte
 // block header enqueued into d_hdr, the batch's stream and a trace mark on it
 sdb_status knn_finish_for_shard(Corpus* c, uint32_t ticket, bool* repaired);
@@ -596,7 +601,7 @@ void knn_trace_mark(Corpus* c, uint32_t ticket, const char* name);
 sdb_status topk_merge_launch(Ctx* ctx, uint32_t n_lists, uint32_t nq, uint32_t k, const uint64_t* d_rows,
                              const double* d_dist, const uint32_t* d_counts, uint64_t stride_rows, uint64_t stride_dist,
                              uint64_t stride_counts, uint64_t* d_out_rows, double* d_out_dist, uint32_t* d_out_count,
-                             cudaStream_t st);
+                             bool desc, cudaStream_t st);
 
 // tiling shared by the f32 Lp screen (screen_lp.cu) and the count path (count.cu)
 constexpr int LP_THREADS = 256;

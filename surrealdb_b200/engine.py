@@ -292,6 +292,35 @@ class VectorColumn:
                                                                C.c_void_p(d_out_count), C.byref(t)))
         return t.value
 
+    def order_sharded_submit_host(self, h_queries, nq, k, fn, order, h_out_rows, h_out_values, h_out_count,
+                                  h_filters=None, n_filters=0, query_filter=None, n_rows_total=0):
+        """`ORDER BY vector::<fn>(field, $q) ASC|DESC LIMIT k` on a row-sharded column, collective like
+        sharded_submit_host: raw host pointers (ints, valid until sharded_wait; h_queries 0 for MAGNITUDE), fn and order
+        as in order_topk.  h_filters: optional host bitmaps over the GLOBAL rows (n_filters x ceil(n_rows_total / 32)
+        words); query_filter is a host array (or None)."""
+        qf = _query_filter(query_filter, nq)
+        t = C.c_uint32()
+        L.check(L.lib().sdb_corpus_order_sharded_submit(self.h, C.c_void_p(h_queries or None), int(nq),
+                                                        self._fn_code(fn), self._order_code(order), int(k),
+                                                        C.c_void_p(h_filters or None), int(n_filters),
+                                                        None if qf is None else _ptr(qf), int(n_rows_total),
+                                                        C.c_void_p(h_out_rows), C.c_void_p(h_out_values),
+                                                        C.c_void_p(h_out_count), C.byref(t)))
+        return t.value
+
+    def order_sharded_submit_device(self, d_queries, nq, k, fn, order, d_out_rows, d_out_values, d_out_count,
+                                    d_filters=None, n_filters=0, query_filter=None, n_rows_total=0):
+        """order_sharded_submit_host on device pointers (ints): queries, bitmaps over the GLOBAL rows and outputs"""
+        qf = _query_filter(query_filter, nq)
+        t = C.c_uint32()
+        L.check(L.lib().sdb_corpus_order_sharded_submit_device(self.h, C.c_void_p(d_queries or None), int(nq),
+                                                               self._fn_code(fn), self._order_code(order), int(k),
+                                                               C.c_void_p(d_filters or None), int(n_filters),
+                                                               None if qf is None else _ptr(qf), int(n_rows_total),
+                                                               C.c_void_p(d_out_rows), C.c_void_p(d_out_values),
+                                                               C.c_void_p(d_out_count), C.byref(t)))
+        return t.value
+
     def sharded_wait(self, ticket):
         L.check(L.lib().sdb_knn_sharded_wait(self.h, int(ticket)))
 
@@ -405,6 +434,15 @@ def topk_merge_device(ctx, n_lists, nq, k, d_rows, d_dist, d_counts, d_out_rows,
                                           C.c_void_p(d_out_rows), C.c_void_p(d_out_dist), C.c_void_p(d_out_count)))
 
 
+def order_merge_device(ctx, n_lists, nq, k, order, d_rows, d_values, d_counts, d_out_rows, d_out_values, d_out_count,
+                       stride_rows=0, stride_values=0, stride_counts=0):
+    """topk_merge_device for an ORDER BY ranking: lists and result in (value, row) order for order "ASC" / "DESC"."""
+    L.check(L.lib().sdb_order_merge_device(ctx.h, n_lists, nq, k, VectorColumn._order_code(order), C.c_void_p(d_rows),
+                                           C.c_void_p(d_values), C.c_void_p(d_counts), stride_rows, stride_values,
+                                           stride_counts, C.c_void_p(d_out_rows), C.c_void_p(d_out_values),
+                                           C.c_void_p(d_out_count)))
+
+
 def shard_block_layout(nq, k):
     """byte layout of one rank's result block inside the all-gather buffer:
     rows u64[nq*k] | dist f64[nq*k] | count u32[nq] (padded to 16 bytes)."""
@@ -434,3 +472,31 @@ def knn_sharded_multi(shards, queries, k, filters=None, query_filter=None, n_row
                                                        None if qf is None else _ptr(qf), int(n_rows_total),
                                                        _ptr(rows), _ptr(dist), _ptr(cnt)))
     return rows[:, :k], dist[:, :k], cnt
+
+
+def order_sharded_multi(shards, queries, k, fn, order, filters=None, query_filter=None, n_rows_total=None):
+    """`ORDER BY vector::<fn>(field, $q) ASC|DESC LIMIT k` over one process's N GPUs: shards as in knn_sharded_multi,
+    fn and order as in VectorColumn.order_topk (queries None for "MAGNITUDE", nq = 1), filters over the GLOBAL rows.
+    -> (rows u64 (nq,k), values f64 (nq,k), count u32 (nq,))"""
+    if queries is None:
+        q, nq = None, 1
+    else:
+        q = np.ascontiguousarray(queries, np.float64)
+        if q.ndim == 1:
+            q = q[None, :]
+        nq = q.shape[0]
+    rows = np.zeros((nq, max(k, 1)), np.uint64)
+    vals = np.zeros((nq, max(k, 1)), np.float64)
+    cnt = np.zeros(nq, np.uint32)
+    hs = (C.c_void_p * len(shards))(*[s.h for s in shards])
+    f, qf = None, None
+    if filters is not None:
+        if n_rows_total is None:
+            n_rows_total = max(s.row_base + len(s) for s in shards)
+        f, qf = _filter_args(filters, query_filter, nq, int(n_rows_total))
+    L.check(L.lib().sdb_corpus_order_sharded_multi(hs, len(shards), None if q is None else _ptr(q), nq,
+                                                   VectorColumn._fn_code(fn), VectorColumn._order_code(order), int(k),
+                                                   None if f is None else _ptr(f), 0 if f is None else f.shape[0],
+                                                   None if qf is None else _ptr(qf), int(n_rows_total or 0),
+                                                   _ptr(rows), _ptr(vals), _ptr(cnt)))
+    return rows[:, :k], vals[:, :k], cnt
