@@ -307,12 +307,11 @@ static sdb_status enqueue_direct(Corpus* c, Ticket& t, const Run& r) {
   Scratch& s = c->sets[t.set];
   const View v = view_of(c, t.rank);
   SDB_TRY(scratch_for(c, s, r.nq, DIRECT_MAX_ROWS));
-  SDB_TRY(prep_queries(c, s, r.d_queries, r.nq, st, v, t.rank.desc));
+  SDB_TRY(prep_queries(c, s, r.d_queries, r.nq, st, v));
   SDB_TRY(cand_begin(c, s, r.nq, SDB_SCREEN_NONE_EXACT, st, v));
   SDB_TRY(cand_direct(c, s, r.filt, r.nq, st));
-  SDB_TRY(cand_rerank(c, s, r.filt, r.nq, st, false, t.rank.desc, v));
-  SDB_TRY(cand_final(c, s, r.filt, r.nq, t.k, t.row_base, r.d_out_rows, r.d_out_dist, r.d_out_count, st,
-                     t.rank.desc, v));
+  SDB_TRY(cand_rerank(c, s, r.filt, r.nq, st, false, v));
+  SDB_TRY(cand_final(c, s, r.filt, r.nq, t.k, t.row_base, r.d_out_rows, r.d_out_dist, r.d_out_count, st, v));
   return copy_flags(s, r, st);
 }
 
@@ -369,7 +368,7 @@ static sdb_status enqueue_counted(Corpus* c, Ticket& t, const Run& r, Enqueued* 
   trace_mark(ctx, t, "begin", st);
   const View v = view_of(c, t.rank);
   SDB_TRY(scratch_for(c, s, nq, std::max(4096u, count_ranges(c, nq, k) * k)));
-  SDB_TRY(prep_queries(c, s, r.d_queries, nq, st, v, t.rank.desc));
+  SDB_TRY(prep_queries(c, s, r.d_queries, nq, st, v));
   SDB_TRY(cand_begin(c, s, nq, SDB_SCREEN_NONE_EXACT, st, v));
   if (c->last_main && c->last_main != t.ev_main) SDB_CUDA(cudaStreamWaitEvent(st, c->last_main, 0));
   SDB_CUDA(cudaEventRecord(t.ev_screen0, st));
@@ -383,8 +382,7 @@ static sdb_status enqueue_counted(Corpus* c, Ticket& t, const Run& r, Enqueued* 
   c->last_main = t.ev_main;
   SDB_CUDA(cudaEventRecord(t.ev_screen1, st));
   trace_mark(ctx, t, "counted", st);
-  SDB_TRY(cand_final(c, s, r.filt, nq, k, t.row_base, r.d_out_rows, r.d_out_dist, r.d_out_count, st, t.rank.desc,
-                     v));
+  SDB_TRY(cand_final(c, s, r.filt, nq, k, t.row_base, r.d_out_rows, r.d_out_dist, r.d_out_count, st, v));
   SDB_TRY(copy_flags(s, r, st));
   SDB_CUDA(cudaEventRecord(t.ev_end, st));
   trace_mark(ctx, t, "end", st);
@@ -411,7 +409,7 @@ static sdb_status enqueue_screened(Corpus* c, Ticket& t, const Run& r, Enqueued*
   if (rungs.empty()) {  // exact-only: the exact kernel needs the prepared queries (f64 copy, |q|, flags)
     e->screen = SDB_SCREEN_NONE_EXACT;
     SDB_TRY(scratch_for(c, s, nq, 4096));
-    SDB_TRY(prep_queries(c, s, r.d_queries, nq, st, v, t.rank.desc));
+    SDB_TRY(prep_queries(c, s, r.d_queries, nq, st, v));
     SDB_CUDA(cudaEventRecord(t.ev_screen0, st));
     SDB_CUDA(cudaEventRecord(t.ev_screen1, st));
     SDB_CUDA(cudaMemsetAsync(r.d_out_count, 0, sizeof(uint32_t) * nq, st));
@@ -429,7 +427,7 @@ static sdb_status enqueue_screened(Corpus* c, Ticket& t, const Run& r, Enqueued*
   const bool int8 = rs == SDB_SCREEN_TC_INT8;
   SDB_TRY(scratch_for(c, s, nq, rg.cap));
   const uint32_t cap = s.sc_cap;
-  SDB_TRY(prep_queries(c, s, r.d_queries, nq, st, v, t.rank.desc));
+  SDB_TRY(prep_queries(c, s, r.d_queries, nq, st, v));
   SDB_TRY(cand_begin(c, s, nq, (int)rs, st, v));
   // Screens are persistent one-CTA-per-SM kernels: two of them in flight on different streams would split the SMs,
   // run in two waves and starve the refiners of the CTAs that are not resident yet.  So the screen of this batch waits
@@ -445,7 +443,7 @@ static sdb_status enqueue_screened(Corpus* c, Ticket& t, const Run& r, Enqueued*
       SDB_CUDA(cudaEventRecord(t.ev_main, st));
       c->last_main = t.ev_main;
       if (r.tap) SDB_TRY(tap_gathered(s, r.tap, nq, 0u, st));
-      SDB_TRY(cand_select(c, s, nq, k, int8, 0u, false, st));
+      SDB_TRY(cand_select(c, s, nq, k, int8, 0u, st));
       e->n_passes++;
     } else if (pm.count) {
       SDB_TRY(screen_tc_pass(c, s, r.filt, nq, k, p0, int8, 3, st, v));  // probe: chunk maxima of a few tiles
@@ -456,7 +454,7 @@ static sdb_status enqueue_screened(Corpus* c, Ticket& t, const Run& r, Enqueued*
       SDB_CUDA(cudaEventRecord(t.ev_main, st));
       c->last_main = t.ev_main;
       if (r.tap) SDB_TRY(tap_gathered(s, r.tap, nq, s.last_slots, st));
-      SDB_TRY(cand_select(c, s, nq, k, int8, s.last_slots, false, st));
+      SDB_TRY(cand_select(c, s, nq, k, int8, s.last_slots, st));
       e->n_passes += 2;
     }
   } else {
@@ -472,7 +470,7 @@ static sdb_status enqueue_screened(Corpus* c, Ticket& t, const Run& r, Enqueued*
       else if (family(c) == Family::Lp) SDB_TRY(screen_lp_pass(c, s, r.filt, nq, p, st));
       else SDB_TRY(screen_simt_pass(c, s, r.filt, nq, p, st, v));
       if (r.tap) SDB_TRY(tap_gathered(s, r.tap, nq, tc ? s.last_slots : 0u, st));
-      SDB_TRY(cand_select(c, s, nq, k, int8, tc ? s.last_slots : 0u, false, st));
+      SDB_TRY(cand_select(c, s, nq, k, int8, tc ? s.last_slots : 0u, st));
       first_pass = false;
       e->n_passes++;
     }
@@ -488,15 +486,14 @@ static sdb_status enqueue_screened(Corpus* c, Ticket& t, const Run& r, Enqueued*
   if (tc && c->exact && !no_refine) {
     SDB_TRY(cand_refine(c, s, nq, st, v));
     if (r.tap) SDB_TRY(tap_list(s, nq, &r.tap->list_r, nullptr, st));
-    SDB_TRY(cand_select(c, s, nq, k, false, 0u, false, st, 1));
+    SDB_TRY(cand_select(c, s, nq, k, false, 0u, st, 1));
     refined = true;
     trace_mark(ctx, t, "refined", st);
   }
   if (r.filt.bits) SDB_TRY(cand_add_specials(c, s, r.filt, nq, st, v));  // each query re-ranks its passing special rows
-  SDB_TRY(cand_rerank(c, s, r.filt, nq, st, refined, t.rank.desc, v));
+  SDB_TRY(cand_rerank(c, s, r.filt, nq, st, refined, v));
   trace_mark(ctx, t, "reranked", st);
-  SDB_TRY(cand_final(c, s, r.filt, nq, k, t.row_base, r.d_out_rows, r.d_out_dist, r.d_out_count, st, t.rank.desc,
-                     v));
+  SDB_TRY(cand_final(c, s, r.filt, nq, k, t.row_base, r.d_out_rows, r.d_out_dist, r.d_out_count, st, v));
   trace_mark(ctx, t, "final", st);
   SDB_TRY(copy_flags(s, r, st));
   SDB_CUDA(cudaEventRecord(t.ev_end, st));
@@ -1748,7 +1745,7 @@ static sdb_status debug_screen_batch(sdb_corpus* c, const double* queries, uint3
     SDB_CUDA(cudaMemcpyAsync(d_q, queries, sizeof(double) * (size_t)nq * c->dim, cudaMemcpyHostToDevice, st));
     if (score_all) {  // one pass-0 launch over every tile (SIMT: tau stays -inf), nothing selected
       const PassDesc all{1u, 0u, (uint32_t)(n_pad / TILE_ROWS), 0u};
-      SDB_TRY(prep_queries(c, s, d_q, nq, st, v, rank.desc));
+      SDB_TRY(prep_queries(c, s, d_q, nq, st, v));
       SDB_TRY(cand_begin(c, s, nq, (int)screen, st, v));
       SDB_TRY(tc                ? screen_tc_pass(c, s, t->filt, nq, k, all, int8, 0, st, v)
               : f == Family::Lp ? screen_lp_pass(c, s, t->filt, nq, all, st)
@@ -2051,7 +2048,7 @@ sdb_status sdb_corpus_project(sdb_corpus* c, const double* query, int fn, double
     if (query) SDB_CUDA(cudaMemcpyAsync(d_q, query, sizeof(double) * c->dim, cudaMemcpyHostToDevice, st));
     else SDB_CUDA(cudaMemsetAsync(d_q, 0, sizeof(double) * c->dim, st));
     SDB_TRY(scratch_for(c, s, 1, 4096));
-    SDB_TRY(prep_queries(c, s, d_q, 1, st, view_of(c, Ranking()), false));
+    SDB_TRY(prep_queries(c, s, d_q, 1, st, view_of(c, Ranking())));
     SDB_TRY(exact_project(c, fn, s.d_q64, s.d_qmag, s.d_qflags, d_vals, st));
     SDB_CUDA(cudaMemcpyAsync(out, d_vals, sizeof(double) * c->n, cudaMemcpyDeviceToHost, st));
     return SDB_OK;

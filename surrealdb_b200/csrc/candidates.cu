@@ -620,7 +620,7 @@ sdb_status scratch_for(const Corpus* c, Scratch& s, uint32_t nq, uint32_t cap) {
 }
 
 sdb_status prep_queries(const Corpus* c, Scratch& s, const double* d_queries, uint32_t nq, cudaStream_t st,
-                        const View& v, bool desc) {
+                        const View& v) {
   // d_queries may alias s.d_q64
   if (d_queries != s.d_q64)
     SDB_CUDA(cudaMemcpyAsync(s.d_q64, d_queries, sizeof(double) * (size_t)nq * c->dim, cudaMemcpyDeviceToDevice, st));
@@ -628,7 +628,7 @@ sdb_status prep_queries(const Corpus* c, Scratch& s, const double* d_queries, ui
   const Family f = family(c);
   if (f == Family::Centred)
     prep_queries_pearson_kernel<<<nq_pad, 128, 0, st>>>(s.d_q64, c->dim, c->dim_pad, s.d_q32, s.d_qbf16, s.d_qmag,
-                                                        s.d_qmom, s.d_qflags, s.d_qbferr, nq, desc);
+                                                        s.d_qmom, s.d_qflags, s.d_qbferr, nq, v.desc);
   else if (v.neg || v.sc == Score::Dot || v.cross) {
     // the query rule of the view's score: Cosine and Dot (COSINE's) send a zero or non-finite |q| to the exact kernel
     // -- a cosine view of a EUCLIDEAN corpus with |q| = 0 is NaN for every row --, Euclid / EuclidFar a non-finite one
@@ -840,16 +840,12 @@ sdb_status cand_seed_from_probe(const Corpus* c, Scratch& s, uint32_t nq, uint32
 // than k candidates exist everything is kept and tau stays where it is.  tau only ever rises: all rows with a score
 // >= an earlier tau were appended under thresholds <= that tau, so the kept set always contains every row seen so far
 // whose score reaches the current tau.
-// seed: (re)build the query's histogram for the streaming pass -- geometry from (tau | the score range) and the margin,
-// counts from the kept candidates.
 __global__ void __launch_bounds__(256) cand_select_kernel(Cand* __restrict__ cand, uint32_t* __restrict__ cnt,
                                                            float* __restrict__ tau, uint32_t* __restrict__ flags,
                                                            uint32_t cap, uint32_t k, const float* __restrict__ margin,
                                                            const float* __restrict__ snorm, const Cand* __restrict__ sub,
                                                            const uint32_t* __restrict__ sub_cnt, uint32_t n_slots,
-                                                           uint32_t subcap, HistParam* __restrict__ hparam,
-                                                           uint32_t* __restrict__ hist, const float* __restrict__ qlow,
-                                                           const float* __restrict__ qcap, uint32_t* __restrict__ stat,
+                                                           uint32_t subcap, uint32_t* __restrict__ stat,
                                                            uint64_t* __restrict__ g_keys, uint32_t g_stride) {
   // keys live in a small shared-memory window (the kernel must fit next to a resident screen CTA: 12 KB); a query that
   // gathered more -- a tight cluster -- sorts in its row of the (still unused) re-rank key buffer instead
@@ -972,51 +968,33 @@ __global__ void __launch_bounds__(256) cand_select_kernel(Cand* __restrict__ can
   }
   // ---- keep: everything while no threshold exists; else score >= tau (approximate mode, margin 0: key >= k-th key) ----
   const bool by_key = (k != 0 && n >= k) && !(mg > 0.f) && tau_new == key_to_cand(kth).score;
-  HistParam hp;
-  if (hparam) {
-    const float lo = tau_new > __int_as_float(0xff800000) ? tau_new : qlow[q];
-    float w0 = fmaxf(mg * 0.25f, (qcap[q] - qlow[q]) * 6.1035156e-5f);
-    if (!(w0 > 1e-30f) || !isfinite(w0)) w0 = 1e-30f;
-    hp.lo = lo;
-    hp.w0 = w0;
-    hp.inv_w0 = 1.f / w0;
-    hp.margin = mg;
-    s_hist[threadIdx.x] = 0;
-  }
-  __syncthreads();
   // the kept entries overwrite the head of the main list: positions < n_main were all read during the gather above
   for (uint32_t i = threadIdx.x; i < n; i += blockDim.x) {
     const uint64_t key = s_keys[i];
     const Cand cd = key_to_cand(key);
     const bool keep = by_key ? key >= kth : cd.score >= tau_new;  // tau_new = -inf keeps everything
-    if (keep) {
-      cq[atomicAdd(&s_out, 1u)] = cd;
-      if (hparam) atomicAdd(&s_hist[hist_bin(hp, cd.score)], 1u);
-    }
+    if (keep) cq[atomicAdd(&s_out, 1u)] = cd;
   }
   __syncthreads();
   if (threadIdx.x == 0) {
     tau[q] = tau_new;
     cnt[q] = s_out;
-    if (hparam) hparam[q] = hp;
   }
-  if (hparam) hist[(size_t)q * HIST_BINS + threadIdx.x] = s_hist[threadIdx.x];
 }
 
 sdb_status cand_select(const Corpus* c, Scratch& s, uint32_t nq, uint32_t k, bool drop_invalid, uint32_t n_slots,
-                       bool seed_hist, cudaStream_t st, int stage) {
+                       cudaStream_t st, int stage) {
   if (stage == 1) {  // stage B: the lists hold f32 scores now; own threshold / margin, nothing else to gather
     cand_select_kernel<<<nq, 256, 0, st>>>(s.d_cand, s.d_cand_cnt, s.d_tau2, s.d_flags, s.sc_cap, k, s.d_margin2,
-                                           nullptr, s.d_sub, s.d_sub_cnt, 0u, s.sub_cap, nullptr, s.d_hist, s.d_qlow,
-                                           s.d_qcap, nullptr, s.d_rr_key, s.rr_stride);
+                                           nullptr, s.d_sub, s.d_sub_cnt, 0u, s.sub_cap, nullptr, s.d_rr_key,
+                                           s.rr_stride);
     count_launch(c->ctx);
     SDB_CUDA(cudaGetLastError());
     return SDB_OK;
   }
   cand_select_kernel<<<nq, 256, 0, st>>>(  // 256 threads: several blocks per SM, the whole batch is one wave
       s.d_cand, s.d_cand_cnt, s.d_tau, s.d_flags, s.sc_cap, k, s.d_margin, drop_invalid ? c->d_snorm.get() : nullptr,
-      s.d_sub, s.d_sub_cnt, n_slots, s.sub_cap, seed_hist ? s.d_hparam.get() : nullptr, s.d_hist, s.d_qlow, s.d_qcap,
-      s.d_stat, s.d_rr_key, s.rr_stride);
+      s.d_sub, s.d_sub_cnt, n_slots, s.sub_cap, s.d_stat, s.d_rr_key, s.rr_stride);
   count_launch(c->ctx);
   SDB_CUDA(cudaGetLastError());
   return SDB_OK;
@@ -1471,23 +1449,21 @@ static void rerank_entry(const Corpus* c, Scratch& s, uint32_t nq, uint32_t n_sp
 }
 
 template <typename T>
-static void rerank_packed(const Corpus* c, Scratch& s, uint32_t nq, uint32_t n_sp, bool desc, const View& v,
-                          cudaStream_t st) {
+static void rerank_packed(const Corpus* c, Scratch& s, uint32_t nq, uint32_t n_sp, const View& v, cudaStream_t st) {
   auto kern = v.steps == SDB_FN_DOT ? cand_rerank_packed_kernel<T, SDB_FN_DOT>
               : v.steps == SDB_COSINE ? cand_rerank_packed_kernel<T, SDB_COSINE>
                                       : cand_rerank_packed_kernel<T, SDB_EUCLIDEAN>;
   kern<<<(nq + 7) / 8, 128, 0, st>>>((const T*)c->d_rows.get(), c->dim, c->d_mag, s.d_q64, s.d_qmag, s.d_qflags,
                                      s.d_cand, s.d_cand_cnt, s.sc_cap, view_special(c, v), n_sp, nq,
-                                     rr_out(s, desc, v.sim));
+                                     rr_out(s, v.desc, v.sim));
 }
 
 // COSINE / EUCLIDEAN: the packed kernel for the small sets stage B leaves; otherwise the vectorised one for f32 rows
 // of a length divisible by 4, the staged one for the rest
 template <bool DOT>
-static void rerank_wide(const Corpus* c, Scratch& s, uint32_t nq, uint32_t n_sp, bool desc, const View& v,
-                        cudaStream_t st) {
+static void rerank_wide(const Corpus* c, Scratch& s, uint32_t nq, uint32_t n_sp, const View& v, cudaStream_t st) {
   const dim3 grid(nq, RR_GROUPS_Y);
-  const RerankOut out = rr_out(s, desc, v.sim);
+  const RerankOut out = rr_out(s, v.desc, v.sim);
   const int metric = DOT ? (int)SDB_COSINE : v.steps;
   const uint32_t* sp = view_special(c, v);
   if (c->dtype == SDB_F32 && c->dim % 4 == 0)
@@ -1503,33 +1479,33 @@ static void rerank_wide(const Corpus* c, Scratch& s, uint32_t nq, uint32_t n_sp,
                                                                    c->d_mag, s.d_q64, s.d_qmag, s.d_qflags, s.d_cand,
                                                                    s.d_cand_cnt, s.sc_cap, sp, n_sp, out);
 }
-static void rerank_dot(const Corpus* c, Scratch& s, uint32_t nq, bool small_sets, uint32_t n_sp, bool desc,
-                       const View& v, cudaStream_t st) {
-  if (small_sets && c->dtype == SDB_F32) rerank_packed<float>(c, s, nq, n_sp, desc, v, st);
-  else if (small_sets) rerank_packed<double>(c, s, nq, n_sp, desc, v, st);
-  else if (v.sc == Score::Dot) rerank_wide<true>(c, s, nq, n_sp, desc, v, st);
-  else rerank_wide<false>(c, s, nq, n_sp, desc, v, st);
+static void rerank_dot(const Corpus* c, Scratch& s, uint32_t nq, bool small_sets, uint32_t n_sp, const View& v,
+                       cudaStream_t st) {
+  if (small_sets && c->dtype == SDB_F32) rerank_packed<float>(c, s, nq, n_sp, v, st);
+  else if (small_sets) rerank_packed<double>(c, s, nq, n_sp, v, st);
+  else if (v.sc == Score::Dot) rerank_wide<true>(c, s, nq, n_sp, v, st);
+  else rerank_wide<false>(c, s, nq, n_sp, v, st);
 }
 
 sdb_status cand_rerank(const Corpus* c, Scratch& s, const FiltArg& filt, uint32_t nq, cudaStream_t st,
-                       bool small_sets, bool desc, const View& v) {
+                       bool small_sets, const View& v) {
   const uint32_t n_sp = filt.bits ? 0u : view_n_special(c, v);  // filtered: the passing special rows are in the lists
   switch (family(c)) {
     case Family::Count:  // (the direct regime only; no special rows)
-      if (c->metric == SDB_HAMMING) rerank_entry<SDB_HAMMING>(c, s, nq, n_sp, desc, st);
-      else rerank_entry<SDB_JACCARD>(c, s, nq, n_sp, desc, st);
+      if (c->metric == SDB_HAMMING) rerank_entry<SDB_HAMMING>(c, s, nq, n_sp, v.desc, st);
+      else rerank_entry<SDB_JACCARD>(c, s, nq, n_sp, v.desc, st);
       break;
     case Family::Lp:
-      if (c->metric == SDB_MANHATTAN) rerank_entry<SDB_MANHATTAN>(c, s, nq, n_sp, desc, st);
-      else if (c->metric == SDB_MINKOWSKI) rerank_entry<SDB_MINKOWSKI>(c, s, nq, n_sp, desc, st);
-      else rerank_entry<SDB_CHEBYSHEV>(c, s, nq, n_sp, desc, st);
+      if (c->metric == SDB_MANHATTAN) rerank_entry<SDB_MANHATTAN>(c, s, nq, n_sp, v.desc, st);
+      else if (c->metric == SDB_MINKOWSKI) rerank_entry<SDB_MINKOWSKI>(c, s, nq, n_sp, v.desc, st);
+      else rerank_entry<SDB_CHEBYSHEV>(c, s, nq, n_sp, v.desc, st);
       break;
     case Family::Centred:  // one kernel for small (after stage B) and large (direct regime, no stage B) sets
-      rerank_entry<SDB_PEARSON>(c, s, nq, n_sp, desc, st);
+      rerank_entry<SDB_PEARSON>(c, s, nq, n_sp, v.desc, st);
       break;
     case Family::Dot:
     case Family::Exact:  // (never reaches the re-rank: the exact kernel alone ranks it)
-      rerank_dot(c, s, nq, small_sets, n_sp, desc, v, st);
+      rerank_dot(c, s, nq, small_sets, n_sp, v, st);
       break;
   }
   count_launch(c->ctx);
@@ -1566,22 +1542,76 @@ __device__ __forceinline__ void bitonic_pairs(uint64_t* s_key, uint64_t* s_idx, 
   }
 }
 
-// The proof of the family F's bound: Dot (cosine / euclidean, also the count path's lists, whose tau stays -inf), Lp, or
-// Centred (the cosine proof on the centred operands, eps_ref = the gap between their cosine and the reference's
-// pearson, DESIGN.md section 2; 0 for the other families).  DOT: Score::Dot batches of Dot corpora, whose eps_ref is the
-// reference's relative rounding times max_norm (per unit of |q|).  kind, neg: the view's score (View::sc as an int) and
-// query sign, on which the Dot family's other proofs switch; EuclidFar's eps_ref is the reference's relative rounding
-// of the euclidean distance
-template <Family F, bool DOT = false>
+// What a batch's screens scored, and so which bound the proof derives from a threshold (cand_final picks it from the
+// corpus family and the view):
+//   Dot        Score::Dot batches; eps_ref = the reference's relative rounding of the dot times max_norm (per |q|)
+//   Lp         Lp corpora
+//   Centred    the cosine of the centred operands (PEARSON); eps_ref = the gap between it and the reference's pearson
+//              (DESIGN.md section 2)
+//   CosineNeg  Score::Cosine against the copy of -q (cosine distance DESC, similarity ASC)
+//   EuclidFar  Score::EuclidFar; eps_ref = the reference's relative rounding of the euclidean distance
+//   Cosine     Score::Cosine against the copy of q
+//   Euclid     Score::Euclid; also the count path's lists, whose tau stays -inf
+enum class Proof { Dot, Lp, Centred, CosineNeg, EuclidFar, Cosine, Euclid };
+
+// The least key, in the batch's direction, that a row the threshold t excluded can have: its screened score is below t,
+// the screen's error is at most beps and its scores are in units of bscale / |q| (stage B: tau2, beps2, bscale 1).
+// 0 when the form gives no bound (a NaN or non-positive intermediate): no k-th key is below it, so nothing is proven.
+template <Proof P>
+__device__ __forceinline__ uint64_t proof_bound(float t, float bscale, float beps, double qm, double eps_ref,
+                                                bool desc) {
+  if (P == Proof::Dot) {
+    // (cand_begin_dot_kernel) a non-candidate's dot with the screened query (q DESC, -q ASC) is at most t + beps, and
+    // the reference's sequential f64 dot -- the value keyed -- is within eps_ref |q| of the real one.  DESC: value <= U
+    // = t + beps + eps_ref |q|; ASC: value >= -U.  U is rounded up (so -U down)
+    const double U = __dadd_ru(__dadd_ru((double)t, (double)beps), __dmul_ru(eps_ref, qm));
+    return U == U ? order_key(desc ? U : -U, desc) : 0;
+  } else if (P == Proof::Lp) {
+    // score = -s~ < t for a non-candidate, so s~ > -t and d >= s~ - beps > -t - beps, rounded down.  No stage B runs
+    // (tau2 = -inf)
+    return dist_key((-(double)t - (double)beps) * (1.0 - 1e-12));
+  } else if (P == Proof::Centred) {
+    // the screen scored s = cos(dx, +-dq) |dq| / bscale (+dq DESC).  DESC: cos(dx, dq) <= t bscale / |dq| + beps  =>
+    // pearson <= a + beps + eps_ref; ASC: cos(dx, dq) >= -a - beps  =>  pearson >= -a - beps - eps_ref; each bound
+    // evaluated with directed rounding so that it is rounded outward
+    const double a = __ddiv_ru(__dmul_ru((double)t, (double)bscale), qm);
+    if (desc) return order_key(__dadd_ru(__dadd_ru(a, (double)beps), eps_ref), true);
+    return dist_key(__dsub_rd(__dsub_rd(-a, (double)beps), eps_ref));
+  } else if (P == Proof::CosineNeg) {
+    // cos(x, -q) <= U = t bscale / |q| + beps, and the reference's value is within 1e-9 of the real one: sim >= -U,
+    // dist = 1 - sim <= 1 + U.  U is rounded up; DESC keys the distance's upper bound, ASC the similarity's lower one
+    const double U = __dadd_ru(__dadd_ru(__ddiv_ru(__dmul_ru((double)t, (double)bscale), qm), (double)beps), 1e-9);
+    return U == U ? (desc ? order_key(__dadd_ru(1.0, U), true) : dist_key(-U)) : 0;
+  } else if (P == Proof::EuclidFar) {
+    // 2 x.(-q)~ + |x|^2~ < t for a non-candidate, so d^2 - |q|^2 = |x|^2 - 2 x.q <= t + beps: d^2 <= U = t + beps
+    // + |q|^2 (+ the reference's f64 underflow), rounded up, and the reference's distance is at most sqrt(U)
+    // (1 + eps_ref), rounded up (keyed descending)
+    const double U = __dadd_ru(__dadd_ru(__dadd_ru((double)t, (double)beps), __dmul_ru(qm, qm)), 0x1p-1000);
+    const double d = __dmul_ru(__dsqrt_ru(fmax(U, 0.0)), 1.0 + eps_ref);
+    return U == U ? order_key(d, true) : 0;
+  } else if (P == Proof::Cosine) {
+    // non-candidate: score <= t  =>  sim <= t bscale / |q| + eps.  DESC (similarity descending): that upper bound;
+    // ASC: dist >= 1 - t bscale / |q| - eps
+    if (desc) return order_key((double)t * (double)bscale / qm + (double)beps + 1e-9, true);
+    return dist_key(1.0 - (double)t * (double)bscale / qm - (double)beps - 1e-9);
+  } else {
+    // score = 2 dot~ - |x|^2~ <= t  =>  d^2 = |x|^2 - 2 dot + |q|^2 >= -t + |q|^2 - eps_e.  |q|^2 - t is one fused
+    // rounding: written out, the product the two thresholds share may be computed once and rounded on its own
+    const double L = fma(qm, qm, -(double)t) - (double)beps;
+    return L > 0.0 ? dist_key(sqrt(L) * (1.0 - 1e-12)) : 0;
+  }
+}
+
+template <Proof P>
 __global__ void __launch_bounds__(256)
     cand_final_kernel(const uint64_t* __restrict__ rr_key, const double* __restrict__ rr_dist,
                       const uint32_t* __restrict__ rr_row, uint32_t rr_stride, const uint32_t* __restrict__ cnt,
                       uint32_t cap, uint32_t n_special, const float* __restrict__ tau, const double* __restrict__ qmag,
                       const float* __restrict__ bscale, const float* __restrict__ beps, const float* __restrict__ tau2,
                       const float* __restrict__ beps2, uint32_t* __restrict__ flags, const uint32_t* __restrict__ qflags,
-                      uint32_t* __restrict__ stat, int metric, uint32_t k, uint64_t row_base,
-                      uint64_t* __restrict__ out_rows, double* __restrict__ out_dist, uint32_t* __restrict__ out_count,
-                      int debug, double eps_ref, bool desc, int kind, bool neg) {
+                      uint32_t* __restrict__ stat, uint32_t k, uint64_t row_base, uint64_t* __restrict__ out_rows,
+                      double* __restrict__ out_dist, uint32_t* __restrict__ out_count, int debug, double eps_ref,
+                      bool desc) {
   __shared__ uint64_t s_key[FIN_WIN];  // distance key
   __shared__ uint64_t s_idx[FIN_WIN];  // (row << 32 | entry): secondary order by row (unique), entry = index into rr_*
   const uint32_t q = blockIdx.x;
@@ -1633,93 +1663,14 @@ __global__ void __launch_bounds__(256)
     if (t > __int_as_float(0xff800000) && n_e >= k && k > 0) {  // tau == -inf: every screened-in row is a candidate
       const double qm = qmag[q];
       const uint64_t kth = s_key[k - 1];
-      bool ok;
-      if (DOT) {
-        // Score::Dot (cand_begin_dot_kernel): a non-candidate's screened score is below tau, so its dot with the
-        // screened query (q DESC, -q ASC) is at most tau + beps, and the reference's sequential f64 dot -- the value
-        // keyed -- is within eps_ref |q| of the real one.  DESC: value <= U = tau + beps + eps_ref |q|; ASC: value >= -U.
-        // U is rounded up (so -U down); proven when that bound sorts strictly after the k-th entry
-        const double U = __dadd_ru(__dadd_ru((double)t, (double)beps[q]), __dmul_ru(eps_ref, qm));
-        ok = U == U && order_key(desc ? U : -U, desc) > kth;
-      } else if (F == Family::Lp) {
-        // score = -s~ < tau for a non-candidate, so s~ > -tau and d >= s~ - beps > -tau - beps: the row cannot reach
-        // the top k if that bound (rounded down) is strictly above the k-th exact key.  No stage B ran (tau2 = -inf).
-        const double L = (-(double)t - (double)beps[q]) * (1.0 - 1e-12);
-        ok = dist_key(L) > kth;
-      } else if (F == Family::Centred && desc) {
-        // PEARSON DESC: the screen scored s = cos(dx, +dq) |dq| / bscale and the entries are pearsons keyed descending.
-        // Non-candidate: cos(dx, dq) <= tau bscale / |dq| + beps  =>  pearson <= tau bscale / |dq| + beps + eps_ref,
-        // rounded up; proven when that upper bound sorts strictly after the k-th entry
-        const double a = __ddiv_ru(__dmul_ru((double)t, (double)bscale[q]), qm);
-        const double U = __dadd_ru(__dadd_ru(a, (double)beps[q]), eps_ref);
-        ok = order_key(U, true) > kth;
-      } else if (F == Family::Centred) {
-        // the screen scored s = cos(dx, -dq) |dq| / bscale.  Non-candidate: score <= tau  =>  cos(dx, dq) >= -tau
-        // bscale / |dq| - beps  =>  pearson >= -tau bscale / |dq| - beps - eps_ref, evaluated with directed rounding
-        // so that the bound itself is rounded down
-        const double a = __ddiv_ru(__dmul_ru((double)t, (double)bscale[q]), qm);
-        const double L = __dsub_rd(__dsub_rd(-a, (double)beps[q]), eps_ref);
-        ok = dist_key(L) > kth;
-      } else if (kind == (int)Score::Cosine && neg) {
-        // the copy of -q (cosine distance DESC, similarity ASC): a non-candidate has cos(x, -q) <= U = tau bscale / |q|
-        // + beps, and the reference's value is within 1e-9 of the real one: sim >= -U, dist = 1 - sim <= 1 + U.  U is
-        // rounded up; proven when that bound sorts strictly after the k-th entry in the batch's direction
-        const double U = __dadd_ru(__dadd_ru(__ddiv_ru(__dmul_ru((double)t, (double)bscale[q]), qm), (double)beps[q]), 1e-9);
-        ok = U == U && (desc ? order_key(__dadd_ru(1.0, U), true) : dist_key(-U)) > kth;
-      } else if (kind == (int)Score::EuclidFar) {
-        // 2 x.(-q)~ + |x|^2~ < tau for a non-candidate, so d^2 - |q|^2 = |x|^2 - 2 x.q <= tau + beps: d^2 <= U = tau + beps
-        // + |q|^2 (+ the reference's f64 underflow), rounded up, and the reference's distance is at most
-        // sqrt(U) (1 + eps_ref), rounded up; proven when that bound sorts strictly after the k-th entry (descending)
-        const double U = __dadd_ru(__dadd_ru(__dadd_ru((double)t, (double)beps[q]), __dmul_ru(qm, qm)), 0x1p-1000);
-        const double d = __dmul_ru(__dsqrt_ru(fmax(U, 0.0)), 1.0 + eps_ref);
-        ok = U == U && order_key(d, true) > kth;
-      } else if (kind == (int)Score::Cosine && desc) {
-        // similarity descending: the entries are similarities keyed descending.  Non-candidate: sim <= tau * bscale /
-        // |q| + eps, so it cannot reach the top k if that upper bound sorts strictly after the k-th entry
-        const double upper = (double)t * (double)bscale[q] / qm + (double)beps[q] + 1e-9;
-        ok = order_key(upper, true) > kth;
-      } else if (kind == (int)Score::Cosine) {
-        // non-candidate: score <= tau  =>  sim <= tau * bscale / |q| + eps  =>  dist >= 1 - tau * bscale / |q| - eps
-        const double bound = 1.0 - (double)t * (double)bscale[q] / qm - (double)beps[q] - 1e-9;
-        ok = dist_key(bound) > kth;
-      } else {
-        // score = 2 dot~ - |x|^2~ <= tau  =>  d^2 = |x|^2 - 2 dot + |q|^2 >= -tau + |q|^2 - eps_e
-        const double L = -(double)t + qm * qm - (double)beps[q];
-        ok = L > 0.0 && dist_key(sqrt(L) * (1.0 - 1e-12)) > kth;
-      }
-      // stage B dropped candidates whose f32 score is below tau2: the same proof with the f32 bound
+      // proven when the bound sorts strictly after the k-th entry
+      bool ok = proof_bound<P>(t, bscale[q], beps[q], qm, eps_ref, desc) > kth;
+      // stage B dropped candidates whose f32 score is below tau2: the same proof with the f32 bound (bscale 1)
       const float t2 = tau2[q];
-      if (ok && t2 > __int_as_float(0xff800000)) {
-        if (DOT) {
-          const double U2 = __dadd_ru(__dadd_ru((double)t2, (double)beps2[q]), __dmul_ru(eps_ref, qm));
-          ok = U2 == U2 && order_key(desc ? U2 : -U2, desc) > kth;
-        } else if (F == Family::Centred && desc) {
-          const double U2 = __dadd_ru(__dadd_ru(__ddiv_ru((double)t2, qm), (double)beps2[q]), eps_ref);
-          ok = order_key(U2, true) > kth;
-        } else if (F == Family::Centred) {  // stage B scores in the same units with bscale 1
-          const double L2 = __dsub_rd(__dsub_rd(-__ddiv_ru((double)t2, qm), (double)beps2[q]), eps_ref);
-          ok = dist_key(L2) > kth;
-        } else if (kind == (int)Score::Cosine && neg) {  // stage B scores in similarity x |q| units (bscale 1)
-          const double U2 = __dadd_ru(__dadd_ru(__ddiv_ru((double)t2, qm), (double)beps2[q]), 1e-9);
-          ok = U2 == U2 && (desc ? order_key(__dadd_ru(1.0, U2), true) : dist_key(-U2)) > kth;
-        } else if (kind == (int)Score::EuclidFar) {
-          const double U2 = __dadd_ru(__dadd_ru(__dadd_ru((double)t2, (double)beps2[q]), __dmul_ru(qm, qm)), 0x1p-1000);
-          const double d2 = __dmul_ru(__dsqrt_ru(fmax(U2, 0.0)), 1.0 + eps_ref);
-          ok = U2 == U2 && order_key(d2, true) > kth;
-        } else if (kind == (int)Score::Cosine && desc) {
-          const double upper2 = (double)t2 / qm + (double)beps2[q] + 1e-9;
-          ok = order_key(upper2, true) > kth;
-        } else if (kind == (int)Score::Cosine) {
-          const double bound2 = 1.0 - (double)t2 / qm - (double)beps2[q] - 1e-9;
-          ok = dist_key(bound2) > kth;
-        } else {
-          const double L2 = -(double)t2 + qm * qm - (double)beps2[q];
-          ok = L2 > 0.0 && dist_key(sqrt(L2) * (1.0 - 1e-12)) > kth;
-        }
-      }
+      if (ok && t2 > __int_as_float(0xff800000)) ok = proof_bound<P>(t2, 1.f, beps2[q], qm, eps_ref, desc) > kth;
       if (!ok) fl |= 2u;
       if (debug && q == 0)
-        printf("[sdb final] q0 metric=%d tau=%g qmag=%g beps=%g n_e=%u kth_key=%llx ok=%d\n", metric, (double)t, qm,
+        printf("[sdb final] q0 proof=%d tau=%g qmag=%g beps=%g n_e=%u kth_key=%llx ok=%d\n", (int)P, (double)t, qm,
                (double)beps[q], n_e, (unsigned long long)kth, (int)ok);
     }
     if (fl & 1u) fl |= 2u;  // overflowed candidate buffer => exact re-run
@@ -1731,7 +1682,7 @@ __global__ void __launch_bounds__(256)
 }
 
 sdb_status cand_final(const Corpus* c, Scratch& s, const FiltArg& filt, uint32_t nq, uint32_t k, uint64_t row_base,
-                      uint64_t* d_out_rows, double* d_out_dist, uint32_t* d_out_count, cudaStream_t st, bool desc,
+                      uint64_t* d_out_rows, double* d_out_dist, uint32_t* d_out_count, cudaStream_t st,
                       const View& v) {
   if (k > FIN_KEEP) {
     set_error("cand_final: k = %u exceeds the screened path's limit of %u", k, FIN_KEEP);
@@ -1739,38 +1690,40 @@ sdb_status cand_final(const Corpus* c, Scratch& s, const FiltArg& filt, uint32_t
   }
   static const int debug = getenv("SDB_DEBUG") != nullptr;
   const uint32_t n_sp = filt.bits ? 0u : view_n_special(c, v);  // filtered: the passing special rows are in the lists
-  auto fin = cand_final_kernel<Family::Dot>;
+  auto fin = cand_final_kernel<Proof::Euclid>;
   double eps_ref = 0.0;
   switch (family(c)) {
     case Family::Dot:
       if (v.sc == Score::EuclidFar) {
+        fin = cand_final_kernel<Proof::EuclidFar>;
         // the reference's distance sqrt(sum (x_i - q_i)^2) in sequential f64: D roundings of differences, squares and
         // sums err by at most (D + 2) 2^-53 relative on the sum (gamma_D), the square root halves that and adds 2^-53
         eps_ref = (c->dim + 4.0) * 0x1p-53;
       } else if (v.sc == Score::Dot) {
-        fin = cand_final_kernel<Family::Dot, true>;
+        fin = cand_final_kernel<Proof::Dot>;
         // the reference's sequential f64 dot of D terms errs by at most gamma_D sum |x_i q_i| <= gamma_D |x||q|,
         // gamma_D = D 2^-53 / (1 - D 2^-53) <= (D + 2) 2^-53; |x| <= max_norm; (1 + 2^-20) covers the rounding of
         // |q| (qmag) and of this figure
         eps_ref = (c->dim + 2.0) * 0x1p-53 * (double)c->max_norm * (1.0 + 0x1p-20);
+      } else if (v.sc == Score::Cosine) {
+        fin = v.neg ? cand_final_kernel<Proof::CosineNeg> : cand_final_kernel<Proof::Cosine>;
       }
       break;
     case Family::Count:  // (tau = -inf: nothing to prove)
     case Family::Exact:  // (never reaches cand_final)
       break;
     case Family::Centred:
-      fin = cand_final_kernel<Family::Centred>;
+      fin = cand_final_kernel<Proof::Centred>;
       // |pearson - cos(dx, dq)| <= (2 D + 6) 2^-53 to first order (DESIGN.md section 2); +2 covers the rest
       eps_ref = (2.0 * c->dim + 8.0) * 0x1p-53;
       break;
     case Family::Lp:
-      fin = cand_final_kernel<Family::Lp>;
+      fin = cand_final_kernel<Proof::Lp>;
       break;
   }
   fin<<<nq, 256, 0, st>>>(s.d_rr_key, s.d_rr_dist, s.d_rr_row, s.rr_stride, s.d_cand_cnt, s.sc_cap, n_sp,
                           s.d_tau, s.d_qmag, s.d_bscale, s.d_beps, s.d_tau2, s.d_beps2, s.d_flags, s.d_qflags,
-                          s.d_stat, (int)c->metric, k, row_base, d_out_rows, d_out_dist, d_out_count, debug, eps_ref,
-                          desc, (int)v.sc, v.neg);
+                          s.d_stat, k, row_base, d_out_rows, d_out_dist, d_out_count, debug, eps_ref, v.desc);
   count_launch(c->ctx);
   SDB_CUDA(cudaGetLastError());
   return SDB_OK;

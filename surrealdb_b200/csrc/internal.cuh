@@ -542,9 +542,11 @@ struct View {
   bool cross = false;  // per-row array and special list: the cross state (d_xnorm, d_xspecial), else d_snorm, d_special
   int steps = SDB_EUCLIDEAN;  // the re-rank's accumulation: SDB_COSINE (x.q), SDB_EUCLIDEAN ((x - q)^2), SDB_FN_DOT
   bool sim = false;    // ... and its finish: the cosine similarity instead of the cosine distance
+  bool desc = false;   // the ranking's direction (Ranking::desc): the re-rank keys descending, cand_final proves that
 };
 inline View view_of(const Corpus* c, const Ranking& r) {
   View v;
+  v.desc = r.desc;
   if (dot_ranking(c, r)) {
     v.sc = Score::Dot, v.neg = !r.desc, v.steps = SDB_FN_DOT;
   } else if (cross_ranking(c, r) && r.fn != SDB_EUCLIDEAN) {
@@ -640,20 +642,20 @@ bool screen_tc_available();
 // candidates.cu
 // grows s to nq queries x cap candidates (a set that grows loses its contents)
 sdb_status scratch_for(const Corpus* c, Scratch& s, uint32_t nq, uint32_t cap);
-// v, desc: the batch's view and direction.  Centred: desc takes the screen copies of +dq / |dq| (a metric_desc batch)
-// instead of -dq / |dq|; Dot corpora: View::neg takes the screen copies of -q (the re-rank keeps q)
+// v: the batch's view.  Centred: View::desc takes the screen copies of +dq / |dq| (a metric_desc batch) instead of
+// -dq / |dq|; Dot corpora: View::neg takes the screen copies of -q (the re-rank keeps q)
 sdb_status prep_queries(const Corpus* c, Scratch& s, const double* d_queries, uint32_t nq, cudaStream_t st,
-                        const View& v, bool desc);
+                        const View& v);
 // one query prepared into the fallback scratch (d_fb_*), independent of the batch scratch
 sdb_status prep_fallback_query(Corpus* c, const double* d_query, cudaStream_t st);
 // resets tau / counts / flags and derives, per query, the screen's error bound, the selection margin and the score range
 sdb_status cand_begin(const Corpus* c, Scratch& s, uint32_t nq, int screen, cudaStream_t st, const View& v);
 sdb_status cand_set_count(const Corpus* c, Scratch& s, uint32_t nq, uint32_t value, cudaStream_t st);
 // per query: gather the main list + the private sub-lists, find the k-th best score s_k, keep every candidate with
-// score >= tau = s_k - margin (all of them while fewer than k exist), publish tau.  seed_hist: also (re)build the
-// query's histogram (geometry + counts of the kept candidates) for the streaming pass that follows.
+// score >= tau = s_k - margin (all of them while fewer than k exist), publish tau.  (The streaming pass's histogram is
+// seeded by cand_seed_from_probe.)
 sdb_status cand_select(const Corpus* c, Scratch& s, uint32_t nq, uint32_t k, bool drop_invalid, uint32_t n_slots,
-                       bool seed_hist, cudaStream_t st, int stage = 0);
+                       cudaStream_t st, int stage = 0);
 // stage B: re-score every kept candidate in f32 (master rows x f32 query) so that cand_select(stage 1) can shrink the
 // set before the FP64-bound exact re-rank
 sdb_status cand_refine(const Corpus* c, Scratch& s, uint32_t nq, cudaStream_t st, const View& v);
@@ -669,13 +671,13 @@ sdb_status cand_add_specials(const Corpus* c, Scratch& s, const FiltArg& filt, u
                              const View& v);
 // direct regime (filtered): each query's list = the rows its filter passes that are neither skipped nor removed
 sdb_status cand_direct(const Corpus* c, Scratch& s, const FiltArg& filt, uint32_t nq, cudaStream_t st);
-// desc (the descending screened rankings): the re-rank keys its values descending, and cand_final proves that order.
-// v (Dot corpora): the re-rank computes the view's function (View::steps, View::sim) over its special list, and
+// View::desc (the descending screened rankings): the re-rank keys its values descending, and cand_final proves that
+// order.  v (Dot corpora): the re-rank computes the view's function (View::steps, View::sim) over its special list, and
 // cand_final proves the order with the bound of the view's score
 sdb_status cand_rerank(const Corpus* c, Scratch& s, const FiltArg& filt, uint32_t nq, cudaStream_t st,
-                       bool small_sets, bool desc, const View& v);
+                       bool small_sets, const View& v);
 sdb_status cand_final(const Corpus* c, Scratch& s, const FiltArg& filt, uint32_t nq, uint32_t k, uint64_t row_base,
-                      uint64_t* d_out_rows, double* d_out_dist, uint32_t* d_out_count, cudaStream_t st, bool desc,
+                      uint64_t* d_out_rows, double* d_out_dist, uint32_t* d_out_count, cudaStream_t st,
                       const View& v);
 // exact.cu: query vector / |q| / flags are passed explicitly (a batch scratch row or the fallback scratch).
 // filter: nullptr, or the query's bitmap (filter_words words): rows whose bit is clear are not ranked.
