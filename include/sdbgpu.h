@@ -255,7 +255,10 @@ sdb_status sdb_corpus_read_rows(sdb_corpus*, uint64_t first_row, uint64_t n, voi
  * MINKOWSKI goes through pow(): CUDA's libm here, the platform libm in the reference -- each call agrees to within an
  * ulp or two, so Minkowski distances are equal to ~1e-14 relative rather than bit for bit (every other metric is
  * bit-exact).  Integer orders 1 .. 8 are screened (f32 Lp screen + exact re-rank), every other order is ranked by the
- * exact kernel; the order may change after finalize. */
+ * exact kernel; the order may change after finalize, but not while a batch of the corpus is in flight (between a submit
+ * and its wait): the kernels of that batch read the order when they run.
+ * The screen, schedule and exact settings below apply to the batches submitted after the call: a batch in flight keeps
+ * the screen, schedule and exact mode it was submitted with, its repairs at wait time included. */
 sdb_status sdb_corpus_set_minkowski_order(sdb_corpus*, double order);
 sdb_status sdb_corpus_set_screen(sdb_corpus*, sdb_screen);
 /* schedule of the tensor-core screens (results are identical; tuning / A-B only).  streaming = 1 (default): a scored

@@ -18,19 +18,8 @@ void set_error(const char* fmt, ...) {
 
 
 // schedule ratio of the LEGACY multi-pass schedule (f32 SIMT screen; tensor-core screens when streaming refinement is
-// switched off): every pass looks at (R-1) x the rows seen so far; SDB_PASS_RATIO overrides it (tuning only)
-static uint32_t pass_ratio(uint32_t nq) {
-  static int env = -1;
-  if (env < 0) {
-    env = 0;
-    if (const char* e = getenv("SDB_PASS_RATIO")) {
-      const int v = atoi(e);
-      if (v >= 2 && v <= 64) env = v;
-    }
-  }
-  if (env) return (uint32_t)env;
-  return nq >= 512 ? 4u : PASS_RATIO;
-}
+// switched off): every pass looks at (R-1) x the rows seen so far
+static uint32_t pass_ratio(uint32_t nq) { return nq >= 512 ? 4u : PASS_RATIO; }
 
 static std::vector<PassDesc> build_passes(uint64_t n_rows, uint32_t cand_cap, uint32_t nq) {
   std::vector<PassDesc> v;
@@ -73,17 +62,13 @@ static void build_stream_passes(uint64_t n_rows, uint32_t cand_cap, uint32_t k, 
     probe->count = (uint32_t)T;
     return;
   }
-  uint64_t P = k <= 32 ? 16 : PROBE_TILES_MAX;  // 8 chunk maxima per tile: 128 / 512 values >= 4 k / 2 k
-  if (const char* e = getenv("SDB_PROBE_TILES")) {  // tuning knob: a larger probe starts the thresholds higher
-    const int v = atoi(e);
-    if (v >= (int)P && v <= (int)PROBE_TILES_MAX) P = (uint64_t)v;
-  }
+  const uint64_t P = k <= 32 ? 16 : PROBE_TILES_MAX;  // 8 chunk maxima per tile: 128 / 512 values >= 4 k / 2 k
   const uint64_t stride = T / P;                       // T > max0 >= 16; for P = 64 and T < 64 every tile is probed
   if (stride == 0) *probe = PassDesc{1u, 0u, (uint32_t)T, 0u};
   else *probe = PassDesc{(uint32_t)stride, 0u, (uint32_t)P, 0u};
   const uint32_t cnt = (uint32_t)T;
   uint32_t perm = 0;
-  if (cnt >= 8 && !getenv("SDB_STREAM_INORDER")) {
+  if (cnt >= 8) {
     perm = (uint32_t)(cnt * 0.6180339887498949) | 1u;
     while (gcd_u32(perm, cnt) != 1) perm += 2;
     if (perm >= cnt) perm = 0;
@@ -91,19 +76,37 @@ static void build_stream_passes(uint64_t n_rows, uint32_t cand_cap, uint32_t k, 
   *main = PassDesc{1u, 0u, cnt, perm};
 }
 
-struct Rung {
-  sdb_screen scr;
-  uint32_t cap;  // candidate-list capacity per query
-};
+// The plan of a batch of nq queries ranked by `rank`, k results each, under the screen and tensor-core schedule asked
+// for (the corpus' settings, or those a debug batch names).
 // The precision ladder, cheapest first.  The candidate set of a query is "every row whose screened score is within the
 // screen's error margin of the k-th best", so its size adapts to the data (a handful on spread-out data, a whole
 // cluster on tightly packed data); a rung fails for a query only when that set overflows the list.  When that happens
 // to more than a handful of queries the batch is re-screened with a tighter screen / longer lists instead of paying
-// one exact pass over the corpus per failed query; the rung that worked is remembered per corpus and k.
-// screen: the corpus' screen choice (Corpus::screen, or the one a debug batch asks for)
-static std::vector<Rung> build_rungs(const Corpus* c, sdb_screen screen, uint32_t k, uint32_t nq, const Ranking& rank,
-                                     sdb_screen* first) {
+// one exact pass over the corpus per failed query; the rung that worked is remembered per corpus, k and view.
+static Plan plan_batch(const Corpus* c, const Ranking& rank, uint32_t k, uint32_t nq, sdb_screen screen,
+                       bool stream_refine) {
+  Plan p;
   const Family f = family(c);
+  const bool screened = screened_ranking(c, rank), counted = screened && count_ranked(c, k, screen);
+  p.rank = rank;
+  p.v = view_of(c, rank);
+  p.stream_refine = stream_refine;
+  p.exact = c->exact;
+  // direct regime: the re-rank and cand_final serve every family but Exact (Count: when the count path would rank the
+  // batch), k <= 256
+  p.direct_ok =
+      k > 0 && k <= 256 && screened && (f == Family::Dot || f == Family::Centred || f == Family::Lp || counted);
+  if (nq == 0 || k == 0) return p;  // Route::Empty: nothing to search
+  // vector::dot and the cross views were ranked by the exact kernel, which reports a cancel raised while a batch is in
+  // flight (it polls before every query); on the screens they still report it, from the wait
+  p.cancel_at_wait = dot_ranking(c, rank) || cross_ranking(c, rank);
+  // MANHATTAN / CHEBYSHEV: a single query streams the rows once either way, and the exact kernel does it at the higher
+  // HBM rate (DESIGN.md section 5): AUTO ranks it there; an explicit SIMT_F32 request is kept.  MINKOWSKI's exact
+  // kernel is bound by its f64 pow() calls, not by HBM, and the screen is faster for a single query too (section 5).
+  // HAMMING likewise: AUTO ranks one query with the exact kernel; JACCARD's exact kernel is O(D^2) per row, so the
+  // count path takes a single query too.
+  p.single_exact = screen == SDB_SCREEN_AUTO &&
+                   (c->metric == SDB_MANHATTAN || c->metric == SDB_CHEBYSHEV || c->metric == SDB_HAMMING);
   const bool int8_ok = c->d_i8 && screen_tc_available();  // (COSINE and Centred corpora hold an int8 copy)
   sdb_screen scr = screen;
   if (scr == SDB_SCREEN_AUTO)
@@ -113,8 +116,7 @@ static std::vector<Rung> build_rungs(const Corpus* c, sdb_screen screen, uint32_
   // the int8 copy holds x / |x| and its integer threshold compare takes no per-row scale: only the cosine score on the
   // own screening norm runs on it (towards q or -q, whose int8 copy is the negation of q's); dot batches and the
   // other views start on bf16
-  const View v = view_of(c, rank);
-  if (scr == SDB_SCREEN_TC_INT8 && (v.sc != Score::Cosine || v.cross)) scr = SDB_SCREEN_TC_BF16;
+  if (scr == SDB_SCREEN_TC_INT8 && (p.v.sc != Score::Cosine || p.v.cross)) scr = SDB_SCREEN_TC_BF16;
   // (Lp corpora hold no bf16 copy: the f32 Lp screen, screen_lp.cu, is their only screen, for f32 and f64 rows)
   if (scr == SDB_SCREEN_TC_BF16 && (!screen_tc_available() || !c->d_bf16)) scr = SDB_SCREEN_SIMT_F32;
   // the SIMT screen streams f32 rows: an f64 Dot corpus is screened on the tensor cores or not at all, and so is a
@@ -124,32 +126,33 @@ static std::vector<Rung> build_rungs(const Corpus* c, sdb_screen screen, uint32_
   // (Count: the count path, enqueue_counted, or the exact kernel)
   if (c->special_overflow || k > 256 || f == Family::Count || f == Family::Exact) scr = SDB_SCREEN_NONE_EXACT;
   // a view on the cross state whose special list overflowed
-  if (v.cross && c->xspecial_overflow) scr = SDB_SCREEN_NONE_EXACT;
+  if (p.v.cross && c->xspecial_overflow) scr = SDB_SCREEN_NONE_EXACT;
   // a ranking the screens do not serve (screened_ranking): the exact kernel
-  if (!screened_ranking(c, rank)) scr = SDB_SCREEN_NONE_EXACT;
-  // MANHATTAN / CHEBYSHEV: a single query streams the rows once either way, and the exact kernel does it at the higher
-  // HBM rate (DESIGN.md section 5): AUTO ranks it there; an explicit SIMT_F32 request is kept.  MINKOWSKI's exact
-  // kernel is bound by its f64 pow() calls, not by HBM, and the screen is faster for a single query too (section 5).
-  if (f == Family::Lp && c->metric != SDB_MINKOWSKI && nq == 1 && screen == SDB_SCREEN_AUTO)
-    scr = SDB_SCREEN_NONE_EXACT;
-  *first = scr;
-  std::vector<Rung> r;
-  if (scr == SDB_SCREEN_TC_INT8)
-    r = {{SDB_SCREEN_TC_INT8, 4096}, {SDB_SCREEN_TC_INT8, 16384}, {SDB_SCREEN_TC_BF16, 4096}, {SDB_SCREEN_TC_BF16, 16384}};
-  else if (scr == SDB_SCREEN_TC_BF16) r = {{SDB_SCREEN_TC_BF16, 4096}, {SDB_SCREEN_TC_BF16, 16384}};
-  else if (scr == SDB_SCREEN_SIMT_F32 && f == Family::Lp) r = {{SDB_SCREEN_SIMT_F32, 4096}, {SDB_SCREEN_SIMT_F32, 16384}};
-  else if (scr == SDB_SCREEN_SIMT_F32) r = {{SDB_SCREEN_SIMT_F32, 4096}};
+  if (!screened) scr = SDB_SCREEN_NONE_EXACT;
+  auto push = [&](sdb_screen s, uint32_t cap) { p.ladder[p.n_ladder++] = Rung{s, cap}; };
+  if (scr == SDB_SCREEN_TC_INT8) {
+    push(SDB_SCREEN_TC_INT8, 4096), push(SDB_SCREEN_TC_INT8, 16384);
+    push(SDB_SCREEN_TC_BF16, 4096), push(SDB_SCREEN_TC_BF16, 16384);
+  } else if (scr == SDB_SCREEN_TC_BF16) {
+    push(SDB_SCREEN_TC_BF16, 4096), push(SDB_SCREEN_TC_BF16, 16384);
+  } else if (scr == SDB_SCREEN_SIMT_F32 && f == Family::Lp) {
+    push(SDB_SCREEN_SIMT_F32, 4096), push(SDB_SCREEN_SIMT_F32, 16384);
+  } else if (scr == SDB_SCREEN_SIMT_F32) {
+    push(SDB_SCREEN_SIMT_F32, 4096);
+  }
   // the f32 stream (error bound ~500x tighter than bf16) as the last rung before the exact kernel -- only ever used
   // for the few queries of a batch that every tensor-core rung failed to prove (finish_local), never for a whole batch
-  if (!r.empty() && r.back().scr != SDB_SCREEN_SIMT_F32 && c->dtype == SDB_F32 && f == Family::Dot)
-    r.push_back({SDB_SCREEN_SIMT_F32, 4096});
-  return r;
-}
-static uint32_t n_batch_rungs(const std::vector<Rung>& r) {  // rungs a WHOLE batch may be re-screened on
-  uint32_t n = (uint32_t)r.size();
-  // (the f32 stream behind tensor-core rungs is for single queries; an all-SIMT ladder re-screens whole batches)
-  if (n > 1 && r.back().scr == SDB_SCREEN_SIMT_F32 && r[n - 2].scr != SDB_SCREEN_SIMT_F32) n--;
-  return n;
+  if (p.n_ladder && p.ladder[p.n_ladder - 1].scr != SDB_SCREEN_SIMT_F32 && c->dtype == SDB_F32 && f == Family::Dot)
+    push(SDB_SCREEN_SIMT_F32, 4096);
+  p.route = counted ? Plan::Route::Counted : p.n_ladder ? Plan::Route::Screened : Plan::Route::Exact;
+  // the whole batch: its first-choice screen and the rungs it may be re-screened on (the f32 stream behind tensor-core
+  // rungs is for single queries; an all-SIMT ladder re-screens whole batches)
+  const uint32_t n = p.rungs(nq);
+  const bool f32_tail =
+      n > 1 && p.ladder[n - 1].scr == SDB_SCREEN_SIMT_F32 && p.ladder[n - 2].scr != SDB_SCREEN_SIMT_F32;
+  p.n_batch_rungs = f32_tail ? n - 1 : n;
+  p.key = RungKey{n ? p.ladder[0].scr : SDB_SCREEN_NONE_EXACT, k, view_key(p.v)};
+  return p;
 }
 
 static cudaError_t drain(Ctx* ctx) {  // both batch streams idle
@@ -273,7 +276,7 @@ static sdb_status scatter_results(Corpus* c, Ticket& t) {
 }
 
 // One run of the enqueue functions: a whole batch, the screened head or the direct tail of a mixed one, or the failed
-// queries of a per-query repair.  The ticket holds what every run of the batch shares: stream, scratch set, k,
+// queries of a per-query repair.  The ticket holds what every run of the batch shares: plan, stream, scratch set, k,
 // row_base, events and cancel flag.
 struct Run {
   const double* d_queries;
@@ -281,8 +284,6 @@ struct Run {
   uint64_t* d_out_rows; double* d_out_dist; uint32_t* d_out_count;
   FiltArg filt;
   uint32_t rung;
-  sdb_screen screen;   // the screen asked for (Corpus::screen, or a debug batch's)
-  bool stream_refine;  // ... and the tensor-core schedule (Corpus::stream_refine)
   ScreenTap* tap;      // test-only (see ScreenTap)
   uint32_t *h_flags, *h_qflags;  // pinned: where the run's per-query flags go
   uint32_t* h_stat;              // pinned: where its counters go (nullptr: nowhere)
@@ -305,10 +306,10 @@ static sdb_status copy_flags(const Scratch& s, const Run& r, cudaStream_t st) {
 static sdb_status enqueue_direct(Corpus* c, Ticket& t, const Run& r) {
   cudaStream_t st = t.stream;
   Scratch& s = c->sets[t.set];
-  const View v = view_of(c, t.rank);
+  const View& v = t.plan.v;
   SDB_TRY(scratch_for(c, s, r.nq, DIRECT_MAX_ROWS));
   SDB_TRY(prep_queries(c, s, r.d_queries, r.nq, st, v));
-  SDB_TRY(cand_begin(c, s, r.nq, SDB_SCREEN_NONE_EXACT, st, v));
+  SDB_TRY(cand_begin(c, s, r.nq, SDB_SCREEN_NONE_EXACT, st, v, t.plan.exact));
   SDB_TRY(cand_direct(c, s, r.filt, r.nq, st));
   SDB_TRY(cand_rerank(c, s, r.filt, r.nq, st, false, v));
   SDB_TRY(cand_final(c, s, r.filt, r.nq, t.k, t.row_base, r.d_out_rows, r.d_out_dist, r.d_out_count, st, v));
@@ -366,10 +367,10 @@ static sdb_status enqueue_counted(Corpus* c, Ticket& t, const Run& r, Enqueued* 
   e->n_passes = 1;
   SDB_CUDA(cudaEventRecord(t.ev_begin, st));
   trace_mark(ctx, t, "begin", st);
-  const View v = view_of(c, t.rank);
+  const View& v = t.plan.v;
   SDB_TRY(scratch_for(c, s, nq, std::max(4096u, count_ranges(c, nq, k) * k)));
   SDB_TRY(prep_queries(c, s, r.d_queries, nq, st, v));
-  SDB_TRY(cand_begin(c, s, nq, SDB_SCREEN_NONE_EXACT, st, v));
+  SDB_TRY(cand_begin(c, s, nq, SDB_SCREEN_NONE_EXACT, st, v, t.plan.exact));
   if (c->last_main && c->last_main != t.ev_main) SDB_CUDA(cudaStreamWaitEvent(st, c->last_main, 0));
   SDB_CUDA(cudaEventRecord(t.ev_screen0, st));
   if ((t.cancel && *t.cancel) || ctx_cancelled(ctx)) {
@@ -377,7 +378,7 @@ static sdb_status enqueue_counted(Corpus* c, Ticket& t, const Run& r, Enqueued* 
     set_error("query cancelled");
     return SDB_ECANCELLED;
   }
-  SDB_TRY(count_pass(c, s, r.filt, nq, k, st, t.rank.desc));
+  SDB_TRY(count_pass(c, s, r.filt, nq, k, st, v.desc));
   SDB_CUDA(cudaEventRecord(t.ev_main, st));
   c->last_main = t.ev_main;
   SDB_CUDA(cudaEventRecord(t.ev_screen1, st));
@@ -394,19 +395,14 @@ static sdb_status enqueue_screened(Corpus* c, Ticket& t, const Run& r, Enqueued*
   cudaStream_t st = t.stream;
   Scratch& s = c->sets[t.set];
   const uint32_t nq = r.nq, k = t.k;
-  const View v = view_of(c, t.rank);
-  // HAMMING: AUTO ranks a batch of one query with the exact kernel, which streams the rows once at the higher rate
-  // (DESIGN.md section 5); an explicit screen request still counts it.  JACCARD's exact kernel is O(D^2) per row: the
-  // count path takes a single query too
-  if (screened_ranking(c, t.rank) && count_ranked(c, k) &&
-      (nq > 1 || r.screen != SDB_SCREEN_AUTO || c->metric == SDB_JACCARD))
-    return enqueue_counted(c, t, r, e);
-  sdb_screen first;
-  const std::vector<Rung> rungs = build_rungs(c, r.screen, k, nq, t.rank, &first);
+  const Plan& plan = t.plan;
+  const View& v = plan.v;
+  if (plan.counted(nq)) return enqueue_counted(c, t, r, e);
+  const uint32_t n_rungs = plan.rungs(nq);
   e->n_passes = 0;
   SDB_CUDA(cudaEventRecord(t.ev_begin, st));
   trace_mark(ctx, t, "begin", st);
-  if (rungs.empty()) {  // exact-only: the exact kernel needs the prepared queries (f64 copy, |q|, flags)
+  if (n_rungs == 0) {  // exact-only: the exact kernel needs the prepared queries (f64 copy, |q|, flags)
     e->screen = SDB_SCREEN_NONE_EXACT;
     SDB_TRY(scratch_for(c, s, nq, 4096));
     SDB_TRY(prep_queries(c, s, r.d_queries, nq, st, v));
@@ -420,7 +416,7 @@ static sdb_status enqueue_screened(Corpus* c, Ticket& t, const Run& r, Enqueued*
     SDB_CUDA(cudaEventRecord(t.ev_end, st));
     return SDB_OK;
   }
-  const Rung rg = rungs[std::min<size_t>(r.rung, rungs.size() - 1)];
+  const Rung rg = plan.ladder[std::min(r.rung, n_rungs - 1)];
   const sdb_screen rs = rg.scr;
   e->screen = (int)rs;
   const bool tc = rs == SDB_SCREEN_TC_INT8 || rs == SDB_SCREEN_TC_BF16;
@@ -428,14 +424,14 @@ static sdb_status enqueue_screened(Corpus* c, Ticket& t, const Run& r, Enqueued*
   SDB_TRY(scratch_for(c, s, nq, rg.cap));
   const uint32_t cap = s.sc_cap;
   SDB_TRY(prep_queries(c, s, r.d_queries, nq, st, v));
-  SDB_TRY(cand_begin(c, s, nq, (int)rs, st, v));
+  SDB_TRY(cand_begin(c, s, nq, (int)rs, st, v, plan.exact));
   // Screens are persistent one-CTA-per-SM kernels: two of them in flight on different streams would split the SMs,
   // run in two waves and starve the refiners of the CTAs that are not resident yet.  So the screen of this batch waits
   // for the end of the previous batch's screen -- only the TAIL of the previous batch overlaps with it.
   if (c->last_main && c->last_main != t.ev_main) SDB_CUDA(cudaStreamWaitEvent(st, c->last_main, 0));
   SDB_CUDA(cudaEventRecord(t.ev_screen0, st));  // after the wait: screen_ms is this batch's screen, not the queueing
   trace_mark(ctx, t, "screen0", st);
-  if (tc && r.stream_refine) {
+  if (tc && plan.stream_refine) {
     PassDesc p0, pm;
     build_stream_passes(c->n, cap, k, &p0, &pm);
     if (p0.count && !pm.count) {  // the whole corpus fits the lists: score everything once
@@ -481,9 +477,8 @@ static sdb_status enqueue_screened(Corpus* c, Ticket& t, const Run& r, Enqueued*
   SDB_CUDA(cudaEventRecord(t.ev_screen1, st));
   trace_mark(ctx, t, "selected", st);
   // stage B: the coarse screens' candidates are re-scored in f32 and narrowed before the (FP64-bound) exact re-rank
-  static const bool no_refine = getenv("SDB_NO_REFINE") != nullptr;
   bool refined = false;
-  if (tc && c->exact && !no_refine) {
+  if (tc && plan.exact) {
     SDB_TRY(cand_refine(c, s, nq, st, v));
     if (r.tap) SDB_TRY(tap_list(s, nq, &r.tap->list_r, nullptr, st));
     SDB_TRY(cand_select(c, s, nq, k, false, 0u, st, 1));
@@ -503,8 +498,8 @@ static sdb_status enqueue_screened(Corpus* c, Ticket& t, const Run& r, Enqueued*
 
 // the whole batch at its rung, with what it decided recorded on the ticket
 static sdb_status enqueue_ticket(Corpus* c, Ticket& t) {
-  const Run r{t.d_queries, t.nq, t.d_out_rows, t.d_out_dist, t.d_out_count, t.filt, t.rung, c->screen,
-              c->stream_refine, nullptr, t.h_flags, t.h_qflags, t.h_stat};
+  const Run r{t.d_queries, t.nq, t.d_out_rows, t.d_out_dist, t.d_out_count, t.filt, t.rung, nullptr,
+              t.h_flags, t.h_qflags, t.h_stat};
   Enqueued e;
   SDB_TRY(enqueue_batch(c, t, r, &e));
   t.screen = e.screen;
@@ -524,23 +519,29 @@ static sdb_status copy_out(Corpus* c, Ticket& t) {  // host-buffer entry points:
   return SDB_OK;
 }
 
+// rungs the batch's screened queries may climb, which a mixed batch screens on their own (those of the whole batch when
+// every query is direct).  0: the batch ran no screen whose counters stay on the device -- exact-only, counted, empty,
+// or a mixed batch whose one screened query took the exact kernel -- and the host holds its counters.
+static uint32_t screened_rungs(const Ticket& t) {
+  return t.plan.rungs(t.n_direct < t.nq ? t.nq - t.n_direct : t.nq);
+}
+
 // local (this shard's) part of the completion: ladder re-runs and exact fallbacks.  *repaired = the device result
 // changed after the batch's own kernels had produced it.
 static sdb_status finish_local(Corpus* c, Ticket& t, uint32_t* n_fallback, bool* repaired) {
   Ctx* ctx = c->ctx;
   cudaStream_t st = t.stream;
-  const uint32_t nq = t.nq, k = t.k;
+  const Plan& p = t.plan;
+  const uint32_t nq = t.nq, k = t.k, n_rungs = screened_rungs(t);
   *repaired = false;
   *n_fallback = 0;
   SDB_CUDA(cudaEventSynchronize(t.ev_end));
-  // vector::dot and the cross views were ranked by the exact kernel, which reports a cancel raised while a batch is in
-  // flight (it polls before every query); on the screens they still report it, here
-  if ((dot_ranking(c, t.rank) || cross_ranking(c, t.rank)) && nq && k && ((t.cancel && *t.cancel) || ctx_cancelled(ctx))) {
+  if (p.cancel_at_wait && ((t.cancel && *t.cancel) || ctx_cancelled(ctx))) {
     set_error("query cancelled");
     return SDB_ECANCELLED;
   }
-  if (t.screen != SDB_SCREEN_NONE_EXACT && c->exact) {
-    while (t.rung + 1 < t.n_batch_rungs) {  // many failures: the whole batch moves up one rung (and stays there)
+  if (t.screen != SDB_SCREEN_NONE_EXACT && p.exact) {
+    while (t.rung + 1 < p.n_batch_rungs) {  // many failures: the whole batch moves up one rung (and stays there)
       uint32_t n_fail = 0;
       for (uint32_t q = 0; q < nq; q++) n_fail += (t.h_flags[q] & 2u) ? 1u : 0u;
       if (n_fail <= 2 + nq / 64) break;
@@ -551,27 +552,20 @@ static sdb_status finish_local(Corpus* c, Ticket& t, uint32_t* n_fallback, bool*
       *repaired = true;
     }
   }
-  if (t.n_rungs) {
-    sdb_screen first;
-    build_rungs(c, c->screen, k, nq, t.rank, &first);
-    c->rung_scr = first;
-    c->rung_k = k;
-    c->rung_view = view_key(view_of(c, t.rank));
-    c->rung = t.rung;
-  }
+  if (n_rungs) c->remembered = {p.key, t.rung};
   // ---- what the batch's rung could not prove ----
   std::vector<uint32_t> fails, exacts;
   for (uint32_t q = 0; q < nq; q++) {
     if (t.h_qflags[q] & 1u) exacts.push_back(q);  // zero / non-finite query norm: ranked by the exact kernel
-    else if ((t.h_flags[q] & 2u) && (c->exact || t.screen == SDB_SCREEN_NONE_EXACT)) fails.push_back(q);
+    else if ((t.h_flags[q] & 2u) && (p.exact || t.screen == SDB_SCREEN_NONE_EXACT)) fails.push_back(q);
   }
   if (fails.empty() && exacts.empty()) return SDB_OK;
   SDB_CUDA(drain(ctx));  // the repair below shares scratch (and the exact kernel's keys) with every batch in flight
   // A few failures: only THOSE queries climb the remaining rungs, as a small batch of their own (a bf16 pass over the
   // corpus costs about as much for 60 queries as for 1, and far less than one sequential-f64 pass per query); the f32
   // stream is the last rung.  Whatever is still unproven after that goes to the exact kernel.
-  if (!fails.empty() && t.screen != SDB_SCREEN_NONE_EXACT && c->exact && k) {
-    for (uint32_t rung = t.rung + 1; rung < t.n_rungs && !fails.empty(); rung++) {
+  if (!fails.empty() && t.screen != SDB_SCREEN_NONE_EXACT && p.exact && k) {
+    for (uint32_t rung = t.rung + 1; rung < n_rungs && !fails.empty(); rung++) {
       if ((t.cancel && *t.cancel) || ctx_cancelled(ctx)) break;
       const uint32_t nf = (uint32_t)fails.size();
       const size_t need_q = (size_t)nf * c->dim, need_o = (size_t)nf * k;
@@ -598,8 +592,8 @@ static sdb_status finish_local(Corpus* c, Ticket& t, uint32_t* n_fallback, bool*
       }
       // the failed queries are screened ones (a direct query's proof cannot fail); their flags go to the batch's first
       // entries, which were read above
-      const Run rp{c->d_rp_q, nf, c->rp.rows, c->rp.dist, c->rp.count, filt, rung, c->screen, c->stream_refine,
-                   nullptr, t.h_flags, t.h_qflags, nullptr};
+      const Run rp{c->d_rp_q, nf, c->rp.rows, c->rp.dist, c->rp.count, filt, rung, nullptr, t.h_flags, t.h_qflags,
+                   nullptr};
       Enqueued ignored;
       SDB_TRY(enqueue_screened(c, t, rp, &ignored));
       SDB_CUDA(cudaEventSynchronize(t.ev_end));
@@ -631,7 +625,7 @@ static sdb_status finish_local(Corpus* c, Ticket& t, uint32_t* n_fallback, bool*
     SDB_TRY(prep_fallback_query(c, t.d_queries + (size_t)q * c->dim, st));
     const uint32_t* q_filter = t.filt.bits ? t.filt.bits + (size_t)t.h_qf[q] * t.filt.words : nullptr;
     SDB_TRY(exact_query(c, c->d_fb_q, c->d_fb_qmag, c->d_fb_qflags, k, t.row_base, t.d_out_rows + (size_t)q * k,
-                        t.d_out_dist + (size_t)q * k, t.d_out_count + q, st, q_filter, t.filt.words, t.rank));
+                        t.d_out_dist + (size_t)q * k, t.d_out_count + q, st, q_filter, t.filt.words, p.rank));
     (*n_fallback)++;
     *repaired = true;
   }
@@ -679,9 +673,10 @@ static void release_ticket(Ticket& t) {
   t.h_out_count = nullptr;
 }
 
-// filtered batch (submit_locked, sdb_debug_screen_batch_filtered): the per query filter index on the host (exact
-// fallbacks, repairs), the direct / screened split (query indices in batch order) and FiltArg::mask_hits
-static void plan_filtered(const Corpus* c, Ticket& t, uint32_t nq, uint32_t k, const uint32_t* d_filters,
+// filtered batch (submit_locked, sdb_debug_screen_batch_filtered), on a ticket whose plan is set: the per query filter
+// index on the host (exact fallbacks, repairs), the direct / screened split (query indices in batch order) and
+// FiltArg::mask_hits
+static void plan_filtered(const Corpus* c, Ticket& t, uint32_t nq, const uint32_t* d_filters,
                           const uint32_t* query_filter, const uint64_t* filter_rows, std::vector<uint32_t>* scr,
                           std::vector<uint32_t>* dir) {
   t.h_qf.assign(nq, 0u);
@@ -689,11 +684,8 @@ static void plan_filtered(const Corpus* c, Ticket& t, uint32_t nq, uint32_t k, c
   t.filt.bits = d_filters;
   t.filt.words = (uint32_t)((c->n + 31) / 32);
   // direct regime: a query whose filter passes at most DIRECT_MAX_ROWS rows (filter_rows: set bits, an upper bound
-  // of the rows it passes) skips the screen; the re-rank and cand_final serve every family but Exact (Count: when the
-  // count path would rank the batch), k <= 256
-  const Family f = family(c);
-  const bool direct_ok = filter_rows && k > 0 && k <= 256 && screened_ranking(c, t.rank) &&
-                         (f == Family::Dot || f == Family::Centred || f == Family::Lp || count_ranked(c, k));
+  // of the rows it passes) skips the screen, where the plan allows it
+  const bool direct_ok = filter_rows && t.plan.direct_ok;
   for (uint32_t q = 0; q < nq; q++) {
     const uint64_t rows_q = filter_rows ? filter_rows[t.h_qf[q]] : ~0ull;
     if (direct_ok && rows_q <= DIRECT_MAX_ROWS) dir->push_back(q);
@@ -736,10 +728,11 @@ static sdb_status submit_locked(Corpus* c, Ticket* t, const double* d_queries, u
   t->filt = FiltArg();
   t->n_direct = 0;
   t->permuted = false;
-  t->rank = rank;
+  t->plan = plan_batch(c, rank, k, nq, c->screen, c->stream_refine);
+  const Plan& p = t->plan;
   if (d_filters) {
     std::vector<uint32_t> scr, dir;
-    plan_filtered(c, *t, nq, k, d_filters, query_filter, filter_rows, &scr, &dir);
+    plan_filtered(c, *t, nq, d_filters, query_filter, filter_rows, &scr, &dir);
     if (!dir.empty() && !scr.empty()) {  // mixed: run permuted, screened queries first (see Ticket::permuted)
       std::vector<uint32_t> perm(scr);
       perm.insert(perm.end(), dir.begin(), dir.end());
@@ -766,17 +759,8 @@ static sdb_status submit_locked(Corpus* c, Ticket* t, const double* d_queries, u
   t->cancel = cancel;
   t->launches0 = c->ctx->launches;
   t->n_repaired = 0;
-  sdb_screen first, first_scr;
-  const std::vector<Rung> rungs = build_rungs(c, c->screen, k, nq, rank, &first);
-  t->rung = (c->rung_scr == first && c->rung_k == k && c->rung_view == view_key(view_of(c, rank)) &&
-             c->rung < n_batch_rungs(rungs))
-                ? c->rung
-                : 0;
-  t->n_batch_rungs = n_batch_rungs(rungs);
-  // the ladder of its screened queries, which a mixed batch screens on their own (one Lp query has none, build_rungs)
-  const uint32_t n_scr = t->n_direct < nq ? nq - t->n_direct : nq;
-  t->n_rungs = (uint32_t)build_rungs(c, c->screen, k, n_scr, rank, &first_scr).size();
-  if (nq == 0 || k == 0) {  // nothing to search: counts are zero
+  t->rung = c->remembered.key == p.key && c->remembered.rung < p.n_batch_rungs ? c->remembered.rung : 0;
+  if (p.route == Plan::Route::Empty) {  // nothing to search: counts are zero
     cudaStream_t st = t->stream;
     SDB_CUDA(cudaEventRecord(t->ev_begin, st));
     SDB_CUDA(cudaEventRecord(t->ev_screen0, st));
@@ -785,7 +769,6 @@ static sdb_status submit_locked(Corpus* c, Ticket* t, const double* d_queries, u
     for (uint32_t q = 0; q < nq; q++) t->h_flags[q] = t->h_qflags[q] = 0;
     t->h_stat[0] = t->h_stat[1] = t->h_stat[2] = t->h_stat[3] = 0;
     t->screen = SDB_SCREEN_NONE_EXACT;
-    t->n_rungs = 0;
     t->n_passes = 0;
     SDB_CUDA(cudaEventRecord(t->ev_end, st));
     t->busy = true;
@@ -847,7 +830,7 @@ sdb_status knn_shard_header(Corpus* c, uint32_t ticket, void* d_hdr) {
   Ticket* t = find_ticket(c, ticket);
   if (!t) return SDB_EINVAL;
   cudaStream_t st = t->stream;
-  if (t->n_rungs == 0) {  // exact-only or counted batch: the counters the host holds
+  if (screened_rungs(*t) == 0) {  // the counters the host holds
     SDB_CUDA(cudaMemcpyAsync(d_hdr, t->h_stat, 16, cudaMemcpyHostToDevice, st));
   } else if (t->permuted) {
     sum_flagged_kernel<<<1, 32, 0, st>>>(c->sets[t->set].d_stat, t->d_stat_scr, (uint32_t*)d_hdr);
@@ -1287,6 +1270,7 @@ sdb_status sdb_corpus_finalize(sdb_corpus* c) {
 }
 sdb_status sdb_corpus_set_screen(sdb_corpus* c, sdb_screen s) {
   if (!c || (int)s < 0 || (int)s > 4) return SDB_EINVAL;
+  std::lock_guard<std::mutex> g(c->mu);
   c->screen = s;
   return SDB_OK;
 }
@@ -1308,16 +1292,19 @@ sdb_status sdb_corpus_read_rows(sdb_corpus* c, uint64_t first_row, uint64_t n, v
 }
 sdb_status sdb_corpus_set_minkowski_order(sdb_corpus* c, double order) {
   if (!c || !(order == order)) return SDB_EINVAL;
+  std::lock_guard<std::mutex> g(c->mu);
   c->minkowski_p = order;
   return SDB_OK;
 }
 sdb_status sdb_corpus_set_schedule(sdb_corpus* c, int streaming) {
   if (!c) return SDB_EINVAL;
+  std::lock_guard<std::mutex> g(c->mu);
   c->stream_refine = streaming != 0;
   return SDB_OK;
 }
 sdb_status sdb_corpus_set_exact(sdb_corpus* c, int exact) {
   if (!c) return SDB_EINVAL;
+  std::lock_guard<std::mutex> g(c->mu);
   c->exact = exact != 0;
   return SDB_OK;
 }
@@ -1680,6 +1667,8 @@ static sdb_status debug_screen_batch(sdb_corpus* c, const double* queries, uint3
   }
   if (filters) SDB_TRY(check_filters(nq, filters, n_filters, query_filter));
   std::lock_guard<std::mutex> g(c->mu);
+  const Plan p = plan_batch(c, rank, k, nq, screen, streaming != 0);
+  const View& v = p.v;
   const bool int8 = screen == SDB_SCREEN_TC_INT8;
   // Dot: any screen on f32 rows, the tensor cores on f64 ones; Centred: the tensor cores; Lp: SIMT_F32 (the Lp screen)
   const Family f = family(c);
@@ -1688,7 +1677,7 @@ static sdb_status debug_screen_batch(sdb_corpus* c, const double* queries, uint3
                       : f == Family::Lp      ? screen == SDB_SCREEN_SIMT_F32
                                              : false;
   if (!c->finalized || !served || (int8 && !c->d_i8) || c->special_overflow || !c->n ||
-      (view_of(c, rank).cross && c->xspecial_overflow)) {
+      (v.cross && c->xspecial_overflow)) {
     set_error("sdb_debug_screen_batch: needs a finalized, non-empty F32 cosine / euclidean corpus, an F64 one with "
               "screen copies and a tensor-core screen (int8: cosine), a PEARSON one with screen copies and a "
               "tensor-core screen, or a MANHATTAN / CHEBYSHEV / MINKOWSKI (integer order 1 .. 8) one with SIMT_F32");
@@ -1714,8 +1703,7 @@ static sdb_status debug_screen_batch(sdb_corpus* c, const double* queries, uint3
   t->filt = FiltArg();
   t->n_direct = 0;
   t->permuted = false;
-  t->rank = rank;
-  const View v = view_of(c, rank);
+  t->plan = p;
   if (filters) {
     const uint32_t* bits = nullptr;
     std::vector<uint64_t> rows_per_filter;
@@ -1723,7 +1711,7 @@ static sdb_status debug_screen_batch(sdb_corpus* c, const double* queries, uint3
     SDB_CUDA(cudaEventRecord(t->ev_h2d, ctx->copy_stream));
     SDB_CUDA(cudaStreamWaitEvent(st, t->ev_h2d, 0));
     std::vector<uint32_t> scr, dir;
-    plan_filtered(c, *t, nq, k, bits, query_filter, rows_per_filter.data(), &scr, &dir);
+    plan_filtered(c, *t, nq, bits, query_filter, rows_per_filter.data(), &scr, &dir);
     if (!score_all && !scr.empty() && !dir.empty()) {
       t->filt = FiltArg();
       t->n_direct = 0;
@@ -1736,6 +1724,10 @@ static sdb_status debug_screen_batch(sdb_corpus* c, const double* queries, uint3
     t->filt.qf = t->d_qf;
   }
   const bool direct = !score_all && t->n_direct == nq;
+  if (!score_all && !direct && p.key.first != screen) {  // the plan's rung 0 is another screen
+    set_error("sdb_debug_screen_batch: the corpus does not offer screen %d", (int)screen);
+    return SDB_EINVAL;
+  }
   DevBuf<double> d_q;
   ResultBufs out;
   ScreenTap tap;
@@ -1746,7 +1738,7 @@ static sdb_status debug_screen_batch(sdb_corpus* c, const double* queries, uint3
     if (score_all) {  // one pass-0 launch over every tile (SIMT: tau stays -inf), nothing selected
       const PassDesc all{1u, 0u, (uint32_t)(n_pad / TILE_ROWS), 0u};
       SDB_TRY(prep_queries(c, s, d_q, nq, st, v));
-      SDB_TRY(cand_begin(c, s, nq, (int)screen, st, v));
+      SDB_TRY(cand_begin(c, s, nq, (int)screen, st, v, p.exact));
       SDB_TRY(tc                ? screen_tc_pass(c, s, t->filt, nq, k, all, int8, 0, st, v)
               : f == Family::Lp ? screen_lp_pass(c, s, t->filt, nq, all, st)
                                 : screen_simt_pass(c, s, t->filt, nq, all, st, v));
@@ -1758,16 +1750,11 @@ static sdb_status debug_screen_batch(sdb_corpus* c, const double* queries, uint3
     t->k = k;
     t->row_base = 0;
     t->cancel = nullptr;
-    const Run r{d_q, nq, out.rows, out.dist, out.count, t->filt, 0u, screen, streaming != 0, &tap,
-                t->h_flags, t->h_qflags, t->h_stat};
+    const Run r{d_q, nq, out.rows, out.dist, out.count, t->filt, 0u, &tap, t->h_flags, t->h_qflags, t->h_stat};
     Enqueued e;
     SDB_TRY(enqueue_batch(c, *t, r, &e));
     SDB_CUDA(cudaStreamSynchronize(st));
     if (direct) return tap_list(s, nq, &tap.list_a, &tap.cnt_a, st);  // no screen ran: the lists are the direct ones
-    if (e.screen != (int)screen) {
-      set_error("sdb_debug_screen_batch: the corpus does not offer screen %d", (int)screen);
-      return SDB_EINVAL;
-    }
     return SDB_OK;
   };
   sdb_status rc = run();
@@ -1805,7 +1792,7 @@ static sdb_status debug_screen_batch(sdb_corpus* c, const double* queries, uint3
     if (rc == SDB_OK && cudaStreamSynchronize(st) != cudaSuccess) rc = SDB_ECUDA;
     if (rc == SDB_OK) {
       // (filtered: the passing special rows are in the stage-B list)
-      const uint32_t n_special = score_all || filters ? 0u : view_n_special(c, view_of(c, rank));
+      const uint32_t n_special = score_all || filters ? 0u : view_n_special(c, v);
       auto bits = [](float v) {
         uint32_t u;
         memcpy(&u, &v, 4);

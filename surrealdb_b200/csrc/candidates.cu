@@ -491,12 +491,13 @@ __global__ void cand_begin_dot_kernel(float* __restrict__ tau, uint32_t* __restr
               __double2float_ru(hi));
 }
 
-sdb_status cand_begin(const Corpus* c, Scratch& s, uint32_t nq, int screen, cudaStream_t st, const View& v) {
+sdb_status cand_begin(const Corpus* c, Scratch& s, uint32_t nq, int screen, cudaStream_t st, const View& v,
+                      bool exact) {
   if (v.sc == Score::Dot) {
     cand_begin_dot_kernel<<<(nq + 255) / 256, 256, 0, st>>>(s.d_tau, s.d_cand_cnt, s.d_flags, s.d_stat, s.d_bscale,
                                                             s.d_beps, s.d_margin, s.d_margin2, s.d_beps2, s.d_tau2,
                                                             s.d_qlow, s.d_qcap, s.d_qmag, s.d_qbferr, nq, screen,
-                                                            c->dim, c->bf16_rel_err, c->max_norm, c->exact ? 1 : 0,
+                                                            c->dim, c->bf16_rel_err, c->max_norm, exact ? 1 : 0,
                                                             c->dtype == SDB_F64 ? 1 : 0);
     count_launch(c->ctx);
     SDB_CUDA(cudaGetLastError());
@@ -511,13 +512,13 @@ sdb_status cand_begin(const Corpus* c, Scratch& s, uint32_t nq, int screen, cuda
                                                                   s.d_bscale, s.d_beps, s.d_margin, s.d_margin2,
                                                                   s.d_beps2, s.d_tau2, s.d_qlow, s.d_qcap, s.d_q32,
                                                                   nq, c->dim, p, c->max_norm, s.d_mscale,
-                                                                  c->exact ? 1 : 0);
+                                                                  exact ? 1 : 0);
         count_launch(c->ctx);
       } else {
         cand_begin_lp_kernel<<<(nq + 3) / 4, 128, 0, st>>>(s.d_tau, s.d_cand_cnt, s.d_flags, s.d_stat,
                                                            s.d_bscale, s.d_beps, s.d_margin, s.d_margin2,
                                                            s.d_beps2, s.d_tau2, s.d_qlow, s.d_qcap, s.d_q32, nq,
-                                                           (int)c->metric, c->dim, c->max_norm, c->exact ? 1 : 0);
+                                                           (int)c->metric, c->dim, c->max_norm, exact ? 1 : 0);
       }
       break;
     case Family::Centred:
@@ -528,7 +529,7 @@ sdb_status cand_begin(const Corpus* c, Scratch& s, uint32_t nq, int screen, cuda
                                                           s.d_qlow, s.d_qcap, s.d_qmag, s.d_q8scale, s.d_q8err,
                                                           s.d_qbferr, nq, screen, (int)SDB_COSINE, c->dim,
                                                           c->max_rel_qerr, c->i8_scale, c->bf16_rel_err, c->max_norm,
-                                                          c->exact ? 1 : 0, 1, 0);
+                                                          exact ? 1 : 0, 1, 0);
       break;
     case Family::Dot: {
       // the bound's form is the view's score, not the corpus metric: Cosine (relative, with the F64 rows' underflow
@@ -539,7 +540,7 @@ sdb_status cand_begin(const Corpus* c, Scratch& s, uint32_t nq, int screen, cuda
                                                           s.d_beps, s.d_margin, s.d_margin2, s.d_beps2, s.d_tau2,
                                                           s.d_qlow, s.d_qcap, s.d_qmag, s.d_q8scale, s.d_q8err,
                                                           s.d_qbferr, nq, screen, form, c->dim, c->max_rel_qerr,
-                                                          c->i8_scale, c->bf16_rel_err, c->max_norm, c->exact ? 1 : 0,
+                                                          c->i8_scale, c->bf16_rel_err, c->max_norm, exact ? 1 : 0,
                                                           c->dtype == SDB_F64 ? 1 : 0, v.sc == Score::EuclidFar);
       break;
     }
@@ -550,7 +551,7 @@ sdb_status cand_begin(const Corpus* c, Scratch& s, uint32_t nq, int screen, cuda
                                                           s.d_qlow, s.d_qcap, s.d_qmag, s.d_q8scale, s.d_q8err,
                                                           s.d_qbferr, nq, screen, (int)c->metric, c->dim,
                                                           c->max_rel_qerr, c->i8_scale, c->bf16_rel_err, c->max_norm,
-                                                          c->exact ? 1 : 0, c->dtype == SDB_F64 ? 1 : 0, 0);
+                                                          exact ? 1 : 0, c->dtype == SDB_F64 ? 1 : 0, 0);
       break;
   }
   count_launch(c->ctx);

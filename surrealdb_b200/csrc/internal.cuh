@@ -239,6 +239,59 @@ struct Ranking {
   bool desc = false;
 };
 
+// What the Dot and Centred screens score per row:
+//   Cosine     acc / |x|          (own: COSINE corpora and the centred operands of PEARSON ones; cross: EUCLIDEAN ones)
+//   Euclid     2 acc - |x|^2      (own: EUCLIDEAN corpora; cross: COSINE ones)
+//   Dot        acc                dot_ranking batches on either Dot metric
+//   EuclidFar  2 acc + |x|^2      euclidean descending, acc against -q: |x|^2 - 2 x.q = d^2 - |q|^2
+// acc = x~.q~, the dot of the screen copies.  (Lp / Count / Exact corpora: Euclid, which none of their stages reads.)
+enum class Score { Cosine, Euclid, Dot, EuclidFar };
+// A batch's view of a Dot or Centred corpus, decided once per batch (view_of) and handed to every stage that depends on
+// it (prep_queries, cand_begin, the screens, cand_refine, cand_add_specials, the re-rank, cand_final).
+struct View {
+  Score sc = Score::Euclid;
+  bool neg = false;    // the screen copies are those of -q (the re-rank keeps q)
+  bool cross = false;  // per-row array and special list: the cross state (d_xnorm, d_xspecial), else d_snorm, d_special
+  int steps = SDB_EUCLIDEAN;  // the re-rank's accumulation: SDB_COSINE (x.q), SDB_EUCLIDEAN ((x - q)^2), SDB_FN_DOT
+  bool sim = false;    // ... and its finish: the cosine similarity instead of the cosine distance
+  bool desc = false;   // the ranking's direction (Ranking::desc): the re-rank keys descending, cand_final proves that
+};
+// One rung of a batch's precision ladder (plan_batch, api.cu): a screen and the candidate-list capacity per query.
+struct Rung {
+  sdb_screen scr;
+  uint32_t cap;
+};
+// What a remembered ladder rung belongs to (Corpus::remembered): the first-choice screen of the batch that settled on
+// it, its k and the view_key of its view (dot batches' candidate sets are not KNN's)
+struct RungKey {
+  sdb_screen first = SDB_SCREEN_AUTO;
+  uint32_t k = 0;
+  int view = 0;
+  bool operator==(const RungKey& o) const { return first == o.first && k == o.k && view == o.view; }
+};
+// How a brute-force batch runs, decided once at submit (plan_batch, api.cu) from the corpus, the ranking, k and the
+// corpus' screen, schedule and proof mode as they stand then.  Every stage and the wait read the plan instead of those
+// settings, so a batch in flight is finished the way it was submitted.
+struct Plan {
+  enum class Route { Empty, Exact, Counted, Screened };  // of the whole batch
+  Route route = Route::Empty;
+  Ranking rank;
+  View v;
+  Rung ladder[5] = {};          // Screened: the precision ladder, cheapest first
+  uint32_t n_ladder = 0;
+  uint32_t n_batch_rungs = 0;   // rungs a whole batch may climb
+  RungKey key;                  // key.first: the whole batch's first-choice screen (NONE_EXACT: none)
+  bool single_exact = false;    // a run of one query takes the exact kernel (AUTO on MANHATTAN, CHEBYSHEV, HAMMING)
+  bool direct_ok = false;       // filtered queries may take the direct regime
+  bool stream_refine = true;    // tensor-core schedule: one streaming launch (else the multi-pass schedule)
+  bool exact = true;            // proof and exact fallbacks (false: approximate mode); stage B on tensor-core screens
+  bool cancel_at_wait = false;  // dot and cross rankings report a cancel raised while the batch is in flight
+  // a run of nq queries: the whole batch, a mixed batch's screened head or a repair sub-batch.  The single-query rule
+  // applies to the run's own query count.
+  bool counted(uint32_t nq) const { return route == Route::Counted && !(single_exact && nq == 1); }
+  uint32_t rungs(uint32_t nq) const { return single_exact && nq == 1 ? 0u : n_ladder; }
+};
+
 struct Comm;  // comm.cu: NCCL communicator attached to a context (nullptr = single shard)
 
 struct Ctx {
@@ -296,8 +349,9 @@ struct Ticket {
   const volatile int* cancel = nullptr;
   cudaStream_t stream = nullptr;  // every kernel / copy of this batch (slot parity picks the context's stream)
   int set = 0;                    // scratch set of this batch
+  Plan plan;
   int screen = 0;       // sdb_screen this batch ran
-  uint32_t rung = 0, n_rungs = 0, n_batch_rungs = 0, n_repaired = 0;
+  uint32_t rung = 0, n_repaired = 0;  // rung: of plan.ladder, where the whole batch stands
   uint32_t n_passes = 0;
   uint64_t launches0 = 0;
   cudaEvent_t ev_begin = nullptr, ev_screen0 = nullptr, ev_screen1 = nullptr, ev_end = nullptr;
@@ -333,7 +387,6 @@ struct Ticket {
   uint64_t* d_fin_rows = nullptr;
   double* d_fin_dist = nullptr;
   uint32_t* d_fin_count = nullptr;
-  Ranking rank;  // what the batch ranks (KNN: the corpus metric ascending)
   // SDB_TRACE=1: named timestamps of this batch on its stream, printed at wait time relative to the context's epoch
   std::vector<std::pair<const char*, cudaEvent_t>> trace;
 };
@@ -406,10 +459,10 @@ struct Corpus {
   bool exact = true;   // false: skip the proof / exact fallback (approximate mode)
   bool stream_refine = true;  // tensor-core screens: one streaming launch with in-kernel threshold refinement
   double minkowski_p = 3.0;   // order of SDB_MINKOWSKI
-  sdb_screen rung_scr = SDB_SCREEN_AUTO;  // the first-choice screen the remembered rung belongs to
-  uint32_t rung_k = 0;                    // ... and the k it was learnt for
-  int rung_view = 0;                      // ... and the view_key of its batch (dot batches' candidate sets are not KNN's)
-  uint32_t rung = 0;                     // rung of the precision ladder the last batch settled on (api.cu)
+  struct {
+    RungKey key;
+    uint32_t rung = 0;
+  } remembered;  // the ladder rung the last screened batch settled on, and what it belongs to (api.cu)
   uint64_t cap = 0, n = 0;
   uint64_t row_base = 0;            // global id of row 0 (row-sharded corpora)
   bool finalized = false;
@@ -485,8 +538,8 @@ inline Family family(const Corpus* c) {
   }
 }
 constexpr uint32_t COUNT_CAP_MAX = 16384;  // candidate entries per query of the count path: n_ranges k at most
-inline bool count_ranked(const Corpus* c, uint32_t k) {
-  return family(c) == Family::Count && k >= 1 && k <= 256 && c->screen != SDB_SCREEN_NONE_EXACT;
+inline bool count_ranked(const Corpus* c, uint32_t k, sdb_screen screen) {
+  return family(c) == Family::Count && k >= 1 && k <= 256 && screen != SDB_SCREEN_NONE_EXACT;
 }
 // The ranking of KNN itself, the corpus metric ascending: KnnTopK's DistanceEntry order and SortTopK's are both
 // Number::cmp and then scan position, so it takes the KNN path unchanged.
@@ -527,23 +580,6 @@ inline bool cross_ranking(const Corpus* c, const Ranking& r) {
 inline bool screened_ranking(const Corpus* c, const Ranking& r) {
   return knn_ranking(c, r) || cosine_desc(c, r) || metric_desc(c, r) || dot_ranking(c, r) || cross_ranking(c, r);
 }
-// What the Dot and Centred screens score per row:
-//   Cosine     acc / |x|          (own: COSINE corpora and the centred operands of PEARSON ones; cross: EUCLIDEAN ones)
-//   Euclid     2 acc - |x|^2      (own: EUCLIDEAN corpora; cross: COSINE ones)
-//   Dot        acc                dot_ranking batches on either Dot metric
-//   EuclidFar  2 acc + |x|^2      euclidean descending, acc against -q: |x|^2 - 2 x.q = d^2 - |q|^2
-// acc = x~.q~, the dot of the screen copies.  (Lp / Count / Exact corpora: Euclid, which none of their stages reads.)
-enum class Score { Cosine, Euclid, Dot, EuclidFar };
-// A batch's view of a Dot or Centred corpus, decided once per batch (view_of) and handed to every stage that depends on
-// it (prep_queries, cand_begin, the screens, cand_refine, cand_add_specials, the re-rank, cand_final).
-struct View {
-  Score sc = Score::Euclid;
-  bool neg = false;    // the screen copies are those of -q (the re-rank keeps q)
-  bool cross = false;  // per-row array and special list: the cross state (d_xnorm, d_xspecial), else d_snorm, d_special
-  int steps = SDB_EUCLIDEAN;  // the re-rank's accumulation: SDB_COSINE (x.q), SDB_EUCLIDEAN ((x - q)^2), SDB_FN_DOT
-  bool sim = false;    // ... and its finish: the cosine similarity instead of the cosine distance
-  bool desc = false;   // the ranking's direction (Ranking::desc): the re-rank keys descending, cand_final proves that
-};
 inline View view_of(const Corpus* c, const Ranking& r) {
   View v;
   v.desc = r.desc;
@@ -649,7 +685,8 @@ sdb_status prep_queries(const Corpus* c, Scratch& s, const double* d_queries, ui
 // one query prepared into the fallback scratch (d_fb_*), independent of the batch scratch
 sdb_status prep_fallback_query(Corpus* c, const double* d_query, cudaStream_t st);
 // resets tau / counts / flags and derives, per query, the screen's error bound, the selection margin and the score range
-sdb_status cand_begin(const Corpus* c, Scratch& s, uint32_t nq, int screen, cudaStream_t st, const View& v);
+// (exact: the batch's proof mode, Plan::exact; approximate mode selects with no margin)
+sdb_status cand_begin(const Corpus* c, Scratch& s, uint32_t nq, int screen, cudaStream_t st, const View& v, bool exact);
 sdb_status cand_set_count(const Corpus* c, Scratch& s, uint32_t nq, uint32_t value, cudaStream_t st);
 // per query: gather the main list + the private sub-lists, find the k-th best score s_k, keep every candidate with
 // score >= tau = s_k - margin (all of them while fewer than k exist), publish tau.  (The streaming pass's histogram is

@@ -789,13 +789,9 @@ sdb_status screen_tc_pass(const Corpus* c, Scratch& s, const FiltArg& filt, uint
     return SDB_EUNSUPPORTED;
   }
   const uint64_t n_pad = (c->n + TILE_ROWS - 1) / TILE_ROWS * TILE_ROWS;
-  // refiner pacing (tuning knobs): it re-reads its queries' histograms at most every sleep_min ns while thresholds
-  // move, backing off to sleep_max when they do not
-  uint32_t sleep_min = 512, sleep_max = 8192;
-  if (const char* e = getenv("SDB_REFINE_SLEEP_MIN")) sleep_min = (uint32_t)atoi(e);
-  if (const char* e = getenv("SDB_REFINE_SLEEP_MAX")) sleep_max = (uint32_t)atoi(e);
-  if (sleep_min < 32) sleep_min = 32;
-  if (sleep_max < sleep_min) sleep_max = sleep_min;
+  // refiner pacing: it re-reads its queries' histograms at most every sleep_min ns while thresholds move, backing off
+  // to sleep_max when they do not
+  const uint32_t sleep_min = 512, sleep_max = 8192;
   const uint32_t k_blocks = int8 ? c->dim_pad8 / (2 * tc::BLOCK_K) : c->dim_pad / tc::BLOCK_K;
   // every launch uses the same grid so that the (CTA, half) slot numbering of the private sub-lists is stable
   const uint32_t chunk_q = tc::MAX_MBLOCKS * tc::BLOCK_M;
